@@ -2,6 +2,7 @@
 """Benchmark of the offline Paraformer hot path (BASELINE.json metric: RTFx = audio-seconds / second).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--config 2|3|4|5] [--mode fp32|fp16x3|fp16x6|fp16] [--impl reference]
+                  [--dump-outputs DIR]
 
 One step = one pass of the hot path over one job of synthetic 16 kHz utterances (BASELINE.json `configs`):
   --config 2 (default, the configuration the metric is quoted on): Paraformer-large, 64 x 30 s per GPU, weak scaling
@@ -18,6 +19,9 @@ overlaps the next job's kernels.  Prints ONE JSON line (rank 0).
 timed region.  `parity` compares the ids of the TIMED job (and the log-probabilities and stage taps — features, encoder output, CIF
 weights, acoustic embeddings — of an untimed taps pass over the same utterances) with the CPU oracle's output for a bounded sample,
 computed by the CPU leg of the same run.
+`--dump-outputs DIR` writes what the last timed step returned to its caller — the token ids of every utterance of the job, in input
+order — as DIR/ids.npy (float64 [utterances, longest], -1 padded) and DIR/ids_lens.npy (float64 [utterances]).  The inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 `--impl reference` times the unmodified reference on the host cores (AutoModel(device="cpu").generate() from the offline
 install under baseline/_ref, kind "reference"; the CPU restatement oracle/, kind "port", when that cannot be imported).
 """
@@ -81,7 +85,8 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 / FP16 989 TFLOP/s — upper bounds, not measurements
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -585,7 +590,10 @@ def main():
     ap.add_argument("--parity-out", default=None, help="(reference leg) write the oracle's ids / log-probs of the sample here")
     ap.add_argument("--port", action="store_true", help="(reference leg) time the oracle port even when the reference imports")
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's token ids as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         return run_reference(args)
 
@@ -644,6 +652,8 @@ def main():
     toks = torch.cat([t.float() for t in job.tok_stats]) if job.tok_stats else torch.zeros(1)
     ntok_mean, n_max = float(toks.mean()), int(toks.max())
     log("device-resident: %.2f ms/step" % (ms_total / args.steps))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_ids)
 
     # ---- e2e: plugin call(s), host (pinned) waveforms in -> token ids on the host out
     for _ in range(2):
@@ -685,7 +695,7 @@ def main():
                            "utterances_this_gpu": len(job.wavs), "batches_this_gpu": len(job.plan["buckets"]),
                            "audio_seconds_total": job.audio_seconds, "gemm_mode": args.mode, "tokens_per_utt_mean": ntok_mean, "n_max": n_max,
                            "parallelism": "utterance-sharded dp%d, one asynchronous all-gather of id rows per job" % world,
-                           "l2": "per-step working set (0.9 GB weights + >1 GB activations) exceeds the 126 MB L2; no flush needed",
+                           "l2": "per-step working set (0.9 GB weights + >1 GB activations) exceeds the 50 MB L2; no flush needed",
                            "algorithmic_gflop_per_job": flops_job / 1e9},
                 "clocks": clocks,
                 "e2e": {"value": job.audio_seconds * args.steps / e2e_s, "unit": "audio-sec/s", "h2d_bytes_per_step": local_samples * 4 + len(job.wavs) * 4,
@@ -695,7 +705,7 @@ def main():
                 "gpu_launches": launches,
                 "per_rank_ms_per_step": [x / args.steps for x in per_rank],
                 "achieved_tflops_algorithmic": ach,
-                "step_frac_of_sustained_peak": ach / world / pk.get("bf16_tflops_sustained", 1400.0),
+                "step_frac_of_sustained_peak": ach / world / pk.get("bf16_tflops_sustained", 989.0),
                 "roofline": roof}
         if world == 1 and not args.no_cpu_baseline:
             try:
@@ -713,10 +723,22 @@ def main():
         dist.destroy_process_group()
 
 
+def dump_outputs(out_dir, ids):
+    """ids: one token-id list per utterance (input order) -> out_dir/ids.npy (-1 padded) and out_dir/ids_lens.npy, float64."""
+    os.makedirs(out_dir, exist_ok=True)
+    width = max([len(r) for r in ids] + [1])
+    arr = np.full((len(ids), width), -1.0, dtype=np.float64)
+    for i, r in enumerate(ids):
+        arr[i, :len(r)] = r
+    np.save(os.path.join(out_dir, "ids.npy"), arr)
+    np.save(os.path.join(out_dir, "ids_lens.npy"), np.array([len(r) for r in ids], dtype=np.float64))
+    log("outputs of the last timed step written to %s" % out_dir)
+
+
 def dominant_gemm_roofline(lib, job, dev, mode, pk, pk_src):
-    """The dominant kernel = the tcgen05 GEMM.  Timed ALONE — exactly the launch the encoder makes for FFN w_1 (A operand = the
-    fp16 planes LayerNorm wrote, plane-emitting epilogue: gemm_tc2_kernel<3,2,EPI_PLANES>) at this job's largest batch — with CUDA
-    events on the launching stream, L2 flushed between launches; algorithmic flops 2MNK vs the measured fp16 burst peak."""
+    """The dominant kernel = the wgmma GEMM.  Timed ALONE — exactly the launch the encoder makes for FFN w_1 (A operand = the
+    fp16 planes LayerNorm wrote, plane-emitting epilogue: gemm_tc_kernel<128,2,2,2,EPI_PLANES>) at this job's largest batch — with
+    CUDA events on the launching stream, L2 flushed between launches; algorithmic flops 2MNK vs the fp16 peak."""
     import ctypes as C
     from funasr_b200 import _abi
     eng = job.eng
@@ -748,19 +770,11 @@ def dominant_gemm_roofline(lib, job, dev, mode, pk, pk_src):
             times.append(e0.elapsed_time(e1))
     ms = sum(times) / len(times)
     ach = algo / (ms / 1e3) / 1e12
-    peak = pk.get("bf16_tflops", 1590.0)
-    traffic, tsrc = None, "no ncu capture of this build committed (profiles/r2_ncu_w1_traffic.json)"
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_w1_traffic.json")))
-        if int(t.get("M", 0)) == M:
-            traffic, tsrc = float(t["dram_read_bytes"]) + float(t["dram_write_bytes"]), "profiles/r2_ncu_w1_traffic.json (%s)" % t.get("source", "ncu --set full")
-        else:
-            tsrc = "profiles/r2_ncu_w1_traffic.json was captured at M=%s, this launch has M=%d" % (t.get("M"), M)
-    except Exception:
-        pass
-    return {"bound": "tensor", "kernel": "gemm_tc2_kernel<3,2,EPI_PLANES> (FFN w_1 as the encoder launches it: M=%d N=2048 K=512, %s, cta_group::2, "
+    peak = pk.get("bf16_tflops", 989.0)
+    traffic, tsrc = None, "not measured"
+    return {"bound": "tensor", "kernel": "gemm_tc_kernel (FFN w_1 as the encoder launches it: M=%d N=2048 K=512, %s, "
                                          "fp16 planes in, ReLU fp16 planes out)" % (M, mode),
-            "achieved": ach, "peak": peak, "peak_source": pk_src + " fp16 burst (MEASURED_PEAKS.json)", "unit": "TFLOP/s", "frac": ach / peak,
+            "achieved": ach, "peak": peak, "peak_source": pk_src + " fp16", "unit": "TFLOP/s", "frac": ach / peak,
             "traffic": traffic, "traffic_source": tsrc,
             "algorithmic_bytes": float(npl * M * K * 2 + 2 * N * K * 2 + npl * M * N * 2),
             "ms": ms, "tensor_passes": passes, "tensor_issue_tflops": ach * passes, "tensor_issue_frac": ach * passes / peak,

@@ -1,4 +1,4 @@
-"""funasr_b200 — B200-native (sm_100a) backend for FunASR's offline Paraformer hot path.
+"""funasr_b200 — H100-native (sm_90a) backend for FunASR's offline Paraformer hot path.
 
 Importing this package registers the drop-in plugin classes (ParaformerB200, WavFrontendB200, SANMEncoderB200,
 CifPredictorV2B200, ParaformerSANMDecoderB200) — into ``funasr.register.tables`` when FunASR is imported, else into

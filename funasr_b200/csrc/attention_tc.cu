@@ -1,20 +1,16 @@
-// tcgen05 / TMEM / TMA fused multi-head attention with fp16 operand splitting (sm_100a).
+// wgmma / TMA fused multi-head attention with fp16 operand splitting (sm_90a).
 //
 // Same contract as attention_f32.cu (sanm/attention.py:288-304 with scores from :324-325; cross-attention :760-794,
 // :811-812): ctx = softmax(mask(q d_k^-0.5 . k^T)) v per head, key-padding mask, heads merged.  Score and context
-// contractions run on the 5th-gen tensor cores with fp32 accumulation in TMEM; operands are fp16 planes (hi, lo) of the
+// contractions run on the tensor cores (wgmma) with fp32 accumulation in registers; operands are fp16 planes (hi, lo) of the
 // fp32 tensors so that S = Qh.Kh + Qh.Kl + Ql.Kh and O = Ph.Vh + Ph.Vl + Pl.Vh carry ~2^-17 relative error (x3 mode),
 // or one plane (x1 mode).  The [B,H,Tq,Tk] score tensor never leaves the SM.
 //
 // One CTA = 128 queries of one (utterance, head), keys in chunks of 64, two passes over the keys:
-//   pass A: S~ = Qh.Kh (one MMA term) -> per-row max m   (softmax is invariant to the choice of m; an approximate
-//           maximum only has to keep exp(s - m) in range, so one fp16 term suffices)
-//   pass B: S (all terms) -> p = exp(s - m), l += sum p, P planes -> smem, O += P.V accumulated in TMEM with no
-//           rescaling traffic; finally O / l -> fp16 planes (A operand of the out-projection GEMM) and/or fp32.
-// Warp roles (384 threads): warp 0 TMA producer, warp 1 MMA issuer, warp 2 TMEM allocator, warps 4-11 softmax + epilogue:
-// TMEM lane == query row; two threads per row (warp w owns lane quarter w%4 and column half (w-4)/4) so that every SM
-// sub-partition has two softmax warps to interleave.  S is double buffered in TMEM so the MMAs of chunk j+1 overlap
-// the softmax of chunk j.
+//   pass A: S~ = Qh.Kh (one MMA term) -> per-row max m   (softmax is invariant to the choice of m)
+//   pass B: S (all terms) -> p = exp(s - m), l += sum p, P planes in registers (the A operand of the next wgmma),
+//           O += P.V accumulated in registers with no rescaling; finally O / l -> fp16 planes (A operand of the
+//           out-projection GEMM) and/or fp32.
 #include "common.cuh"
 #include "kernels.h"
 #include "tc_common.cuh"
@@ -25,13 +21,13 @@ namespace fa {
 
 constexpr int AT_BQ = 128, AT_BKEY = 64, AT_D = 128;
 constexpr uint32_t AT_Q_KBLK = AT_BQ * 128;      // 16 KB: 128 rows x 64 fp16
-constexpr uint32_t AT_K_KBLK = AT_BKEY * 128;    // 8 KB : 64 keys x 64 fp16
-constexpr uint32_t AT_V_TILE = AT_D * 128;       // 16 KB: 128 d-rows x 64 keys
-constexpr uint32_t AT_P_TILE = AT_BQ * 128;      // 16 KB: 128 queries x 64 keys
+constexpr uint32_t AT_BOX = 8192;                // every K / V box: 64 rows x 128 B
+// K/V ring slots: as many as fit next to the Q planes in 227 KB of shared memory
+#define AT_NSLOT(npl) ((npl) == 1 ? 8 : 5)
 
 struct AttTcParams {
   int tq, tk, heads, batch;
-  float o_scale;                                       // round-toward-zero compensation of the P.V accumulation, per k-step (gemm_tc.cu: acc_scale)
+  float o_scale;                                       // truncation compensation of the P.V accumulation, per k-step (gemm_tc.cu: acc_scale)
   int kv_shared;                                       // 1: every utterance attends over the SAME keys / values (hotword memory): K/V planes hold one batch entry
   const int32_t* key_lens;
   int64_t q_plane_rows, k_plane_rows, v_plane_rows;   // rows between planes in the respective 2D maps
@@ -39,83 +35,43 @@ struct AttTcParams {
   plane_t* ctx_planes; int64_t ldp; int out_nplanes;   // fp16 planes [npl][B*tq][ldp] (or null)
 };
 
-// Optional in-kernel timeline (tools/att_trace.py builds a separate library with -DFA_ATT_TRACE; the product build has none
-// of this): role 0 = TMA producer, 1 = MMA issuer, 2 = softmax warp 4 lane 0; (tag, clock64) pairs of one mid-grid CTA.
-#ifdef FA_ATT_TRACE
-__device__ long long g_att_trace[3][512];
-__device__ int g_att_cnt[3];
-#define TRACE_DECL() int tr_n = 0; const bool tr_on = (blockIdx.x == 1 && blockIdx.y == 1 && blockIdx.z == gridDim.z / 2)
-#define TRACE(role, tag) do { if (tr_on && tr_n < 255) { g_att_trace[role][2 * tr_n] = (tag); g_att_trace[role][2 * tr_n + 1] = clock64(); ++tr_n; g_att_cnt[role] = tr_n; } } while (0)
-#else
-#define TRACE_DECL()
-#define TRACE(role, tag)
-#endif
-
-__device__ __forceinline__ void softmax_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the 8 softmax warps
-
-// NPL: operand planes (1 | 2); OPL: context planes written (0 = fp32 context only); CL: cluster size along the query-tile
-// axis (1 | 2 | 4) — the CL CTAs of a cluster work on different query tiles of the SAME (utterance, head) and share every
-// K / V chunk: each CTA fetches 1/CL of a chunk's 8 KB boxes and TMA-multicasts them into all CL shared memories.
-template <int NPL, int OPL, int CL>
+// NPL: operand planes (1 | 2); OPL: context planes written (0 = fp32 context only).
+// One CTA = 128 queries of one (utterance, head), 384 threads: warp 0 is the TMA producer, warps 4-11 are two consumer
+// warpgroups of 64 query rows each.  K and V chunks share ONE shared-memory ring, filled in the order the consumers read them
+//   pass A: Khi(0) .. Khi(nc-1)          pass B: K(0), V(0), K(1), V(1), ..., K(nc-1), V(nc-1)
+// and each slot is released by the eight consumer warps once their MMAs on it have retired.
+template <int NPL, int OPL>
 __global__ void __launch_bounds__(384, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                     const __grid_constant__ CUtensorMap map_v, const AttTcParams p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  constexpr uint32_t BOX = 8192;                          // every K / V box: 64 rows x 128 B
-  constexpr uint32_t Q_BYTES = NPL * 2 * AT_Q_KBLK;       // staging only: Q is moved to TMEM once
-  constexpr uint32_t SLOT_BYTES = NPL * 2 * BOX;          // one K chunk (NPL planes x 2 d-blocks) or one V chunk (NPL x 2 row halves)
-  constexpr int NSLOT = 5, NS = 4;                        // ring slots; S/P stages in TMEM
+  constexpr uint32_t Q_BYTES = NPL * 2 * AT_Q_KBLK;       // Q planes, two 64-dim boxes each, read by the score MMAs in place
+  constexpr uint32_t SLOT_BYTES = NPL * 2 * AT_BOX;       // one K chunk (NPL planes x 2 d-blocks) or one V chunk (NPL x 2 row halves)
+  constexpr int NSLOT = AT_NSLOT(NPL);
   constexpr int NT = NPL == 1 ? 1 : 3;
-  constexpr uint16_t MC_ALL = (uint16_t)((1u << CL) - 1u);
-  // TMEM columns: Q planes [0, NPL*64) | S/P stage st at 128 + 64*st (4 stages) | O at 384 .. 512
-  // (Q in TMEM on purpose.  Round 2 tried the SS form — score MMAs reading Q from the TMA tiles in shared memory, no smem -> registers
-  //  -> TMEM move before the first MMA: every layer's launch got SLOWER, 105.7 -> 117.4 us at B = 64, T = 500; with Q, K and V all
-  //  coming through the shared-memory port the MMAs wait on operand reads.)
-  constexpr uint32_t TM_Q = 0, TM_S = 128, TM_O = 384;
   // align to 1024 B WITHOUT leaving the shared address space (a uintptr_t round trip makes every access a generic LD/ST)
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  unsigned char* sQ = smem;                               // Q staging, later the epilogue's transpose buffer
-  // K and V chunks share ONE ring, filled in exactly the order the MMA warp consumes them
-  //   pass A: Khi(0) .. Khi(nc-1)          pass B: K(0), K(1), K(2), V(0), K(3), V(1), ..., K(nc-1), V(nc-3), V(nc-2), V(nc-1)
-  // (score tiles run TWO chunks ahead of P.V so the softmax of chunk t has two score-MMA durations to finish before the tensor
-  //  pipe needs its probabilities; with four S/P stages the stage S(t+2) overwrites was released by P.V(t-2) long before)
+  unsigned char* sQ = smem;
   unsigned char* sRing = sQ + Q_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sRing + NSLOT * SLOT_BYTES);
-  uint64_t* q_full = bars;            // [1]  TMA -> softmax warps
-  uint64_t* q_ready = bars + 1;       // [1]  Q planes are in TMEM (8 arrivals)
-  uint64_t* r_full = bars + 2;        // [NSLOT]
-  uint64_t* r_empty = bars + 7;       // [NSLOT] CL arrivals: every CTA of the cluster has consumed its copy
-  uint64_t* s_full = bars + 12;       // [NS] score tile complete
-  uint64_t* sa_free = s_full + NS;    // [NS] pass A: 8 softmax warps have read the tile
-  uint64_t* sb_free = sa_free + NS;   // [NS] pass B: the P.V that read the in-place probabilities has retired
-  uint64_t* p_full = sb_free + NS;    // [NS] probabilities written in place (8 arrivals)
-  uint64_t* o_full = p_full + NS;     // [1]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 1);
-  float* s_red = reinterpret_cast<float*>(o_full + 2);   // [2][128] row max / row sum exchange between column halves
+  uint64_t* q_full = reinterpret_cast<uint64_t*>(sRing + NSLOT * SLOT_BYTES);
+  uint64_t* r_full = q_full + 1;      // [NSLOT]
+  uint64_t* r_empty = r_full + NSLOT; // [NSLOT] 8 arrivals: every consumer warp is done with the slot
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * AT_BQ, h = blockIdx.y, b = blockIdx.z;
-  const uint32_t crank = CL > 1 ? cluster_ctarank() : 0u;
 
   if (warp == 0 && lane == 0) { tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_v); }
   if (warp == 1 && lane == 0) {
-    mbar_init(q_full, 1); mbar_init(q_ready, 8); mbar_init(o_full, 1);
-    for (int s = 0; s < NSLOT; ++s) { mbar_init(&r_full[s], 1); mbar_init(&r_empty[s], CL); }
-    for (int s = 0; s < NS; ++s) { mbar_init(&s_full[s], 1); mbar_init(&sa_free[s], 8); mbar_init(&sb_free[s], 1); mbar_init(&p_full[s], 8); }
+    mbar_init(q_full, 1);
+    for (int s = 0; s < NSLOT; ++s) { mbar_init(&r_full[s], 1); mbar_init(&r_empty[s], 8); }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  if (CL > 1) cluster_sync_all();                    // peers' barriers are initialised before anyone multicasts into them
-  tc_fence_after();
-  pdl_wait();                                        // everything above touched only shared / tensor memory
+  pdl_wait();                                        // everything above touched only shared memory
   pdl_trigger();
   const int klen = min(p.key_lens[b], p.tk);
   const int bkv = p.kv_shared ? 0 : b;
-  const int nc = (klen + AT_BKEY - 1) / AT_BKEY;     // key chunks with at least one valid key (same for the whole cluster)
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_o = tmem_base + TM_O;
+  const int nc = (klen + AT_BKEY - 1) / AT_BKEY;     // key chunks with at least one valid key
 
   if (warp == 0) {
     // ===================== TMA producer =====================
@@ -128,644 +84,156 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
           tma_load_2d(sQ + (pl * 2 + kb) * AT_Q_KBLK, &map_q, q_full, h * AT_D + kb * 64,
                       (int)(pl * p.q_plane_rows + (int64_t)b * p.tq + q0));
       uint32_t n = 0;                                       // ring sequence number
-      TRACE_DECL();
-      TRACE(0, 0);
-      // one chunk = nb boxes of 8 KB; box bi is fetched by CTA (bi % CL) and multicast to the whole cluster
-      auto load_chunk = [&](bool is_v, int idx, int nb) {
+      auto load_chunk = [&](bool is_v, int idx, int nb) {  // nb boxes of 8 KB: box bi = plane bi / 2, half bi % 2
         const uint32_t slot = n % NSLOT;
         mbar_wait(&r_empty[slot], ((n / NSLOT) & 1u) ^ 1u);
-        TRACE(0, 100 + (int)n);
-        mbar_expect_tx(&r_full[slot], (uint32_t)nb * BOX);
+        mbar_expect_tx(&r_full[slot], (uint32_t)nb * AT_BOX);
         unsigned char* dst = sRing + slot * SLOT_BYTES;
         for (int bi = 0; bi < nb; ++bi) {
-          if (CL > 1 && (uint32_t)(bi % CL) != crank) continue;
           const int pl = bi >> 1, sub = bi & 1;
-          int c0, c1;
-          const CUtensorMap* mp;
-          if (is_v) { mp = &map_v; c0 = idx * AT_BKEY; c1 = (int)(pl * p.v_plane_rows + ((int64_t)bkv * p.heads + h) * AT_D + sub * 64); }
-          else { mp = &map_k; c0 = h * AT_D + sub * 64; c1 = (int)(pl * p.k_plane_rows + (int64_t)bkv * p.tk + idx * AT_BKEY); }
-          if (CL > 1) tma_load_2d_mc(dst + bi * BOX, mp, &r_full[slot], c0, c1, MC_ALL);
-          else tma_load_2d(dst + bi * BOX, mp, &r_full[slot], c0, c1);
+          if (is_v) tma_load_2d(dst + bi * AT_BOX, &map_v, &r_full[slot], idx * AT_BKEY, (int)(pl * p.v_plane_rows + ((int64_t)bkv * p.heads + h) * AT_D + sub * 64));
+          else tma_load_2d(dst + bi * AT_BOX, &map_k, &r_full[slot], h * AT_D + sub * 64, (int)(pl * p.k_plane_rows + (int64_t)bkv * p.tk + idx * AT_BKEY));
         }
         ++n;
       };
       for (int i = 0; i < nc; ++i) load_chunk(false, i, 2);            // pass A: hi plane only
-      load_chunk(false, 0, NPL * 2);
-      if (nc > 1) load_chunk(false, 1, NPL * 2);
       for (int t = 0; t < nc; ++t) {
-        if (t + 2 < nc) load_chunk(false, t + 2, NPL * 2);
+        load_chunk(false, t, NPL * 2);
         load_chunk(true, t, NPL * 2);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (nc > 0 && elect_one_sync()) {
-      constexpr uint32_t idesc_s = make_idesc_f16(AT_BQ, AT_BKEY);
-      constexpr uint32_t idesc_o = make_idesc_f16(AT_BQ, AT_D);
-      const int ta[3] = {0, 0, 1}, tb[3] = {0, 1, 0};
-      const uint32_t ring_addr = smem_u32(sRing);
-      TRACE_DECL();
-      TRACE(1, 0);
-      mbar_wait(q_ready, 0);
-      tc_fence_after();
-      TRACE(1, 1);
+  } else if (warp >= 4) {
+    // ===================== consumers: warpgroup wg owns query rows [64 wg, +64) =====================
+    // accumulator layout (tc_common.cuh): this thread holds rows r0 and r0 + 8, columns 8 j + cq + {0, 1}
+    const int wg = (warp - 4) >> 2;
+    const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
+    const int ta[3] = {0, 0, 1}, tb[3] = {0, 1, 0};
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+    float o[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) o[i] = 0.f;
+    if (nc > 0) {
+      const uint32_t q_addr = smem_u32(sQ) + wg * (64 * 128), ring_addr = smem_u32(sRing);
       uint32_t n = 0;                                       // ring sequence number
-      auto release_slot = [&](uint32_t slot) {
-        if (CL > 1) umma_commit_mc(&r_empty[slot], MC_ALL); else umma_commit(&r_empty[slot]);
-      };
-      // score tile of job j (pass A: j < nc, one term; pass B: j = nc + t, all terms) into stage j % NS
-      auto issue_qk = [&](int j) {
-        const uint32_t slot = n % NSLOT, st = (uint32_t)j % NS;
-        const int nterm = j < nc ? 1 : NT;
+      auto acquire = [&]() -> uint32_t {
+        const uint32_t slot = n % NSLOT;
         mbar_wait(&r_full[slot], (n / NSLOT) & 1u);
-        TRACE(1, 1000 + j);
-        const int jp = j - NS;                              // previous user of this stage
-        if (jp >= nc) mbar_wait(&sb_free[st], (uint32_t)((jp - nc) / NS) & 1u);        // its P.V has retired
-        else if (jp >= 0) mbar_wait(&sa_free[st], (uint32_t)(jp / NS) & 1u);           // pass A tile has been read
-        tc_fence_after();
-        TRACE(1, 2000 + j);
-        const uint32_t k_addr = ring_addr + slot * SLOT_BYTES;
-        const uint32_t d_s = tmem_base + TM_S + st * AT_BKEY;
+        return ring_addr + slot * SLOT_BYTES;
+      };
+      auto release = [&]() {                                // after wgmma_wait_all: this warp's MMAs on the slot have retired
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&r_empty[n % NSLOT]);
+        ++n;
+      };
+      // S[64 x 64] = sum over the first nterm terms of Q plane ta . K plane tb^T
+      auto scores = [&](float (&s)[32], uint32_t k_addr, int nterm) {
+        wgmma_fence();
         for (int term = 0; term < nterm; ++term) {
 #pragma unroll
           for (int k = 0; k < AT_D / 16; ++k) {
-            const uint32_t a_t = tmem_base + TM_Q + ta[term] * 64 + k * 8;
-            const uint64_t db = make_sw128_desc(k_addr + (tb[term] * 2 + (k >> 2)) * BOX) + 2 * (k & 3);
-            umma_f16_ts(d_s, a_t, db, idesc_s, (term | k) != 0 ? 1u : 0u);
+            const uint64_t da = make_sw128_desc(q_addr + (ta[term] * 2 + (k >> 2)) * AT_Q_KBLK) + 2 * (k & 3);
+            const uint64_t db = make_sw128_desc(k_addr + (tb[term] * 2 + (k >> 2)) * AT_BOX) + 2 * (k & 3);
+            wgmma_m64n64_ss(s, da, db, (term | k) != 0 ? 1u : 0u);
           }
         }
-        umma_commit(&s_full[st]);
-        release_slot(slot);                                 // K chunk is dead once its score MMAs retire
-        ++n;
+        wgmma_commit();
+        wgmma_wait_all();
+        wgmma_fence_regs(s);
       };
-      auto issue_pv = [&](int t) {
-        const uint32_t slot = n % NSLOT, st = (uint32_t)(nc + t) % NS;
-        mbar_wait(&p_full[st], (uint32_t)(t / NS) & 1u);
-        TRACE(1, 3000 + t);
-        mbar_wait(&r_full[slot], (n / NSLOT) & 1u);
-        tc_fence_after();
-        TRACE(1, 4000 + t);
-        const uint32_t v_addr = ring_addr + slot * SLOT_BYTES;
-        const uint32_t p_t = tmem_base + TM_S + st * AT_BKEY;
-        for (int term = 0; term < NT; ++term) {
-          const uint64_t db = make_sw128_desc(v_addr + tb[term] * 2 * BOX);
-#pragma unroll
-          for (int k = 0; k < AT_BKEY / 16; ++k) {
-            // keys 16k..16k+15 of plane ta: half (k>>1) of the stage, 8 columns per step, lo plane 16 columns after hi
-            const uint32_t a_t = p_t + (k >> 1) * 32 + ta[term] * 16 + (k & 1) * 8;
-            umma_f16_ts(tmem_o, a_t, db + 2 * k, idesc_o, (t | term | k) != 0 ? 1u : 0u);
-          }
-        }
-        umma_commit(&sb_free[st]);
-        release_slot(slot);
-        ++n;
-      };
-      for (int i = 0; i < nc; ++i) issue_qk(i);
-      issue_qk(nc);
-      if (nc > 1) issue_qk(nc + 1);
-      for (int t = 0; t < nc; ++t) {
-        if (t + 2 < nc) issue_qk(nc + t + 2);
-        issue_pv(t);
-      }
-      umma_commit(o_full);
-      TRACE(1, 9);
-    }
-  } else if (warp >= 4) {
-    // ===================== softmax + epilogue: two threads per query row =====================
-    const int qw = warp & 3;                   // TMEM lane quarter this warp may access
-    const int hf = (warp - 4) >> 2;            // column half of a 64-key chunk / of the 128 head dims
-    const int r = qw * 32 + lane;              // row in tile == TMEM lane
-    const uint32_t lane_addr = (uint32_t)(qw * 32) << 16;
-    float m = -INFINITY, l = 0.f;
-#ifdef FA_ATT_TRACE
-    int tr_n = 0; const bool tr_on = (blockIdx.x == 1 && blockIdx.y == 1 && blockIdx.z == gridDim.z / 2) && warp == 4 && lane == 0;
-#endif
-    TRACE(2, 0);
-    if (nc > 0) {
-      // ---- Q planes: shared memory (TMA, SWIZZLE_128B) -> TMEM, this thread's row, head dims [64 hf, 64 hf + 64)
       mbar_wait(q_full, 0);
-#pragma unroll
-      for (int pl = 0; pl < NPL; ++pl) {
-        const unsigned char* qrow = sQ + (pl * 2 + hf) * AT_Q_KBLK + (r >> 3) * 1024 + (r & 7) * 128;
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          uint32_t w[16];
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const uint4 x = *reinterpret_cast<const uint4*>(qrow + (((half * 4 + c) ^ (r & 7)) << 4));
-            w[4 * c] = x.x; w[4 * c + 1] = x.y; w[4 * c + 2] = x.z; w[4 * c + 3] = x.w;
-          }
-          tmem_st_32x16(tmem_base + lane_addr + TM_Q + pl * 64 + hf * 32 + half * 16, w);
-        }
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(q_ready);
-      TRACE(2, 1);
-      // ---- pass A: approximate row max over this thread's 32 columns of every chunk
+      // ---- pass A: approximate row max (softmax is invariant to the choice of m; an approximate maximum only has to keep
+      //      exp(s - m) in range, so the hi . hi term suffices)
       for (int i = 0; i < nc; ++i) {
-        const int st = i % NS;
-        mbar_wait(&s_full[st], (uint32_t)(i / NS) & 1u);
-        tc_fence_after();
-        TRACE(2, 1000 + i);
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + lane_addr + TM_S + st * AT_BKEY + hf * 32, v);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sa_free[st]);           // values are in registers: release the score tile first
-        const int kbase = i * AT_BKEY + hf * 32;
-        if (kbase + 32 <= klen) {                       // whole half-chunk valid (warp-uniform): no per-element predicates
+        float s[32];
+        scores(s, acquire(), 1);
+        release();
+        const int kbase = i * AT_BKEY + cq;
 #pragma unroll
-          for (int jj = 0; jj < 32; ++jj) m = fmaxf(m, __uint_as_float(v[jj]));
-        } else {
+        for (int j = 0; j < 8; ++j)
 #pragma unroll
-          for (int jj = 0; jj < 32; ++jj) if (kbase + jj < klen) m = fmaxf(m, __uint_as_float(v[jj]));
-        }
+          for (int e = 0; e < 2; ++e)
+            if (kbase + 8 * j + e < klen) { m0 = fmaxf(m0, s[4 * j + e]); m1 = fmaxf(m1, s[4 * j + 2 + e]); }
       }
-      s_red[hf * 128 + r] = m;
-      softmax_bar();
-      m = fmaxf(m, s_red[(hf ^ 1) * 128 + r]);     // finite: key 0 is always valid when nc > 0
+#pragma unroll
+      for (int o2 = 1; o2 <= 2; o2 <<= 1) {                 // the four lanes of a quad share a row
+        m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, o2));
+        m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, o2));
+      }
       // probabilities are formed as p' = 2^10 exp(s - m): the common factor cancels in O / l, and it keeps probabilities down to
       // 6e-8 inside the fp16 planes' NORMAL range (p' <= ~1100 with the approximate maximum of pass A; fp16 holds 65504)
-      const float mp = m - 6.931471805599453f;
-      // ---- pass B: probabilities, written back IN PLACE over this thread's 32 score columns as fp16 planes
-      //      (columns [32 hf, +16) = hi plane of keys 32 hf .. 32 hf + 31, the next 16 columns = lo plane): the A operand of P.V
+      const float mp0 = m0 - 6.931471805599453f, mp1 = m1 - 6.931471805599453f;
+      // ---- pass B: S (all terms) -> p -> fp16 planes in registers (the A operand of P.V) -> O += P . V
       for (int t = 0; t < nc; ++t) {
-        const int j = nc + t, st = j % NS;
-        mbar_wait(&s_full[st], (uint32_t)(j / NS) & 1u);
-        tc_fence_after();
-        TRACE(2, 2000 + t);
-        const uint32_t my_cols = tmem_base + lane_addr + TM_S + st * AT_BKEY + hf * 32;
-        uint32_t hi[16], lo[16];
-        {
-          uint32_t v[32];
-          tmem_ld_32x32(my_cols, v);
-          const int kbase = t * AT_BKEY + hf * 32;
-          const bool whole = kbase + 32 <= klen;          // warp-uniform
+        float s[32];
+        scores(s, acquire(), NT);
+        release();
+        uint32_t ph[4][4], plo[4][4];                       // [16-key step][A fragment register]
+        const int kbase = t * AT_BKEY + cq;
 #pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            float a = __expf(__uint_as_float(v[2 * e]) - mp), bb = __expf(__uint_as_float(v[2 * e + 1]) - mp);
-            if (!whole) { a = (kbase + 2 * e < klen) ? a : 0.f; bb = (kbase + 2 * e + 1 < klen) ? bb : 0.f; }
-            l += a;                                        // sequential order (matches the row-sum order of earlier builds)
-            l += bb;
-            // packed conversions to the fp16 planes (tc_common.cuh)
-            hi[e] = pack_planes2(a, bb);
-            if (NPL > 1) {
-              const float2 hv = unpack_planes2(hi[e]);
-              lo[e] = pack_planes2(a - hv.x, bb - hv.y);
-            }
+        for (int j = 0; j < 8; ++j) {
+          const bool v0 = kbase + 8 * j < klen, v1 = kbase + 8 * j + 1 < klen;
+          const float a = v0 ? __expf(s[4 * j] - mp0) : 0.f, bb = v1 ? __expf(s[4 * j + 1] - mp0) : 0.f;
+          const float c = v0 ? __expf(s[4 * j + 2] - mp1) : 0.f, dd = v1 ? __expf(s[4 * j + 3] - mp1) : 0.f;
+          l0 += a; l0 += bb; l1 += c; l1 += dd;
+          const uint32_t h01 = pack_planes2(a, bb), h23 = pack_planes2(c, dd);
+          ph[j >> 1][(j & 1) * 2] = h01;
+          ph[j >> 1][(j & 1) * 2 + 1] = h23;
+          if (NPL > 1) {
+            const float2 u = unpack_planes2(h01), w = unpack_planes2(h23);
+            plo[j >> 1][(j & 1) * 2] = pack_planes2(a - u.x, bb - u.y);
+            plo[j >> 1][(j & 1) * 2 + 1] = pack_planes2(c - w.x, dd - w.y);
           }
         }
-        TRACE(2, 3000 + t);
-        tmem_st_32x16(my_cols, hi);
-        if (NPL > 1) tmem_st_32x16(my_cols + 16, lo);
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[st]);
-        TRACE(2, 5000 + t);
-      }
-      softmax_bar();                   // everyone has read the exchanged maxima before the slots are reused
-      s_red[hf * 128 + r] = l;
-      softmax_bar();
-      l += s_red[(hf ^ 1) * 128 + r];
-      mbar_wait(o_full, 0);
-      tc_fence_after();
-      TRACE(2, 8);
-    }
-    // ---- epilogue: O / l for this warp's 32 rows x 64 head dims, staged through shared memory (the K/V ring is dead once
-    //      o_full has fired) so that the context rows leave as coalesced 8-byte (fp16 planes) / 16-byte (fp32) stores
-    const float inv = l > 0.f ? (1.0f + (float)(nc * (AT_BKEY / 16)) * p.o_scale) / l : 0.f;   // nc key chunks x 4 k-steps were accumulated into O
-    float* stage = reinterpret_cast<float*>(sQ) + (warp - 4) * (32 * 36);
-    const int64_t grow0 = (int64_t)b * p.tq + q0 + qw * 32;
-#pragma unroll 1
-    for (int c0 = hf * 64; c0 < hf * 64 + 64; c0 += 32) {
-      {
-        uint32_t v[32];
-        if (nc > 0) tmem_ld_32x32(tmem_o + lane_addr + c0, v);
-        float* srow = stage + lane * 36;
+        const uint32_t v_addr = acquire();
+        wgmma_fence();
 #pragma unroll
-        for (int jj = 0; jj < 32; jj += 4) {
-          float4 o4;
-          o4.x = nc > 0 ? __uint_as_float(v[jj]) * inv : 0.f;
-          o4.y = nc > 0 ? __uint_as_float(v[jj + 1]) * inv : 0.f;
-          o4.z = nc > 0 ? __uint_as_float(v[jj + 2]) * inv : 0.f;
-          o4.w = nc > 0 ? __uint_as_float(v[jj + 3]) * inv : 0.f;
-          *reinterpret_cast<float4*>(srow + jj) = o4;
+        for (int term = 0; term < NT; ++term) {
+          const uint64_t db = make_sw128_desc(v_addr + tb[term] * 2 * AT_BOX);
+#pragma unroll
+          for (int kk = 0; kk < AT_BKEY / 16; ++kk) wgmma_m64n128_rs(o, ta[term] == 0 ? ph[kk] : plo[kk], db + 2 * kk, 1u);
         }
+        wgmma_commit();
+        wgmma_wait_all();
+        wgmma_fence_regs(o);
+        release();
       }
-      __syncwarp();
-      const int rr0 = lane >> 3, c4 = (lane & 7) * 4;
-      const int col = h * AT_D + c0 + c4;
-      const int rows_ok = p.tq - (q0 + qw * 32);                      // valid rows of this warp's 32
-      float* pc = p.ctx ? p.ctx + (grow0 + rr0) * p.ldc + col : nullptr;
-      plane_t* pp = OPL > 0 ? p.ctx_planes + (grow0 + rr0) * p.ldp + col : nullptr;
-      const int64_t plane = (int64_t)p.batch * p.tq * p.ldp;
-      const float* sp = stage + rr0 * 36 + c4;
-#pragma unroll 2
-      for (int it = 0; it < 8; ++it) {
-        if (it * 4 + rr0 < rows_ok) {
-          const float4 o4 = *reinterpret_cast<const float4*>(sp + it * 4 * 36);
-          if (pc) *reinterpret_cast<float4*>(pc + (int64_t)it * 4 * p.ldc) = o4;
-          if (OPL > 0) {
-            float x0 = o4.x, x1 = o4.y, x2 = o4.z, x3 = o4.w;
-            plane_t* dst = pp + (int64_t)it * 4 * p.ldp;
 #pragma unroll
-            for (int pl = 0; pl < OPL; ++pl) {
-              uint2 pk;
-              pk.x = pack_planes2(x0, x1);
-              pk.y = pack_planes2(x2, x3);
-              *reinterpret_cast<uint2*>(dst) = pk;
-              if (pl + 1 < OPL) {
-                dst += plane;
-                const float2 ua = unpack_planes2(pk.x), ub = unpack_planes2(pk.y);
-                x0 -= ua.x; x1 -= ua.y; x2 -= ub.x; x3 -= ub.y;
-              }
-            }
-          }
-        }
-      }
-      __syncwarp();
-    }
-    TRACE(2, 9);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (CL > 1) cluster_sync_all();      // no CTA exits while a peer may still multicast into it or arrive on its barriers
-  if (warp == 2) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
-}
-
-// ------------------------------------------------------------------------------------------------ persistent variant
-// Same arithmetic, one CTA per SM looping over query tiles (tile = ((b * H + h) * n_qt + qt), round robin over the grid), so that
-// the fixed parts of a tile overlap the neighbouring tiles' tensor work instead of leaving the tensor pipe idle:
-//   * the Q tile of tile i+1 is fetched (TMA) while tile i computes, and moved to TMEM as soon as tile i's last score MMA has retired
-//     (barrier q_free) — i.e. under tile i's last P.V MMAs;
-//   * tile i's epilogue (O / l -> planes) is done by four warps of its own (one per TMEM lane quarter) while the softmax warps and
-//     the tensor pipe are already in tile i+1 (the row sums travel through shared memory, l_full / l_free; O is handed back with
-//     o_free before the first P.V of tile i+1);
-//   * barrier initialisation, TMEM allocation and descriptor prefetch happen once per SM instead of once per tile.
-// In the one-tile-per-CTA kernel those parts (Q load + move 3.7 k, epilogue ~4 k, launch ~1.5 k of ~30 k cycles, in-kernel timeline
-// profiles/r1_attention_timeline_v15.txt) left the tensor pipe at 54 % (ncu).  Shared memory: Q 64 KB, K/V ring 4 x 32 KB, epilogue
-// transpose buffer 9 KB (16 rows per pass).  Every barrier keeps a running phase bit because its uses no longer start at zero.
-// Warps: 0 TMA producer, 1 MMA issuer, 2 TMEM allocator, 4-11 softmax (two threads per query row), 12-15 epilogue.
-template <int NPL, int OPL>
-__global__ void __launch_bounds__(512, 1)
-attention_tcp_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
-                     const __grid_constant__ CUtensorMap map_v, const AttTcParams p, const int n_qt, const int n_tiles) {
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  constexpr uint32_t BOX = 8192;
-  constexpr uint32_t Q_BYTES = NPL * 2 * AT_Q_KBLK;
-  constexpr uint32_t SLOT_BYTES = NPL * 2 * BOX;
-  constexpr int NSLOT = 4, NS = 4;
-  constexpr int NT = NPL == 1 ? 1 : 3;
-  constexpr uint32_t EPI_BYTES = 4 * 16 * 36 * 4;              // 4 epilogue warps x [16 rows][36 floats]
-  constexpr uint32_t TM_Q = 0, TM_S = 128, TM_O = 384;
-  unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  unsigned char* sQ = smem;
-  unsigned char* sRing = sQ + Q_BYTES;
-  float* sEpi = reinterpret_cast<float*>(sRing + NSLOT * SLOT_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<unsigned char*>(sEpi) + EPI_BYTES);
-  uint64_t* q_full = bars;            // TMA -> softmax warps: Q planes in shared memory
-  uint64_t* q_ready = bars + 1;       // softmax warps (8) -> MMA: Q planes in TMEM
-  uint64_t* sq_free = bars + 2;       // softmax warps (8) -> producer: sQ has been read
-  uint64_t* q_free = bars + 3;        // MMA -> softmax warps: every score MMA of the tile has retired (TMEM Q region reusable)
-  uint64_t* o_full = bars + 4;        // MMA -> softmax warps: O complete
-  uint64_t* o_free = bars + 5;        // epilogue warps (4) -> MMA: O has been read
-  uint64_t* r_full = bars + 6;        // [NSLOT]
-  uint64_t* r_empty = r_full + NSLOT; // [NSLOT]
-  uint64_t* s_full = r_empty + NSLOT; // [NS]
-  uint64_t* sa_free = s_full + NS;    // [NS] pass A tile read (8)
-  uint64_t* sb_free = sa_free + NS;   // [NS] P.V retired (1)
-  uint64_t* p_full = sb_free + NS;    // [NS] probabilities written (8)
-  uint64_t* l_full = p_full + NS;     // softmax warps of column half 0 (4) -> epilogue warps: row sums of the tile are in s_l
-  uint64_t* l_free = l_full + 1;      // epilogue warps (4) -> softmax warps: s_l has been read
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(l_free + 1);
-  float* s_red = reinterpret_cast<float*>(l_free + 2);        // [2][128] row max / row sum exchange between the column halves
-  float* s_l = s_red + 256;                                   // [128] final row sums of the tile handed to the epilogue warps
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) { tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_v); }
-  if (warp == 1 && lane == 0) {
-    mbar_init(q_full, 1); mbar_init(q_ready, 8); mbar_init(sq_free, 8); mbar_init(q_free, 1); mbar_init(o_full, 1); mbar_init(o_free, 4);
-    mbar_init(l_full, 4); mbar_init(l_free, 4);
-    for (int s = 0; s < NSLOT; ++s) { mbar_init(&r_full[s], 1); mbar_init(&r_empty[s], 1); }
-    for (int s = 0; s < NS; ++s) { mbar_init(&s_full[s], 1); mbar_init(&sa_free[s], 8); mbar_init(&sb_free[s], 1); mbar_init(&p_full[s], 8); }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  pdl_wait();
-  pdl_trigger();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_o = tmem_base + TM_O;
-
-  // tile -> (utterance, head, first query, valid keys, key chunks); identical in every role
-  auto decode = [&](int tile, int& b, int& h, int& q0, int& klen, int& nc) {
-    const int qt = tile % n_qt, bh = tile / n_qt;
-    h = bh % p.heads; b = bh / p.heads; q0 = qt * AT_BQ;
-    klen = min(p.key_lens[b], p.tk);
-    nc = (klen + AT_BKEY - 1) / AT_BKEY;
-  };
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one_sync()) {
-      uint32_t n = 0, tc = 0;                                 // ring sequence number, tiles with keys so far
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        int b, h, q0, klen, nc;
-        decode(tile, b, h, q0, klen, nc);
-        if (nc == 0) continue;
-        const int bkv = p.kv_shared ? 0 : b;
-        mbar_wait(sq_free, (tc & 1u) ^ 1u);                   // the previous tile's Q has left shared memory
-        mbar_expect_tx(q_full, Q_BYTES);
-#pragma unroll
-        for (int pl = 0; pl < NPL; ++pl)
-#pragma unroll
-          for (int kb = 0; kb < 2; ++kb)
-            tma_load_2d(sQ + (pl * 2 + kb) * AT_Q_KBLK, &map_q, q_full, h * AT_D + kb * 64, (int)(pl * p.q_plane_rows + (int64_t)b * p.tq + q0));
-        ++tc;
-        auto load_chunk = [&](bool is_v, int idx, int nb) {
-          const uint32_t slot = n % NSLOT;
-          mbar_wait(&r_empty[slot], ((n / NSLOT) & 1u) ^ 1u);
-          mbar_expect_tx(&r_full[slot], (uint32_t)nb * BOX);
-          unsigned char* dst = sRing + slot * SLOT_BYTES;
-          for (int bi = 0; bi < nb; ++bi) {
-            const int pl = bi >> 1, sub = bi & 1;
-            if (is_v) tma_load_2d(dst + bi * BOX, &map_v, &r_full[slot], idx * AT_BKEY, (int)(pl * p.v_plane_rows + ((int64_t)bkv * p.heads + h) * AT_D + sub * 64));
-            else tma_load_2d(dst + bi * BOX, &map_k, &r_full[slot], h * AT_D + sub * 64, (int)(pl * p.k_plane_rows + (int64_t)bkv * p.tk + idx * AT_BKEY));
-          }
-          ++n;
-        };
-        for (int i = 0; i < nc; ++i) load_chunk(false, i, 2);            // pass A: hi plane only
-        load_chunk(false, 0, NPL * 2);
-        if (nc > 1) load_chunk(false, 1, NPL * 2);
-        for (int t = 0; t < nc; ++t) {
-          if (t + 2 < nc) load_chunk(false, t + 2, NPL * 2);
-          load_chunk(true, t, NPL * 2);
-        }
+      for (int o2 = 1; o2 <= 2; o2 <<= 1) {
+        l0 += __shfl_xor_sync(0xffffffffu, l0, o2);
+        l1 += __shfl_xor_sync(0xffffffffu, l1, o2);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one_sync()) {
-      constexpr uint32_t idesc_s = make_idesc_f16(AT_BQ, AT_BKEY);
-      constexpr uint32_t idesc_o = make_idesc_f16(AT_BQ, AT_D);
-      const int ta[3] = {0, 0, 1}, tb[3] = {0, 1, 0};
-      const uint32_t ring_addr = smem_u32(sRing);
-      uint32_t n = 0, tc = 0, J = 0;                          // ring sequence, tiles with keys, score jobs so far (stage = J % NS)
-      uint32_t kinds = 0, phA = 0, phB = 0, phP = 0;          // per stage: previous user (2 bits: 1 pass A, 2 pass B), phase bits
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        int b, h, q0, klen, nc;
-        decode(tile, b, h, q0, klen, nc);
-        if (nc == 0) continue;
-        mbar_wait(q_ready, tc & 1u);
-        tc_fence_after();
-        auto issue_qk = [&](int nterm, uint32_t kind) {
-          const uint32_t slot = n % NSLOT, st = J % NS;
-          mbar_wait(&r_full[slot], (n / NSLOT) & 1u);
-          const uint32_t prev = (kinds >> (2 * st)) & 3u;     // the stage's previous user must have released it
-          if (prev == 1u) { mbar_wait(&sa_free[st], (phA >> st) & 1u); phA ^= 1u << st; }
-          else if (prev == 2u) { mbar_wait(&sb_free[st], (phB >> st) & 1u); phB ^= 1u << st; }
-          kinds = (kinds & ~(3u << (2 * st))) | (kind << (2 * st));
-          tc_fence_after();
-          const uint32_t k_addr = ring_addr + slot * SLOT_BYTES;
-          const uint32_t d_s = tmem_base + TM_S + st * AT_BKEY;
-          for (int term = 0; term < nterm; ++term) {
+    // ---- epilogue: O / l -> fp32 context and / or fp16 planes (the A operand of the out-projection GEMM)
+    const float comp = 1.0f + (float)(nc * (AT_BKEY / 16)) * p.o_scale;     // nc key chunks x 4 k-steps were accumulated into O
+    const float inv0 = l0 > 0.f ? comp / l0 : 0.f, inv1 = l1 > 0.f ? comp / l1 : 0.f;
+    const int64_t plane = (int64_t)p.batch * p.tq * p.ldp;
 #pragma unroll
-            for (int k = 0; k < AT_D / 16; ++k) {
-              const uint32_t a_t = tmem_base + TM_Q + ta[term] * 64 + k * 8;
-              const uint64_t db = make_sw128_desc(k_addr + (tb[term] * 2 + (k >> 2)) * BOX) + 2 * (k & 3);
-              umma_f16_ts(d_s, a_t, db, idesc_s, (term | k) != 0 ? 1u : 0u);
-            }
-          }
-          umma_commit(&s_full[st]);
-          umma_commit(&r_empty[slot]);
-          ++n; ++J;
-        };
-        const uint32_t Jb = J + (uint32_t)nc;                 // job number of pass-B chunk 0
-        auto issue_pv = [&](int t) {
-          const uint32_t slot = n % NSLOT, st = (Jb + (uint32_t)t) % NS;
-          mbar_wait(&p_full[st], (phP >> st) & 1u); phP ^= 1u << st;
-          if (t == 0 && tc > 0) mbar_wait(o_free, (tc - 1u) & 1u);      // the previous tile's epilogue has read O
-          mbar_wait(&r_full[slot], (n / NSLOT) & 1u);
-          tc_fence_after();
-          const uint32_t v_addr = ring_addr + slot * SLOT_BYTES;
-          const uint32_t p_t = tmem_base + TM_S + st * AT_BKEY;
-          for (int term = 0; term < NT; ++term) {
-            const uint64_t db = make_sw128_desc(v_addr + tb[term] * 2 * BOX);
+    for (int half = 0; half < 2; ++half) {
+      const int row = q0 + r0 + 8 * half;
+      if (row >= p.tq) continue;
+      const int64_t grow = (int64_t)b * p.tq + row;
+      const float inv = half ? inv1 : inv0;
 #pragma unroll
-            for (int k = 0; k < AT_BKEY / 16; ++k) {
-              const uint32_t a_t = p_t + (k >> 1) * 32 + ta[term] * 16 + (k & 1) * 8;
-              umma_f16_ts(tmem_o, a_t, db + 2 * k, idesc_o, (t | term | k) != 0 ? 1u : 0u);
-            }
-          }
-          umma_commit(&sb_free[st]);
-          umma_commit(&r_empty[slot]);
-          ++n;
-        };
-        for (int i = 0; i < nc; ++i) issue_qk(1, 1u);
-        issue_qk(NT, 2u);
-        if (nc > 1) issue_qk(NT, 2u);
-        if (nc <= 2) umma_commit(q_free);                      // that was the tile's last score MMA
-        for (int t = 0; t < nc; ++t) {
-          if (t + 2 < nc) {
-            issue_qk(NT, 2u);
-            if (t + 3 == nc) umma_commit(q_free);
-          }
-          issue_pv(t);
-        }
-        umma_commit(o_full);
-        ++tc;
-      }
-    }
-  } else if (warp >= 12) {
-    // ===================== epilogue: O / l -> fp16 planes and/or fp32, one warp per TMEM lane quarter =====================
-    const int qw = warp & 3;
-    const uint32_t lane_addr = (uint32_t)(qw * 32) << 16;
-    float* stage = sEpi + qw * (16 * 36);
-    uint32_t tc = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      int b, h, q0, klen, nc;
-      decode(tile, b, h, q0, klen, nc);
-      float inv = 0.f;
-      if (nc > 0) {
-        mbar_wait(l_full, tc & 1u);
-        const float l = s_l[qw * 32 + lane];
-        __syncwarp();
-        if (lane == 0) mbar_arrive(l_free);
-        inv = l > 0.f ? (1.0f + (float)(nc * (AT_BKEY / 16)) * p.o_scale) / l : 0.f;   // nc key chunks x 4 k-steps were accumulated into O
-        mbar_wait(o_full, tc & 1u);
-        tc_fence_after();
-      }
-      const int64_t grow0 = (int64_t)b * p.tq + q0 + qw * 32;
-      const int rows_ok = p.tq - (q0 + qw * 32);
-      const int64_t plane = (int64_t)p.batch * p.tq * p.ldp;
-#pragma unroll 1
-      for (int cg = 0; cg < 4; ++cg) {
-        uint32_t v[32];
-        if (nc > 0) {
-          tmem_ld_32x32(tmem_o + lane_addr + cg * 32, v);
-          if (cg == 3) {                                       // O is in registers: the next tile's P.V may overwrite it
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(o_free);
-          }
-        }
+      for (int j = 0; j < 16; ++j) {
+        float x0 = o[4 * j + 2 * half] * inv, x1 = o[4 * j + 2 * half + 1] * inv;
+        const int col = h * AT_D + 8 * j + cq;
+        if (p.ctx) *reinterpret_cast<float2*>(p.ctx + grow * p.ldc + col) = make_float2(x0, x1);
+        if (OPL > 0) {
+          plane_t* dst = p.ctx_planes + grow * p.ldp + col;
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {                 // 16 rows per pass through the transpose buffer
-          if ((lane >> 4) == half) {
-            float* srow = stage + (lane & 15) * 36;
-#pragma unroll
-            for (int jj = 0; jj < 32; jj += 4) {
-              float4 o4;
-              o4.x = nc > 0 ? __uint_as_float(v[jj]) * inv : 0.f;
-              o4.y = nc > 0 ? __uint_as_float(v[jj + 1]) * inv : 0.f;
-              o4.z = nc > 0 ? __uint_as_float(v[jj + 2]) * inv : 0.f;
-              o4.w = nc > 0 ? __uint_as_float(v[jj + 3]) * inv : 0.f;
-              *reinterpret_cast<float4*>(srow + jj) = o4;
-            }
-          }
-          __syncwarp();
-          const int rr0 = lane >> 3, c4 = (lane & 7) * 4;
-          const int col = h * AT_D + cg * 32 + c4;
-          const float* sp = stage + rr0 * 36 + c4;
-#pragma unroll
-          for (int it = 0; it < 4; ++it) {
-            const int row = half * 16 + it * 4 + rr0;
-            if (row < rows_ok) {
-              const float4 o4 = *reinterpret_cast<const float4*>(sp + it * 4 * 36);
-              if (p.ctx) *reinterpret_cast<float4*>(p.ctx + (grow0 + row) * p.ldc + col) = o4;
-              if (OPL > 0) {
-                float x0 = o4.x, x1 = o4.y, x2 = o4.z, x3 = o4.w;
-                plane_t* dst = p.ctx_planes + (grow0 + row) * p.ldp + col;
-#pragma unroll
-                for (int pl = 0; pl < OPL; ++pl) {
-                  uint2 pk;
-                  pk.x = pack_planes2(x0, x1);
-                  pk.y = pack_planes2(x2, x3);
-                  *reinterpret_cast<uint2*>(dst) = pk;
-                  if (pl + 1 < OPL) {
-                    dst += plane;
-                    const float2 ua = unpack_planes2(pk.x), ub = unpack_planes2(pk.y);
-                    x0 -= ua.x; x1 -= ua.y; x2 -= ub.x; x3 -= ub.y;
-                  }
-                }
-              }
-            }
-          }
-          __syncwarp();
-        }
-      }
-      if (nc > 0) ++tc;
-    }
-  } else if (warp >= 4) {
-    // ===================== softmax: two threads per query row =====================
-    const int qw = warp & 3, hf = (warp - 4) >> 2;
-    const int r = qw * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(qw * 32) << 16;
-    uint32_t tc = 0, J = 0, phS = 0;                          // tiles with keys, score jobs, s_full phase bits
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      int b, h, q0, klen, nc;
-      decode(tile, b, h, q0, klen, nc);
-      if (nc == 0) continue;                                   // the epilogue warps write the zero rows
-      // ---- Q planes: shared memory -> TMEM (this thread's row, head dims [64 hf, +64)) once the previous tile's score MMAs are done
-      mbar_wait(q_full, tc & 1u);
-      if (tc > 0) { mbar_wait(q_free, (tc - 1u) & 1u); tc_fence_after(); }
-#pragma unroll
-      for (int pl = 0; pl < NPL; ++pl) {
-        const unsigned char* qrow = sQ + (pl * 2 + hf) * AT_Q_KBLK + (r >> 3) * 1024 + (r & 7) * 128;
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          uint32_t w[16];
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const uint4 x = *reinterpret_cast<const uint4*>(qrow + (((half * 4 + c) ^ (r & 7)) << 4));
-            w[4 * c] = x.x; w[4 * c + 1] = x.y; w[4 * c + 2] = x.z; w[4 * c + 3] = x.w;
-          }
-          tmem_st_32x16(tmem_base + lane_addr + TM_Q + pl * 64 + hf * 32 + half * 16, w);
-        }
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) { mbar_arrive(q_ready); mbar_arrive(sq_free); }
-      float m = -INFINITY, l = 0.f;
-      // ---- pass A: approximate row max
-      for (int i = 0; i < nc; ++i) {
-        const uint32_t st = J % NS;
-        mbar_wait(&s_full[st], (phS >> st) & 1u); phS ^= 1u << st;
-        tc_fence_after();
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + lane_addr + TM_S + st * AT_BKEY + hf * 32, v);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sa_free[st]);
-        const int kbase = i * AT_BKEY + hf * 32;
-        if (kbase + 32 <= klen) {
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj) m = fmaxf(m, __uint_as_float(v[jj]));
-        } else {
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj) if (kbase + jj < klen) m = fmaxf(m, __uint_as_float(v[jj]));
-        }
-        ++J;
-      }
-      s_red[hf * 128 + r] = m;
-      softmax_bar();
-      m = fmaxf(m, s_red[(hf ^ 1) * 128 + r]);
-      const float mp = m - 6.931471805599453f;
-      // ---- pass B: probabilities in place (see attention_tc_kernel)
-      for (int t = 0; t < nc; ++t) {
-        const uint32_t st = J % NS;
-        mbar_wait(&s_full[st], (phS >> st) & 1u); phS ^= 1u << st;
-        tc_fence_after();
-        const uint32_t my_cols = tmem_base + lane_addr + TM_S + st * AT_BKEY + hf * 32;
-        uint32_t hi[16], lo[16];
-        {
-          uint32_t v[32];
-          tmem_ld_32x32(my_cols, v);
-          const int kbase = t * AT_BKEY + hf * 32;
-          const bool whole = kbase + 32 <= klen;
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            float a = __expf(__uint_as_float(v[2 * e]) - mp), bb = __expf(__uint_as_float(v[2 * e + 1]) - mp);
-            if (!whole) { a = (kbase + 2 * e < klen) ? a : 0.f; bb = (kbase + 2 * e + 1 < klen) ? bb : 0.f; }
-            l += a;
-            l += bb;
-            hi[e] = pack_planes2(a, bb);
-            if (NPL > 1) {
-              const float2 hv = unpack_planes2(hi[e]);
-              lo[e] = pack_planes2(a - hv.x, bb - hv.y);
+          for (int pl = 0; pl < OPL; ++pl) {
+            const uint32_t pk = pack_planes2(x0, x1);
+            *reinterpret_cast<uint32_t*>(dst) = pk;
+            if (pl + 1 < OPL) {
+              dst += plane;
+              const float2 u = unpack_planes2(pk);
+              x0 -= u.x; x1 -= u.y;
             }
           }
         }
-        tmem_st_32x16(my_cols, hi);
-        if (NPL > 1) tmem_st_32x16(my_cols + 16, lo);
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[st]);
-        ++J;
       }
-      softmax_bar();                   // everyone has read the exchanged maxima before the slots are reused
-      s_red[hf * 128 + r] = l;
-      softmax_bar();
-      if (hf == 0) {                   // row sums to the epilogue warps (which have consumed the previous tile's by now)
-        l += s_red[128 + r];
-        if (tc > 0) mbar_wait(l_free, (tc - 1u) & 1u);
-        s_l[r] = l;
-        __syncwarp();
-        if (lane == 0) mbar_arrive(l_full);
-      }
-      ++tc;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
 }
 
 // V [B, tk, ldv] (head h at column h*128) -> Vt planes [npl][B*H*128][tkp] (keys contiguous), via a 64x64 smem transpose.
@@ -858,49 +326,14 @@ int attention_tc_launch(const float* q, int64_t ldq, const float* k, int64_t ldk
   return attention_tc_planes_launch(qp, kp, vt, key_lens, batch, heads, tq, tk, ctx, ldc, ctx_planes, ldp, out_nplanes, mode, st, kv_shared);
 }
 
-template <int NPL, int OPL, int CL>
-static int launch_att_c(dim3 grid, const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttTcParams& p, cudaStream_t st) {
-  constexpr size_t smem = (size_t)NPL * (2 * AT_Q_KBLK + 5 * 2 * 8192) + 1024 + 256 + 1024 + 256;
-  static PerDeviceOnce once;
-  FA_RETURN_IF_ERR(ensure_dyn_smem(attention_tc_kernel<NPL, OPL, CL>, smem, once));
-  FA_CUDA_OK(launch_pdl(attention_tc_kernel<NPL, OPL, CL>, grid, dim3(384), smem, st, CL, mq, mk, mv, p));
-  return FA_OK;
-}
-
-// cluster size along the query-tile axis: the largest of {4, 2, 1} that divides the number of query tiles and does not exceed
-// FA_ATT_CLUSTER.  Default 1: measured on B200 (B=64, H=4, T=500) the multicast variants are SLOWER (fa_attention_tc 207 us
-// at CL=1, 215 us at CL=2, 232 us at CL=4) — the kernel is not L2-bandwidth bound and clusters of 4 quantise badly on the
-// 18/20-SM GPCs; the path stays as an opt-in for shapes with many query tiles per (utterance, head).
-static int att_cluster_cap() {
-  static const int v = [] { const char* e = getenv("FA_ATT_CLUSTER"); const int c = e ? atoi(e) : 1; return (c == 2 || c == 4) ? c : 1; }();
-  return v;
-}
-
-// The persistent kernel (one CTA per SM looping over query tiles) is the default: 98.4 us against 106.0 us per encoder layer at
-// B = 64, T = 500 (ncu launch lists of the same build, profiles/README.md).  FA_ATT_PERSIST=0: one CTA per query tile (A/B runs).
-static bool att_persistent() {
-  static const bool on = [] { const char* e = getenv("FA_ATT_PERSIST"); return !(e && e[0] == '0'); }();
-  return on;
-}
-
-template <int NPL, int OPL>
-static int launch_att_p(dim3 grid, const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttTcParams& p, cudaStream_t st) {
-  constexpr size_t smem = (size_t)NPL * (2 * AT_Q_KBLK + 4 * 2 * 8192) + 4 * 16 * 36 * 4 + 2048 + 1024;
-  static PerDeviceOnce once;
-  FA_RETURN_IF_ERR(ensure_dyn_smem(attention_tcp_kernel<NPL, OPL>, smem, once));
-  const int n_qt = (int)grid.x, n_tiles = (int)(grid.x * grid.y * grid.z);
-  const int ctas = n_tiles < sm_count() ? n_tiles : sm_count();
-  FA_CUDA_OK(launch_pdl(attention_tcp_kernel<NPL, OPL>, dim3(ctas), dim3(512), smem, st, 1, mq, mk, mv, p, n_qt, n_tiles));
-  return FA_OK;
-}
-
 template <int NPL, int OPL>
 static int launch_att(dim3 grid, const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttTcParams& p, cudaStream_t st) {
-  if (att_persistent()) return launch_att_p<NPL, OPL>(grid, mq, mk, mv, p, st);
-  const int cap = att_cluster_cap();
-  if (cap >= 4 && grid.x % 4 == 0) return launch_att_c<NPL, OPL, 4>(grid, mq, mk, mv, p, st);
-  if (cap >= 2 && grid.x % 2 == 0) return launch_att_c<NPL, OPL, 2>(grid, mq, mk, mv, p, st);
-  return launch_att_c<NPL, OPL, 1>(grid, mq, mk, mv, p, st);
+  constexpr size_t smem = (size_t)NPL * 2 * AT_Q_KBLK + (size_t)AT_NSLOT(NPL) * NPL * 2 * AT_BOX + 1024 + (1 + 2 * AT_NSLOT(NPL)) * 8;
+  static_assert(smem <= 227 * 1024, "shared memory per block");
+  static PerDeviceOnce once;
+  FA_RETURN_IF_ERR(ensure_dyn_smem(attention_tc_kernel<NPL, OPL>, smem, once));
+  FA_CUDA_OK(launch_pdl(attention_tc_kernel<NPL, OPL>, grid, dim3(384), smem, st, 1, mq, mk, mv, p));
+  return FA_OK;
 }
 
 // Operand planes already in place (written by the producing GEMMs' epilogues, gemm_tc.cu AttnSinks):
@@ -945,13 +378,6 @@ int attention_tc_planes_launch(const plane_t* qp, const plane_t* kp, const plane
 
 }  // namespace fa
 
-#ifdef FA_ATT_TRACE
-extern "C" int fa_debug_att_trace(long long* host_out /* [3][512] */, int* counts /* [3] */) {
-  if (cudaMemcpyFromSymbol(host_out, fa::g_att_trace, sizeof(long long) * 3 * 512) != cudaSuccess) return -1;
-  if (cudaMemcpyFromSymbol(counts, fa::g_att_cnt, sizeof(int) * 3) != cudaSuccess) return -1;
-  return 0;
-}
-#endif
 
 extern "C" size_t fa_attention_tc_workspace_bytes(int32_t batch, int32_t heads, int32_t tq, int32_t tk, int32_t gemm_mode) {
   return fa::attention_tc_scratch_bytes(batch, heads, tq, tk, gemm_mode);

@@ -1,10 +1,12 @@
 #!/bin/bash
-# Builds libfunasr_b200.so in-tree for sm_100a (cross-compiles without a GPU).
+# Builds libfunasr_b200.so in-tree for sm_90a (cross-compiles without a GPU).
 set -e
 cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v --expt-relaxed-constexpr"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v --expt-relaxed-constexpr"
 mkdir -p ../_build
+# objects built with other flags (another architecture) are stale even when newer than their sources
+if [ "$(cat ../_build/flags 2>/dev/null)" != "$FLAGS" ]; then rm -f ../_build/*.o; echo "$FLAGS" > ../_build/flags; fi
 objs=""
 pids=""
 for f in fbank layernorm gemm_f32 gemm_tc attention_tc attention_f32 fsmn cif decode_ops model offline lstm resample vad; do
@@ -32,5 +34,5 @@ if [ ! -f ../_build/host_ops.o ] || [ host_ops.cpp -nt ../_build/host_ops.o ] ||
 fi
 objs="$objs ../_build/host_ops.o"
 for p in $pids; do wait $p || exit 1; done
-$NVCC -gencode arch=compute_100a,code=sm_100a -shared -o ../libfunasr_b200.so $objs -lcudart
+$NVCC -gencode arch=compute_90a,code=sm_90a -shared -o ../libfunasr_b200.so $objs -lcudart
 echo "built $(cd ..; pwd)/libfunasr_b200.so"

@@ -1,4 +1,4 @@
-// Shared helpers for the funasr_b200 sm_100a kernels.
+// Shared helpers for the funasr_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -43,7 +43,7 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 
 // Programmatic dependent launch (PDL): every hot kernel is launched with programmaticStreamSerialization, runs its
-// global-memory-free prologue (barrier init, TMEM alloc, descriptor prefetch) while the previous kernel in the stream drains,
+// global-memory-free prologue (barrier init, descriptor prefetch) while the previous kernel in the stream drains,
 // then pdl_wait() — which returns once the predecessor grid has completed and its writes are visible — before the first
 // global access, and immediately lets its own successor start its prologue (pdl_trigger).  FA_PDL=0 disables the attribute.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -89,10 +89,10 @@ inline int ensure_dyn_smem(K kern, size_t bytes, PerDeviceOnce& once) {
 inline int sm_count() {
   static std::atomic<int> cache[32];
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   int n = cache[dev & 31].load(std::memory_order_relaxed);
   if (n <= 0) {
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cache[dev & 31].store(n, std::memory_order_relaxed);
   }
   return n;

@@ -1,6 +1,6 @@
 // Output-side kernels of the greedy decode: row arg-max with log-sum-exp (log_softmax value of the arg-max,
 // paraformer/model.py:345,642-644), optional in-place log_softmax of the full logits for parity checks, the
-// {blank,sos,eos} filter (:655-666), and the fp32 -> fp16 plane split used by the tcgen05 GEMM weights.
+// {blank,sos,eos} filter (:655-666), and the fp32 -> fp16 plane split used by the tensor-core GEMM weights.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include <math.h>

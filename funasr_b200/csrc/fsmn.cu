@@ -241,7 +241,7 @@ int fsmn_tma_launch(const float* v, int64_t ldv, const int32_t* lens, int batch,
   return fsmn_tma_launch_k<21>(v, ldv, lens, batch, t_max, channels, w, res, ldr, out, ldo, st);
 }
 
-// default on since the round-2 A/B (48.1 -> 39.9 us at the encoder shape, profiles/r2_fsmn_tma_ab.json); FA_FSMN_TMA=0 = SIMT strips only
+// the TMA-staged kernel is the default (tools/fsmn_probe.py compares the two); FA_FSMN_TMA=0 = SIMT strips only
 int fsmn_simt_launch(const float* v, int64_t ldv, const int32_t* lens, int batch, int t_max, int channels, const float* w,
                      int ksize, const float* res, int64_t ldr, float* out, int64_t ldo, cudaStream_t st, int causal);
 

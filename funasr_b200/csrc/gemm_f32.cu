@@ -2,7 +2,7 @@
 //
 // This is the parity-reference contraction path (FA_GEMM_F32_SIMT): plain FFMA accumulation in fp32, the
 // arithmetic closest to the reference's MKL/cuBLAS sgemm (attention.py:256,306; positionwise_feed_forward.py:34).
-// The tcgen05 path (gemm_tc.cu) is validated against it on the device.
+// The tensor-core path (gemm_tc.cu) is validated against it on the device.
 // 128x128x16 tiles, 256 threads, 8x8 outputs per thread, register-prefetch double buffering.
 #include "common.cuh"
 

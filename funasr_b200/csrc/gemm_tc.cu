@@ -1,22 +1,19 @@
-// tcgen05 / TMEM / TMA GEMM with fp16 operand splitting and a fused nn.Linear epilogue (sm_100a only).
+// wgmma / TMA GEMM with fp16 operand splitting and a fused nn.Linear epilogue (sm_90a).
 //
 //   Y[M,N] = act( sum_{(p,q) in terms} A_p[M,K] * W_q[N,K]^T + b ) (+ res1) (+ res2)
 //
 // A_p / W_q are the fp16 planes of the fp32 operands (x = hi + mid + lo, made by split kernels), accumulation is
-// fp32 in TMEM.  Modes: F16X1 = {(0,0)} (fast), F16X3 = {(0,0),(0,1),(1,0)} (~2^-17 relative, the default
+// fp32 in registers.  Modes: F16X1 = {(0,0)} (fast), F16X3 = {(0,0),(0,1),(1,0)} (~2^-17 relative, the default
 // parity mode on tensor cores), F16X6 = X3 + {(1,1),(0,2),(2,0)} (~fp32).  This replaces the torch.nn.Linear calls
 // of the hot path (sanm/attention.py:256,306, transformer/positionwise_feed_forward.py:34,
 // sanm/positionwise_feed_forward.py:33, paraformer/decoder.py:444, cif conv as GEMM).
 //
-// Structure (one persistent CTA per SM, 256 threads):
-//   warp 0 : TMA producer  — cp.async.bulk.tensor.2d (SWIZZLE_128B) of the A/W plane tiles into a smem ring
-//   warp 1 : MMA issuer    — one elected thread issues tcgen05.mma.cta_group::1.kind::f16 (128xBNx16) per K=16
-//                            slice and per split term; tcgen05.commit releases ring slots / publishes accumulators
-//   warp 2 : TMEM allocator (2 accumulators x BN columns, double buffered so the epilogue of tile i overlaps
-//            the MMAs of tile i+1)
-//   warps 4-7 : epilogue   — tcgen05.ld (32 lanes x 32 columns per warp and step) -> bias/ReLU/residuals ->
-//            fp32 rows to HBM, or fp16 planes for a following GEMM.
-// Tensor-pipe bound when operand tiles are reused from L2; roofline notes in DESIGN.md.
+// Structure (one persistent CTA per SM, 384 threads, 128 x BN output tiles):
+//   warp 0     : TMA producer — cp.async.bulk.tensor.2d (SWIZZLE_128B) of the A/W plane tiles into a shared-memory ring
+//   warps 4-11 : two consumer warpgroups — each issues wgmma.mma_async m64nBNk16 for its 64 rows per K=16 slice and per split
+//                term (both operands from shared memory), keeping one k-block of MMAs in flight while the producer refills the
+//                ring; the accumulators are then parked in a shared-memory tile and the same eight warps run the epilogue
+//                (bias/ReLU/residuals -> fp32 rows to HBM, or fp16 planes for a following GEMM).
 #include "common.cuh"
 #include "kernels.h"
 #include "tc_common.cuh"
@@ -25,9 +22,9 @@
 
 namespace fa {
 
-constexpr int TC_BM = 128;      // UMMA M (cta_group::1)
+constexpr int TC_BM = 128;      // tile rows: two consumer warpgroups of wgmma M = 64
 constexpr int TC_BK = 64;       // one 128-byte swizzle span of fp16
-constexpr int TC_UK = 16;       // UMMA K for 16-bit inputs
+constexpr int TC_UK = 16;       // wgmma K for 16-bit inputs
 constexpr uint32_t TC_TILE_BYTES_A = TC_BM * TC_BK * 2;   // 16 KB per plane tile
 
 // ------------------------------------------------------------------------------------------------ kernel
@@ -45,16 +42,11 @@ struct TcParams {
   plane_t* out_planes;             // fp16 plane output [3][M][ldo] (or null)
   int64_t ldo; int out_nplanes;
   int tiles_m, tiles_n;
-  // cta_group::2 kernel only — schedule of the 256 x 256 pair tiles over the P CTA pairs: full_rounds rounds of P whole tiles, then
-  // the tail_tiles leftover tiles cut into tail_sub (1 | 2 | 4) column slices of 256 / tail_sub so that the last, partial wave
-  // costs ceil(tail_tiles * tail_sub / P) / tail_sub of a round instead of a whole one (gemm_tc2_kernel, pick_tail_sub)
-  int full_rounds, tail_tiles, tail_sub;
   AttnSinks att;                          // optional: route column ranges to attention operand planes
-  // tcgen05 accumulates in fp32 with round-toward-zero: every 16-wide k-step shrinks the running sum by a fraction of an ulp, a
-  // SYSTEMATIC relative error that grows linearly in K (tools/noise_probe.py, Gaussian data: -1.70e-6 at K = 512 and -6.35e-6 at
-  // K = 2048 with the x3 split, identical with x6; -1.10e-6 at K = 512 single pass; the fp32 SIMT GEMM shows -3e-10).  The epilogue
-  // multiplies the accumulator by 1 + (K / 16) * c (c = 5.3e-8 per k-step for the split modes, 3.4e-8 for one pass) before the
-  // bias: the expected shrink is undone, what remains is the random part (~1e-6).  FA_RZ_COMP=0 disables it (A/B).
+  // The tensor cores accumulate in fp32 with truncation: every 16-wide k-step shrinks the running sum by a fraction of an ulp, a
+  // SYSTEMATIC relative error that grows linearly in K (tools/noise_probe.py measures it against the fp32 SIMT GEMM).  The epilogue
+  // multiplies the accumulator by 1 + (K / 16) * c (rz_comp_scale; c measured on an H100, DESIGN.md §2) before the bias: the expected
+  // shrink is undone, what remains is the random part.  FA_RZ_COMP=0 disables it (A/B).
   float acc_scale;
 };
 
@@ -67,33 +59,28 @@ static float rz_comp_scale(int kp, int n_terms) {
 __constant__ int c_term_a[6] = {0, 0, 1, 1, 0, 2};
 __constant__ int c_term_w[6] = {0, 1, 0, 1, 2, 0};
 
-// Epilogue of one accumulator tile.  Eight epilogue warps per CTA (two per SM sub-partition, so one warp's TMEM / shared /
-// global latencies are hidden by the other): warp w drains TMEM lane quarter w%4 and every second 16-column chunk.
-//   phase 1  tcgen05.ld 32x32b.x16 (thread = row) -> raw fp32 accumulators into a padded shared-memory tile [32][20]
+// Epilogue of one accumulator tile.  Eight epilogue warps per CTA (two per SM sub-partition, so one warp's shared / global
+// latencies are hidden by the other): warp w drains rows [32 (w%4), +32) of the accumulator tile, every second 16-column chunk.
+//   phase 1  row-per-thread read of 16 fp32 accumulators -> a padded per-warp shared-memory tile [32][20]
 //   phase 2  re-read with the warp laid out as 8 rows x 4 float4 columns, so bias / residual loads and every store are
 //            coalesced 16-byte (fp32) or 8-byte (fp16 plane) accesses; V columns of the attention sink take a
 //            column-per-lane path that writes the per-head transposed planes as 4 consecutive keys (8 bytes) per store.
-// History (profiles/README.md): v1 stored straight from the row-per-thread layout (4-byte stores to 32 lines per
-// instruction); v2 staged through smem but kept 4 epilogue warps and measured SLOWER — ncu showed tensor pipe 17-25 %,
-// warps_active 12 %, 12-36 cycles per issued instruction: the epilogue was instruction-latency bound, not store bound.
 constexpr int EPI_CH = 16;                       // columns per chunk
 constexpr int EPI_LD = 20;                       // padded row pitch (floats): 16-byte aligned, conflict-free float4 phases
 constexpr int EPI_WARP_FLOATS = 32 * EPI_LD;     // 2.5 KB per epilogue warp
 constexpr int EPI_WARPS = 8;
 
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// 32 rows (thread = row) x 16 consecutive fp32 columns of the shared-memory accumulator tile -> 16 registers
+__device__ __forceinline__ void acc_ld_32x16(const float* src, uint32_t (&r)[16]) {
+#pragma unroll
+  for (int j = 0; j < 16; j += 4) {
+    const uint4 v = *reinterpret_cast<const uint4*>(src + j);
+    r[j] = v.x; r[j + 1] = v.y; r[j + 2] = v.z; r[j + 3] = v.w;
+  }
 }
 
 // x = hi + mid + lo split of 4 values into fp16 planes: packed converts (cvt.rn.satfinite.f16x2.f32), packed unpack.  NPL is a compile-
-// time constant: with a runtime plane count the loop compiled to a branchy 4x-unrolled body (ncu: 47 % of all executed
-// instructions of the FFN-w_1 GEMM sat in this function).
+// time constant: with a runtime plane count the loop compiles to a branchy 4x-unrolled body.
 template <int NPL>
 __device__ __forceinline__ void store_planes4(plane_t* dst, int64_t plane_stride, float x0, float x1, float x2, float x3) {
 #pragma unroll
@@ -133,8 +120,7 @@ __device__ __forceinline__ void store_vt16(plane_t* dst, int64_t t_pad, int64_t 
 // so groups of four consecutive keys stay inside one utterance and are 8-byte aligned in the transposed planes): the warp's
 // 32 x 16 chunk is staged at pitch 17 (conflict free for the row-per-lane writes AND for the column reads below), then lane
 // (g = lane & 7, c = lane >> 3) packs keys 4g..4g+3 of columns c, c+4, c+8, c+12 and stores 8 bytes per plane — 8 store
-// instructions per lane and chunk instead of 32 two-byte ones (ncu of the QKV GEMM, round 2: the V third of the tiles spent
-// ~180 instructions per chunk in store_vt16 and its tensor pipe sat at 74 % against 89 % for the plane-emitting FFN w_1).
+// instructions per lane and chunk instead of 32 two-byte ones.
 constexpr int VT_LD = 17;
 template <int NPL>
 __device__ __forceinline__ void store_vt_staged(plane_t* __restrict__ dst_g /* this lane's key group, column 0 of the chunk */, int64_t t_pad,
@@ -175,10 +161,9 @@ __device__ __forceinline__ void store_vt_staged(plane_t* __restrict__ dst_g /* t
 constexpr int EPI_F32 = 0, EPI_PLANES = 1, EPI_ATT = 2, EPI_F32R2 = 3;
 
 // fp32-output interior tiles: the residual rows do not depend on the accumulator, so their loads are software pipelined one
-// chunk ahead and the first chunk's are issued BEFORE waiting for the accumulator (out-projection / FFN-w_2 epilogues were
-// bound by memory-level parallelism: 8 warps x 8 float4 loads in flight per SM sustain ~4 TB/s, measured 262 MB in 66 us).
-__device__ __forceinline__ void epilogue_fast_f32(const TcParams& p, const int BN, uint32_t tmem_acc, int64_t row0, int tile_col0, float* stage, int lane,
-                                                  int half, uint64_t* full_bar, uint32_t full_phase) {
+// chunk ahead (out-projection / FFN-w_2 epilogues are bound by memory-level parallelism).
+__device__ __forceinline__ void epilogue_fast_f32(const TcParams& p, const int BN, const float* acc, int64_t row0, int tile_col0, float* stage, int lane,
+                                                  int half) {
   const int rr0 = lane >> 2, c4 = (lane & 3) * 4;
   const int64_t rfirst = row0 + rr0;
   float* srow = stage + lane * EPI_LD;
@@ -198,8 +183,6 @@ __device__ __forceinline__ void epilogue_fast_f32(const TcParams& p, const int B
     }
   };
   prefetch(half * EPI_CH);
-  mbar_wait(full_bar, full_phase);
-  tc_fence_after();
 #pragma unroll 2
   for (int c0 = half * EPI_CH; c0 < BN; c0 += 2 * EPI_CH) {
     float4 rv1[4], rv2[4];
@@ -208,7 +191,7 @@ __device__ __forceinline__ void epilogue_fast_f32(const TcParams& p, const int B
     if (c0 + 2 * EPI_CH < BN) prefetch(c0 + 2 * EPI_CH);
     {
       uint32_t r[16];
-      tmem_ld_32x16(tmem_acc + c0, r);
+      acc_ld_32x16(acc + lane * (BN + 4) + c0, r);
 #pragma unroll
       for (int j = 0; j < 16; j += 4) *reinterpret_cast<uint4*>(srow + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
     }
@@ -233,12 +216,9 @@ __device__ __forceinline__ void epilogue_fast_f32(const TcParams& p, const int B
 
 // The same for at most ONE residual (every fp32-output GEMM of the model: out-projection + x, FFN w_2 + x): the registers the second
 // residual's pipeline would hold become a 5-deep ring of the first's, so each warp keeps five 16-column chunks (10 KB) of residual
-// rows in flight instead of one.  Measured: out-projection (K = 512, alone, L2 flushed) 63.9 us with one chunk in flight, 60.6 with
-// three, 57.3 with five, 46.1 WITHOUT its residual stream — so only part of the gap to the 26 us MMA floor was memory-level
-// parallelism; the rest is the L2 -> SM bandwidth the operand tiles (512 KB per tile and CTA for K = 512) and the fp32 rows
-// (256 KB in + out) share: 386 MB in 57 us = 6.8 TB/s (tools/gemm_shapes.py, profiles/r2_gemm_shapes_*.json).
-__device__ __forceinline__ void epilogue_fast_f32_r1(const TcParams& p, const int BN, uint32_t tmem_acc, int64_t row0, int tile_col0, float* stage,
-                                                     int lane, int half, uint64_t* full_bar, uint32_t full_phase) {
+// rows in flight instead of one.
+__device__ __forceinline__ void epilogue_fast_f32_r1(const TcParams& p, const int BN, const float* acc, int64_t row0, int tile_col0, float* stage,
+                                                     int lane, int half) {
   const int rr0 = lane >> 2, c4 = (lane & 3) * 4;
   const int64_t rfirst = row0 + rr0;
   float* srow = stage + lane * EPI_LD;
@@ -257,16 +237,14 @@ __device__ __forceinline__ void epilogue_fast_f32_r1(const TcParams& p, const in
   };
 #pragma unroll
   for (int i = 0; i < RING; ++i)
-    if (cb + 32 * i < BN) fetch(ring[i], cb + 32 * i);              // issued BEFORE waiting for the accumulator
-  mbar_wait(full_bar, full_phase);
-  tc_fence_after();
+    if (cb + 32 * i < BN) fetch(ring[i], cb + 32 * i);
 #pragma unroll
   for (int i = 0; i < 8; ++i) {                                      // BN <= 256: at most 8 chunks per warp
     const int c0 = cb + 32 * i;
     if (c0 < BN) {
       {
         uint32_t r[16];
-        tmem_ld_32x16(tmem_acc + c0, r);
+        acc_ld_32x16(acc + lane * (BN + 4) + c0, r);
 #pragma unroll
         for (int j = 0; j < 16; j += 4) *reinterpret_cast<uint4*>(srow + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
       }
@@ -294,7 +272,7 @@ __device__ __forceinline__ void epilogue_fast_f32_r1(const TcParams& p, const in
 // Interior tiles (all 32 rows and all BN columns in range): straight-line code, no bounds predicates, every row base
 // computed once per tile and advanced by constant strides.
 template <int EPI, int NPL>
-__device__ __forceinline__ void epilogue_fast(const TcParams& p, const int BN, uint32_t tmem_acc, int64_t row0, int tile_col0, float* stage, int lane,
+__device__ __forceinline__ void epilogue_fast(const TcParams& p, const int BN, const float* acc, int64_t row0, int tile_col0, float* stage, int lane,
                                               int half) {
   const AttnSinks& a = p.att;
   constexpr int QPL = NPL < 2 ? NPL : 2;             // attention operands carry at most two planes
@@ -330,7 +308,7 @@ __device__ __forceinline__ void epilogue_fast(const TcParams& p, const int BN, u
     const bool v_sink = EPI == EPI_ATT && col0 >= a.v0 && col0 < a.v0 + a.width;
     {
       uint32_t r[16];
-      tmem_ld_32x16(tmem_acc + c0, r);
+      acc_ld_32x16(acc + lane * (BN + 4) + c0, r);
       if (EPI == EPI_ATT && v_sink && vt_staged) {
         float x[16];
 #pragma unroll
@@ -416,7 +394,7 @@ __device__ __forceinline__ void epilogue_fast(const TcParams& p, const int BN, u
 
 // Edge tiles (row tail of M, ragged N such as vocab 8404 / 25055): every access bounds checked.
 template <int EPI, int NPL>
-__device__ __noinline__ void epilogue_edge(const TcParams& p, const int BN, uint32_t tmem_acc, int64_t row0, int tile_col0, float* stage, int lane,
+__device__ __noinline__ void epilogue_edge(const TcParams& p, const int BN, const float* acc, int64_t row0, int tile_col0, float* stage, int lane,
                                            int half) {
   const AttnSinks& a = p.att;
   constexpr int QPL = NPL < 2 ? NPL : 2;
@@ -425,7 +403,7 @@ __device__ __noinline__ void epilogue_edge(const TcParams& p, const int BN, uint
     const int col0 = tile_col0 + c0;
     {
       uint32_t r[16];
-      tmem_ld_32x16(tmem_acc + c0, r);
+      acc_ld_32x16(acc + lane * (BN + 4) + c0, r);
       float* srow = stage + lane * EPI_LD;
 #pragma unroll
       for (int j = 0; j < 16; j += 4) *reinterpret_cast<uint4*>(srow + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
@@ -492,24 +470,28 @@ __device__ __noinline__ void epilogue_edge(const TcParams& p, const int BN, uint
   }
 }
 
-// BN: columns of this accumulator tile (a compile-time constant in the single-CTA kernel; 256 / 128 / 64 in the pair kernel)
+// BN: columns of this accumulator tile; acc: the warp's first row of the accumulator tile in shared memory (pitch BN + 4)
 template <int EPI, int NPL>
-__device__ __forceinline__ void epilogue_warp(const TcParams& p, const int BN, uint32_t tmem_acc, int64_t row0, int tile_col0, float* stage, int lane,
-                                              int half, uint64_t* full_bar, uint32_t full_phase) {
+__device__ __forceinline__ void epilogue_warp(const TcParams& p, const int BN, const float* acc, int64_t row0, int tile_col0, float* stage, int lane,
+                                              int half) {
   constexpr int EPIB = EPI == EPI_F32R2 ? EPI_F32 : EPI;
   const bool interior = row0 + 32 <= p.M && tile_col0 + BN <= p.N;
-  if (EPI == EPI_F32 && interior) {                                                                  // both wait for the accumulator themselves
-    epilogue_fast_f32_r1(p, BN, tmem_acc, row0, tile_col0, stage, lane, half, full_bar, full_phase);
+  if (EPI == EPI_F32 && interior) {
+    epilogue_fast_f32_r1(p, BN, acc, row0, tile_col0, stage, lane, half);
     return;
   }
   if (EPI == EPI_F32R2 && interior) {
-    epilogue_fast_f32(p, BN, tmem_acc, row0, tile_col0, stage, lane, half, full_bar, full_phase);
+    epilogue_fast_f32(p, BN, acc, row0, tile_col0, stage, lane, half);
     return;
   }
-  mbar_wait(full_bar, full_phase);
-  tc_fence_after();
-  if (interior) epilogue_fast<EPIB, NPL>(p, BN, tmem_acc, row0, tile_col0, stage, lane, half);
-  else epilogue_edge<EPIB, NPL>(p, BN, tmem_acc, row0, tile_col0, stage, lane, half);
+  if (interior) epilogue_fast<EPIB, NPL>(p, BN, acc, row0, tile_col0, stage, lane, half);
+  else epilogue_edge<EPIB, NPL>(p, BN, acc, row0, tile_col0, stage, lane, half);
+}
+
+template <int BN>
+__device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  if constexpr (BN == 128) wgmma_m64n128_ss(d, a_desc, b_desc, accumulate);
+  else wgmma_m64n64_ss(d, a_desc, b_desc, accumulate);
 }
 
 template <int BN, int STAGES, int APL, int WPL, int EPI>  // APL / WPL: A / W planes resident per stage
@@ -518,14 +500,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   constexpr uint32_t TILE_W_BYTES = BN * TC_BK * 2;
   constexpr uint32_t STAGE_BYTES = APL * TC_TILE_BYTES_A + WPL * TILE_W_BYTES;
+  constexpr int ACC_LD = BN + 4;
   // align to 1024 B WITHOUT leaving the shared address space (a uintptr_t round trip makes every access a generic LD/ST)
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
+  float* acc_tile = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);          // [TC_BM][ACC_LD]
+  float* epi_stage = acc_tile + TC_BM * ACC_LD;                                       // 8 x [32][20] floats
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + EPI_WARPS * EPI_WARP_FLOATS);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;       // [2]
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* epi_stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + 256);   // 8 x [32][20] floats
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles = p.tiles_m * p.tiles_n;
@@ -536,21 +517,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     tma_prefetch_desc(&map_w);
   }
   if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full[s], 1); mbar_init(&tmem_empty[s], EPI_WARPS); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], EPI_WARPS); }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_base_slot, 2 * BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
   pdl_wait();                                          // prologue above is global-memory free; operands are read below
   pdl_trigger();
 
   if (warp == 0) {
     // ===================== TMA producer =====================
-    if (elect_one_sync()) {          // single elected lane: no waterfall loops around the uniform-datapath TMA / MMA instructions
+    if (elect_one_sync()) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int tm = tile / p.tiles_n, tn = tile - tm * p.tiles_n;
@@ -563,208 +539,51 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             tma_load_2d(st + pl * TC_TILE_BYTES_A, &map_a, &full_bar[stage], kb * TC_BK, (int)(pl * p.a_plane_rows + (int64_t)tm * TC_BM));
 #pragma unroll
           for (int pl = 0; pl < WPL; ++pl)
-#pragma unroll
-            for (int hb = 0; hb < BN / 128; ++hb)   // W box = 128 rows; a 256-wide tile is two boxes, contiguous in smem
-              tma_load_2d(st + APL * TC_TILE_BYTES_A + pl * TILE_W_BYTES + hb * (128 * TC_BK * 2), &map_w, &full_bar[stage], kb * TC_BK,
-                          pl * p.w_plane_rows + tn * BN + hb * 128);
+            tma_load_2d(st + APL * TC_TILE_BYTES_A + pl * TILE_W_BYTES, &map_w, &full_bar[stage], kb * TC_BK, pl * p.w_plane_rows + tn * BN);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one_sync()) {          // single elected lane: no waterfall loops around the uniform-datapath TMA / MMA instructions
-      constexpr uint32_t idesc = make_idesc_f16(TC_BM, BN);
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);       // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t st = smem_u32(smem + stage * STAGE_BYTES);
-          for (int t = 0; t < p.n_terms; ++t) {
-            const uint64_t da = make_sw128_desc(st + c_term_a[t] * TC_TILE_BYTES_A);
-            const uint64_t dw = make_sw128_desc(st + APL * TC_TILE_BYTES_A + c_term_w[t] * TILE_W_BYTES);
-#pragma unroll
-            for (int k = 0; k < TC_BK / TC_UK; ++k) {
-              // advance 32 bytes (16 fp16) inside the 128-byte swizzle span: +2 in 16-byte units
-              umma_f16(d_tmem, da + 2 * k, dw + 2 * k, idesc, (kb | t | k) != 0 ? 1u : 0u);
-            }
-          }
-          umma_commit(&empty_bar[stage]);                  // ring slot free once these MMAs retire
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tmem_full[acc]);                      // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
       }
     }
   } else if (warp >= 4) {
-    // ===================== epilogue (warps 4..11: TMEM lane quarter warp%4, alternate 16-column chunks) =====================
-    const int q = warp & 3, half = (warp - 4) >> 2;
-    int acc = 0; uint32_t acc_phase = 0;
+    // ===================== consumers: warpgroup wg = rows [64 wg, +64) of the tile; then all eight warps run the epilogue =====
+    const int wg = (warp - 4) >> 2, q = warp & 3;
+    int stage = 0; uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       const int tm = tile / p.tiles_n, tn = tile - tm * p.tiles_n;
-      epilogue_warp<EPI, APL>(p, BN, tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN, (int64_t)tm * TC_BM + q * 32, tn * BN,
-                                  epi_stage + (warp - 4) * EPI_WARP_FLOATS, lane, half, &tmem_full[acc], acc_phase);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);        // 4 arrivals (one per epilogue warp) free the accumulator
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2 * BN);
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------ cta_group::2 variant
-// CTA pair (cluster 2x1x1) computes a 256 x 256 output tile: each CTA stages ITS 128 rows of A and ITS 128 rows of W
-// (half of the N tile) per k-block, so operand bytes per MMA cycle are half those of the single-CTA 128x256 tile
-// (64 KB per k-block per SM for the three x3 terms) and three stages fit.  The leader issues
-// tcgen05.mma.cta_group::2 (M=256); each CTA drains its own 128 TMEM lanes in the epilogue.
-//
-// Schedule: pair q of P runs the whole tiles q, q + P, ... of the first full_rounds * P tiles, then the column slices q, q + P, ...
-// of the leftover tiles (item_of).  A 256 x 256 tile takes ~9 us (K = 512, x3) to ~35 us (K = 2048); with 250 tiles on 74 pairs
-// the last round kept 28 pairs busy for a whole tile time while 46 idled (16 % of the FFN-w_2 / out-projection launch).  Slices
-// of 128 / 64 columns (tcgen05.mma N = 128 / 64, the W box of each CTA 64 / 32 rows through a second tensor map) spread those 28
-// tiles over 56 / 112 items.  Narrow slices re-read the A rows from L2 more often, so only the tail uses them.
-struct TcItem { int tm, col0, bn; };
-__device__ __forceinline__ bool item_of(const TcParams& p, int pair, int n_pairs, int it, TcItem& o) {
-  int tile, part = 0;
-  o.bn = 256;
-  if (it < p.full_rounds) {
-    tile = pair + it * n_pairs;
-  } else {
-    const int j = pair + (it - p.full_rounds) * n_pairs;
-    if (j >= p.tail_tiles * p.tail_sub) return false;
-    tile = p.full_rounds * n_pairs + j / p.tail_sub;
-    part = j - (j / p.tail_sub) * p.tail_sub;
-    o.bn = 256 / p.tail_sub;
-  }
-  o.tm = tile / p.tiles_n;
-  o.col0 = (tile - o.tm * p.tiles_n) * 256 + part * o.bn;
-  return true;
-}
-
-template <int STAGES, int PL, int EPI>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(384, 1)
-gemm_tc2_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_w_tail,
-                const __grid_constant__ TcParams p) {
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  constexpr int BN = 256;
-  constexpr uint32_t TILE_BYTES = 128 * TC_BK * 2;                 // 16 KB: 128 rows x 64 fp16
-  constexpr uint32_t STAGE_BYTES = 2 * PL * TILE_BYTES;            // A planes + W-half planes of this CTA
-  // align to 1024 B WITHOUT leaving the shared address space (a uintptr_t round trip makes every access a generic LD/ST)
-  unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full = empty_bar + STAGES;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;       // [2] (used in the leader only: 8 arrivals = 4 epilogue warps x 2 CTAs)
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-  float* epi_stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + 256);   // 8 x [32][20] floats
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int n_pairs = gridDim.x >> 1, pair = blockIdx.x >> 1;
-  const int k_blocks = p.Kp / TC_BK;
-
-  if (warp == 0 && lane == 0) { tma_prefetch_desc(&map_a); tma_prefetch_desc(&map_w); tma_prefetch_desc(&map_w_tail); }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full[s], 1); mbar_init(&tmem_empty[s], 2 * EPI_WARPS); }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc_2sm(tmem_base_slot, 2 * BN);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                  // barriers of both CTAs are initialised before any remote use
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
-  pdl_wait();                                          // prologue above is global-memory free; operands are read below
-  pdl_trigger();
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (elect_one_sync()) {          // single elected lane: no waterfall loops around the uniform-datapath TMA / MMA instructions
-      int stage = 0; uint32_t phase = 0;
-      TcItem it;
-      for (int i = 0; item_of(p, pair, n_pairs, i, it); ++i) {
-        const CUtensorMap* mw = it.bn == BN ? &map_w : &map_w_tail;            // W box: bn / 2 rows per CTA
-        const uint32_t w_bytes = (uint32_t)(it.bn / 2) * (TC_BK * 2);
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          if (leader) mbar_expect_tx(&full_bar[stage], 2 * PL * (TILE_BYTES + w_bytes));   // bytes of BOTH CTAs land on the leader's barrier
-          unsigned char* st = smem + stage * STAGE_BYTES;
+      float d[BN / 2];
 #pragma unroll
-          for (int pl = 0; pl < PL; ++pl)
-            tma_load_2d_2sm(st + pl * TILE_BYTES, &map_a, &full_bar[stage], kb * TC_BK,
-                            (int)(pl * p.a_plane_rows + (int64_t)it.tm * 256 + rank * 128));
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < k_blocks; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t st = smem_u32(smem + stage * STAGE_BYTES);
+        wgmma_fence();
+        for (int t = 0; t < p.n_terms; ++t) {
+          const uint64_t da = make_sw128_desc(st + c_term_a[t] * TC_TILE_BYTES_A + wg * (64 * 128));
+          const uint64_t dw = make_sw128_desc(st + APL * TC_TILE_BYTES_A + c_term_w[t] * TILE_W_BYTES);
 #pragma unroll
-          for (int pl = 0; pl < PL; ++pl)
-            tma_load_2d_2sm(st + (PL + pl) * TILE_BYTES, mw, &full_bar[stage], kb * TC_BK,
-                            pl * p.w_plane_rows + it.col0 + (int)rank * (it.bn / 2));
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          for (int k = 0; k < TC_BK / TC_UK; ++k) wgmma_tile<BN>(d, da + 2 * k, dw + 2 * k, (kb | t | k) != 0 ? 1u : 0u);
         }
+        wgmma_commit();
+        wgmma_wait_pending1();                         // the previous k-block's MMAs have retired: its ring slot is free
+        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (leader && elect_one_sync()) {
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      TcItem it;
-      for (int i = 0; item_of(p, pair, n_pairs, i, it); ++i) {
-        const uint32_t idesc = make_idesc_f16(256, it.bn);
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);       // both CTAs' epilogues have drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < k_blocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t st = smem_u32(smem + stage * STAGE_BYTES);
-          for (int t = 0; t < p.n_terms; ++t) {
-            const uint64_t da = make_sw128_desc(st + c_term_a[t] * TILE_BYTES);
-            const uint64_t dw = make_sw128_desc(st + (PL + c_term_w[t]) * TILE_BYTES);
+      wgmma_wait_all();
+      wgmma_fence_regs(d);
+      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
+      named_bar(1, 256);                               // the previous tile's epilogue has read the accumulator tile
+      float* arow = acc_tile + (64 * wg + 16 * q + (lane >> 2)) * ACC_LD + 2 * (lane & 3);
 #pragma unroll
-            for (int k = 0; k < TC_BK / TC_UK; ++k) umma_f16_2sm(d_tmem, da + 2 * k, dw + 2 * k, idesc, (kb | t | k) != 0 ? 1u : 0u);
-          }
-          umma_commit_2sm(&empty_bar[stage]);              // frees the slot in both CTAs
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit_2sm(&tmem_full[acc]);                  // accumulators complete in both CTAs
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      for (int j = 0; j < BN / 8; ++j) {
+        *reinterpret_cast<float2*>(arow + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
+        *reinterpret_cast<float2*>(arow + 8 * ACC_LD + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
       }
+      named_bar(1, 256);
+      epilogue_warp<EPI, APL>(p, BN, acc_tile + q * 32 * ACC_LD, (int64_t)tm * TC_BM + q * 32, tn * BN,
+                              epi_stage + (warp - 4) * EPI_WARP_FLOATS, lane, wg);
     }
-  } else if (warp >= 4) {
-    // ===================== epilogue (each CTA: its 128 rows) =====================
-    const int q = warp & 3, half = (warp - 4) >> 2;
-    int acc = 0; uint32_t acc_phase = 0;
-    TcItem it;
-    for (int i = 0; item_of(p, pair, n_pairs, i, it); ++i) {
-      epilogue_warp<EPI, PL>(p, it.bn, tmem_base + ((uint32_t)(q * 32) << 16) + acc * BN, (int64_t)it.tm * 256 + rank * 128 + q * 32, it.col0,
-                             epi_stage + (warp - 4) * EPI_WARP_FLOATS, lane, half, &tmem_full[acc], acc_phase);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_leader(&tmem_empty[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                  // the peer may still arrive on / read this CTA's shared memory
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, 2 * BN);
   }
 }
 
@@ -858,7 +677,9 @@ size_t gemm_tc_scratch_bytes(int64_t max_rows, int max_k, int mode) {
 
 template <int BN, int STAGES, int APL, int WPL, int EPI>
 static int launch_cfg_e(const CUtensorMap& ma, const CUtensorMap& mw, const TcParams& p, cudaStream_t st) {
-  constexpr size_t smem = (size_t)STAGES * (APL * TC_TILE_BYTES_A + WPL * BN * TC_BK * 2) + 1024 + 256 + EPI_WARPS * EPI_WARP_FLOATS * 4;
+  constexpr size_t smem = (size_t)STAGES * (APL * TC_TILE_BYTES_A + WPL * BN * TC_BK * 2) + 1024 + (size_t)TC_BM * (BN + 4) * 4 +
+                          EPI_WARPS * EPI_WARP_FLOATS * 4 + 2 * STAGES * 8;
+  static_assert(smem <= 227 * 1024, "shared memory per block");
   static PerDeviceOnce once;
   FA_RETURN_IF_ERR(ensure_dyn_smem(gemm_tc_kernel<BN, STAGES, APL, WPL, EPI>, smem, once));
   const int n_sm = sm_count();
@@ -881,44 +702,6 @@ static int launch_cfg(const CUtensorMap& ma, const CUtensorMap& mw, const TcPara
   }
 }
 
-template <int STAGES, int PL, int EPI>
-static int launch_cfg2_e(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& mwt, const TcParams& p, int pairs, cudaStream_t st) {
-  constexpr size_t smem = (size_t)STAGES * (2 * PL * 128 * TC_BK * 2) + 1024 + 256 + EPI_WARPS * EPI_WARP_FLOATS * 4;
-  static PerDeviceOnce once;
-  FA_RETURN_IF_ERR(ensure_dyn_smem(gemm_tc2_kernel<STAGES, PL, EPI>, smem, once));
-  FA_CUDA_OK(launch_pdl(gemm_tc2_kernel<STAGES, PL, EPI>, dim3(2 * pairs), dim3(384), smem, st, 1, ma, mw, mwt, p));   // cluster dims are compile-time (__cluster_dims__)
-  FA_CHECK_LAUNCH();
-  return FA_OK;
-}
-
-template <int STAGES, int PL>
-static int launch_cfg2(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& mwt, const TcParams& p, int pairs, cudaStream_t st) {
-  switch (epi_kind(p)) {
-    case EPI_ATT: return launch_cfg2_e<STAGES, PL, EPI_ATT>(ma, mw, mwt, p, pairs, st);
-    case EPI_PLANES: return launch_cfg2_e<STAGES, PL, EPI_PLANES>(ma, mw, mwt, p, pairs, st);
-    case EPI_F32R2: return launch_cfg2_e<STAGES, PL, EPI_F32R2>(ma, mw, mwt, p, pairs, st);
-    default: return launch_cfg2_e<STAGES, PL, EPI_F32>(ma, mw, mwt, p, pairs, st);
-  }
-}
-
-// Column slices per leftover tile (1 | 2 | 4): the one that minimises the tail's duration ceil(tail * sub / P) / sub, the coarser
-// one on ties (wider tiles move fewer operand bytes per flop).  FA_GEMM_TAIL=0 keeps whole tiles (A/B runs).
-static int pick_tail_sub(int tail_tiles, int pairs) {
-  static const bool on = [] { const char* e = getenv("FA_GEMM_TAIL"); return !(e && e[0] == '0'); }();
-  if (!on || tail_tiles == 0) return 1;
-  int best = 1, best_q = 4 * ((tail_tiles + pairs - 1) / pairs);           // duration in quarter rounds
-  for (int sub = 2; sub <= 4; sub *= 2) {
-    const int q = ((tail_tiles * sub + pairs - 1) / pairs) * (4 / sub);
-    if (q < best_q) { best_q = q; best = sub; }
-  }
-  return best;
-}
-
-static bool use_2cta() {
-  static const bool on = [] { const char* e = getenv("FA_GEMM_2CTA"); return !(e && e[0] == '0'); }();
-  return on;
-}
-
 // A planes already split: a_planes [npl][M][Kp]
 int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& lin, int relu, const float* r1, int64_t ld1,
                           const float* r2, int64_t ld2, float* y, int64_t ldy, plane_t* out_planes, int64_t ldo,
@@ -933,59 +716,29 @@ int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& li
   if (y && (ldy & 3) == 0 && (((uintptr_t)y) & 15)) return FA_ERR_UNSUPPORTED;
   if ((r1 && (ld1 & 3)) || (r2 && (ld2 & 3))) return FA_ERR_UNSUPPORTED;
   const int npl = planes_for_mode(mode);
-  // 128x256 tiles halve the operand bytes per MMA cycle (the 128x128 tile is L2-bandwidth bound); used when N splits
-  // evenly and there are enough tiles to fill the machine.  x6 keeps 128x128 (three planes per operand do not fit twice).
-  // Ragged N (the vocabulary projections: 8404, 25055) also runs on pair tiles when the output is plain fp32 rows: the last column
-  // tile's W box reaches past row N of a plane — into the next plane's first rows or, for the last plane, out of the tensor map
-  // (zero fill) — so its surplus accumulator columns hold finite garbage that the bounds-checked edge epilogue never stores.
-  const bool ragged_ok = N >= 1024 && !out_planes && !att;
-  if (use_2cta() && npl <= 2 && (N % 256 == 0 || ragged_ok) && M >= 256) {
-    // cta_group::2: 256 x 256 pair tiles (see gemm_tc2_kernel)
-    CUtensorMap ma2, mw2;
-    // rows of the map: every row of every plane whose K_pad elements lie inside the allocation (an overlapping view's last rows do not)
-    const uint64_t a_rows = (uint64_t)apr * npl - (lda < (uint64_t)Kp ? ((uint64_t)Kp - lda + lda - 1) / lda : 0);
-    FA_RETURN_IF_ERR(make_plane_map(&ma2, a_planes, a_rows, (uint64_t)Kp, lda, 128));
-    FA_RETURN_IF_ERR(make_plane_map(&mw2, lin.w_planes, (uint64_t)N * 3, (uint64_t)Kp, (uint64_t)Kp, 128));
-    TcParams p2;
-    p2.M = M; p2.N = N; p2.Kp = Kp; p2.a_plane_rows = apr; p2.w_plane_rows = N;
-    p2.n_terms = mode == FA_GEMM_F16X1 ? 1 : 3;
-    p2.relu = relu; p2.bias = lin.b; p2.r1 = r1; p2.ldr1 = ld1; p2.r2 = r2; p2.ldr2 = ld2; p2.C = y; p2.ldc = ldy;
-    p2.out_planes = out_planes; p2.ldo = ldo; p2.out_nplanes = npl;
-    p2.tiles_m = (int)((M + 255) / 256); p2.tiles_n = (N + 255) / 256;
-    p2.acc_scale = rz_comp_scale(Kp, p2.n_terms);
-    if (att) { p2.att = *att; p2.att.enabled = 1; } else { p2.att = AttnSinks{}; }
-    if (att && (att->width % 32 != 0 || att->t_rows <= 0 || M % att->t_rows != 0)) return FA_ERR_UNSUPPORTED;
-    const int tiles = p2.tiles_m * p2.tiles_n, half_sms = sm_count() / 2;
-    p2.full_rounds = tiles / half_sms;
-    p2.tail_tiles = tiles - p2.full_rounds * half_sms;
-    p2.tail_sub = pick_tail_sub(p2.tail_tiles, half_sms);
-    const int pairs = p2.full_rounds > 0 ? half_sms : (p2.tail_tiles * p2.tail_sub < half_sms ? p2.tail_tiles * p2.tail_sub : half_sms);
-    CUtensorMap mwt = mw2;
-    if (p2.tail_sub > 1) FA_RETURN_IF_ERR(make_plane_map(&mwt, lin.w_planes, (uint64_t)N * 3, (uint64_t)Kp, (uint64_t)Kp, 128 / p2.tail_sub));
-    return npl == 1 ? launch_cfg2<6, 1>(ma2, mw2, mwt, p2, pairs, st) : launch_cfg2<3, 2>(ma2, mw2, mwt, p2, pairs, st);
-  }
-  const bool wide = (npl <= 2) && (N % 256 == 0) && (N >= 1024);
-  const int BN = wide ? 256 : 128;
+  // 128 x 128 tiles (64 wide for x6: three planes per operand, two ring stages and the accumulator tile fill the 227 KB).
+  // Ragged N (the vocabulary projections: 8404, 25055): the last column tile's W box reaches past row N of a plane — into the next
+  // plane's first rows or, for the last plane, out of the tensor map (zero fill) — so its surplus accumulator columns hold finite
+  // garbage that the bounds-checked edge epilogue never stores.
+  const int BN = npl == 3 ? 64 : 128;
   CUtensorMap ma, mw;
   const uint64_t a_rows1 = (uint64_t)apr * npl - (lda < (uint64_t)Kp ? ((uint64_t)Kp - lda + lda - 1) / lda : 0);
   FA_RETURN_IF_ERR(make_plane_map(&ma, a_planes, a_rows1, (uint64_t)Kp, lda, TC_BM));
-  FA_RETURN_IF_ERR(make_plane_map(&mw, lin.w_planes, (uint64_t)N * 3, (uint64_t)Kp, (uint64_t)Kp, wide ? 128 : BN));
+  FA_RETURN_IF_ERR(make_plane_map(&mw, lin.w_planes, (uint64_t)N * 3, (uint64_t)Kp, (uint64_t)Kp, BN));
   TcParams p;
   p.M = M; p.N = N; p.Kp = Kp; p.a_plane_rows = apr; p.w_plane_rows = N;
   p.n_terms = mode == FA_GEMM_F16X1 ? 1 : (mode == FA_GEMM_F16X3 ? 3 : 6);
   p.relu = relu; p.bias = lin.b; p.r1 = r1; p.ldr1 = ld1; p.r2 = r2; p.ldr2 = ld2; p.C = y; p.ldc = ldy;
   p.out_planes = out_planes; p.ldo = ldo; p.out_nplanes = npl;
   p.tiles_m = (int)((M + TC_BM - 1) / TC_BM); p.tiles_n = (N + BN - 1) / BN;
-  p.full_rounds = 0; p.tail_tiles = 0; p.tail_sub = 1;
   p.acc_scale = rz_comp_scale(Kp, p.n_terms);
   if (att) { p.att = *att; p.att.enabled = 1; } else { p.att = AttnSinks{}; }
   if (att && (N % 32 != 0 || att->width % 32 != 0 || att->t_rows <= 0 || M % att->t_rows != 0)) return FA_ERR_UNSUPPORTED;
   if (out_planes && (N % 32 != 0)) return FA_ERR_UNSUPPORTED;
-  if (wide) return npl == 1 ? launch_cfg<256, 4, 1, 1>(ma, mw, p, st) : launch_cfg<256, 2, 2, 2>(ma, mw, p, st);
   switch (npl) {
-    case 1: return launch_cfg<128, 6, 1, 1>(ma, mw, p, st);
-    case 2: return launch_cfg<128, 3, 2, 2>(ma, mw, p, st);
-    default: return launch_cfg<128, 2, 3, 3>(ma, mw, p, st);
+    case 1: return launch_cfg<128, 4, 1, 1>(ma, mw, p, st);
+    case 2: return launch_cfg<128, 2, 2, 2>(ma, mw, p, st);
+    default: return launch_cfg<64, 2, 3, 3>(ma, mw, p, st);
   }
 }
 

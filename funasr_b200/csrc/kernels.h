@@ -8,14 +8,14 @@ namespace fa { typedef __half plane_t; }   // 16-bit operand plane element (tc_c
 
 namespace fa {
 
-// y (fp32) and/or planes (fp16 [nplanes][rows][cols_pad], the A operand of a following tcgen05 GEMM)
+// y (fp32) and/or planes (fp16 [nplanes][rows][cols_pad], the A operand of a following tensor-core GEMM)
 int layernorm_launch(const float* x, int64_t rows, const FaNorm& nm, float* y, const float* pe_inv, float xscale,
                      int rows_per_batch, cudaStream_t st, plane_t* planes = nullptr, int nplanes = 0, int cols_pad = 0,
                      float* emb_out = nullptr);   // emb_out: with pe_inv, also write the embedded (pre-norm) rows there
 int gemm_f32_launch(const float* A, int64_t lda, int64_t M, const float* W, int N, int K, const float* bias, int relu,
                     const float* r1, int64_t ldr1, const float* r2, int64_t ldr2, float* C, int64_t ldc,
                     cudaStream_t st);
-// tcgen05 fp16-split GEMM (gemm_tc.cu)
+// wgmma fp16-split GEMM (gemm_tc.cu)
 size_t gemm_tc_scratch_bytes(int64_t max_rows, int max_k, int mode);
 int gemm_tc_launch(const float* x, int64_t ldx, int64_t rows, const FaLinear& lin, int relu, const float* r1,
                    int64_t ld1, const float* r2, int64_t ld2, float* y, int64_t ldy, int mode, Arena* scratch,
@@ -34,7 +34,7 @@ struct AttnSinks {
   plane_t* k_planes = nullptr;   // [npl][M][width]
   plane_t* vt_planes = nullptr;  // [npl][B*width][t_pad]
 };
-// tcgen05 attention (attention_tc.cu); ctx fp32 and/or fp16 planes [npl][B*tq][ldp]
+// wgmma attention (attention_tc.cu); ctx fp32 and/or fp16 planes [npl][B*tq][ldp]
 int attention_tc_planes_launch(const plane_t* qp, const plane_t* kp, const plane_t* vt, const int32_t* key_lens,
                                int batch, int heads, int tq, int tk, float* ctx, int64_t ldc, plane_t* ctx_planes,
                                int64_t ldp, int out_nplanes, int mode, cudaStream_t st, int kv_shared = 0);

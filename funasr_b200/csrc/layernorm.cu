@@ -3,7 +3,7 @@
 // Optional fused prologue for the first encoder layer: x*sqrt(d_model) + sinusoidal position encoding
 // (SANMEncoder.forward encoder.py:409,428; SinusoidalPositionEncoder embedding.py:396-432).
 // Optional fused epilogue for the tensor-core path: the normalised row is written as fp16 planes (hi, mid, lo) — the A
-// operand of the following tcgen05 GEMM — instead of / in addition to fp32.
+// operand of the following tensor-core GEMM — instead of / in addition to fp32.
 // HBM-bound: algorithmic bytes = 8 B per element (read + write).
 #include "common.cuh"
 #include "tc_common.cuh"

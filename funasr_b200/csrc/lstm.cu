@@ -2,7 +2,7 @@
 // (funasr/models/bicif_paraformer/cif_predictor.py:187-190, :318-320: `output2, _ = self.blstm(output2)` on the 3x upsampled
 // encoder output).  cuDNN needs 34 ms for [64, 1500, 512] in fp32; the recurrence is 1500 strictly sequential steps of a
 // [B,512] x [512,2048] product per direction, so the design goal is the shortest possible step:
-//   * the input projections x W_ih^T + b_ih + b_hh of ALL steps are one tcgen05 GEMM of this library (fa_linear), outside;
+//   * the input projections x W_ih^T + b_ih + b_hh of ALL steps are one tensor-core GEMM of this library (fa_linear), outside;
 //   * weight-stationary recurrence: 2 directions x 64 CTAs, CTA c keeps the 4 gate rows of hidden units [8c, 8c+8) of W_hh
 //     (32 x 512 fp32 = 64 KB) in shared memory for the whole sequence, plus one [64, 512] fp32 copy of h_{t-1} (128 KB);
 //   * per step: gather h_{t-1} (written by the 64 CTAs of this direction into the OUTPUT tensor itself) -> 64 x 32 dot products

@@ -104,7 +104,7 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
   const int din = enc->layers[0].norm1.n;
   const bool embed = enc->pe_inv_timescales != nullptr;   // false: plain stack over an existing [B,T,512] stream
   const int hd = enc->heads > 0 ? D / enc->heads : 0;
-  // the tcgen05 kernels are built for the Paraformer / SenseVoice shape (d = 512, 4 x 128); the fp32 path also runs the small
+  // the tensor-core kernels are built for the Paraformer / SenseVoice shape (d = 512, 4 x 128); the fp32 path also runs the small
   // SAN-M stacks around the hot path (CT-Transformer punctuation: d = 256, 8 x 32)
   if (D < 64 || D > 512 || (D & 15) || enc->heads < 1 || enc->heads * hd != D || hd < 32 || hd > 128 || (hd & 31) || din > 560 || (din & 15) ||
       (!embed && din != D))
@@ -778,7 +778,7 @@ extern "C" int fa_embedding(const int32_t* ids, const float* table, int32_t dim,
   return FA_OK;
 }
 
-extern "C" const char* fa_version(void) { return "funasr_b200 0.1.0 (sm_100a)"; }
+extern "C" const char* fa_version(void) { return "funasr_b200 0.1.0 (sm_90a)"; }
 extern "C" uint64_t fa_launch_count(void) { return (uint64_t)fa::g_launch_count.load(); }
 extern "C" const char* fa_status_string(int status) {
   switch (status) {

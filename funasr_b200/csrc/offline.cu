@@ -4,7 +4,7 @@
 // runtime/onnxruntime/src/paraformer.cpp).  No Python, no torch: weights come from one flat file written by
 // funasr_b200/pack.py (tensors under FunASR's own state_dict names), device memory from cudaMalloc.
 //
-//   fa_offline_init         model file -> handle (weights to HBM, fp16 planes for the tcgen05 GEMMs)
+//   fa_offline_init         model file -> handle (weights to HBM, fp16 planes for the tensor-core GEMMs)
 //   fa_offline_infer        batch of host PCM buffers (f32 in [-1,1] or s16le) -> result (greedy token ids per utterance)
 //   fa_offline_result_*     accessors;  fa_offline_free_result / fa_offline_uninit
 // The tokenizer (ids -> text) stays with the caller, like every other entry point of this ABI.

@@ -1,4 +1,4 @@
-// PTX wrappers shared by the tcgen05 kernels (mbarrier, TMA, TMEM, UMMA descriptors).  sm_100a only.
+// PTX wrappers shared by the Hopper tensor-core kernels (mbarrier, TMA, wgmma descriptors).  sm_90a only.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -11,9 +11,7 @@ namespace fa {
 // ------------------------------------------------------------------------------------------------ PTX helpers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// exactly one lane of a converged warp (elect.sync): the compiler knows the guarded region is single-threaded, so the
-// uniform-datapath tcgen05 instructions inside need no per-instruction "waterfall" loop (if (lane == 0) costs ~9 extra
-// SASS instructions around every UTCHMMA — measured ~55 cycles per 32-cycle MMA in the attention kernel)
+// exactly one lane of a converged warp (elect.sync): the compiler knows the guarded region is single-threaded
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred = 0;
   asm volatile(
@@ -43,7 +41,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "WAIT_DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
   asm volatile(
@@ -54,79 +51,59 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, fp16 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]^T: the A operand (M=128 rows = TMEM lanes, K-major: 16 fp16 = 8 consecutive 32-bit
-// columns per K=16 step, element 2j in the low half of column j) is read from tensor memory, so only B costs shared-memory
-// bandwidth (attention: Q and P planes live in TMEM)
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// commit that arrives on the barrier at this offset in every CTA of ctamask (cluster multicast)
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t ctamask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(ctamask) : "memory");
-}
-// TMA load delivered to the same shared-memory offset (and signalling the same-offset mbarrier) of every CTA in ctamask
-__device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, uint16_t ctamask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(ctamask) : "memory");
-}
-// 16 registers per thread -> 32 lanes x 16 consecutive 32-bit columns (thread i <-> TMEM lane base+i)
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// 32 lanes x 32 consecutive 32-bit columns -> 32 registers per thread (thread i <-> TMEM lane base+i)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// named barrier `id` that completes once `threads` threads (whole warps) have reached it (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
+// ------------------------------------------------------------------------------------------------ wgmma
+// A warpgroup (4 consecutive warps) issues one wgmma.mma_async for a 64 x N x 16 product; D lives in registers with the
+// accumulator layout: warp w of the group, lane l holds rows 16 w + l / 4 (registers 4 j, 4 j + 1) and 16 w + l / 4 + 8
+// (4 j + 2, 4 j + 3) at columns 8 j + 2 (l % 4) + {0, 1}.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_pending1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs that own the registers
+template <int N>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+__device__ __forceinline__ void wgmma_m64n64_ss(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_m64n128_ss(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_m64n128_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
+}
 // ------------------------------------------------------------------------------------------------ operand planes
 // A 16-bit "plane" element of the split x = p0 + p1 (+ p2).  Planes are IEEE fp16 (11-bit significands): two planes carry ~22
 // bits of x, so the three products hi*hi + hi*lo + lo*hi of the x3 mode are good to ~2^-22 relative — 64x tighter than the same
-// three products on bf16 planes (8-bit significands, ~2^-16), at the same tcgen05 kind::f16 rate.  Round 1 used bf16 planes; the
-// B=64 full-depth parity run of round 2 showed log-prob errors up to 9e-3 absolute and ~1 flipped greedy id per 1000 tokens at
-// near-ties — which turned out to be the accumulator's round-toward-zero (gemm_tc.cu: acc_scale), not the operand precision; the
-// fp16 planes stay because they cost nothing: every GEMM operand of this path is LayerNorm-, ReLU- or softmax-bounded and sits far
-// inside the fp16 range (conversions saturate at +-65504 instead of producing inf; values below 2^-14 go subnormal, 6e-8 spacing).
+// three products on bf16 planes (8-bit significands, ~2^-16), at the same tensor-core rate.  Every GEMM operand of this path is
+// LayerNorm-, ReLU- or softmax-bounded and sits far inside the fp16 range (conversions saturate at +-65504 instead of producing
+// inf; values below 2^-14 go subnormal, 6e-8 spacing).
 typedef __half plane_t;
 __device__ __forceinline__ uint32_t pack_planes2(float e0, float e1) {      // {e0 -> low half, e1 -> high half}, round to nearest, saturating
   uint32_t r;
@@ -137,63 +114,15 @@ __device__ __forceinline__ float2 unpack_planes2(uint32_t p) { return __half22fl
 __device__ __forceinline__ plane_t to_plane(float x) { return __ushort_as_half((unsigned short)(pack_planes2(x, 0.f) & 0xFFFFu)); }
 __device__ __forceinline__ float plane_to_float(plane_t h) { return __half2float(h); }
 
-// K-major, SWIZZLE_128B shared-memory operand descriptor (tile rows at 128-byte pitch, 8-row groups 1024 B apart).
+// K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma (tile rows at 128-byte pitch, 8-row groups 1024 B apart, the
+// tile 1024-byte aligned).  Advancing the start address by 32 bytes (+2) steps K by 16 fp16 inside the 128-byte swizzle span.
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // start address, 16-byte units      bits [0,14)
   d |= (uint64_t)1 << 16;                             // leading byte offset (unused for swizzled K-major) [16,30)
   d |= (uint64_t)(1024 >> 4) << 32;                   // stride byte offset: 8 rows x 128 B [32,46)
-  d |= (uint64_t)1 << 46;                             // descriptor version (Blackwell)     [46,48)
-  d |= (uint64_t)2 << 61;                             // layout: SWIZZLE_128B               [61,64)
+  d |= (uint64_t)1 << 62;                             // layout: SWIZZLE_128B               [62,64)
   return d;
-}
-// kind::f16 instruction descriptor: D fp32 (bits 4-5 = 1), A / B format fp16 (bits 7-9 / 10-12 = 0; bf16 would be 1), both
-// K-major, shape M x N.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int m, int n) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-
-
-// ------------------------------------------------------------------------------------------------ cta_group::2 (CTA pair)
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;   // clears the CTA-rank bit of a shared::cluster address -> the pair's CTA 0
-
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA load issued by either CTA of a pair; the transaction bytes are credited to the LEADER CTA's mbarrier.
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-  const uint64_t hint = 0x1000000000000000ull;   // L2 evict-normal
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "l"(hint) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// M=256 MMA across the CTA pair (issued by the leader only): A/B halves are read from both CTAs' shared memory at the
-// same offsets, D rows 0-127 land in the leader's TMEM, rows 128-255 in the peer's.
-__device__ __forceinline__ void umma_f16_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive (once the MMAs issued so far retire) on the barrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-// arrive on the LEADER CTA's barrier from either CTA
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
 }
 
 // host: 2D fp16 tensor map [rows, cols] (row pitch ld elements), box {64 cols, box_rows}, SWIZZLE_128B (gemm_tc.cu)

@@ -319,8 +319,8 @@ class ParaformerEngine(_EngineBase):
     def upsample_timestamp(self, enc: torch.Tensor, lens: torch.Tensor, token_num: torch.Tensor):
         """CifPredictorV3.get_upsample_timestamp (bicif_paraformer/cif_predictor.py:300-352): enc [B,T,512], lens [B] i32,
         token_num [B] i32 (rounded) -> (us_alphas [B,3T], us_peaks [B,3T]).  ConvTranspose1d upsampling = one GEMM of this library,
-        the BLSTM = its input projections as one tcgen05 GEMM + this library's persistent weight-stationary recurrence
-        (fa_blstm_forward_tc: warp-level mma.sync on bf16 hi/lo planes, not tcgen05 — the per-step product is only 64x32x512; or the exact fp32
+        the BLSTM = its input projections as one tensor-core GEMM + this library's persistent weight-stationary recurrence
+        (fa_blstm_forward_tc: warp-level mma.sync on bf16 hi/lo planes, not wgmma — the per-step product is only 64x32x512; or the exact fp32
         fa_blstm_forward with FUNASR_B200_LSTM=simt), the alpha head / rescale / fire scan is fa_cif_upsample_alphas."""
         if not self.bicif:
             raise _abi.FunasrB200Error("engine was not built with bicif=True")

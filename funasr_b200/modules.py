@@ -285,7 +285,7 @@ class ParaformerB200(nn.Module):
         enc_cls = tables.encoder_classes.get(encoder) if isinstance(encoder, str) else encoder
         dec_cls = tables.decoder_classes.get(decoder) if isinstance(decoder, str) else decoder
         pred_cls = tables.predictor_classes.get(predictor) if isinstance(predictor, str) else predictor
-        # an unmodified reference config names the reference classes; they map onto the B200 components
+        # an unmodified reference config names the reference classes; they map onto this backend's components
         enc_cls = enc_cls if (enc_cls is not None and issubclass(enc_cls, _ParamHolder)) else SANMEncoderB200
         dec_cls = dec_cls if (dec_cls is not None and issubclass(dec_cls, _ParamHolder)) else ParaformerSANMDecoderB200
         pred_cls = pred_cls if (pred_cls is not None and issubclass(pred_cls, _ParamHolder)) else CifPredictorV2B200

@@ -84,7 +84,7 @@ def install(override_reference_keys: bool = False):
     """(Re-)register every funasr_b200 class into funasr.register.tables (call after `import funasr`).
 
     With override_reference_keys=True the reference's own keys ("Paraformer", "WavFrontend", "SANMEncoder",
-    "CifPredictorV2", "ParaformerSANMDecoder") are re-pointed at the B200 classes — registration is
+    "CifPredictorV2", "ParaformerSANMDecoder") are re-pointed at this backend's classes — registration is
     last-writer-wins (funasr/register.py:65-70) — so an unmodified config selects this backend.
     """
     t = get_tables()

@@ -1,5 +1,5 @@
 /*
- * funasr_b200 — C ABI of the B200-native (sm_100a) backend for FunASR's offline Paraformer hot path.
+ * funasr_b200 — C ABI of the H100-native (sm_90a) backend for FunASR's offline Paraformer hot path.
  *
  * Every entry point takes plain device pointers, sizes and a CUDA stream (as void*); no torch / C++
  * types cross the boundary.  All functions are stream-ordered, re-entrant, hold no global state, never
@@ -37,13 +37,13 @@ typedef enum {
 /* GEMM arithmetic modes (FaLinear contractions). fp32 accumulate everywhere. */
 typedef enum {
   FA_GEMM_F32_SIMT = 0, /* fp32 FFMA tiles: the parity reference path */
-  FA_GEMM_F16X1 = 1,   /* tcgen05 kind::f16, one fp16 pass (fast mode) */
-  FA_GEMM_F16X3 = 3,   /* tcgen05, fp16 planes x = hi + lo: hi*hi + hi*lo + lo*hi (~2^-22 relative per product) */
-  FA_GEMM_F16X6 = 6    /* tcgen05, three fp16 planes, six products (~fp32) */
+  FA_GEMM_F16X1 = 1,   /* wgmma f16, one fp16 pass (fast mode) */
+  FA_GEMM_F16X3 = 3,   /* wgmma, fp16 planes x = hi + lo: hi*hi + hi*lo + lo*hi (~2^-22 relative per product) */
+  FA_GEMM_F16X6 = 6    /* wgmma, three fp16 planes, six products (~fp32) */
 } FaGemmMode;
 
 /* nn.Linear: y = x W^T + b.  w_planes (optional) holds the fp16 planes made by fa_split_planes for the
- * tcgen05 path: [3][out_f][in_pad] fp16 (hi, mid, lo), in_pad = in_f rounded up to 64. */
+ * tensor-core path: [3][out_f][in_pad] fp16 (hi, mid, lo), in_pad = in_f rounded up to 64. */
 typedef struct {
   const float* w;        /* [out_f, in_f] */
   const float* b;        /* [out_f] or NULL */
@@ -231,7 +231,7 @@ int fa_attention(const float* q, int64_t ldq, const float* k, int64_t ldk, const
                  const int32_t* key_lens, int32_t batch, int32_t heads, int32_t tq, int32_t tk,
                  float* ctx, int64_t ld_ctx, fa_stream_t stream);
 
-/* Same contract on the tcgen05 tensor cores (fp16 operand planes, fp32 accumulation in TMEM):
+/* Same contract on the tensor cores (wgmma; fp16 operand planes, fp32 accumulation in registers):
  * gemm_mode FA_GEMM_F16X1 (one plane) or FA_GEMM_F16X3/X6 (hi+lo planes, three MMA terms).  workspace holds the
  * operand planes (size from fa_attention_tc_workspace_bytes). */
 size_t fa_attention_tc_workspace_bytes(int32_t batch, int32_t heads, int32_t tq, int32_t tk, int32_t gemm_mode);
@@ -429,7 +429,7 @@ int fa_embedding(const int32_t* ids, const float* table, int32_t dim, int32_t vo
 int fa_pcm_decode(const void* pcm, int32_t sample_format, int32_t channels, int64_t frames, float* out, fa_stream_t stream);
 
 /* Split fp32 [rows, cols] into three fp16 planes [3][rows][cols_pad] (hi, mid, lo; zero padded columns):
- * weight repack for the tcgen05 GEMM path (called once per weight after load_pretrained_model). */
+ * weight repack for the tensor-core GEMM path (called once per weight after load_pretrained_model). */
 int fa_split_planes(const float* src, int64_t ld_src, int64_t rows, int32_t cols, int32_t cols_pad,
                   void* planes, fa_stream_t stream);
 

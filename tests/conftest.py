@@ -26,7 +26,7 @@ KNF_CASES = [(16000, 31, "speechlike"), (8123, 32, "noise"), (400, 33, "noise"),
 
 def knf_logmel_cases():
     """-> [(wav fp32 tensor, golden log-mel [frames, 80] of the reference's compiled kaldi-native-fbank, live log-mel or None)].
-    The live column re-runs oracle/_ref/libknf_ref.so when it is present (built here from /root/reference; travels to the GPU box)."""
+    The live column re-runs oracle/_ref/libknf_ref.so when it is present (oracle/knf/Makefile builds it where the reference tree is)."""
     from funasr_b200 import synth
     import knf_ref
     g = np.load(os.path.join(GOLDEN, "knf_fbank.npz"))
@@ -47,8 +47,8 @@ def knf_bound(ref_logmel, scale=1.0):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
-    # a fresh checkout has no built library (it is git-ignored): build it once (nvcc cross-compiles sm_100a without a GPU)
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
+    # a fresh checkout has no built library (it is git-ignored): build it once (nvcc cross-compiles sm_90a without a GPU)
     if not os.path.exists(os.path.join(ROOT, "funasr_b200", "libfunasr_b200.so")):
         import __graft_entry__
         __graft_entry__.build()

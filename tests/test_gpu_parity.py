@@ -143,9 +143,9 @@ def test_linear_fp32_vs_oracle(rows, out_f, in_f):
 
 @pytest.mark.parametrize("mode,tol", [("fp16x6", 1e-5), ("fp16x3", 3e-5), ("fp16", 2e-2)])
 @pytest.mark.parametrize("rows,out_f,in_f", [(1000, 1536, 560), (300, 512, 2048), (130, 8404, 512), (129, 1000, 512), (32000, 512, 512),
-                                             (1000, 8404, 512), (700, 25060, 512)])    # ragged N on pair tiles (vocabulary projections; residual rows need a pitch % 4 == 0)
+                                             (1000, 8404, 512), (700, 25060, 512)])    # ragged N (vocabulary projections) through the edge epilogue; residual rows need a pitch % 4 == 0
 def test_linear_tcgen05_vs_oracle(rows, out_f, in_f, mode, tol):
-    """tcgen05/TMEM/TMA GEMM with fp16 operand splitting against the CPU fp32 nn.Linear (ragged M/N/K tails)."""
+    """wgmma/TMA GEMM with fp16 operand splitting against the CPU fp32 nn.Linear (ragged M/N/K tails)."""
     abi, lib = _lib()
     g = torch.Generator().manual_seed(4)
     x = torch.randn(rows, in_f, generator=g)
@@ -170,7 +170,7 @@ def test_linear_tcgen05_vs_oracle(rows, out_f, in_f, mode, tol):
     ref = torch.relu(torch.nn.functional.linear(x, w, b)) + r1 + r2
     assert not torch.isnan(y).any()
     err = rel_err(y.cpu().numpy(), ref.numpy())
-    print("linear tcgen05 %s rows=%d out=%d in=%d: rel err %.2e (tol %.0e)" % (mode, rows, out_f, in_f, err, tol))
+    print("linear wgmma %s rows=%d out=%d in=%d: rel err %.2e (tol %.0e)" % (mode, rows, out_f, in_f, err, tol))
     assert err <= tol
 
 
@@ -243,9 +243,9 @@ def test_attention_vs_oracle(tq, tk, lens):
 @pytest.mark.parametrize("mode,tol", [("fp16x3", 5e-5), ("fp16", 2e-2)])
 @pytest.mark.parametrize("tq,tk,lens", [(130, 130, [130, 1, 65]), (37, 211, [211, 64, 129]), (500, 500, [500, 83, 499]),
                                         (300, 300, [300, 0, 17]),                                    # an utterance without keys: zero context
-                                        (260, 200, [200, 3, 64, 65, 199] * 10)])                     # 600 tiles: several per persistent CTA
+                                        (260, 200, [200, 3, 64, 65, 199] * 10)])                     # 600 query tiles: several waves of one-tile CTAs
 def test_attention_tcgen05_vs_oracle(tq, tk, lens, mode, tol):
-    """Tensor-core attention (two-pass softmax, fp16 operand planes, TMEM accumulators) vs the CPU reference chain."""
+    """Tensor-core attention (two-pass softmax, fp16 operand planes, register accumulators) vs the CPU reference chain."""
     abi, lib = _lib()
     g = torch.Generator().manual_seed(6)
     B, H, D = len(lens), 4, 512
@@ -293,7 +293,7 @@ def _sub(cfg, t, step):
 @pytest.mark.parametrize("name", list(GOLDEN_CASES))
 def test_paraformer_vs_reference_golden(name, mode):
     """End-to-end against the UNMODIFIED reference's outputs (tests/golden, made by oracle/make_golden.py), with the
-    contractions on the fp32 SIMT path and on the tcgen05 fp16x3 split path."""
+    contractions on the fp32 SIMT path and on the wgmma fp16x3 split path."""
     cfg, wseed, wavs, cmvn, g = load_case(name)
     o = _run_model(cfg, wseed, wavs, cmvn, mode)
     assert o["feat_lens"].cpu().tolist() == g["feat_lens"].tolist()
@@ -784,45 +784,6 @@ def test_full_depth_b64_30s_ids_equal_oracle():
     # allows) — dominated by the tensor cores' accumulation rounding, not by the fp16 operand split (tools/noise_probe.py) — and the
     # top-2 margins of random-weight logits are exponentially distributed from zero, so ~1 token per 1000 sits inside the noise
     assert flipped <= 0.003 * sum(len(r) for r in want_ids), "more near-tie flips than the arithmetic noise explains: %s" % bad
-
-
-def _reference_importable():
-    try:
-        import ref_shim
-        return ref_shim.reference_available()
-    except Exception:
-        return False
-
-
-@pytest.mark.skipif(not _reference_importable(), reason="no reference install (baseline/_ref) on this box")
-def test_automodel_generate_runs_on_this_backend():
-    """Drop-in at the top of the stack: the UNMODIFIED reference's AutoModel (imported from the offline install under
-    baseline/_ref) with its OWN config keys ("Paraformer", "SANMEncoder", "WavFrontend", ...) re-pointed at this backend by
-    funasr_b200.install(override_reference_keys=True) (registration is last-writer-wins, funasr/register.py:65-70):
-    AutoModel(...).generate() -> AutoModel.inference (auto_model.py:806-829) -> ParaformerB200.inference on the GPU; ids equal the
-    golden ids the reference's own classes produced on the CPU."""
-    import tempfile
-    import funasr_b200
-    import ref_runner
-    import ref_shim
-    from funasr_b200 import synth
-    ref_shim.import_reference()
-    from funasr.register import tables
-    saved = {k: getattr(tables, k[0]).get(k[1]) for k in funasr_b200.registry.DROP_IN_KEYS}
-    cfg, wseed, wavs, cmvn, g = load_case("tiny_ragged3")
-    try:
-        funasr_b200.install(override_reference_keys=True)
-        with tempfile.TemporaryDirectory() as tmp:
-            am = ref_runner.build_automodel("paraformer", cfg, wseed, cmvn, tmp, 4, device="cuda:0")
-        assert isinstance(am.model, funasr_b200.ParaformerB200) and isinstance(am.kwargs["frontend"], funasr_b200.WavFrontendB200)
-        ids = ref_runner.generate_ids(am, wavs, batch_size=len(wavs))
-        assert [t for r in ids for t in r] == g["ids_flat"].tolist()
-        one = ref_runner.generate_ids(am, wavs, batch_size=1)          # the reference's default batching: one utterance per call
-        assert [len(r) for r in one] == [len(r) for r in ids]
-    finally:
-        for (tb, key), cls in saved.items():
-            if cls is not None:
-                getattr(tables, tb)[key] = cls
 
 
 def test_two_handles_two_threads_and_shared_hotword_memory(tmp_path):

@@ -67,8 +67,8 @@ def test_timestamps_are_ordered_and_inside_the_utterance(alphas, n_tok, rate, of
 
 
 def test_hotword_list_follows_reference_seg_dict_rules(tmp_path):
-    """funasr_b200.hotwords.generate_hotwords_list against the reference's own function (contextual_paraformer/model.py:528-660)
-    when /root/reference is importable, and against hand-derived expectations otherwise: seg_dict lookup (lower-cased), per-character
+    """funasr_b200.hotwords.generate_hotwords_list against the reference's own function (contextual_paraformer/model.py:528-660,
+    its outputs stored by oracle/make_live_golden.py) and against hand-derived expectations: seg_dict lookup (lower-cased), per-character
     fallback for CJK / digit words, <unk> for the rest, [sos] terminator; .txt files and plain strings."""
     from funasr_b200.hotwords import generate_hotwords_list, seg_tokenize
 
@@ -98,18 +98,14 @@ def test_hotword_list_follows_reference_seg_dict_rules(tmp_path):
     assert generate_hotwords_list("gpu Hello", Tok(), Fe(), sos=1) == [[8], [9], [1]]
     with pytest.raises(ValueError):
         generate_hotwords_list("http://example.com/hw.txt", Tok(), fe, sos=1)
-    if os.path.isdir("/root/reference"):
-        import sys
-        sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle"))
-        import ref_shim
-        ref_shim.import_reference()
-        from funasr.models.contextual_paraformer.model import ContextualParaformer
-
-        class Dummy:
-            sos = 1
-        for src in ["Hello 你好 GPU xyz", str(txt)]:
-            want = ContextualParaformer.generate_hotwords_list(Dummy(), src, tokenizer=Tok(), frontend=fe)
-            assert generate_hotwords_list(src, Tok(), fe, sos=1) == want
+    import json
+    import make_live_golden as ml
+    assert (ml.HOTWORD_SEG_DICT, ml.HOTWORD_TXT, ml.HOTWORD_VOCAB) == ((tmp_path / "seg_dict").read_text(encoding="utf8"),
+                                                                      txt.read_text(encoding="utf8"), Tok.vocab)
+    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "live_reference.json")) as f:
+        want = json.load(f)["hotwords"]
+    assert generate_hotwords_list("Hello 你好 GPU xyz", Tok(), fe, sos=1) == want["string"]
+    assert generate_hotwords_list(str(txt), Tok(), fe, sos=1) == want["txt"]
 
 
 def test_bench_flop_model_matches_the_survey_figures():

@@ -1,6 +1,6 @@
 """Times the host-side (CPU) routines that sit behind the GPU path — the VAD end-point walk and the timestamp post-processing — in
 their Python-specification form and in the form the model classes run (library host code / vectorised).  No GPU needed.
-    python tools/host_probe.py > profiles/r2_host_routines.json"""
+    python tools/host_probe.py > host_routines.json"""
 import json
 import os
 import sys
