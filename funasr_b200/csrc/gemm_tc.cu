@@ -8,12 +8,14 @@
 // of the hot path (sanm/attention.py:256,306, transformer/positionwise_feed_forward.py:34,
 // sanm/positionwise_feed_forward.py:33, paraformer/decoder.py:444, cif conv as GEMM).
 //
-// Structure (one persistent CTA per SM, 384 threads, 128 x BN output tiles):
-//   warp 0     : TMA producer — cp.async.bulk.tensor.2d (SWIZZLE_128B) of the A/W plane tiles into a shared-memory ring
-//   warps 4-11 : two consumer warpgroups — each issues wgmma.mma_async m64nBNk16 for its 64 rows per K=16 slice and per split
-//                term (both operands from shared memory), keeping one k-block of MMAs in flight while the producer refills the
-//                ring; the accumulators are then parked in a shared-memory tile and the same eight warps run the epilogue
-//                (bias/ReLU/residuals -> fp32 rows to HBM, or fp16 planes for a following GEMM).
+// Structure (one persistent CTA per SM, 384 threads, 128 x BN output tiles, "ping-pong" schedule):
+//   warpgroup 0    : TMA producer — one elected lane of warp 0 issues cp.async.bulk.tensor.2d (SWIZZLE_128B) of the A/W plane
+//                    tiles into a shared-memory ring, in the order the MMAs consume them; the warpgroup gives its registers back
+//   warpgroups 1, 2: consumers — each owns whole 128 x BN tiles and takes every second tile of the CTA's persistent sequence.  An
+//                    ordering barrier pair hands the tensor pipe from one to the other: while one issues its tile's
+//                    wgmma.mma_async (two m64nBNk16 per K=16 slice and split term, one k-block of MMAs in flight), the other
+//                    runs the epilogue of its previous tile straight from its accumulator registers (bias/ReLU/residuals ->
+//                    fp32 rows to HBM, or fp16 planes for a following GEMM).
 #include "common.cuh"
 #include "kernels.h"
 #include "tc_common.cuh"
@@ -22,10 +24,12 @@
 
 namespace fa {
 
-constexpr int TC_BM = 128;      // tile rows: two consumer warpgroups of wgmma M = 64
+constexpr int TC_BM = 128;      // tile rows: two wgmma M = 64 halves, both issued by one consumer warpgroup
 constexpr int TC_BK = 64;       // one 128-byte swizzle span of fp16
 constexpr int TC_UK = 16;       // wgmma K for 16-bit inputs
 constexpr uint32_t TC_TILE_BYTES_A = TC_BM * TC_BK * 2;   // 16 KB per plane tile
+constexpr uint32_t TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
+constexpr uint32_t TC_ORDER_BAR = 1;   // named barriers 1, 2: "consumer warpgroup 0 / 1 may issue its tile's MMAs"
 
 // ------------------------------------------------------------------------------------------------ kernel
 struct TcParams {
@@ -59,18 +63,35 @@ static float rz_comp_scale(int kp, int n_terms) {
 __constant__ int c_term_a[6] = {0, 0, 1, 1, 0, 2};
 __constant__ int c_term_w[6] = {0, 1, 0, 1, 2, 0};
 
-// Epilogue of one accumulator tile.  Eight epilogue warps per CTA (two per SM sub-partition, so one warp's shared / global
-// latencies are hidden by the other): warp w drains rows [32 (w%4), +32) of the accumulator tile, every second 16-column chunk.
-//   phase 1  row-per-thread read of 16 fp32 accumulators -> a padded per-warp shared-memory tile [32][20]
+// Accumulators of one 128 x BN tile in a consumer warpgroup: d[h] is the m64 MMA over the tile's 8-row groups h, h + 2, h + 4, ..
+// (descriptor stride 2048 B), so warp q holds exactly rows [32 q, +32): lane l has rows 32 q + 16 e + 8 h + l / 4 (e = 0: registers
+// 4 j, 4 j + 1; e = 1: 4 j + 2, 4 j + 3) at columns 8 j + 2 (l % 4) + {0, 1}.
+//
+// Epilogue of one tile: warp q drains its 32 rows one 16-column chunk at a time.
+//   phase 1  the chunk's 16 accumulators per lane -> a padded per-warp shared-memory tile [32][20] (row = 32-row offset)
 //   phase 2  re-read with the warp laid out as 8 rows x 4 float4 columns, so bias / residual loads and every store are
 //            coalesced 16-byte (fp32) or 8-byte (fp16 plane) accesses; V columns of the attention sink take a
 //            column-per-lane path that writes the per-head transposed planes as 4 consecutive keys (8 bytes) per store.
+// The chunk loops are fully unrolled: the accumulator registers are indexed by compile-time constants only.
 constexpr int EPI_CH = 16;                       // columns per chunk
-constexpr int EPI_LD = 20;                       // padded row pitch (floats): 16-byte aligned, conflict-free float4 phases
-constexpr int EPI_WARP_FLOATS = 32 * EPI_LD;     // 2.5 KB per epilogue warp
+constexpr int EPI_LD = 20;                       // padded row pitch (floats): 16-byte aligned float4 rows
+constexpr int EPI_WARP_FLOATS = 32 * EPI_LD;     // 2.5 KB per consumer warp
 constexpr int EPI_WARPS = 8;
 
-// 32 rows (thread = row) x 16 consecutive fp32 columns of the shared-memory accumulator tile -> 16 registers
+template <int BN>
+__device__ __forceinline__ void acc_chunk_to_stage(const float (&d)[2][BN / 2], const int c0, float* stage, int lane) {
+  float* s = stage + (lane >> 2) * EPI_LD + 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int jj = 0; jj < 2; ++jj) {
+      const int j = c0 / 8 + jj;
+      *reinterpret_cast<float2*>(s + 8 * h * EPI_LD + 8 * jj) = make_float2(d[h][4 * j], d[h][4 * j + 1]);
+      *reinterpret_cast<float2*>(s + (16 + 8 * h) * EPI_LD + 8 * jj) = make_float2(d[h][4 * j + 2], d[h][4 * j + 3]);
+    }
+}
+
+// row `lane` (16 consecutive fp32 columns) of the staged chunk -> 16 registers
 __device__ __forceinline__ void acc_ld_32x16(const float* src, uint32_t (&r)[16]) {
 #pragma unroll
   for (int j = 0; j < 16; j += 4) {
@@ -160,13 +181,13 @@ __device__ __forceinline__ void store_vt_staged(plane_t* __restrict__ dst_g /* t
 //              registers on a deeper ring)
 constexpr int EPI_F32 = 0, EPI_PLANES = 1, EPI_ATT = 2, EPI_F32R2 = 3;
 
-// fp32-output interior tiles: the residual rows do not depend on the accumulator, so their loads are software pipelined one
-// chunk ahead (out-projection / FFN-w_2 epilogues are bound by memory-level parallelism).
-__device__ __forceinline__ void epilogue_fast_f32(const TcParams& p, const int BN, const float* acc, int64_t row0, int tile_col0, float* stage, int lane,
-                                                  int half) {
+// fp32-output interior tiles with two residuals: the residual rows do not depend on the accumulator, so their loads are software
+// pipelined one chunk ahead (out-projection / FFN-w_2 epilogues are bound by memory-level parallelism).
+template <int BN>
+__device__ __forceinline__ void epilogue_fast_f32(const TcParams& p, const float (&d)[2][BN / 2], int64_t row0, int tile_col0, float* stage,
+                                                  int lane) {
   const int rr0 = lane >> 2, c4 = (lane & 3) * 4;
   const int64_t rfirst = row0 + rr0;
-  float* srow = stage + lane * EPI_LD;
   const float* sp = stage + rr0 * EPI_LD + c4;
   float* c_row = p.C + rfirst * p.ldc + c4 + tile_col0;
   const float* r1_row = p.r1 ? p.r1 + rfirst * p.ldr1 + c4 + tile_col0 : nullptr;
@@ -182,19 +203,14 @@ __device__ __forceinline__ void epilogue_fast_f32(const TcParams& p, const int B
       nv2[it] = r2_row ? __ldg(reinterpret_cast<const float4*>(r2_row + c0 + it * s2)) : z4;
     }
   };
-  prefetch(half * EPI_CH);
-#pragma unroll 2
-  for (int c0 = half * EPI_CH; c0 < BN; c0 += 2 * EPI_CH) {
+  prefetch(0);
+#pragma unroll
+  for (int c0 = 0; c0 < BN; c0 += EPI_CH) {
     float4 rv1[4], rv2[4];
 #pragma unroll
     for (int it = 0; it < 4; ++it) { rv1[it] = nv1[it]; rv2[it] = nv2[it]; }
-    if (c0 + 2 * EPI_CH < BN) prefetch(c0 + 2 * EPI_CH);
-    {
-      uint32_t r[16];
-      acc_ld_32x16(acc + lane * (BN + 4) + c0, r);
-#pragma unroll
-      for (int j = 0; j < 16; j += 4) *reinterpret_cast<uint4*>(srow + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
-    }
+    if (c0 + EPI_CH < BN) prefetch(c0 + EPI_CH);
+    acc_chunk_to_stage<BN>(d, c0, stage, lane);
     __syncwarp();
     float4 bias4 = z4;
     if (p.bias) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + tile_col0 + c0 + c4));
@@ -215,65 +231,56 @@ __device__ __forceinline__ void epilogue_fast_f32(const TcParams& p, const int B
 }
 
 // The same for at most ONE residual (every fp32-output GEMM of the model: out-projection + x, FFN w_2 + x): the registers the second
-// residual's pipeline would hold become a 5-deep ring of the first's, so each warp keeps five 16-column chunks (10 KB) of residual
-// rows in flight instead of one.
-__device__ __forceinline__ void epilogue_fast_f32_r1(const TcParams& p, const int BN, const float* acc, int64_t row0, int tile_col0, float* stage,
-                                                     int lane, int half) {
+// residual's pipeline would hold become a RING-deep ring of the first's, so each warp keeps RING 16-column chunks of residual rows
+// in flight instead of one.
+template <int BN>
+__device__ __forceinline__ void epilogue_fast_f32_r1(const TcParams& p, const float (&d)[2][BN / 2], int64_t row0, int tile_col0, float* stage,
+                                                     int lane) {
   const int rr0 = lane >> 2, c4 = (lane & 3) * 4;
   const int64_t rfirst = row0 + rr0;
-  float* srow = stage + lane * EPI_LD;
   const float* sp = stage + rr0 * EPI_LD + c4;
   float* c_row = p.C + rfirst * p.ldc + c4 + tile_col0;
   const float* r_row = p.r1 ? p.r1 + rfirst * p.ldr1 + c4 + tile_col0 : nullptr;
   const int64_t sc = 8 * p.ldc, s1 = 8 * p.ldr1;
   const bool c_vec = (p.ldc & 3) == 0;
   const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-  const int cb = half * EPI_CH;                       // this warp's chunk i covers columns [cb + 32 i, +16)
-  constexpr int RING = 5;
+  constexpr int RING = 4;
+  constexpr int NCH = BN / EPI_CH;
   float4 ring[RING][4];
   auto fetch = [&](float4 (&dst)[4], int c0) {
 #pragma unroll
     for (int it = 0; it < 4; ++it) dst[it] = r_row ? __ldg(reinterpret_cast<const float4*>(r_row + c0 + it * s1)) : z4;
   };
 #pragma unroll
-  for (int i = 0; i < RING; ++i)
-    if (cb + 32 * i < BN) fetch(ring[i], cb + 32 * i);
+  for (int i = 0; i < RING && i < NCH; ++i) fetch(ring[i], EPI_CH * i);
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {                                      // BN <= 256: at most 8 chunks per warp
-    const int c0 = cb + 32 * i;
-    if (c0 < BN) {
-      {
-        uint32_t r[16];
-        acc_ld_32x16(acc + lane * (BN + 4) + c0, r);
+  for (int i = 0; i < NCH; ++i) {
+    const int c0 = EPI_CH * i;
+    acc_chunk_to_stage<BN>(d, c0, stage, lane);
+    __syncwarp();
+    float4 bias4 = z4;
+    if (p.bias) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + tile_col0 + c0 + c4));
+    float* pc = c_row + c0;
 #pragma unroll
-        for (int j = 0; j < 16; j += 4) *reinterpret_cast<uint4*>(srow + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
-      }
-      __syncwarp();
-      float4 bias4 = z4;
-      if (p.bias) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + tile_col0 + c0 + c4));
-      float* pc = c_row + c0;
-#pragma unroll
-      for (int it = 0; it < 4; ++it) {
-        const float4 acc = *reinterpret_cast<const float4*>(sp + it * 8 * EPI_LD);
-        const float4 rv = ring[i % RING][it];
-        float v0 = fmaf(acc.x, p.acc_scale, bias4.x), v1 = fmaf(acc.y, p.acc_scale, bias4.y), v2 = fmaf(acc.z, p.acc_scale, bias4.z), v3 = fmaf(acc.w, p.acc_scale, bias4.w);
-        if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f); }
-        v0 += rv.x; v1 += rv.y; v2 += rv.z; v3 += rv.w;
-        if (c_vec) *reinterpret_cast<float4*>(pc) = make_float4(v0, v1, v2, v3);
-        else { pc[0] = v0; pc[1] = v1; pc[2] = v2; pc[3] = v3; }
-        pc += sc;
-      }
-      __syncwarp();
-      if (c0 + 32 * RING < BN) fetch(ring[i % RING], c0 + 32 * RING);
+    for (int it = 0; it < 4; ++it) {
+      const float4 acc = *reinterpret_cast<const float4*>(sp + it * 8 * EPI_LD);
+      const float4 rv = ring[i % RING][it];
+      float v0 = fmaf(acc.x, p.acc_scale, bias4.x), v1 = fmaf(acc.y, p.acc_scale, bias4.y), v2 = fmaf(acc.z, p.acc_scale, bias4.z), v3 = fmaf(acc.w, p.acc_scale, bias4.w);
+      if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f); }
+      v0 += rv.x; v1 += rv.y; v2 += rv.z; v3 += rv.w;
+      if (c_vec) *reinterpret_cast<float4*>(pc) = make_float4(v0, v1, v2, v3);
+      else { pc[0] = v0; pc[1] = v1; pc[2] = v2; pc[3] = v3; }
+      pc += sc;
     }
+    __syncwarp();
+    if (i + RING < NCH) fetch(ring[i % RING], c0 + EPI_CH * RING);
   }
 }
 
 // Interior tiles (all 32 rows and all BN columns in range): straight-line code, no bounds predicates, every row base
 // computed once per tile and advanced by constant strides.
-template <int EPI, int NPL>
-__device__ __forceinline__ void epilogue_fast(const TcParams& p, const int BN, const float* acc, int64_t row0, int tile_col0, float* stage, int lane,
-                                              int half) {
+template <int BN, int EPI, int NPL>
+__device__ __forceinline__ void epilogue_fast(const TcParams& p, const float (&d)[2][BN / 2], int64_t row0, int tile_col0, float* stage, int lane) {
   const AttnSinks& a = p.att;
   constexpr int QPL = NPL < 2 ? NPL : 2;             // attention operands carry at most two planes
   const int rr0 = lane >> 2, c4 = (lane & 3) * 4;
@@ -281,12 +288,10 @@ __device__ __forceinline__ void epilogue_fast(const TcParams& p, const int BN, c
   float* srow = stage + lane * EPI_LD;
   const float* sp = stage + rr0 * EPI_LD + c4;
   float* c_row = (EPI != EPI_PLANES && p.C) ? p.C + rfirst * p.ldc + c4 : nullptr;
-  const float* r1_row = (EPI == EPI_F32 && p.r1) ? p.r1 + rfirst * p.ldr1 + c4 : nullptr;
-  const float* r2_row = (EPI == EPI_F32 && p.r2) ? p.r2 + rfirst * p.ldr2 + c4 : nullptr;
   plane_t* o_row = EPI == EPI_PLANES ? p.out_planes + rfirst * p.ldo + c4 : nullptr;
   plane_t* q_row = EPI == EPI_ATT ? a.q_planes + rfirst * a.width + c4 : nullptr;
   plane_t* k_row = EPI == EPI_ATT ? a.k_planes + rfirst * a.width + c4 : nullptr;
-  const int64_t sc = 8 * p.ldc, s1 = 8 * p.ldr1, s2 = 8 * p.ldr2, so = 8 * p.ldo, sq = 8 * (int64_t)a.width;
+  const int64_t sc = 8 * p.ldc, so = 8 * p.ldo, sq = 8 * (int64_t)a.width;
   const int64_t plane_o = p.M * p.ldo, plane_q = p.M * (int64_t)a.width;
   const bool c_vec = (p.ldc & 3) == 0;
   plane_t* vt_row = nullptr;
@@ -302,14 +307,16 @@ __device__ __forceinline__ void epilogue_fast(const TcParams& p, const int BN, c
     const int bg = (int)(rg / a.t_rows), tg = (int)(rg - (int64_t)bg * a.t_rows);
     vt_grp = a.vt_planes + (int64_t)bg * a.width * a.t_pad + tg;
   }
-#pragma unroll 1
-  for (int c0 = half * EPI_CH; c0 < BN; c0 += 2 * EPI_CH) {
+#pragma unroll
+  for (int c0 = 0; c0 < BN; c0 += EPI_CH) {
     const int col0 = tile_col0 + c0;
     const bool v_sink = EPI == EPI_ATT && col0 >= a.v0 && col0 < a.v0 + a.width;
-    {
+    acc_chunk_to_stage<BN>(d, c0, stage, lane);
+    __syncwarp();
+    if (EPI == EPI_ATT && v_sink) {
       uint32_t r[16];
-      acc_ld_32x16(acc + lane * (BN + 4) + c0, r);
-      if (EPI == EPI_ATT && v_sink && vt_staged) {
+      acc_ld_32x16(srow, r);
+      if (vt_staged) {
         float x[16];
 #pragma unroll
         for (int j = 0; j < 16; j += 4) {
@@ -318,41 +325,20 @@ __device__ __forceinline__ void epilogue_fast(const TcParams& p, const int BN, c
           x[j] = fmaf(__uint_as_float(r[j]), p.acc_scale, b4.x); x[j + 1] = fmaf(__uint_as_float(r[j + 1]), p.acc_scale, b4.y);
           x[j + 2] = fmaf(__uint_as_float(r[j + 2]), p.acc_scale, b4.z); x[j + 3] = fmaf(__uint_as_float(r[j + 3]), p.acc_scale, b4.w);
         }
-        store_vt_staged<QPL>(vt_grp + (int64_t)(col0 - a.v0) * a.t_pad, a.t_pad, vt_plane, x, stage, lane);   // ends with __syncwarp: stage is free again
-      }
-      if (EPI != EPI_ATT || !v_sink || p.C != nullptr) {
+        __syncwarp();                                  // every lane has its row: the transpose may overwrite the stage
+        store_vt_staged<QPL>(vt_grp + (int64_t)(col0 - a.v0) * a.t_pad, a.t_pad, vt_plane, x, stage, lane);   // ends with __syncwarp
+        if (c_row) {
 #pragma unroll
-        for (int j = 0; j < 16; j += 4) *reinterpret_cast<uint4*>(srow + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
-      }
-      if (EPI == EPI_ATT && v_sink && !vt_staged)
+          for (int j = 0; j < 16; j += 4) *reinterpret_cast<uint4*>(srow + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
+          __syncwarp();
+        }
+      } else {
         store_vt16<QPL>(vt_row + (int64_t)(col0 - a.v0) * a.t_pad, a.t_pad, vt_plane, r, p.bias ? p.bias + col0 : nullptr, p.acc_scale);
+      }
     }
-    __syncwarp();
     float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
     if (p.bias) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + c4));
-    if (EPI == EPI_F32) {
-      float* pc = c_row + col0;
-      const float* pr1 = r1_row ? r1_row + col0 : nullptr;
-      const float* pr2 = r2_row ? r2_row + col0 : nullptr;
-      // residual rows of all four passes are fetched up front (memory-level parallelism)
-      float4 rv1[4], rv2[4];
-#pragma unroll
-      for (int it = 0; it < 4; ++it) {
-        rv1[it] = pr1 ? __ldg(reinterpret_cast<const float4*>(pr1 + it * s1)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        rv2[it] = pr2 ? __ldg(reinterpret_cast<const float4*>(pr2 + it * s2)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-#pragma unroll
-      for (int it = 0; it < 4; ++it) {
-        const float4 acc = *reinterpret_cast<const float4*>(sp + it * 8 * EPI_LD);
-        float v0 = fmaf(acc.x, p.acc_scale, bias4.x), v1 = fmaf(acc.y, p.acc_scale, bias4.y), v2 = fmaf(acc.z, p.acc_scale, bias4.z), v3 = fmaf(acc.w, p.acc_scale, bias4.w);
-        if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f); }
-        v0 += rv1[it].x; v1 += rv1[it].y; v2 += rv1[it].z; v3 += rv1[it].w;
-        v0 += rv2[it].x; v1 += rv2[it].y; v2 += rv2[it].z; v3 += rv2[it].w;
-        if (c_vec) *reinterpret_cast<float4*>(pc) = make_float4(v0, v1, v2, v3);
-        else { pc[0] = v0; pc[1] = v1; pc[2] = v2; pc[3] = v3; }
-        pc += sc;
-      }
-    } else if (EPI == EPI_PLANES) {
+    if (EPI == EPI_PLANES) {
       plane_t* po = o_row + col0;
 #pragma unroll
       for (int it = 0; it < 4; ++it) {
@@ -392,100 +378,93 @@ __device__ __forceinline__ void epilogue_fast(const TcParams& p, const int BN, c
   }
 }
 
-// Edge tiles (row tail of M, ragged N such as vocab 8404 / 25055): every access bounds checked.
+// Edge tiles (row tail of M, ragged N such as vocab 8404 / 25055): one staged 16-column chunk, every access bounds checked.
+// Out of line: edge tiles are rare, and the call keeps the interior paths' code compact.
 template <int EPI, int NPL>
-__device__ __noinline__ void epilogue_edge(const TcParams& p, const int BN, const float* acc, int64_t row0, int tile_col0, float* stage, int lane,
-                                           int half) {
+__device__ __noinline__ void epilogue_edge_chunk(const TcParams& p, int64_t row0, int col0, float* stage, int lane) {
   const AttnSinks& a = p.att;
   constexpr int QPL = NPL < 2 ? NPL : 2;
-#pragma unroll 1
-  for (int c0 = half * EPI_CH; c0 < BN; c0 += 2 * EPI_CH) {
-    const int col0 = tile_col0 + c0;
-    {
-      uint32_t r[16];
-      acc_ld_32x16(acc + lane * (BN + 4) + c0, r);
-      float* srow = stage + lane * EPI_LD;
-#pragma unroll
-      for (int j = 0; j < 16; j += 4) *reinterpret_cast<uint4*>(srow + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
-      if (EPI == EPI_ATT && col0 >= a.v0 && col0 < a.v0 + a.width && row0 + lane < p.M) {
-        const int64_t rw = row0 + lane;
-        const int b2 = (int)(rw / a.t_rows), t2 = (int)(rw - (int64_t)b2 * a.t_rows);
-        store_vt16<QPL>(a.vt_planes + ((int64_t)b2 * a.width + (col0 - a.v0)) * a.t_pad + t2, a.t_pad,
-                        (p.M / a.t_rows) * (int64_t)a.width * a.t_pad, r, p.bias ? p.bias + col0 : nullptr, p.acc_scale);
+  if (EPI == EPI_ATT && col0 >= a.v0 && col0 < a.v0 + a.width && row0 + lane < p.M) {
+    uint32_t r[16];
+    acc_ld_32x16(stage + lane * EPI_LD, r);
+    const int64_t rw = row0 + lane;
+    const int b2 = (int)(rw / a.t_rows), t2 = (int)(rw - (int64_t)b2 * a.t_rows);
+    store_vt16<QPL>(a.vt_planes + ((int64_t)b2 * a.width + (col0 - a.v0)) * a.t_pad + t2, a.t_pad,
+                    (p.M / a.t_rows) * (int64_t)a.width * a.t_pad, r, p.bias ? p.bias + col0 : nullptr, p.acc_scale);
+  }
+  if (col0 < p.N && row0 < p.M) {
+    const bool full = col0 + EPI_CH <= p.N;
+    const bool v_sink = EPI == EPI_ATT && col0 >= a.v0 && col0 < a.v0 + a.width;
+    const bool q_sink = EPI == EPI_ATT && col0 >= a.q0 && col0 < a.q0 + a.width;
+    const bool k_sink = EPI == EPI_ATT && col0 >= a.k0 && col0 < a.k0 + a.width;
+    const bool want_c = EPI == EPI_F32 ? true : (EPI == EPI_ATT ? (p.C != nullptr && v_sink) : false);
+    if (EPI != EPI_ATT || want_c || q_sink || k_sink) {
+      const int rr0 = lane >> 2, c4 = (lane & 3) * 4;
+      const int col = col0 + c4;
+      const int64_t rfirst = row0 + rr0;
+      const int rows_left = (int)((p.M - rfirst + 7) >> 3);        // passes (of 8 rows) with a valid row for this lane
+      float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (p.bias) {
+        if (full) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
+        else { float* bp = reinterpret_cast<float*>(&bias4); for (int e = 0; e < 4; ++e) if (col + e < p.N) bp[e] = __ldg(p.bias + col + e); }
       }
-    }
-    __syncwarp();
-    if (col0 < p.N && row0 < p.M) {
-      const bool full = col0 + EPI_CH <= p.N;
-      const bool v_sink = EPI == EPI_ATT && col0 >= a.v0 && col0 < a.v0 + a.width;
-      const bool q_sink = EPI == EPI_ATT && col0 >= a.q0 && col0 < a.q0 + a.width;
-      const bool k_sink = EPI == EPI_ATT && col0 >= a.k0 && col0 < a.k0 + a.width;
-      const bool want_c = EPI == EPI_F32 ? true : (EPI == EPI_ATT ? (p.C != nullptr && v_sink) : false);
-      if (EPI != EPI_ATT || want_c || q_sink || k_sink) {
-        const int rr0 = lane >> 2, c4 = (lane & 3) * 4;
-        const int col = col0 + c4;
-        const int64_t rfirst = row0 + rr0;
-        const int rows_left = (int)((p.M - rfirst + 7) >> 3);        // passes (of 8 rows) with a valid row for this lane
-        float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (p.bias) {
-          if (full) bias4 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-          else { float* bp = reinterpret_cast<float*>(&bias4); for (int e = 0; e < 4; ++e) if (col + e < p.N) bp[e] = __ldg(p.bias + col + e); }
-        }
-        const float* sp = stage + rr0 * EPI_LD + c4;
-        const bool c_vec = (p.ldc & 3) == 0;
-        for (int it = 0; it < 4 && it < rows_left; ++it) {
-          const int64_t row = rfirst + 8 * it;
-          const float4 acc = *reinterpret_cast<const float4*>(sp + it * 8 * EPI_LD);
-          float vv[4] = {fmaf(acc.x, p.acc_scale, bias4.x), fmaf(acc.y, p.acc_scale, bias4.y), fmaf(acc.z, p.acc_scale, bias4.z), fmaf(acc.w, p.acc_scale, bias4.w)};
-          if (p.relu) { for (int e = 0; e < 4; ++e) vv[e] = fmaxf(vv[e], 0.f); }
-          if (full) {
-            if (EPI == EPI_F32) {
-              for (int e = 0; e < 4; ++e) {
-                if (p.r1) vv[e] += __ldg(p.r1 + row * p.ldr1 + col + e);
-                if (p.r2) vv[e] += __ldg(p.r2 + row * p.ldr2 + col + e);
-              }
-            }
-            if (want_c) {
-              float* pc = p.C + row * p.ldc + col;
-              if (c_vec) *reinterpret_cast<float4*>(pc) = make_float4(vv[0], vv[1], vv[2], vv[3]);
-              else { pc[0] = vv[0]; pc[1] = vv[1]; pc[2] = vv[2]; pc[3] = vv[3]; }
-            }
-            if (EPI == EPI_PLANES) store_planes4<NPL>(p.out_planes + row * p.ldo + col, p.M * p.ldo, vv[0], vv[1], vv[2], vv[3]);
-            if (q_sink) store_planes4<QPL>(a.q_planes + row * a.width + (col - a.q0), p.M * (int64_t)a.width, __fmul_rn(vv[0], a.qscale),
-                                           __fmul_rn(vv[1], a.qscale), __fmul_rn(vv[2], a.qscale), __fmul_rn(vv[3], a.qscale));
-            if (k_sink) store_planes4<QPL>(a.k_planes + row * a.width + (col - a.k0), p.M * (int64_t)a.width, vv[0], vv[1], vv[2], vv[3]);
-          } else {                                                   // ragged N tail: scalar (fp32 output only)
+      const float* sp = stage + rr0 * EPI_LD + c4;
+      const bool c_vec = (p.ldc & 3) == 0;
+      for (int it = 0; it < 4 && it < rows_left; ++it) {
+        const int64_t row = rfirst + 8 * it;
+        const float4 acc = *reinterpret_cast<const float4*>(sp + it * 8 * EPI_LD);
+        float vv[4] = {fmaf(acc.x, p.acc_scale, bias4.x), fmaf(acc.y, p.acc_scale, bias4.y), fmaf(acc.z, p.acc_scale, bias4.z), fmaf(acc.w, p.acc_scale, bias4.w)};
+        if (p.relu) { for (int e = 0; e < 4; ++e) vv[e] = fmaxf(vv[e], 0.f); }
+        if (full) {
+          if (EPI == EPI_F32) {
             for (int e = 0; e < 4; ++e) {
-              if (col + e >= p.N) break;
-              float x = vv[e];
-              if (p.r1) x += __ldg(p.r1 + row * p.ldr1 + col + e);
-              if (p.r2) x += __ldg(p.r2 + row * p.ldr2 + col + e);
-              if (want_c) p.C[row * p.ldc + col + e] = x;
+              if (p.r1) vv[e] += __ldg(p.r1 + row * p.ldr1 + col + e);
+              if (p.r2) vv[e] += __ldg(p.r2 + row * p.ldr2 + col + e);
             }
+          }
+          if (want_c) {
+            float* pc = p.C + row * p.ldc + col;
+            if (c_vec) *reinterpret_cast<float4*>(pc) = make_float4(vv[0], vv[1], vv[2], vv[3]);
+            else { pc[0] = vv[0]; pc[1] = vv[1]; pc[2] = vv[2]; pc[3] = vv[3]; }
+          }
+          if (EPI == EPI_PLANES) store_planes4<NPL>(p.out_planes + row * p.ldo + col, p.M * p.ldo, vv[0], vv[1], vv[2], vv[3]);
+          if (q_sink) store_planes4<QPL>(a.q_planes + row * a.width + (col - a.q0), p.M * (int64_t)a.width, __fmul_rn(vv[0], a.qscale),
+                                         __fmul_rn(vv[1], a.qscale), __fmul_rn(vv[2], a.qscale), __fmul_rn(vv[3], a.qscale));
+          if (k_sink) store_planes4<QPL>(a.k_planes + row * a.width + (col - a.k0), p.M * (int64_t)a.width, vv[0], vv[1], vv[2], vv[3]);
+        } else {                                                   // ragged N tail: scalar (fp32 output only)
+          for (int e = 0; e < 4; ++e) {
+            if (col + e >= p.N) break;
+            float x = vv[e];
+            if (p.r1) x += __ldg(p.r1 + row * p.ldr1 + col + e);
+            if (p.r2) x += __ldg(p.r2 + row * p.ldr2 + col + e);
+            if (want_c) p.C[row * p.ldc + col + e] = x;
           }
         }
       }
     }
-    __syncwarp();
   }
 }
 
-// BN: columns of this accumulator tile; acc: the warp's first row of the accumulator tile in shared memory (pitch BN + 4)
-template <int EPI, int NPL>
-__device__ __forceinline__ void epilogue_warp(const TcParams& p, const int BN, const float* acc, int64_t row0, int tile_col0, float* stage, int lane,
-                                              int half) {
+// row0: the warp's first row (32 rows per warp); tile_col0: the tile's first column
+template <int BN, int EPI, int NPL>
+__device__ __forceinline__ void epilogue_warp(const TcParams& p, const float (&d)[2][BN / 2], int64_t row0, int tile_col0, float* stage, int lane) {
   constexpr int EPIB = EPI == EPI_F32R2 ? EPI_F32 : EPI;
   const bool interior = row0 + 32 <= p.M && tile_col0 + BN <= p.N;
-  if (EPI == EPI_F32 && interior) {
-    epilogue_fast_f32_r1(p, BN, acc, row0, tile_col0, stage, lane, half);
-    return;
+  if (!interior) {
+#pragma unroll
+    for (int c0 = 0; c0 < BN; c0 += EPI_CH) {
+      acc_chunk_to_stage<BN>(d, c0, stage, lane);
+      __syncwarp();
+      epilogue_edge_chunk<EPIB, NPL>(p, row0, tile_col0 + c0, stage, lane);
+      __syncwarp();
+    }
+  } else if constexpr (EPI == EPI_F32) {
+    epilogue_fast_f32_r1<BN>(p, d, row0, tile_col0, stage, lane);
+  } else if constexpr (EPI == EPI_F32R2) {
+    epilogue_fast_f32<BN>(p, d, row0, tile_col0, stage, lane);
+  } else {
+    epilogue_fast<BN, EPI, NPL>(p, d, row0, tile_col0, stage, lane);
   }
-  if (EPI == EPI_F32R2 && interior) {
-    epilogue_fast_f32(p, BN, acc, row0, tile_col0, stage, lane, half);
-    return;
-  }
-  if (interior) epilogue_fast<EPIB, NPL>(p, BN, acc, row0, tile_col0, stage, lane, half);
-  else epilogue_edge<EPIB, NPL>(p, BN, acc, row0, tile_col0, stage, lane, half);
 }
 
 template <int BN>
@@ -494,17 +473,21 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t a_desc, 
   else wgmma_m64n64_ss(d, a_desc, b_desc, accumulate);
 }
 
+// Tile order and hand-offs.  The CTA's tiles are j = 0 .. T-1 (tile blockIdx.x + j gridDim.x); consumer warpgroup c takes
+// j = c, c + 2, ..; the producer loads every tile's k-blocks in j order, so the ring slot of (j, kb) is (j k_blocks + kb) % STAGES.
+// Ordering barrier ORDER_BAR + c ("c may issue"): before tile j > 0 its consumer waits on it (bar.sync), after issuing tile j's MMAs
+// its consumer signals the other's (bar.arrive) only if tile j + 1 exists.  So every wait is matched by exactly one signal and no
+// signal is left unmatched, for any T >= 1 (T = 1: consumer 1 has no tile and never touches the barriers; odd T: consumer 0's
+// last tile signals nothing).  A barrier cannot be signalled twice before it is waited on: the two consumers strictly alternate.
 template <int BN, int STAGES, int APL, int WPL, int EPI>  // APL / WPL: A / W planes resident per stage
 __global__ void __launch_bounds__(384, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w, const __grid_constant__ TcParams p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   constexpr uint32_t TILE_W_BYTES = BN * TC_BK * 2;
   constexpr uint32_t STAGE_BYTES = APL * TC_TILE_BYTES_A + WPL * TILE_W_BYTES;
-  constexpr int ACC_LD = BN + 4;
   // align to 1024 B WITHOUT leaving the shared address space (a uintptr_t round trip makes every access a generic LD/ST)
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  float* acc_tile = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);          // [TC_BM][ACC_LD]
-  float* epi_stage = acc_tile + TC_BM * ACC_LD;                                       // 8 x [32][20] floats
+  float* epi_stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);          // 8 x [32][20] floats
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + EPI_WARPS * EPI_WARP_FLOATS);
   uint64_t* empty_bar = full_bar + STAGES;
 
@@ -517,16 +500,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     tma_prefetch_desc(&map_w);
   }
   if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], EPI_WARPS); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }   // emptied by the 4 warps of one consumer
     fence_barrier_init();
   }
   __syncthreads();
   pdl_wait();                                          // prologue above is global-memory free; operands are read below
   pdl_trigger();
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (elect_one_sync()) {
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
+    if (warp == 0 && elect_one_sync()) {
       int stage = 0; uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const int tm = tile / p.tiles_n, tn = tile - tm * p.tiles_n;
@@ -544,25 +528,37 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         }
       }
     }
-  } else if (warp >= 4) {
-    // ===================== consumers: warpgroup wg = rows [64 wg, +64) of the tile; then all eight warps run the epilogue =====
-    const int wg = (warp - 4) >> 2, q = warp & 3;
-    int stage = 0; uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+  } else {
+    // ===================== consumers: warpgroup cw owns tiles j = cw, cw + 2, ..; warp q drains rows [32 q, +32) =====================
+    setmaxnreg_inc<TC_CONSUMER_REGS>();
+    const int cw = (warp >> 2) - 1, q = warp & 3;
+    const int n_local = (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1;     // grid <= n_tiles: every CTA has a tile
+    float* stage_w = epi_stage + (warp - 4) * EPI_WARP_FLOATS;
+    for (int j = cw; j < n_local; j += 2) {
+      const int tile = blockIdx.x + j * gridDim.x;
       const int tm = tile / p.tiles_n, tn = tile - tm * p.tiles_n;
-      float d[BN / 2];
+      const int it0 = j * k_blocks;
+      int stage = it0 % STAGES; uint32_t phase = (uint32_t)(it0 / STAGES) & 1u;
+      float d[2][BN / 2];
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) d[h][i] = 0.f;
+      if (j > 0) named_bar(TC_ORDER_BAR + cw, 256);    // the other consumer has issued tile j - 1
       int prev = -1;
       for (int kb = 0; kb < k_blocks; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t st = smem_u32(smem + stage * STAGE_BYTES);
         wgmma_fence();
         for (int t = 0; t < p.n_terms; ++t) {
-          const uint64_t da = make_sw128_desc(st + c_term_a[t] * TC_TILE_BYTES_A + wg * (64 * 128));
+          const uint64_t da = make_sw128_desc(st + c_term_a[t] * TC_TILE_BYTES_A, 2048);    // 8-row groups 0, 2, ..; + 64 (1024 B): 1, 3, ..
           const uint64_t dw = make_sw128_desc(st + APL * TC_TILE_BYTES_A + c_term_w[t] * TILE_W_BYTES);
 #pragma unroll
-          for (int k = 0; k < TC_BK / TC_UK; ++k) wgmma_tile<BN>(d, da + 2 * k, dw + 2 * k, (kb | t | k) != 0 ? 1u : 0u);
+          for (int k = 0; k < TC_BK / TC_UK; ++k) {
+            const uint32_t acc = (kb | t | k) != 0 ? 1u : 0u;
+            wgmma_tile<BN>(d[0], da + 2 * k, dw + 2 * k, acc);
+            wgmma_tile<BN>(d[1], da + 64 + 2 * k, dw + 2 * k, acc);
+          }
         }
         wgmma_commit();
         wgmma_wait_pending1();                         // the previous k-block's MMAs have retired: its ring slot is free
@@ -570,19 +566,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      if (j + 1 < n_local) named_bar_arrive(TC_ORDER_BAR + (cw ^ 1), 256);   // tile j + 1 may queue its MMAs behind this tile's last k-block
       wgmma_wait_all();
-      wgmma_fence_regs(d);
+      wgmma_fence_regs(d[0]);
+      wgmma_fence_regs(d[1]);
       if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty_bar[prev]); }
-      named_bar(1, 256);                               // the previous tile's epilogue has read the accumulator tile
-      float* arow = acc_tile + (64 * wg + 16 * q + (lane >> 2)) * ACC_LD + 2 * (lane & 3);
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        *reinterpret_cast<float2*>(arow + 8 * j) = make_float2(d[4 * j], d[4 * j + 1]);
-        *reinterpret_cast<float2*>(arow + 8 * ACC_LD + 8 * j) = make_float2(d[4 * j + 2], d[4 * j + 3]);
-      }
-      named_bar(1, 256);
-      epilogue_warp<EPI, APL>(p, BN, acc_tile + q * 32 * ACC_LD, (int64_t)tm * TC_BM + q * 32, tn * BN,
-                              epi_stage + (warp - 4) * EPI_WARP_FLOATS, lane, wg);
+      epilogue_warp<BN, EPI, APL>(p, d, (int64_t)tm * TC_BM + q * 32, tn * BN, stage_w, lane);
     }
   }
 }
@@ -677,8 +666,8 @@ size_t gemm_tc_scratch_bytes(int64_t max_rows, int max_k, int mode) {
 
 template <int BN, int STAGES, int APL, int WPL, int EPI>
 static int launch_cfg_e(const CUtensorMap& ma, const CUtensorMap& mw, const TcParams& p, cudaStream_t st) {
-  constexpr size_t smem = (size_t)STAGES * (APL * TC_TILE_BYTES_A + WPL * BN * TC_BK * 2) + 1024 + (size_t)TC_BM * (BN + 4) * 4 +
-                          EPI_WARPS * EPI_WARP_FLOATS * 4 + 2 * STAGES * 8;
+  constexpr size_t smem = (size_t)STAGES * (APL * TC_TILE_BYTES_A + WPL * BN * TC_BK * 2) + 1024 + EPI_WARPS * EPI_WARP_FLOATS * 4 +
+                          2 * STAGES * 8;
   static_assert(smem <= 227 * 1024, "shared memory per block");
   static PerDeviceOnce once;
   FA_RETURN_IF_ERR(ensure_dyn_smem(gemm_tc_kernel<BN, STAGES, APL, WPL, EPI>, smem, once));
@@ -716,7 +705,8 @@ int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& li
   if (y && (ldy & 3) == 0 && (((uintptr_t)y) & 15)) return FA_ERR_UNSUPPORTED;
   if ((r1 && (ld1 & 3)) || (r2 && (ld2 & 3))) return FA_ERR_UNSUPPORTED;
   const int npl = planes_for_mode(mode);
-  // 128 x 128 tiles (64 wide for x6: three planes per operand, two ring stages and the accumulator tile fill the 227 KB).
+  // 128 x 128 tiles with a 6 (x1) / 3 (x3) stage ring; 128 x 64 for x6 (three planes per operand: two 72 KB stages, a third does
+  // not fit beside the epilogue staging in 227 KB).
   // Ragged N (the vocabulary projections: 8404, 25055): the last column tile's W box reaches past row N of a plane — into the next
   // plane's first rows or, for the last plane, out of the tensor map (zero fill) — so its surplus accumulator columns hold finite
   // garbage that the bounds-checked edge epilogue never stores.
@@ -736,8 +726,8 @@ int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& li
   if (att && (N % 32 != 0 || att->width % 32 != 0 || att->t_rows <= 0 || M % att->t_rows != 0)) return FA_ERR_UNSUPPORTED;
   if (out_planes && (N % 32 != 0)) return FA_ERR_UNSUPPORTED;
   switch (npl) {
-    case 1: return launch_cfg<128, 4, 1, 1>(ma, mw, p, st);
-    case 2: return launch_cfg<128, 2, 2, 2>(ma, mw, p, st);
+    case 1: return launch_cfg<128, 6, 1, 1>(ma, mw, p, st);
+    case 2: return launch_cfg<128, 3, 2, 2>(ma, mw, p, st);
     default: return launch_cfg<64, 2, 3, 3>(ma, mw, p, st);
   }
 }

@@ -55,6 +55,17 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
 __device__ __forceinline__ void named_bar(uint32_t id, uint32_t threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
+// signal named barrier `id` without waiting: the other `threads` - (this warp group) threads complete it with named_bar
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// per-thread register budget of the executing warpgroup (all four warps execute it): producer warpgroups give registers back,
+// consumer warpgroups take them (the sum over the CTA must stay within the launch's allocation)
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ------------------------------------------------------------------------------------------------ wgmma
 // A warpgroup (4 consecutive warps) issues one wgmma.mma_async for a 64 x N x 16 product; D lives in registers with the
@@ -116,11 +127,12 @@ __device__ __forceinline__ float plane_to_float(plane_t h) { return __half2float
 
 // K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma (tile rows at 128-byte pitch, 8-row groups 1024 B apart, the
 // tile 1024-byte aligned).  Advancing the start address by 32 bytes (+2) steps K by 16 fp16 inside the 128-byte swizzle span.
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
+// sbo_bytes: distance between the 8-row groups the MMA reads (2048 = every second group of the tile).
+__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t sbo_bytes = 1024) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // start address, 16-byte units      bits [0,14)
   d |= (uint64_t)1 << 16;                             // leading byte offset (unused for swizzled K-major) [16,30)
-  d |= (uint64_t)(1024 >> 4) << 32;                   // stride byte offset: 8 rows x 128 B [32,46)
+  d |= (uint64_t)(sbo_bytes >> 4) << 32;              // stride byte offset between 8-row groups [32,46)
   d |= (uint64_t)1 << 62;                             // layout: SWIZZLE_128B               [62,64)
   return d;
 }
