@@ -22,5 +22,7 @@ from .long_audio import LongAudioPipeline, merge_results, pack_segments  # noqa:
 from .punc import CTTransformerB200, PuncEngine, split_to_mini_sentence, split_words  # noqa: F401
 from .audio import decode_pcm, load_audio, parse_wav_header  # noqa: F401
 from .hotwords import generate_hotwords_list, load_seg_dict, seg_tokenize  # noqa: F401
+from .campplus import CAMPPlusB200, CampplusEngine  # noqa: F401
+from . import diarization  # noqa: F401
 
 __version__ = "0.1.0"

@@ -76,6 +76,25 @@ class FaVadOptions(C.Structure):
                [(n, C.c_double) for n in ("speech_2_noise_ratio", "snr_thres", "decibel_thres", "speech_noise_thres", "fe_prior_thres")]
 
 
+class FaCamConv2d(C.Structure):
+    _fields_ = [("w", C.c_void_p), ("b", C.c_void_p), ("c_in", C.c_int32), ("c_out", C.c_int32), ("ksize", C.c_int32), ("stride_f", C.c_int32)]
+
+
+class FaCamLayer(C.Structure):
+    _fields_ = [("bn1_scale", C.c_void_p), ("bn1_shift", C.c_void_p), ("linear1", FaLinear), ("local_w", C.c_void_p), ("w1", C.c_void_p),
+                ("b1", C.c_void_p), ("w2", C.c_void_p), ("b2", C.c_void_p)]
+
+
+class FaCamTransit(C.Structure):
+    _fields_ = [("scale", C.c_void_p), ("shift", C.c_void_p), ("linear", FaLinear)]
+
+
+class FaCampplus(C.Structure):
+    _fields_ = [("fcm", FaCamConv2d * 12), ("tdnn", FaLinear), ("layers", C.POINTER(FaCamLayer)), ("n_layers", C.c_int32 * 3),
+                ("dilation", C.c_int32 * 3), ("transit", FaCamTransit * 3), ("out_scale", C.c_void_p), ("out_shift", C.c_void_p),
+                ("dense", FaLinear)]
+
+
 _vp, _i32, _i64, _sz, _f = C.c_void_p, C.c_int32, C.c_int64, C.c_size_t, C.c_float
 
 # name -> (restype, argtypes); every symbol include/funasr_b200.h declares
@@ -132,6 +151,13 @@ SIGNATURES = {
     "fa_embedding": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _vp, _vp]),
     "fa_pcm_decode": (C.c_int, [_vp, _i32, _i32, _i64, _vp, _vp]),
     "fa_resample": (C.c_int, [_vp, _vp, _i32, _i64, _vp, _i32, _i32, _i32, _vp, _i64, _i32, _vp, _vp]),
+    # CAM++ speaker embedding (campplus.cu)
+    "fa_campplus_features": (C.c_int, [_vp, _vp, _i32, _i64, _vp, _vp, _vp, _i32, _vp]),
+    "fa_campplus_workspace_bytes": (_sz, [C.POINTER(FaCampplus), _i32, _i32, _i32]),
+    "fa_campplus_forward": (C.c_int, [C.POINTER(FaCampplus), _vp, _i32, _i32, _vp, _i32, _vp, _sz, _vp]),
+    "fa_campplus_conv2d": (C.c_int, [C.POINTER(FaCamConv2d), _vp, _i32, _i32, _i32, _vp, _vp, _i32, _vp]),
+    "fa_campplus_cam": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "fa_campplus_stats_pool": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     # handle-style offline recogniser (funasrruntime.h:100-116 counterpart; offline.cu)
     "fa_offline_init": (_vp, [C.c_char_p, _i32, _i32]),
     "fa_offline_infer": (_vp, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32]),

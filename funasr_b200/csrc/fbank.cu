@@ -302,7 +302,7 @@ template <int kLfrM, int kLfrN, int kRows>
 __global__ void __launch_bounds__(kWarps * 32, 3)
 fbank_tab_kernel(const float* __restrict__ wav, const int32_t* __restrict__ wav_lens, int64_t wav_stride, const float* __restrict__ cmvn,
                  const float* __restrict__ tables, float* __restrict__ feats, int32_t* __restrict__ feat_lens, int t_max,
-                 int64_t batch_stride_rows) {
+                 int64_t batch_stride_rows, float wav_scale) {
   constexpr int kFeat = kMel * kLfrM;
   static_assert(kLfrN * (kRows - 1) + kLfrM <= kFramesMax, "too many frames per CTA");
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -353,7 +353,7 @@ fbank_tab_kernel(const float* __restrict__ wav, const int32_t* __restrict__ wav_
   const float* wb = wav + (int64_t)b * wav_stride;
   const bool vec2 = ((reinterpret_cast<uintptr_t>(wb) & 7) == 0);     // frames start at multiples of 160 samples
   for (int f = warp; f < nfr; f += kWarps) {
-    frame_spectrum(wb + (int64_t)(f_lo + f) * kShift, 32768.0f, vec2, s.win, lt, lane, Zs);
+    frame_spectrum(wb + (int64_t)(f_lo + f) * kShift, wav_scale, vec2, s.win, lt, lane, Zs);
     // power spectrum of the real signal: P[k] and P[256 - k] from the same Z[k], Z[256 - k]
     auto Z = [&](int k) -> float2 { return Zs[(k & 7) * kZs + (k >> 3)]; };
     auto pair = [&](int k) {
@@ -486,12 +486,13 @@ __global__ void fbank_tables_kernel(const float* __restrict__ mel_banks, const f
 
 template <int M, int N, int ROWS>
 static int fbank_tab_launch(const float* wav, const int32_t* wav_lens, int batch, int64_t wav_stride, const float* cmvn, const float* tables,
-                            float* feats, int64_t stride_rows, int32_t* feat_lens, int t_max, cudaStream_t st) {
+                            float* feats, int64_t stride_rows, int32_t* feat_lens, int t_max, cudaStream_t st, float wav_scale = 32768.0f) {
   const size_t smem = sizeof(FbankSmemT);
   static PerDeviceOnce once;
   FA_RETURN_IF_ERR(ensure_dyn_smem(fbank_tab_kernel<M, N, ROWS>, smem, once));
   dim3 grid((t_max + ROWS - 1) / ROWS, batch);
-  fbank_tab_kernel<M, N, ROWS><<<grid, kWarps * 32, smem, st>>>(wav, wav_lens, wav_stride, cmvn, tables, feats, feat_lens, t_max, stride_rows);
+  fbank_tab_kernel<M, N, ROWS><<<grid, kWarps * 32, smem, st>>>(wav, wav_lens, wav_stride, cmvn, tables, feats, feat_lens, t_max, stride_rows,
+                                                                wav_scale);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }
@@ -566,6 +567,13 @@ fbank_short_kernel(const float* __restrict__ wav, int n, const float* __restrict
     if (cmvn != nullptr) v = __fmul_rn(__fadd_rn(v, cmvn[idx]), cmvn[lfr_m * kMel + idx]);
     out[idx] = v;
   }
+}
+
+// CAM++ frontend (campplus/utils.py extract_feature: torchaudio kaldi.fbank with its defaults): the waveform is NOT scaled by 32768,
+// no LFR stacking (1 / 1), no CMVN; the window (povey) comes with the tables.  feats [B, t_max, 80].
+int fbank_unscaled_launch(const float* wav, const int32_t* wav_lens, int batch, int64_t wav_stride, const float* tables, float* feats,
+                          int32_t* feat_lens, int t_max, cudaStream_t st) {
+  return fbank_tab_launch<1, 1, 48>(wav, wav_lens, batch, wav_stride, nullptr, tables, feats, t_max, feat_lens, t_max, st, 1.0f);
 }
 
 }  // namespace fa

@@ -69,6 +69,9 @@ int cif_fire_launch(const float* enc, const float* alpha_rows, const int32_t* le
                     cudaStream_t st);
 int ctc_filter_launch(const int32_t* ids, const int32_t* lens, int batch, int t_max, int blank, int32_t* out_ids,
                       int32_t* out_lens, cudaStream_t st);
+// torchaudio kaldi.fbank defaults (no x32768, no LFR, no CMVN) through the table-driven kernel (fbank.cu): the CAM++ frontend
+int fbank_unscaled_launch(const float* wav, const int32_t* wav_lens, int batch, int64_t wav_stride, const float* tables, float* feats,
+                          int32_t* feat_lens, int t_max, cudaStream_t st);
 int argmax_lse_launch(float* logits, int64_t rows, int vocab, int64_t ld, int32_t* ids, float* best_logp,
                       int write_log_softmax, cudaStream_t st);
 

@@ -77,6 +77,7 @@ DROP_IN_KEYS = {
     ("model_classes", "SenseVoiceSmall"): "SenseVoiceSmallB200",
     ("encoder_classes", "SenseVoiceEncoderSmall"): "SenseVoiceEncoderSmallB200",
     ("decoder_classes", "ParaformerSANMDecoder"): "ParaformerSANMDecoderB200",
+    ("model_classes", "CAMPPlus"): "CAMPPlusB200",
 }
 
 

@@ -499,3 +499,72 @@ def make_punc_text(n_words: int, seed: int = 0) -> str:
         else:
             out.append(toks[3 + int(torch.randint(0, PUNC_VOCAB - 4 - 16, (1,), generator=g))])
     return "".join(out).replace("  ", " ").strip()
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# CAM++ speaker model (funasr/models/campplus: template.yaml) and multi-speaker recordings
+# ------------------------------------------------------------------------------------------------------------------
+def make_campplus_state_dict(seed: int = 0, bn_stats=None) -> "OrderedDict[str, torch.Tensor]":
+    """CAMPPlus weights under the reference's names (campplus_specs): kaiming-normal convs (the reference's own init for Conv1d),
+    BatchNorm affines near identity, running statistics mean 0 / var 1.  bn_stats: {name: tensor} overlaid on the running statistics
+    (the calibrated ones the fixtures store: with identity statistics random-weight embeddings of different voices collapse)."""
+    from .campplus import campplus_specs
+    g = torch.Generator().manual_seed(60013 * seed + 5)
+    sd: "OrderedDict[str, torch.Tensor]" = OrderedDict()
+    for name, shape in campplus_specs().items():
+        leaf = name.rsplit(".", 1)[1]
+        if leaf == "num_batches_tracked":
+            sd[name] = torch.tensor(0, dtype=torch.long)
+        elif leaf == "running_mean":
+            sd[name] = torch.zeros(shape)
+        elif leaf == "running_var":
+            sd[name] = torch.ones(shape)
+        elif len(shape) == 1:       # BN affine or conv bias
+            is_bn_w = leaf == "weight"
+            sd[name] = (1.0 + _randn(g, *shape, std=0.1)) if is_bn_w else _randn(g, *shape, std=0.05)
+        else:
+            fan_in = int(math.prod(shape[1:]))
+            sd[name] = _randn(g, *shape, std=math.sqrt(2.0 / fan_in))
+    for k, v in (bn_stats or {}).items():
+        sd[k] = torch.as_tensor(v).to(sd[k].dtype).reshape(sd[k].shape).clone()
+    return sd
+
+
+# (f0 Hz, formant Hz, syllable rate Hz) of the synthetic voices
+VOICES = [(110.0, 700.0, 2.5), (230.0, 1800.0, 7.0), (160.0, 1200.0, 4.5)]
+
+
+def make_voice_wav(pattern, seed: int = 0, lead_s: float = 0.5) -> torch.Tensor:
+    """Multi-speaker 16 kHz test audio: pattern [(voice index, speech_s, silence_s), ...].  Every voice is a harmonic stack on its own
+    f0 with intonation, shaped by one formant resonance that moves with the voice's own syllable rhythm; bursts are separated by
+    near-silence so a VAD cuts them apart.  The voices differ in how their spectra change over time, which survives the per-utterance
+    mean subtraction of a speaker model's frontend (a static spectral difference would not)."""
+    g = torch.Generator().manual_seed(7919 * seed + 3)
+    total = lead_s + sum(sp + sl for _, sp, sl in pattern)
+    n = int(total * 16000)
+    x = torch.zeros(n, dtype=torch.float64)
+    pos = int(lead_s * 16000)
+    for v, sp, sl in pattern:
+        f0, fm, rate = VOICES[v]
+        m = int(sp * 16000)
+        t = torch.arange(m, dtype=torch.float64) / 16000.0
+        phase0 = 2 * math.pi * float(torch.rand(1, generator=g))
+        syl = torch.sin(math.pi * rate * t + phase0) ** 2                         # one syllable per half period
+        inst = f0 * (1.0 + 0.08 * torch.sin(2 * math.pi * 0.5 * rate * t + phase0))
+        phase = 2 * math.pi * torch.cumsum(inst, 0) / 16000.0
+        form = fm * (1.0 + 0.25 * (syl - 0.5))
+        y = torch.zeros(m, dtype=torch.float64)
+        for h in range(1, int(4000 // f0) + 1):
+            amp = torch.exp(-0.5 * ((h * inst - form) / (0.2 * fm)) ** 2) + 0.1 / h
+            y += amp * torch.sin(h * phase + float(torch.rand(1, generator=g)) * 6.283)
+        # breath noise in the formant band, strongest between syllables
+        nz = torch.fft.rfft(torch.randn(m, generator=g, dtype=torch.float64))
+        fr = torch.arange(nz.numel(), dtype=torch.float64) * (16000.0 / m)
+        nz = torch.fft.irfft(nz * torch.exp(-0.5 * ((fr - 1.5 * fm) / (0.4 * fm)) ** 2), n=m)
+        y = y / (y.abs().max() + 1e-9) + 0.15 * v * nz / (nz.std() + 1e-9) * (1.0 - syl)
+        ramp = torch.clamp(torch.minimum(t, sp - t) / 0.02, 0.0, 1.0)
+        y = y * (0.25 + 0.75 * syl) * ramp
+        x[pos:pos + m] = 0.25 * y / (y.abs().max() + 1e-9)
+        pos += m + int(sl * 16000)
+    x += torch.randn(n, generator=g, dtype=torch.float64) * 0.0015
+    return x.clamp_(-1, 1).float().contiguous()

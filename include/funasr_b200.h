@@ -428,6 +428,70 @@ int fa_embedding(const int32_t* ids, const float* table, int32_t dim, int32_t vo
  * 3 = s32le, 4 = u8.  The container (RIFF WAV header) is parsed on the host (funasr_b200/audio.py). */
 int fa_pcm_decode(const void* pcm, int32_t sample_format, int32_t channels, int64_t frames, float* out, fa_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * CAM++ speaker embedding (funasr/models/campplus/model.py CAMPPlus, feat 80, embedding 192, growth 32, bn 128, init 128,
+ * batchnorm-relu).  Eval-mode BatchNorm that follows a conv is folded into that conv's weights and bias by the caller; BatchNorm
+ * that precedes ReLU + conv is passed as a per-channel affine (scale = g / sqrt(var + eps), shift = b - mean * scale).
+ * ------------------------------------------------------------------------------------------- */
+/* FCM conv (Conv2d 3x3 or 1x1 over (freq, time), stride (stride_f, 1), padding ksize / 2) with its BN folded:
+ * w [ksize * ksize][c_in][32] (tap-major kf * ksize + kt, output channels contiguous), b [32]. */
+typedef struct {
+  const float* w;
+  const float* b;
+  int32_t c_in, c_out, ksize, stride_f;
+} FaCamConv2d;
+/* One CAMDenseTDNNLayer (components.py): nonlinear1 as an affine [c_in]; linear1 c_in -> 128 with nonlinear2's BN folded (ReLU
+ * applied); CAMLayer: local_w [3][128][32] (tap, input channel, output channel), linear1 w1 [64][128] + b1, linear2 w2 [32][64] + b2. */
+typedef struct {
+  const float* bn1_scale;
+  const float* bn1_shift;
+  FaLinear linear1;
+  const float* local_w;
+  const float* w1;
+  const float* b1;
+  const float* w2;
+  const float* b2;
+} FaCamLayer;
+typedef struct {
+  const float* scale;   /* nonlinear BN as an affine [in_f] */
+  const float* shift;
+  FaLinear linear;      /* in_f -> in_f / 2, no bias */
+} FaCamTransit;
+/* fcm: head.conv1, layer1.0.{conv1, conv2, shortcut}, layer1.1.{conv1, conv2}, layer2.0.{conv1, conv2, shortcut},
+ * layer2.1.{conv1, conv2}, head.conv2.  tdnn: Conv1d(320, 128, 5, stride 2, pad 2) as [128][5 * 320] (w[o][k * 320 + c]) with its BN
+ * folded.  layers: n_layers[0] + n_layers[1] + n_layers[2] CAM layers in order.  out_*: out_nonlinear BN as an affine [512].
+ * dense: 1024 -> 192 with the affine-free BN folded. */
+typedef struct {
+  FaCamConv2d fcm[12];
+  FaLinear tdnn;
+  const FaCamLayer* layers;
+  int32_t n_layers[3];
+  int32_t dilation[3];
+  FaCamTransit transit[3];
+  const float* out_scale;
+  const float* out_shift;
+  FaLinear dense;
+} FaCampplus;
+/* Features (campplus/utils.py extract_feature): torchaudio kaldi.fbank(wav, num_mel_bins=80) with its defaults (no x32768 scaling,
+ * window from `tables`: fa_fbank_make_tables with the povey window), then each utterance's mean over its own frames is subtracted.
+ * wav [B, wav_stride] (lens >= 400 samples) -> feats [B, t_max, 80] (rows >= feat_lens[b] zero, pad_list(..., 0)), feat_lens [B]. */
+int fa_campplus_features(const float* wav, const int32_t* wav_lens, int32_t batch, int64_t wav_stride, const float* tables,
+                         float* feats, int32_t* feat_lens, int32_t t_max, fa_stream_t stream);
+/* CAMPPlus.forward: feats [B, t, 80] (every frame used, no mask) -> emb [B, 192].  Stream-ordered, no host synchronisation. */
+size_t fa_campplus_workspace_bytes(const FaCampplus* model, int32_t batch, int32_t t, int32_t gemm_mode);
+int fa_campplus_forward(const FaCampplus* model, const float* feats, int32_t batch, int32_t t, float* emb, int32_t gemm_mode,
+                        void* workspace, size_t ws_bytes, fa_stream_t stream);
+/* Layer entry points of the forward (exposed for parity tests).  conv2d: x [B][f_in][t][c_in] channels last -> y [B][f_out][t][32],
+ * y = act(conv(x) + b (+ res)), res in y's layout or NULL. */
+int fa_campplus_conv2d(const FaCamConv2d* conv, const float* x, int32_t batch, int32_t f_in, int32_t t, const float* res, float* y,
+                       int32_t relu, fa_stream_t stream);
+/* CAMLayer: h [B * t, 128] -> out[(b t + i) * ld_out + o] (32 columns); gates [B][ceil(t / 100)][32] receives the context gates. */
+int fa_campplus_cam(const float* h, int32_t batch, int32_t t, int32_t dilation, const float* local_w, const float* w1, const float* b1,
+                    const float* w2, const float* b2, float* gates, float* out, int64_t ld_out, fa_stream_t stream);
+/* out_nonlinear + StatsPool: x [B * t, channels] -> stats [B, 2 * channels] = mean || unbiased std over t of relu(x * scale + shift). */
+int fa_campplus_stats_pool(const float* x, int32_t batch, int32_t t, int32_t channels, const float* scale, const float* shift,
+                           float* stats, fa_stream_t stream);
+
 /* Split fp32 [rows, cols] into three fp16 planes [3][rows][cols_pad] (hi, mid, lo; zero padded columns):
  * weight repack for the tensor-core GEMM path (called once per weight after load_pretrained_model). */
 int fa_split_planes(const float* src, int64_t ld_src, int64_t rows, int32_t cols, int32_t cols_pad,
