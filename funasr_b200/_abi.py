@@ -102,8 +102,6 @@ SIGNATURES = {
     "fa_version": (C.c_char_p, []),
     "fa_launch_count": (C.c_uint64, []),
     "fa_status_string": (C.c_char_p, [C.c_int]),
-    "fa_fbank_lfr_cmvn": (C.c_int, [_vp, _vp, _i32, _i64, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
-    "fa_fbank_lfr_cmvn_strided": (C.c_int, [_vp, _vp, _i32, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _vp]),
     "fa_fbank_tables_bytes": (_sz, []),
     "fa_fbank_make_tables": (C.c_int, [_vp, _vp, _vp, _vp]),
     "fa_fbank_lfr_cmvn_tables": (C.c_int, [_vp, _vp, _i32, _i64, _vp, _vp, _i32, _i32, _vp, _i64, _vp, _i32, _vp]),
@@ -126,7 +124,6 @@ SIGNATURES = {
     "fa_sanm_encoder_forward": (C.c_int, [C.POINTER(FaEncoder), _vp, _vp, _i32, _i32, _vp, _i32, _vp, _sz, _vp]),
     "fa_cif_predictor_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "fa_cif_predictor_forward": (C.c_int, [C.POINTER(FaPredictor), _vp, _vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _sz, _vp]),
-    "fa_paraformer_decoder_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32]),
     "fa_paraformer_decoder_workspace_bytes_hw": (_sz, [_i32, _i32, _i32, _i32, _i32, _i32]),
     "fa_paraformer_decoder_forward": (C.c_int, [C.POINTER(FaDecoder), _vp, _vp, _i32, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _sz, _vp]),
     "fa_row_sum_f32": (C.c_int, [_vp, _i64, _i32, _i32, _vp, _vp]),
@@ -137,10 +134,8 @@ SIGNATURES = {
     "fa_linear_argmax": (C.c_int, [C.POINTER(FaLinear), _vp, _vp, _i64, _vp, _vp, _vp, _i32, _vp, _sz, _vp]),
     "fa_seaco_merge": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
     "fa_cif_upsample_alphas": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _f, _f, _f, _vp, _vp, _vp]),
-    "fa_blstm_forward": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp]),
     "fa_blstm_tc_scratch_bytes": (_sz, [_i32]),
     "fa_blstm_forward_tc": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _sz, _vp]),
-    "fa_debug_blstm_variant": (C.c_int, [_i32, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "fa_fsmn_vad_workspace_bytes": (_sz, [C.POINTER(FaVadEncoder), _i32]),
     "fa_fsmn_vad_forward": (C.c_int, [C.POINTER(FaVadEncoder), _vp, _i64, _i32, _vp, _vp, _vp, _sz, _vp]),
     "fa_frame_decibels": (C.c_int, [_vp, _i64, _i32, _vp, _vp]),

@@ -67,8 +67,6 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();                                        // everything above touched only shared memory
-  pdl_trigger();
   const int klen = min(p.key_lens[b], p.tk);
   const int bkv = p.kv_shared ? 0 : b;
   const int nc = (klen + AT_BKEY - 1) / AT_BKEY;     // key chunks with at least one valid key
@@ -332,7 +330,7 @@ static int launch_att(dim3 grid, const CUtensorMap& mq, const CUtensorMap& mk, c
   static_assert(smem <= 227 * 1024, "shared memory per block");
   static PerDeviceOnce once;
   FA_RETURN_IF_ERR(ensure_dyn_smem(attention_tc_kernel<NPL, OPL>, smem, once));
-  FA_CUDA_OK(launch_pdl(attention_tc_kernel<NPL, OPL>, grid, dim3(384), smem, st, 1, mq, mk, mv, p));
+  attention_tc_kernel<NPL, OPL><<<grid, 384, smem, st>>>(mq, mk, mv, p);
   return FA_OK;
 }
 

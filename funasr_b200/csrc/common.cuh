@@ -42,35 +42,6 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
-// Programmatic dependent launch (PDL): every hot kernel is launched with programmaticStreamSerialization, runs its
-// global-memory-free prologue (barrier init, descriptor prefetch) while the previous kernel in the stream drains,
-// then pdl_wait() — which returns once the predecessor grid has completed and its writes are visible — before the first
-// global access, and immediately lets its own successor start its prologue (pdl_trigger).  FA_PDL=0 disables the attribute.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
-bool pdl_enabled();
-
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, int cluster_x, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  int n = 0;
-  if (pdl_enabled()) {
-    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
-  if (cluster_x > 1) {
-    attr[n].id = cudaLaunchAttributeClusterDimension;
-    attr[n].val.clusterDim.x = cluster_x; attr[n].val.clusterDim.y = 1; attr[n].val.clusterDim.z = 1;
-    ++n;
-  }
-  cfg.attrs = attr; cfg.numAttrs = n;
-  return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
-}
-
 // cudaFuncAttributeMaxDynamicSharedMemorySize and the SM count are PER-DEVICE: a process that drives two GPUs (two handles of
 // the offline API, a server with one worker thread per device) must set / query them once per (kernel instantiation, device).
 struct PerDeviceOnce { std::atomic<uint32_t> mask{0}; };

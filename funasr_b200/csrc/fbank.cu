@@ -5,11 +5,12 @@
 //   (kaldi.py:514-647) -> apply_lfr m=7 n=6 (:63-86) -> apply_cmvn (:46-60) -> pad_sequence(0.0) (:195).
 //
 // HBM-bound by design: algorithmic bytes = 4 B/sample in + 4*560 B/LFR-row out (3.04 MB per 30 s).
-// One CTA owns kRows consecutive LFR rows of one utterance: it stages the (6*kRows+1) frames' worth of
-// samples into shared memory once (coalesced), each warp turns frames into log-mel rows with a
-// register-resident 256-point complex FFT (radix 8 in registers x 32-point across the lanes on shuffles;
-// real 512-point FFT by even/odd packing), and the CTA then writes its LFR rows (7 stacked log-mel frames,
-// CMVN applied) with fully coalesced stores.
+// The per-configuration constants (window, FFT twiddles, mel filter taps) are computed once by fa_fbank_make_tables.
+// One CTA owns kRows consecutive LFR rows of one utterance: it copies the tables into shared memory, each warp reads
+// its frames' samples straight from global memory (coalesced 8-byte loads; the 2.5x overlap between frames hits L1)
+// and turns them into log-mel rows with a register-resident 256-point complex FFT (radix 8 in registers x 32-point
+// across the lanes on shuffles; real 512-point FFT by even/odd packing), and the CTA then writes its LFR rows
+// (7 stacked log-mel frames, CMVN applied) with fully coalesced stores.
 // Adjacent CTAs recompute one overlapping frame (1/48 redundancy) instead of round-tripping log-mel
 // through HBM.
 #include "common.cuh"
@@ -18,7 +19,6 @@ namespace fa {
 
 constexpr int kWin = 400, kShift = 160, kFft = 512, kBins = 257, kMel = 80;
 constexpr int kFramesMax = 49;                         // frames one CTA turns into log-mel rows: 6*(8-1)+7 (ASR, LFR 7/6) or 1*(44-1)+5 (VAD, LFR 5/1)
-constexpr int kSpan = (kFramesMax - 1) * kShift + kWin;   // 8080 samples
 constexpr int kWarps = 8;
 constexpr int kMelPackMax = 1024;
 // Precomputed tables (fa_fbank_make_tables): constants of the configuration that every CTA would otherwise rebuild — the
@@ -33,7 +33,7 @@ constexpr int kTabStart = 0, kTabLen = kMel, kTabOff = 2 * kMel, kTabW = 3 * kMe
 constexpr int kTapFlush = 1 << 16;                     // tap meta: bin | filter << 9 | kTapFlush on a filter's last tap
 constexpr int kZs = 36;                                // spectrum row pitch (float2): at most 2-way bank conflicts on the strided reads
 
-// Shared memory of the table-driven kernel (no waveform staging: 4 CTAs per SM instead of 2).
+// Shared memory of fbank_tab_kernel (no waveform staging: 4 CTAs per SM instead of 2).
 struct FbankSmemT {
   float logmel[kFramesMax * kMel];
   float2 zs[kWarps][8 * kZs];      // per warp: the 256-point spectrum as [k1 = 0..7][k2] rows of pitch kZs
@@ -45,23 +45,12 @@ struct FbankSmemT {
   float tap_w[kTapMax * 32];
 };
 
-struct FbankSmem {
-  float wav[kSpan + 8];
-  float logmel[kFramesMax * kMel];
-  float2 zs[kWarps][8 * kZs];      // per warp: the 256-point spectrum as [k1 = 0..7][k2] rows of pitch kZs
-  float pw[kWarps][264];           // per warp: power spectrum P[0..256]
-  float2 tw[256];
-  float win[kWin];
-  float melw[kMelPackMax];
-  int mel_start[kMel], mel_len[kMel], mel_off[kMel];
-};
-
 // Per-lane constants of the register FFT (hoisted out of the frame loop).
 struct LaneTw { float2 tw8[8]; float2 twl[5]; int rev; };
 
 // One frame -> its 256-point complex spectrum Z (of z[n] = y[2n] + i y[2n+1], y = the DC-removed, pre-emphasised, windowed and
-// zero-padded 512-sample frame) in Zs[k1 * kZs + k2] = Z[k1 + 8 k2].  Warp-collective.  x: the frame's first sample (shared or
-// global memory), vec2: x is 8-byte aligned.
+// zero-padded 512-sample frame) in Zs[k1 * kZs + k2] = Z[k1 + 8 k2].  Warp-collective.  x: the frame's first sample,
+// vec2: x is 8-byte aligned.
 __device__ __forceinline__ void frame_spectrum(const float* __restrict__ x, const float scl, const bool vec2, const float* __restrict__ s_win,
                                                const LaneTw& lt, const int lane, float2* __restrict__ Zs) {
   const float kR = 0.70710678118654752f;
@@ -139,162 +128,11 @@ __device__ __forceinline__ void frame_spectrum(const float* __restrict__ x, cons
   __syncwarp();
 }
 
-// kLfrM / kLfrN: low-frame-rate stacking (7/6 for Paraformer & SenseVoice, 5/1 for the FSMN-VAD); kRows: LFR rows per CTA.
-// tables != nullptr: constants come precomputed from global memory (a 9 KB copy); nullptr: every CTA derives them from
-// mel_banks / window itself (the round-1 behaviour: a 20 k-load scan of the filter matrix per CTA, kept for the plain ABI).
-template <int kLfrM, int kLfrN, int kRows>
-__global__ void __launch_bounds__(kWarps * 32)
-fbank_lfr_cmvn_kernel(const float* __restrict__ wav, const int32_t* __restrict__ wav_lens, int64_t wav_stride,
-                      const float* __restrict__ cmvn, const float* __restrict__ mel_banks,
-                      const float* __restrict__ window, const float* __restrict__ tables, float* __restrict__ feats,
-                      int32_t* __restrict__ feat_lens, int t_max, int64_t batch_stride_rows) {
-  constexpr int kFeat = kMel * kLfrM;
-  static_assert(kLfrN * (kRows - 1) + kLfrM <= kFramesMax, "too many frames per CTA");
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  FbankSmem& s = *reinterpret_cast<FbankSmem*>(smem_raw);
-  const int b = blockIdx.y, i0 = blockIdx.x * kRows;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int n = wav_lens[b];
-  const int m = n >= kWin ? 1 + (n - kWin) / kShift : 0;      // kaldi.py:_get_strided, snip_edges
-  const int t_b = (m + kLfrN - 1) / kLfrN;                    // wav_frontend.py:73
-  if (blockIdx.x == 0 && tid == 0) feat_lens[b] = t_b;
-
-  float* out = feats + ((int64_t)b * batch_stride_rows + i0) * kFeat;
-  if (i0 >= t_b) {  // pure padding rows
-    const int rows = min(kRows, t_max - i0);
-    for (int idx = tid; idx < rows * kFeat; idx += blockDim.x) out[idx] = 0.f;
-    return;
-  }
-  const int f_lo = max(0, kLfrN * i0 - (kLfrM - 1) / 2);
-  const int f_hi = min(m - 1, kLfrN * (i0 + kRows - 1) + (kLfrM - 1) / 2);
-  const int nfr = f_hi - f_lo + 1;
-
-  // ---- stage samples, window, twiddles and the sparse mel filters ----
-  {
-    const float* src = wav + (int64_t)b * wav_stride + (int64_t)f_lo * kShift;
-    const int span = (nfr - 1) * kShift + kWin;
-    for (int j = tid; j < span; j += blockDim.x) s.wav[j] = __ldg(src + j) * 32768.0f;   // exact scaling
-  }
-  if (tables != nullptr) {
-    const int* ti = reinterpret_cast<const int*>(tables);
-    for (int j = tid; j < kMel; j += blockDim.x) {
-      s.mel_start[j] = __ldg(ti + kTabStart + j); s.mel_len[j] = __ldg(ti + kTabLen + j); s.mel_off[j] = __ldg(ti + kTabOff + j);
-    }
-    for (int j = tid; j < kMelPackMax; j += blockDim.x) s.melw[j] = __ldg(tables + kTabW + j);
-    for (int j = tid; j < 256; j += blockDim.x) s.tw[j] = make_float2(__ldg(tables + kTabTw + 2 * j), __ldg(tables + kTabTw + 2 * j + 1));
-    for (int j = tid; j < kWin; j += blockDim.x) s.win[j] = __ldg(tables + kTabWin + j);
-    __syncthreads();
-  } else {
-    for (int j = tid; j < kWin; j += blockDim.x) s.win[j] = window[j];
-    for (int k = tid; k < 256; k += blockDim.x) {
-      float sn, cs;
-      sincospif((float)k * (1.0f / 256.0f), &sn, &cs);        // e^{-2 pi i k / 512}
-      s.tw[k] = make_float2(cs, -sn);
-    }
-    // non-zero support of each triangular filter (kaldi.py:get_mel_banks): warp-parallel coalesced scan
-    for (int j = warp; j < kMel; j += kWarps) {
-      const float* row = mel_banks + j * kBins;
-      int st = kBins, en = -1;
-      for (int k = lane; k < kBins; k += 32) {
-        if (__ldg(row + k) != 0.f) { st = min(st, k); en = max(en, k); }
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        st = min(st, __shfl_xor_sync(0xffffffffu, st, o));
-        en = max(en, __shfl_xor_sync(0xffffffffu, en, o));
-      }
-      if (lane == 0) { s.mel_start[j] = en < 0 ? 0 : st; s.mel_len[j] = en < 0 ? 0 : en - st + 1; }
-    }
-    __syncthreads();
-    if (tid == 0) {
-      int off = 0;
-      for (int j = 0; j < kMel; ++j) { s.mel_off[j] = off; off += s.mel_len[j]; if (off > kMelPackMax) { s.mel_len[j] = 0; off = s.mel_off[j]; } }
-    }
-    __syncthreads();
-    if (tid < kMel) {
-      const float* row = mel_banks + tid * kBins + s.mel_start[tid];
-      float* dst = s.melw + s.mel_off[tid];
-      for (int k = 0; k < s.mel_len[tid]; ++k) dst[k] = row[k];
-    }
-    __syncthreads();
-  }
-
-  // ---- one warp per frame: 512-point real FFT as a 256-point complex FFT held in REGISTERS ----
-  // z[n] = y[2n] + i y[2n+1]; lane L owns z[L + 32 r], r = 0..7.  256 = 8 x 32 (Cooley-Tukey):
-  //   (1) 8-point DFT over r in registers, (2) twiddle W_256^{L k1}, (3) 32-point DFT across the lanes for each k1 as five
-  //   decimation-in-frequency butterfly stages on warp shuffles (no shared-memory round trips; the round-1 kernel made eight
-  //   radix-2 Stockham passes through shared memory per frame and was bound by their latency: 1.12 ms for 64 x 30 s),
-  //   after which lane L holds Z[k1 + 8 rev5(L)].  The spectrum goes to shared memory ONCE for the real-FFT untangling
-  //   (needs Z[k] and Z[256 - k]), the power spectrum and the sparse mel filters.
-  // All twiddles depend only on the lane: hoisted out of the frame loop.
-  float2* Zs = s.zs[warp];                                        // [8][kZs] spectrum, row k1, column k2
-  float* P = s.pw[warp];                                          // [257] power spectrum
-  auto twid = [&](int idx) -> float2 {                            // e^{-2 pi i idx / 512}, idx in [0, 512)
-    const float2 w = s.tw[idx & 255];
-    return idx < 256 ? w : make_float2(-w.x, -w.y);
-  };
-  LaneTw lt;
-#pragma unroll
-  for (int k1 = 1; k1 < 8; ++k1) lt.tw8[k1] = twid(2 * lane * k1);   // W_256^{lane k1}
-  lt.tw8[0] = make_float2(1.f, 0.f);
-#pragma unroll
-  for (int st = 0; st < 5; ++st) {                                   // W_{2m}^{lane mod m} in the upper lane of a butterfly, 1 in the lower
-    const int mm = 16 >> st;
-    lt.twl[st] = (lane & mm) ? twid((lane & (mm - 1)) * (256 / mm)) : make_float2(1.f, 0.f);
-  }
-  lt.rev = (int)(__brev((unsigned)lane) >> 27);
-  for (int f = warp; f < nfr; f += kWarps) {
-    frame_spectrum(s.wav + f * kShift, 1.0f, true, s.win, lt, lane, Zs);
-    // power spectrum of the real signal -> P[0..256]
-    auto Z = [&](int k) -> float2 { return Zs[(k & 7) * kZs + (k >> 3)]; };
-    for (int k = lane; k < kBins; k += 32) {
-      float re, im;
-      if (k == 0) { const float2 z0 = Z(0); re = z0.x + z0.y; im = 0.f; }
-      else if (k == 256) { const float2 z0 = Z(0); re = z0.x - z0.y; im = 0.f; }
-      else {
-        const float2 zk = Z(k), zc = Z(256 - k);
-        const float er = 0.5f * (zk.x + zc.x), ei = 0.5f * (zk.y - zc.y);
-        const float orr = 0.5f * (zk.y + zc.y), oi = -0.5f * (zk.x - zc.x);
-        const float2 w = s.tw[k];
-        re = er + (w.x * orr - w.y * oi);
-        im = ei + (w.x * oi + w.y * orr);
-      }
-      const float mag = sqrtf(re * re + im * im);                   // rfft(..).abs().pow(2.0) :616-618
-      P[k] = mag * mag;
-    }
-    __syncwarp();
-    for (int j = lane; j < kMel; j += 32) {
-      const float* wts = s.melw + s.mel_off[j];
-      const float* pp = P + s.mel_start[j];
-      float acc = 0.f;
-      for (int k = 0; k < s.mel_len[j]; ++k) acc = fmaf(pp[k], wts[k], acc);
-      s.logmel[f * kMel + j] = logf(fmaxf(acc, 1.1920929e-07f));    // :632-633
-    }
-    __syncwarp();
-  }
-  __syncthreads();
-
-  // ---- LFR stacking + CMVN, coalesced row stores ----
-  const int rows = min(kRows, t_max - i0);
-  for (int idx = tid; idx < rows * kFeat; idx += blockDim.x) {
-    const int r = idx / kFeat, col = idx - r * kFeat;
-    const int i = i0 + r;
-    float v = 0.f;
-    if (i < t_b) {
-      const int j = col / kMel, c = col - j * kMel;
-      int fsrc = kLfrN * i - (kLfrM - 1) / 2 + j;
-      fsrc = min(max(fsrc, 0), m - 1);
-      v = s.logmel[(fsrc - f_lo) * kMel + c];
-      if (cmvn != nullptr) v = __fmul_rn(__fadd_rn(v, __ldg(cmvn + col)), __ldg(cmvn + kFeat + col));
-    }
-    out[idx] = v;
-  }
-}
-
-// Table-driven variant (fa_fbank_lfr_cmvn_tables; what the engines launch).  Differences to the kernel above:
+// fa_fbank_lfr_cmvn_tables: kLfrM / kLfrN is the low-frame-rate stacking (7/6 for Paraformer & SenseVoice, 5/1 for the FSMN-VAD,
+// 1/1 for CAM++), kRows the LFR rows per CTA.
 //   * no waveform staging: every warp reads its frame's 400 samples straight from global memory (coalesced 8-byte loads; the 2.5x
-//     overlap between frames hits L1).  The staging loop was 28 % of the stall samples of the previous version (32 dependent
-//     global-load rounds per CTA in front of a barrier) and its 32 KB of shared memory held the kernel at 2 CTAs per SM;
+//     overlap between frames hits L1).  Staging the CTA's samples in shared memory first put 32 dependent global-load rounds in
+//     front of a barrier and its 32 KB of shared memory held the kernel at 2 CTAs per SM;
 //   * power spectrum in pairs: X[k] and X[256 - k] of the real 512-point transform share E_k and O_k, so a lane computes both
 //     from one pair of spectrum loads (4 iterations instead of 9);
 //   * mel filters through the balanced tap schedule of the tables (see kTapMax).
@@ -406,7 +244,8 @@ fbank_tab_kernel(const float* __restrict__ wav, const int32_t* __restrict__ wav_
   }
 }
 
-// fa_fbank_make_tables: the per-configuration constants, computed once (same arithmetic as the in-kernel path)
+// fa_fbank_make_tables: the per-configuration constants, computed once: the non-zero support of each mel filter, its packed
+// weights, the FFT twiddles, the window and the tap schedule that fbank_tab_kernel walks
 __global__ void fbank_tables_kernel(const float* __restrict__ mel_banks, const float* __restrict__ window, float* __restrict__ tables) {
   __shared__ int s_start[kMel], s_len[kMel], s_off[kMel];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -493,20 +332,6 @@ static int fbank_tab_launch(const float* wav, const int32_t* wav_lens, int batch
   dim3 grid((t_max + ROWS - 1) / ROWS, batch);
   fbank_tab_kernel<M, N, ROWS><<<grid, kWarps * 32, smem, st>>>(wav, wav_lens, wav_stride, cmvn, tables, feats, feat_lens, t_max, stride_rows,
                                                                 wav_scale);
-  FA_CHECK_LAUNCH();
-  return FA_OK;
-}
-
-template <int M, int N, int ROWS>
-static int fbank_launch(const float* wav, const int32_t* wav_lens, int batch, int64_t wav_stride, const float* cmvn, const float* mel_banks,
-                        const float* window, const float* tables, float* feats, int64_t stride_rows, int32_t* feat_lens, int t_max,
-                        cudaStream_t st) {
-  const size_t smem = sizeof(FbankSmem);
-  static PerDeviceOnce once;
-  FA_RETURN_IF_ERR(ensure_dyn_smem(fbank_lfr_cmvn_kernel<M, N, ROWS>, smem, once));
-  dim3 grid((t_max + ROWS - 1) / ROWS, batch);
-  fbank_lfr_cmvn_kernel<M, N, ROWS><<<grid, kWarps * 32, smem, st>>>(wav, wav_lens, wav_stride, cmvn, mel_banks, window, tables, feats,
-                                                                    feat_lens, t_max, stride_rows);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }
@@ -606,21 +431,4 @@ extern "C" int fa_fbank_lfr_cmvn_tables(const float* wav, const int32_t* wav_len
   if (lfr_m == 5 && lfr_n == 1)
     return fa::fbank_tab_launch<5, 1, 44>(wav, wav_lens, batch, wav_stride, cmvn, tables, feats, feats_batch_stride_rows, feat_lens, t_max, st);
   return FA_ERR_UNSUPPORTED;
-}
-
-extern "C" int fa_fbank_lfr_cmvn_strided(const float* wav, const int32_t* wav_lens, int32_t batch, int64_t wav_stride,
-                                         const float* cmvn, const float* mel_banks, const float* window, float* feats,
-                                         int64_t feats_batch_stride_rows, int32_t* feat_lens, int32_t t_max,
-                                         fa_stream_t stream) {
-  if (!wav || !wav_lens || !mel_banks || !window || !feats || !feat_lens || batch <= 0 || t_max <= 0 ||
-      feats_batch_stride_rows < t_max)
-    return FA_ERR_ARG;
-  return fa::fbank_launch<7, 6, 8>(wav, wav_lens, batch, wav_stride, cmvn, mel_banks, window, nullptr, feats, feats_batch_stride_rows, feat_lens,
-                                   t_max, (cudaStream_t)stream);
-}
-
-extern "C" int fa_fbank_lfr_cmvn(const float* wav, const int32_t* wav_lens, int32_t batch, int64_t wav_stride,
-                                 const float* cmvn, const float* mel_banks, const float* window, float* feats,
-                                 int32_t* feat_lens, int32_t t_max, fa_stream_t stream) {
-  return fa_fbank_lfr_cmvn_strided(wav, wav_lens, batch, wav_stride, cmvn, mel_banks, window, feats, t_max, feat_lens, t_max, stream);
 }

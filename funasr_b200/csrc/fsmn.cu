@@ -13,11 +13,10 @@
 //                       3-stage shared-memory ring with cp.async.bulk.tensor (3-D tensor map {channel, time, utterance}: the zero
 //                       padding of the convolution at the utterance edges IS the map's out-of-bounds fill), 8 consumer warps slide
 //                       their windows over shared memory (each v element crosses L2->SM once) and store the result rows coalesced.
-//                       Default wherever its shape rules hold (k = 11 / 21, channels % 128 == 0, t_max >= 64, 16-byte aligned rows);
-//                       FA_FSMN_TMA=0 keeps the SIMT kernel everywhere.  A/B at the encoder shape (DESIGN.md §6): 48.1 -> 39.9 us.
+//                       Used wherever its shape rules hold (k = 11 / 21, channels % 128 == 0, t_max >= 64, 16-byte aligned rows);
+//                       the SIMT kernel covers every other shape.  A/B at the encoder shape (DESIGN.md §6): 48.1 -> 39.9 us.
 #include "common.cuh"
 #include "tc_common.cuh"
-#include <cstdlib>
 #include <unordered_map>
 
 namespace fa {
@@ -35,8 +34,6 @@ fsmn_kernel(const float* __restrict__ v, int64_t ldv, const int32_t* __restrict_
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   const int t0 = blockIdx.y * FSMN_TT;
   const int b = blockIdx.z;
-  pdl_wait();
-  pdl_trigger();
   if (c >= channels) return;
   const int len = min(lens[b], t_max);
   float wk[K];
@@ -95,8 +92,6 @@ fsmn_tma_kernel(const __grid_constant__ CUtensorMap vmap, const __grid_constant_
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();                       // everything above is global-memory free
-  pdl_trigger();
 
   if (warp == 0) {
     // ===================== producer: one lane issues the bulk tensor copies =====================
@@ -226,8 +221,7 @@ static int fsmn_tma_launch_k(const float* v, int64_t ldv, const int32_t* lens, i
   const int n_tiles = (int)n_tiles64;
   const int n_sm = sm_count();
   const int grid = n_tiles < n_sm ? n_tiles : n_sm;
-  FA_CUDA_OK(launch_pdl(fsmn_tma_kernel<K>, dim3(grid), dim3(FT_THREADS), smem, st, 1, vm, rm, res ? 1 : 0, lens, t_max, t_tiles, ch_tiles, n_tiles,
-                        w, out, ldo));
+  fsmn_tma_kernel<K><<<grid, FT_THREADS, smem, st>>>(vm, rm, res ? 1 : 0, lens, t_max, t_tiles, ch_tiles, n_tiles, w, out, ldo);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }
@@ -241,20 +235,15 @@ int fsmn_tma_launch(const float* v, int64_t ldv, const int32_t* lens, int batch,
   return fsmn_tma_launch_k<21>(v, ldv, lens, batch, t_max, channels, w, res, ldr, out, ldo, st);
 }
 
-// the TMA-staged kernel is the default (tools/fsmn_probe.py compares the two); FA_FSMN_TMA=0 = SIMT strips only
+// the TMA-staged kernel wherever its shape rules hold, SIMT strips otherwise (tools/fsmn_probe.py compares the two)
 int fsmn_simt_launch(const float* v, int64_t ldv, const int32_t* lens, int batch, int t_max, int channels, const float* w,
                      int ksize, const float* res, int64_t ldr, float* out, int64_t ldo, cudaStream_t st, int causal);
-
-static bool fsmn_tma_default() {
-  static const bool on = [] { const char* e = getenv("FA_FSMN_TMA"); return !(e && e[0] == '0'); }();
-  return on;
-}
 
 int fsmn_launch(const float* v, int64_t ldv, const int32_t* lens, int batch, int t_max, int channels, const float* w,
                 int ksize, const float* res, int64_t ldr, float* out, int64_t ldo, cudaStream_t st, int causal) {
   if (batch <= 0 || t_max <= 0) return FA_OK;
   if (!v || !lens || !w || !out) return FA_ERR_ARG;
-  if (!causal && fsmn_tma_default() && t_max >= FT_TT && fsmn_tma_supported(v, ldv, channels, ksize, res, ldr))
+  if (!causal && t_max >= FT_TT && fsmn_tma_supported(v, ldv, channels, ksize, res, ldr))
     return fsmn_tma_launch(v, ldv, lens, batch, t_max, channels, w, ksize, res, ldr, out, ldo, st);
   return fsmn_simt_launch(v, ldv, lens, batch, t_max, channels, w, ksize, res, ldr, out, ldo, st, causal);
 }
@@ -266,14 +255,14 @@ int fsmn_simt_launch(const float* v, int64_t ldv, const int32_t* lens, int batch
   dim3 grid((channels + 127) / 128, (t_max + FSMN_TT - 1) / FSMN_TT, batch);
   if (causal) {
     if (ksize != 20) return FA_ERR_UNSUPPORTED;
-    FA_CUDA_OK(launch_pdl(fsmn_kernel<20, 19>, grid, dim3(128), 0, st, 1, v, ldv, lens, t_max, channels, w, res, ldr, out, ldo));
+    fsmn_kernel<20, 19><<<grid, 128, 0, st>>>(v, ldv, lens, t_max, channels, w, res, ldr, out, ldo);
     FA_CHECK_LAUNCH();
     return FA_OK;
   }
   switch (ksize) {
-    case 11: FA_CUDA_OK(launch_pdl(fsmn_kernel<11, 5>, grid, dim3(128), 0, st, 1, v, ldv, lens, t_max, channels, w, res, ldr, out, ldo)); break;
-    case 21: FA_CUDA_OK(launch_pdl(fsmn_kernel<21, 10>, grid, dim3(128), 0, st, 1, v, ldv, lens, t_max, channels, w, res, ldr, out, ldo)); break;
-    case 31: FA_CUDA_OK(launch_pdl(fsmn_kernel<31, 15>, grid, dim3(128), 0, st, 1, v, ldv, lens, t_max, channels, w, res, ldr, out, ldo)); break;
+    case 11: fsmn_kernel<11, 5><<<grid, 128, 0, st>>>(v, ldv, lens, t_max, channels, w, res, ldr, out, ldo); break;
+    case 21: fsmn_kernel<21, 10><<<grid, 128, 0, st>>>(v, ldv, lens, t_max, channels, w, res, ldr, out, ldo); break;
+    case 31: fsmn_kernel<31, 15><<<grid, 128, 0, st>>>(v, ldv, lens, t_max, channels, w, res, ldr, out, ldo); break;
     default: return FA_ERR_UNSUPPORTED;
   }
   FA_CHECK_LAUNCH();

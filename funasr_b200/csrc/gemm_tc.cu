@@ -504,8 +504,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();                                          // prologue above is global-memory free; operands are read below
-  pdl_trigger();
 
   if (warp < 4) {
     // ===================== TMA producer =====================
@@ -674,7 +672,7 @@ static int launch_cfg_e(const CUtensorMap& ma, const CUtensorMap& mw, const TcPa
   const int n_sm = sm_count();
   const int tiles = p.tiles_m * p.tiles_n;
   const int grid = tiles < n_sm ? tiles : n_sm;
-  FA_CUDA_OK(launch_pdl(gemm_tc_kernel<BN, STAGES, APL, WPL, EPI>, dim3(grid), dim3(384), smem, st, 1, ma, mw, p));
+  gemm_tc_kernel<BN, STAGES, APL, WPL, EPI><<<grid, 384, smem, st>>>(ma, mw, p);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }

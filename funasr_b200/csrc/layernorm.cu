@@ -18,8 +18,6 @@ layernorm_kernel(const float* x, int64_t rows, int n, const float* __restrict__ 
                  plane_t* __restrict__ planes, int nplanes, int cols_pad, float* __restrict__ emb_out) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  pdl_wait();
-  pdl_trigger();
   if (row >= rows) return;
   const int nvec = n >> 2;
   const float4* xr = reinterpret_cast<const float4*>(x + row * n);
@@ -114,8 +112,8 @@ int layernorm_launch(const float* x, int64_t rows, const FaNorm& nm, float* y, c
   const int npl = planes ? nplanes : 0;
   if (npl < 0 || npl > 3 || (planes && npl == 0)) return FA_ERR_ARG;
 #define FA_LN_LAUNCH(NV, NPL)                                                                                \
-  FA_CUDA_OK(launch_pdl(layernorm_kernel<NV, NPL>, dim3(blocks), dim3(256), 0, st, 1, x, rows, n, nm.g, nm.b, nm.eps, y, pe_inv,   \
-                        xscale, rows_per_batch > 0 ? rows_per_batch : 1, planes, nplanes, cols_pad, emb_out))
+  layernorm_kernel<NV, NPL><<<blocks, 256, 0, st>>>(x, rows, n, nm.g, nm.b, nm.eps, y, pe_inv, xscale,                   \
+                                                   rows_per_batch > 0 ? rows_per_batch : 1, planes, nplanes, cols_pad, emb_out)
 #define FA_LN_CASE(NV)                                                                                       \
   do {                                                                                                       \
     if (npl == 0) FA_LN_LAUNCH(NV, 0); else if (npl == 1) FA_LN_LAUNCH(NV, 1);                               \

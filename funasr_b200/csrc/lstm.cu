@@ -3,13 +3,11 @@
 // encoder output).  cuDNN needs 34 ms for [64, 1500, 512] in fp32; the recurrence is 1500 strictly sequential steps of a
 // [B,512] x [512,2048] product per direction, so the design goal is the shortest possible step:
 //   * the input projections x W_ih^T + b_ih + b_hh of ALL steps are one tensor-core GEMM of this library (fa_linear), outside;
-//   * weight-stationary recurrence: 2 directions x 64 CTAs, CTA c keeps the 4 gate rows of hidden units [8c, 8c+8) of W_hh
-//     (32 x 512 fp32 = 64 KB) in shared memory for the whole sequence, plus one [64, 512] fp32 copy of h_{t-1} (128 KB);
-//   * per step: gather h_{t-1} (written by the 64 CTAs of this direction into the OUTPUT tensor itself) -> 64 x 32 dot products
-//     of length 512 in fp32 (thread = four sequences x the four gates of one hidden unit, cell states in registers) -> gates,
-//     c, h -> write the h slice -> per-direction grid barrier (monotone atomic counter).
-// Exact fp32 arithmetic (no tensor cores): the timestamps are thresholded downstream.  Launched cooperatively so all 128 CTAs
-// are co-resident (the barrier would deadlock otherwise).
+//   * weight-stationary recurrence: 2 directions x 64 CTAs, CTA c keeps the 4 gate rows of hidden units [8c, 8c+8) of W_hh in
+//     shared memory for the whole sequence;
+//   * per step: gather h_{t-1} (published by the 64 CTAs of this direction) -> the recurrent product on tensor cores (below)
+//     -> gates, c, h -> write the h slice -> per-direction grid barrier (monotone atomic counter).
+// Launched cooperatively so all 128 CTAs are co-resident (the barrier would deadlock otherwise).
 #include "common.cuh"
 #include <cuda_bf16.h>
 
@@ -19,201 +17,17 @@ constexpr int LS_H = 512;          // hidden size
 constexpr int LS_UNITS = 8;        // hidden units per CTA
 constexpr int LS_NC = LS_H / LS_UNITS;   // 64 CTAs per direction
 constexpr int LS_ROWS = 4 * LS_UNITS;    // 32 gate rows per CTA
-constexpr int LS_BT = 64;          // sequences per batch tile (128 threads = 16 sequence groups x 8 hidden units)
-constexpr int LS_WLD = LS_H + 4;   // padded weight row pitch (floats): rows of different unit pairs hit different banks
-constexpr int LS_HLD = LS_H + 4;   // padded h row pitch: the 8 sequences of a warp read their float4 from 8 x 4 distinct banks
+constexpr int LS_BT = 64;          // sequences per batch tile (4 warps x 16 sequences)
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 
-// SKIP is a measurement aid (tools/bicif_probe.py): bit 0 drops the recurrent dot products, bit 1 the h gather, bit 2 the
-// inter-CTA step barrier; SKIP == 0 is the product kernel.
-template <int SKIP>
-__global__ void __launch_bounds__(128, 1)
-blstm_kernel(const float* __restrict__ xproj, const float* __restrict__ w_hh_f, const float* __restrict__ w_hh_b, int batch, int T,
-             float* __restrict__ out, unsigned int* __restrict__ counters) {
-  extern __shared__ __align__(16) float smf[];
-  float* sW = smf;                                  // [32][LS_WLD]   local row g*8 + u
-  float* sH = smf + LS_ROWS * LS_WLD;               // [LS_BT][LS_HLD]
-  const int dir = blockIdx.x / LS_NC, c = blockIdx.x % LS_NC;
-  const int tid = threadIdx.x;
-  const float* whh = dir == 0 ? w_hh_f : w_hh_b;
-  // local row r = g*8 + u  <->  W_hh row g*512 + (8c + u)   (PyTorch gate order i, f, g, o)
-  for (int idx = tid; idx < LS_ROWS * (LS_H / 4); idx += blockDim.x) {
-    const int r = idx / (LS_H / 4), k4 = idx % (LS_H / 4);
-    const int g = r / LS_UNITS, u = r % LS_UNITS;
-    const float4 w = __ldg(reinterpret_cast<const float4*>(whh + ((int64_t)g * LS_H + c * LS_UNITS + u) * LS_H) + k4);
-    *reinterpret_cast<float4*>(sW + r * LS_WLD + 4 * k4) = w;
-  }
-  // Register tile: thread (sg, u) owns hidden unit u (its four gates) for the four sequences sg, sg+16, sg+32, sg+48 of a
-  // batch tile: per 4 values of k it reads 4 float4 of h and 4 float4 of W for 64 FMAs (a thread per single output needed
-  // 9 loads per 32 FMAs and was bound by shared-memory bandwidth: LDS.128 always costs four wavefronts).
-  const int sg = tid >> 3, u = tid & 7;
-  const int n_tiles = (batch + LS_BT - 1) / LS_BT;   // <= 4 (checked by the launcher)
-  float cst[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) cst[i][j] = 0.f;
-  __syncthreads();
-  unsigned int* counter = counters + dir;
-  const int64_t out_ld = 2 * LS_H;                   // out [B, T, 2H]
-  const int64_t xp_ld = 2 * 4 * LS_H;                // xproj [B*T, 2 dirs x 4H]
-  const float* wrow = sW + u * LS_WLD;               // gate g at + g * 8 * LS_WLD
-  for (int step = 0; step < T; ++step) {
-    const int t = dir == 0 ? step : T - 1 - step;
-    const int tp = dir == 0 ? t - 1 : t + 1;         // time index of h_{t-1} in processing order
-    // x projections (+ both biases) of tile 0 are independent of h: fetched before the barrier wait, their DRAM latency hides
-    // behind it (the common case batch <= 64 has only this tile)
-    float x0[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int b = sg + 16 * i;
-      const float* xp = xproj + ((int64_t)min(b, batch - 1) * T + t) * xp_ld + dir * 4 * LS_H + c * LS_UNITS + u;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) x0[i][g] = __ldg(xp + g * LS_H);
-    }
-    if (step > 0 && !(SKIP & 4)) {
-      // every CTA of this direction has published its slice of h for the previous step
-      if (tid == 0) {
-        const unsigned int want = (unsigned int)step * LS_NC;
-        while (*reinterpret_cast<volatile unsigned int*>(counter) < want) { }
-        __threadfence();
-      }
-      __syncthreads();
-    }
-#pragma unroll
-    for (int bt = 0; bt < 4; ++bt) {                 // compile-time trip count keeps the cell states in registers
-      if (bt >= n_tiles) break;
-      const int b0 = bt * LS_BT;
-      const int nb = min(LS_BT, batch - b0);
-      // x projections (+ both biases) of this thread's unit for its four sequences: independent of h
-      float acc[4][4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        if (bt == 0) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) acc[i][g] = x0[i][g];
-        } else {
-          const int b = b0 + sg + 16 * i;
-          const float* xp = xproj + ((int64_t)min(b, batch - 1) * T + t) * xp_ld + dir * 4 * LS_H + c * LS_UNITS + u;
-#pragma unroll
-          for (int g = 0; g < 4; ++g) acc[i][g] = __ldg(xp + g * LS_H);
-        }
-      }
-      if (step > 0 && !(SKIP & 2)) {
-        // gather h_{t-1} [nb, 512] of this direction, L2 -> shared memory with 16-byte async copies (cp.async.cg bypasses L1:
-        // the lines were written by other SMs during this launch); all copies of a thread are in flight at once
-        const float* src0 = out + ((int64_t)b0 * T + tp) * out_ld + dir * LS_H;
-        for (int idx = tid; idx < nb * (LS_H / 4); idx += blockDim.x) {
-          const int b = idx / (LS_H / 4), k4 = idx % (LS_H / 4);
-          const uint32_t dst = (uint32_t)__cvta_generic_to_shared(sH + b * LS_HLD + 4 * k4);
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src0 + (int64_t)b * T * out_ld + 4 * k4) : "memory");
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-      }
-      __syncthreads();
-      if (step > 0 && !(SKIP & 1)) {
-        float dot[4][4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int g = 0; g < 4; ++g) dot[i][g] = 0.f;
-        const float* hrow = sH + sg * LS_HLD;        // sequence i at + 16 * i * LS_HLD
-#pragma unroll 2
-        for (int k = 0; k < LS_H; k += 4) {
-          float4 h4[4], w4[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) h4[i] = *reinterpret_cast<const float4*>(hrow + 16 * i * LS_HLD + k);
-#pragma unroll
-          for (int g = 0; g < 4; ++g) w4[g] = *reinterpret_cast<const float4*>(wrow + g * LS_UNITS * LS_WLD + k);
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              float d = dot[i][g];
-              d = fmaf(h4[i].x, w4[g].x, d); d = fmaf(h4[i].y, w4[g].y, d); d = fmaf(h4[i].z, w4[g].z, d); d = fmaf(h4[i].w, w4[g].w, d);
-              dot[i][g] = d;
-            }
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int g = 0; g < 4; ++g) acc[i][g] += dot[i][g];
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int b = b0 + sg + 16 * i;
-        const float ig = sigmoidf_(acc[i][0]), fg = sigmoidf_(acc[i][1]), gg = tanhf(acc[i][2]), og = sigmoidf_(acc[i][3]);
-        const float cn = fg * cst[bt][i] + ig * gg;
-        cst[bt][i] = cn;
-        if (b < batch) out[((int64_t)b * T + t) * out_ld + dir * LS_H + c * LS_UNITS + u] = og * tanhf(cn);
-      }
-      __syncthreads();                               // sH is reused by the next batch tile
-    }
-    if (!(SKIP & 4)) {
-      // publish: all threads' stores -> device scope, then one arrival per CTA
-      __threadfence();
-      __syncthreads();
-      if (tid == 0) atomicAdd(counter, 1u);
-    }
-  }
-}
-
-template <int SKIP>
-static int blstm_launch_t(const float* xproj, const float* w_hh_f, const float* w_hh_b, int batch, int T, int hidden, float* out,
-                          unsigned int* counters, cudaStream_t st) {
-  if (batch <= 0 || T <= 0) return FA_OK;
-  if (!xproj || !w_hh_f || !w_hh_b || !out || !counters) return FA_ERR_ARG;
-  if (hidden != LS_H || batch > 4 * LS_BT) return FA_ERR_UNSUPPORTED;
-  const size_t smem = (size_t)(LS_ROWS * LS_WLD + LS_BT * LS_HLD) * sizeof(float);
-  static PerDeviceOnce once;
-  FA_RETURN_IF_ERR(ensure_dyn_smem(blstm_kernel<SKIP>, smem, once));
-  FA_CUDA_OK(cudaMemsetAsync(counters, 0, 2 * sizeof(unsigned int), st));
-  void* args[] = {(void*)&xproj, (void*)&w_hh_f, (void*)&w_hh_b, (void*)&batch, (void*)&T, (void*)&out, (void*)&counters};
-  FA_CUDA_OK(cudaLaunchCooperativeKernel((const void*)blstm_kernel<SKIP>, dim3(2 * LS_NC), dim3(128), args, smem, st));
-  count_launch();
-  return FA_OK;
-}
-
-int blstm_launch(const float* xproj, const float* w_hh_f, const float* w_hh_b, int batch, int T, int hidden, float* out,
-                 unsigned int* counters, cudaStream_t st) {
-  return blstm_launch_t<0>(xproj, w_hh_f, w_hh_b, batch, T, hidden, out, counters, st);
-}
-
-}  // namespace fa
-
-// One-layer bidirectional LSTM over [B, T, 512] given the input projections of both directions:
-//   xproj [B*T, 2*2048] = x W_ih^T + b_ih + b_hh, columns [0,2048) forward gates (i,f,g,o), [2048,4096) reverse.
-extern "C" int fa_blstm_forward(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, int32_t batch, int32_t t_len,
-                                int32_t hidden, float* out, void* sync_scratch8, fa_stream_t stream) {
-  return fa::blstm_launch(xproj, w_hh_fwd, w_hh_bwd, batch, t_len, hidden, out, static_cast<unsigned int*>(sync_scratch8), (cudaStream_t)stream);
-}
-
-// measurement aid: same call with parts of the step removed (results are then meaningless)
-extern "C" int fa_debug_blstm_variant(int32_t skip_mask, const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, int32_t batch,
-                                      int32_t t_len, float* out, void* sync_scratch8, fa_stream_t stream) {
-  unsigned int* c = static_cast<unsigned int*>(sync_scratch8);
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (skip_mask) {
-    case 1: return fa::blstm_launch_t<1>(xproj, w_hh_fwd, w_hh_bwd, batch, t_len, 512, out, c, st);
-    case 2: return fa::blstm_launch_t<2>(xproj, w_hh_fwd, w_hh_bwd, batch, t_len, 512, out, c, st);
-    case 3: return fa::blstm_launch_t<3>(xproj, w_hh_fwd, w_hh_bwd, batch, t_len, 512, out, c, st);
-    case 4: return fa::blstm_launch_t<4>(xproj, w_hh_fwd, w_hh_bwd, batch, t_len, 512, out, c, st);
-    case 7: return fa::blstm_launch_t<7>(xproj, w_hh_fwd, w_hh_bwd, batch, t_len, 512, out, c, st);
-    default: return fa::blstm_launch_t<0>(xproj, w_hh_fwd, w_hh_bwd, batch, t_len, 512, out, c, st);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------------
-// Tensor-core recurrence (default): the same weight-stationary scheme with the [64 seq] x [32 gate rows] x [512] product of a step
+// Tensor-core recurrence: the the [64 seq] x [32 gate rows] x [512] product of a step
 // on warp-level bf16 MMAs (mma.sync.m16n8k16) with the 3-product operand split used everywhere else in this library
 // (h = hi + lo, w = hi + lo; hi.hi + hi.lo + lo.hi, fp32 accumulate, ~2^-17 relative per product).  W_hh planes stay in shared
 // memory for all steps; every CTA publishes its slice of h_t as bf16 hi / lo planes into a double-buffered exchange tensor that
 // the other CTAs copy straight into shared memory (cp.async) in the row pitch ldmatrix wants.  Fragment layout does the rest:
 // local gate row n = 8 g + u makes n-tile g of the m16n8 accumulator hold gate g of the CTA's 8 units, so one thread ends up
 // with all four gates of its (2 sequences x 2 units) cells.
-namespace fa {
 
 constexpr int LT_PITCH = LS_H * 2 + 16;      // bytes per bf16 row in shared memory (1040): 16-byte rows of 8 lanes hit 8 distinct bank groups
 
@@ -379,7 +193,9 @@ int blstm_tc_launch(const float* xproj, const float* w_hh_f, const float* w_hh_b
 
 }  // namespace fa
 
-// Tensor-core variant of fa_blstm_forward (bf16 operand split, fp32 accumulate): scratch >= fa_blstm_tc_scratch_bytes(batch).
+// One-layer bidirectional LSTM over [B, T, 512] given the input projections of both directions:
+//   xproj [B*T, 2*2048] = x W_ih^T + b_ih + b_hh, columns [0,2048) forward gates (i,f,g,o), [2048,4096) reverse.
+// scratch >= fa_blstm_tc_scratch_bytes(batch).
 extern "C" size_t fa_blstm_tc_scratch_bytes(int32_t batch) {
   const int batch_pad = (batch + fa::LS_BT - 1) / fa::LS_BT * fa::LS_BT;
   return 256 + (size_t)2 * 2 * 2 * batch_pad * fa::LS_H * 2;

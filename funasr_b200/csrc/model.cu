@@ -1,7 +1,6 @@
 // Model-level C-ABI entry points: the kernel sequences of SANMEncoder.forward, CifPredictorV2.forward and
 // ParaformerSANMDecoder.forward (+ greedy arg-max), stream-ordered over a caller-provided workspace.
 #include "common.cuh"
-#include <stdlib.h>
 #include "kernels.h"
 #include <string.h>
 #include <math.h>
@@ -15,15 +14,12 @@ std::atomic<unsigned long long> g_launch_count{0};
 
 // Side stream for the encoder's FSMN memory branch: it depends only on the QKV GEMM (like the attention kernel) and is HBM
 // bound with a tiny footprint, so it runs concurrently with the latency-bound attention kernel and joins before the
-// out-projection.  One lazily created (stream, fork event, join event) per device; FA_OVERLAP_FSMN=0 keeps everything on the
-// caller's stream.
+// out-projection.  One lazily created (stream, fork event, join event) per device.
 // The (side stream, fork event, join event) triple belongs to ONE caller stream on one device: two host threads that run
 // encoders on different streams (two fa_offline handles, one worker thread per model) get different triples, so one thread's
 // fork record can never be consumed by the other's side stream.  Calls that share a caller stream are ordered by that stream.
 struct SideStream { cudaStream_t st = nullptr; cudaEvent_t fork = nullptr, join = nullptr; };
 static SideStream* side_stream(cudaStream_t caller) {
-  static const bool enabled = [] { const char* e = getenv("FA_OVERLAP_FSMN"); return !(e && e[0] == '0'); }();
-  if (!enabled) return nullptr;
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
   static std::mutex mu;
@@ -41,11 +37,6 @@ static SideStream* side_stream(cudaStream_t caller) {
     slot = s;
   }
   return slot;
-}
-
-bool pdl_enabled() {
-  static const bool v = [] { const char* e = getenv("FA_PDL"); return e && e[0] == '1'; }();   // opt-in: measured neutral (46.0 vs 46.1 ms)
-  return v;
 }
 
 static int linear(const float* x, int64_t ldx, int64_t rows, const FaLinear& lin, int relu, const float* r1, int64_t ld1,
@@ -310,10 +301,6 @@ static size_t dec_plan(int batch, int t_max, int n_max, int vocab, int mode, siz
   return s.off + 256;
 }
 
-extern "C" size_t fa_paraformer_decoder_workspace_bytes(int32_t batch, int32_t t_max, int32_t n_max, int32_t vocab,
-                                                        int32_t gemm_mode) {
-  return dec_plan(batch, t_max, n_max, vocab, gemm_mode, dec_scratch_bytes(batch, t_max, n_max, gemm_mode), t_max);
-}
 extern "C" size_t fa_paraformer_decoder_workspace_bytes_hw(int32_t batch, int32_t t_max, int32_t n_max, int32_t vocab,
                                                            int32_t gemm_mode, int32_t n_hotwords) {
   return dec_plan(batch, t_max, n_max, vocab, gemm_mode, dec_scratch_bytes(batch, t_max, n_max, gemm_mode), n_hotwords);

@@ -325,7 +325,7 @@ extern "C" void* fa_offline_infer_hw(void* handle, const void* const* bufs, cons
   FA_OFF(m.ws.reserve(ws), "device allocation failed (workspace)");
   int rc = fa_fbank_lfr_cmvn_tables(wav, static_cast<int32_t*>(m.lens.p), B, stride, m.cmvn, m.fbank_tables, 7, 6, static_cast<float*>(m.feats.p),
                                     T, static_cast<int32_t*>(m.flens.p), T, m.st);
-  FA_OFF(rc == FA_OK, std::string("fa_fbank_lfr_cmvn: ") + fa_status_string(rc));
+  FA_OFF(rc == FA_OK, std::string("fa_fbank_lfr_cmvn_tables: ") + fa_status_string(rc));
   rc = fa_sanm_encoder_forward(&m.enc, static_cast<float*>(m.feats.p), static_cast<int32_t*>(m.flens.p), B, T, static_cast<float*>(m.encb.p),
                                m.mode, m.ws.p, m.ws.cap, m.st);
   FA_OFF(rc == FA_OK, std::string("fa_sanm_encoder_forward: ") + fa_status_string(rc));

@@ -6,7 +6,6 @@ path is a kernel in libfunasr_b200.so.
 from __future__ import annotations
 
 import ctypes as C
-import os
 import math
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -226,18 +225,14 @@ class ParaformerEngine(_EngineBase):
             # out[b, 3t+k, o] = sum_c x[b,t,c] w[c,o,k] + bias[o]  ==  one GEMM with W[(k,o), c], rows viewed as [B, 3T, 512]
             self.up_lin = lin(prefix_pred + "upsample_cnn", weight=self._dev(uw.permute(2, 1, 0).reshape(-1, uw.shape[0])),
                               bias_tensor=self._dev(state[prefix_pred + "upsample_cnn.bias"].repeat(self.up_times)))
-            self.blstm = torch.nn.LSTM(D, D, 1, bias=True, batch_first=True, dropout=0.0, bidirectional=True).to(self.device)
-            self.blstm.load_state_dict({k[len(prefix_pred + "blstm."):]: v for k, v in state.items() if k.startswith(prefix_pred + "blstm.")})
-            self.blstm.eval().requires_grad_(False)               # cuDNN path, kept for A/B (FUNASR_B200_LSTM=cudnn)
-            # this library's BLSTM: input projections of both directions as ONE GEMM ([W_ih_fwd; W_ih_bwd], b_ih + b_hh), then the
-            # persistent weight-stationary recurrence fa_blstm_forward
+            # the BLSTM: input projections of both directions as ONE GEMM ([W_ih_fwd; W_ih_bwd], b_ih + b_hh), then the
+            # persistent weight-stationary recurrence fa_blstm_forward_tc
             bp = prefix_pred + "blstm."
             w_ih = torch.cat([state[bp + "weight_ih_l0"], state[bp + "weight_ih_l0_reverse"]], 0)
             b_all = torch.cat([state[bp + "bias_ih_l0"] + state[bp + "bias_hh_l0"],
                                state[bp + "bias_ih_l0_reverse"] + state[bp + "bias_hh_l0_reverse"]], 0)
             self.lstm_ih = lin(bp + "ih", weight=self._dev(w_ih), bias_tensor=self._dev(b_all))
             self.lstm_hh_f, self.lstm_hh_b = g(bp + "weight_hh_l0"), g(bp + "weight_hh_l0_reverse")
-            self._lstm_sync = torch.zeros(2, dtype=torch.int32, device=self.device)
             self.out2_w, self.out2_b = g(prefix_pred + "cif_output2.weight"), g(prefix_pred + "cif_output2.bias")
             self.smooth2, self.noise2 = float(smooth_factor2), float(noise_threshold2)
         # ---- decoder
@@ -320,8 +315,8 @@ class ParaformerEngine(_EngineBase):
         """CifPredictorV3.get_upsample_timestamp (bicif_paraformer/cif_predictor.py:300-352): enc [B,T,512], lens [B] i32,
         token_num [B] i32 (rounded) -> (us_alphas [B,3T], us_peaks [B,3T]).  ConvTranspose1d upsampling = one GEMM of this library,
         the BLSTM = its input projections as one tensor-core GEMM + this library's persistent weight-stationary recurrence
-        (fa_blstm_forward_tc: warp-level mma.sync on bf16 hi/lo planes, not wgmma — the per-step product is only 64x32x512; or the exact fp32
-        fa_blstm_forward with FUNASR_B200_LSTM=simt), the alpha head / rescale / fire scan is fa_cif_upsample_alphas."""
+        (fa_blstm_forward_tc: warp-level mma.sync on bf16 hi/lo planes, not wgmma — the per-step product is only 64x32x512), the
+        alpha head / rescale / fire scan is fa_cif_upsample_alphas."""
         if not self.bicif:
             raise _abi.FunasrB200Error("engine was not built with bicif=True")
         B, T, D = enc.shape
@@ -330,32 +325,22 @@ class ParaformerEngine(_EngineBase):
         ws = self._workspace(max(8 * B * T * U * D * 4, 1 << 20))
         _abi.check(self.lib.fa_linear(enc.data_ptr(), D, B * T, C.byref(self.up_lin), 0, None, 0, None, 0, up.data_ptr(), U * D, self.mode,
                                       ws.data_ptr(), ws.numel(), self._stream()), "fa_linear(upsample_cnn)")
-        lstm_impl = os.environ.get("FUNASR_B200_LSTM", "tc")     # tc (default) | simt (exact fp32 FMAs) | cudnn (torch.nn.LSTM, A/B only)
-        if lstm_impl == "cudnn":
-            with torch.no_grad(), torch.backends.cudnn.flags(enabled=True, allow_tf32=False):
-                feat, _ = self.blstm(up)
-            feat = feat.contiguous()
-        else:
-            xproj = torch.empty((B * T * U, 8 * D), dtype=torch.float32, device=self.device)
-            _abi.check(self.lib.fa_linear(up.data_ptr(), D, B * T * U, C.byref(self.lstm_ih), 0, None, 0, None, 0, xproj.data_ptr(), 8 * D,
-                                          self.mode, ws.data_ptr(), ws.numel(), self._stream()), "fa_linear(blstm input projections)")
-            feat = torch.empty((B, T * U, 2 * D), dtype=torch.float32, device=self.device)
-            # the recurrence kernel holds at most 256 sequences per launch: larger batches run as consecutive launches (sequences
-            # are independent) — never a library fallback
-            for b0 in range(0, B, 256):
-                bn = min(256, B - b0)
-                xp = xproj.data_ptr() + b0 * T * U * 8 * D * 4
-                fp = feat.data_ptr() + b0 * T * U * 2 * D * 4
-                if lstm_impl == "simt":
-                    _abi.check(self.lib.fa_blstm_forward(xp, self.lstm_hh_f.data_ptr(), self.lstm_hh_b.data_ptr(), bn, T * U, D,
-                                                         fp, self._lstm_sync.data_ptr(), self._stream()), "fa_blstm_forward")
-                else:
-                    nb = int(self.lib.fa_blstm_tc_scratch_bytes(bn))
-                    if getattr(self, "_lstm_scratch", None) is None or self._lstm_scratch.numel() < nb:
-                        self._lstm_scratch = torch.empty(nb, dtype=torch.uint8, device=self.device)
-                    _abi.check(self.lib.fa_blstm_forward_tc(xp, self.lstm_hh_f.data_ptr(), self.lstm_hh_b.data_ptr(), bn, T * U, D,
-                                                            fp, self._lstm_scratch.data_ptr(), self._lstm_scratch.numel(),
-                                                            self._stream()), "fa_blstm_forward_tc")
+        xproj = torch.empty((B * T * U, 8 * D), dtype=torch.float32, device=self.device)
+        _abi.check(self.lib.fa_linear(up.data_ptr(), D, B * T * U, C.byref(self.lstm_ih), 0, None, 0, None, 0, xproj.data_ptr(), 8 * D,
+                                      self.mode, ws.data_ptr(), ws.numel(), self._stream()), "fa_linear(blstm input projections)")
+        feat = torch.empty((B, T * U, 2 * D), dtype=torch.float32, device=self.device)
+        # the recurrence kernel holds at most 256 sequences per launch: larger batches run as consecutive launches (sequences
+        # are independent) — never a library fallback
+        for b0 in range(0, B, 256):
+            bn = min(256, B - b0)
+            xp = xproj.data_ptr() + b0 * T * U * 8 * D * 4
+            fp = feat.data_ptr() + b0 * T * U * 2 * D * 4
+            nb = int(self.lib.fa_blstm_tc_scratch_bytes(bn))
+            if getattr(self, "_lstm_scratch", None) is None or self._lstm_scratch.numel() < nb:
+                self._lstm_scratch = torch.empty(nb, dtype=torch.uint8, device=self.device)
+            _abi.check(self.lib.fa_blstm_forward_tc(xp, self.lstm_hh_f.data_ptr(), self.lstm_hh_b.data_ptr(), bn, T * U, D,
+                                                    fp, self._lstm_scratch.data_ptr(), self._lstm_scratch.numel(),
+                                                    self._stream()), "fa_blstm_forward_tc")
         us_alphas = torch.empty((B, T * U), dtype=torch.float32, device=self.device)
         us_peaks = torch.empty_like(us_alphas)
         lens_up = (lens.to(torch.int32) * U).contiguous()
@@ -507,7 +492,7 @@ class ParaformerEngine(_EngineBase):
         Without taps the stage outputs live in engine-owned buffers (stable addresses) and the decoder + arg-max + filter launch
         sequence (~190 mostly small kernels) is replayed from a CUDA graph once the same (shape, n_max) has been seen twice —
         measured 9.4 -> 8.2 ms at B=64; the encoder (few large kernels, launches already hidden) gains nothing from a graph
-        and is launched directly.  FUNASR_B200_GRAPHS=0 disables the graph path."""
+        and is launched directly."""
         B, T, _ = feats.shape
         fused = not want_taps
         enc = self._encode(self.enc, feats, lens, self.cfg.d_model, out=self._persist("enc", (B, T, self.cfg.d_model)) if fused else None)
@@ -555,7 +540,7 @@ class ParaformerEngine(_EngineBase):
             ids, _, _ = self.decode(enc, lens, acoustic, tok, n_max, out=(bufs[0], bufs[1]))
             self.greedy_filter(ids, tok, sos, eos, blank, out=(bufs[2], bufs[3]))
 
-        if self.contextual or os.environ.get("FUNASR_B200_GRAPHS", "1") == "0":
+        if self.contextual:
             run()
             return bufs[2], bufs[3]
         # size the workspace BEFORE the key is formed: a growth replaces it (and drops every graph)

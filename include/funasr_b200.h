@@ -144,25 +144,18 @@ const char* fa_status_string(int status);
 /* ---------------------------------------------------------------------------------------------
  * Frontend — replaces WavFrontend.forward (funasr/frontends/wav_frontend.py:149-196), i.e.
  * torchaudio.compliance.kaldi.fbank (dither=0, hamming, 25 ms / 10 ms, 80 mel, snip_edges) + apply_lfr
- * (:63-86, m=7 n=6) + apply_cmvn (:46-60), fused.  wav is float32 in [-1,1] (x32768 applied inside,
+ * (:63-86) + apply_cmvn (:46-60), fused.  wav is float32 in [-1,1] (x32768 applied inside,
  * :169).  Rows t >= feat_lens[b] of feats are zero-filled (pad_sequence(..., 0.0), :195).
- *   wav [B, wav_stride], wav_lens[B] (samples, >= 400), cmvn [2,560] or NULL,
- *   mel_banks [80,257] (kaldi.py get_mel_banks + zero column), window [400] (hamming),
- *   feats [B, t_max, 560], feat_lens [B].
  * ------------------------------------------------------------------------------------------- */
-int fa_fbank_lfr_cmvn(const float* wav, const int32_t* wav_lens, int32_t batch, int64_t wav_stride,
-                      const float* cmvn, const float* mel_banks, const float* window,
-                      float* feats, int32_t* feat_lens, int32_t t_max, fa_stream_t stream);
-/* Same, writing utterance b at feats + b * feats_batch_stride_rows * 560 (t_max rows each): lets the caller leave room
- * for prepended frames, e.g. SenseVoiceSmall's 4 query frames (funasr/models/sense_voice/model.py:971-995). */
-int fa_fbank_lfr_cmvn_strided(const float* wav, const int32_t* wav_lens, int32_t batch, int64_t wav_stride,
-                              const float* cmvn, const float* mel_banks, const float* window, float* feats,
-                              int64_t feats_batch_stride_rows, int32_t* feat_lens, int32_t t_max, fa_stream_t stream);
-/* The same kernel fed with PRECOMPUTED constants (what the engines use): fa_fbank_make_tables derives, once per configuration,
- * the sparse support of the 80 mel filters, the FFT twiddles and the window into `tables` (fa_fbank_tables_bytes() bytes of
- * device memory), so that a CTA copies 9 KB instead of re-scanning the [80, 257] filter matrix.  lfr_m / lfr_n select the
- * low-frame-rate stacking: 7 / 6 (Paraformer, SenseVoice: feats [B, t_max, 560]) or 5 / 1 (the FSMN-VAD frontend,
- * fsmn_vad_streaming/template.yaml:54-62: feats [B, t_max, 400], one row per 10 ms frame); cmvn is [2, 80 * lfr_m] or NULL. */
+/* fa_fbank_make_tables derives, once per configuration, the sparse support of the 80 mel filters, the FFT twiddles, the window
+ * and the mel tap schedule into `tables` (fa_fbank_tables_bytes() bytes of device memory) from
+ *   mel_banks [80,257] (kaldi.py get_mel_banks + zero column), window [400] (hamming).
+ * fa_fbank_lfr_cmvn_tables then computes, from those tables,
+ *   wav [B, wav_stride], wav_lens[B] (samples, >= 400), cmvn [2, 80 * lfr_m] or NULL -> feats, feat_lens [B],
+ * writing utterance b at feats + b * feats_batch_stride_rows * 80 * lfr_m (t_max rows each): a stride above t_max leaves room
+ * for prepended frames, e.g. SenseVoiceSmall's 4 query frames (funasr/models/sense_voice/model.py:971-995).  lfr_m / lfr_n select
+ * the low-frame-rate stacking: 7 / 6 (Paraformer, SenseVoice: feats [B, t_max, 560]) or 5 / 1 (the FSMN-VAD frontend,
+ * fsmn_vad_streaming/template.yaml:54-62: feats [B, t_max, 400], one row per 10 ms frame). */
 size_t fa_fbank_tables_bytes(void);
 int fa_fbank_make_tables(const float* mel_banks, const float* window, float* tables, fa_stream_t stream);
 int fa_fbank_lfr_cmvn_tables(const float* wav, const int32_t* wav_lens, int32_t batch, int64_t wav_stride, const float* cmvn,
@@ -171,7 +164,7 @@ int fa_fbank_lfr_cmvn_tables(const float* wav, const int32_t* wav_lens, int32_t 
 /* One utterance shorter than a 25 ms frame (2 <= n_samples < 400): WavFrontend.forward passes frame_length = min(25 ms, len / fs)
  * (funasr/frontends/wav_frontend.py:174), so kaldi.fbank uses the whole utterance as ONE window of n_samples (hamming, `window`),
  * zero-padded to padded_fft = the next power of two, with mel_banks [80, padded_fft / 2 + 1] built for that FFT size; the single
- * log-mel frame is repeated lfr_m times and CMVN'd into feats_row [80 * lfr_m].  (The batched kernels above give such rows
+ * log-mel frame is repeated lfr_m times and CMVN'd into feats_row [80 * lfr_m].  (The batched kernel above gives such rows
  * feat_lens = 0.) */
 int fa_fbank_short(const float* wav, int32_t n_samples, const float* window, const float* mel_banks, int32_t padded_fft,
                    const float* cmvn, int32_t lfr_m, float* feats_row, fa_stream_t stream);
@@ -215,7 +208,7 @@ int fa_fsmn(const float* v, int64_t ldv, const int32_t* lens, int32_t batch, int
 /* The same memory block through the TMA-staged, warp-specialised kernel (persistent CTAs, cp.async.bulk.tensor ring of
  * [64 + k - 1] x 128-channel boxes, results bit-identical to fa_fsmn).  FA_ERR_UNSUPPORTED unless ksize is 11 or 21, channels is a
  * multiple of 128 and v / res are 16-byte aligned with pitches that are multiples of 4 floats.  fa_fsmn and the model-level calls
- * take this route by default when the shape allows it and t_max >= 64 (FA_FSMN_TMA=0: SIMT kernel only). */
+ * take this route when the shape allows it and t_max >= 64. */
 int fa_fsmn_tma(const float* v, int64_t ldv, const int32_t* lens, int32_t batch, int32_t t_max, int32_t channels,
                 const float* w, int32_t ksize, const float* res, int64_t ld_res, float* out, int64_t ld_out,
                 fa_stream_t stream);
@@ -277,34 +270,23 @@ int fa_cif_upsample_alphas(const float* feat, int32_t dz, const float* w, const 
                            float threshold, float* us_alphas, float* us_peaks, fa_stream_t stream);
 
 /* One-layer bidirectional LSTM recurrence (torch.nn.LSTM(512, 512, 1, batch_first=True, bidirectional=True), the `blstm` of
- * CifPredictorV3, bicif_paraformer/cif_predictor.py:187-190) as a persistent weight-stationary kernel.  The caller supplies
- * the input projections of ALL steps (one fa_linear): xproj [B*T, 4096] = x [W_ih_fwd; W_ih_bwd]^T + (b_ih + b_hh), gate order
- * i,f,g,o per direction.  w_hh_* [2048, 512].  out [B, T, 1024] (forward | reverse).  batch <= 256, hidden == 512.
- * sync_scratch8: 8 bytes of device memory (zeroed by the call) for the per-direction step barrier. */
-int fa_blstm_forward(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, int32_t batch, int32_t t_len,
-                     int32_t hidden, float* out, void* sync_scratch8, fa_stream_t stream);
-
-/* Tensor-core variant (default in the plugin): the per-step [B,512] x [512,2048] product on warp-level fp16 MMAs with the
- * 3-product operand split (fp32 accumulate), h exchanged between CTAs as fp16 hi / lo planes.  Same contract as
- * fa_blstm_forward; scratch >= fa_blstm_tc_scratch_bytes(batch) bytes of device memory (zeroed by the call). */
+ * CifPredictorV3, bicif_paraformer/cif_predictor.py:187-190) as a persistent weight-stationary kernel: the per-step
+ * [B,512] x [512,2048] product on warp-level bf16 MMAs with the 3-product operand split (fp32 accumulate), h exchanged between
+ * CTAs as bf16 hi / lo planes.  The caller supplies the input projections of ALL steps (one fa_linear):
+ * xproj [B*T, 4096] = x [W_ih_fwd; W_ih_bwd]^T + (b_ih + b_hh), gate order i,f,g,o per direction.  w_hh_* [2048, 512].
+ * out [B, T, 1024] (forward | reverse).  batch <= 256, hidden == 512.
+ * scratch >= fa_blstm_tc_scratch_bytes(batch) bytes of device memory (zeroed by the call). */
 size_t fa_blstm_tc_scratch_bytes(int32_t batch);
 int fa_blstm_forward_tc(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, int32_t batch, int32_t t_len,
                         int32_t hidden, float* out, void* scratch, size_t scratch_bytes, fa_stream_t stream);
-
-/* Measurement aid for fa_blstm_forward: skip_mask bit 0 drops the recurrent dot products, bit 1 the h gather, bit 2 the step
- * barrier (results are then meaningless); used by tools/bicif_probe.py to attribute the step time. */
-int fa_debug_blstm_variant(int32_t skip_mask, const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, int32_t batch,
-                           int32_t t_len, float* out, void* sync_scratch8, fa_stream_t stream);
 
 /* ParaformerSANMDecoder.forward (decoder.py:397-449) + greedy argmax (paraformer/model.py:642-644).
  *   enc [B,T,512], enc_lens[B]; acoustic [B, ld_acoustic_rows, 512] of which the first n_max rows are used;
  *   tok_lens[B].  Outputs: argmax_ids [B, n_max] int32, argmax_logp [B, n_max] (log-softmax value of the
  *   arg-max, :643), and — if logits != NULL — the full pre-softmax logits [B, n_max, vocab].
  *   If log_softmax != 0 the logits buffer is converted in place to log_softmax (model.py:345). */
-size_t fa_paraformer_decoder_workspace_bytes(int32_t batch, int32_t t_max, int32_t n_max, int32_t vocab,
-                                             int32_t gemm_mode);
-/* Same, for a contextual decoder (FaDecoder.has_bias) with n_hotwords entries in its hotword memory; the plain query above
- * assumes n_hotwords <= t_max. */
+/* Workspace size: n_hotwords is the number of entries in the hotword memory of a contextual decoder (FaDecoder.has_bias), 0 for
+ * a plain one. */
 size_t fa_paraformer_decoder_workspace_bytes_hw(int32_t batch, int32_t t_max, int32_t n_max, int32_t vocab,
                                                 int32_t gemm_mode, int32_t n_hotwords);
 int fa_paraformer_decoder_forward(const FaDecoder* dec, const float* enc, const int32_t* enc_lens, int32_t batch,

@@ -533,7 +533,7 @@ def test_silence_and_minimum_length():
     assert int(ref2["token_num"].max()) == 0 and ref2["ids"] == [[], [], []]
 
 
-def test_abi_error_codes():
+def test_abi_status_codes():
     """The C ABI reports problems as negative status codes (no exceptions, no silent fallback): bad arguments (-1),
     workspace too small (-3), unsupported shapes (-4); the Python layer turns them into FunasrB200Error."""
     abi, lib = _lib()
@@ -553,7 +553,7 @@ def test_abi_error_codes():
     assert lib.fa_sanm_encoder_forward(C.byref(eng.enc), feats.data_ptr(), lens.data_ptr(), 0, T, out.data_ptr(), eng.mode, ws.data_ptr(), need, _st()) == -1
     nm = abi.FaNorm(feats.data_ptr(), feats.data_ptr(), 4100, 1e-12)       # rows longer than the kernel supports
     assert lib.fa_layernorm(feats.data_ptr(), 4, C.byref(nm), out.data_ptr(), None, 1.0, 1, _st()) == -4
-    assert lib.fa_fbank_lfr_cmvn(None, None, 1, 0, None, None, None, None, None, 1, _st()) == -1
+    assert lib.fa_fbank_lfr_cmvn_tables(None, None, 1, 0, None, None, 7, 6, None, 1, None, 1, _st()) == -1
     with pytest.raises(abi.FunasrB200Error):
         abi.check(-3, "demo")
     torch.cuda.synchronize()
@@ -594,7 +594,7 @@ def test_offline_handle_api_vs_reference_golden(tmp_path, mode):
 def test_bicif_vs_reference_golden(name, mode):
     """BiCifParaformer (SURVEY §8f rank 1) against the unmodified reference: CifPredictorV3's sequential fp32 `cif` on the token
     branch (fa_cif_predictor_forward, cif_variant 1), the upsampled timestamp head (ConvTranspose1d as a GEMM of this library,
-    cuDNN BLSTM, fa_cif_upsample_alphas) and the per-token [start_ms, end_ms] the reference derives from it."""
+    the BLSTM fa_blstm_forward_tc, fa_cif_upsample_alphas) and the per-token [start_ms, end_ms] the reference derives from it."""
     from conftest import gold_stamps, load_bicif_case
     from funasr_b200 import synth
     from funasr_b200.engine import FrontendEngine, ParaformerEngine

@@ -1,4 +1,5 @@
-"""Times the BiCifParaformer additions at the benchmark shape (B=64 x 30 s): token path vs the upsampled timestamp head."""
+"""Times the BiCifParaformer additions at the benchmark shape (B=64 x 30 s): token path vs the upsampled timestamp head, and this
+library's BLSTM recurrence against cuDNN's."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -9,7 +10,8 @@ from funasr_b200.engine import FrontendEngine, ParaformerEngine
 B = 64
 dev = "cuda:0"
 cfg = synth.ParaformerConfig()
-eng = ParaformerEngine(synth.make_bicif_state_dict(cfg, 0), cfg, dev, gemm_mode="fp16x3", bicif=True)
+state = synth.make_bicif_state_dict(cfg, 0)
+eng = ParaformerEngine(state, cfg, dev, gemm_mode="fp16x3", bicif=True)
 fe = FrontendEngine(synth.make_cmvn(cfg, 1), dev)
 base = [synth.make_wav(480000, 100 + i) for i in range(4)]
 wav = torch.stack([base[i % 4].roll(977 * i) for i in range(B)]).to(dev)
@@ -34,35 +36,26 @@ out = eng.forward_feats(feats, fl)
 t_tok = timeit(lambda: eng.forward_feats(fe(wav, wl, 500)[0], fl))
 enc, lens, tok = out["enc_dev"], out["lens_dev"], out["tok_dev"]
 t_ts = timeit(lambda: eng.upsample_timestamp(enc, lens, tok))
-# split of the head
-U, D = 3, 512
-up = torch.empty((B, 500 * U, D), device=dev)
+# the recurrence alone: fa_blstm_forward_tc against torch.nn.LSTM (cuDNN, TF32 off) with the same weights and input
+bp = "predictor.blstm."
+lstm = torch.nn.LSTM(512, 512, 1, bias=True, batch_first=True, bidirectional=True).to(dev)
+lstm.load_state_dict({k[len(bp):]: v for k, v in state.items() if k.startswith(bp)})
+lstm.eval().requires_grad_(False)
+x = torch.randn(B, 1500, 512, device=dev) * 0.5
+torch.backends.cuda.matmul.allow_tf32 = False
 with torch.no_grad(), torch.backends.cudnn.flags(enabled=True, allow_tf32=False):
-    t_lstm = timeit(lambda: eng.blstm(up))
-import ctypes as C
+    xproj = torch.cat([x @ lstm.weight_ih_l0.T + (lstm.bias_ih_l0 + lstm.bias_hh_l0),
+                       x @ lstm.weight_ih_l0_reverse.T + (lstm.bias_ih_l0_reverse + lstm.bias_hh_l0_reverse)], -1).reshape(B * 1500, 4096)
+    t_lstm = timeit(lambda: lstm(x))
+    ref, _ = lstm(x)
 from funasr_b200 import _abi
-xproj = torch.randn(B * 1500, 4096, device=dev) * 0.5
-feat = torch.empty(B, 1500, 1024, device=dev)
 st = torch.cuda.current_stream().cuda_stream
-t_rec = timeit(lambda: _abi.check(eng.lib.fa_blstm_forward(xproj.data_ptr(), eng.lstm_hh_f.data_ptr(), eng.lstm_hh_b.data_ptr(), B, 1500, 512,
-                                                          feat.data_ptr(), eng._lstm_sync.data_ptr(), st), "blstm"))
-print(f"fa_blstm_forward (SIMT fp32) alone (recurrence, B={B}, T=1500): {t_rec:.2f} ms = {t_rec / 1500 * 1000:.2f} us per step")
 nbs = int(eng.lib.fa_blstm_tc_scratch_bytes(B))
 scr = torch.empty(nbs, dtype=torch.uint8, device=dev)
-feat_tc = torch.empty_like(feat)
+feat_tc = torch.empty(B, 1500, 1024, device=dev)
 t_tc = timeit(lambda: _abi.check(eng.lib.fa_blstm_forward_tc(xproj.data_ptr(), eng.lstm_hh_f.data_ptr(), eng.lstm_hh_b.data_ptr(), B, 1500, 512,
                                                             feat_tc.data_ptr(), scr.data_ptr(), nbs, st), "blstm tc"))
 torch.cuda.synchronize()
-print(f"fa_blstm_forward_tc (mma.sync fp16x3) alone: {t_tc:.2f} ms = {t_tc / 1500 * 1000:.2f} us per step; max |tc - simt| = {float((feat_tc - feat).abs().max()):.3e}")
-for mask, what in ((1, "no dot products"), (2, "no gather"), (4, "no barrier"), (3, "no dot, no gather"), (7, "x loads + gates + stores only")):
-    tm = timeit(lambda: _abi.check(eng.lib.fa_debug_blstm_variant(mask, xproj.data_ptr(), eng.lstm_hh_f.data_ptr(), eng.lstm_hh_b.data_ptr(), B, 1500,
-                                                                    feat.data_ptr(), eng._lstm_sync.data_ptr(), st), "blstm variant"), n=3)
-    print(f"  variant {mask} ({what}): {tm:.2f} ms = {tm / 1.5:.2f} us per step")
-os.environ["FUNASR_B200_LSTM"] = "cudnn"
-t_ts_cudnn = timeit(lambda: eng.upsample_timestamp(enc, lens, tok))
-os.environ["FUNASR_B200_LSTM"] = "tc"
-a_n, p_n = eng.upsample_timestamp(enc, lens, tok)
-os.environ["FUNASR_B200_LSTM"] = "cudnn"
-a_c, p_c = eng.upsample_timestamp(enc, lens, tok)
-print("native vs cuDNN us_alphas max abs diff %.3e, rel %.3e; head with cuDNN %.2f ms" % (float((a_n - a_c).abs().max()), float((a_n - a_c).abs().max() / a_c.abs().max()), t_ts_cudnn))
-print(f"B={B}: token path (frontend+encoder+CIF(v3)+decoder) {t_tok:.2f} ms; timestamp head {t_ts:.2f} ms of which cuDNN BLSTM [64,1500,512] {t_lstm:.2f} ms")
+print(f"fa_blstm_forward_tc (mma.sync bf16 x3) alone (recurrence, B={B}, T=1500): {t_tc:.2f} ms = {t_tc / 1500 * 1000:.2f} us per step; "
+      f"max |tc - cuDNN| = {float((feat_tc - ref).abs().max()):.3e}")
+print(f"B={B}: token path (frontend+encoder+CIF(v3)+decoder) {t_tok:.2f} ms; timestamp head {t_ts:.2f} ms; cuDNN BLSTM [64,1500,512] {t_lstm:.2f} ms")
