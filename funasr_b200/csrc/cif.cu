@@ -4,9 +4,11 @@
 // and cif_v1 (:853-908).  No host synchronisation: fires are compacted on the device, the token count per
 // utterance is written to token_num and read by the host once per batch.
 //
-// Arithmetic follows the reference's rounding order where it decides integer outcomes: alpha prefix sums in
-// fp64 then cast to fp32 (:835), fires = (fire + ps) - floor(ps) (:846-847), per-channel fp32 running sum of
-// alpha*h with separate multiply and add (:878), frame = ((PH[t_k] - PH[t_{k-1}]) + rem_{k-1} h_{k-1}) - rem_k h_k (:896).
+// Arithmetic follows the reference's rounding order: alpha prefix sums in fp64 then cast to fp32 (:835),
+// fires = (fire + ps) - floor(ps) (:846-847), the per-channel running sum of the fp32 products alpha*h kept in fp64 and
+// rounded to fp32 where it is read (:878: torch's CPU cumsum of a float32 tensor accumulates in double,
+// acc_type<float> = double), frame = ((PH[t_k] - PH[t_{k-1}]) + rem_{k-1} h_{k-1}) - rem_k h_k (:896).  The acoustic
+// embeddings therefore equal the reference's bit for bit.
 #include "common.cuh"
 #include "kernels.h"
 #include "tc_common.cuh"
@@ -136,7 +138,8 @@ __device__ float torch_row_sum_f32(const float* __restrict__ x, int n) {
 //                       sums -> fires / remainders / fire ordinals into shared memory (every channel group of an utterance
 //                       repeats this scalar scan — 500 steps, all groups run concurrently; group 0 writes the per-utterance outputs).
 //   phase 2 (all threads): channel-wise running sum of alpha'*h' over time, emitting one acoustic frame per fire.  The sum is a
-//                       sequential fp32 cumsum per channel (the reference's order), so the kernel is bound by the latency of its
+//                       sequential cumsum per channel in fp64 over the fp32 products, rounded to fp32 at each fire (torch's CPU
+//                       cumsum, which accumulates float32 in double), so the kernel is bound by the latency of its
 //                       loads, not by bytes: 64 channels per CTA put 8 CTAs on every utterance (512 CTAs at B = 64 instead of 64 —
 //                       round 2 launch list: 189 us for 65 MB with one 512-thread CTA per utterance), and the time loop fetches
 //                       CIF_UNROLL frames ahead of the dependent adds.
@@ -190,7 +193,8 @@ cif_fire_kernel(const float* __restrict__ enc, const float* __restrict__ alpha_r
   float* ob = acoustic + (int64_t)b * n_cap * d;
   const int c = blockIdx.y * CIF_CH + threadIdx.x;
   if (c < d) {
-    float acc = 0.f, prev_acc = 0.f, prev_rh = 0.f;
+    double acc = 0.0;                     // PH[t] before its rounding to fp32
+    float prev_ph = 0.f, prev_rh = 0.f;
     for (int t0 = 0; t0 < T1; t0 += CIF_UNROLL) {
       float hh[CIF_UNROLL];
 #pragma unroll
@@ -203,12 +207,13 @@ cif_fire_kernel(const float* __restrict__ enc, const float* __restrict__ alpha_r
         const int t = t0 + u;
         if (t < T1) {
           const float h = hh[u];
-          acc = __fadd_rn(acc, __fmul_rn(s_alpha[t], h));                 // cumsum(alphas * hidden) :878
+          acc = __dadd_rn(acc, (double)__fmul_rn(s_alpha[t], h));         // cumsum(alphas * hidden) :878
           const int k = s_ord[t];
           if (k >= 0) {
+            const float ph = __double2float_rn(acc);                      // the cumsum's fp32 output PH[t]
             const float rh = __fmul_rn(s_rem[t], h);
-            if (k < n_cap) ob[(int64_t)k * d + c] = __fsub_rn(__fadd_rn(__fsub_rn(acc, prev_acc), prev_rh), rh);   // :896
-            prev_acc = acc;
+            if (k < n_cap) ob[(int64_t)k * d + c] = __fsub_rn(__fadd_rn(__fsub_rn(ph, prev_ph), prev_rh), rh);   // :896
+            prev_ph = ph;
             prev_rh = rh;
           }
         }
