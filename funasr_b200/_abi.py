@@ -114,12 +114,16 @@ SIGNATURES = {
     "fa_split_rows": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _i32, _vp, _vp]),
     "fa_linear_planes": (C.c_int, [_vp, _i64, C.POINTER(FaLinear), _i32, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _vp]),
     "fa_linear_planes_to_planes": (C.c_int, [_vp, _i64, C.POINTER(FaLinear), _i32, _vp, _i64, _i32, _vp]),
+    "fa_linear_attn_sinks": (C.c_int, [_vp, _i64, C.POINTER(FaLinear), _i32, _i32, _i32, _i32, _i32, _i32, _f, _vp, _vp, _vp, _vp, _i64,
+                                       _i32, _vp]),
     "fa_fsmn": (C.c_int, [_vp, _i64, _vp, _i32, _i32, _i32, _vp, _i32, _vp, _i64, _vp, _i64, _vp]),
     "fa_fsmn_tma": (C.c_int, [_vp, _i64, _vp, _i32, _i32, _i32, _vp, _i32, _vp, _i64, _vp, _i64, _vp]),
     "fa_fsmn_simt": (C.c_int, [_vp, _i64, _vp, _i32, _i32, _i32, _vp, _i32, _vp, _i64, _vp, _i64, _vp]),
     "fa_attention": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _vp, _i64, _vp]),
     "fa_attention_tc_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32]),
     "fa_attention_tc": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _vp, _i64, _i32, _vp, _sz, _vp]),
+    "fa_attention_tc_planes": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _vp]),
+    "fa_attention_f32_ex": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _i32, _vp]),
     "fa_sanm_encoder_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "fa_sanm_encoder_forward": (C.c_int, [C.POINTER(FaEncoder), _vp, _vp, _i32, _i32, _vp, _i32, _vp, _sz, _vp]),
     "fa_cif_predictor_workspace_bytes": (_sz, [_i32, _i32, _i32]),

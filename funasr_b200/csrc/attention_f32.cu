@@ -225,3 +225,14 @@ extern "C" int fa_attention(const float* q, int64_t ldq, const float* k, int64_t
   return fa::attention_f32_launch(q, ldq, k, ldk, v, ldv, key_lens, batch, heads, tq, tk, ctx, ld_ctx,
                                   (cudaStream_t)stream, 0);
 }
+
+// the kernel choice of the encoder's fp32 path (model.cu): the tiled kernel for 128-wide heads, the warp-per-query one otherwise
+extern "C" int fa_attention_f32_ex(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
+                                   const int32_t* key_lens, int32_t batch, int32_t heads, int32_t head_dim, int32_t tq, int32_t tk,
+                                   float* ctx, int64_t ld_ctx, int32_t kv_shared, fa_stream_t stream) {
+  if (heads < 1) return FA_ERR_ARG;
+  if (head_dim == fa::ATT_D)
+    return fa::attention_f32_launch(q, ldq, k, ldk, v, ldv, key_lens, batch, heads, tq, tk, ctx, ld_ctx, (cudaStream_t)stream, kv_shared);
+  return fa::attention_small_launch(q, ldq, k, ldk, v, ldv, key_lens, batch, heads, head_dim, tq, tk, ctx, ld_ctx, (cudaStream_t)stream,
+                                    kv_shared);
+}

@@ -285,12 +285,17 @@ scale_split_kernel(const float* __restrict__ src, int64_t ld, int64_t rows, int 
   }
 }
 
+// exactly what attention_tc_launch takes from its scratch arena (the same Arena::take sequence; a shared K/V takes less)
 size_t attention_tc_scratch_bytes(int batch, int heads, int tq, int tk, int mode) {
   if (mode == FA_GEMM_F32_SIMT) return 0;
   const int npl = mode == FA_GEMM_F16X1 ? 1 : 2;
   const int tkp = (tk + 63) / 64 * 64;
   const int d = heads * AT_D;
-  return (size_t)npl * 2 * ((size_t)batch * tq * d + (size_t)batch * tk * d + (size_t)batch * d * tkp) + 4096;
+  ArenaSizer s;
+  s.take((size_t)npl * batch * tq * d * sizeof(plane_t));
+  s.take((size_t)npl * batch * tk * d * sizeof(plane_t));
+  s.take((size_t)npl * batch * d * tkp * sizeof(plane_t));
+  return s.off;
 }
 
 int attention_tc_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
@@ -389,4 +394,17 @@ extern "C" int fa_attention_tc(const float* q, int64_t ldq, const float* k, int6
   fa::Arena scratch(workspace, ws_bytes);
   return fa::attention_tc_launch(q, ldq, k, ldk, v, ldv, key_lens, batch, heads, tq, tk, ctx, ld_ctx, nullptr, 0, 0, gemm_mode,
                                  &scratch, (cudaStream_t)stream, 0);
+}
+
+extern "C" int fa_attention_tc_planes(const void* q_planes, const void* k_planes, const void* vt_planes, const int32_t* key_lens,
+                                      int32_t batch, int32_t heads, int32_t tq, int32_t tk, float* ctx, int64_t ld_ctx, void* ctx_planes,
+                                      int64_t ld_planes, int32_t out_nplanes, int32_t gemm_mode, int32_t kv_shared, fa_stream_t stream) {
+  if (gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) return FA_ERR_ARG;
+  if (heads < 1 || heads * fa::AT_D > 4096 || (!ctx && !ctx_planes)) return FA_ERR_ARG;
+  if (ctx && (ld_ctx < heads * fa::AT_D || (ld_ctx & 3))) return FA_ERR_ARG;          // float2 stores
+  if (ctx_planes && (ld_planes < heads * fa::AT_D || (ld_planes & 1))) return FA_ERR_ARG;   // 4-byte stores of two fp16
+  return fa::attention_tc_planes_launch(reinterpret_cast<const fa::plane_t*>(q_planes), reinterpret_cast<const fa::plane_t*>(k_planes),
+                                        reinterpret_cast<const fa::plane_t*>(vt_planes), key_lens, batch, heads, tq, tk, ctx, ld_ctx,
+                                        reinterpret_cast<fa::plane_t*>(ctx_planes), ld_planes, out_nplanes, gemm_mode, (cudaStream_t)stream,
+                                        kv_shared);
 }

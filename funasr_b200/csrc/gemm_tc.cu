@@ -119,13 +119,14 @@ __device__ __forceinline__ void store_planes4(plane_t* dst, int64_t plane_stride
 }
 
 // per-head transposed V planes straight from the row-per-lane registers: for a fixed head dim the 32 lanes hold 32
-// consecutive keys, so every 2-byte store instruction covers one 64-byte run
+// consecutive keys, so every 2-byte store instruction covers one 64-byte run.  The value is fmaf(acc, acc_scale, bias), rounded
+// once, as in every other output of the epilogue (the fp32 V rows the FSMN reads, the staged transpose).
 template <int NPL>
 __device__ __forceinline__ void store_vt16(plane_t* dst, int64_t t_pad, int64_t plane, const uint32_t (&r)[16], const float* bias, float acc_scale) {
 #pragma unroll
   for (int j = 0; j < 16; j += 2) {
-    float x0 = __uint_as_float(r[j]) * acc_scale, x1 = __uint_as_float(r[j + 1]) * acc_scale;
-    if (bias) { x0 += __ldg(bias + j); x1 += __ldg(bias + j + 1); }
+    const float b0 = bias ? __ldg(bias + j) : 0.f, b1 = bias ? __ldg(bias + j + 1) : 0.f;
+    float x0 = fmaf(__uint_as_float(r[j]), acc_scale, b0), x1 = fmaf(__uint_as_float(r[j + 1]), acc_scale, b1);
     plane_t* d0 = dst + (int64_t)j * t_pad;
 #pragma unroll
     for (int pl = 0; pl < NPL; ++pl) {

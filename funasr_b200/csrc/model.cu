@@ -744,6 +744,39 @@ extern "C" int fa_linear_planes(const void* a_planes, int64_t rows, const FaLine
                                nullptr, 0, gemm_mode, (cudaStream_t)stream);
 }
 
+extern "C" int fa_linear_attn_sinks(const void* a_planes, int64_t rows, const FaLinear* lin, int32_t q0, int32_t k0, int32_t v0,
+                                    int32_t width, int32_t t_rows, int32_t t_pad, float qscale, void* q_planes, void* k_planes,
+                                    void* vt_planes, float* v_f32, int64_t ld_v_f32, int32_t gemm_mode, fa_stream_t stream) {
+  if (!a_planes || !lin || rows < 0) return FA_ERR_ARG;
+  if (gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) return FA_ERR_ARG;
+  const int N = lin->out_f;
+  if (width <= 0 || width % 32 != 0 || t_rows <= 0 || rows % t_rows != 0) return FA_ERR_ARG;
+  const int32_t start[3] = {q0, k0, v0};
+  void* const dst[3] = {q_planes, k_planes, vt_planes};
+  int n_on = 0;
+  for (int i = 0; i < 3; ++i) {
+    if (start[i] < 0) continue;                                   // disabled
+    // the epilogue routes whole 16-column chunks, stores 8 bytes at a time, and writes nothing outside the range it was given
+    if (start[i] % 16 != 0 || start[i] + width > N || !dst[i] || (reinterpret_cast<uintptr_t>(dst[i]) & 7)) return FA_ERR_ARG;
+    for (int j = 0; j < i; ++j)
+      if (start[j] >= 0 && start[i] < start[j] + width && start[j] < start[i] + width) return FA_ERR_ARG;   // overlapping sinks
+    ++n_on;
+  }
+  if (n_on == 0) return FA_ERR_ARG;
+  if (v0 >= 0 && t_pad < t_rows) return FA_ERR_ARG;
+  if (v_f32 && (v0 < 0 || ld_v_f32 < N)) return FA_ERR_ARG;       // fp32 V rows are the GEMM's output rows: columns [v0, v0 + width)
+  const int npl = gemm_mode == FA_GEMM_F16X1 ? 1 : 2;
+  AttnSinks sk;
+  if (q0 >= 0) sk.q0 = q0;
+  if (k0 >= 0) sk.k0 = k0;
+  if (v0 >= 0) sk.v0 = v0;
+  sk.width = width; sk.npl = npl; sk.t_rows = t_rows; sk.t_pad = v0 >= 0 ? t_pad : 64; sk.qscale = qscale;
+  sk.q_planes = reinterpret_cast<plane_t*>(q_planes); sk.k_planes = reinterpret_cast<plane_t*>(k_planes);
+  sk.vt_planes = reinterpret_cast<plane_t*>(vt_planes);
+  return gemm_tc_planes_launch(reinterpret_cast<const plane_t*>(a_planes), rows, *lin, 0, nullptr, 0, nullptr, 0, v_f32, ld_v_f32, nullptr, 0,
+                               gemm_mode, (cudaStream_t)stream, &sk);
+}
+
 extern "C" int fa_linear_planes_to_planes(const void* a_planes, int64_t rows, const FaLinear* lin, int32_t relu, void* out_planes,
                                           int64_t ld_out, int32_t gemm_mode, fa_stream_t stream) {
   if (!a_planes || !lin || !out_planes || gemm_mode == FA_GEMM_F32_SIMT) return FA_ERR_ARG;

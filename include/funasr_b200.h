@@ -198,6 +198,16 @@ int fa_linear_planes(const void* a_planes, int64_t rows, const FaLinear* lin, in
  * encoder makes for FFN w_1, whose ReLU output feeds w_2 without an fp32 round trip (bench.py times exactly this launch). */
 int fa_linear_planes_to_planes(const void* a_planes, int64_t rows, const FaLinear* lin, int32_t relu, void* out_planes,
                                int64_t ld_out, int32_t gemm_mode, fa_stream_t stream);
+/* Same GEMM with the attention-operand epilogue the QKV / q / kv projections use (no ReLU): output columns [q0, q0 + width) go to
+ * q_planes [qpl][rows][width] as fp16 planes of fl(y * qscale), [k0, k0 + width) to k_planes [qpl][rows][width], and [v0, v0 + width)
+ * to vt_planes [qpl][rows / t_rows * width][t_pad], V transposed per utterance of t_rows rows (row b * t_rows + t, column c ->
+ * vt row b * width + c, column t; columns [t_rows, t_pad) are not written); qpl = 1 for FA_GEMM_F16X1, else 2.  A negative start
+ * disables that sink; the enabled ranges must start at a multiple of 16, lie inside [0, out_f) and not overlap.  v_f32 != NULL
+ * (leading dim ld_v_f32 >= out_f) also receives the fp32 V columns at their own column positions (the FSMN input); nothing else is
+ * written there.  FA_ERR_ARG for rows % t_rows != 0, t_pad < t_rows with the V sink, or a bad sink range. */
+int fa_linear_attn_sinks(const void* a_planes, int64_t rows, const FaLinear* lin, int32_t q0, int32_t k0, int32_t v0, int32_t width,
+                         int32_t t_rows, int32_t t_pad, float qscale, void* q_planes, void* k_planes, void* vt_planes, float* v_f32,
+                         int64_t ld_v_f32, int32_t gemm_mode, fa_stream_t stream);
 
 /* FSMN memory block: out = m * (v*m + dwconv_k(v*m)) (+ res); m[t] = t < lens[b]
  * (MultiHeadedAttentionSANM.forward_fsmn attention.py:216-239; decoder variant :583-631).  out must not overlap v or res (the staged
@@ -231,6 +241,21 @@ size_t fa_attention_tc_workspace_bytes(int32_t batch, int32_t heads, int32_t tq,
 int fa_attention_tc(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
                     const int32_t* key_lens, int32_t batch, int32_t heads, int32_t tq, int32_t tk,
                     float* ctx, int64_t ld_ctx, int32_t gemm_mode, void* workspace, size_t ws_bytes, fa_stream_t stream);
+/* The tensor-core attention on operand planes already in place, as the models call it after fa_linear_attn_sinks:
+ * q_planes [npl][B * tq][H * 128] (already scaled by d_k^-0.5), k_planes [npl][kb * tk][H * 128], vt_planes [npl][kb * H * 128][tkp]
+ * with tkp = tk rounded up to 64 (columns >= tk are never read), npl = 1 for FA_GEMM_F16X1, else 2; kb = 1 when kv_shared != 0
+ * (every utterance attends over the same keys and values, the hotword memory), else B.  Writes ctx [B * tq][ld_ctx] fp32 and / or
+ * ctx_planes [out_nplanes][B * tq][ld_planes] fp16 (the split of the same fp32 values, the A operand of the out-projection):
+ * out_nplanes 1 for FA_GEMM_F16X1, 2 or 3 otherwise (FA_ERR_UNSUPPORTED for the other pairings, FA_ERR_ARG outside 1..3). */
+int fa_attention_tc_planes(const void* q_planes, const void* k_planes, const void* vt_planes, const int32_t* key_lens, int32_t batch,
+                           int32_t heads, int32_t tq, int32_t tk, float* ctx, int64_t ld_ctx, void* ctx_planes, int64_t ld_planes,
+                           int32_t out_nplanes, int32_t gemm_mode, int32_t kv_shared, fa_stream_t stream);
+/* fp32 attention with the fp32 path's kernel choice: head_dim 128 -> the tiled kernel of fa_attention, any other multiple of 32 up
+ * to 128 -> the warp-per-query kernel (CT-Transformer's 8 x 32 heads; FA_ERR_UNSUPPORTED when 4 * tk floats exceed its 160 KB of
+ * shared memory).  kv_shared != 0: k / v hold one batch entry [tk, ld] that every utterance attends over. */
+int fa_attention_f32_ex(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
+                        const int32_t* key_lens, int32_t batch, int32_t heads, int32_t head_dim, int32_t tq, int32_t tk,
+                        float* ctx, int64_t ld_ctx, int32_t kv_shared, fa_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Model-level entry points
