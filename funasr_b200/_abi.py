@@ -114,6 +114,8 @@ SIGNATURES = {
     "fa_split_rows": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _i32, _vp, _vp]),
     "fa_linear_planes": (C.c_int, [_vp, _i64, C.POINTER(FaLinear), _i32, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _vp]),
     "fa_linear_planes_to_planes": (C.c_int, [_vp, _i64, C.POINTER(FaLinear), _i32, _vp, _i64, _i32, _vp]),
+    "fa_linear_planes_view": (C.c_int, [_vp, _i64, _i64, _i64, C.POINTER(FaLinear), _i32, _vp, _i64, _i32, _vp]),
+    "fa_layernorm_planes": (C.c_int, [_vp, _i64, C.POINTER(FaNorm), _vp, _vp, _i32, _i32, _vp, _f, _i32, _vp, _vp]),
     "fa_linear_attn_sinks": (C.c_int, [_vp, _i64, C.POINTER(FaLinear), _i32, _i32, _i32, _i32, _i32, _i32, _f, _vp, _vp, _vp, _vp, _i64,
                                        _i32, _vp]),
     "fa_fsmn": (C.c_int, [_vp, _i64, _vp, _i32, _i32, _i32, _vp, _i32, _vp, _i64, _vp, _i64, _vp]),

@@ -700,9 +700,14 @@ int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& li
   if (lda & 7) return FA_ERR_UNSUPPORTED;
   if (!lin.w_planes || !a_planes) return FA_ERR_ARG;
   const int N = lin.out_f, Kp = lin.in_pad;
+  if (N <= 0) return FA_ERR_ARG;
   if (Kp % TC_BK != 0 || M * 3 > 0x7fffffffLL) return FA_ERR_UNSUPPORTED;
   if (y && (ldy & 3) == 0 && (((uintptr_t)y) & 15)) return FA_ERR_UNSUPPORTED;
   if ((r1 && (ld1 & 3)) || (r2 && (ld2 & 3))) return FA_ERR_UNSUPPORTED;
+  // the epilogue reads bias and residual rows as float4 and writes output planes as uint2 (store_planes4)
+  if ((lin.b && (((uintptr_t)lin.b) & 15)) || (r1 && (((uintptr_t)r1) & 15)) || (r2 && (((uintptr_t)r2) & 15))) return FA_ERR_UNSUPPORTED;
+  if (out_planes && ((ldo & 3) || (((uintptr_t)out_planes) & 7))) return FA_ERR_UNSUPPORTED;
+  if ((y && ldy < N) || (r1 && ld1 < N) || (r2 && ld2 < N) || (out_planes && ldo < N)) return FA_ERR_ARG;
   const int npl = planes_for_mode(mode);
   // 128 x 128 tiles with a 6 (x1) / 3 (x3) stage ring; 128 x 64 for x6 (three planes per operand: two 72 KB stages, a third does
   // not fit beside the epilogue staging in 227 KB).

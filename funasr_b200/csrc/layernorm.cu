@@ -136,3 +136,17 @@ extern "C" int fa_layernorm(const float* x, int64_t rows, const FaNorm* norm, fl
   if (!norm) return FA_ERR_ARG;
   return fa::layernorm_launch(x, rows, *norm, y, pe_inv, xscale, rows_per_batch, (cudaStream_t)stream, nullptr, 0, 0, nullptr);
 }
+
+// The same LayerNorm with the tensor-core path's fused outputs: fp16 planes [nplanes][rows][cols_pad] (columns [n, cols_pad) zeroed)
+// and, with pe_inv, the embedded rows x * xscale + PE in emb_out.  y may be NULL when planes is set.
+extern "C" int fa_layernorm_planes(const float* x, int64_t rows, const FaNorm* norm, float* y, void* planes, int32_t nplanes,
+                                   int32_t cols_pad, const float* pe_inv, float xscale, int32_t rows_per_batch, float* emb_out,
+                                   fa_stream_t stream) {
+  if (!norm || rows < 0 || (planes && (nplanes < 1 || nplanes > 3)) || (!planes && nplanes != 0)) return FA_ERR_ARG;
+  if (emb_out && !pe_inv) return FA_ERR_ARG;                       // the embedded rows exist only with the PE prologue
+  if (pe_inv && rows_per_batch <= 0) return FA_ERR_ARG;
+  // rows are read and written as float4, planes as uint2
+  if ((((uintptr_t)x) & 15) || (((uintptr_t)y) & 15) || (((uintptr_t)emb_out) & 15) || (((uintptr_t)planes) & 7)) return FA_ERR_UNSUPPORTED;
+  return fa::layernorm_launch(x, rows, *norm, y, pe_inv, xscale, rows_per_batch, (cudaStream_t)stream, reinterpret_cast<fa::plane_t*>(planes),
+                              nplanes, cols_pad, emb_out);
+}

@@ -784,6 +784,21 @@ extern "C" int fa_linear_planes_to_planes(const void* a_planes, int64_t rows, co
                                reinterpret_cast<plane_t*>(out_planes), ld_out, gemm_mode, (cudaStream_t)stream);
 }
 
+// The GEMM over an overlapping ("conv view") A operand, as the CIF conv and the CAM++ TDNN launch it: row r of plane p is the
+// in_pad elements at (p * a_plane_rows + r) * a_ld.  a_plane_rows >= rows + ceil((in_pad - a_ld) / a_ld) keeps every valid row's
+// span inside its own plane, which is also what the tensor map's row count (gemm_tc_planes_launch) relies on.
+extern "C" int fa_linear_planes_view(const void* a_planes, int64_t rows, int64_t a_ld, int64_t a_plane_rows, const FaLinear* lin,
+                                     int32_t relu, float* y, int64_t ldy, int32_t gemm_mode, fa_stream_t stream) {
+  if (!a_planes || !lin || !y || rows < 0 || a_ld <= 0) return FA_ERR_ARG;
+  if (gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) return FA_ERR_ARG;
+  if (a_ld % 8 != 0) return FA_ERR_UNSUPPORTED;
+  const int64_t kp = lin->in_pad;
+  const int64_t extra = a_ld < kp ? (kp - a_ld + a_ld - 1) / a_ld : 0;
+  if (a_plane_rows < rows + extra) return FA_ERR_ARG;
+  return gemm_tc_planes_launch(reinterpret_cast<const plane_t*>(a_planes), rows, *lin, relu, nullptr, 0, nullptr, 0, y, ldy, nullptr, 0,
+                               gemm_mode, (cudaStream_t)stream, nullptr, a_ld, a_plane_rows);
+}
+
 // rows of an embedding table: out[i, :] = table[ids[i], :] (torch.nn.Embedding forward, e.g. CTTransformer.embed ct_transformer/model.py:120)
 __global__ void embedding_kernel(const int32_t* __restrict__ ids, const float* __restrict__ table, int dim, int vocab, int64_t n, float* __restrict__ out) {
   const int64_t i = blockIdx.x;

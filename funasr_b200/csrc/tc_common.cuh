@@ -111,10 +111,13 @@ __device__ __forceinline__ void wgmma_m64n128_rs(float (&d)[64], const uint32_t 
 }
 // ------------------------------------------------------------------------------------------------ operand planes
 // A 16-bit "plane" element of the split x = p0 + p1 (+ p2).  Planes are IEEE fp16 (11-bit significands): two planes carry ~22
-// bits of x, so the three products hi*hi + hi*lo + lo*hi of the x3 mode are good to ~2^-22 relative — 64x tighter than the same
-// three products on bf16 planes (8-bit significands, ~2^-16), at the same tensor-core rate.  Every GEMM operand of this path is
-// LayerNorm-, ReLU- or softmax-bounded and sits far inside the fp16 range (conversions saturate at +-65504 instead of producing
-// inf; values below 2^-14 go subnormal, 6e-8 spacing).
+// bits of x when the mid plane is a normal number, i.e. for |x| >= ~2^-3; the three products hi*hi + hi*lo + lo*hi of the x3 mode
+// are then good to ~2^-22 relative — 64x tighter than the same three products on bf16 planes (8-bit significands, ~2^-16), at the
+// same tensor-core rate.  Below that the mid plane goes subnormal (fp16 subnormals below 2^-14, absolute spacing 2^-24) and the
+// split loses bits: the models' weights (~N(0, 1/K)) are rebuilt from two planes to a median 4.6e-7 relative (2^-21.1) at K = 512
+// and 9.2e-7 (2^-20.1) at K = 2048, and their third plane is almost all zero, so x6 adds nothing over x3 there
+// (tests/test_gemm_gpu.py measures both floors).  Every GEMM operand of this path is LayerNorm-, ReLU- or softmax-bounded and sits
+// far inside the fp16 range (conversions saturate at +-65504 instead of producing inf).
 typedef __half plane_t;
 __device__ __forceinline__ uint32_t pack_planes2(float e0, float e1) {      // {e0 -> low half, e1 -> high half}, round to nearest, saturating
   uint32_t r;

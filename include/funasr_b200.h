@@ -38,8 +38,9 @@ typedef enum {
 typedef enum {
   FA_GEMM_F32_SIMT = 0, /* fp32 FFMA tiles: the parity reference path */
   FA_GEMM_F16X1 = 1,   /* wgmma f16, one fp16 pass (fast mode) */
-  FA_GEMM_F16X3 = 3,   /* wgmma, fp16 planes x = hi + lo: hi*hi + hi*lo + lo*hi (~2^-22 relative per product) */
-  FA_GEMM_F16X6 = 6    /* wgmma, three fp16 planes, six products (~fp32) */
+  FA_GEMM_F16X3 = 3,   /* wgmma, fp16 planes x = hi + lo: hi*hi + hi*lo + lo*hi (~2^-22 relative per product for operands above
+                        * ~2^-3 in magnitude; ~2^-21 / 2^-20 for weights at 1/sqrt(512) / 1/sqrt(2048), whose mid plane is subnormal) */
+  FA_GEMM_F16X6 = 6    /* wgmma, three fp16 planes, six products (~fp32 for operands above ~2^-3; no better than x3 below) */
 } FaGemmMode;
 
 /* nn.Linear: y = x W^T + b.  w_planes (optional) holds the fp16 planes made by fa_split_planes for the
@@ -181,6 +182,13 @@ int fa_broadcast_rows(const float* rows, int32_t n_rows, int32_t cols, float* ds
  * SinusoidalPositionEncoder embedding.py:396-432); rows_per_batch gives t = row % rows_per_batch. */
 int fa_layernorm(const float* x, int64_t rows, const FaNorm* norm, float* y,
                  const float* pe_inv, float xscale, int32_t rows_per_batch, fa_stream_t stream);
+/* The same LayerNorm with the fused outputs of the tensor-core path: planes != NULL receives the normalised rows as fp16 planes
+ * [nplanes][rows][cols_pad] (hi, mid, lo; nplanes 1..3, n <= cols_pad <= 2048, cols_pad % 4 == 0) with columns [n, cols_pad) zero
+ * in every plane: the A operand of the next GEMM (cols_pad = its in_pad).  y (fp32, may equal x) may be NULL when planes is set.
+ * emb_out != NULL (needs pe_inv) also receives the embedded rows x * xscale + PE before the norm.  x, y, emb_out 16-byte aligned,
+ * planes 8-byte aligned (FA_ERR_UNSUPPORTED otherwise). */
+int fa_layernorm_planes(const float* x, int64_t rows, const FaNorm* norm, float* y, void* planes, int32_t nplanes, int32_t cols_pad,
+                        const float* pe_inv, float xscale, int32_t rows_per_batch, float* emb_out, fa_stream_t stream);
 
 /* y[rows, out_f] = act(x[rows, in_f(ldx)] W^T + b) (+ res1) (+ res2); replaces torch.nn.Linear calls
  * (attention.py:256,306; positionwise_feed_forward.py:34).  relu != 0 applies ReLU before residuals. */
@@ -198,6 +206,16 @@ int fa_linear_planes(const void* a_planes, int64_t rows, const FaLinear* lin, in
  * encoder makes for FFN w_1, whose ReLU output feeds w_2 without an fp32 round trip (bench.py times exactly this launch). */
 int fa_linear_planes_to_planes(const void* a_planes, int64_t rows, const FaLinear* lin, int32_t relu, void* out_planes,
                                int64_t ld_out, int32_t gemm_mode, fa_stream_t stream);
+/* fa_linear_planes and fa_linear_planes_to_planes refuse, before any launch: bias / residual bases not 16-byte aligned, y not
+ * 16-byte aligned with ldy % 4 == 0, residual pitches or ld_out not multiples of 4, out_planes not 8-byte aligned
+ * (FA_ERR_UNSUPPORTED); ldy, ld_res1, ld_res2 or ld_out below out_f (FA_ERR_ARG). */
+/* The same GEMM (fp32 output, no residual) over an overlapping "conv view" of the A planes, as the CIF conv (a_ld = 512,
+ * in_pad = 1536: three consecutive frames per row) and the CAM++ TDNN (a_ld = 640, in_pad = 1600: kernel 5, stride 2) run it:
+ * row r of plane p is the lin->in_pad elements starting at element (p * a_plane_rows + r) * a_ld of a_planes.  a_ld % 8 != 0 ->
+ * FA_ERR_UNSUPPORTED; a_plane_rows < rows + ceil((in_pad - a_ld) / a_ld) when a_ld < in_pad (a valid row would reach into the next
+ * plane), or < rows otherwise -> FA_ERR_ARG. */
+int fa_linear_planes_view(const void* a_planes, int64_t rows, int64_t a_ld, int64_t a_plane_rows, const FaLinear* lin, int32_t relu,
+                          float* y, int64_t ldy, int32_t gemm_mode, fa_stream_t stream);
 /* Same GEMM with the attention-operand epilogue the QKV / q / kv projections use (no ReLU): output columns [q0, q0 + width) go to
  * q_planes [qpl][rows][width] as fp16 planes of fl(y * qscale), [k0, k0 + width) to k_planes [qpl][rows][width], and [v0, v0 + width)
  * to vt_planes [qpl][rows / t_rows * width][t_pad], V transposed per utterance of t_rows rows (row b * t_rows + t, column c ->
