@@ -125,6 +125,7 @@ SIGNATURES = {
     "fa_attention_tc_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32]),
     "fa_attention_tc": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _vp, _i64, _i32, _vp, _sz, _vp]),
     "fa_attention_tc_planes": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _vp]),
+    "fa_attention_tc_planes_ex": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _vp]),
     "fa_attention_f32_ex": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _i32, _vp]),
     "fa_sanm_encoder_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "fa_sanm_encoder_forward": (C.c_int, [C.POINTER(FaEncoder), _vp, _vp, _i32, _i32, _vp, _i32, _vp, _sz, _vp]),

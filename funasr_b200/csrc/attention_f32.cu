@@ -142,8 +142,9 @@ attention_f32_kernel(const float* __restrict__ q, int64_t ldq, const float* __re
   }
 }
 
-// Generic head dimension (multiple of 32, <= 128) for the small SAN-M stacks around the hot path — CT-Transformer punctuation:
-// 8 heads x 32 (ct_transformer/template.yaml:31-45) over a few dozen tokens.  One warp per (utterance, head, query): scores of all
+// Generic head dimension (a multiple of 32 up to 128, or 80) for the small SAN-M stacks around the hot path — CT-Transformer
+// punctuation: 8 heads x 32 (ct_transformer/template.yaml:31-45) over a few dozen tokens — and the fp32 parity path of the fa-zh
+// aligner (4 heads x 80).  One warp per (utterance, head, query): scores of all
 // keys into shared memory, max, exp / sum, weighted sum of v.  Same mask semantics as the tiled kernel above.
 __global__ void __launch_bounds__(128)
 attention_small_kernel(const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, int64_t ldk, const float* __restrict__ v,
@@ -158,16 +159,17 @@ attention_small_kernel(const float* __restrict__ q, int64_t ldq, const float* __
   const int b = (int)(row / ((int64_t)tq * heads));
   const int klen = min(key_lens[b], tk);
   const int bkv = kv_shared ? 0 : b;
-  const int per = hd >> 5;                              // dims per lane (1..4)
+  const int per = (hd + 31) >> 5;                       // dims per lane (1..4); lane + 32 j < hd holds a dim
   float* sc = s_sc + warp * tk;
   const float* qr = q + ((int64_t)b * tq + n) * ldq + h * hd;
   float qv[4] = {0.f, 0.f, 0.f, 0.f};
-  for (int j = 0; j < per; ++j) qv[j] = __fmul_rn(qr[lane + 32 * j], qscale);
+  for (int j = 0; j < per; ++j) qv[j] = lane + 32 * j < hd ? __fmul_rn(qr[lane + 32 * j], qscale) : 0.f;
   float mx = -INFINITY;
   for (int t = 0; t < klen; ++t) {
     const float* kr = k + ((int64_t)bkv * tk + t) * ldk + h * hd;
     float acc = 0.f;
-    for (int j = 0; j < per; ++j) acc = fmaf(qv[j], kr[lane + 32 * j], acc);
+    for (int j = 0; j < per; ++j)
+      if (lane + 32 * j < hd) acc = fmaf(qv[j], kr[lane + 32 * j], acc);
     acc = warp_sum(acc);
     if (lane == 0) sc[t] = acc;
     mx = fmaxf(mx, acc);
@@ -181,17 +183,19 @@ attention_small_kernel(const float* __restrict__ q, int64_t ldq, const float* __
   for (int t = 0; t < klen; ++t) {
     const float p = sc[t] / sum;
     const float* vr = v + ((int64_t)bkv * tk + t) * ldv + h * hd;
-    for (int j = 0; j < per; ++j) o[j] = fmaf(p, vr[lane + 32 * j], o[j]);
+    for (int j = 0; j < per; ++j)
+      if (lane + 32 * j < hd) o[j] = fmaf(p, vr[lane + 32 * j], o[j]);
   }
   float* dst = ctx + ((int64_t)b * tq + n) * ldc + h * hd;
-  for (int j = 0; j < per; ++j) dst[lane + 32 * j] = klen > 0 ? o[j] : 0.f;
+  for (int j = 0; j < per; ++j)
+    if (lane + 32 * j < hd) dst[lane + 32 * j] = klen > 0 ? o[j] : 0.f;
 }
 
 int attention_small_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, const int32_t* key_lens,
                            int batch, int heads, int head_dim, int tq, int tk, float* ctx, int64_t ldc, cudaStream_t st, int kv_shared) {
   if (batch <= 0 || tq <= 0) return FA_OK;
   if (!q || !k || !v || !key_lens || !ctx || tk <= 0) return FA_ERR_ARG;
-  if (head_dim < 32 || head_dim > 128 || (head_dim & 31)) return FA_ERR_UNSUPPORTED;
+  if (head_dim < 32 || head_dim > 128 || ((head_dim & 31) && head_dim != 80)) return FA_ERR_UNSUPPORTED;
   const size_t smem = (size_t)4 * tk * sizeof(float);
   if (smem > 160 * 1024) return FA_ERR_UNSUPPORTED;
   if (smem > 48 * 1024) FA_CUDA_OK(cudaFuncSetAttribute(attention_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

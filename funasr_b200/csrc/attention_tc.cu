@@ -35,12 +35,15 @@ struct AttTcParams {
   plane_t* ctx_planes; int64_t ldp; int out_nplanes;   // fp16 planes [npl][B*tq][ldp] (or null)
 };
 
-// NPL: operand planes (1 | 2); OPL: context planes written (0 = fp32 context only).
+// NPL: operand planes (1 | 2); OPL: context planes written (0 = fp32 context only); HD: head dim, 128 or 80.
+// An 80-wide head is read as two 64-dim boxes like a 128-wide one (same 128B swizzle, same descriptors): the score MMAs use only
+// the first 16-dim k-step of the second box, and P.V (n = 80) only its first 16 d-rows.  The rest of that box is the neighbouring
+// head's columns, or the map's zero fill after the last head.
 // One CTA = 128 queries of one (utterance, head), 384 threads: warp 0 is the TMA producer, warps 4-11 are two consumer
 // warpgroups of 64 query rows each.  K and V chunks share ONE shared-memory ring, filled in the order the consumers read them
 //   pass A: Khi(0) .. Khi(nc-1)          pass B: K(0), V(0), K(1), V(1), ..., K(nc-1), V(nc-1)
 // and each slot is released by the eight consumer warps once their MMAs on it have retired.
-template <int NPL, int OPL>
+template <int NPL, int OPL, int HD>
 __global__ void __launch_bounds__(384, 1)
 attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                     const __grid_constant__ CUtensorMap map_v, const AttTcParams p) {
@@ -79,7 +82,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
       for (int pl = 0; pl < NPL; ++pl)
 #pragma unroll
         for (int kb = 0; kb < 2; ++kb)
-          tma_load_2d(sQ + (pl * 2 + kb) * AT_Q_KBLK, &map_q, q_full, h * AT_D + kb * 64,
+          tma_load_2d(sQ + (pl * 2 + kb) * AT_Q_KBLK, &map_q, q_full, h * HD + kb * 64,
                       (int)(pl * p.q_plane_rows + (int64_t)b * p.tq + q0));
       uint32_t n = 0;                                       // ring sequence number
       auto load_chunk = [&](bool is_v, int idx, int nb) {  // nb boxes of 8 KB: box bi = plane bi / 2, half bi % 2
@@ -89,8 +92,8 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
         unsigned char* dst = sRing + slot * SLOT_BYTES;
         for (int bi = 0; bi < nb; ++bi) {
           const int pl = bi >> 1, sub = bi & 1;
-          if (is_v) tma_load_2d(dst + bi * AT_BOX, &map_v, &r_full[slot], idx * AT_BKEY, (int)(pl * p.v_plane_rows + ((int64_t)bkv * p.heads + h) * AT_D + sub * 64));
-          else tma_load_2d(dst + bi * AT_BOX, &map_k, &r_full[slot], h * AT_D + sub * 64, (int)(pl * p.k_plane_rows + (int64_t)bkv * p.tk + idx * AT_BKEY));
+          if (is_v) tma_load_2d(dst + bi * AT_BOX, &map_v, &r_full[slot], idx * AT_BKEY, (int)(pl * p.v_plane_rows + ((int64_t)bkv * p.heads + h) * HD + sub * 64));
+          else tma_load_2d(dst + bi * AT_BOX, &map_k, &r_full[slot], h * HD + sub * 64, (int)(pl * p.k_plane_rows + (int64_t)bkv * p.tk + idx * AT_BKEY));
         }
         ++n;
       };
@@ -107,9 +110,9 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
     const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2), cq = 2 * (lane & 3);
     const int ta[3] = {0, 0, 1}, tb[3] = {0, 1, 0};
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-    float o[64];
+    float o[HD / 2];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) o[i] = 0.f;
+    for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
     if (nc > 0) {
       const uint32_t q_addr = smem_u32(sQ) + wg * (64 * 128), ring_addr = smem_u32(sRing);
       uint32_t n = 0;                                       // ring sequence number
@@ -128,7 +131,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
         wgmma_fence();
         for (int term = 0; term < nterm; ++term) {
 #pragma unroll
-          for (int k = 0; k < AT_D / 16; ++k) {
+          for (int k = 0; k < HD / 16; ++k) {
             const uint64_t da = make_sw128_desc(q_addr + (ta[term] * 2 + (k >> 2)) * AT_Q_KBLK) + 2 * (k & 3);
             const uint64_t db = make_sw128_desc(k_addr + (tb[term] * 2 + (k >> 2)) * AT_BOX) + 2 * (k & 3);
             wgmma_m64n64_ss(s, da, db, (term | k) != 0 ? 1u : 0u);
@@ -188,7 +191,10 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
         for (int term = 0; term < NT; ++term) {
           const uint64_t db = make_sw128_desc(v_addr + tb[term] * 2 * AT_BOX);
 #pragma unroll
-          for (int kk = 0; kk < AT_BKEY / 16; ++kk) wgmma_m64n128_rs(o, ta[term] == 0 ? ph[kk] : plo[kk], db + 2 * kk, 1u);
+          for (int kk = 0; kk < AT_BKEY / 16; ++kk) {
+            if constexpr (HD == 128) wgmma_m64n128_rs(o, ta[term] == 0 ? ph[kk] : plo[kk], db + 2 * kk, 1u);
+            else wgmma_m64n80_rs(o, ta[term] == 0 ? ph[kk] : plo[kk], db + 2 * kk, 1u);
+          }
         }
         wgmma_commit();
         wgmma_wait_all();
@@ -212,9 +218,9 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
       const int64_t grow = (int64_t)b * p.tq + row;
       const float inv = half ? inv1 : inv0;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
+      for (int j = 0; j < HD / 8; ++j) {
         float x0 = o[4 * j + 2 * half] * inv, x1 = o[4 * j + 2 * half + 1] * inv;
-        const int col = h * AT_D + 8 * j + cq;
+        const int col = h * HD + 8 * j + cq;
         if (p.ctx) *reinterpret_cast<float2*>(p.ctx + grow * p.ldc + col) = make_float2(x0, x1);
         if (OPL > 0) {
           plane_t* dst = p.ctx_planes + grow * p.ldp + col;
@@ -329,25 +335,39 @@ int attention_tc_launch(const float* q, int64_t ldq, const float* k, int64_t ldk
   return attention_tc_planes_launch(qp, kp, vt, key_lens, batch, heads, tq, tk, ctx, ldc, ctx_planes, ldp, out_nplanes, mode, st, kv_shared);
 }
 
-template <int NPL, int OPL>
+template <int NPL, int OPL, int HD>
 static int launch_att(dim3 grid, const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const AttTcParams& p, cudaStream_t st) {
   constexpr size_t smem = (size_t)NPL * 2 * AT_Q_KBLK + (size_t)AT_NSLOT(NPL) * NPL * 2 * AT_BOX + 1024 + (1 + 2 * AT_NSLOT(NPL)) * 8;
   static_assert(smem <= 227 * 1024, "shared memory per block");
   static PerDeviceOnce once;
-  FA_RETURN_IF_ERR(ensure_dyn_smem(attention_tc_kernel<NPL, OPL>, smem, once));
-  attention_tc_kernel<NPL, OPL><<<grid, 384, smem, st>>>(mq, mk, mv, p);
+  FA_RETURN_IF_ERR(ensure_dyn_smem(attention_tc_kernel<NPL, OPL, HD>, smem, once));
+  attention_tc_kernel<NPL, OPL, HD><<<grid, 384, smem, st>>>(mq, mk, mv, p);
   return FA_OK;
 }
 
-// Operand planes already in place (written by the producing GEMMs' epilogues, gemm_tc.cu AttnSinks):
-// qp [npl][B*tq][H*128] (scaled), kp [npl][B*tk][H*128], vt [npl][B*H*128][round_up(tk,64)].
+template <int HD>
+static int launch_att_planes(int npl, int opl, dim3 grid, const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv,
+                             const AttTcParams& p, cudaStream_t st) {
+  if (npl == 1) {
+    if (opl > 1) return FA_ERR_UNSUPPORTED;
+    return opl == 0 ? launch_att<1, 0, HD>(grid, mq, mk, mv, p, st) : launch_att<1, 1, HD>(grid, mq, mk, mv, p, st);
+  }
+  if (opl == 1) return FA_ERR_UNSUPPORTED;
+  return opl == 0 ? launch_att<2, 0, HD>(grid, mq, mk, mv, p, st)
+         : opl == 2 ? launch_att<2, 2, HD>(grid, mq, mk, mv, p, st)
+                    : launch_att<2, 3, HD>(grid, mq, mk, mv, p, st);
+}
+
+// Operand planes already in place (written by the producing GEMMs' epilogues, gemm_tc.cu AttnSinks), hd = head_dim:
+// qp [npl][B*tq][H*hd] (scaled), kp [npl][B*tk][H*hd], vt [npl][B*H*hd][round_up(tk,64)].
 int attention_tc_planes_launch(const plane_t* qp, const plane_t* kp, const plane_t* vt, const int32_t* key_lens,
                                int batch, int heads, int tq, int tk, float* ctx, int64_t ldc, plane_t* ctx_planes,
-                               int64_t ldp, int out_nplanes, int mode, cudaStream_t st, int kv_shared) {
+                               int64_t ldp, int out_nplanes, int mode, cudaStream_t st, int kv_shared, int head_dim) {
+  if (head_dim != 128 && head_dim != 80) return FA_ERR_UNSUPPORTED;
   if (batch <= 0 || tq <= 0) return FA_OK;
   if (!qp || !kp || !vt || !key_lens || tk <= 0) return FA_ERR_ARG;
   const int npl = mode == FA_GEMM_F16X1 ? 1 : 2;
-  const int d = heads * AT_D;
+  const int d = heads * head_dim;
   const int tkp = (tk + 63) / 64 * 64;
   const int kvb = kv_shared ? 1 : batch;
   const int64_t mq = (int64_t)batch * tq, mk = (int64_t)kvb * tk, mv = (int64_t)kvb * d;
@@ -366,15 +386,8 @@ int attention_tc_planes_launch(const plane_t* qp, const plane_t* kp, const plane
   dim3 grid((tq + AT_BQ - 1) / AT_BQ, heads, batch);
   const int opl = ctx_planes ? out_nplanes : 0;
   if (ctx_planes && (opl < 1 || opl > 3)) return FA_ERR_ARG;
-  if (npl == 1) {
-    if (opl > 1) return FA_ERR_UNSUPPORTED;
-    FA_RETURN_IF_ERR(opl == 0 ? (launch_att<1, 0>(grid, mq_map, mk_map, mv_map, p, st)) : (launch_att<1, 1>(grid, mq_map, mk_map, mv_map, p, st)));
-  } else {
-    if (opl == 1) return FA_ERR_UNSUPPORTED;
-    FA_RETURN_IF_ERR(opl == 0 ? (launch_att<2, 0>(grid, mq_map, mk_map, mv_map, p, st))
-                     : opl == 2 ? (launch_att<2, 2>(grid, mq_map, mk_map, mv_map, p, st))
-                                : (launch_att<2, 3>(grid, mq_map, mk_map, mv_map, p, st)));
-  }
+  FA_RETURN_IF_ERR(head_dim == 128 ? launch_att_planes<128>(npl, opl, grid, mq_map, mk_map, mv_map, p, st)
+                                    : launch_att_planes<80>(npl, opl, grid, mq_map, mk_map, mv_map, p, st));
   FA_CHECK_LAUNCH();
   return FA_OK;
 }
@@ -396,15 +409,24 @@ extern "C" int fa_attention_tc(const float* q, int64_t ldq, const float* k, int6
                                  &scratch, (cudaStream_t)stream, 0);
 }
 
-extern "C" int fa_attention_tc_planes(const void* q_planes, const void* k_planes, const void* vt_planes, const int32_t* key_lens,
-                                      int32_t batch, int32_t heads, int32_t tq, int32_t tk, float* ctx, int64_t ld_ctx, void* ctx_planes,
-                                      int64_t ld_planes, int32_t out_nplanes, int32_t gemm_mode, int32_t kv_shared, fa_stream_t stream) {
+extern "C" int fa_attention_tc_planes_ex(const void* q_planes, const void* k_planes, const void* vt_planes, const int32_t* key_lens,
+                                         int32_t batch, int32_t heads, int32_t head_dim, int32_t tq, int32_t tk, float* ctx, int64_t ld_ctx,
+                                         void* ctx_planes, int64_t ld_planes, int32_t out_nplanes, int32_t gemm_mode, int32_t kv_shared,
+                                         fa_stream_t stream) {
   if (gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) return FA_ERR_ARG;
-  if (heads < 1 || heads * fa::AT_D > 4096 || (!ctx && !ctx_planes)) return FA_ERR_ARG;
-  if (ctx && (ld_ctx < heads * fa::AT_D || (ld_ctx & 3))) return FA_ERR_ARG;          // float2 stores
-  if (ctx_planes && (ld_planes < heads * fa::AT_D || (ld_planes & 1))) return FA_ERR_ARG;   // 4-byte stores of two fp16
+  if (head_dim != 128 && head_dim != 80) return FA_ERR_UNSUPPORTED;
+  if (heads < 1 || heads * head_dim > 4096 || (!ctx && !ctx_planes)) return FA_ERR_ARG;
+  if (ctx && (ld_ctx < heads * head_dim || (ld_ctx & 3))) return FA_ERR_ARG;          // float2 stores
+  if (ctx_planes && (ld_planes < heads * head_dim || (ld_planes & 1))) return FA_ERR_ARG;   // 4-byte stores of two fp16
   return fa::attention_tc_planes_launch(reinterpret_cast<const fa::plane_t*>(q_planes), reinterpret_cast<const fa::plane_t*>(k_planes),
                                         reinterpret_cast<const fa::plane_t*>(vt_planes), key_lens, batch, heads, tq, tk, ctx, ld_ctx,
                                         reinterpret_cast<fa::plane_t*>(ctx_planes), ld_planes, out_nplanes, gemm_mode, (cudaStream_t)stream,
-                                        kv_shared);
+                                        kv_shared, head_dim);
+}
+
+extern "C" int fa_attention_tc_planes(const void* q_planes, const void* k_planes, const void* vt_planes, const int32_t* key_lens,
+                                      int32_t batch, int32_t heads, int32_t tq, int32_t tk, float* ctx, int64_t ld_ctx, void* ctx_planes,
+                                      int64_t ld_planes, int32_t out_nplanes, int32_t gemm_mode, int32_t kv_shared, fa_stream_t stream) {
+  return fa_attention_tc_planes_ex(q_planes, k_planes, vt_planes, key_lens, batch, heads, fa::AT_D, tq, tk, ctx, ld_ctx, ctx_planes,
+                                   ld_planes, out_nplanes, gemm_mode, kv_shared, stream);
 }

@@ -13,15 +13,15 @@
 
 namespace fa {
 
-constexpr int LS_H = 512;          // hidden size
+// Hidden sizes H: 512 (Paraformer-large family: 64 CTAs per direction) and 320 (fa-zh MonotonicAligner: 40 CTAs per direction).
+constexpr int LS_HMAX = 512;       // largest hidden size: sizes the exchange tensor of fa_blstm_tc_scratch_bytes
 constexpr int LS_UNITS = 8;        // hidden units per CTA
-constexpr int LS_NC = LS_H / LS_UNITS;   // 64 CTAs per direction
 constexpr int LS_ROWS = 4 * LS_UNITS;    // 32 gate rows per CTA
 constexpr int LS_BT = 64;          // sequences per batch tile (4 warps x 16 sequences)
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 
-// Tensor-core recurrence: the the [64 seq] x [32 gate rows] x [512] product of a step
+// Tensor-core recurrence: the [64 seq] x [32 gate rows] x [H] product of a step
 // on warp-level bf16 MMAs (mma.sync.m16n8k16) with the 3-product operand split used everywhere else in this library
 // (h = hi + lo, w = hi + lo; hi.hi + hi.lo + lo.hi, fp32 accumulate, ~2^-17 relative per product).  W_hh planes stay in shared
 // memory for all steps; every CTA publishes its slice of h_t as bf16 hi / lo planes into a double-buffered exchange tensor that
@@ -29,7 +29,10 @@ __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf
 // local gate row n = 8 g + u makes n-tile g of the m16n8 accumulator hold gate g of the CTA's 8 units, so one thread ends up
 // with all four gates of its (2 sequences x 2 units) cells.
 
-constexpr int LT_PITCH = LS_H * 2 + 16;      // bytes per bf16 row in shared memory (1040): 16-byte rows of 8 lanes hit 8 distinct bank groups
+// bytes per bf16 row in shared memory (1040 at H = 512, 656 at 320): an odd number of 16-byte units, so 16-byte rows of 8 lanes
+// hit 8 distinct bank groups
+template <int H>
+constexpr int lt_pitch() { return H * 2 + 16; }
 
 __device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], uint32_t addr) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
@@ -39,10 +42,12 @@ __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// hx: exchange tensor [2 parity][2 dir][2 plane][batch_pad][512] bf16 (batch_pad = tiles * 64)
+// hx: exchange tensor [2 parity][2 dir][2 plane][batch_pad][H] bf16 (batch_pad = tiles * 64)
+template <int H>
 __global__ void __launch_bounds__(128, 1)
 blstm_tc_kernel(const float* __restrict__ xproj, const float* __restrict__ w_hh_f, const float* __restrict__ w_hh_b, int batch, int T,
                 float* __restrict__ out, __nv_bfloat16* __restrict__ hx, unsigned int* __restrict__ counters) {
+  constexpr int LS_H = H, LS_NC = H / LS_UNITS, LT_PITCH = lt_pitch<H>();
   extern __shared__ __align__(16) unsigned char smb[];
   unsigned char* sWp = smb;                                   // [2 planes][32 rows][LT_PITCH]
   unsigned char* sHp = smb + 2 * LS_ROWS * LT_PITCH;          // [2 planes][64 seq][LT_PITCH]
@@ -171,34 +176,41 @@ blstm_tc_kernel(const float* __restrict__ xproj, const float* __restrict__ w_hh_
   }
 }
 
-int blstm_tc_launch(const float* xproj, const float* w_hh_f, const float* w_hh_b, int batch, int T, int hidden, float* out,
-                    void* scratch, size_t scratch_bytes, cudaStream_t st) {
-  if (batch <= 0 || T <= 0) return FA_OK;
-  if (!xproj || !w_hh_f || !w_hh_b || !out || !scratch) return FA_ERR_ARG;
-  if (hidden != LS_H || batch > 4 * LS_BT) return FA_ERR_UNSUPPORTED;
+template <int H>
+static int blstm_tc_launch_h(const float* xproj, const float* w_hh_f, const float* w_hh_b, int batch, int T, float* out,
+                             void* scratch, size_t scratch_bytes, cudaStream_t st) {
   const int batch_pad = (batch + LS_BT - 1) / LS_BT * LS_BT;
-  const size_t need = 256 + (size_t)2 * 2 * 2 * batch_pad * LS_H * sizeof(__nv_bfloat16);
+  const size_t need = 256 + (size_t)2 * 2 * 2 * batch_pad * H * sizeof(__nv_bfloat16);
   if (scratch_bytes < need) return FA_ERR_WORKSPACE;
-  const size_t smem = (size_t)2 * LS_ROWS * LT_PITCH + (size_t)2 * LS_BT * LT_PITCH;
+  const size_t smem = (size_t)2 * LS_ROWS * lt_pitch<H>() + (size_t)2 * LS_BT * lt_pitch<H>();
   static PerDeviceOnce once;
-  FA_RETURN_IF_ERR(ensure_dyn_smem(blstm_tc_kernel, smem, once));
+  FA_RETURN_IF_ERR(ensure_dyn_smem(blstm_tc_kernel<H>, smem, once));
   unsigned int* counters = static_cast<unsigned int*>(scratch);
   __nv_bfloat16* hx = reinterpret_cast<__nv_bfloat16*>(static_cast<char*>(scratch) + 256);
   FA_CUDA_OK(cudaMemsetAsync(scratch, 0, need, st));
   void* args[] = {(void*)&xproj, (void*)&w_hh_f, (void*)&w_hh_b, (void*)&batch, (void*)&T, (void*)&out, (void*)&hx, (void*)&counters};
-  FA_CUDA_OK(cudaLaunchCooperativeKernel((const void*)blstm_tc_kernel, dim3(2 * LS_NC), dim3(128), args, smem, st));
+  FA_CUDA_OK(cudaLaunchCooperativeKernel((const void*)blstm_tc_kernel<H>, dim3(2 * (H / LS_UNITS)), dim3(128), args, smem, st));
   count_launch();
   return FA_OK;
 }
 
+int blstm_tc_launch(const float* xproj, const float* w_hh_f, const float* w_hh_b, int batch, int T, int hidden, float* out,
+                    void* scratch, size_t scratch_bytes, cudaStream_t st) {
+  if (batch <= 0 || T <= 0) return FA_OK;
+  if (!xproj || !w_hh_f || !w_hh_b || !out || !scratch) return FA_ERR_ARG;
+  if ((hidden != 512 && hidden != 320) || batch > 4 * LS_BT) return FA_ERR_UNSUPPORTED;
+  return hidden == 512 ? blstm_tc_launch_h<512>(xproj, w_hh_f, w_hh_b, batch, T, out, scratch, scratch_bytes, st)
+                       : blstm_tc_launch_h<320>(xproj, w_hh_f, w_hh_b, batch, T, out, scratch, scratch_bytes, st);
+}
+
 }  // namespace fa
 
-// One-layer bidirectional LSTM over [B, T, 512] given the input projections of both directions:
-//   xproj [B*T, 2*2048] = x W_ih^T + b_ih + b_hh, columns [0,2048) forward gates (i,f,g,o), [2048,4096) reverse.
-// scratch >= fa_blstm_tc_scratch_bytes(batch).
+// One-layer bidirectional LSTM over [B, T, H], H = 512 or 320, given the input projections of both directions:
+//   xproj [B*T, 2*4H] = x W_ih^T + b_ih + b_hh, columns [0,4H) forward gates (i,f,g,o), [4H,8H) reverse.
+// scratch >= fa_blstm_tc_scratch_bytes(batch) (sized for H = 512, which covers 320).
 extern "C" size_t fa_blstm_tc_scratch_bytes(int32_t batch) {
   const int batch_pad = (batch + fa::LS_BT - 1) / fa::LS_BT * fa::LS_BT;
-  return 256 + (size_t)2 * 2 * 2 * batch_pad * fa::LS_H * 2;
+  return 256 + (size_t)2 * 2 * 2 * batch_pad * fa::LS_HMAX * 2;
 }
 extern "C" int fa_blstm_forward_tc(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, int32_t batch, int32_t t_len,
                                    int32_t hidden, float* out, void* scratch, size_t scratch_bytes, fa_stream_t stream) {

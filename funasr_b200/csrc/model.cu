@@ -95,12 +95,12 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
   const int din = enc->layers[0].norm1.n;
   const bool embed = enc->pe_inv_timescales != nullptr;   // false: plain stack over an existing [B,T,512] stream
   const int hd = enc->heads > 0 ? D / enc->heads : 0;
-  // the tensor-core kernels are built for the Paraformer / SenseVoice shape (d = 512, 4 x 128); the fp32 path also runs the small
-  // SAN-M stacks around the hot path (CT-Transformer punctuation: d = 256, 8 x 32)
-  if (D < 64 || D > 512 || (D & 15) || enc->heads < 1 || enc->heads * hd != D || hd < 32 || hd > 128 || (hd & 31) || din > 560 || (din & 15) ||
-      (!embed && din != D))
+  // the tensor-core kernels are built for two shapes: Paraformer / SenseVoice (d = 512, 4 x 128) and the fa-zh aligner (d = 320,
+  // 4 x 80); the fp32 path also runs the small SAN-M stacks around the hot path (CT-Transformer punctuation: d = 256, 8 x 32)
+  if (D < 64 || D > 512 || (D & 15) || enc->heads < 1 || enc->heads * hd != D || hd < 32 || hd > 128 || ((hd & 31) && hd != 80) ||
+      din > 560 || (din & 15) || (!embed && din != D))
     return FA_ERR_UNSUPPORTED;
-  if (gemm_mode != FA_GEMM_F32_SIMT && (D != 512 || hd != 128)) return FA_ERR_UNSUPPORTED;
+  if (gemm_mode != FA_GEMM_F32_SIMT && !((D == 512 && hd == 128) || (D == 320 && hd == 80))) return FA_ERR_UNSUPPORTED;
   Arena a(workspace, ws_bytes);
   float* u = a.take<float>(M * (size_t)560);
   float* qkv = a.take<float>(M * 1536ull);
@@ -144,7 +144,7 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
       // as fp16 planes plus fp32 v (the only fp32 columns written) for the FSMN branch
       AttnSinks sk;
       sk.q0 = 0; sk.k0 = D; sk.v0 = 2 * D; sk.width = D; sk.npl = npl < 2 ? npl : 2; sk.t_rows = t_max; sk.t_pad = t_pad;
-      sk.qscale = (float)(1.0 / sqrt(128.0)); sk.q_planes = q_planes; sk.k_planes = k_planes; sk.vt_planes = vt_planes;
+      sk.qscale = (float)pow((double)hd, -0.5); sk.q_planes = q_planes; sk.k_planes = k_planes; sk.vt_planes = vt_planes;
       FA_RETURN_IF_ERR(gemm_tc_planes_launch(u_planes, M, L.qkv, 0, nullptr, 0, nullptr, 0, qkv, 3 * D, nullptr, 0, gemm_mode, st, &sk));
     } else {
       FA_RETURN_IF_ERR(linear(u, in, M, L.qkv, 0, nullptr, 0, nullptr, 0, qkv, 3 * D, gemm_mode, &scratch, st));
@@ -181,7 +181,7 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
       // tensor-core path: attention emits the context as fp16 planes (A operand of linear_out); FFN w_1 emits its
       // ReLU output as planes for w_2 — neither intermediate makes an fp32 round trip through HBM
       FA_RETURN_IF_ERR(attention_tc_planes_launch(q_planes, k_planes, vt_planes, lens, batch, enc->heads, t_max, t_max, nullptr, 0,
-                                                  ctx_planes, D, npl, gemm_mode, st));
+                                                  ctx_planes, D, npl, gemm_mode, st, 0, hd));
       if (side) FA_CUDA_OK(cudaStreamWaitEvent(st, side->join, 0));          // join: linear_out adds the FSMN memory
       FA_RETURN_IF_ERR(gemm_tc_planes_launch(ctx_planes, M, L.out, 0, mem, D, nullptr, 0, x2, D, nullptr, 0, gemm_mode, st));   // mem already holds residual + memory
       if (L.w1.out_f != L.w2.in_pad || L.w1.in_pad != D) return FA_ERR_UNSUPPORTED;

@@ -187,6 +187,85 @@ class _EngineBase:
                                                     self.mode, ws.data_ptr(), ws.numel(), self._stream()), "fa_sanm_encoder_forward")
         return out
 
+    def _init_timestamp_head(self, prefix_pred, smooth_factor2, noise_threshold2, threshold):
+        """CifPredictorV3 timestamp head (bicif_paraformer/cif_predictor.py:121-352, upsample_type "cnn_blstm", use_cif1_cnn False),
+        shared by BiCifParaformer / SeacoParaformer and the MonotonicAligner."""
+        state, g, lin = self._state, self._g, self._lin
+        uw = state[prefix_pred + "upsample_cnn.weight"]                      # ConvTranspose1d weight [in, out, k], stride == k == 3
+        self.up_times = int(uw.shape[2])
+        # out[b, 3t+k, o] = sum_c x[b,t,c] w[c,o,k] + bias[o]  ==  one GEMM with W[(k,o), c], rows viewed as [B, 3T, D]
+        self.up_lin = lin(prefix_pred + "upsample_cnn", weight=self._dev(uw.permute(2, 1, 0).reshape(-1, uw.shape[0])),
+                          bias_tensor=self._dev(state[prefix_pred + "upsample_cnn.bias"].repeat(self.up_times)))
+        # the BLSTM: input projections of both directions as ONE GEMM ([W_ih_fwd; W_ih_bwd], b_ih + b_hh), then the
+        # persistent weight-stationary recurrence fa_blstm_forward_tc
+        bp = prefix_pred + "blstm."
+        w_ih = torch.cat([state[bp + "weight_ih_l0"], state[bp + "weight_ih_l0_reverse"]], 0)
+        b_all = torch.cat([state[bp + "bias_ih_l0"] + state[bp + "bias_hh_l0"],
+                           state[bp + "bias_ih_l0_reverse"] + state[bp + "bias_hh_l0_reverse"]], 0)
+        self.lstm_ih = lin(bp + "ih", weight=self._dev(w_ih), bias_tensor=self._dev(b_all))
+        self.lstm_hh_f, self.lstm_hh_b = g(bp + "weight_hh_l0"), g(bp + "weight_hh_l0_reverse")
+        self.out2_w, self.out2_b = g(prefix_pred + "cif_output2.weight"), g(prefix_pred + "cif_output2.bias")
+        self.smooth2, self.noise2, self.ts_threshold = float(smooth_factor2), float(noise_threshold2), float(threshold)
+
+    def upsample_timestamp(self, enc: torch.Tensor, lens: torch.Tensor, token_num: torch.Tensor):
+        """CifPredictorV3.get_upsample_timestamp (bicif_paraformer/cif_predictor.py:300-352): enc [B,T,D] (D = 512 or 320), lens [B] i32,
+        token_num [B] i32 (rounded) -> (us_alphas [B,3T], us_peaks [B,3T]).  ConvTranspose1d upsampling = one GEMM of this library,
+        the BLSTM = its input projections as one tensor-core GEMM + this library's persistent weight-stationary recurrence
+        (fa_blstm_forward_tc: warp-level mma.sync on bf16 hi/lo planes, not wgmma — the per-step product is only 64x32xD), the
+        alpha head / rescale / fire scan is fa_cif_upsample_alphas."""
+        if getattr(self, "up_lin", None) is None:
+            raise _abi.FunasrB200Error("engine was not built with the CifPredictorV3 timestamp head (bicif=True)")
+        B, T, D = enc.shape
+        U = self.up_times
+        up = torch.empty((B, T * U, D), dtype=torch.float32, device=self.device)
+        ws = self._workspace(max(8 * B * T * U * D * 4, 1 << 20))
+        _abi.check(self.lib.fa_linear(enc.data_ptr(), D, B * T, C.byref(self.up_lin), 0, None, 0, None, 0, up.data_ptr(), U * D, self.mode,
+                                      ws.data_ptr(), ws.numel(), self._stream()), "fa_linear(upsample_cnn)")
+        xproj = torch.empty((B * T * U, 8 * D), dtype=torch.float32, device=self.device)
+        _abi.check(self.lib.fa_linear(up.data_ptr(), D, B * T * U, C.byref(self.lstm_ih), 0, None, 0, None, 0, xproj.data_ptr(), 8 * D,
+                                      self.mode, ws.data_ptr(), ws.numel(), self._stream()), "fa_linear(blstm input projections)")
+        feat = torch.empty((B, T * U, 2 * D), dtype=torch.float32, device=self.device)
+        # the recurrence kernel holds at most 256 sequences per launch: larger batches run as consecutive launches (sequences
+        # are independent) — never a library fallback
+        for b0 in range(0, B, 256):
+            bn = min(256, B - b0)
+            xp = xproj.data_ptr() + b0 * T * U * 8 * D * 4
+            fp = feat.data_ptr() + b0 * T * U * 2 * D * 4
+            nb = int(self.lib.fa_blstm_tc_scratch_bytes(bn))
+            if getattr(self, "_lstm_scratch", None) is None or self._lstm_scratch.numel() < nb:
+                self._lstm_scratch = torch.empty(nb, dtype=torch.uint8, device=self.device)
+            _abi.check(self.lib.fa_blstm_forward_tc(xp, self.lstm_hh_f.data_ptr(), self.lstm_hh_b.data_ptr(), bn, T * U, D,
+                                                    fp, self._lstm_scratch.data_ptr(), self._lstm_scratch.numel(),
+                                                    self._stream()), "fa_blstm_forward_tc")
+        us_alphas = torch.empty((B, T * U), dtype=torch.float32, device=self.device)
+        us_peaks = torch.empty_like(us_alphas)
+        lens_up = (lens.to(torch.int32) * U).contiguous()
+        tok = token_num.to(self.device, torch.int32).contiguous()
+        _abi.check(self.lib.fa_cif_upsample_alphas(feat.data_ptr(), 2 * D, self.out2_w.data_ptr(), self.out2_b.data_ptr(), lens_up.data_ptr(),
+                                                   tok.data_ptr(), B, T * U, self.smooth2, self.noise2, self.ts_threshold,
+                                                   us_alphas.data_ptr(), us_peaks.data_ptr(), self._stream()), "fa_cif_upsample_alphas")
+        return us_alphas, us_peaks
+
+
+class AlignerEngine(_EngineBase):
+    """MonotonicAligner (monotonic_aligner/model.py): the SAN-M encoder plus CifPredictorV3's timestamp head — no token
+    predictor, no decoder (`predictor.cif_conv1d` / `cif_output` are not used by get_upsample_timestamp)."""
+
+    def __init__(self, state: Dict[str, torch.Tensor], cfg: ParaformerConfig, device, gemm_mode: str = "fp32",
+                 smooth_factor2: float = 0.25, noise_threshold2: float = 0.01):
+        self._init_base(state, device, gemm_mode, cfg.ln_eps)
+        self.cfg = cfg
+        K = int(state["encoder.encoders0.0.self_attn.fsmn_block.weight"].shape[-1])
+        names = ["encoder." + ("encoders0.0" if i == 0 else "encoders.%d" % (i - 1)) for i in range(cfg.enc_layers)]
+        self.enc = self._enc_stack(names, "encoder.after_norm", cfg.heads, K, cfg.feat_dim)
+        self._init_timestamp_head("predictor.", smooth_factor2, noise_threshold2, cfg.cif_threshold)
+        torch.cuda.current_stream(self.device).synchronize()
+        self._state = None
+
+    def encode(self, feats: torch.Tensor, lens: torch.Tensor) -> torch.Tensor:
+        """SANMEncoder.forward: feats [B,T,560], lens [B] int32 -> [B,T,D]."""
+        return self._encode(self.enc, feats, lens, self.cfg.d_model)
+
 
 class ParaformerEngine(_EngineBase):
     """Packed weights + workspace + the encoder/predictor/decoder ABI calls."""
@@ -219,22 +298,8 @@ class ParaformerEngine(_EngineBase):
         self.pred = _abi.FaPredictor(conv, g(prefix_pred + "cif_output.weight").data_ptr(),
                                      g(prefix_pred + "cif_output.bias").data_ptr(), cfg.cif_threshold,
                                      cfg.tail_threshold, 1.0, 0.0, 1 if bicif else 0, 0)
-        if bicif:   # CifPredictorV3 timestamp head (bicif_paraformer/cif_predictor.py:121-352, upsample_type "cnn_blstm", use_cif1_cnn False)
-            uw = state[prefix_pred + "upsample_cnn.weight"]                      # ConvTranspose1d weight [in, out, k], stride == k == 3
-            self.up_times = int(uw.shape[2])
-            # out[b, 3t+k, o] = sum_c x[b,t,c] w[c,o,k] + bias[o]  ==  one GEMM with W[(k,o), c], rows viewed as [B, 3T, 512]
-            self.up_lin = lin(prefix_pred + "upsample_cnn", weight=self._dev(uw.permute(2, 1, 0).reshape(-1, uw.shape[0])),
-                              bias_tensor=self._dev(state[prefix_pred + "upsample_cnn.bias"].repeat(self.up_times)))
-            # the BLSTM: input projections of both directions as ONE GEMM ([W_ih_fwd; W_ih_bwd], b_ih + b_hh), then the
-            # persistent weight-stationary recurrence fa_blstm_forward_tc
-            bp = prefix_pred + "blstm."
-            w_ih = torch.cat([state[bp + "weight_ih_l0"], state[bp + "weight_ih_l0_reverse"]], 0)
-            b_all = torch.cat([state[bp + "bias_ih_l0"] + state[bp + "bias_hh_l0"],
-                               state[bp + "bias_ih_l0_reverse"] + state[bp + "bias_hh_l0_reverse"]], 0)
-            self.lstm_ih = lin(bp + "ih", weight=self._dev(w_ih), bias_tensor=self._dev(b_all))
-            self.lstm_hh_f, self.lstm_hh_b = g(bp + "weight_hh_l0"), g(bp + "weight_hh_l0_reverse")
-            self.out2_w, self.out2_b = g(prefix_pred + "cif_output2.weight"), g(prefix_pred + "cif_output2.bias")
-            self.smooth2, self.noise2 = float(smooth_factor2), float(noise_threshold2)
+        if bicif:
+            self._init_timestamp_head(prefix_pred, smooth_factor2, noise_threshold2, cfg.cif_threshold)
         # ---- decoder
         def dec_layer(L, p, full=True):
             L.norm1 = norm(p + ".norm1")
@@ -310,45 +375,6 @@ class ParaformerEngine(_EngineBase):
                                                      n_cap, tok.data_ptr(), alphas.data_ptr(), peaks.data_ptr(), self.mode,
                                                      ws.data_ptr(), ws.numel(), self._stream()), "fa_cif_predictor_forward")
         return acoustic, tok, alphas, peaks
-
-    def upsample_timestamp(self, enc: torch.Tensor, lens: torch.Tensor, token_num: torch.Tensor):
-        """CifPredictorV3.get_upsample_timestamp (bicif_paraformer/cif_predictor.py:300-352): enc [B,T,512], lens [B] i32,
-        token_num [B] i32 (rounded) -> (us_alphas [B,3T], us_peaks [B,3T]).  ConvTranspose1d upsampling = one GEMM of this library,
-        the BLSTM = its input projections as one tensor-core GEMM + this library's persistent weight-stationary recurrence
-        (fa_blstm_forward_tc: warp-level mma.sync on bf16 hi/lo planes, not wgmma — the per-step product is only 64x32x512), the
-        alpha head / rescale / fire scan is fa_cif_upsample_alphas."""
-        if not self.bicif:
-            raise _abi.FunasrB200Error("engine was not built with bicif=True")
-        B, T, D = enc.shape
-        U = self.up_times
-        up = torch.empty((B, T * U, D), dtype=torch.float32, device=self.device)
-        ws = self._workspace(max(8 * B * T * U * D * 4, 1 << 20))
-        _abi.check(self.lib.fa_linear(enc.data_ptr(), D, B * T, C.byref(self.up_lin), 0, None, 0, None, 0, up.data_ptr(), U * D, self.mode,
-                                      ws.data_ptr(), ws.numel(), self._stream()), "fa_linear(upsample_cnn)")
-        xproj = torch.empty((B * T * U, 8 * D), dtype=torch.float32, device=self.device)
-        _abi.check(self.lib.fa_linear(up.data_ptr(), D, B * T * U, C.byref(self.lstm_ih), 0, None, 0, None, 0, xproj.data_ptr(), 8 * D,
-                                      self.mode, ws.data_ptr(), ws.numel(), self._stream()), "fa_linear(blstm input projections)")
-        feat = torch.empty((B, T * U, 2 * D), dtype=torch.float32, device=self.device)
-        # the recurrence kernel holds at most 256 sequences per launch: larger batches run as consecutive launches (sequences
-        # are independent) — never a library fallback
-        for b0 in range(0, B, 256):
-            bn = min(256, B - b0)
-            xp = xproj.data_ptr() + b0 * T * U * 8 * D * 4
-            fp = feat.data_ptr() + b0 * T * U * 2 * D * 4
-            nb = int(self.lib.fa_blstm_tc_scratch_bytes(bn))
-            if getattr(self, "_lstm_scratch", None) is None or self._lstm_scratch.numel() < nb:
-                self._lstm_scratch = torch.empty(nb, dtype=torch.uint8, device=self.device)
-            _abi.check(self.lib.fa_blstm_forward_tc(xp, self.lstm_hh_f.data_ptr(), self.lstm_hh_b.data_ptr(), bn, T * U, D,
-                                                    fp, self._lstm_scratch.data_ptr(), self._lstm_scratch.numel(),
-                                                    self._stream()), "fa_blstm_forward_tc")
-        us_alphas = torch.empty((B, T * U), dtype=torch.float32, device=self.device)
-        us_peaks = torch.empty_like(us_alphas)
-        lens_up = (lens.to(torch.int32) * U).contiguous()
-        tok = token_num.to(self.device, torch.int32).contiguous()
-        _abi.check(self.lib.fa_cif_upsample_alphas(feat.data_ptr(), 2 * D, self.out2_w.data_ptr(), self.out2_b.data_ptr(), lens_up.data_ptr(),
-                                                   tok.data_ptr(), B, T * U, self.smooth2, self.noise2, self.cfg.cif_threshold,
-                                                   us_alphas.data_ptr(), us_peaks.data_ptr(), self._stream()), "fa_cif_upsample_alphas")
-        return us_alphas, us_peaks
 
     def set_hotwords(self, hw_embed: torch.Tensor):
         """Hotword memory [Nhw, 512] (LSTM last hidden states) for the contextual bias decoder."""

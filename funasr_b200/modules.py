@@ -23,7 +23,7 @@ import torch
 import torch.nn as nn
 
 from . import _abi
-from .engine import FrontendEngine, ParaformerEngine, SenseVoiceEngine, num_lfr_frames
+from .engine import AlignerEngine, FrontendEngine, ParaformerEngine, SenseVoiceEngine, num_lfr_frames
 from .hotwords import generate_hotwords_list
 from .registry import get_tables, register
 from .synth import ParaformerConfig, SenseVoiceConfig
@@ -128,11 +128,11 @@ class SANMEncoderB200(_ParamHolder):
         super().__init__()
         head_dim = output_size // attention_heads if attention_heads else 0
         if (input_layer, normalize_before, selfattention_layer_type, sanm_shfit) != ("pe", True, "sanm", 0) or input_size > 560 or \
-                output_size % 16 or output_size > 512 or head_dim * attention_heads != output_size or head_dim not in (32, 64, 96, 128) or \
+                output_size % 16 or output_size > 512 or head_dim * attention_heads != output_size or head_dim not in (32, 64, 80, 96, 128) or \
                 linear_units > 2048 or input_size % 16:
             raise _abi.FunasrB200Error("SANMEncoderB200 supports input_layer='pe', sanm, normalize_before, d <= 512 (head dim 32..128), "
-                                       "linear_units <= 2048 — d=512 / 4 heads runs on the tensor cores (Paraformer, SenseVoice), other "
-                                       "shapes (CT-Transformer: d=256 / 8 heads) on the fp32 path")
+                                       "linear_units <= 2048 — d=512 / 4 heads (Paraformer, SenseVoice) and d=320 / 4 heads (fa-zh) run "
+                                       "on the tensor cores, other shapes (CT-Transformer: d=256 / 8 heads) on the fp32 path")
         self.input_size, self._output_size = input_size, output_size
         self.heads, self.ffn, self.num_blocks, self.kernel_size = attention_heads, linear_units, num_blocks, kernel_size
         self._build()
@@ -190,8 +190,8 @@ class CifPredictorV3B200(_ParamHolder):
     def __init__(self, idim, l_order, r_order, threshold=1.0, dropout=0.1, smooth_factor=1.0, noise_threshold=0, tail_threshold=0.0,
                  smooth_factor2=1.0, noise_threshold2=0, upsample_times=5, upsample_type="cnn", use_cif1_cnn=True, tail_mask=True, **kwargs):
         super().__init__()
-        if (idim, l_order, r_order, smooth_factor, noise_threshold, tail_mask) != (512, 1, 1, 1.0, 0, True) or tail_threshold <= 0:
-            raise _abi.FunasrB200Error("CifPredictorV3B200 supports idim=512, l_order=r_order=1, tail_threshold>0, tail_mask")
+        if idim not in (512, 320) or (l_order, r_order, smooth_factor, noise_threshold, tail_mask) != (1, 1, 1.0, 0, True) or tail_threshold <= 0:
+            raise _abi.FunasrB200Error("CifPredictorV3B200 supports idim=512 or 320, l_order=r_order=1, tail_threshold>0, tail_mask")
         if upsample_type != "cnn_blstm" or use_cif1_cnn or upsample_times != 3:
             raise _abi.FunasrB200Error("CifPredictorV3B200 supports upsample_type='cnn_blstm', use_cif1_cnn=False, upsample_times=3")
         self.idim, self.threshold, self.tail_threshold = idim, threshold, tail_threshold
@@ -693,6 +693,118 @@ class BiCifParaformerB200(ParaformerB200):
                     pass
             r["timestamp"] = stamp
         self._last_out = None
+        return results, meta_data
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# MonotonicAligner (fa-zh): timestamps for a transcript the caller already has
+# ------------------------------------------------------------------------------------------------------------------
+def _aligner_tokens(text, tokenizer) -> List[int]:
+    """One transcript as token ids, the way load_audio_text_image_video (load_utils.py:144-146, :148-149) reads data_type "text":
+    a path to an existing text file is read and encoded, any other string is encoded, a sequence of ids is taken as is."""
+    import os
+    if isinstance(text, str):
+        if tokenizer is None:
+            raise _abi.FunasrB200Error("MonotonicAlignerB200 needs a tokenizer to encode a text transcript")
+        if os.path.exists(text):
+            with open(text, "r") as f:
+                text = f.read().strip()
+        return [int(t) for t in tokenizer.encode(text)]
+    if torch.is_tensor(text) or isinstance(text, np.ndarray):
+        text = text.tolist()
+    return [int(t) for t in text]
+
+
+@register("model_classes", "MonotonicAlignerB200")
+class MonotonicAlignerB200(nn.Module):
+    """Drop-in for funasr.models.monotonic_aligner.model.MonotonicAligner.inference (model.py:182-267): given (audio, transcript)
+    pairs, the SAN-M encoder and CifPredictorV3's upsampled timestamp head give [start_ms, end_ms] per transcript character."""
+
+    def __init__(self, input_size: int = 80, specaug=None, specaug_conf=None, normalize=None, normalize_conf=None, encoder: str = None,
+                 encoder_conf: dict = None, predictor: str = None, predictor_conf: dict = None, predictor_bias: int = 0,
+                 length_normalized_loss: bool = False, gemm_mode: str = "fp32", **kwargs):
+        super().__init__()
+        # specaug, predictor_bias and length_normalized_loss only act in training (model.py:100-146)
+        tables = get_tables()
+        enc_cls = tables.encoder_classes.get(encoder) if isinstance(encoder, str) else encoder
+        pred_cls = tables.predictor_classes.get(predictor) if isinstance(predictor, str) else predictor
+        enc_cls = enc_cls if (enc_cls is not None and issubclass(enc_cls, _ParamHolder)) else SANMEncoderB200
+        pred_cls = pred_cls if (pred_cls is not None and issubclass(pred_cls, _ParamHolder)) else CifPredictorV3B200
+        self.encoder = enc_cls(input_size=input_size, **(encoder_conf or {}))
+        self.predictor = pred_cls(**(predictor_conf or {}))
+        if self.predictor.idim != self.encoder.output_size():
+            raise _abi.FunasrB200Error("MonotonicAlignerB200: predictor idim %d != encoder output size %d"
+                                       % (self.predictor.idim, self.encoder.output_size()))
+        self.predictor_bias = predictor_bias
+        self.gemm_mode = gemm_mode
+        self.cfg = ParaformerConfig(d_model=self.encoder.output_size(), heads=self.encoder.heads, ffn=self.encoder.ffn,
+                                    enc_layers=self.encoder.num_blocks, dec_layers=0, kernel=self.encoder.kernel_size,
+                                    tail_threshold=self.predictor.tail_threshold, cif_threshold=self.predictor.threshold)
+        self._engine: Optional[AlignerEngine] = None
+
+    def on_pretrained_model_loaded(self, loaded_keys=None):
+        self._engine = None
+
+    def _apply(self, fn, *a, **k):
+        self._engine = None
+        return super()._apply(fn, *a, **k)
+
+    def engine(self, device=None) -> AlignerEngine:
+        dev = torch.device(device) if device is not None else next(self.parameters()).device
+        if dev.type != "cuda":
+            raise _abi.FunasrB200Error("MonotonicAlignerB200 needs a CUDA device (got %s); there is no CPU path" % dev)
+        if self._engine is None or self._engine.device != dev:
+            self._engine = AlignerEngine(self.state_dict(), self.cfg, dev, gemm_mode=self.gemm_mode,
+                                         smooth_factor2=self.predictor.smooth_factor2, noise_threshold2=self.predictor.noise_threshold2)
+        return self._engine
+
+    def encode(self, speech: torch.Tensor, speech_lengths: torch.Tensor, **kwargs):
+        eng = self.engine(speech.device)
+        lens = speech_lengths.to(speech.device, torch.int32)
+        return eng.encode(speech.contiguous(), lens), lens
+
+    def calc_predictor_timestamp(self, encoder_out, encoder_out_lens, token_num):
+        """model.py:156-168 -> (ds_alphas=None, ds_cif_peak=None, us_alphas, us_peaks)."""
+        us_alphas, us_peaks = self.engine(encoder_out.device).upsample_timestamp(encoder_out, encoder_out_lens.to(torch.int32), token_num)
+        return None, None, us_alphas, us_peaks
+
+    def inference(self, data_in, data_lengths=None, key: list = None, tokenizer=None, frontend=None, **kwargs):
+        """Same contract as MonotonicAligner.inference: data_in is one (audio, text) pair or a list of them, data_type
+        ("sound", "text"); returns ([{"key", "text", "timestamp"}, ...], meta_data)."""
+        from .timestamps import ts_prediction_lfr6_standard
+        device = torch.device(kwargs.get("device", "cuda"))
+        if device.type != "cuda":
+            raise _abi.FunasrB200Error("MonotonicAlignerB200.inference needs device='cuda' (no CPU fallback)")
+        data_type = kwargs.get("data_type", ("sound", "text"))
+        if tuple(data_type) != ("sound", "text"):
+            raise _abi.FunasrB200Error("MonotonicAlignerB200 takes data_type=('sound', 'text') (audio, transcript) pairs")
+        pairs = [data_in] if (isinstance(data_in, tuple) and len(data_in) == 2) else list(data_in)
+        token_lists = [_aligner_tokens(t, tokenizer) for _, t in pairs]
+        kw = {k: v for k, v in kwargs.items() if k != "data_type"}
+        meta_data = {}
+        eng = self.engine(device)
+        speech, lens = ParaformerB200._features(self, [a for a, _ in pairs], data_lengths, frontend, device, kw, meta_data)
+        enc = eng.encode(speech, lens)
+        text_lengths = torch.tensor([len(t) + 1 for t in token_lists], dtype=torch.int32)          # model.py:226-228
+        us_alphas, us_peaks = eng.upsample_timestamp(enc, lens, text_lengths)
+        ua, up, elens = us_alphas.cpu().numpy(), us_peaks.cpu().numpy(), lens.cpu().tolist()
+        b = len(pairs)
+        if key is None:
+            key = ["utt%d" % i for i in range(b)]
+        if isinstance(key[0], (list, tuple)):
+            key = key[0]
+        results = []
+        for i, token_int in enumerate(token_lists):
+            token = tokenizer.ids2tokens(token_int) if tokenizer is not None else [str(t) for t in token_int]
+            n = int(elens[i]) * eng.up_times
+            _, stamp = ts_prediction_lfr6_standard(ua[i][:n], up[i][:n], list(token), want_text=False)       # model.py:243-247
+            text = tokenizer.tokens2text(token) if tokenizer is not None else " ".join(token)
+            try:
+                from funasr.utils import postprocess_utils
+                text, stamp, _ = postprocess_utils.sentence_postprocess(token, stamp)                        # model.py:248-250
+            except ImportError:
+                pass
+            results.append({"key": key[i], "text": text, "timestamp": stamp})
         return results, meta_data
 
 

@@ -78,6 +78,7 @@ DROP_IN_KEYS = {
     ("encoder_classes", "SenseVoiceEncoderSmall"): "SenseVoiceEncoderSmallB200",
     ("decoder_classes", "ParaformerSANMDecoder"): "ParaformerSANMDecoderB200",
     ("model_classes", "CAMPPlus"): "CAMPPlusB200",
+    ("model_classes", "MonotonicAligner"): "MonotonicAlignerB200",
 }
 
 

@@ -160,6 +160,52 @@ def make_bicif_state_dict(cfg: ParaformerConfig = PARAFORMER_LARGE, seed: int = 
     return sd
 
 
+
+# MonotonicAligner fa-zh (monotonic_aligner/template.yaml): SAN-M encoder d = 320, 4 x 80 heads, FFN 1280, 30 blocks, CifPredictorV3
+# idim 320 (BLSTM hidden 320).  vocab only sizes the unused decoder-side tensors make_state_dict also draws.
+ALIGNER_FA_ZH = ParaformerConfig(d_model=320, heads=4, ffn=1280, enc_layers=30, dec_layers=1, kernel=11, vocab=64)
+ALIGNER_TINY = ParaformerConfig(d_model=320, heads=4, ffn=1280, enc_layers=3, dec_layers=1, kernel=11, vocab=64)
+
+
+def aligner_token_list(n_chars: int = 400):
+    """CharTokenizer token list of the synthetic aligner: <blank> <s> </s>, n_chars CJK characters, <unk>."""
+    return ["<blank>", "<s>", "</s>"] + [chr(0x4E00 + i) for i in range(n_chars)] + ["<unk>"]
+
+
+def make_aligner_state_dict(cfg: ParaformerConfig = ALIGNER_FA_ZH, seed: int = 0) -> "OrderedDict[str, torch.Tensor]":
+    """MonotonicAligner (funasr/models/monotonic_aligner/model.py): `encoder.*` and CifPredictorV3's `predictor.*` — cif_conv1d /
+    cif_output (loaded, unused at inference) plus the timestamp head.  The timestamp head's gains make the upsampled CIF weights
+    follow the audio (their spread across frames is several times their mean), so speech and pauses produce uneven stamps;
+    with untuned random weights the weights come out near-constant and the stamps evenly spaced."""
+    base = make_state_dict(cfg, seed)
+    sd: "OrderedDict[str, torch.Tensor]" = OrderedDict((k, v) for k, v in base.items() if k.startswith(("encoder.", "predictor.")))
+    g = torch.Generator().manual_seed(1000003 * seed + 91)
+    D = cfg.d_model
+    sd["predictor.upsample_cnn.weight"] = _randn(g, D, D, 3, std=1.0 / math.sqrt(D))
+    sd["predictor.upsample_cnn.bias"] = _randn(g, D, std=0.05)
+    for suf in ("", "_reverse"):
+        sd["predictor.blstm.weight_ih_l0" + suf] = _randn(g, 4 * D, D, std=1.5 / math.sqrt(D))
+        sd["predictor.blstm.weight_hh_l0" + suf] = _randn(g, 4 * D, D, std=1.0 / math.sqrt(D))
+        sd["predictor.blstm.bias_ih_l0" + suf] = _randn(g, 4 * D, std=0.05)
+        sd["predictor.blstm.bias_hh_l0" + suf] = _randn(g, 4 * D, std=0.05)
+    sd["predictor.cif_output2.weight"] = _randn(g, 1, 2 * D, std=8.0 / math.sqrt(2 * D))
+    sd["predictor.cif_output2.bias"] = torch.full((1,), -1.0)
+    return sd
+
+
+def make_aligner_wav(seconds: float, seed: int = 0) -> torch.Tensor:
+    """Speech-like stretches (0.6-2.0 s) separated by quiet pauses (0.2-0.8 s), 16 kHz: the aligner's stamps then have gaps."""
+    g = torch.Generator().manual_seed(7727 * seed + 3)
+    n, parts, k = int(seconds * 16000), [], 0
+    while sum(p.numel() for p in parts) < n:
+        m = int(16000 * (0.6 + 1.4 * float(torch.rand(1, generator=g))))
+        parts.append(make_wav(m, 100 * seed + k))
+        q = int(16000 * (0.2 + 0.6 * float(torch.rand(1, generator=g))))
+        parts.append(0.01 * make_wav(q, 100 * seed + k + 50, "noise"))
+        k += 1
+    return torch.cat(parts)[:n].contiguous()
+
+
 SEACO_FFN, SEACO_KERNEL, SEACO_LAYERS = 1024, 21, 6      # seaco_paraformer/template.yaml:57-69 (num_blocks 4 < att_layer_num 6 -> 6 layers)
 
 

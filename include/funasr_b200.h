@@ -268,9 +268,14 @@ int fa_attention_tc(const float* q, int64_t ldq, const float* k, int64_t ldk, co
 int fa_attention_tc_planes(const void* q_planes, const void* k_planes, const void* vt_planes, const int32_t* key_lens, int32_t batch,
                            int32_t heads, int32_t tq, int32_t tk, float* ctx, int64_t ld_ctx, void* ctx_planes, int64_t ld_planes,
                            int32_t out_nplanes, int32_t gemm_mode, int32_t kv_shared, fa_stream_t stream);
+/* fa_attention_tc_planes with an explicit head_dim: 128 (the call above) or 80 (the fa-zh aligner, 4 x 80); every 128 of that
+ * contract reads head_dim.  Any other head_dim returns FA_ERR_UNSUPPORTED. */
+int fa_attention_tc_planes_ex(const void* q_planes, const void* k_planes, const void* vt_planes, const int32_t* key_lens, int32_t batch,
+                              int32_t heads, int32_t head_dim, int32_t tq, int32_t tk, float* ctx, int64_t ld_ctx, void* ctx_planes,
+                              int64_t ld_planes, int32_t out_nplanes, int32_t gemm_mode, int32_t kv_shared, fa_stream_t stream);
 /* fp32 attention with the fp32 path's kernel choice: head_dim 128 -> the tiled kernel of fa_attention, any other multiple of 32 up
- * to 128 -> the warp-per-query kernel (CT-Transformer's 8 x 32 heads; FA_ERR_UNSUPPORTED when 4 * tk floats exceed its 160 KB of
- * shared memory).  kv_shared != 0: k / v hold one batch entry [tk, ld] that every utterance attends over. */
+ * to 128, or 80 -> the warp-per-query kernel (CT-Transformer's 8 x 32 heads, the aligner's 4 x 80; FA_ERR_UNSUPPORTED when 4 * tk
+ * floats exceed its 160 KB of shared memory).  kv_shared != 0: k / v hold one batch entry [tk, ld] that every utterance attends over. */
 int fa_attention_f32_ex(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
                         const int32_t* key_lens, int32_t batch, int32_t heads, int32_t head_dim, int32_t tq, int32_t tk,
                         float* ctx, int64_t ld_ctx, int32_t kv_shared, fa_stream_t stream);
@@ -312,12 +317,12 @@ int fa_cif_upsample_alphas(const float* feat, int32_t dz, const float* w, const 
                            const int32_t* token_num, int32_t batch, int32_t t_up, float smooth2, float noise2,
                            float threshold, float* us_alphas, float* us_peaks, fa_stream_t stream);
 
-/* One-layer bidirectional LSTM recurrence (torch.nn.LSTM(512, 512, 1, batch_first=True, bidirectional=True), the `blstm` of
+/* One-layer bidirectional LSTM recurrence (torch.nn.LSTM(H, H, 1, batch_first=True, bidirectional=True), the `blstm` of
  * CifPredictorV3, bicif_paraformer/cif_predictor.py:187-190) as a persistent weight-stationary kernel: the per-step
- * [B,512] x [512,2048] product on warp-level bf16 MMAs with the 3-product operand split (fp32 accumulate), h exchanged between
+ * [B,H] x [H,4H] product on warp-level bf16 MMAs with the 3-product operand split (fp32 accumulate), h exchanged between
  * CTAs as bf16 hi / lo planes.  The caller supplies the input projections of ALL steps (one fa_linear):
- * xproj [B*T, 4096] = x [W_ih_fwd; W_ih_bwd]^T + (b_ih + b_hh), gate order i,f,g,o per direction.  w_hh_* [2048, 512].
- * out [B, T, 1024] (forward | reverse).  batch <= 256, hidden == 512.
+ * xproj [B*T, 8H] = x [W_ih_fwd; W_ih_bwd]^T + (b_ih + b_hh), gate order i,f,g,o per direction.  w_hh_* [4H, H].
+ * out [B, T, 2H] (forward | reverse).  batch <= 256, hidden H == 512 or 320 (else FA_ERR_UNSUPPORTED).
  * scratch >= fa_blstm_tc_scratch_bytes(batch) bytes of device memory (zeroed by the call). */
 size_t fa_blstm_tc_scratch_bytes(int32_t batch);
 int fa_blstm_forward_tc(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, int32_t batch, int32_t t_len,
