@@ -111,6 +111,7 @@ SIGNATURES = {
     "fa_ctc_greedy_forward": (C.c_int, [C.POINTER(FaLinear), _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _sz, _vp]),
     "fa_layernorm": (C.c_int, [_vp, _i64, C.POINTER(FaNorm), _vp, _vp, _f, _i32, _vp]),
     "fa_linear": (C.c_int, [_vp, _i64, _i64, C.POINTER(FaLinear), _i32, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _vp, _sz, _vp]),
+    "fa_linear_workspace_bytes": (_sz, [_i64, _i32, _i32]),
     "fa_split_rows": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _i32, _vp, _vp]),
     "fa_linear_planes": (C.c_int, [_vp, _i64, C.POINTER(FaLinear), _i32, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _vp]),
     "fa_linear_planes_to_planes": (C.c_int, [_vp, _i64, C.POINTER(FaLinear), _i32, _vp, _i64, _i32, _vp]),

@@ -291,17 +291,25 @@ scale_split_kernel(const float* __restrict__ src, int64_t ld, int64_t rows, int 
   }
 }
 
-// exactly what attention_tc_launch takes from its scratch arena (the same Arena::take sequence; a shared K/V takes less)
-size_t attention_tc_scratch_bytes(int batch, int heads, int tq, int tk, int mode) {
-  if (mode == FA_GEMM_F32_SIMT) return 0;
-  const int npl = mode == FA_GEMM_F16X1 ? 1 : 2;
-  const int tkp = (tk + 63) / 64 * 64;
+// attention_tc_launch's scratch: q (scaled) / k planes and v planes transposed per head; a shared K / V is one batch entry
+struct AttnOperands { plane_t *qp, *kp, *vt; };
+static AttnOperands attn_carve(Arena& a, int batch, int heads, int tq, int tk, int mode, int kv_shared) {
+  const int npl = attn_planes(mode);
   const int d = heads * AT_D;
-  ArenaSizer s;
-  s.take((size_t)npl * batch * tq * d * sizeof(plane_t));
-  s.take((size_t)npl * batch * tk * d * sizeof(plane_t));
-  s.take((size_t)npl * batch * d * tkp * sizeof(plane_t));
-  return s.off;
+  const int tkp = (tk + 63) / 64 * 64;
+  const int kvb = kv_shared ? 1 : batch;
+  AttnOperands o;
+  o.qp = a.take<plane_t>((size_t)npl * batch * tq * d);
+  o.kp = a.take<plane_t>((size_t)npl * kvb * tk * d);
+  o.vt = a.take<plane_t>((size_t)npl * kvb * d * tkp);
+  return o;
+}
+
+size_t attention_tc_scratch_bytes(int batch, int heads, int tq, int tk, int mode, int kv_shared) {
+  if (mode == FA_GEMM_F32_SIMT) return 0;
+  Arena m = Arena::measuring();
+  attn_carve(m, batch, heads, tq, tk, mode, kv_shared);
+  return m.bytes();
 }
 
 int attention_tc_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
@@ -310,16 +318,15 @@ int attention_tc_launch(const float* q, int64_t ldq, const float* k, int64_t ldk
   if (batch <= 0 || tq <= 0) return FA_OK;
   if (!q || !k || !v || !key_lens || tk <= 0 || !scratch) return FA_ERR_ARG;
   if ((ldq | ldk | ldv) & 3) return FA_ERR_UNSUPPORTED;
-  const int npl = mode == FA_GEMM_F16X1 ? 1 : 2;
+  const int npl = attn_planes(mode);
   const int d = heads * AT_D;
   const int tkp = (tk + 63) / 64 * 64;
   const int kvb = kv_shared ? 1 : batch;
   const int64_t mq = (int64_t)batch * tq, mk = (int64_t)kvb * tk, mv = (int64_t)kvb * d;
   Arena local(scratch->base, scratch->cap);
-  plane_t* qp = local.take<plane_t>((size_t)npl * mq * d);
-  plane_t* kp = local.take<plane_t>((size_t)npl * mk * d);
-  plane_t* vt = local.take<plane_t>((size_t)npl * mv * tkp);
+  const AttnOperands o = attn_carve(local, batch, heads, tq, tk, mode, kv_shared);
   if (!local.ok()) return FA_ERR_WORKSPACE;
+  plane_t *qp = o.qp, *kp = o.kp, *vt = o.vt;
   const float qscale = (float)(1.0 / sqrt((double)AT_D));
   {
     const int64_t tot = mq * (d / 4);
@@ -366,7 +373,7 @@ int attention_tc_planes_launch(const plane_t* qp, const plane_t* kp, const plane
   if (head_dim != 128 && head_dim != 80) return FA_ERR_UNSUPPORTED;
   if (batch <= 0 || tq <= 0) return FA_OK;
   if (!qp || !kp || !vt || !key_lens || tk <= 0) return FA_ERR_ARG;
-  const int npl = mode == FA_GEMM_F16X1 ? 1 : 2;
+  const int npl = attn_planes(mode);
   const int d = heads * head_dim;
   const int tkp = (tk + 63) / 64 * 64;
   const int kvb = kv_shared ? 1 : batch;
@@ -396,7 +403,7 @@ int attention_tc_planes_launch(const plane_t* qp, const plane_t* kp, const plane
 
 
 extern "C" size_t fa_attention_tc_workspace_bytes(int32_t batch, int32_t heads, int32_t tq, int32_t tk, int32_t gemm_mode) {
-  return fa::attention_tc_scratch_bytes(batch, heads, tq, tk, gemm_mode);
+  return fa::attention_tc_scratch_bytes(batch, heads, tq, tk, gemm_mode, 0);
 }
 
 extern "C" int fa_attention_tc(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,

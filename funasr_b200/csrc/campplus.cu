@@ -354,8 +354,6 @@ static int stats_launch(const float* x, int batch, int T, int C, const float* sc
   return FA_OK;
 }
 
-static inline int cam_npl(int mode) { return mode == FA_GEMM_F16X1 ? 1 : (mode == FA_GEMM_F16X3 ? 2 : 3); }
-
 // Shapes of one forward: T feature frames -> t_out = ceil(T / 2) TDNN frames; P = padded TDNN input rows per chunk (even).
 struct CamShapes {
   int B, T, t_out, P, nseg;
@@ -382,33 +380,27 @@ struct CamBufs {
   size_t scratch_bytes;
 };
 
-template <typename A>
-static void cam_carve(A& a, const CamShapes& s, int mode, CamBufs* out) {
+static void cam_carve(Arena& a, const CamShapes& s, int mode, CamBufs* out) {
   const int64_t BT = (int64_t)s.B * s.T;
   const bool tc = mode != FA_GEMM_F32_SIMT;
-  const int npl = tc ? cam_npl(mode) : 0;
+  const int npl = gemm_planes(mode);
   const int cmax = s.c_final[1] > s.c_final[2] ? s.c_final[1] : s.c_final[2];
-  out->x80 = a.template take<float>(BT * 80 * 32);
-  out->x40a = a.template take<float>(BT * 40 * 32);
-  out->x40b = a.template take<float>(BT * 40 * 32);
-  out->x40c = a.template take<float>(BT * 40 * 32);
-  out->pad = a.template take<float>(s.pad_rows * 320);
-  out->tdnn = a.template take<float>((int64_t)s.B * (s.P / 2) * kCamBn);
-  for (int i = 0; i < 3; ++i) out->buf[i] = a.template take<float>(s.rows * s.c_final[i]);
-  out->h = a.template take<float>(s.rows * kCamBn);
-  out->gates = a.template take<float>((int64_t)s.B * s.nseg * kCamOut);
-  out->stats = a.template take<float>((int64_t)s.B * 1024);
-  out->op = tc ? nullptr : a.template take<float>(s.rows * cmax);
-  out->pad_planes = tc ? a.template take<plane_t>((size_t)npl * s.pad_rows * 320) : nullptr;
-  out->op_planes = tc ? a.template take<plane_t>((size_t)npl * s.rows * ((cmax + 63) / 64 * 64)) : nullptr;
+  out->x80 = a.take<float>(BT * 80 * 32);
+  out->x40a = a.take<float>(BT * 40 * 32);
+  out->x40b = a.take<float>(BT * 40 * 32);
+  out->x40c = a.take<float>(BT * 40 * 32);
+  out->pad = a.take<float>(s.pad_rows * 320);
+  out->tdnn = a.take<float>((int64_t)s.B * (s.P / 2) * kCamBn);
+  for (int i = 0; i < 3; ++i) out->buf[i] = a.take<float>(s.rows * s.c_final[i]);
+  out->h = a.take<float>(s.rows * kCamBn);
+  out->gates = a.take<float>((int64_t)s.B * s.nseg * kCamOut);
+  out->stats = a.take<float>((int64_t)s.B * 1024);
+  out->op = tc ? nullptr : a.take<float>(s.rows * cmax);
+  out->pad_planes = tc ? a.take<plane_t>((size_t)npl * s.pad_rows * 320) : nullptr;
+  out->op_planes = tc ? a.take<plane_t>((size_t)npl * s.rows * ((cmax + 63) / 64 * 64)) : nullptr;
   out->scratch_bytes = tc ? gemm_tc_scratch_bytes(s.B, 1024, mode) : 0;
-  out->scratch = tc ? a.template take<char>(out->scratch_bytes) : nullptr;
+  out->scratch = tc ? a.take<char>(out->scratch_bytes) : nullptr;
 }
-
-struct SizeArena {   // Arena-shaped byte counter
-  size_t off = 0;
-  template <typename T> T* take(size_t n) { off = align_up(off, 256) + n * sizeof(T); return reinterpret_cast<T*>(256); }
-};
 
 // y[rows, out_f] (ldy) = act(A W^T + b) with A = relu(x[:, :in_f] * scale + shift) (fp32 rows or fp16 planes)
 static int bn_relu_linear(const float* x, int64_t ldx, int64_t rows, const float* scale, const float* shift, const FaLinear& lin,
@@ -417,7 +409,7 @@ static int bn_relu_linear(const float* x, int64_t ldx, int64_t rows, const float
     FA_RETURN_IF_ERR(bn_relu_launch(x, ldx, rows, lin.in_f, lin.in_f, scale, shift, bf.op, nullptr, 0, st));
     return gemm_f32_launch(bf.op, lin.in_f, rows, lin.w, lin.out_f, lin.in_f, lin.b, relu, nullptr, 0, nullptr, 0, y, ldy, st);
   }
-  FA_RETURN_IF_ERR(bn_relu_launch(x, ldx, rows, lin.in_f, lin.in_pad, scale, shift, nullptr, bf.op_planes, cam_npl(mode), st));
+  FA_RETURN_IF_ERR(bn_relu_launch(x, ldx, rows, lin.in_f, lin.in_pad, scale, shift, nullptr, bf.op_planes, gemm_planes(mode), st));
   return gemm_tc_planes_launch(bf.op_planes, rows, lin, relu, nullptr, 0, nullptr, 0, y, ldy, nullptr, 0, mode, st);
 }
 
@@ -461,7 +453,7 @@ static int campplus_forward(const FaCampplus* m, const float* feats, int batch, 
   if (!tc) {
     FA_RETURN_IF_ERR(gemm_f32_launch(bf.pad, 640, Mt, m->tdnn.w, kCamBn, 1600, m->tdnn.b, 1, nullptr, 0, nullptr, 0, bf.tdnn, kCamBn, st));
   } else {
-    FA_RETURN_IF_ERR(split_rows_launch(bf.pad, 320, s.pad_rows, 320, 320, cam_npl(mode), bf.pad_planes, st));
+    FA_RETURN_IF_ERR(split_rows_launch(bf.pad, 320, s.pad_rows, 320, 320, gemm_planes(mode), bf.pad_planes, st));
     FA_RETURN_IF_ERR(gemm_tc_planes_launch(bf.pad_planes, Mt, m->tdnn, 1, nullptr, 0, nullptr, 0, bf.tdnn, kCamBn, nullptr, 0, mode, st,
                                            nullptr, 640, s.pad_rows / 2));
   }
@@ -516,10 +508,10 @@ extern "C" int fa_campplus_features(const float* wav, const int32_t* wav_lens, i
 extern "C" size_t fa_campplus_workspace_bytes(const FaCampplus* model, int32_t batch, int32_t t, int32_t gemm_mode) {
   CamShapes s;
   if (!cam_shapes(model, batch, t, &s)) return 0;
-  SizeArena a;
+  Arena m = Arena::measuring();
   CamBufs bf;
-  cam_carve(a, s, gemm_mode, &bf);
-  return a.off + 256;
+  cam_carve(m, s, gemm_mode, &bf);
+  return m.bytes();
 }
 
 extern "C" int fa_campplus_forward(const FaCampplus* model, const float* feats, int32_t batch, int32_t t, float* emb, int32_t gemm_mode,

@@ -71,25 +71,31 @@ inline int sm_count() {
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// Bump allocator over the caller's workspace.
+// fp16 planes of a GEMM operand (the x1 / x3 / x6 splits), and of an attention operand (the kernel reads at most two)
+static inline int gemm_planes(int mode) { return mode == FA_GEMM_F16X1 ? 1 : (mode == FA_GEMM_F16X3 ? 2 : 3); }
+static inline int attn_planes(int mode) { return mode == FA_GEMM_F16X1 ? 1 : 2; }
+
+// Bump allocator over the caller's workspace.  Arena::measuring() runs the same carve without memory: every take succeeds and
+// returns a dummy non-null pointer, and bytes() is the workspace size the carve needs — what the *_workspace_bytes queries return.
 struct Arena {
   char* base;
   size_t cap, off;
+  bool measure = false;
   Arena(void* p, size_t bytes) : base(static_cast<char*>(p)), cap(bytes), off(0) {}
+  static Arena measuring() { Arena a(nullptr, SIZE_MAX); a.measure = true; return a; }
   template <typename T>
   T* take(size_t n) {
     size_t o = align_up(off, 256);
     size_t need = n * sizeof(T);
+    if (measure) { off = o + need; return reinterpret_cast<T*>(uintptr_t(256)); }
     if (base == nullptr || o + need > cap) { off = cap + 1; return nullptr; }
     off = o + need;
     return reinterpret_cast<T*>(base + o);
   }
+  // the next n bytes as an arena of their own: a callee's scratch, which it carves again on every call
+  Arena sub(size_t n) { char* p = take<char>(n); return Arena(p, p ? n : 0); }
   bool ok() const { return off <= cap; }
-};
-// Same arithmetic as Arena::take, for the *_workspace_bytes queries.
-struct ArenaSizer {
-  size_t off = 0;
-  void take(size_t bytes) { off = align_up(off, 256) + bytes; }
+  size_t bytes() const { return off; }
 };
 
 }  // namespace fa

@@ -655,12 +655,15 @@ int make_plane_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t col
   return FA_OK;
 }
 
-static int planes_for_mode(int mode) { return mode == FA_GEMM_F16X1 ? 1 : (mode == FA_GEMM_F16X3 ? 2 : 3); }
+// gemm_tc_launch's scratch: the fp16 planes of the fp32 A operand (none on the fp32 SIMT path, which takes no scratch)
+static plane_t* gemm_carve(Arena& a, int64_t rows, int k_pad, int mode) {
+  return mode == FA_GEMM_F32_SIMT ? nullptr : a.take<plane_t>((size_t)gemm_planes(mode) * rows * k_pad);
+}
 
 size_t gemm_tc_scratch_bytes(int64_t max_rows, int max_k, int mode) {
-  if (mode == FA_GEMM_F32_SIMT) return 0;
-  const int kp = (max_k + 63) / 64 * 64;
-  return (size_t)planes_for_mode(mode) * (size_t)max_rows * kp * 2 + 1024;
+  Arena m = Arena::measuring();
+  gemm_carve(m, max_rows, (max_k + 63) / 64 * 64, mode);
+  return m.bytes();
 }
 
 template <int BN, int STAGES, int APL, int WPL, int EPI>
@@ -708,7 +711,7 @@ int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& li
   if ((lin.b && (((uintptr_t)lin.b) & 15)) || (r1 && (((uintptr_t)r1) & 15)) || (r2 && (((uintptr_t)r2) & 15))) return FA_ERR_UNSUPPORTED;
   if (out_planes && ((ldo & 3) || (((uintptr_t)out_planes) & 7))) return FA_ERR_UNSUPPORTED;
   if ((y && ldy < N) || (r1 && ld1 < N) || (r2 && ld2 < N) || (out_planes && ldo < N)) return FA_ERR_ARG;
-  const int npl = planes_for_mode(mode);
+  const int npl = gemm_planes(mode);
   // 128 x 128 tiles with a 6 (x1) / 3 (x3) stage ring; 128 x 64 for x6 (three planes per operand: two 72 KB stages, a third does
   // not fit beside the epilogue staging in 227 KB).
   // Ragged N (the vocabulary projections: 8404, 25055): the last column tile's W box reaches past row N of a plane — into the next
@@ -751,11 +754,10 @@ int gemm_tc_launch(const float* x, int64_t ldx, int64_t rows, const FaLinear& li
   if (rows <= 0) return FA_OK;
   if (mode != FA_GEMM_F16X1 && mode != FA_GEMM_F16X3 && mode != FA_GEMM_F16X6) return FA_ERR_ARG;
   if (!scratch) return FA_ERR_WORKSPACE;
-  const int npl = planes_for_mode(mode);
   Arena local(scratch->base, scratch->cap);   // scratch is reused by every call (stream ordered)
-  plane_t* planes = local.take<plane_t>((size_t)npl * rows * lin.in_pad);
+  plane_t* planes = gemm_carve(local, rows, lin.in_pad, mode);
   if (!local.ok()) return FA_ERR_WORKSPACE;
-  FA_RETURN_IF_ERR(split_rows_launch(x, ldx, rows, lin.in_f, lin.in_pad, npl, planes, st));
+  FA_RETURN_IF_ERR(split_rows_launch(x, ldx, rows, lin.in_f, lin.in_pad, gemm_planes(mode), planes, st));
   return gemm_tc_planes_launch(planes, rows, lin, relu, r1, ld1, r2, ld2, y, ldy, nullptr, 0, mode, st, nullptr);
 }
 

@@ -38,7 +38,7 @@ struct AttnSinks {
 int attention_tc_planes_launch(const plane_t* qp, const plane_t* kp, const plane_t* vt, const int32_t* key_lens,
                                int batch, int heads, int tq, int tk, float* ctx, int64_t ldc, plane_t* ctx_planes,
                                int64_t ldp, int out_nplanes, int mode, cudaStream_t st, int kv_shared = 0, int head_dim = 128);
-size_t attention_tc_scratch_bytes(int batch, int heads, int tq, int tk, int mode);
+size_t attention_tc_scratch_bytes(int batch, int heads, int tq, int tk, int mode, int kv_shared);
 int attention_tc_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
                         const int32_t* key_lens, int batch, int heads, int tq, int tk, float* ctx, int64_t ldc,
                         plane_t* ctx_planes, int64_t ldp, int out_nplanes, int mode, Arena* scratch, cudaStream_t st,

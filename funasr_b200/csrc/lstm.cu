@@ -176,11 +176,16 @@ blstm_tc_kernel(const float* __restrict__ xproj, const float* __restrict__ w_hh_
   }
 }
 
+// 256 bytes of step counters, then the bf16 hi / lo planes of h for both directions, double buffered
+static size_t blstm_scratch_bytes(int batch, int H) {
+  const int batch_pad = (batch + LS_BT - 1) / LS_BT * LS_BT;
+  return 256 + (size_t)2 * 2 * 2 * batch_pad * H * sizeof(__nv_bfloat16);
+}
+
 template <int H>
 static int blstm_tc_launch_h(const float* xproj, const float* w_hh_f, const float* w_hh_b, int batch, int T, float* out,
                              void* scratch, size_t scratch_bytes, cudaStream_t st) {
-  const int batch_pad = (batch + LS_BT - 1) / LS_BT * LS_BT;
-  const size_t need = 256 + (size_t)2 * 2 * 2 * batch_pad * H * sizeof(__nv_bfloat16);
+  const size_t need = blstm_scratch_bytes(batch, H);
   if (scratch_bytes < need) return FA_ERR_WORKSPACE;
   const size_t smem = (size_t)2 * LS_ROWS * lt_pitch<H>() + (size_t)2 * LS_BT * lt_pitch<H>();
   static PerDeviceOnce once;
@@ -208,10 +213,7 @@ int blstm_tc_launch(const float* xproj, const float* w_hh_f, const float* w_hh_b
 // One-layer bidirectional LSTM over [B, T, H], H = 512 or 320, given the input projections of both directions:
 //   xproj [B*T, 2*4H] = x W_ih^T + b_ih + b_hh, columns [0,4H) forward gates (i,f,g,o), [4H,8H) reverse.
 // scratch >= fa_blstm_tc_scratch_bytes(batch) (sized for H = 512, which covers 320).
-extern "C" size_t fa_blstm_tc_scratch_bytes(int32_t batch) {
-  const int batch_pad = (batch + fa::LS_BT - 1) / fa::LS_BT * fa::LS_BT;
-  return 256 + (size_t)2 * 2 * 2 * batch_pad * fa::LS_HMAX * 2;
-}
+extern "C" size_t fa_blstm_tc_scratch_bytes(int32_t batch) { return fa::blstm_scratch_bytes(batch, fa::LS_HMAX); }
 extern "C" int fa_blstm_forward_tc(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, int32_t batch, int32_t t_len,
                                    int32_t hidden, float* out, void* scratch, size_t scratch_bytes, fa_stream_t stream) {
   return fa::blstm_tc_launch(xproj, w_hh_fwd, w_hh_bwd, batch, t_len, hidden, out, scratch, scratch_bytes, (cudaStream_t)stream);

@@ -47,34 +47,33 @@ static int linear(const float* x, int64_t ldx, int64_t rows, const FaLinear& lin
   return gemm_tc_launch(x, ldx, rows, lin, relu, r1, ld1, r2, ld2, y, ldy, mode, scratch, st);
 }
 
-static inline int npl_for(int mode) { return mode == FA_GEMM_F16X1 ? 1 : (mode == FA_GEMM_F16X3 ? 2 : 3); }
-static inline size_t max_sz(size_t a, size_t b) { return a > b ? a : b; }
-
 // ------------------------------------------------------------------------------------------------ encoder
-static size_t enc_scratch_bytes(int batch, int t_max, int heads, int mode) {
+// Sized for the largest supported stack (d_model 512, input 560, FFN 2048).  The fp32 path keeps every activation in fp32; the
+// tensor-core path passes LayerNorm, attention and FFN w_1 outputs as fp16 planes and writes only the V columns of qkv in fp32.
+struct EncBufs {
+  float *u, *qkv, *mem, *ctx, *xa, *xb, *h;
+  plane_t *ctx_planes, *h_planes, *u_planes, *q_planes, *k_planes, *vt_planes;
+};
+static EncBufs enc_carve(Arena& a, int batch, int t_max, int mode) {
   const int64_t M = (int64_t)batch * t_max;
-  return max_sz(gemm_tc_scratch_bytes(M, 2048, mode), attention_tc_scratch_bytes(batch, heads, t_max, t_max, mode));
-}
-static size_t enc_plan(int batch, int t_max, int din, int mode) {
-  const int64_t M = (int64_t)batch * t_max;
-  ArenaSizer s;
-  s.take(M * (size_t)din * 4);   // u
-  s.take(M * 1536ull * 4);       // qkv
-  s.take(M * 512ull * 4);        // mem
-  s.take(M * 512ull * 4);        // ctx
-  s.take(M * 512ull * 4);        // xa
-  s.take(M * 512ull * 4);        // xb
-  s.take(M * 2048ull * 4);       // h
-  if (mode != FA_GEMM_F32_SIMT) {
-    s.take(3ull * M * 512 * 2);    // ctx planes
-    s.take(3ull * M * 2048 * 2);   // h planes
-    s.take(3ull * M * 576 * 2);    // LN output planes
-    s.take(2ull * M * 512 * 2);    // q planes (scaled)
-    s.take(2ull * M * 512 * 2);    // k planes
-    s.take(2ull * batch * 512 * (size_t)((t_max + 63) / 64 * 64) * 2);   // v planes, transposed per head
-  }
-  s.take(enc_scratch_bytes(batch, t_max, 4, mode));
-  return s.off + 256;
+  const bool tc = mode != FA_GEMM_F32_SIMT;
+  const size_t gpl = gemm_planes(mode), apl = attn_planes(mode);
+  const int t_pad = (t_max + 63) / 64 * 64;
+  EncBufs b;
+  b.u = tc ? nullptr : a.take<float>(M * 560ull);
+  b.qkv = a.take<float>(M * 1536ull);
+  b.mem = a.take<float>(M * 512ull);
+  b.ctx = tc ? nullptr : a.take<float>(M * 512ull);
+  b.xa = a.take<float>(M * 512ull);
+  b.xb = a.take<float>(M * 512ull);
+  b.h = tc ? nullptr : a.take<float>(M * 2048ull);
+  b.ctx_planes = tc ? a.take<plane_t>(gpl * M * 512) : nullptr;
+  b.h_planes = tc ? a.take<plane_t>(gpl * M * 2048) : nullptr;
+  b.u_planes = tc ? a.take<plane_t>(gpl * M * 576) : nullptr;      // LN output: the QKV GEMM's K pad of a 560 input
+  b.q_planes = tc ? a.take<plane_t>(apl * M * 512) : nullptr;      // scaled by d_k^-0.5
+  b.k_planes = tc ? a.take<plane_t>(apl * M * 512) : nullptr;
+  b.vt_planes = tc ? a.take<plane_t>(apl * batch * 512 * (size_t)t_pad) : nullptr;   // transposed per head
+  return b;
 }
 
 }  // namespace fa
@@ -82,7 +81,9 @@ static size_t enc_plan(int batch, int t_max, int din, int mode) {
 using namespace fa;
 
 extern "C" size_t fa_sanm_encoder_workspace_bytes(int32_t batch, int32_t t_max, int32_t gemm_mode) {
-  return enc_plan(batch, t_max, 560, gemm_mode);
+  Arena m = Arena::measuring();
+  enc_carve(m, batch, t_max, gemm_mode);
+  return m.bytes();
 }
 
 extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats, const int32_t* lens, int32_t batch,
@@ -101,34 +102,22 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
       din > 560 || (din & 15) || (!embed && din != D))
     return FA_ERR_UNSUPPORTED;
   if (gemm_mode != FA_GEMM_F32_SIMT && !((D == 512 && hd == 128) || (D == 320 && hd == 80))) return FA_ERR_UNSUPPORTED;
-  Arena a(workspace, ws_bytes);
-  float* u = a.take<float>(M * (size_t)560);
-  float* qkv = a.take<float>(M * 1536ull);
-  float* mem = a.take<float>(M * 512ull);
-  float* ctx = a.take<float>(M * 512ull);
-  float* xa = a.take<float>(M * 512ull);
-  float* xb = a.take<float>(M * 512ull);
-  float* h = a.take<float>(M * 2048ull);
   const bool tc = gemm_mode != FA_GEMM_F32_SIMT;
-  const int npl = npl_for(gemm_mode);
-  plane_t* ctx_planes = tc ? a.take<plane_t>(3ull * M * 512) : nullptr;
-  plane_t* h_planes = tc ? a.take<plane_t>(3ull * M * 2048) : nullptr;
-  plane_t* u_planes = tc ? a.take<plane_t>(3ull * M * 576) : nullptr;
+  const int npl = gemm_planes(gemm_mode);
   const int t_pad = (t_max + 63) / 64 * 64;
-  plane_t* q_planes = tc ? a.take<plane_t>(2ull * M * 512) : nullptr;
-  plane_t* k_planes = tc ? a.take<plane_t>(2ull * M * 512) : nullptr;
-  plane_t* vt_planes = tc ? a.take<plane_t>(2ull * batch * 512 * (size_t)t_pad) : nullptr;
-  const size_t sb = enc_scratch_bytes(batch, t_max, enc->heads, gemm_mode);
-  char* sp = a.take<char>(sb);
+  Arena a(workspace, ws_bytes);
+  const EncBufs b = enc_carve(a, batch, t_max, gemm_mode);
   if (!a.ok()) return FA_ERR_WORKSPACE;
-  Arena scratch(sp, sb);
+  float *u = b.u, *qkv = b.qkv, *mem = b.mem, *ctx = b.ctx, *xa = b.xa, *xb = b.xb, *h = b.h;
+  plane_t *ctx_planes = b.ctx_planes, *h_planes = b.h_planes, *u_planes = b.u_planes;
+  plane_t *q_planes = b.q_planes, *k_planes = b.k_planes, *vt_planes = b.vt_planes;
 
   const float* x = embed ? nullptr : feats;  // residual stream (with PE input: undefined before layer 0, in_size != size)
   for (int l = 0; l < enc->n_layers; ++l) {
     const FaEncLayer& L = enc->layers[l];
     const int in = L.norm1.n;
     if (L.qkv.in_f != in || L.qkv.out_f != 3 * D || L.w1.in_f != D || L.w2.out_f != D || L.w2.in_f != L.w1.out_f) return FA_ERR_ARG;
-    if (L.w1.out_f > 2048) return FA_ERR_UNSUPPORTED;      // the workspace plan sizes the FFN hidden slice for linear_units <= 2048
+    if (L.w1.out_f > 2048) return FA_ERR_UNSUPPORTED;      // enc_carve sizes the FFN hidden slice for linear_units <= 2048
     // x = x*sqrt(D) + PE is folded into the first LayerNorm (encoder.py:409,428)
     // tensor-core path: LayerNorm writes the fp16 planes the QKV GEMM consumes (no fp32 round trip, no split pass)
     if (l > 0 && in != D) return FA_ERR_UNSUPPORTED;
@@ -143,11 +132,11 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
       // QKV GEMM epilogue emits the attention operands directly: q (x d_k^-0.5) / k as fp16 planes, v transposed per head
       // as fp16 planes plus fp32 v (the only fp32 columns written) for the FSMN branch
       AttnSinks sk;
-      sk.q0 = 0; sk.k0 = D; sk.v0 = 2 * D; sk.width = D; sk.npl = npl < 2 ? npl : 2; sk.t_rows = t_max; sk.t_pad = t_pad;
+      sk.q0 = 0; sk.k0 = D; sk.v0 = 2 * D; sk.width = D; sk.npl = attn_planes(gemm_mode); sk.t_rows = t_max; sk.t_pad = t_pad;
       sk.qscale = (float)pow((double)hd, -0.5); sk.q_planes = q_planes; sk.k_planes = k_planes; sk.vt_planes = vt_planes;
       FA_RETURN_IF_ERR(gemm_tc_planes_launch(u_planes, M, L.qkv, 0, nullptr, 0, nullptr, 0, qkv, 3 * D, nullptr, 0, gemm_mode, st, &sk));
     } else {
-      FA_RETURN_IF_ERR(linear(u, in, M, L.qkv, 0, nullptr, 0, nullptr, 0, qkv, 3 * D, gemm_mode, &scratch, st));
+      FA_RETURN_IF_ERR(linear(u, in, M, L.qkv, 0, nullptr, 0, nullptr, 0, qkv, 3 * D, gemm_mode, nullptr, st));
     }
     SideStream* side = tc ? side_stream(st) : nullptr;
     // x2 = (residual if in_size == size) + (linear_out(ctx) + fsmn_memory)     encoder.py:120-137, attention.py:327
@@ -173,10 +162,10 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
       } else {
         FA_RETURN_IF_ERR(attention_small_launch(qkv, 3 * D, qkv + D, 3 * D, qkv + 2 * D, 3 * D, lens, batch, enc->heads, hd, t_max, t_max, ctx, D, st));
       }
-      FA_RETURN_IF_ERR(linear(ctx, D, M, L.out, 0, mem, D, res, D, x2, D, gemm_mode, &scratch, st));
+      FA_RETURN_IF_ERR(linear(ctx, D, M, L.out, 0, mem, D, res, D, x2, D, gemm_mode, nullptr, st));
       FA_RETURN_IF_ERR(layernorm_launch(x2, M, L.norm2, u, nullptr, 1.f, t_max, st));
-      FA_RETURN_IF_ERR(linear(u, D, M, L.w1, 1, nullptr, 0, nullptr, 0, h, L.w1.out_f, gemm_mode, &scratch, st));
-      FA_RETURN_IF_ERR(linear(h, L.w1.out_f, M, L.w2, 0, x2, D, nullptr, 0, x3, D, gemm_mode, &scratch, st));
+      FA_RETURN_IF_ERR(linear(u, D, M, L.w1, 1, nullptr, 0, nullptr, 0, h, L.w1.out_f, gemm_mode, nullptr, st));
+      FA_RETURN_IF_ERR(linear(h, L.w1.out_f, M, L.w2, 0, x2, D, nullptr, 0, x3, D, gemm_mode, nullptr, st));
     } else {
       // tensor-core path: attention emits the context as fp16 planes (A operand of linear_out); FFN w_1 emits its
       // ReLU output as planes for w_2 — neither intermediate makes an fp32 round trip through HBM
@@ -195,14 +184,25 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
 }
 
 // ---------------------------------------------------------------------------------------------- predictor
+// fp32: the im2col rows [M, 3D] and the conv output c [M, D].  Tensor cores: no im2col copy — the GEMM's A operand is the
+// overlapping view of the zero-padded encoder planes pp (cif.cu), and its output c has the padded rows [batch * (t_max + 2), D].
+struct CifBufs { float *xc, *c, *alpha_rows; plane_t* pp; };
+static CifBufs cif_carve(Arena& a, int batch, int t_max, int mode) {
+  const int D = 512;
+  const int64_t M = (int64_t)batch * t_max, Mp = (int64_t)batch * (t_max + 2);
+  const bool tc = mode != FA_GEMM_F32_SIMT;
+  CifBufs b;
+  b.xc = tc ? nullptr : a.take<float>(M * 3ull * D);
+  b.c = a.take<float>((tc ? Mp : M) * (size_t)D);
+  b.alpha_rows = a.take<float>(M);
+  b.pp = tc ? a.take<plane_t>((size_t)gemm_planes(mode) * (Mp + 2) * D) : nullptr;
+  return b;
+}
+
 extern "C" size_t fa_cif_predictor_workspace_bytes(int32_t batch, int32_t t_max, int32_t gemm_mode) {
-  const int64_t M = (int64_t)batch * t_max;
-  ArenaSizer s;
-  s.take(M * 1536ull * 4);
-  s.take(M * 512ull * 4);
-  s.take(M * 4ull);
-  s.take(gemm_tc_scratch_bytes(M, 1536, gemm_mode));
-  return s.off + 256;
+  Arena m = Arena::measuring();
+  cif_carve(m, batch, t_max, gemm_mode);
+  return m.bytes();
 }
 
 extern "C" int fa_cif_predictor_forward(const FaPredictor* pred, const float* enc, const int32_t* lens, int32_t batch,
@@ -214,38 +214,32 @@ extern "C" int fa_cif_predictor_forward(const FaPredictor* pred, const float* en
   cudaStream_t st = (cudaStream_t)stream;
   const int D = 512;
   if (pred->conv.out_f != D || pred->conv.in_f != 3 * D) return FA_ERR_UNSUPPORTED;
+  const bool tc = gemm_mode != FA_GEMM_F32_SIMT;
+  if (tc && !pred->conv.w_planes) return FA_ERR_ARG;
+  if (tc && pred->conv.in_pad != 3 * D) return FA_ERR_UNSUPPORTED;    // the conv view reads K = 3 D unpadded
   const int64_t M = (int64_t)batch * t_max;
   Arena a(workspace, ws_bytes);
-  float* xc = a.take<float>(M * 1536ull);
-  float* c = a.take<float>(M * 512ull);
-  float* alpha_rows = a.take<float>(M);
-  const size_t sb = gemm_tc_scratch_bytes(M, 1536, gemm_mode);
-  char* sp = a.take<char>(sb);
+  const CifBufs b = cif_carve(a, batch, t_max, gemm_mode);
   if (!a.ok()) return FA_ERR_WORKSPACE;
-  Arena scratch(sp, sb);
-  if (gemm_mode != FA_GEMM_F32_SIMT && pred->conv.w_planes && pred->conv.in_pad == 3 * D) {
-    // tensor-core path: no im2col copy — the GEMM's A operand is the overlapping view of the zero-padded encoder planes (cif.cu)
-    const int npl = npl_for(gemm_mode);
+  if (tc) {
+    const int npl = gemm_planes(gemm_mode);
     const int64_t Mp = (int64_t)batch * (t_max + 2), rows_alloc = Mp + 2;
-    plane_t* pp = scratch.take<plane_t>((size_t)npl * rows_alloc * D);          // <= the im2col planes this scratch was sized for
-    if (!scratch.ok()) return FA_ERR_WORKSPACE;
-    float* cp = xc;                                                              // [Mp, D] fits the unused im2col buffer (3 D per row)
-    FA_RETURN_IF_ERR(cif_pad_planes_launch(enc, batch, t_max, D, npl, rows_alloc, pp, st));
-    FA_RETURN_IF_ERR(gemm_tc_planes_launch(pp, Mp, pred->conv, 1, nullptr, 0, nullptr, 0, cp, D, nullptr, 0, gemm_mode, st, nullptr, D, rows_alloc));
-    FA_RETURN_IF_ERR(cif_alpha_launch(cp, D, pred->out_w, pred->out_b, lens, t_max, M, pred->smooth_factor,
-                                      pred->noise_threshold, alpha_rows, st, t_max + 2));
+    FA_RETURN_IF_ERR(cif_pad_planes_launch(enc, batch, t_max, D, npl, rows_alloc, b.pp, st));
+    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.pp, Mp, pred->conv, 1, nullptr, 0, nullptr, 0, b.c, D, nullptr, 0, gemm_mode, st, nullptr, D, rows_alloc));
+    FA_RETURN_IF_ERR(cif_alpha_launch(b.c, D, pred->out_w, pred->out_b, lens, t_max, M, pred->smooth_factor,
+                                      pred->noise_threshold, b.alpha_rows, st, t_max + 2));
   } else {
-    FA_RETURN_IF_ERR(cif_im2col_launch(enc, M, t_max, D, xc, st));
-    FA_RETURN_IF_ERR(linear(xc, 3 * D, M, pred->conv, 1, nullptr, 0, nullptr, 0, c, D, gemm_mode, &scratch, st));
-    FA_RETURN_IF_ERR(cif_alpha_launch(c, D, pred->out_w, pred->out_b, lens, t_max, M, pred->smooth_factor,
-                                      pred->noise_threshold, alpha_rows, st));
+    FA_RETURN_IF_ERR(cif_im2col_launch(enc, M, t_max, D, b.xc, st));
+    FA_RETURN_IF_ERR(linear(b.xc, 3 * D, M, pred->conv, 1, nullptr, 0, nullptr, 0, b.c, D, gemm_mode, nullptr, st));
+    FA_RETURN_IF_ERR(cif_alpha_launch(b.c, D, pred->out_w, pred->out_b, lens, t_max, M, pred->smooth_factor,
+                                      pred->noise_threshold, b.alpha_rows, st));
   }
   FA_CUDA_OK(cudaMemsetAsync(acoustic, 0, (size_t)batch * n_cap * D * sizeof(float), st));
   if (pred->cif_variant == 1)     // CifPredictorV3 (BiCifParaformer): sequential fp32 `cif`
-    return cif_fire_loop_launch(enc, alpha_rows, lens, batch, t_max, D, pred->tail_threshold, pred->threshold, acoustic, n_cap,
+    return cif_fire_loop_launch(enc, b.alpha_rows, lens, batch, t_max, D, pred->tail_threshold, pred->threshold, acoustic, n_cap,
                                 token_num, alphas, peaks, st);
   if (pred->cif_variant != 0) return FA_ERR_ARG;
-  return cif_fire_launch(enc, alpha_rows, lens, batch, t_max, D, pred->tail_threshold, acoustic, n_cap, token_num, alphas,
+  return cif_fire_launch(enc, b.alpha_rows, lens, batch, t_max, D, pred->tail_threshold, acoustic, n_cap, token_num, alphas,
                          peaks, st);
 }
 
@@ -261,58 +255,64 @@ extern "C" int fa_cif_upsample_alphas(const float* feat, int32_t dz, const float
 }
 
 // ------------------------------------------------------------------------------------------------ decoder
-static size_t dec_scratch_bytes(int batch, int t_max, int n_max, int mode) {
+// Workspace of every decoder-stack entry point (d_model 512, 4 heads of 128, FFN <= 2048).  The memory has Mk = batch * t_max rows
+// (an upper bound when it is shared).  contextual: the bias decoder over n_hotwords rows of hotword memory.  probs: the stack's ASF
+// probe (attn_probs), which its query cannot see, so the stack always carves for it.  On the tensor-core path every layer passes
+// its operands as fp16 planes; fp32 q / k|v / context rows and GEMM scratch serve only the calls that take fp32 operands.
+struct DecBuf {
+  float *ya, *yb, *t1, *hq, *f, *qd, *ctx, *kv, *lg, *cat, *kvh;
+  plane_t *ctx_planes, *mem_planes, *t1_planes, *hq_planes, *q_planes, *k_planes, *vt_planes;
+  Arena scratch{nullptr, 0}, hw_scratch{nullptr, 0};
+};
+static void dec_carve(Arena& a, DecBuf& b, int batch, int t_max, int n_max, int vocab, int mode, int n_hotwords, bool probs) {
   const int64_t Mq = (int64_t)batch * n_max, Mk = (int64_t)batch * t_max;
-  return max_sz(gemm_tc_scratch_bytes(Mq > Mk ? Mq : Mk, 2048, mode), attention_tc_scratch_bytes(batch, 4, n_max, t_max, mode));
-}
-// hotword region of the contextual bias decoder: k|v rows of the (shared) hotword memory + GEMM / attention scratch
-static size_t hw_region_bytes(int batch, int n_max, int nh, int mode) {
-  if (nh <= 0) return 0;
-  const int64_t Mq = (int64_t)batch * n_max;
-  ArenaSizer s;
-  s.take((size_t)nh * 1024 * 4);
-  s.take(max_sz(gemm_tc_scratch_bytes(Mq > nh ? Mq : nh, 1024, mode), attention_tc_scratch_bytes(batch, 4, n_max, nh, mode)));
-  return s.off + 256;
-}
-static size_t dec_plan(int batch, int t_max, int n_max, int vocab, int mode, size_t dec_scratch, int n_hotwords) {
-  const int64_t Mq = (int64_t)batch * n_max, Mk = (int64_t)batch * t_max;
-  ArenaSizer s;
-  s.take(Mq * 512ull * 4);   // ya
-  s.take(Mq * 512ull * 4);   // yb
-  s.take(Mq * 512ull * 4);   // t1
-  s.take(Mq * 2048ull * 4);  // hq
-  s.take(Mq * 512ull * 4);   // f
-  s.take(Mq * 512ull * 4);   // qd
-  s.take(Mq * 512ull * 4);   // ctx
-  s.take(Mk * 1024ull * 4);  // kv
-  s.take(Mq * (size_t)vocab * 4);  // logits (used when the caller passes none)
-  s.take(Mq * 1024ull * 4);        // [x_src_attn ; cx] of the contextual decoder
-  s.take(hw_region_bytes(batch, n_max, n_hotwords, mode));
-  if (mode != FA_GEMM_F32_SIMT) {
-    s.take(3ull * Mq * 512 * 2);   // ctx planes
-    s.take(3ull * Mk * 512 * 2);   // enc planes (split once, reused by the 16 kv GEMMs)
-    s.take(3ull * Mq * 512 * 2);   // LN output planes
-    s.take(3ull * Mq * 2048 * 2);  // FFN hidden planes
-    s.take(2ull * Mq * 512 * 2);   // q planes
-    s.take(2ull * Mk * 512 * 2);   // k planes
-    s.take(2ull * batch * 512 * (size_t)((t_max + 63) / 64 * 64) * 2);   // v planes, transposed per head
+  const bool tc = mode != FA_GEMM_F32_SIMT;
+  const bool contextual = n_hotwords > 0;
+  const size_t gpl = gemm_planes(mode), apl = attn_planes(mode);
+  const int t_pad = (t_max + 63) / 64 * 64;
+  b.ya = a.take<float>(Mq * 512ull); b.yb = a.take<float>(Mq * 512ull); b.t1 = a.take<float>(Mq * 512ull);
+  b.hq = a.take<float>(Mq * 2048ull); b.f = a.take<float>(Mq * 512ull);
+  b.qd = (!tc || contextual || probs) ? a.take<float>(Mq * 512ull) : nullptr;
+  b.ctx = (!tc || contextual) ? a.take<float>(Mq * 512ull) : nullptr;
+  b.kv = (!tc || probs) ? a.take<float>(Mk * 1024ull) : nullptr;
+  b.lg = a.take<float>(Mq * (size_t)vocab);                          // logits, used when the caller passes none
+  b.cat = contextual ? a.take<float>(Mq * 1024ull) : nullptr;         // [x_src_attn ; cx]
+  b.kvh = contextual ? a.take<float>((size_t)n_hotwords * 1024) : nullptr;   // k | v rows of the shared hotword memory
+  b.ctx_planes = tc ? a.take<plane_t>(gpl * Mq * 512) : nullptr;
+  b.mem_planes = tc ? a.take<plane_t>(gpl * Mk * 512) : nullptr;      // split once, reused by every layer's k|v GEMM
+  b.t1_planes = tc ? a.take<plane_t>(gpl * Mq * 512) : nullptr;       // LN outputs
+  b.hq_planes = tc ? a.take<plane_t>(gpl * Mq * 2048) : nullptr;      // FFN hidden
+  b.q_planes = tc ? a.take<plane_t>(apl * Mq * 512) : nullptr;
+  b.k_planes = tc ? a.take<plane_t>(apl * Mk * 512) : nullptr;
+  b.vt_planes = tc ? a.take<plane_t>(apl * batch * 512 * (size_t)t_pad) : nullptr;   // transposed per head
+  if (tc && (contextual || probs)) {
+    // contextual: bias_q, bias_out (K 512) and bias_output (K 1024) over Mq rows; probs: q of n_max rows, k|v of t_max rows (K 512)
+    const size_t sc = contextual ? gemm_tc_scratch_bytes(Mq, 1024, mode) : 0;
+    const size_t sp = probs ? gemm_tc_scratch_bytes(n_max > t_max ? n_max : t_max, 512, mode) : 0;
+    b.scratch = a.sub(sc > sp ? sc : sp);
   }
-  s.take(dec_scratch);
-  return s.off + 256;
+  if (tc && contextual) {
+    // the hotword k|v GEMM (n_hotwords rows, K 512), then the attention over the shared hotword memory
+    const size_t sg = gemm_tc_scratch_bytes(n_hotwords, 512, mode), sa = attention_tc_scratch_bytes(batch, 4, n_max, n_hotwords, mode, 1);
+    b.hw_scratch = a.sub(sg > sa ? sg : sa);
+  }
 }
 
 extern "C" size_t fa_paraformer_decoder_workspace_bytes_hw(int32_t batch, int32_t t_max, int32_t n_max, int32_t vocab,
                                                            int32_t gemm_mode, int32_t n_hotwords) {
-  return dec_plan(batch, t_max, n_max, vocab, gemm_mode, dec_scratch_bytes(batch, t_max, n_max, gemm_mode), n_hotwords);
+  Arena m = Arena::measuring();
+  DecBuf b;
+  dec_carve(m, b, batch, t_max, n_max, vocab, gemm_mode, n_hotwords, false);
+  return m.bytes();
 }
 
 static int dec_ffn(const FaDecLayer& L, const float* y, int64_t Mq, float* t1, float* hq, float* f, int mode,
                    Arena* scratch, cudaStream_t st, plane_t* t1_planes, plane_t* hq_planes) {
   // f = w_2( LN_2048( relu( w_1( LN1(y) ) ) ) )   decoder.py:97-100, sanm/positionwise_feed_forward.py:33
   if (L.ffn_w1.in_f != 512 || L.ffn_w2.out_f != 512 || L.ffn_w2.in_f != L.ffn_w1.out_f || L.ffn_norm.n != L.ffn_w1.out_f) return FA_ERR_ARG;
-  if (L.ffn_w1.out_f > 2048) return FA_ERR_UNSUPPORTED;    // dec_plan sizes hq / hq_planes for linear_units <= 2048
+  if (L.ffn_w1.out_f > 2048) return FA_ERR_UNSUPPORTED;    // dec_carve sizes hq / hq_planes for linear_units <= 2048
   if (mode != FA_GEMM_F32_SIMT) {
-    const int npl = npl_for(mode);
+    const int npl = gemm_planes(mode);
     if (L.ffn_w1.in_pad != 512 || L.ffn_w2.in_pad != L.ffn_w1.out_f) return FA_ERR_UNSUPPORTED;
     FA_RETURN_IF_ERR(layernorm_launch(y, Mq, L.norm1, nullptr, nullptr, 1.f, 1, st, t1_planes, npl, 512));
     FA_RETURN_IF_ERR(gemm_tc_planes_launch(t1_planes, Mq, L.ffn_w1, 1, nullptr, 0, nullptr, 0, hq, L.ffn_w1.out_f, nullptr, 0, mode, st));
@@ -363,35 +363,6 @@ attn_probs_kernel(const float* __restrict__ q, int64_t ldq, const float* __restr
   for (int t = lane; t < t_k; t += 32) probs[(int64_t)row * t_k + t] = t < klen ? sc[t] / sum : 0.f;
 }
 
-// Workspace slices shared by every decoder-stack entry point (same carve order as dec_plan).
-struct DecBuf {
-  float *ya, *yb, *t1, *hq, *f, *qd, *ctx, *kv, *lg, *cat;
-  char* hw_region; size_t hwb;
-  plane_t *ctx_planes, *mem_planes, *t1_planes, *hq_planes, *q_planes, *k_planes, *vt_planes;
-  char* sp; size_t sb;
-};
-static bool dec_carve(Arena& a, DecBuf& b, int batch, int t_max, int n_max, int vocab, int mode, int n_hotwords) {
-  const int64_t Mq = (int64_t)batch * n_max, Mk = (int64_t)batch * t_max;
-  const bool tc = mode != FA_GEMM_F32_SIMT;
-  b.ya = a.take<float>(Mq * 512ull); b.yb = a.take<float>(Mq * 512ull); b.t1 = a.take<float>(Mq * 512ull);
-  b.hq = a.take<float>(Mq * 2048ull); b.f = a.take<float>(Mq * 512ull); b.qd = a.take<float>(Mq * 512ull);
-  b.ctx = a.take<float>(Mq * 512ull); b.kv = a.take<float>(Mk * 1024ull); b.lg = a.take<float>(Mq * (size_t)vocab);
-  b.cat = a.take<float>(Mq * 1024ull);
-  b.hwb = hw_region_bytes(batch, n_max, n_hotwords, mode);
-  b.hw_region = a.take<char>(b.hwb);
-  const int t_pad = (t_max + 63) / 64 * 64;
-  b.ctx_planes = tc ? a.take<plane_t>(3ull * Mq * 512) : nullptr;
-  b.mem_planes = tc ? a.take<plane_t>(3ull * Mk * 512) : nullptr;
-  b.t1_planes = tc ? a.take<plane_t>(3ull * Mq * 512) : nullptr;
-  b.hq_planes = tc ? a.take<plane_t>(3ull * Mq * 2048) : nullptr;
-  b.q_planes = tc ? a.take<plane_t>(2ull * Mq * 512) : nullptr;
-  b.k_planes = tc ? a.take<plane_t>(2ull * Mk * 512) : nullptr;
-  b.vt_planes = tc ? a.take<plane_t>(2ull * batch * 512 * (size_t)t_pad) : nullptr;
-  b.sb = dec_scratch_bytes(batch, t_max, n_max, mode);
-  b.sp = a.take<char>(b.sb);
-  return a.ok();
-}
-
 // One run of a SAN-M decoder stack over a cross-attention memory.  memory [mem_batch * t_mem, 512] with mem_batch = batch, or 1
 // when mem_shared (the SeACo / contextual hotword memory: every utterance attends over the same rows — one k/v projection, one
 // copy).  tgt [batch, n_max, 512] lives in b.ya on entry.
@@ -415,7 +386,7 @@ static int dec_attention_layer(const DecRun& r, const FaDecLayer& L, float* yin,
   const int D = 512;
   const int64_t Mq = r.Mq(), Mk = r.Mk();
   const bool tc = r.mode != FA_GEMM_F32_SIMT;
-  const int npl = npl_for(r.mode);
+  const int npl = gemm_planes(r.mode);
   const int t_pad = (r.t_mem + 63) / 64 * 64;
   cudaStream_t st = r.st;
   FA_RETURN_IF_ERR(dec_ffn(L, yin, Mq, b.t1, b.hq, b.f, r.mode, r.scratch, st, b.t1_planes, b.hq_planes));
@@ -442,7 +413,7 @@ static int dec_attention_layer(const DecRun& r, const FaDecLayer& L, float* yin,
   if (tc) {
     FA_RETURN_IF_ERR(layernorm_launch(x2, Mq, L.norm3, nullptr, nullptr, 1.f, 1, st, b.t1_planes, npl, D));
     AttnSinks sq;                       // q -> scaled fp16 planes only (no fp32 round trip)
-    sq.q0 = 0; sq.width = D; sq.npl = npl < 2 ? npl : 2; sq.t_rows = r.n_max; sq.qscale = (float)(1.0 / sqrt(128.0)); sq.q_planes = b.q_planes;
+    sq.q0 = 0; sq.width = D; sq.npl = attn_planes(r.mode); sq.t_rows = r.n_max; sq.qscale = (float)(1.0 / sqrt(128.0)); sq.q_planes = b.q_planes;
     FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.t1_planes, Mq, L.q, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, r.mode, st, &sq));
   } else {
     FA_RETURN_IF_ERR(layernorm_launch(x2, Mq, L.norm3, b.t1, nullptr, 1.f, 1, st));
@@ -459,7 +430,7 @@ static int dec_attention_layer(const DecRun& r, const FaDecLayer& L, float* yin,
     FA_RETURN_IF_ERR(linear(b.ctx, D, Mq, L.out, 0, res, D, nullptr, 0, dst, ldd, r.mode, r.scratch, st));
   } else {
     AttnSinks skv;                      // k -> planes, v -> transposed planes; nothing in fp32
-    skv.k0 = 0; skv.v0 = D; skv.width = D; skv.npl = npl < 2 ? npl : 2; skv.t_rows = r.t_mem; skv.t_pad = t_pad;
+    skv.k0 = 0; skv.v0 = D; skv.width = D; skv.npl = attn_planes(r.mode); skv.t_rows = r.t_mem; skv.t_pad = t_pad;
     skv.k_planes = b.k_planes; skv.vt_planes = b.vt_planes;
     FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.mem_planes, Mk, L.kv, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, r.mode, st, &skv));
     FA_RETURN_IF_ERR(attention_tc_planes_launch(b.q_planes, b.k_planes, b.vt_planes, r.mem_lens, r.batch, r.heads, r.n_max, r.t_mem, nullptr, 0,
@@ -475,7 +446,7 @@ static int dec_finish(const DecRun& r, const FaDecoder* dec, float* y, float* hi
   DecBuf& b = *r.b;
   const bool tc = r.mode != FA_GEMM_F32_SIMT;
   FA_RETURN_IF_ERR(dec_ffn(dec->last, y, r.Mq(), b.t1, b.hq, b.f, r.mode, r.scratch, r.st, b.t1_planes, b.hq_planes));
-  if (tc) return layernorm_launch(b.f, r.Mq(), dec->after_norm, hidden_out, nullptr, 1.f, 1, r.st, b.t1_planes, npl_for(r.mode), 512);
+  if (tc) return layernorm_launch(b.f, r.Mq(), dec->after_norm, hidden_out, nullptr, 1.f, 1, r.st, b.t1_planes, gemm_planes(r.mode), 512);
   return layernorm_launch(b.f, r.Mq(), dec->after_norm, hidden_out ? hidden_out : b.t1, nullptr, 1.f, 1, r.st);
 }
 
@@ -491,12 +462,15 @@ static int decoder_forward_impl(const FaDecoder* dec, const float* enc, const in
   if (dec->after_norm.n != D || dec->heads * 128 != D) return FA_ERR_UNSUPPORTED;
   const int64_t Mq = (int64_t)batch * n_max, Mk = (int64_t)batch * t_max;
   const int V = dec->vocab;
+  const bool tc = gemm_mode != FA_GEMM_F32_SIMT;
+  const bool contextual = dec->has_bias != 0;
+  const int nh = dec->n_hotwords;
+  if (contextual && (!dec->hw_embed || !dec->hw_lens || nh <= 0 || dec->clas_scale != 1.0f)) return FA_ERR_UNSUPPORTED;
   Arena a(workspace, ws_bytes);
   DecBuf b;
-  if (!dec_carve(a, b, batch, t_max, n_max, V, gemm_mode, dec->has_bias ? dec->n_hotwords : 0)) return FA_ERR_WORKSPACE;
-  Arena scratch(b.sp, b.sb);
-  const bool tc = gemm_mode != FA_GEMM_F32_SIMT;
-  const int npl = npl_for(gemm_mode);
+  dec_carve(a, b, batch, t_max, n_max, V, gemm_mode, contextual ? nh : 0, false);
+  if (!a.ok()) return FA_ERR_WORKSPACE;
+  const int npl = gemm_planes(gemm_mode);
   float* lg = logits ? logits : b.lg;
   if (tc) FA_RETURN_IF_ERR(split_rows_launch(enc, D, Mk, D, D, npl, b.mem_planes, st));   // memory is layer-invariant
 
@@ -504,39 +478,32 @@ static int decoder_forward_impl(const FaDecoder* dec, const float* enc, const in
   FA_CUDA_OK(cudaMemcpy2DAsync(b.ya, (size_t)n_max * D * 4, acoustic, (size_t)ld_acoustic_rows * D * 4, (size_t)n_max * D * 4,
                                batch, cudaMemcpyDeviceToDevice, st));
   fa::count_launch();
-  DecRun r{batch, n_max, t_max, dec->heads, dec->fsmn_k, gemm_mode, 0, enc, enc_lens, tok_lens, st, &b, &scratch};
+  DecRun r{batch, n_max, t_max, dec->heads, dec->fsmn_k, gemm_mode, 0, enc, enc_lens, tok_lens, st, &b, &b.scratch};
   float* y = b.ya;
   for (int l = 0; l < dec->n_layers; ++l) {
     float* xs = nullptr;
     FA_RETURN_IF_ERR(dec_attention_layer(r, dec->layers[l], y, &xs, nullptr, 0, &y, nullptr));
   }
-  if (dec->has_bias) {
+  if (contextual) {
     // ContextualParaformerDecoder.forward decoder.py:325-340
-    const int nh = dec->n_hotwords;
-    if (!dec->hw_embed || !dec->hw_lens || nh <= 0 || dec->clas_scale != 1.0f) return FA_ERR_UNSUPPORTED;
     float* x_self = nullptr;
     FA_RETURN_IF_ERR(dec_attention_layer(r, dec->bias_last, y, &x_self, b.cat, 2 * D, nullptr, nullptr));      // cat[:, :512] = x_src_attn
     // bias decoder: cross attention of LN3(x_self_attn) over the hotword memory (identical for every utterance)
     FA_RETURN_IF_ERR(layernorm_launch(x_self, Mq, dec->bias_norm3, b.t1, nullptr, 1.f, 1, st));
-    FA_RETURN_IF_ERR(linear(b.t1, D, Mq, dec->bias_q, 0, nullptr, 0, nullptr, 0, b.qd, D, gemm_mode, &scratch, st));
+    FA_RETURN_IF_ERR(linear(b.t1, D, Mq, dec->bias_q, 0, nullptr, 0, nullptr, 0, b.qd, D, gemm_mode, &b.scratch, st));
     // the hotword k | v rows [nh, 1024] are the same for every utterance: one copy, attended with kv_shared (no per-utterance
     // replication, so the hotword count is independent of t_max)
-    Arena a2(b.hw_region, b.hwb);
-    float* kvh = a2.take<float>((size_t)nh * 1024);
-    const size_t sb2 = max_sz(gemm_tc_scratch_bytes(Mq > nh ? Mq : nh, 1024, gemm_mode), attention_tc_scratch_bytes(batch, 4, n_max, nh, gemm_mode));
-    char* sp2 = a2.take<char>(sb2);
-    if (!a2.ok()) return FA_ERR_WORKSPACE;
-    Arena scratch2(sp2, sb2);
-    FA_RETURN_IF_ERR(linear(dec->hw_embed, D, nh, dec->bias_kv, 0, nullptr, 0, nullptr, 0, kvh, 2 * D, gemm_mode, &scratch2, st));
+    float* kvh = b.kvh;
+    FA_RETURN_IF_ERR(linear(dec->hw_embed, D, nh, dec->bias_kv, 0, nullptr, 0, nullptr, 0, kvh, 2 * D, gemm_mode, &b.hw_scratch, st));
     if (!tc) {
       FA_RETURN_IF_ERR(attention_f32_launch(b.qd, D, kvh, 2 * D, kvh + D, 2 * D, dec->hw_lens, batch, dec->heads, n_max, nh, b.ctx, D, st, 1));
     } else {
       FA_RETURN_IF_ERR(attention_tc_launch(b.qd, D, kvh, 2 * D, kvh + D, 2 * D, dec->hw_lens, batch, dec->heads, n_max, nh, b.ctx, D,
-                                           nullptr, 0, 0, gemm_mode, &scratch2, st, 1));
+                                           nullptr, 0, 0, gemm_mode, &b.hw_scratch, st, 1));
     }
-    FA_RETURN_IF_ERR(linear(b.ctx, D, Mq, dec->bias_out, 0, nullptr, 0, nullptr, 0, b.cat + D, 2 * D, gemm_mode, &scratch, st));   // cat[:, 512:] = cx
+    FA_RETURN_IF_ERR(linear(b.ctx, D, Mq, dec->bias_out, 0, nullptr, 0, nullptr, 0, b.cat + D, 2 * D, gemm_mode, &b.scratch, st));   // cat[:, 512:] = cx
     float* y2 = (x_self == b.ya) ? b.yb : b.ya;
-    FA_RETURN_IF_ERR(linear(b.cat, 2 * D, Mq, dec->bias_output, 0, x_self, D, nullptr, 0, y2, D, gemm_mode, &scratch, st));
+    FA_RETURN_IF_ERR(linear(b.cat, 2 * D, Mq, dec->bias_output, 0, x_self, D, nullptr, 0, y2, D, gemm_mode, &b.scratch, st));
     y = y2;
   }
   // decoders3, after_norm (-> hidden), output_layer
@@ -544,7 +511,7 @@ static int decoder_forward_impl(const FaDecoder* dec, const float* enc, const in
   if (tc) {
     FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.t1_planes, Mq, dec->output, 0, nullptr, 0, nullptr, 0, lg, V, nullptr, 0, gemm_mode, st));
   } else {
-    FA_RETURN_IF_ERR(linear(hidden_out ? hidden_out : b.t1, D, Mq, dec->output, 0, nullptr, 0, nullptr, 0, lg, V, gemm_mode, &scratch, st));
+    FA_RETURN_IF_ERR(linear(hidden_out ? hidden_out : b.t1, D, Mq, dec->output, 0, nullptr, 0, nullptr, 0, lg, V, gemm_mode, nullptr, st));
   }
   return argmax_lse_launch(lg, Mq, V, V, argmax_ids, argmax_logp, (logits && log_softmax) ? 1 : 0, st);
 }
@@ -578,7 +545,10 @@ extern "C" int fa_paraformer_decoder_forward_hidden(const FaDecoder* dec, const 
 //   attn_probs != 0  -> instead, layer n_run - 1 stops at its cross-attention and writes utterance 0's probability matrix
 //                       [heads, n_max, t_mem] (forward_asf6 / get_attn_mat, decoder.py:485-513,123-146); hidden is not written.
 extern "C" size_t fa_sanm_decoder_stack_workspace_bytes(int32_t batch, int32_t t_mem, int32_t n_max, int32_t gemm_mode) {
-  return dec_plan(batch, t_mem, n_max, 0, gemm_mode, dec_scratch_bytes(batch, t_mem, n_max, gemm_mode), 0);
+  Arena m = Arena::measuring();
+  DecBuf b;
+  dec_carve(m, b, batch, t_mem, n_max, 0, gemm_mode, 0, true);
+  return m.bytes();
 }
 
 extern "C" int fa_sanm_decoder_stack_forward(const FaDecoder* dec, const float* memory, const int32_t* mem_lens, int32_t mem_shared,
@@ -594,11 +564,11 @@ extern "C" int fa_sanm_decoder_stack_forward(const FaDecoder* dec, const float* 
   if (dec->after_norm.n != D || dec->heads * 128 != D) return FA_ERR_UNSUPPORTED;
   Arena a(workspace, ws_bytes);
   DecBuf b;
-  if (!dec_carve(a, b, batch, t_mem, n_max, 0, gemm_mode, 0)) return FA_ERR_WORKSPACE;
-  Arena scratch(b.sp, b.sb);
+  dec_carve(a, b, batch, t_mem, n_max, 0, gemm_mode, 0, true);
+  if (!a.ok()) return FA_ERR_WORKSPACE;
   const bool tc = gemm_mode != FA_GEMM_F32_SIMT;
-  DecRun r{batch, n_max, t_mem, dec->heads, dec->fsmn_k, gemm_mode, mem_shared ? 1 : 0, memory, mem_lens, tok_lens, st, &b, &scratch};
-  if (tc) FA_RETURN_IF_ERR(split_rows_launch(memory, D, r.Mk(), D, D, npl_for(gemm_mode), b.mem_planes, st));
+  DecRun r{batch, n_max, t_mem, dec->heads, dec->fsmn_k, gemm_mode, mem_shared ? 1 : 0, memory, mem_lens, tok_lens, st, &b, &b.scratch};
+  if (tc) FA_RETURN_IF_ERR(split_rows_launch(memory, D, r.Mk(), D, D, gemm_planes(gemm_mode), b.mem_planes, st));
   FA_CUDA_OK(cudaMemcpy2DAsync(b.ya, (size_t)n_max * D * 4, x, (size_t)ld_x_rows * D * 4, (size_t)n_max * D * 4, batch,
                                cudaMemcpyDeviceToDevice, st));
   fa::count_launch();
@@ -649,12 +619,20 @@ extern "C" int fa_seaco_merge(const int32_t* dec_ids, const float* dec_best, con
 
 // hotword_output_layer + log-softmax arg-max over hidden rows (seaco_paraformer/model.py:352-355): logits = (a + b) W^T + bias for
 // the two attended streams a = cif_attended, b = dec_attended (model.py:351: merged = cif_attended + dec_attended).
+// a + b (carved whether or not b is given), logits (whether or not the caller takes them), GEMM scratch for K <= 512
+struct LinArgmaxBufs { float *sum, *lg; Arena scratch{nullptr, 0}; };
+static LinArgmaxBufs lin_argmax_carve(Arena& a, int64_t rows, int vocab, int mode) {
+  LinArgmaxBufs b;
+  b.sum = a.take<float>((size_t)rows * 512);
+  b.lg = a.take<float>((size_t)rows * vocab);
+  if (mode != FA_GEMM_F32_SIMT) b.scratch = a.sub(gemm_tc_scratch_bytes(rows, 512, mode));
+  return b;
+}
+
 extern "C" size_t fa_linear_argmax_workspace_bytes(int64_t rows, int32_t vocab, int32_t gemm_mode) {
-  ArenaSizer s;
-  s.take((size_t)rows * 512 * 4);
-  s.take((size_t)rows * vocab * 4);
-  s.take(gemm_tc_scratch_bytes(rows, 512, gemm_mode));
-  return s.off + 256;
+  Arena m = Arena::measuring();
+  lin_argmax_carve(m, rows, vocab, gemm_mode);
+  return m.bytes();
 }
 
 __global__ void add_rows_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ o, int64_t n4) {
@@ -670,32 +648,36 @@ extern "C" int fa_linear_argmax(const FaLinear* lin, const float* a, const float
   cudaStream_t st = (cudaStream_t)stream;
   const int V = lin->out_f, K = lin->in_f;
   Arena ar(workspace, ws_bytes);
-  float* sum = ar.take<float>((size_t)rows * 512);
-  float* lg = ar.take<float>((size_t)rows * V);
-  const size_t sb = gemm_tc_scratch_bytes(rows, 512, gemm_mode);
-  char* sp = ar.take<char>(sb);
+  LinArgmaxBufs w = lin_argmax_carve(ar, rows, V, gemm_mode);
   if (!ar.ok()) return FA_ERR_WORKSPACE;
-  Arena scratch(sp, sb);
   const float* x = a;
   if (b_or_null) {
     const int64_t n4 = rows * (K / 4);
-    add_rows_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>(a, b_or_null, sum, n4);
+    add_rows_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>(a, b_or_null, w.sum, n4);
     FA_CHECK_LAUNCH();
-    x = sum;
+    x = w.sum;
   }
-  if (logp) lg = logp;
-  FA_RETURN_IF_ERR(linear(x, K, rows, *lin, 0, nullptr, 0, nullptr, 0, lg, V, gemm_mode, &scratch, st));
+  float* lg = logp ? logp : w.lg;
+  FA_RETURN_IF_ERR(linear(x, K, rows, *lin, 0, nullptr, 0, nullptr, 0, lg, V, gemm_mode, &w.scratch, st));
   return argmax_lse_launch(lg, rows, V, V, ids, best_logp, logp ? 1 : 0, st);
 }
 
 // ------------------------------------------------------------------------------------------ CTC greedy head
+// internal logits rows are pitched to a multiple of 4 floats (25055 -> 25056) so the GEMM epilogue and the arg-max sweep use
+// 16-byte accesses (carved whether or not the caller takes the log-probs), best log-probs, GEMM scratch for K <= 512
+struct CtcBufs { float *lg, *best; Arena scratch{nullptr, 0}; };
+static CtcBufs ctc_carve(Arena& a, int64_t M, int vocab, int mode) {
+  CtcBufs b;
+  b.lg = a.take<float>(M * (size_t)((vocab + 3) & ~3));
+  b.best = a.take<float>(M);
+  if (mode != FA_GEMM_F32_SIMT) b.scratch = a.sub(gemm_tc_scratch_bytes(M, 512, mode));
+  return b;
+}
+
 extern "C" size_t fa_ctc_greedy_workspace_bytes(int32_t batch, int32_t t_max, int32_t vocab, int32_t gemm_mode) {
-  const int64_t M = (int64_t)batch * t_max;
-  ArenaSizer s;
-  s.take(M * (size_t)((vocab + 3) & ~3) * 4);
-  s.take(M * 4ull);
-  s.take(gemm_tc_scratch_bytes(M, 512, gemm_mode));
-  return s.off + 256;
+  Arena m = Arena::measuring();
+  ctc_carve(m, (int64_t)batch * t_max, vocab, gemm_mode);
+  return m.bytes();
 }
 
 extern "C" int fa_ctc_greedy_forward(const FaLinear* ctc_lo, const float* enc, const int32_t* lens, int32_t batch,
@@ -706,22 +688,22 @@ extern "C" int fa_ctc_greedy_forward(const FaLinear* ctc_lo, const float* enc, c
   const int64_t M = (int64_t)batch * t_max;
   const int V = ctc_lo->out_f;
   Arena a(workspace, ws_bytes);
-  // internal logits rows are pitched to a multiple of 4 floats (25055 -> 25056) so the GEMM epilogue and the arg-max sweep use
-  // 16-byte accesses; a caller-provided log-prob tensor keeps the dense [M, V] layout
-  const int64_t ldv = logp ? V : ((V + 3) & ~3);
-  float* lg = a.take<float>(M * (size_t)((V + 3) & ~3));
-  float* best = a.take<float>(M);
-  const size_t sb = gemm_tc_scratch_bytes(M, 512, gemm_mode);
-  char* sp = a.take<char>(sb);
+  CtcBufs w = ctc_carve(a, M, V, gemm_mode);
   if (!a.ok()) return FA_ERR_WORKSPACE;
-  Arena scratch(sp, sb);
-  if (logp) lg = logp;
-  FA_RETURN_IF_ERR(linear(enc, ctc_lo->in_f, M, *ctc_lo, 0, nullptr, 0, nullptr, 0, lg, ldv, gemm_mode, &scratch, st));
-  FA_RETURN_IF_ERR(argmax_lse_launch(lg, M, V, ldv, argmax_ids, best, logp ? 1 : 0, st));
+  // a caller-provided log-prob tensor keeps the dense [M, V] layout
+  const int64_t ldv = logp ? V : ((V + 3) & ~3);
+  float* lg = logp ? logp : w.lg;
+  FA_RETURN_IF_ERR(linear(enc, ctc_lo->in_f, M, *ctc_lo, 0, nullptr, 0, nullptr, 0, lg, ldv, gemm_mode, &w.scratch, st));
+  FA_RETURN_IF_ERR(argmax_lse_launch(lg, M, V, ldv, argmax_ids, w.best, logp ? 1 : 0, st));
   return ctc_filter_launch(argmax_ids, lens, batch, t_max, blank, out_ids, out_lens, st);
 }
 
 // ------------------------------------------------------------------------------------------ op-level + info
+extern "C" size_t fa_linear_workspace_bytes(int64_t rows, int32_t in_f, int32_t gemm_mode) {
+  if (rows < 0 || in_f <= 0) return 0;
+  return gemm_tc_scratch_bytes(rows, in_f, gemm_mode);
+}
+
 extern "C" int fa_linear(const float* x, int64_t ldx, int64_t rows, const FaLinear* lin, int32_t relu, const float* res1,
                          int64_t ld_res1, const float* res2, int64_t ld_res2, float* y, int64_t ldy, int32_t gemm_mode,
                          void* workspace, size_t ws_bytes, fa_stream_t stream) {
@@ -765,7 +747,7 @@ extern "C" int fa_linear_attn_sinks(const void* a_planes, int64_t rows, const Fa
   if (n_on == 0) return FA_ERR_ARG;
   if (v0 >= 0 && t_pad < t_rows) return FA_ERR_ARG;
   if (v_f32 && (v0 < 0 || ld_v_f32 < N)) return FA_ERR_ARG;       // fp32 V rows are the GEMM's output rows: columns [v0, v0 + width)
-  const int npl = gemm_mode == FA_GEMM_F16X1 ? 1 : 2;
+  const int npl = attn_planes(gemm_mode);
   AttnSinks sk;
   if (q0 >= 0) sk.q0 = q0;
   if (k0 >= 0) sk.k0 = k0;

@@ -48,22 +48,34 @@ frame_decibel_kernel(const float* __restrict__ wav, int frames, float* __restric
 
 static inline int pad16(int k) { return (k + 15) / 16 * 16; }
 
+// Activations at their padded widths, then the metadata.  The order matters: the forward zeroes a1 .. meta as one range.
+struct VadBufs {
+  float *a1, *h0, *h1, *q, *qm, *o1, *lg;
+  int32_t* meta;   // [0] = t (lens of the single "utterance"), [4..8) = silence ids
+};
+static VadBufs vad_carve(Arena& a, const FaVadEncoder* enc, int t) {
+  const int Ap = pad16(enc->in1.out_f), Lp = pad16(enc->in2.out_f), Op = pad16(enc->out1.out_f), Vp = pad16(enc->out2.out_f);
+  VadBufs b;
+  b.a1 = a.take<float>((size_t)t * Ap);
+  b.h0 = a.take<float>((size_t)t * Lp);
+  b.h1 = a.take<float>((size_t)t * Lp);
+  b.q = a.take<float>((size_t)t * 128);
+  b.qm = a.take<float>((size_t)t * 128);
+  b.o1 = a.take<float>((size_t)t * Op);
+  b.lg = a.take<float>((size_t)t * Vp);
+  b.meta = a.take<int32_t>(16);
+  return b;
+}
+
 }  // namespace fa
 
 using namespace fa;
 
 extern "C" size_t fa_fsmn_vad_workspace_bytes(const FaVadEncoder* enc, int32_t t) {
   if (!enc || t <= 0) return 0;
-  ArenaSizer s;
-  s.take((size_t)t * pad16(enc->in1.out_f) * 4);
-  s.take((size_t)t * pad16(enc->in2.out_f) * 4);
-  s.take((size_t)t * pad16(enc->in2.out_f) * 4);
-  s.take((size_t)t * 128 * 4);
-  s.take((size_t)t * 128 * 4);
-  s.take((size_t)t * pad16(enc->out1.out_f) * 4);
-  s.take((size_t)t * pad16(enc->out2.out_f) * 4);
-  s.take(256);
-  return s.off + 256;
+  Arena m = Arena::measuring();
+  vad_carve(m, enc, t);
+  return m.bytes();
 }
 
 extern "C" int fa_fsmn_vad_forward(const FaVadEncoder* enc, const float* feats, int64_t ld_feats, int32_t t, float* sil_prob,
@@ -75,15 +87,10 @@ extern "C" int fa_fsmn_vad_forward(const FaVadEncoder* enc, const float* feats, 
   // every GEMM reads K = the previous layer's PADDED width (zero columns in the activations, zero columns in the packed weights)
   if (enc->in1.in_f % 16 || enc->in2.in_f != Ap || enc->out1.in_f != Lp || enc->out2.in_f != Op) return FA_ERR_UNSUPPORTED;
   Arena a(workspace, ws_bytes);
-  float* a1 = a.take<float>((size_t)t * Ap);
-  float* h0 = a.take<float>((size_t)t * Lp);
-  float* h1 = a.take<float>((size_t)t * Lp);
-  float* q = a.take<float>((size_t)t * 128);
-  float* qm = a.take<float>((size_t)t * 128);
-  float* o1 = a.take<float>((size_t)t * Op);
-  float* lg = a.take<float>((size_t)t * Vp);
-  int32_t* meta = a.take<int32_t>(16);                     // [0] = t (lens of the single "utterance"), [4..8) = silence ids
+  const VadBufs b = vad_carve(a, enc, t);
   if (!a.ok()) return FA_ERR_WORKSPACE;
+  float *a1 = b.a1, *h0 = b.h0, *h1 = b.h1, *q = b.q, *qm = b.qm, *o1 = b.o1, *lg = b.lg;
+  int32_t* meta = b.meta;
   FA_CUDA_OK(cudaMemsetAsync(a1, 0, (size_t)((char*)meta - (char*)a1), st));      // padded columns must read as zero
   int32_t host_meta[16] = {0};
   host_meta[0] = t;

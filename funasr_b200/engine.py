@@ -218,7 +218,7 @@ class _EngineBase:
         B, T, D = enc.shape
         U = self.up_times
         up = torch.empty((B, T * U, D), dtype=torch.float32, device=self.device)
-        ws = self._workspace(max(8 * B * T * U * D * 4, 1 << 20))
+        ws = self._workspace(self.lib.fa_linear_workspace_bytes(B * T * U, D, self.mode))     # the larger of the two calls
         _abi.check(self.lib.fa_linear(enc.data_ptr(), D, B * T, C.byref(self.up_lin), 0, None, 0, None, 0, up.data_ptr(), U * D, self.mode,
                                       ws.data_ptr(), ws.numel(), self._stream()), "fa_linear(upsample_cnn)")
         xproj = torch.empty((B * T * U, 8 * D), dtype=torch.float32, device=self.device)

@@ -4,7 +4,9 @@
  * Every entry point takes plain device pointers, sizes and a CUDA stream (as void*); no torch / C++
  * types cross the boundary.  All functions are stream-ordered, re-entrant, hold no global state, never
  * synchronise the device, and return FA_OK (0) or a negative FaStatus.  The caller owns every buffer
- * (inputs, outputs, workspace); weights are borrowed pointers.
+ * (inputs, outputs, workspace); weights are borrowed pointers.  An entry point that takes a workspace has a *_workspace_bytes
+ * (or *_scratch_bytes) query: it returns exactly the bytes the forward carves for the path its arguments select, and a workspace
+ * of that size is enough.  A smaller one returns FA_ERR_WORKSPACE before any work is enqueued.
  *
  * Each entry point names the reference interface it replaces (paths relative to the FunASR tree,
  * commit 3c58cb5 / funasr 1.4.3).  The tensor-level operator boundary mirrors the reference's own
@@ -195,6 +197,8 @@ int fa_layernorm_planes(const float* x, int64_t rows, const FaNorm* norm, float*
 int fa_linear(const float* x, int64_t ldx, int64_t rows, const FaLinear* lin, int32_t relu,
               const float* res1, int64_t ld_res1, const float* res2, int64_t ld_res2,
               float* y, int64_t ldy, int32_t gemm_mode, void* workspace, size_t ws_bytes, fa_stream_t stream);
+/* fa_linear's workspace: the fp16 planes of x for rows x in_f (in_pad = in_f rounded up to 64); 0 for FA_GEMM_F32_SIMT. */
+size_t fa_linear_workspace_bytes(int64_t rows, int32_t in_f, int32_t gemm_mode);
 
 /* The tensor-core GEMM alone, A operand already split into fp16 planes [npl][rows][lin->in_pad] (npl = 1 / 2 / 3 for
  * F16X1 / X3 / X6) by fa_split_rows: what the model-level calls launch between fused producers and consumers. */
@@ -254,7 +258,7 @@ int fa_attention(const float* q, int64_t ldq, const float* k, int64_t ldk, const
 
 /* Same contract on the tensor cores (wgmma; fp16 operand planes, fp32 accumulation in registers):
  * gemm_mode FA_GEMM_F16X1 (one plane) or FA_GEMM_F16X3/X6 (hi+lo planes, three MMA terms).  workspace holds the
- * operand planes (size from fa_attention_tc_workspace_bytes). */
+ * operand planes (size from fa_attention_tc_workspace_bytes, exactly what the call carves). */
 size_t fa_attention_tc_workspace_bytes(int32_t batch, int32_t heads, int32_t tq, int32_t tk, int32_t gemm_mode);
 int fa_attention_tc(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
                     const int32_t* key_lens, int32_t batch, int32_t heads, int32_t tq, int32_t tk,
@@ -286,7 +290,8 @@ int fa_attention_f32_ex(const float* q, int64_t ldq, const float* k, int64_t ldk
 /* SANMEncoder.forward (encoder.py:392-461): feats [B,T,560], lens[B] -> enc [B,T,512].
  * If enc->pe_inv_timescales == NULL the struct describes a plain stack of 512->512 SAN-M layers applied to an
  * existing [B,T,512] stream (no x*sqrt(d)+PE, every layer has its residual): SenseVoiceEncoderSmall's `tp_encoders`
- * + `tp_norm` (sense_voice/model.py:650-655). */
+ * + `tp_norm` (sense_voice/model.py:650-655).
+ * Workspace: sized for d_model <= 512, input <= 560 and FFN <= 2048; exactly what the forward carves for gemm_mode. */
 size_t fa_sanm_encoder_workspace_bytes(int32_t batch, int32_t t_max, int32_t gemm_mode);
 int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats, const int32_t* lens, int32_t batch,
                             int32_t t_max, float* out, int32_t gemm_mode, void* workspace, size_t ws_bytes,
@@ -296,7 +301,9 @@ int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats, const int3
  * :853-908).  enc [B,T,512], lens[B] ->
  *   acoustic [B, n_cap, 512] (rows >= fires zero-filled; n_cap >= 1, tokens beyond n_cap are dropped),
  *   token_num [B] int32 (= floor(sum alpha'), the reference's pre_token_length),
- *   alphas [B, T+1], peaks [B, T+1] (cif_peak / "fires"). */
+ *   alphas [B, T+1], peaks [B, T+1] (cif_peak / "fires").
+ * The tensor-core modes need conv.in_pad == 1536 (FA_ERR_UNSUPPORTED otherwise).  The workspace query returns exactly what the
+ * forward carves for gemm_mode. */
 size_t fa_cif_predictor_workspace_bytes(int32_t batch, int32_t t_max, int32_t gemm_mode);
 int fa_cif_predictor_forward(const FaPredictor* pred, const float* enc, const int32_t* lens, int32_t batch,
                              int32_t t_max, float* acoustic, int32_t n_cap, int32_t* token_num, float* alphas,
@@ -333,8 +340,9 @@ int fa_blstm_forward_tc(const float* xproj, const float* w_hh_fwd, const float* 
  *   tok_lens[B].  Outputs: argmax_ids [B, n_max] int32, argmax_logp [B, n_max] (log-softmax value of the
  *   arg-max, :643), and — if logits != NULL — the full pre-softmax logits [B, n_max, vocab].
  *   If log_softmax != 0 the logits buffer is converted in place to log_softmax (model.py:345). */
-/* Workspace size: n_hotwords is the number of entries in the hotword memory of a contextual decoder (FaDecoder.has_bias), 0 for
- * a plain one. */
+/* Workspace size, exactly what the forward carves: n_hotwords is the number of entries in the hotword memory of a contextual
+ * decoder (FaDecoder.has_bias), 0 for a plain one.  The logits slice is always counted (the query cannot see whether the caller
+ * passes logits). */
 size_t fa_paraformer_decoder_workspace_bytes_hw(int32_t batch, int32_t t_max, int32_t n_max, int32_t vocab,
                                                 int32_t gemm_mode, int32_t n_hotwords);
 int fa_paraformer_decoder_forward(const FaDecoder* dec, const float* enc, const int32_t* enc_lens, int32_t batch,
@@ -359,7 +367,9 @@ int fa_paraformer_decoder_forward_hidden(const FaDecoder* dec, const float* enc,
  *   n_run attention layers are run (<= dec->n_layers), then
  *     finish != 0     : decoders3 + after_norm -> hidden [B, n_max, 512]  (ParaformerSANMDecoder.forward, decoder.py:397-449)
  *     attn_probs != 0 : layer n_run-1 stops at its cross-attention and writes utterance 0's probability matrix
- *                       [heads, n_max, t_mem] (forward_asf6 / get_attn_mat, decoder.py:485-513, :123-146); hidden untouched. */
+ *                       [heads, n_max, t_mem] (forward_asf6 / get_attn_mat, decoder.py:485-513, :123-146); hidden untouched.
+ * The workspace query returns exactly what the forward carves; it counts the attn_probs path and a per-utterance memory, which
+ * cover every call. */
 size_t fa_sanm_decoder_stack_workspace_bytes(int32_t batch, int32_t t_mem, int32_t n_max, int32_t gemm_mode);
 int fa_sanm_decoder_stack_forward(const FaDecoder* dec, const float* memory, const int32_t* mem_lens, int32_t mem_shared,
                                   int32_t batch, int32_t t_mem, const float* x, int64_t ld_x_rows, const int32_t* tok_lens,
@@ -367,7 +377,9 @@ int fa_sanm_decoder_stack_forward(const FaDecoder* dec, const float* memory, con
                                   int32_t gemm_mode, void* workspace, size_t ws_bytes, fa_stream_t stream);
 
 /* ids / best_logp [rows] = arg-max and its log-softmax value of (a (+ b)) W^T + bias — SeACo's hotword_output_layer over
- * cif_attended + dec_attended (seaco_paraformer/model.py:351-355); logp != NULL receives the full log-softmax rows [rows, out_f]. */
+ * cif_attended + dec_attended (seaco_paraformer/model.py:351-355); logp != NULL receives the full log-softmax rows [rows, out_f].
+ * The workspace query returns exactly what the forward carves, counting the a + b rows and the logits whether or not b and logp
+ * are given. */
 size_t fa_linear_argmax_workspace_bytes(int64_t rows, int32_t vocab, int32_t gemm_mode);
 int fa_linear_argmax(const FaLinear* lin, const float* a, const float* b_or_null, int64_t rows, int32_t* ids, float* best_logp,
                      float* logp, int32_t gemm_mode, void* workspace, size_t ws_bytes, fa_stream_t stream);
@@ -437,7 +449,8 @@ int fa_greedy_filter(const int32_t* argmax_ids, const int32_t* tok_lens, int32_t
 /* CTC greedy head of SenseVoiceSmall (sense_voice/model.py:1003-1025, ctc/ctc.py:192-203): logits = enc W^T + b,
  * log_softmax, arg-max per frame, torch.unique_consecutive, drop blank.
  *   enc [B,T,512], lens[B] -> out_ids [B,T] (padded with -1), out_lens [B]; if logp != NULL it receives the
- *   full log_softmax [B,T,vocab] (parity checks); argmax_ids [B,T] is scratch/diagnostic output. */
+ *   full log_softmax [B,T,vocab] (parity checks); argmax_ids [B,T] is scratch/diagnostic output.  The workspace query returns
+ *   exactly what the forward carves, counting the logits whether or not logp is given. */
 size_t fa_ctc_greedy_workspace_bytes(int32_t batch, int32_t t_max, int32_t vocab, int32_t gemm_mode);
 int fa_ctc_greedy_forward(const FaLinear* ctc_lo, const float* enc, const int32_t* lens, int32_t batch, int32_t t_max,
                           int32_t blank, int32_t* argmax_ids, int32_t* out_ids, int32_t* out_lens, float* logp,

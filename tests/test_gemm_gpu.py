@@ -319,7 +319,7 @@ def test_int_linear_split_then_gemm_bit_exact(lib, case, mode):
     b = _bias(g, N)
     r1 = torch.randn(M, N, generator=g, device=DEV)
     lin = _lin(abi, W, b, N, in_f, in_pad)
-    ws = torch.empty(NPL[mode] * M * in_pad * 2 + 1024, dtype=torch.uint8, device=DEV)
+    ws = torch.empty(L.fa_linear_workspace_bytes(M, in_f, abi.GEMM_MODES[mode]), dtype=torch.uint8, device=DEV)
     y = torch.full((M, N), NAN, device=DEV)
     assert L.fa_linear(x.data_ptr(), ldx, M, C.byref(lin), 1, r1.data_ptr(), N, None, 0, y.data_ptr(), N, abi.GEMM_MODES[mode],
                        ws.data_ptr(), ws.numel(), _st()) == 0
@@ -380,7 +380,7 @@ def test_gemm_empty_and_status(lib):
     out = torch.full((3, M, N + 8), NAN, dtype=F16, device=DEV)
     lin = _lin(abi, W, b, N, Kp, Kp)
     x3 = abi.GEMM_F16X3
-    ws = torch.empty(3 * M * Kp * 2 + 1024, dtype=torch.uint8, device=DEV)
+    ws = torch.empty(L.fa_linear_workspace_bytes(M, Kp, x3), dtype=torch.uint8, device=DEV)
     xf = torch.zeros(M, Kp, device=DEV)
     # empty
     assert L.fa_linear_planes(A.data_ptr(), 0, C.byref(lin), 0, None, 0, None, 0, y.data_ptr(), N, x3, _st()) == 0
@@ -475,7 +475,7 @@ def test_conv_view_gemm(lib, case, mode):
     y = torch.full((rows, N + 4), NAN, device=DEV)
     assert L.fa_linear_planes_view(planes.data_ptr(), rows, a_ld, apr, C.byref(lin), 1, y.data_ptr(), N + 4, gm, _st()) == 0
     # the same rows materialised by the split pass (fa_linear with ldx = a_ld < in_f): same products, same order
-    ws = torch.empty(npl * rows * kp * 2 + 1024, dtype=torch.uint8, device=DEV)
+    ws = torch.empty(L.fa_linear_workspace_bytes(rows, kp, gm), dtype=torch.uint8, device=DEV)
     y2 = torch.full((rows, N), NAN, device=DEV)
     assert L.fa_linear(padd.data_ptr(), a_ld, rows, C.byref(lin), 1, None, 0, None, 0, y2.data_ptr(), N, gm, ws.data_ptr(), ws.numel(),
                        _st()) == 0
