@@ -376,8 +376,7 @@ static bool cam_shapes(const FaCampplus* m, int batch, int T, CamShapes* s) {
 struct CamBufs {
   float *x80, *x40a, *x40b, *x40c, *pad, *tdnn, *buf[3], *h, *gates, *op, *stats;
   plane_t *pad_planes, *op_planes;
-  char* scratch;
-  size_t scratch_bytes;
+  Arena scratch{nullptr, 0};   // the dense layer's GEMM
 };
 
 static void cam_carve(Arena& a, const CamShapes& s, int mode, CamBufs* out) {
@@ -398,8 +397,7 @@ static void cam_carve(Arena& a, const CamShapes& s, int mode, CamBufs* out) {
   out->op = tc ? nullptr : a.take<float>(s.rows * cmax);
   out->pad_planes = tc ? a.take<plane_t>((size_t)npl * s.pad_rows * 320) : nullptr;
   out->op_planes = tc ? a.take<plane_t>((size_t)npl * s.rows * ((cmax + 63) / 64 * 64)) : nullptr;
-  out->scratch_bytes = tc ? gemm_tc_scratch_bytes(s.B, 1024, mode) : 0;
-  out->scratch = tc ? a.take<char>(out->scratch_bytes) : nullptr;
+  if (tc) out->scratch = a.sub(gemm_tc_scratch_bytes(s.B, 1024, mode));
 }
 
 // y[rows, out_f] (ldy) = act(A W^T + b) with A = relu(x[:, :in_f] * scale + shift) (fp32 rows or fp16 planes)
@@ -407,10 +405,10 @@ static int bn_relu_linear(const float* x, int64_t ldx, int64_t rows, const float
                           int relu, float* y, int64_t ldy, int mode, const CamBufs& bf, cudaStream_t st) {
   if (mode == FA_GEMM_F32_SIMT) {
     FA_RETURN_IF_ERR(bn_relu_launch(x, ldx, rows, lin.in_f, lin.in_f, scale, shift, bf.op, nullptr, 0, st));
-    return gemm_f32_launch(bf.op, lin.in_f, rows, lin.w, lin.out_f, lin.in_f, lin.b, relu, nullptr, 0, nullptr, 0, y, ldy, st);
+    return gemm_f32_launch(bf.op, lin.in_f, rows, lin.w, lin.out_f, lin.in_f, lin.b, GemmEpi().relu(relu).to(y, ldy), st);
   }
   FA_RETURN_IF_ERR(bn_relu_launch(x, ldx, rows, lin.in_f, lin.in_pad, scale, shift, nullptr, bf.op_planes, gemm_planes(mode), st));
-  return gemm_tc_planes_launch(bf.op_planes, rows, lin, relu, nullptr, 0, nullptr, 0, y, ldy, nullptr, 0, mode, st);
+  return gemm_tc_planes_launch(bf.op_planes, rows, lin, GemmEpi().relu(relu).to(y, ldy), mode, st);
 }
 
 static int campplus_forward(const FaCampplus* m, const float* feats, int batch, int T, float* emb, int mode, void* ws, size_t ws_bytes,
@@ -451,11 +449,10 @@ static int campplus_forward(const FaCampplus* m, const float* feats, int batch, 
   // TDNN: Conv1d(320 -> 128, k 5, stride 2, pad 2) + folded BN + ReLU as one GEMM over the overlapping view (row pitch 640)
   const int64_t Mt = (int64_t)B * (s.P / 2);
   if (!tc) {
-    FA_RETURN_IF_ERR(gemm_f32_launch(bf.pad, 640, Mt, m->tdnn.w, kCamBn, 1600, m->tdnn.b, 1, nullptr, 0, nullptr, 0, bf.tdnn, kCamBn, st));
+    FA_RETURN_IF_ERR(gemm_f32_launch(bf.pad, 640, Mt, m->tdnn.w, kCamBn, 1600, m->tdnn.b, GemmEpi().relu().to(bf.tdnn, kCamBn), st));
   } else {
     FA_RETURN_IF_ERR(split_rows_launch(bf.pad, 320, s.pad_rows, 320, 320, gemm_planes(mode), bf.pad_planes, st));
-    FA_RETURN_IF_ERR(gemm_tc_planes_launch(bf.pad_planes, Mt, m->tdnn, 1, nullptr, 0, nullptr, 0, bf.tdnn, kCamBn, nullptr, 0, mode, st,
-                                           nullptr, 640, s.pad_rows / 2));
+    FA_RETURN_IF_ERR(gemm_tc_planes_launch(bf.pad_planes, Mt, m->tdnn, GemmEpi().relu().to(bf.tdnn, kCamBn), mode, st, 640, s.pad_rows / 2));
   }
   {
     const int64_t total = s.rows * (kCamBn / 4);
@@ -484,11 +481,7 @@ static int campplus_forward(const FaCampplus* m, const float* feats, int batch, 
   const int c_out = s.c_final[2] / 2;
   if (2 * c_out != m->dense.in_f) return FA_ERR_ARG;
   FA_RETURN_IF_ERR(stats_launch(bf.buf[0], B, s.t_out, c_out, m->out_scale, m->out_shift, bf.stats, st));
-  if (!tc)
-    return gemm_f32_launch(bf.stats, 2 * c_out, B, m->dense.w, m->dense.out_f, 2 * c_out, m->dense.b, 0, nullptr, 0, nullptr, 0, emb,
-                           m->dense.out_f, st);
-  Arena scratch(bf.scratch, bf.scratch_bytes);
-  return gemm_tc_launch(bf.stats, 2 * c_out, B, m->dense, 0, nullptr, 0, nullptr, 0, emb, m->dense.out_f, mode, &scratch, st);
+  return gemm_rows(bf.stats, 2 * c_out, B, m->dense, GemmEpi().to(emb, m->dense.out_f), mode, &bf.scratch, st);
 }
 
 }  // namespace fa

@@ -5,6 +5,7 @@
 // The tensor-core path (gemm_tc.cu) is validated against it on the device.
 // 128x128x16 tiles, 256 threads, 8x8 outputs per thread, register-prefetch double buffering.
 #include "common.cuh"
+#include "kernels.h"
 
 namespace fa {
 
@@ -98,14 +99,12 @@ gemm_f32_kernel(const float* __restrict__ A, int64_t lda, const float* __restric
   }
 }
 
-int gemm_f32_launch(const float* A, int64_t lda, int64_t M, const float* W, int N, int K, const float* bias, int relu,
-                    const float* r1, int64_t ldr1, const float* r2, int64_t ldr2, float* C, int64_t ldc,
-                    cudaStream_t st) {
+int gemm_f32_launch(const float* A, int64_t lda, int64_t M, const float* W, int N, int K, const float* bias, const GemmEpi& epi, cudaStream_t st) {
   if (M <= 0 || N <= 0) return FA_OK;
-  if (!A || !W || !C) return FA_ERR_ARG;
+  if (!A || !W || !epi.y || epi.planes || epi.att) return FA_ERR_ARG;
   if (K % BK != 0 || lda % 4 != 0 || (((uintptr_t)A) & 15) || (((uintptr_t)W) & 15)) return FA_ERR_UNSUPPORTED;
   dim3 grid((N + BN - 1) / BN, (unsigned)((M + BM - 1) / BM));
-  gemm_f32_kernel<<<grid, 256, 0, st>>>(A, lda, W, K, bias, relu, r1, ldr1, r2, ldr2, C, ldc, M, N, K);
+  gemm_f32_kernel<<<grid, 256, 0, st>>>(A, lda, W, K, bias, epi.relu_on, epi.r1, epi.ld1, epi.r2, epi.ld2, epi.y, epi.ldy, M, N, K);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }

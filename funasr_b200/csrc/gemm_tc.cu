@@ -655,7 +655,7 @@ int make_plane_map(CUtensorMap* m, const void* base, uint64_t rows, uint64_t col
   return FA_OK;
 }
 
-// gemm_tc_launch's scratch: the fp16 planes of the fp32 A operand (none on the fp32 SIMT path, which takes no scratch)
+// gemm_rows' scratch: the fp16 planes of the fp32 A operand (none on the fp32 SIMT path, which takes no scratch)
 static plane_t* gemm_carve(Arena& a, int64_t rows, int k_pad, int mode) {
   return mode == FA_GEMM_F32_SIMT ? nullptr : a.take<plane_t>((size_t)gemm_planes(mode) * rows * k_pad);
 }
@@ -694,9 +694,8 @@ static int launch_cfg(const CUtensorMap& ma, const CUtensorMap& mw, const TcPara
 }
 
 // A planes already split: a_planes [npl][M][Kp]
-int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& lin, int relu, const float* r1, int64_t ld1,
-                          const float* r2, int64_t ld2, float* y, int64_t ldy, plane_t* out_planes, int64_t ldo,
-                          int mode, cudaStream_t st, const AttnSinks* att, int64_t a_ld, int64_t a_plane_rows) {
+int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& lin, const GemmEpi& epi, int mode, cudaStream_t st,
+                          int64_t a_ld, int64_t a_plane_rows) {
   if (M <= 0) return FA_OK;
   const uint64_t lda = a_ld > 0 ? (uint64_t)a_ld : (uint64_t)lin.in_pad;          // A row pitch (overlapping view: < K_pad)
   const int64_t apr = a_plane_rows > 0 ? a_plane_rows : M;                         // rows between consecutive A planes
@@ -705,12 +704,12 @@ int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& li
   const int N = lin.out_f, Kp = lin.in_pad;
   if (N <= 0) return FA_ERR_ARG;
   if (Kp % TC_BK != 0 || M * 3 > 0x7fffffffLL) return FA_ERR_UNSUPPORTED;
-  if (y && (ldy & 3) == 0 && (((uintptr_t)y) & 15)) return FA_ERR_UNSUPPORTED;
-  if ((r1 && (ld1 & 3)) || (r2 && (ld2 & 3))) return FA_ERR_UNSUPPORTED;
+  if (epi.y && (epi.ldy & 3) == 0 && (((uintptr_t)epi.y) & 15)) return FA_ERR_UNSUPPORTED;
+  if ((epi.r1 && (epi.ld1 & 3)) || (epi.r2 && (epi.ld2 & 3))) return FA_ERR_UNSUPPORTED;
   // the epilogue reads bias and residual rows as float4 and writes output planes as uint2 (store_planes4)
-  if ((lin.b && (((uintptr_t)lin.b) & 15)) || (r1 && (((uintptr_t)r1) & 15)) || (r2 && (((uintptr_t)r2) & 15))) return FA_ERR_UNSUPPORTED;
-  if (out_planes && ((ldo & 3) || (((uintptr_t)out_planes) & 7))) return FA_ERR_UNSUPPORTED;
-  if ((y && ldy < N) || (r1 && ld1 < N) || (r2 && ld2 < N) || (out_planes && ldo < N)) return FA_ERR_ARG;
+  if ((lin.b && (((uintptr_t)lin.b) & 15)) || (epi.r1 && (((uintptr_t)epi.r1) & 15)) || (epi.r2 && (((uintptr_t)epi.r2) & 15))) return FA_ERR_UNSUPPORTED;
+  if (epi.planes && ((epi.ldp & 3) || (((uintptr_t)epi.planes) & 7))) return FA_ERR_UNSUPPORTED;
+  if ((epi.y && epi.ldy < N) || (epi.r1 && epi.ld1 < N) || (epi.r2 && epi.ld2 < N) || (epi.planes && epi.ldp < N)) return FA_ERR_ARG;
   const int npl = gemm_planes(mode);
   // 128 x 128 tiles with a 6 (x1) / 3 (x3) stage ring; 128 x 64 for x6 (three planes per operand: two 72 KB stages, a third does
   // not fit beside the epilogue staging in 227 KB).
@@ -725,13 +724,13 @@ int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& li
   TcParams p;
   p.M = M; p.N = N; p.Kp = Kp; p.a_plane_rows = apr; p.w_plane_rows = N;
   p.n_terms = mode == FA_GEMM_F16X1 ? 1 : (mode == FA_GEMM_F16X3 ? 3 : 6);
-  p.relu = relu; p.bias = lin.b; p.r1 = r1; p.ldr1 = ld1; p.r2 = r2; p.ldr2 = ld2; p.C = y; p.ldc = ldy;
-  p.out_planes = out_planes; p.ldo = ldo; p.out_nplanes = npl;
+  p.relu = epi.relu_on; p.bias = lin.b; p.r1 = epi.r1; p.ldr1 = epi.ld1; p.r2 = epi.r2; p.ldr2 = epi.ld2; p.C = epi.y; p.ldc = epi.ldy;
+  p.out_planes = epi.planes; p.ldo = epi.ldp; p.out_nplanes = npl;
   p.tiles_m = (int)((M + TC_BM - 1) / TC_BM); p.tiles_n = (N + BN - 1) / BN;
   p.acc_scale = rz_comp_scale(Kp, p.n_terms);
-  if (att) { p.att = *att; p.att.enabled = 1; } else { p.att = AttnSinks{}; }
-  if (att && (N % 32 != 0 || att->width % 32 != 0 || att->t_rows <= 0 || M % att->t_rows != 0)) return FA_ERR_UNSUPPORTED;
-  if (out_planes && (N % 32 != 0)) return FA_ERR_UNSUPPORTED;
+  if (epi.att) { p.att = *epi.att; p.att.enabled = 1; } else { p.att = AttnSinks{}; }
+  if (epi.att && (N % 32 != 0 || epi.att->width % 32 != 0 || epi.att->t_rows <= 0 || M % epi.att->t_rows != 0)) return FA_ERR_UNSUPPORTED;
+  if (epi.planes && (N % 32 != 0)) return FA_ERR_UNSUPPORTED;
   switch (npl) {
     case 1: return launch_cfg<128, 6, 1, 1>(ma, mw, p, st);
     case 2: return launch_cfg<128, 3, 2, 2>(ma, mw, p, st);
@@ -749,8 +748,9 @@ int split_rows_launch(const float* x, int64_t ldx, int64_t rows, int cols, int c
   return FA_OK;
 }
 
-int gemm_tc_launch(const float* x, int64_t ldx, int64_t rows, const FaLinear& lin, int relu, const float* r1, int64_t ld1,
-                   const float* r2, int64_t ld2, float* y, int64_t ldy, int mode, Arena* scratch, cudaStream_t st) {
+int gemm_rows(const float* x, int64_t ldx, int64_t rows, const FaLinear& lin, const GemmEpi& epi, int mode, Arena* scratch, cudaStream_t st) {
+  if (!lin.w) return FA_ERR_ARG;
+  if (mode == FA_GEMM_F32_SIMT) return gemm_f32_launch(x, ldx, rows, lin.w, lin.out_f, lin.in_f, lin.b, epi, st);
   if (rows <= 0) return FA_OK;
   if (mode != FA_GEMM_F16X1 && mode != FA_GEMM_F16X3 && mode != FA_GEMM_F16X6) return FA_ERR_ARG;
   if (!scratch) return FA_ERR_WORKSPACE;
@@ -758,7 +758,7 @@ int gemm_tc_launch(const float* x, int64_t ldx, int64_t rows, const FaLinear& li
   plane_t* planes = gemm_carve(local, rows, lin.in_pad, mode);
   if (!local.ok()) return FA_ERR_WORKSPACE;
   FA_RETURN_IF_ERR(split_rows_launch(x, ldx, rows, lin.in_f, lin.in_pad, gemm_planes(mode), planes, st));
-  return gemm_tc_planes_launch(planes, rows, lin, relu, r1, ld1, r2, ld2, y, ldy, nullptr, 0, mode, st, nullptr);
+  return gemm_tc_planes_launch(planes, rows, lin, epi, mode, st);
 }
 
 }  // namespace fa

@@ -12,14 +12,6 @@ namespace fa {
 int layernorm_launch(const float* x, int64_t rows, const FaNorm& nm, float* y, const float* pe_inv, float xscale,
                      int rows_per_batch, cudaStream_t st, plane_t* planes = nullptr, int nplanes = 0, int cols_pad = 0,
                      float* emb_out = nullptr);   // emb_out: with pe_inv, also write the embedded (pre-norm) rows there
-int gemm_f32_launch(const float* A, int64_t lda, int64_t M, const float* W, int N, int K, const float* bias, int relu,
-                    const float* r1, int64_t ldr1, const float* r2, int64_t ldr2, float* C, int64_t ldc,
-                    cudaStream_t st);
-// wgmma fp16-split GEMM (gemm_tc.cu)
-size_t gemm_tc_scratch_bytes(int64_t max_rows, int max_k, int mode);
-int gemm_tc_launch(const float* x, int64_t ldx, int64_t rows, const FaLinear& lin, int relu, const float* r1,
-                   int64_t ld1, const float* r2, int64_t ld2, float* y, int64_t ldy, int mode, Arena* scratch,
-                   cudaStream_t st);
 // Column-range sinks of a GEMM epilogue feeding the tensor-core attention (gemm_tc.cu): columns [q0, q0+width) -> q planes
 // (scaled), [k0, k0+width) -> k planes, [v0, v0+width) -> transposed v planes (+ fp32 into the GEMM's C when C != null).
 // A range is disabled by placing it outside [0, N) (e.g. -1000000).
@@ -34,6 +26,28 @@ struct AttnSinks {
   plane_t* k_planes = nullptr;   // [npl][M][width]
   plane_t* vt_planes = nullptr;  // [npl][B*width][t_pad]
 };
+// What a GEMM's epilogue does with act(A W^T + b), the bias being the FaLinear's: fp32 rows y = that (+ r1) (+ r2), and / or fp16
+// planes [nplanes][M][ldp] (the A operand of a following tensor-core GEMM), and / or the attention sinks.  A call names what it sets.
+struct GemmEpi {
+  int relu_on = 0;
+  const float* r1 = nullptr; int64_t ld1 = 0;
+  const float* r2 = nullptr; int64_t ld2 = 0;
+  float* y = nullptr; int64_t ldy = 0;
+  plane_t* planes = nullptr; int64_t ldp = 0;
+  const AttnSinks* att = nullptr;
+  GemmEpi& relu(int on = 1) { relu_on = on; return *this; }
+  GemmEpi& add(const float* r, int64_t ld, const float* r_2 = nullptr, int64_t ld_2 = 0) { r1 = r; ld1 = ld; r2 = r_2; ld2 = ld_2; return *this; }
+  GemmEpi& to(float* out, int64_t ld) { y = out; ldy = ld; return *this; }
+  GemmEpi& to(plane_t* out, int64_t ld) { planes = out; ldp = ld; return *this; }
+  GemmEpi& sinks(const AttnSinks* s) { att = s; return *this; }
+};
+// fp32 SIMT GEMM (gemm_f32.cu), K a multiple of 16; fp32 rows only (FA_ERR_ARG for planes or sinks)
+int gemm_f32_launch(const float* A, int64_t lda, int64_t M, const float* W, int N, int K, const float* bias, const GemmEpi& epi, cudaStream_t st);
+// wgmma fp16-split GEMM (gemm_tc.cu)
+size_t gemm_tc_scratch_bytes(int64_t max_rows, int max_k, int mode);
+// A GEMM over fp32 rows x [rows, lin.in_f] in any mode: the SIMT GEMM, or the split into fp16 planes carved from scratch
+// (gemm_tc_scratch_bytes) and the tensor-core GEMM
+int gemm_rows(const float* x, int64_t ldx, int64_t rows, const FaLinear& lin, const GemmEpi& epi, int mode, Arena* scratch, cudaStream_t st);
 // wgmma attention (attention_tc.cu); ctx fp32 and/or fp16 planes [npl][B*tq][ldp]; head_dim 128 or 80
 int attention_tc_planes_launch(const plane_t* qp, const plane_t* kp, const plane_t* vt, const int32_t* key_lens,
                                int batch, int heads, int tq, int tk, float* ctx, int64_t ldc, plane_t* ctx_planes,
@@ -43,9 +57,8 @@ int attention_tc_launch(const float* q, int64_t ldq, const float* k, int64_t ldk
                         const int32_t* key_lens, int batch, int heads, int tq, int tk, float* ctx, int64_t ldc,
                         plane_t* ctx_planes, int64_t ldp, int out_nplanes, int mode, Arena* scratch, cudaStream_t st,
                         int kv_shared = 0);   // kv_shared: k / v hold ONE batch entry that every utterance attends over
-int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& lin, int relu, const float* r1, int64_t ld1,
-                          const float* r2, int64_t ld2, float* y, int64_t ldy, plane_t* out_planes, int64_t ldo,
-                          int mode, cudaStream_t st, const AttnSinks* att = nullptr, int64_t a_ld = 0, int64_t a_plane_rows = 0);
+int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& lin, const GemmEpi& epi, int mode, cudaStream_t st,
+                          int64_t a_ld = 0, int64_t a_plane_rows = 0);
 // a_ld / a_plane_rows (0 = dense: K_pad / M): row pitch of the A planes and rows between planes when A is an overlapping view
 int split_rows_launch(const float* x, int64_t ldx, int64_t rows, int cols, int cols_pad, int nplanes, plane_t* planes,
                       cudaStream_t st);

@@ -39,14 +39,6 @@ static SideStream* side_stream(cudaStream_t caller) {
   return slot;
 }
 
-static int linear(const float* x, int64_t ldx, int64_t rows, const FaLinear& lin, int relu, const float* r1, int64_t ld1,
-                  const float* r2, int64_t ld2, float* y, int64_t ldy, int mode, Arena* scratch, cudaStream_t st) {
-  if (!lin.w) return FA_ERR_ARG;
-  if (mode == FA_GEMM_F32_SIMT)
-    return gemm_f32_launch(x, ldx, rows, lin.w, lin.out_f, lin.in_f, lin.b, relu, r1, ld1, r2, ld2, y, ldy, st);
-  return gemm_tc_launch(x, ldx, rows, lin, relu, r1, ld1, r2, ld2, y, ldy, mode, scratch, st);
-}
-
 // ------------------------------------------------------------------------------------------------ encoder
 // Sized for the largest supported stack (d_model 512, input 560, FFN 2048).  The fp32 path keeps every activation in fp32; the
 // tensor-core path passes LayerNorm, attention and FFN w_1 outputs as fp16 planes and writes only the V columns of qkv in fp32.
@@ -134,9 +126,9 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
       AttnSinks sk;
       sk.q0 = 0; sk.k0 = D; sk.v0 = 2 * D; sk.width = D; sk.npl = attn_planes(gemm_mode); sk.t_rows = t_max; sk.t_pad = t_pad;
       sk.qscale = (float)pow((double)hd, -0.5); sk.q_planes = q_planes; sk.k_planes = k_planes; sk.vt_planes = vt_planes;
-      FA_RETURN_IF_ERR(gemm_tc_planes_launch(u_planes, M, L.qkv, 0, nullptr, 0, nullptr, 0, qkv, 3 * D, nullptr, 0, gemm_mode, st, &sk));
+      FA_RETURN_IF_ERR(gemm_tc_planes_launch(u_planes, M, L.qkv, GemmEpi().to(qkv, 3 * D).sinks(&sk), gemm_mode, st));
     } else {
-      FA_RETURN_IF_ERR(linear(u, in, M, L.qkv, 0, nullptr, 0, nullptr, 0, qkv, 3 * D, gemm_mode, nullptr, st));
+      FA_RETURN_IF_ERR(gemm_rows(u, in, M, L.qkv, GemmEpi().to(qkv, 3 * D), gemm_mode, nullptr, st));
     }
     SideStream* side = tc ? side_stream(st) : nullptr;
     // x2 = (residual if in_size == size) + (linear_out(ctx) + fsmn_memory)     encoder.py:120-137, attention.py:327
@@ -162,21 +154,21 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
       } else {
         FA_RETURN_IF_ERR(attention_small_launch(qkv, 3 * D, qkv + D, 3 * D, qkv + 2 * D, 3 * D, lens, batch, enc->heads, hd, t_max, t_max, ctx, D, st));
       }
-      FA_RETURN_IF_ERR(linear(ctx, D, M, L.out, 0, mem, D, res, D, x2, D, gemm_mode, nullptr, st));
+      FA_RETURN_IF_ERR(gemm_rows(ctx, D, M, L.out, GemmEpi().add(mem, D, res, D).to(x2, D), gemm_mode, nullptr, st));
       FA_RETURN_IF_ERR(layernorm_launch(x2, M, L.norm2, u, nullptr, 1.f, t_max, st));
-      FA_RETURN_IF_ERR(linear(u, D, M, L.w1, 1, nullptr, 0, nullptr, 0, h, L.w1.out_f, gemm_mode, nullptr, st));
-      FA_RETURN_IF_ERR(linear(h, L.w1.out_f, M, L.w2, 0, x2, D, nullptr, 0, x3, D, gemm_mode, nullptr, st));
+      FA_RETURN_IF_ERR(gemm_rows(u, D, M, L.w1, GemmEpi().relu().to(h, L.w1.out_f), gemm_mode, nullptr, st));
+      FA_RETURN_IF_ERR(gemm_rows(h, L.w1.out_f, M, L.w2, GemmEpi().add(x2, D).to(x3, D), gemm_mode, nullptr, st));
     } else {
       // tensor-core path: attention emits the context as fp16 planes (A operand of linear_out); FFN w_1 emits its
       // ReLU output as planes for w_2 — neither intermediate makes an fp32 round trip through HBM
       FA_RETURN_IF_ERR(attention_tc_planes_launch(q_planes, k_planes, vt_planes, lens, batch, enc->heads, t_max, t_max, nullptr, 0,
                                                   ctx_planes, D, npl, gemm_mode, st, 0, hd));
       if (side) FA_CUDA_OK(cudaStreamWaitEvent(st, side->join, 0));          // join: linear_out adds the FSMN memory
-      FA_RETURN_IF_ERR(gemm_tc_planes_launch(ctx_planes, M, L.out, 0, mem, D, nullptr, 0, x2, D, nullptr, 0, gemm_mode, st));   // mem already holds residual + memory
+      FA_RETURN_IF_ERR(gemm_tc_planes_launch(ctx_planes, M, L.out, GemmEpi().add(mem, D).to(x2, D), gemm_mode, st));   // mem already holds residual + memory
       if (L.w1.out_f != L.w2.in_pad || L.w1.in_pad != D) return FA_ERR_UNSUPPORTED;
       FA_RETURN_IF_ERR(layernorm_launch(x2, M, L.norm2, nullptr, nullptr, 1.f, t_max, st, u_planes, npl, D));
-      FA_RETURN_IF_ERR(gemm_tc_planes_launch(u_planes, M, L.w1, 1, nullptr, 0, nullptr, 0, nullptr, 0, h_planes, L.w1.out_f, gemm_mode, st));
-      FA_RETURN_IF_ERR(gemm_tc_planes_launch(h_planes, M, L.w2, 0, x2, D, nullptr, 0, x3, D, nullptr, 0, gemm_mode, st));
+      FA_RETURN_IF_ERR(gemm_tc_planes_launch(u_planes, M, L.w1, GemmEpi().relu().to(h_planes, L.w1.out_f), gemm_mode, st));
+      FA_RETURN_IF_ERR(gemm_tc_planes_launch(h_planes, M, L.w2, GemmEpi().add(x2, D).to(x3, D), gemm_mode, st));
     }
     x = x3;
   }
@@ -225,12 +217,12 @@ extern "C" int fa_cif_predictor_forward(const FaPredictor* pred, const float* en
     const int npl = gemm_planes(gemm_mode);
     const int64_t Mp = (int64_t)batch * (t_max + 2), rows_alloc = Mp + 2;
     FA_RETURN_IF_ERR(cif_pad_planes_launch(enc, batch, t_max, D, npl, rows_alloc, b.pp, st));
-    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.pp, Mp, pred->conv, 1, nullptr, 0, nullptr, 0, b.c, D, nullptr, 0, gemm_mode, st, nullptr, D, rows_alloc));
+    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.pp, Mp, pred->conv, GemmEpi().relu().to(b.c, D), gemm_mode, st, D, rows_alloc));
     FA_RETURN_IF_ERR(cif_alpha_launch(b.c, D, pred->out_w, pred->out_b, lens, t_max, M, pred->smooth_factor,
                                       pred->noise_threshold, b.alpha_rows, st, t_max + 2));
   } else {
     FA_RETURN_IF_ERR(cif_im2col_launch(enc, M, t_max, D, b.xc, st));
-    FA_RETURN_IF_ERR(linear(b.xc, 3 * D, M, pred->conv, 1, nullptr, 0, nullptr, 0, b.c, D, gemm_mode, nullptr, st));
+    FA_RETURN_IF_ERR(gemm_rows(b.xc, 3 * D, M, pred->conv, GemmEpi().relu().to(b.c, D), gemm_mode, nullptr, st));
     FA_RETURN_IF_ERR(cif_alpha_launch(b.c, D, pred->out_w, pred->out_b, lens, t_max, M, pred->smooth_factor,
                                       pred->noise_threshold, b.alpha_rows, st));
   }
@@ -315,14 +307,14 @@ static int dec_ffn(const FaDecLayer& L, const float* y, int64_t Mq, float* t1, f
     const int npl = gemm_planes(mode);
     if (L.ffn_w1.in_pad != 512 || L.ffn_w2.in_pad != L.ffn_w1.out_f) return FA_ERR_UNSUPPORTED;
     FA_RETURN_IF_ERR(layernorm_launch(y, Mq, L.norm1, nullptr, nullptr, 1.f, 1, st, t1_planes, npl, 512));
-    FA_RETURN_IF_ERR(gemm_tc_planes_launch(t1_planes, Mq, L.ffn_w1, 1, nullptr, 0, nullptr, 0, hq, L.ffn_w1.out_f, nullptr, 0, mode, st));
+    FA_RETURN_IF_ERR(gemm_tc_planes_launch(t1_planes, Mq, L.ffn_w1, GemmEpi().relu().to(hq, L.ffn_w1.out_f), mode, st));
     FA_RETURN_IF_ERR(layernorm_launch(hq, Mq, L.ffn_norm, nullptr, nullptr, 1.f, 1, st, hq_planes, npl, L.ffn_w1.out_f));
-    return gemm_tc_planes_launch(hq_planes, Mq, L.ffn_w2, 0, nullptr, 0, nullptr, 0, f, 512, nullptr, 0, mode, st);
+    return gemm_tc_planes_launch(hq_planes, Mq, L.ffn_w2, GemmEpi().to(f, 512), mode, st);
   }
   FA_RETURN_IF_ERR(layernorm_launch(y, Mq, L.norm1, t1, nullptr, 1.f, 1, st));
-  FA_RETURN_IF_ERR(linear(t1, 512, Mq, L.ffn_w1, 1, nullptr, 0, nullptr, 0, hq, L.ffn_w1.out_f, mode, scratch, st));
+  FA_RETURN_IF_ERR(gemm_rows(t1, 512, Mq, L.ffn_w1, GemmEpi().relu().to(hq, L.ffn_w1.out_f), mode, scratch, st));
   FA_RETURN_IF_ERR(layernorm_launch(hq, Mq, L.ffn_norm, hq, nullptr, 1.f, 1, st));
-  return linear(hq, L.ffn_w1.out_f, Mq, L.ffn_w2, 0, nullptr, 0, nullptr, 0, f, 512, mode, scratch, st);
+  return gemm_rows(hq, L.ffn_w1.out_f, Mq, L.ffn_w2, GemmEpi().to(f, 512), mode, scratch, st);
 }
 
 // Cross-attention probabilities of ONE utterance (DecoderLayerSANM.get_attn_mat, decoder.py:123-146 ->
@@ -398,8 +390,8 @@ static int dec_attention_layer(const DecRun& r, const FaDecLayer& L, float* yin,
   if (attn_probs) {
     // q / k in fp32 through the mode's GEMM; only utterance 0's rows are needed (seaco_paraformer/model.py:325: hotword_scores[0])
     FA_RETURN_IF_ERR(layernorm_launch(x2, r.n_max, L.norm3, b.t1, nullptr, 1.f, 1, st));
-    FA_RETURN_IF_ERR(linear(b.t1, D, r.n_max, L.q, 0, nullptr, 0, nullptr, 0, b.qd, D, r.mode, r.scratch, st));
-    FA_RETURN_IF_ERR(linear(r.memory, D, r.t_mem, L.kv, 0, nullptr, 0, nullptr, 0, b.kv, 2 * D, r.mode, r.scratch, st));
+    FA_RETURN_IF_ERR(gemm_rows(b.t1, D, r.n_max, L.q, GemmEpi().to(b.qd, D), r.mode, r.scratch, st));
+    FA_RETURN_IF_ERR(gemm_rows(r.memory, D, r.t_mem, L.kv, GemmEpi().to(b.kv, 2 * D), r.mode, r.scratch, st));
     const int rows = r.heads * r.n_max;
     const size_t smem = (size_t)4 * r.t_mem * sizeof(float);
     if (smem > 96 * 1024) return FA_ERR_UNSUPPORTED;
@@ -414,28 +406,28 @@ static int dec_attention_layer(const DecRun& r, const FaDecLayer& L, float* yin,
     FA_RETURN_IF_ERR(layernorm_launch(x2, Mq, L.norm3, nullptr, nullptr, 1.f, 1, st, b.t1_planes, npl, D));
     AttnSinks sq;                       // q -> scaled fp16 planes only (no fp32 round trip)
     sq.q0 = 0; sq.width = D; sq.npl = attn_planes(r.mode); sq.t_rows = r.n_max; sq.qscale = (float)(1.0 / sqrt(128.0)); sq.q_planes = b.q_planes;
-    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.t1_planes, Mq, L.q, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, r.mode, st, &sq));
+    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.t1_planes, Mq, L.q, GemmEpi().sinks(&sq), r.mode, st));
   } else {
     FA_RETURN_IF_ERR(layernorm_launch(x2, Mq, L.norm3, b.t1, nullptr, 1.f, 1, st));
-    FA_RETURN_IF_ERR(linear(b.t1, D, Mq, L.q, 0, nullptr, 0, nullptr, 0, b.qd, D, r.mode, r.scratch, st));
+    FA_RETURN_IF_ERR(gemm_rows(b.t1, D, Mq, L.q, GemmEpi().to(b.qd, D), r.mode, r.scratch, st));
   }
   float* y2 = (x2 == b.ya) ? b.yb : b.ya;
   float* dst = src_out ? src_out : y2;
   const int64_t ldd = src_out ? ld_src : D;
   const float* res = src_out ? nullptr : x2;
   if (!tc) {
-    FA_RETURN_IF_ERR(linear(r.memory, D, Mk, L.kv, 0, nullptr, 0, nullptr, 0, b.kv, 2 * D, r.mode, r.scratch, st));
+    FA_RETURN_IF_ERR(gemm_rows(r.memory, D, Mk, L.kv, GemmEpi().to(b.kv, 2 * D), r.mode, r.scratch, st));
     FA_RETURN_IF_ERR(attention_f32_launch(b.qd, D, b.kv, 2 * D, b.kv + D, 2 * D, r.mem_lens, r.batch, r.heads, r.n_max, r.t_mem, b.ctx, D, st,
                                           r.mem_shared));
-    FA_RETURN_IF_ERR(linear(b.ctx, D, Mq, L.out, 0, res, D, nullptr, 0, dst, ldd, r.mode, r.scratch, st));
+    FA_RETURN_IF_ERR(gemm_rows(b.ctx, D, Mq, L.out, GemmEpi().add(res, D).to(dst, ldd), r.mode, r.scratch, st));
   } else {
     AttnSinks skv;                      // k -> planes, v -> transposed planes; nothing in fp32
     skv.k0 = 0; skv.v0 = D; skv.width = D; skv.npl = attn_planes(r.mode); skv.t_rows = r.t_mem; skv.t_pad = t_pad;
     skv.k_planes = b.k_planes; skv.vt_planes = b.vt_planes;
-    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.mem_planes, Mk, L.kv, 0, nullptr, 0, nullptr, 0, nullptr, 0, nullptr, 0, r.mode, st, &skv));
+    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.mem_planes, Mk, L.kv, GemmEpi().sinks(&skv), r.mode, st));
     FA_RETURN_IF_ERR(attention_tc_planes_launch(b.q_planes, b.k_planes, b.vt_planes, r.mem_lens, r.batch, r.heads, r.n_max, r.t_mem, nullptr, 0,
                                                 b.ctx_planes, D, npl, r.mode, st, r.mem_shared));
-    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.ctx_planes, Mq, L.out, 0, res, D, nullptr, 0, dst, ldd, nullptr, 0, r.mode, st));
+    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.ctx_planes, Mq, L.out, GemmEpi().add(res, D).to(dst, ldd), r.mode, st));
   }
   if (y_next) *y_next = y2;
   return FA_OK;
@@ -490,28 +482,28 @@ static int decoder_forward_impl(const FaDecoder* dec, const float* enc, const in
     FA_RETURN_IF_ERR(dec_attention_layer(r, dec->bias_last, y, &x_self, b.cat, 2 * D, nullptr, nullptr));      // cat[:, :512] = x_src_attn
     // bias decoder: cross attention of LN3(x_self_attn) over the hotword memory (identical for every utterance)
     FA_RETURN_IF_ERR(layernorm_launch(x_self, Mq, dec->bias_norm3, b.t1, nullptr, 1.f, 1, st));
-    FA_RETURN_IF_ERR(linear(b.t1, D, Mq, dec->bias_q, 0, nullptr, 0, nullptr, 0, b.qd, D, gemm_mode, &b.scratch, st));
+    FA_RETURN_IF_ERR(gemm_rows(b.t1, D, Mq, dec->bias_q, GemmEpi().to(b.qd, D), gemm_mode, &b.scratch, st));
     // the hotword k | v rows [nh, 1024] are the same for every utterance: one copy, attended with kv_shared (no per-utterance
     // replication, so the hotword count is independent of t_max)
     float* kvh = b.kvh;
-    FA_RETURN_IF_ERR(linear(dec->hw_embed, D, nh, dec->bias_kv, 0, nullptr, 0, nullptr, 0, kvh, 2 * D, gemm_mode, &b.hw_scratch, st));
+    FA_RETURN_IF_ERR(gemm_rows(dec->hw_embed, D, nh, dec->bias_kv, GemmEpi().to(kvh, 2 * D), gemm_mode, &b.hw_scratch, st));
     if (!tc) {
       FA_RETURN_IF_ERR(attention_f32_launch(b.qd, D, kvh, 2 * D, kvh + D, 2 * D, dec->hw_lens, batch, dec->heads, n_max, nh, b.ctx, D, st, 1));
     } else {
       FA_RETURN_IF_ERR(attention_tc_launch(b.qd, D, kvh, 2 * D, kvh + D, 2 * D, dec->hw_lens, batch, dec->heads, n_max, nh, b.ctx, D,
                                            nullptr, 0, 0, gemm_mode, &b.hw_scratch, st, 1));
     }
-    FA_RETURN_IF_ERR(linear(b.ctx, D, Mq, dec->bias_out, 0, nullptr, 0, nullptr, 0, b.cat + D, 2 * D, gemm_mode, &b.scratch, st));   // cat[:, 512:] = cx
+    FA_RETURN_IF_ERR(gemm_rows(b.ctx, D, Mq, dec->bias_out, GemmEpi().to(b.cat + D, 2 * D), gemm_mode, &b.scratch, st));   // cat[:, 512:] = cx
     float* y2 = (x_self == b.ya) ? b.yb : b.ya;
-    FA_RETURN_IF_ERR(linear(b.cat, 2 * D, Mq, dec->bias_output, 0, x_self, D, nullptr, 0, y2, D, gemm_mode, &b.scratch, st));
+    FA_RETURN_IF_ERR(gemm_rows(b.cat, 2 * D, Mq, dec->bias_output, GemmEpi().add(x_self, D).to(y2, D), gemm_mode, &b.scratch, st));
     y = y2;
   }
   // decoders3, after_norm (-> hidden), output_layer
   FA_RETURN_IF_ERR(dec_finish(r, dec, y, hidden_out));
   if (tc) {
-    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.t1_planes, Mq, dec->output, 0, nullptr, 0, nullptr, 0, lg, V, nullptr, 0, gemm_mode, st));
+    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.t1_planes, Mq, dec->output, GemmEpi().to(lg, V), gemm_mode, st));
   } else {
-    FA_RETURN_IF_ERR(linear(hidden_out ? hidden_out : b.t1, D, Mq, dec->output, 0, nullptr, 0, nullptr, 0, lg, V, gemm_mode, nullptr, st));
+    FA_RETURN_IF_ERR(gemm_rows(hidden_out ? hidden_out : b.t1, D, Mq, dec->output, GemmEpi().to(lg, V), gemm_mode, nullptr, st));
   }
   return argmax_lse_launch(lg, Mq, V, V, argmax_ids, argmax_logp, (logits && log_softmax) ? 1 : 0, st);
 }
@@ -658,7 +650,7 @@ extern "C" int fa_linear_argmax(const FaLinear* lin, const float* a, const float
     x = w.sum;
   }
   float* lg = logp ? logp : w.lg;
-  FA_RETURN_IF_ERR(linear(x, K, rows, *lin, 0, nullptr, 0, nullptr, 0, lg, V, gemm_mode, &w.scratch, st));
+  FA_RETURN_IF_ERR(gemm_rows(x, K, rows, *lin, GemmEpi().to(lg, V), gemm_mode, &w.scratch, st));
   return argmax_lse_launch(lg, rows, V, V, ids, best_logp, logp ? 1 : 0, st);
 }
 
@@ -693,7 +685,7 @@ extern "C" int fa_ctc_greedy_forward(const FaLinear* ctc_lo, const float* enc, c
   // a caller-provided log-prob tensor keeps the dense [M, V] layout
   const int64_t ldv = logp ? V : ((V + 3) & ~3);
   float* lg = logp ? logp : w.lg;
-  FA_RETURN_IF_ERR(linear(enc, ctc_lo->in_f, M, *ctc_lo, 0, nullptr, 0, nullptr, 0, lg, ldv, gemm_mode, &w.scratch, st));
+  FA_RETURN_IF_ERR(gemm_rows(enc, ctc_lo->in_f, M, *ctc_lo, GemmEpi().to(lg, ldv), gemm_mode, &w.scratch, st));
   FA_RETURN_IF_ERR(argmax_lse_launch(lg, M, V, ldv, argmax_ids, w.best, logp ? 1 : 0, st));
   return ctc_filter_launch(argmax_ids, lens, batch, t_max, blank, out_ids, out_lens, st);
 }
@@ -709,7 +701,8 @@ extern "C" int fa_linear(const float* x, int64_t ldx, int64_t rows, const FaLine
                          void* workspace, size_t ws_bytes, fa_stream_t stream) {
   if (!lin || !x || !y) return FA_ERR_ARG;
   Arena scratch(workspace, ws_bytes);
-  return linear(x, ldx, rows, *lin, relu, res1, ld_res1, res2, ld_res2, y, ldy, gemm_mode, &scratch, (cudaStream_t)stream);
+  return gemm_rows(x, ldx, rows, *lin, GemmEpi().relu(relu).add(res1, ld_res1, res2, ld_res2).to(y, ldy), gemm_mode, &scratch,
+                   (cudaStream_t)stream);
 }
 
 extern "C" int fa_split_rows(const float* x, int64_t ldx, int64_t rows, int32_t cols, int32_t cols_pad, int32_t nplanes, void* planes,
@@ -722,8 +715,8 @@ extern "C" int fa_linear_planes(const void* a_planes, int64_t rows, const FaLine
                                 int64_t ld_res1, const float* res2, int64_t ld_res2, float* y, int64_t ldy, int32_t gemm_mode,
                                 fa_stream_t stream) {
   if (!a_planes || !lin || !y || gemm_mode == FA_GEMM_F32_SIMT) return FA_ERR_ARG;
-  return gemm_tc_planes_launch(reinterpret_cast<const plane_t*>(a_planes), rows, *lin, relu, res1, ld_res1, res2, ld_res2, y, ldy,
-                               nullptr, 0, gemm_mode, (cudaStream_t)stream);
+  return gemm_tc_planes_launch(reinterpret_cast<const plane_t*>(a_planes), rows, *lin,
+                               GemmEpi().relu(relu).add(res1, ld_res1, res2, ld_res2).to(y, ldy), gemm_mode, (cudaStream_t)stream);
 }
 
 extern "C" int fa_linear_attn_sinks(const void* a_planes, int64_t rows, const FaLinear* lin, int32_t q0, int32_t k0, int32_t v0,
@@ -755,15 +748,15 @@ extern "C" int fa_linear_attn_sinks(const void* a_planes, int64_t rows, const Fa
   sk.width = width; sk.npl = npl; sk.t_rows = t_rows; sk.t_pad = v0 >= 0 ? t_pad : 64; sk.qscale = qscale;
   sk.q_planes = reinterpret_cast<plane_t*>(q_planes); sk.k_planes = reinterpret_cast<plane_t*>(k_planes);
   sk.vt_planes = reinterpret_cast<plane_t*>(vt_planes);
-  return gemm_tc_planes_launch(reinterpret_cast<const plane_t*>(a_planes), rows, *lin, 0, nullptr, 0, nullptr, 0, v_f32, ld_v_f32, nullptr, 0,
-                               gemm_mode, (cudaStream_t)stream, &sk);
+  return gemm_tc_planes_launch(reinterpret_cast<const plane_t*>(a_planes), rows, *lin, GemmEpi().to(v_f32, ld_v_f32).sinks(&sk), gemm_mode,
+                               (cudaStream_t)stream);
 }
 
 extern "C" int fa_linear_planes_to_planes(const void* a_planes, int64_t rows, const FaLinear* lin, int32_t relu, void* out_planes,
                                           int64_t ld_out, int32_t gemm_mode, fa_stream_t stream) {
   if (!a_planes || !lin || !out_planes || gemm_mode == FA_GEMM_F32_SIMT) return FA_ERR_ARG;
-  return gemm_tc_planes_launch(reinterpret_cast<const plane_t*>(a_planes), rows, *lin, relu, nullptr, 0, nullptr, 0, nullptr, 0,
-                               reinterpret_cast<plane_t*>(out_planes), ld_out, gemm_mode, (cudaStream_t)stream);
+  return gemm_tc_planes_launch(reinterpret_cast<const plane_t*>(a_planes), rows, *lin,
+                               GemmEpi().relu(relu).to(reinterpret_cast<plane_t*>(out_planes), ld_out), gemm_mode, (cudaStream_t)stream);
 }
 
 // The GEMM over an overlapping ("conv view") A operand, as the CIF conv and the CAM++ TDNN launch it: row r of plane p is the
@@ -777,8 +770,8 @@ extern "C" int fa_linear_planes_view(const void* a_planes, int64_t rows, int64_t
   const int64_t kp = lin->in_pad;
   const int64_t extra = a_ld < kp ? (kp - a_ld + a_ld - 1) / a_ld : 0;
   if (a_plane_rows < rows + extra) return FA_ERR_ARG;
-  return gemm_tc_planes_launch(reinterpret_cast<const plane_t*>(a_planes), rows, *lin, relu, nullptr, 0, nullptr, 0, y, ldy, nullptr, 0,
-                               gemm_mode, (cudaStream_t)stream, nullptr, a_ld, a_plane_rows);
+  return gemm_tc_planes_launch(reinterpret_cast<const plane_t*>(a_planes), rows, *lin, GemmEpi().relu(relu).to(y, ldy), gemm_mode,
+                               (cudaStream_t)stream, a_ld, a_plane_rows);
 }
 
 // rows of an embedding table: out[i, :] = table[ids[i], :] (torch.nn.Embedding forward, e.g. CTTransformer.embed ct_transformer/model.py:120)

@@ -96,20 +96,20 @@ extern "C" int fa_fsmn_vad_forward(const FaVadEncoder* enc, const float* feats, 
   host_meta[0] = t;
   for (int k = 0; k < enc->n_sil; ++k) host_meta[4 + k] = enc->sil_ids[k];
   FA_CUDA_OK(cudaMemcpyAsync(meta, host_meta, sizeof(host_meta), cudaMemcpyHostToDevice, st));
-  FA_RETURN_IF_ERR(gemm_f32_launch(feats, ld_feats, t, enc->in1.w, A, enc->in1.in_f, enc->in1.b, 0, nullptr, 0, nullptr, 0, a1, Ap, st));
-  FA_RETURN_IF_ERR(gemm_f32_launch(a1, Ap, t, enc->in2.w, L, Ap, enc->in2.b, 1, nullptr, 0, nullptr, 0, h0, Lp, st));
+  FA_RETURN_IF_ERR(gemm_f32_launch(feats, ld_feats, t, enc->in1.w, A, enc->in1.in_f, enc->in1.b, GemmEpi().to(a1, Ap), st));
+  FA_RETURN_IF_ERR(gemm_f32_launch(a1, Ap, t, enc->in2.w, L, Ap, enc->in2.b, GemmEpi().relu().to(h0, Lp), st));
   float* h = h0;
   for (int l = 0; l < enc->n_layers; ++l) {
     const FaVadLayer& Y = enc->layers[l];
     if (Y.lin.out_f != 128 || Y.lin.in_f != Lp || Y.affine.in_f != 128 || Y.affine.out_f != L || !Y.conv_w) return FA_ERR_UNSUPPORTED;
-    FA_RETURN_IF_ERR(gemm_f32_launch(h, Lp, t, Y.lin.w, 128, Lp, nullptr, 0, nullptr, 0, nullptr, 0, q, 128, st));
+    FA_RETURN_IF_ERR(gemm_f32_launch(h, Lp, t, Y.lin.w, 128, Lp, nullptr, GemmEpi().to(q, 128), st));
     FA_RETURN_IF_ERR(fsmn_launch(q, 128, meta, 1, t, 128, Y.conv_w, enc->lorder, nullptr, 0, qm, 128, st, 1));
     float* hn = (h == h0) ? h1 : h0;
-    FA_RETURN_IF_ERR(gemm_f32_launch(qm, 128, t, Y.affine.w, L, 128, Y.affine.b, 1, nullptr, 0, nullptr, 0, hn, Lp, st));
+    FA_RETURN_IF_ERR(gemm_f32_launch(qm, 128, t, Y.affine.w, L, 128, Y.affine.b, GemmEpi().relu().to(hn, Lp), st));
     h = hn;
   }
-  FA_RETURN_IF_ERR(gemm_f32_launch(h, Lp, t, enc->out1.w, O, Lp, enc->out1.b, 0, nullptr, 0, nullptr, 0, o1, Op, st));
-  FA_RETURN_IF_ERR(gemm_f32_launch(o1, Op, t, enc->out2.w, V, Op, enc->out2.b, 0, nullptr, 0, nullptr, 0, lg, Vp, st));
+  FA_RETURN_IF_ERR(gemm_f32_launch(h, Lp, t, enc->out1.w, O, Lp, enc->out1.b, GemmEpi().to(o1, Op), st));
+  FA_RETURN_IF_ERR(gemm_f32_launch(o1, Op, t, enc->out2.w, V, Op, enc->out2.b, GemmEpi().to(lg, Vp), st));
   vad_softmax_sil_kernel<<<(t + 7) / 8, 256, 0, st>>>(lg, Vp, t, V, meta + 4, enc->n_sil, sil_prob, scores);
   FA_CHECK_LAUNCH();
   return FA_OK;
