@@ -6,6 +6,7 @@
 // The [B,H,Tq,Tk] score tensor (256 MB at B=64,T=500) never touches HBM.
 // One CTA = 64 queries of one (utterance, head); keys/values streamed in tiles of 64.
 #include "common.cuh"
+#include "kernels.h"
 #include <math.h>
 
 namespace fa {
@@ -191,34 +192,38 @@ attention_small_kernel(const float* __restrict__ q, int64_t ldq, const float* __
     if (lane + 32 * j < hd) dst[lane + 32 * j] = klen > 0 ? o[j] : 0.f;
 }
 
-int attention_small_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, const int32_t* key_lens,
-                           int batch, int heads, int head_dim, int tq, int tk, float* ctx, int64_t ldc, cudaStream_t st, int kv_shared) {
-  if (batch <= 0 || tq <= 0) return FA_OK;
-  if (!q || !k || !v || !key_lens || !ctx || tk <= 0) return FA_ERR_ARG;
-  if (head_dim < 32 || head_dim > 128 || ((head_dim & 31) && head_dim != 80)) return FA_ERR_UNSUPPORTED;
-  const size_t smem = (size_t)4 * tk * sizeof(float);
+static int attention_small_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, const AttnShape& s,
+                                  const int32_t* key_lens, const AttnOut& out, cudaStream_t st) {
+  if (s.head_dim < 32 || s.head_dim > 128 || ((s.head_dim & 31) && s.head_dim != 80)) return FA_ERR_UNSUPPORTED;
+  const size_t smem = (size_t)4 * s.tk * sizeof(float);
   if (smem > 160 * 1024) return FA_ERR_UNSUPPORTED;
   if (smem > 48 * 1024) FA_CUDA_OK(cudaFuncSetAttribute(attention_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int64_t rows = (int64_t)batch * heads * tq;
-  attention_small_kernel<<<(unsigned)((rows + 3) / 4), 128, smem, st>>>(q, ldq, k, ldk, v, ldv, key_lens, heads, head_dim, tq, tk, ctx, ldc,
-                                                                       (float)(1.0 / sqrt((double)head_dim)), kv_shared ? 1 : 0, rows);
+  const int64_t rows = (int64_t)s.batch * s.heads * s.tq;
+  attention_small_kernel<<<(unsigned)((rows + 3) / 4), 128, smem, st>>>(q, ldq, k, ldk, v, ldv, key_lens, s.heads, s.head_dim, s.tq, s.tk,
+                                                                       out.ctx, out.ldc, attn_qscale(s.head_dim), s.kv_shared ? 1 : 0, rows);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }
 
-int attention_f32_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
-                         const int32_t* key_lens, int batch, int heads, int tq, int tk, float* ctx, int64_t ldc,
-                         cudaStream_t st, int kv_shared) {
-  if (batch <= 0 || tq <= 0) return FA_OK;
-  if (!q || !k || !v || !key_lens || !ctx || tk <= 0) return FA_ERR_ARG;
-  if ((ldq | ldk | ldv | ldc) & 3) return FA_ERR_UNSUPPORTED;
+static int attention_f32_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, const AttnShape& s,
+                                const int32_t* key_lens, const AttnOut& out, cudaStream_t st) {
+  if ((ldq | ldk | ldv | out.ldc) & 3) return FA_ERR_UNSUPPORTED;
   static PerDeviceOnce once;
   FA_RETURN_IF_ERR(ensure_dyn_smem(attention_f32_kernel, sizeof(AttSmem), once));
-  dim3 grid((tq + ATT_BQ - 1) / ATT_BQ, heads, batch);
-  const float qscale = (float)(1.0 / sqrt((double)ATT_D));  // float(d_k ** -0.5), attention.py:324
-  attention_f32_kernel<<<grid, 256, sizeof(AttSmem), st>>>(q, ldq, k, ldk, v, ldv, key_lens, tq, tk, ctx, ldc, qscale, kv_shared ? 1 : 0);
+  dim3 grid((s.tq + ATT_BQ - 1) / ATT_BQ, s.heads, s.batch);
+  attention_f32_kernel<<<grid, 256, sizeof(AttSmem), st>>>(q, ldq, k, ldk, v, ldv, key_lens, s.tq, s.tk, out.ctx, out.ldc,
+                                                           attn_qscale(ATT_D), s.kv_shared ? 1 : 0);
   FA_CHECK_LAUNCH();
   return FA_OK;
+}
+
+// attention_rows in fp32 mode: the tiled kernel for 128-wide heads, the warp-per-query one otherwise
+int attention_f32_rows(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, const AttnShape& s,
+                       const int32_t* key_lens, const AttnOut& out, cudaStream_t st) {
+  if (s.batch <= 0 || s.tq <= 0) return FA_OK;
+  if (!q || !k || !v || !key_lens || !out.ctx || s.tk <= 0) return FA_ERR_ARG;
+  if (s.head_dim == ATT_D) return attention_f32_launch(q, ldq, k, ldk, v, ldv, s, key_lens, out, st);
+  return attention_small_launch(q, ldq, k, ldk, v, ldv, s, key_lens, out, st);
 }
 
 }  // namespace fa
@@ -226,17 +231,14 @@ int attention_f32_launch(const float* q, int64_t ldq, const float* k, int64_t ld
 extern "C" int fa_attention(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
                             const int32_t* key_lens, int32_t batch, int32_t heads, int32_t tq, int32_t tk, float* ctx,
                             int64_t ld_ctx, fa_stream_t stream) {
-  return fa::attention_f32_launch(q, ldq, k, ldk, v, ldv, key_lens, batch, heads, tq, tk, ctx, ld_ctx,
-                                  (cudaStream_t)stream, 0);
+  return fa::attention_rows(q, ldq, k, ldk, v, ldv, fa::AttnShape{batch, heads, fa::ATT_D, tq, tk, 0}, key_lens, fa::AttnOut().to(ctx, ld_ctx),
+                            FA_GEMM_F32_SIMT, nullptr, (cudaStream_t)stream);
 }
 
-// the kernel choice of the encoder's fp32 path (model.cu): the tiled kernel for 128-wide heads, the warp-per-query one otherwise
 extern "C" int fa_attention_f32_ex(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
                                    const int32_t* key_lens, int32_t batch, int32_t heads, int32_t head_dim, int32_t tq, int32_t tk,
                                    float* ctx, int64_t ld_ctx, int32_t kv_shared, fa_stream_t stream) {
   if (heads < 1) return FA_ERR_ARG;
-  if (head_dim == fa::ATT_D)
-    return fa::attention_f32_launch(q, ldq, k, ldk, v, ldv, key_lens, batch, heads, tq, tk, ctx, ld_ctx, (cudaStream_t)stream, kv_shared);
-  return fa::attention_small_launch(q, ldq, k, ldk, v, ldv, key_lens, batch, heads, head_dim, tq, tk, ctx, ld_ctx, (cudaStream_t)stream,
-                                    kv_shared);
+  return fa::attention_rows(q, ldq, k, ldk, v, ldv, fa::AttnShape{batch, heads, head_dim, tq, tk, kv_shared}, key_lens,
+                            fa::AttnOut().to(ctx, ld_ctx), FA_GEMM_F32_SIMT, nullptr, (cudaStream_t)stream);
 }

@@ -291,55 +291,63 @@ scale_split_kernel(const float* __restrict__ src, int64_t ld, int64_t rows, int 
   }
 }
 
-// attention_tc_launch's scratch: q (scaled) / k planes and v planes transposed per head; a shared K / V is one batch entry
-struct AttnOperands { plane_t *qp, *kp, *vt; };
-static AttnOperands attn_carve(Arena& a, int batch, int heads, int tq, int tk, int mode, int kv_shared) {
-  const int npl = attn_planes(mode);
-  const int d = heads * AT_D;
-  const int tkp = (tk + 63) / 64 * 64;
-  const int kvb = kv_shared ? 1 : batch;
-  AttnOperands o;
-  o.qp = a.take<plane_t>((size_t)npl * batch * tq * d);
-  o.kp = a.take<plane_t>((size_t)npl * kvb * tk * d);
-  o.vt = a.take<plane_t>((size_t)npl * kvb * d * tkp);
-  return o;
+static int key_pitch(int tk) { return (tk + 63) / 64 * 64; }   // the V^T planes' keys, padded to whole 64-key chunks
+
+AttnPlanes attn_carve(Arena& a, int batch, int tq, int kv_batch, int tk, int width, int mode) {
+  AttnPlanes p;
+  p.npl = attn_planes(mode);
+  p.t_pad = key_pitch(tk);
+  p.q = a.take<plane_t>((size_t)p.npl * batch * tq * width);
+  p.k = a.take<plane_t>((size_t)p.npl * kv_batch * tk * width);
+  p.vt = a.take<plane_t>((size_t)p.npl * kv_batch * width * p.t_pad);
+  return p;
 }
 
+AttnSinks attn_sinks(const AttnPlanes& p, int q0, int k0, int v0, int width, int t_rows, float qscale) {
+  AttnSinks s;
+  if (q0 >= 0) s.q0 = q0;
+  if (k0 >= 0) s.k0 = k0;
+  if (v0 >= 0) s.v0 = v0;
+  s.width = width; s.npl = p.npl; s.t_rows = t_rows; s.t_pad = p.t_pad; s.qscale = qscale;
+  s.q_planes = p.q; s.k_planes = p.k; s.vt_planes = p.vt;
+  return s;
+}
+
+// attention_rows' scratch in the tensor-core modes: the planes of a 128-wide head; a shared K / V is one batch entry
 size_t attention_tc_scratch_bytes(int batch, int heads, int tq, int tk, int mode, int kv_shared) {
   if (mode == FA_GEMM_F32_SIMT) return 0;
   Arena m = Arena::measuring();
-  attn_carve(m, batch, heads, tq, tk, mode, kv_shared);
+  attn_carve(m, batch, tq, kv_shared ? 1 : batch, tk, heads * AT_D, mode);
   return m.bytes();
 }
 
-int attention_tc_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
-                        const int32_t* key_lens, int batch, int heads, int tq, int tk, float* ctx, int64_t ldc,
-                        plane_t* ctx_planes, int64_t ldp, int out_nplanes, int mode, Arena* scratch, cudaStream_t st, int kv_shared) {
-  if (batch <= 0 || tq <= 0) return FA_OK;
-  if (!q || !k || !v || !key_lens || tk <= 0 || !scratch) return FA_ERR_ARG;
+// the fp32 mode of attention_rows (attention_f32.cu)
+int attention_f32_rows(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, const AttnShape& s,
+                       const int32_t* key_lens, const AttnOut& out, cudaStream_t st);
+
+int attention_rows(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, const AttnShape& s,
+                   const int32_t* key_lens, const AttnOut& out, int mode, Arena* scratch, cudaStream_t st) {
+  if (mode == FA_GEMM_F32_SIMT) return attention_f32_rows(q, ldq, k, ldk, v, ldv, s, key_lens, out, st);
+  if (s.head_dim != AT_D) return FA_ERR_UNSUPPORTED;
+  if (s.batch <= 0 || s.tq <= 0) return FA_OK;
+  if (!q || !k || !v || !key_lens || s.tk <= 0 || !scratch) return FA_ERR_ARG;
   if ((ldq | ldk | ldv) & 3) return FA_ERR_UNSUPPORTED;
-  const int npl = attn_planes(mode);
-  const int d = heads * AT_D;
-  const int tkp = (tk + 63) / 64 * 64;
-  const int kvb = kv_shared ? 1 : batch;
-  const int64_t mq = (int64_t)batch * tq, mk = (int64_t)kvb * tk, mv = (int64_t)kvb * d;
+  const int d = s.heads * AT_D;
+  const int kvb = s.kv_shared ? 1 : s.batch;
+  const int64_t mq = (int64_t)s.batch * s.tq, mk = (int64_t)kvb * s.tk, mv = (int64_t)kvb * d;
   Arena local(scratch->base, scratch->cap);
-  const AttnOperands o = attn_carve(local, batch, heads, tq, tk, mode, kv_shared);
+  const AttnPlanes p = attn_carve(local, s.batch, s.tq, kvb, s.tk, d, mode);
   if (!local.ok()) return FA_ERR_WORKSPACE;
-  plane_t *qp = o.qp, *kp = o.kp, *vt = o.vt;
-  const float qscale = (float)(1.0 / sqrt((double)AT_D));
-  {
-    const int64_t tot = mq * (d / 4);
-    scale_split_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(q, ldq, mq, d, qscale, npl, qp);
-    FA_CHECK_LAUNCH();
-    const int64_t totk = mk * (d / 4);
-    scale_split_kernel<<<(unsigned)((totk + 255) / 256), 256, 0, st>>>(k, ldk, mk, d, 1.0f, npl, kp);
-    FA_CHECK_LAUNCH();
-    dim3 g((tkp + 63) / 64, heads * 2, kvb);
-    vt_planes_kernel<<<g, 256, 0, st>>>(v, ldv, tk, tkp, heads, npl, mv * tkp, vt);
-    FA_CHECK_LAUNCH();
-  }
-  return attention_tc_planes_launch(qp, kp, vt, key_lens, batch, heads, tq, tk, ctx, ldc, ctx_planes, ldp, out_nplanes, mode, st, kv_shared);
+  const int64_t tot = mq * (d / 4);
+  scale_split_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(q, ldq, mq, d, attn_qscale(AT_D), p.npl, p.q);
+  FA_CHECK_LAUNCH();
+  const int64_t totk = mk * (d / 4);
+  scale_split_kernel<<<(unsigned)((totk + 255) / 256), 256, 0, st>>>(k, ldk, mk, d, 1.0f, p.npl, p.k);
+  FA_CHECK_LAUNCH();
+  dim3 g(p.t_pad / 64, s.heads * 2, kvb);
+  vt_planes_kernel<<<g, 256, 0, st>>>(v, ldv, s.tk, p.t_pad, s.heads, p.npl, mv * p.t_pad, p.vt);
+  FA_CHECK_LAUNCH();
+  return attention_planes(p, s, key_lens, out, st);
 }
 
 template <int NPL, int OPL, int HD>
@@ -365,36 +373,32 @@ static int launch_att_planes(int npl, int opl, dim3 grid, const CUtensorMap& mq,
                     : launch_att<2, 3, HD>(grid, mq, mk, mv, p, st);
 }
 
-// Operand planes already in place (written by the producing GEMMs' epilogues, gemm_tc.cu AttnSinks), hd = head_dim:
-// qp [npl][B*tq][H*hd] (scaled), kp [npl][B*tk][H*hd], vt [npl][B*H*hd][round_up(tk,64)].
-int attention_tc_planes_launch(const plane_t* qp, const plane_t* kp, const plane_t* vt, const int32_t* key_lens,
-                               int batch, int heads, int tq, int tk, float* ctx, int64_t ldc, plane_t* ctx_planes,
-                               int64_t ldp, int out_nplanes, int mode, cudaStream_t st, int kv_shared, int head_dim) {
-  if (head_dim != 128 && head_dim != 80) return FA_ERR_UNSUPPORTED;
-  if (batch <= 0 || tq <= 0) return FA_OK;
-  if (!qp || !kp || !vt || !key_lens || tk <= 0) return FA_ERR_ARG;
-  const int npl = attn_planes(mode);
-  const int d = heads * head_dim;
-  const int tkp = (tk + 63) / 64 * 64;
-  const int kvb = kv_shared ? 1 : batch;
-  const int64_t mq = (int64_t)batch * tq, mk = (int64_t)kvb * tk, mv = (int64_t)kvb * d;
+// Operand planes already in place (written by the producing GEMMs' epilogues, gemm_tc.cu AttnSinks, or by attention_rows)
+int attention_planes(const AttnPlanes& pl, const AttnShape& s, const int32_t* key_lens, const AttnOut& out, cudaStream_t st) {
+  if (s.head_dim != 128 && s.head_dim != 80) return FA_ERR_UNSUPPORTED;
+  if (s.batch <= 0 || s.tq <= 0) return FA_OK;
+  if (!pl.q || !pl.k || !pl.vt || !key_lens || s.tk <= 0) return FA_ERR_ARG;
+  const int npl = pl.npl;
+  const int d = s.heads * s.head_dim;
+  const int kvb = s.kv_shared ? 1 : s.batch;
+  const int64_t mq = (int64_t)s.batch * s.tq, mk = (int64_t)kvb * s.tk, mv = (int64_t)kvb * d;
   CUtensorMap mq_map, mk_map, mv_map;
-  FA_RETURN_IF_ERR(make_plane_map(&mq_map, qp, (uint64_t)mq * npl, (uint64_t)d, (uint64_t)d, AT_BQ));
-  FA_RETURN_IF_ERR(make_plane_map(&mk_map, kp, (uint64_t)mk * npl, (uint64_t)d, (uint64_t)d, AT_BKEY));
-  FA_RETURN_IF_ERR(make_plane_map(&mv_map, vt, (uint64_t)mv * npl, (uint64_t)tk, (uint64_t)tkp, 64));   // 8 KB boxes: 64 d-rows x 64 keys
+  FA_RETURN_IF_ERR(make_plane_map(&mq_map, pl.q, (uint64_t)mq * npl, (uint64_t)d, (uint64_t)d, AT_BQ));
+  FA_RETURN_IF_ERR(make_plane_map(&mk_map, pl.k, (uint64_t)mk * npl, (uint64_t)d, (uint64_t)d, AT_BKEY));
+  FA_RETURN_IF_ERR(make_plane_map(&mv_map, pl.vt, (uint64_t)mv * npl, (uint64_t)s.tk, (uint64_t)pl.t_pad, 64));   // 8 KB boxes: 64 d-rows x 64 keys
   AttTcParams p;
-  p.tq = tq; p.tk = tk; p.heads = heads; p.batch = batch; p.key_lens = key_lens; p.kv_shared = kv_shared ? 1 : 0;
+  p.tq = s.tq; p.tk = s.tk; p.heads = s.heads; p.batch = s.batch; p.key_lens = key_lens; p.kv_shared = s.kv_shared ? 1 : 0;
   {
     static const bool rz_on = [] { const char* e = getenv("FA_RZ_COMP"); return !(e && e[0] == '0'); }();
     p.o_scale = rz_on ? (npl > 1 ? 5.3e-8f : 3.4e-8f) : 0.f;                                   // relative shrink per 16-key k-step
   }
   p.q_plane_rows = mq; p.k_plane_rows = mk; p.v_plane_rows = mv;
-  p.ctx = ctx; p.ldc = ldc; p.ctx_planes = ctx_planes; p.ldp = ldp; p.out_nplanes = out_nplanes;
-  dim3 grid((tq + AT_BQ - 1) / AT_BQ, heads, batch);
-  const int opl = ctx_planes ? out_nplanes : 0;
-  if (ctx_planes && (opl < 1 || opl > 3)) return FA_ERR_ARG;
-  FA_RETURN_IF_ERR(head_dim == 128 ? launch_att_planes<128>(npl, opl, grid, mq_map, mk_map, mv_map, p, st)
-                                    : launch_att_planes<80>(npl, opl, grid, mq_map, mk_map, mv_map, p, st));
+  p.ctx = out.ctx; p.ldc = out.ldc; p.ctx_planes = out.planes; p.ldp = out.ldp; p.out_nplanes = out.nplanes;
+  dim3 grid((s.tq + AT_BQ - 1) / AT_BQ, s.heads, s.batch);
+  const int opl = out.planes ? out.nplanes : 0;
+  if (out.planes && (opl < 1 || opl > 3)) return FA_ERR_ARG;
+  FA_RETURN_IF_ERR(s.head_dim == 128 ? launch_att_planes<128>(npl, opl, grid, mq_map, mk_map, mv_map, p, st)
+                                      : launch_att_planes<80>(npl, opl, grid, mq_map, mk_map, mv_map, p, st));
   FA_CHECK_LAUNCH();
   return FA_OK;
 }
@@ -412,8 +416,8 @@ extern "C" int fa_attention_tc(const float* q, int64_t ldq, const float* k, int6
   if (!ctx || heads * fa::AT_D > 4096 || (ld_ctx & 3)) return FA_ERR_ARG;
   if (gemm_mode == FA_GEMM_F32_SIMT) return FA_ERR_ARG;
   fa::Arena scratch(workspace, ws_bytes);
-  return fa::attention_tc_launch(q, ldq, k, ldk, v, ldv, key_lens, batch, heads, tq, tk, ctx, ld_ctx, nullptr, 0, 0, gemm_mode,
-                                 &scratch, (cudaStream_t)stream, 0);
+  return fa::attention_rows(q, ldq, k, ldk, v, ldv, fa::AttnShape{batch, heads, fa::AT_D, tq, tk, 0}, key_lens, fa::AttnOut().to(ctx, ld_ctx),
+                            gemm_mode, &scratch, (cudaStream_t)stream);
 }
 
 extern "C" int fa_attention_tc_planes_ex(const void* q_planes, const void* k_planes, const void* vt_planes, const int32_t* key_lens,
@@ -425,10 +429,11 @@ extern "C" int fa_attention_tc_planes_ex(const void* q_planes, const void* k_pla
   if (heads < 1 || heads * head_dim > 4096 || (!ctx && !ctx_planes)) return FA_ERR_ARG;
   if (ctx && (ld_ctx < heads * head_dim || (ld_ctx & 3))) return FA_ERR_ARG;          // float2 stores
   if (ctx_planes && (ld_planes < heads * head_dim || (ld_planes & 1))) return FA_ERR_ARG;   // 4-byte stores of two fp16
-  return fa::attention_tc_planes_launch(reinterpret_cast<const fa::plane_t*>(q_planes), reinterpret_cast<const fa::plane_t*>(k_planes),
-                                        reinterpret_cast<const fa::plane_t*>(vt_planes), key_lens, batch, heads, tq, tk, ctx, ld_ctx,
-                                        reinterpret_cast<fa::plane_t*>(ctx_planes), ld_planes, out_nplanes, gemm_mode, (cudaStream_t)stream,
-                                        kv_shared, head_dim);
+  auto in = [](const void* p) { return static_cast<fa::plane_t*>(const_cast<void*>(p)); };   // read only
+  const fa::AttnPlanes pl{in(q_planes), in(k_planes), in(vt_planes), fa::attn_planes(gemm_mode), fa::key_pitch(tk)};
+  return fa::attention_planes(pl, fa::AttnShape{batch, heads, head_dim, tq, tk, kv_shared}, key_lens,
+                              fa::AttnOut().to(ctx, ld_ctx).to(static_cast<fa::plane_t*>(ctx_planes), ld_planes, out_nplanes),
+                              (cudaStream_t)stream);
 }
 
 extern "C" int fa_attention_tc_planes(const void* q_planes, const void* k_planes, const void* vt_planes, const int32_t* key_lens,

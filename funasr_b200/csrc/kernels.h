@@ -3,6 +3,7 @@
 #include "common.cuh"
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <math.h>
 
 namespace fa { typedef __half plane_t; }   // 16-bit operand plane element (tc_common.cuh)
 
@@ -48,25 +49,37 @@ size_t gemm_tc_scratch_bytes(int64_t max_rows, int max_k, int mode);
 // A GEMM over fp32 rows x [rows, lin.in_f] in any mode: the SIMT GEMM, or the split into fp16 planes carved from scratch
 // (gemm_tc_scratch_bytes) and the tensor-core GEMM
 int gemm_rows(const float* x, int64_t ldx, int64_t rows, const FaLinear& lin, const GemmEpi& epi, int mode, Arena* scratch, cudaStream_t st);
-// wgmma attention (attention_tc.cu); ctx fp32 and/or fp16 planes [npl][B*tq][ldp]; head_dim 128 or 80
-int attention_tc_planes_launch(const plane_t* qp, const plane_t* kp, const plane_t* vt, const int32_t* key_lens,
-                               int batch, int heads, int tq, int tk, float* ctx, int64_t ldc, plane_t* ctx_planes,
-                               int64_t ldp, int out_nplanes, int mode, cudaStream_t st, int kv_shared = 0, int head_dim = 128);
+// The query scale d_k^-0.5 of scaled dot-product attention, rounded like the reference's float(d_k ** -0.5)
+inline float attn_qscale(int head_dim) { return (float)(1.0 / sqrt((double)head_dim)); }
+// The tensor-core attention's operand planes (attention_tc.cu owns this layout): q [npl][B*tq][width] (scaled by d_k^-0.5),
+// k [npl][kv_batch*tk][width] and v transposed per head, vt [npl][kv_batch*width][t_pad], keys padded to t_pad = round_up(tk, 64)
+struct AttnPlanes { plane_t *q = nullptr, *k = nullptr, *vt = nullptr; int npl = 0, t_pad = 0; };
+// The planes for up to (batch, tq) queries over (kv_batch, tk) keys of the given width, attn_planes(mode) planes each
+AttnPlanes attn_carve(Arena& a, int batch, int tq, int kv_batch, int tk, int width, int mode);
+// The sinks of a GEMM epilogue that writes p: columns [q0, q0+width) -> q (x qscale), [k0, +width) -> k, [v0, +width) -> vt, with
+// t_rows GEMM rows per utterance; a negative start leaves its range off
+AttnSinks attn_sinks(const AttnPlanes& p, int q0, int k0, int v0, int width, int t_rows, float qscale);
+// batch utterances of tq queries over tk keys, heads x head_dim wide; kv_shared: K / V hold ONE batch entry that all attend over
+struct AttnShape { int batch, heads, head_dim, tq, tk, kv_shared; };
+// What an attention call writes: fp32 context rows [B*tq][ldc] and / or fp16 planes [nplanes][B*tq][ldp] (the out-projection's A)
+struct AttnOut {
+  float* ctx = nullptr; int64_t ldc = 0;
+  plane_t* planes = nullptr; int64_t ldp = 0; int nplanes = 0;
+  AttnOut& to(float* out, int64_t ld) { ctx = out; ldc = ld; return *this; }
+  AttnOut& to(plane_t* out, int64_t ld, int n) { planes = out; ldp = ld; nplanes = n; return *this; }
+};
+// wgmma attention over operand planes already in place (attention_tc.cu); head_dim 128 or 80
+int attention_planes(const AttnPlanes& p, const AttnShape& s, const int32_t* key_lens, const AttnOut& out, cudaStream_t st);
+// Attention over fp32 rows in any mode: the fp32 kernels (fp32 context only), or the split into planes carved from scratch
+// (attention_tc_scratch_bytes; head_dim 128) and attention_planes
+int attention_rows(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, const AttnShape& s,
+                   const int32_t* key_lens, const AttnOut& out, int mode, Arena* scratch, cudaStream_t st);
 size_t attention_tc_scratch_bytes(int batch, int heads, int tq, int tk, int mode, int kv_shared);
-int attention_tc_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
-                        const int32_t* key_lens, int batch, int heads, int tq, int tk, float* ctx, int64_t ldc,
-                        plane_t* ctx_planes, int64_t ldp, int out_nplanes, int mode, Arena* scratch, cudaStream_t st,
-                        int kv_shared = 0);   // kv_shared: k / v hold ONE batch entry that every utterance attends over
 int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& lin, const GemmEpi& epi, int mode, cudaStream_t st,
                           int64_t a_ld = 0, int64_t a_plane_rows = 0);
 // a_ld / a_plane_rows (0 = dense: K_pad / M): row pitch of the A planes and rows between planes when A is an overlapping view
 int split_rows_launch(const float* x, int64_t ldx, int64_t rows, int cols, int cols_pad, int nplanes, plane_t* planes,
                       cudaStream_t st);
-int attention_f32_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
-                         const int32_t* key_lens, int batch, int heads, int tq, int tk, float* ctx, int64_t ldc,
-                         cudaStream_t st, int kv_shared = 0);
-int attention_small_launch(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, const int32_t* key_lens,
-                           int batch, int heads, int head_dim, int tq, int tk, float* ctx, int64_t ldc, cudaStream_t st, int kv_shared = 0);
 int fsmn_launch(const float* v, int64_t ldv, const int32_t* lens, int batch, int t_max, int channels, const float* w,
                 int ksize, const float* res, int64_t ldr, float* out, int64_t ldo, cudaStream_t st, int causal = 0);
 int cif_im2col_launch(const float* enc, int64_t rows, int t_max, int d, float* xc, cudaStream_t st);

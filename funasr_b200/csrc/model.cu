@@ -44,13 +44,13 @@ static SideStream* side_stream(cudaStream_t caller) {
 // tensor-core path passes LayerNorm, attention and FFN w_1 outputs as fp16 planes and writes only the V columns of qkv in fp32.
 struct EncBufs {
   float *u, *qkv, *mem, *ctx, *xa, *xb, *h;
-  plane_t *ctx_planes, *h_planes, *u_planes, *q_planes, *k_planes, *vt_planes;
+  plane_t *ctx_planes, *h_planes, *u_planes;
+  AttnPlanes att;                                                   // sized for width 512, whatever the model's width
 };
 static EncBufs enc_carve(Arena& a, int batch, int t_max, int mode) {
   const int64_t M = (int64_t)batch * t_max;
   const bool tc = mode != FA_GEMM_F32_SIMT;
-  const size_t gpl = gemm_planes(mode), apl = attn_planes(mode);
-  const int t_pad = (t_max + 63) / 64 * 64;
+  const size_t gpl = gemm_planes(mode);
   EncBufs b;
   b.u = tc ? nullptr : a.take<float>(M * 560ull);
   b.qkv = a.take<float>(M * 1536ull);
@@ -62,9 +62,7 @@ static EncBufs enc_carve(Arena& a, int batch, int t_max, int mode) {
   b.ctx_planes = tc ? a.take<plane_t>(gpl * M * 512) : nullptr;
   b.h_planes = tc ? a.take<plane_t>(gpl * M * 2048) : nullptr;
   b.u_planes = tc ? a.take<plane_t>(gpl * M * 576) : nullptr;      // LN output: the QKV GEMM's K pad of a 560 input
-  b.q_planes = tc ? a.take<plane_t>(apl * M * 512) : nullptr;      // scaled by d_k^-0.5
-  b.k_planes = tc ? a.take<plane_t>(apl * M * 512) : nullptr;
-  b.vt_planes = tc ? a.take<plane_t>(apl * batch * 512 * (size_t)t_pad) : nullptr;   // transposed per head
+  if (tc) b.att = attn_carve(a, batch, t_max, batch, t_max, 512, mode);
   return b;
 }
 
@@ -96,13 +94,12 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
   if (gemm_mode != FA_GEMM_F32_SIMT && !((D == 512 && hd == 128) || (D == 320 && hd == 80))) return FA_ERR_UNSUPPORTED;
   const bool tc = gemm_mode != FA_GEMM_F32_SIMT;
   const int npl = gemm_planes(gemm_mode);
-  const int t_pad = (t_max + 63) / 64 * 64;
   Arena a(workspace, ws_bytes);
   const EncBufs b = enc_carve(a, batch, t_max, gemm_mode);
   if (!a.ok()) return FA_ERR_WORKSPACE;
   float *u = b.u, *qkv = b.qkv, *mem = b.mem, *ctx = b.ctx, *xa = b.xa, *xb = b.xb, *h = b.h;
   plane_t *ctx_planes = b.ctx_planes, *h_planes = b.h_planes, *u_planes = b.u_planes;
-  plane_t *q_planes = b.q_planes, *k_planes = b.k_planes, *vt_planes = b.vt_planes;
+  const AttnShape shape{batch, enc->heads, hd, t_max, t_max, 0};
 
   const float* x = embed ? nullptr : feats;  // residual stream (with PE input: undefined before layer 0, in_size != size)
   for (int l = 0; l < enc->n_layers; ++l) {
@@ -123,9 +120,7 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
     if (tc) {
       // QKV GEMM epilogue emits the attention operands directly: q (x d_k^-0.5) / k as fp16 planes, v transposed per head
       // as fp16 planes plus fp32 v (the only fp32 columns written) for the FSMN branch
-      AttnSinks sk;
-      sk.q0 = 0; sk.k0 = D; sk.v0 = 2 * D; sk.width = D; sk.npl = attn_planes(gemm_mode); sk.t_rows = t_max; sk.t_pad = t_pad;
-      sk.qscale = (float)pow((double)hd, -0.5); sk.q_planes = q_planes; sk.k_planes = k_planes; sk.vt_planes = vt_planes;
+      const AttnSinks sk = attn_sinks(b.att, 0, D, 2 * D, D, t_max, attn_qscale(hd));
       FA_RETURN_IF_ERR(gemm_tc_planes_launch(u_planes, M, L.qkv, GemmEpi().to(qkv, 3 * D).sinks(&sk), gemm_mode, st));
     } else {
       FA_RETURN_IF_ERR(gemm_rows(u, in, M, L.qkv, GemmEpi().to(qkv, 3 * D), gemm_mode, nullptr, st));
@@ -148,12 +143,7 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
       FA_RETURN_IF_ERR(fsmn_launch(qkv + 2 * D, 3 * D, lens, batch, t_max, D, L.fsmn_w, enc->fsmn_k, fsmn_res, D, mem, D, st));
     }
     if (!tc) {
-      if (hd == 128) {
-        FA_RETURN_IF_ERR(attention_f32_launch(qkv, 3 * D, qkv + D, 3 * D, qkv + 2 * D, 3 * D, lens, batch, enc->heads, t_max,
-                                              t_max, ctx, D, st));
-      } else {
-        FA_RETURN_IF_ERR(attention_small_launch(qkv, 3 * D, qkv + D, 3 * D, qkv + 2 * D, 3 * D, lens, batch, enc->heads, hd, t_max, t_max, ctx, D, st));
-      }
+      FA_RETURN_IF_ERR(attention_rows(qkv, 3 * D, qkv + D, 3 * D, qkv + 2 * D, 3 * D, shape, lens, AttnOut().to(ctx, D), gemm_mode, nullptr, st));
       FA_RETURN_IF_ERR(gemm_rows(ctx, D, M, L.out, GemmEpi().add(mem, D, res, D).to(x2, D), gemm_mode, nullptr, st));
       FA_RETURN_IF_ERR(layernorm_launch(x2, M, L.norm2, u, nullptr, 1.f, t_max, st));
       FA_RETURN_IF_ERR(gemm_rows(u, D, M, L.w1, GemmEpi().relu().to(h, L.w1.out_f), gemm_mode, nullptr, st));
@@ -161,8 +151,7 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
     } else {
       // tensor-core path: attention emits the context as fp16 planes (A operand of linear_out); FFN w_1 emits its
       // ReLU output as planes for w_2 — neither intermediate makes an fp32 round trip through HBM
-      FA_RETURN_IF_ERR(attention_tc_planes_launch(q_planes, k_planes, vt_planes, lens, batch, enc->heads, t_max, t_max, nullptr, 0,
-                                                  ctx_planes, D, npl, gemm_mode, st, 0, hd));
+      FA_RETURN_IF_ERR(attention_planes(b.att, shape, lens, AttnOut().to(ctx_planes, D, npl), st));
       if (side) FA_CUDA_OK(cudaStreamWaitEvent(st, side->join, 0));          // join: linear_out adds the FSMN memory
       FA_RETURN_IF_ERR(gemm_tc_planes_launch(ctx_planes, M, L.out, GemmEpi().add(mem, D).to(x2, D), gemm_mode, st));   // mem already holds residual + memory
       if (L.w1.out_f != L.w2.in_pad || L.w1.in_pad != D) return FA_ERR_UNSUPPORTED;
@@ -253,15 +242,15 @@ extern "C" int fa_cif_upsample_alphas(const float* feat, int32_t dz, const float
 // its operands as fp16 planes; fp32 q / k|v / context rows and GEMM scratch serve only the calls that take fp32 operands.
 struct DecBuf {
   float *ya, *yb, *t1, *hq, *f, *qd, *ctx, *kv, *lg, *cat, *kvh;
-  plane_t *ctx_planes, *mem_planes, *t1_planes, *hq_planes, *q_planes, *k_planes, *vt_planes;
+  plane_t *ctx_planes, *mem_planes, *t1_planes, *hq_planes;
+  AttnPlanes att;                     // per-utterance K / V: the stack's query cannot see mem_shared
   Arena scratch{nullptr, 0}, hw_scratch{nullptr, 0};
 };
 static void dec_carve(Arena& a, DecBuf& b, int batch, int t_max, int n_max, int vocab, int mode, int n_hotwords, bool probs) {
   const int64_t Mq = (int64_t)batch * n_max, Mk = (int64_t)batch * t_max;
   const bool tc = mode != FA_GEMM_F32_SIMT;
   const bool contextual = n_hotwords > 0;
-  const size_t gpl = gemm_planes(mode), apl = attn_planes(mode);
-  const int t_pad = (t_max + 63) / 64 * 64;
+  const size_t gpl = gemm_planes(mode);
   b.ya = a.take<float>(Mq * 512ull); b.yb = a.take<float>(Mq * 512ull); b.t1 = a.take<float>(Mq * 512ull);
   b.hq = a.take<float>(Mq * 2048ull); b.f = a.take<float>(Mq * 512ull);
   b.qd = (!tc || contextual || probs) ? a.take<float>(Mq * 512ull) : nullptr;
@@ -274,9 +263,7 @@ static void dec_carve(Arena& a, DecBuf& b, int batch, int t_max, int n_max, int 
   b.mem_planes = tc ? a.take<plane_t>(gpl * Mk * 512) : nullptr;      // split once, reused by every layer's k|v GEMM
   b.t1_planes = tc ? a.take<plane_t>(gpl * Mq * 512) : nullptr;       // LN outputs
   b.hq_planes = tc ? a.take<plane_t>(gpl * Mq * 2048) : nullptr;      // FFN hidden
-  b.q_planes = tc ? a.take<plane_t>(apl * Mq * 512) : nullptr;
-  b.k_planes = tc ? a.take<plane_t>(apl * Mk * 512) : nullptr;
-  b.vt_planes = tc ? a.take<plane_t>(apl * batch * 512 * (size_t)t_pad) : nullptr;   // transposed per head
+  if (tc) b.att = attn_carve(a, batch, n_max, batch, t_max, 512, mode);
   if (tc && (contextual || probs)) {
     // contextual: bias_q, bias_out (K 512) and bias_output (K 1024) over Mq rows; probs: q of n_max rows, k|v of t_max rows (K 512)
     const size_t sc = contextual ? gemm_tc_scratch_bytes(Mq, 1024, mode) : 0;
@@ -379,7 +366,7 @@ static int dec_attention_layer(const DecRun& r, const FaDecLayer& L, float* yin,
   const int64_t Mq = r.Mq(), Mk = r.Mk();
   const bool tc = r.mode != FA_GEMM_F32_SIMT;
   const int npl = gemm_planes(r.mode);
-  const int t_pad = (r.t_mem + 63) / 64 * 64;
+  const AttnShape shape{r.batch, r.heads, 128, r.n_max, r.t_mem, r.mem_shared};
   cudaStream_t st = r.st;
   FA_RETURN_IF_ERR(dec_ffn(L, yin, Mq, b.t1, b.hq, b.f, r.mode, r.scratch, st, b.t1_planes, b.hq_planes));
   // x = residual + fsmn(LN2(f), tgt_mask)     decoder.py:103-107
@@ -397,15 +384,14 @@ static int dec_attention_layer(const DecRun& r, const FaDecLayer& L, float* yin,
     if (smem > 96 * 1024) return FA_ERR_UNSUPPORTED;
     if (smem > 48 * 1024) FA_CUDA_OK(cudaFuncSetAttribute(attn_probs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attn_probs_kernel<<<(rows + 3) / 4, 128, smem, st>>>(b.qd, D, b.kv, 2 * D, r.heads, r.n_max, r.t_mem, r.mem_lens,
-                                                         (float)(1.0 / sqrt(128.0)), attn_probs);
+                                                         attn_qscale(shape.head_dim), attn_probs);
     FA_CHECK_LAUNCH();
     return FA_OK;
   }
   // x = residual + src_attn(LN3(x), memory)    decoder.py:109-118, attention.py:796-813
   if (tc) {
     FA_RETURN_IF_ERR(layernorm_launch(x2, Mq, L.norm3, nullptr, nullptr, 1.f, 1, st, b.t1_planes, npl, D));
-    AttnSinks sq;                       // q -> scaled fp16 planes only (no fp32 round trip)
-    sq.q0 = 0; sq.width = D; sq.npl = attn_planes(r.mode); sq.t_rows = r.n_max; sq.qscale = (float)(1.0 / sqrt(128.0)); sq.q_planes = b.q_planes;
+    const AttnSinks sq = attn_sinks(b.att, 0, -1, -1, D, r.n_max, attn_qscale(shape.head_dim));   // q -> scaled fp16 planes only (no fp32 round trip)
     FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.t1_planes, Mq, L.q, GemmEpi().sinks(&sq), r.mode, st));
   } else {
     FA_RETURN_IF_ERR(layernorm_launch(x2, Mq, L.norm3, b.t1, nullptr, 1.f, 1, st));
@@ -417,16 +403,12 @@ static int dec_attention_layer(const DecRun& r, const FaDecLayer& L, float* yin,
   const float* res = src_out ? nullptr : x2;
   if (!tc) {
     FA_RETURN_IF_ERR(gemm_rows(r.memory, D, Mk, L.kv, GemmEpi().to(b.kv, 2 * D), r.mode, r.scratch, st));
-    FA_RETURN_IF_ERR(attention_f32_launch(b.qd, D, b.kv, 2 * D, b.kv + D, 2 * D, r.mem_lens, r.batch, r.heads, r.n_max, r.t_mem, b.ctx, D, st,
-                                          r.mem_shared));
+    FA_RETURN_IF_ERR(attention_rows(b.qd, D, b.kv, 2 * D, b.kv + D, 2 * D, shape, r.mem_lens, AttnOut().to(b.ctx, D), r.mode, nullptr, st));
     FA_RETURN_IF_ERR(gemm_rows(b.ctx, D, Mq, L.out, GemmEpi().add(res, D).to(dst, ldd), r.mode, r.scratch, st));
   } else {
-    AttnSinks skv;                      // k -> planes, v -> transposed planes; nothing in fp32
-    skv.k0 = 0; skv.v0 = D; skv.width = D; skv.npl = attn_planes(r.mode); skv.t_rows = r.t_mem; skv.t_pad = t_pad;
-    skv.k_planes = b.k_planes; skv.vt_planes = b.vt_planes;
+    const AttnSinks skv = attn_sinks(b.att, -1, 0, D, D, r.t_mem, 1.f);   // k -> planes, v -> transposed planes; nothing in fp32
     FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.mem_planes, Mk, L.kv, GemmEpi().sinks(&skv), r.mode, st));
-    FA_RETURN_IF_ERR(attention_tc_planes_launch(b.q_planes, b.k_planes, b.vt_planes, r.mem_lens, r.batch, r.heads, r.n_max, r.t_mem, nullptr, 0,
-                                                b.ctx_planes, D, npl, r.mode, st, r.mem_shared));
+    FA_RETURN_IF_ERR(attention_planes(b.att, shape, r.mem_lens, AttnOut().to(b.ctx_planes, D, npl), st));
     FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.ctx_planes, Mq, L.out, GemmEpi().add(res, D).to(dst, ldd), r.mode, st));
   }
   if (y_next) *y_next = y2;
@@ -487,12 +469,8 @@ static int decoder_forward_impl(const FaDecoder* dec, const float* enc, const in
     // replication, so the hotword count is independent of t_max)
     float* kvh = b.kvh;
     FA_RETURN_IF_ERR(gemm_rows(dec->hw_embed, D, nh, dec->bias_kv, GemmEpi().to(kvh, 2 * D), gemm_mode, &b.hw_scratch, st));
-    if (!tc) {
-      FA_RETURN_IF_ERR(attention_f32_launch(b.qd, D, kvh, 2 * D, kvh + D, 2 * D, dec->hw_lens, batch, dec->heads, n_max, nh, b.ctx, D, st, 1));
-    } else {
-      FA_RETURN_IF_ERR(attention_tc_launch(b.qd, D, kvh, 2 * D, kvh + D, 2 * D, dec->hw_lens, batch, dec->heads, n_max, nh, b.ctx, D,
-                                           nullptr, 0, 0, gemm_mode, &b.hw_scratch, st, 1));
-    }
+    FA_RETURN_IF_ERR(attention_rows(b.qd, D, kvh, 2 * D, kvh + D, 2 * D, AttnShape{batch, dec->heads, 128, n_max, nh, 1}, dec->hw_lens,
+                                    AttnOut().to(b.ctx, D), gemm_mode, &b.hw_scratch, st));
     FA_RETURN_IF_ERR(gemm_rows(b.ctx, D, Mq, dec->bias_out, GemmEpi().to(b.cat + D, 2 * D), gemm_mode, &b.scratch, st));   // cat[:, 512:] = cx
     float* y2 = (x_self == b.ya) ? b.yb : b.ya;
     FA_RETURN_IF_ERR(gemm_rows(b.cat, 2 * D, Mq, dec->bias_output, GemmEpi().add(x_self, D).to(y2, D), gemm_mode, &b.scratch, st));
@@ -740,14 +718,9 @@ extern "C" int fa_linear_attn_sinks(const void* a_planes, int64_t rows, const Fa
   if (n_on == 0) return FA_ERR_ARG;
   if (v0 >= 0 && t_pad < t_rows) return FA_ERR_ARG;
   if (v_f32 && (v0 < 0 || ld_v_f32 < N)) return FA_ERR_ARG;       // fp32 V rows are the GEMM's output rows: columns [v0, v0 + width)
-  const int npl = attn_planes(gemm_mode);
-  AttnSinks sk;
-  if (q0 >= 0) sk.q0 = q0;
-  if (k0 >= 0) sk.k0 = k0;
-  if (v0 >= 0) sk.v0 = v0;
-  sk.width = width; sk.npl = npl; sk.t_rows = t_rows; sk.t_pad = v0 >= 0 ? t_pad : 64; sk.qscale = qscale;
-  sk.q_planes = reinterpret_cast<plane_t*>(q_planes); sk.k_planes = reinterpret_cast<plane_t*>(k_planes);
-  sk.vt_planes = reinterpret_cast<plane_t*>(vt_planes);
+  const AttnPlanes pl{static_cast<plane_t*>(q_planes), static_cast<plane_t*>(k_planes), static_cast<plane_t*>(vt_planes),
+                      attn_planes(gemm_mode), t_pad};   // t_pad is read only by a v sink
+  const AttnSinks sk = attn_sinks(pl, q0, k0, v0, width, t_rows, qscale);
   return gemm_tc_planes_launch(reinterpret_cast<const plane_t*>(a_planes), rows, *lin, GemmEpi().to(v_f32, ld_v_f32).sinks(&sk), gemm_mode,
                                (cudaStream_t)stream);
 }
