@@ -76,6 +76,15 @@ class FaVadOptions(C.Structure):
                [(n, C.c_double) for n in ("speech_2_noise_ratio", "snr_thres", "decibel_thres", "speech_noise_thres", "fe_prior_thres")]
 
 
+class FaVadRunOptions(C.Structure):
+    _fields_ = [("dynamic_silence", C.c_int32), ("max_end_silence_time", C.c_int32), ("speech_noise_thres", C.c_double)]
+
+
+class FaLongAudioOptions(C.Structure):
+    _fields_ = [("batch_size_s", C.c_int32), ("batch_size_threshold_s", C.c_int32), ("merge_vad", C.c_int32), ("merge_length_s", C.c_int32),
+                ("vad", FaVadRunOptions)]
+
+
 class FaCamConv2d(C.Structure):
     _fields_ = [("w", C.c_void_p), ("b", C.c_void_p), ("c_in", C.c_int32), ("c_out", C.c_int32), ("ksize", C.c_int32), ("stride_f", C.c_int32)]
 
@@ -173,6 +182,19 @@ SIGNATURES = {
     "fa_offline_free_result": (None, [_vp]),
     "fa_offline_uninit": (None, [_vp]),
     "fa_offline_last_error": (C.c_char_p, []),
+    # handle-style FSMN-VAD and long-audio recognition (offline.cu; fa_pack_segments / fa_merge_vad: vad_detector.cpp)
+    "fa_vad_init": (_vp, [C.c_char_p, _i32]),
+    "fa_vad_uninit": (None, [_vp]),
+    "fa_vad_infer": (_vp, [_vp, _vp, _i64, _i32, C.POINTER(FaVadRunOptions)]),
+    "fa_vad_result_segments": (C.POINTER(_i32), [_vp, C.POINTER(_i64)]),
+    "fa_vad_result_frames": (C.POINTER(C.c_float), [_vp, C.POINTER(_i64)]),
+    "fa_vad_result_audio_seconds": (C.c_float, [_vp]),
+    "fa_vad_free_result": (None, [_vp]),
+    "fa_offline_infer_vad": (_vp, [_vp, _vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp, _i32, C.POINTER(FaLongAudioOptions)]),
+    "fa_offline_result_segments": (C.POINTER(_i32), [_vp, _i32, C.POINTER(_i32)]),
+    "fa_gather_segments": (C.c_int, [_vp, _i64, _vp, _vp, _i32, _i64, _vp, _vp]),
+    "fa_pack_segments": (_i64, [_vp, _i64, _i32, _i32, _vp, _vp]),
+    "fa_merge_vad": (_i64, [_vp, _i64, _i32, _i32, _vp]),
 }
 
 _lib = None

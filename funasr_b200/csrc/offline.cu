@@ -7,10 +7,14 @@
 //   fa_offline_init         model file -> handle (weights to HBM, fp16 planes for the tensor-core GEMMs)
 //   fa_offline_infer        batch of host PCM buffers (f32 in [-1,1] or s16le) -> result (greedy token ids per utterance)
 //   fa_offline_result_*     accessors;  fa_offline_free_result / fa_offline_uninit
+//   fa_vad_init / fa_vad_infer       FSMN-VAD model file -> handle; one recording -> [start_ms, end_ms] segments
+//   fa_offline_infer_vad    long recordings: VAD -> segments packed by duration -> each pack gathered on the device and decoded
 // The tokenizer (ids -> text) stays with the caller, like every other entry point of this ABI.
 #include "common.cuh"
+#include <math.h>
 #include <stdio.h>
 #include <string.h>
+#include <algorithm>
 #include <exception>
 #include <map>
 #include <string>
@@ -57,6 +61,7 @@ struct Model {
   float* fbank_tables = nullptr;                     // fa_fbank_make_tables output (owned)
   cudaStream_t st = nullptr;
   DevBuf wav, pcm16, lens, feats, flens, encb, acoustic, tok, alphas, peaks, ws, ids, best, fids, flens_out, hw, hw_lens;
+  DevBuf rec, gmeta;                                 // fa_offline_infer_vad: the device-resident recording, per-pack gather offsets
   bool contextual = false;                           // ContextualParaformer: decoder with a hotword bias branch
   std::map<std::string, std::vector<float>> host_cache;   // fa_offline_host_tensor
   ~Model() {
@@ -69,6 +74,7 @@ struct Model {
 struct Result {
   std::vector<std::vector<int32_t>> ids;
   std::vector<int32_t> token_num;
+  std::vector<std::vector<int32_t>> segs;            // fa_offline_infer_vad: {start_ms, end_ms, n_tokens} per segment, per recording
   float audio_seconds = 0.f;
 };
 
@@ -81,7 +87,7 @@ bool read_exact(FILE* f, void* dst, size_t n) { return fread(dst, 1, n, f) == n;
 
 // File layout (funasr_b200/pack.py): "FAB2MDL1", u32 n_tensors, then per tensor:
 //   u32 name_len, name, u32 ndim, i64 dims[ndim], u64 nbytes, zero padding to a 16-byte file offset, fp32 data
-bool load_file(Model& m, const char* path) {
+bool load_file(std::map<std::string, Tensor>& tensors, const char* path) {
   FILE* f = fopen(path, "rb");
   if (!f) { set_err(std::string("cannot open ") + path); return false; }
   char magic[8];
@@ -111,7 +117,7 @@ bool load_file(Model& m, const char* path) {
     if (!ok) break;
     if (cudaMalloc(&tt.dev, nbytes ? nbytes : 4) != cudaSuccess) { ok = false; set_err("cudaMalloc failed for " + name); break; }
     cudaMemcpy(tt.dev, host.data(), nbytes, cudaMemcpyHostToDevice);
-    m.t[name] = tt;
+    tensors[name] = tt;
   }
   fclose(f);
   if (!ok && g_err.empty()) set_err(std::string("malformed model file ") + path);
@@ -229,90 +235,21 @@ int num_lfr_frames(int64_t n) {       // wav_frontend.py:73 after kaldi.py snip_
   return (int)((mfr + 5) / 6);
 }
 
-}  // namespace
-
-extern "C" const char* fa_offline_last_error(void) { return g_err.c_str(); }
-extern "C" void* fa_offline_infer_hw(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
-                                     const float* hw_embed, int32_t n_hotwords);
-
-extern "C" void* fa_offline_init(const char* model_file, int32_t device, int32_t gemm_mode) {
-  g_err.clear();
-  if (!model_file) { set_err("model_file is NULL"); return nullptr; }
-  if (gemm_mode != FA_GEMM_F32_SIMT && gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) {
-    set_err("bad gemm_mode"); return nullptr;
-  }
-  if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); set_err("no such CUDA device (this library has no CPU path)"); return nullptr; }
-  Model* m = new Model();
-  m->device = device; m->mode = gemm_mode;
-  if (cudaStreamCreateWithFlags(&m->st, cudaStreamNonBlocking) != cudaSuccess) { set_err("cudaStreamCreate failed"); delete m; return nullptr; }
-  bool ok = false;
-  try {                                   // a malformed file can ask for an absurd allocation: no C++ exception may cross the C ABI
-    ok = load_file(*m, model_file) && build(*m);
-  } catch (const std::exception& e) {
-    set_err(std::string("model file rejected: ") + e.what());
-  }
-  if (!ok) { delete m; return nullptr; }
-  return m;
-}
-
-extern "C" void fa_offline_uninit(void* handle) { delete static_cast<Model*>(handle); }
-
-extern "C" int32_t fa_offline_is_contextual(const void* handle) { return handle && static_cast<const Model*>(handle)->contextual ? 1 : 0; }
-
-extern "C" const float* fa_offline_host_tensor(void* handle, const char* name, int64_t* numel) {
-  Model* m = static_cast<Model*>(handle);
-  if (numel) *numel = 0;
-  if (!m || !name) return nullptr;
-  auto it = m->t.find(name);
-  if (it == m->t.end()) return nullptr;
-  auto& hc = m->host_cache[name];
-  if (hc.empty() && it->second.numel() > 0) {
-    hc.resize((size_t)it->second.numel());
-    cudaSetDevice(m->device);
-    if (cudaMemcpy(hc.data(), it->second.dev, hc.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess) { hc.clear(); return nullptr; }
-  }
-  if (numel) *numel = (int64_t)hc.size();
-  return hc.data();
-}
-
-extern "C" void* fa_offline_infer(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format) {
-  return fa_offline_infer_hw(handle, bufs, n_samples, batch, pcm_format, nullptr, 0);
-}
-
-extern "C" void* fa_offline_infer_hw(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
-                                     const float* hw_embed, int32_t n_hotwords) {
-  g_err.clear();
-  Model* mp = static_cast<Model*>(handle);
-  if (!mp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) { set_err("bad argument"); return nullptr; }
-  Model& m = *mp;
-  if (m.contextual && (!hw_embed || n_hotwords < 1)) { set_err("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)"); return nullptr; }
-  cudaSetDevice(m.device);
-  int64_t nmax = 0;
-  double seconds = 0.0;
-  std::vector<int32_t> lens_h(batch);
+// The recogniser over a padded batch already on the device: wav [B, stride] fp32 (m.wav or any buffer the call does not reuse),
+// lens_h [B] samples (>= 400 each).  Everything after the host-to-device copy of fa_offline_infer_hw; fa_offline_infer_vad feeds it the
+// gathered VAD segments of one pack.
+Result* decode_batch(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const float* hw_embed, int32_t n_hotwords) {
+  const int B = (int)lens_h.size(), D = m.d_model;
   int t_max = 0;
-  for (int i = 0; i < batch; ++i) {
-    if (!bufs[i] || n_samples[i] < 400 || n_samples[i] > 0x7fffffffLL) { set_err("every buffer needs >= 400 samples (25 ms)"); return nullptr; }
-    lens_h[i] = (int32_t)n_samples[i];
-    nmax = n_samples[i] > nmax ? n_samples[i] : nmax;
-    seconds += (double)n_samples[i] / 16000.0;
-    const int t = num_lfr_frames(n_samples[i]);
+  double seconds = 0.0;
+  for (int i = 0; i < B; ++i) {
+    const int t = num_lfr_frames(lens_h[i]);
     t_max = t > t_max ? t : t_max;
+    seconds += (double)lens_h[i] / 16000.0;
   }
-  const int B = batch, D = m.d_model, T = t_max;
-  const int64_t stride = (nmax + 3) / 4 * 4;
+  const int T = t_max;
 #define FA_OFF(x, msg) do { if (!(x)) { set_err(msg); return nullptr; } } while (0)
-  FA_OFF(m.wav.reserve((size_t)B * stride * 4) && m.lens.reserve((size_t)B * 4), "device allocation failed (waveforms)");
-  float* wav = static_cast<float*>(m.wav.p);
-  if (pcm_format == 1) {
-    FA_OFF(m.pcm16.reserve((size_t)B * stride * 2), "device allocation failed (pcm)");
-    int16_t* p16 = static_cast<int16_t*>(m.pcm16.p);
-    for (int i = 0; i < B; ++i) cudaMemcpyAsync(p16 + (int64_t)i * stride, bufs[i], (size_t)n_samples[i] * 2, cudaMemcpyHostToDevice, m.st);
-    const int64_t tot = (int64_t)B * stride;
-    pcm16_to_f32_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, m.st>>>(p16, wav, tot);
-  } else {
-    for (int i = 0; i < B; ++i) cudaMemcpyAsync(wav + (int64_t)i * stride, bufs[i], (size_t)n_samples[i] * 4, cudaMemcpyHostToDevice, m.st);
-  }
+  FA_OFF(m.lens.reserve((size_t)B * 4), "device allocation failed (lengths)");
   cudaMemcpyAsync(m.lens.p, lens_h.data(), (size_t)B * 4, cudaMemcpyHostToDevice, m.st);
   const int n_cap = T + 1;
   FA_OFF(m.feats.reserve((size_t)B * T * m.feat_dim * 4) && m.flens.reserve((size_t)B * 4) && m.encb.reserve((size_t)B * T * D * 4) &&
@@ -372,6 +309,87 @@ extern "C" void* fa_offline_infer_hw(void* handle, const void* const* bufs, cons
   return r;
 }
 
+}  // namespace
+
+extern "C" const char* fa_offline_last_error(void) { return g_err.c_str(); }
+extern "C" void* fa_offline_infer_hw(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
+                                     const float* hw_embed, int32_t n_hotwords);
+
+extern "C" void* fa_offline_init(const char* model_file, int32_t device, int32_t gemm_mode) {
+  g_err.clear();
+  if (!model_file) { set_err("model_file is NULL"); return nullptr; }
+  if (gemm_mode != FA_GEMM_F32_SIMT && gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) {
+    set_err("bad gemm_mode"); return nullptr;
+  }
+  if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); set_err("no such CUDA device (this library has no CPU path)"); return nullptr; }
+  Model* m = new Model();
+  m->device = device; m->mode = gemm_mode;
+  if (cudaStreamCreateWithFlags(&m->st, cudaStreamNonBlocking) != cudaSuccess) { set_err("cudaStreamCreate failed"); delete m; return nullptr; }
+  bool ok = false;
+  try {                                   // a malformed file can ask for an absurd allocation: no C++ exception may cross the C ABI
+    ok = load_file(m->t, model_file) && build(*m);
+  } catch (const std::exception& e) {
+    set_err(std::string("model file rejected: ") + e.what());
+  }
+  if (!ok) { delete m; return nullptr; }
+  return m;
+}
+
+extern "C" void fa_offline_uninit(void* handle) { delete static_cast<Model*>(handle); }
+
+extern "C" int32_t fa_offline_is_contextual(const void* handle) { return handle && static_cast<const Model*>(handle)->contextual ? 1 : 0; }
+
+extern "C" const float* fa_offline_host_tensor(void* handle, const char* name, int64_t* numel) {
+  Model* m = static_cast<Model*>(handle);
+  if (numel) *numel = 0;
+  if (!m || !name) return nullptr;
+  auto it = m->t.find(name);
+  if (it == m->t.end()) return nullptr;
+  auto& hc = m->host_cache[name];
+  if (hc.empty() && it->second.numel() > 0) {
+    hc.resize((size_t)it->second.numel());
+    cudaSetDevice(m->device);
+    if (cudaMemcpy(hc.data(), it->second.dev, hc.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess) { hc.clear(); return nullptr; }
+  }
+  if (numel) *numel = (int64_t)hc.size();
+  return hc.data();
+}
+
+extern "C" void* fa_offline_infer(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format) {
+  return fa_offline_infer_hw(handle, bufs, n_samples, batch, pcm_format, nullptr, 0);
+}
+
+extern "C" void* fa_offline_infer_hw(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
+                                     const float* hw_embed, int32_t n_hotwords) {
+  g_err.clear();
+  Model* mp = static_cast<Model*>(handle);
+  if (!mp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) { set_err("bad argument"); return nullptr; }
+  Model& m = *mp;
+  if (m.contextual && (!hw_embed || n_hotwords < 1)) { set_err("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)"); return nullptr; }
+  cudaSetDevice(m.device);
+  int64_t nmax = 0;
+  std::vector<int32_t> lens_h(batch);
+  for (int i = 0; i < batch; ++i) {
+    if (!bufs[i] || n_samples[i] < 400 || n_samples[i] > 0x7fffffffLL) { set_err("every buffer needs >= 400 samples (25 ms)"); return nullptr; }
+    lens_h[i] = (int32_t)n_samples[i];
+    nmax = n_samples[i] > nmax ? n_samples[i] : nmax;
+  }
+  const int B = batch;
+  const int64_t stride = (nmax + 3) / 4 * 4;
+  if (!m.wav.reserve((size_t)B * stride * 4)) { set_err("device allocation failed (waveforms)"); return nullptr; }
+  float* wav = static_cast<float*>(m.wav.p);
+  if (pcm_format == 1) {
+    if (!m.pcm16.reserve((size_t)B * stride * 2)) { set_err("device allocation failed (pcm)"); return nullptr; }
+    int16_t* p16 = static_cast<int16_t*>(m.pcm16.p);
+    for (int i = 0; i < B; ++i) cudaMemcpyAsync(p16 + (int64_t)i * stride, bufs[i], (size_t)n_samples[i] * 2, cudaMemcpyHostToDevice, m.st);
+    const int64_t tot = (int64_t)B * stride;
+    pcm16_to_f32_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, m.st>>>(p16, wav, tot);
+  } else {
+    for (int i = 0; i < B; ++i) cudaMemcpyAsync(wav + (int64_t)i * stride, bufs[i], (size_t)n_samples[i] * 4, cudaMemcpyHostToDevice, m.st);
+  }
+  return decode_batch(m, wav, stride, lens_h, hw_embed, n_hotwords);
+}
+
 extern "C" int32_t fa_offline_result_count(const void* result) { return result ? (int32_t)static_cast<const Result*>(result)->ids.size() : 0; }
 
 extern "C" const int32_t* fa_offline_result_ids(const void* result, int32_t index, int32_t* n_ids) {
@@ -384,3 +402,369 @@ extern "C" const int32_t* fa_offline_result_ids(const void* result, int32_t inde
 extern "C" float fa_offline_result_audio_seconds(const void* result) { return result ? static_cast<const Result*>(result)->audio_seconds : 0.f; }
 
 extern "C" void fa_offline_free_result(void* result) { delete static_cast<Result*>(result); }
+
+// ------------------------------------------------------------------------------------------------ FSMN-VAD handle + long audio
+namespace {
+
+// __vad_config__ of funasr_b200/pack.py:write_vad_model_file: float64 values stored as the bytes of an fp32 tensor (the detector
+// compares in double precision: 0.6 and 1e-4 must arrive unrounded)
+enum { kVadCfgInts = 14, kVadCfgDoubles = 5, kVadCfgLorder = 19, kVadCfgNSil = 20, kVadCfgSil = 21, kVadCfgLen = 25 };
+
+struct Vad {
+  int device = 0;
+  std::map<std::string, Tensor> t;
+  std::vector<void*> owned;                          // padded weights, fbank tables
+  std::vector<FaVadLayer> layers;
+  FaVadEncoder enc{};
+  FaVadOptions opts{};
+  const float* cmvn = nullptr;
+  float* fbank_tables = nullptr;
+  cudaStream_t st = nullptr;
+  DevBuf wav, pcm16, lens, feats, flens, frames, ws;
+  ~Vad() {
+    for (auto& kv : t) if (kv.second.dev) cudaFree(kv.second.dev);
+    for (void* p : owned) cudaFree(p);
+    if (st) cudaStreamDestroy(st);
+  }
+};
+
+struct VadResult {
+  std::vector<int32_t> seg;                          // {start_ms, end_ms} pairs
+  std::vector<float> frames;                         // [2][frames]: silence posterior, frame energy
+  float audio_seconds = 0.f;
+};
+
+bool build_vad(Vad& v) {
+  auto get = [&](const std::string& k) -> const Tensor* {
+    auto it = v.t.find(k);
+    if (it == v.t.end()) { set_err("missing tensor " + k); return nullptr; }
+    return &it->second;
+  };
+  const Tensor* cfg = get("__vad_config__");
+  if (!cfg) return false;
+  if (cfg->numel() != 2 * kVadCfgLen) { set_err("bad __vad_config__"); return false; }
+  double c[kVadCfgLen];
+  if (cudaMemcpy(c, cfg->dev, sizeof(c), cudaMemcpyDeviceToHost) != cudaSuccess) { set_err("cudaMemcpy failed"); return false; }
+  int32_t* oi = &v.opts.sample_rate;                 // the 14 int32 fields, in declaration order
+  for (int k = 0; k < kVadCfgInts; ++k) oi[k] = (int32_t)c[k];
+  v.opts.speech_2_noise_ratio = c[14]; v.opts.snr_thres = c[15]; v.opts.decibel_thres = c[16]; v.opts.speech_noise_thres = c[17];
+  v.opts.fe_prior_thres = c[18];
+  const int lorder = (int)c[kVadCfgLorder], n_sil = (int)c[kVadCfgNSil];
+  if (lorder != 20 || n_sil < 1 || n_sil > 4 || v.opts.frame_in_ms <= 0 || v.opts.window_size_ms < v.opts.frame_in_ms) {
+    set_err("unsupported VAD config"); return false;
+  }
+  const Tensor* mel = get("frontend.mel_banks");
+  const Tensor* win = get("frontend.window");
+  if (!mel || !win) return false;
+  void* tb = nullptr;
+  if (cudaMalloc(&tb, fa_fbank_tables_bytes()) != cudaSuccess) { set_err("cudaMalloc fbank tables"); return false; }
+  v.owned.push_back(tb);
+  v.fbank_tables = static_cast<float*>(tb);
+  if (fa_fbank_make_tables(mel->dev, win->dev, v.fbank_tables, v.st) != FA_OK) { set_err("fa_fbank_make_tables failed"); return false; }
+  if (v.t.count("frontend.cmvn")) {
+    if (v.t["frontend.cmvn"].numel() != 2 * 400) { set_err("frontend.cmvn must be [2, 400]"); return false; }
+    v.cmvn = v.t["frontend.cmvn"].dev;
+  }
+  bool ok = true;
+  // weights [out, in] -> [out, in rounded up to 16] with zero columns (VadEngine._lin): the fp32 GEMMs read K = the padded width
+  auto lin = [&](const std::string& p, bool bias) -> FaLinear {
+    FaLinear L{};
+    const Tensor* w = get(p + ".weight");
+    if (!w || w->shape.size() != 2) { if (ok && w) set_err("bad weight " + p); ok = false; return L; }
+    const int out_f = (int)w->shape[0], in_f = (int)w->shape[1], kp = (in_f + 15) / 16 * 16;
+    void* wp = nullptr;
+    if (cudaMalloc(&wp, (size_t)out_f * kp * 4) != cudaSuccess) { set_err("cudaMalloc weights"); ok = false; return L; }
+    v.owned.push_back(wp);
+    if (cudaMemset(wp, 0, (size_t)out_f * kp * 4) != cudaSuccess ||
+        cudaMemcpy2D(wp, (size_t)kp * 4, w->dev, (size_t)in_f * 4, (size_t)in_f * 4, out_f, cudaMemcpyDeviceToDevice) != cudaSuccess) {
+      set_err("weight copy failed"); ok = false; return L;
+    }
+    L.w = static_cast<const float*>(wp);
+    if (bias) {
+      const Tensor* b = get(p + ".bias");
+      if (!b || b->numel() != out_f) { if (ok && b) set_err("bad bias " + p); ok = false; return L; }
+      L.b = b->dev;
+    }
+    L.out_f = out_f; L.in_f = kp; L.in_pad = kp;
+    return L;
+  };
+  int n_layers = 0;
+  while (v.t.count("encoder.fsmn." + std::to_string(n_layers) + ".linear.linear.weight")) ++n_layers;
+  v.layers.resize(n_layers > 0 ? n_layers : 1);
+  v.enc.in1 = lin("encoder.in_linear1.linear", true);
+  v.enc.in2 = lin("encoder.in_linear2.linear", true);
+  for (int i = 0; i < n_layers && ok; ++i) {
+    const std::string p = "encoder.fsmn." + std::to_string(i) + ".";
+    if (v.t.count(p + "fsmn_block.conv_right.weight")) { set_err("FSMN-VAD with a right-context memory (rorder > 0) is not supported"); return false; }
+    v.layers[i].lin = lin(p + "linear.linear", false);
+    const Tensor* cw = get(p + "fsmn_block.conv_left.weight");   // [proj, 1, lorder, 1] = [proj, lorder] contiguous
+    if (!cw || cw->shape.size() != 4 || cw->shape[1] != 1 || cw->shape[2] != lorder || cw->shape[3] != 1) {
+      if (ok && cw) set_err("bad " + p + "fsmn_block.conv_left.weight");
+      return false;
+    }
+    v.layers[i].conv_w = cw->dev;
+    v.layers[i].affine = lin(p + "affine.linear", true);
+  }
+  v.enc.layers = v.layers.data(); v.enc.n_layers = n_layers; v.enc.lorder = lorder;
+  v.enc.out1 = lin("encoder.out_linear1.linear", true);
+  v.enc.out2 = lin("encoder.out_linear2.linear", true);
+  for (int k = 0; k < n_sil; ++k) v.enc.sil_ids[k] = (int32_t)c[kVadCfgSil + k];
+  v.enc.n_sil = n_sil;
+  if (!ok) return false;
+  if (v.enc.in1.in_f != 400) { set_err("the VAD frontend is 80 mel x LFR 5: in_linear1 must take 400 inputs"); return false; }
+  for (int k = 0; k < n_sil; ++k)
+    if (v.enc.sil_ids[k] < 0 || v.enc.sil_ids[k] >= v.enc.out2.out_f) { set_err("sil_pdf_ids outside the output"); return false; }
+  return cudaStreamSynchronize(v.st) == cudaSuccess;
+}
+
+const double kSilenceSchedule[] = {10000, 2000, 20000, 1000, 30000, 800, 40000, 600, 50000, 400, 60000, 200, -1, 100};   // vad.py
+
+// VAD of one device-resident recording wav [n] fp32 on stream st (the VAD's own, or the recogniser's in fa_offline_infer_vad)
+bool vad_run(Vad& v, const float* wav, int64_t n, cudaStream_t st, const FaVadRunOptions& ro, VadResult& out) {
+  out.audio_seconds = (float)((double)n / 16000.0);
+  const int64_t T = n >= 400 ? (n - 400) / 160 + 1 : 0;
+  out.seg.clear();
+  out.frames.assign((size_t)(2 * T), 0.f);
+  if (T == 0) return true;                                   // shorter than one frame: nothing to score
+  const int32_t n32 = (int32_t)n;
+  const size_t ws = fa_fsmn_vad_workspace_bytes(&v.enc, (int32_t)T);
+  if (!(v.lens.reserve(4) && v.feats.reserve((size_t)T * 400 * 4) && v.flens.reserve(4) && v.frames.reserve((size_t)T * 8) && v.ws.reserve(ws))) {
+    set_err("device allocation failed (VAD)"); return false;
+  }
+  float* frames = static_cast<float*>(v.frames.p);
+  cudaMemcpyAsync(v.lens.p, &n32, 4, cudaMemcpyHostToDevice, st);
+  int rc = fa_fbank_lfr_cmvn_tables(wav, static_cast<int32_t*>(v.lens.p), 1, n, v.cmvn, v.fbank_tables, 5, 1, static_cast<float*>(v.feats.p), T,
+                                    static_cast<int32_t*>(v.flens.p), (int32_t)T, st);
+  if (rc == FA_OK) rc = fa_fsmn_vad_forward(&v.enc, static_cast<float*>(v.feats.p), 400, (int32_t)T, frames, nullptr, v.ws.p, v.ws.cap, st);
+  if (rc == FA_OK) rc = fa_frame_decibels(wav, n, (int32_t)T, frames + T, st);
+  if (rc != FA_OK) { set_err(std::string("VAD: ") + fa_status_string(rc)); return false; }
+  cudaMemcpyAsync(out.frames.data(), frames, (size_t)T * 8, cudaMemcpyDeviceToHost, st);     // the one copy back: two floats per frame
+  if (cudaStreamSynchronize(st) != cudaSuccess) { set_err(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError())); return false; }
+  std::vector<double> sil(out.frames.begin(), out.frames.begin() + T), db(out.frames.begin() + T, out.frames.end());
+  FaVadOptions o = v.opts;
+  if (!ro.dynamic_silence && ro.max_end_silence_time > 0) o.max_end_silence_time = ro.max_end_silence_time;
+  std::vector<int32_t> seg(128);
+  for (;;) {
+    const int64_t cap = (int64_t)seg.size() / 2;
+    const int64_t k = fa_vad_detect_segments(sil.data(), db.data(), T, n, &o, 60000, ro.dynamic_silence ? 1 : 0, kSilenceSchedule,
+                                             (int32_t)(sizeof(kSilenceSchedule) / sizeof(double) / 2), ro.speech_noise_thres, seg.data(), cap);
+    if (k < 0) { set_err("fa_vad_detect_segments failed: posteriors must lie inside (0, 1)"); return false; }
+    if (k <= cap) { seg.resize((size_t)(2 * k)); break; }
+    seg.resize((size_t)(2 * k));
+  }
+  out.seg.swap(seg);
+  return true;
+}
+
+FaVadRunOptions default_vad_run() {
+  FaVadRunOptions r;
+  r.dynamic_silence = 1; r.max_end_silence_time = 0; r.speech_noise_thres = NAN;
+  return r;
+}
+
+// one recording (host) -> fp32 on the device in `dst` (s16 through `pcm16`)
+bool upload(const void* buf, int64_t n, int32_t pcm_format, DevBuf& dst, DevBuf& pcm16, cudaStream_t st) {
+  const int64_t cap = (n + 3) / 4 * 4;
+  if (!dst.reserve((size_t)(cap > 0 ? cap : 4) * 4)) { set_err("device allocation failed (recording)"); return false; }
+  float* wav = static_cast<float*>(dst.p);
+  if (n == 0) return true;
+  if (pcm_format == 1) {
+    if (!pcm16.reserve((size_t)n * 2)) { set_err("device allocation failed (pcm)"); return false; }
+    cudaMemcpyAsync(pcm16.p, buf, (size_t)n * 2, cudaMemcpyHostToDevice, st);
+    pcm16_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(static_cast<const int16_t*>(pcm16.p), wav, n);
+  } else {
+    cudaMemcpyAsync(wav, buf, (size_t)n * 4, cudaMemcpyHostToDevice, st);
+  }
+  return true;
+}
+
+// four consecutive output columns per thread: scalar reads (a segment starts anywhere), one 16-byte store
+__global__ void __launch_bounds__(256)
+gather_segments_kernel(const float* __restrict__ rec, int64_t n_rec, const int64_t* __restrict__ starts, const int32_t* __restrict__ lens,
+                       int64_t stride, float* __restrict__ out) {
+  const int r = blockIdx.y;
+  const int64_t c = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+  if (c >= stride) return;
+  const int64_t s = starts[r];
+  const int32_t len = lens[r];
+  float v[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int64_t j = c + k, src = s + j;
+    v[k] = (j < len && src >= 0 && src < n_rec) ? rec[src] : 0.f;
+  }
+  *reinterpret_cast<float4*>(out + (int64_t)r * stride + c) = make_float4(v[0], v[1], v[2], v[3]);
+}
+
+}  // namespace
+
+extern "C" int fa_gather_segments(const float* rec, int64_t n_rec, const int64_t* starts, const int32_t* lens, int32_t rows, int64_t stride,
+                                  float* out, fa_stream_t stream) {
+  if (rows < 0 || rows > 65535 || n_rec < 0 || (rows > 0 && (!rec || !starts || !lens || !out || stride <= 0))) return FA_ERR_ARG;
+  if (rows == 0) return FA_OK;
+  if (stride % 4 || reinterpret_cast<uintptr_t>(out) % 16) return FA_ERR_UNSUPPORTED;
+  const int64_t blocks = (stride / 4 + 255) / 256;
+  if (blocks > 0x7fffffffLL) return FA_ERR_ARG;
+  gather_segments_kernel<<<dim3((unsigned)blocks, (unsigned)rows), 256, 0, (cudaStream_t)stream>>>(rec, n_rec, starts, lens, stride, out);
+  FA_CHECK_LAUNCH();
+  return FA_OK;
+}
+
+extern "C" void* fa_vad_init(const char* model_file, int32_t device) {
+  g_err.clear();
+  if (!model_file) { set_err("model_file is NULL"); return nullptr; }
+  if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); set_err("no such CUDA device (this library has no CPU path)"); return nullptr; }
+  Vad* v = new Vad();
+  v->device = device;
+  if (cudaStreamCreateWithFlags(&v->st, cudaStreamNonBlocking) != cudaSuccess) { set_err("cudaStreamCreate failed"); delete v; return nullptr; }
+  bool ok = false;
+  try {                                   // no C++ exception may cross the C ABI
+    ok = load_file(v->t, model_file) && build_vad(*v);
+  } catch (const std::exception& e) {
+    set_err(std::string("model file rejected: ") + e.what());
+  }
+  if (!ok) { delete v; return nullptr; }
+  return v;
+}
+
+extern "C" void fa_vad_uninit(void* vad) { delete static_cast<Vad*>(vad); }
+
+extern "C" void* fa_vad_infer(void* vad, const void* buf, int64_t n_samples, int32_t pcm_format, const FaVadRunOptions* opts) {
+  g_err.clear();
+  Vad* v = static_cast<Vad*>(vad);
+  if (!v || (!buf && n_samples > 0) || n_samples < 0 || n_samples > 0x7fffffffLL || (pcm_format != 0 && pcm_format != 1)) {
+    set_err("bad argument"); return nullptr;
+  }
+  cudaSetDevice(v->device);
+  VadResult* r = new VadResult();
+  try {
+    if (!upload(buf, n_samples, pcm_format, v->wav, v->pcm16, v->st) ||
+        !vad_run(*v, static_cast<const float*>(v->wav.p), n_samples, v->st, opts ? *opts : default_vad_run(), *r)) {
+      delete r; return nullptr;
+    }
+  } catch (const std::exception& e) {
+    set_err(std::string("fa_vad_infer: ") + e.what()); delete r; return nullptr;
+  }
+  return r;
+}
+
+extern "C" const int32_t* fa_vad_result_segments(const void* result, int64_t* n_segments) {
+  const VadResult* r = static_cast<const VadResult*>(result);
+  if (n_segments) *n_segments = r ? (int64_t)r->seg.size() / 2 : 0;
+  return r && !r->seg.empty() ? r->seg.data() : nullptr;
+}
+
+extern "C" const float* fa_vad_result_frames(const void* result, int64_t* frames) {
+  const VadResult* r = static_cast<const VadResult*>(result);
+  if (frames) *frames = r ? (int64_t)r->frames.size() / 2 : 0;
+  return r && !r->frames.empty() ? r->frames.data() : nullptr;
+}
+
+extern "C" float fa_vad_result_audio_seconds(const void* result) { return result ? static_cast<const VadResult*>(result)->audio_seconds : 0.f; }
+
+extern "C" void fa_vad_free_result(void* result) { delete static_cast<VadResult*>(result); }
+
+namespace {
+
+// one recording of fa_offline_infer_vad: inference_with_vad (auto_model.py:852-1035, funasr_b200/long_audio.py:LongAudioPipeline.generate)
+bool long_audio_one(Model& m, Vad& v, int rec_index, const void* buf, int64_t n, int32_t pcm_format, const float* hw_embed, int32_t n_hotwords,
+                    const FaLongAudioOptions& o, std::vector<int32_t>& ids, std::vector<int32_t>& segs_out) {
+  if (!upload(buf, n, pcm_format, m.rec, m.pcm16, m.st)) return false;
+  const float* rec = static_cast<const float*>(m.rec.p);
+  VadResult vr;
+  if (!vad_run(v, rec, n, m.st, o.vad, vr)) return false;
+  std::vector<int32_t> segs = vr.seg;
+  if (o.merge_vad) {
+    segs.resize(2 * vr.seg.size() + 2);
+    const int64_t k = fa_merge_vad(vr.seg.data(), (int64_t)vr.seg.size() / 2, o.merge_length_s * 1000, 0, segs.data());
+    if (k < 0) { set_err("fa_merge_vad failed"); return false; }
+    segs.resize((size_t)(2 * k));
+  }
+  const int64_t ns = (int64_t)segs.size() / 2;
+  if (ns == 0) return true;                                  // no speech: no segment, no id
+  std::vector<int32_t> order((size_t)ns), packs((size_t)(2 * ns));
+  const int64_t np = fa_pack_segments(segs.data(), ns, o.batch_size_s, o.batch_size_threshold_s, order.data(), packs.data());
+  if (np < 0) { set_err("fa_pack_segments failed"); return false; }
+  std::vector<std::vector<int32_t>> seg_ids((size_t)ns);
+  bool emptied = false;
+  for (int64_t p = 0; p < np && !emptied; ++p) {
+    const int beg = packs[2 * p], end = packs[2 * p + 1], B = end - beg;
+    std::vector<int64_t> starts(B);
+    std::vector<int32_t> lens(B);
+    int64_t lmax = 0;
+    for (int j = 0; j < B; ++j) {                            // slice_padding_audio_samples (utils/vad_utils.py:44-51)
+      const int s = order[beg + j];
+      const int64_t b0 = (int64_t)segs[2 * s] * 16, b1 = std::min<int64_t>((int64_t)segs[2 * s + 1] * 16, n), len = b1 - b0;
+      if (len < 400) {
+        set_err("recording " + std::to_string(rec_index) + ": VAD segment " + std::to_string(s) + " [" + std::to_string(segs[2 * s]) + ", " +
+                std::to_string(segs[2 * s + 1]) + "] ms has " + std::to_string(len > 0 ? len : 0) + " samples; the recogniser needs >= 400 (25 ms)");
+        return false;
+      }
+      starts[j] = b0; lens[j] = (int32_t)len;
+      lmax = len > lmax ? len : lmax;
+    }
+    const int64_t stride = (lmax + 3) / 4 * 4;
+    if (!(m.gmeta.reserve((size_t)B * 12) && m.wav.reserve((size_t)B * stride * 4))) { set_err("device allocation failed (segments)"); return false; }
+    int64_t* starts_d = static_cast<int64_t*>(m.gmeta.p);
+    int32_t* lens_d = reinterpret_cast<int32_t*>(starts_d + B);
+    cudaMemcpyAsync(starts_d, starts.data(), (size_t)B * 8, cudaMemcpyHostToDevice, m.st);
+    cudaMemcpyAsync(lens_d, lens.data(), (size_t)B * 4, cudaMemcpyHostToDevice, m.st);
+    float* wav = static_cast<float*>(m.wav.p);
+    const int rc = fa_gather_segments(rec, n, starts_d, lens_d, B, stride, wav, m.st);
+    if (rc != FA_OK) { set_err(std::string("fa_gather_segments: ") + fa_status_string(rc)); return false; }
+    Result* pr = decode_batch(m, wav, stride, lens, hw_embed, n_hotwords);
+    if (!pr) return false;
+    int tmax = 0;
+    for (int32_t t : pr->token_num) tmax = t > tmax ? t : tmax;
+    if (tmax < 1) emptied = true;                            // no token in the whole pack: the recording's result is empty (:990-999)
+    else for (int j = 0; j < B; ++j) seg_ids[order[beg + j]].swap(pr->ids[j]);
+    delete pr;
+  }
+  for (int64_t s = 0; s < ns; ++s) {
+    const int32_t k = emptied ? 0 : (int32_t)seg_ids[s].size();
+    segs_out.insert(segs_out.end(), {segs[2 * s], segs[2 * s + 1], k});
+    if (!emptied) ids.insert(ids.end(), seg_ids[s].begin(), seg_ids[s].end());
+  }
+  return true;
+}
+
+}  // namespace
+
+extern "C" void* fa_offline_infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
+                                      const float* hw_embed, int32_t n_hotwords, const FaLongAudioOptions* opts) {
+  g_err.clear();
+  Model* mp = static_cast<Model*>(asr);
+  Vad* vp = static_cast<Vad*>(vad);
+  if (!mp || !vp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) { set_err("bad argument"); return nullptr; }
+  if (mp->device != vp->device) { set_err("the recogniser and the VAD live on different devices"); return nullptr; }
+  if (mp->contextual && (!hw_embed || n_hotwords < 1)) { set_err("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)"); return nullptr; }
+  FaLongAudioOptions o;
+  if (opts) o = *opts;
+  else { o.batch_size_s = 300; o.batch_size_threshold_s = 60; o.merge_vad = 0; o.merge_length_s = 15; o.vad = default_vad_run(); }
+  for (int i = 0; i < batch; ++i)
+    if ((!bufs[i] && n_samples[i] > 0) || n_samples[i] < 0 || n_samples[i] > 0x7fffffffLL) { set_err("bad recording " + std::to_string(i)); return nullptr; }
+  cudaSetDevice(mp->device);
+  Result* r = new Result();
+  r->ids.resize(batch);
+  r->segs.resize(batch);
+  r->token_num.assign(batch, 0);
+  double seconds = 0.0;
+  try {
+    for (int i = 0; i < batch; ++i) {
+      seconds += (double)n_samples[i] / 16000.0;
+      if (!long_audio_one(*mp, *vp, i, bufs[i], n_samples[i], pcm_format, hw_embed, n_hotwords, o, r->ids[i], r->segs[i])) { delete r; return nullptr; }
+      r->token_num[i] = (int32_t)r->ids[i].size();
+    }
+  } catch (const std::exception& e) {
+    set_err(std::string("fa_offline_infer_vad: ") + e.what()); delete r; return nullptr;
+  }
+  r->audio_seconds = (float)seconds;
+  return r;
+}
+
+extern "C" const int32_t* fa_offline_result_segments(const void* result, int32_t index, int32_t* n_segments) {
+  const Result* r = static_cast<const Result*>(result);
+  if (!r || index < 0 || index >= (int32_t)r->segs.size() || r->segs[index].empty()) { if (n_segments) *n_segments = 0; return nullptr; }
+  if (n_segments) *n_segments = (int32_t)(r->segs[index].size() / 3);
+  return r->segs[index].data();
+}

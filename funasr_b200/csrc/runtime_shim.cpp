@@ -2,7 +2,8 @@
 // their exact C++ signatures, over this library's handle API (offline.cu: fa_offline_*).  Host-only C++: file / buffer decoding
 // (raw s16le PCM, RIFF WAV PCM16 / float32), the hotword encoder of ContextualParaformer (Embedding + 1-layer LSTM, O(#hotwords):
 // the reference runs it on the CPU too — model_eb.onnx, runtime/onnxruntime/src/paraformer.cpp CompileHotwordEmbedding) and the
-// ids -> text join.  Everything per audio frame runs in fa_offline_infer_hw on the GPU.
+// ids -> text join.  Everything per audio frame runs in fa_offline_infer_hw on the GPU — or, with a VAD model ("vad-dir"), in
+// fa_offline_infer_vad.  FsmnVad* are the runtime's VAD entry points over fa_vad_infer.
 #include "../../include/funasrruntime_b200.h"
 #include "../../include/funasr_b200.h"
 
@@ -18,10 +19,33 @@ thread_local std::string g_shim_err;
 
 struct OfflineStream {
   void* h = nullptr;
+  void* vad = nullptr;                 // fa_vad_init handle when model_path["vad-dir"] is given
+  int batch_size_s = 300;
   std::vector<std::string> vocab;
   std::unordered_map<std::string, int> token_id;
   int batch = 1;
 };
+
+struct VadStream {
+  void* v = nullptr;
+};
+
+struct VadShimResult {
+  std::vector<std::vector<int>> segments;
+  float snippet_time = 0.f;
+};
+
+// the C++ runtime's VAD reads a fixed max_end_silence_time from its config (fsmn-vad.cpp) and has no dynamic schedule
+FaVadRunOptions runtime_vad_options() {
+  FaVadRunOptions o;
+  o.dynamic_silence = 0; o.max_end_silence_time = 0; o.speech_noise_thres = NAN;
+  return o;
+}
+
+int parse_device(std::map<std::string, std::string>& model_path) {
+  auto gi = model_path.find("gpu-id");
+  return gi != model_path.end() ? atoi(gi->second.c_str()) : 0;
+}
 
 struct ShimResult {
   std::vector<std::string> msgs;
@@ -116,6 +140,25 @@ FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, int 
   }
   const void* bufs[1] = {data};
   const int64_t lens[1] = {n};
+  if (s->vad) {                        // segment texts concatenated in time order (funasrruntime.cpp:287-296)
+    FaLongAudioOptions o;
+    o.batch_size_s = s->batch_size_s; o.batch_size_threshold_s = 60; o.merge_vad = 0; o.merge_length_s = 15; o.vad = runtime_vad_options();
+    void* r = fa_offline_infer_vad(s->h, s->vad, bufs, lens, 1, fmt, n_hw ? hw.data() : nullptr, n_hw, &o);
+    if (!r) { g_shim_err = fa_offline_last_error(); return nullptr; }
+    int32_t k = 0, nseg = 0;
+    const int32_t* ids = fa_offline_result_ids(r, 0, &k);
+    const int32_t* seg = fa_offline_result_segments(r, 0, &nseg);
+    std::string text;
+    for (int32_t i = 0, pos = 0; i < nseg && ids; ++i) {
+      text += join_tokens(*s, ids + pos, seg[3 * i + 2]);
+      pos += seg[3 * i + 2];
+    }
+    ShimResult* out = new ShimResult();
+    out->msgs.push_back(text);
+    out->snippet_time = fa_offline_result_audio_seconds(r);
+    fa_offline_free_result(r);
+    return out;
+  }
   void* r = fa_offline_infer_hw(s->h, bufs, lens, 1, fmt, n_hw ? hw.data() : nullptr, n_hw);
   if (!r) { g_shim_err = fa_offline_last_error(); return nullptr; }
   ShimResult* out = new ShimResult();
@@ -148,12 +191,19 @@ FUNASR_HANDLE FunOfflineInit(std::map<std::string, std::string>& model_path, int
     else if (gm->second == "fp16x6") mode = FA_GEMM_F16X6;
     else if (gm->second != "fp16x3") { g_shim_err = "unknown gemm-mode " + gm->second; return nullptr; }
   }
-  auto gi = model_path.find("gpu-id");
-  if (gi != model_path.end()) device = atoi(gi->second.c_str());
+  device = parse_device(model_path);
   OfflineStream* s = new OfflineStream();
   s->batch = batch_size > 0 ? batch_size : 1;
+  auto bs = model_path.find("batch-size-s");
+  if (bs != model_path.end()) s->batch_size_s = atoi(bs->second.c_str());
+  if (s->batch_size_s <= 0) { g_shim_err = "batch-size-s must be a positive number of seconds"; delete s; return nullptr; }
   s->h = fa_offline_init((dir + "/model.fab2").c_str(), device, mode);
   if (!s->h) { g_shim_err = fa_offline_last_error(); delete s; return nullptr; }
+  auto vd = model_path.find("vad-dir");
+  if (vd != model_path.end()) {
+    s->vad = fa_vad_init((vd->second + "/vad.fab2").c_str(), device);
+    if (!s->vad) { g_shim_err = fa_offline_last_error(); fa_offline_uninit(s->h); delete s; return nullptr; }
+  }
   std::ifstream tf(dir + "/tokens.txt");
   std::string line;
   while (tf && std::getline(tf, line)) {
@@ -170,6 +220,7 @@ void FunOfflineUninit(FUNASR_HANDLE handle) {
   OfflineStream* s = static_cast<OfflineStream*>(handle);
   if (!s) return;
   fa_offline_uninit(s->h);
+  fa_vad_uninit(s->vad);
   delete s;
 }
 
@@ -275,6 +326,71 @@ const char* FunASRGetStampSents(FUNASR_RESULT result) { return result ? static_c
 const int FunASRGetRetNumber(FUNASR_RESULT result) { return result ? (int)static_cast<ShimResult*>(result)->msgs.size() : 0; }
 void FunASRFreeResult(FUNASR_RESULT result) { delete static_cast<ShimResult*>(result); }
 const float FunASRGetRetSnippetTime(FUNASR_RESULT result) { return result ? static_cast<ShimResult*>(result)->snippet_time : 0.f; }
+
+FUNASR_HANDLE FsmnVadInit(std::map<std::string, std::string>& model_path, int thread_num) {
+  (void)thread_num;
+  g_shim_err.clear();
+  auto it = model_path.find("model-dir");
+  if (it == model_path.end()) { g_shim_err = "model_path[\"model-dir\"] is missing"; return nullptr; }
+  VadStream* s = new VadStream();
+  s->v = fa_vad_init((it->second + "/vad.fab2").c_str(), parse_device(model_path));
+  if (!s->v) { g_shim_err = fa_offline_last_error(); delete s; return nullptr; }
+  return s;
+}
+
+FUNASR_RESULT FsmnVadInferBuffer(FUNASR_HANDLE handle, const char* sz_buf, int n_len, QM_CALLBACK fn_callback, bool input_finished, int sampling_rate,
+                                 std::string wav_format) {
+  g_shim_err.clear();
+  VadStream* s = static_cast<VadStream*>(handle);
+  if (!s || !sz_buf || n_len <= 0) { g_shim_err = "bad argument"; return nullptr; }
+  if (!input_finished) { g_shim_err = "only offline VAD is provided: input_finished must be true"; return nullptr; }
+  const char* data = sz_buf;
+  size_t nb = (size_t)n_len;
+  int fmt = 1, rate = sampling_rate;
+  std::string holder;
+  if (wav_format == "wav") {
+    holder.assign(sz_buf, (size_t)n_len);
+    if (!parse_wav(holder, &data, &nb, &fmt, &rate)) { g_shim_err = "unsupported WAV (need mono PCM16 or float32)"; return nullptr; }
+  } else if (wav_format != "pcm" && wav_format != "PCM") { g_shim_err = "wav_format must be \"pcm\" (s16le) or \"wav\""; return nullptr; }
+  if (rate != 16000) { g_shim_err = "audio must be 16 kHz"; return nullptr; }
+  const FaVadRunOptions o = runtime_vad_options();
+  void* r = fa_vad_infer(s->v, data, (int64_t)(nb / (fmt == 1 ? 2 : 4)), fmt, &o);
+  if (!r) { g_shim_err = fa_offline_last_error(); return nullptr; }
+  VadShimResult* out = new VadShimResult();
+  int64_t n = 0;
+  const int32_t* seg = fa_vad_result_segments(r, &n);
+  for (int64_t i = 0; i < n; ++i) out->segments.push_back({seg[2 * i], seg[2 * i + 1]});
+  out->snippet_time = fa_vad_result_audio_seconds(r);
+  fa_vad_free_result(r);
+  if (fn_callback) fn_callback(1, 1);
+  return out;
+}
+
+FUNASR_RESULT FsmnVadInfer(FUNASR_HANDLE handle, const char* sz_filename, QM_CALLBACK fn_callback, int sampling_rate) {
+  g_shim_err.clear();
+  if (!sz_filename) { g_shim_err = "bad argument"; return nullptr; }
+  std::ifstream f(sz_filename, std::ios::binary);
+  if (!f) { g_shim_err = std::string("cannot open ") + sz_filename; return nullptr; }
+  std::stringstream ss;
+  ss << f.rdbuf();
+  const std::string bytes = ss.str();
+  const std::string name = sz_filename;
+  const bool wav = name.size() > 4 && (name.compare(name.size() - 4, 4, ".wav") == 0 || name.compare(name.size() - 4, 4, ".WAV") == 0);
+  return FsmnVadInferBuffer(handle, bytes.data(), (int)bytes.size(), fn_callback, true, sampling_rate, wav ? "wav" : "pcm");
+}
+
+std::vector<std::vector<int>>* FsmnVadGetResult(FUNASR_RESULT result, int n_index) {
+  VadShimResult* r = static_cast<VadShimResult*>(result);
+  return r && n_index == 0 ? &r->segments : nullptr;
+}
+void FsmnVadFreeResult(FUNASR_RESULT result) { delete static_cast<VadShimResult*>(result); }
+void FsmnVadUninit(FUNASR_HANDLE handle) {
+  VadStream* s = static_cast<VadStream*>(handle);
+  if (!s) return;
+  fa_vad_uninit(s->v);
+  delete s;
+}
+const float FsmnVadGetRetSnippetTime(FUNASR_RESULT result) { return result ? static_cast<VadShimResult*>(result)->snippet_time : 0.f; }
 
 FUNASR_DEC_HANDLE FunASRWfstDecoderInit(FUNASR_HANDLE, int, float, float, float) { return nullptr; }
 void FunASRWfstDecoderUninit(FUNASR_DEC_HANDLE) {}

@@ -249,3 +249,58 @@ extern "C" int64_t fa_vad_detect_segments(const double* sil_prob, const double* 
   }
   return (int64_t)found.size();
 }
+
+// What inference_with_vad does with the segments before decoding (funasr_b200/long_audio.py: pack_segments, vad.py: merge_vad stay the
+// specification; tests hold the two identical).
+extern "C" int64_t fa_pack_segments(const int32_t* segments, int64_t n, int32_t batch_size_s, int32_t batch_size_threshold_s, int32_t* order,
+                                    int32_t* packs) {
+  if (n < 0 || n > 0x7fffffff || (n > 0 && (!segments || !order || !packs))) return FA_ERR_ARG;
+  if (n == 0) return 0;
+  auto len = [&](int64_t i) { return (int64_t)segments[2 * i + 1] - (int64_t)segments[2 * i]; };
+  std::vector<int32_t> idx((size_t)n);
+  for (int64_t i = 0; i < n; ++i) idx[(size_t)i] = (int32_t)i;
+  std::stable_sort(idx.begin(), idx.end(), [&](int32_t a, int32_t b) { return len(a) < len(b); });   // ties keep time order
+  for (int64_t i = 0; i < n; ++i) order[i] = idx[(size_t)i];
+  int64_t batch_size = std::max<int64_t>((int64_t)batch_size_s * 1000, 1);
+  const int64_t threshold_ms = (int64_t)batch_size_threshold_s * 1000;
+  batch_size = std::max(batch_size, len(idx[0]));
+  int64_t n_packs = 0, beg = 0, end = 1, max_len = 0;
+  for (int64_t j = 0; j < n; ++j) {
+    const int64_t length = len(idx[(size_t)j]);
+    const int64_t potential = std::max(max_len, length) * (j + 1 - beg);
+    if (j < n - 1 && length < threshold_ms && potential < batch_size) {
+      max_len = std::max(max_len, length);
+      ++end;
+      continue;
+    }
+    packs[2 * n_packs] = (int32_t)beg;
+    packs[2 * n_packs + 1] = (int32_t)end;
+    ++n_packs;
+    beg = end;
+    ++end;
+    max_len = length;
+  }
+  return n_packs;
+}
+
+extern "C" int64_t fa_merge_vad(const int32_t* segments, int64_t n, int32_t max_length_ms, int32_t min_length_ms, int32_t* out) {
+  if (n < 0 || (n > 0 && (!segments || !out))) return FA_ERR_ARG;
+  if (n <= 1) {                                              // returned as given
+    for (int64_t i = 0; i < 2 * n; ++i) out[i] = segments[i];
+    return n;
+  }
+  std::vector<int32_t> steps(segments, segments + 2 * n);
+  std::sort(steps.begin(), steps.end());
+  steps.erase(std::unique(steps.begin(), steps.end()), steps.end());
+  int64_t cnt = 0;
+  int64_t bg = 0;
+  for (size_t i = 0; i + 1 < steps.size(); ++i) {
+    const int64_t time = steps[i];
+    if ((int64_t)steps[i + 1] - bg < max_length_ms) continue;
+    if (time - bg > min_length_ms) { out[2 * cnt] = (int32_t)bg; out[2 * cnt + 1] = (int32_t)time; ++cnt; }
+    bg = time;
+  }
+  out[2 * cnt] = (int32_t)bg;
+  out[2 * cnt + 1] = steps.back();
+  return cnt + 1;
+}

@@ -1,14 +1,77 @@
 """ctypes binding of the handle-style C API (include/funasr_b200.h: fa_offline_*), the counterpart of FunASR's C++ runtime
 FunOfflineInit / FunOfflineInferBuffer / FunASRGetResult (runtime/onnxruntime/include/funasrruntime.h:100-116).
-Nothing here touches torch on the data path: host PCM buffers in, token ids out."""
+Nothing here touches torch on the data path: host PCM buffers in, token ids out.  `OfflineVad` binds the FSMN-VAD handle
+(fa_vad_*) and `OfflineRecognizer.infer_long` the long-audio entry (fa_offline_infer_vad): VAD segments packed by duration and decoded
+batch by batch, the same results as LongAudioPipeline.generate."""
 from __future__ import annotations
 
 import ctypes as C
-from typing import List, Sequence
+from typing import List, Optional, Sequence
 
 import numpy as np
 
 from . import _abi
+
+
+def _pcm_batch(wavs):
+    arrs = [np.ascontiguousarray(w) for w in wavs]
+    kinds = {a.dtype for a in arrs}
+    if kinds == {np.dtype(np.float32)}:
+        fmt = 0
+    elif kinds == {np.dtype(np.int16)}:
+        fmt = 1
+    else:
+        raise _abi.FunasrB200Error("waveforms must all be float32 or all be int16, got %s" % kinds)
+    return arrs, fmt
+
+
+def _vad_run_options(max_end_silence_time: Optional[int] = None, speech_noise_thres: Optional[float] = None,
+                     dynamic_silence: Optional[bool] = None) -> "_abi.FaVadRunOptions":
+    """FsmnVADStreamingB200.inference's keywords: an explicit max_end_silence_time switches the dynamic schedule off."""
+    if dynamic_silence is None:
+        dynamic_silence = max_end_silence_time is None
+    return _abi.FaVadRunOptions(1 if dynamic_silence else 0, int(max_end_silence_time or 0),
+                                float("nan") if speech_noise_thres is None else float(speech_noise_thres))
+
+
+class OfflineVad:
+    """ctypes binding of fa_vad_init / fa_vad_infer: FSMN-VAD from a model file written by pack.write_vad_model_file."""
+
+    def __init__(self, model_file: str, device: int = 0):
+        self.lib = _abi.load()
+        self.handle = self.lib.fa_vad_init(model_file.encode(), device)
+        if not self.handle:
+            raise _abi.FunasrB200Error("fa_vad_init failed: %s" % self.lib.fa_offline_last_error().decode())
+
+    def segments(self, wav: np.ndarray, want_frames: bool = False, **vad_kwargs):
+        """wav: float32 in [-1, 1] or int16, 16 kHz mono -> [[start_ms, end_ms], ...] (and the [2, frames] silence posterior / energy)."""
+        (a,), fmt = _pcm_batch([wav])
+        opts = _vad_run_options(**vad_kwargs)
+        res = self.lib.fa_vad_infer(self.handle, a.ctypes.data, a.shape[0], fmt, C.byref(opts))
+        if not res:
+            raise _abi.FunasrB200Error("fa_vad_infer failed: %s" % self.lib.fa_offline_last_error().decode())
+        try:
+            n = C.c_int64(0)
+            p = self.lib.fa_vad_result_segments(res, C.byref(n))
+            segs = [[int(p[2 * i]), int(p[2 * i + 1])] for i in range(n.value)]
+            if not want_frames:
+                return segs
+            f = self.lib.fa_vad_result_frames(res, C.byref(n))
+            frames = np.ctypeslib.as_array(f, shape=(2, n.value)).copy() if n.value else np.zeros((2, 0), np.float32)
+            return segs, frames
+        finally:
+            self.lib.fa_vad_free_result(res)
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self.lib.fa_vad_uninit(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class OfflineRecognizer:
@@ -21,14 +84,7 @@ class OfflineRecognizer:
 
     def infer(self, wavs: Sequence[np.ndarray]) -> List[List[int]]:
         """wavs: float32 arrays in [-1, 1] or int16 PCM arrays (all the same dtype), 16 kHz mono, >= 400 samples each."""
-        arrs = [np.ascontiguousarray(w) for w in wavs]
-        kinds = {a.dtype for a in arrs}
-        if kinds == {np.dtype(np.float32)}:
-            fmt = 0
-        elif kinds == {np.dtype(np.int16)}:
-            fmt = 1
-        else:
-            raise _abi.FunasrB200Error("waveforms must all be float32 or all be int16, got %s" % kinds)
+        arrs, fmt = _pcm_batch(wavs)
         n = len(arrs)
         ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
         lens = (C.c_int64 * n)(*[a.shape[0] for a in arrs])
@@ -41,6 +97,40 @@ class OfflineRecognizer:
             for i in range(self.lib.fa_offline_result_count(res)):
                 p = self.lib.fa_offline_result_ids(res, i, C.byref(cnt))
                 out.append([int(p[k]) for k in range(cnt.value)])
+            self.last_audio_seconds = float(self.lib.fa_offline_result_audio_seconds(res))
+            return out
+        finally:
+            self.lib.fa_offline_free_result(res)
+
+    def infer_long(self, wavs: Sequence[np.ndarray], vad: OfflineVad, batch_size_s: int = 300, batch_size_threshold_s: int = 60,
+                   merge_vad: bool = False, merge_length_s: int = 15, hotword_embeddings: Optional[np.ndarray] = None,
+                   **vad_kwargs) -> List[dict]:
+        """Long recordings through fa_offline_infer_vad, each on its own as LongAudioPipeline.generate treats it -> per recording
+        {"token_int": ids in time order, "vad_segments": [[start_ms, end_ms], ...], "n_tokens": tokens per segment}.
+        hotword_embeddings: [n, 512] float32 rows (ContextualParaformer; last row the <s> entry)."""
+        arrs, fmt = _pcm_batch(wavs)
+        n = len(arrs)
+        ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
+        lens = (C.c_int64 * n)(*[a.shape[0] for a in arrs])
+        opts = _abi.FaLongAudioOptions(int(batch_size_s), int(batch_size_threshold_s), 1 if merge_vad else 0, int(merge_length_s),
+                                       _vad_run_options(**vad_kwargs))
+        hw, n_hw = None, 0
+        if hotword_embeddings is not None:
+            hw = np.ascontiguousarray(hotword_embeddings, dtype=np.float32)
+            n_hw = hw.shape[0]
+        res = self.lib.fa_offline_infer_vad(self.handle, vad.handle, ptrs, lens, n, fmt, None if hw is None else hw.ctypes.data, n_hw,
+                                            C.byref(opts))
+        if not res:
+            raise _abi.FunasrB200Error("fa_offline_infer_vad failed: %s" % self.lib.fa_offline_last_error().decode())
+        try:
+            out = []
+            cnt = C.c_int32(0)
+            for i in range(self.lib.fa_offline_result_count(res)):
+                p = self.lib.fa_offline_result_ids(res, i, C.byref(cnt))
+                ids = [int(p[k]) for k in range(cnt.value)]
+                s = self.lib.fa_offline_result_segments(res, i, C.byref(cnt))
+                trip = [[int(s[3 * k]), int(s[3 * k + 1]), int(s[3 * k + 2])] for k in range(cnt.value)]
+                out.append({"token_int": ids, "vad_segments": [t[:2] for t in trip], "n_tokens": [t[2] for t in trip]})
             self.last_audio_seconds = float(self.lib.fa_offline_result_audio_seconds(res))
             return out
         finally:

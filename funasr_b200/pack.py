@@ -9,6 +9,16 @@ model.pt + am.mvn), plus the derived tables the kernels take as inputs:
     encoder.pe_inv_timescales [280]    SinusoidalPositionEncoder timescales (transformer/embedding.py:409-414)
     predictor.cif_conv1d.gemm_weight   Conv1d(512,512,3) weight repacked to a [512, 3*512] GEMM weight
 
+The FSMN-VAD file (csrc/offline.cu: fa_vad_init) uses the same layout: the encoder's weights under the reference's names
+(encoder.in_linear1.linear.weight, encoder.fsmn.{i}.fsmn_block.conv_left.weight, ...), frontend.mel_banks / window / cmvn [2, 400]
+and
+
+    __vad_config__                     [50] the bytes of 25 float64 values: the VADXOptions fields in FaVadOptions order (14 integer
+                                            fields, then speech_2_noise_ratio, snr_thres, decibel_thres, speech_noise_thres,
+                                            fe_prior_thres), lorder, len(sil_pdf_ids), sil_pdf_ids padded to 4
+
+The detector compares posteriors in double precision against speech_noise_thres and fe_prior_thres, so the options travel as float64.
+
 Layout: b"FAB2MDL1", u32 n_tensors, then per tensor: u32 name_len, name (utf-8), u32 ndim, i64 dims[ndim], u64 nbytes,
 zero padding to a 16-byte file offset, little-endian fp32 data.
 """
@@ -44,7 +54,84 @@ def model_tensors(state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: O
 
 
 def write_model_file(path: str, state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: Optional[torch.Tensor] = None) -> int:
-    tensors = model_tensors(state, cfg, cmvn)
+    return _write(path, model_tensors(state, cfg, cmvn))
+
+
+VAD_INT_FIELDS = ("sample_rate", "detect_mode", "max_end_silence_time", "max_start_silence_time", "window_size_ms", "sil_to_speech_time_thres",
+                  "speech_to_sil_time_thres", "do_extend", "lookback_time_start_point", "lookahead_time_end_point", "max_single_segment_time",
+                  "noise_frame_num_used_for_snr", "frame_in_ms", "frame_length_ms")
+VAD_REAL_FIELDS = ("speech_2_noise_ratio", "snr_thres", "decibel_thres", "speech_noise_thres", "fe_prior_thres")
+
+
+def vad_model_tensors(state: Dict[str, torch.Tensor], cmvn: Optional[torch.Tensor], vad_conf: Optional[dict] = None) -> Dict[str, np.ndarray]:
+    """The tensors of a FSMN-VAD model file.  state: FsmnVADStreaming's state_dict (encoder.* names); vad_conf: its model_conf
+    (VADXOptions, `VadOptions.from_conf`), optionally with the "encoder_conf" of the model's config.  Refuses what FSMNB200 / VadEngine
+    refuse."""
+    from .engine import kaldi_mel_banks
+    from .vad import VadOptions
+    conf = dict(vad_conf or {})
+    enc_conf = conf.pop("encoder_conf", None)
+    if enc_conf is not None:
+        from .vad_model import FSMNB200
+        FSMNB200(**enc_conf)                                         # raises for the shapes the kernels are not built for
+    o = VadOptions.from_conf(conf)
+    if any(k.endswith("fsmn_block.conv_right.weight") for k in state):
+        raise ValueError("FSMN-VAD with a right-context memory (rorder > 0) is not supported")
+    n_layers = 0
+    while "encoder.fsmn.%d.linear.linear.weight" % n_layers in state:
+        n_layers += 1
+    if n_layers == 0 or "encoder.in_linear1.linear.weight" not in state:
+        raise ValueError("not an FSMN-VAD state_dict (encoder.in_linear1 / encoder.fsmn.{i} missing)")
+    if tuple(state["encoder.in_linear1.linear.weight"].shape)[1:] != (400,):
+        raise ValueError("the VAD frontend is 80 mel x LFR 5: in_linear1 must take 400 inputs")
+    lorder = 20
+    for i in range(n_layers):
+        cw = state["encoder.fsmn.%d.fsmn_block.conv_left.weight" % i]
+        if tuple(cw.shape) != (128, 1, lorder, 1) or state["encoder.fsmn.%d.linear.linear.weight" % i].shape[0] != 128:
+            raise ValueError("FSMN-VAD layer %d: need proj 128 and lorder 20 (conv_left weight [128, 1, 20, 1])" % i)
+    sil = [int(v) for v in o.sil_pdf_ids]
+    if not 1 <= len(sil) <= 4:
+        raise ValueError("sil_pdf_ids must hold 1 to 4 ids")
+    ints = []
+    for name in VAD_INT_FIELDS:
+        v = getattr(o, name)
+        if float(v) != int(v):
+            raise ValueError("VAD option %s = %r is not a whole number" % (name, v))
+        ints.append(int(v))
+    if o.frame_in_ms <= 0 or o.window_size_ms < o.frame_in_ms:
+        raise ValueError("VAD options need frame_in_ms > 0 and window_size_ms >= frame_in_ms")
+    cfg = np.array(ints + [float(getattr(o, n)) for n in VAD_REAL_FIELDS] + [lorder, len(sil)] + sil + [0] * (4 - len(sil)), dtype="<f8")
+    out: Dict[str, np.ndarray] = {"__vad_config__": cfg.view("<f4")}
+    out["frontend.mel_banks"] = kaldi_mel_banks().numpy()
+    out["frontend.window"] = torch.hamming_window(400, periodic=False, alpha=0.54, beta=0.46, dtype=torch.float32).numpy()
+    if cmvn is not None:
+        c = cmvn.detach().float().cpu().numpy()
+        if c.shape != (2, 400):
+            raise ValueError("the VAD's cmvn must be [2, 400]")
+        out["frontend.cmvn"] = c
+    for k, v in state.items():
+        if k.startswith("encoder.") and torch.is_floating_point(v):
+            out[k] = v.detach().float().cpu().contiguous().numpy()
+    return out
+
+
+def write_vad_model_file(path: str, state: Dict[str, torch.Tensor], cmvn: Optional[torch.Tensor] = None, vad_conf: Optional[dict] = None) -> int:
+    return _write(path, vad_model_tensors(state, cmvn, vad_conf))
+
+
+def read_vad_config(tensors: Dict[str, np.ndarray]) -> dict:
+    """The options of a VAD model file read back (tests): {field: value, ..., "lorder", "sil_pdf_ids"}."""
+    c = np.ascontiguousarray(tensors["__vad_config__"], dtype="<f4").view("<f8")
+    n_int = len(VAD_INT_FIELDS)
+    out = {n: int(c[i]) for i, n in enumerate(VAD_INT_FIELDS)}
+    out.update({n: float(c[n_int + i]) for i, n in enumerate(VAD_REAL_FIELDS)})
+    base = n_int + len(VAD_REAL_FIELDS)
+    out["lorder"] = int(c[base])
+    out["sil_pdf_ids"] = [int(v) for v in c[base + 2: base + 2 + int(c[base + 1])]]
+    return out
+
+
+def _write(path: str, tensors: Dict[str, np.ndarray]) -> int:
     with open(path, "wb") as f:
         f.write(MAGIC)
         f.write(struct.pack("<I", len(tensors)))

@@ -571,6 +571,68 @@ void fa_offline_free_result(void* result);
 void fa_offline_uninit(void* handle);
 const char* fa_offline_last_error(void);
 
+/* ---------------------------------------------------------------------------------------------
+ * Handle-style FSMN-VAD and long-audio recognition (no Python, no torch) — FunASR's `vad_model` path: FsmnVADStreaming.inference
+ * (fsmn_vad_streaming/model.py) and AutoModel.inference_with_vad (auto/auto_model.py:852-1035), one recording at a time.
+ * ------------------------------------------------------------------------------------------- */
+/* Run options of the VAD: what FsmnVADStreaming.inference accepts.  dynamic_silence != 0: the per-chunk dynamic end-silence schedule
+ * (the default when no max_end_silence_time is given, model.py:1003-1067); 0: a fixed end silence of max_end_silence_time ms, or of
+ * the model file's value when max_end_silence_time <= 0 (the C++ runtime's fixed threshold).  speech_noise_thres: NaN = the model's. */
+typedef struct {
+  int32_t dynamic_silence;
+  int32_t max_end_silence_time;
+  double speech_noise_thres;
+} FaVadRunOptions;
+/* fa_vad_init: model file written by funasr_b200/pack.py:write_vad_model_file (FSMN weights under the reference's state_dict names,
+ * the frontend tables, CMVN [2, 400] and the VADXOptions; input dimensions are zero-padded to a multiple of 16 here).
+ * fa_vad_infer: ONE host recording (pcm_format 0 = float32 in [-1, 1], 1 = s16le; 16 kHz) -> segments [start_ms, end_ms].  On the
+ * device: Fbank + LFR 5/1 + CMVN, the FSMN and the frame energies; then one copy of two floats per frame to the host and the end-point
+ * walk of fa_vad_detect_segments.  opts NULL = dynamic schedule, the model's threshold.  A recording shorter than one 25 ms frame gives
+ * no segment.  NULL on error (fa_offline_last_error()). */
+void* fa_vad_init(const char* model_file, int32_t device);
+void fa_vad_uninit(void* vad);
+void* fa_vad_infer(void* vad, const void* buf, int64_t n_samples, int32_t pcm_format, const FaVadRunOptions* opts);
+/* n_segments {start_ms, end_ms} pairs, owned by the result. */
+const int32_t* fa_vad_result_segments(const void* result, int64_t* n_segments);
+/* The per-frame values the walk read: [2][frames] (silence posterior, then frame energy in dB), owned by the result. */
+const float* fa_vad_result_frames(const void* result, int64_t* frames);
+float fa_vad_result_audio_seconds(const void* result);
+void fa_vad_free_result(void* result);
+
+/* Long-audio options: auto_model.py's batch_size_s / batch_size_threshold_s (seconds) and merge_vad / merge_length_s
+ * (utils/vad_utils.py:57-91), plus the VAD run options.  NULL = 300, 60, no merge, 15, dynamic schedule. */
+typedef struct {
+  int32_t batch_size_s;
+  int32_t batch_size_threshold_s;
+  int32_t merge_vad;
+  int32_t merge_length_s;
+  FaVadRunOptions vad;
+} FaLongAudioOptions;
+/* Every recording on its own, as inference_with_vad treats it: VAD, optional merge, segments sorted by duration and packed
+ * (fa_pack_segments), each pack gathered from the device-resident recording into one zero-padded batch (fa_gather_segments) and
+ * decoded like fa_offline_infer_hw (the same hotword memory for every segment), results restored to time order.  Result entry i
+ * holds recording i: fa_offline_result_ids = the ids of its segments concatenated in time order, fa_offline_result_segments = its
+ * segments.  A pack whose segments all yield no token empties the recording's ids (auto_model.py:990-999; its segments are kept with
+ * 0 tokens); a recording without speech has no segment.  A segment shorter than 400 samples fails the call with a message naming it.
+ * asr and vad must live on the same device.  NULL on error (fa_offline_last_error()). */
+void* fa_offline_infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
+                           const float* hw_embed, int32_t n_hotwords, const FaLongAudioOptions* opts);
+/* n_segments {start_ms, end_ms, n_tokens} triples of recording `index` (time order); NULL with 0 for results of fa_offline_infer. */
+const int32_t* fa_offline_result_segments(const void* result, int32_t index, int32_t* n_segments);
+/* out [rows, stride] = rec[starts[r] .. starts[r] + lens[r]) then zeros (rec [n_rec] fp32; starts int64 / lens int32 [rows] device;
+ * stride % 4 == 0, 16-byte aligned out; 0 <= lens[r] <= stride; samples at or beyond n_rec read as zero): the batch of VAD segments
+ * that slice_padding_audio_samples (utils/vad_utils.py:28-54) + pad_sequence form. */
+int fa_gather_segments(const float* rec, int64_t n_rec, const int64_t* starts, const int32_t* lens, int32_t rows, int64_t stride,
+                       float* out, fa_stream_t stream);
+/* Host only: the packing of auto_model.py:916-989 (funasr_b200/long_audio.py:pack_segments).  segments [n][2] ms -> order [n]
+ * (indices sorted by duration, ties in time order) and packs [n][2] ([begin, end) ranges into order).  Returns the pack count, or
+ * FA_ERR_ARG. */
+int64_t fa_pack_segments(const int32_t* segments, int64_t n, int32_t batch_size_s, int32_t batch_size_threshold_s, int32_t* order,
+                         int32_t* packs);
+/* Host only: merge_vad (utils/vad_utils.py:57-91, funasr_b200/vad.py:merge_vad).  segments [n][2] -> out [<= 2n][2]; returns the
+ * count, or FA_ERR_ARG. */
+int64_t fa_merge_vad(const int32_t* segments, int64_t n, int32_t max_length_ms, int32_t min_length_ms, int32_t* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,6 +7,13 @@
  *   optional keys "gemm-mode" (fp32 | fp16 | fp16x3 | fp16x6, default fp16x3) and "gpu-id" (default 0);
  *   there is no CPU path (use_gpu is ignored); audio must be 16 kHz; the WFST / LM decoder entry points are accepted and ignored
  *   (greedy decoding, like the reference without --lm-dir).
+ *   model_path["vad-dir"] (optional) names a directory holding `vad.fab2` (funasr_b200/pack.py: write_vad_model_file, from the FSMN-VAD
+ *   model.pt + am.mvn + the model_conf of its config.yaml).  With it FunOfflineInfer / FunOfflineInferBuffer segment the audio first
+ *   (fa_offline_infer_vad) with the runtime's semantics: a FIXED end silence (the file's max_end_silence_time, fsmn-vad.cpp), segment
+ *   texts concatenated in time order (funasrruntime.cpp:287-296); optional key "batch-size-s" sets the segment packing (default 300).
+ *   Without it a buffer is decoded as one utterance, as before.
+ *   FsmnVadInit: model_path["model-dir"] holds `vad.fab2` ("gpu-id" as above); FsmnVadInferBuffer is offline only (input_finished
+ *   must be true) and takes "pcm" (s16le) or "wav" (PCM16 / float32); FsmnVadOnlineInit is not provided.
  */
 #pragma once
 #include <stdint.h>
@@ -51,6 +58,16 @@ _FUNASRAPI const char* FunASRGetStampSents(FUNASR_RESULT result);
 _FUNASRAPI const int FunASRGetRetNumber(FUNASR_RESULT result);
 _FUNASRAPI void FunASRFreeResult(FUNASR_RESULT result);
 _FUNASRAPI const float FunASRGetRetSnippetTime(FUNASR_RESULT result);
+
+// VAD (funasrruntime.h:81-91, without FsmnVadOnlineInit)
+_FUNASRAPI FUNASR_HANDLE FsmnVadInit(std::map<std::string, std::string>& model_path, int thread_num);
+_FUNASRAPI FUNASR_RESULT FsmnVadInferBuffer(FUNASR_HANDLE handle, const char* sz_buf, int n_len, QM_CALLBACK fn_callback, bool input_finished = true,
+                                            int sampling_rate = 16000, std::string wav_format = "pcm");
+_FUNASRAPI FUNASR_RESULT FsmnVadInfer(FUNASR_HANDLE handle, const char* sz_filename, QM_CALLBACK fn_callback, int sampling_rate = 16000);
+_FUNASRAPI std::vector<std::vector<int>>* FsmnVadGetResult(FUNASR_RESULT result, int n_index);
+_FUNASRAPI void FsmnVadFreeResult(FUNASR_RESULT result);
+_FUNASRAPI void FsmnVadUninit(FUNASR_HANDLE handle);
+_FUNASRAPI const float FsmnVadGetRetSnippetTime(FUNASR_RESULT result);
 
 // WFST decoder (funasrruntime.h:134-138): accepted, no effect (greedy decoding)
 _FUNASRAPI FUNASR_DEC_HANDLE FunASRWfstDecoderInit(FUNASR_HANDLE handle, int asr_type, float glob_beam, float lat_beam, float am_scale);
