@@ -283,12 +283,13 @@ stats_pool_kernel(const float* __restrict__ x, int T, int C, const float* __rest
 }
 
 // CMN of the CAM++ frontend (campplus/utils.py extract_feature): feats[b, t, :] -= mean over the utterance's own frames; padded rows
-// stay zero.  One thread per (utterance, mel bin), sequential time-order sum (deterministic).
+// stay zero.  One thread per (utterance, mel bin), sequential time-order sum (deterministic).  An utterance longer than t_max has only
+// t_max rows in feats: the mean is over those, and no row of the next utterance (or past the buffer) is touched.
 __global__ void cmn_kernel(float* __restrict__ feats, const int32_t* __restrict__ lens, int t_max, int batch) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= batch * 80) return;
   const int b = i / 80, c = i % 80;
-  const int n = lens[b];
+  const int n = min(lens[b], t_max);
   float* f = feats + (int64_t)b * t_max * 80 + c;
   float s = 0.f;
   for (int t = 0; t < n; ++t) s += f[(int64_t)t * 80];

@@ -158,7 +158,8 @@ const char* fa_status_string(int status);
  * writing utterance b at feats + b * feats_batch_stride_rows * 80 * lfr_m (t_max rows each): a stride above t_max leaves room
  * for prepended frames, e.g. SenseVoiceSmall's 4 query frames (funasr/models/sense_voice/model.py:971-995).  lfr_m / lfr_n select
  * the low-frame-rate stacking: 7 / 6 (Paraformer, SenseVoice: feats [B, t_max, 560]) or 5 / 1 (the FSMN-VAD frontend,
- * fsmn_vad_streaming/template.yaml:54-62: feats [B, t_max, 400], one row per 10 ms frame). */
+ * fsmn_vad_streaming/template.yaml:54-62: feats [B, t_max, 400], one row per 10 ms frame).  An utterance with more than t_max rows
+ * keeps its first t_max (the values an untruncated call gives them) and feat_lens[b] still reports its full row count. */
 size_t fa_fbank_tables_bytes(void);
 int fa_fbank_make_tables(const float* mel_banks, const float* window, float* tables, fa_stream_t stream);
 int fa_fbank_lfr_cmvn_tables(const float* wav, const int32_t* wav_lens, int32_t batch, int64_t wav_stride, const float* cmvn,
@@ -517,7 +518,9 @@ typedef struct {
 } FaCampplus;
 /* Features (campplus/utils.py extract_feature): torchaudio kaldi.fbank(wav, num_mel_bins=80) with its defaults (no x32768 scaling,
  * window from `tables`: fa_fbank_make_tables with the povey window), then each utterance's mean over its own frames is subtracted.
- * wav [B, wav_stride] (lens >= 400 samples) -> feats [B, t_max, 80] (rows >= feat_lens[b] zero, pad_list(..., 0)), feat_lens [B]. */
+ * wav [B, wav_stride] (lens >= 400 samples) -> feats [B, t_max, 80] (rows >= feat_lens[b] zero, pad_list(..., 0)), feat_lens [B].
+ * feat_lens[b] is the utterance's full frame count even when it exceeds t_max; such an utterance keeps its first t_max frames, and
+ * the mean subtracted from them is the mean over those t_max frames.  Nothing outside feats [B, t_max, 80] is written. */
 int fa_campplus_features(const float* wav, const int32_t* wav_lens, int32_t batch, int64_t wav_stride, const float* tables,
                          float* feats, int32_t* feat_lens, int32_t t_max, fa_stream_t stream);
 /* CAMPPlus.forward: feats [B, t, 80] (every frame used, no mask) -> emb [B, 192].  Stream-ordered, no host synchronisation. */
