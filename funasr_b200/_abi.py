@@ -157,6 +157,7 @@ SIGNATURES = {
     "fa_fsmn_vad_forward": (C.c_int, [C.POINTER(FaVadEncoder), _vp, _i64, _i32, _vp, _vp, _vp, _sz, _vp]),
     "fa_frame_decibels": (C.c_int, [_vp, _i64, _i32, _vp, _vp]),
     "fa_cif_wo_hidden_host": (C.c_int, [_vp, _i64, C.c_float, _vp]),
+    "fa_ts_stamps_host": (_i64, [_vp, _vp, _i64, _i64, _i32, C.c_double, _vp, _i64]),
     "fa_vad_detect_segments": (_i64, [_vp, _vp, _i64, _i64, C.POINTER(FaVadOptions), _i32, _i32, _vp, _i32, C.c_double, _vp, _i64]),
     "fa_greedy_filter": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "fa_split_planes": (C.c_int, [_vp, _i64, _i64, _i32, _i32, _vp, _vp]),
@@ -175,10 +176,12 @@ SIGNATURES = {
     "fa_offline_infer": (_vp, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32]),
     "fa_offline_infer_hw": (_vp, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp, _i32]),
     "fa_offline_is_contextual": (_i32, [_vp]),
+    "fa_offline_has_timestamps": (_i32, [_vp]),
     "fa_offline_host_tensor": (_vp, [_vp, C.c_char_p, C.POINTER(_i64)]),
     "fa_offline_result_count": (_i32, [_vp]),
     "fa_offline_result_ids": (C.POINTER(_i32), [_vp, _i32, C.POINTER(_i32)]),
     "fa_offline_result_audio_seconds": (C.c_float, [_vp]),
+    "fa_offline_result_stamps": (C.POINTER(_i32), [_vp, _i32, C.POINTER(_i32)]),
     "fa_offline_free_result": (None, [_vp]),
     "fa_offline_uninit": (None, [_vp]),
     "fa_offline_last_error": (C.c_char_p, []),

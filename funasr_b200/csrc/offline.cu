@@ -7,6 +7,7 @@
 //   fa_offline_init         model file -> handle (weights to HBM, fp16 planes for the tensor-core GEMMs)
 //   fa_offline_infer        batch of host PCM buffers (f32 in [-1,1] or s16le) -> result (greedy token ids per utterance)
 //   fa_offline_result_*     accessors;  fa_offline_free_result / fa_offline_uninit
+//                           a BiCifParaformer file (its upsampled CIF timestamp head) adds per-token [start_ms, end_ms] stamps
 //   fa_vad_init / fa_vad_infer       FSMN-VAD model file -> handle; one recording -> [start_ms, end_ms] segments
 //   fa_offline_infer_vad    long recordings: VAD -> segments packed by duration -> each pack gathered on the device and decoded
 // The tokenizer (ids -> text) stays with the caller, like every other entry point of this ABI.
@@ -28,6 +29,7 @@ void set_err(const std::string& s) { g_err = s; }
 struct Tensor {
   float* dev = nullptr;
   std::vector<int64_t> shape;
+  std::vector<float> host;           // load_file(..., to_device = false): the payload of the "__" configuration tensors
   int64_t numel() const { int64_t n = 1; for (auto d : shape) n *= d; return n; }
 };
 
@@ -63,6 +65,12 @@ struct Model {
   DevBuf wav, pcm16, lens, feats, flens, encb, acoustic, tok, alphas, peaks, ws, ids, best, fids, flens_out, hw, hw_lens;
   DevBuf rec, gmeta;                                 // fa_offline_infer_vad: the device-resident recording, per-pack gather offsets
   bool contextual = false;                           // ContextualParaformer: decoder with a hotword bias branch
+  // BiCifParaformer: CifPredictorV3's upsampled timestamp head (bicif_paraformer/cif_predictor.py:300-352)
+  bool ts = false;
+  float smooth2 = 0.f, noise2 = 0.f;                 // __ts_config__
+  FaLinear up_lin{}, ih_lin{};                       // upsample_cnn as a [3*512, 512] GEMM; both BLSTM input projections [8*512, 512]
+  const float *hh_f = nullptr, *hh_b = nullptr, *out2_w = nullptr, *out2_b = nullptr;
+  DevBuf up, xproj, feat, us_alphas, us_peaks, lens_up, lstm_scratch;
   std::map<std::string, std::vector<float>> host_cache;   // fa_offline_host_tensor
   ~Model() {
     for (auto& kv : t) if (kv.second.dev) cudaFree(kv.second.dev);
@@ -75,6 +83,8 @@ struct Result {
   std::vector<std::vector<int32_t>> ids;
   std::vector<int32_t> token_num;
   std::vector<std::vector<int32_t>> segs;            // fa_offline_infer_vad: {start_ms, end_ms, n_tokens} per segment, per recording
+  bool ts = false;                                   // the model has the timestamp head: stamps[i] = {start_ms, end_ms} pairs
+  std::vector<std::vector<int32_t>> stamps;
   float audio_seconds = 0.f;
 };
 
@@ -83,11 +93,18 @@ __global__ void pcm16_to_f32_kernel(const int16_t* __restrict__ src, float* __re
   if (i < n) dst[i] = (float)src[i] * (1.0f / 32768.0f);     // exact; the frontend multiplies by 32768 again (wav_frontend.py:169)
 }
 
+__global__ void scale_lens_kernel(const int32_t* __restrict__ lens, int32_t k, int32_t n, int32_t* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = lens[i] * k;
+}
+
 bool read_exact(FILE* f, void* dst, size_t n) { return fread(dst, 1, n, f) == n; }
 
 // File layout (funasr_b200/pack.py): "FAB2MDL1", u32 n_tensors, then per tensor:
 //   u32 name_len, name, u32 ndim, i64 dims[ndim], u64 nbytes, zero padding to a 16-byte file offset, fp32 data
-bool load_file(std::map<std::string, Tensor>& tensors, const char* path) {
+// to_device = false reads the index only (names, shapes, and the payload of the "__" configuration tensors into Tensor::host):
+// what can be checked before any device is touched.
+bool load_file(std::map<std::string, Tensor>& tensors, const char* path, bool to_device = true) {
   FILE* f = fopen(path, "rb");
   if (!f) { set_err(std::string("cannot open ") + path); return false; }
   char magic[8];
@@ -112,6 +129,17 @@ bool load_file(std::map<std::string, Tensor>& tensors, const char* path) {
     ok = fseek(f, pad, SEEK_CUR) == 0 && nbytes == (uint64_t)tt.numel() * 4 &&
          pos + pad <= fsize && nbytes <= (uint64_t)(fsize - (pos + pad));   // the payload lies inside the file: a corrupt size cannot drive an allocation
     if (!ok) break;
+    if (!to_device) {
+      if (name.compare(0, 2, "__") == 0) {
+        tt.host.resize(nbytes / 4);
+        ok = read_exact(f, tt.host.data(), nbytes);
+      } else {
+        ok = fseek(f, (long)nbytes, SEEK_CUR) == 0;
+      }
+      if (!ok) break;
+      tensors[name] = tt;
+      continue;
+    }
     host.resize(nbytes / 4);
     ok = read_exact(f, host.data(), nbytes);
     if (!ok) break;
@@ -139,12 +167,12 @@ struct Builder {
     nm.g = w ? w->dev : nullptr; nm.b = ptr(p + ".bias"); nm.n = w ? (int32_t)w->numel() : 0; nm.eps = m.ln_eps;
     return nm;
   }
-  FaLinear lin(const std::string& p, bool bias = true, const char* weight_key = nullptr) {
+  FaLinear lin(const std::string& p, bool bias = true, const char* weight_key = nullptr, const char* bias_key = nullptr) {
     FaLinear L{};
     const Tensor* w = get(weight_key ? std::string(weight_key) : p + ".weight");
     // [out, in] or a k = 1 Conv1d weight [out, in, 1] (bias_output, contextual_paraformer/decoder.py:287)
     if (!w || !(w->shape.size() == 2 || (w->shape.size() == 3 && w->shape[2] == 1))) { if (ok) set_err("bad weight " + p); ok = false; return L; }
-    L.w = w->dev; L.b = bias ? ptr(p + ".bias") : nullptr;
+    L.w = w->dev; L.b = bias ? ptr(bias_key ? std::string(bias_key) : p + ".bias") : nullptr;
     L.out_f = (int32_t)w->shape[0]; L.in_f = (int32_t)w->shape[1]; L.in_pad = (L.in_f + 63) / 64 * 64;
     if (m.mode != FA_GEMM_F32_SIMT) {
       void* planes = nullptr;
@@ -156,6 +184,42 @@ struct Builder {
     return L;
   }
 };
+
+// BiCifParaformer's timestamp head, recognised by predictor.upsample_cnn.weight, on the file's index (no device needed): every
+// tensor the launches read, in the shapes pack.py:timestamp_head_tensors writes, and __ts_config__.  A file without the head passes.
+struct TsHeadConfig {
+  bool present = false;
+  float smooth2 = 0.f, noise2 = 0.f;
+};
+
+bool check_ts_head(const std::map<std::string, Tensor>& t, TsHeadConfig& out) {
+  out = TsHeadConfig();
+  if (!t.count("predictor.upsample_cnn.weight")) return true;
+  auto cfg = t.find("__ts_config__");
+  if (cfg == t.end() || cfg->second.host.size() < 3) {
+    set_err("BiCif timestamp head without __ts_config__ (a file packed before the handle read the head): re-pack it with "
+            "funasr_b200.pack.write_model_file");
+    return false;
+  }
+  const float* c = cfg->second.host.data();
+  if (c[0] != 3.f) { set_err("BiCif timestamp head: upsample_times " + std::to_string(c[0]) + " in __ts_config__, only 3 is supported"); return false; }
+  const struct { const char* name; int64_t d0, d1; } need[] = {
+      {"predictor.upsample_cnn.gemm_weight", 3 * 512, 512}, {"predictor.upsample_cnn.gemm_bias", 3 * 512, -1},
+      {"predictor.blstm.ih_gemm_weight", 8 * 512, 512},     {"predictor.blstm.ih_gemm_bias", 8 * 512, -1},
+      {"predictor.blstm.weight_hh_l0", 4 * 512, 512},       {"predictor.blstm.weight_hh_l0_reverse", 4 * 512, 512},
+      {"predictor.cif_output2.weight", 2 * 512, 0},         {"predictor.cif_output2.bias", 1, 0}};
+  for (const auto& n : need) {
+    auto it = t.find(n.name);
+    if (it == t.end()) { set_err(std::string("BiCif timestamp head: missing tensor ") + n.name); return false; }
+    const std::vector<int64_t>& sh = it->second.shape;
+    // d1 > 0: exactly [d0, d1]; d1 < 0: exactly [d0]; d1 == 0: d0 elements in any shape
+    const bool ok = n.d1 > 0 ? (sh.size() == 2 && sh[0] == n.d0 && sh[1] == n.d1) : n.d1 < 0 ? (sh.size() == 1 && sh[0] == n.d0)
+                                                                                          : it->second.numel() == n.d0;
+    if (!ok) { set_err(std::string("BiCif timestamp head: bad shape of ") + n.name); return false; }
+  }
+  out.present = true; out.smooth2 = c[1]; out.noise2 = c[2];
+  return true;
+}
 
 bool build(Model& m) {
   Builder b{m};
@@ -197,6 +261,13 @@ bool build(Model& m) {
   m.pred.conv = b.lin("predictor.cif_conv1d", true, "predictor.cif_conv1d.gemm_weight");
   m.pred.out_w = b.ptr("predictor.cif_output.weight"); m.pred.out_b = b.ptr("predictor.cif_output.bias");
   m.pred.threshold = m.cif_threshold; m.pred.tail_threshold = m.tail_threshold; m.pred.smooth_factor = 1.f; m.pred.noise_threshold = 0.f;
+  if (m.ts) {                   // BiCifParaformer: CifPredictorV3's sequential fp32 `cif` (bicif_paraformer/cif_predictor.py:37-84) + its head
+    m.pred.cif_variant = 1;
+    m.up_lin = b.lin("predictor.upsample_cnn", true, "predictor.upsample_cnn.gemm_weight", "predictor.upsample_cnn.gemm_bias");
+    m.ih_lin = b.lin("predictor.blstm.ih", true, "predictor.blstm.ih_gemm_weight", "predictor.blstm.ih_gemm_bias");
+    m.hh_f = b.ptr("predictor.blstm.weight_hh_l0"); m.hh_b = b.ptr("predictor.blstm.weight_hh_l0_reverse");
+    m.out2_w = b.ptr("predictor.cif_output2.weight"); m.out2_b = b.ptr("predictor.cif_output2.bias");
+  }
   // decoder (ParaformerSANMDecoder decoder.py:234-449)
   auto dec_layer = [&](FaDecLayer& L, const std::string& p, bool full) {
     L.norm1 = b.norm(p + ".norm1");
@@ -273,6 +344,8 @@ Result* decode_batch(Model& m, const float* wav, int64_t stride, const std::vect
   Result* r = new Result();
   r->audio_seconds = (float)seconds;
   r->token_num.resize(B);
+  r->ts = m.ts;
+  if (m.ts) r->stamps.resize(B);
   cudaMemcpyAsync(r->token_num.data(), m.tok.p, (size_t)B * 4, cudaMemcpyDeviceToHost, m.st);
   if (cudaStreamSynchronize(m.st) != cudaSuccess) { set_err(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError())); delete r; return nullptr; }
   int n_max = 0;                                             // the path's one host sync (cif_predictor.py:311)
@@ -283,6 +356,16 @@ Result* decode_batch(Model& m, const float* wav, int64_t stride, const std::vect
   if (!(m.ids.reserve((size_t)B * n_max * 4) && m.best.reserve((size_t)B * n_max * 4) && m.fids.reserve((size_t)B * n_max * 4) &&
         m.flens_out.reserve((size_t)B * 4) && m.ws.reserve(fa_paraformer_decoder_workspace_bytes_hw(B, T, n_max, m.vocab, m.mode, nh)))) {
     set_err("device allocation failed (decoder)"); delete r; return nullptr;
+  }
+  // the timestamp head over the [B, 3T] upsampled frames; its two GEMMs share the workspace, the larger carve is the B*3T-row one
+  const int U = 3, TU = T * U;
+  const int64_t rows_up = (int64_t)B * TU;
+  const int lstm_rows = B < 256 ? B : 256;                   // fa_blstm_forward_tc holds at most 256 sequences per launch
+  if (m.ts && !(m.up.reserve((size_t)rows_up * D * 4) && m.xproj.reserve((size_t)rows_up * 8 * D * 4) &&
+                m.feat.reserve((size_t)rows_up * 2 * D * 4) && m.us_alphas.reserve((size_t)rows_up * 4) && m.us_peaks.reserve((size_t)rows_up * 4) &&
+                m.lens_up.reserve((size_t)B * 4) && m.lstm_scratch.reserve(fa_blstm_tc_scratch_bytes(lstm_rows)) &&
+                m.ws.reserve(fa_linear_workspace_bytes(rows_up, D, m.mode)))) {
+    set_err("device allocation failed (timestamp head)"); delete r; return nullptr;
   }
   if (m.contextual) {                                        // hotword memory [n_hw, 512] (contextual_paraformer/model.py:350-372) + per-utterance counts
     if (!(m.hw.reserve((size_t)nh * D * 4) && m.hw_lens.reserve((size_t)B * 4))) { set_err("device allocation failed (hotwords)"); delete r; return nullptr; }
@@ -300,11 +383,47 @@ Result* decode_batch(Model& m, const float* wav, int64_t stride, const std::vect
     rc = fa_greedy_filter(static_cast<int32_t*>(m.ids.p), static_cast<int32_t*>(m.tok.p), B, n_max, 1, 2, 0, static_cast<int32_t*>(m.fids.p),
                           static_cast<int32_t*>(m.flens_out.p), m.st);
   if (rc != FA_OK) { set_err(std::string("decoder: ") + fa_status_string(rc)); delete r; return nullptr; }
-  std::vector<int32_t> fids((size_t)B * n_max), fl(B);
+  if (m.ts) {                   // CifPredictorV3.get_upsample_timestamp (bicif_paraformer/cif_predictor.py:300-352), engine.upsample_timestamp
+    float* up = static_cast<float*>(m.up.p);
+    float* xproj = static_cast<float*>(m.xproj.p);
+    float* feat = static_cast<float*>(m.feat.p);
+    rc = fa_linear(static_cast<float*>(m.encb.p), D, (int64_t)B * T, &m.up_lin, 0, nullptr, 0, nullptr, 0, up, (int64_t)U * D, m.mode, m.ws.p,
+                   m.ws.cap, m.st);
+    if (rc == FA_OK)
+      rc = fa_linear(up, D, rows_up, &m.ih_lin, 0, nullptr, 0, nullptr, 0, xproj, (int64_t)8 * D, m.mode, m.ws.p, m.ws.cap, m.st);
+    for (int b0 = 0; b0 < B && rc == FA_OK; b0 += 256) {     // sequences are independent: larger batches run as consecutive launches
+      const int bn = B - b0 < 256 ? B - b0 : 256;
+      rc = fa_blstm_forward_tc(xproj + (int64_t)b0 * TU * 8 * D, m.hh_f, m.hh_b, bn, TU, D, feat + (int64_t)b0 * TU * 2 * D, m.lstm_scratch.p,
+                               m.lstm_scratch.cap, m.st);
+    }
+    if (rc == FA_OK) {
+      scale_lens_kernel<<<(B + 255) / 256, 256, 0, m.st>>>(static_cast<const int32_t*>(m.flens.p), U, B, static_cast<int32_t*>(m.lens_up.p));
+      rc = fa_cif_upsample_alphas(feat, 2 * D, m.out2_w, m.out2_b, static_cast<const int32_t*>(m.lens_up.p), static_cast<const int32_t*>(m.tok.p), B, TU,
+                                  m.smooth2, m.noise2, m.cif_threshold, static_cast<float*>(m.us_alphas.p), static_cast<float*>(m.us_peaks.p), m.st);
+    }
+    if (rc != FA_OK) { set_err(std::string("timestamp head: ") + fa_status_string(rc)); delete r; return nullptr; }
+  }
+  std::vector<int32_t> fids((size_t)B * n_max), fl(B), enc_lens(m.ts ? B : 0);
+  std::vector<float> us_alphas(m.ts ? rows_up : 0), us_peaks(m.ts ? rows_up : 0);
   cudaMemcpyAsync(fids.data(), m.fids.p, fids.size() * 4, cudaMemcpyDeviceToHost, m.st);
   cudaMemcpyAsync(fl.data(), m.flens_out.p, (size_t)B * 4, cudaMemcpyDeviceToHost, m.st);
+  if (m.ts) {                                                // on the same synchronisation as the ids
+    cudaMemcpyAsync(enc_lens.data(), m.flens.p, (size_t)B * 4, cudaMemcpyDeviceToHost, m.st);
+    cudaMemcpyAsync(us_alphas.data(), m.us_alphas.p, (size_t)rows_up * 4, cudaMemcpyDeviceToHost, m.st);
+    cudaMemcpyAsync(us_peaks.data(), m.us_peaks.p, (size_t)rows_up * 4, cudaMemcpyDeviceToHost, m.st);
+  }
   if (cudaStreamSynchronize(m.st) != cudaSuccess) { set_err(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError())); delete r; return nullptr; }
   for (int i = 0; i < B; ++i) r->ids[i].assign(fids.begin() + (size_t)i * n_max, fids.begin() + (size_t)i * n_max + fl[i]);
+  if (m.ts) {                                                // bicif_paraformer/model.py:402-407: each utterance's first 3 * enc_len frames
+    for (int i = 0; i < B; ++i) {
+      const int64_t n = (int64_t)U * enc_lens[i];
+      std::vector<int32_t>& st = r->stamps[i];
+      st.resize((size_t)(2 * (n > 0 ? n : 1)));              // at most n - 1 spans
+      const int64_t k = fa_ts_stamps_host(us_alphas.data() + (size_t)i * TU, us_peaks.data() + (size_t)i * TU, n, (int64_t)r->ids[i].size(), U, 0.0,
+                                          st.data(), n);
+      st.resize(k > 0 ? (size_t)(2 * k) : 0);
+    }
+  }
 #undef FA_OFF
   return r;
 }
@@ -321,9 +440,17 @@ extern "C" void* fa_offline_init(const char* model_file, int32_t device, int32_t
   if (gemm_mode != FA_GEMM_F32_SIMT && gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) {
     set_err("bad gemm_mode"); return nullptr;
   }
+  TsHeadConfig head;
+  try {                                   // what the file's index alone decides (the timestamp head) is refused before any device work
+    std::map<std::string, Tensor> index;
+    if (!load_file(index, model_file, false) || !check_ts_head(index, head)) return nullptr;
+  } catch (const std::exception& e) {
+    set_err(std::string("model file rejected: ") + e.what()); return nullptr;
+  }
   if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); set_err("no such CUDA device (this library has no CPU path)"); return nullptr; }
   Model* m = new Model();
   m->device = device; m->mode = gemm_mode;
+  m->ts = head.present; m->smooth2 = head.smooth2; m->noise2 = head.noise2;
   if (cudaStreamCreateWithFlags(&m->st, cudaStreamNonBlocking) != cudaSuccess) { set_err("cudaStreamCreate failed"); delete m; return nullptr; }
   bool ok = false;
   try {                                   // a malformed file can ask for an absurd allocation: no C++ exception may cross the C ABI
@@ -338,6 +465,8 @@ extern "C" void* fa_offline_init(const char* model_file, int32_t device, int32_t
 extern "C" void fa_offline_uninit(void* handle) { delete static_cast<Model*>(handle); }
 
 extern "C" int32_t fa_offline_is_contextual(const void* handle) { return handle && static_cast<const Model*>(handle)->contextual ? 1 : 0; }
+
+extern "C" int32_t fa_offline_has_timestamps(const void* handle) { return handle && static_cast<const Model*>(handle)->ts ? 1 : 0; }
 
 extern "C" const float* fa_offline_host_tensor(void* handle, const char* name, int64_t* numel) {
   Model* m = static_cast<Model*>(handle);
@@ -400,6 +529,13 @@ extern "C" const int32_t* fa_offline_result_ids(const void* result, int32_t inde
 }
 
 extern "C" float fa_offline_result_audio_seconds(const void* result) { return result ? static_cast<const Result*>(result)->audio_seconds : 0.f; }
+
+extern "C" const int32_t* fa_offline_result_stamps(const void* result, int32_t index, int32_t* n_stamps) {
+  const Result* r = static_cast<const Result*>(result);
+  if (!r || !r->ts || index < 0 || index >= (int32_t)r->stamps.size() || r->stamps[index].empty()) { if (n_stamps) *n_stamps = 0; return nullptr; }
+  if (n_stamps) *n_stamps = (int32_t)(r->stamps[index].size() / 2);
+  return r->stamps[index].data();
+}
 
 extern "C" void fa_offline_free_result(void* result) { delete static_cast<Result*>(result); }
 
@@ -668,7 +804,7 @@ namespace {
 
 // one recording of fa_offline_infer_vad: inference_with_vad (auto_model.py:852-1035, funasr_b200/long_audio.py:LongAudioPipeline.generate)
 bool long_audio_one(Model& m, Vad& v, int rec_index, const void* buf, int64_t n, int32_t pcm_format, const float* hw_embed, int32_t n_hotwords,
-                    const FaLongAudioOptions& o, std::vector<int32_t>& ids, std::vector<int32_t>& segs_out) {
+                    const FaLongAudioOptions& o, std::vector<int32_t>& ids, std::vector<int32_t>& segs_out, std::vector<int32_t>& stamps) {
   if (!upload(buf, n, pcm_format, m.rec, m.pcm16, m.st)) return false;
   const float* rec = static_cast<const float*>(m.rec.p);
   VadResult vr;
@@ -685,7 +821,7 @@ bool long_audio_one(Model& m, Vad& v, int rec_index, const void* buf, int64_t n,
   std::vector<int32_t> order((size_t)ns), packs((size_t)(2 * ns));
   const int64_t np = fa_pack_segments(segs.data(), ns, o.batch_size_s, o.batch_size_threshold_s, order.data(), packs.data());
   if (np < 0) { set_err("fa_pack_segments failed"); return false; }
-  std::vector<std::vector<int32_t>> seg_ids((size_t)ns);
+  std::vector<std::vector<int32_t>> seg_ids((size_t)ns), seg_stamps((size_t)ns);
   bool emptied = false;
   for (int64_t p = 0; p < np && !emptied; ++p) {
     const int beg = packs[2 * p], end = packs[2 * p + 1], B = end - beg;
@@ -717,13 +853,19 @@ bool long_audio_one(Model& m, Vad& v, int rec_index, const void* buf, int64_t n,
     int tmax = 0;
     for (int32_t t : pr->token_num) tmax = t > tmax ? t : tmax;
     if (tmax < 1) emptied = true;                            // no token in the whole pack: the recording's result is empty (:990-999)
-    else for (int j = 0; j < B; ++j) seg_ids[order[beg + j]].swap(pr->ids[j]);
+    else
+      for (int j = 0; j < B; ++j) {
+        seg_ids[order[beg + j]].swap(pr->ids[j]);
+        if (pr->ts) seg_stamps[order[beg + j]].swap(pr->stamps[j]);
+      }
     delete pr;
   }
   for (int64_t s = 0; s < ns; ++s) {
     const int32_t k = emptied ? 0 : (int32_t)seg_ids[s].size();
     segs_out.insert(segs_out.end(), {segs[2 * s], segs[2 * s + 1], k});
-    if (!emptied) ids.insert(ids.end(), seg_ids[s].begin(), seg_ids[s].end());
+    if (emptied) continue;
+    ids.insert(ids.end(), seg_ids[s].begin(), seg_ids[s].end());
+    for (int32_t t : seg_stamps[s]) stamps.push_back(t + segs[2 * s]);       // absolute ms (auto_model.py:1008-1022)
   }
   return true;
 }
@@ -748,11 +890,15 @@ extern "C" void* fa_offline_infer_vad(void* asr, void* vad, const void* const* b
   r->ids.resize(batch);
   r->segs.resize(batch);
   r->token_num.assign(batch, 0);
+  r->ts = mp->ts;
+  r->stamps.resize(batch);
   double seconds = 0.0;
   try {
     for (int i = 0; i < batch; ++i) {
       seconds += (double)n_samples[i] / 16000.0;
-      if (!long_audio_one(*mp, *vp, i, bufs[i], n_samples[i], pcm_format, hw_embed, n_hotwords, o, r->ids[i], r->segs[i])) { delete r; return nullptr; }
+      if (!long_audio_one(*mp, *vp, i, bufs[i], n_samples[i], pcm_format, hw_embed, n_hotwords, o, r->ids[i], r->segs[i], r->stamps[i])) {
+        delete r; return nullptr;
+      }
       r->token_num[i] = (int32_t)r->ids[i].size();
     }
   } catch (const std::exception& e) {

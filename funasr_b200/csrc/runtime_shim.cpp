@@ -4,6 +4,13 @@
 // the reference runs it on the CPU too — model_eb.onnx, runtime/onnxruntime/src/paraformer.cpp CompileHotwordEmbedding) and the
 // ids -> text join.  Everything per audio frame runs in fa_offline_infer_hw on the GPU — or, with a VAD model ("vad-dir"), in
 // fa_offline_infer_vad.  FsmnVad* are the runtime's VAD entry points over fa_vad_infer.
+//
+// Timestamps: with a BiCifParaformer model file FunASRGetStamp returns the runtime's "[[b,e],[b,e],...]" (integer ms, absolute with
+// "vad-dir"; funasrruntime.cpp:297-310), one pair per stamp of fa_offline_result_stamps.  The values are the library's one timestamp
+// definition, the one the reference's Python BiCifParaformer produces (timestamp_tools.py:ts_prediction_lfr6_standard): the shim does
+// not restate the runtime's own TimestampOnnx (util.cpp:838-965), which cuts tokens at 30 frames instead of 12, re-integrates in fp32
+// with a tail fix-up and re-parses seconds strings to ms.  FunASRGetStampSents stays empty: it pairs text characters with stamps
+// through Vector2StringV2 / TimestampSentence, which the token join below does not restate either.
 #include "../../include/funasrruntime_b200.h"
 #include "../../include/funasr_b200.h"
 
@@ -52,6 +59,15 @@ struct ShimResult {
   std::string stamp, stamp_sents;
   float snippet_time = 0.f;
 };
+
+// "[[b,e],[b,e],...]" of entry `index` of a handle result; "" without stamps, as the runtime leaves it
+std::string render_stamps(const void* r, int32_t index) {
+  int32_t n = 0;
+  const int32_t* p = fa_offline_result_stamps(r, index, &n);
+  std::string s;
+  for (int32_t i = 0; i < n; ++i) s += (i ? ",[" : "[[") + std::to_string(p[2 * i]) + "," + std::to_string(p[2 * i + 1]) + "]";
+  return n ? s + "]" : s;
+}
 
 bool is_ascii_word(const std::string& s) {
   if (s.empty()) return false;
@@ -155,6 +171,7 @@ FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, int 
     }
     ShimResult* out = new ShimResult();
     out->msgs.push_back(text);
+    out->stamp = render_stamps(r, 0);
     out->snippet_time = fa_offline_result_audio_seconds(r);
     fa_offline_free_result(r);
     return out;
@@ -167,6 +184,7 @@ FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, int 
     int32_t k = 0;
     const int32_t* ids = fa_offline_result_ids(r, i, &k);
     out->msgs.push_back(join_tokens(*s, ids, k));
+    if (i == 0) out->stamp = render_stamps(r, 0);
   }
   out->snippet_time = fa_offline_result_audio_seconds(r);
   fa_offline_free_result(r);

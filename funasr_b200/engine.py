@@ -190,21 +190,15 @@ class _EngineBase:
     def _init_timestamp_head(self, prefix_pred, smooth_factor2, noise_threshold2, threshold):
         """CifPredictorV3 timestamp head (bicif_paraformer/cif_predictor.py:121-352, upsample_type "cnn_blstm", use_cif1_cnn False),
         shared by BiCifParaformer / SeacoParaformer and the MonotonicAligner."""
-        state, g, lin = self._state, self._g, self._lin
-        uw = state[prefix_pred + "upsample_cnn.weight"]                      # ConvTranspose1d weight [in, out, k], stride == k == 3
-        self.up_times = int(uw.shape[2])
-        # out[b, 3t+k, o] = sum_c x[b,t,c] w[c,o,k] + bias[o]  ==  one GEMM with W[(k,o), c], rows viewed as [B, 3T, D]
-        self.up_lin = lin(prefix_pred + "upsample_cnn", weight=self._dev(uw.permute(2, 1, 0).reshape(-1, uw.shape[0])),
-                          bias_tensor=self._dev(state[prefix_pred + "upsample_cnn.bias"].repeat(self.up_times)))
-        # the BLSTM: input projections of both directions as ONE GEMM ([W_ih_fwd; W_ih_bwd], b_ih + b_hh), then the
-        # persistent weight-stationary recurrence fa_blstm_forward_tc
-        bp = prefix_pred + "blstm."
-        w_ih = torch.cat([state[bp + "weight_ih_l0"], state[bp + "weight_ih_l0_reverse"]], 0)
-        b_all = torch.cat([state[bp + "bias_ih_l0"] + state[bp + "bias_hh_l0"],
-                           state[bp + "bias_ih_l0_reverse"] + state[bp + "bias_hh_l0_reverse"]], 0)
-        self.lstm_ih = lin(bp + "ih", weight=self._dev(w_ih), bias_tensor=self._dev(b_all))
-        self.lstm_hh_f, self.lstm_hh_b = g(bp + "weight_hh_l0"), g(bp + "weight_hh_l0_reverse")
-        self.out2_w, self.out2_b = g(prefix_pred + "cif_output2.weight"), g(prefix_pred + "cif_output2.bias")
+        from .pack import timestamp_head_tensors
+        head = {k[len(prefix_pred):]: self._dev(v) for k, v in timestamp_head_tensors(self._state, prefix_pred).items()}
+        self.up_times = int(self._state[prefix_pred + "upsample_cnn.weight"].shape[2])   # ConvTranspose1d weight [in, out, k], stride == k
+        # the upsampling as one GEMM over rows viewed as [B, 3T, D]; the BLSTM: input projections of both directions as ONE GEMM
+        # ([W_ih_fwd; W_ih_bwd], b_ih + b_hh), then the persistent weight-stationary recurrence fa_blstm_forward_tc
+        self.up_lin = self._lin("upsample_cnn", weight=head["upsample_cnn.gemm_weight"], bias_tensor=head["upsample_cnn.gemm_bias"])
+        self.lstm_ih = self._lin("blstm.ih", weight=head["blstm.ih_gemm_weight"], bias_tensor=head["blstm.ih_gemm_bias"])
+        self.lstm_hh_f, self.lstm_hh_b = head["blstm.weight_hh_l0"], head["blstm.weight_hh_l0_reverse"]
+        self.out2_w, self.out2_b = head["cif_output2.weight"], head["cif_output2.bias"]
         self.smooth2, self.noise2, self.ts_threshold = float(smooth_factor2), float(noise_threshold2), float(threshold)
 
     def upsample_timestamp(self, enc: torch.Tensor, lens: torch.Tensor, token_num: torch.Tensor):

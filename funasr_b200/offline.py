@@ -2,7 +2,8 @@
 FunOfflineInit / FunOfflineInferBuffer / FunASRGetResult (runtime/onnxruntime/include/funasrruntime.h:100-116).
 Nothing here touches torch on the data path: host PCM buffers in, token ids out.  `OfflineVad` binds the FSMN-VAD handle
 (fa_vad_*) and `OfflineRecognizer.infer_long` the long-audio entry (fa_offline_infer_vad): VAD segments packed by duration and decoded
-batch by batch, the same results as LongAudioPipeline.generate."""
+batch by batch, the same results as LongAudioPipeline.generate.  A BiCifParaformer model file adds per-token [start_ms, end_ms] stamps
+(`infer_stamped`, and "timestamp" in `infer_long`'s results)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -82,8 +83,17 @@ class OfflineRecognizer:
         if not self.handle:
             raise _abi.FunasrB200Error("fa_offline_init failed: %s" % self.lib.fa_offline_last_error().decode())
 
-    def infer(self, wavs: Sequence[np.ndarray]) -> List[List[int]]:
-        """wavs: float32 arrays in [-1, 1] or int16 PCM arrays (all the same dtype), 16 kHz mono, >= 400 samples each."""
+    @property
+    def has_timestamps(self) -> bool:
+        """True for a BiCifParaformer model file: results carry per-token stamps from its upsampled CIF head."""
+        return bool(self.lib.fa_offline_has_timestamps(self.handle))
+
+    def _stamps(self, res, i) -> List[List[int]]:
+        cnt = C.c_int32(0)
+        p = self.lib.fa_offline_result_stamps(res, i, C.byref(cnt))
+        return [[int(p[2 * k]), int(p[2 * k + 1])] for k in range(cnt.value)]
+
+    def _infer(self, wavs, stamped: bool):
         arrs, fmt = _pcm_batch(wavs)
         n = len(arrs)
         ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
@@ -96,17 +106,28 @@ class OfflineRecognizer:
             cnt = C.c_int32(0)
             for i in range(self.lib.fa_offline_result_count(res)):
                 p = self.lib.fa_offline_result_ids(res, i, C.byref(cnt))
-                out.append([int(p[k]) for k in range(cnt.value)])
+                ids = [int(p[k]) for k in range(cnt.value)]
+                out.append({"token_int": ids, "timestamp": self._stamps(res, i)} if stamped else ids)
             self.last_audio_seconds = float(self.lib.fa_offline_result_audio_seconds(res))
             return out
         finally:
             self.lib.fa_offline_free_result(res)
 
+    def infer(self, wavs: Sequence[np.ndarray]) -> List[List[int]]:
+        """wavs: float32 arrays in [-1, 1] or int16 PCM arrays (all the same dtype), 16 kHz mono, >= 400 samples each."""
+        return self._infer(wavs, False)
+
+    def infer_stamped(self, wavs: Sequence[np.ndarray]) -> List[dict]:
+        """Like `infer`, per utterance {"token_int": ids, "timestamp": [[start_ms, end_ms], ...]} (BiCifParaformer.inference's result;
+        no stamps for a model without the timestamp head)."""
+        return self._infer(wavs, True)
+
     def infer_long(self, wavs: Sequence[np.ndarray], vad: OfflineVad, batch_size_s: int = 300, batch_size_threshold_s: int = 60,
                    merge_vad: bool = False, merge_length_s: int = 15, hotword_embeddings: Optional[np.ndarray] = None,
                    **vad_kwargs) -> List[dict]:
         """Long recordings through fa_offline_infer_vad, each on its own as LongAudioPipeline.generate treats it -> per recording
-        {"token_int": ids in time order, "vad_segments": [[start_ms, end_ms], ...], "n_tokens": tokens per segment}.
+        {"token_int": ids in time order, "vad_segments": [[start_ms, end_ms], ...], "n_tokens": tokens per segment}, plus
+        "timestamp": [[start_ms, end_ms], ...] in absolute ms when the model has the timestamp head (`has_timestamps`).
         hotword_embeddings: [n, 512] float32 rows (ContextualParaformer; last row the <s> entry)."""
         arrs, fmt = _pcm_batch(wavs)
         n = len(arrs)
@@ -125,12 +146,15 @@ class OfflineRecognizer:
         try:
             out = []
             cnt = C.c_int32(0)
+            stamped = self.has_timestamps
             for i in range(self.lib.fa_offline_result_count(res)):
                 p = self.lib.fa_offline_result_ids(res, i, C.byref(cnt))
                 ids = [int(p[k]) for k in range(cnt.value)]
                 s = self.lib.fa_offline_result_segments(res, i, C.byref(cnt))
                 trip = [[int(s[3 * k]), int(s[3 * k + 1]), int(s[3 * k + 2])] for k in range(cnt.value)]
                 out.append({"token_int": ids, "vad_segments": [t[:2] for t in trip], "n_tokens": [t[2] for t in trip]})
+                if stamped:
+                    out[-1]["timestamp"] = self._stamps(res, i)
             self.last_audio_seconds = float(self.lib.fa_offline_result_audio_seconds(res))
             return out
         finally:

@@ -9,6 +9,17 @@ model.pt + am.mvn), plus the derived tables the kernels take as inputs:
     encoder.pe_inv_timescales [280]    SinusoidalPositionEncoder timescales (transformer/embedding.py:409-414)
     predictor.cif_conv1d.gemm_weight   Conv1d(512,512,3) weight repacked to a [512, 3*512] GEMM weight
 
+A BiCifParaformer (CifPredictorV3 with the upsampled timestamp head, recognised by predictor.upsample_cnn.weight) also carries
+the head in the form the library's launches take it (`timestamp_head_tensors`, the one owner of this repack):
+
+    predictor.upsample_cnn.gemm_weight [3*512, 512] ConvTranspose1d(512,512,3,stride 3) weight as a GEMM weight, W[k*512+o, c] = w[c,o,k]
+    predictor.upsample_cnn.gemm_bias   [3*512]      its bias repeated 3x
+    predictor.blstm.ih_gemm_weight     [8*512, 512] [weight_ih_l0; weight_ih_l0_reverse]: both input projections as one GEMM
+    predictor.blstm.ih_gemm_bias       [8*512]      [bias_ih_l0 + bias_hh_l0; bias_ih_l0_reverse + bias_hh_l0_reverse]
+    predictor.blstm.weight_hh_l0 / weight_hh_l0_reverse [4*512, 512], predictor.cif_output2.weight [1, 1024] / .bias [1]
+                                                    (the reference's names, copied like every predictor.* tensor)
+    __ts_config__                      [3] upsample_times, smooth_factor2, noise_threshold2
+
 The FSMN-VAD file (csrc/offline.cu: fa_vad_init) uses the same layout: the encoder's weights under the reference's names
 (encoder.in_linear1.linear.weight, encoder.fsmn.{i}.fsmn_block.conv_left.weight, ...), frontend.mel_banks / window / cmvn [2, 400]
 and
@@ -35,7 +46,8 @@ from .synth import ParaformerConfig, sinusoid_inv_timescales
 MAGIC = b"FAB2MDL1"
 
 
-def model_tensors(state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: Optional[torch.Tensor]) -> Dict[str, np.ndarray]:
+def model_tensors(state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: Optional[torch.Tensor], smooth_factor2: float = 0.25,
+                  noise_threshold2: float = 0.01) -> Dict[str, np.ndarray]:
     from .engine import kaldi_mel_banks
     out: Dict[str, np.ndarray] = {}
     out["__config__"] = np.array([cfg.enc_layers, cfg.dec_layers, cfg.d_model, cfg.heads, cfg.kernel, cfg.vocab, cfg.feat_dim,
@@ -50,11 +62,44 @@ def model_tensors(state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: O
             out[k] = v.detach().float().cpu().contiguous().numpy()
     cw = state["predictor.cif_conv1d.weight"].detach().float().cpu()
     out["predictor.cif_conv1d.gemm_weight"] = cw.permute(0, 2, 1).reshape(cw.shape[0], -1).contiguous().numpy()
+    if "predictor." + TS_HEAD_KEY in state:
+        for k, v in timestamp_head_tensors(state).items():
+            out[k] = v.cpu().numpy()
+        up_times = int(state["predictor." + TS_HEAD_KEY].shape[2])
+        out["__ts_config__"] = np.array([up_times, smooth_factor2, noise_threshold2], dtype=np.float32)
     return out
 
 
-def write_model_file(path: str, state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: Optional[torch.Tensor] = None) -> int:
-    return _write(path, model_tensors(state, cfg, cmvn))
+def write_model_file(path: str, state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: Optional[torch.Tensor] = None,
+                     smooth_factor2: float = 0.25, noise_threshold2: float = 0.01) -> int:
+    """smooth_factor2 / noise_threshold2: CifPredictorV3's predictor_conf values (paraformer-large-vad-punc's by default); used only
+    when the state dict has the BiCif timestamp head."""
+    return _write(path, model_tensors(state, cfg, cmvn, smooth_factor2, noise_threshold2))
+
+
+TS_HEAD_KEY = "upsample_cnn.weight"
+
+
+def timestamp_head_tensors(state: Dict[str, torch.Tensor], prefix: str = "predictor.") -> Dict[str, torch.Tensor]:
+    """CifPredictorV3's timestamp head (bicif_paraformer/cif_predictor.py:121-352, upsample_type "cnn_blstm") repacked for this
+    library's launches, on the device the state lives on: {name: fp32 tensor} under the names of the module docstring.  Both the
+    engine (engine.py:_init_timestamp_head) and the model file take the head from here."""
+    uw = state[prefix + TS_HEAD_KEY].detach().float()                     # ConvTranspose1d weight [in, out, k], stride == k
+    up_times = int(uw.shape[2])
+    bp = prefix + "blstm."
+    f = lambda k: state[k].detach().float()                               # noqa: E731
+    return {
+        # out[b, 3t+k, o] = sum_c x[b,t,c] w[c,o,k] + bias[o]  ==  one GEMM with W[(k,o), c], rows viewed as [B, 3T, D]
+        prefix + "upsample_cnn.gemm_weight": uw.permute(2, 1, 0).reshape(-1, uw.shape[0]).contiguous(),
+        prefix + "upsample_cnn.gemm_bias": f(prefix + "upsample_cnn.bias").repeat(up_times).contiguous(),
+        bp + "ih_gemm_weight": torch.cat([f(bp + "weight_ih_l0"), f(bp + "weight_ih_l0_reverse")], 0).contiguous(),
+        bp + "ih_gemm_bias": torch.cat([f(bp + "bias_ih_l0") + f(bp + "bias_hh_l0"),
+                                        f(bp + "bias_ih_l0_reverse") + f(bp + "bias_hh_l0_reverse")], 0).contiguous(),
+        bp + "weight_hh_l0": f(bp + "weight_hh_l0").contiguous(),
+        bp + "weight_hh_l0_reverse": f(bp + "weight_hh_l0_reverse").contiguous(),
+        prefix + "cif_output2.weight": f(prefix + "cif_output2.weight").contiguous(),
+        prefix + "cif_output2.bias": f(prefix + "cif_output2.bias").contiguous(),
+    }
 
 
 VAD_INT_FIELDS = ("sample_rate", "detect_mode", "max_end_silence_time", "max_start_silence_time", "window_size_ms", "sil_to_speech_time_thres",

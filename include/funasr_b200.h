@@ -438,6 +438,16 @@ int64_t fa_vad_detect_segments(const double* sil_prob, const double* decibel, in
  * sum, reduced by `threshold` after every frame that reaches it; trace[t] = the value before the reduction) — the re-integration step of
  * ts_prediction_lfr6_standard (:67-72). */
 int fa_cif_wo_hidden_host(const float* alphas, int64_t n, float threshold, float* trace);
+/* Host only: the [start_ms, end_ms] stamps of one utterance from its upsampled CIF weights / fires (us_alphas, us_peaks [n_frames]) and
+ * its token count, as funasr/utils/timestamp_tools.py:37-123 (ts_prediction_lfr6_standard, force_time_shift -1.5) computes the stamps
+ * (funasr_b200/timestamps.py:_stamps_only is the specification): the weights are rescaled and re-integrated (fa_cif_wo_hidden_host) when
+ * the fire count is not n_tokens + 1; one stamp per span between consecutive fires, so the count is not always n_tokens (spans past the
+ * token list are stamps too); every value in double arithmetic, + vad_offset_ms, truncated to integer ms.  upsample_rate: 3 for the
+ * BiCif head, 1 for plain CIF fires.  The <sil> / </s> rules of the Python routine read token strings: the caller passes n_tokens
+ * without a trailing </s>, and no token is spelled <sil>.  out receives the first max_out {start_ms, end_ms} pairs; returns the stamp
+ * count (0 when nothing fires or n_tokens == 0), or FA_ERR_ARG. */
+int64_t fa_ts_stamps_host(const float* us_alphas, const float* us_peaks, int64_t n_frames, int64_t n_tokens, int32_t upsample_rate,
+                          double vad_offset_ms, int32_t* out, int64_t max_out);
 /* decibel[f] = 10 log10(sum_{j<400} wav[160 f + j]^2 + 1e-6), f < frames (ComputeDecibel, model.py:516-525). */
 int fa_frame_decibels(const float* wav, int64_t n_samples, int32_t frames, float* decibel, fa_stream_t stream);
 
@@ -554,7 +564,9 @@ int fa_split_planes(const float* src, int64_t ld_src, int64_t rows, int32_t cols
  * model_file: flat tensor file written by funasr_b200/pack.py from a FunASR state_dict (same tensor names as model.pt) plus
  * am.mvn and the kaldi mel/window tables.  pcm_format: 0 = float32 in [-1,1], 1 = int16 little endian (converted on the
  * device, halves the H2D bytes).  bufs are HOST pointers, n_samples[i] >= 400.  Returns NULL on error
- * (fa_offline_last_error() says why); there is no CPU fallback.
+ * (fa_offline_last_error() says why); there is no CPU fallback.  fa_offline_init refuses a BiCif timestamp head (recognised by
+ * predictor.upsample_cnn.weight) without __ts_config__, with a missing or misshapen tensor or with upsample_times != 3 before it
+ * touches a device, naming the piece.
  * ------------------------------------------------------------------------------------------- */
 void* fa_offline_init(const char* model_file, int32_t device, int32_t gemm_mode);
 void* fa_offline_infer(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format);
@@ -564,12 +576,24 @@ void* fa_offline_infer(void* handle, const void* const* bufs, const int64_t* n_s
 void* fa_offline_infer_hw(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
                           const float* hw_embed, int32_t n_hotwords);
 int32_t fa_offline_is_contextual(const void* handle);
+/* 1 when the model file carries BiCifParaformer's upsampled CIF timestamp head (predictor.upsample_cnn.*, predictor.blstm.*,
+ * predictor.cif_output2.* and __ts_config__, written by funasr_b200/pack.py): its token branch then runs CifPredictorV3's sequential
+ * fp32 `cif`, and every result carries per-token stamps (fa_offline_result_stamps).  0 otherwise, or for NULL. */
+int32_t fa_offline_has_timestamps(const void* handle);
 /* Host copy of a tensor of the model file by its FunASR state_dict name (e.g. "bias_embed.weight" for the hotword encoder that
  * runs on the host); owned by the handle.  NULL if absent. */
 const float* fa_offline_host_tensor(void* handle, const char* name, int64_t* numel);
 int32_t fa_offline_result_count(const void* result);
 const int32_t* fa_offline_result_ids(const void* result, int32_t index, int32_t* n_ids);
 float fa_offline_result_audio_seconds(const void* result);
+/* n_stamps {start_ms, end_ms} pairs of entry `index` (owned by the result): the stamps the reference's BiCifParaformer.inference
+ * gives (bicif_paraformer/model.py:402-407), computed by fa_ts_stamps_host from the head's upsampled weights.  One stamp per span
+ * between fires, which is one per token id in the usual case; the count is returned on its own.  Stamps are per token id: the
+ * <sil>-entry and </s> rules of the Python routine read token strings, which the handle does not have; ids 0 / 1 / 2 (blank, <s>,
+ * </s>) are already removed by the greedy filter.  For fa_offline_infer_vad results the stamps are absolute: each segment's are
+ * shifted by its start ms and concatenated in time order (auto_model.py:1008-1022).  NULL with 0 for a model without the head, for
+ * an entry without stamps and for NULL / out-of-range arguments. */
+const int32_t* fa_offline_result_stamps(const void* result, int32_t index, int32_t* n_stamps);
 void fa_offline_free_result(void* result);
 void fa_offline_uninit(void* handle);
 const char* fa_offline_last_error(void);
@@ -615,7 +639,8 @@ typedef struct {
  * (fa_pack_segments), each pack gathered from the device-resident recording into one zero-padded batch (fa_gather_segments) and
  * decoded like fa_offline_infer_hw (the same hotword memory for every segment), results restored to time order.  Result entry i
  * holds recording i: fa_offline_result_ids = the ids of its segments concatenated in time order, fa_offline_result_segments = its
- * segments.  A pack whose segments all yield no token empties the recording's ids (auto_model.py:990-999; its segments are kept with
+ * segments, fa_offline_result_stamps = its absolute stamps (BiCif).  A pack whose segments all yield no token empties the recording's
+ * ids and stamps (auto_model.py:990-999; its segments are kept with
  * 0 tokens); a recording without speech has no segment.  A segment shorter than 400 samples fails the call with a message naming it.
  * asr and vad must live on the same device.  NULL on error (fa_offline_last_error()). */
 void* fa_offline_infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
