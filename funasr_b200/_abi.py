@@ -59,6 +59,11 @@ class FaDecoder(C.Structure):
                 ("_pad2", C.c_int32)]
 
 
+class FaTimestampHead(C.Structure):
+    _fields_ = [("upsample", FaLinear), ("blstm_ih", FaLinear), ("w_hh_fwd", C.c_void_p), ("w_hh_bwd", C.c_void_p), ("out2_w", C.c_void_p),
+                ("out2_b", C.c_void_p), ("up_times", C.c_int32), ("smooth2", C.c_float), ("noise2", C.c_float), ("threshold", C.c_float)]
+
+
 class FaVadLayer(C.Structure):
     _fields_ = [("lin", FaLinear), ("conv_w", C.c_void_p), ("affine", FaLinear)]
 
@@ -153,6 +158,8 @@ SIGNATURES = {
     "fa_cif_upsample_alphas": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _f, _f, _f, _vp, _vp, _vp]),
     "fa_blstm_tc_scratch_bytes": (_sz, [_i32]),
     "fa_blstm_forward_tc": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _sz, _vp]),
+    "fa_timestamp_head_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32]),
+    "fa_timestamp_head_forward": (C.c_int, [C.POINTER(FaTimestampHead), _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _vp, _sz, _vp]),
     "fa_fsmn_vad_workspace_bytes": (_sz, [C.POINTER(FaVadEncoder), _i32]),
     "fa_fsmn_vad_forward": (C.c_int, [C.POINTER(FaVadEncoder), _vp, _i64, _i32, _vp, _vp, _vp, _sz, _vp]),
     "fa_frame_decibels": (C.c_int, [_vp, _i64, _i32, _vp, _vp]),

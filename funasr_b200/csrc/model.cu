@@ -235,6 +235,65 @@ extern "C" int fa_cif_upsample_alphas(const float* feat, int32_t dz, const float
   return cif_upsample_scan_launch(us_alphas, token_num, batch, t_up, (float)((double)threshold - 1e-4), us_peaks, st);
 }
 
+// The timestamp head over B * U * t_max upsampled rows: the upsampled rows, both directions' input projections, the BLSTM output,
+// the recurrence's scratch for one launch, the GEMM scratch for the larger (upsampled) GEMM — both have K = D — and lens x U
+// (last: the other takes are whole multiples of 256 bytes, so the carve adds no padding)
+static const int kBlstmMaxBatch = 256;          // fa_blstm_forward_tc holds at most 256 sequences per launch
+struct TsHeadBufs { float *up, *xproj, *feat; void* lstm; size_t lstm_bytes; Arena gemm{nullptr, 0}; int32_t* lens_up; };
+static TsHeadBufs ts_head_carve(Arena& a, int batch, int t_max, int d, int up_times, int mode) {
+  const int64_t rows = (int64_t)batch * t_max * up_times;
+  TsHeadBufs b;
+  b.up = a.take<float>((size_t)rows * d);
+  b.xproj = a.take<float>((size_t)rows * 8 * d);
+  b.feat = a.take<float>((size_t)rows * 2 * d);
+  b.lstm_bytes = fa_blstm_tc_scratch_bytes(batch < kBlstmMaxBatch ? batch : kBlstmMaxBatch);
+  b.lstm = a.take<char>(b.lstm_bytes);
+  if (mode != FA_GEMM_F32_SIMT) b.gemm = a.sub(gemm_tc_scratch_bytes(rows, d, mode));
+  b.lens_up = a.take<int32_t>(batch);
+  return b;
+}
+
+__global__ void scale_lens_kernel(const int32_t* __restrict__ lens, int32_t k, int32_t n, int32_t* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = lens[i] * k;
+}
+
+extern "C" size_t fa_timestamp_head_workspace_bytes(int32_t batch, int32_t t_max, int32_t d_model, int32_t up_times, int32_t gemm_mode) {
+  if (batch <= 0 || t_max <= 0 || d_model <= 0 || up_times <= 0) return 0;
+  Arena m = Arena::measuring();
+  ts_head_carve(m, batch, t_max, d_model, up_times, gemm_mode);
+  return m.bytes();
+}
+
+extern "C" int fa_timestamp_head_forward(const FaTimestampHead* head, const float* enc, const int32_t* lens, const int32_t* token_num,
+                                         int32_t batch, int32_t t_max, float* us_alphas, float* us_peaks, int32_t gemm_mode, void* workspace,
+                                         size_t ws_bytes, fa_stream_t stream) {
+  if (!head || !enc || !lens || !token_num || !us_alphas || !us_peaks || batch <= 0 || t_max <= 0 || head->up_times <= 0) return FA_ERR_ARG;
+  if (!head->w_hh_fwd || !head->w_hh_bwd || !head->out2_w || !head->out2_b) return FA_ERR_ARG;
+  if (gemm_mode != FA_GEMM_F32_SIMT && gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) return FA_ERR_ARG;
+  const FaLinear &up_lin = head->upsample, &ih_lin = head->blstm_ih;
+  const int D = up_lin.in_f, U = head->up_times;
+  if (D != 512 && D != 320) return FA_ERR_UNSUPPORTED;        // the shapes the recurrence is built for
+  if (up_lin.out_f != U * D || ih_lin.out_f != 8 * D || ih_lin.in_f != D) return FA_ERR_ARG;
+  if (gemm_mode != FA_GEMM_F32_SIMT && (!up_lin.w_planes || !ih_lin.w_planes)) return FA_ERR_ARG;
+  Arena a(workspace, ws_bytes);
+  TsHeadBufs b = ts_head_carve(a, batch, t_max, D, U, gemm_mode);
+  if (!a.ok()) return FA_ERR_WORKSPACE;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int TU = t_max * U;
+  FA_RETURN_IF_ERR(gemm_rows(enc, D, (int64_t)batch * t_max, up_lin, GemmEpi().to(b.up, (int64_t)U * D), gemm_mode, &b.gemm, st));
+  FA_RETURN_IF_ERR(gemm_rows(b.up, D, (int64_t)batch * TU, ih_lin, GemmEpi().to(b.xproj, 8 * D), gemm_mode, &b.gemm, st));
+  for (int b0 = 0; b0 < batch; b0 += kBlstmMaxBatch) {       // sequences are independent: larger batches run as consecutive launches
+    const int bn = batch - b0 < kBlstmMaxBatch ? batch - b0 : kBlstmMaxBatch;
+    FA_RETURN_IF_ERR(fa_blstm_forward_tc(b.xproj + (int64_t)b0 * TU * 8 * D, head->w_hh_fwd, head->w_hh_bwd, bn, TU, D,
+                                         b.feat + (int64_t)b0 * TU * 2 * D, b.lstm, b.lstm_bytes, stream));
+  }
+  scale_lens_kernel<<<(batch + 255) / 256, 256, 0, st>>>(lens, U, batch, b.lens_up);
+  FA_CHECK_LAUNCH();
+  return fa_cif_upsample_alphas(b.feat, 2 * D, head->out2_w, head->out2_b, b.lens_up, token_num, batch, TU, head->smooth2, head->noise2,
+                                head->threshold, us_alphas, us_peaks, stream);
+}
+
 // ------------------------------------------------------------------------------------------------ decoder
 // Workspace of every decoder-stack entry point (d_model 512, 4 heads of 128, FFN <= 2048).  The memory has Mk = batch * t_max rows
 // (an upper bound when it is shared).  contextual: the bias decoder over n_hotwords rows of hotword memory.  probs: the stack's ASF

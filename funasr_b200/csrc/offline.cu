@@ -18,6 +18,7 @@
 #include <algorithm>
 #include <exception>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -25,11 +26,24 @@ namespace {
 
 thread_local std::string g_err;
 void set_err(const std::string& s) { g_err = s; }
+std::nullptr_t fail(const std::string& s) { set_err(s); return nullptr; }
+
+// f() with every C++ exception turned into an error message: none may cross the C ABI (a malformed file can ask for an absurd
+// allocation)
+template <typename F>
+bool no_throw(const char* what, F f) {
+  try {
+    return f();
+  } catch (const std::exception& e) {
+    set_err(std::string(what) + e.what());
+    return false;
+  }
+}
 
 struct Tensor {
-  float* dev = nullptr;
+  float* dev = nullptr;              // weights
+  std::vector<float> host;           // the payload of the "__" configuration tensors, which stay on the host
   std::vector<int64_t> shape;
-  std::vector<float> host;           // load_file(..., to_device = false): the payload of the "__" configuration tensors
   int64_t numel() const { int64_t n = 1; for (auto d : shape) n *= d; return n; }
 };
 
@@ -48,62 +62,12 @@ struct DevBuf {                      // grow-only device allocation
   ~DevBuf() { if (p) cudaFree(p); }
 };
 
-struct Model {
-  int device = 0, mode = 3;
-  int enc_layers = 0, dec_layers = 0, d_model = 512, heads = 4, kernel = 11, vocab = 0, feat_dim = 560;
-  float ln_eps = 1e-12f, cif_threshold = 1.f, tail_threshold = 0.45f;
-  std::map<std::string, Tensor> t;
-  std::vector<void*> owned;                    // weight planes etc.
-  std::vector<FaEncLayer> enc_l;
-  std::vector<FaDecLayer> dec_l;
-  FaEncoder enc{};
-  FaPredictor pred{};
-  FaDecoder dec{};
-  const float *mel = nullptr, *window = nullptr, *cmvn = nullptr;
-  float* fbank_tables = nullptr;                     // fa_fbank_make_tables output (owned)
-  cudaStream_t st = nullptr;
-  DevBuf wav, pcm16, lens, feats, flens, encb, acoustic, tok, alphas, peaks, ws, ids, best, fids, flens_out, hw, hw_lens;
-  DevBuf rec, gmeta;                                 // fa_offline_infer_vad: the device-resident recording, per-pack gather offsets
-  bool contextual = false;                           // ContextualParaformer: decoder with a hotword bias branch
-  // BiCifParaformer: CifPredictorV3's upsampled timestamp head (bicif_paraformer/cif_predictor.py:300-352)
-  bool ts = false;
-  float smooth2 = 0.f, noise2 = 0.f;                 // __ts_config__
-  FaLinear up_lin{}, ih_lin{};                       // upsample_cnn as a [3*512, 512] GEMM; both BLSTM input projections [8*512, 512]
-  const float *hh_f = nullptr, *hh_b = nullptr, *out2_w = nullptr, *out2_b = nullptr;
-  DevBuf up, xproj, feat, us_alphas, us_peaks, lens_up, lstm_scratch;
-  std::map<std::string, std::vector<float>> host_cache;   // fa_offline_host_tensor
-  ~Model() {
-    for (auto& kv : t) if (kv.second.dev) cudaFree(kv.second.dev);
-    for (void* p : owned) cudaFree(p);
-    if (st) cudaStreamDestroy(st);
-  }
-};
-
-struct Result {
-  std::vector<std::vector<int32_t>> ids;
-  std::vector<int32_t> token_num;
-  std::vector<std::vector<int32_t>> segs;            // fa_offline_infer_vad: {start_ms, end_ms, n_tokens} per segment, per recording
-  bool ts = false;                                   // the model has the timestamp head: stamps[i] = {start_ms, end_ms} pairs
-  std::vector<std::vector<int32_t>> stamps;
-  float audio_seconds = 0.f;
-};
-
-__global__ void pcm16_to_f32_kernel(const int16_t* __restrict__ src, float* __restrict__ dst, int64_t n) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) dst[i] = (float)src[i] * (1.0f / 32768.0f);     // exact; the frontend multiplies by 32768 again (wav_frontend.py:169)
-}
-
-__global__ void scale_lens_kernel(const int32_t* __restrict__ lens, int32_t k, int32_t n, int32_t* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = lens[i] * k;
-}
-
 bool read_exact(FILE* f, void* dst, size_t n) { return fread(dst, 1, n, f) == n; }
 
 // File layout (funasr_b200/pack.py): "FAB2MDL1", u32 n_tensors, then per tensor:
 //   u32 name_len, name, u32 ndim, i64 dims[ndim], u64 nbytes, zero padding to a 16-byte file offset, fp32 data
-// to_device = false reads the index only (names, shapes, and the payload of the "__" configuration tensors into Tensor::host):
-// what can be checked before any device is touched.
+// The payload of a "__" configuration tensor is read into Tensor::host.  to_device = false skips the weights (names and shapes
+// only): what can be checked before any device is touched.
 bool load_file(std::map<std::string, Tensor>& tensors, const char* path, bool to_device = true) {
   FILE* f = fopen(path, "rb");
   if (!f) { set_err(std::string("cannot open ") + path); return false; }
@@ -129,22 +93,19 @@ bool load_file(std::map<std::string, Tensor>& tensors, const char* path, bool to
     ok = fseek(f, pad, SEEK_CUR) == 0 && nbytes == (uint64_t)tt.numel() * 4 &&
          pos + pad <= fsize && nbytes <= (uint64_t)(fsize - (pos + pad));   // the payload lies inside the file: a corrupt size cannot drive an allocation
     if (!ok) break;
-    if (!to_device) {
-      if (name.compare(0, 2, "__") == 0) {
-        tt.host.resize(nbytes / 4);
-        ok = read_exact(f, tt.host.data(), nbytes);
-      } else {
-        ok = fseek(f, (long)nbytes, SEEK_CUR) == 0;
-      }
+    if (name.compare(0, 2, "__") == 0) {
+      tt.host.resize(nbytes / 4);
+      ok = read_exact(f, tt.host.data(), nbytes);
+    } else if (!to_device) {
+      ok = fseek(f, (long)nbytes, SEEK_CUR) == 0;
+    } else {
+      host.resize(nbytes / 4);
+      ok = read_exact(f, host.data(), nbytes);
       if (!ok) break;
-      tensors[name] = tt;
-      continue;
+      if (cudaMalloc(&tt.dev, nbytes ? nbytes : 4) != cudaSuccess) { ok = false; set_err("cudaMalloc failed for " + name); break; }
+      cudaMemcpy(tt.dev, host.data(), nbytes, cudaMemcpyHostToDevice);
     }
-    host.resize(nbytes / 4);
-    ok = read_exact(f, host.data(), nbytes);
     if (!ok) break;
-    if (cudaMalloc(&tt.dev, nbytes ? nbytes : 4) != cudaSuccess) { ok = false; set_err("cudaMalloc failed for " + name); break; }
-    cudaMemcpy(tt.dev, host.data(), nbytes, cudaMemcpyHostToDevice);
     tensors[name] = tt;
   }
   fclose(f);
@@ -152,19 +113,95 @@ bool load_file(std::map<std::string, Tensor>& tensors, const char* path, bool to
   return ok;
 }
 
+// One model file loaded onto one device: its tensors, what the handle allocates beside them (weight planes, padded weights, the
+// fbank tables), and the handle's stream
+struct Loaded {
+  int device = 0;
+  std::map<std::string, Tensor> t;
+  std::vector<void*> owned;
+  cudaStream_t st = nullptr;
+  float* fbank_tables = nullptr;
+  bool open(const char* path, int dev) {
+    if (!path) { set_err("model_file is NULL"); return false; }
+    if (cudaSetDevice(dev) != cudaSuccess) { cudaGetLastError(); set_err("no such CUDA device (this library has no CPU path)"); return false; }
+    device = dev;
+    if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) { set_err("cudaStreamCreate failed"); return false; }
+    return load_file(t, path);
+  }
+  ~Loaded() {
+    for (auto& kv : t) if (kv.second.dev) cudaFree(kv.second.dev);
+    for (void* p : owned) cudaFree(p);
+    if (st) cudaStreamDestroy(st);
+  }
+};
+
+struct Model {
+  Loaded file;
+  int mode = 3;
+  int enc_layers = 0, dec_layers = 0, d_model = 512, heads = 4, kernel = 11, vocab = 0, feat_dim = 560;
+  float ln_eps = 1e-12f, cif_threshold = 1.f, tail_threshold = 0.45f;
+  std::vector<FaEncLayer> enc_l;
+  std::vector<FaDecLayer> dec_l;
+  FaEncoder enc{};
+  FaPredictor pred{};
+  FaDecoder dec{};
+  const float* cmvn = nullptr;
+  DevBuf wav, pcm16, lens, feats, flens, encb, acoustic, tok, alphas, peaks, ws, ids, best, fids, flens_out, hw, hw_lens;
+  DevBuf rec, gmeta;                                 // fa_offline_infer_vad: the device-resident recording, per-pack gather offsets
+  bool contextual = false;                           // ContextualParaformer: decoder with a hotword bias branch
+  bool ts = false;                                   // BiCifParaformer: CifPredictorV3's upsampled timestamp head
+  FaTimestampHead head{};
+  DevBuf us_alphas, us_peaks;
+  std::map<std::string, std::vector<float>> host_cache;   // fa_offline_host_tensor
+};
+
+struct Result {
+  std::vector<std::vector<int32_t>> ids;
+  std::vector<int32_t> token_num;
+  std::vector<std::vector<int32_t>> segs;            // fa_offline_infer_vad: {start_ms, end_ms, n_tokens} per segment, per recording
+  bool ts = false;                                   // the model has the timestamp head: stamps[i] = {start_ms, end_ms} pairs
+  std::vector<std::vector<int32_t>> stamps;
+  float audio_seconds = 0.f;
+};
+
+__global__ void pcm16_to_f32_kernel(const int16_t* __restrict__ src, float* __restrict__ dst, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = (float)src[i] * (1.0f / 32768.0f);     // exact; the frontend multiplies by 32768 again (wav_frontend.py:169)
+}
+
+// B host recordings bufs[i] of n[i] samples (f32, or s16le staged in pcm16) into rows of `stride` floats of dst
+bool upload(const void* const* bufs, const int64_t* n, int B, int64_t stride, int32_t pcm_format, DevBuf& dst, DevBuf& pcm16,
+            cudaStream_t st) {
+  const int64_t tot = (int64_t)B * stride;
+  if (!dst.reserve((size_t)(tot > 0 ? tot : 4) * 4)) { set_err("device allocation failed (waveforms)"); return false; }
+  if (tot == 0) return true;
+  float* wav = static_cast<float*>(dst.p);
+  if (pcm_format == 1) {
+    if (!pcm16.reserve((size_t)tot * 2)) { set_err("device allocation failed (pcm)"); return false; }
+    int16_t* p16 = static_cast<int16_t*>(pcm16.p);
+    for (int i = 0; i < B; ++i) cudaMemcpyAsync(p16 + (int64_t)i * stride, bufs[i], (size_t)n[i] * 2, cudaMemcpyHostToDevice, st);
+    pcm16_to_f32_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(p16, wav, tot);
+  } else {
+    for (int i = 0; i < B; ++i) cudaMemcpyAsync(wav + (int64_t)i * stride, bufs[i], (size_t)n[i] * 4, cudaMemcpyHostToDevice, st);
+  }
+  return true;
+}
+
 struct Builder {
-  Model& m;
+  Loaded& f;
+  int mode = FA_GEMM_F32_SIMT;
+  float ln_eps = 0.f;
   bool ok = true;
   const Tensor* get(const std::string& k) {
-    auto it = m.t.find(k);
-    if (it == m.t.end()) { if (ok) set_err("missing tensor " + k); ok = false; return nullptr; }
+    auto it = f.t.find(k);
+    if (it == f.t.end()) { if (ok) set_err("missing tensor " + k); ok = false; return nullptr; }
     return &it->second;
   }
   const float* ptr(const std::string& k) { const Tensor* t = get(k); return t ? t->dev : nullptr; }
   FaNorm norm(const std::string& p) {
     FaNorm nm{};
     const Tensor* w = get(p + ".weight");
-    nm.g = w ? w->dev : nullptr; nm.b = ptr(p + ".bias"); nm.n = w ? (int32_t)w->numel() : 0; nm.eps = m.ln_eps;
+    nm.g = w ? w->dev : nullptr; nm.b = ptr(p + ".bias"); nm.n = w ? (int32_t)w->numel() : 0; nm.eps = ln_eps;
     return nm;
   }
   FaLinear lin(const std::string& p, bool bias = true, const char* weight_key = nullptr, const char* bias_key = nullptr) {
@@ -174,26 +211,34 @@ struct Builder {
     if (!w || !(w->shape.size() == 2 || (w->shape.size() == 3 && w->shape[2] == 1))) { if (ok) set_err("bad weight " + p); ok = false; return L; }
     L.w = w->dev; L.b = bias ? ptr(bias_key ? std::string(bias_key) : p + ".bias") : nullptr;
     L.out_f = (int32_t)w->shape[0]; L.in_f = (int32_t)w->shape[1]; L.in_pad = (L.in_f + 63) / 64 * 64;
-    if (m.mode != FA_GEMM_F32_SIMT) {
+    if (mode != FA_GEMM_F32_SIMT) {
       void* planes = nullptr;
       if (cudaMalloc(&planes, (size_t)3 * L.out_f * L.in_pad * 2) != cudaSuccess) { ok = false; set_err("cudaMalloc planes"); return L; }
-      m.owned.push_back(planes);
-      if (fa_split_planes(L.w, L.in_f, L.out_f, L.in_f, L.in_pad, planes, m.st) != FA_OK) { ok = false; set_err("fa_split_planes failed"); }
+      f.owned.push_back(planes);
+      if (fa_split_planes(L.w, L.in_f, L.out_f, L.in_f, L.in_pad, planes, f.st) != FA_OK) { ok = false; set_err("fa_split_planes failed"); }
       L.w_planes = planes;
     }
     return L;
   }
+  // the frontend's fbank tables (fa_fbank_make_tables) from frontend.mel_banks and frontend.window
+  bool fbank_tables() {
+    const Tensor* mel = get("frontend.mel_banks");
+    const Tensor* win = get("frontend.window");
+    if (!mel || !win) return false;
+    void* tb = nullptr;
+    if (cudaMalloc(&tb, fa_fbank_tables_bytes()) != cudaSuccess) { set_err("cudaMalloc fbank tables"); return false; }
+    f.owned.push_back(tb);
+    f.fbank_tables = static_cast<float*>(tb);
+    if (fa_fbank_make_tables(mel->dev, win->dev, f.fbank_tables, f.st) != FA_OK) { set_err("fa_fbank_make_tables failed"); return false; }
+    return true;
+  }
 };
 
 // BiCifParaformer's timestamp head, recognised by predictor.upsample_cnn.weight, on the file's index (no device needed): every
-// tensor the launches read, in the shapes pack.py:timestamp_head_tensors writes, and __ts_config__.  A file without the head passes.
-struct TsHeadConfig {
-  bool present = false;
-  float smooth2 = 0.f, noise2 = 0.f;
-};
-
-bool check_ts_head(const std::map<std::string, Tensor>& t, TsHeadConfig& out) {
-  out = TsHeadConfig();
+// tensor the launches read, in the shapes pack.py:timestamp_head_tensors writes, and __ts_config__, whose values go into `head`.
+// A file without the head passes with head.up_times = 0.
+bool check_ts_head(const std::map<std::string, Tensor>& t, FaTimestampHead& head) {
+  head = FaTimestampHead{};
   if (!t.count("predictor.upsample_cnn.weight")) return true;
   auto cfg = t.find("__ts_config__");
   if (cfg == t.end() || cfg->second.host.size() < 3) {
@@ -217,34 +262,27 @@ bool check_ts_head(const std::map<std::string, Tensor>& t, TsHeadConfig& out) {
                                                                                           : it->second.numel() == n.d0;
     if (!ok) { set_err(std::string("BiCif timestamp head: bad shape of ") + n.name); return false; }
   }
-  out.present = true; out.smooth2 = c[1]; out.noise2 = c[2];
+  head.up_times = 3; head.smooth2 = c[1]; head.noise2 = c[2];
   return true;
 }
 
 bool build(Model& m) {
-  Builder b{m};
+  Builder b{m.file, m.mode};
   const Tensor* cfg = b.get("__config__");
-  if (!cfg || cfg->numel() < 10) { set_err("missing __config__"); return false; }
-  float c[10];
-  cudaMemcpy(c, cfg->dev, sizeof(c), cudaMemcpyDeviceToHost);
+  if (!cfg || cfg->host.size() < 10) { set_err("missing __config__"); return false; }
+  const float* c = cfg->host.data();
   m.enc_layers = (int)c[0]; m.dec_layers = (int)c[1]; m.d_model = (int)c[2]; m.heads = (int)c[3]; m.kernel = (int)c[4];
   m.vocab = (int)c[5]; m.feat_dim = (int)c[6]; m.ln_eps = c[7]; m.cif_threshold = c[8]; m.tail_threshold = c[9];
   if (m.enc_layers < 1 || m.dec_layers < 1 || m.d_model != 512 || m.heads * 128 != m.d_model) { set_err("unsupported config"); return false; }
+  b.ln_eps = m.ln_eps;
   // the FSMN tap count is read from each stack's own weight [512, 1, K]: encoder and decoder kernel_size are independent
   // constructor arguments in the reference (sanm/encoder.py:188, paraformer/decoder.py:234 — decoder default 21)
   auto fsmn_taps = [&](const char* key) -> int {
     const Tensor* t = b.get(key);
     return (t && t->shape.size() == 3) ? (int)t->shape[2] : m.kernel;
   };
-  m.mel = b.ptr("frontend.mel_banks"); m.window = b.ptr("frontend.window");
-  if (m.mel && m.window) {
-    void* tb = nullptr;
-    if (cudaMalloc(&tb, fa_fbank_tables_bytes()) != cudaSuccess) { set_err("cudaMalloc fbank tables"); return false; }
-    m.owned.push_back(tb);
-    m.fbank_tables = static_cast<float*>(tb);
-    if (fa_fbank_make_tables(m.mel, m.window, m.fbank_tables, m.st) != FA_OK) { set_err("fa_fbank_make_tables failed"); return false; }
-  }
-  m.cmvn = m.t.count("frontend.cmvn") ? m.t["frontend.cmvn"].dev : nullptr;
+  if (!b.fbank_tables()) return false;
+  m.cmvn = m.file.t.count("frontend.cmvn") ? m.file.t["frontend.cmvn"].dev : nullptr;
   // encoder (engine.py:_enc_stack; SANMEncoder encoder.py:188-461)
   m.enc_l.resize(m.enc_layers);
   for (int i = 0; i < m.enc_layers; ++i) {
@@ -263,10 +301,12 @@ bool build(Model& m) {
   m.pred.threshold = m.cif_threshold; m.pred.tail_threshold = m.tail_threshold; m.pred.smooth_factor = 1.f; m.pred.noise_threshold = 0.f;
   if (m.ts) {                   // BiCifParaformer: CifPredictorV3's sequential fp32 `cif` (bicif_paraformer/cif_predictor.py:37-84) + its head
     m.pred.cif_variant = 1;
-    m.up_lin = b.lin("predictor.upsample_cnn", true, "predictor.upsample_cnn.gemm_weight", "predictor.upsample_cnn.gemm_bias");
-    m.ih_lin = b.lin("predictor.blstm.ih", true, "predictor.blstm.ih_gemm_weight", "predictor.blstm.ih_gemm_bias");
-    m.hh_f = b.ptr("predictor.blstm.weight_hh_l0"); m.hh_b = b.ptr("predictor.blstm.weight_hh_l0_reverse");
-    m.out2_w = b.ptr("predictor.cif_output2.weight"); m.out2_b = b.ptr("predictor.cif_output2.bias");
+    FaTimestampHead& h = m.head;
+    h.upsample = b.lin("predictor.upsample_cnn", true, "predictor.upsample_cnn.gemm_weight", "predictor.upsample_cnn.gemm_bias");
+    h.blstm_ih = b.lin("predictor.blstm.ih", true, "predictor.blstm.ih_gemm_weight", "predictor.blstm.ih_gemm_bias");
+    h.w_hh_fwd = b.ptr("predictor.blstm.weight_hh_l0"); h.w_hh_bwd = b.ptr("predictor.blstm.weight_hh_l0_reverse");
+    h.out2_w = b.ptr("predictor.cif_output2.weight"); h.out2_b = b.ptr("predictor.cif_output2.bias");
+    h.threshold = m.cif_threshold;
   }
   // decoder (ParaformerSANMDecoder decoder.py:234-449)
   auto dec_layer = [&](FaDecLayer& L, const std::string& p, bool full) {
@@ -280,7 +320,7 @@ bool build(Model& m) {
   };
   // ContextualParaformerDecoder (contextual_paraformer/decoder.py:133-352): the last attention layer is `last_decoder`, plus the
   // hotword branch bias_decoder (norm3 + cross attention) and bias_output (Conv1d 1024 -> 512, k = 1)
-  m.contextual = m.t.count("decoder.bias_decoder.norm3.weight") > 0;
+  m.contextual = m.file.t.count("decoder.bias_decoder.norm3.weight") > 0;
   const int n_plain = m.contextual ? m.dec_layers - 1 : m.dec_layers;
   m.dec_l.resize(n_plain > 0 ? n_plain : 1);
   for (int i = 0; i < n_plain; ++i) dec_layer(m.dec_l[i], "decoder.decoders." + std::to_string(i), true);
@@ -298,7 +338,7 @@ bool build(Model& m) {
     m.dec.clas_scale = 1.0f;
   }
   if (!b.ok) return false;
-  return cudaStreamSynchronize(m.st) == cudaSuccess;
+  return cudaStreamSynchronize(m.file.st) == cudaSuccess;
 }
 
 int num_lfr_frames(int64_t n) {       // wav_frontend.py:73 after kaldi.py snip_edges framing
@@ -309,8 +349,10 @@ int num_lfr_frames(int64_t n) {       // wav_frontend.py:73 after kaldi.py snip_
 // The recogniser over a padded batch already on the device: wav [B, stride] fp32 (m.wav or any buffer the call does not reuse),
 // lens_h [B] samples (>= 400 each).  Everything after the host-to-device copy of fa_offline_infer_hw; fa_offline_infer_vad feeds it the
 // gathered VAD segments of one pack.
-Result* decode_batch(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const float* hw_embed, int32_t n_hotwords) {
+std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const float* hw_embed,
+                                     int32_t n_hotwords) {
   const int B = (int)lens_h.size(), D = m.d_model;
+  cudaStream_t st = m.file.st;
   int t_max = 0;
   double seconds = 0.0;
   for (int i = 0; i < B; ++i) {
@@ -319,112 +361,91 @@ Result* decode_batch(Model& m, const float* wav, int64_t stride, const std::vect
     seconds += (double)lens_h[i] / 16000.0;
   }
   const int T = t_max;
-#define FA_OFF(x, msg) do { if (!(x)) { set_err(msg); return nullptr; } } while (0)
-  FA_OFF(m.lens.reserve((size_t)B * 4), "device allocation failed (lengths)");
-  cudaMemcpyAsync(m.lens.p, lens_h.data(), (size_t)B * 4, cudaMemcpyHostToDevice, m.st);
+  if (!m.lens.reserve((size_t)B * 4)) return fail("device allocation failed (lengths)");
+  cudaMemcpyAsync(m.lens.p, lens_h.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st);
   const int n_cap = T + 1;
-  FA_OFF(m.feats.reserve((size_t)B * T * m.feat_dim * 4) && m.flens.reserve((size_t)B * 4) && m.encb.reserve((size_t)B * T * D * 4) &&
-             m.acoustic.reserve((size_t)B * n_cap * D * 4) && m.tok.reserve((size_t)B * 4) && m.alphas.reserve((size_t)B * n_cap * 4) &&
-             m.peaks.reserve((size_t)B * n_cap * 4),
-         "device allocation failed (activations)");
+  if (!(m.feats.reserve((size_t)B * T * m.feat_dim * 4) && m.flens.reserve((size_t)B * 4) && m.encb.reserve((size_t)B * T * D * 4) &&
+        m.acoustic.reserve((size_t)B * n_cap * D * 4) && m.tok.reserve((size_t)B * 4) && m.alphas.reserve((size_t)B * n_cap * 4) &&
+        m.peaks.reserve((size_t)B * n_cap * 4)))
+    return fail("device allocation failed (activations)");
   size_t ws = fa_sanm_encoder_workspace_bytes(B, T, m.mode);
   const size_t ws2 = fa_cif_predictor_workspace_bytes(B, T, m.mode);
   ws = ws2 > ws ? ws2 : ws;
-  FA_OFF(m.ws.reserve(ws), "device allocation failed (workspace)");
-  int rc = fa_fbank_lfr_cmvn_tables(wav, static_cast<int32_t*>(m.lens.p), B, stride, m.cmvn, m.fbank_tables, 7, 6, static_cast<float*>(m.feats.p),
-                                    T, static_cast<int32_t*>(m.flens.p), T, m.st);
-  FA_OFF(rc == FA_OK, std::string("fa_fbank_lfr_cmvn_tables: ") + fa_status_string(rc));
+  if (!m.ws.reserve(ws)) return fail("device allocation failed (workspace)");
+  int rc = fa_fbank_lfr_cmvn_tables(wav, static_cast<int32_t*>(m.lens.p), B, stride, m.cmvn, m.file.fbank_tables, 7, 6, static_cast<float*>(m.feats.p),
+                                    T, static_cast<int32_t*>(m.flens.p), T, st);
+  if (rc != FA_OK) return fail(std::string("fa_fbank_lfr_cmvn_tables: ") + fa_status_string(rc));
   rc = fa_sanm_encoder_forward(&m.enc, static_cast<float*>(m.feats.p), static_cast<int32_t*>(m.flens.p), B, T, static_cast<float*>(m.encb.p),
-                               m.mode, m.ws.p, m.ws.cap, m.st);
-  FA_OFF(rc == FA_OK, std::string("fa_sanm_encoder_forward: ") + fa_status_string(rc));
+                               m.mode, m.ws.p, m.ws.cap, st);
+  if (rc != FA_OK) return fail(std::string("fa_sanm_encoder_forward: ") + fa_status_string(rc));
   rc = fa_cif_predictor_forward(&m.pred, static_cast<float*>(m.encb.p), static_cast<int32_t*>(m.flens.p), B, T, static_cast<float*>(m.acoustic.p),
                                 n_cap, static_cast<int32_t*>(m.tok.p), static_cast<float*>(m.alphas.p), static_cast<float*>(m.peaks.p), m.mode,
-                                m.ws.p, m.ws.cap, m.st);
-  FA_OFF(rc == FA_OK, std::string("fa_cif_predictor_forward: ") + fa_status_string(rc));
-  Result* r = new Result();
+                                m.ws.p, m.ws.cap, st);
+  if (rc != FA_OK) return fail(std::string("fa_cif_predictor_forward: ") + fa_status_string(rc));
+  std::unique_ptr<Result> r(new Result());
   r->audio_seconds = (float)seconds;
   r->token_num.resize(B);
   r->ts = m.ts;
   if (m.ts) r->stamps.resize(B);
-  cudaMemcpyAsync(r->token_num.data(), m.tok.p, (size_t)B * 4, cudaMemcpyDeviceToHost, m.st);
-  if (cudaStreamSynchronize(m.st) != cudaSuccess) { set_err(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError())); delete r; return nullptr; }
+  cudaMemcpyAsync(r->token_num.data(), m.tok.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess) return fail(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError()));
   int n_max = 0;                                             // the path's one host sync (cif_predictor.py:311)
   for (int i = 0; i < B; ++i) n_max = r->token_num[i] > n_max ? r->token_num[i] : n_max;
   r->ids.resize(B);
   if (n_max < 1) return r;                                   // paraformer/model.py:615-616
   const int nh = m.contextual ? n_hotwords : 0;
-  if (!(m.ids.reserve((size_t)B * n_max * 4) && m.best.reserve((size_t)B * n_max * 4) && m.fids.reserve((size_t)B * n_max * 4) &&
-        m.flens_out.reserve((size_t)B * 4) && m.ws.reserve(fa_paraformer_decoder_workspace_bytes_hw(B, T, n_max, m.vocab, m.mode, nh)))) {
-    set_err("device allocation failed (decoder)"); delete r; return nullptr;
-  }
-  // the timestamp head over the [B, 3T] upsampled frames; its two GEMMs share the workspace, the larger carve is the B*3T-row one
-  const int U = 3, TU = T * U;
+  // the timestamp head over the [B, 3T] upsampled frames shares the workspace with the decoder
+  const int U = m.head.up_times, TU = T * U;
   const int64_t rows_up = (int64_t)B * TU;
-  const int lstm_rows = B < 256 ? B : 256;                   // fa_blstm_forward_tc holds at most 256 sequences per launch
-  if (m.ts && !(m.up.reserve((size_t)rows_up * D * 4) && m.xproj.reserve((size_t)rows_up * 8 * D * 4) &&
-                m.feat.reserve((size_t)rows_up * 2 * D * 4) && m.us_alphas.reserve((size_t)rows_up * 4) && m.us_peaks.reserve((size_t)rows_up * 4) &&
-                m.lens_up.reserve((size_t)B * 4) && m.lstm_scratch.reserve(fa_blstm_tc_scratch_bytes(lstm_rows)) &&
-                m.ws.reserve(fa_linear_workspace_bytes(rows_up, D, m.mode)))) {
-    set_err("device allocation failed (timestamp head)"); delete r; return nullptr;
-  }
+  size_t ws_dec = fa_paraformer_decoder_workspace_bytes_hw(B, T, n_max, m.vocab, m.mode, nh);
+  if (m.ts) ws_dec = std::max(ws_dec, fa_timestamp_head_workspace_bytes(B, T, D, U, m.mode));
+  if (!(m.ids.reserve((size_t)B * n_max * 4) && m.best.reserve((size_t)B * n_max * 4) && m.fids.reserve((size_t)B * n_max * 4) &&
+        m.flens_out.reserve((size_t)B * 4) && m.ws.reserve(ws_dec)))
+    return fail("device allocation failed (decoder)");
+  if (m.ts && !(m.us_alphas.reserve((size_t)rows_up * 4) && m.us_peaks.reserve((size_t)rows_up * 4)))
+    return fail("device allocation failed (timestamp head)");
   if (m.contextual) {                                        // hotword memory [n_hw, 512] (contextual_paraformer/model.py:350-372) + per-utterance counts
-    if (!(m.hw.reserve((size_t)nh * D * 4) && m.hw_lens.reserve((size_t)B * 4))) { set_err("device allocation failed (hotwords)"); delete r; return nullptr; }
+    if (!(m.hw.reserve((size_t)nh * D * 4) && m.hw_lens.reserve((size_t)B * 4))) return fail("device allocation failed (hotwords)");
     std::vector<int32_t> hl(B, nh);
-    cudaMemcpyAsync(m.hw.p, hw_embed, (size_t)nh * D * 4, cudaMemcpyHostToDevice, m.st);
-    cudaMemcpyAsync(m.hw_lens.p, hl.data(), (size_t)B * 4, cudaMemcpyHostToDevice, m.st);
-    cudaStreamSynchronize(m.st);                             // hl is a stack vector
+    cudaMemcpyAsync(m.hw.p, hw_embed, (size_t)nh * D * 4, cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(m.hw_lens.p, hl.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st);
+    cudaStreamSynchronize(st);                               // hl is a stack vector
     m.dec.has_bias = 1; m.dec.n_hotwords = nh;
     m.dec.hw_embed = static_cast<const float*>(m.hw.p); m.dec.hw_lens = static_cast<const int32_t*>(m.hw_lens.p);
   }
   rc = fa_paraformer_decoder_forward(&m.dec, static_cast<float*>(m.encb.p), static_cast<int32_t*>(m.flens.p), B, T, static_cast<float*>(m.acoustic.p),
                                      n_cap, static_cast<int32_t*>(m.tok.p), n_max, static_cast<int32_t*>(m.ids.p), static_cast<float*>(m.best.p),
-                                     nullptr, 1, m.mode, m.ws.p, m.ws.cap, m.st);
+                                     nullptr, 1, m.mode, m.ws.p, m.ws.cap, st);
   if (rc == FA_OK)
     rc = fa_greedy_filter(static_cast<int32_t*>(m.ids.p), static_cast<int32_t*>(m.tok.p), B, n_max, 1, 2, 0, static_cast<int32_t*>(m.fids.p),
-                          static_cast<int32_t*>(m.flens_out.p), m.st);
-  if (rc != FA_OK) { set_err(std::string("decoder: ") + fa_status_string(rc)); delete r; return nullptr; }
+                          static_cast<int32_t*>(m.flens_out.p), st);
+  if (rc != FA_OK) return fail(std::string("decoder: ") + fa_status_string(rc));
   if (m.ts) {                   // CifPredictorV3.get_upsample_timestamp (bicif_paraformer/cif_predictor.py:300-352), engine.upsample_timestamp
-    float* up = static_cast<float*>(m.up.p);
-    float* xproj = static_cast<float*>(m.xproj.p);
-    float* feat = static_cast<float*>(m.feat.p);
-    rc = fa_linear(static_cast<float*>(m.encb.p), D, (int64_t)B * T, &m.up_lin, 0, nullptr, 0, nullptr, 0, up, (int64_t)U * D, m.mode, m.ws.p,
-                   m.ws.cap, m.st);
-    if (rc == FA_OK)
-      rc = fa_linear(up, D, rows_up, &m.ih_lin, 0, nullptr, 0, nullptr, 0, xproj, (int64_t)8 * D, m.mode, m.ws.p, m.ws.cap, m.st);
-    for (int b0 = 0; b0 < B && rc == FA_OK; b0 += 256) {     // sequences are independent: larger batches run as consecutive launches
-      const int bn = B - b0 < 256 ? B - b0 : 256;
-      rc = fa_blstm_forward_tc(xproj + (int64_t)b0 * TU * 8 * D, m.hh_f, m.hh_b, bn, TU, D, feat + (int64_t)b0 * TU * 2 * D, m.lstm_scratch.p,
-                               m.lstm_scratch.cap, m.st);
-    }
-    if (rc == FA_OK) {
-      scale_lens_kernel<<<(B + 255) / 256, 256, 0, m.st>>>(static_cast<const int32_t*>(m.flens.p), U, B, static_cast<int32_t*>(m.lens_up.p));
-      rc = fa_cif_upsample_alphas(feat, 2 * D, m.out2_w, m.out2_b, static_cast<const int32_t*>(m.lens_up.p), static_cast<const int32_t*>(m.tok.p), B, TU,
-                                  m.smooth2, m.noise2, m.cif_threshold, static_cast<float*>(m.us_alphas.p), static_cast<float*>(m.us_peaks.p), m.st);
-    }
-    if (rc != FA_OK) { set_err(std::string("timestamp head: ") + fa_status_string(rc)); delete r; return nullptr; }
+    rc = fa_timestamp_head_forward(&m.head, static_cast<float*>(m.encb.p), static_cast<int32_t*>(m.flens.p), static_cast<int32_t*>(m.tok.p), B, T,
+                                   static_cast<float*>(m.us_alphas.p), static_cast<float*>(m.us_peaks.p), m.mode, m.ws.p, m.ws.cap, st);
+    if (rc != FA_OK) return fail(std::string("timestamp head: ") + fa_status_string(rc));
   }
   std::vector<int32_t> fids((size_t)B * n_max), fl(B), enc_lens(m.ts ? B : 0);
   std::vector<float> us_alphas(m.ts ? rows_up : 0), us_peaks(m.ts ? rows_up : 0);
-  cudaMemcpyAsync(fids.data(), m.fids.p, fids.size() * 4, cudaMemcpyDeviceToHost, m.st);
-  cudaMemcpyAsync(fl.data(), m.flens_out.p, (size_t)B * 4, cudaMemcpyDeviceToHost, m.st);
+  cudaMemcpyAsync(fids.data(), m.fids.p, fids.size() * 4, cudaMemcpyDeviceToHost, st);
+  cudaMemcpyAsync(fl.data(), m.flens_out.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st);
   if (m.ts) {                                                // on the same synchronisation as the ids
-    cudaMemcpyAsync(enc_lens.data(), m.flens.p, (size_t)B * 4, cudaMemcpyDeviceToHost, m.st);
-    cudaMemcpyAsync(us_alphas.data(), m.us_alphas.p, (size_t)rows_up * 4, cudaMemcpyDeviceToHost, m.st);
-    cudaMemcpyAsync(us_peaks.data(), m.us_peaks.p, (size_t)rows_up * 4, cudaMemcpyDeviceToHost, m.st);
+    cudaMemcpyAsync(enc_lens.data(), m.flens.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st);
+    cudaMemcpyAsync(us_alphas.data(), m.us_alphas.p, (size_t)rows_up * 4, cudaMemcpyDeviceToHost, st);
+    cudaMemcpyAsync(us_peaks.data(), m.us_peaks.p, (size_t)rows_up * 4, cudaMemcpyDeviceToHost, st);
   }
-  if (cudaStreamSynchronize(m.st) != cudaSuccess) { set_err(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError())); delete r; return nullptr; }
+  if (cudaStreamSynchronize(st) != cudaSuccess) return fail(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError()));
   for (int i = 0; i < B; ++i) r->ids[i].assign(fids.begin() + (size_t)i * n_max, fids.begin() + (size_t)i * n_max + fl[i]);
   if (m.ts) {                                                // bicif_paraformer/model.py:402-407: each utterance's first 3 * enc_len frames
     for (int i = 0; i < B; ++i) {
       const int64_t n = (int64_t)U * enc_lens[i];
-      std::vector<int32_t>& st = r->stamps[i];
-      st.resize((size_t)(2 * (n > 0 ? n : 1)));              // at most n - 1 spans
+      std::vector<int32_t>& sp = r->stamps[i];
+      sp.resize((size_t)(2 * (n > 0 ? n : 1)));              // at most n - 1 spans
       const int64_t k = fa_ts_stamps_host(us_alphas.data() + (size_t)i * TU, us_peaks.data() + (size_t)i * TU, n, (int64_t)r->ids[i].size(), U, 0.0,
-                                          st.data(), n);
-      st.resize(k > 0 ? (size_t)(2 * k) : 0);
+                                          sp.data(), n);
+      sp.resize(k > 0 ? (size_t)(2 * k) : 0);
     }
   }
-#undef FA_OFF
   return r;
 }
 
@@ -436,30 +457,15 @@ extern "C" void* fa_offline_infer_hw(void* handle, const void* const* bufs, cons
 
 extern "C" void* fa_offline_init(const char* model_file, int32_t device, int32_t gemm_mode) {
   g_err.clear();
-  if (!model_file) { set_err("model_file is NULL"); return nullptr; }
-  if (gemm_mode != FA_GEMM_F32_SIMT && gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) {
-    set_err("bad gemm_mode"); return nullptr;
-  }
-  TsHeadConfig head;
-  try {                                   // what the file's index alone decides (the timestamp head) is refused before any device work
-    std::map<std::string, Tensor> index;
-    if (!load_file(index, model_file, false) || !check_ts_head(index, head)) return nullptr;
-  } catch (const std::exception& e) {
-    set_err(std::string("model file rejected: ") + e.what()); return nullptr;
-  }
-  if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); set_err("no such CUDA device (this library has no CPU path)"); return nullptr; }
-  Model* m = new Model();
-  m->device = device; m->mode = gemm_mode;
-  m->ts = head.present; m->smooth2 = head.smooth2; m->noise2 = head.noise2;
-  if (cudaStreamCreateWithFlags(&m->st, cudaStreamNonBlocking) != cudaSuccess) { set_err("cudaStreamCreate failed"); delete m; return nullptr; }
-  bool ok = false;
-  try {                                   // a malformed file can ask for an absurd allocation: no C++ exception may cross the C ABI
-    ok = load_file(m->t, model_file) && build(*m);
-  } catch (const std::exception& e) {
-    set_err(std::string("model file rejected: ") + e.what());
-  }
-  if (!ok) { delete m; return nullptr; }
-  return m;
+  if (!model_file) return fail("model_file is NULL");
+  if (gemm_mode != FA_GEMM_F32_SIMT && gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) return fail("bad gemm_mode");
+  FaTimestampHead head{};
+  std::map<std::string, Tensor> index;          // what the file's index alone decides (the timestamp head) is refused before any device work
+  if (!no_throw("model file rejected: ", [&] { return load_file(index, model_file, false) && check_ts_head(index, head); })) return nullptr;
+  std::unique_ptr<Model> m(new Model());
+  m->mode = gemm_mode; m->head = head; m->ts = head.up_times > 0;
+  if (!no_throw("model file rejected: ", [&] { return m->file.open(model_file, device) && build(*m); })) return nullptr;
+  return m.release();
 }
 
 extern "C" void fa_offline_uninit(void* handle) { delete static_cast<Model*>(handle); }
@@ -472,13 +478,18 @@ extern "C" const float* fa_offline_host_tensor(void* handle, const char* name, i
   Model* m = static_cast<Model*>(handle);
   if (numel) *numel = 0;
   if (!m || !name) return nullptr;
-  auto it = m->t.find(name);
-  if (it == m->t.end()) return nullptr;
+  auto it = m->file.t.find(name);
+  if (it == m->file.t.end()) return nullptr;
+  const Tensor& t = it->second;
+  if (!t.dev) {                                 // a "__" configuration tensor: its payload is on the host already
+    if (numel) *numel = (int64_t)t.host.size();
+    return t.host.data();
+  }
   auto& hc = m->host_cache[name];
-  if (hc.empty() && it->second.numel() > 0) {
-    hc.resize((size_t)it->second.numel());
-    cudaSetDevice(m->device);
-    if (cudaMemcpy(hc.data(), it->second.dev, hc.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess) { hc.clear(); return nullptr; }
+  if (hc.empty() && t.numel() > 0) {
+    hc.resize((size_t)t.numel());
+    cudaSetDevice(m->file.device);
+    if (cudaMemcpy(hc.data(), t.dev, hc.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess) { hc.clear(); return nullptr; }
   }
   if (numel) *numel = (int64_t)hc.size();
   return hc.data();
@@ -492,31 +503,20 @@ extern "C" void* fa_offline_infer_hw(void* handle, const void* const* bufs, cons
                                      const float* hw_embed, int32_t n_hotwords) {
   g_err.clear();
   Model* mp = static_cast<Model*>(handle);
-  if (!mp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) { set_err("bad argument"); return nullptr; }
+  if (!mp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) return fail("bad argument");
   Model& m = *mp;
-  if (m.contextual && (!hw_embed || n_hotwords < 1)) { set_err("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)"); return nullptr; }
-  cudaSetDevice(m.device);
+  if (m.contextual && (!hw_embed || n_hotwords < 1)) return fail("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)");
+  cudaSetDevice(m.file.device);
   int64_t nmax = 0;
   std::vector<int32_t> lens_h(batch);
   for (int i = 0; i < batch; ++i) {
-    if (!bufs[i] || n_samples[i] < 400 || n_samples[i] > 0x7fffffffLL) { set_err("every buffer needs >= 400 samples (25 ms)"); return nullptr; }
+    if (!bufs[i] || n_samples[i] < 400 || n_samples[i] > 0x7fffffffLL) return fail("every buffer needs >= 400 samples (25 ms)");
     lens_h[i] = (int32_t)n_samples[i];
     nmax = n_samples[i] > nmax ? n_samples[i] : nmax;
   }
-  const int B = batch;
   const int64_t stride = (nmax + 3) / 4 * 4;
-  if (!m.wav.reserve((size_t)B * stride * 4)) { set_err("device allocation failed (waveforms)"); return nullptr; }
-  float* wav = static_cast<float*>(m.wav.p);
-  if (pcm_format == 1) {
-    if (!m.pcm16.reserve((size_t)B * stride * 2)) { set_err("device allocation failed (pcm)"); return nullptr; }
-    int16_t* p16 = static_cast<int16_t*>(m.pcm16.p);
-    for (int i = 0; i < B; ++i) cudaMemcpyAsync(p16 + (int64_t)i * stride, bufs[i], (size_t)n_samples[i] * 2, cudaMemcpyHostToDevice, m.st);
-    const int64_t tot = (int64_t)B * stride;
-    pcm16_to_f32_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, m.st>>>(p16, wav, tot);
-  } else {
-    for (int i = 0; i < B; ++i) cudaMemcpyAsync(wav + (int64_t)i * stride, bufs[i], (size_t)n_samples[i] * 4, cudaMemcpyHostToDevice, m.st);
-  }
-  return decode_batch(m, wav, stride, lens_h, hw_embed, n_hotwords);
+  if (!upload(bufs, n_samples, batch, stride, pcm_format, m.wav, m.pcm16, m.file.st)) return nullptr;
+  return decode_batch(m, static_cast<const float*>(m.wav.p), stride, lens_h, hw_embed, n_hotwords).release();
 }
 
 extern "C" int32_t fa_offline_result_count(const void* result) { return result ? (int32_t)static_cast<const Result*>(result)->ids.size() : 0; }
@@ -547,21 +547,12 @@ namespace {
 enum { kVadCfgInts = 14, kVadCfgDoubles = 5, kVadCfgLorder = 19, kVadCfgNSil = 20, kVadCfgSil = 21, kVadCfgLen = 25 };
 
 struct Vad {
-  int device = 0;
-  std::map<std::string, Tensor> t;
-  std::vector<void*> owned;                          // padded weights, fbank tables
+  Loaded file;
   std::vector<FaVadLayer> layers;
   FaVadEncoder enc{};
   FaVadOptions opts{};
   const float* cmvn = nullptr;
-  float* fbank_tables = nullptr;
-  cudaStream_t st = nullptr;
   DevBuf wav, pcm16, lens, feats, flens, frames, ws;
-  ~Vad() {
-    for (auto& kv : t) if (kv.second.dev) cudaFree(kv.second.dev);
-    for (void* p : owned) cudaFree(p);
-    if (st) cudaStreamDestroy(st);
-  }
 };
 
 struct VadResult {
@@ -571,16 +562,12 @@ struct VadResult {
 };
 
 bool build_vad(Vad& v) {
-  auto get = [&](const std::string& k) -> const Tensor* {
-    auto it = v.t.find(k);
-    if (it == v.t.end()) { set_err("missing tensor " + k); return nullptr; }
-    return &it->second;
-  };
-  const Tensor* cfg = get("__vad_config__");
+  Builder b{v.file};
+  const Tensor* cfg = b.get("__vad_config__");
   if (!cfg) return false;
-  if (cfg->numel() != 2 * kVadCfgLen) { set_err("bad __vad_config__"); return false; }
+  if (cfg->host.size() != 2 * kVadCfgLen) { set_err("bad __vad_config__"); return false; }
   double c[kVadCfgLen];
-  if (cudaMemcpy(c, cfg->dev, sizeof(c), cudaMemcpyDeviceToHost) != cudaSuccess) { set_err("cudaMemcpy failed"); return false; }
+  memcpy(c, cfg->host.data(), sizeof(c));
   int32_t* oi = &v.opts.sample_rate;                 // the 14 int32 fields, in declaration order
   for (int k = 0; k < kVadCfgInts; ++k) oi[k] = (int32_t)c[k];
   v.opts.speech_2_noise_ratio = c[14]; v.opts.snr_thres = c[15]; v.opts.decibel_thres = c[16]; v.opts.speech_noise_thres = c[17];
@@ -589,53 +576,45 @@ bool build_vad(Vad& v) {
   if (lorder != 20 || n_sil < 1 || n_sil > 4 || v.opts.frame_in_ms <= 0 || v.opts.window_size_ms < v.opts.frame_in_ms) {
     set_err("unsupported VAD config"); return false;
   }
-  const Tensor* mel = get("frontend.mel_banks");
-  const Tensor* win = get("frontend.window");
-  if (!mel || !win) return false;
-  void* tb = nullptr;
-  if (cudaMalloc(&tb, fa_fbank_tables_bytes()) != cudaSuccess) { set_err("cudaMalloc fbank tables"); return false; }
-  v.owned.push_back(tb);
-  v.fbank_tables = static_cast<float*>(tb);
-  if (fa_fbank_make_tables(mel->dev, win->dev, v.fbank_tables, v.st) != FA_OK) { set_err("fa_fbank_make_tables failed"); return false; }
-  if (v.t.count("frontend.cmvn")) {
-    if (v.t["frontend.cmvn"].numel() != 2 * 400) { set_err("frontend.cmvn must be [2, 400]"); return false; }
-    v.cmvn = v.t["frontend.cmvn"].dev;
+  if (!b.fbank_tables()) return false;
+  if (v.file.t.count("frontend.cmvn")) {
+    if (v.file.t["frontend.cmvn"].numel() != 2 * 400) { set_err("frontend.cmvn must be [2, 400]"); return false; }
+    v.cmvn = v.file.t["frontend.cmvn"].dev;
   }
-  bool ok = true;
   // weights [out, in] -> [out, in rounded up to 16] with zero columns (VadEngine._lin): the fp32 GEMMs read K = the padded width
   auto lin = [&](const std::string& p, bool bias) -> FaLinear {
     FaLinear L{};
-    const Tensor* w = get(p + ".weight");
-    if (!w || w->shape.size() != 2) { if (ok && w) set_err("bad weight " + p); ok = false; return L; }
+    const Tensor* w = b.get(p + ".weight");
+    if (!w || w->shape.size() != 2) { if (b.ok && w) set_err("bad weight " + p); b.ok = false; return L; }
     const int out_f = (int)w->shape[0], in_f = (int)w->shape[1], kp = (in_f + 15) / 16 * 16;
     void* wp = nullptr;
-    if (cudaMalloc(&wp, (size_t)out_f * kp * 4) != cudaSuccess) { set_err("cudaMalloc weights"); ok = false; return L; }
-    v.owned.push_back(wp);
+    if (cudaMalloc(&wp, (size_t)out_f * kp * 4) != cudaSuccess) { set_err("cudaMalloc weights"); b.ok = false; return L; }
+    v.file.owned.push_back(wp);
     if (cudaMemset(wp, 0, (size_t)out_f * kp * 4) != cudaSuccess ||
         cudaMemcpy2D(wp, (size_t)kp * 4, w->dev, (size_t)in_f * 4, (size_t)in_f * 4, out_f, cudaMemcpyDeviceToDevice) != cudaSuccess) {
-      set_err("weight copy failed"); ok = false; return L;
+      set_err("weight copy failed"); b.ok = false; return L;
     }
     L.w = static_cast<const float*>(wp);
     if (bias) {
-      const Tensor* b = get(p + ".bias");
-      if (!b || b->numel() != out_f) { if (ok && b) set_err("bad bias " + p); ok = false; return L; }
-      L.b = b->dev;
+      const Tensor* bt = b.get(p + ".bias");
+      if (!bt || bt->numel() != out_f) { if (b.ok && bt) set_err("bad bias " + p); b.ok = false; return L; }
+      L.b = bt->dev;
     }
     L.out_f = out_f; L.in_f = kp; L.in_pad = kp;
     return L;
   };
   int n_layers = 0;
-  while (v.t.count("encoder.fsmn." + std::to_string(n_layers) + ".linear.linear.weight")) ++n_layers;
+  while (v.file.t.count("encoder.fsmn." + std::to_string(n_layers) + ".linear.linear.weight")) ++n_layers;
   v.layers.resize(n_layers > 0 ? n_layers : 1);
   v.enc.in1 = lin("encoder.in_linear1.linear", true);
   v.enc.in2 = lin("encoder.in_linear2.linear", true);
-  for (int i = 0; i < n_layers && ok; ++i) {
+  for (int i = 0; i < n_layers && b.ok; ++i) {
     const std::string p = "encoder.fsmn." + std::to_string(i) + ".";
-    if (v.t.count(p + "fsmn_block.conv_right.weight")) { set_err("FSMN-VAD with a right-context memory (rorder > 0) is not supported"); return false; }
+    if (v.file.t.count(p + "fsmn_block.conv_right.weight")) { set_err("FSMN-VAD with a right-context memory (rorder > 0) is not supported"); return false; }
     v.layers[i].lin = lin(p + "linear.linear", false);
-    const Tensor* cw = get(p + "fsmn_block.conv_left.weight");   // [proj, 1, lorder, 1] = [proj, lorder] contiguous
+    const Tensor* cw = b.get(p + "fsmn_block.conv_left.weight");   // [proj, 1, lorder, 1] = [proj, lorder] contiguous
     if (!cw || cw->shape.size() != 4 || cw->shape[1] != 1 || cw->shape[2] != lorder || cw->shape[3] != 1) {
-      if (ok && cw) set_err("bad " + p + "fsmn_block.conv_left.weight");
+      if (b.ok && cw) set_err("bad " + p + "fsmn_block.conv_left.weight");
       return false;
     }
     v.layers[i].conv_w = cw->dev;
@@ -646,11 +625,11 @@ bool build_vad(Vad& v) {
   v.enc.out2 = lin("encoder.out_linear2.linear", true);
   for (int k = 0; k < n_sil; ++k) v.enc.sil_ids[k] = (int32_t)c[kVadCfgSil + k];
   v.enc.n_sil = n_sil;
-  if (!ok) return false;
+  if (!b.ok) return false;
   if (v.enc.in1.in_f != 400) { set_err("the VAD frontend is 80 mel x LFR 5: in_linear1 must take 400 inputs"); return false; }
   for (int k = 0; k < n_sil; ++k)
     if (v.enc.sil_ids[k] < 0 || v.enc.sil_ids[k] >= v.enc.out2.out_f) { set_err("sil_pdf_ids outside the output"); return false; }
-  return cudaStreamSynchronize(v.st) == cudaSuccess;
+  return cudaStreamSynchronize(v.file.st) == cudaSuccess;
 }
 
 const double kSilenceSchedule[] = {10000, 2000, 20000, 1000, 30000, 800, 40000, 600, 50000, 400, 60000, 200, -1, 100};   // vad.py
@@ -669,7 +648,7 @@ bool vad_run(Vad& v, const float* wav, int64_t n, cudaStream_t st, const FaVadRu
   }
   float* frames = static_cast<float*>(v.frames.p);
   cudaMemcpyAsync(v.lens.p, &n32, 4, cudaMemcpyHostToDevice, st);
-  int rc = fa_fbank_lfr_cmvn_tables(wav, static_cast<int32_t*>(v.lens.p), 1, n, v.cmvn, v.fbank_tables, 5, 1, static_cast<float*>(v.feats.p), T,
+  int rc = fa_fbank_lfr_cmvn_tables(wav, static_cast<int32_t*>(v.lens.p), 1, n, v.cmvn, v.file.fbank_tables, 5, 1, static_cast<float*>(v.feats.p), T,
                                     static_cast<int32_t*>(v.flens.p), (int32_t)T, st);
   if (rc == FA_OK) rc = fa_fsmn_vad_forward(&v.enc, static_cast<float*>(v.feats.p), 400, (int32_t)T, frames, nullptr, v.ws.p, v.ws.cap, st);
   if (rc == FA_OK) rc = fa_frame_decibels(wav, n, (int32_t)T, frames + T, st);
@@ -698,20 +677,9 @@ FaVadRunOptions default_vad_run() {
   return r;
 }
 
-// one recording (host) -> fp32 on the device in `dst` (s16 through `pcm16`)
-bool upload(const void* buf, int64_t n, int32_t pcm_format, DevBuf& dst, DevBuf& pcm16, cudaStream_t st) {
-  const int64_t cap = (n + 3) / 4 * 4;
-  if (!dst.reserve((size_t)(cap > 0 ? cap : 4) * 4)) { set_err("device allocation failed (recording)"); return false; }
-  float* wav = static_cast<float*>(dst.p);
-  if (n == 0) return true;
-  if (pcm_format == 1) {
-    if (!pcm16.reserve((size_t)n * 2)) { set_err("device allocation failed (pcm)"); return false; }
-    cudaMemcpyAsync(pcm16.p, buf, (size_t)n * 2, cudaMemcpyHostToDevice, st);
-    pcm16_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(static_cast<const int16_t*>(pcm16.p), wav, n);
-  } else {
-    cudaMemcpyAsync(wav, buf, (size_t)n * 4, cudaMemcpyHostToDevice, st);
-  }
-  return true;
+// one recording (host) -> fp32 on the device in `dst`, its row rounded up to 4 samples
+bool upload_one(const void* buf, int64_t n, int32_t pcm_format, DevBuf& dst, DevBuf& pcm16, cudaStream_t st) {
+  return upload(&buf, &n, 1, (n + 3) / 4 * 4, pcm_format, dst, pcm16, st);
 }
 
 // four consecutive output columns per thread: scalar reads (a segment starts anywhere), one 16-byte store
@@ -748,19 +716,9 @@ extern "C" int fa_gather_segments(const float* rec, int64_t n_rec, const int64_t
 
 extern "C" void* fa_vad_init(const char* model_file, int32_t device) {
   g_err.clear();
-  if (!model_file) { set_err("model_file is NULL"); return nullptr; }
-  if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); set_err("no such CUDA device (this library has no CPU path)"); return nullptr; }
-  Vad* v = new Vad();
-  v->device = device;
-  if (cudaStreamCreateWithFlags(&v->st, cudaStreamNonBlocking) != cudaSuccess) { set_err("cudaStreamCreate failed"); delete v; return nullptr; }
-  bool ok = false;
-  try {                                   // no C++ exception may cross the C ABI
-    ok = load_file(v->t, model_file) && build_vad(*v);
-  } catch (const std::exception& e) {
-    set_err(std::string("model file rejected: ") + e.what());
-  }
-  if (!ok) { delete v; return nullptr; }
-  return v;
+  std::unique_ptr<Vad> v(new Vad());
+  if (!no_throw("model file rejected: ", [&] { return v->file.open(model_file, device) && build_vad(*v); })) return nullptr;
+  return v.release();
 }
 
 extern "C" void fa_vad_uninit(void* vad) { delete static_cast<Vad*>(vad); }
@@ -768,20 +726,15 @@ extern "C" void fa_vad_uninit(void* vad) { delete static_cast<Vad*>(vad); }
 extern "C" void* fa_vad_infer(void* vad, const void* buf, int64_t n_samples, int32_t pcm_format, const FaVadRunOptions* opts) {
   g_err.clear();
   Vad* v = static_cast<Vad*>(vad);
-  if (!v || (!buf && n_samples > 0) || n_samples < 0 || n_samples > 0x7fffffffLL || (pcm_format != 0 && pcm_format != 1)) {
-    set_err("bad argument"); return nullptr;
-  }
-  cudaSetDevice(v->device);
-  VadResult* r = new VadResult();
-  try {
-    if (!upload(buf, n_samples, pcm_format, v->wav, v->pcm16, v->st) ||
-        !vad_run(*v, static_cast<const float*>(v->wav.p), n_samples, v->st, opts ? *opts : default_vad_run(), *r)) {
-      delete r; return nullptr;
-    }
-  } catch (const std::exception& e) {
-    set_err(std::string("fa_vad_infer: ") + e.what()); delete r; return nullptr;
-  }
-  return r;
+  if (!v || (!buf && n_samples > 0) || n_samples < 0 || n_samples > 0x7fffffffLL || (pcm_format != 0 && pcm_format != 1)) return fail("bad argument");
+  cudaSetDevice(v->file.device);
+  std::unique_ptr<VadResult> r(new VadResult());
+  if (!no_throw("fa_vad_infer: ", [&] {
+        return upload_one(buf, n_samples, pcm_format, v->wav, v->pcm16, v->file.st) &&
+               vad_run(*v, static_cast<const float*>(v->wav.p), n_samples, v->file.st, opts ? *opts : default_vad_run(), *r);
+      }))
+    return nullptr;
+  return r.release();
 }
 
 extern "C" const int32_t* fa_vad_result_segments(const void* result, int64_t* n_segments) {
@@ -805,10 +758,11 @@ namespace {
 // one recording of fa_offline_infer_vad: inference_with_vad (auto_model.py:852-1035, funasr_b200/long_audio.py:LongAudioPipeline.generate)
 bool long_audio_one(Model& m, Vad& v, int rec_index, const void* buf, int64_t n, int32_t pcm_format, const float* hw_embed, int32_t n_hotwords,
                     const FaLongAudioOptions& o, std::vector<int32_t>& ids, std::vector<int32_t>& segs_out, std::vector<int32_t>& stamps) {
-  if (!upload(buf, n, pcm_format, m.rec, m.pcm16, m.st)) return false;
+  cudaStream_t st = m.file.st;
+  if (!upload_one(buf, n, pcm_format, m.rec, m.pcm16, st)) return false;
   const float* rec = static_cast<const float*>(m.rec.p);
   VadResult vr;
-  if (!vad_run(v, rec, n, m.st, o.vad, vr)) return false;
+  if (!vad_run(v, rec, n, st, o.vad, vr)) return false;
   std::vector<int32_t> segs = vr.seg;
   if (o.merge_vad) {
     segs.resize(2 * vr.seg.size() + 2);
@@ -843,12 +797,12 @@ bool long_audio_one(Model& m, Vad& v, int rec_index, const void* buf, int64_t n,
     if (!(m.gmeta.reserve((size_t)B * 12) && m.wav.reserve((size_t)B * stride * 4))) { set_err("device allocation failed (segments)"); return false; }
     int64_t* starts_d = static_cast<int64_t*>(m.gmeta.p);
     int32_t* lens_d = reinterpret_cast<int32_t*>(starts_d + B);
-    cudaMemcpyAsync(starts_d, starts.data(), (size_t)B * 8, cudaMemcpyHostToDevice, m.st);
-    cudaMemcpyAsync(lens_d, lens.data(), (size_t)B * 4, cudaMemcpyHostToDevice, m.st);
+    cudaMemcpyAsync(starts_d, starts.data(), (size_t)B * 8, cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(lens_d, lens.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st);
     float* wav = static_cast<float*>(m.wav.p);
-    const int rc = fa_gather_segments(rec, n, starts_d, lens_d, B, stride, wav, m.st);
+    const int rc = fa_gather_segments(rec, n, starts_d, lens_d, B, stride, wav, st);
     if (rc != FA_OK) { set_err(std::string("fa_gather_segments: ") + fa_status_string(rc)); return false; }
-    Result* pr = decode_batch(m, wav, stride, lens, hw_embed, n_hotwords);
+    const std::unique_ptr<Result> pr = decode_batch(m, wav, stride, lens, hw_embed, n_hotwords);
     if (!pr) return false;
     int tmax = 0;
     for (int32_t t : pr->token_num) tmax = t > tmax ? t : tmax;
@@ -858,7 +812,6 @@ bool long_audio_one(Model& m, Vad& v, int rec_index, const void* buf, int64_t n,
         seg_ids[order[beg + j]].swap(pr->ids[j]);
         if (pr->ts) seg_stamps[order[beg + j]].swap(pr->stamps[j]);
       }
-    delete pr;
   }
   for (int64_t s = 0; s < ns; ++s) {
     const int32_t k = emptied ? 0 : (int32_t)seg_ids[s].size();
@@ -877,35 +830,34 @@ extern "C" void* fa_offline_infer_vad(void* asr, void* vad, const void* const* b
   g_err.clear();
   Model* mp = static_cast<Model*>(asr);
   Vad* vp = static_cast<Vad*>(vad);
-  if (!mp || !vp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) { set_err("bad argument"); return nullptr; }
-  if (mp->device != vp->device) { set_err("the recogniser and the VAD live on different devices"); return nullptr; }
-  if (mp->contextual && (!hw_embed || n_hotwords < 1)) { set_err("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)"); return nullptr; }
+  if (!mp || !vp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) return fail("bad argument");
+  if (mp->file.device != vp->file.device) return fail("the recogniser and the VAD live on different devices");
+  if (mp->contextual && (!hw_embed || n_hotwords < 1)) return fail("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)");
   FaLongAudioOptions o;
   if (opts) o = *opts;
   else { o.batch_size_s = 300; o.batch_size_threshold_s = 60; o.merge_vad = 0; o.merge_length_s = 15; o.vad = default_vad_run(); }
   for (int i = 0; i < batch; ++i)
-    if ((!bufs[i] && n_samples[i] > 0) || n_samples[i] < 0 || n_samples[i] > 0x7fffffffLL) { set_err("bad recording " + std::to_string(i)); return nullptr; }
-  cudaSetDevice(mp->device);
-  Result* r = new Result();
+    if ((!bufs[i] && n_samples[i] > 0) || n_samples[i] < 0 || n_samples[i] > 0x7fffffffLL) return fail("bad recording " + std::to_string(i));
+  cudaSetDevice(mp->file.device);
+  std::unique_ptr<Result> r(new Result());
   r->ids.resize(batch);
   r->segs.resize(batch);
   r->token_num.assign(batch, 0);
   r->ts = mp->ts;
   r->stamps.resize(batch);
   double seconds = 0.0;
-  try {
-    for (int i = 0; i < batch; ++i) {
-      seconds += (double)n_samples[i] / 16000.0;
-      if (!long_audio_one(*mp, *vp, i, bufs[i], n_samples[i], pcm_format, hw_embed, n_hotwords, o, r->ids[i], r->segs[i], r->stamps[i])) {
-        delete r; return nullptr;
-      }
-      r->token_num[i] = (int32_t)r->ids[i].size();
-    }
-  } catch (const std::exception& e) {
-    set_err(std::string("fa_offline_infer_vad: ") + e.what()); delete r; return nullptr;
-  }
+  if (!no_throw("fa_offline_infer_vad: ", [&] {
+        for (int i = 0; i < batch; ++i) {
+          seconds += (double)n_samples[i] / 16000.0;
+          if (!long_audio_one(*mp, *vp, i, bufs[i], n_samples[i], pcm_format, hw_embed, n_hotwords, o, r->ids[i], r->segs[i], r->stamps[i]))
+            return false;
+          r->token_num[i] = (int32_t)r->ids[i].size();
+        }
+        return true;
+      }))
+    return nullptr;
   r->audio_seconds = (float)seconds;
-  return r;
+  return r.release();
 }
 
 extern "C" const int32_t* fa_offline_result_segments(const void* result, int32_t index, int32_t* n_segments) {

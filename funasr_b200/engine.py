@@ -192,52 +192,30 @@ class _EngineBase:
         shared by BiCifParaformer / SeacoParaformer and the MonotonicAligner."""
         from .pack import timestamp_head_tensors
         head = {k[len(prefix_pred):]: self._dev(v) for k, v in timestamp_head_tensors(self._state, prefix_pred).items()}
-        self.up_times = int(self._state[prefix_pred + "upsample_cnn.weight"].shape[2])   # ConvTranspose1d weight [in, out, k], stride == k
-        # the upsampling as one GEMM over rows viewed as [B, 3T, D]; the BLSTM: input projections of both directions as ONE GEMM
-        # ([W_ih_fwd; W_ih_bwd], b_ih + b_hh), then the persistent weight-stationary recurrence fa_blstm_forward_tc
-        self.up_lin = self._lin("upsample_cnn", weight=head["upsample_cnn.gemm_weight"], bias_tensor=head["upsample_cnn.gemm_bias"])
-        self.lstm_ih = self._lin("blstm.ih", weight=head["blstm.ih_gemm_weight"], bias_tensor=head["blstm.ih_gemm_bias"])
-        self.lstm_hh_f, self.lstm_hh_b = head["blstm.weight_hh_l0"], head["blstm.weight_hh_l0_reverse"]
-        self.out2_w, self.out2_b = head["cif_output2.weight"], head["cif_output2.bias"]
-        self.smooth2, self.noise2, self.ts_threshold = float(smooth_factor2), float(noise_threshold2), float(threshold)
+        self.ts_head = _abi.FaTimestampHead(
+            self._lin("upsample_cnn", weight=head["upsample_cnn.gemm_weight"], bias_tensor=head["upsample_cnn.gemm_bias"]),
+            self._lin("blstm.ih", weight=head["blstm.ih_gemm_weight"], bias_tensor=head["blstm.ih_gemm_bias"]),
+            head["blstm.weight_hh_l0"].data_ptr(), head["blstm.weight_hh_l0_reverse"].data_ptr(),
+            head["cif_output2.weight"].data_ptr(), head["cif_output2.bias"].data_ptr(),
+            int(self._state[prefix_pred + "upsample_cnn.weight"].shape[2]),   # ConvTranspose1d weight [in, out, k], stride == k
+            float(smooth_factor2), float(noise_threshold2), float(threshold))
 
     def upsample_timestamp(self, enc: torch.Tensor, lens: torch.Tensor, token_num: torch.Tensor):
         """CifPredictorV3.get_upsample_timestamp (bicif_paraformer/cif_predictor.py:300-352): enc [B,T,D] (D = 512 or 320), lens [B] i32,
-        token_num [B] i32 (rounded) -> (us_alphas [B,3T], us_peaks [B,3T]).  ConvTranspose1d upsampling = one GEMM of this library,
-        the BLSTM = its input projections as one tensor-core GEMM + this library's persistent weight-stationary recurrence
-        (fa_blstm_forward_tc: warp-level mma.sync on bf16 hi/lo planes, not wgmma — the per-step product is only 64x32xD), the
-        alpha head / rescale / fire scan is fa_cif_upsample_alphas."""
-        if getattr(self, "up_lin", None) is None:
+        token_num [B] i32 (rounded) -> (us_alphas [B,3T], us_peaks [B,3T]), one fa_timestamp_head_forward.  Its workspace is the
+        engine's: it grows once to the head's size, after which the head and the decoder graphs keep the same address."""
+        if getattr(self, "ts_head", None) is None:
             raise _abi.FunasrB200Error("engine was not built with the CifPredictorV3 timestamp head (bicif=True)")
         B, T, D = enc.shape
-        U = self.up_times
-        up = torch.empty((B, T * U, D), dtype=torch.float32, device=self.device)
-        ws = self._workspace(self.lib.fa_linear_workspace_bytes(B * T * U, D, self.mode))     # the larger of the two calls
-        _abi.check(self.lib.fa_linear(enc.data_ptr(), D, B * T, C.byref(self.up_lin), 0, None, 0, None, 0, up.data_ptr(), U * D, self.mode,
-                                      ws.data_ptr(), ws.numel(), self._stream()), "fa_linear(upsample_cnn)")
-        xproj = torch.empty((B * T * U, 8 * D), dtype=torch.float32, device=self.device)
-        _abi.check(self.lib.fa_linear(up.data_ptr(), D, B * T * U, C.byref(self.lstm_ih), 0, None, 0, None, 0, xproj.data_ptr(), 8 * D,
-                                      self.mode, ws.data_ptr(), ws.numel(), self._stream()), "fa_linear(blstm input projections)")
-        feat = torch.empty((B, T * U, 2 * D), dtype=torch.float32, device=self.device)
-        # the recurrence kernel holds at most 256 sequences per launch: larger batches run as consecutive launches (sequences
-        # are independent) — never a library fallback
-        for b0 in range(0, B, 256):
-            bn = min(256, B - b0)
-            xp = xproj.data_ptr() + b0 * T * U * 8 * D * 4
-            fp = feat.data_ptr() + b0 * T * U * 2 * D * 4
-            nb = int(self.lib.fa_blstm_tc_scratch_bytes(bn))
-            if getattr(self, "_lstm_scratch", None) is None or self._lstm_scratch.numel() < nb:
-                self._lstm_scratch = torch.empty(nb, dtype=torch.uint8, device=self.device)
-            _abi.check(self.lib.fa_blstm_forward_tc(xp, self.lstm_hh_f.data_ptr(), self.lstm_hh_b.data_ptr(), bn, T * U, D,
-                                                    fp, self._lstm_scratch.data_ptr(), self._lstm_scratch.numel(),
-                                                    self._stream()), "fa_blstm_forward_tc")
+        U = self.ts_head.up_times
         us_alphas = torch.empty((B, T * U), dtype=torch.float32, device=self.device)
         us_peaks = torch.empty_like(us_alphas)
-        lens_up = (lens.to(torch.int32) * U).contiguous()
+        lens = lens.to(self.device, torch.int32).contiguous()
         tok = token_num.to(self.device, torch.int32).contiguous()
-        _abi.check(self.lib.fa_cif_upsample_alphas(feat.data_ptr(), 2 * D, self.out2_w.data_ptr(), self.out2_b.data_ptr(), lens_up.data_ptr(),
-                                                   tok.data_ptr(), B, T * U, self.smooth2, self.noise2, self.ts_threshold,
-                                                   us_alphas.data_ptr(), us_peaks.data_ptr(), self._stream()), "fa_cif_upsample_alphas")
+        ws = self._workspace(self.lib.fa_timestamp_head_workspace_bytes(B, T, D, U, self.mode))
+        _abi.check(self.lib.fa_timestamp_head_forward(C.byref(self.ts_head), enc.data_ptr(), lens.data_ptr(), tok.data_ptr(), B, T,
+                                                      us_alphas.data_ptr(), us_peaks.data_ptr(), self.mode, ws.data_ptr(), ws.numel(),
+                                                      self._stream()), "fa_timestamp_head_forward")
         return us_alphas, us_peaks
 
 

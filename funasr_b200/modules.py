@@ -682,7 +682,7 @@ class BiCifParaformerB200(ParaformerB200):
         for i, r in enumerate(results):
             ids = out["ids"][i]
             token = tokenizer.ids2tokens(ids) if tokenizer is not None else [str(t) for t in ids]
-            n = int(lens[i]) * eng.up_times
+            n = int(lens[i]) * eng.ts_head.up_times
             _, stamp = ts_prediction_lfr6_standard(ua[i][:n], up[i][:n], list(token), vad_offset=kwargs.get("begin_time", 0),
                                                    want_text=False)                                                                 # model.py:402-407
             if tokenizer is not None:
@@ -796,7 +796,7 @@ class MonotonicAlignerB200(nn.Module):
         results = []
         for i, token_int in enumerate(token_lists):
             token = tokenizer.ids2tokens(token_int) if tokenizer is not None else [str(t) for t in token_int]
-            n = int(elens[i]) * eng.up_times
+            n = int(elens[i]) * eng.ts_head.up_times
             _, stamp = ts_prediction_lfr6_standard(ua[i][:n], up[i][:n], list(token), want_text=False)       # model.py:243-247
             text = tokenizer.tokens2text(token) if tokenizer is not None else " ".join(token)
             try:

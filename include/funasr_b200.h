@@ -325,6 +325,28 @@ int fa_cif_upsample_alphas(const float* feat, int32_t dz, const float* w, const 
                            const int32_t* token_num, int32_t batch, int32_t t_up, float smooth2, float noise2,
                            float threshold, float* us_alphas, float* us_peaks, fa_stream_t stream);
 
+/* CifPredictorV3's upsampled timestamp head (upsample_type "cnn_blstm", bicif_paraformer/cif_predictor.py:121-352) in the layout
+ * funasr_b200/pack.py:timestamp_head_tensors writes; D = d_model (512 or 320), U = up_times. */
+typedef struct {
+  FaLinear upsample;        /* upsample_cnn (ConvTranspose1d, stride == kernel == U) as a GEMM: [U*D, D], bias repeated U times */
+  FaLinear blstm_ih;        /* both BLSTM input projections [W_ih_fwd; W_ih_bwd]: [8D, D], bias b_ih + b_hh */
+  const float* w_hh_fwd;    /* blstm.weight_hh_l0 [4D, D] */
+  const float* w_hh_bwd;    /* blstm.weight_hh_l0_reverse [4D, D] */
+  const float* out2_w;      /* cif_output2.weight [2D] */
+  const float* out2_b;      /* cif_output2.bias [1] */
+  int32_t up_times;         /* U */
+  float smooth2, noise2;    /* smooth_factor2, noise_threshold2 */
+  float threshold;          /* the CIF threshold */
+} FaTimestampHead;
+/* CifPredictorV3.get_upsample_timestamp (:300-352): enc [B, t_max, D], lens[B] encoder lengths, token_num[B] ->
+ * us_alphas / us_peaks [B, U * t_max].  The upsample GEMM, the input-projection GEMM, fa_blstm_forward_tc over at most 256
+ * sequences per launch, lens x U, then fa_cif_upsample_alphas.  D other than 512 / 320 -> FA_ERR_UNSUPPORTED; GEMM shapes other
+ * than the struct's comments say -> FA_ERR_ARG.  The workspace query returns exactly what the forward carves. */
+size_t fa_timestamp_head_workspace_bytes(int32_t batch, int32_t t_max, int32_t d_model, int32_t up_times, int32_t gemm_mode);
+int fa_timestamp_head_forward(const FaTimestampHead* head, const float* enc, const int32_t* lens, const int32_t* token_num,
+                              int32_t batch, int32_t t_max, float* us_alphas, float* us_peaks, int32_t gemm_mode, void* workspace,
+                              size_t ws_bytes, fa_stream_t stream);
+
 /* One-layer bidirectional LSTM recurrence (torch.nn.LSTM(H, H, 1, batch_first=True, bidirectional=True), the `blstm` of
  * CifPredictorV3, bicif_paraformer/cif_predictor.py:187-190) as a persistent weight-stationary kernel: the per-step
  * [B,H] x [H,4H] product on warp-level bf16 MMAs with the 3-product operand split (fp32 accumulate), h exchanged between

@@ -297,7 +297,8 @@ def test_product_never_touches_the_oracle_or_the_reference_tree():
 
 def test_host_side_entry_points_from_plain_c(tmp_path):
     """The two host-only routines of the ABI (no GPU needed) called from a C99 program: the integrate-and-fire trace and the VAD
-    end-point walk give the values the Python specifications give."""
+    end-point walk give the values the Python specifications give.  The timestamp head's workspace query, and the refusals its
+    forward makes before touching a device (NULL head, unsupported D, mismatched GEMM shapes, a short workspace)."""
     src = tmp_path / "host_calls.c"
     src.write_text(r'''
 #include <math.h>
@@ -325,6 +326,22 @@ int main(void) {
   for (int i = 0; i < n && i < 8; ++i) printf(" [%d,%d]", seg[2 * i], seg[2 * i + 1]);
   printf("\n");
   printf("bad %lld\n", (long long)fa_vad_detect_segments(sil, db, F, 48000, NULL, 60000, 0, NULL, 0, NAN, seg, 8));
+  /* the timestamp head's query and its refusals, all decided before any device work */
+  FaTimestampHead h;
+  memset(&h, 0, sizeof h);
+  const float* p = tr;
+  int32_t* ip = seg;
+  float* out = tr;
+  h.w_hh_fwd = h.w_hh_bwd = h.out2_w = h.out2_b = p;
+  h.up_times = 3; h.upsample.in_f = 256; h.upsample.out_f = 768; h.blstm_ih.in_f = 256; h.blstm_ih.out_f = 2048;
+  const int unsupported = fa_timestamp_head_forward(&h, p, ip, ip, 3, 37, out, out, FA_GEMM_F32_SIMT, NULL, 0, NULL);
+  h.upsample.in_f = 512; h.upsample.out_f = 1536; h.blstm_ih.in_f = 320; h.blstm_ih.out_f = 4096;
+  const int bad_shape = fa_timestamp_head_forward(&h, p, ip, ip, 3, 37, out, out, FA_GEMM_F32_SIMT, NULL, 0, NULL);
+  h.blstm_ih.in_f = 512;
+  const size_t need = fa_timestamp_head_workspace_bytes(3, 37, 512, 3, FA_GEMM_F32_SIMT);
+  const int short_ws = fa_timestamp_head_forward(&h, p, ip, ip, 3, 37, out, out, FA_GEMM_F32_SIMT, NULL, need - 1, NULL);
+  printf("ts %zu %d %d %d %d\n", need, fa_timestamp_head_forward(NULL, p, ip, ip, 3, 37, out, out, FA_GEMM_F32_SIMT, NULL, 0, NULL),
+         unsupported, bad_shape, short_ws);
   return 0;
 }
 ''')
@@ -343,3 +360,4 @@ int main(void) {
     want = vad.detect_segments(sil, [0.0] * 300, 400 + 160 * 299, max_end_silence_time=800)
     assert want and lines[1] == "segments %d" % len(want) + "".join(" [%d,%d]" % (s, e) for s, e in want)
     assert lines[2] == "bad -1"
+    assert lines[3] == "ts 8026380 -1 -4 -1 -3"

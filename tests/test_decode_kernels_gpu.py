@@ -490,6 +490,63 @@ def test_upsample_scan_random():
     assert torch.equal(_bits(us_p), _bits(O.cif_wo_hidden_loop(us_a, thr)))
 
 
+def _head_composed(abi, lib, head, mode, enc, lens, tok):
+    """The timestamp head as the handle and the engine each launched it before fa_timestamp_head_forward, from public entries: the
+    upsample fa_linear, the input-projection fa_linear, fa_blstm_forward_tc over at most 256 sequences per launch, lens x U (torch),
+    fa_cif_upsample_alphas."""
+    st = _st()
+    B, T, d = enc.shape
+    U = head.up_times
+    ws = torch.empty(lib.fa_linear_workspace_bytes(B * T * U, d, mode) + 1, dtype=torch.uint8, device=DEV)
+    up = torch.empty(B * T * U, d, device=DEV)
+    xproj = torch.empty(B * T * U, 8 * d, device=DEV)
+    feat = torch.empty(B * T * U, 2 * d, device=DEV)
+    abi.check(lib.fa_linear(enc.data_ptr(), d, B * T, C.byref(head.upsample), 0, None, 0, None, 0, up.data_ptr(), U * d, mode, ws.data_ptr(),
+                            ws.numel(), st), "fa_linear(upsample)")
+    abi.check(lib.fa_linear(up.data_ptr(), d, B * T * U, C.byref(head.blstm_ih), 0, None, 0, None, 0, xproj.data_ptr(), 8 * d, mode,
+                            ws.data_ptr(), ws.numel(), st), "fa_linear(blstm ih)")
+    scratch = torch.empty(lib.fa_blstm_tc_scratch_bytes(min(B, 256)), dtype=torch.uint8, device=DEV)
+    for b0 in range(0, B, 256):
+        bn = min(256, B - b0)
+        abi.check(lib.fa_blstm_forward_tc(xproj[b0 * T * U:].data_ptr(), head.w_hh_fwd, head.w_hh_bwd, bn, T * U, d, feat[b0 * T * U:].data_ptr(),
+                                          scratch.data_ptr(), scratch.numel(), st), "fa_blstm_forward_tc")
+    lens_up = (lens * U).to(torch.int32)
+    us_a, us_p = torch.empty(B, T * U, device=DEV), torch.empty(B, T * U, device=DEV)
+    abi.check(lib.fa_cif_upsample_alphas(feat.data_ptr(), 2 * d, head.out2_w, head.out2_b, lens_up.data_ptr(), tok.data_ptr(), B, T * U, head.smooth2,
+                                         head.noise2, head.threshold, us_a.data_ptr(), us_p.data_ptr(), st), "fa_cif_upsample_alphas")
+    return us_a, us_p
+
+
+@pytest.mark.parametrize("mode", ["fp32", "fp16", "fp16x3", "fp16x6"])
+@pytest.mark.parametrize("kind", ["bicif", "aligner"])
+def test_timestamp_head_entry_is_the_composed_sequence(kind, mode):
+    """fa_timestamp_head_forward (through the engine's upsample_timestamp) gives bit for bit what the composed public entries give,
+    at D 512 (BiCif) and 320 (the aligner), B = 300 so that the recurrence runs as a 256- and a 44-sequence launch; the entry counts
+    exactly one launch more (lens x U, which the composition does in torch)."""
+    from funasr_b200 import synth
+    from funasr_b200.engine import AlignerEngine, ParaformerEngine
+    abi, lib = _lib()
+    if kind == "aligner":
+        eng = AlignerEngine(synth.make_aligner_state_dict(synth.ALIGNER_TINY, 3), synth.ALIGNER_TINY, DEV, gemm_mode=mode)
+    else:
+        eng = ParaformerEngine(synth.make_bicif_state_dict(synth.PARAFORMER_TINY, 3), synth.PARAFORMER_TINY, DEV, gemm_mode=mode, bicif=True)
+    g = torch.Generator(device=DEV).manual_seed(21)
+    B, T, d = 300, 7, eng.cfg.d_model
+    enc = torch.randn(B, T, d, generator=g, device=DEV)
+    lens = torch.randint(1, T + 1, (B,), generator=g, device=DEV, dtype=torch.int32)
+    lens[::5] = T
+    tok = torch.randint(0, 6, (B,), generator=g, device=DEV, dtype=torch.int32)
+    n0 = lib.fa_launch_count()
+    us_a, us_p = eng.upsample_timestamp(enc, lens, tok)
+    n1 = lib.fa_launch_count()
+    ref_a, ref_p = _head_composed(abi, lib, eng.ts_head, eng.mode, enc, lens, tok)
+    n2 = lib.fa_launch_count()
+    torch.cuda.synchronize()
+    assert torch.equal(_bits(us_a), _bits(ref_a)) and torch.equal(_bits(us_p), _bits(ref_p))
+    assert float(us_p.sum()) > 0
+    assert n1 - n0 == n2 - n1 + 1
+
+
 # ============================================================================================== arg-max / log-softmax
 ARGMAX_MODES = ["fp32", "fp16x3", "fp16"]
 VOCABS = [1, 5, 9216, 9217, 25055, 28672, 28673, 61440]

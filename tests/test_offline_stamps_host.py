@@ -128,7 +128,7 @@ def test_bicif_model_file_round_trips_the_head(tmp_path):
         assert np.array_equal(back[k], v.numpy()), k
 
 
-def test_engine_takes_the_head_from_the_packer():
+def test_engine_head_struct_holds_the_packers_tensors():
     """The engine's timestamp head (fp32 mode needs no device for its weights) holds exactly the tensors the model file holds."""
     from funasr_b200.engine import _EngineBase
     st = _bicif_state()
@@ -137,14 +137,16 @@ def test_engine_takes_the_head_from_the_packer():
     e._init_timestamp_head("predictor.", 0.25, 0.01, 1.0)
     kept = {t.data_ptr(): t for t in e._keep}
     head = pack.timestamp_head_tensors(st)
-    assert e.up_times == 3
-    used = {"predictor.upsample_cnn.gemm_weight": e.up_lin.w, "predictor.upsample_cnn.gemm_bias": e.up_lin.b,
-            "predictor.blstm.ih_gemm_weight": e.lstm_ih.w, "predictor.blstm.ih_gemm_bias": e.lstm_ih.b,
-            "predictor.blstm.weight_hh_l0": e.lstm_hh_f.data_ptr(), "predictor.blstm.weight_hh_l0_reverse": e.lstm_hh_b.data_ptr(),
-            "predictor.cif_output2.weight": e.out2_w.data_ptr(), "predictor.cif_output2.bias": e.out2_b.data_ptr()}
+    h = e.ts_head
+    assert h.up_times == 3
+    used = {"predictor.upsample_cnn.gemm_weight": h.upsample.w, "predictor.upsample_cnn.gemm_bias": h.upsample.b,
+            "predictor.blstm.ih_gemm_weight": h.blstm_ih.w, "predictor.blstm.ih_gemm_bias": h.blstm_ih.b,
+            "predictor.blstm.weight_hh_l0": h.w_hh_fwd, "predictor.blstm.weight_hh_l0_reverse": h.w_hh_bwd,
+            "predictor.cif_output2.weight": h.out2_w, "predictor.cif_output2.bias": h.out2_b}
     for k, ptr in used.items():
         assert torch.equal(kept[ptr].reshape(head[k].shape), head[k]), k
-    assert (e.up_lin.out_f, e.up_lin.in_f, e.lstm_ih.out_f, e.lstm_ih.in_f) == (1536, 512, 4096, 512)
+    assert (h.upsample.out_f, h.upsample.in_f, h.blstm_ih.out_f, h.blstm_ih.in_f) == (1536, 512, 4096, 512)
+    assert (h.smooth2, h.noise2, h.threshold) == (0.25, np.float32(0.01), 1.0)
 
 
 def test_plain_paraformer_file_is_unchanged():

@@ -176,6 +176,21 @@ def test_decoder_stack_workspace(kind, mode):
                                                                 eng.mode, p, n, _st()), outs)
 
 
+@pytest.mark.parametrize("mode", MODES)
+@pytest.mark.parametrize("kind", ["bicif", "aligner"])
+def test_timestamp_head_workspace(kind, mode):
+    lib = _lib()
+    eng = _engine(kind, mode)
+    d = 320 if kind == "aligner" else 512
+    enc = _randn(B, T, d, seed=20)
+    lens, tok = _lens(LENS), _lens([9, 4, 7])
+    us_alphas, us_peaks = torch.empty(B, 3 * T, device=DEV), torch.empty(B, 3 * T, device=DEV)
+    need = lib.fa_timestamp_head_workspace_bytes(B, T, d, 3, eng.mode)
+    _check(need, lambda p, n: lib.fa_timestamp_head_forward(C.byref(eng.ts_head), enc.data_ptr(), lens.data_ptr(), tok.data_ptr(), B, T,
+                                                            us_alphas.data_ptr(), us_peaks.data_ptr(), eng.mode, p, n, _st()),
+           [us_alphas, us_peaks])
+
+
 # ------------------------------------------------------------------------------------------- output heads
 @pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("with_b", [False, True])
@@ -248,10 +263,10 @@ def test_attention_tc_workspace(mode):
 
 
 @pytest.mark.parametrize("mode", MODES)
-def test_linear_workspace(mode):
+def test_linear_workspace_on_the_head_projection(mode):
     lib = _lib()
     eng = _engine("bicif", mode)
-    lin = eng.lstm_ih
+    lin = eng.ts_head.blstm_ih
     rows = B * T
     x = _randn(rows, lin.in_f, seed=16)
     y = torch.empty(rows, lin.out_f, device=DEV)

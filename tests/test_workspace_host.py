@@ -54,6 +54,9 @@ CASES = [
     ("fa_blstm_tc_scratch_bytes", "tiny", (3,)),
     ("fa_blstm_tc_scratch_bytes", "aligner", (8,)),
     ("fa_blstm_tc_scratch_bytes", "max", (256,)),
+    ("fa_timestamp_head_workspace_bytes", "tiny", (3, 37, 512, 3, "m")),
+    ("fa_timestamp_head_workspace_bytes", "config2", (64, 500, 512, 3, "m")),
+    ("fa_timestamp_head_workspace_bytes", "aligner", (8, 300, 320, 3, "m")),
 ]
 
 # (query, shape, mode) -> (value before the queries ran the forward's carve, value now)
@@ -151,6 +154,19 @@ VALUES = {
     ("fa_blstm_tc_scratch_bytes", "tiny", None): (524544, 524544),
     ("fa_blstm_tc_scratch_bytes", "aligner", None): (524544, 524544),
     ("fa_blstm_tc_scratch_bytes", "max", None): (2097408, 2097408),
+    # "before": the buffers the handle held for the head (test_timestamp_head_before_is_the_handles_buffers)
+    ("fa_timestamp_head_workspace_bytes", "tiny", "fp32"): (8026380, 8026380),
+    ("fa_timestamp_head_workspace_bytes", "tiny", "fp16"): (8367372, 8367372),
+    ("fa_timestamp_head_workspace_bytes", "tiny", "fp16x3"): (8708364, 8708364),
+    ("fa_timestamp_head_workspace_bytes", "tiny", "fp16x6"): (9049356, 9049356),
+    ("fa_timestamp_head_workspace_bytes", "config2", "fp32"): (2163212800, 2163212800),
+    ("fa_timestamp_head_workspace_bytes", "config2", "fp16"): (2261516800, 2261516800),
+    ("fa_timestamp_head_workspace_bytes", "config2", "fp16x3"): (2359820800, 2359820800),
+    ("fa_timestamp_head_workspace_bytes", "config2", "fp16x6"): (2458124800, 2458124800),
+    ("fa_timestamp_head_workspace_bytes", "aligner", "fp32"): (101900576, 101900576),
+    ("fa_timestamp_head_workspace_bytes", "aligner", "fp16"): (106508576, 106508576),
+    ("fa_timestamp_head_workspace_bytes", "aligner", "fp16x3"): (111116576, 111116576),
+    ("fa_timestamp_head_workspace_bytes", "aligner", "fp16x6"): (115724576, 115724576),
 }
 
 
@@ -203,6 +219,20 @@ def test_encoder_and_predictor_at_config2():
     lib = _abi.load()
     assert lib.fa_sanm_encoder_workspace_bytes(64, 500, _abi.GEMM_F16X3) == 992804864
     assert lib.fa_cif_predictor_workspace_bytes(64, 500, _abi.GEMM_F16X3) == 131728384
+
+
+@pytest.mark.parametrize("mode", list(MODES))
+def test_timestamp_head_before_is_the_handles_buffers(mode):
+    """The pinned "before" of the head's query is what the handle reserved for the head when it sequenced the launches itself:
+    the payloads of the upsampled rows, the input projections, the BLSTM output, lens x 3 and the recurrence's scratch for at most
+    256 sequences, plus the workspace of the larger GEMM (B * 3T rows, K = D)."""
+    lib = _abi.load()
+    for shape, (B, T, D) in {"tiny": (3, 37, 512), "config2": (64, 500, 512), "aligner": (8, 300, 320)}.items():
+        rows = B * 3 * T
+        held = rows * (1 + 8 + 2) * D * 4 + B * 4 + lib.fa_blstm_tc_scratch_bytes(min(B, 256)) + \
+            lib.fa_linear_workspace_bytes(rows, D, MODES[mode])
+        assert VALUES[("fa_timestamp_head_workspace_bytes", shape, mode)][0] == held
+    assert lib.fa_timestamp_head_workspace_bytes(0, 37, 512, 3, MODES[mode]) == 0
 
 
 @pytest.mark.parametrize("mode", list(MODES))

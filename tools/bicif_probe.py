@@ -53,7 +53,7 @@ st = torch.cuda.current_stream().cuda_stream
 nbs = int(eng.lib.fa_blstm_tc_scratch_bytes(B))
 scr = torch.empty(nbs, dtype=torch.uint8, device=dev)
 feat_tc = torch.empty(B, 1500, 1024, device=dev)
-t_tc = timeit(lambda: _abi.check(eng.lib.fa_blstm_forward_tc(xproj.data_ptr(), eng.lstm_hh_f.data_ptr(), eng.lstm_hh_b.data_ptr(), B, 1500, 512,
+t_tc = timeit(lambda: _abi.check(eng.lib.fa_blstm_forward_tc(xproj.data_ptr(), eng.ts_head.w_hh_fwd, eng.ts_head.w_hh_bwd, B, 1500, 512,
                                                             feat_tc.data_ptr(), scr.data_ptr(), nbs, st), "blstm tc"))
 torch.cuda.synchronize()
 print(f"fa_blstm_forward_tc (mma.sync bf16 x3) alone (recurrence, B={B}, T=1500): {t_tc:.2f} ms = {t_tc / 1500 * 1000:.2f} us per step; "
