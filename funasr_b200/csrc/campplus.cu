@@ -420,6 +420,21 @@ static int campplus_forward(const FaCampplus* m, const float* feats, int batch, 
   const bool tc = mode != FA_GEMM_F32_SIMT;
   if (tc && (!m->tdnn.w_planes || !m->dense.w_planes || m->tdnn.in_pad != 1600)) return FA_ERR_ARG;
   if (m->tdnn.in_f != 1600 || m->tdnn.out_f != kCamBn || m->dense.in_f != 1024) return FA_ERR_UNSUPPORTED;
+  // every layer's shape is checked before the first launch: a malformed layer enqueues nothing
+  {
+    const FaCamLayer* L = m->layers;
+    for (int blk = 0; blk < 3; ++blk) {
+      const int cf = s.c_final[blk];
+      for (int l = 0; l < m->n_layers[blk]; ++l, ++L) {
+        if (L->linear1.in_f != cf - 32 * (m->n_layers[blk] - l) || L->linear1.out_f != kCamBn) return FA_ERR_ARG;
+        if (tc && !L->linear1.w_planes) return FA_ERR_ARG;
+      }
+      const FaCamTransit& tr = m->transit[blk];
+      if (tr.linear.in_f != cf || tr.linear.out_f != cf / 2) return FA_ERR_ARG;
+      if (tc && !tr.linear.w_planes) return FA_ERR_ARG;
+    }
+    if (2 * (s.c_final[2] / 2) != m->dense.in_f) return FA_ERR_ARG;
+  }
   Arena a(ws, ws_bytes);
   CamBufs bf;
   cam_carve(a, s, mode, &bf);
@@ -467,20 +482,15 @@ static int campplus_forward(const FaCampplus* m, const float* feats, int batch, 
     float* buf = bf.buf[blk];
     for (int l = 0; l < m->n_layers[blk]; ++l, ++L) {
       const int c_in = cf - 32 * (m->n_layers[blk] - l);
-      if (L->linear1.in_f != c_in || L->linear1.out_f != kCamBn) return FA_ERR_ARG;
-      if (tc && !L->linear1.w_planes) return FA_ERR_ARG;
       FA_RETURN_IF_ERR(bn_relu_linear(buf, cf, s.rows, L->bn1_scale, L->bn1_shift, L->linear1, 1, bf.h, kCamBn, mode, bf, st));
       FA_RETURN_IF_ERR(cam_launch(bf.h, B, s.t_out, m->dilation[blk], L->local_w, L->w1, L->b1, L->w2, L->b2, bf.gates, buf + c_in, cf, st));
     }
     const FaCamTransit& tr = m->transit[blk];
-    if (tr.linear.in_f != cf || tr.linear.out_f != cf / 2) return FA_ERR_ARG;
-    if (tc && !tr.linear.w_planes) return FA_ERR_ARG;
     float* dst = blk < 2 ? bf.buf[blk + 1] : bf.buf[0];
     const int64_t ldd = blk < 2 ? s.c_final[blk + 1] : cf / 2;
     FA_RETURN_IF_ERR(bn_relu_linear(buf, cf, s.rows, tr.scale, tr.shift, tr.linear, 0, dst, ldd, mode, bf, st));
   }
   const int c_out = s.c_final[2] / 2;
-  if (2 * c_out != m->dense.in_f) return FA_ERR_ARG;
   FA_RETURN_IF_ERR(stats_launch(bf.buf[0], B, s.t_out, c_out, m->out_scale, m->out_shift, bf.stats, st));
   return gemm_rows(bf.stats, 2 * c_out, B, m->dense, GemmEpi().to(emb, m->dense.out_f), mode, &bf.scratch, st);
 }

@@ -93,6 +93,15 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
     return FA_ERR_UNSUPPORTED;
   if (gemm_mode != FA_GEMM_F32_SIMT && !((D == 512 && hd == 128) || (D == 320 && hd == 80))) return FA_ERR_UNSUPPORTED;
   const bool tc = gemm_mode != FA_GEMM_F32_SIMT;
+  // every layer's shape is checked before the first launch: a malformed layer enqueues nothing
+  for (int l = 0; l < enc->n_layers; ++l) {
+    const FaEncLayer& L = enc->layers[l];
+    const int in = L.norm1.n;
+    if (L.qkv.in_f != in || L.qkv.out_f != 3 * D || L.w1.in_f != D || L.w2.out_f != D || L.w2.in_f != L.w1.out_f) return FA_ERR_ARG;
+    if (L.w1.out_f > 2048) return FA_ERR_UNSUPPORTED;      // enc_carve sizes the FFN hidden slice for linear_units <= 2048
+    if (l > 0 && in != D) return FA_ERR_UNSUPPORTED;
+    if (tc && (L.w1.out_f != L.w2.in_pad || L.w1.in_pad != D)) return FA_ERR_UNSUPPORTED;
+  }
   const int npl = gemm_planes(gemm_mode);
   Arena a(workspace, ws_bytes);
   const EncBufs b = enc_carve(a, batch, t_max, gemm_mode);
@@ -105,11 +114,8 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
   for (int l = 0; l < enc->n_layers; ++l) {
     const FaEncLayer& L = enc->layers[l];
     const int in = L.norm1.n;
-    if (L.qkv.in_f != in || L.qkv.out_f != 3 * D || L.w1.in_f != D || L.w2.out_f != D || L.w2.in_f != L.w1.out_f) return FA_ERR_ARG;
-    if (L.w1.out_f > 2048) return FA_ERR_UNSUPPORTED;      // enc_carve sizes the FFN hidden slice for linear_units <= 2048
     // x = x*sqrt(D) + PE is folded into the first LayerNorm (encoder.py:409,428)
     // tensor-core path: LayerNorm writes the fp16 planes the QKV GEMM consumes (no fp32 round trip, no split pass)
-    if (l > 0 && in != D) return FA_ERR_UNSUPPORTED;
     const bool first = embed && l == 0;
     // a first layer with in_size == size keeps its residual (encoder.py:120-126): the embedded rows x*sqrt(d) + PE are then needed
     // beside their LayerNorm (CT-Transformer: 256 -> 256; Paraformer / SenseVoice: 560 -> 512, no residual)
@@ -154,7 +160,6 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
       FA_RETURN_IF_ERR(attention_planes(b.att, shape, lens, AttnOut().to(ctx_planes, D, npl), st));
       if (side) FA_CUDA_OK(cudaStreamWaitEvent(st, side->join, 0));          // join: linear_out adds the FSMN memory
       FA_RETURN_IF_ERR(gemm_tc_planes_launch(ctx_planes, M, L.out, GemmEpi().add(mem, D).to(x2, D), gemm_mode, st));   // mem already holds residual + memory
-      if (L.w1.out_f != L.w2.in_pad || L.w1.in_pad != D) return FA_ERR_UNSUPPORTED;
       FA_RETURN_IF_ERR(layernorm_launch(x2, M, L.norm2, nullptr, nullptr, 1.f, t_max, st, u_planes, npl, D));
       FA_RETURN_IF_ERR(gemm_tc_planes_launch(u_planes, M, L.w1, GemmEpi().relu().to(h_planes, L.w1.out_f), gemm_mode, st));
       FA_RETURN_IF_ERR(gemm_tc_planes_launch(h_planes, M, L.w2, GemmEpi().add(x2, D).to(x3, D), gemm_mode, st));
@@ -344,14 +349,19 @@ extern "C" size_t fa_paraformer_decoder_workspace_bytes_hw(int32_t batch, int32_
   return m.bytes();
 }
 
+// The FFN shapes dec_ffn runs, checked by every decoder entry for each layer it will run before its first launch
+static int dec_ffn_check(const FaDecLayer& L, int mode) {
+  if (L.ffn_w1.in_f != 512 || L.ffn_w2.out_f != 512 || L.ffn_w2.in_f != L.ffn_w1.out_f || L.ffn_norm.n != L.ffn_w1.out_f) return FA_ERR_ARG;
+  if (L.ffn_w1.out_f > 2048) return FA_ERR_UNSUPPORTED;    // dec_carve sizes hq / hq_planes for linear_units <= 2048
+  if (mode != FA_GEMM_F32_SIMT && (L.ffn_w1.in_pad != 512 || L.ffn_w2.in_pad != L.ffn_w1.out_f)) return FA_ERR_UNSUPPORTED;
+  return FA_OK;
+}
+
 static int dec_ffn(const FaDecLayer& L, const float* y, int64_t Mq, float* t1, float* hq, float* f, int mode,
                    Arena* scratch, cudaStream_t st, plane_t* t1_planes, plane_t* hq_planes) {
   // f = w_2( LN_2048( relu( w_1( LN1(y) ) ) ) )   decoder.py:97-100, sanm/positionwise_feed_forward.py:33
-  if (L.ffn_w1.in_f != 512 || L.ffn_w2.out_f != 512 || L.ffn_w2.in_f != L.ffn_w1.out_f || L.ffn_norm.n != L.ffn_w1.out_f) return FA_ERR_ARG;
-  if (L.ffn_w1.out_f > 2048) return FA_ERR_UNSUPPORTED;    // dec_carve sizes hq / hq_planes for linear_units <= 2048
   if (mode != FA_GEMM_F32_SIMT) {
     const int npl = gemm_planes(mode);
-    if (L.ffn_w1.in_pad != 512 || L.ffn_w2.in_pad != L.ffn_w1.out_f) return FA_ERR_UNSUPPORTED;
     FA_RETURN_IF_ERR(layernorm_launch(y, Mq, L.norm1, nullptr, nullptr, 1.f, 1, st, t1_planes, npl, 512));
     FA_RETURN_IF_ERR(gemm_tc_planes_launch(t1_planes, Mq, L.ffn_w1, GemmEpi().relu().to(hq, L.ffn_w1.out_f), mode, st));
     FA_RETURN_IF_ERR(layernorm_launch(hq, Mq, L.ffn_norm, nullptr, nullptr, 1.f, 1, st, hq_planes, npl, L.ffn_w1.out_f));
@@ -401,6 +411,10 @@ attn_probs_kernel(const float* __restrict__ q, int64_t ldq, const float* __restr
   for (int t = lane; t < t_k; t += 32) probs[(int64_t)row * t_k + t] = t < klen ? sc[t] / sum : 0.f;
 }
 
+// attn_probs_kernel's dynamic shared memory: one row of t_k scores per warp; above 48 KB it needs the opt-in
+static size_t attn_probs_smem(int t_k) { return (size_t)4 * t_k * sizeof(float); }
+static const size_t kAttnProbsMaxSmem = 96 * 1024;
+
 // One run of a SAN-M decoder stack over a cross-attention memory.  memory [mem_batch * t_mem, 512] with mem_batch = batch, or 1
 // when mem_shared (the SeACo / contextual hotword memory: every utterance attends over the same rows — one k/v projection, one
 // copy).  tgt [batch, n_max, 512] lives in b.ya on entry.
@@ -439,8 +453,7 @@ static int dec_attention_layer(const DecRun& r, const FaDecLayer& L, float* yin,
     FA_RETURN_IF_ERR(gemm_rows(b.t1, D, r.n_max, L.q, GemmEpi().to(b.qd, D), r.mode, r.scratch, st));
     FA_RETURN_IF_ERR(gemm_rows(r.memory, D, r.t_mem, L.kv, GemmEpi().to(b.kv, 2 * D), r.mode, r.scratch, st));
     const int rows = r.heads * r.n_max;
-    const size_t smem = (size_t)4 * r.t_mem * sizeof(float);
-    if (smem > 96 * 1024) return FA_ERR_UNSUPPORTED;
+    const size_t smem = attn_probs_smem(r.t_mem);              // <= kAttnProbsMaxSmem: checked by the entry point
     if (smem > 48 * 1024) FA_CUDA_OK(cudaFuncSetAttribute(attn_probs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attn_probs_kernel<<<(rows + 3) / 4, 128, smem, st>>>(b.qd, D, b.kv, 2 * D, r.heads, r.n_max, r.t_mem, r.mem_lens,
                                                          attn_qscale(shape.head_dim), attn_probs);
@@ -499,6 +512,9 @@ static int decoder_forward_impl(const FaDecoder* dec, const float* enc, const in
   const bool contextual = dec->has_bias != 0;
   const int nh = dec->n_hotwords;
   if (contextual && (!dec->hw_embed || !dec->hw_lens || nh <= 0 || dec->clas_scale != 1.0f)) return FA_ERR_UNSUPPORTED;
+  for (int l = 0; l < dec->n_layers; ++l) FA_RETURN_IF_ERR(dec_ffn_check(dec->layers[l], gemm_mode));   // nothing enqueued on a refusal
+  if (contextual) FA_RETURN_IF_ERR(dec_ffn_check(dec->bias_last, gemm_mode));
+  FA_RETURN_IF_ERR(dec_ffn_check(dec->last, gemm_mode));
   Arena a(workspace, ws_bytes);
   DecBuf b;
   dec_carve(a, b, batch, t_max, n_max, V, gemm_mode, contextual ? nh : 0, false);
@@ -591,6 +607,9 @@ extern "C" int fa_sanm_decoder_stack_forward(const FaDecoder* dec, const float* 
   cudaStream_t st = (cudaStream_t)stream;
   const int D = 512;
   if (dec->after_norm.n != D || dec->heads * 128 != D) return FA_ERR_UNSUPPORTED;
+  for (int l = 0; l < n_run; ++l) FA_RETURN_IF_ERR(dec_ffn_check(dec->layers[l], gemm_mode));   // nothing enqueued on a refusal
+  if (!attn_probs && finish) FA_RETURN_IF_ERR(dec_ffn_check(dec->last, gemm_mode));
+  if (attn_probs && attn_probs_smem(t_mem) > kAttnProbsMaxSmem) return FA_ERR_UNSUPPORTED;
   Arena a(workspace, ws_bytes);
   DecBuf b;
   dec_carve(a, b, batch, t_mem, n_max, 0, gemm_mode, 0, true);

@@ -199,6 +199,40 @@ def test_embeddings_vs_reference(mode):
     assert rel(got, ref) < 1e-3
 
 
+@pytest.mark.parametrize("mode", MODES)
+def test_malformed_last_layer_launches_nothing(mode):
+    """A malformed last dense layer or last transit is refused (-1) before the first launch: fa_launch_count() is unchanged."""
+    from funasr_b200 import _abi
+    eng = _engine(mode)
+    lib = eng.lib
+    n = sum(eng.model.n_layers)
+    B, T = 2, 148
+    feats = torch.randn(B, T, 80, device=DEV)
+    emb = torch.empty(B, eng.model.dense.out_f, device=DEV)
+
+    def run(m):
+        ws = torch.empty(int(lib.fa_campplus_workspace_bytes(C.byref(m), B, T, eng.mode)), dtype=torch.uint8, device=DEV)
+        torch.cuda.synchronize()
+        n0 = lib.fa_launch_count()
+        rc = lib.fa_campplus_forward(C.byref(m), feats.data_ptr(), B, T, emb.data_ptr(), eng.mode, ws.data_ptr(), ws.numel(), _st())
+        torch.cuda.synchronize()
+        return rc, int(lib.fa_launch_count() - n0)
+
+    rc, launched = run(eng.model)
+    assert rc == 0 and launched > 0
+    for fault in ("layer", "transit"):
+        layers = (_abi.FaCamLayer * n)()
+        for i in range(n):
+            layers[i] = _abi.FaCamLayer.from_buffer_copy(eng.layers[i])
+        m = _abi.FaCampplus.from_buffer_copy(eng.model)
+        m.layers = layers
+        if fault == "layer":
+            layers[n - 1].linear1.in_f += 32
+        else:
+            m.transit[2].linear.in_f += 1
+        assert run(m) == (-1, 0)
+
+
 def test_inference_contract_ragged():
     """CAMPPlusB200.inference: a list of ragged waveforms -> [{"spk_embedding": [B, 192]}], features zero-padded to the longest input
     (pad_list) and every padded frame taking part, batch_data_time in seconds."""
