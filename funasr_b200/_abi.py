@@ -111,6 +111,9 @@ class FaCampplus(C.Structure):
 
 _vp, _i32, _i64, _sz, _f = C.c_void_p, C.c_int32, C.c_int64, C.c_size_t, C.c_float
 
+# fa_punc_score_fn: (ctx, ids, lens, batch, t_max, punc_out) -> 0 on success
+PUNC_SCORE_FN = C.CFUNCTYPE(_i32, _vp, c_i32p, c_i32p, _i32, _i32, c_i32p)
+
 # name -> (restype, argtypes); every symbol include/funasr_b200.h declares
 SIGNATURES = {
     "fa_version": (C.c_char_p, []),
@@ -205,7 +208,18 @@ SIGNATURES = {
     "fa_gather_segments": (C.c_int, [_vp, _i64, _vp, _vp, _i32, _i64, _vp, _vp]),
     "fa_pack_segments": (_i64, [_vp, _i64, _i32, _i32, _vp, _vp]),
     "fa_merge_vad": (_i64, [_vp, _i64, _i32, _i32, _vp]),
+    # handle-style CT-Transformer punctuation (offline.cu; the text walk: punc_text.cpp)
+    "fa_punc_init": (_vp, [C.c_char_p, _i32]),
+    "fa_punc_infer": (_vp, [_vp, C.POINTER(C.c_char_p), _i32]),
+    "fa_punc_result_text": (C.c_char_p, [_vp, _i32]),
+    "fa_punc_result_ids": (C.POINTER(_i32), [_vp, _i32, C.POINTER(_i32)]),
+    "fa_punc_result_steps": (_i64, [_vp]),
+    "fa_punc_free_result": (None, [_vp]),
+    "fa_punc_uninit": (None, [_vp]),
+    "fa_punc_walk_host": (_vp, [C.POINTER(C.c_char_p), _i32, C.POINTER(C.c_char_p), _i32, C.POINTER(C.c_char_p), _i32, _i32, _i32, _i64,
+                                PUNC_SCORE_FN, _vp]),
 }
+
 
 _lib = None
 

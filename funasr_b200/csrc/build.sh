@@ -10,7 +10,7 @@ if [ "$(cat ../_build/flags 2>/dev/null)" != "$FLAGS" ]; then rm -f ../_build/*.
 objs=""
 pids=""
 for f in fbank layernorm gemm_f32 gemm_tc attention_tc attention_f32 fsmn cif decode_ops model offline lstm resample vad campplus; do
-  if [ ! -f ../_build/$f.o ] || [ $f.cu -nt ../_build/$f.o ] || [ common.cuh -nt ../_build/$f.o ] || [ kernels.h -nt ../_build/$f.o ] || [ tc_common.cuh -nt ../_build/$f.o ] || [ ../../include/funasr_b200.h -nt ../_build/$f.o ]; then
+  if [ ! -f ../_build/$f.o ] || [ $f.cu -nt ../_build/$f.o ] || [ common.cuh -nt ../_build/$f.o ] || [ kernels.h -nt ../_build/$f.o ] || [ tc_common.cuh -nt ../_build/$f.o ] || [ ../../include/funasr_b200.h -nt ../_build/$f.o ] || [ punc_text.h -nt ../_build/$f.o ]; then
     ( $NVCC $FLAGS -c $f.cu -o ../_build/$f.o 2> ../_build/$f.ptxas.log || { cat ../_build/$f.ptxas.log; rm -f ../_build/$f.o; exit 1; } ) &
     pids="$pids $!"
   fi
@@ -33,6 +33,12 @@ if [ ! -f ../_build/host_ops.o ] || [ host_ops.cpp -nt ../_build/host_ops.o ] ||
   pids="$pids $!"
 fi
 objs="$objs ../_build/host_ops.o"
+# host-only C++: the text side of CT-Transformer punctuation (fa_punc_walk_host / fa_punc_infer's walk)
+if [ ! -f ../_build/punc_text.o ] || [ punc_text.cpp -nt ../_build/punc_text.o ] || [ punc_text.h -nt ../_build/punc_text.o ]; then
+  ( g++ -O2 -std=c++17 -fPIC -c punc_text.cpp -o ../_build/punc_text.o 2> ../_build/punc_text.log || { cat ../_build/punc_text.log; rm -f ../_build/punc_text.o; exit 1; } ) &
+  pids="$pids $!"
+fi
+objs="$objs ../_build/punc_text.o"
 for p in $pids; do wait $p || exit 1; done
 $NVCC -gencode arch=compute_90a,code=sm_90a -shared -o ../libfunasr_b200.so $objs -lcudart
 echo "built $(cd ..; pwd)/libfunasr_b200.so"

@@ -10,8 +10,11 @@
 //                           a BiCifParaformer file (its upsampled CIF timestamp head) adds per-token [start_ms, end_ms] stamps
 //   fa_vad_init / fa_vad_infer       FSMN-VAD model file -> handle; one recording -> [start_ms, end_ms] segments
 //   fa_offline_infer_vad    long recordings: VAD -> segments packed by duration -> each pack gathered on the device and decoded
+//   fa_punc_init / fa_punc_infer     CT-Transformer model file -> handle; many texts -> punctuated texts, every text one window per
+//                           lockstep step (the text walk: punc_text.cpp)
 // The tokenizer (ids -> text) stays with the caller, like every other entry point of this ABI.
 #include "common.cuh"
+#include "punc_text.h"
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -866,3 +869,216 @@ extern "C" const int32_t* fa_offline_result_segments(const void* result, int32_t
   if (n_segments) *n_segments = (int32_t)(r->segs[index].size() / 3);
   return r->segs[index].data();
 }
+
+// ------------------------------------------------------------------------------------------------ CT-Transformer punctuation handle
+namespace {
+
+// __punc_config__ of funasr_b200/pack.py:write_punc_model_file
+enum { kPuncLayers = 0, kPuncDModel, kPuncHeads, kPuncKernel, kPuncSentenceEnd, kPuncSplit, kPuncCfgLen };
+
+struct Punc {
+  Loaded file;
+  fa_punc::Vocab vocab;
+  int layers = 0, d_model = 0, heads = 0, d_in = 0, n_embed = 0;
+  int64_t max_window = 0;                            // 0: no bound (128-wide heads run the tiled attention kernel)
+  std::vector<FaEncLayer> enc_l;
+  FaEncoder enc{};
+  FaLinear out{};
+  const float* embed = nullptr;
+  DevBuf io, x, h, pids, best, ws;                   // grow-only, sized by each step's t_max
+  std::vector<int32_t> host_io;                      // ids [batch, t_max] then lens [batch]: one host-to-device copy per step
+};
+
+// a newline-joined UTF-8 list stored as the bytes of an fp32 tensor
+std::vector<std::string> blob_lines(const Tensor& t) {
+  std::string s(reinterpret_cast<const char*>(t.host.data()), t.host.size() * 4);
+  while (!s.empty() && s.back() == '\0') s.pop_back();
+  std::vector<std::string> out;
+  for (size_t a = 0;;) {
+    const size_t b = s.find('\n', a);
+    out.push_back(s.substr(a, b == std::string::npos ? std::string::npos : b - a));
+    if (b == std::string::npos) break;
+    a = b + 1;
+  }
+  return out;
+}
+
+std::string layer_prefix(int i) { return i == 0 ? "encoder.encoders0.0" : "encoder.encoders." + std::to_string(i - 1); }
+
+// everything the file's index decides (configuration, lists, every tensor and the shapes the kernels take), before any device work
+bool check_punc(const std::map<std::string, Tensor>& t, Punc& p) {
+  auto get = [&](const std::string& k) -> const Tensor* {
+    auto it = t.find(k);
+    if (it == t.end()) { set_err("punctuation model: missing tensor " + k); return nullptr; }
+    return &it->second;
+  };
+  auto shaped = [&](const std::string& k, std::initializer_list<int64_t> dims) -> const Tensor* {
+    const Tensor* x = get(k);
+    if (x && !std::equal(dims.begin(), dims.end(), x->shape.begin(), x->shape.end())) { set_err("punctuation model: bad shape of " + k); return nullptr; }
+    return x;
+  };
+  const Tensor* cfg = get("__punc_config__");
+  const Tensor* pl = get("__punc_list__");
+  const Tensor* tl = cfg && pl ? get("__punc_tokens__") : nullptr;
+  if (!tl) return false;
+  if (cfg->host.size() != kPuncCfgLen) { set_err("punctuation model: bad __punc_config__"); return false; }
+  const float* c = cfg->host.data();
+  p.layers = (int)c[kPuncLayers]; p.d_model = (int)c[kPuncDModel]; p.heads = (int)c[kPuncHeads];
+  const int D = p.d_model, K = (int)c[kPuncKernel];
+  if (p.layers < 1) { set_err("punctuation model: no encoder layer"); return false; }
+  if (K != 11 && K != 21 && K != 31) { set_err("punctuation model: FSMN kernel " + std::to_string(K) + " (the fp32 FSMN kernel takes 11, 21 or 31)"); return false; }
+  if (D > 512 || D < 64 || D % 16) { set_err("punctuation model: d_model " + std::to_string(D) + " (the encoder takes a multiple of 16 up to 512)"); return false; }
+  const int hd = p.heads > 0 && D % p.heads == 0 ? D / p.heads : 0;
+  if (hd < 32 || hd > 128 || hd % 32) {
+    set_err("punctuation model: " + std::to_string(p.heads) + " heads of d_model " + std::to_string(D) + " (the head dim must be a multiple of 32 up to 128)");
+    return false;
+  }
+  std::string err;
+  if (!p.vocab.init(blob_lines(*tl), blob_lines(*pl), (int32_t)c[kPuncSentenceEnd], (int32_t)c[kPuncSplit], err)) { set_err("punctuation model: " + err); return false; }
+  const Tensor* emb = get("embed.weight");
+  if (!emb) return false;
+  if (emb->shape.size() != 2 || emb->shape[1] > 560 || emb->shape[1] % 16 || emb->shape[0] < 1) { set_err("punctuation model: bad shape of embed.weight"); return false; }
+  p.n_embed = (int)emb->shape[0]; p.d_in = (int)emb->shape[1];
+  if (!shaped("encoder.pe_inv_timescales", {p.d_in / 2})) return false;
+  for (int i = 0; i < p.layers; ++i) {
+    const std::string q = layer_prefix(i);
+    const int in = i == 0 ? p.d_in : D;
+    const Tensor* w1 = get(q + ".feed_forward.w_1.weight");
+    if (!w1) return false;
+    const int64_t F = w1->shape.size() == 2 ? w1->shape[0] : 0;
+    if (F < 1 || F > 2048) { set_err("punctuation model: bad shape of " + q + ".feed_forward.w_1.weight (at most 2048 units)"); return false; }
+    if (!(shaped(q + ".norm1.weight", {in}) && shaped(q + ".norm1.bias", {in}) && shaped(q + ".norm2.weight", {D}) && shaped(q + ".norm2.bias", {D}) &&
+          shaped(q + ".self_attn.linear_q_k_v.weight", {3 * D, in}) && shaped(q + ".self_attn.linear_q_k_v.bias", {3 * D}) &&
+          shaped(q + ".self_attn.linear_out.weight", {D, D}) && shaped(q + ".self_attn.linear_out.bias", {D}) &&
+          shaped(q + ".self_attn.fsmn_block.weight", {D, 1, K}) && shaped(q + ".feed_forward.w_1.weight", {F, D}) &&
+          shaped(q + ".feed_forward.w_1.bias", {F}) && shaped(q + ".feed_forward.w_2.weight", {D, F}) && shaped(q + ".feed_forward.w_2.bias", {D})))
+      return false;
+  }
+  if (t.count("encoder.encoders." + std::to_string(p.layers - 1) + ".norm1.weight")) { set_err("punctuation model: more encoder layers than __punc_config__ says"); return false; }
+  const int64_t n_punc = (int64_t)p.vocab.punc.size();
+  if (!(shaped("encoder.after_norm.weight", {D}) && shaped("encoder.after_norm.bias", {D}) && shaped("decoder.weight", {n_punc, D}) &&
+        shaped("decoder.bias", {n_punc})))
+    return false;
+  p.max_window = hd == 128 ? 0 : 160 * 1024 / 16;     // fa_attention_f32_ex's warp-per-query kernel: 4 * tk floats of shared memory
+  return true;
+}
+
+bool build_punc(Punc& p) {
+  Builder b{p.file};                                 // the fp32 path whatever the recogniser's gemm-mode (PuncEngine)
+  b.ln_eps = 1e-12f;                                 // SANMEncoder's LayerNorm
+  p.enc_l.resize(p.layers);
+  for (int i = 0; i < p.layers; ++i) {
+    const std::string q = layer_prefix(i);
+    FaEncLayer& L = p.enc_l[i];
+    L.norm1 = b.norm(q + ".norm1"); L.norm2 = b.norm(q + ".norm2");
+    L.qkv = b.lin(q + ".self_attn.linear_q_k_v"); L.out = b.lin(q + ".self_attn.linear_out");
+    L.fsmn_w = b.ptr(q + ".self_attn.fsmn_block.weight");
+    L.w1 = b.lin(q + ".feed_forward.w_1"); L.w2 = b.lin(q + ".feed_forward.w_2");
+  }
+  p.enc.layers = p.enc_l.data(); p.enc.n_layers = p.layers; p.enc.heads = p.heads;
+  p.enc.fsmn_k = (int)p.file.t["encoder.encoders0.0.self_attn.fsmn_block.weight"].shape[2];
+  p.enc.after_norm = b.norm("encoder.after_norm"); p.enc.pe_inv_timescales = b.ptr("encoder.pe_inv_timescales");
+  p.out = b.lin("decoder");
+  p.embed = b.ptr("embed.weight");
+  if (!b.ok) return false;
+  return cudaStreamSynchronize(p.file.st) == cudaSuccess;
+}
+
+// one lockstep step on the GPU: punc_forward (model.py:112-125) + arg-max over a padded batch of windows
+bool punc_step(Punc& p, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, int32_t* punc_out, std::string& err) {
+  cudaStream_t st = p.file.st;
+  const int64_t M = (int64_t)B * T;
+  const int n_punc = p.out.out_f;
+  const size_t ws = std::max(fa_sanm_encoder_workspace_bytes(B, T, FA_GEMM_F32_SIMT), fa_linear_argmax_workspace_bytes(M, n_punc, FA_GEMM_F32_SIMT));
+  if (!(p.io.reserve((size_t)(M + B) * 4) && p.x.reserve((size_t)M * p.d_in * 4) && p.h.reserve((size_t)M * p.d_model * 4) &&
+        p.pids.reserve((size_t)M * 4) && p.best.reserve((size_t)M * 4) && p.ws.reserve(ws))) {
+    err = "device allocation failed (punctuation)";
+    return false;
+  }
+  p.host_io.assign(ids, ids + M);
+  p.host_io.insert(p.host_io.end(), lens, lens + B);
+  int32_t* ids_d = static_cast<int32_t*>(p.io.p);
+  cudaMemcpyAsync(ids_d, p.host_io.data(), (size_t)(M + B) * 4, cudaMemcpyHostToDevice, st);
+  float* x = static_cast<float*>(p.x.p);
+  float* h = static_cast<float*>(p.h.p);
+  int rc = fa_embedding(ids_d, p.embed, p.d_in, p.n_embed, M, x, st);
+  if (rc == FA_OK) rc = fa_sanm_encoder_forward(&p.enc, x, ids_d + M, B, T, h, FA_GEMM_F32_SIMT, p.ws.p, p.ws.cap, st);
+  if (rc == FA_OK)
+    rc = fa_linear_argmax(&p.out, h, nullptr, M, static_cast<int32_t*>(p.pids.p), static_cast<float*>(p.best.p), nullptr, FA_GEMM_F32_SIMT, p.ws.p,
+                          p.ws.cap, st);
+  if (rc != FA_OK) { err = std::string("punctuation forward: ") + fa_status_string(rc); return false; }
+  cudaMemcpyAsync(punc_out, p.pids.p, (size_t)M * 4, cudaMemcpyDeviceToHost, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess) { err = std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError()); return false; }
+  return true;
+}
+
+}  // namespace
+
+extern "C" void* fa_punc_init(const char* model_file, int32_t device) {
+  g_err.clear();
+  if (!model_file) return fail("model_file is NULL");
+  std::unique_ptr<Punc> p(new Punc());
+  std::map<std::string, Tensor> index;          // refused on the file's index alone, before any device work
+  if (!no_throw("model file rejected: ", [&] { return load_file(index, model_file, false) && check_punc(index, *p); })) return nullptr;
+  if (!no_throw("model file rejected: ", [&] { return p->file.open(model_file, device) && build_punc(*p); })) return nullptr;
+  return p.release();
+}
+
+extern "C" void fa_punc_uninit(void* punc) { delete static_cast<Punc*>(punc); }
+
+extern "C" void* fa_punc_infer(void* punc, const char* const* texts, int32_t n) {
+  g_err.clear();
+  Punc* p = static_cast<Punc*>(punc);
+  if (!p || (!texts && n > 0) || n < 0) return fail("bad argument");
+  for (int32_t i = 0; i < n; ++i)
+    if (!texts[i]) return fail("text " + std::to_string(i) + " is NULL");
+  cudaSetDevice(p->file.device);
+  std::unique_ptr<fa_punc::Result> r(new fa_punc::Result());
+  std::string err;
+  const fa_punc::Scorer score = [p](const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, int32_t* out, std::string& e) {
+    return punc_step(*p, ids, lens, B, T, out, e);
+  };
+  if (!no_throw("fa_punc_infer: ", [&] { return fa_punc::walk(p->vocab, texts, n, p->max_window, score, *r, err) || (set_err(err), false); }))
+    return nullptr;
+  return r.release();
+}
+
+extern "C" void* fa_punc_walk_host(const char* const* texts, int32_t n, const char* const* tokens, int32_t n_tokens, const char* const* punc_list,
+                                   int32_t n_punc, int32_t sentence_end_id, int32_t split_size, int64_t max_window, fa_punc_score_fn score_fn,
+                                   void* ctx) {
+  g_err.clear();
+  if ((!texts && n > 0) || n < 0 || !tokens || n_tokens < 1 || !punc_list || n_punc < 1 || !score_fn) return fail("bad argument");
+  for (int32_t i = 0; i < n; ++i)
+    if (!texts[i]) return fail("text " + std::to_string(i) + " is NULL");
+  std::unique_ptr<fa_punc::Result> r(new fa_punc::Result());
+  std::string err;
+  const bool ok = no_throw("fa_punc_walk_host: ", [&] {
+    for (int32_t i = 0; i < n_tokens; ++i) if (!tokens[i]) { err = "token " + std::to_string(i) + " is NULL"; set_err(err); return false; }
+    for (int32_t i = 0; i < n_punc; ++i) if (!punc_list[i]) { err = "punctuation " + std::to_string(i) + " is NULL"; set_err(err); return false; }
+    std::vector<std::string> tok(tokens, tokens + n_tokens), pl(punc_list, punc_list + n_punc);
+    fa_punc::Vocab v;
+    const fa_punc::Scorer score = [&](const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, int32_t* out, std::string& e) {
+      const int32_t rc = score_fn(ctx, ids, lens, B, T, out);
+      if (rc != 0) e = "scorer failed (" + std::to_string(rc) + ")";
+      return rc == 0;
+    };
+    return (v.init(tok, pl, sentence_end_id, split_size, err) && fa_punc::walk(v, texts, n, max_window, score, *r, err)) || (set_err(err), false);
+  });
+  return ok ? r.release() : nullptr;
+}
+
+extern "C" const char* fa_punc_result_text(const void* result, int32_t index) {
+  const fa_punc::Result* r = static_cast<const fa_punc::Result*>(result);
+  return r && index >= 0 && index < (int32_t)r->text.size() ? r->text[index].c_str() : nullptr;
+}
+
+extern "C" const int32_t* fa_punc_result_ids(const void* result, int32_t index, int32_t* n) {
+  const fa_punc::Result* r = static_cast<const fa_punc::Result*>(result);
+  if (!r || index < 0 || index >= (int32_t)r->ids.size() || r->ids[index].empty()) { if (n) *n = 0; return nullptr; }
+  if (n) *n = (int32_t)r->ids[index].size();
+  return r->ids[index].data();
+}
+
+extern "C" int64_t fa_punc_result_steps(const void* result) { return result ? static_cast<const fa_punc::Result*>(result)->steps : 0; }
+
+extern "C" void fa_punc_free_result(void* result) { delete static_cast<fa_punc::Result*>(result); }

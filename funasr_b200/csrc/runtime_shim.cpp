@@ -9,8 +9,12 @@
 // "vad-dir"; funasrruntime.cpp:297-310), one pair per stamp of fa_offline_result_stamps.  The values are the library's one timestamp
 // definition, the one the reference's Python BiCifParaformer produces (timestamp_tools.py:ts_prediction_lfr6_standard): the shim does
 // not restate the runtime's own TimestampOnnx (util.cpp:838-965), which cuts tokens at 30 frames instead of 12, re-integrates in fp32
-// with a tail fix-up and re-parses seconds strings to ms.  FunASRGetStampSents stays empty: it pairs text characters with stamps
-// through Vector2StringV2 / TimestampSentence, which the token join below does not restate either.
+// with a tail fix-up and re-parses seconds strings to ms.  With "punc-dir" FunASRGetStampSents is the runtime's TimestampSentence over
+// the punctuated text and those stamps; without it, it stays empty.
+//
+// Punctuation: with model_path["punc-dir"] FunOfflineInfer / FunOfflineInferBuffer punctuate each result text after the join, with or
+// without "vad-dir" (funasrruntime.cpp:311-314), through fa_punc_infer; CTTransformer* are the runtime's offline punctuation entry
+// points over the same handle.
 #include "../../include/funasrruntime_b200.h"
 #include "../../include/funasr_b200.h"
 
@@ -27,6 +31,7 @@ thread_local std::string g_shim_err;
 struct OfflineStream {
   void* h = nullptr;
   void* vad = nullptr;                 // fa_vad_init handle when model_path["vad-dir"] is given
+  void* punc = nullptr;                // fa_punc_init handle when model_path["punc-dir"] is given
   int batch_size_s = 300;
   std::vector<std::string> vocab;
   std::unordered_map<std::string, int> token_id;
@@ -59,6 +64,115 @@ struct ShimResult {
   std::string stamp, stamp_sents;
   float snippet_time = 0.f;
 };
+
+// TimestampSentence of the C++ runtime (runtime/onnxruntime/src/util.cpp:569-637): the punctuated text split as
+// TimestampSplitChiEngCharacters does (EncodeConverter's UTF-8 -> UTF-16 units: 3- and 2-byte sequences only, any other byte one 0
+// unit that adds nothing; CJK, digits and the unit punctuation ranges are one character each, spaces split Latin words), the stamps of
+// "[[b,e],...]" dealt out to the non-punctuation characters, one JSON object per punctuation mark (the bytewise TimestampIsPunctuation)
+// and one for a tail without it.  tests/stampsent_ref.py restates the same function in Python, pinned to the compiled runtime.
+bool unit_punc(uint32_t u) {
+  if (u == 0x26 || u == 0x27 || u == 0x2D) return false;
+  return (u >= 0x21 && u <= 0x2F) || (u >= 0x3A && u <= 0x40) || (u >= 0x5B && u <= 0x60) || (u >= 0x7B && u <= 0x7E) ||
+         (u >= 0x2000 && u <= 0x206F) || (u >= 0x3000 && u <= 0x303F);
+}
+
+std::string unit_utf8(uint32_t u) {
+  std::string s;
+  if (u < 0x80) s += (char)u;
+  else if (u < 0x800) { s += (char)(0xC0 | (u >> 6)); s += (char)(0x80 | (u & 0x3F)); }
+  else { s += (char)(0xE0 | (u >> 12)); s += (char)(0x80 | ((u >> 6) & 0x3F)); s += (char)(0x80 | (u & 0x3F)); }
+  return s;
+}
+
+std::vector<std::string> split_chi_eng(const std::string& text) {
+  std::vector<std::string> chars;
+  std::string eng;
+  const unsigned char* b = reinterpret_cast<const unsigned char*>(text.data());
+  const size_t n = text.size();
+  auto flush = [&] { if (!eng.empty()) { chars.push_back(eng); eng.clear(); } };
+  for (size_t i = 0; i < n;) {
+    uint32_t u = 0;
+    size_t step = 1;
+    if ((b[i] & 0xF0) == 0xE0 && n - i >= 3) {
+      if ((b[i + 1] & 0xC0) == 0x80 && (b[i + 2] & 0xC0) == 0x80) {
+        u = ((b[i] & 0x0Fu) << 12) | ((b[i + 1] & 0x3Fu) << 6) | (b[i + 2] & 0x3Fu);
+        if (u >= 0x800) step = 3; else u = 0;
+      }
+    } else if ((b[i] & 0xE0) == 0xC0 && n - i >= 2) {
+      if ((b[i + 1] & 0xC0) == 0x80) {
+        u = ((b[i] & 0x1Fu) << 6) | (b[i + 1] & 0x3Fu);
+        if (u >= 0x80) step = 2; else u = 0;
+      }
+    } else if (b[i] < 0x80) {
+      u = b[i];
+    }
+    i += step;
+    if ((u >= 0x4E00 && u <= 0x9FFF) || (u >= 0x3400 && u <= 0x4DFF) || (u >= 0x30 && u <= 0x39) || unit_punc(u)) {
+      flush();
+      chars.push_back(unit_utf8(u));
+    } else if (u == 0x20) {
+      flush();
+    } else if (u != 0) {
+      eng += unit_utf8(u);
+    }
+  }
+  flush();
+  return chars;
+}
+
+bool is_punctuation(const std::string& s) {
+  static const std::string punc = "，。？、,?";
+  for (char c : s) if (punc.find(c) == std::string::npos) return false;
+  return true;
+}
+
+std::string render_pairs(const std::vector<std::pair<int, int>>& v) {
+  std::string s = "[";
+  for (size_t i = 0; i < v.size(); ++i) s += (i ? ",[" : "[") + std::to_string(v[i].first) + "," + std::to_string(v[i].second) + "]";
+  return s + "]";
+}
+
+std::string timestamp_sentence(const std::string& text, const void* r, int32_t index) {
+  int32_t n_ts = 0;
+  const int32_t* p = fa_offline_result_stamps(r, index, &n_ts);   // the pairs FunASRGetStamp renders, without the round trip
+  const std::vector<std::string> chars = split_chi_eng(text);
+  int idx_ts = 0, start = -1, end = -1;
+  std::string text_seg, out;
+  std::vector<std::pair<int, int>> seg;
+  for (size_t i = 0; i < chars.size(); ++i) {
+    if (is_punctuation(chars[i])) {
+      if (!seg.empty()) { start = seg.front().first; end = seg.back().second; }
+      out += "{\"text_seg\":\"" + text_seg + "\",\"punc\":\"" + chars[i] + "\",\"start\":" + std::to_string(start) + ",\"end\":" +
+             std::to_string(end) + ",\"ts_list\":" + render_pairs(seg) + "}";
+      if (i != chars.size() - 1) out += ",";
+      text_seg.clear(); start = 0; end = 0; seg.clear();
+    } else if (idx_ts < n_ts) {
+      text_seg = text_seg.empty() ? chars[i] : text_seg + " " + chars[i];
+      seg.emplace_back(p[2 * idx_ts], p[2 * idx_ts + 1]);
+      ++idx_ts;
+    }
+  }
+  if (!seg.empty())
+    out += "{\"text_seg\":\"" + text_seg + "\",\"punc\":\"\",\"start\":" + std::to_string(seg.front().first) + ",\"end\":" +
+           std::to_string(seg.back().second) + ",\"ts_list\":" + render_pairs(seg) + "}";
+  return "[" + out + "]";
+}
+
+struct PuncShimResult {
+  std::string msg;
+};
+
+// every text of `msgs` replaced by its punctuated form, in one fa_punc_infer call
+bool punctuate(void* punc, std::vector<std::string>& msgs) {
+  if (msgs.empty()) return true;
+  std::vector<const char*> texts;
+  for (const std::string& m : msgs) texts.push_back(m.c_str());
+  void* r = fa_punc_infer(punc, texts.data(), (int32_t)texts.size());
+  if (!r) { g_shim_err = fa_offline_last_error(); return false; }
+  for (size_t i = 0; i < msgs.size(); ++i) msgs[i] = fa_punc_result_text(r, (int32_t)i);
+  fa_punc_free_result(r);
+  return true;
+}
 
 // "[[b,e],[b,e],...]" of entry `index` of a handle result; "" without stamps, as the runtime leaves it
 std::string render_stamps(const void* r, int32_t index) {
@@ -173,6 +287,8 @@ FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, int 
     out->msgs.push_back(text);
     out->stamp = render_stamps(r, 0);
     out->snippet_time = fa_offline_result_audio_seconds(r);
+    if (s->punc && !punctuate(s->punc, out->msgs)) { fa_offline_free_result(r); delete out; return nullptr; }
+    if (s->punc && !out->stamp.empty()) out->stamp_sents = timestamp_sentence(out->msgs[0], r, 0);   // funasrruntime.cpp:327-329
     fa_offline_free_result(r);
     return out;
   }
@@ -187,6 +303,8 @@ FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, int 
     if (i == 0) out->stamp = render_stamps(r, 0);
   }
   out->snippet_time = fa_offline_result_audio_seconds(r);
+  if (s->punc && !punctuate(s->punc, out->msgs)) { fa_offline_free_result(r); delete out; return nullptr; }
+  if (s->punc && !out->stamp.empty() && !out->msgs.empty()) out->stamp_sents = timestamp_sentence(out->msgs[0], r, 0);
   fa_offline_free_result(r);
   return out;
 }
@@ -222,6 +340,11 @@ FUNASR_HANDLE FunOfflineInit(std::map<std::string, std::string>& model_path, int
     s->vad = fa_vad_init((vd->second + "/vad.fab2").c_str(), device);
     if (!s->vad) { g_shim_err = fa_offline_last_error(); fa_offline_uninit(s->h); delete s; return nullptr; }
   }
+  auto pd = model_path.find("punc-dir");
+  if (pd != model_path.end()) {
+    s->punc = fa_punc_init((pd->second + "/punc.fab2").c_str(), device);
+    if (!s->punc) { g_shim_err = fa_offline_last_error(); fa_vad_uninit(s->vad); fa_offline_uninit(s->h); delete s; return nullptr; }
+  }
   std::ifstream tf(dir + "/tokens.txt");
   std::string line;
   while (tf && std::getline(tf, line)) {
@@ -239,6 +362,7 @@ void FunOfflineUninit(FUNASR_HANDLE handle) {
   if (!s) return;
   fa_offline_uninit(s->h);
   fa_vad_uninit(s->vad);
+  fa_punc_uninit(s->punc);
   delete s;
 }
 
@@ -409,6 +533,33 @@ void FsmnVadUninit(FUNASR_HANDLE handle) {
   delete s;
 }
 const float FsmnVadGetRetSnippetTime(FUNASR_RESULT result) { return result ? static_cast<VadShimResult*>(result)->snippet_time : 0.f; }
+
+FUNASR_HANDLE CTTransformerInit(std::map<std::string, std::string>& model_path, int thread_num, PUNC_TYPE type) {
+  (void)thread_num;
+  g_shim_err.clear();
+  if (type != PUNC_OFFLINE) { g_shim_err = "only offline punctuation is provided: type must be PUNC_OFFLINE"; return nullptr; }
+  auto it = model_path.find("model-dir");
+  if (it == model_path.end()) { g_shim_err = "model_path[\"model-dir\"] is missing"; return nullptr; }
+  void* p = fa_punc_init((it->second + "/punc.fab2").c_str(), parse_device(model_path));
+  if (!p) g_shim_err = fa_offline_last_error();
+  return p;
+}
+
+FUNASR_RESULT CTTransformerInfer(FUNASR_HANDLE handle, const char* sz_sentence, FUNASR_MODE, QM_CALLBACK fn_callback, PUNC_TYPE type, FUNASR_RESULT) {
+  g_shim_err.clear();
+  if (!handle || !sz_sentence) { g_shim_err = "bad argument"; return nullptr; }
+  if (type != PUNC_OFFLINE) { g_shim_err = "only offline punctuation is provided: type must be PUNC_OFFLINE"; return nullptr; }
+  std::vector<std::string> msgs{sz_sentence};
+  if (!punctuate(handle, msgs)) return nullptr;
+  if (fn_callback) fn_callback(1, 1);
+  PuncShimResult* r = new PuncShimResult();
+  r->msg.swap(msgs[0]);
+  return r;
+}
+
+const char* CTTransformerGetResult(FUNASR_RESULT result, int) { return result ? static_cast<PuncShimResult*>(result)->msg.c_str() : nullptr; }
+void CTTransformerFreeResult(FUNASR_RESULT result) { delete static_cast<PuncShimResult*>(result); }
+void CTTransformerUninit(FUNASR_HANDLE handle) { fa_punc_uninit(handle); }
 
 FUNASR_DEC_HANDLE FunASRWfstDecoderInit(FUNASR_HANDLE, int, float, float, float) { return nullptr; }
 void FunASRWfstDecoderUninit(FUNASR_DEC_HANDLE) {}

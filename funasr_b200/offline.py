@@ -3,7 +3,8 @@ FunOfflineInit / FunOfflineInferBuffer / FunASRGetResult (runtime/onnxruntime/in
 Nothing here touches torch on the data path: host PCM buffers in, token ids out.  `OfflineVad` binds the FSMN-VAD handle
 (fa_vad_*) and `OfflineRecognizer.infer_long` the long-audio entry (fa_offline_infer_vad): VAD segments packed by duration and decoded
 batch by batch, the same results as LongAudioPipeline.generate.  A BiCifParaformer model file adds per-token [start_ms, end_ms] stamps
-(`infer_stamped`, and "timestamp" in `infer_long`'s results)."""
+(`infer_stamped`, and "timestamp" in `infer_long`'s results).  `OfflinePunc` binds the CT-Transformer punctuation handle (fa_punc_*),
+and `punc_walk_host` its text walk with any scorer in place of the network."""
 from __future__ import annotations
 
 import ctypes as C
@@ -73,6 +74,91 @@ class OfflineVad:
             self.close()
         except Exception:
             pass
+
+
+def _punc_result(lib, res, n: int) -> List[dict]:
+    out = []
+    cnt = C.c_int32(0)
+    for i in range(n):
+        p = lib.fa_punc_result_ids(res, i, C.byref(cnt))
+        out.append({"text": lib.fa_punc_result_text(res, i).decode("utf-8"), "punc_array": [int(p[k]) for k in range(cnt.value)]})
+    return out
+
+
+def _c_strings(items: Sequence[str]):
+    enc = [s.encode("utf-8") for s in items]
+    return (C.c_char_p * max(len(enc), 1))(*enc), enc
+
+
+class OfflinePunc:
+    """ctypes binding of fa_punc_init / fa_punc_infer: CT-Transformer punctuation from a model file written by
+    pack.write_punc_model_file.  `infer` punctuates many texts in one call, all of them advancing one window per step."""
+
+    def __init__(self, model_file: str, device: int = 0):
+        self.lib = _abi.load()
+        self.handle = self.lib.fa_punc_init(model_file.encode(), device)
+        if not self.handle:
+            raise _abi.FunasrB200Error("fa_punc_init failed: %s" % self.lib.fa_offline_last_error().decode())
+        self.last_steps = 0
+
+    def infer(self, texts: Sequence[str]) -> List[dict]:
+        """texts -> per text {"text": punctuated text, "punc_array": punctuation id per word} (CTTransformer.inference's result;
+        "" and [] for an empty text)."""
+        arr, _keep = _c_strings(texts)
+        res = self.lib.fa_punc_infer(self.handle, arr, len(texts))
+        if not res:
+            raise _abi.FunasrB200Error("fa_punc_infer failed: %s" % self.lib.fa_offline_last_error().decode())
+        try:
+            self.last_steps = int(self.lib.fa_punc_result_steps(res))
+            return _punc_result(self.lib, res, len(texts))
+        finally:
+            self.lib.fa_punc_free_result(res)
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self.lib.fa_punc_uninit(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def punc_walk_host(texts: Sequence[str], token_list: Sequence[str], punc_list: Sequence[str], sentence_end_id: int, score,
+                   split_size: int = 20, max_window: int = 0) -> List[dict]:
+    """fa_punc_walk_host: the punctuation walk of fa_punc_infer with `score` in place of the network.  score(ids [batch, t_max] int32,
+    lens [batch] int32) -> punctuation ids [batch, t_max] (only each row's first lens[b] entries are read)."""
+    lib = _abi.load()
+    err = []
+
+    def cb(_ctx, ids, lens, batch, t_max, out):
+        try:
+            i = np.ctypeslib.as_array(ids, shape=(batch, t_max)).copy()
+            n = np.ctypeslib.as_array(lens, shape=(batch,)).copy()
+            np.ctypeslib.as_array(out, shape=(batch, t_max))[:] = np.asarray(score(i, n), dtype=np.int32)
+            return 0
+        except Exception as e:                                  # an exception must not cross the C frames
+            err.append(e)
+            return 1
+
+    fn = _abi.PUNC_SCORE_FN(cb)
+    ta, _k1 = _c_strings(texts)
+    tok, _k2 = _c_strings(token_list)
+    pl, _k3 = _c_strings(punc_list)
+    res = lib.fa_punc_walk_host(ta, len(texts), tok, len(token_list), pl, len(punc_list), int(sentence_end_id), int(split_size), int(max_window),
+                                fn, None)
+    if err:
+        if res:
+            lib.fa_punc_free_result(res)
+        raise err[0]
+    if not res:
+        raise _abi.FunasrB200Error("fa_punc_walk_host failed: %s" % lib.fa_offline_last_error().decode())
+    try:
+        return _punc_result(lib, res, len(texts))
+    finally:
+        lib.fa_punc_free_result(res)
 
 
 class OfflineRecognizer:

@@ -30,6 +30,13 @@ and
 
 The detector compares posteriors in double precision against speech_noise_thres and fe_prior_thres, so the options travel as float64.
 
+The CT-Transformer punctuation file (csrc/offline.cu: fa_punc_init) holds embed.weight, encoder.encoders0.0.*, encoder.encoders.{i}.*,
+encoder.after_norm.* and decoder.* under the reference's names, the derived encoder.pe_inv_timescales [embed_unit / 2], and
+
+    __punc_config__                    [6] layers, d_model, heads, fsmn kernel, sentence_end_id, split_size (20)
+    __punc_list__ / __punc_tokens__    the UTF-8 bytes of punc_list / token_list, newline-joined, zero-padded to a multiple of 4 and
+                                       stored as the bytes of an fp32 tensor (like __vad_config__); the handle keeps them on the host
+
 Layout: b"FAB2MDL1", u32 n_tensors, then per tensor: u32 name_len, name (utf-8), u32 ndim, i64 dims[ndim], u64 nbytes,
 zero padding to a 16-byte file offset, little-endian fp32 data.
 """
@@ -174,6 +181,63 @@ def read_vad_config(tensors: Dict[str, np.ndarray]) -> dict:
     out["lorder"] = int(c[base])
     out["sil_pdf_ids"] = [int(v) for v in c[base + 2: base + 2 + int(c[base + 1])]]
     return out
+
+
+PUNC_SPLIT_SIZE = 20
+
+
+def _text_blob(items) -> np.ndarray:
+    for s in items:
+        if "\n" in s or "\0" in s or not s:
+            raise ValueError("list entry %r: entries must be non-empty and hold no newline or NUL" % (s,))
+    b = "\n".join(items).encode("utf-8")
+    return np.frombuffer(b + b"\0" * ((4 - len(b) % 4) % 4), dtype="<f4").copy()
+
+
+def _blob_text(arr: np.ndarray) -> list:
+    return np.ascontiguousarray(arr, dtype="<f4").tobytes().rstrip(b"\0").decode("utf-8").split("\n")
+
+
+def punc_model_tensors(state: Dict[str, torch.Tensor], punc_list, token_list, sentence_end_id: int, encoder_conf: dict) -> Dict[str, np.ndarray]:
+    """The tensors of a CT-Transformer punctuation model file.  state: CTTransformer's state_dict; encoder_conf: its SANMEncoder conf
+    (attention_heads, kernel_size; the layer count and widths are read from the weights)."""
+    layers = 0
+    while "encoder.encoders.%d.norm1.weight" % layers in state:
+        layers += 1
+    if "embed.weight" not in state or "encoder.encoders0.0.norm1.weight" not in state:
+        raise ValueError("not a CT-Transformer state_dict (embed.weight / encoder.encoders0.0 missing)")
+    if "<unk>" not in token_list:
+        raise ValueError("token_list has no <unk> entry")
+    if not 0 <= int(sentence_end_id) < len(punc_list):
+        raise ValueError("sentence_end_id outside punc_list")
+    layout = {k: encoder_conf.get(k, v) for k, v in (("sanm_shfit", 0), ("input_layer", "pe"), ("normalize_before", True),
+                                                       ("selfattention_layer_type", "sanm"))}
+    if layout != {"sanm_shfit": 0, "input_layer": "pe", "normalize_before": True, "selfattention_layer_type": "sanm"}:
+        raise ValueError("the punctuation encoder runs sanm_shfit 0, input_layer \"pe\", normalize_before, \"sanm\" attention; got %r" % layout)
+    d_model = int(state["encoder.after_norm.weight"].numel())
+    heads = int(encoder_conf.get("attention_heads", 8))
+    kernel = int(state["encoder.encoders0.0.self_attn.fsmn_block.weight"].shape[-1])
+    d_in = int(state["embed.weight"].shape[1])
+    out: Dict[str, np.ndarray] = {}
+    out["__punc_config__"] = np.array([layers + 1, d_model, heads, kernel, int(sentence_end_id), PUNC_SPLIT_SIZE], dtype=np.float32)
+    out["__punc_list__"] = _text_blob(list(punc_list))
+    out["__punc_tokens__"] = _text_blob(list(token_list))
+    out["encoder.pe_inv_timescales"] = sinusoid_inv_timescales(d_in).float().numpy()
+    for k, v in state.items():
+        if k.startswith(("embed.", "encoder.", "decoder.")) and torch.is_floating_point(v):
+            out[k] = v.detach().float().cpu().contiguous().numpy()
+    return out
+
+
+def write_punc_model_file(path: str, state: Dict[str, torch.Tensor], punc_list, token_list, sentence_end_id: int, encoder_conf: dict) -> int:
+    return _write(path, punc_model_tensors(state, punc_list, token_list, sentence_end_id, encoder_conf))
+
+
+def read_punc_config(tensors: Dict[str, np.ndarray]) -> dict:
+    """The configuration and both lists of a punctuation model file read back (tests)."""
+    c = [int(v) for v in tensors["__punc_config__"]]
+    return {"layers": c[0], "d_model": c[1], "heads": c[2], "kernel": c[3], "sentence_end_id": c[4], "split_size": c[5],
+            "punc_list": _blob_text(tensors["__punc_list__"]), "token_list": _blob_text(tensors["__punc_tokens__"])}
 
 
 def _write(path: str, tensors: Dict[str, np.ndarray]) -> int:

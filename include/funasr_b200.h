@@ -683,6 +683,36 @@ int64_t fa_pack_segments(const int32_t* segments, int64_t n, int32_t batch_size_
  * count, or FA_ERR_ARG. */
 int64_t fa_merge_vad(const int32_t* segments, int64_t n, int32_t max_length_ms, int32_t min_length_ms, int32_t* out);
 
+/* ---- CT-Transformer punctuation (CTTransformer.inference, ct_transformer/model.py:309-473; funasr_b200/punc.py is the specification)
+ * fa_punc_init: model file written by funasr_b200/pack.py:write_punc_model_file (the reference's state_dict names, __punc_config__ and
+ * both lists).  Refused before any device is touched, naming the piece: d_model > 512 (the encoder workspace bound), a head dim that
+ * is not a multiple of 32 up to 128, a missing tensor or list, a token list without <unk>.  The network always runs the fp32 path.
+ * fa_punc_infer: n UTF-8 texts -> their punctuated texts and per-word punctuation ids (punc_array, after the forced sentence end).
+ * The texts advance in lockstep: step s scores window s (split_size words plus the unfinished tail carried over) of every text that
+ * still has one as ONE padded batch -- fa_embedding, fa_sanm_encoder_forward, fa_linear_argmax -- with one host-to-device copy of the
+ * ids and lengths and one copy of the punctuation ids back; the carry runs on the host.  Each text's result equals punctuating it
+ * alone.  An empty or whitespace-only text gives "" and no ids.  A window with more words than the fp32 attention kernel takes keys
+ * (4 * t floats of shared memory within 160 KB, for heads narrower than 128) fails the call before that step's first launch, naming
+ * the text: the carried tail grows without bound when the model predicts no comma and no sentence end.  NULL on error
+ * (fa_offline_last_error()). */
+void* fa_punc_init(const char* model_file, int32_t device);
+void* fa_punc_infer(void* punc, const char* const* texts, int32_t n);
+/* text i (NUL-terminated UTF-8; NULL for an out-of-range index) / its n punctuation ids (NULL with 0 for an empty text) */
+const char* fa_punc_result_text(const void* result, int32_t index);
+const int32_t* fa_punc_result_ids(const void* result, int32_t index, int32_t* n);
+/* the lockstep steps the call ran (the longest text's window count) */
+int64_t fa_punc_result_steps(const void* result);
+void fa_punc_free_result(void* result);
+void fa_punc_uninit(void* punc);
+/* Host only: the same walk with a caller's scorer in place of the network.  score_fn(ctx, ids [batch, t_max], lens [batch], batch,
+ * t_max, punc_out [batch, t_max]) scores one lockstep step (row b valid for its first lens[b] entries, padding ids 0) and returns 0,
+ * or nonzero to fail the call.  tokens [n_tokens] / punc_list [n_punc]: the vocabulary and the punctuation classes; split_size words per
+ * window; max_window > 0 refuses longer windows as fa_punc_infer does.  Returns a result for the fa_punc_result_* accessors, NULL on
+ * error (fa_offline_last_error()). */
+typedef int32_t (*fa_punc_score_fn)(void* ctx, const int32_t* ids, const int32_t* lens, int32_t batch, int32_t t_max, int32_t* punc_out);
+void* fa_punc_walk_host(const char* const* texts, int32_t n, const char* const* tokens, int32_t n_tokens, const char* const* punc_list,
+                        int32_t n_punc, int32_t sentence_end_id, int32_t split_size, int64_t max_window, fa_punc_score_fn score_fn, void* ctx);
+
 #ifdef __cplusplus
 }
 #endif

@@ -12,6 +12,17 @@
  *   (fa_offline_infer_vad) with the runtime's semantics: a FIXED end silence (the file's max_end_silence_time, fsmn-vad.cpp), segment
  *   texts concatenated in time order (funasrruntime.cpp:287-296); optional key "batch-size-s" sets the segment packing (default 300).
  *   Without it a buffer is decoded as one utterance, as before.
+ *   model_path["punc-dir"] (optional) names a directory holding `punc.fab2` (funasr_b200/pack.py: write_punc_model_file, from the
+ *   CT-Transformer model.pt + its punc_list / token_list + config).  With it FunOfflineInfer / FunOfflineInferBuffer punctuate each
+ *   result text after the join, with or without "vad-dir" (funasrruntime.cpp:311-314); without it results are unpunctuated, as before.
+ *   The punctuation is the Python model's (CTTransformer.inference): its word split, exact lookup with <unk>, 20-word windows with the
+ *   unfinished tail carried over and a long window cut at its last comma when the comma lies at index 2 or later.  The runtime's own
+ *   AddPunc (ct-transformer.cpp) differs: it has its own tokenizer and cuts at any comma with nLastCommaIndex > 0.  This library keeps
+ *   one definition, as it does for stamps.  ITN is not provided (itn is ignored).
+ *   With "punc-dir" and a BiCif model FunASRGetStampSents is the runtime's TimestampSentence (util.cpp:569-637) over the punctuated
+ *   text and the FunASRGetStamp pairs; without "punc-dir" it stays empty.
+ *   CTTransformerInit: model_path["model-dir"] holds `punc.fab2` ("gpu-id" as above); only PUNC_OFFLINE is provided (PUNC_ONLINE is
+ *   refused with a FunB200LastError message); CTTransformerGetResult ignores n_index, as the runtime does.
  *   FsmnVadInit: model_path["model-dir"] holds `vad.fab2` ("gpu-id" as above); FsmnVadInferBuffer is offline only (input_finished
  *   must be true) and takes "pcm" (s16le) or "wav" (PCM16 / float32); FsmnVadOnlineInit is not provided.
  */
@@ -35,6 +46,7 @@ typedef unsigned char FUNASR_BOOL;
 
 typedef enum { RASR_NONE = -1, RASRM_CTC_GREEDY_SEARCH = 0, RASRM_CTC_RPEFIX_BEAM_SEARCH = 1, RASRM_ATTENSION_RESCORING = 2 } FUNASR_MODE;
 typedef enum { ASR_OFFLINE = 0, ASR_ONLINE = 1, ASR_TWO_PASS = 2 } ASR_TYPE;
+typedef enum { PUNC_OFFLINE = 0, PUNC_ONLINE = 1 } PUNC_TYPE;
 
 typedef void (*QM_CALLBACK)(int cur_step, int n_total);
 
@@ -68,6 +80,14 @@ _FUNASRAPI std::vector<std::vector<int>>* FsmnVadGetResult(FUNASR_RESULT result,
 _FUNASRAPI void FsmnVadFreeResult(FUNASR_RESULT result);
 _FUNASRAPI void FsmnVadUninit(FUNASR_HANDLE handle);
 _FUNASRAPI const float FsmnVadGetRetSnippetTime(FUNASR_RESULT result);
+
+// punctuation (funasrruntime.h:94-98), offline only
+_FUNASRAPI FUNASR_HANDLE CTTransformerInit(std::map<std::string, std::string>& model_path, int thread_num, PUNC_TYPE type = PUNC_OFFLINE);
+_FUNASRAPI FUNASR_RESULT CTTransformerInfer(FUNASR_HANDLE handle, const char* sz_sentence, FUNASR_MODE mode, QM_CALLBACK fn_callback,
+                                            PUNC_TYPE type = PUNC_OFFLINE, FUNASR_RESULT pre_result = nullptr);
+_FUNASRAPI const char* CTTransformerGetResult(FUNASR_RESULT result, int n_index);
+_FUNASRAPI void CTTransformerFreeResult(FUNASR_RESULT result);
+_FUNASRAPI void CTTransformerUninit(FUNASR_HANDLE handle);
 
 // WFST decoder (funasrruntime.h:134-138): accepted, no effect (greedy decoding)
 _FUNASRAPI FUNASR_DEC_HANDLE FunASRWfstDecoderInit(FUNASR_HANDLE handle, int asr_type, float glob_beam, float lat_beam, float am_scale);
