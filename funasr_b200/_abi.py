@@ -124,6 +124,7 @@ SIGNATURES = {
     "fa_fbank_lfr_cmvn_tables": (C.c_int, [_vp, _vp, _i32, _i64, _vp, _vp, _i32, _i32, _vp, _i64, _vp, _i32, _vp]),
     "fa_fbank_short": (C.c_int, [_vp, _i32, _vp, _vp, _i32, _vp, _i32, _vp, _vp]),
     "fa_broadcast_rows": (C.c_int, [_vp, _i32, _i32, _vp, _i64, _i32, _vp]),
+    "fa_sv_query_rows": (C.c_int, [_vp, _i32, _i32, _vp, _i32, _vp, _i64, _vp]),
     "fa_ctc_greedy_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32]),
     "fa_ctc_greedy_forward": (C.c_int, [C.POINTER(FaLinear), _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _sz, _vp]),
     "fa_layernorm": (C.c_int, [_vp, _i64, C.POINTER(FaNorm), _vp, _vp, _f, _i32, _vp]),
@@ -192,6 +193,9 @@ SIGNATURES = {
     "fa_offline_result_ids": (C.POINTER(_i32), [_vp, _i32, C.POINTER(_i32)]),
     "fa_offline_result_audio_seconds": (C.c_float, [_vp]),
     "fa_offline_result_stamps": (C.POINTER(_i32), [_vp, _i32, C.POINTER(_i32)]),
+    "fa_offline_is_sensevoice": (_i32, [_vp]),
+    "fa_offline_infer_sv": (_vp, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp, _vp]),
+    "fa_sv_ctc_text_host": (_i64, [_vp, _i32, C.POINTER(C.c_char_p), _i32, C.c_char_p, _i64]),
     "fa_offline_free_result": (None, [_vp]),
     "fa_offline_uninit": (None, [_vp]),
     "fa_offline_last_error": (C.c_char_p, []),
@@ -204,6 +208,7 @@ SIGNATURES = {
     "fa_vad_result_audio_seconds": (C.c_float, [_vp]),
     "fa_vad_free_result": (None, [_vp]),
     "fa_offline_infer_vad": (_vp, [_vp, _vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp, _i32, C.POINTER(FaLongAudioOptions)]),
+    "fa_offline_infer_vad_sv": (_vp, [_vp, _vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp, _vp, C.POINTER(FaLongAudioOptions)]),
     "fa_offline_result_segments": (C.POINTER(_i32), [_vp, _i32, C.POINTER(_i32)]),
     "fa_gather_segments": (C.c_int, [_vp, _i64, _vp, _vp, _i32, _i64, _vp, _vp]),
     "fa_pack_segments": (_i64, [_vp, _i64, _i32, _i32, _vp, _vp]),

@@ -151,6 +151,19 @@ __global__ void broadcast_rows_kernel(const float* __restrict__ rows, int n_rows
   if (i < n_rows * cols) dst[(int64_t)b * batch_stride_rows * cols + i] = rows[i];
 }
 
+// dst[b, r, :] = embed[q(b, r), :] with q(b, .) = {ids[2b], 1, 2, ids[2b + 1]}: SenseVoice's per-utterance query rows.  Ids are
+// clamped to the table (the callers validate them on the host first).
+__global__ void sv_query_rows_kernel(const float* __restrict__ embed, int n_embed, int cols, const int32_t* __restrict__ ids,
+                                     float* __restrict__ dst, int64_t batch_stride_rows) {
+  const int b = blockIdx.y;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 4 * cols) return;
+  const int r = i / cols, c = i - r * cols;
+  int q = r == 0 ? ids[2 * b] : r == 3 ? ids[2 * b + 1] : r;
+  q = min(max(q, 0), n_embed - 1);
+  dst[(int64_t)b * batch_stride_rows * cols + i] = embed[(int64_t)q * cols + c];
+}
+
 int ctc_filter_launch(const int32_t* ids, const int32_t* lens, int batch, int t_max, int blank, int32_t* out_ids,
                       int32_t* out_lens, cudaStream_t st) {
   ctc_filter_kernel<<<batch, 32, 0, st>>>(ids, lens, t_max, blank, out_ids, out_lens);
@@ -205,6 +218,15 @@ extern "C" int fa_broadcast_rows(const float* rows, int32_t n_rows, int32_t cols
   if (!rows || !dst || n_rows <= 0 || cols <= 0 || batch <= 0 || dst_batch_stride_rows < n_rows) return FA_ERR_ARG;
   dim3 grid((n_rows * cols + 255) / 256, batch);
   fa::broadcast_rows_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(rows, n_rows, cols, dst, dst_batch_stride_rows);
+  FA_CHECK_LAUNCH();
+  return FA_OK;
+}
+
+extern "C" int fa_sv_query_rows(const float* embed, int32_t n_embed, int32_t cols, const int32_t* ids, int32_t batch, float* dst,
+                                int64_t dst_batch_stride_rows, fa_stream_t stream) {
+  if (!embed || !ids || !dst || n_embed < 3 || cols <= 0 || batch <= 0 || batch > 65535 || dst_batch_stride_rows < 4) return FA_ERR_ARG;
+  dim3 grid((4 * cols + 255) / 256, batch);
+  fa::sv_query_rows_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(embed, n_embed, cols, ids, dst, dst_batch_stride_rows);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }

@@ -12,6 +12,8 @@
 //   fa_offline_infer_vad    long recordings: VAD -> segments packed by duration -> each pack gathered on the device and decoded
 //   fa_punc_init / fa_punc_infer     CT-Transformer model file -> handle; many texts -> punctuated texts, every text one window per
 //                           lockstep step (the text walk: punc_text.cpp)
+//   a SenseVoiceSmall file (__sv_config__) makes the same handle run SenseVoiceEngine's chain: per-utterance query rows
+//                           (fa_sv_query_rows), the SAN-M and tp stacks, the CTC head; fa_offline_infer_sv / fa_offline_infer_vad_sv
 // The tokenizer (ids -> text) stays with the caller, like every other entry point of this ABI.
 #include "common.cuh"
 #include "punc_text.h"
@@ -156,6 +158,13 @@ struct Model {
   FaTimestampHead head{};
   DevBuf us_alphas, us_peaks;
   std::map<std::string, std::vector<float>> host_cache;   // fa_offline_host_tensor
+  bool sv = false;                                   // SenseVoiceSmall (__sv_config__): query rows, the SAN-M and tp stacks, the CTC head
+  int tp_layers = 0, n_embed = 0, blank = 0;
+  std::vector<FaEncLayer> tp_l;
+  FaEncoder tp{};
+  FaLinear ctc{};
+  const float* embed = nullptr;
+  DevBuf enc2, am;
 };
 
 struct Result {
@@ -452,6 +461,186 @@ std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride,
   return r;
 }
 
+// ------------------------------------------------------------------------------------------------ SenseVoiceSmall
+// __sv_config__ of funasr_b200/pack.py:write_sensevoice_model_file
+enum { kSvEnc = 0, kSvTp, kSvDModel, kSvHeads, kSvKernel, kSvVocab, kSvFeat, kSvEps, kSvBlank, kSvCfgLen };
+const int32_t kSvAuto = 0, kSvWoItn = 15;             // SenseVoiceSmall.inference's defaults: language "auto", text norm "woitn"
+
+std::string sv_layer(bool tp, int i) {
+  return tp ? "encoder.tp_encoders." + std::to_string(i) : i == 0 ? "encoder.encoders0.0" : "encoder.encoders." + std::to_string(i - 1);
+}
+
+// everything the file's index decides (configuration, every tensor the chain reads, the shapes the kernels take), before any device work
+bool check_sv(const std::map<std::string, Tensor>& t, Model& m) {
+  auto need = [&](const std::string& k) -> const Tensor* {
+    auto it = t.find(k);
+    if (it == t.end()) { set_err("SenseVoice model: missing tensor " + k); return nullptr; }
+    return &it->second;
+  };
+  if (t.count("__config__")) { set_err("SenseVoice model: the file carries both __config__ (Paraformer) and __sv_config__"); return false; }
+  const Tensor* cfg = need("__sv_config__");
+  if (!cfg) return false;
+  if (cfg->host.size() != kSvCfgLen) { set_err("SenseVoice model: bad __sv_config__"); return false; }
+  const float* c = cfg->host.data();
+  m.enc_layers = (int)c[kSvEnc]; m.tp_layers = (int)c[kSvTp]; m.d_model = (int)c[kSvDModel]; m.heads = (int)c[kSvHeads];
+  m.kernel = (int)c[kSvKernel]; m.vocab = (int)c[kSvVocab]; m.feat_dim = (int)c[kSvFeat]; m.ln_eps = c[kSvEps]; m.blank = (int)c[kSvBlank];
+  if (m.enc_layers < 1 || m.tp_layers < 0) { set_err("SenseVoice model: no encoder layer"); return false; }
+  if (m.d_model != 512 || m.heads != 4) {
+    set_err("SenseVoice model: d_model " + std::to_string(m.d_model) + " with " + std::to_string(m.heads) +
+            " heads (the tensor-core attention runs d_model 512 as 4 heads of 128)");
+    return false;
+  }
+  if (m.vocab < 1 || m.vocab > 61440) {
+    set_err("SenseVoice model: vocabulary of " + std::to_string(m.vocab) + " tokens (the CTC arg-max takes at most 61440)");
+    return false;
+  }
+  if (m.feat_dim != 560) { set_err("SenseVoice model: feat_dim " + std::to_string(m.feat_dim) + " (the frontend is 80 mel x LFR 7 = 560)"); return false; }
+  if (m.blank < 0 || m.blank >= m.vocab) { set_err("SenseVoice model: blank_id outside the vocabulary"); return false; }
+  std::vector<std::string> names = {"frontend.mel_banks", "frontend.window", "encoder.pe_inv_timescales", "encoder.after_norm.weight",
+                                    "encoder.after_norm.bias", "ctc.ctc_lo.bias"};
+  if (m.tp_layers > 0) names.insert(names.end(), {"encoder.tp_norm.weight", "encoder.tp_norm.bias"});
+  const char* layer_keys[] = {".norm1.weight", ".norm1.bias", ".norm2.weight", ".norm2.bias", ".self_attn.linear_q_k_v.weight",
+                              ".self_attn.linear_q_k_v.bias", ".self_attn.linear_out.weight", ".self_attn.linear_out.bias",
+                              ".self_attn.fsmn_block.weight", ".feed_forward.w_1.weight", ".feed_forward.w_1.bias", ".feed_forward.w_2.weight",
+                              ".feed_forward.w_2.bias"};
+  for (int s = 0; s < 2; ++s)
+    for (int i = 0; i < (s ? m.tp_layers : m.enc_layers); ++i)
+      for (const char* k : layer_keys) names.push_back(sv_layer(s == 1, i) + k);
+  for (const std::string& n : names)
+    if (!need(n)) return false;
+  const Tensor* ctc = need("ctc.ctc_lo.weight");
+  const Tensor* emb = ctc ? need("embed.weight") : nullptr;
+  if (!emb) return false;
+  if (ctc->shape != std::vector<int64_t>{(int64_t)m.vocab, (int64_t)m.d_model}) { set_err("SenseVoice model: bad shape of ctc.ctc_lo.weight (want [vocab, 512])"); return false; }
+  if (emb->shape.size() != 2 || emb->shape[0] < 3 || emb->shape[1] != m.feat_dim) { set_err("SenseVoice model: bad shape of embed.weight (want [>= 3, 560])"); return false; }
+  auto cm = t.find("frontend.cmvn");
+  if (cm != t.end() && cm->second.numel() != 2 * m.feat_dim) { set_err("SenseVoice model: frontend.cmvn must be [2, 560]"); return false; }
+  m.n_embed = (int)emb->shape[0];
+  m.sv = true;
+  return true;
+}
+
+// the SenseVoiceEngine of engine.py: the same weights, the same planes per gemm_mode
+bool build_sv(Model& m) {
+  Builder b{m.file, m.mode};
+  b.ln_eps = m.ln_eps;
+  if (!b.fbank_tables()) return false;
+  m.cmvn = m.file.t.count("frontend.cmvn") ? m.file.t["frontend.cmvn"].dev : nullptr;
+  auto stack = [&](bool tp, int n, std::vector<FaEncLayer>& L, FaEncoder& e) {
+    L.resize(n > 0 ? n : 1);
+    for (int i = 0; i < n; ++i) {
+      const std::string p = sv_layer(tp, i);
+      L[i].norm1 = b.norm(p + ".norm1"); L[i].norm2 = b.norm(p + ".norm2");
+      L[i].qkv = b.lin(p + ".self_attn.linear_q_k_v"); L[i].out = b.lin(p + ".self_attn.linear_out");
+      L[i].fsmn_w = b.ptr(p + ".self_attn.fsmn_block.weight");
+      L[i].w1 = b.lin(p + ".feed_forward.w_1"); L[i].w2 = b.lin(p + ".feed_forward.w_2");
+    }
+    const Tensor* fw = n > 0 ? b.get(sv_layer(tp, 0) + ".self_attn.fsmn_block.weight") : nullptr;
+    e.layers = L.data(); e.n_layers = n; e.heads = m.heads; e.fsmn_k = fw && !fw->shape.empty() ? (int)fw->shape.back() : m.kernel;
+    if (n > 0) e.after_norm = b.norm(tp ? "encoder.tp_norm" : "encoder.after_norm");
+    e.pe_inv_timescales = tp ? nullptr : b.ptr("encoder.pe_inv_timescales");    // the tp blocks take no position encoding
+  };
+  stack(false, m.enc_layers, m.enc_l, m.enc);
+  stack(true, m.tp_layers, m.tp_l, m.tp);
+  m.ctc = b.lin("ctc.ctc_lo");
+  m.embed = b.ptr("embed.weight");
+  if (!b.ok) return false;
+  return cudaStreamSynchronize(m.file.st) == cudaSuccess;
+}
+
+// every query id inside the embedding table; `what` names the unit ("utterance", "recording")
+bool check_queries(const Model& m, const int32_t* lang, const int32_t* tn, int n, const char* what) {
+  for (int i = 0; i < n; ++i) {
+    const int32_t l = lang ? lang[i] : kSvAuto, t = tn ? tn[i] : kSvWoItn;
+    if (l < 0 || l >= m.n_embed || t < 0 || t >= m.n_embed) {
+      set_err(std::string(what) + " " + std::to_string(i) + ": " + (l < 0 || l >= m.n_embed ? "language id " + std::to_string(l) : "textnorm id " + std::to_string(t)) +
+              " outside the embedding table [0, " + std::to_string(m.n_embed) + ")");
+      return false;
+    }
+  }
+  return true;
+}
+
+// SenseVoiceEngine.forward_wav over a padded batch already on the device (wav [B, stride], lens_h >= 400 samples each), utterance i
+// queried with (lang[i], tn[i]) (NULL: the defaults; validated by check_queries).  The CTC head materialises the logits [B, T, vocab].
+std::unique_ptr<Result> decode_sv(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const int32_t* lang,
+                                  const int32_t* tn) {
+  const int B = (int)lens_h.size(), D = m.d_model, F = m.feat_dim;
+  cudaStream_t st = m.file.st;
+  int t_feat = 0;
+  double seconds = 0.0;
+  // one host-to-device copy: sample counts [B], encoder lengths [B] (frames + the 4 query rows), query ids [B][2]
+  std::vector<int32_t> io((size_t)4 * B);
+  for (int i = 0; i < B; ++i) {
+    const int t = num_lfr_frames(lens_h[i]);
+    t_feat = t > t_feat ? t : t_feat;
+    seconds += (double)lens_h[i] / 16000.0;
+    io[i] = lens_h[i];
+    io[B + i] = t + 4;
+    io[2 * B + 2 * i] = lang ? lang[i] : kSvAuto;
+    io[2 * B + 2 * i + 1] = tn ? tn[i] : kSvWoItn;
+  }
+  const int T = t_feat + 4;
+  const size_t rows = (size_t)B * T;
+  const size_t ws = std::max(fa_sanm_encoder_workspace_bytes(B, T, m.mode), fa_ctc_greedy_workspace_bytes(B, T, m.vocab, m.mode));
+  if (!(m.lens.reserve(io.size() * 4) && m.feats.reserve(rows * F * 4) && m.flens.reserve((size_t)B * 4) && m.encb.reserve(rows * D * 4) &&
+        m.enc2.reserve(rows * D * 4) && m.am.reserve(rows * 4) && m.ids.reserve(rows * 4) && m.flens_out.reserve((size_t)B * 4) && m.ws.reserve(ws)))
+    return fail("device allocation failed (SenseVoice)");
+  int32_t* io_d = static_cast<int32_t*>(m.lens.p);
+  float* x = static_cast<float*>(m.feats.p);
+  float* enc = static_cast<float*>(m.encb.p);
+  cudaMemcpyAsync(io_d, io.data(), io.size() * 4, cudaMemcpyHostToDevice, st);
+  int rc = fa_fbank_lfr_cmvn_tables(wav, io_d, B, stride, m.cmvn, m.file.fbank_tables, 7, 6, x + 4 * F, T, static_cast<int32_t*>(m.flens.p), t_feat, st);
+  if (rc == FA_OK) rc = fa_sv_query_rows(m.embed, m.n_embed, F, io_d + 2 * B, B, x, T, st);
+  if (rc == FA_OK) rc = fa_sanm_encoder_forward(&m.enc, x, io_d + B, B, T, enc, m.mode, m.ws.p, m.ws.cap, st);
+  if (rc == FA_OK && m.tp_layers > 0) {
+    rc = fa_sanm_encoder_forward(&m.tp, enc, io_d + B, B, T, static_cast<float*>(m.enc2.p), m.mode, m.ws.p, m.ws.cap, st);
+    enc = static_cast<float*>(m.enc2.p);
+  }
+  if (rc == FA_OK)
+    rc = fa_ctc_greedy_forward(&m.ctc, enc, io_d + B, B, T, m.blank, static_cast<int32_t*>(m.am.p), static_cast<int32_t*>(m.ids.p),
+                               static_cast<int32_t*>(m.flens_out.p), nullptr, m.mode, m.ws.p, m.ws.cap, st);
+  if (rc != FA_OK) return fail(std::string("SenseVoice: ") + fa_status_string(rc));
+  std::unique_ptr<Result> r(new Result());
+  r->audio_seconds = (float)seconds;
+  r->token_num.resize(B);
+  r->ids.resize(B);
+  std::vector<int32_t> ids(rows);
+  cudaMemcpyAsync(ids.data(), m.ids.p, rows * 4, cudaMemcpyDeviceToHost, st);
+  cudaMemcpyAsync(r->token_num.data(), m.flens_out.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess) return fail(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError()));
+  for (int i = 0; i < B; ++i) r->ids[i].assign(ids.begin() + (size_t)i * T, ids.begin() + (size_t)i * T + r->token_num[i]);
+  return r;
+}
+
+// one padded batch on the device decoded by the handle's model kind: the hotword memory reaches a contextual Paraformer, the queries
+// (per row, NULL = the defaults) a SenseVoice model
+std::unique_ptr<Result> decode_pack(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const float* hw_embed,
+                                    int32_t n_hotwords, const int32_t* lang, const int32_t* tn) {
+  return m.sv ? decode_sv(m, wav, stride, lens_h, lang, tn) : decode_batch(m, wav, stride, lens_h, hw_embed, n_hotwords);
+}
+
+// fa_offline_infer_hw / fa_offline_infer_sv: host buffers -> one padded batch -> decode_pack
+void* infer_batch(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format, const float* hw_embed,
+                  int32_t n_hotwords, const int32_t* lang, const int32_t* tn) {
+  Model* mp = static_cast<Model*>(handle);
+  if (!mp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) return fail("bad argument");
+  Model& m = *mp;
+  if (m.contextual && (!hw_embed || n_hotwords < 1)) return fail("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)");
+  if (m.sv && !check_queries(m, lang, tn, batch, "utterance")) return nullptr;
+  cudaSetDevice(m.file.device);
+  int64_t nmax = 0;
+  std::vector<int32_t> lens_h(batch);
+  for (int i = 0; i < batch; ++i) {
+    if (!bufs[i] || n_samples[i] < 400 || n_samples[i] > 0x7fffffffLL) return fail("every buffer needs >= 400 samples (25 ms)");
+    lens_h[i] = (int32_t)n_samples[i];
+    nmax = n_samples[i] > nmax ? n_samples[i] : nmax;
+  }
+  const int64_t stride = (nmax + 3) / 4 * 4;
+  if (!upload(bufs, n_samples, batch, stride, pcm_format, m.wav, m.pcm16, m.file.st)) return nullptr;
+  return decode_pack(m, static_cast<const float*>(m.wav.p), stride, lens_h, hw_embed, n_hotwords, lang, tn).release();
+}
+
 }  // namespace
 
 extern "C" const char* fa_offline_last_error(void) { return g_err.c_str(); }
@@ -463,12 +652,26 @@ extern "C" void* fa_offline_init(const char* model_file, int32_t device, int32_t
   if (!model_file) return fail("model_file is NULL");
   if (gemm_mode != FA_GEMM_F32_SIMT && gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) return fail("bad gemm_mode");
   FaTimestampHead head{};
-  std::map<std::string, Tensor> index;          // what the file's index alone decides (the timestamp head) is refused before any device work
-  if (!no_throw("model file rejected: ", [&] { return load_file(index, model_file, false) && check_ts_head(index, head); })) return nullptr;
   std::unique_ptr<Model> m(new Model());
+  // what the file's index alone decides (the model kind, SenseVoice's configuration and tensors, the timestamp head) is refused before
+  // any device work
+  std::map<std::string, Tensor> index;
+  if (!no_throw("model file rejected: ", [&] {
+        return load_file(index, model_file, false) && (index.count("__sv_config__") ? check_sv(index, *m) : check_ts_head(index, head));
+      }))
+    return nullptr;
   m->mode = gemm_mode; m->head = head; m->ts = head.up_times > 0;
-  if (!no_throw("model file rejected: ", [&] { return m->file.open(model_file, device) && build(*m); })) return nullptr;
+  if (!no_throw("model file rejected: ", [&] { return m->file.open(model_file, device) && (m->sv ? build_sv(*m) : build(*m)); })) return nullptr;
   return m.release();
+}
+
+extern "C" int32_t fa_offline_is_sensevoice(const void* handle) { return handle && static_cast<const Model*>(handle)->sv ? 1 : 0; }
+
+extern "C" void* fa_offline_infer_sv(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
+                                     const int32_t* language_ids, const int32_t* textnorm_ids) {
+  g_err.clear();
+  if (handle && !static_cast<Model*>(handle)->sv) return fail("fa_offline_infer_sv: not a SenseVoice model file");
+  return infer_batch(handle, bufs, n_samples, batch, pcm_format, nullptr, 0, language_ids, textnorm_ids);
 }
 
 extern "C" void fa_offline_uninit(void* handle) { delete static_cast<Model*>(handle); }
@@ -505,21 +708,7 @@ extern "C" void* fa_offline_infer(void* handle, const void* const* bufs, const i
 extern "C" void* fa_offline_infer_hw(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
                                      const float* hw_embed, int32_t n_hotwords) {
   g_err.clear();
-  Model* mp = static_cast<Model*>(handle);
-  if (!mp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) return fail("bad argument");
-  Model& m = *mp;
-  if (m.contextual && (!hw_embed || n_hotwords < 1)) return fail("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)");
-  cudaSetDevice(m.file.device);
-  int64_t nmax = 0;
-  std::vector<int32_t> lens_h(batch);
-  for (int i = 0; i < batch; ++i) {
-    if (!bufs[i] || n_samples[i] < 400 || n_samples[i] > 0x7fffffffLL) return fail("every buffer needs >= 400 samples (25 ms)");
-    lens_h[i] = (int32_t)n_samples[i];
-    nmax = n_samples[i] > nmax ? n_samples[i] : nmax;
-  }
-  const int64_t stride = (nmax + 3) / 4 * 4;
-  if (!upload(bufs, n_samples, batch, stride, pcm_format, m.wav, m.pcm16, m.file.st)) return nullptr;
-  return decode_batch(m, static_cast<const float*>(m.wav.p), stride, lens_h, hw_embed, n_hotwords).release();
+  return infer_batch(handle, bufs, n_samples, batch, pcm_format, hw_embed, n_hotwords, nullptr, nullptr);
 }
 
 extern "C" int32_t fa_offline_result_count(const void* result) { return result ? (int32_t)static_cast<const Result*>(result)->ids.size() : 0; }
@@ -759,8 +948,10 @@ extern "C" void fa_vad_free_result(void* result) { delete static_cast<VadResult*
 namespace {
 
 // one recording of fa_offline_infer_vad: inference_with_vad (auto_model.py:852-1035, funasr_b200/long_audio.py:LongAudioPipeline.generate)
+// (lang, tn): the recording's SenseVoice query, the same for all its segments
 bool long_audio_one(Model& m, Vad& v, int rec_index, const void* buf, int64_t n, int32_t pcm_format, const float* hw_embed, int32_t n_hotwords,
-                    const FaLongAudioOptions& o, std::vector<int32_t>& ids, std::vector<int32_t>& segs_out, std::vector<int32_t>& stamps) {
+                    int32_t lang, int32_t tn, const FaLongAudioOptions& o, std::vector<int32_t>& ids, std::vector<int32_t>& segs_out,
+                    std::vector<int32_t>& stamps) {
   cudaStream_t st = m.file.st;
   if (!upload_one(buf, n, pcm_format, m.rec, m.pcm16, st)) return false;
   const float* rec = static_cast<const float*>(m.rec.p);
@@ -805,11 +996,14 @@ bool long_audio_one(Model& m, Vad& v, int rec_index, const void* buf, int64_t n,
     float* wav = static_cast<float*>(m.wav.p);
     const int rc = fa_gather_segments(rec, n, starts_d, lens_d, B, stride, wav, st);
     if (rc != FA_OK) { set_err(std::string("fa_gather_segments: ") + fa_status_string(rc)); return false; }
-    const std::unique_ptr<Result> pr = decode_batch(m, wav, stride, lens, hw_embed, n_hotwords);
+    const std::vector<int32_t> lang_v(B, lang), tn_v(B, tn);
+    const std::unique_ptr<Result> pr = decode_pack(m, wav, stride, lens, hw_embed, n_hotwords, lang_v.data(), tn_v.data());
     if (!pr) return false;
     int tmax = 0;
     for (int32_t t : pr->token_num) tmax = t > tmax ? t : tmax;
-    if (tmax < 1) emptied = true;                            // no token in the whole pack: the recording's result is empty (:990-999)
+    // no token in the whole pack: the recording's result is empty (:990-999).  SenseVoiceSmall.inference returns a result for every
+    // utterance, empty or not, so its packs never empty a recording.
+    if (tmax < 1 && !m.sv) emptied = true;
     else
       for (int j = 0; j < B; ++j) {
         seg_ids[order[beg + j]].swap(pr->ids[j]);
@@ -826,16 +1020,15 @@ bool long_audio_one(Model& m, Vad& v, int rec_index, const void* buf, int64_t n,
   return true;
 }
 
-}  // namespace
-
-extern "C" void* fa_offline_infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
-                                      const float* hw_embed, int32_t n_hotwords, const FaLongAudioOptions* opts) {
-  g_err.clear();
+// fa_offline_infer_vad / fa_offline_infer_vad_sv: every recording on its own; lang / tn one query per recording (NULL = the defaults)
+void* infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format, const float* hw_embed,
+                int32_t n_hotwords, const int32_t* lang, const int32_t* tn, const FaLongAudioOptions* opts) {
   Model* mp = static_cast<Model*>(asr);
   Vad* vp = static_cast<Vad*>(vad);
   if (!mp || !vp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) return fail("bad argument");
   if (mp->file.device != vp->file.device) return fail("the recogniser and the VAD live on different devices");
   if (mp->contextual && (!hw_embed || n_hotwords < 1)) return fail("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)");
+  if (mp->sv && !check_queries(*mp, lang, tn, batch, "recording")) return nullptr;
   FaLongAudioOptions o;
   if (opts) o = *opts;
   else { o.batch_size_s = 300; o.batch_size_threshold_s = 60; o.merge_vad = 0; o.merge_length_s = 15; o.vad = default_vad_run(); }
@@ -852,7 +1045,8 @@ extern "C" void* fa_offline_infer_vad(void* asr, void* vad, const void* const* b
   if (!no_throw("fa_offline_infer_vad: ", [&] {
         for (int i = 0; i < batch; ++i) {
           seconds += (double)n_samples[i] / 16000.0;
-          if (!long_audio_one(*mp, *vp, i, bufs[i], n_samples[i], pcm_format, hw_embed, n_hotwords, o, r->ids[i], r->segs[i], r->stamps[i]))
+          if (!long_audio_one(*mp, *vp, i, bufs[i], n_samples[i], pcm_format, hw_embed, n_hotwords, lang ? lang[i] : kSvAuto,
+                              tn ? tn[i] : kSvWoItn, o, r->ids[i], r->segs[i], r->stamps[i]))
             return false;
           r->token_num[i] = (int32_t)r->ids[i].size();
         }
@@ -861,6 +1055,21 @@ extern "C" void* fa_offline_infer_vad(void* asr, void* vad, const void* const* b
     return nullptr;
   r->audio_seconds = (float)seconds;
   return r.release();
+}
+
+}  // namespace
+
+extern "C" void* fa_offline_infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
+                                      const float* hw_embed, int32_t n_hotwords, const FaLongAudioOptions* opts) {
+  g_err.clear();
+  return infer_vad(asr, vad, bufs, n_samples, batch, pcm_format, hw_embed, n_hotwords, nullptr, nullptr, opts);
+}
+
+extern "C" void* fa_offline_infer_vad_sv(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
+                                         const int32_t* language_ids, const int32_t* textnorm_ids, const FaLongAudioOptions* opts) {
+  g_err.clear();
+  if (asr && !static_cast<Model*>(asr)->sv) return fail("fa_offline_infer_vad_sv: not a SenseVoice model file");
+  return infer_vad(asr, vad, bufs, n_samples, batch, pcm_format, nullptr, 0, language_ids, textnorm_ids, opts);
 }
 
 extern "C" const int32_t* fa_offline_result_segments(const void* result, int32_t index, int32_t* n_segments) {

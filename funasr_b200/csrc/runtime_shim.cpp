@@ -232,6 +232,57 @@ std::vector<std::string> split_units(const std::string& w) {
 
 inline float sigm(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// SenseVoice: the runtime's lid_map (sensevoice-small.h:110-118); an unknown svs_lang is "auto" (sensevoice-small.cpp:458-465)
+const std::map<std::string, int32_t> kSvLidMap = {{"auto", 0}, {"zh", 3}, {"en", 4}, {"yue", 7}, {"ja", 11}, {"ko", 12}, {"nospeech", 13}};
+
+// SenseVoiceSmall::CTCSearch (sensevoice-small.cpp:305-355) after its arg-max and collapse, over the handle's ids.  The runtime reads
+// tokens[3] whenever it has at least 3 tokens, one past the end with exactly 3; here that fourth tag is empty.
+std::string sv_ctc_text(const int32_t* ids, int n, const std::vector<std::string>& vocab) {
+  auto piece = [&](int32_t id) { return id >= 0 && id < (int32_t)vocab.size() ? vocab[id] : std::to_string(id); };
+  std::string lang, emo, event, itn, text;
+  if (n >= 3) { lang = piece(ids[0]); emo = piece(ids[1]); event = piece(ids[2]); }
+  if (n >= 4) itn = piece(ids[3]);
+  for (int i = 4; i < n; ++i) {
+    const std::string w = piece(ids[i]);
+    text += w.find("\xe2\x96\x81") != std::string::npos ? " " + w.substr(3) : w;      // U+2581, three bytes
+  }
+  if (itn == "<|withitn|>") text += lang == "<|zh|>" ? "\xe3\x80\x82" : ".";              // U+3002
+  return lang + emo + event + " " + text;
+}
+
+FaLongAudioOptions runtime_long_audio_options(const OfflineStream& s) {
+  FaLongAudioOptions o;
+  o.batch_size_s = s.batch_size_s; o.batch_size_threshold_s = 60; o.merge_vad = 0; o.merge_length_s = 15; o.vad = runtime_vad_options();
+  return o;
+}
+
+// a SenseVoice handle: the query from svs_lang / svs_itn, each segment's CTCSearch text concatenated in time order without a separator
+// (funasrruntime.cpp:287-296 for a language other than en-bpe); punctuation, ITN and stamps do not apply (offline-stream.cpp:147-150)
+FUNASR_RESULT infer_sv(OfflineStream* s, const void* const* bufs, const int64_t* lens, int fmt, const std::string& svs_lang, bool svs_itn) {
+  auto it = kSvLidMap.find(svs_lang);
+  const int32_t lid = it != kSvLidMap.end() ? it->second : 0, itn = svs_itn ? 14 : 15;
+  const FaLongAudioOptions o = runtime_long_audio_options(*s);
+  void* r = s->vad ? fa_offline_infer_vad_sv(s->h, s->vad, bufs, lens, 1, fmt, &lid, &itn, &o) : fa_offline_infer_sv(s->h, bufs, lens, 1, fmt, &lid, &itn);
+  if (!r) { g_shim_err = fa_offline_last_error(); return nullptr; }
+  int32_t k = 0, nseg = 0;
+  const int32_t* ids = fa_offline_result_ids(r, 0, &k);
+  std::string text;
+  if (s->vad) {
+    const int32_t* seg = fa_offline_result_segments(r, 0, &nseg);
+    for (int32_t i = 0, pos = 0; i < nseg; ++i) {
+      text += sv_ctc_text(ids + pos, seg[3 * i + 2], s->vocab);
+      pos += seg[3 * i + 2];
+    }
+  } else {
+    text = sv_ctc_text(ids, k, s->vocab);
+  }
+  ShimResult* out = new ShimResult();
+  out->msgs.push_back(text);
+  out->snippet_time = fa_offline_result_audio_seconds(r);
+  fa_offline_free_result(r);
+  return out;
+}
+
 // RIFF WAVE: returns the PCM payload and its format (1 = s16le, 0 = float32); mono or the first channel layout is required
 bool parse_wav(const std::string& bytes, const char** data, size_t* n_bytes, int* fmt, int* rate) {
   if (bytes.size() < 44 || memcmp(bytes.data(), "RIFF", 4) != 0 || memcmp(bytes.data() + 8, "WAVE", 4) != 0) return false;
@@ -260,19 +311,20 @@ bool parse_wav(const std::string& bytes, const char** data, size_t* n_bytes, int
   return false;
 }
 
-FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, int fmt, const std::vector<std::vector<float>>& hw_emb) {
+FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, int fmt, const std::vector<std::vector<float>>& hw_emb,
+                        const std::string& svs_lang, bool svs_itn) {
   const int64_t n = (int64_t)(n_bytes / (fmt == 1 ? 2 : 4));
+  const void* bufs[1] = {data};
+  const int64_t lens[1] = {n};
+  if (fa_offline_is_sensevoice(s->h)) return infer_sv(s, bufs, lens, fmt, svs_lang, svs_itn);
   std::vector<float> hw;
   int n_hw = 0;
   if (fa_offline_is_contextual(s->h)) {
     for (const auto& row : hw_emb) if (row.size() == 512) { hw.insert(hw.end(), row.begin(), row.end()); ++n_hw; }
     if (n_hw == 0) { g_shim_err = "contextual model: hw_emb must hold [n, 512] rows from CompileHotwordEmbedding"; return nullptr; }
   }
-  const void* bufs[1] = {data};
-  const int64_t lens[1] = {n};
   if (s->vad) {                        // segment texts concatenated in time order (funasrruntime.cpp:287-296)
-    FaLongAudioOptions o;
-    o.batch_size_s = s->batch_size_s; o.batch_size_threshold_s = 60; o.merge_vad = 0; o.merge_length_s = 15; o.vad = runtime_vad_options();
+    const FaLongAudioOptions o = runtime_long_audio_options(*s);
     void* r = fa_offline_infer_vad(s->h, s->vad, bufs, lens, 1, fmt, n_hw ? hw.data() : nullptr, n_hw, &o);
     if (!r) { g_shim_err = fa_offline_last_error(); return nullptr; }
     int32_t k = 0, nseg = 0;
@@ -312,6 +364,22 @@ FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, int 
 }  // namespace
 
 const char* FunB200LastError() { return g_shim_err.c_str(); }
+
+extern "C" int64_t fa_sv_ctc_text_host(const int32_t* ids, int32_t n, const char* const* tokens, int32_t n_tokens, char* out, int64_t cap) {
+  if ((!ids && n > 0) || n < 0 || (!tokens && n_tokens > 0) || n_tokens < 0 || (!out && cap > 0)) return -1;
+  std::vector<std::string> vocab;
+  for (int32_t i = 0; i < n_tokens; ++i) {
+    if (!tokens[i]) return -1;
+    vocab.push_back(tokens[i]);
+  }
+  const std::string s = sv_ctc_text(ids, n, vocab);
+  if (cap > 0) {
+    const size_t k = std::min<size_t>(s.size(), (size_t)(cap - 1));
+    memcpy(out, s.data(), k);
+    out[k] = '\0';
+  }
+  return (int64_t)s.size();
+}
 
 FUNASR_HANDLE FunOfflineInit(std::map<std::string, std::string>& model_path, int thread_num, bool use_gpu, int batch_size) {
   (void)thread_num; (void)use_gpu;
@@ -368,7 +436,7 @@ void FunOfflineUninit(FUNASR_HANDLE handle) {
 
 FUNASR_RESULT FunOfflineInferBuffer(FUNASR_HANDLE handle, const char* sz_buf, int n_len, FUNASR_MODE, QM_CALLBACK fn_callback,
                                     const std::vector<std::vector<float>>& hw_emb, int sampling_rate, std::string wav_format, bool,
-                                    FUNASR_DEC_HANDLE, std::string, bool) {
+                                    FUNASR_DEC_HANDLE, std::string svs_lang, bool svs_itn) {
   g_shim_err.clear();
   OfflineStream* s = static_cast<OfflineStream*>(handle);
   if (!s || !sz_buf || n_len <= 0) { g_shim_err = "bad argument"; return nullptr; }
@@ -381,7 +449,7 @@ FUNASR_RESULT FunOfflineInferBuffer(FUNASR_HANDLE handle, const char* sz_buf, in
     if (!parse_wav(holder, &data, &nb, &fmt, &rate)) { g_shim_err = "unsupported WAV (need mono PCM16 or float32)"; return nullptr; }
   } else if (wav_format != "pcm") { g_shim_err = "wav_format must be \"pcm\" (s16le) or \"wav\""; return nullptr; }
   if (rate != 16000) { g_shim_err = "audio must be 16 kHz"; return nullptr; }
-  FUNASR_RESULT r = infer_pcm(s, data, nb, fmt, hw_emb);
+  FUNASR_RESULT r = infer_pcm(s, data, nb, fmt, hw_emb, svs_lang, svs_itn);
   if (fn_callback) fn_callback(1, 1);
   return r;
 }
@@ -406,6 +474,7 @@ const std::vector<std::vector<float>> CompileHotwordEmbedding(FUNASR_HANDLE hand
   g_shim_err.clear();
   std::vector<std::vector<float>> out;
   OfflineStream* s = static_cast<OfflineStream*>(handle);
+  if (s && fa_offline_is_sensevoice(s->h)) return {std::vector<float>(512, 0.f)};    // one zero row (sensevoice-small.cpp:423-429)
   if (!s || !fa_offline_is_contextual(s->h)) return out;
   int64_t n_emb = 0, n_ih = 0, n_hh = 0, n_bi = 0, n_bh = 0;
   const float* emb = fa_offline_host_tensor(s->h, "bias_embed.weight", &n_emb);

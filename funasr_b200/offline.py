@@ -161,6 +161,20 @@ def punc_walk_host(texts: Sequence[str], token_list: Sequence[str], punc_list: S
         lib.fa_punc_free_result(res)
 
 
+def sv_query_ids(n: int, language=None, use_itn=None):
+    """SenseVoice queries of n utterances or recordings -> (language ids, textnorm ids) as int32 arrays, through SenseVoiceSmallB200's
+    lid_dict / textnorm_dict (an unknown language is "auto", as in SenseVoiceSmall.inference).  language: one name or one per item
+    (default "auto"); use_itn: one bool or one per item (default False)."""
+    from .modules import SenseVoiceSmallB200
+    langs = ["auto" if language is None else language] * n if language is None or isinstance(language, str) else list(language)
+    itns = [bool(use_itn)] * n if use_itn is None or isinstance(use_itn, (bool, int, np.bool_)) else [bool(v) for v in use_itn]
+    if len(langs) != n or len(itns) != n:
+        raise _abi.FunasrB200Error("language / use_itn: one value or one per item (%d items)" % n)
+    tn = SenseVoiceSmallB200.textnorm_dict
+    lid = np.array([SenseVoiceSmallB200.lid_dict.get(x, 0) for x in langs], dtype=np.int32)
+    return lid, np.array([tn["withitn" if v else "woitn"] for v in itns], dtype=np.int32)
+
+
 class OfflineRecognizer:
     def __init__(self, model_file: str, device: int = 0, gemm_mode: str = "fp16x3"):
         self.lib = _abi.load()
@@ -174,17 +188,33 @@ class OfflineRecognizer:
         """True for a BiCifParaformer model file: results carry per-token stamps from its upsampled CIF head."""
         return bool(self.lib.fa_offline_has_timestamps(self.handle))
 
+    @property
+    def is_sensevoice(self) -> bool:
+        """True for a SenseVoiceSmall model file: `infer` / `infer_long` take `language` and `use_itn`."""
+        return bool(self.lib.fa_offline_is_sensevoice(self.handle))
+
+    def _queries(self, n: int, language, use_itn):
+        if not self.is_sensevoice:
+            if language is not None or use_itn is not None:
+                raise _abi.FunasrB200Error("language / use_itn apply to a SenseVoice model file only")
+            return None
+        return sv_query_ids(n, language, use_itn)
+
     def _stamps(self, res, i) -> List[List[int]]:
         cnt = C.c_int32(0)
         p = self.lib.fa_offline_result_stamps(res, i, C.byref(cnt))
         return [[int(p[2 * k]), int(p[2 * k + 1])] for k in range(cnt.value)]
 
-    def _infer(self, wavs, stamped: bool):
+    def _infer(self, wavs, stamped: bool, language=None, use_itn=None):
         arrs, fmt = _pcm_batch(wavs)
         n = len(arrs)
         ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
         lens = (C.c_int64 * n)(*[a.shape[0] for a in arrs])
-        res = self.lib.fa_offline_infer(self.handle, ptrs, lens, n, fmt)
+        q = self._queries(n, language, use_itn)
+        if q is None:
+            res = self.lib.fa_offline_infer(self.handle, ptrs, lens, n, fmt)
+        else:
+            res = self.lib.fa_offline_infer_sv(self.handle, ptrs, lens, n, fmt, q[0].ctypes.data, q[1].ctypes.data)
         if not res:
             raise _abi.FunasrB200Error("fa_offline_infer failed: %s" % self.lib.fa_offline_last_error().decode())
         try:
@@ -199,9 +229,11 @@ class OfflineRecognizer:
         finally:
             self.lib.fa_offline_free_result(res)
 
-    def infer(self, wavs: Sequence[np.ndarray]) -> List[List[int]]:
-        """wavs: float32 arrays in [-1, 1] or int16 PCM arrays (all the same dtype), 16 kHz mono, >= 400 samples each."""
-        return self._infer(wavs, False)
+    def infer(self, wavs: Sequence[np.ndarray], language=None, use_itn=None) -> List[List[int]]:
+        """wavs: float32 arrays in [-1, 1] or int16 PCM arrays (all the same dtype), 16 kHz mono, >= 400 samples each.
+        SenseVoice model file: language (one name or one per utterance, default "auto") and use_itn (default False) choose each
+        utterance's query; the ids include the four tag tokens (SenseVoiceSmall.inference's token_int)."""
+        return self._infer(wavs, False, language, use_itn)
 
     def infer_stamped(self, wavs: Sequence[np.ndarray]) -> List[dict]:
         """Like `infer`, per utterance {"token_int": ids, "timestamp": [[start_ms, end_ms], ...]} (BiCifParaformer.inference's result;
@@ -210,11 +242,12 @@ class OfflineRecognizer:
 
     def infer_long(self, wavs: Sequence[np.ndarray], vad: OfflineVad, batch_size_s: int = 300, batch_size_threshold_s: int = 60,
                    merge_vad: bool = False, merge_length_s: int = 15, hotword_embeddings: Optional[np.ndarray] = None,
-                   **vad_kwargs) -> List[dict]:
+                   language=None, use_itn=None, **vad_kwargs) -> List[dict]:
         """Long recordings through fa_offline_infer_vad, each on its own as LongAudioPipeline.generate treats it -> per recording
         {"token_int": ids in time order, "vad_segments": [[start_ms, end_ms], ...], "n_tokens": tokens per segment}, plus
         "timestamp": [[start_ms, end_ms], ...] in absolute ms when the model has the timestamp head (`has_timestamps`).
-        hotword_embeddings: [n, 512] float32 rows (ContextualParaformer; last row the <s> entry)."""
+        hotword_embeddings: [n, 512] float32 rows (ContextualParaformer; last row the <s> entry).  SenseVoice model file
+        (fa_offline_infer_vad_sv): language / use_itn as in `infer`, one per recording, applied to all its segments."""
         arrs, fmt = _pcm_batch(wavs)
         n = len(arrs)
         ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
@@ -225,8 +258,12 @@ class OfflineRecognizer:
         if hotword_embeddings is not None:
             hw = np.ascontiguousarray(hotword_embeddings, dtype=np.float32)
             n_hw = hw.shape[0]
-        res = self.lib.fa_offline_infer_vad(self.handle, vad.handle, ptrs, lens, n, fmt, None if hw is None else hw.ctypes.data, n_hw,
-                                            C.byref(opts))
+        q = self._queries(n, language, use_itn)
+        if q is None:
+            res = self.lib.fa_offline_infer_vad(self.handle, vad.handle, ptrs, lens, n, fmt, None if hw is None else hw.ctypes.data, n_hw,
+                                                C.byref(opts))
+        else:
+            res = self.lib.fa_offline_infer_vad_sv(self.handle, vad.handle, ptrs, lens, n, fmt, q[0].ctypes.data, q[1].ctypes.data, C.byref(opts))
         if not res:
             raise _abi.FunasrB200Error("fa_offline_infer_vad failed: %s" % self.lib.fa_offline_last_error().decode())
         try:

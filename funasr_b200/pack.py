@@ -37,6 +37,12 @@ encoder.after_norm.* and decoder.* under the reference's names, the derived enco
     __punc_list__ / __punc_tokens__    the UTF-8 bytes of punc_list / token_list, newline-joined, zero-padded to a multiple of 4 and
                                        stored as the bytes of an fp32 tensor (like __vad_config__); the handle keeps them on the host
 
+The SenseVoiceSmall file (csrc/offline.cu: fa_offline_init, recognised by __sv_config__) holds encoder.encoders0.0.*,
+encoder.encoders.{i}.*, encoder.after_norm.*, encoder.tp_encoders.{i}.*, encoder.tp_norm.*, ctc.ctc_lo.* and embed.weight under the
+reference's names, the frontend tables and encoder.pe_inv_timescales of the Paraformer file, and
+
+    __sv_config__                      [9] enc_layers, tp_layers, d_model, heads, fsmn kernel, vocab, feat_dim, ln_eps, blank_id
+
 Layout: b"FAB2MDL1", u32 n_tensors, then per tensor: u32 name_len, name (utf-8), u32 ndim, i64 dims[ndim], u64 nbytes,
 zero padding to a 16-byte file offset, little-endian fp32 data.
 """
@@ -53,17 +59,22 @@ from .synth import ParaformerConfig, sinusoid_inv_timescales
 MAGIC = b"FAB2MDL1"
 
 
-def model_tensors(state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: Optional[torch.Tensor], smooth_factor2: float = 0.25,
-                  noise_threshold2: float = 0.01) -> Dict[str, np.ndarray]:
+def _frontend_tensors(out: Dict[str, np.ndarray], cmvn: Optional[torch.Tensor], feat_dim: int) -> None:
+    """The derived tables of a recogniser file: mel banks, window, optional CMVN and the encoder's PE timescales."""
     from .engine import kaldi_mel_banks
-    out: Dict[str, np.ndarray] = {}
-    out["__config__"] = np.array([cfg.enc_layers, cfg.dec_layers, cfg.d_model, cfg.heads, cfg.kernel, cfg.vocab, cfg.feat_dim,
-                                  cfg.ln_eps, cfg.cif_threshold, cfg.tail_threshold], dtype=np.float32)
     out["frontend.mel_banks"] = kaldi_mel_banks().numpy()
     out["frontend.window"] = torch.hamming_window(400, periodic=False, alpha=0.54, beta=0.46, dtype=torch.float32).numpy()
     if cmvn is not None:
         out["frontend.cmvn"] = cmvn.detach().float().cpu().numpy()
-    out["encoder.pe_inv_timescales"] = sinusoid_inv_timescales(cfg.feat_dim).float().numpy()
+    out["encoder.pe_inv_timescales"] = sinusoid_inv_timescales(feat_dim).float().numpy()
+
+
+def model_tensors(state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: Optional[torch.Tensor], smooth_factor2: float = 0.25,
+                  noise_threshold2: float = 0.01) -> Dict[str, np.ndarray]:
+    out: Dict[str, np.ndarray] = {}
+    out["__config__"] = np.array([cfg.enc_layers, cfg.dec_layers, cfg.d_model, cfg.heads, cfg.kernel, cfg.vocab, cfg.feat_dim,
+                                  cfg.ln_eps, cfg.cif_threshold, cfg.tail_threshold], dtype=np.float32)
+    _frontend_tensors(out, cmvn, cfg.feat_dim)
     for k, v in state.items():
         if k.startswith(("encoder.", "predictor.", "decoder.", "bias_encoder.", "bias_embed.")) and torch.is_floating_point(v):
             out[k] = v.detach().float().cpu().contiguous().numpy()
@@ -82,6 +93,25 @@ def write_model_file(path: str, state: Dict[str, torch.Tensor], cfg: ParaformerC
     """smooth_factor2 / noise_threshold2: CifPredictorV3's predictor_conf values (paraformer-large-vad-punc's by default); used only
     when the state dict has the BiCif timestamp head."""
     return _write(path, model_tensors(state, cfg, cmvn, smooth_factor2, noise_threshold2))
+
+
+def sensevoice_model_tensors(state: Dict[str, torch.Tensor], cfg, cmvn: Optional[torch.Tensor], blank_id: int = 0) -> Dict[str, np.ndarray]:
+    """The tensors of a SenseVoiceSmall model file.  state: SenseVoiceSmall's state_dict; cfg: synth.SenseVoiceConfig (its ln_eps, 1e-5,
+    travels in the file: the handle's Paraformer default is 1e-12)."""
+    if "embed.weight" not in state or "ctc.ctc_lo.weight" not in state or "encoder.encoders0.0.norm1.weight" not in state:
+        raise ValueError("not a SenseVoiceSmall state_dict (embed.weight / ctc.ctc_lo / encoder.encoders0.0 missing)")
+    out: Dict[str, np.ndarray] = {}
+    out["__sv_config__"] = np.array([cfg.enc_layers, cfg.tp_layers, cfg.d_model, cfg.heads, cfg.kernel, cfg.vocab, cfg.feat_dim, cfg.ln_eps,
+                                     blank_id], dtype=np.float32)
+    _frontend_tensors(out, cmvn, cfg.feat_dim)
+    for k, v in state.items():
+        if k.startswith(("encoder.", "ctc.", "embed.")) and torch.is_floating_point(v):
+            out[k] = v.detach().float().cpu().contiguous().numpy()
+    return out
+
+
+def write_sensevoice_model_file(path: str, state: Dict[str, torch.Tensor], cfg, cmvn: Optional[torch.Tensor] = None, blank_id: int = 0) -> int:
+    return _write(path, sensevoice_model_tensors(state, cfg, cmvn, blank_id))
 
 
 TS_HEAD_KEY = "upsample_cnn.weight"

@@ -176,6 +176,11 @@ int fa_fbank_short(const float* wav, int32_t n_samples, const float* window, con
  * the query-frame prepend `torch.cat((input_query, speech), dim=1)` of sense_voice/model.py:985-995. */
 int fa_broadcast_rows(const float* rows, int32_t n_rows, int32_t cols, float* dst, int64_t dst_batch_stride_rows,
                       int32_t batch, fa_stream_t stream);
+/* The same prepend with a query per utterance: dst[b, 0..3, :] = embed[ids[2b]], embed[1], embed[2], embed[ids[2b + 1]] (language,
+ * event, emotion, text norm; sense_voice/model.py:971-995).  embed [n_embed, cols] and ids [batch, 2] (language id, textnorm id) are
+ * device memory; ids are clamped to [0, n_embed) (validate them first).  Only the 4 query rows of every utterance are written. */
+int fa_sv_query_rows(const float* embed, int32_t n_embed, int32_t cols, const int32_t* ids, int32_t batch, float* dst,
+                     int64_t dst_batch_stride_rows, fa_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Operator-level entry points (each is used by the model-level calls below and exposed for parity tests)
@@ -616,6 +621,26 @@ float fa_offline_result_audio_seconds(const void* result);
  * shifted by its start ms and concatenated in time order (auto_model.py:1008-1022).  NULL with 0 for a model without the head, for
  * an entry without stamps and for NULL / out-of-range arguments. */
 const int32_t* fa_offline_result_stamps(const void* result, int32_t index, int32_t* n_stamps);
+/* SenseVoiceSmall (sense_voice/model.py:918-1034).  fa_offline_init recognises its model file (funasr_b200/pack.py:
+ * write_sensevoice_model_file) by __sv_config__ and refuses, before it touches a device and naming the piece: a file with both
+ * __config__ and __sv_config__, a missing tensor, d_model != 512 or heads != 4 (the tensor-core attention shapes), a vocabulary above
+ * 61440 (the CTC arg-max).  fa_offline_is_sensevoice: 1 for such a handle, 0 otherwise or for NULL.
+ * fa_offline_infer_sv: like fa_offline_infer, utterance i queried with the embedding rows language_ids[i], 1, 2, textnorm_ids[i]
+ * (SenseVoiceSmall.lid_dict / textnorm_dict ids; NULL = 0 "auto" / 15 "woitn", the Python model's defaults).  An id outside the
+ * embedding table fails the call before any launch, naming the utterance.  Each result is the CTC-collapsed ids including the four tag
+ * tokens (SenseVoiceSmall.inference's token_int); no stamps.  The CTC head materialises the logits: vocab x 4 bytes per frame (25055
+ * tokens: about 3.2 GB at 64 utterances of 30 s).  fa_offline_infer / fa_offline_infer_hw on a SenseVoice handle use the defaults and
+ * ignore hotwords; fa_offline_infer_sv on any other handle fails. */
+int32_t fa_offline_is_sensevoice(const void* handle);
+void* fa_offline_infer_sv(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
+                          const int32_t* language_ids, const int32_t* textnorm_ids);
+/* Host only: the result text of SenseVoice's CTCSearch in FunASR's C++ runtime (runtime/onnxruntime/src/sensevoice-small.cpp:305-355)
+ * over ids [n] and the token list tokens [n_tokens] (an id outside it, or any id when n_tokens is 0, reads as its decimal number):
+ * the first three tags concatenated, " ", then the pieces from the fifth id on, a piece containing U+2581 adding " " and the piece
+ * without its first 3 bytes; U+3002 after the language tag <|zh|> and "." otherwise when the fourth tag is <|withitn|>.  With exactly 3 ids the
+ * fourth tag reads as empty (the runtime reads one past its token vector there).  Writes at most cap - 1 bytes and a NUL to out when
+ * cap > 0; returns the text's length in bytes, or -1 for a bad argument. */
+int64_t fa_sv_ctc_text_host(const int32_t* ids, int32_t n, const char* const* tokens, int32_t n_tokens, char* out, int64_t cap);
 void fa_offline_free_result(void* result);
 void fa_offline_uninit(void* handle);
 const char* fa_offline_last_error(void);
@@ -667,6 +692,12 @@ typedef struct {
  * asr and vad must live on the same device.  NULL on error (fa_offline_last_error()). */
 void* fa_offline_infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
                            const float* hw_embed, int32_t n_hotwords, const FaLongAudioOptions* opts);
+/* The same for a SenseVoice handle with one query per recording (language_ids[i], textnorm_ids[i]; NULL = the defaults), applied to
+ * all of that recording's segments; an id outside the embedding table fails the call naming the recording.  SenseVoiceSmall.inference
+ * returns a result for every segment, so a pack never empties a recording.  fa_offline_infer_vad on a SenseVoice handle uses the
+ * defaults; fa_offline_infer_vad_sv on any other handle fails. */
+void* fa_offline_infer_vad_sv(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
+                              const int32_t* language_ids, const int32_t* textnorm_ids, const FaLongAudioOptions* opts);
 /* n_segments {start_ms, end_ms, n_tokens} triples of recording `index` (time order); NULL with 0 for results of fa_offline_infer. */
 const int32_t* fa_offline_result_segments(const void* result, int32_t index, int32_t* n_segments);
 /* out [rows, stride] = rec[starts[r] .. starts[r] + lens[r]) then zeros (rec [n_rec] fp32; starts int64 / lens int32 [rows] device;

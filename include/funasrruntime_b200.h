@@ -21,6 +21,13 @@
  *   one definition, as it does for stamps.  ITN is not provided (itn is ignored).
  *   With "punc-dir" and a BiCif model FunASRGetStampSents is the runtime's TimestampSentence (util.cpp:569-637) over the punctuated
  *   text and the FunASRGetStamp pairs; without "punc-dir" it stays empty.
+ *   A SenseVoiceSmall `model.fab2` (funasr_b200/pack.py: write_sensevoice_model_file) makes a SenseVoice handle: the file decides
+ *   the model kind (the runtime decides by "SenseVoiceSmall" in the directory name).  FunOfflineInferBuffer maps svs_lang through the
+ *   runtime's lid_map (an unknown name is "auto") and svs_itn to text norm 14 / 15; FunOfflineInfer uses "auto" / true.  The text is
+ *   the runtime's CTCSearch over the ids and tokens.txt, except that with exactly 3 ids the fourth tag is empty (the runtime reads one
+ *   past its vector there); the ids are the Python model's arg-max of log_softmax.  With "vad-dir" segment texts are concatenated
+ *   without a separator; "punc-dir" and ITN are ignored, FunASRGetStamp / FunASRGetStampSents stay empty, and CompileHotwordEmbedding
+ *   returns one zero row of 512.
  *   CTTransformerInit: model_path["model-dir"] holds `punc.fab2` ("gpu-id" as above); only PUNC_OFFLINE is provided (PUNC_ONLINE is
  *   refused with a FunB200LastError message); CTTransformerGetResult ignores n_index, as the runtime does.
  *   FsmnVadInit: model_path["model-dir"] holds `vad.fab2` ("gpu-id" as above); FsmnVadInferBuffer is offline only (input_finished
