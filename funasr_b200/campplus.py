@@ -33,6 +33,8 @@ FCM_CONVS = ["conv1", "layer1.0.conv1", "layer1.0.conv2", "layer1.0.shortcut.0",
 FCM_BNS = ["bn1", "layer1.0.bn1", "layer1.0.bn2", "layer1.0.shortcut.1", "layer1.1.bn1", "layer1.1.bn2",
            "layer2.0.bn1", "layer2.0.bn2", "layer2.0.shortcut.1", "layer2.1.bn1", "layer2.1.bn2", "bn2"]
 FCM_STRIDE = [1, 2, 1, 2, 1, 1, 2, 1, 2, 1, 1, 2]
+# fa_campplus_forward's longest input (~188 s): the CAM context gate keeps at most 94 segment means of 100 TDNN frames per chunk
+MAX_FEAT_FRAMES = 18800
 
 
 def campplus_specs() -> "OrderedDict[str, tuple]":
@@ -175,7 +177,7 @@ class CampplusEngine(_EngineBase):
         out = torch.empty((B, EMB_DIM), dtype=torch.float32, device=self.device)
         per = int(self.lib.fa_campplus_workspace_bytes(C.byref(self.model), 1, T, self.mode))
         if per == 0:
-            raise _abi.FunasrB200Error("CAM++ needs at least 2 feature frames per input (got %d)" % T)
+            raise _abi.FunasrB200Error("CAM++ takes 2 ... %d feature frames per input (got %d)" % (MAX_FEAT_FRAMES, T))
         step = max(1, min(B, self.WORKSPACE_CAP // per))
         for b0 in range(0, B, step):
             nb = min(step, B - b0)

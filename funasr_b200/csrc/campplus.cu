@@ -15,6 +15,10 @@ namespace fa {
 constexpr int kCamBn = 128, kCamOut = 32, kCamHid = 64, kCamSeg = 100;
 constexpr int kCamTile = 32;                  // output rows per tile of the local conv
 constexpr int kCamMaxDil = 8;
+// cam_gate_kernel holds every segment mean of a chunk in (non-opt-in) shared memory: nseg <= 94, i.e. t <= 9 400 TDNN frames
+// (18 800 feature frames, ~188 s)
+constexpr size_t kCamGateSmemMax = 48 * 1024;
+static size_t cam_gate_smem(int nseg) { return ((size_t)nseg * kCamBn + kCamBn + kCamHid) * sizeof(float); }
 
 // ------------------------------------------------------------------------------------------------ FCM 2-D convolutions
 // in (b, f, t, c) at in[b * isb + f * isf + t * ist + c]; out (b, f, t, o) at out[b * osb + f * osf + t * ost + o * osc]; res (the
@@ -333,8 +337,8 @@ static int cam_launch(const float* h, int batch, int T, int dil, const float* lo
   if (batch <= 0 || T <= 0) return FA_OK;
   if (dil < 1 || dil > kCamMaxDil || !local_w || !w1 || !b1 || !w2 || !b2) return FA_ERR_ARG;
   const int nseg = (T + kCamSeg - 1) / kCamSeg;
-  const size_t gsm = ((size_t)nseg * kCamBn + kCamBn + kCamHid) * sizeof(float);
-  if (gsm > 48 * 1024) return FA_ERR_UNSUPPORTED;       // nseg <= 94: utterances up to ~188 s
+  const size_t gsm = cam_gate_smem(nseg);
+  if (gsm > kCamGateSmemMax) return FA_ERR_UNSUPPORTED;
   cam_gate_kernel<<<batch, kCamBn, gsm, st>>>(h, T, nseg, w1, b1, w2, b2, gates);
   FA_CHECK_LAUNCH();
   const size_t lsm = (size_t)(3 * kCamBn * kCamOut + (kCamTile + 2 * kCamMaxDil) * kCamBn) * sizeof(float);
@@ -361,17 +365,20 @@ struct CamShapes {
   int64_t rows, pad_rows;
   int c_final[3];
 };
-static bool cam_shapes(const FaCampplus* m, int batch, int T, CamShapes* s) {
-  if (!m || batch <= 0 || T < 2) return false;
+// FA_ERR_ARG for a null model, batch < 1 or T < 2; FA_ERR_UNSUPPORTED for more CAM segments than cam_launch accepts (T > 18 800),
+// so that the forward refuses such an input before its first launch and the workspace query returns 0 for it.
+static int cam_shapes(const FaCampplus* m, int batch, int T, CamShapes* s) {
+  if (!m || batch <= 0 || T < 2) return FA_ERR_ARG;
   s->B = batch; s->T = T;
   s->t_out = (T - 1) / 2 + 1;
   s->P = (T + 4 + 1) / 2 * 2;
   s->nseg = (s->t_out + kCamSeg - 1) / kCamSeg;
+  if (cam_gate_smem(s->nseg) > kCamGateSmemMax) return FA_ERR_UNSUPPORTED;
   s->rows = (int64_t)batch * s->t_out;
   s->pad_rows = (int64_t)batch * s->P + 4;
   int c = 128;
   for (int i = 0; i < 3; ++i) { s->c_final[i] = c + 32 * m->n_layers[i]; c = s->c_final[i] / 2; }
-  return true;
+  return FA_OK;
 }
 
 struct CamBufs {
@@ -415,7 +422,8 @@ static int bn_relu_linear(const float* x, int64_t ldx, int64_t rows, const float
 static int campplus_forward(const FaCampplus* m, const float* feats, int batch, int T, float* emb, int mode, void* ws, size_t ws_bytes,
                             cudaStream_t st) {
   CamShapes s;
-  if (!cam_shapes(m, batch, T, &s) || !feats || !emb) return FA_ERR_ARG;
+  if (!feats || !emb) return FA_ERR_ARG;
+  FA_RETURN_IF_ERR(cam_shapes(m, batch, T, &s));
   if (mode != FA_GEMM_F32_SIMT && mode != FA_GEMM_F16X1 && mode != FA_GEMM_F16X3 && mode != FA_GEMM_F16X6) return FA_ERR_ARG;
   const bool tc = mode != FA_GEMM_F32_SIMT;
   if (tc && (!m->tdnn.w_planes || !m->dense.w_planes || m->tdnn.in_pad != 1600)) return FA_ERR_ARG;
@@ -511,7 +519,7 @@ extern "C" int fa_campplus_features(const float* wav, const int32_t* wav_lens, i
 
 extern "C" size_t fa_campplus_workspace_bytes(const FaCampplus* model, int32_t batch, int32_t t, int32_t gemm_mode) {
   CamShapes s;
-  if (!cam_shapes(model, batch, t, &s)) return 0;
+  if (cam_shapes(model, batch, t, &s) != FA_OK) return 0;
   Arena m = Arena::measuring();
   CamBufs bf;
   cam_carve(m, s, gemm_mode, &bf);

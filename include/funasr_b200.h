@@ -560,7 +560,10 @@ typedef struct {
  * the mean subtracted from them is the mean over those t_max frames.  Nothing outside feats [B, t_max, 80] is written. */
 int fa_campplus_features(const float* wav, const int32_t* wav_lens, int32_t batch, int64_t wav_stride, const float* tables,
                          float* feats, int32_t* feat_lens, int32_t t_max, fa_stream_t stream);
-/* CAMPPlus.forward: feats [B, t, 80] (every frame used, no mask) -> emb [B, 192].  Stream-ordered, no host synchronisation. */
+/* CAMPPlus.forward: feats [B, t, 80] (every frame used, no mask) -> emb [B, 192].  Stream-ordered, no host synchronisation.
+ * 2 <= t <= 18 800 (at most 94 CAM segments of 100 TDNN frames, ~188 s): t < 2 -> FA_ERR_ARG, t > 18 800 -> FA_ERR_UNSUPPORTED,
+ * both before anything is enqueued, and the workspace query returns 0 for either.  At t == 2 the single TDNN frame's unbiased
+ * std is 0 / 0, so emb is NaN, as in the reference. */
 size_t fa_campplus_workspace_bytes(const FaCampplus* model, int32_t batch, int32_t t, int32_t gemm_mode);
 int fa_campplus_forward(const FaCampplus* model, const float* feats, int32_t batch, int32_t t, float* emb, int32_t gemm_mode,
                         void* workspace, size_t ws_bytes, fa_stream_t stream);

@@ -8,6 +8,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from campplus_ref import cam_layer_ref, campplus_ref
 from test_spk_host import SPK_CASES, campplus_state_dict, load_spk_case
 
 pytestmark = pytest.mark.gpu
@@ -20,62 +21,6 @@ def _st():
     return torch.cuda.current_stream(DEV).cuda_stream
 
 
-# ---------------------------------------------------------------------------------------------- CPU restatement (float64)
-def _bn(sd, p, x, dim=1):
-    shape = [1] * x.dim()
-    shape[dim] = -1
-    y = (x - sd[p + ".running_mean"].double().view(shape)) / torch.sqrt(sd[p + ".running_var"].double().view(shape) + 1e-5)
-    if (p + ".weight") in sd:
-        y = y * sd[p + ".weight"].double().view(shape) + sd[p + ".bias"].double().view(shape)
-    return y
-
-
-def cam_layer_ref(h, wl, w1, b1, w2, b2, dil):
-    """CAMLayer.forward on h [B, C, T] (float64)."""
-    y = F.conv1d(h, wl, padding=dil, dilation=dil)
-    T = h.shape[-1]
-    seg = F.avg_pool1d(h, kernel_size=100, stride=100, ceil_mode=True)
-    seg = seg.unsqueeze(-1).expand(*seg.shape, 100).reshape(*seg.shape[:-1], -1)[..., :T]
-    ctx = h.mean(-1, keepdim=True) + seg
-    m = torch.sigmoid(F.conv1d(F.relu(F.conv1d(ctx, w1, b1)), w2, b2))
-    return y * m
-
-
-def campplus_ref(sd, feats):
-    """CAMPPlus.forward (eval) in float64 on the CPU: feats [B, T, 80] -> [B, 192]."""
-    sd = {k: v.double() if v.is_floating_point() else v for k, v in sd.items()}
-    x = feats.double().permute(0, 2, 1).unsqueeze(1)
-
-    def conv_bn(x, conv, bn, stride=1, pad=1):
-        return _bn(sd, "head." + bn, F.conv2d(x, sd["head." + conv + ".weight"], stride=(stride, 1), padding=pad))
-
-    x = F.relu(conv_bn(x, "conv1", "bn1"))
-    for layer in ("layer1", "layer2"):
-        for b in (0, 1):
-            p = "%s.%d." % (layer, b)
-            s = 2 if b == 0 else 1
-            out = F.relu(conv_bn(x, p + "conv1", p + "bn1", s))
-            out = conv_bn(out, p + "conv2", p + "bn2")
-            sc = conv_bn(x, p + "shortcut.0", p + "shortcut.1", s, 0) if b == 0 else x
-            x = F.relu(out + sc)
-    x = F.relu(conv_bn(x, "conv2", "bn2", 2))
-    x = x.reshape(x.shape[0], -1, x.shape[-1])
-    x = F.relu(_bn(sd, "xvector.tdnn.nonlinear.batchnorm", F.conv1d(x, sd["xvector.tdnn.linear.weight"], stride=2, padding=2)))
-    for i, (n, dil) in enumerate(zip((12, 24, 16), (1, 2, 2))):
-        for l in range(n):
-            p = "xvector.block%d.tdnnd%d." % (i + 1, l + 1)
-            h = F.conv1d(F.relu(_bn(sd, p + "nonlinear1.batchnorm", x)), sd[p + "linear1.weight"])
-            h = F.relu(_bn(sd, p + "nonlinear2.batchnorm", h))
-            y = cam_layer_ref(h, sd[p + "cam_layer.linear_local.weight"], sd[p + "cam_layer.linear1.weight"], sd[p + "cam_layer.linear1.bias"],
-                              sd[p + "cam_layer.linear2.weight"], sd[p + "cam_layer.linear2.bias"], dil)
-            x = torch.cat([x, y], 1)
-        p = "xvector.transit%d." % (i + 1)
-        x = F.conv1d(F.relu(_bn(sd, p + "nonlinear.batchnorm", x)), sd[p + "linear.weight"])
-    x = F.relu(_bn(sd, "xvector.out_nonlinear.batchnorm", x))
-    x = torch.cat([x.mean(-1), x.std(-1, unbiased=True)], -1)
-    return _bn(sd, "xvector.dense.nonlinear.batchnorm", F.conv1d(x.unsqueeze(-1), sd["xvector.dense.linear.weight"]).squeeze(-1))
-
-
 def rel(a, b):
     a, b = torch.as_tensor(a).double().cpu(), torch.as_tensor(b).double().cpu()
     return float((a - b).abs().max() / b.abs().max())
@@ -84,7 +29,10 @@ def rel(a, b):
 # ---------------------------------------------------------------------------------------------- kernels
 @pytest.mark.parametrize("cin,k,stride,f_in,t,res,relu", [(1, 3, 1, 80, 148, False, True), (32, 3, 2, 80, 37, False, True),
                                                            (32, 3, 1, 40, 61, True, True), (32, 1, 2, 40, 29, False, False),
-                                                           (32, 3, 2, 20, 5, False, True)])
+                                                           (32, 3, 2, 20, 5, False, True),
+                                                           # a partial kConvTP = 4 time tile only
+                                                           (1, 3, 1, 80, 1, False, True), (32, 3, 1, 40, 2, True, True),
+                                                           (32, 3, 2, 20, 3, False, True)])
 def test_fcm_conv_kernel(cin, k, stride, f_in, t, res, relu):
     from funasr_b200 import _abi
     lib = _abi.load()
@@ -111,10 +59,25 @@ def test_fcm_conv_kernel(cin, k, stride, f_in, t, res, relu):
     assert rel(y.permute(0, 3, 1, 2), ref) < 1e-5
 
 
-@pytest.mark.parametrize("t,dil", [(74, 1), (74, 2), (150, 2), (201, 1), (1, 2)])
+# t 100 / 101 / 199: one full segment, a one-row last segment, a 99-row last segment; dil 8 is kCamMaxDil; t 9 400 is the most segments
+# (94) the gate kernel's shared memory holds.  dil 9 and t 9 401 are refused before any launch.
+@pytest.mark.parametrize("t,dil", [(74, 1), (74, 2), (150, 2), (201, 1), (1, 2), (100, 2), (101, 2), (199, 2), (74, 8), (9400, 2),
+                                   (74, 9), (9401, 2)])
 def test_cam_kernel(t, dil):
     from funasr_b200 import _abi
     lib = _abi.load()
+    if dil > 8 or t > 9400:
+        B = 2
+        h = torch.zeros(B * t, 128, device=DEV)
+        w = torch.zeros(3 * 128 * 32, device=DEV)
+        gates = torch.empty(B, (t + 99) // 100, 32, device=DEV)
+        out = torch.empty(B * t, 32, device=DEV)
+        torch.cuda.synchronize()
+        n0 = lib.fa_launch_count()
+        rc = lib.fa_campplus_cam(h.data_ptr(), B, t, dil, *([w.data_ptr()] * 5), gates.data_ptr(), out.data_ptr(), 32, _st())
+        torch.cuda.synchronize()
+        assert rc == (-1 if dil > 8 else -4) and lib.fa_launch_count() == n0
+        return
     g = torch.Generator().manual_seed(t * 10 + dil)
     B = 5
     h = F.relu(torch.randn(B, 128, t, generator=g))
@@ -131,11 +94,13 @@ def test_cam_kernel(t, dil):
     _abi.check(lib.fa_campplus_cam(hd.data_ptr(), B, t, dil, *[u.data_ptr() for u in dev], gates.data_ptr(), out[:, 32:].data_ptr(), ld, _st()),
                "fa_campplus_cam")
     got = out[:, 32:64].reshape(B, t, 32).permute(0, 2, 1)
+    print("campplus cam t%d dil%d: rel %.3e" % (t, dil, rel(got, ref)))
     assert rel(got, ref) < 1e-5
     assert bool((out[:, :32] == 7.0).all()) and bool((out[:, 64:] == 7.0).all())        # only its column slice is written
 
 
-@pytest.mark.parametrize("t", [74, 3, 257])
+# t 1: the mean is y itself and the unbiased std 0 / 0 (NaN, as torch.std(unbiased=True) gives); t 9 400: the longest fp32 time sum
+@pytest.mark.parametrize("t", [74, 3, 257, 1, 2, 9400])
 def test_stats_pool_kernel(t):
     from funasr_b200 import _abi
     lib = _abi.load()
@@ -148,7 +113,13 @@ def test_stats_pool_kernel(t):
     xd, sd_, shd = x.to(DEV), s.to(DEV), sh.to(DEV)
     out = torch.empty(B, 2 * Cc, device=DEV)
     _abi.check(lib.fa_campplus_stats_pool(xd.data_ptr(), B, t, Cc, sd_.data_ptr(), shd.data_ptr(), out.data_ptr(), _st()), "fa_campplus_stats_pool")
-    assert rel(out, ref) < 1e-5
+    if t == 1:
+        assert torch.equal(out[:, :Cc].cpu(), y[:, 0].float())          # fmaf rounds x * s + sh once, like float64 then fp32
+        assert bool(torch.isnan(out[:, Cc:]).all()) and bool(torch.isnan(ref[:, Cc:]).all())
+        return
+    print("campplus stats t%d: rel %.3e" % (t, rel(out, ref)))
+    # the time sums run in fp32 in time order, so their rounding grows with t: 2.8e-5 at t 9 400 on an H100 (8.7e-7 at t 257)
+    assert rel(out, ref) < (1.2e-4 if t > 1000 else 1e-5)
 
 
 # ---------------------------------------------------------------------------------------------- model level
@@ -182,7 +153,8 @@ def test_features_vs_reference(name):
 
 @pytest.mark.parametrize("mode", MODES)
 def test_embeddings_vs_reference(mode):
-    """Embeddings of every fixture chunk against the reference CAMPPlus (stored), and against the float64 restatement."""
+    """Embeddings of every fixture chunk, from the waveform, against the reference CAMPPlus (stored).  The float64 parity of the
+    forward in every mode is test_campplus_entries_gpu.py's."""
     eng = _engine(mode)
     errs = []
     for name in SPK_CASES:
@@ -192,11 +164,6 @@ def test_embeddings_vs_reference(mode):
         errs.append(rel(emb, g["cb_in"]))
     print("CAM++ %s embeddings: max rel err vs reference %.2e" % (mode, max(errs)))
     assert max(errs) < 1e-3
-    feats = torch.from_numpy(load_spk_case("spk_few_chunks")["features"])
-    ref = campplus_ref(campplus_state_dict(), feats)
-    got = eng.embed_feats(feats.to(DEV))
-    print("CAM++ %s embeddings: rel err vs float64 restatement %.2e" % (mode, rel(got, ref)))
-    assert rel(got, ref) < 1e-3
 
 
 @pytest.mark.parametrize("mode", MODES)
