@@ -45,6 +45,13 @@ bool no_throw(const char* what, F f) {
   }
 }
 
+// the stream's work finished, or "CUDA error: ..." set
+bool sync_stream(cudaStream_t st) {
+  if (cudaStreamSynchronize(st) == cudaSuccess) return true;
+  set_err(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError()));
+  return false;
+}
+
 struct Tensor {
   float* dev = nullptr;              // weights
   std::vector<float> host;           // the payload of the "__" configuration tensors, which stay on the host
@@ -127,7 +134,6 @@ struct Loaded {
   cudaStream_t st = nullptr;
   float* fbank_tables = nullptr;
   bool open(const char* path, int dev) {
-    if (!path) { set_err("model_file is NULL"); return false; }
     if (cudaSetDevice(dev) != cudaSuccess) { cudaGetLastError(); set_err("no such CUDA device (this library has no CPU path)"); return false; }
     device = dev;
     if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) { set_err("cudaStreamCreate failed"); return false; }
@@ -199,17 +205,35 @@ bool upload(const void* const* bufs, const int64_t* n, int B, int64_t stride, in
   return true;
 }
 
+// One model kind's description, run twice: over the file's index (f == nullptr: names and shapes only, nothing touches a device),
+// then over the loaded file.  A file the index pass accepts is refused later only for a device failure.
 struct Builder {
-  Loaded& f;
+  const std::map<std::string, Tensor>& t;
+  Loaded* f;                                         // nullptr: the index pass
   int mode = FA_GEMM_F32_SIMT;
   float ln_eps = 0.f;
-  bool ok = true;
-  const Tensor* get(const std::string& k) {
-    auto it = f.t.find(k);
-    if (it == f.t.end()) { if (ok) set_err("missing tensor " + k); ok = false; return nullptr; }
-    return &it->second;
+  std::string what;                                  // prefix of every message: the model kind or the part being bound
+  bool ok = true;                                    // the first refusal is the one reported
+  bool refuse(const std::string& s) {
+    if (ok) set_err(what + s);
+    ok = false;
+    return false;
   }
-  const float* ptr(const std::string& k) { const Tensor* t = get(k); return t ? t->dev : nullptr; }
+  const Tensor* opt(const std::string& k) const {
+    auto it = t.find(k);
+    return it == t.end() ? nullptr : &it->second;
+  }
+  const Tensor* get(const std::string& k) {
+    const Tensor* x = opt(k);
+    if (!x) refuse("missing tensor " + k);
+    return x;
+  }
+  const Tensor* shaped(const std::string& k, std::initializer_list<int64_t> dims) {
+    const Tensor* x = get(k);
+    if (x && !std::equal(dims.begin(), dims.end(), x->shape.begin(), x->shape.end())) refuse("bad shape of " + k);
+    return x;
+  }
+  const float* ptr(const std::string& k) { const Tensor* x = get(k); return x ? x->dev : nullptr; }   // nullptr on the index
   FaNorm norm(const std::string& p) {
     FaNorm nm{};
     const Tensor* w = get(p + ".weight");
@@ -220,105 +244,137 @@ struct Builder {
     FaLinear L{};
     const Tensor* w = get(weight_key ? std::string(weight_key) : p + ".weight");
     // [out, in] or a k = 1 Conv1d weight [out, in, 1] (bias_output, contextual_paraformer/decoder.py:287)
-    if (!w || !(w->shape.size() == 2 || (w->shape.size() == 3 && w->shape[2] == 1))) { if (ok) set_err("bad weight " + p); ok = false; return L; }
+    if (!w || !(w->shape.size() == 2 || (w->shape.size() == 3 && w->shape[2] == 1))) { if (w) refuse("bad weight " + p); return L; }
     L.w = w->dev; L.b = bias ? ptr(bias_key ? std::string(bias_key) : p + ".bias") : nullptr;
     L.out_f = (int32_t)w->shape[0]; L.in_f = (int32_t)w->shape[1]; L.in_pad = (L.in_f + 63) / 64 * 64;
-    if (mode != FA_GEMM_F32_SIMT) {
+    if (mode != FA_GEMM_F32_SIMT && f) {
       void* planes = nullptr;
-      if (cudaMalloc(&planes, (size_t)3 * L.out_f * L.in_pad * 2) != cudaSuccess) { ok = false; set_err("cudaMalloc planes"); return L; }
-      f.owned.push_back(planes);
-      if (fa_split_planes(L.w, L.in_f, L.out_f, L.in_f, L.in_pad, planes, f.st) != FA_OK) { ok = false; set_err("fa_split_planes failed"); }
+      if (cudaMalloc(&planes, (size_t)3 * L.out_f * L.in_pad * 2) != cudaSuccess) { refuse("cudaMalloc planes"); return L; }
+      f->owned.push_back(planes);
+      if (fa_split_planes(L.w, L.in_f, L.out_f, L.in_f, L.in_pad, planes, f->st) != FA_OK) refuse("fa_split_planes failed");
       L.w_planes = planes;
     }
     return L;
   }
   // the frontend's fbank tables (fa_fbank_make_tables) from frontend.mel_banks and frontend.window
-  bool fbank_tables() {
+  void fbank_tables() {
     const Tensor* mel = get("frontend.mel_banks");
     const Tensor* win = get("frontend.window");
-    if (!mel || !win) return false;
+    if (!mel || !win || !f) return;
     void* tb = nullptr;
-    if (cudaMalloc(&tb, fa_fbank_tables_bytes()) != cudaSuccess) { set_err("cudaMalloc fbank tables"); return false; }
-    f.owned.push_back(tb);
-    f.fbank_tables = static_cast<float*>(tb);
-    if (fa_fbank_make_tables(mel->dev, win->dev, f.fbank_tables, f.st) != FA_OK) { set_err("fa_fbank_make_tables failed"); return false; }
-    return true;
+    if (cudaMalloc(&tb, fa_fbank_tables_bytes()) != cudaSuccess) { refuse("cudaMalloc fbank tables"); return; }
+    f->owned.push_back(tb);
+    f->fbank_tables = static_cast<float*>(tb);
+    if (fa_fbank_make_tables(mel->dev, win->dev, f->fbank_tables, f->st) != FA_OK) refuse("fa_fbank_make_tables failed");
   }
 };
 
-// BiCifParaformer's timestamp head, recognised by predictor.upsample_cnn.weight, on the file's index (no device needed): every
-// tensor the launches read, in the shapes pack.py:timestamp_head_tensors writes, and __ts_config__, whose values go into `head`.
-// A file without the head passes with head.up_times = 0.
-bool check_ts_head(const std::map<std::string, Tensor>& t, FaTimestampHead& head) {
-  head = FaTimestampHead{};
-  if (!t.count("predictor.upsample_cnn.weight")) return true;
-  auto cfg = t.find("__ts_config__");
-  if (cfg == t.end() || cfg->second.host.size() < 3) {
-    set_err("BiCif timestamp head without __ts_config__ (a file packed before the handle read the head): re-pack it with "
-            "funasr_b200.pack.write_model_file");
-    return false;
-  }
-  const float* c = cfg->second.host.data();
-  if (c[0] != 3.f) { set_err("BiCif timestamp head: upsample_times " + std::to_string(c[0]) + " in __ts_config__, only 3 is supported"); return false; }
-  const struct { const char* name; int64_t d0, d1; } need[] = {
-      {"predictor.upsample_cnn.gemm_weight", 3 * 512, 512}, {"predictor.upsample_cnn.gemm_bias", 3 * 512, -1},
-      {"predictor.blstm.ih_gemm_weight", 8 * 512, 512},     {"predictor.blstm.ih_gemm_bias", 8 * 512, -1},
-      {"predictor.blstm.weight_hh_l0", 4 * 512, 512},       {"predictor.blstm.weight_hh_l0_reverse", 4 * 512, 512},
-      {"predictor.cif_output2.weight", 2 * 512, 0},         {"predictor.cif_output2.bias", 1, 0}};
-  for (const auto& n : need) {
-    auto it = t.find(n.name);
-    if (it == t.end()) { set_err(std::string("BiCif timestamp head: missing tensor ") + n.name); return false; }
-    const std::vector<int64_t>& sh = it->second.shape;
-    // d1 > 0: exactly [d0, d1]; d1 < 0: exactly [d0]; d1 == 0: d0 elements in any shape
-    const bool ok = n.d1 > 0 ? (sh.size() == 2 && sh[0] == n.d0 && sh[1] == n.d1) : n.d1 < 0 ? (sh.size() == 1 && sh[0] == n.d0)
-                                                                                          : it->second.numel() == n.d0;
-    if (!ok) { set_err(std::string("BiCif timestamp head: bad shape of ") + n.name); return false; }
-  }
-  head.up_times = 3; head.smooth2 = c[1]; head.noise2 = c[2];
-  return true;
+// fa_offline_init / fa_vad_init / fa_punc_init: build() over the file's index into a throwaway handle (every refusal before any device
+// work, naming the piece), then over the loaded file into the handle returned
+template <typename H>
+H* open_handle(const char* path, int device, int mode, bool (*build)(H&, Builder&)) {
+  if (!path) return fail("model_file is NULL");
+  std::unique_ptr<H> h;
+  const bool ok = no_throw("model file rejected: ", [&] {
+    std::map<std::string, Tensor> index;
+    H probe;
+    Builder on_index{index, nullptr, mode};
+    if (!load_file(index, path, false) || !build(probe, on_index)) return false;
+    h.reset(new H());
+    Builder on_device{h->file.t, &h->file, mode};
+    return h->file.open(path, device) && build(*h, on_device) && sync_stream(h->file.st);
+  });
+  return ok ? h.release() : nullptr;
 }
 
-bool build(Model& m) {
-  Builder b{m.file, m.mode};
-  const Tensor* cfg = b.get("__config__");
-  if (!cfg || cfg->host.size() < 10) { set_err("missing __config__"); return false; }
-  const float* c = cfg->host.data();
-  m.enc_layers = (int)c[0]; m.dec_layers = (int)c[1]; m.d_model = (int)c[2]; m.heads = (int)c[3]; m.kernel = (int)c[4];
-  m.vocab = (int)c[5]; m.feat_dim = (int)c[6]; m.ln_eps = c[7]; m.cif_threshold = c[8]; m.tail_threshold = c[9];
-  if (m.enc_layers < 1 || m.dec_layers < 1 || m.d_model != 512 || m.heads * 128 != m.d_model) { set_err("unsupported config"); return false; }
-  b.ln_eps = m.ln_eps;
-  // the FSMN tap count is read from each stack's own weight [512, 1, K]: encoder and decoder kernel_size are independent
-  // constructor arguments in the reference (sanm/encoder.py:188, paraformer/decoder.py:234 — decoder default 21)
-  auto fsmn_taps = [&](const char* key) -> int {
-    const Tensor* t = b.get(key);
-    return (t && t->shape.size() == 3) ? (int)t->shape[2] : m.kernel;
+// SANMEncoder keeps its first layer (input width -> d_model) apart as encoders0.0 (sanm/encoder.py:188-461); SenseVoice's
+// tp_encoders are one plain list
+std::string enc_layer_prefix(bool tp, int i) {
+  if (tp) return "encoder.tp_encoders." + std::to_string(i);
+  return i == 0 ? "encoder.encoders0.0" : "encoder.encoders." + std::to_string(i - 1);
+}
+
+// A SAN-M stack of n layers over `in` input features into e and L, in the shapes fa_sanm_encoder_forward takes: QKV [3D, in], FSMN
+// [D, 1, K] with layer 0's K in every layer, FFN [F, D] / [D, F] with F <= 2048 (enc_carve's bound).  The main stack takes the
+// position encoding and ends in encoder.after_norm; SenseVoice's tp stack (D in, possibly empty) in encoder.tp_norm.
+void bind_stack(Builder& b, bool tp, int n, int in, int D, int heads, std::vector<FaEncLayer>& L, FaEncoder& e) {
+  auto norm = [&](const std::string& p, int64_t w) {
+    b.shaped(p + ".weight", {w}); b.shaped(p + ".bias", {w});
+    return b.norm(p);
   };
-  if (!b.fbank_tables()) return false;
-  m.cmvn = m.file.t.count("frontend.cmvn") ? m.file.t["frontend.cmvn"].dev : nullptr;
-  // encoder (engine.py:_enc_stack; SANMEncoder encoder.py:188-461)
-  m.enc_l.resize(m.enc_layers);
-  for (int i = 0; i < m.enc_layers; ++i) {
-    const std::string p = i == 0 ? "encoder.encoders0.0" : "encoder.encoders." + std::to_string(i - 1);
-    FaEncLayer& L = m.enc_l[i];
-    L.norm1 = b.norm(p + ".norm1"); L.norm2 = b.norm(p + ".norm2");
-    L.qkv = b.lin(p + ".self_attn.linear_q_k_v"); L.out = b.lin(p + ".self_attn.linear_out");
-    L.fsmn_w = b.ptr(p + ".self_attn.fsmn_block.weight");
-    L.w1 = b.lin(p + ".feed_forward.w_1"); L.w2 = b.lin(p + ".feed_forward.w_2");
+  auto lin = [&](const std::string& p, int64_t out, int64_t k) {
+    b.shaped(p + ".weight", {out, k}); b.shaped(p + ".bias", {out});
+    return b.lin(p);
+  };
+  const Tensor* k0 = n > 0 ? b.get(enc_layer_prefix(tp, 0) + ".self_attn.fsmn_block.weight") : nullptr;
+  const int64_t K = k0 && k0->shape.size() == 3 ? k0->shape[2] : 0;
+  L.assign(n > 0 ? n : 1, FaEncLayer{});
+  for (int i = 0; i < n; ++i) {
+    const std::string p = enc_layer_prefix(tp, i);
+    const int64_t x = i == 0 ? in : D;
+    const Tensor* w1 = b.get(p + ".feed_forward.w_1.weight");
+    const int64_t F = w1 && w1->shape.size() == 2 ? w1->shape[0] : 0;
+    if (w1 && (F < 1 || F > 2048)) b.refuse("bad shape of " + p + ".feed_forward.w_1.weight (at most 2048 units)");
+    L[i].norm1 = norm(p + ".norm1", x); L[i].norm2 = norm(p + ".norm2", D);
+    L[i].qkv = lin(p + ".self_attn.linear_q_k_v", 3 * D, x); L[i].out = lin(p + ".self_attn.linear_out", D, D);
+    b.shaped(p + ".self_attn.fsmn_block.weight", {D, 1, K});
+    L[i].fsmn_w = b.ptr(p + ".self_attn.fsmn_block.weight");
+    L[i].w1 = lin(p + ".feed_forward.w_1", F, D); L[i].w2 = lin(p + ".feed_forward.w_2", D, F);
   }
-  m.enc.layers = m.enc_l.data(); m.enc.n_layers = m.enc_layers; m.enc.heads = m.heads; m.enc.fsmn_k = fsmn_taps("encoder.encoders0.0.self_attn.fsmn_block.weight");
-  m.enc.after_norm = b.norm("encoder.after_norm"); m.enc.pe_inv_timescales = b.ptr("encoder.pe_inv_timescales");
-  // predictor (CifPredictorV2 cif_predictor.py:209-314); conv weight already repacked to [512, 3*512] by pack.py
-  m.pred.conv = b.lin("predictor.cif_conv1d", true, "predictor.cif_conv1d.gemm_weight");
-  m.pred.out_w = b.ptr("predictor.cif_output.weight"); m.pred.out_b = b.ptr("predictor.cif_output.bias");
-  m.pred.threshold = m.cif_threshold; m.pred.tail_threshold = m.tail_threshold; m.pred.smooth_factor = 1.f; m.pred.noise_threshold = 0.f;
-  if (m.ts) {                   // BiCifParaformer: CifPredictorV3's sequential fp32 `cif` (bicif_paraformer/cif_predictor.py:37-84) + its head
-    m.pred.cif_variant = 1;
+  e = FaEncoder{};
+  e.layers = L.data(); e.n_layers = n; e.heads = heads; e.fsmn_k = (int)K;
+  if (n > 0) e.after_norm = norm(tp ? "encoder.tp_norm" : "encoder.after_norm", D);
+  if (!tp) {
+    b.shaped("encoder.pe_inv_timescales", {in / 2});
+    e.pe_inv_timescales = b.ptr("encoder.pe_inv_timescales");
+  }
+}
+
+// A Paraformer file (ParaformerEngine, engine.py): plain, contextual (a hotword bias decoder) or BiCif (a timestamp head)
+bool build_paraformer(Model& m, Builder& b) {
+  m.mode = b.mode;
+  // BiCifParaformer's timestamp head, recognised by predictor.upsample_cnn.weight: the tensors its launches read, in the shapes
+  // pack.py:timestamp_head_tensors writes, and __ts_config__.  Bound first: its refusals come before the rest of the file's.
+  m.ts = b.opt("predictor.upsample_cnn.weight") != nullptr;
+  if (m.ts) {
+    const Tensor* tc = b.opt("__ts_config__");
+    if (!tc || tc->host.size() < 3)
+      return b.refuse("BiCif timestamp head without __ts_config__ (a file packed before the handle read the head): re-pack it with "
+                      "funasr_b200.pack.write_model_file");
+    const float* c = tc->host.data();
+    if (c[0] != 3.f) return b.refuse("BiCif timestamp head: upsample_times " + std::to_string(c[0]) + " in __ts_config__, only 3 is supported");
+    b.what = "BiCif timestamp head: ";
+    b.shaped("predictor.upsample_cnn.gemm_weight", {3 * 512, 512}); b.shaped("predictor.upsample_cnn.gemm_bias", {3 * 512});
+    b.shaped("predictor.blstm.ih_gemm_weight", {8 * 512, 512});     b.shaped("predictor.blstm.ih_gemm_bias", {8 * 512});
+    b.shaped("predictor.blstm.weight_hh_l0", {4 * 512, 512});       b.shaped("predictor.blstm.weight_hh_l0_reverse", {4 * 512, 512});
+    b.shaped("predictor.cif_output2.weight", {1, 2 * 512});         b.shaped("predictor.cif_output2.bias", {1});
     FaTimestampHead& h = m.head;
+    h.up_times = 3; h.smooth2 = c[1]; h.noise2 = c[2];
     h.upsample = b.lin("predictor.upsample_cnn", true, "predictor.upsample_cnn.gemm_weight", "predictor.upsample_cnn.gemm_bias");
     h.blstm_ih = b.lin("predictor.blstm.ih", true, "predictor.blstm.ih_gemm_weight", "predictor.blstm.ih_gemm_bias");
     h.w_hh_fwd = b.ptr("predictor.blstm.weight_hh_l0"); h.w_hh_bwd = b.ptr("predictor.blstm.weight_hh_l0_reverse");
     h.out2_w = b.ptr("predictor.cif_output2.weight"); h.out2_b = b.ptr("predictor.cif_output2.bias");
-    h.threshold = m.cif_threshold;
+    b.what.clear();
+  }
+  const Tensor* cfg = b.opt("__config__");
+  if (!cfg || cfg->host.size() < 10) return b.refuse("missing __config__");
+  const float* c = cfg->host.data();
+  m.enc_layers = (int)c[0]; m.dec_layers = (int)c[1]; m.d_model = (int)c[2]; m.heads = (int)c[3]; m.kernel = (int)c[4];
+  m.vocab = (int)c[5]; m.feat_dim = (int)c[6]; m.ln_eps = c[7]; m.cif_threshold = c[8]; m.tail_threshold = c[9];
+  if (m.enc_layers < 1 || m.dec_layers < 1 || m.d_model != 512 || m.heads * 128 != m.d_model) return b.refuse("unsupported config");
+  b.ln_eps = m.ln_eps;
+  b.fbank_tables();
+  const Tensor* cmvn = b.opt("frontend.cmvn");
+  m.cmvn = cmvn ? cmvn->dev : nullptr;
+  // encoder (engine.py:_enc_stack; SANMEncoder encoder.py:188-461)
+  bind_stack(b, false, m.enc_layers, m.feat_dim, m.d_model, m.heads, m.enc_l, m.enc);
+  // predictor (CifPredictorV2 cif_predictor.py:209-314); conv weight already repacked to [512, 3*512] by pack.py
+  m.pred.conv = b.lin("predictor.cif_conv1d", true, "predictor.cif_conv1d.gemm_weight");
+  m.pred.out_w = b.ptr("predictor.cif_output.weight"); m.pred.out_b = b.ptr("predictor.cif_output.bias");
+  m.pred.threshold = m.cif_threshold; m.pred.tail_threshold = m.tail_threshold; m.pred.smooth_factor = 1.f; m.pred.noise_threshold = 0.f;
+  if (m.ts) {                   // BiCifParaformer: CifPredictorV3's sequential fp32 `cif` (bicif_paraformer/cif_predictor.py:37-84)
+    m.pred.cif_variant = 1;
+    m.head.threshold = m.cif_threshold;
   }
   // decoder (ParaformerSANMDecoder decoder.py:234-449)
   auto dec_layer = [&](FaDecLayer& L, const std::string& p, bool full) {
@@ -332,12 +388,15 @@ bool build(Model& m) {
   };
   // ContextualParaformerDecoder (contextual_paraformer/decoder.py:133-352): the last attention layer is `last_decoder`, plus the
   // hotword branch bias_decoder (norm3 + cross attention) and bias_output (Conv1d 1024 -> 512, k = 1)
-  m.contextual = m.file.t.count("decoder.bias_decoder.norm3.weight") > 0;
+  m.contextual = b.opt("decoder.bias_decoder.norm3.weight") != nullptr;
   const int n_plain = m.contextual ? m.dec_layers - 1 : m.dec_layers;
   m.dec_l.resize(n_plain > 0 ? n_plain : 1);
   for (int i = 0; i < n_plain; ++i) dec_layer(m.dec_l[i], "decoder.decoders." + std::to_string(i), true);
   m.dec.layers = m.dec_l.data(); m.dec.n_layers = n_plain; m.dec.heads = m.heads; m.dec.vocab = m.vocab;
-  m.dec.fsmn_k = fsmn_taps(n_plain > 0 ? "decoder.decoders.0.self_attn.fsmn_block.weight" : "decoder.last_decoder.self_attn.fsmn_block.weight");
+  // the decoder's FSMN tap count is its own: encoder and decoder kernel_size are independent constructor arguments in the reference
+  // (sanm/encoder.py:188, paraformer/decoder.py:234 — decoder default 21)
+  const Tensor* dk = b.get(n_plain > 0 ? "decoder.decoders.0.self_attn.fsmn_block.weight" : "decoder.last_decoder.self_attn.fsmn_block.weight");
+  m.dec.fsmn_k = dk && dk->shape.size() == 3 ? (int)dk->shape[2] : m.kernel;
   dec_layer(m.dec.last, "decoder.decoders3.0", false);
   m.dec.after_norm = b.norm("decoder.after_norm"); m.dec.output = b.lin("decoder.output_layer");
   m.dec.has_bias = 0;
@@ -349,8 +408,7 @@ bool build(Model& m) {
     m.dec.bias_output = b.lin("decoder.bias_output", false);
     m.dec.clas_scale = 1.0f;
   }
-  if (!b.ok) return false;
-  return cudaStreamSynchronize(m.file.st) == cudaSuccess;
+  return b.ok;
 }
 
 int num_lfr_frames(int64_t n) {       // wav_frontend.py:73 after kaldi.py snip_edges framing
@@ -400,7 +458,7 @@ std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride,
   r->ts = m.ts;
   if (m.ts) r->stamps.resize(B);
   cudaMemcpyAsync(r->token_num.data(), m.tok.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st);
-  if (cudaStreamSynchronize(st) != cudaSuccess) return fail(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError()));
+  if (!sync_stream(st)) return nullptr;
   int n_max = 0;                                             // the path's one host sync (cif_predictor.py:311)
   for (int i = 0; i < B; ++i) n_max = r->token_num[i] > n_max ? r->token_num[i] : n_max;
   r->ids.resize(B);
@@ -446,7 +504,7 @@ std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride,
     cudaMemcpyAsync(us_alphas.data(), m.us_alphas.p, (size_t)rows_up * 4, cudaMemcpyDeviceToHost, st);
     cudaMemcpyAsync(us_peaks.data(), m.us_peaks.p, (size_t)rows_up * 4, cudaMemcpyDeviceToHost, st);
   }
-  if (cudaStreamSynchronize(st) != cudaSuccess) return fail(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError()));
+  if (!sync_stream(st)) return nullptr;
   for (int i = 0; i < B; ++i) r->ids[i].assign(fids.begin() + (size_t)i * n_max, fids.begin() + (size_t)i * n_max + fl[i]);
   if (m.ts) {                                                // bicif_paraformer/model.py:402-407: each utterance's first 3 * enc_len frames
     for (int i = 0; i < B; ++i) {
@@ -466,86 +524,42 @@ std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride,
 enum { kSvEnc = 0, kSvTp, kSvDModel, kSvHeads, kSvKernel, kSvVocab, kSvFeat, kSvEps, kSvBlank, kSvCfgLen };
 const int32_t kSvAuto = 0, kSvWoItn = 15;             // SenseVoiceSmall.inference's defaults: language "auto", text norm "woitn"
 
-std::string sv_layer(bool tp, int i) {
-  return tp ? "encoder.tp_encoders." + std::to_string(i) : i == 0 ? "encoder.encoders0.0" : "encoder.encoders." + std::to_string(i - 1);
-}
-
-// everything the file's index decides (configuration, every tensor the chain reads, the shapes the kernels take), before any device work
-bool check_sv(const std::map<std::string, Tensor>& t, Model& m) {
-  auto need = [&](const std::string& k) -> const Tensor* {
-    auto it = t.find(k);
-    if (it == t.end()) { set_err("SenseVoice model: missing tensor " + k); return nullptr; }
-    return &it->second;
-  };
-  if (t.count("__config__")) { set_err("SenseVoice model: the file carries both __config__ (Paraformer) and __sv_config__"); return false; }
-  const Tensor* cfg = need("__sv_config__");
+// SenseVoiceEngine of engine.py: the same weights, the same planes per gemm_mode
+bool build_sv(Model& m, Builder& b) {
+  m.mode = b.mode;
+  b.what = "SenseVoice model: ";
+  if (b.opt("__config__")) return b.refuse("the file carries both __config__ (Paraformer) and __sv_config__");
+  const Tensor* cfg = b.get("__sv_config__");
   if (!cfg) return false;
-  if (cfg->host.size() != kSvCfgLen) { set_err("SenseVoice model: bad __sv_config__"); return false; }
+  if (cfg->host.size() != kSvCfgLen) return b.refuse("bad __sv_config__");
   const float* c = cfg->host.data();
   m.enc_layers = (int)c[kSvEnc]; m.tp_layers = (int)c[kSvTp]; m.d_model = (int)c[kSvDModel]; m.heads = (int)c[kSvHeads];
   m.kernel = (int)c[kSvKernel]; m.vocab = (int)c[kSvVocab]; m.feat_dim = (int)c[kSvFeat]; m.ln_eps = c[kSvEps]; m.blank = (int)c[kSvBlank];
-  if (m.enc_layers < 1 || m.tp_layers < 0) { set_err("SenseVoice model: no encoder layer"); return false; }
-  if (m.d_model != 512 || m.heads != 4) {
-    set_err("SenseVoice model: d_model " + std::to_string(m.d_model) + " with " + std::to_string(m.heads) +
-            " heads (the tensor-core attention runs d_model 512 as 4 heads of 128)");
-    return false;
-  }
-  if (m.vocab < 1 || m.vocab > 61440) {
-    set_err("SenseVoice model: vocabulary of " + std::to_string(m.vocab) + " tokens (the CTC arg-max takes at most 61440)");
-    return false;
-  }
-  if (m.feat_dim != 560) { set_err("SenseVoice model: feat_dim " + std::to_string(m.feat_dim) + " (the frontend is 80 mel x LFR 7 = 560)"); return false; }
-  if (m.blank < 0 || m.blank >= m.vocab) { set_err("SenseVoice model: blank_id outside the vocabulary"); return false; }
-  std::vector<std::string> names = {"frontend.mel_banks", "frontend.window", "encoder.pe_inv_timescales", "encoder.after_norm.weight",
-                                    "encoder.after_norm.bias", "ctc.ctc_lo.bias"};
-  if (m.tp_layers > 0) names.insert(names.end(), {"encoder.tp_norm.weight", "encoder.tp_norm.bias"});
-  const char* layer_keys[] = {".norm1.weight", ".norm1.bias", ".norm2.weight", ".norm2.bias", ".self_attn.linear_q_k_v.weight",
-                              ".self_attn.linear_q_k_v.bias", ".self_attn.linear_out.weight", ".self_attn.linear_out.bias",
-                              ".self_attn.fsmn_block.weight", ".feed_forward.w_1.weight", ".feed_forward.w_1.bias", ".feed_forward.w_2.weight",
-                              ".feed_forward.w_2.bias"};
-  for (int s = 0; s < 2; ++s)
-    for (int i = 0; i < (s ? m.tp_layers : m.enc_layers); ++i)
-      for (const char* k : layer_keys) names.push_back(sv_layer(s == 1, i) + k);
-  for (const std::string& n : names)
-    if (!need(n)) return false;
-  const Tensor* ctc = need("ctc.ctc_lo.weight");
-  const Tensor* emb = ctc ? need("embed.weight") : nullptr;
+  if (m.enc_layers < 1 || m.tp_layers < 0) return b.refuse("no encoder layer");
+  if (m.d_model != 512 || m.heads != 4)
+    return b.refuse("d_model " + std::to_string(m.d_model) + " with " + std::to_string(m.heads) +
+                    " heads (the tensor-core attention runs d_model 512 as 4 heads of 128)");
+  if (m.vocab < 1 || m.vocab > 61440)
+    return b.refuse("vocabulary of " + std::to_string(m.vocab) + " tokens (the CTC arg-max takes at most 61440)");
+  if (m.feat_dim != 560) return b.refuse("feat_dim " + std::to_string(m.feat_dim) + " (the frontend is 80 mel x LFR 7 = 560)");
+  if (m.blank < 0 || m.blank >= m.vocab) return b.refuse("blank_id outside the vocabulary");
+  b.ln_eps = m.ln_eps;
+  b.fbank_tables();
+  const Tensor* cmvn = b.opt("frontend.cmvn");
+  if (cmvn && cmvn->numel() != 2 * m.feat_dim) return b.refuse("frontend.cmvn must be [2, 560]");
+  m.cmvn = cmvn ? cmvn->dev : nullptr;
+  bind_stack(b, false, m.enc_layers, m.feat_dim, m.d_model, m.heads, m.enc_l, m.enc);
+  bind_stack(b, true, m.tp_layers, m.d_model, m.d_model, m.heads, m.tp_l, m.tp);
+  const Tensor* ctc = b.get("ctc.ctc_lo.weight");
+  if (ctc && ctc->shape != std::vector<int64_t>{m.vocab, m.d_model}) return b.refuse("bad shape of ctc.ctc_lo.weight (want [vocab, 512])");
+  m.ctc = b.lin("ctc.ctc_lo");
+  const Tensor* emb = b.get("embed.weight");
   if (!emb) return false;
-  if (ctc->shape != std::vector<int64_t>{(int64_t)m.vocab, (int64_t)m.d_model}) { set_err("SenseVoice model: bad shape of ctc.ctc_lo.weight (want [vocab, 512])"); return false; }
-  if (emb->shape.size() != 2 || emb->shape[0] < 3 || emb->shape[1] != m.feat_dim) { set_err("SenseVoice model: bad shape of embed.weight (want [>= 3, 560])"); return false; }
-  auto cm = t.find("frontend.cmvn");
-  if (cm != t.end() && cm->second.numel() != 2 * m.feat_dim) { set_err("SenseVoice model: frontend.cmvn must be [2, 560]"); return false; }
+  if (emb->shape.size() != 2 || emb->shape[0] < 3 || emb->shape[1] != m.feat_dim) return b.refuse("bad shape of embed.weight (want [>= 3, 560])");
+  m.embed = emb->dev;
   m.n_embed = (int)emb->shape[0];
   m.sv = true;
-  return true;
-}
-
-// the SenseVoiceEngine of engine.py: the same weights, the same planes per gemm_mode
-bool build_sv(Model& m) {
-  Builder b{m.file, m.mode};
-  b.ln_eps = m.ln_eps;
-  if (!b.fbank_tables()) return false;
-  m.cmvn = m.file.t.count("frontend.cmvn") ? m.file.t["frontend.cmvn"].dev : nullptr;
-  auto stack = [&](bool tp, int n, std::vector<FaEncLayer>& L, FaEncoder& e) {
-    L.resize(n > 0 ? n : 1);
-    for (int i = 0; i < n; ++i) {
-      const std::string p = sv_layer(tp, i);
-      L[i].norm1 = b.norm(p + ".norm1"); L[i].norm2 = b.norm(p + ".norm2");
-      L[i].qkv = b.lin(p + ".self_attn.linear_q_k_v"); L[i].out = b.lin(p + ".self_attn.linear_out");
-      L[i].fsmn_w = b.ptr(p + ".self_attn.fsmn_block.weight");
-      L[i].w1 = b.lin(p + ".feed_forward.w_1"); L[i].w2 = b.lin(p + ".feed_forward.w_2");
-    }
-    const Tensor* fw = n > 0 ? b.get(sv_layer(tp, 0) + ".self_attn.fsmn_block.weight") : nullptr;
-    e.layers = L.data(); e.n_layers = n; e.heads = m.heads; e.fsmn_k = fw && !fw->shape.empty() ? (int)fw->shape.back() : m.kernel;
-    if (n > 0) e.after_norm = b.norm(tp ? "encoder.tp_norm" : "encoder.after_norm");
-    e.pe_inv_timescales = tp ? nullptr : b.ptr("encoder.pe_inv_timescales");    // the tp blocks take no position encoding
-  };
-  stack(false, m.enc_layers, m.enc_l, m.enc);
-  stack(true, m.tp_layers, m.tp_l, m.tp);
-  m.ctc = b.lin("ctc.ctc_lo");
-  m.embed = b.ptr("embed.weight");
-  if (!b.ok) return false;
-  return cudaStreamSynchronize(m.file.st) == cudaSuccess;
+  return b.ok;
 }
 
 // every query id inside the embedding table; `what` names the unit ("utterance", "recording")
@@ -608,7 +622,7 @@ std::unique_ptr<Result> decode_sv(Model& m, const float* wav, int64_t stride, co
   std::vector<int32_t> ids(rows);
   cudaMemcpyAsync(ids.data(), m.ids.p, rows * 4, cudaMemcpyDeviceToHost, st);
   cudaMemcpyAsync(r->token_num.data(), m.flens_out.p, (size_t)B * 4, cudaMemcpyDeviceToHost, st);
-  if (cudaStreamSynchronize(st) != cudaSuccess) return fail(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError()));
+  if (!sync_stream(st)) return nullptr;
   for (int i = 0; i < B; ++i) r->ids[i].assign(ids.begin() + (size_t)i * T, ids.begin() + (size_t)i * T + r->token_num[i]);
   return r;
 }
@@ -641,6 +655,9 @@ void* infer_batch(void* handle, const void* const* bufs, const int64_t* n_sample
   return decode_pack(m, static_cast<const float*>(m.wav.p), stride, lens_h, hw_embed, n_hotwords, lang, tn).release();
 }
 
+// the model kind is the file's: SenseVoiceSmall by __sv_config__, Paraformer otherwise
+bool build_offline(Model& m, Builder& b) { return b.opt("__sv_config__") ? build_sv(m, b) : build_paraformer(m, b); }
+
 }  // namespace
 
 extern "C" const char* fa_offline_last_error(void) { return g_err.c_str(); }
@@ -651,18 +668,7 @@ extern "C" void* fa_offline_init(const char* model_file, int32_t device, int32_t
   g_err.clear();
   if (!model_file) return fail("model_file is NULL");
   if (gemm_mode != FA_GEMM_F32_SIMT && gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) return fail("bad gemm_mode");
-  FaTimestampHead head{};
-  std::unique_ptr<Model> m(new Model());
-  // what the file's index alone decides (the model kind, SenseVoice's configuration and tensors, the timestamp head) is refused before
-  // any device work
-  std::map<std::string, Tensor> index;
-  if (!no_throw("model file rejected: ", [&] {
-        return load_file(index, model_file, false) && (index.count("__sv_config__") ? check_sv(index, *m) : check_ts_head(index, head));
-      }))
-    return nullptr;
-  m->mode = gemm_mode; m->head = head; m->ts = head.up_times > 0;
-  if (!no_throw("model file rejected: ", [&] { return m->file.open(model_file, device) && (m->sv ? build_sv(*m) : build(*m)); })) return nullptr;
-  return m.release();
+  return open_handle(model_file, device, gemm_mode, build_offline);
 }
 
 extern "C" int32_t fa_offline_is_sensevoice(const void* handle) { return handle && static_cast<const Model*>(handle)->sv ? 1 : 0; }
@@ -753,11 +759,10 @@ struct VadResult {
   float audio_seconds = 0.f;
 };
 
-bool build_vad(Vad& v) {
-  Builder b{v.file};
+bool build_vad(Vad& v, Builder& b) {
   const Tensor* cfg = b.get("__vad_config__");
   if (!cfg) return false;
-  if (cfg->host.size() != 2 * kVadCfgLen) { set_err("bad __vad_config__"); return false; }
+  if (cfg->host.size() != 2 * kVadCfgLen) return b.refuse("bad __vad_config__");
   double c[kVadCfgLen];
   memcpy(c, cfg->host.data(), sizeof(c));
   int32_t* oi = &v.opts.sample_rate;                 // the 14 int32 fields, in declaration order
@@ -765,50 +770,45 @@ bool build_vad(Vad& v) {
   v.opts.speech_2_noise_ratio = c[14]; v.opts.snr_thres = c[15]; v.opts.decibel_thres = c[16]; v.opts.speech_noise_thres = c[17];
   v.opts.fe_prior_thres = c[18];
   const int lorder = (int)c[kVadCfgLorder], n_sil = (int)c[kVadCfgNSil];
-  if (lorder != 20 || n_sil < 1 || n_sil > 4 || v.opts.frame_in_ms <= 0 || v.opts.window_size_ms < v.opts.frame_in_ms) {
-    set_err("unsupported VAD config"); return false;
-  }
-  if (!b.fbank_tables()) return false;
-  if (v.file.t.count("frontend.cmvn")) {
-    if (v.file.t["frontend.cmvn"].numel() != 2 * 400) { set_err("frontend.cmvn must be [2, 400]"); return false; }
-    v.cmvn = v.file.t["frontend.cmvn"].dev;
-  }
+  if (lorder != 20 || n_sil < 1 || n_sil > 4 || v.opts.frame_in_ms <= 0 || v.opts.window_size_ms < v.opts.frame_in_ms)
+    return b.refuse("unsupported VAD config");
+  b.fbank_tables();
+  const Tensor* cmvn = b.opt("frontend.cmvn");
+  if (cmvn && cmvn->numel() != 2 * 400) return b.refuse("frontend.cmvn must be [2, 400]");
+  v.cmvn = cmvn ? cmvn->dev : nullptr;
   // weights [out, in] -> [out, in rounded up to 16] with zero columns (VadEngine._lin): the fp32 GEMMs read K = the padded width
   auto lin = [&](const std::string& p, bool bias) -> FaLinear {
     FaLinear L{};
     const Tensor* w = b.get(p + ".weight");
-    if (!w || w->shape.size() != 2) { if (b.ok && w) set_err("bad weight " + p); b.ok = false; return L; }
+    if (!w || w->shape.size() != 2) { if (w) b.refuse("bad weight " + p); return L; }
     const int out_f = (int)w->shape[0], in_f = (int)w->shape[1], kp = (in_f + 15) / 16 * 16;
-    void* wp = nullptr;
-    if (cudaMalloc(&wp, (size_t)out_f * kp * 4) != cudaSuccess) { set_err("cudaMalloc weights"); b.ok = false; return L; }
-    v.file.owned.push_back(wp);
-    if (cudaMemset(wp, 0, (size_t)out_f * kp * 4) != cudaSuccess ||
-        cudaMemcpy2D(wp, (size_t)kp * 4, w->dev, (size_t)in_f * 4, (size_t)in_f * 4, out_f, cudaMemcpyDeviceToDevice) != cudaSuccess) {
-      set_err("weight copy failed"); b.ok = false; return L;
-    }
-    L.w = static_cast<const float*>(wp);
-    if (bias) {
-      const Tensor* bt = b.get(p + ".bias");
-      if (!bt || bt->numel() != out_f) { if (b.ok && bt) set_err("bad bias " + p); b.ok = false; return L; }
-      L.b = bt->dev;
-    }
+    const Tensor* bt = bias ? b.get(p + ".bias") : nullptr;
+    if (bt && bt->numel() != out_f) b.refuse("bad bias " + p);
+    if (!b.ok) return L;
+    L.b = bt ? bt->dev : nullptr;
     L.out_f = out_f; L.in_f = kp; L.in_pad = kp;
+    if (!b.f) return L;
+    void* wp = nullptr;
+    if (cudaMalloc(&wp, (size_t)out_f * kp * 4) != cudaSuccess) { b.refuse("cudaMalloc weights"); return L; }
+    b.f->owned.push_back(wp);
+    if (cudaMemset(wp, 0, (size_t)out_f * kp * 4) != cudaSuccess ||
+        cudaMemcpy2D(wp, (size_t)kp * 4, w->dev, (size_t)in_f * 4, (size_t)in_f * 4, out_f, cudaMemcpyDeviceToDevice) != cudaSuccess)
+      b.refuse("weight copy failed");
+    L.w = static_cast<const float*>(wp);
     return L;
   };
   int n_layers = 0;
-  while (v.file.t.count("encoder.fsmn." + std::to_string(n_layers) + ".linear.linear.weight")) ++n_layers;
+  while (b.opt("encoder.fsmn." + std::to_string(n_layers) + ".linear.linear.weight")) ++n_layers;
   v.layers.resize(n_layers > 0 ? n_layers : 1);
   v.enc.in1 = lin("encoder.in_linear1.linear", true);
   v.enc.in2 = lin("encoder.in_linear2.linear", true);
   for (int i = 0; i < n_layers && b.ok; ++i) {
     const std::string p = "encoder.fsmn." + std::to_string(i) + ".";
-    if (v.file.t.count(p + "fsmn_block.conv_right.weight")) { set_err("FSMN-VAD with a right-context memory (rorder > 0) is not supported"); return false; }
+    if (b.opt(p + "fsmn_block.conv_right.weight")) return b.refuse("FSMN-VAD with a right-context memory (rorder > 0) is not supported");
     v.layers[i].lin = lin(p + "linear.linear", false);
     const Tensor* cw = b.get(p + "fsmn_block.conv_left.weight");   // [proj, 1, lorder, 1] = [proj, lorder] contiguous
-    if (!cw || cw->shape.size() != 4 || cw->shape[1] != 1 || cw->shape[2] != lorder || cw->shape[3] != 1) {
-      if (b.ok && cw) set_err("bad " + p + "fsmn_block.conv_left.weight");
-      return false;
-    }
+    if (!cw) return false;
+    if (cw->shape.size() != 4 || cw->shape[1] != 1 || cw->shape[2] != lorder || cw->shape[3] != 1) return b.refuse("bad " + p + "fsmn_block.conv_left.weight");
     v.layers[i].conv_w = cw->dev;
     v.layers[i].affine = lin(p + "affine.linear", true);
   }
@@ -818,10 +818,10 @@ bool build_vad(Vad& v) {
   for (int k = 0; k < n_sil; ++k) v.enc.sil_ids[k] = (int32_t)c[kVadCfgSil + k];
   v.enc.n_sil = n_sil;
   if (!b.ok) return false;
-  if (v.enc.in1.in_f != 400) { set_err("the VAD frontend is 80 mel x LFR 5: in_linear1 must take 400 inputs"); return false; }
+  if (v.enc.in1.in_f != 400) return b.refuse("the VAD frontend is 80 mel x LFR 5: in_linear1 must take 400 inputs");
   for (int k = 0; k < n_sil; ++k)
-    if (v.enc.sil_ids[k] < 0 || v.enc.sil_ids[k] >= v.enc.out2.out_f) { set_err("sil_pdf_ids outside the output"); return false; }
-  return cudaStreamSynchronize(v.file.st) == cudaSuccess;
+    if (v.enc.sil_ids[k] < 0 || v.enc.sil_ids[k] >= v.enc.out2.out_f) return b.refuse("sil_pdf_ids outside the output");
+  return true;
 }
 
 const double kSilenceSchedule[] = {10000, 2000, 20000, 1000, 30000, 800, 40000, 600, 50000, 400, 60000, 200, -1, 100};   // vad.py
@@ -846,7 +846,7 @@ bool vad_run(Vad& v, const float* wav, int64_t n, cudaStream_t st, const FaVadRu
   if (rc == FA_OK) rc = fa_frame_decibels(wav, n, (int32_t)T, frames + T, st);
   if (rc != FA_OK) { set_err(std::string("VAD: ") + fa_status_string(rc)); return false; }
   cudaMemcpyAsync(out.frames.data(), frames, (size_t)T * 8, cudaMemcpyDeviceToHost, st);     // the one copy back: two floats per frame
-  if (cudaStreamSynchronize(st) != cudaSuccess) { set_err(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError())); return false; }
+  if (!sync_stream(st)) return false;
   std::vector<double> sil(out.frames.begin(), out.frames.begin() + T), db(out.frames.begin() + T, out.frames.end());
   FaVadOptions o = v.opts;
   if (!ro.dynamic_silence && ro.max_end_silence_time > 0) o.max_end_silence_time = ro.max_end_silence_time;
@@ -908,9 +908,7 @@ extern "C" int fa_gather_segments(const float* rec, int64_t n_rec, const int64_t
 
 extern "C" void* fa_vad_init(const char* model_file, int32_t device) {
   g_err.clear();
-  std::unique_ptr<Vad> v(new Vad());
-  if (!no_throw("model file rejected: ", [&] { return v->file.open(model_file, device) && build_vad(*v); })) return nullptr;
-  return v.release();
+  return open_handle(model_file, device, FA_GEMM_F32_SIMT, build_vad);
 }
 
 extern "C" void fa_vad_uninit(void* vad) { delete static_cast<Vad*>(vad); }
@@ -1112,85 +1110,38 @@ std::vector<std::string> blob_lines(const Tensor& t) {
   return out;
 }
 
-std::string layer_prefix(int i) { return i == 0 ? "encoder.encoders0.0" : "encoder.encoders." + std::to_string(i - 1); }
-
-// everything the file's index decides (configuration, lists, every tensor and the shapes the kernels take), before any device work
-bool check_punc(const std::map<std::string, Tensor>& t, Punc& p) {
-  auto get = [&](const std::string& k) -> const Tensor* {
-    auto it = t.find(k);
-    if (it == t.end()) { set_err("punctuation model: missing tensor " + k); return nullptr; }
-    return &it->second;
-  };
-  auto shaped = [&](const std::string& k, std::initializer_list<int64_t> dims) -> const Tensor* {
-    const Tensor* x = get(k);
-    if (x && !std::equal(dims.begin(), dims.end(), x->shape.begin(), x->shape.end())) { set_err("punctuation model: bad shape of " + k); return nullptr; }
-    return x;
-  };
-  const Tensor* cfg = get("__punc_config__");
-  const Tensor* pl = get("__punc_list__");
-  const Tensor* tl = cfg && pl ? get("__punc_tokens__") : nullptr;
+bool build_punc(Punc& p, Builder& b) {
+  b.what = "punctuation model: ";
+  b.ln_eps = 1e-12f;                                 // SANMEncoder's LayerNorm; the fp32 path whatever the recogniser's gemm-mode (PuncEngine)
+  const Tensor* cfg = b.get("__punc_config__");
+  const Tensor* pl = b.get("__punc_list__");
+  const Tensor* tl = cfg && pl ? b.get("__punc_tokens__") : nullptr;
   if (!tl) return false;
-  if (cfg->host.size() != kPuncCfgLen) { set_err("punctuation model: bad __punc_config__"); return false; }
+  if (cfg->host.size() != kPuncCfgLen) return b.refuse("bad __punc_config__");
   const float* c = cfg->host.data();
   p.layers = (int)c[kPuncLayers]; p.d_model = (int)c[kPuncDModel]; p.heads = (int)c[kPuncHeads];
   const int D = p.d_model, K = (int)c[kPuncKernel];
-  if (p.layers < 1) { set_err("punctuation model: no encoder layer"); return false; }
-  if (K != 11 && K != 21 && K != 31) { set_err("punctuation model: FSMN kernel " + std::to_string(K) + " (the fp32 FSMN kernel takes 11, 21 or 31)"); return false; }
-  if (D > 512 || D < 64 || D % 16) { set_err("punctuation model: d_model " + std::to_string(D) + " (the encoder takes a multiple of 16 up to 512)"); return false; }
+  if (p.layers < 1) return b.refuse("no encoder layer");
+  if (K != 11 && K != 21 && K != 31) return b.refuse("FSMN kernel " + std::to_string(K) + " (the fp32 FSMN kernel takes 11, 21 or 31)");
+  if (D > 512 || D < 64 || D % 16) return b.refuse("d_model " + std::to_string(D) + " (the encoder takes a multiple of 16 up to 512)");
   const int hd = p.heads > 0 && D % p.heads == 0 ? D / p.heads : 0;
-  if (hd < 32 || hd > 128 || hd % 32) {
-    set_err("punctuation model: " + std::to_string(p.heads) + " heads of d_model " + std::to_string(D) + " (the head dim must be a multiple of 32 up to 128)");
-    return false;
-  }
+  if (hd < 32 || hd > 128 || hd % 32)
+    return b.refuse(std::to_string(p.heads) + " heads of d_model " + std::to_string(D) + " (the head dim must be a multiple of 32 up to 128)");
   std::string err;
-  if (!p.vocab.init(blob_lines(*tl), blob_lines(*pl), (int32_t)c[kPuncSentenceEnd], (int32_t)c[kPuncSplit], err)) { set_err("punctuation model: " + err); return false; }
-  const Tensor* emb = get("embed.weight");
+  if (!p.vocab.init(blob_lines(*tl), blob_lines(*pl), (int32_t)c[kPuncSentenceEnd], (int32_t)c[kPuncSplit], err)) return b.refuse(err);
+  const Tensor* emb = b.get("embed.weight");
   if (!emb) return false;
-  if (emb->shape.size() != 2 || emb->shape[1] > 560 || emb->shape[1] % 16 || emb->shape[0] < 1) { set_err("punctuation model: bad shape of embed.weight"); return false; }
+  if (emb->shape.size() != 2 || emb->shape[1] > 560 || emb->shape[1] % 16 || emb->shape[0] < 1) return b.refuse("bad shape of embed.weight");
   p.n_embed = (int)emb->shape[0]; p.d_in = (int)emb->shape[1];
-  if (!shaped("encoder.pe_inv_timescales", {p.d_in / 2})) return false;
-  for (int i = 0; i < p.layers; ++i) {
-    const std::string q = layer_prefix(i);
-    const int in = i == 0 ? p.d_in : D;
-    const Tensor* w1 = get(q + ".feed_forward.w_1.weight");
-    if (!w1) return false;
-    const int64_t F = w1->shape.size() == 2 ? w1->shape[0] : 0;
-    if (F < 1 || F > 2048) { set_err("punctuation model: bad shape of " + q + ".feed_forward.w_1.weight (at most 2048 units)"); return false; }
-    if (!(shaped(q + ".norm1.weight", {in}) && shaped(q + ".norm1.bias", {in}) && shaped(q + ".norm2.weight", {D}) && shaped(q + ".norm2.bias", {D}) &&
-          shaped(q + ".self_attn.linear_q_k_v.weight", {3 * D, in}) && shaped(q + ".self_attn.linear_q_k_v.bias", {3 * D}) &&
-          shaped(q + ".self_attn.linear_out.weight", {D, D}) && shaped(q + ".self_attn.linear_out.bias", {D}) &&
-          shaped(q + ".self_attn.fsmn_block.weight", {D, 1, K}) && shaped(q + ".feed_forward.w_1.weight", {F, D}) &&
-          shaped(q + ".feed_forward.w_1.bias", {F}) && shaped(q + ".feed_forward.w_2.weight", {D, F}) && shaped(q + ".feed_forward.w_2.bias", {D})))
-      return false;
-  }
-  if (t.count("encoder.encoders." + std::to_string(p.layers - 1) + ".norm1.weight")) { set_err("punctuation model: more encoder layers than __punc_config__ says"); return false; }
+  p.embed = emb->dev;
+  b.shaped(enc_layer_prefix(false, 0) + ".self_attn.fsmn_block.weight", {D, 1, K});     // bind_stack holds every layer to layer 0's taps
+  bind_stack(b, false, p.layers, p.d_in, D, p.heads, p.enc_l, p.enc);
+  if (b.opt(enc_layer_prefix(false, p.layers) + ".norm1.weight")) return b.refuse("more encoder layers than __punc_config__ says");
   const int64_t n_punc = (int64_t)p.vocab.punc.size();
-  if (!(shaped("encoder.after_norm.weight", {D}) && shaped("encoder.after_norm.bias", {D}) && shaped("decoder.weight", {n_punc, D}) &&
-        shaped("decoder.bias", {n_punc})))
-    return false;
-  p.max_window = hd == 128 ? 0 : 160 * 1024 / 16;     // fa_attention_f32_ex's warp-per-query kernel: 4 * tk floats of shared memory
-  return true;
-}
-
-bool build_punc(Punc& p) {
-  Builder b{p.file};                                 // the fp32 path whatever the recogniser's gemm-mode (PuncEngine)
-  b.ln_eps = 1e-12f;                                 // SANMEncoder's LayerNorm
-  p.enc_l.resize(p.layers);
-  for (int i = 0; i < p.layers; ++i) {
-    const std::string q = layer_prefix(i);
-    FaEncLayer& L = p.enc_l[i];
-    L.norm1 = b.norm(q + ".norm1"); L.norm2 = b.norm(q + ".norm2");
-    L.qkv = b.lin(q + ".self_attn.linear_q_k_v"); L.out = b.lin(q + ".self_attn.linear_out");
-    L.fsmn_w = b.ptr(q + ".self_attn.fsmn_block.weight");
-    L.w1 = b.lin(q + ".feed_forward.w_1"); L.w2 = b.lin(q + ".feed_forward.w_2");
-  }
-  p.enc.layers = p.enc_l.data(); p.enc.n_layers = p.layers; p.enc.heads = p.heads;
-  p.enc.fsmn_k = (int)p.file.t["encoder.encoders0.0.self_attn.fsmn_block.weight"].shape[2];
-  p.enc.after_norm = b.norm("encoder.after_norm"); p.enc.pe_inv_timescales = b.ptr("encoder.pe_inv_timescales");
+  b.shaped("decoder.weight", {n_punc, D}); b.shaped("decoder.bias", {n_punc});
   p.out = b.lin("decoder");
-  p.embed = b.ptr("embed.weight");
-  if (!b.ok) return false;
-  return cudaStreamSynchronize(p.file.st) == cudaSuccess;
+  p.max_window = hd == 128 ? 0 : 160 * 1024 / 16;     // fa_attention_f32_ex's warp-per-query kernel: 4 * tk floats of shared memory
+  return b.ok;
 }
 
 // one lockstep step on the GPU: punc_forward (model.py:112-125) + arg-max over a padded batch of windows
@@ -1217,7 +1168,7 @@ bool punc_step(Punc& p, const int32_t* ids, const int32_t* lens, int32_t B, int3
                           p.ws.cap, st);
   if (rc != FA_OK) { err = std::string("punctuation forward: ") + fa_status_string(rc); return false; }
   cudaMemcpyAsync(punc_out, p.pids.p, (size_t)M * 4, cudaMemcpyDeviceToHost, st);
-  if (cudaStreamSynchronize(st) != cudaSuccess) { err = std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError()); return false; }
+  if (!sync_stream(st)) { err = g_err; return false; }
   return true;
 }
 
@@ -1225,12 +1176,7 @@ bool punc_step(Punc& p, const int32_t* ids, const int32_t* lens, int32_t B, int3
 
 extern "C" void* fa_punc_init(const char* model_file, int32_t device) {
   g_err.clear();
-  if (!model_file) return fail("model_file is NULL");
-  std::unique_ptr<Punc> p(new Punc());
-  std::map<std::string, Tensor> index;          // refused on the file's index alone, before any device work
-  if (!no_throw("model file rejected: ", [&] { return load_file(index, model_file, false) && check_punc(index, *p); })) return nullptr;
-  if (!no_throw("model file rejected: ", [&] { return p->file.open(model_file, device) && build_punc(*p); })) return nullptr;
-  return p.release();
+  return open_handle(model_file, device, FA_GEMM_F32_SIMT, build_punc);
 }
 
 extern "C" void fa_punc_uninit(void* punc) { delete static_cast<Punc*>(punc); }

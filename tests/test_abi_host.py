@@ -218,6 +218,44 @@ def test_offline_api_rejects_bad_arguments_without_a_gpu():
     assert lib.fa_offline_result_count(None) == 0
 
 
+def test_paraformer_init_refusals_name_the_piece_without_a_device(tmp_path):
+    """A Paraformer file is checked on its index alone, before any device work: a refusal names the piece on any machine, and a
+    well-formed plain, contextual or BiCif file fails only for want of a device (or opens where there is one)."""
+    from funasr_b200 import pack
+    lib = _abi.load()
+    cfg = synth.PARAFORMER_TINY
+    plain, ctx = synth.make_state_dict(cfg, 3), synth.make_contextual_state_dict(cfg, 6)
+
+    def init(state, edit=lambda t: None):
+        t = pack.model_tensors(state, cfg, None)
+        edit(t)
+        path = str(tmp_path / "p.fab2")
+        pack._write(path, t)
+        h = lib.fa_offline_init(path.encode(), 0, _abi.GEMM_MODES["fp16x3"])
+        return h, lib.fa_offline_last_error().decode()
+
+    def refused(state, edit):
+        h, msg = init(state, edit)
+        assert not h
+        return msg
+
+    def d_model_768(t):
+        t["__config__"] = t["__config__"].copy()
+        t["__config__"][2] = 768
+
+    assert refused(plain, lambda t: t.pop("encoder.encoders.1.norm1.weight")) == "missing tensor encoder.encoders.1.norm1.weight"
+    assert refused(plain, lambda t: t.pop("decoder.decoders.1.feed_forward.w_1.weight")) == "missing tensor decoder.decoders.1.feed_forward.w_1.weight"
+    assert refused(ctx, lambda t: t.pop("decoder.bias_decoder.src_attn.linear_k_v.weight")) == \
+        "missing tensor decoder.bias_decoder.src_attn.linear_k_v.weight"
+    assert refused(plain, d_model_768) == "unsupported config"
+    qkv = "encoder.encoders.0.self_attn.linear_q_k_v.weight"
+    assert refused(plain, lambda t: t.__setitem__(qkv, t[qkv][:, :256])) == "bad shape of " + qkv
+    for state in (plain, ctx, synth.make_bicif_state_dict(cfg, 8)):
+        h, msg = init(state)
+        assert h or msg == "no such CUDA device (this library has no CPU path)", msg
+        lib.fa_offline_uninit(h)
+
+
 def test_resample_table_matches_torchaudio():
     """funasr_b200.resample restates torchaudio's _get_sinc_resample_kernel (the resampler behind load_utils.py:176-178)."""
     import math

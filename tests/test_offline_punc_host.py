@@ -124,7 +124,14 @@ def test_punc_init_refusals_name_the_piece_without_a_device(tmp_path):
                     t[name] = np.zeros((synth.PUNC_DIM, 1, k), np.float32)
             _set_cfg(3, k)(t)
         assert "FSMN kernel %d" % k in _refused(tmp_path, kern)
+    fsmn = "encoder.encoders.1.self_attn.fsmn_block.weight"                  # one layer with 21 taps in an 11-tap stack
+    assert "bad shape of " + fsmn in _refused(tmp_path, lambda t: t.__setitem__(fsmn, np.zeros((synth.PUNC_DIM, 1, 21), np.float32)))
     lib = _abi.load()
+    path = str(tmp_path / "punc.fab2")                                       # a well-formed file fails only for want of a device
+    pack.write_punc_model_file(path, synth.make_punc_state_dict(0), synth.PUNC_LIST, synth.punc_token_list(), 3, ENC_CONF)
+    h = lib.fa_punc_init(path.encode(), 0)
+    assert h or lib.fa_offline_last_error() == b"no such CUDA device (this library has no CPU path)"
+    lib.fa_punc_uninit(h)
     assert not lib.fa_punc_init(None, 0) and lib.fa_offline_last_error() == b"model_file is NULL"
     assert not lib.fa_punc_init(str(tmp_path / "missing.fab2").encode(), 0) and b"cannot open" in lib.fa_offline_last_error()
     assert not lib.fa_punc_infer(None, None, 0) and lib.fa_offline_last_error() == b"bad argument"

@@ -76,6 +76,14 @@ def test_sensevoice_init_refusals_name_the_piece_without_a_device(tmp_path, sv_s
     assert "bad shape of ctc.ctc_lo.weight" in _refused(tmp_path, sv_state, _set_cfg(5, 1300))
     assert "bad shape of embed.weight" in _refused(tmp_path, sv_state, lambda t: t.__setitem__("embed.weight", t["embed.weight"][:2]))
     assert "bad __sv_config__" in _refused(tmp_path, sv_state, lambda t: t.__setitem__("__sv_config__", t["__sv_config__"][:8]))
+    w1 = "encoder.tp_encoders.1.feed_forward.w_1.weight"
+    assert "bad shape of " + w1 in _refused(tmp_path, sv_state, lambda t: t.__setitem__(w1, t[w1][:, :256]))
+    path = str(tmp_path / "sv.fab2")                                         # a well-formed file fails only for want of a device
+    pack.write_sensevoice_model_file(path, sv_state, CFG)
+    lib = _abi.load()
+    h = lib.fa_offline_init(path.encode(), 0, _abi.GEMM_MODES["fp16x3"])
+    assert h or lib.fa_offline_last_error() == b"no such CUDA device (this library has no CPU path)"
+    lib.fa_offline_uninit(h)
 
 
 # ------------------------------------------------------------------------------------------------------------ CTCSearch text

@@ -120,7 +120,8 @@ def test_vad_model_file_refuses_unsupported_shapes(tmp_path):
 
 
 def test_vad_handle_refuses_bad_files_and_null_handles(tmp_path):
-    """Missing, truncated or wrong-magic files and NULL handles: NULL plus a message, never an exception across the ABI."""
+    """Missing, truncated or wrong-magic files, files with a bad piece and NULL handles: NULL plus a message, never an exception across
+    the ABI.  A file is checked on its index before any device work, so the message names the piece on any machine."""
     lib = _abi.load()
     good = str(tmp_path / "vad.fab2")
     pack.write_vad_model_file(good, synth.make_vad_state_dict(synth.VAD_DEFAULT, 0), synth.make_vad_cmvn(0), {})
@@ -128,9 +129,34 @@ def test_vad_handle_refuses_bad_files_and_null_handles(tmp_path):
     (tmp_path / "trunc.fab2").write_bytes(blob[: len(blob) // 2])
     (tmp_path / "magic.fab2").write_bytes(b"XXXXXXXX" + blob[8:])
     (tmp_path / "empty.fab2").write_bytes(b"")
-    for p in ("missing.fab2", "trunc.fab2", "magic.fab2", "empty.fab2"):
+    assert not lib.fa_vad_init(str(tmp_path / "missing.fab2").encode(), 0) and b"cannot open" in lib.fa_offline_last_error()
+    for p in ("trunc.fab2", "magic.fab2", "empty.fab2"):
         assert not lib.fa_vad_init(str(tmp_path / p).encode(), 0)
-        assert lib.fa_offline_last_error() != b""
+        assert b"malformed" in lib.fa_offline_last_error()
+
+    def refused(edit):
+        t = pack.vad_model_tensors(synth.make_vad_state_dict(synth.VAD_DEFAULT, 0), synth.make_vad_cmvn(0), {})
+        edit(t)
+        path = str(tmp_path / "bad.fab2")
+        pack._write(path, t)
+        assert not lib.fa_vad_init(path.encode(), 0)
+        return lib.fa_offline_last_error().decode()
+
+    def set_cfg(i, v):
+        def f(t):
+            c = t["__vad_config__"].view("<f8").copy()
+            c[i] = v
+            t["__vad_config__"] = c.view("<f4")
+        return f
+
+    assert "right-context" in refused(lambda t: t.__setitem__("encoder.fsmn.1.fsmn_block.conv_right.weight", np.zeros((128, 1, 2, 1), np.float32)))
+    assert refused(lambda t: t.pop("encoder.out_linear2.linear.weight")) == "missing tensor encoder.out_linear2.linear.weight"
+    assert refused(lambda t: t.__setitem__("__vad_config__", t["__vad_config__"][:48])) == "bad __vad_config__"
+    assert refused(set_cfg(19, 10)) == "unsupported VAD config"                     # lorder
+    assert refused(set_cfg(21, 248)) == "sil_pdf_ids outside the output"            # out_linear2 has 248 outputs
+    h = lib.fa_vad_init(good.encode(), 0)
+    assert h or lib.fa_offline_last_error() == b"no such CUDA device (this library has no CPU path)"
+    lib.fa_vad_uninit(h)
     assert not lib.fa_vad_init(None, 0)
     assert lib.fa_offline_last_error() == b"model_file is NULL"
     x = np.zeros(16000, np.float32)
