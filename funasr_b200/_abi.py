@@ -64,6 +64,10 @@ class FaTimestampHead(C.Structure):
                 ("out2_b", C.c_void_p), ("up_times", C.c_int32), ("smooth2", C.c_float), ("noise2", C.c_float), ("threshold", C.c_float)]
 
 
+class FaHotwordEncoder(C.Structure):
+    _fields_ = [("embed", C.c_void_p), ("vocab", C.c_int32), ("n_layers", C.c_int32), ("ih", C.POINTER(FaLinear)), ("hh", C.POINTER(FaLinear))]
+
+
 class FaVadLayer(C.Structure):
     _fields_ = [("lin", FaLinear), ("conv_w", C.c_void_p), ("affine", FaLinear)]
 
@@ -159,6 +163,9 @@ SIGNATURES = {
     "fa_linear_argmax_workspace_bytes": (_sz, [_i64, _i32, _i32]),
     "fa_linear_argmax": (C.c_int, [C.POINTER(FaLinear), _vp, _vp, _i64, _vp, _vp, _vp, _i32, _vp, _sz, _vp]),
     "fa_seaco_merge": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
+    "fa_seaco_asf_select_host": (_i32, [_vp, _i32, _i32, _i32, _i32, _vp]),
+    "fa_hotword_encoder_workspace_bytes": (_sz, [_i32, _i64, _i32]),
+    "fa_hotword_encoder_forward": (C.c_int, [C.POINTER(FaHotwordEncoder), _vp, _vp, _i32, _vp, _i32, _vp, _sz, _vp]),
     "fa_cif_upsample_alphas": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _f, _f, _f, _vp, _vp, _vp]),
     "fa_blstm_tc_scratch_bytes": (_sz, [_i32]),
     "fa_blstm_forward_tc": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _sz, _vp]),
@@ -194,6 +201,8 @@ SIGNATURES = {
     "fa_offline_result_audio_seconds": (C.c_float, [_vp]),
     "fa_offline_result_stamps": (C.POINTER(_i32), [_vp, _i32, C.POINTER(_i32)]),
     "fa_offline_is_sensevoice": (_i32, [_vp]),
+    "fa_offline_is_seaco": (_i32, [_vp]),
+    "fa_offline_hotword_embed": (C.c_int, [_vp, _vp, _vp, _i32, _vp]),
     "fa_offline_infer_sv": (_vp, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp, _vp]),
     "fa_sv_ctc_text_host": (_i64, [_vp, _i32, C.POINTER(C.c_char_p), _i32, C.c_char_p, _i64]),
     "fa_offline_free_result": (None, [_vp]),

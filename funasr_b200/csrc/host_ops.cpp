@@ -2,6 +2,9 @@
 // work keeps up with the GPU (64 utterances per ~40 ms step).
 #include "../../include/funasr_b200.h"
 
+#include <algorithm>
+#include <cmath>
+#include <utility>
 #include <vector>
 
 // Integrate-and-fire trace of one utterance, funasr/utils/timestamp_tools.py:14-34 (`cif_wo_hidden`): fp32 running sum of the
@@ -96,4 +99,78 @@ extern "C" int64_t fa_ts_stamps_host(const float* us_alphas, const float* us_pea
     out[2 * i + 1] = (int32_t)(int64_t)(end * 1000);
   }
   return n_span;
+}
+
+namespace {
+
+// torch's CPU sum over an outer (strided) dimension, float32 accumulation (aten/src/ATen/native/cpu/SumKernel.cpp): one column of
+// `size` values `stride` apart.  multi_row_sum is a four-level cascade: 16-element blocks (2^level_power, level_power = max(4,
+// ceil(log2 size) / 4)) summed left to right into level 0, each finished block added one level up, a level carried further up whenever
+// the position is a multiple of the next level's span; the tail then goes into level 0, and the levels are added 0 + 1 + 2 + 3.
+int64_t ceil_log2(int64_t n) {
+  int64_t r = 0;
+  while (((int64_t)1 << r) < n) ++r;
+  return r;
+}
+
+float cascade_sum(const float* a, int64_t stride, int64_t size) {
+  const int64_t level_power = std::max<int64_t>(4, ceil_log2(size) / 4), level_step = (int64_t)1 << level_power, mask = level_step - 1;
+  float acc[4] = {0.f, 0.f, 0.f, 0.f};
+  int64_t i = 0;
+  while (i + level_step <= size) {
+    for (int64_t j = 0; j < level_step; ++j) acc[0] += a[(i + j) * stride];
+    i += level_step;
+    for (int j = 1; j < 4; ++j) {
+      acc[j] += acc[j - 1];
+      acc[j - 1] = 0.f;
+      if (i & (mask << (j * level_power))) break;
+    }
+  }
+  for (; i < size; ++i) acc[0] += a[i * stride];
+  return ((acc[0] + acc[1]) + acc[2]) + acc[3];
+}
+
+// row_sum: the column read as [size / 4, 4], four interleaved cascades, the tail added to the first, then the four added in order
+float interleaved_sum(const float* a, int64_t stride, int64_t size) {
+  const int64_t q = size / 4;
+  float p[4];
+  for (int k = 0; k < 4; ++k) p[k] = cascade_sum(a + k * stride, 4 * stride, q);
+  for (int64_t i = 4 * q; i < size; ++i) p[0] += a[i * stride];
+  return ((p[0] + p[1]) + p[2]) + p[3];
+}
+
+// x.sum(0) of a contiguous [size0, size1] float32 tensor: the vectorised outer-reduction path cascades columns in blocks of 32 (four
+// vectors of 8 lanes); the columns after the last whole block go through row_sum.  Worker threads split the columns at multiples of
+// 128 bytes (32 columns), which leaves every column's path, and so every bit of the result, as in one thread.
+void torch_sum_dim0(const float* x, int64_t size0, int64_t size1, float* out) {
+  const int64_t blocked = size1 / 32 * 32;
+  for (int64_t j = 0; j < size1; ++j) out[j] = j < blocked ? cascade_sum(x + j, size1, size0) : interleaved_sum(x + j, size1, size0);
+}
+
+}  // namespace
+
+// SeACo's attention-score filter on the host (seaco_paraformer/model.py:320-343 as funasr_b200/engine.py:seaco_decode computes it with
+// torch on the CPU): scores = probs.sum(0).sum(0) over probs [heads, n_rows, n_hw] in torch's summation order, then
+// torch.topk(scores, k = min(nfilter, n_hw - 1)) in its order among equal scores (std::partial_sort when 64 k <= n_hw, else
+// std::nth_element and a sort of the first k - 1, on (score, index) pairs in index order, greater-than), followed by n_hw - 1.
+extern "C" int32_t fa_seaco_asf_select_host(const float* probs, int32_t heads, int32_t n_rows, int32_t n_hw, int32_t nfilter, int32_t* picked) {
+  if (!probs || !picked || heads < 1 || n_rows < 1 || n_hw < 2 || nfilter < 1) return FA_ERR_ARG;
+  const int64_t cols = (int64_t)n_rows * n_hw;
+  std::vector<float> per_row((size_t)cols), scores((size_t)n_hw);
+  torch_sum_dim0(probs, heads, cols, per_row.data());
+  torch_sum_dim0(per_row.data(), n_rows, n_hw, scores.data());
+  const int64_t k = std::min<int64_t>(nfilter, n_hw - 1);
+  typedef std::pair<float, int64_t> elem_t;
+  std::vector<elem_t> queue((size_t)n_hw);
+  for (int64_t j = 0; j < n_hw; ++j) queue[j] = elem_t(scores[j], j);
+  auto greater = [](const elem_t& x, const elem_t& y) -> bool { return (std::isnan(x.first) && !std::isnan(y.first)) || (x.first > y.first); };
+  if (k * 64 <= n_hw) {
+    std::partial_sort(queue.begin(), queue.begin() + k, queue.end(), greater);
+  } else {
+    std::nth_element(queue.begin(), queue.begin() + k - 1, queue.end(), greater);
+    std::sort(queue.begin(), queue.begin() + k - 1, greater);
+  }
+  for (int64_t j = 0; j < k; ++j) picked[j] = (int32_t)queue[j].second;
+  picked[k] = n_hw - 1;
+  return (int32_t)(k + 1);
 }

@@ -14,6 +14,8 @@
 //                           lockstep step (the text walk: punc_text.cpp)
 //   a SenseVoiceSmall file (__sv_config__) makes the same handle run SenseVoiceEngine's chain: per-utterance query rows
 //                           (fa_sv_query_rows), the SAN-M and tp stacks, the CTC head; fa_offline_infer_sv / fa_offline_infer_vad_sv
+//   a SeacoParaformer file (__seaco_config__): fa_offline_hotword_embed runs its hotword encoder (hotword.cu), the decode takes those
+//                           rows through _seaco_decode_with_ASF (seaco_bias)
 // The tokenizer (ids -> text) stays with the caller, like every other entry point of this ABI.
 #include "common.cuh"
 #include "punc_text.h"
@@ -171,6 +173,14 @@ struct Model {
   FaLinear ctc{};
   const float* embed = nullptr;
   DevBuf enc2, am;
+  bool seaco = false;                                // SeacoParaformer (__seaco_config__): hotword encoder, SeACo decoder, NO_BIAS merge
+  int no_bias = 0, nfilter = 0;
+  std::vector<FaDecLayer> seaco_l;
+  FaDecoder seaco_dec{};
+  FaLinear hw_out{};
+  std::vector<FaLinear> hw_ih, hw_hh;
+  FaHotwordEncoder hw_enc{};
+  DevBuf hw_rows, hidden, cif_att, dec_att, dha_ids, dha_best, sids, sbest, probs, hw_sel, sel_lens;
 };
 
 struct Result {
@@ -389,6 +399,8 @@ bool build_paraformer(Model& m, Builder& b) {
   // ContextualParaformerDecoder (contextual_paraformer/decoder.py:133-352): the last attention layer is `last_decoder`, plus the
   // hotword branch bias_decoder (norm3 + cross attention) and bias_output (Conv1d 1024 -> 512, k = 1)
   m.contextual = b.opt("decoder.bias_decoder.norm3.weight") != nullptr;
+  if (m.contextual && b.opt("__seaco_config__"))
+    return b.refuse("SeACo model: the file carries both a contextual decoder.bias_decoder and __seaco_config__");
   const int n_plain = m.contextual ? m.dec_layers - 1 : m.dec_layers;
   m.dec_l.resize(n_plain > 0 ? n_plain : 1);
   for (int i = 0; i < n_plain; ++i) dec_layer(m.dec_l[i], "decoder.decoders." + std::to_string(i), true);
@@ -408,12 +420,126 @@ bool build_paraformer(Model& m, Builder& b) {
     m.dec.bias_output = b.lin("decoder.bias_output", false);
     m.dec.clas_scale = 1.0f;
   }
+  const Tensor* sc = b.opt("__seaco_config__");
+  m.seaco = sc != nullptr;
+  if (m.seaco && b.ok) {
+    b.what = "SeACo model: ";
+    if (sc->host.size() != 3) return b.refuse("bad __seaco_config__");
+    m.no_bias = (int)sc->host[0]; m.nfilter = (int)sc->host[1];
+    const int layers = (int)sc->host[2], D = m.d_model;
+    if (m.no_bias < 0 || m.no_bias >= m.vocab)
+      return b.refuse("no_bias " + std::to_string(m.no_bias) + " outside the vocabulary [0, " + std::to_string(m.vocab) + ")");
+    if (m.nfilter < 0) return b.refuse("nfilter " + std::to_string(m.nfilter) + " < 0");
+    if (layers < 1 || layers > FA_HOTWORD_MAX_LAYERS) return b.refuse("bias_encoder with " + std::to_string(layers) + " layers");
+    // the hotword encoder (seaco_paraformer/model.py:384-420): decoder.embed, then the bias_encoder LSTM; the GEMM bias b_ih + b_hh
+    // comes folded from pack.py
+    const Tensor* emb = b.shaped("decoder.embed.0.weight", {m.vocab, D});
+    m.hw_ih.assign(layers, FaLinear{}); m.hw_hh.assign(layers, FaLinear{});
+    for (int k = 0; k < layers; ++k) {
+      const std::string s = std::to_string(k);
+      b.shaped("bias_encoder.weight_ih_l" + s, {4 * D, D}); b.shaped("bias_encoder.weight_hh_l" + s, {4 * D, D});
+      b.shaped("bias_encoder.bias_ih_l" + s, {4 * D}); b.shaped("bias_encoder.bias_hh_l" + s, {4 * D});
+      b.shaped("bias_encoder.gemm_bias_l" + s, {4 * D});
+      if (!b.ok) return false;
+      m.hw_ih[k] = b.lin("bias_encoder.ih_l" + s, true, ("bias_encoder.weight_ih_l" + s).c_str(), ("bias_encoder.gemm_bias_l" + s).c_str());
+      m.hw_hh[k] = b.lin("bias_encoder.hh_l" + s, false, ("bias_encoder.weight_hh_l" + s).c_str());
+    }
+    if (b.opt("bias_encoder.weight_ih_l" + std::to_string(layers))) return b.refuse("more bias_encoder layers than __seaco_config__ says");
+    m.hw_enc = FaHotwordEncoder{emb ? emb->dev : nullptr, m.vocab, layers, m.hw_ih.data(), m.hw_hh.data()};
+    // the SeACo decoder (model.py:100-110): ParaformerSANMDecoder without input / output layer; forward_asf6 reads layers 0..5
+    int n_s = 0;
+    while (b.opt("seaco_decoder.decoders." + std::to_string(n_s) + ".norm1.weight")) ++n_s;
+    if (n_s < 6) return b.refuse(n_s == 0 ? std::string("missing tensor seaco_decoder.decoders.0.norm1.weight")
+                                           : "seaco_decoder with " + std::to_string(n_s) + " attention layers (the attention-score filter reads 6)");
+    const Tensor* sk = b.get("seaco_decoder.decoders.0.self_attn.fsmn_block.weight");
+    const int64_t K = sk && sk->shape.size() == 3 ? sk->shape[2] : 0;
+    m.seaco_l.assign(n_s, FaDecLayer{});
+    for (int i = 0; i < n_s && b.ok; ++i) {
+      const std::string p = "seaco_decoder.decoders." + std::to_string(i);
+      const Tensor* w1 = b.get(p + ".feed_forward.w_1.weight");
+      const int64_t F = w1 && w1->shape.size() == 2 ? w1->shape[0] : 0;
+      if (w1 && (F < 1 || F > 2048)) return b.refuse("bad shape of " + p + ".feed_forward.w_1.weight (at most 2048 units)");
+      b.shaped(p + ".feed_forward.w_1.weight", {F, D}); b.shaped(p + ".feed_forward.w_2.weight", {D, F});
+      b.shaped(p + ".self_attn.fsmn_block.weight", {D, 1, K});
+      b.shaped(p + ".src_attn.linear_q.weight", {D, D}); b.shaped(p + ".src_attn.linear_k_v.weight", {2 * D, D});
+      b.shaped(p + ".src_attn.linear_out.weight", {D, D});
+      dec_layer(m.seaco_l[i], p, true);
+    }
+    m.seaco_dec = FaDecoder{};
+    m.seaco_dec.layers = m.seaco_l.data(); m.seaco_dec.n_layers = n_s; m.seaco_dec.heads = m.heads; m.seaco_dec.fsmn_k = (int)K;
+    dec_layer(m.seaco_dec.last, "seaco_decoder.decoders3.0", false);
+    m.seaco_dec.after_norm = b.norm("seaco_decoder.after_norm");
+    b.shaped("hotword_output_layer.weight", {m.vocab, D}); b.shaped("hotword_output_layer.bias", {m.vocab});
+    m.hw_out = b.lin("hotword_output_layer");
+    b.what.clear();
+  }
   return b.ok;
 }
 
 int num_lfr_frames(int64_t n) {       // wav_frontend.py:73 after kaldi.py snip_edges framing
   const int64_t mfr = n >= 400 ? 1 + (n - 400) / 160 : 0;
   return (int)((mfr + 5) / 6);
+}
+
+// SeACo's hotword biasing after the decoder (_seaco_decode_with_ASF, seaco_paraformer/model.py:271-382, as ParaformerEngine.seaco_decode
+// runs it): the host hotword rows hw_host [n_hw, 512] on the device; with more rows than nfilter, the attention-score filter on
+// utterance 0 (one host round trip: its probabilities out, fa_seaco_asf_select_host, the picked host rows back in); the SeACo decoder
+// over the acoustic embeddings and over the decoder's hidden states; hotword_output_layer's arg-max over their sum; the NO_BIAS merge
+// into m.sids.  m.ids / m.best / m.hidden hold the decoder's outputs, the workspace is sized for the stack and the arg-max.
+bool seaco_bias(Model& m, int B, int n_max, int n_cap, const float* hw_host, int n_hw) {
+  cudaStream_t st = m.file.st;
+  const int D = m.d_model, V = m.vocab, n_s = m.seaco_dec.n_layers;
+  const int64_t rows = (int64_t)B * n_max;
+  if (!(m.hw_rows.reserve((size_t)n_hw * D * 4) && m.cif_att.reserve((size_t)rows * D * 4) && m.dec_att.reserve((size_t)rows * D * 4) &&
+        m.dha_ids.reserve((size_t)rows * 4) && m.dha_best.reserve((size_t)rows * 4) && m.sids.reserve((size_t)rows * 4) &&
+        m.sbest.reserve((size_t)rows * 4) && m.sel_lens.reserve((size_t)B * 4))) {
+    set_err("device allocation failed (SeACo)");
+    return false;
+  }
+  const float* hidden = static_cast<const float*>(m.hidden.p);
+  const int32_t* tok = static_cast<const int32_t*>(m.tok.p);
+  float* mem = static_cast<float*>(m.hw_rows.p);
+  int32_t* mem_lens = static_cast<int32_t*>(m.sel_lens.p);
+  cudaMemcpyAsync(mem, hw_host, (size_t)n_hw * D * 4, cudaMemcpyHostToDevice, st);
+  int n_sel = n_hw;
+  std::vector<float> picked_rows;
+  int rc = FA_OK;
+  if (m.nfilter > 0 && m.nfilter < n_hw) {                   // ASF (model.py:320-343): forward_asf6 on utterance 0
+    const int H = m.seaco_dec.heads;
+    const int32_t one = n_hw;
+    if (!m.probs.reserve((size_t)H * n_max * n_hw * 4)) { set_err("device allocation failed (SeACo filter)"); return false; }
+    cudaMemcpyAsync(mem_lens, &one, 4, cudaMemcpyHostToDevice, st);
+    rc = fa_sanm_decoder_stack_forward(&m.seaco_dec, mem, mem_lens, 1, 1, n_hw, hidden, n_max, tok, n_max, 6, 0, nullptr,
+                                       static_cast<float*>(m.probs.p), m.mode, m.ws.p, m.ws.cap, st);
+    if (rc != FA_OK) { set_err(std::string("SeACo filter: ") + fa_status_string(rc)); return false; }
+    std::vector<float> probs((size_t)H * n_max * n_hw);
+    cudaMemcpyAsync(probs.data(), m.probs.p, probs.size() * 4, cudaMemcpyDeviceToHost, st);
+    if (!sync_stream(st)) return false;
+    std::vector<int32_t> picked((size_t)n_hw);
+    n_sel = fa_seaco_asf_select_host(probs.data(), H, n_max, n_hw, m.nfilter, picked.data());
+    if (n_sel < 1) { set_err("fa_seaco_asf_select_host failed"); return false; }
+    picked_rows.resize((size_t)n_sel * D);
+    for (int j = 0; j < n_sel; ++j) std::copy(hw_host + (size_t)picked[j] * D, hw_host + (size_t)(picked[j] + 1) * D, picked_rows.begin() + (size_t)j * D);
+    cudaMemcpyAsync(mem, picked_rows.data(), picked_rows.size() * 4, cudaMemcpyHostToDevice, st);
+  }
+  const std::vector<int32_t> lens_h(B, n_sel);
+  cudaMemcpyAsync(mem_lens, lens_h.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st);
+  float* cif_att = static_cast<float*>(m.cif_att.p);
+  float* dec_att = static_cast<float*>(m.dec_att.p);
+  rc = fa_sanm_decoder_stack_forward(&m.seaco_dec, mem, mem_lens, 1, B, n_sel, static_cast<const float*>(m.acoustic.p), n_cap, tok, n_max, n_s, 1,
+                                     cif_att, nullptr, m.mode, m.ws.p, m.ws.cap, st);
+  if (rc == FA_OK)
+    rc = fa_sanm_decoder_stack_forward(&m.seaco_dec, mem, mem_lens, 1, B, n_sel, hidden, n_max, tok, n_max, n_s, 1, dec_att, nullptr, m.mode,
+                                       m.ws.p, m.ws.cap, st);
+  if (rc == FA_OK)
+    rc = fa_linear_argmax(&m.hw_out, cif_att, dec_att, rows, static_cast<int32_t*>(m.dha_ids.p), static_cast<float*>(m.dha_best.p), nullptr,
+                          m.mode, m.ws.p, m.ws.cap, st);
+  if (rc == FA_OK)
+    rc = fa_seaco_merge(static_cast<int32_t*>(m.ids.p), static_cast<float*>(m.best.p), static_cast<int32_t*>(m.dha_ids.p),
+                        static_cast<float*>(m.dha_best.p), rows, m.no_bias, static_cast<int32_t*>(m.sids.p), static_cast<float*>(m.sbest.p),
+                        nullptr, nullptr, nullptr, V, st);
+  if (rc != FA_OK) { set_err(std::string("SeACo decoder: ") + fa_status_string(rc)); return false; }
+  return sync_stream(st);                                    // lens_h and picked_rows are host vectors of this frame
 }
 
 // The recogniser over a padded batch already on the device: wav [B, stride] fp32 (m.wav or any buffer the call does not reuse),
@@ -467,8 +593,11 @@ std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride,
   // the timestamp head over the [B, 3T] upsampled frames shares the workspace with the decoder
   const int U = m.head.up_times, TU = T * U;
   const int64_t rows_up = (int64_t)B * TU;
+  const int n_sw = m.seaco && hw_embed ? n_hotwords : 0;     // SeACo hotword rows (none: the plain decoder distribution)
   size_t ws_dec = fa_paraformer_decoder_workspace_bytes_hw(B, T, n_max, m.vocab, m.mode, nh);
   if (m.ts) ws_dec = std::max(ws_dec, fa_timestamp_head_workspace_bytes(B, T, D, U, m.mode));
+  if (n_sw > 0)
+    ws_dec = std::max({ws_dec, fa_sanm_decoder_stack_workspace_bytes(B, n_sw, n_max, m.mode), fa_linear_argmax_workspace_bytes((int64_t)B * n_max, m.vocab, m.mode)});
   if (!(m.ids.reserve((size_t)B * n_max * 4) && m.best.reserve((size_t)B * n_max * 4) && m.fids.reserve((size_t)B * n_max * 4) &&
         m.flens_out.reserve((size_t)B * 4) && m.ws.reserve(ws_dec)))
     return fail("device allocation failed (decoder)");
@@ -483,11 +612,24 @@ std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride,
     m.dec.has_bias = 1; m.dec.n_hotwords = nh;
     m.dec.hw_embed = static_cast<const float*>(m.hw.p); m.dec.hw_lens = static_cast<const int32_t*>(m.hw_lens.p);
   }
-  rc = fa_paraformer_decoder_forward(&m.dec, static_cast<float*>(m.encb.p), static_cast<int32_t*>(m.flens.p), B, T, static_cast<float*>(m.acoustic.p),
-                                     n_cap, static_cast<int32_t*>(m.tok.p), n_max, static_cast<int32_t*>(m.ids.p), static_cast<float*>(m.best.p),
-                                     nullptr, 1, m.mode, m.ws.p, m.ws.cap, st);
+  const int32_t* final_ids = static_cast<int32_t*>(m.ids.p);
+  if (m.seaco) {                                             // return_hidden: the decoder_hidden the SeACo decoder attends from
+    if (!m.hidden.reserve((size_t)B * n_max * D * 4)) return fail("device allocation failed (SeACo)");
+    rc = fa_paraformer_decoder_forward_hidden(&m.dec, static_cast<float*>(m.encb.p), static_cast<int32_t*>(m.flens.p), B, T,
+                                              static_cast<float*>(m.acoustic.p), n_cap, static_cast<int32_t*>(m.tok.p), n_max,
+                                              static_cast<int32_t*>(m.ids.p), static_cast<float*>(m.best.p), nullptr, 1,
+                                              static_cast<float*>(m.hidden.p), m.mode, m.ws.p, m.ws.cap, st);
+    if (rc == FA_OK && n_sw > 0) {
+      if (!seaco_bias(m, B, n_max, n_cap, hw_embed, n_sw)) return nullptr;
+      final_ids = static_cast<int32_t*>(m.sids.p);
+    }
+  } else {
+    rc = fa_paraformer_decoder_forward(&m.dec, static_cast<float*>(m.encb.p), static_cast<int32_t*>(m.flens.p), B, T, static_cast<float*>(m.acoustic.p),
+                                       n_cap, static_cast<int32_t*>(m.tok.p), n_max, static_cast<int32_t*>(m.ids.p), static_cast<float*>(m.best.p),
+                                       nullptr, 1, m.mode, m.ws.p, m.ws.cap, st);
+  }
   if (rc == FA_OK)
-    rc = fa_greedy_filter(static_cast<int32_t*>(m.ids.p), static_cast<int32_t*>(m.tok.p), B, n_max, 1, 2, 0, static_cast<int32_t*>(m.fids.p),
+    rc = fa_greedy_filter(final_ids, static_cast<int32_t*>(m.tok.p), B, n_max, 1, 2, 0, static_cast<int32_t*>(m.fids.p),
                           static_cast<int32_t*>(m.flens_out.p), st);
   if (rc != FA_OK) return fail(std::string("decoder: ") + fa_status_string(rc));
   if (m.ts) {                   // CifPredictorV3.get_upsample_timestamp (bicif_paraformer/cif_predictor.py:300-352), engine.upsample_timestamp
@@ -641,6 +783,7 @@ void* infer_batch(void* handle, const void* const* bufs, const int64_t* n_sample
   if (!mp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) return fail("bad argument");
   Model& m = *mp;
   if (m.contextual && (!hw_embed || n_hotwords < 1)) return fail("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)");
+  if (m.seaco && (n_hotwords < 0 || (n_hotwords > 0 && !hw_embed))) return fail("bad hotword rows: hw_embed must hold n_hotwords rows of 512");
   if (m.sv && !check_queries(m, lang, tn, batch, "utterance")) return nullptr;
   cudaSetDevice(m.file.device);
   int64_t nmax = 0;
@@ -685,6 +828,37 @@ extern "C" void fa_offline_uninit(void* handle) { delete static_cast<Model*>(han
 extern "C" int32_t fa_offline_is_contextual(const void* handle) { return handle && static_cast<const Model*>(handle)->contextual ? 1 : 0; }
 
 extern "C" int32_t fa_offline_has_timestamps(const void* handle) { return handle && static_cast<const Model*>(handle)->ts ? 1 : 0; }
+
+extern "C" int32_t fa_offline_is_seaco(const void* handle) { return handle && static_cast<const Model*>(handle)->seaco ? 1 : 0; }
+
+extern "C" int fa_offline_hotword_embed(void* handle, const int32_t* ids, const int32_t* lens, int32_t n, float* rows_host) {
+  g_err.clear();
+  Model* m = static_cast<Model*>(handle);
+  if (!m || !ids || !lens || n < 1 || !rows_host) { set_err("fa_offline_hotword_embed: bad argument"); return FA_ERR_ARG; }
+  if (!m->seaco) { set_err("fa_offline_hotword_embed: not a SeACo model file (ContextualParaformer rows come from its own encoder)"); return FA_ERR_ARG; }
+  int64_t n_tok = 0;
+  for (int32_t i = 0; i < n; ++i) {                 // every id named before any launch
+    if (lens[i] < 1) { set_err("hotword " + std::to_string(i) + " has no token"); return FA_ERR_ARG; }
+    for (int32_t k = 0; k < lens[i]; ++k)
+      if (ids[n_tok + k] < 0 || ids[n_tok + k] >= m->vocab) {
+        set_err("hotword " + std::to_string(i) + ": token id " + std::to_string(ids[n_tok + k]) + " outside the vocabulary [0, " +
+                std::to_string(m->vocab) + ")");
+        return FA_ERR_ARG;
+      }
+    n_tok += lens[i];
+  }
+  cudaSetDevice(m->file.device);
+  cudaStream_t st = m->file.st;
+  const size_t ws = fa_hotword_encoder_workspace_bytes(n, n_tok, m->mode);
+  if (ws == 0 || !m->ws.reserve(ws) || !m->hw_rows.reserve((size_t)n * m->d_model * 4)) {
+    set_err("device allocation failed (hotword encoder)");
+    return FA_ERR_CUDA;
+  }
+  const int rc = fa_hotword_encoder_forward(&m->hw_enc, ids, lens, n, static_cast<float*>(m->hw_rows.p), m->mode, m->ws.p, m->ws.cap, st);
+  if (rc != FA_OK) { set_err(std::string("fa_hotword_encoder_forward: ") + fa_status_string(rc)); return rc; }
+  cudaMemcpyAsync(rows_host, m->hw_rows.p, (size_t)n * m->d_model * 4, cudaMemcpyDeviceToHost, st);
+  return sync_stream(st) ? FA_OK : FA_ERR_CUDA;
+}
 
 extern "C" const float* fa_offline_host_tensor(void* handle, const char* name, int64_t* numel) {
   Model* m = static_cast<Model*>(handle);
@@ -1026,6 +1200,7 @@ void* infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_
   if (!mp || !vp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) return fail("bad argument");
   if (mp->file.device != vp->file.device) return fail("the recogniser and the VAD live on different devices");
   if (mp->contextual && (!hw_embed || n_hotwords < 1)) return fail("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)");
+  if (mp->seaco && (n_hotwords < 0 || (n_hotwords > 0 && !hw_embed))) return fail("bad hotword rows: hw_embed must hold n_hotwords rows of 512");
   if (mp->sv && !check_queries(*mp, lang, tn, batch, "recording")) return nullptr;
   FaLongAudioOptions o;
   if (opts) o = *opts;

@@ -5,6 +5,9 @@
 // ids -> text join.  Everything per audio frame runs in fa_offline_infer_hw on the GPU — or, with a VAD model ("vad-dir"), in
 // fa_offline_infer_vad.  FsmnVad* are the runtime's VAD entry points over fa_vad_infer.
 //
+// SeACo (paraformer-zh): CompileHotwordEmbedding parses the hotword string as for ContextualParaformer and takes the rows from the
+// handle's GPU hotword encoder (fa_offline_hotword_embed); FunOfflineInferBuffer passes them on, with or without "vad-dir".
+//
 // Timestamps: with a BiCifParaformer model file FunASRGetStamp returns the runtime's "[[b,e],[b,e],...]" (integer ms, absolute with
 // "vad-dir"; funasrruntime.cpp:297-310), one pair per stamp of fa_offline_result_stamps.  The values are the library's one timestamp
 // definition, the one the reference's Python BiCifParaformer produces (timestamp_tools.py:ts_prediction_lfr6_standard): the shim does
@@ -230,6 +233,30 @@ std::vector<std::string> split_units(const std::string& w) {
   return u;
 }
 
+// The hotword token lists of one hotword string (generate_hotwords_list for ContextualParaformer and SeacoParaformer alike): each
+// whitespace-separated hotword split into vocabulary units (split_units, tokens.txt; decimal ids without it), a hotword with a unit
+// outside the vocabulary dropped, then the <s> entry {1}
+std::vector<std::vector<int>> hotword_lists(const OfflineStream& s, const std::string& hotwords, int vocab) {
+  std::vector<std::vector<int>> lists;
+  std::stringstream ss(hotwords);
+  std::string w;
+  while (ss >> w) {
+    std::vector<int> ids;
+    bool ok = true;
+    for (const std::string& u : split_units(w)) {
+      int id = -1;
+      auto it = s.token_id.find(u);
+      if (it != s.token_id.end()) id = it->second;
+      else if (s.vocab.empty()) id = atoi(u.c_str());                   // no vocabulary file: decimal token ids
+      if (id < 0 || id >= vocab) { ok = false; break; }
+      ids.push_back(id);
+    }
+    if (ok && !ids.empty()) lists.push_back(ids);                      // hotwords with out-of-vocabulary units are dropped
+  }
+  lists.push_back({1});                                                // <s>
+  return lists;
+}
+
 inline float sigm(float x) { return 1.0f / (1.0f + expf(-x)); }
 
 // SenseVoice: the runtime's lid_map (sensevoice-small.h:110-118); an unknown svs_lang is "auto" (sensevoice-small.cpp:458-465)
@@ -319,9 +346,9 @@ FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, int 
   if (fa_offline_is_sensevoice(s->h)) return infer_sv(s, bufs, lens, fmt, svs_lang, svs_itn);
   std::vector<float> hw;
   int n_hw = 0;
-  if (fa_offline_is_contextual(s->h)) {
+  if (fa_offline_is_contextual(s->h) || fa_offline_is_seaco(s->h)) {   // SeACo without rows: the plain decoder distribution
     for (const auto& row : hw_emb) if (row.size() == 512) { hw.insert(hw.end(), row.begin(), row.end()); ++n_hw; }
-    if (n_hw == 0) { g_shim_err = "contextual model: hw_emb must hold [n, 512] rows from CompileHotwordEmbedding"; return nullptr; }
+    if (n_hw == 0 && fa_offline_is_contextual(s->h)) { g_shim_err = "contextual model: hw_emb must hold [n, 512] rows from CompileHotwordEmbedding"; return nullptr; }
   }
   if (s->vad) {                        // segment texts concatenated in time order (funasrruntime.cpp:287-296)
     const FaLongAudioOptions o = runtime_long_audio_options(*s);
@@ -475,6 +502,15 @@ const std::vector<std::vector<float>> CompileHotwordEmbedding(FUNASR_HANDLE hand
   std::vector<std::vector<float>> out;
   OfflineStream* s = static_cast<OfflineStream*>(handle);
   if (s && fa_offline_is_sensevoice(s->h)) return {std::vector<float>(512, 0.f)};    // one zero row (sensevoice-small.cpp:423-429)
+  if (s && fa_offline_is_seaco(s->h)) {                                 // the same hotword list, rows from the handle's GPU encoder
+    const std::vector<std::vector<int>> lists = hotword_lists(*s, hotwords, (int)fa_offline_host_tensor(s->h, "__config__", nullptr)[5]);
+    std::vector<int32_t> ids, lens;
+    for (const auto& l : lists) { ids.insert(ids.end(), l.begin(), l.end()); lens.push_back((int32_t)l.size()); }
+    std::vector<float> rows(lens.size() * 512);
+    if (fa_offline_hotword_embed(s->h, ids.data(), lens.data(), (int32_t)lens.size(), rows.data()) != 0) { g_shim_err = fa_offline_last_error(); return out; }
+    for (size_t i = 0; i < lens.size(); ++i) out.emplace_back(rows.begin() + i * 512, rows.begin() + (i + 1) * 512);
+    return out;
+  }
   if (!s || !fa_offline_is_contextual(s->h)) return out;
   int64_t n_emb = 0, n_ih = 0, n_hh = 0, n_bi = 0, n_bh = 0;
   const float* emb = fa_offline_host_tensor(s->h, "bias_embed.weight", &n_emb);
@@ -484,24 +520,7 @@ const std::vector<std::vector<float>> CompileHotwordEmbedding(FUNASR_HANDLE hand
   const float* b_hh = fa_offline_host_tensor(s->h, "bias_encoder.bias_hh_l0", &n_bh);
   const int D = 512;
   if (!emb || !w_ih || !w_hh || !b_ih || !b_hh || n_ih != 4 * D * D || n_hh != 4 * D * D) { g_shim_err = "model file has no hotword encoder"; return out; }
-  const int vocab = (int)(n_emb / D);
-  std::vector<std::vector<int>> lists;
-  std::stringstream ss(hotwords);
-  std::string w;
-  while (ss >> w) {
-    std::vector<int> ids;
-    bool ok = true;
-    for (const std::string& u : split_units(w)) {
-      int id = -1;
-      auto it = s->token_id.find(u);
-      if (it != s->token_id.end()) id = it->second;
-      else if (s->vocab.empty()) id = atoi(u.c_str());                  // no vocabulary file: decimal token ids
-      if (id < 0 || id >= vocab) { ok = false; break; }
-      ids.push_back(id);
-    }
-    if (ok && !ids.empty()) lists.push_back(ids);                      // hotwords with out-of-vocabulary units are dropped
-  }
-  lists.push_back({1});                                                // <s>
+  const std::vector<std::vector<int>> lists = hotword_lists(*s, hotwords, (int)(n_emb / D));
   std::vector<float> h(D), c(D), gates(4 * D);
   for (const auto& ids : lists) {
     std::fill(h.begin(), h.end(), 0.f);

@@ -3,7 +3,8 @@ FunOfflineInit / FunOfflineInferBuffer / FunASRGetResult (runtime/onnxruntime/in
 Nothing here touches torch on the data path: host PCM buffers in, token ids out.  `OfflineVad` binds the FSMN-VAD handle
 (fa_vad_*) and `OfflineRecognizer.infer_long` the long-audio entry (fa_offline_infer_vad): VAD segments packed by duration and decoded
 batch by batch, the same results as LongAudioPipeline.generate.  A BiCifParaformer model file adds per-token [start_ms, end_ms] stamps
-(`infer_stamped`, and "timestamp" in `infer_long`'s results).  `OfflinePunc` binds the CT-Transformer punctuation handle (fa_punc_*),
+(`infer_stamped`, and "timestamp" in `infer_long`'s results); a SeacoParaformer model file takes hotword rows from
+`hotword_embeddings` (its hotword encoder on the GPU).  `OfflinePunc` binds the CT-Transformer punctuation handle (fa_punc_*),
 and `punc_walk_host` its text walk with any scorer in place of the network."""
 from __future__ import annotations
 
@@ -193,6 +194,22 @@ class OfflineRecognizer:
         """True for a SenseVoiceSmall model file: `infer` / `infer_long` take `language` and `use_itn`."""
         return bool(self.lib.fa_offline_is_sensevoice(self.handle))
 
+    @property
+    def is_seaco(self) -> bool:
+        """True for a SeacoParaformer model file: `hotword_embeddings` gives the rows `infer` / `infer_long` take."""
+        return bool(self.lib.fa_offline_is_seaco(self.handle))
+
+    def hotword_embeddings(self, hw_lists: Sequence[Sequence[int]]) -> np.ndarray:
+        """SeACo hotword rows (fa_offline_hotword_embed): token-id lists, the <s> entry [1] last as generate_hotwords_list returns them,
+        -> [n, 512] float32, each hotword's bias_encoder output at its last token, computed on the GPU."""
+        lens = np.array([len(h) for h in hw_lists], dtype=np.int32)
+        ids = np.array([t for h in hw_lists for t in h], dtype=np.int32)
+        rows = np.zeros((len(hw_lists), 512), dtype=np.float32)
+        rc = self.lib.fa_offline_hotword_embed(self.handle, ids.ctypes.data, lens.ctypes.data, len(hw_lists), rows.ctypes.data)
+        if rc != 0:
+            raise _abi.FunasrB200Error("fa_offline_hotword_embed failed: %s" % self.lib.fa_offline_last_error().decode())
+        return rows
+
     def _queries(self, n: int, language, use_itn):
         if not self.is_sensevoice:
             if language is not None or use_itn is not None:
@@ -205,13 +222,16 @@ class OfflineRecognizer:
         p = self.lib.fa_offline_result_stamps(res, i, C.byref(cnt))
         return [[int(p[2 * k]), int(p[2 * k + 1])] for k in range(cnt.value)]
 
-    def _infer(self, wavs, stamped: bool, language=None, use_itn=None):
+    def _infer(self, wavs, stamped: bool, language=None, use_itn=None, hotword_embeddings=None):
         arrs, fmt = _pcm_batch(wavs)
         n = len(arrs)
         ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
         lens = (C.c_int64 * n)(*[a.shape[0] for a in arrs])
         q = self._queries(n, language, use_itn)
-        if q is None:
+        if hotword_embeddings is not None:
+            hw = np.ascontiguousarray(hotword_embeddings, dtype=np.float32)
+            res = self.lib.fa_offline_infer_hw(self.handle, ptrs, lens, n, fmt, hw.ctypes.data, hw.shape[0])
+        elif q is None:
             res = self.lib.fa_offline_infer(self.handle, ptrs, lens, n, fmt)
         else:
             res = self.lib.fa_offline_infer_sv(self.handle, ptrs, lens, n, fmt, q[0].ctypes.data, q[1].ctypes.data)
@@ -229,16 +249,17 @@ class OfflineRecognizer:
         finally:
             self.lib.fa_offline_free_result(res)
 
-    def infer(self, wavs: Sequence[np.ndarray], language=None, use_itn=None) -> List[List[int]]:
+    def infer(self, wavs: Sequence[np.ndarray], language=None, use_itn=None, hotword_embeddings: Optional[np.ndarray] = None) -> List[List[int]]:
         """wavs: float32 arrays in [-1, 1] or int16 PCM arrays (all the same dtype), 16 kHz mono, >= 400 samples each.
         SenseVoice model file: language (one name or one per utterance, default "auto") and use_itn (default False) choose each
-        utterance's query; the ids include the four tag tokens (SenseVoiceSmall.inference's token_int)."""
-        return self._infer(wavs, False, language, use_itn)
+        utterance's query; the ids include the four tag tokens (SenseVoiceSmall.inference's token_int).  hotword_embeddings: [n, 512]
+        float32 rows, the last one the <s> entry (ContextualParaformer's encoder, or `hotword_embeddings()` of a SeACo model file)."""
+        return self._infer(wavs, False, language, use_itn, hotword_embeddings)
 
-    def infer_stamped(self, wavs: Sequence[np.ndarray]) -> List[dict]:
+    def infer_stamped(self, wavs: Sequence[np.ndarray], hotword_embeddings: Optional[np.ndarray] = None) -> List[dict]:
         """Like `infer`, per utterance {"token_int": ids, "timestamp": [[start_ms, end_ms], ...]} (BiCifParaformer.inference's result;
         no stamps for a model without the timestamp head)."""
-        return self._infer(wavs, True)
+        return self._infer(wavs, True, hotword_embeddings=hotword_embeddings)
 
     def infer_long(self, wavs: Sequence[np.ndarray], vad: OfflineVad, batch_size_s: int = 300, batch_size_threshold_s: int = 60,
                    merge_vad: bool = False, merge_length_s: int = 15, hotword_embeddings: Optional[np.ndarray] = None,
@@ -246,7 +267,7 @@ class OfflineRecognizer:
         """Long recordings through fa_offline_infer_vad, each on its own as LongAudioPipeline.generate treats it -> per recording
         {"token_int": ids in time order, "vad_segments": [[start_ms, end_ms], ...], "n_tokens": tokens per segment}, plus
         "timestamp": [[start_ms, end_ms], ...] in absolute ms when the model has the timestamp head (`has_timestamps`).
-        hotword_embeddings: [n, 512] float32 rows (ContextualParaformer; last row the <s> entry).  SenseVoice model file
+        hotword_embeddings: [n, 512] float32 rows (ContextualParaformer or SeACo; last row the <s> entry).  SenseVoice model file
         (fa_offline_infer_vad_sv): language / use_itn as in `infer`, one per recording, applied to all its segments."""
         arrs, fmt = _pcm_batch(wavs)
         n = len(arrs)

@@ -20,6 +20,12 @@ the head in the form the library's launches take it (`timestamp_head_tensors`, t
                                                     (the reference's names, copied like every predictor.* tensor)
     __ts_config__                      [3] upsample_times, smooth_factor2, noise_threshold2
 
+A SeacoParaformer file (`write_seaco_model_file`, recognised by __seaco_config__) adds seaco_decoder.*, hotword_output_layer.* and
+bias_encoder.* under the reference's names, and
+
+    bias_encoder.gemm_bias_l{k} [2048]  bias_ih_l{k} + bias_hh_l{k}: the hotword LSTM's input-projection GEMM bias
+    __seaco_config__                    [3] no_bias, nfilter, LSTM layers
+
 The FSMN-VAD file (csrc/offline.cu: fa_vad_init) uses the same layout: the encoder's weights under the reference's names
 (encoder.in_linear1.linear.weight, encoder.fsmn.{i}.fsmn_block.conv_left.weight, ...), frontend.mel_banks / window / cmvn [2, 400]
 and
@@ -93,6 +99,42 @@ def write_model_file(path: str, state: Dict[str, torch.Tensor], cfg: ParaformerC
     """smooth_factor2 / noise_threshold2: CifPredictorV3's predictor_conf values (paraformer-large-vad-punc's by default); used only
     when the state dict has the BiCif timestamp head."""
     return _write(path, model_tensors(state, cfg, cmvn, smooth_factor2, noise_threshold2))
+
+
+def seaco_model_tensors(state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: Optional[torch.Tensor] = None, no_bias: int = 8377,
+                        nfilter: int = 50, smooth_factor2: float = 0.25, noise_threshold2: float = 0.01) -> Dict[str, np.ndarray]:
+    """The tensors of a SeacoParaformer model file: everything `model_tensors` writes (the BiCif timestamp head included; decoder.embed.0
+    is the hotword embedding table), seaco_decoder.*, hotword_output_layer.* and bias_encoder.* under the reference's names, plus
+    bias_encoder.gemm_bias_l{k} = bias_ih_l{k} + bias_hh_l{k} (the input projection's GEMM bias) and __seaco_config__ [no_bias, nfilter,
+    lstm layers].  nfilter travels with the file because it is a model choice: the attention-score filter keeps that many hotwords."""
+    if any(k.startswith("lstm_proj.") for k in state):
+        raise ValueError("SeACo with bias_encoder_bid (a bidirectional hotword LSTM and lstm_proj) is not supported: the handle runs the "
+                         "unidirectional bias_encoder")
+    if any(k.startswith("bias_embed.") for k in state) or "bias_encoder.weight_ih_l0" not in state:
+        raise ValueError("SeACo with bias_encoder_type 'mean' (bias_embed, no LSTM) is not supported: the handle runs the 'lstm' "
+                         "bias_encoder")
+    if "hotword_output_layer.weight" not in state or not any(k.startswith("seaco_decoder.") for k in state):
+        raise ValueError("not a SeacoParaformer state_dict (seaco_decoder / hotword_output_layer missing)")
+    if not 0 <= int(no_bias) < cfg.vocab or int(nfilter) < 0:
+        raise ValueError("no_bias must lie inside the vocabulary and nfilter must be >= 0")
+    out = model_tensors(state, cfg, cmvn, smooth_factor2, noise_threshold2)
+    for k, v in state.items():
+        if k.startswith(("seaco_decoder.", "hotword_output_layer.")) and torch.is_floating_point(v):
+            out[k] = v.detach().float().cpu().contiguous().numpy()
+    layers = 0
+    while "bias_encoder.weight_ih_l%d" % layers in state:
+        f = lambda n: state["bias_encoder.%s_l%d" % (n, layers)].detach().float().cpu()      # noqa: E731
+        out["bias_encoder.gemm_bias_l%d" % layers] = (f("bias_ih") + f("bias_hh")).contiguous().numpy()
+        layers += 1
+    out["__seaco_config__"] = np.array([int(no_bias), int(nfilter), layers], dtype=np.float32)
+    return out
+
+
+def write_seaco_model_file(path: str, state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: Optional[torch.Tensor] = None,
+                           no_bias: int = 8377, nfilter: int = 50, smooth_factor2: float = 0.25, noise_threshold2: float = 0.01) -> int:
+    """A SeacoParaformer (`paraformer-zh`) model file for the handle: `seaco_model_tensors`.  no_bias: the model's NO_BIAS token id;
+    nfilter: the attention-score filter's hotword count (SeacoParaformer.inference's default 50)."""
+    return _write(path, seaco_model_tensors(state, cfg, cmvn, no_bias, nfilter, smooth_factor2, noise_threshold2))
 
 
 def sensevoice_model_tensors(state: Dict[str, torch.Tensor], cfg, cmvn: Optional[torch.Tensor], blank_id: int = 0) -> Dict[str, np.ndarray]:

@@ -419,6 +419,33 @@ int fa_seaco_merge(const int32_t* dec_ids, const float* dec_best, const int32_t*
                    int32_t no_bias, int32_t* out_ids, float* out_best, const float* dec_logp, const float* dha_logp,
                    float* merged, int32_t vocab, fa_stream_t stream);
 
+/* SeACo's hotword encoder (_hotword_representation, seaco_paraformer/model.py:384-420): decoder.embed, then the n_layers LSTM
+ * `bias_encoder` (512 -> 512, gate order i, f, g, o) over the packed batch, then each hotword's top-layer output at its last token.
+ * ih[k] = weight_ih_l{k} [2048, 512] with bias b_ih + b_hh [2048] (the input projection of all tokens is one GEMM), hh[k] =
+ * weight_hh_l{k} [2048, 512] without bias; in the tensor-core modes both carry their weight planes. */
+#define FA_HOTWORD_MAX_LAYERS 8
+typedef struct {
+  const float* embed;       /* [vocab, 512] */
+  int32_t vocab;
+  int32_t n_layers;         /* 1 .. FA_HOTWORD_MAX_LAYERS */
+  const FaLinear* ih;       /* [n_layers] */
+  const FaLinear* hh;       /* [n_layers] */
+} FaHotwordEncoder;
+/* ids: HOST int32, the hotwords' token ids concatenated (sum of lens entries); lens: HOST [n_hw], each >= 1.  rows: device [n_hw, 512],
+ * row i = hotword i's output.  Hotwords run longest first so that step t works on a row prefix: per layer one GEMM over all tokens, then
+ * per step one [n_t, 512] x [512, 2048] GEMM and one fused cell launch; no host synchronisation between steps.  Every id is checked
+ * against [0, vocab) on the host before anything is enqueued (FA_ERR_ARG, as for n_hw < 1, a length < 1 or a NULL pointer).  The
+ * workspace query takes n_hw and the token count (the sum of lens) and returns exactly what the forward carves. */
+/* Host only: SeACo's attention-score filter (seaco_paraformer/model.py:320-343) over utterance 0's cross-attention probabilities
+ * probs [heads, n_rows, n_hw] (fa_sanm_decoder_stack_forward's attn_probs): picked = torch.topk(probs.sum(0).sum(0),
+ * k = min(nfilter, n_hw - 1)).indices followed by n_hw - 1 (the <s> entry), with torch's CPU summation order (a cascade per column, not
+ * a left fold) and torch.topk's order among equal scores: the selected rows feed the next attention in that order.  picked holds
+ * k + 1 entries; returns k + 1, or FA_ERR_ARG (n_hw < 2, nfilter < 1, a NULL pointer). */
+int32_t fa_seaco_asf_select_host(const float* probs, int32_t heads, int32_t n_rows, int32_t n_hw, int32_t nfilter, int32_t* picked);
+size_t fa_hotword_encoder_workspace_bytes(int32_t n_hw, int64_t n_tokens, int32_t gemm_mode);
+int fa_hotword_encoder_forward(const FaHotwordEncoder* enc, const int32_t* ids, const int32_t* lens, int32_t n_hw, float* rows,
+                               int32_t gemm_mode, void* workspace, size_t ws_bytes, fa_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------
  * FSMN-VAD (funasr/models/fsmn_vad_streaming): the encoder FSMN.forward (encoder.py:355-377) over the LFR-5/1 features of a whole
  * waveform, reduced to the silence posterior per 10 ms frame that the end-point detector reads (model.py:789-792), and the frame
@@ -610,6 +637,23 @@ int32_t fa_offline_is_contextual(const void* handle);
  * predictor.cif_output2.* and __ts_config__, written by funasr_b200/pack.py): its token branch then runs CifPredictorV3's sequential
  * fp32 `cif`, and every result carries per-token stamps (fa_offline_result_stamps).  0 otherwise, or for NULL. */
 int32_t fa_offline_has_timestamps(const void* handle);
+/* SeacoParaformer (paraformer-zh; seaco_paraformer/model.py:50-581), recognised by __seaco_config__ [no_bias, nfilter, lstm layers]
+ * (funasr_b200/pack.py:write_seaco_model_file).  Before it touches a device fa_offline_init refuses, naming the piece: a file that is
+ * also contextual, decoder.embed.0.weight other than [vocab, 512], a bias_encoder weight other than [2048, 512] or bias other than
+ * [2048], fewer than 6 SeACo decoder layers or a misshapen one, hotword_output_layer other than [vocab, 512], no_bias outside
+ * [0, vocab), nfilter < 0.  fa_offline_is_seaco: 1 for such a handle, 0 otherwise or for NULL.
+ * fa_offline_hotword_embed: the hotword rows of a SeACo handle, the `hw_emb` of FunOfflineInferBuffer: ids (HOST, the hotwords' token
+ * ids concatenated) and lens [n] (HOST) -> rows_host [n, 512] (HOST), each hotword's top-layer bias_encoder output at its last token
+ * (fa_hotword_encoder_forward in the handle's gemm_mode).  The caller appends the <s> entry ({1}) as generate_hotwords_list does.  An
+ * id outside the vocabulary fails before any launch, naming the hotword; any other handle kind is refused.  FA_OK or a negative status
+ * (fa_offline_last_error()).
+ * fa_offline_infer_hw / fa_offline_infer_vad on a SeACo handle take these rows (hw_embed [n_hotwords, 512], last row the <s> entry).
+ * No rows (n_hotwords 0): the plain decoder distribution (model.py:381-382).  Otherwise _seaco_decode_with_ASF: with more rows than
+ * nfilter, the SeACo decoder's attention on utterance 0 (of each VAD pack for long audio) keeps the nfilter rows it attends to most
+ * plus the <s> row (fa_seaco_asf_select_host); the SeACo decoder over the acoustic embeddings and over the decoder's hidden states,
+ * hotword_output_layer's arg-max of their sum, and the NO_BIAS merge.  Stamps as for BiCif when the file has the timestamp head. */
+int32_t fa_offline_is_seaco(const void* handle);
+int fa_offline_hotword_embed(void* handle, const int32_t* ids, const int32_t* lens, int32_t n, float* rows_host);
 /* Host copy of a tensor of the model file by its FunASR state_dict name (e.g. "bias_embed.weight" for the hotword encoder that
  * runs on the host); owned by the handle.  NULL if absent. */
 const float* fa_offline_host_tensor(void* handle, const char* name, int64_t* numel);
