@@ -222,6 +222,25 @@ SIGNATURES = {
     "fa_gather_segments": (C.c_int, [_vp, _i64, _vp, _vp, _i32, _i64, _vp, _vp]),
     "fa_pack_segments": (_i64, [_vp, _i64, _i32, _i32, _vp, _vp]),
     "fa_merge_vad": (_i64, [_vp, _i64, _i32, _i32, _vp]),
+    # speaker diarization: the CAM++ handle and long audio (offline.cu), the clustering kernels (spk_cluster.cu), host routines (host_ops.cpp)
+    "fa_spk_init": (_vp, [C.c_char_p, _i32, _i32]),
+    "fa_spk_uninit": (None, [_vp]),
+    "fa_spk_embed": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp]),
+    "fa_spk_cluster": (C.c_int, [_vp, _vp, _i32, _i32, _vp]),
+    "fa_offline_infer_vad_spk": (_vp, [_vp, _vp, _vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp, _i32, _vp, _vp,
+                                       C.POINTER(FaLongAudioOptions), _i32]),
+    "fa_offline_result_spk": (C.POINTER(_i32), [_vp, _i32, C.POINTER(_i32)]),
+    "fa_spk_effective_pval": (C.c_double, [_i32, C.c_double]),
+    "fa_spk_laplacian_workspace_bytes": (_sz, [_i32, _i32]),
+    "fa_spk_laplacian": (C.c_int, [_vp, _i32, _i32, C.c_double, _vp, _vp, _sz, _vp]),
+    "fa_spk_tridiagonalize_workspace_bytes": (_sz, [_i32]),
+    "fa_spk_tridiagonalize": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "fa_spk_back_transform": (C.c_int, [_vp, _vp, _i32, _vp, _i32, _vp]),
+    "fa_sym_tridiag_smallest_host": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    "fa_spk_kmeans_host": (C.c_int, [_vp, _i64, _i32, _i32, C.c_uint64, _i32, _i32, _vp]),
+    "fa_spk_merge_by_cos_host": (C.c_int, [_vp, _vp, _i64, _i32, C.c_double]),
+    "fa_spk_postprocess_host": (_i64, [_vp, _vp, _i64, _vp]),
+    "fa_spk_distribute_host": (C.c_int, [_vp, _i64, _vp, _i64, _vp]),
     # handle-style CT-Transformer punctuation (offline.cu; the text walk: punc_text.cpp)
     "fa_punc_init": (_vp, [C.c_char_p, _i32]),
     "fa_punc_infer": (_vp, [_vp, C.POINTER(C.c_char_p), _i32]),

@@ -3,6 +3,8 @@
 #include "../../include/funasr_b200.h"
 
 #include <algorithm>
+#include <cstdio>
+#include <cstdlib>
 #include <cmath>
 #include <utility>
 #include <vector>
@@ -173,4 +175,343 @@ extern "C" int32_t fa_seaco_asf_select_host(const float* probs, int32_t heads, i
   for (int64_t j = 0; j < k; ++j) picked[j] = (int32_t)queue[j].second;
   picked[k] = n_hw - 1;
   return (int32_t)(k + 1);
+}
+
+// ------------------------------------------------------------------------------------------------ speaker clustering, host side
+// The parts of ClusterBackend / campplus utils.py that are small or sequential (funasr_b200/diarization.py is the specification): the
+// tridiagonal eigenproblem left by fa_spk_tridiagonalize, k-means, merge_by_cos and the label post-processing.
+namespace {
+
+// eigenvalues of T below x (Sturm sequence of the LDL^T pivots; a pivot below pivmin counts as -pivmin)
+int64_t sturm_count(const double* d, const double* e, int64_t n, double x, double pivmin) {
+  int64_t c = 0;
+  double q = d[0] - x;
+  if (std::fabs(q) < pivmin) q = -pivmin;
+  if (q < 0) ++c;
+  for (int64_t i = 1; i < n; ++i) {
+    q = d[i] - x - e[i - 1] * e[i - 1] / q;
+    if (std::fabs(q) < pivmin) q = -pivmin;
+    if (q < 0) ++c;
+  }
+  return c;
+}
+
+// deterministic generator of the host routines (splitmix64)
+struct SplitMix {
+  uint64_t s;
+  uint64_t next() {
+    uint64_t z = (s += 0x9E3779B97F4A7C15ull);
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+  }
+  double uniform() { return (double)(next() >> 11) * (1.0 / 9007199254740992.0); }
+};
+
+// T - lambda I = P L U with partial pivoting (LAPACK dlagtf's elimination): U has two superdiagonals
+struct TridiagLU {
+  std::vector<double> u0, u1, u2, l;
+  std::vector<char> piv;
+  void factor(const double* d, const double* e, int64_t n, double lambda, double tiny) {
+    u0.assign(n, 0.0); u1.assign(n, 0.0); u2.assign(n, 0.0); l.assign(n, 0.0); piv.assign(n, 0);
+    double r0 = d[0] - lambda, r1 = n > 1 ? e[0] : 0.0, r2 = 0.0;
+    for (int64_t i = 0; i + 1 < n; ++i) {
+      const double s0 = e[i], s1 = d[i + 1] - lambda, s2 = i + 2 < n ? e[i + 1] : 0.0;
+      double n0, n1;
+      if (std::fabs(s0) > std::fabs(r0)) {
+        piv[i] = 1;
+        u0[i] = s0; u1[i] = s1; u2[i] = s2;
+        l[i] = r0 / s0;
+        n0 = r1 - l[i] * s1; n1 = r2 - l[i] * s2;
+      } else {
+        if (r0 == 0.0) r0 = tiny;
+        u0[i] = r0; u1[i] = r1; u2[i] = r2;
+        l[i] = s0 / r0;
+        n0 = s1 - l[i] * r1; n1 = s2 - l[i] * r2;
+      }
+      if (std::fabs(u0[i]) < tiny) u0[i] = std::copysign(tiny, u0[i]);
+      r0 = n0; r1 = n1; r2 = 0.0;
+    }
+    u0[n - 1] = std::fabs(r0) < tiny ? std::copysign(tiny, r0) : r0;
+  }
+  void solve(double* b, int64_t n) const {
+    for (int64_t i = 0; i + 1 < n; ++i) {
+      if (piv[i]) std::swap(b[i], b[i + 1]);
+      b[i + 1] -= l[i] * b[i];
+    }
+    for (int64_t i = n - 1; i >= 0; --i) {
+      double s = b[i];
+      if (i + 1 < n) s -= u1[i] * b[i + 1];
+      if (i + 2 < n) s -= u2[i] * b[i + 2];
+      b[i] = s / u0[i];
+    }
+  }
+};
+
+double norm2(const double* x, int64_t n) {
+  double s = 0.0;
+  for (int64_t i = 0; i < n; ++i) s += x[i] * x[i];
+  return std::sqrt(s);
+}
+
+double sq_dist(const double* a, const double* b, int32_t dim) {
+  double s = 0.0;
+  for (int32_t c = 0; c < dim; ++c) {
+    const double t = a[c] - b[c];
+    s += t * t;
+  }
+  return s;
+}
+
+// Python's round(x, 2): correctly rounded, ties to even on the exact binary value (glibc's %.2f rounds the same way)
+double round2(double x) {
+  char buf[64];
+  snprintf(buf, sizeof buf, "%.2f", x);
+  return strtod(buf, nullptr);
+}
+
+struct Turn { double st, ed; int32_t spk; };
+
+// merge_seque: consecutive turns of one speaker that touch or overlap become one
+std::vector<Turn> merge_seque(const std::vector<Turn>& res) {
+  std::vector<Turn> out;
+  for (const Turn& r : res) {
+    if (out.empty() || r.spk != out.back().spk || r.st > out.back().ed) out.push_back(r);
+    else out.back().ed = r.ed;
+  }
+  return out;
+}
+
+}  // namespace
+
+// The m smallest eigenvalues w[m] (ascending) of the symmetric tridiagonal T (d [n], e [n - 1]) by bisection on Sturm counts, and
+// the eigenvectors of the first k as rows of z [k, n] by inverse iteration on T - w_j I (four solves from a fixed pseudo-random
+// start), orthogonalised by Gram-Schmidt against the earlier vectors of the same cluster (eigenvalues closer than 1e-3 ||T||): a
+// Laplacian with several connected components has a repeated eigenvalue 0.  The vectors span the eigenspaces scipy's would; within a
+// cluster the basis may differ by a rotation, and a vector by its sign.  Returns FA_OK or FA_ERR_ARG.
+extern "C" int fa_sym_tridiag_smallest_host(const double* d, const double* e, int32_t n, int32_t m, int32_t k, double* w, double* z) {
+  if (!d || n < 1 || (n > 1 && !e) || m < 1 || m > n || k < 0 || k > m || !w || (k > 0 && !z)) return FA_ERR_ARG;
+  double lo = d[0], hi = d[0], emax2 = 0.0;
+  for (int32_t i = 0; i < n; ++i) {
+    const double r = (i > 0 ? std::fabs(e[i - 1]) : 0.0) + (i + 1 < n ? std::fabs(e[i]) : 0.0);
+    lo = std::min(lo, d[i] - r);
+    hi = std::max(hi, d[i] + r);
+    if (i + 1 < n) emax2 = std::max(emax2, e[i] * e[i]);
+  }
+  const double eps = 2.220446049250313e-16, tnorm = std::max(std::fabs(lo), std::fabs(hi));
+  const double pivmin = 2.2250738585072014e-308 * std::max(1.0, emax2);
+  lo -= 2 * eps * tnorm + pivmin;
+  hi += 2 * eps * tnorm + pivmin;
+  for (int32_t i = 0; i < m; ++i) {                // the (i + 1)-th smallest: count(a) <= i < count(b)
+    double a = i > 0 ? w[i - 1] - 4 * eps * tnorm - pivmin : lo, b = hi;
+    if (sturm_count(d, e, n, a, pivmin) > i) a = lo;
+    for (int it = 0; it < 200 && b - a > 2 * eps * std::max(std::fabs(a), std::fabs(b)) + pivmin; ++it) {
+      const double mid = 0.5 * (a + b);
+      if (mid <= a || mid >= b) break;
+      if (sturm_count(d, e, n, mid, pivmin) > i) b = mid;
+      else a = mid;
+    }
+    w[i] = 0.5 * (a + b);
+  }
+  const double ortol = 1e-3 * tnorm, tiny = eps * std::max(tnorm, 1e-300);
+  TridiagLU lu;
+  int32_t first = 0;                               // the current cluster's first vector
+  for (int32_t j = 0; j < k; ++j) {
+    if (j > 0 && w[j] - w[j - 1] > ortol) first = j;
+    double* x = z + (int64_t)j * n;
+    SplitMix rng{0x5eedull + (uint64_t)j};
+    for (int32_t i = 0; i < n; ++i) x[i] = 2.0 * rng.uniform() - 1.0;
+    lu.factor(d, e, n, w[j], tiny);
+    for (int it = 0; it < 5; ++it) {
+      for (int pass = 0; pass < 2; ++pass)
+        for (int32_t q = first; q < j; ++q) {
+          const double* y = z + (int64_t)q * n;
+          double s = 0.0;
+          for (int32_t i = 0; i < n; ++i) s += x[i] * y[i];
+          for (int32_t i = 0; i < n; ++i) x[i] -= s * y[i];
+        }
+      double nx = norm2(x, n);
+      if (!(nx > 0.0)) { x[j % n] = 1.0; nx = 1.0; }
+      for (int32_t i = 0; i < n; ++i) x[i] /= nx;
+      if (it == 4) break;
+      lu.solve(x, n);
+      const double big = norm2(x, n);
+      if (std::isfinite(big) && big > 0.0)
+        for (int32_t i = 0; i < n; ++i) x[i] /= big;
+    }
+  }
+  return FA_OK;
+}
+
+// k-means on x [n, dim] (float64): k-means++ seeding and Lloyd iterations (at most max_iter, until the assignment repeats), the best
+// inertia of n_init starts (diarization.kmeans; the generator is this library's, so only the partition is comparable).  An empty
+// cluster keeps its centre.  labels [n] in 0 .. k - 1.  Returns FA_OK or FA_ERR_ARG.
+extern "C" int fa_spk_kmeans_host(const double* x, int64_t n, int32_t dim, int32_t k, uint64_t seed, int32_t n_init, int32_t max_iter,
+                                  int32_t* labels) {
+  if (!x || !labels || n < 1 || dim < 1 || k < 1 || k > n || n_init < 1 || max_iter < 1) return FA_ERR_ARG;
+  SplitMix rng{seed};
+  std::vector<double> centers((size_t)k * dim), d2((size_t)n), sums((size_t)k * dim);
+  std::vector<int32_t> lab((size_t)n), cnt((size_t)k);
+  double best = INFINITY;
+  bool have = false;
+  for (int32_t run = 0; run < n_init; ++run) {
+    const int64_t i0 = (int64_t)(rng.next() % (uint64_t)n);
+    std::copy(x + i0 * dim, x + (i0 + 1) * dim, centers.begin());
+    for (int64_t i = 0; i < n; ++i) d2[i] = sq_dist(x + i * dim, centers.data(), dim);
+    for (int32_t j = 1; j < k; ++j) {
+      double tot = 0.0;
+      for (int64_t i = 0; i < n; ++i) tot += d2[i];
+      int64_t pick = (int64_t)(rng.next() % (uint64_t)n);
+      if (tot > 0.0) {
+        const double r = rng.uniform() * tot;
+        double c = 0.0;
+        for (int64_t i = 0; i < n; ++i) {
+          if (d2[i] > 0.0) pick = i;
+          c += d2[i];
+          if (c > r && d2[i] > 0.0) break;
+        }
+      }
+      std::copy(x + pick * dim, x + (pick + 1) * dim, centers.begin() + (size_t)j * dim);
+      for (int64_t i = 0; i < n; ++i) d2[i] = std::min(d2[i], sq_dist(x + i * dim, centers.data() + (size_t)j * dim, dim));
+    }
+    for (int32_t it = 0; it < max_iter; ++it) {
+      bool changed = it == 0;
+      for (int64_t i = 0; i < n; ++i) {
+        int32_t arg = 0;
+        double dm = INFINITY;
+        for (int32_t j = 0; j < k; ++j) {
+          const double t = sq_dist(x + i * dim, centers.data() + (size_t)j * dim, dim);
+          if (t < dm) { dm = t; arg = j; }
+        }
+        if (lab[i] != arg) changed = true;
+        lab[i] = arg;
+      }
+      if (!changed) break;
+      std::fill(sums.begin(), sums.end(), 0.0);
+      std::fill(cnt.begin(), cnt.end(), 0);
+      for (int64_t i = 0; i < n; ++i) {
+        ++cnt[lab[i]];
+        for (int32_t c = 0; c < dim; ++c) sums[(size_t)lab[i] * dim + c] += x[i * dim + c];
+      }
+      for (int32_t j = 0; j < k; ++j)
+        if (cnt[j] > 0)
+          for (int32_t c = 0; c < dim; ++c) centers[(size_t)j * dim + c] = sums[(size_t)j * dim + c] / cnt[j];
+    }
+    double inertia = 0.0;
+    for (int64_t i = 0; i < n; ++i) inertia += sq_dist(x + i * dim, centers.data() + (size_t)lab[i] * dim, dim);
+    if (!have || inertia < best) {
+      best = inertia;
+      have = true;
+      std::copy(lab.begin(), lab.end(), labels);
+    }
+  }
+  return FA_OK;
+}
+
+// ClusterBackend.merge_by_cos: while two clusters' mean embeddings (emb [n, dim] fp32) have a cosine of at least thr, the pair with
+// the largest cosine (first in row-major order) merges into the lower label and the labels above close up.  labels in place.
+extern "C" int fa_spk_merge_by_cos_host(int32_t* labels, const float* emb, int64_t n, int32_t dim, double thr) {
+  if (!labels || !emb || n < 1 || dim < 1) return FA_ERR_ARG;
+  for (;;) {
+    int32_t spk = 0;
+    for (int64_t i = 0; i < n; ++i) {
+      if (labels[i] < 0) return FA_ERR_ARG;
+      spk = std::max(spk, labels[i] + 1);
+    }
+    if (spk <= 1) break;
+    std::vector<double> c((size_t)spk * dim, 0.0);
+    std::vector<int64_t> cnt((size_t)spk, 0);
+    for (int64_t i = 0; i < n; ++i) {
+      ++cnt[labels[i]];
+      for (int32_t t = 0; t < dim; ++t) c[(size_t)labels[i] * dim + t] += emb[i * dim + t];
+    }
+    for (int32_t s = 0; s < spk; ++s) {              // an empty label's centre is NaN, as numpy's mean of nothing
+      double nn = 0.0;
+      for (int32_t t = 0; t < dim; ++t) c[(size_t)s * dim + t] /= (double)cnt[s];
+      for (int32_t t = 0; t < dim; ++t) nn += c[(size_t)s * dim + t] * c[(size_t)s * dim + t];
+      nn = std::sqrt(nn);
+      for (int32_t t = 0; t < dim; ++t) c[(size_t)s * dim + t] /= nn;
+    }
+    int32_t a = 0, b = 0;
+    double bestv = 0.0;                              // np.triu(aff, 1): the zeroed entries take part in the arg-max
+    bool nan = false;
+    for (int32_t i = 0; i < spk && !nan; ++i)
+      for (int32_t j = i + 1; j < spk; ++j) {
+        double v = 0.0;
+        for (int32_t t = 0; t < dim; ++t) v += c[(size_t)i * dim + t] * c[(size_t)j * dim + t];
+        if (std::isnan(v)) { a = i; b = j; nan = true; break; }   // np.argmax stops at the first NaN, and NaN < thr is false
+        if (v > bestv) { bestv = v; a = i; b = j; }
+      }
+    if (!nan && (a == b ? 0.0 : bestv) < thr) break;
+    if (a == b) break;
+    for (int64_t i = 0; i < n; ++i) {
+      if (labels[i] == b) labels[i] = a;
+      else if (labels[i] > b) labels[i] -= 1;
+    }
+  }
+  return FA_OK;
+}
+
+// postprocess (campplus utils.py): chunks [n][2] seconds in time order with their labels -> speaker turns [<= n][3] (start_s, end_s,
+// speaker): labels renumbered in order of first appearance (correct_labels), merge_seque, overlapping turns meet at the midpoint,
+// then smooth (times rounded to 2 decimals as Python's round, turns shorter than 0.7 s take a neighbour's speaker, merge_seque
+// again).  Returns the number of turns, or FA_ERR_ARG.
+extern "C" int64_t fa_spk_postprocess_host(const double* chunks, const int32_t* labels, int64_t n, double* turns) {
+  if (n < 1 || !chunks || !labels || !turns) return FA_ERR_ARG;
+  std::vector<int32_t> seen;
+  std::vector<Turn> res;
+  for (int64_t i = 0; i < n; ++i) {
+    auto it = std::find(seen.begin(), seen.end(), labels[i]);
+    const int32_t l = (int32_t)(it - seen.begin());
+    if (it == seen.end()) seen.push_back(labels[i]);
+    res.push_back(Turn{chunks[2 * i], chunks[2 * i + 1], l});
+  }
+  res = merge_seque(res);
+  for (size_t i = 1; i < res.size(); ++i)
+    if (res[i - 1].ed > res[i].st + 1e-4) {
+      const double p = (res[i].st + res[i - 1].ed) / 2;
+      res[i].st = p;
+      res[i - 1].ed = p;
+    }
+  if (res.size() >= 2) {                             // smooth; a single turn is returned unrounded
+    const double mindur = 0.7;
+    const size_t m = res.size();
+    for (size_t i = 0; i < m; ++i) {
+      res[i].st = round2(res[i].st);
+      res[i].ed = round2(res[i].ed);
+      if (res[i].ed - res[i].st < mindur) {
+        if (i == 0) res[i].spk = res[i + 1].spk;
+        else if (i == m - 1) res[i].spk = res[i - 1].spk;
+        else if (res[i].st - res[i - 1].ed <= res[i + 1].st - res[i].ed) res[i].spk = res[i - 1].spk;
+        else res[i].spk = res[i + 1].spk;
+      }
+    }
+    res = merge_seque(res);
+  }
+  for (size_t i = 0; i < res.size(); ++i) {
+    turns[3 * i] = res[i].st;
+    turns[3 * i + 1] = res[i].ed;
+    turns[3 * i + 2] = res[i].spk;
+  }
+  return (int64_t)res.size();
+}
+
+// distribute_spk: every sentence {start_ms, end_ms} (sentences [ns][2]) takes the speaker whose turns (turns [nt][3], seconds) overlap
+// it most, with the reference's running tally (a turn of the leading speaker adds its overlap again).  spk [ns].
+extern "C" int fa_spk_distribute_host(const int32_t* sentences, int64_t ns, const double* turns, int64_t nt, int32_t* spk) {
+  if (ns < 0 || nt < 0 || (ns > 0 && (!sentences || !spk)) || (nt > 0 && !turns)) return FA_ERR_ARG;
+  for (int64_t s = 0; s < ns; ++s) {
+    const double s0 = sentences[2 * s], s1 = sentences[2 * s + 1];
+    int32_t best = 0;
+    double max_ov = 0.0;
+    for (int64_t t = 0; t < nt; ++t) {
+      const double st = turns[3 * t] * 1000, ed = turns[3 * t + 1] * 1000;
+      const int32_t sp = (int32_t)turns[3 * t + 2];
+      const double ov = std::max(std::min(s1, ed) - std::max(s0, st), 0.0);
+      if (ov > max_ov) { max_ov = ov; best = sp; }
+      if (ov > 0 && best == sp) max_ov += ov;
+    }
+    spk[s] = best;
+  }
+  return FA_OK;
 }

@@ -5,7 +5,8 @@ Nothing here touches torch on the data path: host PCM buffers in, token ids out.
 batch by batch, the same results as LongAudioPipeline.generate.  A BiCifParaformer model file adds per-token [start_ms, end_ms] stamps
 (`infer_stamped`, and "timestamp" in `infer_long`'s results); a SeacoParaformer model file takes hotword rows from
 `hotword_embeddings` (its hotword encoder on the GPU).  `OfflinePunc` binds the CT-Transformer punctuation handle (fa_punc_*),
-and `punc_walk_host` its text walk with any scorer in place of the network."""
+and `punc_walk_host` its text walk with any scorer in place of the network.  `OfflineSpeaker` binds the CAM++ speaker handle (fa_spk_*);
+passed to `infer_long(spk=...)` it diarizes long audio (fa_offline_infer_vad_spk)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -176,6 +177,39 @@ def sv_query_ids(n: int, language=None, use_itn=None):
     return lid, np.array([tn["withitn" if v else "woitn"] for v in itns], dtype=np.int32)
 
 
+class OfflineSpeaker:
+    """CAM++ speaker embeddings through the C handle (fa_spk_init / fa_spk_embed) from a pack.write_campplus_model_file file; pass it
+    to OfflineRecognizer.infer_long(spk=...) to diarize long audio."""
+
+    def __init__(self, model_file: str, device: int = 0, gemm_mode: str = "fp32"):
+        self.lib = _abi.load()
+        self.handle = self.lib.fa_spk_init(model_file.encode(), int(device), _abi.GEMM_MODES[gemm_mode])
+        if not self.handle:
+            raise _abi.FunasrB200Error("fa_spk_init failed: %s" % self.lib.fa_offline_last_error().decode())
+
+    def embed(self, wavs: Sequence[np.ndarray]) -> np.ndarray:
+        """Ragged recordings (float32 in [-1, 1] or int16, 16 kHz) -> [B, 192] float32, CAMPPlusB200.inference's embeddings."""
+        arrs, fmt = _pcm_batch(wavs)
+        n = len(arrs)
+        ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
+        lens = (C.c_int64 * n)(*[a.shape[0] for a in arrs])
+        out = np.empty((n, 192), dtype=np.float32)
+        if self.lib.fa_spk_embed(self.handle, ptrs, lens, n, fmt, out.ctypes.data) != 0:
+            raise _abi.FunasrB200Error("fa_spk_embed failed: %s" % self.lib.fa_offline_last_error().decode())
+        return out
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self.lib.fa_spk_uninit(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class OfflineRecognizer:
     def __init__(self, model_file: str, device: int = 0, gemm_mode: str = "fp16x3"):
         self.lib = _abi.load()
@@ -263,12 +297,15 @@ class OfflineRecognizer:
 
     def infer_long(self, wavs: Sequence[np.ndarray], vad: OfflineVad, batch_size_s: int = 300, batch_size_threshold_s: int = 60,
                    merge_vad: bool = False, merge_length_s: int = 15, hotword_embeddings: Optional[np.ndarray] = None,
-                   language=None, use_itn=None, **vad_kwargs) -> List[dict]:
+                   language=None, use_itn=None, spk: Optional["OfflineSpeaker"] = None, preset_spk_num: Optional[int] = None,
+                   **vad_kwargs) -> List[dict]:
         """Long recordings through fa_offline_infer_vad, each on its own as LongAudioPipeline.generate treats it -> per recording
         {"token_int": ids in time order, "vad_segments": [[start_ms, end_ms], ...], "n_tokens": tokens per segment}, plus
         "timestamp": [[start_ms, end_ms], ...] in absolute ms when the model has the timestamp head (`has_timestamps`).
         hotword_embeddings: [n, 512] float32 rows (ContextualParaformer or SeACo; last row the <s> entry).  SenseVoice model file
-        (fa_offline_infer_vad_sv): language / use_itn as in `infer`, one per recording, applied to all its segments."""
+        (fa_offline_infer_vad_sv): language / use_itn as in `infer`, one per recording, applied to all its segments.
+        spk (an OfflineSpeaker on the same device): fa_offline_infer_vad_spk also diarizes every recording that decoded a token and adds
+        "spk", one speaker per VAD segment (vad_segment mode), with preset_spk_num as LongAudioPipeline.generate takes it."""
         arrs, fmt = _pcm_batch(wavs)
         n = len(arrs)
         ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
@@ -280,7 +317,11 @@ class OfflineRecognizer:
             hw = np.ascontiguousarray(hotword_embeddings, dtype=np.float32)
             n_hw = hw.shape[0]
         q = self._queries(n, language, use_itn)
-        if q is None:
+        if spk is not None:
+            res = self.lib.fa_offline_infer_vad_spk(self.handle, vad.handle, spk.handle, ptrs, lens, n, fmt, None if hw is None else hw.ctypes.data,
+                                                    n_hw, None if q is None else q[0].ctypes.data, None if q is None else q[1].ctypes.data,
+                                                    C.byref(opts), int(preset_spk_num or 0))
+        elif q is None:
             res = self.lib.fa_offline_infer_vad(self.handle, vad.handle, ptrs, lens, n, fmt, None if hw is None else hw.ctypes.data, n_hw,
                                                 C.byref(opts))
         else:
@@ -299,6 +340,9 @@ class OfflineRecognizer:
                 out.append({"token_int": ids, "vad_segments": [t[:2] for t in trip], "n_tokens": [t[2] for t in trip]})
                 if stamped:
                     out[-1]["timestamp"] = self._stamps(res, i)
+                if spk is not None:
+                    p = self.lib.fa_offline_result_spk(res, i, C.byref(cnt))
+                    out[-1]["spk"] = [int(p[k]) for k in range(cnt.value)]
             self.last_audio_seconds = float(self.lib.fa_offline_result_audio_seconds(res))
             return out
         finally:

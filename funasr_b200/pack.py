@@ -49,6 +49,14 @@ reference's names, the frontend tables and encoder.pe_inv_timescales of the Para
 
     __sv_config__                      [9] enc_layers, tp_layers, d_model, heads, fsmn kernel, vocab, feat_dim, ln_eps, blank_id
 
+The CAM++ speaker file (csrc/offline.cu: fa_spk_init, recognised by __spk_config__) holds every CAMPPlus state_dict tensor
+(head.*, xvector.*) under the reference's names, unfolded and without num_batches_tracked, frontend.mel_banks [80, 257] and the povey
+window frontend.window [400] (torchaudio kaldi.fbank's defaults), and
+
+    __spk_config__                     [5] feat_dim 80, embedding 192, growth 32, bn_size 4, init_channels 128
+
+The handle folds the BatchNorms itself, in float64, the same way CampplusEngine does.
+
 Layout: b"FAB2MDL1", u32 n_tensors, then per tensor: u32 name_len, name (utf-8), u32 ndim, i64 dims[ndim], u64 nbytes,
 zero padding to a 16-byte file offset, little-endian fp32 data.
 """
@@ -150,6 +158,32 @@ def sensevoice_model_tensors(state: Dict[str, torch.Tensor], cfg, cmvn: Optional
         if k.startswith(("encoder.", "ctc.", "embed.")) and torch.is_floating_point(v):
             out[k] = v.detach().float().cpu().contiguous().numpy()
     return out
+
+
+def campplus_model_tensors(state: Dict[str, torch.Tensor]) -> Dict[str, np.ndarray]:
+    """The CAM++ speaker file's tensors; refuses any state_dict that is not CAMPPlusB200's template.yaml shape."""
+    from .campplus import BN_CH, EMB_DIM, FEAT_DIM, GROWTH, INIT_CH, campplus_specs, povey_window
+    from .engine import kaldi_mel_banks
+    out: Dict[str, np.ndarray] = {}
+    for name, shape in campplus_specs().items():
+        if name.endswith("num_batches_tracked"):
+            continue
+        if name not in state:
+            raise ValueError("CAM++ state_dict lacks %s (CAMPPlusB200 is built for the template.yaml shape: feat 80, embedding 192, "
+                             "growth 32, bn_size 4, init 128)" % name)
+        v = state[name]
+        if tuple(v.shape) != tuple(shape):
+            raise ValueError("CAM++ tensor %s has shape %s, the template.yaml shape needs %s" % (name, tuple(v.shape), tuple(shape)))
+        out[name] = v.detach().float().cpu().contiguous().numpy()
+    out["frontend.mel_banks"] = kaldi_mel_banks().numpy()
+    out["frontend.window"] = povey_window().numpy()
+    out["__spk_config__"] = np.array([FEAT_DIM, EMB_DIM, GROWTH, BN_CH // GROWTH, INIT_CH], dtype=np.float32)
+    return out
+
+
+def write_campplus_model_file(state: Dict[str, torch.Tensor], path: str) -> int:
+    """CAMPPlus state_dict -> the speaker handle's model file (fa_spk_init)."""
+    return _write(path, campplus_model_tensors(state))
 
 
 def write_sensevoice_model_file(path: str, state: Dict[str, torch.Tensor], cfg, cmvn: Optional[torch.Tensor] = None, blank_id: int = 0) -> int:

@@ -761,6 +761,67 @@ int64_t fa_pack_segments(const int32_t* segments, int64_t n, int32_t batch_size_
  * count, or FA_ERR_ARG. */
 int64_t fa_merge_vad(const int32_t* segments, int64_t n, int32_t max_length_ms, int32_t min_length_ms, int32_t* out);
 
+/* ---- Speaker diarization (CAMPPlus, campplus/model.py; ClusterBackend and the post-processing of campplus/cluster_backend.py and
+ * utils.py; funasr_b200/diarization.py and long_audio.py are the specification)
+ * fa_spk_init: model file written by funasr_b200/pack.py:write_campplus_model_file (the CAMPPlus state_dict under its own names,
+ * unfolded, the povey-window fbank tables and __spk_config__ [80, 192, 32, 4, 128]).  Refused before any device is touched, naming the
+ * piece: a missing or misshapen tensor, another __spk_config__, a file that also carries another model kind's config.  The BatchNorms
+ * are folded on the host in float64 exactly as CampplusEngine folds them, so embeddings are bit-identical to it in every gemm_mode.
+ * fa_spk_embed: batch HOST recordings (pcm_format 0 = float32, 1 = s16le; 16 kHz; ragged) -> emb_host [batch, 192]: CAMPPlus.inference
+ * (features zero-padded to the longest input, the padded frames taking part in every mean; fa_campplus_features, fa_campplus_forward in
+ * slices of 1 GiB of workspace).  An input under 400 samples (FA_ERR_ARG) or with more than 18 800 feature frames (FA_ERR_UNSUPPORTED)
+ * fails the call before any launch, naming the input.  FA_OK or a negative status (fa_offline_last_error()).
+ * fa_spk_cluster: ClusterBackend()(emb_host [n, 192], oracle_num = preset_spk_num > 0 ? preset_spk_num : None) -> labels [n] (before
+ * correct_labels): fewer than 20 rows one speaker; fewer than 2048 the spectral path (fa_spk_laplacian, fa_spk_tridiagonalize,
+ * fa_sym_tridiag_smallest_host, fa_spk_back_transform, the eigengap count unless preset, k-means); 2048 or more k-means on the
+ * normalised rows with a preset count, and without one FA_ERR_UNSUPPORTED (the reference's UMAP + HDBSCAN path is not provided);
+ * merge_by_cos at 0.78 when no count is preset. */
+void* fa_spk_init(const char* model_file, int32_t device, int32_t gemm_mode);
+void fa_spk_uninit(void* spk);
+int fa_spk_embed(void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format, float* emb_host);
+int fa_spk_cluster(void* spk, const float* emb_host, int32_t n, int32_t preset_spk_num, int32_t* labels);
+/* fa_offline_infer_vad (language_ids / textnorm_ids: fa_offline_infer_vad_sv's, NULL except on SenseVoice) followed, for every
+ * recording that decoded at least one token, by LongAudioPipeline.generate's diarization in vad_segment mode: sv_chunk's 1.5 s windows
+ * every 0.75 s over each VAD segment (the last pulled back), gathered from the device-resident recording with zero tails
+ * (fa_gather_segments) and embedded in slices, clustered as fa_spk_cluster (preset_spk_num <= 0: none), post-processed (postprocess,
+ * distribute_spk) -> one speaker per segment: fa_offline_result_spk.  spk must live on the recogniser's device.  NULL on error. */
+void* fa_offline_infer_vad_spk(void* asr, void* vad, void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch,
+                               int32_t pcm_format, const float* hw_embed, int32_t n_hotwords, const int32_t* language_ids,
+                               const int32_t* textnorm_ids, const FaLongAudioOptions* opts, int32_t preset_spk_num);
+/* n speakers of recording `index`, one per segment in fa_offline_result_segments' order (labels in order of first appearance); NULL
+ * with 0 for a recording that was not diarized and for results of the other entry points. */
+const int32_t* fa_offline_result_spk(const void* result, int32_t index, int32_t* n);
+/* p-pruning's effective pval for n rows (SpectralCluster.p_pruning): 6 / n when n * pval < 6, else pval (float64). */
+double fa_spk_effective_pval(int32_t n, double pval);
+/* SpectralCluster.sim_mat -> p_pruning -> 0.5 (P + P^T) -> laplacian over device embeddings emb [n, dim] fp32 (1 <= n <= 2047,
+ * dim <= 1024): rows L2-normalised (a zero norm counts as 1), cosine similarity in fp32, per row the int((1 - pval') n) smallest
+ * entries zeroed (pval' = fa_spk_effective_pval(n, pval); one CTA sorts each row's keys; equal values are taken in column order, the
+ * one place where numpy's unstable argsort may pick others), symmetrised, zero diagonal, D - M -> lap [n, n] float64 (device).
+ * Workspace: fa_spk_laplacian_workspace_bytes (0 for an unsupported shape). */
+size_t fa_spk_laplacian_workspace_bytes(int32_t n, int32_t dim);
+int fa_spk_laplacian(const float* emb, int32_t n, int32_t dim, double pval, double* lap, void* workspace, size_t ws_bytes, fa_stream_t stream);
+/* Householder tridiagonalisation (LAPACK dsytd2, lower, unblocked) of the symmetric lap [n, n] float64 in place (n <= 2047):
+ * T = Q^T lap Q with diagonal d [n] and off-diagonal e [n - 1]; Q = H(0) ... H(n - 2), H(j) = I - tau[j] v v^T, v = (1, lap[j][j+2:])
+ * kept in row j (and column j) of lap.  Three launches per column, no grid-wide synchronisation; deterministic.  Device arrays. */
+size_t fa_spk_tridiagonalize_workspace_bytes(int32_t n);
+int fa_spk_tridiagonalize(double* lap, int32_t n, double* d, double* e, double* tau, void* workspace, size_t ws_bytes, fa_stream_t stream);
+/* z [k, n] (device, one tridiagonal eigenvector per row) := Q z with fa_spk_tridiagonalize's reflectors (lap, tau): the eigenvectors
+ * of the Laplacian.  One CTA per vector. */
+int fa_spk_back_transform(const double* lap, const double* tau, int32_t n, double* z, int32_t k, fa_stream_t stream);
+/* Host only.  The m smallest eigenvalues w [m] of the symmetric tridiagonal (d [n], e [n - 1]) by bisection with Sturm counts, and the
+ * eigenvectors of the first k (k <= m) as rows of z [k, n] by inverse iteration, Gram-Schmidt within clusters of close eigenvalues. */
+int fa_sym_tridiag_smallest_host(const double* d, const double* e, int32_t n, int32_t m, int32_t k, double* w, double* z);
+/* Host only: k-means++ seeding, Lloyd iterations (at most max_iter), the best inertia of n_init starts, float64, from this library's
+ * generator seeded by seed: x [n, dim] -> labels [n]. */
+int fa_spk_kmeans_host(const double* x, int64_t n, int32_t dim, int32_t k, uint64_t seed, int32_t n_init, int32_t max_iter, int32_t* labels);
+/* Host only: ClusterBackend.merge_by_cos over emb [n, dim] fp32 with threshold thr; labels [n] in place. */
+int fa_spk_merge_by_cos_host(int32_t* labels, const float* emb, int64_t n, int32_t dim, double thr);
+/* Host only: postprocess (correct_labels, merge_seque, overlap midpoint, smooth with Python's round(x, 2)) of chunks [n][2] seconds
+ * and labels [n] -> turns [<= n][3] (start_s, end_s, speaker); returns the turn count or FA_ERR_ARG. */
+int64_t fa_spk_postprocess_host(const double* chunks, const int32_t* labels, int64_t n, double* turns);
+/* Host only: distribute_spk: sentences [ns][2] {start_ms, end_ms} -> spk [ns], the speaker of the turns [nt][3] overlapping most. */
+int fa_spk_distribute_host(const int32_t* sentences, int64_t ns, const double* turns, int64_t nt, int32_t* spk);
+
 /* ---- CT-Transformer punctuation (CTTransformer.inference, ct_transformer/model.py:309-473; funasr_b200/punc.py is the specification)
  * fa_punc_init: model file written by funasr_b200/pack.py:write_punc_model_file (the reference's state_dict names, __punc_config__ and
  * both lists).  Refused before any device is touched, naming the piece: d_model > 512 (the encoder workspace bound), a head dim that
