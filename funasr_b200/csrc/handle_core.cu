@@ -1,0 +1,174 @@
+// Core of the handle-style C API (handle.h): the model-file loader, the SAN-M stack binder, the upload of host PCM and the device
+// gather of recording segments.
+#include "handle.h"
+#include <stdio.h>
+#include <string.h>
+
+namespace {
+
+bool read_exact(FILE* f, void* dst, size_t n) { return fread(dst, 1, n, f) == n; }
+
+__global__ void pcm16_to_f32_kernel(const int16_t* __restrict__ src, float* __restrict__ dst, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = (float)src[i] * (1.0f / 32768.0f);     // exact; the frontend multiplies by 32768 again (wav_frontend.py:169)
+}
+
+// four consecutive output columns per thread: scalar reads (a segment starts anywhere), one 16-byte store
+__global__ void __launch_bounds__(256)
+gather_segments_kernel(const float* __restrict__ rec, int64_t n_rec, const int64_t* __restrict__ starts, const int32_t* __restrict__ lens,
+                       int64_t stride, float* __restrict__ out) {
+  const int r = blockIdx.y;
+  const int64_t c = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+  if (c >= stride) return;
+  const int64_t s = starts[r];
+  const int32_t len = lens[r];
+  float v[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int64_t j = c + k, src = s + j;
+    v[k] = (j < len && src >= 0 && src < n_rec) ? rec[src] : 0.f;
+  }
+  *reinterpret_cast<float4*>(out + (int64_t)r * stride + c) = make_float4(v[0], v[1], v[2], v[3]);
+}
+
+}  // namespace
+
+namespace fa_handle {
+
+thread_local std::string g_err;
+
+bool sync_stream(cudaStream_t st) {
+  if (cudaStreamSynchronize(st) == cudaSuccess) return true;
+  set_err(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError()));
+  return false;
+}
+
+bool load_file(std::map<std::string, Tensor>& tensors, const char* path, bool to_device) {
+  FILE* f = fopen(path, "rb");
+  if (!f) { set_err(std::string("cannot open ") + path); return false; }
+  char magic[8];
+  uint32_t n = 0;
+  long fsize = 0;
+  if (fseek(f, 0, SEEK_END) == 0) fsize = ftell(f);
+  rewind(f);
+  bool ok = fsize > 0 && read_exact(f, magic, 8) && memcmp(magic, "FAB2MDL1", 8) == 0 && read_exact(f, &n, 4);
+  std::vector<float> host;
+  for (uint32_t i = 0; ok && i < n; ++i) {
+    uint32_t nl = 0, nd = 0;
+    uint64_t nbytes = 0;
+    ok = read_exact(f, &nl, 4) && nl < 4096;
+    std::string name(ok ? nl : 0, '\0');
+    ok = ok && read_exact(f, &name[0], nl) && read_exact(f, &nd, 4) && nd <= 8;
+    Tensor tt;
+    tt.shape.resize(nd);
+    ok = ok && (nd == 0 || read_exact(f, tt.shape.data(), 8 * nd)) && read_exact(f, &nbytes, 8);
+    if (!ok) break;
+    const long pos = ftell(f);
+    const long pad = (16 - pos % 16) % 16;
+    ok = fseek(f, pad, SEEK_CUR) == 0 && nbytes == (uint64_t)tt.numel() * 4 &&
+         pos + pad <= fsize && nbytes <= (uint64_t)(fsize - (pos + pad));   // the payload lies inside the file: a corrupt size cannot drive an allocation
+    if (!ok) break;
+    if (name.compare(0, 2, "__") == 0) {
+      tt.host.resize(nbytes / 4);
+      ok = read_exact(f, tt.host.data(), nbytes);
+    } else if (!to_device) {
+      ok = fseek(f, (long)nbytes, SEEK_CUR) == 0;
+    } else {
+      host.resize(nbytes / 4);
+      ok = read_exact(f, host.data(), nbytes);
+      if (!ok) break;
+      if (cudaMalloc(&tt.dev, nbytes ? nbytes : 4) != cudaSuccess) { ok = false; set_err("cudaMalloc failed for " + name); break; }
+      cudaMemcpy(tt.dev, host.data(), nbytes, cudaMemcpyHostToDevice);
+    }
+    if (!ok) break;
+    tensors[name] = tt;
+  }
+  fclose(f);
+  if (!ok && g_err.empty()) set_err(std::string("malformed model file ") + path);
+  return ok;
+}
+
+// SANMEncoder keeps its first layer (input width -> d_model) apart as encoders0.0 (sanm/encoder.py:188-461); SenseVoice's
+// tp_encoders are one plain list
+std::string enc_layer_prefix(bool tp, int i) {
+  if (tp) return "encoder.tp_encoders." + std::to_string(i);
+  return i == 0 ? "encoder.encoders0.0" : "encoder.encoders." + std::to_string(i - 1);
+}
+
+// QKV [3D, in], FSMN [D, 1, K] with layer 0's K in every layer, FFN [F, D] / [D, F] with F <= 2048 (enc_carve's bound).  The main
+// stack takes the position encoding and ends in encoder.after_norm; SenseVoice's tp stack (D in, possibly empty) in encoder.tp_norm.
+void bind_stack(Builder& b, bool tp, int n, int in, int D, int heads, std::vector<FaEncLayer>& L, FaEncoder& e) {
+  auto norm = [&](const std::string& p, int64_t w) {
+    b.shaped(p + ".weight", {w}); b.shaped(p + ".bias", {w});
+    return b.norm(p);
+  };
+  auto lin = [&](const std::string& p, int64_t out, int64_t k) {
+    b.shaped(p + ".weight", {out, k}); b.shaped(p + ".bias", {out});
+    return b.lin(p);
+  };
+  const Tensor* k0 = n > 0 ? b.get(enc_layer_prefix(tp, 0) + ".self_attn.fsmn_block.weight") : nullptr;
+  const int64_t K = k0 && k0->shape.size() == 3 ? k0->shape[2] : 0;
+  L.assign(n > 0 ? n : 1, FaEncLayer{});
+  for (int i = 0; i < n; ++i) {
+    const std::string p = enc_layer_prefix(tp, i);
+    const int64_t x = i == 0 ? in : D;
+    const Tensor* w1 = b.get(p + ".feed_forward.w_1.weight");
+    const int64_t F = w1 && w1->shape.size() == 2 ? w1->shape[0] : 0;
+    if (w1 && (F < 1 || F > 2048)) b.refuse("bad shape of " + p + ".feed_forward.w_1.weight (at most 2048 units)");
+    L[i].norm1 = norm(p + ".norm1", x); L[i].norm2 = norm(p + ".norm2", D);
+    L[i].qkv = lin(p + ".self_attn.linear_q_k_v", 3 * D, x); L[i].out = lin(p + ".self_attn.linear_out", D, D);
+    b.shaped(p + ".self_attn.fsmn_block.weight", {D, 1, K});
+    L[i].fsmn_w = b.ptr(p + ".self_attn.fsmn_block.weight");
+    L[i].w1 = lin(p + ".feed_forward.w_1", F, D); L[i].w2 = lin(p + ".feed_forward.w_2", D, F);
+  }
+  e = FaEncoder{};
+  e.layers = L.data(); e.n_layers = n; e.heads = heads; e.fsmn_k = (int)K;
+  if (n > 0) e.after_norm = norm(tp ? "encoder.tp_norm" : "encoder.after_norm", D);
+  if (!tp) {
+    b.shaped("encoder.pe_inv_timescales", {in / 2});
+    e.pe_inv_timescales = b.ptr("encoder.pe_inv_timescales");
+  }
+}
+
+bool upload(const void* const* bufs, const int64_t* n, int B, int64_t stride, int32_t pcm_format, DevBuf& buf, cudaStream_t st, float** wav) {
+  const int64_t tot = (int64_t)B * stride;
+  int16_t* p16 = nullptr;
+  if (!carve(buf, "waveforms", [&](fa::Arena& a) {
+        *wav = a.take<float>((size_t)(tot > 0 ? tot : 4));
+        if (pcm_format == 1) p16 = a.take<int16_t>((size_t)tot);
+      }))
+    return false;
+  if (tot == 0) return true;
+  if (pcm_format == 1) {
+    for (int i = 0; i < B; ++i) cudaMemcpyAsync(p16 + (int64_t)i * stride, bufs[i], (size_t)n[i] * 2, cudaMemcpyHostToDevice, st);
+    pcm16_to_f32_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(p16, *wav, tot);
+  } else {
+    for (int i = 0; i < B; ++i) cudaMemcpyAsync(*wav + (int64_t)i * stride, bufs[i], (size_t)n[i] * 4, cudaMemcpyHostToDevice, st);
+  }
+  return true;
+}
+
+bool gather(const float* rec, int64_t n, const int64_t* starts, const int32_t* lens, int rows, int64_t stride, int64_t* starts_d,
+            int32_t* lens_d, float* out, cudaStream_t st) {
+  cudaMemcpyAsync(starts_d, starts, (size_t)rows * 8, cudaMemcpyHostToDevice, st);
+  cudaMemcpyAsync(lens_d, lens, (size_t)rows * 4, cudaMemcpyHostToDevice, st);
+  const int rc = fa_gather_segments(rec, n, starts_d, lens_d, rows, stride, out, st);
+  if (rc != FA_OK) { set_err(std::string("fa_gather_segments: ") + fa_status_string(rc)); return false; }
+  return true;
+}
+
+}  // namespace fa_handle
+
+extern "C" const char* fa_offline_last_error(void) { return fa_handle::g_err.c_str(); }
+
+extern "C" int fa_gather_segments(const float* rec, int64_t n_rec, const int64_t* starts, const int32_t* lens, int32_t rows, int64_t stride,
+                                  float* out, fa_stream_t stream) {
+  if (rows < 0 || rows > 65535 || n_rec < 0 || (rows > 0 && (!rec || !starts || !lens || !out || stride <= 0))) return FA_ERR_ARG;
+  if (rows == 0) return FA_OK;
+  if (stride % 4 || reinterpret_cast<uintptr_t>(out) % 16) return FA_ERR_UNSUPPORTED;
+  const int64_t blocks = (stride / 4 + 255) / 256;
+  if (blocks > 0x7fffffffLL) return FA_ERR_ARG;
+  gather_segments_kernel<<<dim3((unsigned)blocks, (unsigned)rows), 256, 0, (cudaStream_t)stream>>>(rec, n_rec, starts, lens, stride, out);
+  FA_CHECK_LAUNCH();
+  return FA_OK;
+}

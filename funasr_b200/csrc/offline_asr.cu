@@ -1,0 +1,588 @@
+// Handle-style offline recogniser over the kernels of this library — the C-ABI counterpart of FunASR's C++ runtime surface
+// (runtime/onnxruntime/include/funasrruntime.h:100-116: FunOfflineInit / FunOfflineInferBuffer / FunASRGetResult / FunASRFreeResult /
+// FunOfflineUninit; its Paraformer::Forward is the same op chain with ONNX Runtime in the middle, runtime/onnxruntime/src/paraformer.cpp).
+// No Python, no torch: weights come from one flat file written by funasr_b200/pack.py (tensors under FunASR's own state_dict names),
+// device memory from cudaMalloc.
+//
+//   fa_offline_init         model file -> handle (weights to HBM, fp16 planes for the tensor-core GEMMs)
+//   fa_offline_infer        batch of host PCM buffers (f32 in [-1,1] or s16le) -> result (greedy token ids per utterance)
+//   fa_offline_result_*     accessors;  fa_offline_free_result / fa_offline_uninit
+//                           a BiCifParaformer file (its upsampled CIF timestamp head) adds per-token [start_ms, end_ms] stamps
+//   a SenseVoiceSmall file (__sv_config__) makes the same handle run SenseVoiceEngine's chain: per-utterance query rows
+//                           (fa_sv_query_rows), the SAN-M and tp stacks, the CTC head; fa_offline_infer_sv
+//   a SeacoParaformer file (__seaco_config__): fa_offline_hotword_embed runs its hotword encoder (hotword.cu), the decode takes those
+//                           rows through _seaco_decode_with_ASF (seaco_bias)
+// Long audio (VAD segments decoded in packs) is offline_long.cu.  The tokenizer (ids -> text) stays with the caller, like every other
+// entry point of this ABI.
+#include "handle.h"
+
+using namespace fa_handle;
+
+namespace {
+
+// A Paraformer file (ParaformerEngine, engine.py): plain, contextual (a hotword bias decoder) or BiCif (a timestamp head)
+bool build_paraformer(Model& m, Builder& b) {
+  m.mode = b.mode;
+  // BiCifParaformer's timestamp head, recognised by predictor.upsample_cnn.weight: the tensors its launches read, in the shapes
+  // pack.py:timestamp_head_tensors writes, and __ts_config__.  Bound first: its refusals come before the rest of the file's.
+  m.ts = b.opt("predictor.upsample_cnn.weight") != nullptr;
+  if (m.ts) {
+    const Tensor* tc = b.opt("__ts_config__");
+    if (!tc || tc->host.size() < 3)
+      return b.refuse("BiCif timestamp head without __ts_config__ (a file packed before the handle read the head): re-pack it with "
+                      "funasr_b200.pack.write_model_file");
+    const float* c = tc->host.data();
+    if (c[0] != 3.f) return b.refuse("BiCif timestamp head: upsample_times " + std::to_string(c[0]) + " in __ts_config__, only 3 is supported");
+    b.what = "BiCif timestamp head: ";
+    b.shaped("predictor.upsample_cnn.gemm_weight", {3 * 512, 512}); b.shaped("predictor.upsample_cnn.gemm_bias", {3 * 512});
+    b.shaped("predictor.blstm.ih_gemm_weight", {8 * 512, 512});     b.shaped("predictor.blstm.ih_gemm_bias", {8 * 512});
+    b.shaped("predictor.blstm.weight_hh_l0", {4 * 512, 512});       b.shaped("predictor.blstm.weight_hh_l0_reverse", {4 * 512, 512});
+    b.shaped("predictor.cif_output2.weight", {1, 2 * 512});         b.shaped("predictor.cif_output2.bias", {1});
+    FaTimestampHead& h = m.head;
+    h.up_times = 3; h.smooth2 = c[1]; h.noise2 = c[2];
+    h.upsample = b.lin("predictor.upsample_cnn", true, "predictor.upsample_cnn.gemm_weight", "predictor.upsample_cnn.gemm_bias");
+    h.blstm_ih = b.lin("predictor.blstm.ih", true, "predictor.blstm.ih_gemm_weight", "predictor.blstm.ih_gemm_bias");
+    h.w_hh_fwd = b.ptr("predictor.blstm.weight_hh_l0"); h.w_hh_bwd = b.ptr("predictor.blstm.weight_hh_l0_reverse");
+    h.out2_w = b.ptr("predictor.cif_output2.weight"); h.out2_b = b.ptr("predictor.cif_output2.bias");
+    b.what.clear();
+  }
+  const Tensor* cfg = b.opt("__config__");
+  if (!cfg || cfg->host.size() < 10) return b.refuse("missing __config__");
+  const float* c = cfg->host.data();
+  m.enc_layers = (int)c[0]; m.dec_layers = (int)c[1]; m.d_model = (int)c[2]; m.heads = (int)c[3]; m.kernel = (int)c[4];
+  m.vocab = (int)c[5]; m.feat_dim = (int)c[6]; m.ln_eps = c[7]; m.cif_threshold = c[8]; m.tail_threshold = c[9];
+  if (m.enc_layers < 1 || m.dec_layers < 1 || m.d_model != 512 || m.heads * 128 != m.d_model) return b.refuse("unsupported config");
+  b.ln_eps = m.ln_eps;
+  b.fbank_tables();
+  const Tensor* cmvn = b.opt("frontend.cmvn");
+  m.cmvn = cmvn ? cmvn->dev : nullptr;
+  // encoder (engine.py:_enc_stack; SANMEncoder encoder.py:188-461)
+  bind_stack(b, false, m.enc_layers, m.feat_dim, m.d_model, m.heads, m.enc_l, m.enc);
+  // predictor (CifPredictorV2 cif_predictor.py:209-314); conv weight already repacked to [512, 3*512] by pack.py
+  m.pred.conv = b.lin("predictor.cif_conv1d", true, "predictor.cif_conv1d.gemm_weight");
+  m.pred.out_w = b.ptr("predictor.cif_output.weight"); m.pred.out_b = b.ptr("predictor.cif_output.bias");
+  m.pred.threshold = m.cif_threshold; m.pred.tail_threshold = m.tail_threshold; m.pred.smooth_factor = 1.f; m.pred.noise_threshold = 0.f;
+  if (m.ts) {                   // BiCifParaformer: CifPredictorV3's sequential fp32 `cif` (bicif_paraformer/cif_predictor.py:37-84)
+    m.pred.cif_variant = 1;
+    m.head.threshold = m.cif_threshold;
+  }
+  // decoder (ParaformerSANMDecoder decoder.py:234-449)
+  auto dec_layer = [&](FaDecLayer& L, const std::string& p, bool full) {
+    L.norm1 = b.norm(p + ".norm1");
+    L.ffn_w1 = b.lin(p + ".feed_forward.w_1"); L.ffn_norm = b.norm(p + ".feed_forward.norm"); L.ffn_w2 = b.lin(p + ".feed_forward.w_2", false);
+    if (full) {
+      L.norm2 = b.norm(p + ".norm2"); L.norm3 = b.norm(p + ".norm3");
+      L.fsmn_w = b.ptr(p + ".self_attn.fsmn_block.weight");
+      L.q = b.lin(p + ".src_attn.linear_q"); L.kv = b.lin(p + ".src_attn.linear_k_v"); L.out = b.lin(p + ".src_attn.linear_out");
+    }
+  };
+  // ContextualParaformerDecoder (contextual_paraformer/decoder.py:133-352): the last attention layer is `last_decoder`, plus the
+  // hotword branch bias_decoder (norm3 + cross attention) and bias_output (Conv1d 1024 -> 512, k = 1)
+  m.contextual = b.opt("decoder.bias_decoder.norm3.weight") != nullptr;
+  if (m.contextual && b.opt("__seaco_config__"))
+    return b.refuse("SeACo model: the file carries both a contextual decoder.bias_decoder and __seaco_config__");
+  const int n_plain = m.contextual ? m.dec_layers - 1 : m.dec_layers;
+  m.dec_l.resize(n_plain > 0 ? n_plain : 1);
+  for (int i = 0; i < n_plain; ++i) dec_layer(m.dec_l[i], "decoder.decoders." + std::to_string(i), true);
+  m.dec.layers = m.dec_l.data(); m.dec.n_layers = n_plain; m.dec.heads = m.heads; m.dec.vocab = m.vocab;
+  // the decoder's FSMN tap count is its own: encoder and decoder kernel_size are independent constructor arguments in the reference
+  // (sanm/encoder.py:188, paraformer/decoder.py:234 — decoder default 21)
+  const Tensor* dk = b.get(n_plain > 0 ? "decoder.decoders.0.self_attn.fsmn_block.weight" : "decoder.last_decoder.self_attn.fsmn_block.weight");
+  m.dec.fsmn_k = dk && dk->shape.size() == 3 ? (int)dk->shape[2] : m.kernel;
+  dec_layer(m.dec.last, "decoder.decoders3.0", false);
+  m.dec.after_norm = b.norm("decoder.after_norm"); m.dec.output = b.lin("decoder.output_layer");
+  m.dec.has_bias = 0;
+  if (m.contextual) {
+    dec_layer(m.dec.bias_last, "decoder.last_decoder", true);
+    m.dec.bias_norm3 = b.norm("decoder.bias_decoder.norm3");
+    m.dec.bias_q = b.lin("decoder.bias_decoder.src_attn.linear_q"); m.dec.bias_kv = b.lin("decoder.bias_decoder.src_attn.linear_k_v");
+    m.dec.bias_out = b.lin("decoder.bias_decoder.src_attn.linear_out");
+    m.dec.bias_output = b.lin("decoder.bias_output", false);
+    m.dec.clas_scale = 1.0f;
+  }
+  const Tensor* sc = b.opt("__seaco_config__");
+  m.seaco = sc != nullptr;
+  if (m.seaco && b.ok) {
+    b.what = "SeACo model: ";
+    if (sc->host.size() != 3) return b.refuse("bad __seaco_config__");
+    m.no_bias = (int)sc->host[0]; m.nfilter = (int)sc->host[1];
+    const int layers = (int)sc->host[2], D = m.d_model;
+    if (m.no_bias < 0 || m.no_bias >= m.vocab)
+      return b.refuse("no_bias " + std::to_string(m.no_bias) + " outside the vocabulary [0, " + std::to_string(m.vocab) + ")");
+    if (m.nfilter < 0) return b.refuse("nfilter " + std::to_string(m.nfilter) + " < 0");
+    if (layers < 1 || layers > FA_HOTWORD_MAX_LAYERS) return b.refuse("bias_encoder with " + std::to_string(layers) + " layers");
+    // the hotword encoder (seaco_paraformer/model.py:384-420): decoder.embed, then the bias_encoder LSTM; the GEMM bias b_ih + b_hh
+    // comes folded from pack.py
+    const Tensor* emb = b.shaped("decoder.embed.0.weight", {m.vocab, D});
+    m.hw_ih.assign(layers, FaLinear{}); m.hw_hh.assign(layers, FaLinear{});
+    for (int k = 0; k < layers; ++k) {
+      const std::string s = std::to_string(k);
+      b.shaped("bias_encoder.weight_ih_l" + s, {4 * D, D}); b.shaped("bias_encoder.weight_hh_l" + s, {4 * D, D});
+      b.shaped("bias_encoder.bias_ih_l" + s, {4 * D}); b.shaped("bias_encoder.bias_hh_l" + s, {4 * D});
+      b.shaped("bias_encoder.gemm_bias_l" + s, {4 * D});
+      if (!b.ok) return false;
+      m.hw_ih[k] = b.lin("bias_encoder.ih_l" + s, true, ("bias_encoder.weight_ih_l" + s).c_str(), ("bias_encoder.gemm_bias_l" + s).c_str());
+      m.hw_hh[k] = b.lin("bias_encoder.hh_l" + s, false, ("bias_encoder.weight_hh_l" + s).c_str());
+    }
+    if (b.opt("bias_encoder.weight_ih_l" + std::to_string(layers))) return b.refuse("more bias_encoder layers than __seaco_config__ says");
+    m.hw_enc = FaHotwordEncoder{emb ? emb->dev : nullptr, m.vocab, layers, m.hw_ih.data(), m.hw_hh.data()};
+    // the SeACo decoder (model.py:100-110): ParaformerSANMDecoder without input / output layer; forward_asf6 reads layers 0..5
+    int n_s = 0;
+    while (b.opt("seaco_decoder.decoders." + std::to_string(n_s) + ".norm1.weight")) ++n_s;
+    if (n_s < 6) return b.refuse(n_s == 0 ? std::string("missing tensor seaco_decoder.decoders.0.norm1.weight")
+                                           : "seaco_decoder with " + std::to_string(n_s) + " attention layers (the attention-score filter reads 6)");
+    const Tensor* sk = b.get("seaco_decoder.decoders.0.self_attn.fsmn_block.weight");
+    const int64_t K = sk && sk->shape.size() == 3 ? sk->shape[2] : 0;
+    m.seaco_l.assign(n_s, FaDecLayer{});
+    for (int i = 0; i < n_s && b.ok; ++i) {
+      const std::string p = "seaco_decoder.decoders." + std::to_string(i);
+      const Tensor* w1 = b.get(p + ".feed_forward.w_1.weight");
+      const int64_t F = w1 && w1->shape.size() == 2 ? w1->shape[0] : 0;
+      if (w1 && (F < 1 || F > 2048)) return b.refuse("bad shape of " + p + ".feed_forward.w_1.weight (at most 2048 units)");
+      b.shaped(p + ".feed_forward.w_1.weight", {F, D}); b.shaped(p + ".feed_forward.w_2.weight", {D, F});
+      b.shaped(p + ".self_attn.fsmn_block.weight", {D, 1, K});
+      b.shaped(p + ".src_attn.linear_q.weight", {D, D}); b.shaped(p + ".src_attn.linear_k_v.weight", {2 * D, D});
+      b.shaped(p + ".src_attn.linear_out.weight", {D, D});
+      dec_layer(m.seaco_l[i], p, true);
+    }
+    m.seaco_dec = FaDecoder{};
+    m.seaco_dec.layers = m.seaco_l.data(); m.seaco_dec.n_layers = n_s; m.seaco_dec.heads = m.heads; m.seaco_dec.fsmn_k = (int)K;
+    dec_layer(m.seaco_dec.last, "seaco_decoder.decoders3.0", false);
+    m.seaco_dec.after_norm = b.norm("seaco_decoder.after_norm");
+    b.shaped("hotword_output_layer.weight", {m.vocab, D}); b.shaped("hotword_output_layer.bias", {m.vocab});
+    m.hw_out = b.lin("hotword_output_layer");
+    b.what.clear();
+  }
+  return b.ok;
+}
+
+int num_lfr_frames(int64_t n) {       // wav_frontend.py:73 after kaldi.py snip_edges framing
+  const int64_t mfr = n >= 400 ? 1 + (n - 400) / 160 : 0;
+  return (int)((mfr + 5) / 6);
+}
+
+// SeACo's hotword biasing after the decoder (_seaco_decode_with_ASF, seaco_paraformer/model.py:271-382, as ParaformerEngine.seaco_decode
+// runs it): the host hotword rows hw_host [n_hw, 512] on the device; with more rows than nfilter, the attention-score filter on
+// utterance 0 (one host round trip: its probabilities out, fa_seaco_asf_select_host, the picked host rows back in); the SeACo decoder
+// over the acoustic embeddings and over the decoder's hidden states; hotword_output_layer's arg-max over their sum; the NO_BIAS merge
+// of the decoder's ids / best into *sids.  The workspace is sized for the stack and the arg-max.
+bool seaco_bias(Model& m, int B, int n_max, int n_cap, const float* hw_host, int n_hw, const float* acoustic, const float* hidden,
+                const int32_t* tok, const int32_t* ids, const float* best, int32_t** sids) {
+  cudaStream_t st = m.file.st;
+  const int D = m.d_model, V = m.vocab, n_s = m.seaco_dec.n_layers, H = m.seaco_dec.heads;
+  const int64_t rows = (int64_t)B * n_max;
+  const bool asf = m.nfilter > 0 && m.nfilter < n_hw;       // ASF (model.py:320-343): forward_asf6 on utterance 0
+  float *mem, *cif_att, *dec_att, *dha_best, *sbest, *probs = nullptr;
+  int32_t *dha_ids, *mem_lens;
+  if (!carve(m.seaco_bias, "SeACo", [&](fa::Arena& a) {
+        mem = a.take<float>((size_t)n_hw * D);
+        cif_att = a.take<float>((size_t)rows * D); dec_att = a.take<float>((size_t)rows * D);
+        dha_ids = a.take<int32_t>(rows); dha_best = a.take<float>(rows);
+        *sids = a.take<int32_t>(rows); sbest = a.take<float>(rows);
+        mem_lens = a.take<int32_t>(B);
+        if (asf) probs = a.take<float>((size_t)H * n_max * n_hw);
+      }))
+    return false;
+  cudaMemcpyAsync(mem, hw_host, (size_t)n_hw * D * 4, cudaMemcpyHostToDevice, st);
+  int n_sel = n_hw;
+  std::vector<float> picked_rows;
+  int rc = FA_OK;
+  if (asf) {
+    const int32_t one = n_hw;
+    cudaMemcpyAsync(mem_lens, &one, 4, cudaMemcpyHostToDevice, st);
+    rc = fa_sanm_decoder_stack_forward(&m.seaco_dec, mem, mem_lens, 1, 1, n_hw, hidden, n_max, tok, n_max, 6, 0, nullptr, probs, m.mode,
+                                       m.ws.p, m.ws.cap, st);
+    if (rc != FA_OK) { set_err(std::string("SeACo filter: ") + fa_status_string(rc)); return false; }
+    std::vector<float> probs_h((size_t)H * n_max * n_hw);
+    cudaMemcpyAsync(probs_h.data(), probs, probs_h.size() * 4, cudaMemcpyDeviceToHost, st);
+    if (!sync_stream(st)) return false;
+    std::vector<int32_t> picked((size_t)n_hw);
+    n_sel = fa_seaco_asf_select_host(probs_h.data(), H, n_max, n_hw, m.nfilter, picked.data());
+    if (n_sel < 1) { set_err("fa_seaco_asf_select_host failed"); return false; }
+    picked_rows.resize((size_t)n_sel * D);
+    for (int j = 0; j < n_sel; ++j) std::copy(hw_host + (size_t)picked[j] * D, hw_host + (size_t)(picked[j] + 1) * D, picked_rows.begin() + (size_t)j * D);
+    cudaMemcpyAsync(mem, picked_rows.data(), picked_rows.size() * 4, cudaMemcpyHostToDevice, st);
+  }
+  const std::vector<int32_t> lens_h(B, n_sel);
+  cudaMemcpyAsync(mem_lens, lens_h.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st);
+  rc = fa_sanm_decoder_stack_forward(&m.seaco_dec, mem, mem_lens, 1, B, n_sel, acoustic, n_cap, tok, n_max, n_s, 1, cif_att, nullptr, m.mode,
+                                     m.ws.p, m.ws.cap, st);
+  if (rc == FA_OK)
+    rc = fa_sanm_decoder_stack_forward(&m.seaco_dec, mem, mem_lens, 1, B, n_sel, hidden, n_max, tok, n_max, n_s, 1, dec_att, nullptr, m.mode,
+                                       m.ws.p, m.ws.cap, st);
+  if (rc == FA_OK) rc = fa_linear_argmax(&m.hw_out, cif_att, dec_att, rows, dha_ids, dha_best, nullptr, m.mode, m.ws.p, m.ws.cap, st);
+  if (rc == FA_OK) rc = fa_seaco_merge(ids, best, dha_ids, dha_best, rows, m.no_bias, *sids, sbest, nullptr, nullptr, nullptr, V, st);
+  if (rc != FA_OK) { set_err(std::string("SeACo decoder: ") + fa_status_string(rc)); return false; }
+  return sync_stream(st);                                    // lens_h and picked_rows are host vectors of this frame
+}
+
+// The recogniser over a padded batch already on the device: wav [B, stride] fp32, lens_h [B] samples (>= 400 each).  Everything
+// after the host-to-device copy of fa_offline_infer_hw; long audio feeds it the gathered VAD segments of one pack.
+std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const float* hw_embed,
+                                     int32_t n_hotwords) {
+  const int B = (int)lens_h.size(), D = m.d_model;
+  cudaStream_t st = m.file.st;
+  int t_max = 0;
+  double seconds = 0.0;
+  for (int i = 0; i < B; ++i) {
+    const int t = num_lfr_frames(lens_h[i]);
+    t_max = t > t_max ? t : t_max;
+    seconds += (double)lens_h[i] / 16000.0;
+  }
+  const int T = t_max;
+  const int n_cap = T + 1;
+  int32_t *lens, *flens, *tok;
+  float *feats, *encb, *acoustic, *alphas, *peaks;
+  if (!carve(m.encode, "activations", [&](fa::Arena& a) {
+        lens = a.take<int32_t>(B); flens = a.take<int32_t>(B); tok = a.take<int32_t>(B);
+        feats = a.take<float>((size_t)B * T * m.feat_dim); encb = a.take<float>((size_t)B * T * D);
+        acoustic = a.take<float>((size_t)B * n_cap * D);
+        alphas = a.take<float>((size_t)B * n_cap); peaks = a.take<float>((size_t)B * n_cap);
+      }))
+    return nullptr;
+  cudaMemcpyAsync(lens, lens_h.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st);
+  size_t ws = fa_sanm_encoder_workspace_bytes(B, T, m.mode);
+  const size_t ws2 = fa_cif_predictor_workspace_bytes(B, T, m.mode);
+  ws = ws2 > ws ? ws2 : ws;
+  if (!m.ws.reserve(ws)) return fail("device allocation failed (workspace)");
+  int rc = fa_fbank_lfr_cmvn_tables(wav, lens, B, stride, m.cmvn, m.file.fbank_tables, 7, 6, feats, T, flens, T, st);
+  if (rc != FA_OK) return fail(std::string("fa_fbank_lfr_cmvn_tables: ") + fa_status_string(rc));
+  rc = fa_sanm_encoder_forward(&m.enc, feats, flens, B, T, encb, m.mode, m.ws.p, m.ws.cap, st);
+  if (rc != FA_OK) return fail(std::string("fa_sanm_encoder_forward: ") + fa_status_string(rc));
+  rc = fa_cif_predictor_forward(&m.pred, encb, flens, B, T, acoustic, n_cap, tok, alphas, peaks, m.mode, m.ws.p, m.ws.cap, st);
+  if (rc != FA_OK) return fail(std::string("fa_cif_predictor_forward: ") + fa_status_string(rc));
+  std::unique_ptr<Result> r(new Result());
+  r->audio_seconds = (float)seconds;
+  r->token_num.resize(B);
+  r->ts = m.ts;
+  if (m.ts) r->stamps.resize(B);
+  cudaMemcpyAsync(r->token_num.data(), tok, (size_t)B * 4, cudaMemcpyDeviceToHost, st);
+  if (!sync_stream(st)) return nullptr;
+  int n_max = 0;                                             // the path's one host sync (cif_predictor.py:311)
+  for (int i = 0; i < B; ++i) n_max = r->token_num[i] > n_max ? r->token_num[i] : n_max;
+  r->ids.resize(B);
+  if (n_max < 1) return r;                                   // paraformer/model.py:615-616
+  const int nh = m.contextual ? n_hotwords : 0;
+  // the timestamp head over the [B, 3T] upsampled frames shares the workspace with the decoder
+  const int U = m.head.up_times, TU = T * U;
+  const int64_t rows_up = (int64_t)B * TU;
+  const int n_sw = m.seaco && hw_embed ? n_hotwords : 0;     // SeACo hotword rows (none: the plain decoder distribution)
+  size_t ws_dec = fa_paraformer_decoder_workspace_bytes_hw(B, T, n_max, m.vocab, m.mode, nh);
+  if (m.ts) ws_dec = std::max(ws_dec, fa_timestamp_head_workspace_bytes(B, T, D, U, m.mode));
+  if (n_sw > 0)
+    ws_dec = std::max({ws_dec, fa_sanm_decoder_stack_workspace_bytes(B, n_sw, n_max, m.mode), fa_linear_argmax_workspace_bytes((int64_t)B * n_max, m.vocab, m.mode)});
+  int32_t *ids, *fids, *flens_out, *hw_lens = nullptr;
+  float *best, *us_alphas = nullptr, *us_peaks = nullptr, *hw = nullptr, *hidden = nullptr;
+  if (!carve(m.decode, "decoder", [&](fa::Arena& a) {
+        ids = a.take<int32_t>((size_t)B * n_max); best = a.take<float>((size_t)B * n_max); fids = a.take<int32_t>((size_t)B * n_max);
+        flens_out = a.take<int32_t>(B);
+        if (m.ts) { us_alphas = a.take<float>(rows_up); us_peaks = a.take<float>(rows_up); }
+        if (m.contextual) { hw = a.take<float>((size_t)nh * D); hw_lens = a.take<int32_t>(B); }
+        if (m.seaco) hidden = a.take<float>((size_t)B * n_max * D);
+      }))
+    return nullptr;
+  if (!m.ws.reserve(ws_dec)) return fail("device allocation failed (decoder)");
+  if (m.contextual) {                                        // hotword memory [n_hw, 512] (contextual_paraformer/model.py:350-372) + per-utterance counts
+    std::vector<int32_t> hl(B, nh);
+    cudaMemcpyAsync(hw, hw_embed, (size_t)nh * D * 4, cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(hw_lens, hl.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st);
+    cudaStreamSynchronize(st);                               // hl is a stack vector
+    m.dec.has_bias = 1; m.dec.n_hotwords = nh;
+    m.dec.hw_embed = hw; m.dec.hw_lens = hw_lens;
+  }
+  const int32_t* final_ids = ids;
+  if (m.seaco) {                                             // return_hidden: the decoder_hidden the SeACo decoder attends from
+    rc = fa_paraformer_decoder_forward_hidden(&m.dec, encb, flens, B, T, acoustic, n_cap, tok, n_max, ids, best, nullptr, 1, hidden, m.mode,
+                                              m.ws.p, m.ws.cap, st);
+    if (rc == FA_OK && n_sw > 0) {
+      int32_t* sids = nullptr;
+      if (!seaco_bias(m, B, n_max, n_cap, hw_embed, n_sw, acoustic, hidden, tok, ids, best, &sids)) return nullptr;
+      final_ids = sids;
+    }
+  } else {
+    rc = fa_paraformer_decoder_forward(&m.dec, encb, flens, B, T, acoustic, n_cap, tok, n_max, ids, best, nullptr, 1, m.mode, m.ws.p, m.ws.cap, st);
+  }
+  if (rc == FA_OK) rc = fa_greedy_filter(final_ids, tok, B, n_max, 1, 2, 0, fids, flens_out, st);
+  if (rc != FA_OK) return fail(std::string("decoder: ") + fa_status_string(rc));
+  if (m.ts) {                   // CifPredictorV3.get_upsample_timestamp (bicif_paraformer/cif_predictor.py:300-352), engine.upsample_timestamp
+    rc = fa_timestamp_head_forward(&m.head, encb, flens, tok, B, T, us_alphas, us_peaks, m.mode, m.ws.p, m.ws.cap, st);
+    if (rc != FA_OK) return fail(std::string("timestamp head: ") + fa_status_string(rc));
+  }
+  std::vector<int32_t> fids_h((size_t)B * n_max), fl(B), enc_lens(m.ts ? B : 0);
+  std::vector<float> us_alphas_h(m.ts ? rows_up : 0), us_peaks_h(m.ts ? rows_up : 0);
+  cudaMemcpyAsync(fids_h.data(), fids, fids_h.size() * 4, cudaMemcpyDeviceToHost, st);
+  cudaMemcpyAsync(fl.data(), flens_out, (size_t)B * 4, cudaMemcpyDeviceToHost, st);
+  if (m.ts) {                                                // on the same synchronisation as the ids
+    cudaMemcpyAsync(enc_lens.data(), flens, (size_t)B * 4, cudaMemcpyDeviceToHost, st);
+    cudaMemcpyAsync(us_alphas_h.data(), us_alphas, (size_t)rows_up * 4, cudaMemcpyDeviceToHost, st);
+    cudaMemcpyAsync(us_peaks_h.data(), us_peaks, (size_t)rows_up * 4, cudaMemcpyDeviceToHost, st);
+  }
+  if (!sync_stream(st)) return nullptr;
+  for (int i = 0; i < B; ++i) r->ids[i].assign(fids_h.begin() + (size_t)i * n_max, fids_h.begin() + (size_t)i * n_max + fl[i]);
+  if (m.ts) {                                                // bicif_paraformer/model.py:402-407: each utterance's first 3 * enc_len frames
+    for (int i = 0; i < B; ++i) {
+      const int64_t n = (int64_t)U * enc_lens[i];
+      std::vector<int32_t>& sp = r->stamps[i];
+      sp.resize((size_t)(2 * (n > 0 ? n : 1)));              // at most n - 1 spans
+      const int64_t k = fa_ts_stamps_host(us_alphas_h.data() + (size_t)i * TU, us_peaks_h.data() + (size_t)i * TU, n, (int64_t)r->ids[i].size(), U,
+                                          0.0, sp.data(), n);
+      sp.resize(k > 0 ? (size_t)(2 * k) : 0);
+    }
+  }
+  return r;
+}
+
+// ------------------------------------------------------------------------------------------------ SenseVoiceSmall
+// __sv_config__ of funasr_b200/pack.py:write_sensevoice_model_file
+enum { kSvEnc = 0, kSvTp, kSvDModel, kSvHeads, kSvKernel, kSvVocab, kSvFeat, kSvEps, kSvBlank, kSvCfgLen };
+
+// SenseVoiceEngine of engine.py: the same weights, the same planes per gemm_mode
+bool build_sv(Model& m, Builder& b) {
+  m.mode = b.mode;
+  b.what = "SenseVoice model: ";
+  if (b.opt("__config__")) return b.refuse("the file carries both __config__ (Paraformer) and __sv_config__");
+  const Tensor* cfg = b.get("__sv_config__");
+  if (!cfg) return false;
+  if (cfg->host.size() != kSvCfgLen) return b.refuse("bad __sv_config__");
+  const float* c = cfg->host.data();
+  m.enc_layers = (int)c[kSvEnc]; m.tp_layers = (int)c[kSvTp]; m.d_model = (int)c[kSvDModel]; m.heads = (int)c[kSvHeads];
+  m.kernel = (int)c[kSvKernel]; m.vocab = (int)c[kSvVocab]; m.feat_dim = (int)c[kSvFeat]; m.ln_eps = c[kSvEps]; m.blank = (int)c[kSvBlank];
+  if (m.enc_layers < 1 || m.tp_layers < 0) return b.refuse("no encoder layer");
+  if (m.d_model != 512 || m.heads != 4)
+    return b.refuse("d_model " + std::to_string(m.d_model) + " with " + std::to_string(m.heads) +
+                    " heads (the tensor-core attention runs d_model 512 as 4 heads of 128)");
+  if (m.vocab < 1 || m.vocab > 61440)
+    return b.refuse("vocabulary of " + std::to_string(m.vocab) + " tokens (the CTC arg-max takes at most 61440)");
+  if (m.feat_dim != 560) return b.refuse("feat_dim " + std::to_string(m.feat_dim) + " (the frontend is 80 mel x LFR 7 = 560)");
+  if (m.blank < 0 || m.blank >= m.vocab) return b.refuse("blank_id outside the vocabulary");
+  b.ln_eps = m.ln_eps;
+  b.fbank_tables();
+  const Tensor* cmvn = b.opt("frontend.cmvn");
+  if (cmvn && cmvn->numel() != 2 * m.feat_dim) return b.refuse("frontend.cmvn must be [2, 560]");
+  m.cmvn = cmvn ? cmvn->dev : nullptr;
+  bind_stack(b, false, m.enc_layers, m.feat_dim, m.d_model, m.heads, m.enc_l, m.enc);
+  bind_stack(b, true, m.tp_layers, m.d_model, m.d_model, m.heads, m.tp_l, m.tp);
+  const Tensor* ctc = b.get("ctc.ctc_lo.weight");
+  if (ctc && ctc->shape != std::vector<int64_t>{m.vocab, m.d_model}) return b.refuse("bad shape of ctc.ctc_lo.weight (want [vocab, 512])");
+  m.ctc = b.lin("ctc.ctc_lo");
+  const Tensor* emb = b.get("embed.weight");
+  if (!emb) return false;
+  if (emb->shape.size() != 2 || emb->shape[0] < 3 || emb->shape[1] != m.feat_dim) return b.refuse("bad shape of embed.weight (want [>= 3, 560])");
+  m.embed = emb->dev;
+  m.n_embed = (int)emb->shape[0];
+  m.sv = true;
+  return b.ok;
+}
+
+// SenseVoiceEngine.forward_wav over a padded batch already on the device (wav [B, stride], lens_h >= 400 samples each), utterance i
+// queried with (lang[i], tn[i]) (NULL: the defaults; validated by check_queries).  The CTC head materialises the logits [B, T, vocab].
+std::unique_ptr<Result> decode_sv(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const int32_t* lang,
+                                  const int32_t* tn) {
+  const int B = (int)lens_h.size(), D = m.d_model, F = m.feat_dim;
+  cudaStream_t st = m.file.st;
+  int t_feat = 0;
+  double seconds = 0.0;
+  // one host-to-device copy: sample counts [B], encoder lengths [B] (frames + the 4 query rows), query ids [B][2]
+  std::vector<int32_t> io((size_t)4 * B);
+  for (int i = 0; i < B; ++i) {
+    const int t = num_lfr_frames(lens_h[i]);
+    t_feat = t > t_feat ? t : t_feat;
+    seconds += (double)lens_h[i] / 16000.0;
+    io[i] = lens_h[i];
+    io[B + i] = t + 4;
+    io[2 * B + 2 * i] = lang ? lang[i] : kSvAuto;
+    io[2 * B + 2 * i + 1] = tn ? tn[i] : kSvWoItn;
+  }
+  const int T = t_feat + 4;
+  const size_t rows = (size_t)B * T;
+  const size_t ws = std::max(fa_sanm_encoder_workspace_bytes(B, T, m.mode), fa_ctc_greedy_workspace_bytes(B, T, m.vocab, m.mode));
+  int32_t *io_d, *flens, *am, *ids, *flens_out;
+  float *x, *enc, *enc2;
+  if (!carve(m.decode_sv, "SenseVoice", [&](fa::Arena& a) {
+        io_d = a.take<int32_t>(io.size()); flens = a.take<int32_t>(B);
+        x = a.take<float>(rows * F); enc = a.take<float>(rows * D); enc2 = a.take<float>(rows * D);
+        am = a.take<int32_t>(rows); ids = a.take<int32_t>(rows); flens_out = a.take<int32_t>(B);
+      }))
+    return nullptr;
+  if (!m.ws.reserve(ws)) return fail("device allocation failed (SenseVoice)");
+  cudaMemcpyAsync(io_d, io.data(), io.size() * 4, cudaMemcpyHostToDevice, st);
+  int rc = fa_fbank_lfr_cmvn_tables(wav, io_d, B, stride, m.cmvn, m.file.fbank_tables, 7, 6, x + 4 * F, T, flens, t_feat, st);
+  if (rc == FA_OK) rc = fa_sv_query_rows(m.embed, m.n_embed, F, io_d + 2 * B, B, x, T, st);
+  if (rc == FA_OK) rc = fa_sanm_encoder_forward(&m.enc, x, io_d + B, B, T, enc, m.mode, m.ws.p, m.ws.cap, st);
+  if (rc == FA_OK && m.tp_layers > 0) {
+    rc = fa_sanm_encoder_forward(&m.tp, enc, io_d + B, B, T, enc2, m.mode, m.ws.p, m.ws.cap, st);
+    enc = enc2;
+  }
+  if (rc == FA_OK) rc = fa_ctc_greedy_forward(&m.ctc, enc, io_d + B, B, T, m.blank, am, ids, flens_out, nullptr, m.mode, m.ws.p, m.ws.cap, st);
+  if (rc != FA_OK) return fail(std::string("SenseVoice: ") + fa_status_string(rc));
+  std::unique_ptr<Result> r(new Result());
+  r->audio_seconds = (float)seconds;
+  r->token_num.resize(B);
+  r->ids.resize(B);
+  std::vector<int32_t> ids_h(rows);
+  cudaMemcpyAsync(ids_h.data(), ids, rows * 4, cudaMemcpyDeviceToHost, st);
+  cudaMemcpyAsync(r->token_num.data(), flens_out, (size_t)B * 4, cudaMemcpyDeviceToHost, st);
+  if (!sync_stream(st)) return nullptr;
+  for (int i = 0; i < B; ++i) r->ids[i].assign(ids_h.begin() + (size_t)i * T, ids_h.begin() + (size_t)i * T + r->token_num[i]);
+  return r;
+}
+
+// fa_offline_infer_hw / fa_offline_infer_sv: host buffers -> one padded batch -> decode_pack
+void* infer_batch(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format, const float* hw_embed,
+                  int32_t n_hotwords, const int32_t* lang, const int32_t* tn) {
+  Model* mp = static_cast<Model*>(handle);
+  if (!mp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) return fail("bad argument");
+  Model& m = *mp;
+  if (!check_hotword_rows(m, hw_embed, n_hotwords)) return nullptr;
+  if (m.sv && !check_queries(m, lang, tn, batch, "utterance")) return nullptr;
+  cudaSetDevice(m.file.device);
+  int64_t nmax = 0;
+  std::vector<int32_t> lens_h(batch);
+  for (int i = 0; i < batch; ++i) {
+    if (!bufs[i] || n_samples[i] < 400 || n_samples[i] > 0x7fffffffLL) return fail("every buffer needs >= 400 samples (25 ms)");
+    lens_h[i] = (int32_t)n_samples[i];
+    nmax = n_samples[i] > nmax ? n_samples[i] : nmax;
+  }
+  const int64_t stride = (nmax + 3) / 4 * 4;
+  float* wav = nullptr;
+  if (!upload(bufs, n_samples, batch, stride, pcm_format, m.upload, m.file.st, &wav)) return nullptr;
+  return decode_pack(m, wav, stride, lens_h, hw_embed, n_hotwords, lang, tn).release();
+}
+
+// the model kind is the file's: SenseVoiceSmall by __sv_config__, Paraformer otherwise
+bool build_offline(Model& m, Builder& b) { return b.opt("__sv_config__") ? build_sv(m, b) : build_paraformer(m, b); }
+
+const Result* as_result(const void* r) { return static_cast<const Result*>(r); }
+
+}  // namespace
+
+namespace fa_handle {
+
+bool check_hotword_rows(const Model& m, const float* hw_embed, int32_t n_hotwords) {
+  if (m.contextual && (!hw_embed || n_hotwords < 1)) {
+    set_err("this model has a hotword bias decoder: pass hotword embeddings (at least the <s> entry)");
+    return false;
+  }
+  if (m.seaco && (n_hotwords < 0 || (n_hotwords > 0 && !hw_embed))) {
+    set_err("bad hotword rows: hw_embed must hold n_hotwords rows of 512");
+    return false;
+  }
+  return true;
+}
+
+bool check_queries(const Model& m, const int32_t* lang, const int32_t* tn, int n, const char* what) {
+  for (int i = 0; i < n; ++i) {
+    const int32_t l = lang ? lang[i] : kSvAuto, t = tn ? tn[i] : kSvWoItn;
+    if (l < 0 || l >= m.n_embed || t < 0 || t >= m.n_embed) {
+      set_err(std::string(what) + " " + std::to_string(i) + ": " + (l < 0 || l >= m.n_embed ? "language id " + std::to_string(l) : "textnorm id " + std::to_string(t)) +
+              " outside the embedding table [0, " + std::to_string(m.n_embed) + ")");
+      return false;
+    }
+  }
+  return true;
+}
+
+std::unique_ptr<Result> decode_pack(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const float* hw_embed,
+                                    int32_t n_hotwords, const int32_t* lang, const int32_t* tn) {
+  return m.sv ? decode_sv(m, wav, stride, lens_h, lang, tn) : decode_batch(m, wav, stride, lens_h, hw_embed, n_hotwords);
+}
+
+}  // namespace fa_handle
+
+extern "C" void* fa_offline_init(const char* model_file, int32_t device, int32_t gemm_mode) {
+  g_err.clear();
+  if (!model_file) return fail("model_file is NULL");
+  if (!valid_gemm_mode(gemm_mode)) return fail("bad gemm_mode");
+  return open_handle(model_file, device, gemm_mode, build_offline);
+}
+
+extern "C" int32_t fa_offline_is_sensevoice(const void* handle) { return handle && static_cast<const Model*>(handle)->sv ? 1 : 0; }
+
+extern "C" void* fa_offline_infer_sv(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
+                                     const int32_t* language_ids, const int32_t* textnorm_ids) {
+  g_err.clear();
+  if (handle && !static_cast<Model*>(handle)->sv) return fail("fa_offline_infer_sv: not a SenseVoice model file");
+  return infer_batch(handle, bufs, n_samples, batch, pcm_format, nullptr, 0, language_ids, textnorm_ids);
+}
+
+extern "C" void fa_offline_uninit(void* handle) { delete static_cast<Model*>(handle); }
+
+extern "C" int32_t fa_offline_is_contextual(const void* handle) { return handle && static_cast<const Model*>(handle)->contextual ? 1 : 0; }
+
+extern "C" int32_t fa_offline_has_timestamps(const void* handle) { return handle && static_cast<const Model*>(handle)->ts ? 1 : 0; }
+
+extern "C" int32_t fa_offline_is_seaco(const void* handle) { return handle && static_cast<const Model*>(handle)->seaco ? 1 : 0; }
+
+extern "C" int fa_offline_hotword_embed(void* handle, const int32_t* ids, const int32_t* lens, int32_t n, float* rows_host) {
+  g_err.clear();
+  Model* m = static_cast<Model*>(handle);
+  if (!m || !ids || !lens || n < 1 || !rows_host) { set_err("fa_offline_hotword_embed: bad argument"); return FA_ERR_ARG; }
+  if (!m->seaco) { set_err("fa_offline_hotword_embed: not a SeACo model file (ContextualParaformer rows come from its own encoder)"); return FA_ERR_ARG; }
+  int64_t n_tok = 0;
+  for (int32_t i = 0; i < n; ++i) {                 // every id named before any launch
+    if (lens[i] < 1) { set_err("hotword " + std::to_string(i) + " has no token"); return FA_ERR_ARG; }
+    for (int32_t k = 0; k < lens[i]; ++k)
+      if (ids[n_tok + k] < 0 || ids[n_tok + k] >= m->vocab) {
+        set_err("hotword " + std::to_string(i) + ": token id " + std::to_string(ids[n_tok + k]) + " outside the vocabulary [0, " +
+                std::to_string(m->vocab) + ")");
+        return FA_ERR_ARG;
+      }
+    n_tok += lens[i];
+  }
+  cudaSetDevice(m->file.device);
+  cudaStream_t st = m->file.st;
+  const size_t ws = fa_hotword_encoder_workspace_bytes(n, n_tok, m->mode);
+  float* rows = nullptr;
+  if (ws == 0 || !m->ws.reserve(ws)) { set_err("device allocation failed (hotword encoder)"); return FA_ERR_CUDA; }
+  if (!carve(m->hotword_embed, "hotword encoder", [&](fa::Arena& a) { rows = a.take<float>((size_t)n * m->d_model); })) return FA_ERR_CUDA;
+  const int rc = fa_hotword_encoder_forward(&m->hw_enc, ids, lens, n, rows, m->mode, m->ws.p, m->ws.cap, st);
+  if (rc != FA_OK) { set_err(std::string("fa_hotword_encoder_forward: ") + fa_status_string(rc)); return rc; }
+  cudaMemcpyAsync(rows_host, rows, (size_t)n * m->d_model * 4, cudaMemcpyDeviceToHost, st);
+  return sync_stream(st) ? FA_OK : FA_ERR_CUDA;
+}
+
+extern "C" const float* fa_offline_host_tensor(void* handle, const char* name, int64_t* numel) {
+  Model* m = static_cast<Model*>(handle);
+  if (numel) *numel = 0;
+  if (!m || !name) return nullptr;
+  auto it = m->file.t.find(name);
+  if (it == m->file.t.end()) return nullptr;
+  const Tensor& t = it->second;
+  if (!t.dev) {                                 // a "__" configuration tensor: its payload is on the host already
+    if (numel) *numel = (int64_t)t.host.size();
+    return t.host.data();
+  }
+  auto& hc = m->host_cache[name];
+  if (hc.empty() && t.numel() > 0) {
+    hc.resize((size_t)t.numel());
+    cudaSetDevice(m->file.device);
+    if (cudaMemcpy(hc.data(), t.dev, hc.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess) { hc.clear(); return nullptr; }
+  }
+  if (numel) *numel = (int64_t)hc.size();
+  return hc.data();
+}
+
+extern "C" void* fa_offline_infer_hw(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
+                                     const float* hw_embed, int32_t n_hotwords) {
+  g_err.clear();
+  return infer_batch(handle, bufs, n_samples, batch, pcm_format, hw_embed, n_hotwords, nullptr, nullptr);
+}
+
+extern "C" void* fa_offline_infer(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format) {
+  return fa_offline_infer_hw(handle, bufs, n_samples, batch, pcm_format, nullptr, 0);
+}
+
+extern "C" int32_t fa_offline_result_count(const void* result) { return result ? (int32_t)as_result(result)->ids.size() : 0; }
+
+// an empty row is still a row: its (possibly NULL) data with *n_ids = 0
+extern "C" const int32_t* fa_offline_result_ids(const void* result, int32_t index, int32_t* n_ids) {
+  return result_row(result ? &as_result(result)->ids : nullptr, index, n_ids, 1, true);
+}
+
+extern "C" float fa_offline_result_audio_seconds(const void* result) { return result ? as_result(result)->audio_seconds : 0.f; }
+
+extern "C" const int32_t* fa_offline_result_stamps(const void* result, int32_t index, int32_t* n_stamps) {
+  return result_row(result && as_result(result)->ts ? &as_result(result)->stamps : nullptr, index, n_stamps, 2, false);
+}
+
+extern "C" void fa_offline_free_result(void* result) { delete static_cast<Result*>(result); }

@@ -1,0 +1,414 @@
+// Handle-style CAM++ speaker model: fa_spk_init (model file -> handle, the BatchNorms folded on the host), fa_spk_embed (host PCM ->
+// 192-dim embeddings), fa_spk_cluster (ClusterBackend over host embeddings), and diarize, which long audio (offline_long.cu) runs on a
+// recording already on the device.
+#include "handle.h"
+#include <math.h>
+
+using namespace fa_handle;
+
+namespace {
+
+// __spk_config__ of funasr_b200/pack.py:write_campplus_model_file: CAMPPlusB200's one supported shape
+enum { kSpkFeat = 0, kSpkEmb, kSpkGrowth, kSpkBnSize, kSpkInit, kSpkCfgLen };
+const float kSpkConfig[kSpkCfgLen] = {80, 192, 32, 4, 128};
+const int kCamLayers[3] = {12, 24, 16}, kCamDilation[3] = {1, 2, 2};
+const char* const kFcmConvs[12] = {"conv1", "layer1.0.conv1", "layer1.0.conv2", "layer1.0.shortcut.0", "layer1.1.conv1", "layer1.1.conv2",
+                                   "layer2.0.conv1", "layer2.0.conv2", "layer2.0.shortcut.0", "layer2.1.conv1", "layer2.1.conv2", "conv2"};
+const char* const kFcmBns[12] = {"bn1", "layer1.0.bn1", "layer1.0.bn2", "layer1.0.shortcut.1", "layer1.1.bn1", "layer1.1.bn2",
+                                 "layer2.0.bn1", "layer2.0.bn2", "layer2.0.shortcut.1", "layer2.1.bn1", "layer2.1.bn2", "bn2"};
+const int kFcmStride[12] = {1, 2, 1, 2, 1, 1, 2, 1, 2, 1, 1, 2};
+const int kSpkEmbDim = 192, kSpkMaxFrames = 18800, kChunkLen = 24000, kChunkShift = 12000;
+const size_t kSpkWorkspaceCap = (size_t)1 << 30;    // CampplusEngine.WORKSPACE_CAP: larger batches run in slices
+const int kSpectralMaxChunks = 2048, kMaxSpks = 15;
+const double kSpkPval = 0.022, kMergeThr = 0.78;
+
+// every tensor of the reference CAMPPlus state_dict but num_batches_tracked (campplus.py:campplus_specs), in its order
+template <typename F>
+void campplus_spec(F f) {
+  auto bn = [&](const std::string& p, int64_t n, bool affine) {
+    if (affine) { f(p + ".weight", std::vector<int64_t>{n}); f(p + ".bias", std::vector<int64_t>{n}); }
+    f(p + ".running_mean", std::vector<int64_t>{n}); f(p + ".running_var", std::vector<int64_t>{n});
+  };
+  for (int i = 0; i < 12; ++i) {
+    const std::string conv = kFcmConvs[i];
+    const int64_t cin = i == 0 ? 1 : 32, k = conv.size() > 10 && conv.compare(conv.size() - 10, 10, "shortcut.0") == 0 ? 1 : 3;
+    f("head." + conv + ".weight", std::vector<int64_t>{32, cin, k, k});
+    bn("head." + std::string(kFcmBns[i]), 32, true);
+  }
+  f("xvector.tdnn.linear.weight", std::vector<int64_t>{128, 320, 5});
+  bn("xvector.tdnn.nonlinear.batchnorm", 128, true);
+  int64_t c = 128;
+  for (int i = 0; i < 3; ++i) {
+    for (int l = 0; l < kCamLayers[i]; ++l) {
+      const std::string p = "xvector.block" + std::to_string(i + 1) + ".tdnnd" + std::to_string(l + 1) + ".";
+      bn(p + "nonlinear1.batchnorm", c + l * 32, true);
+      f(p + "linear1.weight", std::vector<int64_t>{128, c + l * 32, 1});
+      bn(p + "nonlinear2.batchnorm", 128, true);
+      f(p + "cam_layer.linear_local.weight", std::vector<int64_t>{32, 128, 3});
+      f(p + "cam_layer.linear1.weight", std::vector<int64_t>{64, 128, 1}); f(p + "cam_layer.linear1.bias", std::vector<int64_t>{64});
+      f(p + "cam_layer.linear2.weight", std::vector<int64_t>{32, 64, 1}); f(p + "cam_layer.linear2.bias", std::vector<int64_t>{32});
+    }
+    c += kCamLayers[i] * 32;
+    bn("xvector.transit" + std::to_string(i + 1) + ".nonlinear.batchnorm", c, true);
+    f("xvector.transit" + std::to_string(i + 1) + ".linear.weight", std::vector<int64_t>{c / 2, c, 1});
+    c /= 2;
+  }
+  bn("xvector.out_nonlinear.batchnorm", c, true);
+  f("xvector.dense.linear.weight", std::vector<int64_t>{192, 2 * c, 1});
+  bn("xvector.dense.nonlinear.batchnorm", 192, false);
+}
+
+// The BatchNorm folding of CampplusEngine (campplus.py: _bn, _folded, conv2d) on the host in float64 — the same IEEE multiplies,
+// divisions and square roots, then one rounding to fp32 — so the folded weights are bit-identical to the Python engine's.  Runs on the
+// loaded file only (b.f).
+struct CamFolder {
+  Builder& b;
+  std::vector<float> host(const std::string& k) {
+    const Tensor* t = b.get(k);
+    std::vector<float> h(t ? (size_t)t->numel() : 0);
+    if (t && !h.empty() && cudaMemcpy(h.data(), t->dev, h.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess) b.refuse("copy of " + k + " failed");
+    return h;
+  }
+  const float* up(const std::vector<double>& v) {
+    std::vector<float> h(v.begin(), v.end());
+    void* p = b.f->alloc((h.size() ? h.size() : 1) * 4);
+    if (!p) { b.refuse("cudaMalloc failed"); return nullptr; }
+    if (cudaMemcpy(p, h.data(), h.size() * 4, cudaMemcpyHostToDevice) != cudaSuccess) b.refuse("weight upload failed");
+    return static_cast<const float*>(p);
+  }
+  // eval BatchNorm as y = x s + t
+  void bn(const std::string& p, bool affine, std::vector<double>& s, std::vector<double>& t) {
+    const std::vector<float> var = host(p + ".running_var"), mean = host(p + ".running_mean");
+    const std::vector<float> g = affine ? host(p + ".weight") : std::vector<float>(), beta = affine ? host(p + ".bias") : std::vector<float>();
+    s.resize(var.size()); t.resize(var.size());
+    for (size_t i = 0; i < var.size(); ++i) {
+      s[i] = 1.0 / std::sqrt((double)var[i] + 1e-5);
+      if (affine) {
+        s[i] = s[i] * (double)g[i];
+        t[i] = (double)beta[i] - (double)mean[i] * s[i];
+      } else {
+        t[i] = -(double)mean[i] * s[i];
+      }
+    }
+  }
+  // weights [out, in] (float64) -> FaLinear with the tensor-core planes of the handle's mode
+  FaLinear lin(const std::vector<double>& w, int out_f, int in_f, const std::vector<double>* bias) {
+    FaLinear L{};
+    L.w = up(w); L.b = bias ? up(*bias) : nullptr;
+    L.out_f = out_f; L.in_f = in_f; L.in_pad = (in_f + 63) / 64 * 64;
+    if (b.mode != FA_GEMM_F32_SIMT && b.ok) b.split_planes(L);
+    return L;
+  }
+  // conv (as [out, in]) followed by BN -> one Linear with bias
+  FaLinear folded(const std::vector<float>& w, int out_f, int in_f, const std::string& bn_p, bool affine) {
+    std::vector<double> s, t, wd((size_t)out_f * in_f);
+    bn(bn_p, affine, s, t);
+    for (int o = 0; o < out_f; ++o)
+      for (int i = 0; i < in_f; ++i) wd[(size_t)o * in_f + i] = (double)w[(size_t)o * in_f + i] * s[o];
+    return lin(wd, out_f, in_f, &t);
+  }
+  const float* plain(const std::string& k) {
+    const std::vector<float> h = host(k);
+    return up(std::vector<double>(h.begin(), h.end()));
+  }
+};
+
+bool build_spk(Spk& h, Builder& b) {
+  b.what = "CAM++ model: ";
+  h.mode = b.mode;
+  for (const char* other : {"__config__", "__sv_config__", "__seaco_config__", "__punc_config__", "__vad_config__"})
+    if (b.opt(other)) return b.refuse(std::string("the file carries ") + other + " beside __spk_config__");
+  const Tensor* cfg = b.get("__spk_config__");
+  if (!cfg) return false;
+  if (cfg->host.size() != kSpkCfgLen || !std::equal(cfg->host.begin(), cfg->host.end(), kSpkConfig))
+    return b.refuse("bad __spk_config__ (the kernels are built for feat 80, embedding 192, growth 32, bn_size 4, init 128)");
+  b.shaped("frontend.mel_banks", {80, 257});
+  b.shaped("frontend.window", {400});
+  campplus_spec([&](const std::string& k, const std::vector<int64_t>& dims) {
+    const Tensor* x = b.get(k);
+    if (x && x->shape != dims) b.refuse("bad shape of " + k);
+  });
+  if (!b.ok || !b.f) return b.ok;
+  b.fbank_tables();
+  CamFolder F{b};
+  FaCampplus& m = h.model;
+  for (int i = 0; i < 12; ++i) {                     // [kf * k + kt][ci][o] = w[o][ci][kf][kt] s[o]
+    const std::vector<float> w = F.host("head." + std::string(kFcmConvs[i]) + ".weight");
+    std::vector<double> s, t;
+    F.bn("head." + std::string(kFcmBns[i]), true, s, t);
+    const int cin = i == 0 ? 1 : 32, k = w.size() == (size_t)32 * cin ? 1 : 3;
+    std::vector<double> wf((size_t)k * k * cin * 32);
+    for (int o = 0; o < 32; ++o)
+      for (int ci = 0; ci < cin; ++ci)
+        for (int kk = 0; kk < k * k; ++kk) wf[((size_t)kk * cin + ci) * 32 + o] = (double)w[((size_t)o * cin + ci) * k * k + kk] * s[o];
+    m.fcm[i] = FaCamConv2d{F.up(wf), F.up(t), cin, 32, k, kFcmStride[i]};
+  }
+  {                                                  // [o][k * 320 + c] = w[o][c][k]
+    const std::vector<float> w = F.host("xvector.tdnn.linear.weight");
+    std::vector<float> wp((size_t)128 * 1600);
+    for (int o = 0; o < 128; ++o)
+      for (int c = 0; c < 320; ++c)
+        for (int k = 0; k < 5; ++k) wp[(size_t)o * 1600 + k * 320 + c] = w[((size_t)o * 320 + c) * 5 + k];
+    m.tdnn = F.folded(wp, 128, 1600, "xvector.tdnn.nonlinear.batchnorm", true);
+  }
+  h.layers.assign(kCamLayers[0] + kCamLayers[1] + kCamLayers[2], FaCamLayer{});
+  int li = 0, c = 128;
+  for (int i = 0; i < 3; ++i) {
+    m.n_layers[i] = kCamLayers[i]; m.dilation[i] = kCamDilation[i];
+    for (int l = 0; l < kCamLayers[i]; ++l, ++li) {
+      const std::string p = "xvector.block" + std::to_string(i + 1) + ".tdnnd" + std::to_string(l + 1) + ".";
+      FaCamLayer& L = h.layers[li];
+      std::vector<double> s, t;
+      F.bn(p + "nonlinear1.batchnorm", true, s, t);
+      L.bn1_scale = F.up(s); L.bn1_shift = F.up(t);
+      L.linear1 = F.folded(F.host(p + "linear1.weight"), 128, c + l * 32, p + "nonlinear2.batchnorm", true);
+      const std::vector<float> lw = F.host(p + "cam_layer.linear_local.weight");     // [k][c][o] = w[o][c][k]
+      std::vector<double> lp((size_t)3 * 128 * 32);
+      for (int o = 0; o < 32; ++o)
+        for (int ci = 0; ci < 128; ++ci)
+          for (int k = 0; k < 3; ++k) lp[((size_t)k * 128 + ci) * 32 + o] = lw[((size_t)o * 128 + ci) * 3 + k];
+      L.local_w = F.up(lp);
+      L.w1 = F.plain(p + "cam_layer.linear1.weight"); L.b1 = F.plain(p + "cam_layer.linear1.bias");
+      L.w2 = F.plain(p + "cam_layer.linear2.weight"); L.b2 = F.plain(p + "cam_layer.linear2.bias");
+    }
+    c += kCamLayers[i] * 32;
+    const std::string p = "xvector.transit" + std::to_string(i + 1) + ".";
+    std::vector<double> s, t;
+    F.bn(p + "nonlinear.batchnorm", true, s, t);
+    m.transit[i].scale = F.up(s); m.transit[i].shift = F.up(t);
+    const std::vector<float> w = F.host(p + "linear.weight");
+    m.transit[i].linear = F.lin(std::vector<double>(w.begin(), w.end()), c / 2, c, nullptr);
+    c /= 2;
+  }
+  m.layers = h.layers.data();
+  std::vector<double> s, t;
+  F.bn("xvector.out_nonlinear.batchnorm", true, s, t);
+  m.out_scale = F.up(s); m.out_shift = F.up(t);
+  m.dense = F.folded(F.host("xvector.dense.linear.weight"), kSpkEmbDim, 2 * c, "xvector.dense.nonlinear.batchnorm", false);
+  return b.ok;
+}
+
+int fbank_frames(int64_t n) { return n >= 400 ? (int)(1 + (n - 400) / 160) : 0; }
+
+// embeddings of a padded batch on the device (wav [B, stride], lens_d [B] on the device) -> emb [B, 192] on the device:
+// fa_campplus_features with t_max frames, then fa_campplus_forward in slices of CampplusEngine.embed_feats' workspace cap
+bool spk_embed_rows(Spk& s, const float* wav, int64_t stride, const int32_t* lens_d, int B, int t_max, float* emb) {
+  cudaStream_t st = s.file.st;
+  const size_t per = fa_campplus_workspace_bytes(&s.model, 1, t_max, s.mode);
+  if (per == 0) { set_err("CAM++ takes 2 ... 18800 feature frames per input (got " + std::to_string(t_max) + ")"); return false; }
+  const int step = (int)std::max<size_t>(1, std::min<size_t>((size_t)B, kSpkWorkspaceCap / per));
+  const size_t ws_bytes = fa_campplus_workspace_bytes(&s.model, step, t_max, s.mode);
+  float* feats;
+  int32_t* flens;
+  void* ws;
+  if (!carve(s.spk_embed_rows, "CAM++", [&](fa::Arena& a) {
+        feats = a.take<float>((size_t)B * t_max * 80); flens = a.take<int32_t>(B); ws = a.take<char>(ws_bytes);
+      }))
+    return false;
+  int rc = fa_campplus_features(wav, lens_d, B, stride, s.file.fbank_tables, feats, flens, t_max, st);
+  for (int b0 = 0; b0 < B && rc == FA_OK; b0 += step) {
+    const int nb = std::min(step, B - b0);
+    rc = fa_campplus_forward(&s.model, feats + (size_t)b0 * t_max * 80, nb, t_max, emb + (size_t)b0 * kSpkEmbDim, s.mode, ws, ws_bytes, st);
+  }
+  if (rc != FA_OK) { set_err(std::string("CAM++: ") + fa_status_string(rc)); return false; }
+  return true;
+}
+
+// ClusterBackend over n embeddings emb_d [n, 192] on the device (emb_h: the same on the host) -> labels [n] (before correct_labels).
+// preset <= 0: no preset count.  Fewer than 20 -> one speaker; fewer than 2048 -> the spectral path (the Laplacian and its
+// tridiagonalisation on the device, the 16 smallest eigenvalues on the host, the eigengap count unless preset, k-means on the
+// back-transformed vectors); otherwise k-means on the normalised rows with a preset count; merge_by_cos when no count was preset.
+bool spk_cluster(Spk& s, const float* emb_d, int n, int preset, const float* emb_h, std::vector<int32_t>& labels, const std::string& what) {
+  labels.assign((size_t)n, 0);
+  if (n < 20) return true;
+  if (preset > n) { set_err(what + "preset_spk_num " + std::to_string(preset) + " exceeds the " + std::to_string(n) + " speaker chunks"); return false; }
+  std::vector<double> x;
+  int k = preset, dim = 0;
+  if (n < kSpectralMaxChunks) {
+    cudaStream_t st = s.file.st;
+    const size_t ws_bytes = std::max(fa_spk_laplacian_workspace_bytes(n, kSpkEmbDim), fa_spk_tridiagonalize_workspace_bytes(n));
+    const int m = std::max(std::min(kMaxSpks + 1, n), k);
+    double *lap, *d, *zd;
+    void* ws;
+    if (!carve(s.spk_cluster, "speaker clustering", [&](fa::Arena& a) {
+          lap = a.take<double>((size_t)n * n); d = a.take<double>((size_t)3 * n); zd = a.take<double>((size_t)m * n); ws = a.take<char>(ws_bytes);
+        }))
+      return false;
+    int rc = fa_spk_laplacian(emb_d, n, kSpkEmbDim, kSpkPval, lap, ws, ws_bytes, st);
+    if (rc == FA_OK) rc = fa_spk_tridiagonalize(lap, n, d, d + n, d + 2 * n, ws, ws_bytes, st);
+    if (rc != FA_OK) { set_err(what + "speaker clustering: " + fa_status_string(rc)); return false; }
+    std::vector<double> de((size_t)2 * n), w((size_t)m);
+    cudaMemcpyAsync(de.data(), d, (size_t)2 * n * 8, cudaMemcpyDeviceToHost, st);
+    if (!sync_stream(st)) return false;
+    if (k <= 0) {                                    // the largest gap among the 16 smallest eigenvalues (spec_embs)
+      fa_sym_tridiag_smallest_host(de.data(), de.data() + n, n, m, 0, w.data(), nullptr);
+      const int ne = std::min(kMaxSpks + 1, n);
+      double gmax = -INFINITY;
+      for (int i = 0; i + 1 < ne; ++i)
+        if (w[i + 1] - w[i] > gmax) { gmax = w[i + 1] - w[i]; k = i + 1; }
+    }
+    std::vector<double> z((size_t)k * n);
+    fa_sym_tridiag_smallest_host(de.data(), de.data() + n, n, std::max(m, k), k, w.data(), z.data());
+    cudaMemcpyAsync(zd, z.data(), z.size() * 8, cudaMemcpyHostToDevice, st);
+    rc = fa_spk_back_transform(lap, d + 2 * n, n, zd, k, st);
+    if (rc != FA_OK) { set_err(what + "speaker clustering: " + fa_status_string(rc)); return false; }
+    cudaMemcpyAsync(z.data(), zd, z.size() * 8, cudaMemcpyDeviceToHost, st);
+    if (!sync_stream(st)) return false;
+    x.resize((size_t)n * k);
+    for (int i = 0; i < n; ++i)
+      for (int j = 0; j < k; ++j) x[(size_t)i * k + j] = z[(size_t)j * n + i];
+    dim = k;
+  } else if (preset > 0) {                           // _normalize_rows in fp32
+    x.resize((size_t)n * kSpkEmbDim);
+    for (int i = 0; i < n; ++i) {
+      const float* r = emb_h + (size_t)i * kSpkEmbDim;
+      float ss = 0.f;
+      for (int c = 0; c < kSpkEmbDim; ++c) ss += r[c] * r[c];
+      float nrm = std::sqrt(ss);
+      if (nrm == 0.f) nrm = 1.f;
+      for (int c = 0; c < kSpkEmbDim; ++c) x[(size_t)i * kSpkEmbDim + c] = (double)(r[c] / nrm);
+    }
+    dim = kSpkEmbDim;
+  } else {
+    set_err(what + std::to_string(n) + " speaker chunks without preset_spk_num: the reference clusters 2048 or more chunks with UMAP + "
+            "HDBSCAN, which this backend does not provide; pass preset_spk_num or diarize fewer than 2048 chunks");
+    return false;
+  }
+  if (fa_spk_kmeans_host(x.data(), n, dim, k, 0, 10, 300, labels.data()) != FA_OK) { set_err(what + "k-means failed"); return false; }
+  if (preset <= 0 && fa_spk_merge_by_cos_host(labels.data(), emb_h, n, kSpkEmbDim, kMergeThr) != FA_OK) {
+    set_err(what + "merge_by_cos failed"); return false;
+  }
+  return true;
+}
+
+}  // namespace
+
+namespace fa_handle {
+
+// sv_chunk windows over every VAD segment (vad_segment mode), gathered with zero tails and embedded in slices, clustered,
+// post-processed and distributed over the segments
+bool diarize(Spk& s, const float* rec, int64_t n, const std::vector<int32_t>& segs, int preset, std::vector<int32_t>& spk, const std::string& what) {
+  cudaStream_t st = s.file.st;
+  const int64_t ns = (int64_t)segs.size() / 3;
+  std::vector<int64_t> starts;
+  std::vector<double> times;
+  for (int64_t g = 0; g < ns; ++g) {                 // long_audio.speaker_chunks / diarization.chunk_bounds
+    const int64_t b0 = (int64_t)segs[3 * g] * 16, b1 = std::min<int64_t>((int64_t)segs[3 * g + 1] * 16, n), len = std::max<int64_t>(b1 - b0, 0);
+    int64_t last_ed = 0;
+    for (int64_t a = 0; a < len; a += kChunkShift) {
+      const int64_t ed = std::min<int64_t>(a + kChunkLen, len);
+      if (ed <= last_ed) break;
+      last_ed = ed;
+      const int64_t c0 = std::max<int64_t>(0, ed - kChunkLen);
+      starts.push_back(b0 + c0);
+      times.push_back((double)c0 / 16000 + (double)segs[3 * g] / 1000.0);
+      times.push_back((double)ed / 16000 + (double)segs[3 * g] / 1000.0);
+      starts.push_back(ed - c0);                     // interleaved: first sample, sample count
+    }
+  }
+  const int nc = (int)(starts.size() / 2);
+  spk.assign((size_t)ns, 0);
+  if (nc == 0) return true;
+  const int t_max = fbank_frames(kChunkLen);
+  const size_t per = fa_campplus_workspace_bytes(&s.model, 1, t_max, s.mode);
+  const int step = (int)std::max<size_t>(1, std::min<size_t>({(size_t)nc, kSpkWorkspaceCap / (per ? per : 1), (size_t)65535}));
+  float *emb, *wav;
+  int64_t* starts_d;
+  int32_t *lens_d, *full_d;
+  if (!carve(s.diarize, "speaker chunks", [&](fa::Arena& a) {
+        emb = a.take<float>((size_t)nc * kSpkEmbDim); wav = a.take<float>((size_t)step * kChunkLen);
+        starts_d = a.take<int64_t>(step); lens_d = a.take<int32_t>(step); full_d = a.take<int32_t>(step);
+      }))
+    return false;
+  const std::vector<int32_t> full((size_t)step, kChunkLen);    // every window counts as 1.5 s of samples, its zero tail included
+  cudaMemcpyAsync(full_d, full.data(), (size_t)step * 4, cudaMemcpyHostToDevice, st);
+  std::vector<int64_t> sb((size_t)step);
+  std::vector<int32_t> lb((size_t)step);
+  for (int c0 = 0; c0 < nc; c0 += step) {
+    const int nb = std::min(step, nc - c0);
+    if (!sync_stream(st)) return false;               // sb / lb are reused: the previous slice's copies are done
+    for (int r = 0; r < nb; ++r) { sb[r] = starts[2 * (c0 + r)]; lb[r] = (int32_t)starts[2 * (c0 + r) + 1]; }
+    if (!gather(rec, n, sb.data(), lb.data(), nb, kChunkLen, starts_d, lens_d, wav, st)) return false;
+    if (!spk_embed_rows(s, wav, kChunkLen, full_d, nb, t_max, emb + (size_t)c0 * kSpkEmbDim)) return false;
+  }
+  std::vector<float> emb_h((size_t)nc * kSpkEmbDim);
+  cudaMemcpyAsync(emb_h.data(), emb, emb_h.size() * 4, cudaMemcpyDeviceToHost, st);
+  if (!sync_stream(st)) return false;
+  std::vector<int32_t> labels;
+  if (!spk_cluster(s, emb, nc, preset, emb_h.data(), labels, what)) return false;
+  std::vector<double> turns((size_t)3 * nc);
+  const int64_t nt = fa_spk_postprocess_host(times.data(), labels.data(), nc, turns.data());
+  std::vector<int32_t> sent((size_t)2 * ns);
+  for (int64_t g = 0; g < ns; ++g) { sent[2 * g] = segs[3 * g]; sent[2 * g + 1] = segs[3 * g + 1]; }
+  if (nt < 0 || fa_spk_distribute_host(sent.data(), ns, turns.data(), nt, spk.data()) != FA_OK) { set_err(what + "speaker post-processing failed"); return false; }
+  return true;
+}
+
+}  // namespace fa_handle
+
+extern "C" void* fa_spk_init(const char* model_file, int32_t device, int32_t gemm_mode) {
+  g_err.clear();
+  if (!valid_gemm_mode(gemm_mode)) return fail("bad gemm_mode");
+  return open_handle(model_file, device, gemm_mode, build_spk);
+}
+
+extern "C" void fa_spk_uninit(void* spk) { delete static_cast<Spk*>(spk); }
+
+extern "C" int fa_spk_embed(void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format, float* emb_host) {
+  g_err.clear();
+  Spk* s = static_cast<Spk*>(spk);
+  if (!s || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1) || !emb_host) { set_err("fa_spk_embed: bad argument"); return FA_ERR_ARG; }
+  int64_t nmax = 0;
+  int longest = 0;
+  for (int32_t i = 0; i < batch; ++i) {              // every input checked before any launch
+    if (!bufs[i] || n_samples[i] < 400 || n_samples[i] > 0x7fffffffLL) {
+      set_err("input " + std::to_string(i) + " has " + std::to_string(n_samples[i]) + " samples; CAM++ needs at least 400 (one 25 ms frame)");
+      return FA_ERR_ARG;
+    }
+    if (n_samples[i] > nmax) { nmax = n_samples[i]; longest = i; }
+  }
+  const int t_max = fbank_frames(nmax);
+  if (t_max > kSpkMaxFrames) {
+    set_err("input " + std::to_string(longest) + " has " + std::to_string(t_max) + " feature frames; CAM++ takes at most " +
+            std::to_string(kSpkMaxFrames) + " (MAX_FEAT_FRAMES)");
+    return FA_ERR_UNSUPPORTED;
+  }
+  cudaSetDevice(s->file.device);
+  cudaStream_t st = s->file.st;
+  const int64_t stride = (nmax + 3) / 4 * 4;
+  std::vector<int32_t> lens_h(batch);
+  for (int32_t i = 0; i < batch; ++i) lens_h[i] = (int32_t)n_samples[i];
+  const bool ok = no_throw("fa_spk_embed: ", [&] {
+    int32_t* lens;
+    float *emb, *wav;
+    if (!carve(s->embed, "CAM++", [&](fa::Arena& a) { lens = a.take<int32_t>(batch); emb = a.take<float>((size_t)batch * kSpkEmbDim); })) return false;
+    if (!upload(bufs, n_samples, batch, stride, pcm_format, s->upload, st, &wav)) return false;
+    cudaMemcpyAsync(lens, lens_h.data(), (size_t)batch * 4, cudaMemcpyHostToDevice, st);
+    if (!spk_embed_rows(*s, wav, stride, lens, batch, t_max, emb)) return false;
+    cudaMemcpyAsync(emb_host, emb, (size_t)batch * kSpkEmbDim * 4, cudaMemcpyDeviceToHost, st);
+    return sync_stream(st);
+  });
+  return ok ? FA_OK : FA_ERR_CUDA;
+}
+
+extern "C" int fa_spk_cluster(void* spk, const float* emb_host, int32_t n, int32_t preset_spk_num, int32_t* labels) {
+  g_err.clear();
+  Spk* s = static_cast<Spk*>(spk);
+  if (!s || !emb_host || n < 1 || !labels) { set_err("fa_spk_cluster: bad argument"); return FA_ERR_ARG; }
+  if (n >= kSpectralMaxChunks && preset_spk_num <= 0) {
+    set_err(std::to_string(n) + " speaker chunks without preset_spk_num: the reference clusters 2048 or more chunks with UMAP + HDBSCAN, which "
+            "this backend does not provide; pass preset_spk_num or diarize fewer than 2048 chunks");
+    return FA_ERR_UNSUPPORTED;
+  }
+  cudaSetDevice(s->file.device);
+  std::vector<int32_t> lab;
+  const bool ok = no_throw("fa_spk_cluster: ", [&] {
+    float* emb;
+    if (!carve(s->cluster_input, "speaker clustering", [&](fa::Arena& a) { emb = a.take<float>((size_t)n * kSpkEmbDim); })) return false;
+    cudaMemcpyAsync(emb, emb_host, (size_t)n * kSpkEmbDim * 4, cudaMemcpyHostToDevice, s->file.st);
+    return spk_cluster(*s, emb, n, preset_spk_num, emb_host, lab, "");
+  });
+  if (!ok) return FA_ERR_CUDA;
+  std::copy(lab.begin(), lab.end(), labels);
+  return FA_OK;
+}

@@ -1,6 +1,6 @@
 // Host text side of CT-Transformer punctuation (punc_text.cpp; no CUDA): the word split, the vocabulary lookup and the mini-sentence
 // walk of CTTransformer.inference, run in lockstep over many texts.  Shared by fa_punc_walk_host (any scorer) and fa_punc_infer (the
-// GPU forward as the scorer) in offline.cu: there is one walk.
+// GPU forward as the scorer) in offline_punc.cu: there is one walk.
 #pragma once
 #include <stdint.h>
 #include <functional>

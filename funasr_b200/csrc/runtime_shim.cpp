@@ -1,5 +1,5 @@
 // FunOffline* — the OfflineStream entry points of FunASR's C++ runtime (runtime/onnxruntime/include/funasrruntime.h:100-116) with
-// their exact C++ signatures, over this library's handle API (offline.cu: fa_offline_*).  Host-only C++: file / buffer decoding
+// their exact C++ signatures, over this library's handle API (offline_asr.cu / offline_long.cu: fa_offline_*).  Host-only C++: file / buffer decoding
 // (raw s16le PCM, RIFF WAV PCM16 / float32), the hotword encoder of ContextualParaformer (Embedding + 1-layer LSTM, O(#hotwords):
 // the reference runs it on the CPU too — model_eb.onnx, runtime/onnxruntime/src/paraformer.cpp CompileHotwordEmbedding) and the
 // ids -> text join.  Everything per audio frame runs in fa_offline_infer_hw on the GPU — or, with a VAD model ("vad-dir"), in

@@ -1,4 +1,4 @@
-"""Flat model file for the handle-style C API (csrc/offline.cu: fa_offline_init).
+"""Flat model file for the handle-style C API (csrc/offline_asr.cu: fa_offline_init).
 
 One file = every tensor the path needs under FunASR's own state_dict names (so it can be produced from an unmodified
 model.pt + am.mvn), plus the derived tables the kernels take as inputs:
@@ -26,7 +26,7 @@ bias_encoder.* under the reference's names, and
     bias_encoder.gemm_bias_l{k} [2048]  bias_ih_l{k} + bias_hh_l{k}: the hotword LSTM's input-projection GEMM bias
     __seaco_config__                    [3] no_bias, nfilter, LSTM layers
 
-The FSMN-VAD file (csrc/offline.cu: fa_vad_init) uses the same layout: the encoder's weights under the reference's names
+The FSMN-VAD file (csrc/offline_vad.cu: fa_vad_init) uses the same layout: the encoder's weights under the reference's names
 (encoder.in_linear1.linear.weight, encoder.fsmn.{i}.fsmn_block.conv_left.weight, ...), frontend.mel_banks / window / cmvn [2, 400]
 and
 
@@ -36,20 +36,20 @@ and
 
 The detector compares posteriors in double precision against speech_noise_thres and fe_prior_thres, so the options travel as float64.
 
-The CT-Transformer punctuation file (csrc/offline.cu: fa_punc_init) holds embed.weight, encoder.encoders0.0.*, encoder.encoders.{i}.*,
+The CT-Transformer punctuation file (csrc/offline_punc.cu: fa_punc_init) holds embed.weight, encoder.encoders0.0.*, encoder.encoders.{i}.*,
 encoder.after_norm.* and decoder.* under the reference's names, the derived encoder.pe_inv_timescales [embed_unit / 2], and
 
     __punc_config__                    [6] layers, d_model, heads, fsmn kernel, sentence_end_id, split_size (20)
     __punc_list__ / __punc_tokens__    the UTF-8 bytes of punc_list / token_list, newline-joined, zero-padded to a multiple of 4 and
                                        stored as the bytes of an fp32 tensor (like __vad_config__); the handle keeps them on the host
 
-The SenseVoiceSmall file (csrc/offline.cu: fa_offline_init, recognised by __sv_config__) holds encoder.encoders0.0.*,
+The SenseVoiceSmall file (csrc/offline_asr.cu: fa_offline_init, recognised by __sv_config__) holds encoder.encoders0.0.*,
 encoder.encoders.{i}.*, encoder.after_norm.*, encoder.tp_encoders.{i}.*, encoder.tp_norm.*, ctc.ctc_lo.* and embed.weight under the
 reference's names, the frontend tables and encoder.pe_inv_timescales of the Paraformer file, and
 
     __sv_config__                      [9] enc_layers, tp_layers, d_model, heads, fsmn kernel, vocab, feat_dim, ln_eps, blank_id
 
-The CAM++ speaker file (csrc/offline.cu: fa_spk_init, recognised by __spk_config__) holds every CAMPPlus state_dict tensor
+The CAM++ speaker file (csrc/offline_spk.cu: fa_spk_init, recognised by __spk_config__) holds every CAMPPlus state_dict tensor
 (head.*, xvector.*) under the reference's names, unfolded and without num_batches_tracked, frontend.mel_banks [80, 257] and the povey
 window frontend.window [400] (torchaudio kaldi.fbank's defaults), and
 
@@ -364,7 +364,7 @@ def _write(path: str, tensors: Dict[str, np.ndarray]) -> int:
 
 
 def read_model_file(path: str) -> Dict[str, np.ndarray]:
-    """Python reader of the same layout (tests; mirrors load_file() in csrc/offline.cu)."""
+    """Python reader of the same layout (tests; mirrors load_file() in csrc/handle_core.cu)."""
     out: Dict[str, np.ndarray] = {}
     with open(path, "rb") as f:
         if f.read(8) != MAGIC:
