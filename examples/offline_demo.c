@@ -2,7 +2,10 @@
  * FunOfflineInit / FunOfflineInferBuffer / FunASRGetResult (runtime/onnxruntime/include/funasrruntime.h:100-116).
  *
  *   gcc -std=c99 -Iinclude examples/offline_demo.c -Lfunasr_b200 -lfunasr_b200 -Wl,-rpath,$PWD/funasr_b200 -o offline_demo
- *   ./offline_demo model.fab2 audio.pcm        (audio.pcm: 16 kHz mono s16le; model.fab2 from funasr_b200/pack.py)
+ *   ./offline_demo model.fab2 audio.pcm [rate]  (audio.pcm: mono s16le, 16 kHz unless rate says otherwise; model.fab2 from
+ *                                               funasr_b200/pack.py)
+ * At 16 kHz it calls fa_offline_infer; at any other rate fa_offline_infer_audio, which resamples on the GPU with the C++ runtime's
+ * LinearResample (FA_RESAMPLE_RUNTIME).
  */
 #include <stdio.h>
 #include <stdlib.h>
@@ -28,7 +31,9 @@ int main(int argc, char** argv) {
   fclose(f);
   const void* bufs[1] = {pcm};
   int64_t n[1] = {bytes / 2};
-  void* r = fa_offline_infer(h, bufs, n, 1, /*pcm_format=*/1);
+  const int rate = argc > 3 ? atoi(argv[3]) : 16000;
+  const FaAudioFormat fmt = {/*sample_format=*/1, /*channels=*/1, rate, FA_RESAMPLE_RUNTIME};
+  void* r = rate == 16000 ? fa_offline_infer(h, bufs, n, 1, /*pcm_format=*/1) : fa_offline_infer_audio(h, bufs, n, 1, &fmt, NULL, 0, NULL, NULL);
   if (!r) { fprintf(stderr, "infer: %s\n", fa_offline_last_error()); return 1; }
   int32_t k = 0;
   const int32_t* ids = fa_offline_result_ids(r, 0, &k);

@@ -94,6 +94,19 @@ class FaLongAudioOptions(C.Structure):
                 ("vad", FaVadRunOptions)]
 
 
+class FaAudioFormat(C.Structure):
+    _fields_ = [("sample_format", C.c_int32), ("channels", C.c_int32), ("sample_rate", C.c_int32), ("resampler", C.c_int32)]
+
+
+RESAMPLE_LOADER, RESAMPLE_RUNTIME = 0, 1
+RESAMPLERS = {"loader": RESAMPLE_LOADER, "runtime": RESAMPLE_RUNTIME}
+
+
+class FaIngestTable(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("in_unit", C.c_int32), ("out_unit", C.c_int32), ("width", C.c_int32), ("taps", C.c_int32),
+                ("_pad", C.c_int32), ("weights", C.c_void_p), ("first", C.c_void_p), ("n_taps", C.c_void_p)]
+
+
 class FaCamConv2d(C.Structure):
     _fields_ = [("w", C.c_void_p), ("b", C.c_void_p), ("c_in", C.c_int32), ("c_out", C.c_int32), ("ksize", C.c_int32), ("stride_f", C.c_int32)]
 
@@ -182,6 +195,16 @@ SIGNATURES = {
     "fa_embedding": (C.c_int, [_vp, _vp, _i32, _i32, _i64, _vp, _vp]),
     "fa_pcm_decode": (C.c_int, [_vp, _i32, _i32, _i64, _vp, _vp]),
     "fa_resample": (C.c_int, [_vp, _vp, _i32, _i64, _vp, _i32, _i32, _i32, _vp, _i64, _i32, _vp, _vp]),
+    # audio at any rate and PCM layout: the host tables (host_ops.cpp), the ingest kernel (resample.cu) and the handle entries
+    "fa_loader_resample_table_host": (_i64, [_i32, _i32, c_i32p, c_i32p, c_i32p, _vp, _i64]),
+    "fa_runtime_resample_table_host": (_i64, [_i32, _i32, c_i32p, c_i32p, c_i32p, _vp, _vp, _vp, _i64]),
+    "fa_runtime_resample_out_len_host": (_i64, [_i32, _i32, _i64]),
+    "fa_ingest_pcm": (C.c_int, [_vp, _vp, _i32, _i32, _i32, C.POINTER(FaIngestTable), _vp, _i64, _vp]),
+    "fa_offline_infer_audio": (_vp, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, C.POINTER(FaAudioFormat), _vp, _i32, _vp, _vp]),
+    "fa_offline_infer_vad_audio": (_vp, [_vp, _vp, _vp, C.POINTER(_vp), C.POINTER(_i64), _i32, C.POINTER(FaAudioFormat), _vp, _i32, _vp, _vp,
+                                         C.POINTER(FaLongAudioOptions), _i32]),
+    "fa_vad_infer_audio": (_vp, [_vp, _vp, _i64, C.POINTER(FaAudioFormat), C.POINTER(FaVadRunOptions)]),
+    "fa_spk_embed_audio": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, C.POINTER(FaAudioFormat), _vp]),
     # CAM++ speaker embedding (campplus.cu)
     "fa_campplus_features": (C.c_int, [_vp, _vp, _i32, _i64, _vp, _vp, _vp, _i32, _vp]),
     "fa_campplus_workspace_bytes": (_sz, [C.POINTER(FaCampplus), _i32, _i32, _i32]),

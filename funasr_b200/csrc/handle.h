@@ -2,7 +2,7 @@
 // fa_offline_last_error, the model-file loader, the two-pass Builder, the grow-only device buffers each call carves its memory from,
 // and the handle structs and functions that cross files (long audio runs the recogniser, the VAD and the speaker model).
 //
-//   handle_core.cu   file loader, Builder, upload (pcm16_to_f32_kernel), fa_gather_segments (gather_segments_kernel)
+//   handle_core.cu   file loader, Builder, plan_audio / upload (pcm16_to_f32_kernel, fa_ingest_pcm), fa_gather_segments
 //   offline_asr.cu   recogniser (Paraformer, contextual, BiCif, SeACo, SenseVoice): fa_offline_*
 //   offline_vad.cu   FSMN-VAD: fa_vad_*
 //   offline_spk.cu   CAM++ speaker embeddings, clustering, diarization: fa_spk_*
@@ -201,8 +201,43 @@ std::string enc_layer_prefix(bool tp, int i);
 // encoders and punctuation's)
 void bind_stack(Builder& b, bool tp, int n, int in, int D, int heads, std::vector<FaEncLayer>& L, FaEncoder& e);
 
-// B host recordings bufs[i] of n[i] samples (f32, or s16le staged on the device) into rows of `stride` floats, *wav, carved from buf
-bool upload(const void* const* bufs, const int64_t* n, int B, int64_t stride, int32_t pcm_format, DevBuf& buf, cudaStream_t st, float** wav);
+// ------------------------------------------------------------------------------------------------ audio in (FaAudioFormat)
+// One (rate, resampler)'s host tables; fa_ingest_pcm reads their device copy
+struct ResampleTable {
+  FaIngestTable t{};                                 // the shape; the device pointers are set per upload
+  std::vector<float> weights;
+  std::vector<int32_t> first, n_taps;                // runtime: each phase's first input index and taps; loader: each row's nonzero span
+};
+
+// A handle's resampling tables keyed by (rate, resampler), built on the host when first needed and kept (grow-only, like its
+// buffers), and the host rows of the last upload
+struct ResampleCache {
+  std::map<std::pair<int32_t, int32_t>, ResampleTable> tables;
+  std::vector<int64_t> rows;
+};
+
+// The caller's audio layout, checked, with its table (nullptr at 16 kHz)
+struct Audio {
+  FaAudioFormat fmt{};
+  const ResampleTable* tab = nullptr;
+  // 16 kHz mono f32 / s16: the upload the 16 kHz entries always had (a copy, or the s16 conversion kernel)
+  bool direct() const { return fmt.sample_rate == 16000 && fmt.channels == 1 && (fmt.sample_format == 0 || fmt.sample_format == 1); }
+  int64_t frame_bytes() const;
+  int64_t len16(int64_t frames) const;               // the 16 kHz samples of `frames` frames
+  double seconds(const int64_t* n, int B) const;     // the caller's frames at the caller's rate
+  std::string at16k() const { return fmt.sample_rate == 16000 ? "" : " at 16 kHz"; }
+};
+
+// fmt checked (NULL, sample_format, channels 1..64, resampler, rate 1 000..192 000, a table above 32 MiB) and its table built or
+// found in cache; false: the refusal set, nothing touched a device
+bool plan_audio(const FaAudioFormat* fmt, ResampleCache& cache, Audio& a);
+// f = the descriptor of a 16 kHz entry's pcm_format; &f for 0 (f32) and 1 (s16le), NULL for any other value (a bad argument)
+const FaAudioFormat* pcm16k_format(int32_t pcm_format, FaAudioFormat& f);
+
+// B host recordings bufs[i] of n[i] frames in a's layout into 16 kHz rows of `stride` floats, *wav, carved from buf with the staged
+// bytes and the table: direct() as the 16 kHz entries always did, otherwise one fa_ingest_pcm launch
+bool upload(const void* const* bufs, const int64_t* n, int B, int64_t stride, const Audio& a, ResampleCache& cache, DevBuf& buf,
+            cudaStream_t st, float** wav);
 
 // rows segments of the device recording rec [n]: the host starts / lengths (samples) copied into starts_d / lens_d, then
 // fa_gather_segments into out [rows, stride] with zero tails.  The caller keeps the host arrays alive until the stream passes them.
@@ -248,6 +283,7 @@ struct Model {
   std::vector<FaLinear> hw_ih, hw_hh;
   FaHotwordEncoder hw_enc{};
   // device memory, each DevBuf carved by the function it is named after
+  ResampleCache resample;
   DevBuf upload;                                     // the host batch of fa_offline_infer*, the recording of long audio
   DevBuf encode, decode, seaco_bias, decode_sv;      // decode_batch before and after its token-count sync; seaco_bias; decode_sv
   DevBuf hotword_embed;                              // fa_offline_hotword_embed's rows
@@ -282,6 +318,7 @@ struct Vad {
   FaVadEncoder enc{};
   FaVadOptions opts{};
   const float* cmvn = nullptr;
+  ResampleCache resample;
   DevBuf upload;                                     // fa_vad_infer's recording
   DevBuf vad_run;
 };
@@ -301,6 +338,7 @@ struct Spk {
   int mode = FA_GEMM_F32_SIMT;
   FaCampplus model{};
   std::vector<FaCamLayer> layers;
+  ResampleCache resample;
   DevBuf upload;                                     // fa_spk_embed's batch
   DevBuf embed, cluster_input;                       // fa_spk_embed's lengths and embeddings; fa_spk_cluster's embeddings
   DevBuf spk_embed_rows, diarize, spk_cluster;

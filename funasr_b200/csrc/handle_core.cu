@@ -1,5 +1,5 @@
-// Core of the handle-style C API (handle.h): the model-file loader, the SAN-M stack binder, the upload of host PCM and the device
-// gather of recording segments.
+// Core of the handle-style C API (handle.h): the model-file loader, the SAN-M stack binder, the checked audio layout and the upload
+// of host PCM in it, and the device gather of recording segments.
 #include "handle.h"
 #include <stdio.h>
 #include <string.h>
@@ -130,21 +130,143 @@ void bind_stack(Builder& b, bool tp, int n, int in, int D, int heads, std::vecto
   }
 }
 
-bool upload(const void* const* bufs, const int64_t* n, int B, int64_t stride, int32_t pcm_format, DevBuf& buf, cudaStream_t st, float** wav) {
+int64_t Audio::frame_bytes() const {
+  static const int kBytes[5] = {4, 2, 3, 4, 1};
+  return (int64_t)kBytes[fmt.sample_format] * fmt.channels;
+}
+
+int64_t Audio::len16(int64_t frames) const {
+  if (!tab) return frames;
+  if (tab->t.mode == FA_RESAMPLE_LOADER) return ((int64_t)tab->t.out_unit * frames + tab->t.in_unit - 1) / tab->t.in_unit;   // fa_resample's
+  return fa_runtime_resample_out_len_host(fmt.sample_rate, 16000, frames);
+}
+
+double Audio::seconds(const int64_t* n, int B) const {
+  double s = 0.0;
+  for (int i = 0; i < B; ++i) s += (double)n[i] / fmt.sample_rate;
+  return s;
+}
+
+bool plan_audio(const FaAudioFormat* fmt, ResampleCache& cache, Audio& a) {
+  if (!fmt) { set_err("audio format is NULL"); return false; }
+  const FaAudioFormat f = *fmt;
+  if (f.sample_format < 0 || f.sample_format > 4) {
+    set_err("bad sample_format " + std::to_string(f.sample_format) + " (0 f32, 1 s16le, 2 s24le, 3 s32le, 4 u8)");
+    return false;
+  }
+  if (f.channels < 1 || f.channels > 64) { set_err("channels " + std::to_string(f.channels) + " outside 1..64"); return false; }
+  if (f.resampler != FA_RESAMPLE_LOADER && f.resampler != FA_RESAMPLE_RUNTIME) {
+    set_err("bad resampler " + std::to_string(f.resampler) + " (0 FA_RESAMPLE_LOADER, 1 FA_RESAMPLE_RUNTIME)");
+    return false;
+  }
+  if (f.sample_rate < 1000 || f.sample_rate > 192000) {
+    set_err("sample rate " + std::to_string(f.sample_rate) + " Hz outside 1000..192000 Hz");
+    return false;
+  }
+  a.fmt = f;
+  a.tab = nullptr;
+  if (f.sample_rate == 16000) return true;
+  const std::pair<int32_t, int32_t> key(f.sample_rate, f.resampler);
+  auto it = cache.tables.find(key);
+  if (it != cache.tables.end()) { a.tab = &it->second; return true; }
+  ResampleTable t;
+  FaIngestTable& d = t.t;
+  d.mode = f.resampler;
+  int64_t need = 0;
+  if (f.resampler == FA_RESAMPLE_LOADER) {
+    need = fa_loader_resample_table_host(f.sample_rate, 16000, &d.in_unit, &d.out_unit, &d.width, nullptr, 0);
+    if (need > 0) {
+      d.taps = 2 * d.width + d.in_unit;
+      t.weights.resize((size_t)need);
+      need = fa_loader_resample_table_host(f.sample_rate, 16000, &d.in_unit, &d.out_unit, &d.width, t.weights.data(), need);
+      t.first.assign(d.out_unit, 0); t.n_taps.assign(d.out_unit, 0);
+      for (int32_t j = 0; j < d.out_unit; ++j) {     // each row's nonzero span: 34 of 475 taps at 44.1 kHz
+        const float* row = t.weights.data() + (size_t)j * d.taps;
+        int32_t k0 = 0, k1 = d.taps;
+        while (k0 < k1 && row[k0] == 0.0f) ++k0;
+        while (k1 > k0 && row[k1 - 1] == 0.0f) --k1;
+        t.first[j] = k0; t.n_taps[j] = k1 - k0;
+      }
+    }
+  } else {
+    need = fa_runtime_resample_table_host(f.sample_rate, 16000, &d.in_unit, &d.out_unit, &d.taps, nullptr, nullptr, nullptr, 0);
+    if (need > 0) {
+      t.weights.resize((size_t)need); t.first.resize(d.out_unit); t.n_taps.resize(d.out_unit);
+      need = fa_runtime_resample_table_host(f.sample_rate, 16000, &d.in_unit, &d.out_unit, &d.taps, t.first.data(), t.n_taps.data(),
+                                            t.weights.data(), need);
+    }
+  }
+  if (need <= 0) {
+    set_err("sample rate " + std::to_string(f.sample_rate) + " Hz: its " + (f.resampler == FA_RESAMPLE_LOADER ? "loader" : "runtime") +
+            " resampling table to 16 kHz exceeds 32 MiB");
+    return false;
+  }
+  a.tab = &(cache.tables[key] = std::move(t));
+  return true;
+}
+
+const FaAudioFormat* pcm16k_format(int32_t pcm_format, FaAudioFormat& f) {
+  f = FaAudioFormat{pcm_format, 1, 16000, FA_RESAMPLE_LOADER};
+  return pcm_format == 0 || pcm_format == 1 ? &f : nullptr;
+}
+
+bool upload(const void* const* bufs, const int64_t* n, int B, int64_t stride, const Audio& au, ResampleCache& cache, DevBuf& buf,
+            cudaStream_t st, float** wav) {
   const int64_t tot = (int64_t)B * stride;
-  int16_t* p16 = nullptr;
+  if (au.direct()) {
+    const int32_t pcm_format = au.fmt.sample_format;
+    int16_t* p16 = nullptr;
+    if (!carve(buf, "waveforms", [&](fa::Arena& a) {
+          *wav = a.take<float>((size_t)(tot > 0 ? tot : 4));
+          if (pcm_format == 1) p16 = a.take<int16_t>((size_t)tot);
+        }))
+      return false;
+    if (tot == 0) return true;
+    if (pcm_format == 1) {
+      for (int i = 0; i < B; ++i) cudaMemcpyAsync(p16 + (int64_t)i * stride, bufs[i], (size_t)n[i] * 2, cudaMemcpyHostToDevice, st);
+      pcm16_to_f32_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(p16, *wav, tot);
+    } else {
+      for (int i = 0; i < B; ++i) cudaMemcpyAsync(*wav + (int64_t)i * stride, bufs[i], (size_t)n[i] * 4, cudaMemcpyHostToDevice, st);
+    }
+    return true;
+  }
+  // rows {byte offset, frames, 16 kHz length}; each row's bytes start 16-byte aligned
+  std::vector<int64_t>& rows = cache.rows;
+  rows.resize((size_t)3 * B);
+  int64_t bytes = 0;
+  for (int i = 0; i < B; ++i) {
+    rows[3 * i] = bytes; rows[3 * i + 1] = n[i]; rows[3 * i + 2] = au.len16(n[i]);
+    bytes += (n[i] * au.frame_bytes() + 15) / 16 * 16;
+  }
+  FaIngestTable t = au.tab ? au.tab->t : FaIngestTable{};
+  if (!au.tab) t.mode = -1;
+  unsigned char* raw;
+  int64_t* rows_d;
+  float* w = nullptr;
+  int32_t *first = nullptr, *n_taps = nullptr;
   if (!carve(buf, "waveforms", [&](fa::Arena& a) {
         *wav = a.take<float>((size_t)(tot > 0 ? tot : 4));
-        if (pcm_format == 1) p16 = a.take<int16_t>((size_t)tot);
+        raw = a.take<unsigned char>((size_t)(bytes > 0 ? bytes : 16));
+        rows_d = a.take<int64_t>((size_t)3 * B);
+        if (au.tab) w = a.take<float>(au.tab->weights.size());
+        if (au.tab && !au.tab->first.empty()) { first = a.take<int32_t>(au.tab->first.size()); n_taps = a.take<int32_t>(au.tab->n_taps.size()); }
       }))
     return false;
   if (tot == 0) return true;
-  if (pcm_format == 1) {
-    for (int i = 0; i < B; ++i) cudaMemcpyAsync(p16 + (int64_t)i * stride, bufs[i], (size_t)n[i] * 2, cudaMemcpyHostToDevice, st);
-    pcm16_to_f32_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(p16, *wav, tot);
-  } else {
-    for (int i = 0; i < B; ++i) cudaMemcpyAsync(*wav + (int64_t)i * stride, bufs[i], (size_t)n[i] * 4, cudaMemcpyHostToDevice, st);
+  // pageable host sources: each copy returns once its bytes are staged, so rows and the cached tables may change after it
+  for (int i = 0; i < B; ++i) cudaMemcpyAsync(raw + rows[3 * i], bufs[i], (size_t)(n[i] * au.frame_bytes()), cudaMemcpyHostToDevice, st);
+  cudaMemcpyAsync(rows_d, rows.data(), rows.size() * 8, cudaMemcpyHostToDevice, st);
+  if (au.tab) {
+    cudaMemcpyAsync(w, au.tab->weights.data(), au.tab->weights.size() * 4, cudaMemcpyHostToDevice, st);
+    t.weights = w;
+    if (first) {
+      cudaMemcpyAsync(first, au.tab->first.data(), au.tab->first.size() * 4, cudaMemcpyHostToDevice, st);
+      cudaMemcpyAsync(n_taps, au.tab->n_taps.data(), au.tab->n_taps.size() * 4, cudaMemcpyHostToDevice, st);
+      t.first = first; t.n_taps = n_taps;
+    }
   }
+  const int rc = fa_ingest_pcm(raw, rows_d, B, au.fmt.sample_format, au.fmt.channels, &t, *wav, stride, st);
+  if (rc != FA_OK) { set_err(std::string("fa_ingest_pcm: ") + fa_status_string(rc)); return false; }
   return true;
 }
 

@@ -515,3 +515,122 @@ extern "C" int fa_spk_distribute_host(const int32_t* sentences, int64_t ns, cons
   }
   return FA_OK;
 }
+
+// ------------------------------------------------------------------------------------------------ resampling tables (to 16 kHz)
+namespace {
+
+const int64_t kMaxTableFloats = (32ll << 20) / 4;   // 32 MiB of weights
+
+int32_t gcd32(int32_t a, int32_t b) {
+  while (b) { const int32_t t = a % b; a = b; b = t; }
+  return a;
+}
+
+bool rate_ok(int32_t rate, int32_t new_rate) { return rate >= 1000 && rate <= 192000 && new_rate >= 1000 && new_rate <= 192000; }
+
+// LinearResample's phase p < out_unit (kaldi feat/resample.cc SetIndexesAndWeights): output time p / out_rate, the input indices
+// within num_zeros / (2 cutoff) seconds of it (ceil of the lower edge, floor of the upper), weight FilterFunc(float(dt)) / in_rate.
+// The arithmetic mixes float and double as the definition does: the cutoff is a float, FilterFunc takes and returns a float, its
+// window and sinc are evaluated in double.
+struct LinearResampleDef {
+  int32_t in_rate, out_rate, in_unit, out_unit;
+  float cutoff;
+  int32_t zeros = 6;
+  LinearResampleDef(int32_t in, int32_t out) : in_rate(in), out_rate(out) {
+    const int32_t g = gcd32(in, out);
+    in_unit = in / g; out_unit = out / g;
+    const float min_freq = (float)std::min(in, out);
+    cutoff = (float)(0.99 * 0.5 * min_freq);
+  }
+  double window_width() const { return zeros / (2.0 * cutoff); }
+  float filter(float t) const {
+    const double two_pi = 6.283185307179586476925286766559005, pi = 3.1415926535897932384626433832795;
+    float window, f;
+    if (std::fabs(t) < zeros / (2.0 * cutoff)) window = (float)(0.5 * (1 + std::cos(two_pi * cutoff / zeros * t)));
+    else window = 0.0f;
+    if (t != 0) f = (float)(std::sin(two_pi * cutoff * t) / (pi * t));
+    else f = 2 * cutoff;
+    return f * window;
+  }
+  void span(int32_t p, int32_t* first, int32_t* n) const {
+    const double ww = window_width(), out_t = p / (double)out_rate;
+    const double min_t = out_t - ww, max_t = out_t + ww;
+    const int32_t lo = (int32_t)std::ceil(min_t * in_rate), hi = (int32_t)std::floor(max_t * in_rate);
+    *first = lo; *n = hi - lo + 1;
+  }
+  float weight(int32_t p, int32_t index) const {
+    const double out_t = p / (double)out_rate, in_t = index / (double)in_rate, dt = in_t - out_t;
+    return filter((float)dt) / in_rate;
+  }
+};
+
+}  // namespace
+
+// resample.sinc_resample_table (torchaudio's _get_sinc_resample_kernel, lowpass width 6, rolloff 0.99): the shift j / new rounded to
+// float32 (torch divides an int64 arange by an int there), the grid in float64, the window cos(t pi / 6 / 2) squared, sin(pi t) /
+// (pi t) with 1 at 0, times base / orig, rounded to float32.  glibc's sin / cos are numpy's on x86-64.
+extern "C" int64_t fa_loader_resample_table_host(int32_t rate, int32_t new_rate, int32_t* orig_out, int32_t* nnew_out, int32_t* width_out,
+                                                 float* table, int64_t cap) {
+  if (!rate_ok(rate, new_rate)) return FA_ERR_ARG;
+  const int32_t g = gcd32(rate, new_rate), orig = rate / g, nw = new_rate / g;
+  const double lpw = 6, base = std::min(orig, nw) * 0.99;
+  const int32_t width = (int32_t)std::ceil(6 * orig / base);
+  const int64_t taps = 2 * (int64_t)width + orig, need = (int64_t)nw * taps;
+  if (need > kMaxTableFloats) return FA_ERR_UNSUPPORTED;
+  if (orig_out) *orig_out = orig;
+  if (nnew_out) *nnew_out = nw;
+  if (width_out) *width_out = width;
+  if (!table) return need;
+  if (cap < need) return FA_ERR_ARG;
+  const double scale = base / orig, pi = 3.141592653589793;
+  for (int32_t j = 0; j < nw; ++j) {
+    const double shift = (double)((float)(-j) / (float)nw);
+    for (int64_t k = 0; k < taps; ++k) {
+      const double idx = (double)(k - width) / orig;
+      double t = (shift + idx) * base;
+      t = std::min(std::max(t, -lpw), lpw);
+      double w = std::cos(t * pi / lpw / 2);
+      w = w * w;
+      t = t * pi;
+      const double kern = t == 0 ? 1.0 : std::sin(t) / t;
+      table[(int64_t)j * taps + k] = (float)(kern * w * scale);
+    }
+  }
+  return need;
+}
+
+extern "C" int64_t fa_runtime_resample_table_host(int32_t rate, int32_t new_rate, int32_t* in_unit, int32_t* out_unit, int32_t* max_taps,
+                                                  int32_t* first, int32_t* n_taps, float* weights, int64_t cap) {
+  if (!rate_ok(rate, new_rate)) return FA_ERR_ARG;
+  const LinearResampleDef d(rate, new_rate);
+  int32_t longest = 0;
+  for (int32_t p = 0; p < d.out_unit; ++p) {
+    int32_t lo, n;
+    d.span(p, &lo, &n);
+    longest = std::max(longest, n);
+  }
+  const int64_t need = (int64_t)d.out_unit * longest;
+  if (need > kMaxTableFloats) return FA_ERR_UNSUPPORTED;
+  if (in_unit) *in_unit = d.in_unit;
+  if (out_unit) *out_unit = d.out_unit;
+  if (max_taps) *max_taps = longest;
+  if (!weights) return need;
+  if (cap < need || !first || !n_taps) return FA_ERR_ARG;
+  for (int32_t p = 0; p < d.out_unit; ++p) {
+    d.span(p, &first[p], &n_taps[p]);
+    float* row = weights + (int64_t)p * longest;
+    for (int32_t j = 0; j < longest; ++j) row[j] = j < n_taps[p] ? d.weight(p, first[p] + j) : 0.0f;
+  }
+  return need;
+}
+
+// the largest count c with (c - 1) / out_rate inside [0, n / in_rate), in ticks of 1 / lcm(in_rate, out_rate)
+extern "C" int64_t fa_runtime_resample_out_len_host(int32_t rate, int32_t new_rate, int64_t n) {
+  if (!rate_ok(rate, new_rate) || n < 0) return FA_ERR_ARG;
+  const int64_t tick = (int64_t)rate / gcd32(rate, new_rate) * new_rate;
+  const int64_t ticks = n * (tick / rate), per_out = tick / new_rate;
+  if (ticks <= 0) return 0;
+  int64_t last = ticks / per_out;
+  if (last * per_out == ticks) --last;
+  return last + 1;
+}

@@ -427,26 +427,31 @@ std::unique_ptr<Result> decode_sv(Model& m, const float* wav, int64_t stride, co
   return r;
 }
 
-// fa_offline_infer_hw / fa_offline_infer_sv: host buffers -> one padded batch -> decode_pack
-void* infer_batch(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format, const float* hw_embed,
+// fa_offline_infer_hw / fa_offline_infer_sv / fa_offline_infer_audio: host buffers -> one padded 16 kHz batch -> decode_pack
+void* infer_batch(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, const FaAudioFormat* fmt, const float* hw_embed,
                   int32_t n_hotwords, const int32_t* lang, const int32_t* tn) {
   Model* mp = static_cast<Model*>(handle);
-  if (!mp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) return fail("bad argument");
+  if (!mp || !bufs || !n_samples || batch <= 0) return fail("bad argument");
   Model& m = *mp;
+  Audio au;
+  if (!plan_audio(fmt, m.resample, au)) return nullptr;
   if (!check_hotword_rows(m, hw_embed, n_hotwords)) return nullptr;
   if (m.sv && !check_queries(m, lang, tn, batch, "utterance")) return nullptr;
   cudaSetDevice(m.file.device);
   int64_t nmax = 0;
   std::vector<int32_t> lens_h(batch);
   for (int i = 0; i < batch; ++i) {
-    if (!bufs[i] || n_samples[i] < 400 || n_samples[i] > 0x7fffffffLL) return fail("every buffer needs >= 400 samples (25 ms)");
-    lens_h[i] = (int32_t)n_samples[i];
-    nmax = n_samples[i] > nmax ? n_samples[i] : nmax;
+    const int64_t n16 = bufs[i] && n_samples[i] >= 0 && n_samples[i] <= 0x7fffffffLL ? au.len16(n_samples[i]) : 0;
+    if (n16 < 400 || n16 > 0x7fffffffLL) return fail("every buffer needs >= 400 samples (25 ms)" + au.at16k());
+    lens_h[i] = (int32_t)n16;
+    nmax = n16 > nmax ? n16 : nmax;
   }
   const int64_t stride = (nmax + 3) / 4 * 4;
   float* wav = nullptr;
-  if (!upload(bufs, n_samples, batch, stride, pcm_format, m.upload, m.file.st, &wav)) return nullptr;
-  return decode_pack(m, wav, stride, lens_h, hw_embed, n_hotwords, lang, tn).release();
+  if (!upload(bufs, n_samples, batch, stride, au, m.resample, m.upload, m.file.st, &wav)) return nullptr;
+  std::unique_ptr<Result> r = decode_pack(m, wav, stride, lens_h, hw_embed, n_hotwords, lang, tn);
+  if (r) r->audio_seconds = (float)au.seconds(n_samples, batch);
+  return r.release();
 }
 
 // the model kind is the file's: SenseVoiceSmall by __sv_config__, Paraformer otherwise
@@ -502,7 +507,9 @@ extern "C" void* fa_offline_infer_sv(void* handle, const void* const* bufs, cons
                                      const int32_t* language_ids, const int32_t* textnorm_ids) {
   g_err.clear();
   if (handle && !static_cast<Model*>(handle)->sv) return fail("fa_offline_infer_sv: not a SenseVoice model file");
-  return infer_batch(handle, bufs, n_samples, batch, pcm_format, nullptr, 0, language_ids, textnorm_ids);
+  FaAudioFormat f;
+  if (!pcm16k_format(pcm_format, f)) return fail("bad argument");
+  return infer_batch(handle, bufs, n_samples, batch, &f, nullptr, 0, language_ids, textnorm_ids);
 }
 
 extern "C" void fa_offline_uninit(void* handle) { delete static_cast<Model*>(handle); }
@@ -565,7 +572,17 @@ extern "C" const float* fa_offline_host_tensor(void* handle, const char* name, i
 extern "C" void* fa_offline_infer_hw(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
                                      const float* hw_embed, int32_t n_hotwords) {
   g_err.clear();
-  return infer_batch(handle, bufs, n_samples, batch, pcm_format, hw_embed, n_hotwords, nullptr, nullptr);
+  FaAudioFormat f;
+  if (!pcm16k_format(pcm_format, f)) return fail("bad argument");
+  return infer_batch(handle, bufs, n_samples, batch, &f, hw_embed, n_hotwords, nullptr, nullptr);
+}
+
+extern "C" void* fa_offline_infer_audio(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, const FaAudioFormat* fmt,
+                                        const float* hw_embed, int32_t n_hotwords, const int32_t* language_ids, const int32_t* textnorm_ids) {
+  g_err.clear();
+  if (handle && !static_cast<Model*>(handle)->sv && (language_ids || textnorm_ids))
+    return fail("fa_offline_infer_audio: language / text-norm ids need a SenseVoice model file");
+  return infer_batch(handle, bufs, n_samples, batch, fmt, hw_embed, n_hotwords, language_ids, textnorm_ids);
 }
 
 extern "C" void* fa_offline_infer(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format) {

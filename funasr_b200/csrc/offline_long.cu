@@ -77,14 +77,17 @@ bool long_audio_one(Model& m, Vad& v, int rec_index, const float* rec, int64_t n
   return true;
 }
 
-// fa_offline_infer_vad / fa_offline_infer_vad_sv: every recording on its own; lang / tn one query per recording (NULL = the defaults)
+// fa_offline_infer_vad* / fa_offline_infer_vad_audio: every recording on its own; lang / tn one query per recording (NULL = the defaults)
 // spk: diarize every recording that decoded at least one token (LongAudioPipeline.generate), preset_spk_num <= 0: no preset count
-void* infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format, const float* hw_embed,
+// fmt: the recordings' layout (the 16 kHz entries pass their pcm_format's)
+void* infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, const FaAudioFormat* fmt, const float* hw_embed,
                 int32_t n_hotwords, const int32_t* lang, const int32_t* tn, const FaLongAudioOptions* opts, Spk* spk = nullptr,
                 int32_t preset_spk_num = 0) {
   Model* mp = static_cast<Model*>(asr);
   Vad* vp = static_cast<Vad*>(vad);
-  if (!mp || !vp || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1)) return fail("bad argument");
+  if (!mp || !vp || !bufs || !n_samples || batch <= 0) return fail("bad argument");
+  Audio au;
+  if (!plan_audio(fmt, mp->resample, au)) return nullptr;
   if (mp->file.device != vp->file.device) return fail("the recogniser and the VAD live on different devices");
   if (spk && spk->file.device != mp->file.device) return fail("the recogniser and the speaker model live on different devices");
   if (!check_hotword_rows(*mp, hw_embed, n_hotwords)) return nullptr;
@@ -92,8 +95,12 @@ void* infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_
   FaLongAudioOptions o;
   if (opts) o = *opts;
   else { o.batch_size_s = 300; o.batch_size_threshold_s = 60; o.merge_vad = 0; o.merge_length_s = 15; o.vad = default_vad_run(); }
-  for (int i = 0; i < batch; ++i)
+  std::vector<int64_t> n16(batch);
+  for (int i = 0; i < batch; ++i) {
     if ((!bufs[i] && n_samples[i] > 0) || n_samples[i] < 0 || n_samples[i] > 0x7fffffffLL) return fail("bad recording " + std::to_string(i));
+    n16[i] = au.len16(n_samples[i]);
+    if (n16[i] > 0x7fffffffLL) return fail("bad recording " + std::to_string(i));
+  }
   cudaSetDevice(mp->file.device);
   std::unique_ptr<Result> r(new Result());
   r->ids.resize(batch);
@@ -102,25 +109,23 @@ void* infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_
   r->ts = mp->ts;
   r->stamps.resize(batch);
   r->spk.resize(batch);
-  double seconds = 0.0;
   if (!no_throw("fa_offline_infer_vad: ", [&] {
         for (int i = 0; i < batch; ++i) {
-          seconds += (double)n_samples[i] / 16000.0;
           float* rec = nullptr;
-          if (!upload(&bufs[i], &n_samples[i], 1, (n_samples[i] + 3) / 4 * 4, pcm_format, mp->upload, mp->file.st, &rec) ||
-              !long_audio_one(*mp, *vp, i, rec, n_samples[i], hw_embed, n_hotwords, lang ? lang[i] : kSvAuto, tn ? tn[i] : kSvWoItn, o, r->ids[i],
+          if (!upload(&bufs[i], &n_samples[i], 1, (n16[i] + 3) / 4 * 4, au, mp->resample, mp->upload, mp->file.st, &rec) ||
+              !long_audio_one(*mp, *vp, i, rec, n16[i], hw_embed, n_hotwords, lang ? lang[i] : kSvAuto, tn ? tn[i] : kSvWoItn, o, r->ids[i],
                               r->segs[i], r->stamps[i]))
             return false;
           r->token_num[i] = (int32_t)r->ids[i].size();
           // the recogniser's stream is idle here (its results are on the host); the speaker work runs on the speaker handle's stream
           if (spk && !r->ids[i].empty() &&
-              !diarize(*spk, rec, n_samples[i], r->segs[i], preset_spk_num, r->spk[i], "recording " + std::to_string(i) + ": "))
+              !diarize(*spk, rec, n16[i], r->segs[i], preset_spk_num, r->spk[i], "recording " + std::to_string(i) + ": "))
             return false;
         }
         return true;
       }))
     return nullptr;
-  r->audio_seconds = (float)seconds;
+  r->audio_seconds = (float)au.seconds(n_samples, batch);
   return r.release();
 }
 
@@ -131,14 +136,18 @@ const Result* as_result(const void* r) { return static_cast<const Result*>(r); }
 extern "C" void* fa_offline_infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
                                       const float* hw_embed, int32_t n_hotwords, const FaLongAudioOptions* opts) {
   g_err.clear();
-  return infer_vad(asr, vad, bufs, n_samples, batch, pcm_format, hw_embed, n_hotwords, nullptr, nullptr, opts);
+  FaAudioFormat f;
+  if (!pcm16k_format(pcm_format, f)) return fail("bad argument");
+  return infer_vad(asr, vad, bufs, n_samples, batch, &f, hw_embed, n_hotwords, nullptr, nullptr, opts);
 }
 
 extern "C" void* fa_offline_infer_vad_sv(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format,
                                          const int32_t* language_ids, const int32_t* textnorm_ids, const FaLongAudioOptions* opts) {
   g_err.clear();
   if (asr && !static_cast<Model*>(asr)->sv) return fail("fa_offline_infer_vad_sv: not a SenseVoice model file");
-  return infer_vad(asr, vad, bufs, n_samples, batch, pcm_format, nullptr, 0, language_ids, textnorm_ids, opts);
+  FaAudioFormat f;
+  if (!pcm16k_format(pcm_format, f)) return fail("bad argument");
+  return infer_vad(asr, vad, bufs, n_samples, batch, &f, nullptr, 0, language_ids, textnorm_ids, opts);
 }
 
 extern "C" void* fa_offline_infer_vad_spk(void* asr, void* vad, void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch,
@@ -147,7 +156,19 @@ extern "C" void* fa_offline_infer_vad_spk(void* asr, void* vad, void* spk, const
   g_err.clear();
   if (!spk) return fail("fa_offline_infer_vad_spk: spk is NULL");
   if (asr && !static_cast<Model*>(asr)->sv && (language_ids || textnorm_ids)) return fail("fa_offline_infer_vad_spk: language / text-norm ids need a SenseVoice model file");
-  return infer_vad(asr, vad, bufs, n_samples, batch, pcm_format, hw_embed, n_hotwords, language_ids, textnorm_ids, opts, static_cast<Spk*>(spk),
+  FaAudioFormat f;
+  if (!pcm16k_format(pcm_format, f)) return fail("bad argument");
+  return infer_vad(asr, vad, bufs, n_samples, batch, &f, hw_embed, n_hotwords, language_ids, textnorm_ids, opts, static_cast<Spk*>(spk),
+                   preset_spk_num);
+}
+
+extern "C" void* fa_offline_infer_vad_audio(void* asr, void* vad, void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch,
+                                            const FaAudioFormat* fmt, const float* hw_embed, int32_t n_hotwords, const int32_t* language_ids,
+                                            const int32_t* textnorm_ids, const FaLongAudioOptions* opts, int32_t preset_spk_num) {
+  g_err.clear();
+  if (asr && !static_cast<Model*>(asr)->sv && (language_ids || textnorm_ids))
+    return fail("fa_offline_infer_vad_audio: language / text-norm ids need a SenseVoice model file");
+  return infer_vad(asr, vad, bufs, n_samples, batch, fmt, hw_embed, n_hotwords, language_ids, textnorm_ids, opts, static_cast<Spk*>(spk),
                    preset_spk_num);
 }
 

@@ -354,18 +354,25 @@ extern "C" void* fa_spk_init(const char* model_file, int32_t device, int32_t gem
 
 extern "C" void fa_spk_uninit(void* spk) { delete static_cast<Spk*>(spk); }
 
-extern "C" int fa_spk_embed(void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format, float* emb_host) {
-  g_err.clear();
+namespace {
+
+// fa_spk_embed / fa_spk_embed_audio: every input checked at 16 kHz before any launch, then one padded 16 kHz batch
+int spk_embed(void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch, const FaAudioFormat* fmt, float* emb_host) {
   Spk* s = static_cast<Spk*>(spk);
-  if (!s || !bufs || !n_samples || batch <= 0 || (pcm_format != 0 && pcm_format != 1) || !emb_host) { set_err("fa_spk_embed: bad argument"); return FA_ERR_ARG; }
+  if (!s || !bufs || !n_samples || batch <= 0 || !emb_host) { set_err("fa_spk_embed: bad argument"); return FA_ERR_ARG; }
+  Audio au;
+  if (!plan_audio(fmt, s->resample, au)) return FA_ERR_ARG;
   int64_t nmax = 0;
   int longest = 0;
+  std::vector<int32_t> lens_h(batch);
   for (int32_t i = 0; i < batch; ++i) {              // every input checked before any launch
-    if (!bufs[i] || n_samples[i] < 400 || n_samples[i] > 0x7fffffffLL) {
-      set_err("input " + std::to_string(i) + " has " + std::to_string(n_samples[i]) + " samples; CAM++ needs at least 400 (one 25 ms frame)");
+    const int64_t n16 = n_samples[i] >= 0 && n_samples[i] <= 0x7fffffffLL ? au.len16(n_samples[i]) : n_samples[i];
+    if (!bufs[i] || n16 < 400 || n16 > 0x7fffffffLL) {
+      set_err("input " + std::to_string(i) + " has " + std::to_string(n16) + " samples" + au.at16k() + "; CAM++ needs at least 400 (one 25 ms frame)");
       return FA_ERR_ARG;
     }
-    if (n_samples[i] > nmax) { nmax = n_samples[i]; longest = i; }
+    lens_h[i] = (int32_t)n16;
+    if (n16 > nmax) { nmax = n16; longest = i; }
   }
   const int t_max = fbank_frames(nmax);
   if (t_max > kSpkMaxFrames) {
@@ -376,19 +383,31 @@ extern "C" int fa_spk_embed(void* spk, const void* const* bufs, const int64_t* n
   cudaSetDevice(s->file.device);
   cudaStream_t st = s->file.st;
   const int64_t stride = (nmax + 3) / 4 * 4;
-  std::vector<int32_t> lens_h(batch);
-  for (int32_t i = 0; i < batch; ++i) lens_h[i] = (int32_t)n_samples[i];
   const bool ok = no_throw("fa_spk_embed: ", [&] {
     int32_t* lens;
     float *emb, *wav;
     if (!carve(s->embed, "CAM++", [&](fa::Arena& a) { lens = a.take<int32_t>(batch); emb = a.take<float>((size_t)batch * kSpkEmbDim); })) return false;
-    if (!upload(bufs, n_samples, batch, stride, pcm_format, s->upload, st, &wav)) return false;
+    if (!upload(bufs, n_samples, batch, stride, au, s->resample, s->upload, st, &wav)) return false;
     cudaMemcpyAsync(lens, lens_h.data(), (size_t)batch * 4, cudaMemcpyHostToDevice, st);
     if (!spk_embed_rows(*s, wav, stride, lens, batch, t_max, emb)) return false;
     cudaMemcpyAsync(emb_host, emb, (size_t)batch * kSpkEmbDim * 4, cudaMemcpyDeviceToHost, st);
     return sync_stream(st);
   });
   return ok ? FA_OK : FA_ERR_CUDA;
+}
+
+}  // namespace
+
+extern "C" int fa_spk_embed(void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format, float* emb_host) {
+  g_err.clear();
+  FaAudioFormat f;
+  if (!pcm16k_format(pcm_format, f)) { set_err("fa_spk_embed: bad argument"); return FA_ERR_ARG; }
+  return spk_embed(spk, bufs, n_samples, batch, &f, emb_host);
+}
+
+extern "C" int fa_spk_embed_audio(void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch, const FaAudioFormat* fmt, float* emb_host) {
+  g_err.clear();
+  return spk_embed(spk, bufs, n_samples, batch, fmt, emb_host);
 }
 
 extern "C" int fa_spk_cluster(void* spk, const float* emb_host, int32_t n, int32_t preset_spk_num, int32_t* labels) {

@@ -136,19 +136,40 @@ extern "C" void* fa_vad_init(const char* model_file, int32_t device) {
 
 extern "C" void fa_vad_uninit(void* vad) { delete static_cast<Vad*>(vad); }
 
-extern "C" void* fa_vad_infer(void* vad, const void* buf, int64_t n_samples, int32_t pcm_format, const FaVadRunOptions* opts) {
-  g_err.clear();
+namespace {
+
+// fa_vad_infer / fa_vad_infer_audio: one host recording -> 16 kHz on the device -> vad_run
+void* vad_infer(void* vad, const void* buf, int64_t n_samples, const FaAudioFormat* fmt, const FaVadRunOptions* opts) {
   Vad* v = static_cast<Vad*>(vad);
-  if (!v || (!buf && n_samples > 0) || n_samples < 0 || n_samples > 0x7fffffffLL || (pcm_format != 0 && pcm_format != 1)) return fail("bad argument");
+  if (!v || (!buf && n_samples > 0) || n_samples < 0 || n_samples > 0x7fffffffLL) return fail("bad argument");
+  Audio au;
+  if (!plan_audio(fmt, v->resample, au)) return nullptr;
+  const int64_t n16 = au.len16(n_samples);
+  if (n16 > 0x7fffffffLL) return fail("bad argument");
   cudaSetDevice(v->file.device);
   std::unique_ptr<VadResult> r(new VadResult());
   float* wav = nullptr;
   if (!no_throw("fa_vad_infer: ", [&] {
-        return upload(&buf, &n_samples, 1, (n_samples + 3) / 4 * 4, pcm_format, v->upload, v->file.st, &wav) &&
-               vad_run(*v, wav, n_samples, v->file.st, opts ? *opts : default_vad_run(), *r);
+        return upload(&buf, &n_samples, 1, (n16 + 3) / 4 * 4, au, v->resample, v->upload, v->file.st, &wav) &&
+               vad_run(*v, wav, n16, v->file.st, opts ? *opts : default_vad_run(), *r);
       }))
     return nullptr;
+  r->audio_seconds = (float)au.seconds(&n_samples, 1);
   return r.release();
+}
+
+}  // namespace
+
+extern "C" void* fa_vad_infer(void* vad, const void* buf, int64_t n_samples, int32_t pcm_format, const FaVadRunOptions* opts) {
+  g_err.clear();
+  FaAudioFormat f;
+  if (!pcm16k_format(pcm_format, f)) return fail("bad argument");
+  return vad_infer(vad, buf, n_samples, &f, opts);
+}
+
+extern "C" void* fa_vad_infer_audio(void* vad, const void* buf, int64_t n_samples, const FaAudioFormat* fmt, const FaVadRunOptions* opts) {
+  g_err.clear();
+  return vad_infer(vad, buf, n_samples, fmt, opts);
 }
 
 extern "C" const int32_t* fa_vad_result_segments(const void* result, int64_t* n_segments) {

@@ -2,8 +2,12 @@
 // their exact C++ signatures, over this library's handle API (offline_asr.cu / offline_long.cu: fa_offline_*).  Host-only C++: file / buffer decoding
 // (raw s16le PCM, RIFF WAV PCM16 / float32), the hotword encoder of ContextualParaformer (Embedding + 1-layer LSTM, O(#hotwords):
 // the reference runs it on the CPU too — model_eb.onnx, runtime/onnxruntime/src/paraformer.cpp CompileHotwordEmbedding) and the
-// ids -> text join.  Everything per audio frame runs in fa_offline_infer_hw on the GPU — or, with a VAD model ("vad-dir"), in
-// fa_offline_infer_vad.  FsmnVad* are the runtime's VAD entry points over fa_vad_infer.
+// ids -> text join.  Everything per audio frame runs in fa_offline_infer_audio on the GPU — or, with a VAD model ("vad-dir"), in
+// fa_offline_infer_vad_audio.  FsmnVad* are the runtime's VAD entry points over fa_vad_infer_audio.
+//
+// Sample rates: audio at any rate (sampling_rate for "pcm", the header's for a WAV file or "wav" buffer) is resampled to 16 kHz on
+// the device with FA_RESAMPLE_RUNTIME, the runtime's LinearResample.  One known difference: the runtime sends "wav" BUFFERS through
+// ffmpeg (swresample) when it is built with it; the shim uses LinearResample for them as for everything else.
 //
 // SeACo (paraformer-zh): CompileHotwordEmbedding parses the hotword string as for ContextualParaformer and takes the rows from the
 // handle's GPU hotword encoder (fa_offline_hotword_embed); FunOfflineInferBuffer passes them on, with or without "vad-dir".
@@ -285,11 +289,13 @@ FaLongAudioOptions runtime_long_audio_options(const OfflineStream& s) {
 
 // a SenseVoice handle: the query from svs_lang / svs_itn, each segment's CTCSearch text concatenated in time order without a separator
 // (funasrruntime.cpp:287-296 for a language other than en-bpe); punctuation, ITN and stamps do not apply (offline-stream.cpp:147-150)
-FUNASR_RESULT infer_sv(OfflineStream* s, const void* const* bufs, const int64_t* lens, int fmt, const std::string& svs_lang, bool svs_itn) {
+FUNASR_RESULT infer_sv(OfflineStream* s, const void* const* bufs, const int64_t* lens, const FaAudioFormat& fmt, const std::string& svs_lang,
+                       bool svs_itn) {
   auto it = kSvLidMap.find(svs_lang);
   const int32_t lid = it != kSvLidMap.end() ? it->second : 0, itn = svs_itn ? 14 : 15;
   const FaLongAudioOptions o = runtime_long_audio_options(*s);
-  void* r = s->vad ? fa_offline_infer_vad_sv(s->h, s->vad, bufs, lens, 1, fmt, &lid, &itn, &o) : fa_offline_infer_sv(s->h, bufs, lens, 1, fmt, &lid, &itn);
+  void* r = s->vad ? fa_offline_infer_vad_audio(s->h, s->vad, nullptr, bufs, lens, 1, &fmt, nullptr, 0, &lid, &itn, &o, 0)
+                   : fa_offline_infer_audio(s->h, bufs, lens, 1, &fmt, nullptr, 0, &lid, &itn);
   if (!r) { g_shim_err = fa_offline_last_error(); return nullptr; }
   int32_t k = 0, nseg = 0;
   const int32_t* ids = fa_offline_result_ids(r, 0, &k);
@@ -338,9 +344,14 @@ bool parse_wav(const std::string& bytes, const char** data, size_t* n_bytes, int
   return false;
 }
 
-FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, int fmt, const std::vector<std::vector<float>>& hw_emb,
+// The runtime's Audio loaders scale s16 by 1/32768 and resample at the caller's rate with LinearResample (WavResample): the
+// handle's FA_RESAMPLE_RUNTIME.  Scaling by a power of two commutes exactly with the filter's products and sums, so decoding to
+// [-1, 1) before the filter gives the runtime's samples.
+FaAudioFormat runtime_format(int fmt, int rate) { return FaAudioFormat{fmt, 1, rate, FA_RESAMPLE_RUNTIME}; }
+
+FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, const FaAudioFormat& fmt, const std::vector<std::vector<float>>& hw_emb,
                         const std::string& svs_lang, bool svs_itn) {
-  const int64_t n = (int64_t)(n_bytes / (fmt == 1 ? 2 : 4));
+  const int64_t n = (int64_t)(n_bytes / (fmt.sample_format == 1 ? 2 : 4));
   const void* bufs[1] = {data};
   const int64_t lens[1] = {n};
   if (fa_offline_is_sensevoice(s->h)) return infer_sv(s, bufs, lens, fmt, svs_lang, svs_itn);
@@ -352,7 +363,7 @@ FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, int 
   }
   if (s->vad) {                        // segment texts concatenated in time order (funasrruntime.cpp:287-296)
     const FaLongAudioOptions o = runtime_long_audio_options(*s);
-    void* r = fa_offline_infer_vad(s->h, s->vad, bufs, lens, 1, fmt, n_hw ? hw.data() : nullptr, n_hw, &o);
+    void* r = fa_offline_infer_vad_audio(s->h, s->vad, nullptr, bufs, lens, 1, &fmt, n_hw ? hw.data() : nullptr, n_hw, nullptr, nullptr, &o, 0);
     if (!r) { g_shim_err = fa_offline_last_error(); return nullptr; }
     int32_t k = 0, nseg = 0;
     const int32_t* ids = fa_offline_result_ids(r, 0, &k);
@@ -371,7 +382,7 @@ FUNASR_RESULT infer_pcm(OfflineStream* s, const char* data, size_t n_bytes, int 
     fa_offline_free_result(r);
     return out;
   }
-  void* r = fa_offline_infer_hw(s->h, bufs, lens, 1, fmt, n_hw ? hw.data() : nullptr, n_hw);
+  void* r = fa_offline_infer_audio(s->h, bufs, lens, 1, &fmt, n_hw ? hw.data() : nullptr, n_hw, nullptr, nullptr);
   if (!r) { g_shim_err = fa_offline_last_error(); return nullptr; }
   ShimResult* out = new ShimResult();
   const int cnt = fa_offline_result_count(r);
@@ -475,8 +486,7 @@ FUNASR_RESULT FunOfflineInferBuffer(FUNASR_HANDLE handle, const char* sz_buf, in
     holder.assign(sz_buf, (size_t)n_len);
     if (!parse_wav(holder, &data, &nb, &fmt, &rate)) { g_shim_err = "unsupported WAV (need mono PCM16 or float32)"; return nullptr; }
   } else if (wav_format != "pcm") { g_shim_err = "wav_format must be \"pcm\" (s16le) or \"wav\""; return nullptr; }
-  if (rate != 16000) { g_shim_err = "audio must be 16 kHz"; return nullptr; }
-  FUNASR_RESULT r = infer_pcm(s, data, nb, fmt, hw_emb, svs_lang, svs_itn);
+  FUNASR_RESULT r = infer_pcm(s, data, nb, runtime_format(fmt, rate), hw_emb, svs_lang, svs_itn);
   if (fn_callback) fn_callback(1, 1);
   return r;
 }
@@ -582,9 +592,9 @@ FUNASR_RESULT FsmnVadInferBuffer(FUNASR_HANDLE handle, const char* sz_buf, int n
     holder.assign(sz_buf, (size_t)n_len);
     if (!parse_wav(holder, &data, &nb, &fmt, &rate)) { g_shim_err = "unsupported WAV (need mono PCM16 or float32)"; return nullptr; }
   } else if (wav_format != "pcm" && wav_format != "PCM") { g_shim_err = "wav_format must be \"pcm\" (s16le) or \"wav\""; return nullptr; }
-  if (rate != 16000) { g_shim_err = "audio must be 16 kHz"; return nullptr; }
   const FaVadRunOptions o = runtime_vad_options();
-  void* r = fa_vad_infer(s->v, data, (int64_t)(nb / (fmt == 1 ? 2 : 4)), fmt, &o);
+  const FaAudioFormat f = runtime_format(fmt, rate);
+  void* r = fa_vad_infer_audio(s->v, data, (int64_t)(nb / (fmt == 1 ? 2 : 4)), &f, &o);
   if (!r) { g_shim_err = fa_offline_last_error(); return nullptr; }
   VadShimResult* out = new VadShimResult();
   int64_t n = 0;

@@ -17,16 +17,30 @@ import numpy as np
 from . import _abi
 
 
-def _pcm_batch(wavs):
+_SAMPLE_FORMATS = {np.dtype(np.float32): 0, np.dtype(np.int16): 1, np.dtype(np.int32): 3, np.dtype(np.uint8): 4}
+
+
+def _pcm_batch(wavs, fs: int = 16000, resampler: str = "loader"):
+    """-> (contiguous arrays, pcm_format, FaAudioFormat or None).  None: 16 kHz mono float32 / int16, which the 16 kHz entries take;
+    otherwise the descriptor of the `_audio` entries.  Arrays are 1-D (mono) or 2-D [frames, channels] of one dtype: float32 in
+    [-1, 1], int16, int32 or uint8 PCM (s24 only through the C API)."""
     arrs = [np.ascontiguousarray(w) for w in wavs]
     kinds = {a.dtype for a in arrs}
-    if kinds == {np.dtype(np.float32)}:
-        fmt = 0
-    elif kinds == {np.dtype(np.int16)}:
-        fmt = 1
-    else:
-        raise _abi.FunasrB200Error("waveforms must all be float32 or all be int16, got %s" % kinds)
-    return arrs, fmt
+    if len(kinds) != 1 or next(iter(kinds)) not in _SAMPLE_FORMATS:
+        raise _abi.FunasrB200Error("waveforms must all be float32, all int16, all int32 or all uint8, got %s" % kinds)
+    if any(a.ndim not in (1, 2) for a in arrs) or len({1 if a.ndim == 1 else a.shape[1] for a in arrs}) != 1:
+        raise _abi.FunasrB200Error("waveforms must be 1-D or [frames, channels] with the same channel count")
+    if resampler not in _abi.RESAMPLERS:
+        raise _abi.FunasrB200Error("resampler must be one of %s, got %r" % (sorted(_abi.RESAMPLERS), resampler))
+    fmt = _SAMPLE_FORMATS[kinds.pop()]
+    channels = 1 if arrs[0].ndim == 1 else arrs[0].shape[1]
+    if int(fs) == 16000 and fmt in (0, 1) and all(a.ndim == 1 for a in arrs):
+        return arrs, fmt, None
+    return arrs, fmt, _abi.FaAudioFormat(fmt, channels, int(fs), _abi.RESAMPLERS[resampler])
+
+
+def _ptr(a: Optional[np.ndarray]):
+    return None if a is None else a.ctypes.data
 
 
 def _vad_run_options(max_end_silence_time: Optional[int] = None, speech_noise_thres: Optional[float] = None,
@@ -47,11 +61,15 @@ class OfflineVad:
         if not self.handle:
             raise _abi.FunasrB200Error("fa_vad_init failed: %s" % self.lib.fa_offline_last_error().decode())
 
-    def segments(self, wav: np.ndarray, want_frames: bool = False, **vad_kwargs):
-        """wav: float32 in [-1, 1] or int16, 16 kHz mono -> [[start_ms, end_ms], ...] (and the [2, frames] silence posterior / energy)."""
-        (a,), fmt = _pcm_batch([wav])
+    def segments(self, wav: np.ndarray, want_frames: bool = False, fs: int = 16000, resampler: str = "loader", **vad_kwargs):
+        """wav: float32 in [-1, 1] or int16 (int32, uint8) PCM, 1-D or [frames, channels], at fs Hz (resampled to 16 kHz on the GPU
+        by `resampler`: "loader" or "runtime") -> [[start_ms, end_ms], ...] (and the [2, frames] silence posterior / energy)."""
+        (a,), fmt, desc = _pcm_batch([wav], fs, resampler)
         opts = _vad_run_options(**vad_kwargs)
-        res = self.lib.fa_vad_infer(self.handle, a.ctypes.data, a.shape[0], fmt, C.byref(opts))
+        if desc is None:
+            res = self.lib.fa_vad_infer(self.handle, a.ctypes.data, a.shape[0], fmt, C.byref(opts))
+        else:
+            res = self.lib.fa_vad_infer_audio(self.handle, a.ctypes.data, a.shape[0], C.byref(desc), C.byref(opts))
         if not res:
             raise _abi.FunasrB200Error("fa_vad_infer failed: %s" % self.lib.fa_offline_last_error().decode())
         try:
@@ -187,14 +205,17 @@ class OfflineSpeaker:
         if not self.handle:
             raise _abi.FunasrB200Error("fa_spk_init failed: %s" % self.lib.fa_offline_last_error().decode())
 
-    def embed(self, wavs: Sequence[np.ndarray]) -> np.ndarray:
-        """Ragged recordings (float32 in [-1, 1] or int16, 16 kHz) -> [B, 192] float32, CAMPPlusB200.inference's embeddings."""
-        arrs, fmt = _pcm_batch(wavs)
+    def embed(self, wavs: Sequence[np.ndarray], fs: int = 16000, resampler: str = "loader") -> np.ndarray:
+        """Ragged recordings (float32 in [-1, 1] or int16 (int32, uint8) PCM, 1-D or [frames, channels], at fs Hz; `resampler` as in
+        OfflineVad.segments) -> [B, 192] float32, CAMPPlusB200.inference's embeddings."""
+        arrs, fmt, desc = _pcm_batch(wavs, fs, resampler)
         n = len(arrs)
         ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
         lens = (C.c_int64 * n)(*[a.shape[0] for a in arrs])
         out = np.empty((n, 192), dtype=np.float32)
-        if self.lib.fa_spk_embed(self.handle, ptrs, lens, n, fmt, out.ctypes.data) != 0:
+        rc = (self.lib.fa_spk_embed(self.handle, ptrs, lens, n, fmt, out.ctypes.data) if desc is None else
+              self.lib.fa_spk_embed_audio(self.handle, ptrs, lens, n, C.byref(desc), out.ctypes.data))
+        if rc != 0:
             raise _abi.FunasrB200Error("fa_spk_embed failed: %s" % self.lib.fa_offline_last_error().decode())
         return out
 
@@ -256,13 +277,17 @@ class OfflineRecognizer:
         p = self.lib.fa_offline_result_stamps(res, i, C.byref(cnt))
         return [[int(p[2 * k]), int(p[2 * k + 1])] for k in range(cnt.value)]
 
-    def _infer(self, wavs, stamped: bool, language=None, use_itn=None, hotword_embeddings=None):
-        arrs, fmt = _pcm_batch(wavs)
+    def _infer(self, wavs, stamped: bool, language=None, use_itn=None, hotword_embeddings=None, fs: int = 16000, resampler: str = "loader"):
+        arrs, fmt, desc = _pcm_batch(wavs, fs, resampler)
         n = len(arrs)
         ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
         lens = (C.c_int64 * n)(*[a.shape[0] for a in arrs])
         q = self._queries(n, language, use_itn)
-        if hotword_embeddings is not None:
+        if desc is not None:
+            hw = None if hotword_embeddings is None else np.ascontiguousarray(hotword_embeddings, dtype=np.float32)
+            res = self.lib.fa_offline_infer_audio(self.handle, ptrs, lens, n, C.byref(desc), _ptr(hw), 0 if hw is None else hw.shape[0],
+                                                  None if q is None else q[0].ctypes.data, None if q is None else q[1].ctypes.data)
+        elif hotword_embeddings is not None:
             hw = np.ascontiguousarray(hotword_embeddings, dtype=np.float32)
             res = self.lib.fa_offline_infer_hw(self.handle, ptrs, lens, n, fmt, hw.ctypes.data, hw.shape[0])
         elif q is None:
@@ -283,30 +308,35 @@ class OfflineRecognizer:
         finally:
             self.lib.fa_offline_free_result(res)
 
-    def infer(self, wavs: Sequence[np.ndarray], language=None, use_itn=None, hotword_embeddings: Optional[np.ndarray] = None) -> List[List[int]]:
-        """wavs: float32 arrays in [-1, 1] or int16 PCM arrays (all the same dtype), 16 kHz mono, >= 400 samples each.
+    def infer(self, wavs: Sequence[np.ndarray], language=None, use_itn=None, hotword_embeddings: Optional[np.ndarray] = None,
+              fs: int = 16000, resampler: str = "loader") -> List[List[int]]:
+        """wavs: float32 arrays in [-1, 1] or int16 PCM arrays (all the same dtype; int32 and uint8 PCM too), 1-D or [frames, channels],
+        at fs Hz, >= 400 samples each at 16 kHz.  Other rates and layouts are averaged to mono and resampled to 16 kHz on the GPU:
+        resampler "loader" as FunASR's Python loader and inference(fs=) (torchaudio's sinc), "runtime" as the C++ runtime (LinearResample).
         SenseVoice model file: language (one name or one per utterance, default "auto") and use_itn (default False) choose each
         utterance's query; the ids include the four tag tokens (SenseVoiceSmall.inference's token_int).  hotword_embeddings: [n, 512]
         float32 rows, the last one the <s> entry (ContextualParaformer's encoder, or `hotword_embeddings()` of a SeACo model file)."""
-        return self._infer(wavs, False, language, use_itn, hotword_embeddings)
+        return self._infer(wavs, False, language, use_itn, hotword_embeddings, fs, resampler)
 
-    def infer_stamped(self, wavs: Sequence[np.ndarray], hotword_embeddings: Optional[np.ndarray] = None) -> List[dict]:
+    def infer_stamped(self, wavs: Sequence[np.ndarray], hotword_embeddings: Optional[np.ndarray] = None, fs: int = 16000,
+                      resampler: str = "loader") -> List[dict]:
         """Like `infer`, per utterance {"token_int": ids, "timestamp": [[start_ms, end_ms], ...]} (BiCifParaformer.inference's result;
         no stamps for a model without the timestamp head)."""
-        return self._infer(wavs, True, hotword_embeddings=hotword_embeddings)
+        return self._infer(wavs, True, hotword_embeddings=hotword_embeddings, fs=fs, resampler=resampler)
 
     def infer_long(self, wavs: Sequence[np.ndarray], vad: OfflineVad, batch_size_s: int = 300, batch_size_threshold_s: int = 60,
                    merge_vad: bool = False, merge_length_s: int = 15, hotword_embeddings: Optional[np.ndarray] = None,
                    language=None, use_itn=None, spk: Optional["OfflineSpeaker"] = None, preset_spk_num: Optional[int] = None,
-                   **vad_kwargs) -> List[dict]:
+                   fs: int = 16000, resampler: str = "loader", **vad_kwargs) -> List[dict]:
         """Long recordings through fa_offline_infer_vad, each on its own as LongAudioPipeline.generate treats it -> per recording
         {"token_int": ids in time order, "vad_segments": [[start_ms, end_ms], ...], "n_tokens": tokens per segment}, plus
         "timestamp": [[start_ms, end_ms], ...] in absolute ms when the model has the timestamp head (`has_timestamps`).
         hotword_embeddings: [n, 512] float32 rows (ContextualParaformer or SeACo; last row the <s> entry).  SenseVoice model file
         (fa_offline_infer_vad_sv): language / use_itn as in `infer`, one per recording, applied to all its segments.
         spk (an OfflineSpeaker on the same device): fa_offline_infer_vad_spk also diarizes every recording that decoded a token and adds
-        "spk", one speaker per VAD segment (vad_segment mode), with preset_spk_num as LongAudioPipeline.generate takes it."""
-        arrs, fmt = _pcm_batch(wavs)
+        "spk", one speaker per VAD segment (vad_segment mode), with preset_spk_num as LongAudioPipeline.generate takes it.
+        fs / resampler and the array layouts as in `infer` (fa_offline_infer_vad_audio); segments and stamps are ms of the recording."""
+        arrs, fmt, desc = _pcm_batch(wavs, fs, resampler)
         n = len(arrs)
         ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
         lens = (C.c_int64 * n)(*[a.shape[0] for a in arrs])
@@ -317,7 +347,11 @@ class OfflineRecognizer:
             hw = np.ascontiguousarray(hotword_embeddings, dtype=np.float32)
             n_hw = hw.shape[0]
         q = self._queries(n, language, use_itn)
-        if spk is not None:
+        if desc is not None:
+            res = self.lib.fa_offline_infer_vad_audio(self.handle, vad.handle, None if spk is None else spk.handle, ptrs, lens, n, C.byref(desc),
+                                                      _ptr(hw), n_hw, None if q is None else q[0].ctypes.data,
+                                                      None if q is None else q[1].ctypes.data, C.byref(opts), int(preset_spk_num or 0))
+        elif spk is not None:
             res = self.lib.fa_offline_infer_vad_spk(self.handle, vad.handle, spk.handle, ptrs, lens, n, fmt, None if hw is None else hw.ctypes.data,
                                                     n_hw, None if q is None else q[0].ctypes.data, None if q is None else q[1].ctypes.data,
                                                     C.byref(opts), int(preset_spk_num or 0))

@@ -536,6 +536,55 @@ int fa_embedding(const int32_t* ids, const float* table, int32_t dim, int32_t vo
  * 3 = s32le, 4 = u8.  The container (RIFF WAV header) is parsed on the host (funasr_b200/audio.py). */
 int fa_pcm_decode(const void* pcm, int32_t sample_format, int32_t channels, int64_t frames, float* out, fa_stream_t stream);
 
+/* ---- Audio at any sample rate and PCM layout: the input descriptor of fa_offline_infer_audio, fa_offline_infer_vad_audio,
+ * fa_vad_infer_audio and fa_spk_embed_audio.  Two resamplers to 16 kHz, each pinned to its own reference:
+ *   FA_RESAMPLE_LOADER   torchaudio's sinc resampler (hann window, 6 zeros, rolloff 0.99) as FunASR's Python loader and
+ *                        inference(fs=) apply it: the table of fa_loader_resample_table_host and fa_resample's arithmetic.
+ *   FA_RESAMPLE_RUNTIME  the C++ runtime's kaldi LinearResample (cutoff 0.99 * 0.5 * min rate, 6 zeros, flushed) as its WavResample
+ *                        applies it: the tables of fa_runtime_resample_table_host, sums in tap order without contraction.
+ * At 16 000 Hz neither resamples (both references skip it).  Both give ceil(16000 n / rate) samples for n frames. */
+#define FA_RESAMPLE_LOADER 0
+#define FA_RESAMPLE_RUNTIME 1
+typedef struct FaAudioFormat {
+  int32_t sample_format;  /* fa_pcm_decode's codes: 0 f32, 1 s16le, 2 s24le packed, 3 s32le, 4 u8 */
+  int32_t channels;       /* 1..64, interleaved; averaged to mono like the loader */
+  int32_t sample_rate;    /* Hz of the caller's buffers, 1 000..192 000 */
+  int32_t resampler;      /* FA_RESAMPLE_LOADER or FA_RESAMPLE_RUNTIME */
+} FaAudioFormat;
+/* Host only.  Rates outside 1 000..192 000 Hz -> FA_ERR_ARG; a table above 32 MiB (for example 16 001 Hz in loader mode, 1 GB) ->
+ * FA_ERR_UNSUPPORTED.  Otherwise the number of floats of the weight table, written when weights is not NULL and cap holds it.
+ * fa_loader_resample_table_host: resample.sinc_resample_table(rate, new_rate) bit for bit: *orig / *nnew the rates over their gcd,
+ *   *width, table [nnew, 2 * width + orig].
+ * fa_runtime_resample_table_host: LinearResample(rate, new_rate, 0.99 * 0.5 * min rate, 6)'s weights: *in_unit / *out_unit the
+ *   rates over their gcd, per output phase p < out_unit the first input index first[p] (may be negative) and n_taps[p] weights in
+ *   row p of weights [out_unit, *max_taps] (zero padded).  first / n_taps are written with the weights.
+ * fa_runtime_resample_out_len_host: LinearResample's flushed output count for n input frames (64-bit tick arithmetic). */
+int64_t fa_loader_resample_table_host(int32_t rate, int32_t new_rate, int32_t* orig, int32_t* nnew, int32_t* width, float* table, int64_t cap);
+int64_t fa_runtime_resample_table_host(int32_t rate, int32_t new_rate, int32_t* in_unit, int32_t* out_unit, int32_t* max_taps,
+                                       int32_t* first, int32_t* n_taps, float* weights, int64_t cap);
+int64_t fa_runtime_resample_out_len_host(int32_t rate, int32_t new_rate, int64_t n);
+/* One uploaded resampling table (device pointers).  mode: FA_RESAMPLE_LOADER (in_unit / out_unit = orig / nnew, width, taps =
+ * 2 * width + orig, weights [out_unit, taps]; first / n_taps NULL, or [out_unit] each row's span of nonzero taps, which is all a sum
+ * over finite samples needs: most of a row lies outside the window, where the table is exactly zero), FA_RESAMPLE_RUNTIME (in_unit /
+ * out_unit, taps = the longest row, weights [out_unit, taps], first / n_taps [out_unit]); or -1: decode only (16 kHz input), every
+ * other field ignored. */
+typedef struct FaIngestTable {
+  int32_t mode;
+  int32_t in_unit, out_unit, width, taps;
+  int32_t _pad;
+  const float* weights;
+  const int32_t* first;
+  const int32_t* n_taps;
+} FaIngestTable;
+/* The handle's ingest, one launch: ragged interleaved PCM rows in device memory -> y [batch, stride] mono fp32 at 16 kHz.  rows
+ * [batch][3] int64 on the device: byte offset of the row in raw (a multiple of the sample size), frames n, output length (<= stride).
+ * Each output decodes the frames it needs straight from the bytes (fa_pcm_decode's operations and channel mean) and applies the
+ * table: loader mode bit for bit fa_pcm_decode then fa_resample (with spans: for finite samples, which every integer format is); runtime mode out[t] = sum over taps j of w[p][j] * x[first[p] +
+ * u * in_unit + j] (u = t / out_unit, p = t % out_unit), indices outside [0, n) skipped, each product and add rounded on its own.
+ * Zero past each row's output length. */
+int fa_ingest_pcm(const void* raw, const int64_t* rows, int32_t batch, int32_t sample_format, int32_t channels, const FaIngestTable* table,
+                  float* y, int64_t stride, fa_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------
  * CAM++ speaker embedding (funasr/models/campplus/model.py CAMPPlus, feat 80, embedding 192, growth 32, bn 128, init 128,
  * batchnorm-relu).  Eval-mode BatchNorm that follows a conv is folded into that conv's weights and bias by the caller; BatchNorm
@@ -791,6 +840,25 @@ void* fa_offline_infer_vad_spk(void* asr, void* vad, void* spk, const void* cons
 /* n speakers of recording `index`, one per segment in fa_offline_result_segments' order (labels in order of first appearance); NULL
  * with 0 for a recording that was not diarized and for results of the other entry points. */
 const int32_t* fa_offline_result_spk(const void* result, int32_t index, int32_t* n);
+
+/* ---- The handle entries for audio at any sample rate and PCM layout (FaAudioFormat).  Each is its 16 kHz counterpart with the
+ * input turned into 16 kHz mono fp32 rows on the device first (fa_ingest_pcm, one launch per upload; 16 kHz mono f32 / s16 take the
+ * old path and launch exactly what the old entries launch).  n_samples[i] counts frames (samples per channel).  Before any launch:
+ * the descriptor is checked (NULL, sample_format, channels 1..64, rate 1 000..192 000, resampler, a table above 32 MiB), every 16 kHz
+ * length is computed (ceil(16000 n / rate)) and the old entries' checks apply to it (400 samples, CAM++'s 18 800 frames).
+ * audio_seconds counts the caller's frames at the caller's rate; segments and stamps are in ms of the same timeline.  An old entry
+ * is the new one with {pcm_format, 1, 16000, either resampler}.
+ *   fa_offline_infer_audio      fa_offline_infer_hw / fa_offline_infer_sv (language_ids / textnorm_ids: SenseVoice only, NULL = the defaults)
+ *   fa_offline_infer_vad_audio  fa_offline_infer_vad / _sv / _spk (spk NULL: no diarization)
+ *   fa_vad_infer_audio          fa_vad_infer
+ *   fa_spk_embed_audio          fa_spk_embed */
+void* fa_offline_infer_audio(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, const FaAudioFormat* fmt,
+                             const float* hw_embed, int32_t n_hotwords, const int32_t* language_ids, const int32_t* textnorm_ids);
+void* fa_offline_infer_vad_audio(void* asr, void* vad, void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch,
+                                 const FaAudioFormat* fmt, const float* hw_embed, int32_t n_hotwords, const int32_t* language_ids,
+                                 const int32_t* textnorm_ids, const FaLongAudioOptions* opts, int32_t preset_spk_num);
+void* fa_vad_infer_audio(void* vad, const void* buf, int64_t n_samples, const FaAudioFormat* fmt, const FaVadRunOptions* opts);
+int fa_spk_embed_audio(void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch, const FaAudioFormat* fmt, float* emb_host);
 /* p-pruning's effective pval for n rows (SpectralCluster.p_pruning): 6 / n when n * pval < 6, else pval (float64). */
 double fa_spk_effective_pval(int32_t n, double pval);
 /* SpectralCluster.sim_mat -> p_pruning -> 0.5 (P + P^T) -> laplacian over device embeddings emb [n, dim] fp32 (1 <= n <= 2047,

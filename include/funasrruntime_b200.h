@@ -5,8 +5,13 @@
  *   model_path["model-dir"] names a directory holding `model.fab2` (funasr_b200/pack.py, written from an unmodified model.pt +
  *   am.mvn) and optionally `tokens.txt` (one token per line; without it results carry the token ids in decimal);
  *   optional keys "gemm-mode" (fp32 | fp16 | fp16x3 | fp16x6, default fp16x3) and "gpu-id" (default 0);
- *   there is no CPU path (use_gpu is ignored); audio must be 16 kHz; the WFST / LM decoder entry points are accepted and ignored
- *   (greedy decoding, like the reference without --lm-dir).
+ *   there is no CPU path (use_gpu is ignored); the WFST / LM decoder entry points are accepted and ignored (greedy decoding, like
+ *   the reference without --lm-dir).
+ *   Audio at any sampling_rate from 1 000 to 192 000 Hz ("pcm" s16le mono; a WAV file or "wav" buffer at its header's rate, mono s16
+ *   or float32) is resampled to 16 kHz on the GPU with the runtime's own LinearResample (FA_RESAMPLE_RUNTIME, as Audio::WavResample
+ *   applies it), in FunOfflineInfer / FunOfflineInferBuffer with or without "vad-dir" and in FsmnVadInfer / FsmnVadInferBuffer.  One
+ *   known difference: the runtime decodes "wav" buffers with ffmpeg (swresample) where it is built with it; here they take
+ *   LinearResample too.
  *   model_path["vad-dir"] (optional) names a directory holding `vad.fab2` (funasr_b200/pack.py: write_vad_model_file, from the FSMN-VAD
  *   model.pt + am.mvn + the model_conf of its config.yaml).  With it FunOfflineInfer / FunOfflineInferBuffer segment the audio first
  *   (fa_offline_infer_vad) with the runtime's semantics: a FIXED end silence (the file's max_end_silence_time, fsmn-vad.cpp), segment
