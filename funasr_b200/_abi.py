@@ -264,6 +264,10 @@ SIGNATURES = {
     "fa_spk_merge_by_cos_host": (C.c_int, [_vp, _vp, _i64, _i32, C.c_double]),
     "fa_spk_postprocess_host": (_i64, [_vp, _vp, _i64, _vp]),
     "fa_spk_distribute_host": (C.c_int, [_vp, _i64, _vp, _i64, _vp]),
+    # handle-style MonotonicAligner forced alignment (offline_align.cu); results through the fa_offline_result_* accessors
+    "fa_align_init": (_vp, [C.c_char_p, _i32, _i32]),
+    "fa_align_infer": (_vp, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, C.POINTER(FaAudioFormat), C.POINTER(_vp), C.POINTER(_i32)]),
+    "fa_align_uninit": (None, [_vp]),
     # handle-style CT-Transformer punctuation (offline_punc.cu; the text walk: punc_text.cpp)
     "fa_punc_init": (_vp, [C.c_char_p, _i32]),
     "fa_punc_infer": (_vp, [_vp, C.POINTER(C.c_char_p), _i32]),

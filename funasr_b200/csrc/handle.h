@@ -8,6 +8,7 @@
 //   offline_spk.cu   CAM++ speaker embeddings, clustering, diarization: fa_spk_*
 //   offline_long.cu  long audio: fa_offline_infer_vad*, fa_offline_result_{segments,spk}
 //   offline_punc.cu  CT-Transformer punctuation: fa_punc_*
+//   offline_align.cu MonotonicAligner (fa-zh) forced alignment: fa_align_*
 #pragma once
 #include "common.cuh"
 #include <algorithm>
@@ -194,12 +195,23 @@ H* open_handle(const char* path, int device, int mode, bool (*build)(H&, Builder
   return ok ? h.release() : nullptr;
 }
 
+// LFR frames of n 16 kHz samples (wav_frontend.py:73 after kaldi.py snip_edges framing)
+inline int num_lfr_frames(int64_t n) {
+  const int64_t mfr = n >= 400 ? 1 + (n - 400) / 160 : 0;
+  return (int)((mfr + 5) / 6);
+}
+
 // SANMEncoder's layer names: encoders0.0 then encoders.{i - 1}; SenseVoice's tp_encoders one plain list
 std::string enc_layer_prefix(bool tp, int i);
 
 // A SAN-M stack of n layers over `in` input features into e and L, in the shapes fa_sanm_encoder_forward takes (the recogniser's
 // encoders and punctuation's)
 void bind_stack(Builder& b, bool tp, int n, int in, int D, int heads, std::vector<FaEncLayer>& L, FaEncoder& e);
+
+// CifPredictorV3's upsampled timestamp head at width D into h: __ts_config__ (upsample_times 3, smooth_factor2, noise_threshold2) and
+// the tensors pack.py:timestamp_head_tensors writes, in their shapes; h.threshold is the caller's.  Every refusal is prefixed by b.what
+// (the BiCif recogniser's and the aligner's).
+void bind_ts_head(Builder& b, int D, FaTimestampHead& h);
 
 // ------------------------------------------------------------------------------------------------ audio in (FaAudioFormat)
 // One (rate, resampler)'s host tables; fa_ingest_pcm reads their device copy

@@ -130,6 +130,22 @@ void bind_stack(Builder& b, bool tp, int n, int in, int D, int heads, std::vecto
   }
 }
 
+void bind_ts_head(Builder& b, int D, FaTimestampHead& h) {
+  const Tensor* tc = b.opt("__ts_config__");
+  if (!tc || tc->host.size() < 3) { b.refuse("missing __ts_config__"); return; }
+  const float* c = tc->host.data();
+  if (c[0] != 3.f) { b.refuse("upsample_times " + std::to_string(c[0]) + " in __ts_config__, only 3 is supported"); return; }
+  b.shaped("predictor.upsample_cnn.gemm_weight", {3 * D, D}); b.shaped("predictor.upsample_cnn.gemm_bias", {3 * D});
+  b.shaped("predictor.blstm.ih_gemm_weight", {8 * D, D});     b.shaped("predictor.blstm.ih_gemm_bias", {8 * D});
+  b.shaped("predictor.blstm.weight_hh_l0", {4 * D, D});       b.shaped("predictor.blstm.weight_hh_l0_reverse", {4 * D, D});
+  b.shaped("predictor.cif_output2.weight", {1, 2 * D});       b.shaped("predictor.cif_output2.bias", {1});
+  h.up_times = 3; h.smooth2 = c[1]; h.noise2 = c[2];
+  h.upsample = b.lin("predictor.upsample_cnn", true, "predictor.upsample_cnn.gemm_weight", "predictor.upsample_cnn.gemm_bias");
+  h.blstm_ih = b.lin("predictor.blstm.ih", true, "predictor.blstm.ih_gemm_weight", "predictor.blstm.ih_gemm_bias");
+  h.w_hh_fwd = b.ptr("predictor.blstm.weight_hh_l0"); h.w_hh_bwd = b.ptr("predictor.blstm.weight_hh_l0_reverse");
+  h.out2_w = b.ptr("predictor.cif_output2.weight"); h.out2_b = b.ptr("predictor.cif_output2.bias");
+}
+
 int64_t Audio::frame_bytes() const {
   static const int kBytes[5] = {4, 2, 3, 4, 1};
   return (int64_t)kBytes[fmt.sample_format] * fmt.channels;

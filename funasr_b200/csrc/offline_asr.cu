@@ -31,19 +31,9 @@ bool build_paraformer(Model& m, Builder& b) {
     if (!tc || tc->host.size() < 3)
       return b.refuse("BiCif timestamp head without __ts_config__ (a file packed before the handle read the head): re-pack it with "
                       "funasr_b200.pack.write_model_file");
-    const float* c = tc->host.data();
-    if (c[0] != 3.f) return b.refuse("BiCif timestamp head: upsample_times " + std::to_string(c[0]) + " in __ts_config__, only 3 is supported");
     b.what = "BiCif timestamp head: ";
-    b.shaped("predictor.upsample_cnn.gemm_weight", {3 * 512, 512}); b.shaped("predictor.upsample_cnn.gemm_bias", {3 * 512});
-    b.shaped("predictor.blstm.ih_gemm_weight", {8 * 512, 512});     b.shaped("predictor.blstm.ih_gemm_bias", {8 * 512});
-    b.shaped("predictor.blstm.weight_hh_l0", {4 * 512, 512});       b.shaped("predictor.blstm.weight_hh_l0_reverse", {4 * 512, 512});
-    b.shaped("predictor.cif_output2.weight", {1, 2 * 512});         b.shaped("predictor.cif_output2.bias", {1});
-    FaTimestampHead& h = m.head;
-    h.up_times = 3; h.smooth2 = c[1]; h.noise2 = c[2];
-    h.upsample = b.lin("predictor.upsample_cnn", true, "predictor.upsample_cnn.gemm_weight", "predictor.upsample_cnn.gemm_bias");
-    h.blstm_ih = b.lin("predictor.blstm.ih", true, "predictor.blstm.ih_gemm_weight", "predictor.blstm.ih_gemm_bias");
-    h.w_hh_fwd = b.ptr("predictor.blstm.weight_hh_l0"); h.w_hh_bwd = b.ptr("predictor.blstm.weight_hh_l0_reverse");
-    h.out2_w = b.ptr("predictor.cif_output2.weight"); h.out2_b = b.ptr("predictor.cif_output2.bias");
+    bind_ts_head(b, 512, m.head);
+    if (!b.ok) return false;
     b.what.clear();
   }
   const Tensor* cfg = b.opt("__config__");
@@ -154,11 +144,6 @@ bool build_paraformer(Model& m, Builder& b) {
     b.what.clear();
   }
   return b.ok;
-}
-
-int num_lfr_frames(int64_t n) {       // wav_frontend.py:73 after kaldi.py snip_edges framing
-  const int64_t mfr = n >= 400 ? 1 + (n - 400) / 160 : 0;
-  return (int)((mfr + 5) / 6);
 }
 
 // SeACo's hotword biasing after the decoder (_seaco_decode_with_ASF, seaco_paraformer/model.py:271-382, as ParaformerEngine.seaco_decode
@@ -454,8 +439,11 @@ void* infer_batch(void* handle, const void* const* bufs, const int64_t* n_sample
   return r.release();
 }
 
-// the model kind is the file's: SenseVoiceSmall by __sv_config__, Paraformer otherwise
-bool build_offline(Model& m, Builder& b) { return b.opt("__sv_config__") ? build_sv(m, b) : build_paraformer(m, b); }
+// the model kind is the file's: SenseVoiceSmall by __sv_config__, Paraformer otherwise; a MonotonicAligner file is fa_align_init's
+bool build_offline(Model& m, Builder& b) {
+  if (b.opt("__aligner_config__")) return b.refuse("a MonotonicAligner file (__aligner_config__): open it with fa_align_init");
+  return b.opt("__sv_config__") ? build_sv(m, b) : build_paraformer(m, b);
+}
 
 const Result* as_result(const void* r) { return static_cast<const Result*>(r); }
 

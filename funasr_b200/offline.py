@@ -6,7 +6,8 @@ batch by batch, the same results as LongAudioPipeline.generate.  A BiCifParaform
 (`infer_stamped`, and "timestamp" in `infer_long`'s results); a SeacoParaformer model file takes hotword rows from
 `hotword_embeddings` (its hotword encoder on the GPU).  `OfflinePunc` binds the CT-Transformer punctuation handle (fa_punc_*),
 and `punc_walk_host` its text walk with any scorer in place of the network.  `OfflineSpeaker` binds the CAM++ speaker handle (fa_spk_*);
-passed to `infer_long(spk=...)` it diarizes long audio (fa_offline_infer_vad_spk)."""
+passed to `infer_long(spk=...)` it diarizes long audio (fa_offline_infer_vad_spk).  `OfflineAligner` binds the MonotonicAligner's
+forced-alignment handle (fa_align_*): per-token stamps for transcripts the caller already has."""
 from __future__ import annotations
 
 import ctypes as C
@@ -222,6 +223,59 @@ class OfflineSpeaker:
     def close(self):
         if getattr(self, "handle", None):
             self.lib.fa_spk_uninit(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class OfflineAligner:
+    """Forced alignment through the C handle (fa_align_init / fa_align_infer): the MonotonicAligner (fa-zh) from a
+    pack.write_aligner_model_file file."""
+
+    def __init__(self, model_file: str, device: int = 0, gemm_mode: str = "fp16x3"):
+        self.lib = _abi.load()
+        mode = _abi.GEMM_MODES[gemm_mode] if isinstance(gemm_mode, str) else int(gemm_mode)
+        self.handle = self.lib.fa_align_init(model_file.encode(), int(device), mode)
+        if not self.handle:
+            raise _abi.FunasrB200Error("fa_align_init failed: %s" % self.lib.fa_offline_last_error().decode())
+
+    def align(self, wavs: Sequence[np.ndarray], token_ids: Sequence[Sequence[int]], fs: int = 16000,
+              resampler: str = "loader") -> List[List[List[int]]]:
+        """wavs (float32 in [-1, 1] or int16 (int32, uint8) PCM, 1-D or [frames, channels], at fs Hz; `resampler` as in
+        OfflineRecognizer.infer) and one transcript of token ids per wav -> per wav [[start_ms, end_ms], ...], MonotonicAligner.inference's
+        "timestamp" for CJK character tokens: one stamp per token (a trailing </s> dropped), fewer when the audio cannot fire for
+        them all."""
+        arrs, fmt, _ = _pcm_batch(wavs, fs, resampler)
+        n = len(arrs)
+        if len(token_ids) != n:
+            raise _abi.FunasrB200Error("one transcript per waveform: %d waveforms, %d transcripts" % (n, len(token_ids)))
+        desc = _abi.FaAudioFormat(fmt, 1 if arrs[0].ndim == 1 else arrs[0].shape[1], int(fs), _abi.RESAMPLERS[resampler])
+        toks = [np.ascontiguousarray(t, dtype=np.int32).reshape(-1) for t in token_ids]
+        ptrs = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
+        lens = (C.c_int64 * n)(*[a.shape[0] for a in arrs])
+        id_ptrs = (C.c_void_p * n)(*[t.ctypes.data if t.size else None for t in toks])
+        n_ids = (C.c_int32 * n)(*[t.size for t in toks])
+        res = self.lib.fa_align_infer(self.handle, ptrs, lens, n, C.byref(desc), id_ptrs, n_ids)
+        if not res:
+            raise _abi.FunasrB200Error("fa_align_infer failed: %s" % self.lib.fa_offline_last_error().decode())
+        try:
+            cnt = C.c_int32(0)
+            out = []
+            for i in range(self.lib.fa_offline_result_count(res)):
+                p = self.lib.fa_offline_result_stamps(res, i, C.byref(cnt))
+                out.append([[int(p[2 * k]), int(p[2 * k + 1])] for k in range(cnt.value)])
+            self.last_audio_seconds = float(self.lib.fa_offline_result_audio_seconds(res))
+            return out
+        finally:
+            self.lib.fa_offline_free_result(res)
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self.lib.fa_align_uninit(self.handle)
             self.handle = None
 
     def __del__(self):

@@ -57,6 +57,15 @@ window frontend.window [400] (torchaudio kaldi.fbank's defaults), and
 
 The handle folds the BatchNorms itself, in float64, the same way CampplusEngine does.
 
+The MonotonicAligner (fa-zh) file (csrc/offline_align.cu: fa_align_init, recognised by __aligner_config__) holds encoder.* under the
+reference's names, the timestamp head as `timestamp_head_tensors` repacks it (at the model's width: 320 for fa-zh), __ts_config__ with
+its BiCif meaning, the frontend tables and encoder.pe_inv_timescales of the Paraformer file, and
+
+    __aligner_config__                 [7] enc_layers, d_model, heads, feat_dim, ln_eps, cif threshold, eos_id (the index of "</s>" in the
+                                           token list, -1 without one)
+
+predictor.cif_conv1d / cif_output are left out: get_upsample_timestamp does not read them.
+
 Layout: b"FAB2MDL1", u32 n_tensors, then per tensor: u32 name_len, name (utf-8), u32 ndim, i64 dims[ndim], u64 nbytes,
 zero padding to a 16-byte file offset, little-endian fp32 data.
 """
@@ -158,6 +167,34 @@ def sensevoice_model_tensors(state: Dict[str, torch.Tensor], cfg, cmvn: Optional
         if k.startswith(("encoder.", "ctc.", "embed.")) and torch.is_floating_point(v):
             out[k] = v.detach().float().cpu().contiguous().numpy()
     return out
+
+
+def aligner_model_tensors(state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: Optional[torch.Tensor], token_list=None,
+                          smooth_factor2: float = 0.25, noise_threshold2: float = 0.01) -> Dict[str, np.ndarray]:
+    """The tensors of a MonotonicAligner model file.  state: MonotonicAligner's state_dict (synth.make_aligner_state_dict uses the same
+    names); cfg: its encoder shape and CIF threshold; cmvn: am.mvn as [2, 560]; token_list: the tokenizer's list, which only gives
+    eos_id; smooth_factor2 / noise_threshold2: CifPredictorV3's predictor_conf values."""
+    if "encoder.encoders0.0.norm1.weight" not in state or "predictor." + TS_HEAD_KEY not in state:
+        raise ValueError("not a MonotonicAligner state_dict (encoder.encoders0.0 / predictor.upsample_cnn missing)")
+    eos_id = list(token_list).index("</s>") if token_list is not None and "</s>" in token_list else -1
+    out: Dict[str, np.ndarray] = {}
+    out["__aligner_config__"] = np.array([cfg.enc_layers, cfg.d_model, cfg.heads, cfg.feat_dim, cfg.ln_eps, cfg.cif_threshold, eos_id],
+                                         dtype=np.float32)
+    _frontend_tensors(out, cmvn, cfg.feat_dim)
+    for k, v in state.items():
+        if k.startswith("encoder.") and torch.is_floating_point(v):
+            out[k] = v.detach().float().cpu().contiguous().numpy()
+    for k, v in timestamp_head_tensors(state).items():
+        out[k] = v.cpu().numpy()
+    up_times = int(state["predictor." + TS_HEAD_KEY].shape[2])
+    out["__ts_config__"] = np.array([up_times, smooth_factor2, noise_threshold2], dtype=np.float32)
+    return out
+
+
+def write_aligner_model_file(path: str, state: Dict[str, torch.Tensor], cfg: ParaformerConfig, cmvn: Optional[torch.Tensor] = None,
+                             token_list=None, smooth_factor2: float = 0.25, noise_threshold2: float = 0.01) -> int:
+    """A MonotonicAligner (fa-zh) model file for the forced-alignment handle (fa_align_init): `aligner_model_tensors`."""
+    return _write(path, aligner_model_tensors(state, cfg, cmvn, token_list, smooth_factor2, noise_threshold2))
 
 
 def campplus_model_tensors(state: Dict[str, torch.Tensor]) -> Dict[str, np.ndarray]:

@@ -859,6 +859,31 @@ void* fa_offline_infer_vad_audio(void* asr, void* vad, void* spk, const void* co
                                  const int32_t* textnorm_ids, const FaLongAudioOptions* opts, int32_t preset_spk_num);
 void* fa_vad_infer_audio(void* vad, const void* buf, int64_t n_samples, const FaAudioFormat* fmt, const FaVadRunOptions* opts);
 int fa_spk_embed_audio(void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch, const FaAudioFormat* fmt, float* emb_host);
+/* ---- Forced alignment: MonotonicAligner (fa-zh; monotonic_aligner/model.py:182-267, funasr_b200/modules.py MonotonicAlignerB200 is
+ * the specification) -- [start_ms, end_ms] for each token of a transcript the caller already has.
+ * fa_align_init: model file written by funasr_b200/pack.py:write_aligner_model_file (encoder.*, the repacked timestamp head,
+ * __ts_config__, the frontend tables and CMVN, __aligner_config__).  Refused before any device is touched, naming the piece: no
+ * __aligner_config__, a file that also carries __config__ or __sv_config__, (d_model, head dim) other than (320, 80) or (512, 128),
+ * feat_dim != 560, CMVN other than [2, 560], upsample_times != 3, a missing or misshapen encoder or head tensor.  fa_offline_init
+ * refuses an aligner file.
+ * fa_align_infer: batch HOST recordings bufs[i] of n_frames[i] frames in fmt's layout (resampled to 16 kHz on the device as for
+ * fa_offline_infer_audio) and transcripts ids[i] [n_ids[i]] -> a result for the recogniser's accessors:
+ *   fa_offline_result_stamps(r, i)  utterance i's {start_ms, end_ms} pairs: ts_prediction_lfr6_standard over the timestamp head's
+ *                                   first 3 * enc_len upsampled frames, run with token_num = n_ids[i] + 1 (the transcript and its </s>)
+ *                                   and stamping n_ids[i] tokens, n_ids[i] - 1 when the last id is the file's eos_id (the routine drops
+ *                                   a trailing "</s>").  An empty transcript gives no stamp; one with more tokens than the audio
+ *                                   fires for gives fewer stamps than tokens (the count is returned on its own).
+ *   fa_offline_result_ids(r, i)     the tokens those stamps belong to: the transcript without a trailing eos_id.
+ *   fa_offline_result_count / fa_offline_result_audio_seconds / fa_offline_free_result as for recogniser results.
+ * Stamps are per token id: the caller applies sentence_postprocess's merges of English sub-word pieces (nothing to merge for CJK
+ * characters), and a token spelled "<sil>", whose stamp the Python routine drops by name, keeps its stamp here.
+ * Before any launch, with the handle usable afterwards: NULL handle, bufs, n_frames, fmt or n_ids, batch < 1, n_ids[i] < 0, ids (or
+ * ids[i]) NULL with n_ids[i] > 0, an utterance under 400 samples at 16 kHz (named by index), and every refusal of the audio
+ * descriptor.  NULL on error (fa_offline_last_error()). */
+void* fa_align_init(const char* model_file, int32_t device, int32_t gemm_mode);
+void* fa_align_infer(void* aligner, const void* const* bufs, const int64_t* n_frames, int32_t batch, const FaAudioFormat* fmt,
+                     const int32_t* const* ids, const int32_t* n_ids);
+void fa_align_uninit(void* aligner);
 /* p-pruning's effective pval for n rows (SpectralCluster.p_pruning): 6 / n when n * pval < 6, else pval (float64). */
 double fa_spk_effective_pval(int32_t n, double pval);
 /* SpectralCluster.sim_mat -> p_pruning -> 0.5 (P + P^T) -> laplacian over device embeddings emb [n, dim] fp32 (1 <= n <= 2047,
