@@ -187,6 +187,9 @@ SIGNATURES = {
     "fa_fsmn_vad_workspace_bytes": (_sz, [C.POINTER(FaVadEncoder), _i32]),
     "fa_fsmn_vad_forward": (C.c_int, [C.POINTER(FaVadEncoder), _vp, _i64, _i32, _vp, _vp, _vp, _sz, _vp]),
     "fa_frame_decibels": (C.c_int, [_vp, _i64, _i32, _vp, _vp]),
+    "fa_fsmn_vad_batch_workspace_bytes": (_sz, [C.POINTER(FaVadEncoder), _i32, _i32]),
+    "fa_fsmn_vad_forward_batch": (C.c_int, [C.POINTER(FaVadEncoder), _vp, _i64, _vp, _i32, _i32, _vp, _vp, _sz, _vp]),
+    "fa_frame_decibels_batch": (C.c_int, [_vp, _i64, _vp, _i32, _i32, _vp, _vp]),
     "fa_cif_wo_hidden_host": (C.c_int, [_vp, _i64, C.c_float, _vp]),
     "fa_ts_stamps_host": (_i64, [_vp, _vp, _i64, _i64, _i32, C.c_double, _vp, _i64]),
     "fa_vad_detect_segments": (_i64, [_vp, _vp, _i64, _i64, C.POINTER(FaVadOptions), _i32, _i32, _vp, _i32, C.c_double, _vp, _i64]),

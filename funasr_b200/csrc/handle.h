@@ -15,6 +15,7 @@
 #include <exception>
 #include <map>
 #include <memory>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -224,8 +225,9 @@ struct ResampleTable {
 // A handle's resampling tables keyed by (rate, resampler), built on the host when first needed and kept (grow-only, like its
 // buffers), and the host rows of the last upload
 struct ResampleCache {
+  std::mutex mu;                                     // plan_audio's lookup and insertion: callers check their format concurrently
   std::map<std::pair<int32_t, int32_t>, ResampleTable> tables;
-  std::vector<int64_t> rows;
+  std::vector<int64_t> rows;                         // written by upload, under the handle's device lock
 };
 
 // The caller's audio layout, checked, with its table (nullptr at 16 kHz)
@@ -266,7 +268,11 @@ const T* result_row(const std::vector<std::vector<T>>* rows, int32_t index, int3
 }
 
 // ------------------------------------------------------------------------------------------------ handles that cross files
+// Any handle may be shared by many threads.  Each handle has a device lock (`mu`), held by a call for all of its work on the handle's
+// stream and buffers; argument checks run before it is taken.  A call that needs several handles takes their locks in one order,
+// recogniser -> VAD -> speaker (-> punctuation, aligner: never held with another), so two recognisers sharing a VAD cannot deadlock.
 struct Model {
+  std::mutex mu;
   Loaded file;
   int mode = 3;
   int enc_layers = 0, dec_layers = 0, d_model = 512, heads = 4, kernel = 11, vocab = 0, feat_dim = 560;
@@ -280,6 +286,7 @@ struct Model {
   bool contextual = false;                           // ContextualParaformer: decoder with a hotword bias branch
   bool ts = false;                                   // BiCifParaformer: CifPredictorV3's upsampled timestamp head
   FaTimestampHead head{};
+  std::mutex host_cache_mu;                          // host_cache alone: host readers do not wait for a decode on the handle
   std::map<std::string, std::vector<float>> host_cache;   // fa_offline_host_tensor
   bool sv = false;                                   // SenseVoiceSmall (__sv_config__): query rows, the SAN-M and tp stacks, the CTC head
   int tp_layers = 0, n_embed = 0, blank = 0;
@@ -325,6 +332,7 @@ std::unique_ptr<Result> decode_pack(Model& m, const float* wav, int64_t stride, 
                                     int32_t n_hotwords, const int32_t* lang, const int32_t* tn);
 
 struct Vad {
+  std::mutex mu;
   Loaded file;
   std::vector<FaVadLayer> layers;
   FaVadEncoder enc{};
@@ -344,8 +352,13 @@ struct VadResult {
 FaVadRunOptions default_vad_run();
 // VAD of one device-resident recording wav [n] fp32 on stream st (the VAD's own, or the recogniser's in long audio)
 bool vad_run(Vad& v, const float* wav, int64_t n, cudaStream_t st, const FaVadRunOptions& ro, VadResult& out);
+// The same for B device-resident recordings wav [B, stride] of n[i] samples in one batched pass (fa_fsmn_vad_forward_batch,
+// fa_frame_decibels_batch, one copy back), each recording's end points then walked on its own -> out[i], equal to vad_run on it
+bool vad_run_batch(Vad& v, const float* wav, int64_t stride, const int64_t* n, int B, cudaStream_t st, const FaVadRunOptions& ro,
+                   std::vector<VadResult>& out);
 
 struct Spk {
+  std::mutex mu;
   Loaded file;
   int mode = FA_GEMM_F32_SIMT;
   FaCampplus model{};

@@ -183,6 +183,7 @@ bool plan_audio(const FaAudioFormat* fmt, ResampleCache& cache, Audio& a) {
   a.tab = nullptr;
   if (f.sample_rate == 16000) return true;
   const std::pair<int32_t, int32_t> key(f.sample_rate, f.resampler);
+  std::lock_guard<std::mutex> lock(cache.mu);        // entries are never removed: a table found stays where it is
   auto it = cache.tables.find(key);
   if (it != cache.tables.end()) { a.tab = &it->second; return true; }
   ResampleTable t;

@@ -15,6 +15,7 @@ namespace {
 enum { kAlEnc = 0, kAlDModel, kAlHeads, kAlFeat, kAlEps, kAlThreshold, kAlEos, kAlCfgLen };
 
 struct Aligner {
+  std::mutex mu;                                     // device lock
   Loaded file;
   int mode = FA_GEMM_F32_SIMT;
   int enc_layers = 0, d_model = 0, heads = 0, feat_dim = 0, eos_id = -1;
@@ -153,6 +154,7 @@ extern "C" void* fa_align_infer(void* aligner, const void* const* bufs, const in
     lens_h[i] = (int32_t)n16;
     nmax = std::max(nmax, n16);
   }
+  std::lock_guard<std::mutex> dev(m.mu);
   cudaSetDevice(m.file.device);
   const int64_t stride = (nmax + 3) / 4 * 4;
   std::unique_ptr<Result> r(new Result());

@@ -422,6 +422,7 @@ void* infer_batch(void* handle, const void* const* bufs, const int64_t* n_sample
   if (!plan_audio(fmt, m.resample, au)) return nullptr;
   if (!check_hotword_rows(m, hw_embed, n_hotwords)) return nullptr;
   if (m.sv && !check_queries(m, lang, tn, batch, "utterance")) return nullptr;
+  std::lock_guard<std::mutex> dev(m.mu);
   cudaSetDevice(m.file.device);
   int64_t nmax = 0;
   std::vector<int32_t> lens_h(batch);
@@ -524,6 +525,7 @@ extern "C" int fa_offline_hotword_embed(void* handle, const int32_t* ids, const 
       }
     n_tok += lens[i];
   }
+  std::lock_guard<std::mutex> dev(m->mu);
   cudaSetDevice(m->file.device);
   cudaStream_t st = m->file.st;
   const size_t ws = fa_hotword_encoder_workspace_bytes(n, n_tok, m->mode);
@@ -543,6 +545,7 @@ extern "C" const float* fa_offline_host_tensor(void* handle, const char* name, i
   auto it = m->file.t.find(name);
   if (it == m->file.t.end()) return nullptr;
   const Tensor& t = it->second;
+  std::lock_guard<std::mutex> lock(m->host_cache_mu);
   if (!t.dev) {                                 // a "__" configuration tensor: its payload is on the host already
     if (numel) *numel = (int64_t)t.host.size();
     return t.host.data();

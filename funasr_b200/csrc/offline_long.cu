@@ -1,5 +1,5 @@
-// Long audio through the handle API: each recording uploaded once, FSMN-VAD on the device (vad_run), segments merged and packed by
-// duration on the host (fa_merge_vad / fa_pack_segments), each pack gathered on the device and decoded by the recogniser
+// Long audio through the handle API: the call's recordings uploaded together and scored by one batched FSMN-VAD pass (vad_run_batch),
+// then per recording its segments merged and packed by duration on the host (fa_merge_vad / fa_pack_segments), each pack gathered on the device and decoded by the recogniser
 // (decode_pack); fa_offline_infer_vad_spk then diarizes every recording with the CAM++ handle (diarize).
 #include "handle.h"
 
@@ -7,13 +7,16 @@ using namespace fa_handle;
 
 namespace {
 
+// padded 16 kHz samples one long-audio call uploads and scores at once: an hour of audio (230 MB of fp32 rows)
+const int64_t kVadGroupSamples = 3600LL * 16000;
+
 // one recording of fa_offline_infer_vad: inference_with_vad (auto_model.py:852-1035, funasr_b200/long_audio.py:LongAudioPipeline.generate)
-// on the device recording rec [n]; (lang, tn): the recording's SenseVoice query, the same for all its segments
-bool long_audio_one(Model& m, Vad& v, int rec_index, const float* rec, int64_t n, const float* hw_embed, int32_t n_hotwords, int32_t lang,
-                    int32_t tn, const FaLongAudioOptions& o, std::vector<int32_t>& ids, std::vector<int32_t>& segs_out, std::vector<int32_t>& stamps) {
+// (lang, tn): the recording's SenseVoice query, the same for all its segments
+// on the device recording rec [n] with its VAD result vr
+bool long_audio_one(Model& m, const VadResult& vr, int rec_index, const float* rec, int64_t n, const float* hw_embed, int32_t n_hotwords,
+                    int32_t lang, int32_t tn, const FaLongAudioOptions& o, std::vector<int32_t>& ids, std::vector<int32_t>& segs_out,
+                    std::vector<int32_t>& stamps) {
   cudaStream_t st = m.file.st;
-  VadResult vr;
-  if (!vad_run(v, rec, n, st, o.vad, vr)) return false;
   std::vector<int32_t> segs = vr.seg;
   if (o.merge_vad) {
     segs.resize(2 * vr.seg.size() + 2);
@@ -77,7 +80,7 @@ bool long_audio_one(Model& m, Vad& v, int rec_index, const float* rec, int64_t n
   return true;
 }
 
-// fa_offline_infer_vad* / fa_offline_infer_vad_audio: every recording on its own; lang / tn one query per recording (NULL = the defaults)
+// fa_offline_infer_vad* / fa_offline_infer_vad_audio: every recording decoded on its own; lang / tn one query per recording (NULL = the defaults)
 // spk: diarize every recording that decoded at least one token (LongAudioPipeline.generate), preset_spk_num <= 0: no preset count
 // fmt: the recordings' layout (the 16 kHz entries pass their pcm_format's)
 void* infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_samples, int32_t batch, const FaAudioFormat* fmt, const float* hw_embed,
@@ -101,6 +104,11 @@ void* infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_
     n16[i] = au.len16(n_samples[i]);
     if (n16[i] > 0x7fffffffLL) return fail("bad recording " + std::to_string(i));
   }
+  // recogniser -> VAD -> speaker (handle.h)
+  std::lock_guard<std::mutex> asr_lock(mp->mu);
+  std::lock_guard<std::mutex> vad_lock(vp->mu);
+  std::unique_lock<std::mutex> spk_lock;
+  if (spk) spk_lock = std::unique_lock<std::mutex>(spk->mu);
   cudaSetDevice(mp->file.device);
   std::unique_ptr<Result> r(new Result());
   r->ids.resize(batch);
@@ -110,17 +118,31 @@ void* infer_vad(void* asr, void* vad, const void* const* bufs, const int64_t* n_
   r->stamps.resize(batch);
   r->spk.resize(batch);
   if (!no_throw("fa_offline_infer_vad: ", [&] {
-        for (int i = 0; i < batch; ++i) {
-          float* rec = nullptr;
-          if (!upload(&bufs[i], &n_samples[i], 1, (n16[i] + 3) / 4 * 4, au, mp->resample, mp->upload, mp->file.st, &rec) ||
-              !long_audio_one(*mp, *vp, i, rec, n16[i], hw_embed, n_hotwords, lang ? lang[i] : kSvAuto, tn ? tn[i] : kSvWoItn, o, r->ids[i],
-                              r->segs[i], r->stamps[i]))
+        // recordings in arrival order, uploaded together in groups of at most kVadGroupSamples padded samples (a longer recording is
+        // a group of its own) and scored by one batched VAD pass; then each recording's segments are packed and decoded on their own
+        for (int g0 = 0, g1; g0 < batch; g0 = g1) {
+          int64_t stride = (n16[g0] + 3) / 4 * 4;
+          for (g1 = g0 + 1; g1 < batch; ++g1) {
+            const int64_t w = std::max(stride, (n16[g1] + 3) / 4 * 4);
+            if ((g1 - g0 + 1) * w > kVadGroupSamples) break;
+            stride = w;
+          }
+          float* recs = nullptr;
+          std::vector<VadResult> vr;
+          if (!upload(&bufs[g0], &n_samples[g0], g1 - g0, stride, au, mp->resample, mp->upload, mp->file.st, &recs) ||
+              !vad_run_batch(*vp, recs, stride, &n16[g0], g1 - g0, mp->file.st, o.vad, vr))
             return false;
-          r->token_num[i] = (int32_t)r->ids[i].size();
-          // the recogniser's stream is idle here (its results are on the host); the speaker work runs on the speaker handle's stream
-          if (spk && !r->ids[i].empty() &&
-              !diarize(*spk, rec, n16[i], r->segs[i], preset_spk_num, r->spk[i], "recording " + std::to_string(i) + ": "))
-            return false;
+          for (int i = g0; i < g1; ++i) {
+            const float* rec = recs + (int64_t)(i - g0) * stride;
+            if (!long_audio_one(*mp, vr[i - g0], i, rec, n16[i], hw_embed, n_hotwords, lang ? lang[i] : kSvAuto, tn ? tn[i] : kSvWoItn, o,
+                                r->ids[i], r->segs[i], r->stamps[i]))
+              return false;
+            r->token_num[i] = (int32_t)r->ids[i].size();
+            // the recogniser's stream is idle here (its results are on the host); the speaker work runs on the speaker handle's stream
+            if (spk && !r->ids[i].empty() &&
+                !diarize(*spk, rec, n16[i], r->segs[i], preset_spk_num, r->spk[i], "recording " + std::to_string(i) + ": "))
+              return false;
+          }
         }
         return true;
       }))

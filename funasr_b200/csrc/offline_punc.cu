@@ -11,6 +11,7 @@ namespace {
 enum { kPuncLayers = 0, kPuncDModel, kPuncHeads, kPuncKernel, kPuncSentenceEnd, kPuncSplit, kPuncCfgLen };
 
 struct Punc {
+  std::mutex mu;                                     // device lock
   Loaded file;
   fa_punc::Vocab vocab;
   int layers = 0, d_model = 0, heads = 0, d_in = 0, n_embed = 0;
@@ -114,6 +115,7 @@ extern "C" void* fa_punc_infer(void* punc, const char* const* texts, int32_t n) 
   if (!p || (!texts && n > 0) || n < 0) return fail("bad argument");
   for (int32_t i = 0; i < n; ++i)
     if (!texts[i]) return fail("text " + std::to_string(i) + " is NULL");
+  std::lock_guard<std::mutex> dev(p->mu);
   cudaSetDevice(p->file.device);
   std::unique_ptr<fa_punc::Result> r(new fa_punc::Result());
   std::string err;

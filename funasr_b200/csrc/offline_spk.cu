@@ -380,6 +380,7 @@ int spk_embed(void* spk, const void* const* bufs, const int64_t* n_samples, int3
             std::to_string(kSpkMaxFrames) + " (MAX_FEAT_FRAMES)");
     return FA_ERR_UNSUPPORTED;
   }
+  std::lock_guard<std::mutex> dev(s->mu);
   cudaSetDevice(s->file.device);
   cudaStream_t st = s->file.st;
   const int64_t stride = (nmax + 3) / 4 * 4;
@@ -419,6 +420,7 @@ extern "C" int fa_spk_cluster(void* spk, const float* emb_host, int32_t n, int32
             "this backend does not provide; pass preset_spk_num or diarize fewer than 2048 chunks");
     return FA_ERR_UNSUPPORTED;
   }
+  std::lock_guard<std::mutex> dev(s->mu);
   cudaSetDevice(s->file.device);
   std::vector<int32_t> lab;
   const bool ok = no_throw("fa_spk_cluster: ", [&] {

@@ -82,42 +82,65 @@ const double kSilenceSchedule[] = {10000, 2000, 20000, 1000, 30000, 800, 40000, 
 
 namespace fa_handle {
 
-bool vad_run(Vad& v, const float* wav, int64_t n, cudaStream_t st, const FaVadRunOptions& ro, VadResult& out) {
-  out.audio_seconds = (float)((double)n / 16000.0);
-  const int64_t T = n >= 400 ? (n - 400) / 160 + 1 : 0;
-  out.seg.clear();
-  out.frames.assign((size_t)(2 * T), 0.f);
-  if (T == 0) return true;                                   // shorter than one frame: nothing to score
-  const int32_t n32 = (int32_t)n;
-  const size_t ws_bytes = fa_fsmn_vad_workspace_bytes(&v.enc, (int32_t)T);
-  int32_t *lens, *flens;
+bool vad_run_batch(Vad& v, const float* wav, int64_t stride, const int64_t* n, int B, cudaStream_t st, const FaVadRunOptions& ro,
+                   std::vector<VadResult>& out) {
+  out.assign(B, VadResult());
+  std::vector<int32_t> io(2 * (size_t)B);                    // sample counts, then frame counts
+  int32_t t_max = 0;
+  for (int i = 0; i < B; ++i) {
+    const int64_t T = n[i] >= 400 ? (n[i] - 400) / 160 + 1 : 0;
+    out[i].audio_seconds = (float)((double)n[i] / 16000.0);
+    out[i].frames.assign((size_t)(2 * T), 0.f);
+    io[i] = (int32_t)n[i];
+    io[B + i] = (int32_t)T;
+    t_max = std::max(t_max, (int32_t)T);
+  }
+  if (t_max == 0) return true;                               // every recording shorter than one frame: nothing to score
+  const size_t rows = (size_t)B * t_max;
+  const size_t ws_bytes = fa_fsmn_vad_batch_workspace_bytes(&v.enc, B, t_max);
+  int32_t *io_d, *flens;
   float *feats, *frames;
   void* ws;
   if (!carve(v.vad_run, "VAD", [&](fa::Arena& a) {
-        lens = a.take<int32_t>(1); flens = a.take<int32_t>(1);
-        feats = a.take<float>((size_t)T * 400); frames = a.take<float>((size_t)T * 2); ws = a.take<char>(ws_bytes);
+        io_d = a.take<int32_t>(io.size()); flens = a.take<int32_t>(B);
+        feats = a.take<float>(rows * 400); frames = a.take<float>(rows * 2); ws = a.take<char>(ws_bytes);
       }))
     return false;
-  cudaMemcpyAsync(lens, &n32, 4, cudaMemcpyHostToDevice, st);
-  int rc = fa_fbank_lfr_cmvn_tables(wav, lens, 1, n, v.cmvn, v.file.fbank_tables, 5, 1, feats, T, flens, (int32_t)T, st);
-  if (rc == FA_OK) rc = fa_fsmn_vad_forward(&v.enc, feats, 400, (int32_t)T, frames, nullptr, ws, ws_bytes, st);
-  if (rc == FA_OK) rc = fa_frame_decibels(wav, n, (int32_t)T, frames + T, st);
+  cudaMemcpyAsync(io_d, io.data(), io.size() * 4, cudaMemcpyHostToDevice, st);
+  int rc = fa_fbank_lfr_cmvn_tables(wav, io_d, B, stride, v.cmvn, v.file.fbank_tables, 5, 1, feats, t_max, flens, t_max, st);
+  if (rc == FA_OK) rc = fa_fsmn_vad_forward_batch(&v.enc, feats, 400, io.data() + B, B, t_max, frames, ws, ws_bytes, st);
+  if (rc == FA_OK) rc = fa_frame_decibels_batch(wav, stride, io_d + B, B, t_max, frames + rows, st);
   if (rc != FA_OK) { set_err(std::string("VAD: ") + fa_status_string(rc)); return false; }
-  cudaMemcpyAsync(out.frames.data(), frames, (size_t)T * 8, cudaMemcpyDeviceToHost, st);     // the one copy back: two floats per frame
+  std::vector<float> frames_h(rows * 2);
+  cudaMemcpyAsync(frames_h.data(), frames, rows * 8, cudaMemcpyDeviceToHost, st);     // the one copy back: two floats per frame
   if (!sync_stream(st)) return false;
-  std::vector<double> sil(out.frames.begin(), out.frames.begin() + T), db(out.frames.begin() + T, out.frames.end());
-  FaVadOptions o = v.opts;
-  if (!ro.dynamic_silence && ro.max_end_silence_time > 0) o.max_end_silence_time = ro.max_end_silence_time;
-  std::vector<int32_t> seg(128);
-  for (;;) {
-    const int64_t cap = (int64_t)seg.size() / 2;
-    const int64_t k = fa_vad_detect_segments(sil.data(), db.data(), T, n, &o, 60000, ro.dynamic_silence ? 1 : 0, kSilenceSchedule,
-                                             (int32_t)(sizeof(kSilenceSchedule) / sizeof(double) / 2), ro.speech_noise_thres, seg.data(), cap);
-    if (k < 0) { set_err("fa_vad_detect_segments failed: posteriors must lie inside (0, 1)"); return false; }
-    if (k <= cap) { seg.resize((size_t)(2 * k)); break; }
-    seg.resize((size_t)(2 * k));
+  for (int i = 0; i < B; ++i) {
+    const int64_t T = io[B + i];
+    VadResult& r = out[i];
+    if (T == 0) continue;
+    std::copy(frames_h.begin() + (size_t)i * t_max, frames_h.begin() + (size_t)i * t_max + T, r.frames.begin());
+    std::copy(frames_h.begin() + rows + (size_t)i * t_max, frames_h.begin() + rows + (size_t)i * t_max + T, r.frames.begin() + T);
+    std::vector<double> sil(r.frames.begin(), r.frames.begin() + T), db(r.frames.begin() + T, r.frames.end());
+    FaVadOptions o = v.opts;
+    if (!ro.dynamic_silence && ro.max_end_silence_time > 0) o.max_end_silence_time = ro.max_end_silence_time;
+    std::vector<int32_t> seg(128);
+    for (;;) {
+      const int64_t cap = (int64_t)seg.size() / 2;
+      const int64_t k = fa_vad_detect_segments(sil.data(), db.data(), T, n[i], &o, 60000, ro.dynamic_silence ? 1 : 0, kSilenceSchedule,
+                                               (int32_t)(sizeof(kSilenceSchedule) / sizeof(double) / 2), ro.speech_noise_thres, seg.data(), cap);
+      if (k < 0) { set_err("fa_vad_detect_segments failed: posteriors must lie inside (0, 1)"); return false; }
+      if (k <= cap) { seg.resize((size_t)(2 * k)); break; }
+      seg.resize((size_t)(2 * k));
+    }
+    r.seg.swap(seg);
   }
-  out.seg.swap(seg);
+  return true;
+}
+
+bool vad_run(Vad& v, const float* wav, int64_t n, cudaStream_t st, const FaVadRunOptions& ro, VadResult& out) {
+  std::vector<VadResult> r;
+  if (!vad_run_batch(v, wav, n, &n, 1, st, ro, r)) return false;
+  out = std::move(r[0]);
   return true;
 }
 
@@ -146,6 +169,7 @@ void* vad_infer(void* vad, const void* buf, int64_t n_samples, const FaAudioForm
   if (!plan_audio(fmt, v->resample, au)) return nullptr;
   const int64_t n16 = au.len16(n_samples);
   if (n16 > 0x7fffffffLL) return fail("bad argument");
+  std::lock_guard<std::mutex> dev(v->mu);
   cudaSetDevice(v->file.device);
   std::unique_ptr<VadResult> r(new VadResult());
   float* wav = nullptr;

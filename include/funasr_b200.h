@@ -504,6 +504,18 @@ int64_t fa_ts_stamps_host(const float* us_alphas, const float* us_peaks, int64_t
                           double vad_offset_ms, int32_t* out, int64_t max_out);
 /* decibel[f] = 10 log10(sum_{j<400} wav[160 f + j]^2 + 1e-6), f < frames (ComputeDecibel, model.py:516-525). */
 int fa_frame_decibels(const float* wav, int64_t n_samples, int32_t frames, float* decibel, fa_stream_t stream);
+/* The same two stages over a ragged batch of recordings, for long audio over many recordings at once.
+ * fa_fsmn_vad_forward_batch: feats [batch * t_max, ld_feats] (row b's frames at rows b * t_max ..), frames [batch] HOST (row b's frame
+ * count, <= t_max) -> sil_prob [batch, t_max]; workspace of fa_fsmn_vad_batch_workspace_bytes(enc, batch, t_max).  Row b's valid
+ * values equal fa_fsmn_vad_forward on that row alone, bit for bit (every stage computes a frame on its own and the memory is causal and
+ * masked at the row's length); values past frames[b] are unspecified.
+ * fa_frame_decibels_batch: wav [batch, stride], frames [batch] DEVICE (each row needs (frames - 1) * 160 + 400 samples) ->
+ * decibel [batch, t_max], frames past frames[b] unwritten; row b equals fa_frame_decibels on that row alone. */
+size_t fa_fsmn_vad_batch_workspace_bytes(const FaVadEncoder* enc, int32_t batch, int32_t t_max);
+int fa_fsmn_vad_forward_batch(const FaVadEncoder* enc, const float* feats, int64_t ld_feats, const int32_t* frames, int32_t batch, int32_t t_max,
+                              float* sil_prob, void* workspace, size_t ws_bytes, fa_stream_t stream);
+int fa_frame_decibels_batch(const float* wav, int64_t stride, const int32_t* frames, int32_t batch, int32_t t_max, float* decibel,
+                            fa_stream_t stream);
 
 /* Greedy post-filter (paraformer/model.py:655-666): keep argmax_ids[b, k] for k < tok_lens[b] that are not
  * in {blank=0, sos=1, eos=2}; out_ids [B, n_max] (padded with -1), out_lens [B]. */
@@ -740,6 +752,11 @@ int64_t fa_sv_ctc_text_host(const int32_t* ids, int32_t n, const char* const* to
 void fa_offline_free_result(void* result);
 void fa_offline_uninit(void* handle);
 const char* fa_offline_last_error(void);
+/* Threads.  Every handle (recogniser, VAD, speaker, punctuation, aligner) may be shared by any number of threads.  A call checks its
+ * arguments on the calling thread, then holds the handle's lock for its device work, so calls on one handle run one after another
+ * and each gives exactly what it gives alone; calls on different handles run concurrently.  A call that uses several handles
+ * (fa_offline_infer_vad*) locks them in the order recogniser, VAD, speaker, so recognisers that share a VAD handle cannot deadlock.
+ * fa_offline_last_error is per thread.  Uninit a handle only after every call on it has returned. */
 
 /* ---------------------------------------------------------------------------------------------
  * Handle-style FSMN-VAD and long-audio recognition (no Python, no torch) — FunASR's `vad_model` path: FsmnVADStreaming.inference
@@ -778,7 +795,8 @@ typedef struct {
   int32_t merge_length_s;
   FaVadRunOptions vad;
 } FaLongAudioOptions;
-/* Every recording on its own, as inference_with_vad treats it: VAD, optional merge, segments sorted by duration and packed
+/* Every recording on its own, as inference_with_vad treats it (the recordings are uploaded together and scored by one batched VAD
+ * pass, which gives each the values it gets alone): VAD, optional merge, segments sorted by duration and packed
  * (fa_pack_segments), each pack gathered from the device-resident recording into one zero-padded batch (fa_gather_segments) and
  * decoded like fa_offline_infer_hw (the same hotword memory for every segment), results restored to time order.  Result entry i
  * holds recording i: fa_offline_result_ids = the ids of its segments concatenated in time order, fa_offline_result_segments = its

@@ -1,7 +1,11 @@
 /* The OfflineStream surface of FunASR's C++ runtime — runtime/onnxruntime/include/funasrruntime.h:21-77,100-116 — with the SAME
  * names, argument lists and defaults, implemented over this library's handle API (funasr_b200.h: fa_offline_*).  A server written
  * against funasrruntime.h (runtime/websocket, runtime/http, bin/funasr-onnx-offline.cpp) links against libfunasr_b200.so with this
- * header in place of the original for the offline ASR calls it makes.  Differences, all at run time, none in the signatures:
+ * header in place of the original for the offline ASR calls it makes.  One handle may be shared by any number of threads, as the
+ * reference's servers share it among their decoder threads: FunOfflineInfer / FunOfflineInferBuffer, CompileHotwordEmbedding,
+ * FsmnVad* and CTTransformer* are safe on shared handles (funasr_b200.h, "Threads"); calls on one handle take turns on its GPU
+ * stream.  thread_num and batch_size stay ignored: segments are packed by "batch-size-s".
+ * Differences, all at run time, none in the signatures:
  *   model_path["model-dir"] names a directory holding `model.fab2` (funasr_b200/pack.py, written from an unmodified model.pt +
  *   am.mvn) and optionally `tokens.txt` (one token per line; without it results carry the token ids in decimal);
  *   optional keys "gemm-mode" (fp32 | fp16 | fp16x3 | fp16x6, default fp16x3) and "gpu-id" (default 0);
