@@ -167,6 +167,9 @@ SIGNATURES = {
     "fa_sanm_encoder_forward": (C.c_int, [C.POINTER(FaEncoder), _vp, _vp, _i32, _i32, _vp, _i32, _vp, _sz, _vp]),
     "fa_cif_predictor_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "fa_cif_predictor_forward": (C.c_int, [C.POINTER(FaPredictor), _vp, _vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _sz, _vp]),
+    "fa_cif_predictor_ext_workspace_bytes": (_sz, [_i32, _i32, _i32]),
+    "fa_cif_predictor_forward_ext": (C.c_int, [C.POINTER(FaPredictor), _vp, _vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _sz, _vp,
+                                               _vp, _vp]),
     "fa_paraformer_decoder_workspace_bytes_hw": (_sz, [_i32, _i32, _i32, _i32, _i32, _i32]),
     "fa_paraformer_decoder_forward": (C.c_int, [C.POINTER(FaDecoder), _vp, _vp, _i32, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _sz, _vp]),
     "fa_row_sum_f32": (C.c_int, [_vp, _i64, _i32, _i32, _vp, _vp]),
@@ -181,8 +184,12 @@ SIGNATURES = {
     "fa_hotword_encoder_forward": (C.c_int, [C.POINTER(FaHotwordEncoder), _vp, _vp, _i32, _vp, _i32, _vp, _sz, _vp]),
     "fa_cif_upsample_alphas": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _f, _f, _f, _vp, _vp, _vp]),
     "fa_blstm_tc_scratch_bytes": (_sz, [_i32]),
+    "fa_blstm_tc_ext_scratch_bytes": (_sz, [_i32]),
+    "fa_blstm_forward_tc_ext": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _sz, _vp, _vp]),
     "fa_blstm_forward_tc": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _sz, _vp]),
     "fa_timestamp_head_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32]),
+    "fa_timestamp_head_ext_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32]),
+    "fa_timestamp_head_forward_ext": (C.c_int, [C.POINTER(FaTimestampHead), _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _vp, _sz, _vp, _vp, _vp]),
     "fa_timestamp_head_forward": (C.c_int, [C.POINTER(FaTimestampHead), _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _vp, _sz, _vp]),
     "fa_fsmn_vad_workspace_bytes": (_sz, [C.POINTER(FaVadEncoder), _i32]),
     "fa_fsmn_vad_forward": (C.c_int, [C.POINTER(FaVadEncoder), _vp, _i64, _i32, _vp, _vp, _vp, _sz, _vp]),
@@ -221,6 +228,7 @@ SIGNATURES = {
     "fa_offline_infer_hw": (_vp, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp, _i32]),
     "fa_offline_is_contextual": (_i32, [_vp]),
     "fa_offline_has_timestamps": (_i32, [_vp]),
+    "fa_offline_pool_stats": (C.c_int, [_vp, C.POINTER(_i64), C.POINTER(_i64)]),
     "fa_offline_host_tensor": (_vp, [_vp, C.c_char_p, C.POINTER(_i64)]),
     "fa_offline_result_count": (_i32, [_vp]),
     "fa_offline_result_ids": (C.POINTER(_i32), [_vp, _i32, C.POINTER(_i32)]),

@@ -16,9 +16,10 @@
 
 namespace fa {
 
-// Xc[(b,t), k*D + c] = enc[b, t+k-1, c], zero outside [0, T)  (ConstantPad1d((1,1)) + Conv1d(k=3), :275-276)
+// Xc[(b,t), k*D + c] = enc[b, t+k-1, c], zero outside [0, ext[b])  (ConstantPad1d((1,1)) + Conv1d(k=3), :275-276).  ext (NULL: t_max
+// for every row) is the padded length the row's batch had in the reference: its conv at t = len - 1 reads frame len when len < ext.
 __global__ void __launch_bounds__(256)
-cif_im2col_kernel(const float* __restrict__ enc, int t_max, int d, float* __restrict__ xc, int64_t total4) {
+cif_im2col_kernel(const float* __restrict__ enc, int t_max, const int32_t* __restrict__ ext, int d, float* __restrict__ xc, int64_t total4) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total4) return;
   const int d4 = d >> 2;
@@ -27,8 +28,9 @@ cif_im2col_kernel(const float* __restrict__ enc, int t_max, int d, float* __rest
   const int k = (int)(rk % 3);
   const int64_t row = rk / 3;
   const int t = (int)(row % t_max) + k - 1;
+  const int te = ext ? ext[row / t_max] : t_max;
   float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (t >= 0 && t < t_max) val = __ldg(reinterpret_cast<const float4*>(enc + (row + k - 1) * d) + c4);
+  if (t >= 0 && t < te) val = __ldg(reinterpret_cast<const float4*>(enc + (row + k - 1) * d) + c4);
   reinterpret_cast<float4*>(xc)[i] = val;
 }
 
@@ -36,10 +38,11 @@ cif_im2col_kernel(const float* __restrict__ enc, int t_max, int d, float* __rest
 // front of and behind every utterance, P[b][0] = 0, P[b][1 + t] = enc[b, t], P[b][T + 1] = 0 (row pitch d).  The im2col row of
 // (b, t) — enc[b, t-1] | enc[b, t] | enc[b, t+1] — is then the 3 d CONTIGUOUS elements starting at P[b][t], i.e. the im2col matrix is
 // the overlapping 2-D view {rows b (T + 2) + t, 3 d columns, row pitch d}, which a TMA tensor map describes directly.  Rows
-// b (T + 2) + T and + T + 1 of that view mix two utterances: their outputs are computed and never read.
+// b (T + 2) + T and + T + 1 of that view mix two utterances: their outputs are computed and never read.  Frames at or past ext[b]
+// (NULL: t_max) are zero planes, as in im2col above.
 __global__ void __launch_bounds__(256)
-cif_pad_planes_kernel(const float* __restrict__ enc, int t_max, int d, int nplanes, int64_t rows_alloc, int64_t rows_valid,
-                      plane_t* __restrict__ planes) {
+cif_pad_planes_kernel(const float* __restrict__ enc, int t_max, const int32_t* __restrict__ ext, int d, int nplanes, int64_t rows_alloc,
+                      int64_t rows_valid, plane_t* __restrict__ planes) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int d4 = d >> 2;
   if (i >= rows_alloc * d4) return;
@@ -49,7 +52,7 @@ cif_pad_planes_kernel(const float* __restrict__ enc, int t_max, int d, int nplan
   const int64_t b = r / tp;
   const int t = (int)(r - b * tp) - 1;
   float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (r < rows_valid && t >= 0 && t < t_max) x = __ldg(reinterpret_cast<const float4*>(enc + (b * t_max + t) * d + c));
+  if (r < rows_valid && t >= 0 && t < (ext ? ext[b] : t_max)) x = __ldg(reinterpret_cast<const float4*>(enc + (b * t_max + t) * d + c));
   float v[4] = {x.x, x.y, x.z, x.w};
   const int64_t plane = rows_alloc * d;
   for (int pl = 0; pl < nplanes; ++pl) {
@@ -143,11 +146,13 @@ __device__ float torch_row_sum_f32(const float* __restrict__ x, int n) {
 //                       loads, not by bytes: 64 channels per CTA put 8 CTAs on every utterance (512 CTAs at B = 64 instead of 64 —
 //                       round 2 launch list: 189 us for 65 MB with one 512-thread CTA per utterance), and the time loop fetches
 //                       CIF_UNROLL frames ahead of the dependent adds.
+// ext[b] (NULL: t_max) is the row's padded length in the reference's batch: the token count sums the ext[b] + 1 weights of that row
+// and the hidden frames past ext[b] read zero.  The weights past ext[b] are zero, so nothing fires there.
 constexpr int CIF_CH = 64;
 constexpr int CIF_UNROLL = 16;
 __global__ void __launch_bounds__(CIF_CH)
 cif_fire_kernel(const float* __restrict__ enc, const float* __restrict__ alpha_rows, const int32_t* __restrict__ lens,
-                int t_max, int d, float tail, float* __restrict__ acoustic, int n_cap, int32_t* __restrict__ token_num,
+                const int32_t* __restrict__ ext, int t_max, int d, float tail, float* __restrict__ acoustic, int n_cap, int32_t* __restrict__ token_num,
                 float* __restrict__ alphas_out, float* __restrict__ peaks_out) {
   extern __shared__ float sm[];
   float* s_alpha = sm;                    // [T+1]
@@ -156,6 +161,7 @@ cif_fire_kernel(const float* __restrict__ enc, const float* __restrict__ alpha_r
   const int b = blockIdx.x;
   const bool first_group = blockIdx.y == 0;
   const int T1 = t_max + 1;
+  const int te = ext ? ext[b] : t_max, T1e = te + 1;
   const int len = min(lens[b], t_max);
   for (int t = threadIdx.x; t < T1; t += blockDim.x) {
     float a = t < t_max ? alpha_rows[(int64_t)b * t_max + t] : 0.f;
@@ -165,7 +171,7 @@ cif_fire_kernel(const float* __restrict__ enc, const float* __restrict__ alpha_r
   __syncthreads();
   __shared__ float s_total;
   if ((threadIdx.x >> 5) == 1) {                    // warp 1, beside thread 0's scan: token_num = floor(alphas.sum(-1)) in torch's fp32 order
-    const float tot = torch_row_sum_f32(s_alpha, T1);
+    const float tot = torch_row_sum_f32(s_alpha, T1e);
     if ((threadIdx.x & 31) == 0) s_total = tot;
   }
   if (threadIdx.x == 0) {
@@ -195,17 +201,17 @@ cif_fire_kernel(const float* __restrict__ enc, const float* __restrict__ alpha_r
   if (c < d) {
     double acc = 0.0;                     // PH[t] before its rounding to fp32
     float prev_ph = 0.f, prev_rh = 0.f;
-    for (int t0 = 0; t0 < T1; t0 += CIF_UNROLL) {
+    for (int t0 = 0; t0 < T1e; t0 += CIF_UNROLL) {
       float hh[CIF_UNROLL];
 #pragma unroll
       for (int u = 0; u < CIF_UNROLL; ++u) {                              // the loads of CIF_UNROLL frames go out before the first dependent add
         const int t = t0 + u;
-        hh[u] = t < t_max ? __ldg(hb + (int64_t)t * d + c) : 0.f;         // hidden gets one zero frame appended (:441-442)
+        hh[u] = t < te ? __ldg(hb + (int64_t)t * d + c) : 0.f;            // hidden gets one zero frame appended (:441-442)
       }
 #pragma unroll
       for (int u = 0; u < CIF_UNROLL; ++u) {
         const int t = t0 + u;
-        if (t < T1) {
+        if (t < T1e) {
           const float h = hh[u];
           acc = __dadd_rn(acc, (double)__fmul_rn(s_alpha[t], h));         // cumsum(alphas * hidden) :878
           const int k = s_ord[t];
@@ -226,10 +232,10 @@ cif_fire_kernel(const float* __restrict__ enc, const float* __restrict__ alpha_r
 // BiCif flavour (CifPredictorV3.forward -> `cif`, funasr/models/bicif_paraformer/cif_predictor.py:37-84): the integrate-and-fire
 // recurrence runs sequentially in fp32 (no fp64 prefix sums), a fire subtracts exactly 1.0, and a frame is the running
 // fp32 sum  frame += cur * h  (multiply, then add) that restarts at  remainds * h  after every fire.  Same launch geometry
-// as cif_fire_kernel: thread 0 resolves the scalar recurrence into shared memory, then one thread per channel.
+// as cif_fire_kernel: thread 0 resolves the scalar recurrence into shared memory, then one thread per channel.  ext as there.
 __global__ void __launch_bounds__(512)
 cif_fire_loop_kernel(const float* __restrict__ enc, const float* __restrict__ alpha_rows, const int32_t* __restrict__ lens,
-                     int t_max, int d, float tail, float threshold, float* __restrict__ acoustic, int n_cap,
+                     const int32_t* __restrict__ ext, int t_max, int d, float tail, float threshold, float* __restrict__ acoustic, int n_cap,
                      int32_t* __restrict__ token_num, float* __restrict__ alphas_out, float* __restrict__ peaks_out) {
   extern __shared__ float sm[];
   float* s_cur = sm;                      // [T+1] weight of frame t inside the token being integrated
@@ -237,6 +243,7 @@ cif_fire_loop_kernel(const float* __restrict__ enc, const float* __restrict__ al
   int* s_ord = reinterpret_cast<int*>(sm + 2 * (t_max + 1));  // [T+1] fire ordinal or -1
   const int b = blockIdx.x;
   const int T1 = t_max + 1;
+  const int te = ext ? ext[b] : t_max, T1e = te + 1;
   const int len = min(lens[b], t_max);
   for (int t = threadIdx.x; t < T1; t += blockDim.x) {
     float a = t < t_max ? alpha_rows[(int64_t)b * t_max + t] : 0.f;
@@ -246,7 +253,7 @@ cif_fire_loop_kernel(const float* __restrict__ enc, const float* __restrict__ al
   __syncthreads();
   __shared__ float s_total;
   float total_w1 = 0.f;
-  if ((threadIdx.x >> 5) == 1) total_w1 = torch_row_sum_f32(s_cur, T1);   // before thread 0 overwrites s_cur with the per-frame weights
+  if ((threadIdx.x >> 5) == 1) total_w1 = torch_row_sum_f32(s_cur, T1e);   // before thread 0 overwrites s_cur with the per-frame weights
   __syncthreads();
   if (threadIdx.x == 32) s_total = total_w1;
   if (threadIdx.x == 0) {
@@ -272,8 +279,8 @@ cif_fire_loop_kernel(const float* __restrict__ enc, const float* __restrict__ al
   float* ob = acoustic + (int64_t)b * n_cap * d;
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
     float frame = 0.f;
-    for (int t = 0; t < T1; ++t) {
-      const float h = t < t_max ? __ldg(hb + (int64_t)t * d + c) : 0.f;   // hidden gets one zero frame appended (:371-372)
+    for (int t = 0; t < T1e; ++t) {
+      const float h = t < te ? __ldg(hb + (int64_t)t * d + c) : 0.f;      // hidden gets one zero frame appended (:371-372)
       frame = __fadd_rn(frame, __fmul_rn(s_cur[t], h));                   // :66
       const int k = s_ord[t];
       if (k >= 0) {
@@ -286,13 +293,14 @@ cif_fire_loop_kernel(const float* __restrict__ enc, const float* __restrict__ al
 
 // Upsampled timestamp head of CifPredictorV3.get_upsample_timestamp (:300-352), after the BLSTM: per utterance
 //   alphas2 *= token_num / sum(alphas2);  us_peaks = cif_wo_hidden(alphas2, threshold - 1e-4)  (fp32, sequential).
-__global__ void cif_upsample_scan_kernel(float* __restrict__ alphas2, const int32_t* __restrict__ token_num, int t3, float thr,
-                                         float* __restrict__ us_peaks) {
+// The sum runs over the row's padded length ext_up[b] (NULL: t3); the weights past it are zero.
+__global__ void cif_upsample_scan_kernel(float* __restrict__ alphas2, const int32_t* __restrict__ token_num, const int32_t* __restrict__ ext_up,
+                                         int t3, float thr, float* __restrict__ us_peaks) {
   const int b = blockIdx.x;
   float* a = alphas2 + (int64_t)b * t3;
   __shared__ float s_scale;
   if (threadIdx.x < 32) {
-    const float tot = torch_row_sum_f32(a, t3);                  // _token_num = alphas2.sum(-1) (:343), torch's fp32 summation order
+    const float tot = torch_row_sum_f32(a, ext_up ? ext_up[b] : t3);                  // _token_num = alphas2.sum(-1) (:343), torch's fp32 summation order
     if (threadIdx.x == 0) s_scale = __fdiv_rn((float)token_num[b], tot);       // (token_num / _token_num) :345
   }
   __syncthreads();
@@ -315,10 +323,10 @@ __global__ void row_sum_f32_kernel(const float* __restrict__ x, int64_t ld, int 
   if (threadIdx.x == 0) out[blockIdx.x] = s;
 }
 
-int cif_im2col_launch(const float* enc, int64_t rows, int t_max, int d, float* xc, cudaStream_t st) {
+int cif_im2col_launch(const float* enc, int64_t rows, int t_max, const int32_t* ext, int d, float* xc, cudaStream_t st) {
   const int64_t total4 = rows * 3 * (d / 4);
   if (total4 <= 0) return FA_OK;
-  cif_im2col_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>(enc, t_max, d, xc, total4);
+  cif_im2col_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>(enc, t_max, ext, d, xc, total4);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }
@@ -332,40 +340,43 @@ int cif_alpha_launch(const float* c, int d, const float* w, const float* b0, con
   return FA_OK;
 }
 
-int cif_pad_planes_launch(const float* enc, int batch, int t_max, int d, int nplanes, int64_t rows_alloc, plane_t* planes, cudaStream_t st) {
+int cif_pad_planes_launch(const float* enc, int batch, int t_max, const int32_t* ext, int d, int nplanes, int64_t rows_alloc, plane_t* planes,
+                          cudaStream_t st) {
   if ((d & 3) || nplanes < 1 || nplanes > 3) return FA_ERR_UNSUPPORTED;
   const int64_t total = rows_alloc * (d / 4);
-  cif_pad_planes_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(enc, t_max, d, nplanes, rows_alloc, (int64_t)batch * (t_max + 2), planes);
+  cif_pad_planes_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(enc, t_max, ext, d, nplanes, rows_alloc, (int64_t)batch * (t_max + 2),
+                                                                         planes);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }
 
-int cif_fire_launch(const float* enc, const float* alpha_rows, const int32_t* lens, int batch, int t_max, int d,
+int cif_fire_launch(const float* enc, const float* alpha_rows, const int32_t* lens, const int32_t* ext, int batch, int t_max, int d,
                     float tail, float* acoustic, int n_cap, int32_t* token_num, float* alphas, float* peaks,
                     cudaStream_t st) {
   const size_t smem = (size_t)3 * (t_max + 1) * sizeof(float);
   if (smem > 200 * 1024) return FA_ERR_UNSUPPORTED;
   if (smem > 48 * 1024) FA_CUDA_OK(cudaFuncSetAttribute(cif_fire_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  cif_fire_kernel<<<dim3(batch, (d + CIF_CH - 1) / CIF_CH), CIF_CH, smem, st>>>(enc, alpha_rows, lens, t_max, d, tail, acoustic, n_cap, token_num,
+  cif_fire_kernel<<<dim3(batch, (d + CIF_CH - 1) / CIF_CH), CIF_CH, smem, st>>>(enc, alpha_rows, lens, ext, t_max, d, tail, acoustic, n_cap, token_num,
                                                                                 alphas, peaks);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }
 
-int cif_fire_loop_launch(const float* enc, const float* alpha_rows, const int32_t* lens, int batch, int t_max, int d,
+int cif_fire_loop_launch(const float* enc, const float* alpha_rows, const int32_t* lens, const int32_t* ext, int batch, int t_max, int d,
                          float tail, float threshold, float* acoustic, int n_cap, int32_t* token_num, float* alphas, float* peaks,
                          cudaStream_t st) {
   const size_t smem = (size_t)3 * (t_max + 1) * sizeof(float);
   if (smem > 200 * 1024) return FA_ERR_UNSUPPORTED;
   if (smem > 48 * 1024) FA_CUDA_OK(cudaFuncSetAttribute(cif_fire_loop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  cif_fire_loop_kernel<<<batch, 512, smem, st>>>(enc, alpha_rows, lens, t_max, d, tail, threshold, acoustic, n_cap, token_num, alphas,
+  cif_fire_loop_kernel<<<batch, 512, smem, st>>>(enc, alpha_rows, lens, ext, t_max, d, tail, threshold, acoustic, n_cap, token_num, alphas,
                                                  peaks);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }
 
-int cif_upsample_scan_launch(float* alphas2, const int32_t* token_num, int batch, int t3, float thr, float* us_peaks, cudaStream_t st) {
-  cif_upsample_scan_kernel<<<batch, 256, 0, st>>>(alphas2, token_num, t3, thr, us_peaks);
+int cif_upsample_scan_launch(float* alphas2, const int32_t* token_num, const int32_t* ext_up, int batch, int t3, float thr, float* us_peaks,
+                             cudaStream_t st) {
+  cif_upsample_scan_kernel<<<batch, 256, 0, st>>>(alphas2, token_num, ext_up, t3, thr, us_peaks);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }

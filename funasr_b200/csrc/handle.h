@@ -7,11 +7,15 @@
 //   offline_vad.cu   FSMN-VAD: fa_vad_*
 //   offline_spk.cu   CAM++ speaker embeddings, clustering, diarization: fa_spk_*
 //   offline_long.cu  long audio: fa_offline_infer_vad*, fa_offline_result_{segments,spk}
+//   offline_pool.cu  the recogniser's request pool: every decoding call's passes, GPU packs and scatter; fa_offline_pool_stats
 //   offline_punc.cu  CT-Transformer punctuation: fa_punc_*
 //   offline_align.cu MonotonicAligner (fa-zh) forced alignment: fa_align_*
 #pragma once
 #include "common.cuh"
 #include <algorithm>
+#include <atomic>
+#include <condition_variable>
+#include <deque>
 #include <exception>
 #include <map>
 #include <memory>
@@ -271,6 +275,34 @@ const T* result_row(const std::vector<std::vector<T>>* rows, int32_t index, int3
 // Any handle may be shared by many threads.  Each handle has a device lock (`mu`), held by a call for all of its work on the handle's
 // stream and buffers; argument checks run before it is taken.  A call that needs several handles takes their locks in one order,
 // recogniser -> VAD -> speaker (-> punctuation, aligner: never held with another), so two recognisers sharing a VAD cannot deadlock.
+// The recogniser's decoding calls do not take `mu` themselves: they post a Ticket to the handle's request pool (offline_pool.cu), and
+// the thread that leads the next pass decodes every queued compatible call in shared GPU packs.
+struct Vad;
+struct Spk;
+struct Result;
+
+// One call of fa_offline_infer* (an utterance batch) or fa_offline_infer_vad* (long audio), its arguments checked, waiting in the pool
+struct Ticket {
+  const void* const* bufs = nullptr;
+  const int64_t* n_samples = nullptr;                // the caller's frames
+  int batch = 0;
+  Audio au;
+  std::vector<int64_t> n16;                          // 16 kHz samples per buffer
+  const float* hw_embed = nullptr;                   // hotword rows: such a call is never merged with another (solo)
+  int32_t n_hotwords = 0;
+  const int32_t *lang = nullptr, *tn = nullptr;      // SenseVoice queries per buffer (NULL: the defaults)
+  bool long_audio = false;                           // fa_offline_infer_vad*: VAD, then packs of each recording's segments
+  Vad* vad = nullptr;
+  FaLongAudioOptions opts{};
+  Spk* spk = nullptr;                                // diarized (solo)
+  int32_t preset_spk_num = 0;
+  bool solo() const { return spk || (hw_embed && n_hotwords > 0); }
+  // written by the pass, read by the owner once done
+  std::unique_ptr<Result> res;
+  std::string err;
+  bool done = false;
+};
+
 struct Model {
   std::mutex mu;
   Loaded file;
@@ -306,8 +338,15 @@ struct Model {
   DevBuf upload;                                     // the host batch of fa_offline_infer*, the recording of long audio
   DevBuf encode, decode, seaco_bias, decode_sv;      // decode_batch before and after its token-count sync; seaco_bias; decode_sv
   DevBuf hotword_embed;                              // fa_offline_hotword_embed's rows
-  DevBuf pack;                                       // long_audio_one: one pack's gather offsets and padded rows
+  DevBuf pool_recs;                                  // a pass's recordings and utterances, one row each (pool_group)
+  DevBuf pack;                                       // pool_group: one GPU pack's gather offsets and padded rows
   DevBuf ws;                                         // the GEMM workspace every stage above uses in turn
+  // the request pool: queued tickets in arrival order, whether a leader is running a pass, counters since init
+  std::mutex pool_mu;
+  std::condition_variable pool_cv;
+  std::deque<Ticket*> pool_q;
+  bool pool_busy = false;
+  std::atomic<int64_t> pool_calls{0}, pool_packs{0};
 };
 
 struct Result {
@@ -327,9 +366,14 @@ bool check_hotword_rows(const Model& m, const float* hw_embed, int32_t n_hotword
 // every query id inside the embedding table; `what` names the unit ("utterance", "recording")
 bool check_queries(const Model& m, const int32_t* lang, const int32_t* tn, int n, const char* what);
 // one padded batch on the device (wav [B, stride], lens_h >= 400 samples each) decoded by the handle's model kind: the hotword memory
-// reaches a contextual or SeACo Paraformer, the queries (per row, NULL = the defaults) a SenseVoice model
-std::unique_ptr<Result> decode_pack(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const float* hw_embed,
-                                    int32_t n_hotwords, const int32_t* lang, const int32_t* tn);
+// reaches a contextual or SeACo Paraformer, the queries (per row, NULL = the defaults) a SenseVoice model.  ext_h [B]: each row's
+// padded length in LFR frames, the t_max of the batch the reference decodes it in (num_lfr_frames(lens_h[b]) <= ext_h[b]); the CIF
+// predictor and the timestamp head give row b exactly what that batch gives it.
+std::unique_ptr<Result> decode_pack(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const std::vector<int32_t>& ext_h,
+                                    const float* hw_embed, int32_t n_hotwords, const int32_t* lang, const int32_t* tn);
+// t's call through the recogniser's request pool: queued, decoded by whichever thread leads the pass that drains it -> its result, or
+// nullptr with its own message set as this thread's error
+void* pool_call(Model& m, Ticket& t);
 
 struct Vad {
   std::mutex mu;

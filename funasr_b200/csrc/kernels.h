@@ -82,17 +82,23 @@ int split_rows_launch(const float* x, int64_t ldx, int64_t rows, int cols, int c
                       cudaStream_t st);
 int fsmn_launch(const float* v, int64_t ldv, const int32_t* lens, int batch, int t_max, int channels, const float* w,
                 int ksize, const float* res, int64_t ldr, float* out, int64_t ldo, cudaStream_t st, int causal = 0);
-int cif_im2col_launch(const float* enc, int64_t rows, int t_max, int d, float* xc, cudaStream_t st);
-int cif_fire_loop_launch(const float* enc, const float* alpha_rows, const int32_t* lens, int batch, int t_max, int d,
+// ext / ext_up: each row's padded length on the device (NULL: t_max / t3 for every row), cif.cu
+int cif_im2col_launch(const float* enc, int64_t rows, int t_max, const int32_t* ext, int d, float* xc, cudaStream_t st);
+int cif_fire_loop_launch(const float* enc, const float* alpha_rows, const int32_t* lens, const int32_t* ext, int batch, int t_max, int d,
                          float tail, float threshold, float* acoustic, int n_cap, int32_t* token_num, float* alphas, float* peaks,
                          cudaStream_t st);
-int cif_upsample_scan_launch(float* alphas2, const int32_t* token_num, int batch, int t3, float thr, float* us_peaks, cudaStream_t st);
+int cif_upsample_scan_launch(float* alphas2, const int32_t* token_num, const int32_t* ext_up, int batch, int t3, float thr, float* us_peaks,
+                             cudaStream_t st);
 int cif_alpha_launch(const float* c, int d, const float* w, const float* b0, const int32_t* lens, int t_max,
                      int64_t rows, float smooth, float noise, float* alpha_rows, cudaStream_t st, int c_rows_per_batch = 0);
-int cif_pad_planes_launch(const float* enc, int batch, int t_max, int d, int nplanes, int64_t rows_alloc, plane_t* planes, cudaStream_t st);
-int cif_fire_launch(const float* enc, const float* alpha_rows, const int32_t* lens, int batch, int t_max, int d,
+int cif_pad_planes_launch(const float* enc, int batch, int t_max, const int32_t* ext, int d, int nplanes, int64_t rows_alloc, plane_t* planes,
+                          cudaStream_t st);
+int cif_fire_launch(const float* enc, const float* alpha_rows, const int32_t* lens, const int32_t* ext, int batch, int t_max, int d,
                     float tail, float* acoustic, int n_cap, int32_t* token_num, float* alphas, float* peaks,
                     cudaStream_t st);
+// the persistent BLSTM (lstm.cu): T lockstep steps over sequences of t_ld steps, ext their own lengths on the device (NULL: T each)
+int blstm_tc_launch(const float* xproj, const float* w_hh_f, const float* w_hh_b, int batch, int T, int t_ld, const int32_t* ext, int hidden,
+                    float* out, void* scratch, size_t scratch_bytes, cudaStream_t st);
 int ctc_filter_launch(const int32_t* ids, const int32_t* lens, int batch, int t_max, int blank, int32_t* out_ids,
                       int32_t* out_lens, cudaStream_t st);
 // torchaudio kaldi.fbank defaults (no x32768, no LFR, no CMVN) through the table-driven kernel (fbank.cu): the CAM++ frontend

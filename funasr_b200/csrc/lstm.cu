@@ -42,11 +42,15 @@ __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// hx: exchange tensor [2 parity][2 dir][2 plane][batch_pad][H] bf16 (batch_pad = tiles * 64)
+// hx: exchange tensor [2 parity][2 dir][2 plane][batch_pad][H] bf16 (batch_pad = tiles * 64).  xproj and out hold t_ld steps per
+// sequence.  ext[b] (NULL: T for every sequence) is sequence b's own length: the grid runs T = max(ext) steps in lockstep, sequence b's
+// forward direction reads and writes t = step and its backward direction t = ext[b] - 1 - step, both from a zero state, and both stop
+// writing at step ext[b] (a sequence past its length computes finite values nobody reads)
 template <int H>
 __global__ void __launch_bounds__(128, 1)
 blstm_tc_kernel(const float* __restrict__ xproj, const float* __restrict__ w_hh_f, const float* __restrict__ w_hh_b, int batch, int T,
-                float* __restrict__ out, __nv_bfloat16* __restrict__ hx, unsigned int* __restrict__ counters) {
+                int t_ld, const int32_t* __restrict__ ext, float* __restrict__ out, __nv_bfloat16* __restrict__ hx,
+                unsigned int* __restrict__ counters) {
   constexpr int LS_H = H, LS_NC = H / LS_UNITS, LT_PITCH = lt_pitch<H>();
   extern __shared__ __align__(16) unsigned char smb[];
   unsigned char* sWp = smb;                                   // [2 planes][32 rows][LT_PITCH]
@@ -83,7 +87,6 @@ blstm_tc_kernel(const float* __restrict__ xproj, const float* __restrict__ w_hh_
   const int64_t plane_stride = (int64_t)batch_pad * LS_H;                 // elements between hi and lo plane
   const int64_t dir_stride = 2 * plane_stride, par_stride = 2 * dir_stride;
   for (int step = 0; step < T; ++step) {
-    const int t = dir == 0 ? step : T - 1 - step;
     const __nv_bfloat16* hx_rd = hx + (int64_t)((step + 1) & 1) * par_stride + dir * dir_stride;   // written during step-1
     __nv_bfloat16* hx_wr = hx + (int64_t)(step & 1) * par_stride + dir * dir_stride;
     if (step > 0) {
@@ -100,10 +103,14 @@ blstm_tc_kernel(const float* __restrict__ xproj, const float* __restrict__ w_hh_
       const int b0 = bt * LS_BT;
       // x projections (+ biases) of this thread's 2 sequences x 2 units x 4 gates
       float acc[4][4];                     // [gate][d-fragment element: (r0,cu) (r0,cu+1) (r0+8,cu) (r0+8,cu+1)]
+      int ts[2];                           // the time index of this thread's 2 sequences; -1 past their length
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const int b = min(b0 + warp * 16 + r0 + 8 * hh, batch - 1);
-        const float* xp = xproj + ((int64_t)b * T + t) * xp_ld + dir * 4 * LS_H + c * LS_UNITS + cu;
+        const int eb = ext ? ext[b] : T;
+        const int t = dir == 0 ? step : eb - 1 - step;
+        ts[hh] = step < eb ? t : -1;
+        const float* xp = xproj + ((int64_t)b * t_ld + max(t, 0)) * xp_ld + dir * 4 * LS_H + c * LS_UNITS + cu;
 #pragma unroll
         for (int g = 0; g < 4; ++g) {
           const float2 x2 = __ldg(reinterpret_cast<const float2*>(xp + g * LS_H));
@@ -159,7 +166,7 @@ blstm_tc_kernel(const float* __restrict__ xproj, const float* __restrict__ w_hh_
           cst[bt][hh][uu] = cn;
           hv[uu] = og * tanhf(cn);
         }
-        if (bseq < batch) *reinterpret_cast<float2*>(out + ((int64_t)bseq * T + t) * out_ld + dir * LS_H + c * LS_UNITS + cu) = make_float2(hv[0], hv[1]);
+        if (bseq < batch && ts[hh] >= 0) *reinterpret_cast<float2*>(out + ((int64_t)bseq * t_ld + ts[hh]) * out_ld + dir * LS_H + c * LS_UNITS + cu) = make_float2(hv[0], hv[1]);
         // publish bf16 planes of h_t for the next step (padded sequences publish finite garbage that nobody reads back into results)
         const __nv_bfloat162 h2 = __floats2bfloat162_rn(hv[0], hv[1]);
         const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h2);
@@ -183,8 +190,8 @@ static size_t blstm_scratch_bytes(int batch, int H) {
 }
 
 template <int H>
-static int blstm_tc_launch_h(const float* xproj, const float* w_hh_f, const float* w_hh_b, int batch, int T, float* out,
-                             void* scratch, size_t scratch_bytes, cudaStream_t st) {
+static int blstm_tc_launch_h(const float* xproj, const float* w_hh_f, const float* w_hh_b, int batch, int T, int t_ld, const int32_t* ext,
+                             float* out, void* scratch, size_t scratch_bytes, cudaStream_t st) {
   const size_t need = blstm_scratch_bytes(batch, H);
   if (scratch_bytes < need) return FA_ERR_WORKSPACE;
   const size_t smem = (size_t)2 * LS_ROWS * lt_pitch<H>() + (size_t)2 * LS_BT * lt_pitch<H>();
@@ -193,19 +200,26 @@ static int blstm_tc_launch_h(const float* xproj, const float* w_hh_f, const floa
   unsigned int* counters = static_cast<unsigned int*>(scratch);
   __nv_bfloat16* hx = reinterpret_cast<__nv_bfloat16*>(static_cast<char*>(scratch) + 256);
   FA_CUDA_OK(cudaMemsetAsync(scratch, 0, need, st));
-  void* args[] = {(void*)&xproj, (void*)&w_hh_f, (void*)&w_hh_b, (void*)&batch, (void*)&T, (void*)&out, (void*)&hx, (void*)&counters};
+  void* args[] = {(void*)&xproj, (void*)&w_hh_f, (void*)&w_hh_b, (void*)&batch, (void*)&T, (void*)&t_ld, (void*)&ext, (void*)&out, (void*)&hx,
+                  (void*)&counters};
   FA_CUDA_OK(cudaLaunchCooperativeKernel((const void*)blstm_tc_kernel<H>, dim3(2 * (H / LS_UNITS)), dim3(128), args, smem, st));
   count_launch();
   return FA_OK;
 }
 
-int blstm_tc_launch(const float* xproj, const float* w_hh_f, const float* w_hh_b, int batch, int T, int hidden, float* out,
-                    void* scratch, size_t scratch_bytes, cudaStream_t st) {
+// T steps of sequences t_ld long; ext: their lengths on the device (NULL: T = t_ld for all)
+int blstm_tc_launch(const float* xproj, const float* w_hh_f, const float* w_hh_b, int batch, int T, int t_ld, const int32_t* ext, int hidden,
+                    float* out, void* scratch, size_t scratch_bytes, cudaStream_t st) {
   if (batch <= 0 || T <= 0) return FA_OK;
   if (!xproj || !w_hh_f || !w_hh_b || !out || !scratch) return FA_ERR_ARG;
   if ((hidden != 512 && hidden != 320) || batch > 4 * LS_BT) return FA_ERR_UNSUPPORTED;
-  return hidden == 512 ? blstm_tc_launch_h<512>(xproj, w_hh_f, w_hh_b, batch, T, out, scratch, scratch_bytes, st)
-                       : blstm_tc_launch_h<320>(xproj, w_hh_f, w_hh_b, batch, T, out, scratch, scratch_bytes, st);
+  return hidden == 512 ? blstm_tc_launch_h<512>(xproj, w_hh_f, w_hh_b, batch, T, t_ld, ext, out, scratch, scratch_bytes, st)
+                       : blstm_tc_launch_h<320>(xproj, w_hh_f, w_hh_b, batch, T, t_ld, ext, out, scratch, scratch_bytes, st);
+}
+
+// the per-sequence lengths ext_h [batch] (host, 1 <= ext_h[b] <= t_len) after the recurrence's scratch, 256-byte aligned
+static size_t blstm_ext_scratch_bytes(int batch) {
+  return blstm_scratch_bytes(batch, LS_HMAX) + (size_t)(batch > 0 ? batch : 0) * sizeof(int32_t);
 }
 
 }  // namespace fa
@@ -216,5 +230,24 @@ int blstm_tc_launch(const float* xproj, const float* w_hh_f, const float* w_hh_b
 extern "C" size_t fa_blstm_tc_scratch_bytes(int32_t batch) { return fa::blstm_scratch_bytes(batch, fa::LS_HMAX); }
 extern "C" int fa_blstm_forward_tc(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, int32_t batch, int32_t t_len,
                                    int32_t hidden, float* out, void* scratch, size_t scratch_bytes, fa_stream_t stream) {
-  return fa::blstm_tc_launch(xproj, w_hh_fwd, w_hh_bwd, batch, t_len, hidden, out, scratch, scratch_bytes, (cudaStream_t)stream);
+  return fa::blstm_tc_launch(xproj, w_hh_fwd, w_hh_bwd, batch, t_len, t_len, nullptr, hidden, out, scratch, scratch_bytes, (cudaStream_t)stream);
+}
+
+extern "C" size_t fa_blstm_tc_ext_scratch_bytes(int32_t batch) { return fa::blstm_ext_scratch_bytes(batch); }
+extern "C" int fa_blstm_forward_tc_ext(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, int32_t batch, int32_t t_len,
+                                       int32_t hidden, float* out, void* scratch, size_t scratch_bytes, fa_stream_t stream, const int32_t* ext_h) {
+  if (!ext_h || batch < 0 || t_len < 0) return FA_ERR_ARG;
+  int32_t t_run = 0;
+  for (int32_t b = 0; b < batch; ++b) {
+    if (ext_h[b] < 1 || ext_h[b] > t_len) return FA_ERR_ARG;
+    t_run = ext_h[b] > t_run ? ext_h[b] : t_run;
+  }
+  if (batch == 0 || t_len == 0) return FA_OK;
+  if (!xproj || !w_hh_fwd || !w_hh_bwd || !out || !scratch) return FA_ERR_ARG;
+  if ((hidden != 512 && hidden != 320) || batch > 4 * fa::LS_BT) return FA_ERR_UNSUPPORTED;
+  if (scratch_bytes < fa::blstm_ext_scratch_bytes(batch)) return FA_ERR_WORKSPACE;
+  const size_t lstm_bytes = fa::blstm_scratch_bytes(batch, fa::LS_HMAX);
+  int32_t* ext_d = reinterpret_cast<int32_t*>(static_cast<char*>(scratch) + lstm_bytes);
+  FA_CUDA_OK(cudaMemcpyAsync(ext_d, ext_h, (size_t)batch * sizeof(int32_t), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  return fa::blstm_tc_launch(xproj, w_hh_fwd, w_hh_bwd, batch, t_run, t_len, ext_d, hidden, out, scratch, lstm_bytes, (cudaStream_t)stream);
 }

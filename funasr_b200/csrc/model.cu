@@ -4,7 +4,9 @@
 #include "kernels.h"
 #include <string.h>
 #include <math.h>
+#include <algorithm>
 #include <map>
+#include <vector>
 #include <mutex>
 #include <utility>
 
@@ -172,8 +174,8 @@ extern "C" int fa_sanm_encoder_forward(const FaEncoder* enc, const float* feats,
 // ---------------------------------------------------------------------------------------------- predictor
 // fp32: the im2col rows [M, 3D] and the conv output c [M, D].  Tensor cores: no im2col copy — the GEMM's A operand is the
 // overlapping view of the zero-padded encoder planes pp (cif.cu), and its output c has the padded rows [batch * (t_max + 2), D].
-struct CifBufs { float *xc, *c, *alpha_rows; plane_t* pp; };
-static CifBufs cif_carve(Arena& a, int batch, int t_max, int mode) {
+struct CifBufs { float *xc, *c, *alpha_rows; plane_t* pp; int32_t* ext; };
+static CifBufs cif_carve(Arena& a, int batch, int t_max, int mode, bool ext) {
   const int D = 512;
   const int64_t M = (int64_t)batch * t_max, Mp = (int64_t)batch * (t_max + 2);
   const bool tc = mode != FA_GEMM_F32_SIMT;
@@ -182,13 +184,56 @@ static CifBufs cif_carve(Arena& a, int batch, int t_max, int mode) {
   b.c = a.take<float>((tc ? Mp : M) * (size_t)D);
   b.alpha_rows = a.take<float>(M);
   b.pp = tc ? a.take<plane_t>((size_t)gemm_planes(mode) * (Mp + 2) * D) : nullptr;
+  b.ext = ext ? a.take<int32_t>(batch) : nullptr;                 // last: the carve above is unchanged without it
   return b;
 }
 
 extern "C" size_t fa_cif_predictor_workspace_bytes(int32_t batch, int32_t t_max, int32_t gemm_mode) {
   Arena m = Arena::measuring();
-  cif_carve(m, batch, t_max, gemm_mode);
+  cif_carve(m, batch, t_max, gemm_mode, false);
   return m.bytes();
+}
+
+extern "C" size_t fa_cif_predictor_ext_workspace_bytes(int32_t batch, int32_t t_max, int32_t gemm_mode) {
+  Arena m = Arena::measuring();
+  cif_carve(m, batch, t_max, gemm_mode, true);
+  return m.bytes();
+}
+
+// ext_h: each row's padded length (host, NULL: t_max for every row), copied into the workspace
+static int cif_predictor(const FaPredictor* pred, const float* enc, const int32_t* lens, int32_t batch, int32_t t_max, float* acoustic,
+                         int32_t n_cap, int32_t* token_num, float* alphas, float* peaks, int32_t gemm_mode, void* workspace, size_t ws_bytes,
+                         cudaStream_t st, const int32_t* ext_h) {
+  const int D = 512;
+  if (pred->conv.out_f != D || pred->conv.in_f != 3 * D) return FA_ERR_UNSUPPORTED;
+  const bool tc = gemm_mode != FA_GEMM_F32_SIMT;
+  if (tc && !pred->conv.w_planes) return FA_ERR_ARG;
+  if (tc && pred->conv.in_pad != 3 * D) return FA_ERR_UNSUPPORTED;    // the conv view reads K = 3 D unpadded
+  const int64_t M = (int64_t)batch * t_max;
+  Arena a(workspace, ws_bytes);
+  const CifBufs b = cif_carve(a, batch, t_max, gemm_mode, ext_h != nullptr);
+  if (!a.ok()) return FA_ERR_WORKSPACE;
+  if (ext_h) FA_CUDA_OK(cudaMemcpyAsync(b.ext, ext_h, (size_t)batch * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (tc) {
+    const int npl = gemm_planes(gemm_mode);
+    const int64_t Mp = (int64_t)batch * (t_max + 2), rows_alloc = Mp + 2;
+    FA_RETURN_IF_ERR(cif_pad_planes_launch(enc, batch, t_max, b.ext, D, npl, rows_alloc, b.pp, st));
+    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.pp, Mp, pred->conv, GemmEpi().relu().to(b.c, D), gemm_mode, st, D, rows_alloc));
+    FA_RETURN_IF_ERR(cif_alpha_launch(b.c, D, pred->out_w, pred->out_b, lens, t_max, M, pred->smooth_factor,
+                                      pred->noise_threshold, b.alpha_rows, st, t_max + 2));
+  } else {
+    FA_RETURN_IF_ERR(cif_im2col_launch(enc, M, t_max, b.ext, D, b.xc, st));
+    FA_RETURN_IF_ERR(gemm_rows(b.xc, 3 * D, M, pred->conv, GemmEpi().relu().to(b.c, D), gemm_mode, nullptr, st));
+    FA_RETURN_IF_ERR(cif_alpha_launch(b.c, D, pred->out_w, pred->out_b, lens, t_max, M, pred->smooth_factor,
+                                      pred->noise_threshold, b.alpha_rows, st));
+  }
+  FA_CUDA_OK(cudaMemsetAsync(acoustic, 0, (size_t)batch * n_cap * D * sizeof(float), st));
+  if (pred->cif_variant == 1)     // CifPredictorV3 (BiCifParaformer): sequential fp32 `cif`
+    return cif_fire_loop_launch(enc, b.alpha_rows, lens, b.ext, batch, t_max, D, pred->tail_threshold, pred->threshold, acoustic, n_cap,
+                                token_num, alphas, peaks, st);
+  if (pred->cif_variant != 0) return FA_ERR_ARG;
+  return cif_fire_launch(enc, b.alpha_rows, lens, b.ext, batch, t_max, D, pred->tail_threshold, acoustic, n_cap, token_num, alphas,
+                         peaks, st);
 }
 
 extern "C" int fa_cif_predictor_forward(const FaPredictor* pred, const float* enc, const int32_t* lens, int32_t batch,
@@ -197,36 +242,27 @@ extern "C" int fa_cif_predictor_forward(const FaPredictor* pred, const float* en
                                         fa_stream_t stream) {
   if (!pred || !enc || !lens || !acoustic || !token_num || !alphas || !peaks || batch <= 0 || t_max <= 0 || n_cap <= 0)
     return FA_ERR_ARG;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int D = 512;
-  if (pred->conv.out_f != D || pred->conv.in_f != 3 * D) return FA_ERR_UNSUPPORTED;
-  const bool tc = gemm_mode != FA_GEMM_F32_SIMT;
-  if (tc && !pred->conv.w_planes) return FA_ERR_ARG;
-  if (tc && pred->conv.in_pad != 3 * D) return FA_ERR_UNSUPPORTED;    // the conv view reads K = 3 D unpadded
-  const int64_t M = (int64_t)batch * t_max;
-  Arena a(workspace, ws_bytes);
-  const CifBufs b = cif_carve(a, batch, t_max, gemm_mode);
-  if (!a.ok()) return FA_ERR_WORKSPACE;
-  if (tc) {
-    const int npl = gemm_planes(gemm_mode);
-    const int64_t Mp = (int64_t)batch * (t_max + 2), rows_alloc = Mp + 2;
-    FA_RETURN_IF_ERR(cif_pad_planes_launch(enc, batch, t_max, D, npl, rows_alloc, b.pp, st));
-    FA_RETURN_IF_ERR(gemm_tc_planes_launch(b.pp, Mp, pred->conv, GemmEpi().relu().to(b.c, D), gemm_mode, st, D, rows_alloc));
-    FA_RETURN_IF_ERR(cif_alpha_launch(b.c, D, pred->out_w, pred->out_b, lens, t_max, M, pred->smooth_factor,
-                                      pred->noise_threshold, b.alpha_rows, st, t_max + 2));
-  } else {
-    FA_RETURN_IF_ERR(cif_im2col_launch(enc, M, t_max, D, b.xc, st));
-    FA_RETURN_IF_ERR(gemm_rows(b.xc, 3 * D, M, pred->conv, GemmEpi().relu().to(b.c, D), gemm_mode, nullptr, st));
-    FA_RETURN_IF_ERR(cif_alpha_launch(b.c, D, pred->out_w, pred->out_b, lens, t_max, M, pred->smooth_factor,
-                                      pred->noise_threshold, b.alpha_rows, st));
-  }
-  FA_CUDA_OK(cudaMemsetAsync(acoustic, 0, (size_t)batch * n_cap * D * sizeof(float), st));
-  if (pred->cif_variant == 1)     // CifPredictorV3 (BiCifParaformer): sequential fp32 `cif`
-    return cif_fire_loop_launch(enc, b.alpha_rows, lens, batch, t_max, D, pred->tail_threshold, pred->threshold, acoustic, n_cap,
-                                token_num, alphas, peaks, st);
-  if (pred->cif_variant != 0) return FA_ERR_ARG;
-  return cif_fire_launch(enc, b.alpha_rows, lens, batch, t_max, D, pred->tail_threshold, acoustic, n_cap, token_num, alphas,
-                         peaks, st);
+  return cif_predictor(pred, enc, lens, batch, t_max, acoustic, n_cap, token_num, alphas, peaks, gemm_mode, workspace, ws_bytes,
+                       (cudaStream_t)stream, nullptr);
+}
+
+// every row's padded length ext_h[b] inside [lens_h[b], t_max] (host arrays)
+static bool ext_rows_ok(const int32_t* lens_h, const int32_t* ext_h, int32_t batch, int32_t t_max) {
+  if (!lens_h || !ext_h) return false;
+  for (int32_t b = 0; b < batch; ++b)
+    if (lens_h[b] < 0 || ext_h[b] < lens_h[b] || ext_h[b] > t_max || ext_h[b] < 1) return false;
+  return true;
+}
+
+extern "C" int fa_cif_predictor_forward_ext(const FaPredictor* pred, const float* enc, const int32_t* lens, int32_t batch,
+                                            int32_t t_max, float* acoustic, int32_t n_cap, int32_t* token_num,
+                                            float* alphas, float* peaks, int32_t gemm_mode, void* workspace, size_t ws_bytes,
+                                            fa_stream_t stream, const int32_t* lens_h, const int32_t* ext_h) {
+  if (!pred || !enc || !lens || !acoustic || !token_num || !alphas || !peaks || batch <= 0 || t_max <= 0 || n_cap <= 0 ||
+      !ext_rows_ok(lens_h, ext_h, batch, t_max))
+    return FA_ERR_ARG;
+  return cif_predictor(pred, enc, lens, batch, t_max, acoustic, n_cap, token_num, alphas, peaks, gemm_mode, workspace, ws_bytes,
+                       (cudaStream_t)stream, ext_h);
 }
 
 // CifPredictorV3.get_upsample_timestamp after the BLSTM (bicif_paraformer/cif_predictor.py:331-352)
@@ -237,15 +273,15 @@ extern "C" int fa_cif_upsample_alphas(const float* feat, int32_t dz, const float
     return FA_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
   FA_RETURN_IF_ERR(cif_alpha_launch(feat, dz, w, b, lens_up, t_up, (int64_t)batch * t_up, smooth2, noise2, us_alphas, st));
-  return cif_upsample_scan_launch(us_alphas, token_num, batch, t_up, (float)((double)threshold - 1e-4), us_peaks, st);
+  return cif_upsample_scan_launch(us_alphas, token_num, nullptr, batch, t_up, (float)((double)threshold - 1e-4), us_peaks, st);
 }
 
 // The timestamp head over B * U * t_max upsampled rows: the upsampled rows, both directions' input projections, the BLSTM output,
 // the recurrence's scratch for one launch, the GEMM scratch for the larger (upsampled) GEMM — both have K = D — and lens x U
-// (last: the other takes are whole multiples of 256 bytes, so the carve adds no padding)
+// (last: the other takes are whole multiples of 256 bytes, so the carve adds no padding); with per-row extents, ext and ext x U after it
 static const int kBlstmMaxBatch = 256;          // fa_blstm_forward_tc holds at most 256 sequences per launch
-struct TsHeadBufs { float *up, *xproj, *feat; void* lstm; size_t lstm_bytes; Arena gemm{nullptr, 0}; int32_t* lens_up; };
-static TsHeadBufs ts_head_carve(Arena& a, int batch, int t_max, int d, int up_times, int mode) {
+struct TsHeadBufs { float *up, *xproj, *feat; void* lstm; size_t lstm_bytes; Arena gemm{nullptr, 0}; int32_t *lens_up, *ext, *ext_up; };
+static TsHeadBufs ts_head_carve(Arena& a, int batch, int t_max, int d, int up_times, int mode, bool ext) {
   const int64_t rows = (int64_t)batch * t_max * up_times;
   TsHeadBufs b;
   b.up = a.take<float>((size_t)rows * d);
@@ -255,6 +291,8 @@ static TsHeadBufs ts_head_carve(Arena& a, int batch, int t_max, int d, int up_ti
   b.lstm = a.take<char>(b.lstm_bytes);
   if (mode != FA_GEMM_F32_SIMT) b.gemm = a.sub(gemm_tc_scratch_bytes(rows, d, mode));
   b.lens_up = a.take<int32_t>(batch);
+  b.ext = ext ? a.take<int32_t>(batch) : nullptr;
+  b.ext_up = ext ? a.take<int32_t>(batch) : nullptr;
   return b;
 }
 
@@ -266,14 +304,20 @@ __global__ void scale_lens_kernel(const int32_t* __restrict__ lens, int32_t k, i
 extern "C" size_t fa_timestamp_head_workspace_bytes(int32_t batch, int32_t t_max, int32_t d_model, int32_t up_times, int32_t gemm_mode) {
   if (batch <= 0 || t_max <= 0 || d_model <= 0 || up_times <= 0) return 0;
   Arena m = Arena::measuring();
-  ts_head_carve(m, batch, t_max, d_model, up_times, gemm_mode);
+  ts_head_carve(m, batch, t_max, d_model, up_times, gemm_mode, false);
   return m.bytes();
 }
 
-extern "C" int fa_timestamp_head_forward(const FaTimestampHead* head, const float* enc, const int32_t* lens, const int32_t* token_num,
-                                         int32_t batch, int32_t t_max, float* us_alphas, float* us_peaks, int32_t gemm_mode, void* workspace,
-                                         size_t ws_bytes, fa_stream_t stream) {
-  if (!head || !enc || !lens || !token_num || !us_alphas || !us_peaks || batch <= 0 || t_max <= 0 || head->up_times <= 0) return FA_ERR_ARG;
+extern "C" size_t fa_timestamp_head_ext_workspace_bytes(int32_t batch, int32_t t_max, int32_t d_model, int32_t up_times, int32_t gemm_mode) {
+  if (batch <= 0 || t_max <= 0 || d_model <= 0 || up_times <= 0) return 0;
+  Arena m = Arena::measuring();
+  ts_head_carve(m, batch, t_max, d_model, up_times, gemm_mode, true);
+  return m.bytes();
+}
+
+static int timestamp_head(const FaTimestampHead* head, const float* enc, const int32_t* lens, const int32_t* token_num, int32_t batch,
+                          int32_t t_max, float* us_alphas, float* us_peaks, int32_t gemm_mode, void* workspace, size_t ws_bytes,
+                          fa_stream_t stream, const int32_t* ext_h) {
   if (!head->w_hh_fwd || !head->w_hh_bwd || !head->out2_w || !head->out2_b) return FA_ERR_ARG;
   if (gemm_mode != FA_GEMM_F32_SIMT && gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) return FA_ERR_ARG;
   const FaLinear &up_lin = head->upsample, &ih_lin = head->blstm_ih;
@@ -282,21 +326,46 @@ extern "C" int fa_timestamp_head_forward(const FaTimestampHead* head, const floa
   if (up_lin.out_f != U * D || ih_lin.out_f != 8 * D || ih_lin.in_f != D) return FA_ERR_ARG;
   if (gemm_mode != FA_GEMM_F32_SIMT && (!up_lin.w_planes || !ih_lin.w_planes)) return FA_ERR_ARG;
   Arena a(workspace, ws_bytes);
-  TsHeadBufs b = ts_head_carve(a, batch, t_max, D, U, gemm_mode);
+  TsHeadBufs b = ts_head_carve(a, batch, t_max, D, U, gemm_mode, ext_h != nullptr);
   if (!a.ok()) return FA_ERR_WORKSPACE;
   cudaStream_t st = (cudaStream_t)stream;
   const int TU = t_max * U;
+  std::vector<int32_t> run_h;                 // per BLSTM launch: its longest sequence, in upsampled steps
+  if (ext_h) {
+    FA_CUDA_OK(cudaMemcpyAsync(b.ext, ext_h, (size_t)batch * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    scale_lens_kernel<<<(batch + 255) / 256, 256, 0, st>>>(b.ext, U, batch, b.ext_up);
+    FA_CHECK_LAUNCH();
+    for (int b0 = 0; b0 < batch; b0 += kBlstmMaxBatch)
+      run_h.push_back(U * *std::max_element(ext_h + b0, ext_h + std::min(batch, b0 + kBlstmMaxBatch)));
+  }
   FA_RETURN_IF_ERR(gemm_rows(enc, D, (int64_t)batch * t_max, up_lin, GemmEpi().to(b.up, (int64_t)U * D), gemm_mode, &b.gemm, st));
   FA_RETURN_IF_ERR(gemm_rows(b.up, D, (int64_t)batch * TU, ih_lin, GemmEpi().to(b.xproj, 8 * D), gemm_mode, &b.gemm, st));
   for (int b0 = 0; b0 < batch; b0 += kBlstmMaxBatch) {       // sequences are independent: larger batches run as consecutive launches
     const int bn = batch - b0 < kBlstmMaxBatch ? batch - b0 : kBlstmMaxBatch;
-    FA_RETURN_IF_ERR(fa_blstm_forward_tc(b.xproj + (int64_t)b0 * TU * 8 * D, head->w_hh_fwd, head->w_hh_bwd, bn, TU, D,
-                                         b.feat + (int64_t)b0 * TU * 2 * D, b.lstm, b.lstm_bytes, stream));
+    FA_RETURN_IF_ERR(blstm_tc_launch(b.xproj + (int64_t)b0 * TU * 8 * D, head->w_hh_fwd, head->w_hh_bwd, bn, ext_h ? run_h[b0 / kBlstmMaxBatch] : TU,
+                                     TU, ext_h ? b.ext_up + b0 : nullptr, D, b.feat + (int64_t)b0 * TU * 2 * D, b.lstm, b.lstm_bytes, st));
   }
   scale_lens_kernel<<<(batch + 255) / 256, 256, 0, st>>>(lens, U, batch, b.lens_up);
   FA_CHECK_LAUNCH();
-  return fa_cif_upsample_alphas(b.feat, 2 * D, head->out2_w, head->out2_b, b.lens_up, token_num, batch, TU, head->smooth2, head->noise2,
-                                head->threshold, us_alphas, us_peaks, stream);
+  FA_RETURN_IF_ERR(cif_alpha_launch(b.feat, 2 * D, head->out2_w, head->out2_b, b.lens_up, TU, (int64_t)batch * TU, head->smooth2, head->noise2,
+                                    us_alphas, st));
+  return cif_upsample_scan_launch(us_alphas, token_num, b.ext_up, batch, TU, (float)((double)head->threshold - 1e-4), us_peaks, st);
+}
+
+extern "C" int fa_timestamp_head_forward(const FaTimestampHead* head, const float* enc, const int32_t* lens, const int32_t* token_num,
+                                         int32_t batch, int32_t t_max, float* us_alphas, float* us_peaks, int32_t gemm_mode, void* workspace,
+                                         size_t ws_bytes, fa_stream_t stream) {
+  if (!head || !enc || !lens || !token_num || !us_alphas || !us_peaks || batch <= 0 || t_max <= 0 || head->up_times <= 0) return FA_ERR_ARG;
+  return timestamp_head(head, enc, lens, token_num, batch, t_max, us_alphas, us_peaks, gemm_mode, workspace, ws_bytes, stream, nullptr);
+}
+
+extern "C" int fa_timestamp_head_forward_ext(const FaTimestampHead* head, const float* enc, const int32_t* lens, const int32_t* token_num,
+                                             int32_t batch, int32_t t_max, float* us_alphas, float* us_peaks, int32_t gemm_mode, void* workspace,
+                                             size_t ws_bytes, fa_stream_t stream, const int32_t* lens_h, const int32_t* ext_h) {
+  if (!head || !enc || !lens || !token_num || !us_alphas || !us_peaks || batch <= 0 || t_max <= 0 || head->up_times <= 0 ||
+      !ext_rows_ok(lens_h, ext_h, batch, t_max))
+    return FA_ERR_ARG;
+  return timestamp_head(head, enc, lens, token_num, batch, t_max, us_alphas, us_peaks, gemm_mode, workspace, ws_bytes, stream, ext_h);
 }
 
 // ------------------------------------------------------------------------------------------------ decoder

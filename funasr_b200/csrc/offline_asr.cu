@@ -201,16 +201,18 @@ bool seaco_bias(Model& m, int B, int n_max, int n_cap, const float* hw_host, int
   return sync_stream(st);                                    // lens_h and picked_rows are host vectors of this frame
 }
 
-// The recogniser over a padded batch already on the device: wav [B, stride] fp32, lens_h [B] samples (>= 400 each).  Everything
-// after the host-to-device copy of fa_offline_infer_hw; long audio feeds it the gathered VAD segments of one pack.
-std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const float* hw_embed,
-                                     int32_t n_hotwords) {
+// The recogniser over a padded batch already on the device: wav [B, stride] fp32, lens_h [B] samples (>= 400 each), ext_h [B] each
+// row's padded length in frames (decode_pack).  Everything after the pool gathered the pack's rows.
+std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const std::vector<int32_t>& ext_h,
+                                     const float* hw_embed, int32_t n_hotwords) {
   const int B = (int)lens_h.size(), D = m.d_model;
   cudaStream_t st = m.file.st;
   int t_max = 0;
   double seconds = 0.0;
+  std::vector<int32_t> fl_h(B);                              // encoder lengths, the host copy the _ext entries check ext_h against
   for (int i = 0; i < B; ++i) {
     const int t = num_lfr_frames(lens_h[i]);
+    fl_h[i] = t;
     t_max = t > t_max ? t : t_max;
     seconds += (double)lens_h[i] / 16000.0;
   }
@@ -227,14 +229,15 @@ std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride,
     return nullptr;
   cudaMemcpyAsync(lens, lens_h.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st);
   size_t ws = fa_sanm_encoder_workspace_bytes(B, T, m.mode);
-  const size_t ws2 = fa_cif_predictor_workspace_bytes(B, T, m.mode);
+  const size_t ws2 = fa_cif_predictor_ext_workspace_bytes(B, T, m.mode);
   ws = ws2 > ws ? ws2 : ws;
   if (!m.ws.reserve(ws)) return fail("device allocation failed (workspace)");
   int rc = fa_fbank_lfr_cmvn_tables(wav, lens, B, stride, m.cmvn, m.file.fbank_tables, 7, 6, feats, T, flens, T, st);
   if (rc != FA_OK) return fail(std::string("fa_fbank_lfr_cmvn_tables: ") + fa_status_string(rc));
   rc = fa_sanm_encoder_forward(&m.enc, feats, flens, B, T, encb, m.mode, m.ws.p, m.ws.cap, st);
   if (rc != FA_OK) return fail(std::string("fa_sanm_encoder_forward: ") + fa_status_string(rc));
-  rc = fa_cif_predictor_forward(&m.pred, encb, flens, B, T, acoustic, n_cap, tok, alphas, peaks, m.mode, m.ws.p, m.ws.cap, st);
+  rc = fa_cif_predictor_forward_ext(&m.pred, encb, flens, B, T, acoustic, n_cap, tok, alphas, peaks, m.mode, m.ws.p, m.ws.cap, st, fl_h.data(),
+                                    ext_h.data());
   if (rc != FA_OK) return fail(std::string("fa_cif_predictor_forward: ") + fa_status_string(rc));
   std::unique_ptr<Result> r(new Result());
   r->audio_seconds = (float)seconds;
@@ -253,7 +256,7 @@ std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride,
   const int64_t rows_up = (int64_t)B * TU;
   const int n_sw = m.seaco && hw_embed ? n_hotwords : 0;     // SeACo hotword rows (none: the plain decoder distribution)
   size_t ws_dec = fa_paraformer_decoder_workspace_bytes_hw(B, T, n_max, m.vocab, m.mode, nh);
-  if (m.ts) ws_dec = std::max(ws_dec, fa_timestamp_head_workspace_bytes(B, T, D, U, m.mode));
+  if (m.ts) ws_dec = std::max(ws_dec, fa_timestamp_head_ext_workspace_bytes(B, T, D, U, m.mode));
   if (n_sw > 0)
     ws_dec = std::max({ws_dec, fa_sanm_decoder_stack_workspace_bytes(B, n_sw, n_max, m.mode), fa_linear_argmax_workspace_bytes((int64_t)B * n_max, m.vocab, m.mode)});
   int32_t *ids, *fids, *flens_out, *hw_lens = nullptr;
@@ -290,7 +293,7 @@ std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride,
   if (rc == FA_OK) rc = fa_greedy_filter(final_ids, tok, B, n_max, 1, 2, 0, fids, flens_out, st);
   if (rc != FA_OK) return fail(std::string("decoder: ") + fa_status_string(rc));
   if (m.ts) {                   // CifPredictorV3.get_upsample_timestamp (bicif_paraformer/cif_predictor.py:300-352), engine.upsample_timestamp
-    rc = fa_timestamp_head_forward(&m.head, encb, flens, tok, B, T, us_alphas, us_peaks, m.mode, m.ws.p, m.ws.cap, st);
+    rc = fa_timestamp_head_forward_ext(&m.head, encb, flens, tok, B, T, us_alphas, us_peaks, m.mode, m.ws.p, m.ws.cap, st, fl_h.data(), ext_h.data());
     if (rc != FA_OK) return fail(std::string("timestamp head: ") + fa_status_string(rc));
   }
   std::vector<int32_t> fids_h((size_t)B * n_max), fl(B), enc_lens(m.ts ? B : 0);
@@ -412,32 +415,26 @@ std::unique_ptr<Result> decode_sv(Model& m, const float* wav, int64_t stride, co
   return r;
 }
 
-// fa_offline_infer_hw / fa_offline_infer_sv / fa_offline_infer_audio: host buffers -> one padded 16 kHz batch -> decode_pack
+// fa_offline_infer_hw / fa_offline_infer_sv / fa_offline_infer_audio: the call checked on its own thread, then decoded through the
+// request pool as one reference pack (the whole batch, as the reference decodes it)
 void* infer_batch(void* handle, const void* const* bufs, const int64_t* n_samples, int32_t batch, const FaAudioFormat* fmt, const float* hw_embed,
                   int32_t n_hotwords, const int32_t* lang, const int32_t* tn) {
   Model* mp = static_cast<Model*>(handle);
   if (!mp || !bufs || !n_samples || batch <= 0) return fail("bad argument");
   Model& m = *mp;
-  Audio au;
-  if (!plan_audio(fmt, m.resample, au)) return nullptr;
+  Ticket t;
+  if (!plan_audio(fmt, m.resample, t.au)) return nullptr;
   if (!check_hotword_rows(m, hw_embed, n_hotwords)) return nullptr;
   if (m.sv && !check_queries(m, lang, tn, batch, "utterance")) return nullptr;
-  std::lock_guard<std::mutex> dev(m.mu);
-  cudaSetDevice(m.file.device);
-  int64_t nmax = 0;
-  std::vector<int32_t> lens_h(batch);
+  t.n16.resize(batch);
   for (int i = 0; i < batch; ++i) {
-    const int64_t n16 = bufs[i] && n_samples[i] >= 0 && n_samples[i] <= 0x7fffffffLL ? au.len16(n_samples[i]) : 0;
-    if (n16 < 400 || n16 > 0x7fffffffLL) return fail("every buffer needs >= 400 samples (25 ms)" + au.at16k());
-    lens_h[i] = (int32_t)n16;
-    nmax = n16 > nmax ? n16 : nmax;
+    const int64_t n16 = bufs[i] && n_samples[i] >= 0 && n_samples[i] <= 0x7fffffffLL ? t.au.len16(n_samples[i]) : 0;
+    if (n16 < 400 || n16 > 0x7fffffffLL) return fail("every buffer needs >= 400 samples (25 ms)" + t.au.at16k());
+    t.n16[i] = n16;
   }
-  const int64_t stride = (nmax + 3) / 4 * 4;
-  float* wav = nullptr;
-  if (!upload(bufs, n_samples, batch, stride, au, m.resample, m.upload, m.file.st, &wav)) return nullptr;
-  std::unique_ptr<Result> r = decode_pack(m, wav, stride, lens_h, hw_embed, n_hotwords, lang, tn);
-  if (r) r->audio_seconds = (float)au.seconds(n_samples, batch);
-  return r.release();
+  t.bufs = bufs; t.n_samples = n_samples; t.batch = batch;
+  t.hw_embed = hw_embed; t.n_hotwords = n_hotwords; t.lang = lang; t.tn = tn;
+  return pool_call(m, t);
 }
 
 // the model kind is the file's: SenseVoiceSmall by __sv_config__, Paraformer otherwise; a MonotonicAligner file is fa_align_init's
@@ -476,9 +473,10 @@ bool check_queries(const Model& m, const int32_t* lang, const int32_t* tn, int n
   return true;
 }
 
-std::unique_ptr<Result> decode_pack(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const float* hw_embed,
-                                    int32_t n_hotwords, const int32_t* lang, const int32_t* tn) {
-  return m.sv ? decode_sv(m, wav, stride, lens_h, lang, tn) : decode_batch(m, wav, stride, lens_h, hw_embed, n_hotwords);
+std::unique_ptr<Result> decode_pack(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const std::vector<int32_t>& ext_h,
+                                    const float* hw_embed, int32_t n_hotwords, const int32_t* lang, const int32_t* tn) {
+  // SenseVoice has no CIF predictor: its rows read nothing past their own length
+  return m.sv ? decode_sv(m, wav, stride, lens_h, lang, tn) : decode_batch(m, wav, stride, lens_h, ext_h, hw_embed, n_hotwords);
 }
 
 }  // namespace fa_handle

@@ -315,6 +315,18 @@ int fa_cif_predictor_forward(const FaPredictor* pred, const float* enc, const in
                              int32_t t_max, float* acoustic, int32_t n_cap, int32_t* token_num, float* alphas,
                              float* peaks, int32_t gemm_mode, void* workspace, size_t ws_bytes,
                              fa_stream_t stream);
+/* The same with a padded length per row.  The reference's predictor reads past a row's end: the k = 3 conv at t = len - 1 reads
+ * frame len, and tail_process_fn adds 0.45 * hidden[len] and sums the weights over the whole padded row.  So a row's result depends
+ * on how far its batch was padded.  Row b here behaves exactly as in a batch padded to ext_h[b] frames: encoder frames at or past
+ * ext_h[b] read zero, and token_num sums its ext_h[b] + 1 weights.  lens_h / ext_h [B] are HOST copies of the lengths and the
+ * extents, lens_h[b] <= ext_h[b] <= t_max and ext_h[b] >= 1 (FA_ERR_ARG otherwise, before any device work).  Outputs past
+ * ext_h[b] + 1 in alphas / peaks are not the reference's (it has none).  ext_h[b] == t_max for every row is
+ * fa_cif_predictor_forward bit for bit.  Workspace: fa_cif_predictor_ext_workspace_bytes. */
+size_t fa_cif_predictor_ext_workspace_bytes(int32_t batch, int32_t t_max, int32_t gemm_mode);
+int fa_cif_predictor_forward_ext(const FaPredictor* pred, const float* enc, const int32_t* lens, int32_t batch,
+                                 int32_t t_max, float* acoustic, int32_t n_cap, int32_t* token_num, float* alphas,
+                                 float* peaks, int32_t gemm_mode, void* workspace, size_t ws_bytes,
+                                 fa_stream_t stream, const int32_t* lens_h, const int32_t* ext_h);
 
 /* out[r] = x[r, :n].sum() in fp32 with the summation order of torch's CPU kernel (ATen SumKernel.cpp: 8 SIMD lanes x 4 ILP
  * accumulators, 4-level cascade): the CIF predictor's integer token count is floor(alphas.sum(-1)) (cif_predictor.py:443-444),
@@ -351,6 +363,15 @@ size_t fa_timestamp_head_workspace_bytes(int32_t batch, int32_t t_max, int32_t d
 int fa_timestamp_head_forward(const FaTimestampHead* head, const float* enc, const int32_t* lens, const int32_t* token_num,
                               int32_t batch, int32_t t_max, float* us_alphas, float* us_peaks, int32_t gemm_mode, void* workspace,
                               size_t ws_bytes, fa_stream_t stream);
+/* The same with a padded length per row, as fa_cif_predictor_forward_ext (lens_h / ext_h host arrays, the same refusals).  The
+ * reference's BLSTM runs without packing, so its backward direction starts at the batch's padded end, and alphas2 is summed over the
+ * padded row.  Row b behaves exactly as in a batch padded to ext_h[b] frames: its BLSTM runs fa_blstm_forward_tc_ext with U * ext_h[b]
+ * steps, and the sum covers U * ext_h[b] weights.  Outputs past U * ext_h[b] are not the reference's.  ext_h[b] == t_max for every
+ * row is fa_timestamp_head_forward bit for bit.  Workspace: fa_timestamp_head_ext_workspace_bytes. */
+size_t fa_timestamp_head_ext_workspace_bytes(int32_t batch, int32_t t_max, int32_t d_model, int32_t up_times, int32_t gemm_mode);
+int fa_timestamp_head_forward_ext(const FaTimestampHead* head, const float* enc, const int32_t* lens, const int32_t* token_num,
+                                  int32_t batch, int32_t t_max, float* us_alphas, float* us_peaks, int32_t gemm_mode, void* workspace,
+                                  size_t ws_bytes, fa_stream_t stream, const int32_t* lens_h, const int32_t* ext_h);
 
 /* One-layer bidirectional LSTM recurrence (torch.nn.LSTM(H, H, 1, batch_first=True, bidirectional=True), the `blstm` of
  * CifPredictorV3, bicif_paraformer/cif_predictor.py:187-190) as a persistent weight-stationary kernel: the per-step
@@ -362,6 +383,13 @@ int fa_timestamp_head_forward(const FaTimestampHead* head, const float* enc, con
 size_t fa_blstm_tc_scratch_bytes(int32_t batch);
 int fa_blstm_forward_tc(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, int32_t batch, int32_t t_len,
                         int32_t hidden, float* out, void* scratch, size_t scratch_bytes, fa_stream_t stream);
+/* The same over sequences of their own lengths ext_h[b] (HOST array, 1 <= ext_h[b] <= t_len, FA_ERR_ARG otherwise before any device
+ * work): sequence b equals fa_blstm_forward_tc run on its first ext_h[b] steps alone.  Its backward direction starts at step
+ * ext_h[b] - 1 from a zero state.  Rows t >= ext_h[b] of out are not written.  The launch runs max(ext_h) steps.
+ * scratch >= fa_blstm_tc_ext_scratch_bytes(batch). */
+size_t fa_blstm_tc_ext_scratch_bytes(int32_t batch);
+int fa_blstm_forward_tc_ext(const float* xproj, const float* w_hh_fwd, const float* w_hh_bwd, int32_t batch, int32_t t_len,
+                            int32_t hidden, float* out, void* scratch, size_t scratch_bytes, fa_stream_t stream, const int32_t* ext_h);
 
 /* ParaformerSANMDecoder.forward (decoder.py:397-449) + greedy argmax (paraformer/model.py:642-644).
  *   enc [B,T,512], enc_lens[B]; acoustic [B, ld_acoustic_rows, 512] of which the first n_max rows are used;
@@ -753,10 +781,21 @@ void fa_offline_free_result(void* result);
 void fa_offline_uninit(void* handle);
 const char* fa_offline_last_error(void);
 /* Threads.  Every handle (recogniser, VAD, speaker, punctuation, aligner) may be shared by any number of threads.  A call checks its
- * arguments on the calling thread, then holds the handle's lock for its device work, so calls on one handle run one after another
- * and each gives exactly what it gives alone; calls on different handles run concurrently.  A call that uses several handles
- * (fa_offline_infer_vad*) locks them in the order recogniser, VAD, speaker, so recognisers that share a VAD handle cannot deadlock.
- * fa_offline_last_error is per thread.  Uninit a handle only after every call on it has returned. */
+ * arguments on the calling thread; a malformed call fails there, with its own fa_offline_last_error, before it touches the device.
+ * The recogniser's decoding calls (fa_offline_infer*, fa_offline_infer_vad*) then join the handle's request pool: the thread that
+ * finds no pass running leads one, draining the queued calls that may share GPU packs (in arrival order, up to an hour of padded
+ * audio), decoding them together and waking their threads; the others wait.  The library creates no thread.  Each call still gets
+ * exactly what it gets alone: every row carries the padded length of the batch the reference decodes it in (the call's whole batch;
+ * a long recording's own packs), and the CIF predictor and timestamp head give it what that batch gives it
+ * (fa_cif_predictor_forward_ext).  Calls with hotword rows and diarized calls (fa_offline_infer_vad_spk) pass through the same queue
+ * but never share a pack with another call; long-audio calls share passes only with the same VAD handle and FaLongAudioOptions.
+ * A device failure during a pass fails every call of that pass with its message.  Other handles' calls hold the handle's lock
+ * for their device work and run one after another.  A call that uses several handles (fa_offline_infer_vad*) locks them in the order
+ * recogniser, VAD, speaker, so recognisers that share a VAD handle cannot deadlock.  fa_offline_last_error is per thread.  Uninit a
+ * handle only after every call on it has returned. */
+/* Calls the recogniser handle's pool has decoded since init, and the GPU packs it decoded them in (packs < calls: calls were pooled).
+ * 0, or FA_ERR_ARG for a NULL argument. */
+int fa_offline_pool_stats(const void* handle, int64_t* calls, int64_t* packs);
 
 /* ---------------------------------------------------------------------------------------------
  * Handle-style FSMN-VAD and long-audio recognition (no Python, no torch) — FunASR's `vad_model` path: FsmnVADStreaming.inference

@@ -3,8 +3,9 @@
  * against funasrruntime.h (runtime/websocket, runtime/http, bin/funasr-onnx-offline.cpp) links against libfunasr_b200.so with this
  * header in place of the original for the offline ASR calls it makes.  One handle may be shared by any number of threads, as the
  * reference's servers share it among their decoder threads: FunOfflineInfer / FunOfflineInferBuffer, CompileHotwordEmbedding,
- * FsmnVad* and CTTransformer* are safe on shared handles (funasr_b200.h, "Threads"); calls on one handle take turns on its GPU
- * stream.  thread_num and batch_size stay ignored: segments are packed by "batch-size-s".
+ * FsmnVad* and CTTransformer* are safe on shared handles (funasr_b200.h, "Threads"); FunOfflineInfer* calls from many threads on
+ * one handle are decoded together in shared GPU packs, each giving what it gives alone.  thread_num and batch_size stay ignored:
+ * segments are packed by "batch-size-s".
  * Differences, all at run time, none in the signatures:
  *   model_path["model-dir"] names a directory holding `model.fab2` (funasr_b200/pack.py, written from an unmodified model.pt +
  *   am.mvn) and optionally `tokens.txt` (one token per line; without it results carry the token ids in decimal);
