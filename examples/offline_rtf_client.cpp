@@ -1,8 +1,8 @@
 // The call sequence of FunASR's own throughput client (runtime/onnxruntime/bin/funasr-onnx-offline-rtf.cpp) against this library:
 // one FunOfflineInit handle shared by N threads, each taking the next WAV of a list (FunASRWfstDecoderInit, CompileHotwordEmbedding,
 // one warm-up FunOfflineInfer, then FunOfflineInfer -> FunASRGetResult / FunASRGetRetSnippetTime -> FunASRFreeResult per file), and
-// the real-time factor of the whole run.  Concurrent calls on the one handle take turns under its lock, each giving what it gives
-// alone.
+// the real-time factor of the whole run.  Concurrent calls on the one handle, with or without hotword rows, are pooled into shared GPU
+// batches, each giving what it gives alone.
 // Build (the header can be the reference's own funasrruntime.h: the signatures are identical):
 //   g++ -std=c++17 -pthread -DFUNASR_RUNTIME_HEADER='"funasrruntime_b200.h"' -Iinclude examples/offline_rtf_client.cpp -Lfunasr_b200 -lfunasr_b200
 // usage: offline_rtf_client <model-dir> <wav-list> <thread-num> [vad-model-dir|- [punc-model-dir|- [gemm-mode]]]

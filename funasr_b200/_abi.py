@@ -163,6 +163,9 @@ SIGNATURES = {
     "fa_attention_tc_planes": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _vp]),
     "fa_attention_tc_planes_ex": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _vp]),
     "fa_attention_f32_ex": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _i32, _vp]),
+    "fa_attention_grouped_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32, _i32]),
+    "fa_attention_grouped": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _i32, _vp, _sz,
+                                       _vp]),
     "fa_sanm_encoder_workspace_bytes": (_sz, [_i32, _i32, _i32]),
     "fa_sanm_encoder_forward": (C.c_int, [C.POINTER(FaEncoder), _vp, _vp, _i32, _i32, _vp, _i32, _vp, _sz, _vp]),
     "fa_cif_predictor_workspace_bytes": (_sz, [_i32, _i32, _i32]),
@@ -176,6 +179,12 @@ SIGNATURES = {
     "fa_paraformer_decoder_forward_hidden": (C.c_int, [C.POINTER(FaDecoder), _vp, _vp, _i32, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _i32, _vp, _sz, _vp]),
     "fa_sanm_decoder_stack_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32]),
     "fa_sanm_decoder_stack_forward": (C.c_int, [C.POINTER(FaDecoder), _vp, _vp, _i32, _i32, _i32, _vp, _i64, _vp, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _sz, _vp]),
+    "fa_paraformer_decoder_grouped_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32, _i32, _i32]),
+    "fa_paraformer_decoder_forward_grouped": (C.c_int, [C.POINTER(FaDecoder), _vp, _vp, _i32, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i32, _vp,
+                                                        _vp, _vp, _vp, _i32, _i32, _i32, _vp, _sz, _vp]),
+    "fa_sanm_decoder_stack_grouped_workspace_bytes": (_sz, [_i32, _i32, _i32, _i32, _i32, _i32]),
+    "fa_sanm_decoder_stack_forward_grouped": (C.c_int, [C.POINTER(FaDecoder), _vp, _vp, _vp, _i32, _i32, _i32, _vp, _i64, _vp, _i32, _i32, _i32,
+                                                        _vp, _vp, _vp, _i32, _i32, _vp, _sz, _vp]),
     "fa_linear_argmax_workspace_bytes": (_sz, [_i64, _i32, _i32]),
     "fa_linear_argmax": (C.c_int, [C.POINTER(FaLinear), _vp, _vp, _i64, _vp, _vp, _vp, _i32, _vp, _sz, _vp]),
     "fa_seaco_merge": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),

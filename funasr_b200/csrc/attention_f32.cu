@@ -25,7 +25,7 @@ static_assert(sizeof(PsRow) * ATT_BQ <= sizeof(float) * ATT_D * (ATT_BK + 4), "P
 __global__ void __launch_bounds__(256)
 attention_f32_kernel(const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, int64_t ldk,
                      const float* __restrict__ v, int64_t ldv, const int32_t* __restrict__ key_lens, int tq, int tk,
-                     float* __restrict__ ctx, int64_t ldc, float qscale, int kv_shared) {
+                     float* __restrict__ ctx, int64_t ldc, float qscale, int kv_shared, const int32_t* __restrict__ kv_index) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   AttSmem& s = *reinterpret_cast<AttSmem*>(smem_raw);
   const int b = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * ATT_BQ;
@@ -33,7 +33,7 @@ attention_f32_kernel(const float* __restrict__ q, int64_t ldq, const float* __re
   const int klen = min(key_lens[b], tk);
   PsRow* Ps = reinterpret_cast<PsRow*>(&s.Kt[0][0]);
   const float* qb = q + ((int64_t)b * tq) * ldq + h * ATT_D;
-  const int bkv = kv_shared ? 0 : b;                       // hotword memory: one k / v entry shared by every utterance
+  const int bkv = kv_index ? kv_index[b] : kv_shared ? 0 : b;   // hotword memory: one k / v entry shared by every utterance, or one per group
   const float* kb = k + ((int64_t)bkv * tk) * ldk + h * ATT_D;
   const float* vb = v + ((int64_t)bkv * tk) * ldv + h * ATT_D;
 
@@ -150,7 +150,7 @@ attention_f32_kernel(const float* __restrict__ q, int64_t ldq, const float* __re
 __global__ void __launch_bounds__(128)
 attention_small_kernel(const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, int64_t ldk, const float* __restrict__ v,
                        int64_t ldv, const int32_t* __restrict__ key_lens, int heads, int hd, int tq, int tk, float* __restrict__ ctx,
-                       int64_t ldc, float qscale, int kv_shared, int64_t n_rows) {
+                       int64_t ldc, float qscale, int kv_shared, const int32_t* __restrict__ kv_index, int64_t n_rows) {
   extern __shared__ float s_sc[];                       // [4 warps][tk]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * 4 + warp;   // ((b * heads) + h) * tq + n
@@ -159,7 +159,7 @@ attention_small_kernel(const float* __restrict__ q, int64_t ldq, const float* __
   const int h = (int)((row / tq) % heads);
   const int b = (int)(row / ((int64_t)tq * heads));
   const int klen = min(key_lens[b], tk);
-  const int bkv = kv_shared ? 0 : b;
+  const int bkv = kv_index ? kv_index[b] : kv_shared ? 0 : b;
   const int per = (hd + 31) >> 5;                       // dims per lane (1..4); lane + 32 j < hd holds a dim
   float* sc = s_sc + warp * tk;
   const float* qr = q + ((int64_t)b * tq + n) * ldq + h * hd;
@@ -200,7 +200,7 @@ static int attention_small_launch(const float* q, int64_t ldq, const float* k, i
   if (smem > 48 * 1024) FA_CUDA_OK(cudaFuncSetAttribute(attention_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int64_t rows = (int64_t)s.batch * s.heads * s.tq;
   attention_small_kernel<<<(unsigned)((rows + 3) / 4), 128, smem, st>>>(q, ldq, k, ldk, v, ldv, key_lens, s.heads, s.head_dim, s.tq, s.tk,
-                                                                       out.ctx, out.ldc, attn_qscale(s.head_dim), s.kv_shared ? 1 : 0, rows);
+                                                                       out.ctx, out.ldc, attn_qscale(s.head_dim), s.kv_shared ? 1 : 0, s.kv_index, rows);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }
@@ -212,7 +212,7 @@ static int attention_f32_launch(const float* q, int64_t ldq, const float* k, int
   FA_RETURN_IF_ERR(ensure_dyn_smem(attention_f32_kernel, sizeof(AttSmem), once));
   dim3 grid((s.tq + ATT_BQ - 1) / ATT_BQ, s.heads, s.batch);
   attention_f32_kernel<<<grid, 256, sizeof(AttSmem), st>>>(q, ldq, k, ldk, v, ldv, key_lens, s.tq, s.tk, out.ctx, out.ldc,
-                                                           attn_qscale(ATT_D), s.kv_shared ? 1 : 0);
+                                                           attn_qscale(ATT_D), s.kv_shared ? 1 : 0, s.kv_index);
   FA_CHECK_LAUNCH();
   return FA_OK;
 }

@@ -16,6 +16,7 @@
 #include "tc_common.cuh"
 #include <math.h>
 #include <stdlib.h>
+#include <vector>
 
 namespace fa {
 
@@ -29,6 +30,7 @@ struct AttTcParams {
   int tq, tk, heads, batch;
   float o_scale;                                       // truncation compensation of the P.V accumulation, per k-step (gemm_tc.cu: acc_scale)
   int kv_shared;                                       // 1: every utterance attends over the SAME keys / values (hotword memory): K/V planes hold one batch entry
+  const int32_t* kv_index;                             // or: utterance b attends over K/V entry kv_index[b] (AttnShape)
   const int32_t* key_lens;
   int64_t q_plane_rows, k_plane_rows, v_plane_rows;   // rows between planes in the respective 2D maps
   float* ctx; int64_t ldc;                             // fp32 output (or null)
@@ -71,7 +73,7 @@ attention_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_cons
   }
   __syncthreads();
   const int klen = min(p.key_lens[b], p.tk);
-  const int bkv = p.kv_shared ? 0 : b;
+  const int bkv = p.kv_index ? p.kv_index[b] : p.kv_shared ? 0 : b;
   const int nc = (klen + AT_BKEY - 1) / AT_BKEY;     // key chunks with at least one valid key
 
   if (warp == 0) {
@@ -313,11 +315,11 @@ AttnSinks attn_sinks(const AttnPlanes& p, int q0, int k0, int v0, int width, int
   return s;
 }
 
-// attention_rows' scratch in the tensor-core modes: the planes of a 128-wide head; a shared K / V is one batch entry
-size_t attention_tc_scratch_bytes(int batch, int heads, int tq, int tk, int mode, int kv_shared) {
+// attention_rows' scratch in the tensor-core modes: the planes of a 128-wide head over kv_batch K / V entries
+size_t attention_tc_scratch_bytes(int batch, int heads, int tq, int kv_batch, int tk, int mode) {
   if (mode == FA_GEMM_F32_SIMT) return 0;
   Arena m = Arena::measuring();
-  attn_carve(m, batch, tq, kv_shared ? 1 : batch, tk, heads * AT_D, mode);
+  attn_carve(m, batch, tq, kv_batch, tk, heads * AT_D, mode);
   return m.bytes();
 }
 
@@ -333,7 +335,7 @@ int attention_rows(const float* q, int64_t ldq, const float* k, int64_t ldk, con
   if (!q || !k || !v || !key_lens || s.tk <= 0 || !scratch) return FA_ERR_ARG;
   if ((ldq | ldk | ldv) & 3) return FA_ERR_UNSUPPORTED;
   const int d = s.heads * AT_D;
-  const int kvb = s.kv_shared ? 1 : s.batch;
+  const int kvb = s.kv_entries();
   const int64_t mq = (int64_t)s.batch * s.tq, mk = (int64_t)kvb * s.tk, mv = (int64_t)kvb * d;
   Arena local(scratch->base, scratch->cap);
   const AttnPlanes p = attn_carve(local, s.batch, s.tq, kvb, s.tk, d, mode);
@@ -380,14 +382,14 @@ int attention_planes(const AttnPlanes& pl, const AttnShape& s, const int32_t* ke
   if (!pl.q || !pl.k || !pl.vt || !key_lens || s.tk <= 0) return FA_ERR_ARG;
   const int npl = pl.npl;
   const int d = s.heads * s.head_dim;
-  const int kvb = s.kv_shared ? 1 : s.batch;
+  const int kvb = s.kv_entries();
   const int64_t mq = (int64_t)s.batch * s.tq, mk = (int64_t)kvb * s.tk, mv = (int64_t)kvb * d;
   CUtensorMap mq_map, mk_map, mv_map;
   FA_RETURN_IF_ERR(make_plane_map(&mq_map, pl.q, (uint64_t)mq * npl, (uint64_t)d, (uint64_t)d, AT_BQ));
   FA_RETURN_IF_ERR(make_plane_map(&mk_map, pl.k, (uint64_t)mk * npl, (uint64_t)d, (uint64_t)d, AT_BKEY));
   FA_RETURN_IF_ERR(make_plane_map(&mv_map, pl.vt, (uint64_t)mv * npl, (uint64_t)s.tk, (uint64_t)pl.t_pad, 64));   // 8 KB boxes: 64 d-rows x 64 keys
   AttTcParams p;
-  p.tq = s.tq; p.tk = s.tk; p.heads = s.heads; p.batch = s.batch; p.key_lens = key_lens; p.kv_shared = s.kv_shared ? 1 : 0;
+  p.tq = s.tq; p.tk = s.tk; p.heads = s.heads; p.batch = s.batch; p.key_lens = key_lens; p.kv_shared = s.kv_shared ? 1 : 0; p.kv_index = s.kv_index;
   {
     static const bool rz_on = [] { const char* e = getenv("FA_RZ_COMP"); return !(e && e[0] == '0'); }();
     p.o_scale = rz_on ? (npl > 1 ? 5.3e-8f : 3.4e-8f) : 0.f;                                   // relative shrink per 16-key k-step
@@ -407,7 +409,7 @@ int attention_planes(const AttnPlanes& pl, const AttnShape& s, const int32_t* ke
 
 
 extern "C" size_t fa_attention_tc_workspace_bytes(int32_t batch, int32_t heads, int32_t tq, int32_t tk, int32_t gemm_mode) {
-  return fa::attention_tc_scratch_bytes(batch, heads, tq, tk, gemm_mode, 0);
+  return fa::attention_tc_scratch_bytes(batch, heads, tq, batch, tk, gemm_mode);
 }
 
 extern "C" int fa_attention_tc(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
@@ -418,6 +420,45 @@ extern "C" int fa_attention_tc(const float* q, int64_t ldq, const float* k, int6
   fa::Arena scratch(workspace, ws_bytes);
   return fa::attention_rows(q, ldq, k, ldk, v, ldv, fa::AttnShape{batch, heads, fa::AT_D, tq, tk, 0}, key_lens, fa::AttnOut().to(ctx, ld_ctx),
                             gemm_mode, &scratch, (cudaStream_t)stream);
+}
+
+// utterance b over K / V entry kv_index_h[b]: the index in the workspace's first ints, then attention_rows' planes (tensor-core modes)
+static fa::Arena attn_grouped_carve(fa::Arena& a, int batch, int heads, int tq, int kv_batch, int tk, int mode, int32_t** idx) {
+  *idx = a.take<int32_t>(batch);
+  return a.sub(fa::attention_tc_scratch_bytes(batch, heads, tq, kv_batch, tk, mode));
+}
+
+extern "C" size_t fa_attention_grouped_workspace_bytes(int32_t batch, int32_t heads, int32_t tq, int32_t kv_batch, int32_t tk, int32_t gemm_mode) {
+  if (batch < 1 || heads < 1 || tq < 1 || kv_batch < 1 || tk < 1) return 0;
+  fa::Arena m = fa::Arena::measuring();
+  int32_t* idx;
+  attn_grouped_carve(m, batch, heads, tq, kv_batch, tk, gemm_mode, &idx);
+  return m.bytes();
+}
+
+extern "C" int fa_attention_grouped(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, const int32_t* key_lens,
+                                    const int32_t* kv_index_h, int32_t kv_batch, int32_t batch, int32_t heads, int32_t head_dim, int32_t tq,
+                                    int32_t tk, float* ctx, int64_t ld_ctx, int32_t gemm_mode, void* workspace, size_t ws_bytes,
+                                    fa_stream_t stream) {
+  if (gemm_mode != FA_GEMM_F32_SIMT && gemm_mode != FA_GEMM_F16X1 && gemm_mode != FA_GEMM_F16X3 && gemm_mode != FA_GEMM_F16X6) return FA_ERR_ARG;
+  if (!q || !k || !v || !key_lens || !kv_index_h || !ctx || batch < 1 || heads < 1 || tq < 1 || tk < 1 || kv_batch < 1 || head_dim < 1 ||
+      heads * head_dim > 4096 || ld_ctx < heads * head_dim || (ld_ctx & 3))
+    return FA_ERR_ARG;
+  for (int32_t b = 0; b < batch; ++b)
+    if (kv_index_h[b] < 0 || kv_index_h[b] >= kv_batch) return FA_ERR_ARG;
+  if (gemm_mode != FA_GEMM_F32_SIMT && head_dim != fa::AT_D) return FA_ERR_UNSUPPORTED;
+  fa::Arena a(workspace, ws_bytes);
+  int32_t* idx;
+  fa::Arena scratch = attn_grouped_carve(a, batch, heads, tq, kv_batch, tk, gemm_mode, &idx);
+  if (!a.ok()) return FA_ERR_WORKSPACE;
+  cudaStream_t st = (cudaStream_t)stream;
+  // staged through pageable memory of this frame, which the copy has read when it returns: the caller may reuse kv_index_h at once,
+  // whatever memory it lives in
+  const std::vector<int32_t> staged(kv_index_h, kv_index_h + batch);
+  FA_CUDA_OK(cudaMemcpyAsync(idx, staged.data(), (size_t)batch * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  fa::AttnShape s{batch, heads, head_dim, tq, tk, 0};
+  s.kv_batch = kv_batch; s.kv_index = idx;
+  return fa::attention_rows(q, ldq, k, ldk, v, ldv, s, key_lens, fa::AttnOut().to(ctx, ld_ctx), gemm_mode, &scratch, st);
 }
 
 extern "C" int fa_attention_tc_planes_ex(const void* q_planes, const void* k_planes, const void* vt_planes, const int32_t* key_lens,

@@ -288,15 +288,16 @@ struct Ticket {
   int batch = 0;
   Audio au;
   std::vector<int64_t> n16;                          // 16 kHz samples per buffer
-  const float* hw_embed = nullptr;                   // hotword rows: such a call is never merged with another (solo)
+  const float* hw_embed = nullptr;                   // hotword rows [n_hotwords, 512] on the host
   int32_t n_hotwords = 0;
+  int hw_set = -1;                                   // the pass's index of its hotword rows (identical rows: one set), -1 without
   const int32_t *lang = nullptr, *tn = nullptr;      // SenseVoice queries per buffer (NULL: the defaults)
   bool long_audio = false;                           // fa_offline_infer_vad*: VAD, then packs of each recording's segments
   Vad* vad = nullptr;
   FaLongAudioOptions opts{};
   Spk* spk = nullptr;                                // diarized (solo)
   int32_t preset_spk_num = 0;
-  bool solo() const { return spk || (hw_embed && n_hotwords > 0); }
+  bool solo() const { return spk != nullptr; }
   // written by the pass, read by the owner once done
   std::unique_ptr<Result> res;
   std::string err;
@@ -365,12 +366,21 @@ const int32_t kSvAuto = 0, kSvWoItn = 15;            // SenseVoiceSmall.inferenc
 bool check_hotword_rows(const Model& m, const float* hw_embed, int32_t n_hotwords);
 // every query id inside the embedding table; `what` names the unit ("utterance", "recording")
 bool check_queries(const Model& m, const int32_t* lang, const int32_t* tn, int n, const char* what);
-// one padded batch on the device (wav [B, stride], lens_h >= 400 samples each) decoded by the handle's model kind: the hotword memory
-// reaches a contextual or SeACo Paraformer, the queries (per row, NULL = the defaults) a SenseVoice model.  ext_h [B]: each row's
-// padded length in LFR frames, the t_max of the batch the reference decodes it in (num_lfr_frames(lens_h[b]) <= ext_h[b]); the CIF
-// predictor and the timestamp head give row b exactly what that batch gives it.
+// A GPU pack's hotword rows: its distinct host row sets, and per reference pack (rows the reference decodes as one batch, contiguous
+// in the GPU pack) its first row, row count and set (-1: the call passed none, a SeACo call decoded without biasing)
+struct PackHotwords {
+  std::vector<const float*> rows;                    // per set: [n[s], 512] on the host
+  std::vector<int32_t> n;
+  struct Ref { int first, count, set; };
+  std::vector<Ref> refs;
+};
+// one padded batch on the device (wav [B, stride], lens_h >= 400 samples each) decoded by the handle's model kind: the hotword memories
+// reach a contextual or SeACo Paraformer (hw: NULL or no reference pack with a set = none), the queries (per row, NULL = the defaults)
+// a SenseVoice model.  ext_h [B]: each row's padded length in LFR frames, the t_max of the batch the reference decodes it in
+// (num_lfr_frames(lens_h[b]) <= ext_h[b]); the CIF predictor and the timestamp head give row b exactly what that batch gives it, and
+// each reference pack's hotword biasing is the one the reference gives that batch.
 std::unique_ptr<Result> decode_pack(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const std::vector<int32_t>& ext_h,
-                                    const float* hw_embed, int32_t n_hotwords, const int32_t* lang, const int32_t* tn);
+                                    const PackHotwords* hw, const int32_t* lang, const int32_t* tn);
 // t's call through the recogniser's request pool: queued, decoded by whichever thread leads the pass that drains it -> its result, or
 // nullptr with its own message set as this thread's error
 void* pool_call(Model& m, Ticket& t);

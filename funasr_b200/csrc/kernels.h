@@ -59,8 +59,15 @@ AttnPlanes attn_carve(Arena& a, int batch, int tq, int kv_batch, int tk, int wid
 // The sinks of a GEMM epilogue that writes p: columns [q0, q0+width) -> q (x qscale), [k0, +width) -> k, [v0, +width) -> vt, with
 // t_rows GEMM rows per utterance; a negative start leaves its range off
 AttnSinks attn_sinks(const AttnPlanes& p, int q0, int k0, int v0, int width, int t_rows, float qscale);
-// batch utterances of tq queries over tk keys, heads x head_dim wide; kv_shared: K / V hold ONE batch entry that all attend over
-struct AttnShape { int batch, heads, head_dim, tq, tk, kv_shared; };
+// batch utterances of tq queries over tk keys, heads x head_dim wide.  K / V hold kv_entries() entries of tk keys and utterance b
+// attends over entry kv_index[b] (device, kv_batch entries); without an index, entry 0 when kv_shared (ONE entry that all attend
+// over: hotword memory), else entry b
+struct AttnShape {
+  int batch, heads, head_dim, tq, tk, kv_shared;
+  int kv_batch = 0;
+  const int32_t* kv_index = nullptr;
+  int kv_entries() const { return kv_index ? kv_batch : kv_shared ? 1 : batch; }
+};
 // What an attention call writes: fp32 context rows [B*tq][ldc] and / or fp16 planes [nplanes][B*tq][ldp] (the out-projection's A)
 struct AttnOut {
   float* ctx = nullptr; int64_t ldc = 0;
@@ -74,7 +81,7 @@ int attention_planes(const AttnPlanes& p, const AttnShape& s, const int32_t* key
 // (attention_tc_scratch_bytes; head_dim 128) and attention_planes
 int attention_rows(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, const AttnShape& s,
                    const int32_t* key_lens, const AttnOut& out, int mode, Arena* scratch, cudaStream_t st);
-size_t attention_tc_scratch_bytes(int batch, int heads, int tq, int tk, int mode, int kv_shared);
+size_t attention_tc_scratch_bytes(int batch, int heads, int tq, int kv_batch, int tk, int mode);
 int gemm_tc_planes_launch(const plane_t* a_planes, int64_t M, const FaLinear& lin, const GemmEpi& epi, int mode, cudaStream_t st,
                           int64_t a_ld = 0, int64_t a_plane_rows = 0);
 // a_ld / a_plane_rows (0 = dense: K_pad / M): row pitch of the A planes and rows between planes when A is an overlapping view
@@ -106,5 +113,10 @@ int fbank_unscaled_launch(const float* wav, const int32_t* wav_lens, int batch, 
                           int32_t* feat_lens, int t_max, cudaStream_t st);
 int argmax_lse_launch(float* logits, int64_t rows, int vocab, int64_t ld, int32_t* ids, float* best_logp,
                       int write_log_softmax, cudaStream_t st);
+// fa_sanm_decoder_stack_forward_grouped (finish, no probe) with its per-utterance [key count | memory] rows_d [2 * batch] already on the
+// device (model.cu); its workspace is fa_sanm_decoder_stack_grouped_workspace_bytes(batch, n_groups, t_mem, n_max, 0, mode)
+int sanm_stack_grouped_dev(const FaDecoder* dec, const float* memory, const int32_t* rows_d, int32_t n_groups, int32_t batch, int32_t t_mem,
+                           const float* x, int64_t ld_x_rows, const int32_t* tok_lens, int32_t n_max, int32_t n_run, float* hidden, int32_t gemm_mode,
+                           void* workspace, size_t ws_bytes, cudaStream_t st);
 
 }  // namespace fa

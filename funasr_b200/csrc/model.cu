@@ -373,14 +373,20 @@ extern "C" int fa_timestamp_head_forward_ext(const FaTimestampHead* head, const 
 // (an upper bound when it is shared).  contextual: the bias decoder over n_hotwords rows of hotword memory.  probs: the stack's ASF
 // probe (attn_probs), which its query cannot see, so the stack always carves for it.  On the tensor-core path every layer passes
 // its operands as fp16 planes; fp32 q / k|v / context rows and GEMM scratch serve only the calls that take fp32 operands.
+// The grouped entries: mem_entries memories of t_max rows (0: batch of them), hw_groups hotword memories of n_hotwords rows each, and
+// n_ints ints after the rest (the rows' key counts, memory indices and probed rows, copied from the host), so the other entries'
+// carves are unchanged.
 struct DecBuf {
   float *ya, *yb, *t1, *hq, *f, *qd, *ctx, *kv, *lg, *cat, *kvh;
   plane_t *ctx_planes, *mem_planes, *t1_planes, *hq_planes;
   AttnPlanes att;                     // per-utterance K / V: the stack's query cannot see mem_shared
   Arena scratch{nullptr, 0}, hw_scratch{nullptr, 0};
+  int32_t* ints = nullptr;
 };
-static void dec_carve(Arena& a, DecBuf& b, int batch, int t_max, int n_max, int vocab, int mode, int n_hotwords, bool probs) {
-  const int64_t Mq = (int64_t)batch * n_max, Mk = (int64_t)batch * t_max;
+static void dec_carve(Arena& a, DecBuf& b, int batch, int t_max, int n_max, int vocab, int mode, int n_hotwords, bool probs, int hw_groups = 1,
+                      int mem_entries = 0, int n_ints = 0) {
+  const bool grouped = mem_entries > 0;
+  const int64_t Mq = (int64_t)batch * n_max, Mk = (int64_t)(grouped ? mem_entries : batch) * t_max;
   const bool tc = mode != FA_GEMM_F32_SIMT;
   const bool contextual = n_hotwords > 0;
   const size_t gpl = gemm_planes(mode);
@@ -391,23 +397,26 @@ static void dec_carve(Arena& a, DecBuf& b, int batch, int t_max, int n_max, int 
   b.kv = (!tc || probs) ? a.take<float>(Mk * 1024ull) : nullptr;
   b.lg = a.take<float>(Mq * (size_t)vocab);                          // logits, used when the caller passes none
   b.cat = contextual ? a.take<float>(Mq * 1024ull) : nullptr;         // [x_src_attn ; cx]
-  b.kvh = contextual ? a.take<float>((size_t)n_hotwords * 1024) : nullptr;   // k | v rows of the shared hotword memory
+  b.kvh = contextual ? a.take<float>((size_t)hw_groups * n_hotwords * 1024) : nullptr;   // k | v rows of the hotword memories
   b.ctx_planes = tc ? a.take<plane_t>(gpl * Mq * 512) : nullptr;
   b.mem_planes = tc ? a.take<plane_t>(gpl * Mk * 512) : nullptr;      // split once, reused by every layer's k|v GEMM
   b.t1_planes = tc ? a.take<plane_t>(gpl * Mq * 512) : nullptr;       // LN outputs
   b.hq_planes = tc ? a.take<plane_t>(gpl * Mq * 2048) : nullptr;      // FFN hidden
-  if (tc) b.att = attn_carve(a, batch, n_max, batch, t_max, 512, mode);
+  if (tc) b.att = attn_carve(a, batch, n_max, grouped ? mem_entries : batch, t_max, 512, mode);
   if (tc && (contextual || probs)) {
-    // contextual: bias_q, bias_out (K 512) and bias_output (K 1024) over Mq rows; probs: q of n_max rows, k|v of t_max rows (K 512)
+    // contextual: bias_q, bias_out (K 512) and bias_output (K 1024) over Mq rows; probs: q of n_max rows, k|v of t_max rows (K 512),
+    // grouped: q of every row, k|v of every memory
     const size_t sc = contextual ? gemm_tc_scratch_bytes(Mq, 1024, mode) : 0;
-    const size_t sp = probs ? gemm_tc_scratch_bytes(n_max > t_max ? n_max : t_max, 512, mode) : 0;
+    const size_t sp = !probs ? 0 : grouped ? gemm_tc_scratch_bytes(std::max(Mq, Mk), 512, mode) : gemm_tc_scratch_bytes(n_max > t_max ? n_max : t_max, 512, mode);
     b.scratch = a.sub(sc > sp ? sc : sp);
   }
   if (tc && contextual) {
-    // the hotword k|v GEMM (n_hotwords rows, K 512), then the attention over the shared hotword memory
-    const size_t sg = gemm_tc_scratch_bytes(n_hotwords, 512, mode), sa = attention_tc_scratch_bytes(batch, 4, n_max, n_hotwords, mode, 1);
+    // the hotword k|v GEMM (hw_groups x n_hotwords rows, K 512), then the attention over the hotword memories
+    const size_t sg = gemm_tc_scratch_bytes((int64_t)hw_groups * n_hotwords, 512, mode);
+    const size_t sa = attention_tc_scratch_bytes(batch, 4, n_max, hw_groups, n_hotwords, mode);
     b.hw_scratch = a.sub(sg > sa ? sg : sa);
   }
+  if (n_ints > 0) b.ints = a.take<int32_t>(n_ints);
 }
 
 extern "C" size_t fa_paraformer_decoder_workspace_bytes_hw(int32_t batch, int32_t t_max, int32_t n_max, int32_t vocab,
@@ -442,22 +451,26 @@ static int dec_ffn(const FaDecLayer& L, const float* y, int64_t Mq, float* t1, f
   return gemm_rows(hq, L.ffn_w1.out_f, Mq, L.ffn_w2, GemmEpi().to(f, 512), mode, scratch, st);
 }
 
-// Cross-attention probabilities of ONE utterance (DecoderLayerSANM.get_attn_mat, decoder.py:123-146 ->
-// MultiHeadedAttentionCrossAtt.forward_attention with ret_attn, sanm/attention.py:760-794): probs[h, n, t] =
-// softmax_t( (q[n, h] * d_k^-0.5) . k[t, h] ) with keys t >= klen masked to -inf before and to 0 after the softmax.
-// SeACo's attention-score filtering sums this matrix over heads and tokens on the host exactly like the reference
-// (seaco_paraformer/model.py:325-328), so the matrix itself is the output.  One warp per (head, query); tiny (N x n_hotwords).
+// Cross-attention probabilities of the probed utterances (DecoderLayerSANM.get_attn_mat, decoder.py:123-146 ->
+// MultiHeadedAttentionCrossAtt.forward_attention with ret_attn, sanm/attention.py:760-794): probs[p, h, n, t] =
+// softmax_t( (q[b, n, h] * d_k^-0.5) . k[g, t, h] ) for utterance b = rows[p] (NULL: utterance 0) over memory g = kv_index[b] (NULL:
+// memory 0), with keys t >= key_lens[b] masked to -inf before and to 0 after the softmax.  SeACo's attention-score filtering sums this
+// matrix over heads and tokens on the host exactly like the reference (seaco_paraformer/model.py:325-328), so the matrix itself is the
+// output.  One warp per (probe, head, query); tiny (N x n_hotwords).
 __global__ void __launch_bounds__(128)
 attn_probs_kernel(const float* __restrict__ q, int64_t ldq, const float* __restrict__ k, int64_t ldk, int heads, int n_q, int t_k,
-                  const int32_t* __restrict__ key_lens, float qscale, float* __restrict__ probs) {
+                  const int32_t* __restrict__ key_lens, const int32_t* __restrict__ rows, const int32_t* __restrict__ kv_index, int n_probe,
+                  float qscale, float* __restrict__ probs) {
   extern __shared__ float s_sc[];                       // [4 warps][t_k]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int row = blockIdx.x * 4 + warp;                // h * n_q + n
-  if (row >= heads * n_q) return;
-  const int h = row / n_q, n = row - h * n_q;
-  const int klen = min(key_lens[0], t_k);                // utterance 0's key count
+  const int row = blockIdx.x * 4 + warp;                // (p * heads + h) * n_q + n
+  if (row >= n_probe * heads * n_q) return;
+  const int n = row % n_q, h = (row / n_q) % heads, p = row / (n_q * heads);
+  const int b = rows ? rows[p] : 0;
+  const int klen = min(key_lens[b], t_k);
   float* sc = s_sc + warp * t_k;
-  const float* qr = q + (int64_t)n * ldq + h * 128;
+  const float* qr = q + ((int64_t)b * n_q + n) * ldq + h * 128;
+  k += (int64_t)(kv_index ? kv_index[b] : 0) * t_k * ldk;
   float qv[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) qv[j] = __fmul_rn(qr[lane + 32 * j], qscale);
@@ -486,21 +499,26 @@ static const size_t kAttnProbsMaxSmem = 96 * 1024;
 
 // One run of a SAN-M decoder stack over a cross-attention memory.  memory [mem_batch * t_mem, 512] with mem_batch = batch, or 1
 // when mem_shared (the SeACo / contextual hotword memory: every utterance attends over the same rows — one k/v projection, one
-// copy).  tgt [batch, n_max, 512] lives in b.ya on entry.
+// copy), or mem_entries when utterance b attends over memory kv_index[b] (device).  tgt [batch, n_max, 512] lives in b.ya on entry.
+// The ASF probe reads utterances probe_rows[0 .. n_probe) (device; NULL: utterance 0).
 struct DecRun {
   int batch, n_max, t_mem, heads, fsmn_k, mode, mem_shared;
   const float* memory; const int32_t* mem_lens; const int32_t* tok_lens;
   cudaStream_t st;
   DecBuf* b; Arena* scratch;
+  int mem_entries = 0;
+  const int32_t* kv_index = nullptr;
+  const int32_t* probe_rows = nullptr;
+  int n_probe = 1;
   int64_t Mq() const { return (int64_t)batch * n_max; }
-  int64_t Mk() const { return (int64_t)(mem_shared ? 1 : batch) * t_mem; }
+  int64_t Mk() const { return (int64_t)(kv_index ? mem_entries : mem_shared ? 1 : batch) * t_mem; }
 };
 
 // One attention decoder layer (DecoderLayerSANM.forward, paraformer/decoder.py:78-121).  *x_self_out receives `residual +
 // fsmn(...)` (x_self_attn); if src_out != nullptr the cross-attention output is written there WITHOUT the residual (x_src_attn,
 // leading dim ld_src) and *y_next is not produced — the ContextualDecoderLayer contract (contextual_paraformer/decoder.py:60-100).
-// attn_probs != nullptr: stop at the cross-attention and write utterance 0's probability matrix [heads, n_max, t_mem] instead
-// (get_attn_mat, decoder.py:123-146).
+// attn_probs != nullptr: stop at the cross-attention and write the probed utterances' probability matrices [n_probe, heads, n_max,
+// t_mem] instead (get_attn_mat, decoder.py:123-146).
 static int dec_attention_layer(const DecRun& r, const FaDecLayer& L, float* yin, float** x_self_out, float* src_out, int64_t ld_src,
                                float** y_next, float* attn_probs) {
   DecBuf& b = *r.b;
@@ -508,7 +526,8 @@ static int dec_attention_layer(const DecRun& r, const FaDecLayer& L, float* yin,
   const int64_t Mq = r.Mq(), Mk = r.Mk();
   const bool tc = r.mode != FA_GEMM_F32_SIMT;
   const int npl = gemm_planes(r.mode);
-  const AttnShape shape{r.batch, r.heads, 128, r.n_max, r.t_mem, r.mem_shared};
+  AttnShape shape{r.batch, r.heads, 128, r.n_max, r.t_mem, r.mem_shared};
+  shape.kv_batch = r.mem_entries; shape.kv_index = r.kv_index;
   cudaStream_t st = r.st;
   FA_RETURN_IF_ERR(dec_ffn(L, yin, Mq, b.t1, b.hq, b.f, r.mode, r.scratch, st, b.t1_planes, b.hq_planes));
   // x = residual + fsmn(LN2(f), tgt_mask)     decoder.py:103-107
@@ -517,15 +536,17 @@ static int dec_attention_layer(const DecRun& r, const FaDecLayer& L, float* yin,
   FA_RETURN_IF_ERR(fsmn_launch(b.t1, D, r.tok_lens, r.batch, r.n_max, D, L.fsmn_w, r.fsmn_k, yin, D, x2, D, st));
   *x_self_out = x2;
   if (attn_probs) {
-    // q / k in fp32 through the mode's GEMM; only utterance 0's rows are needed (seaco_paraformer/model.py:325: hotword_scores[0])
-    FA_RETURN_IF_ERR(layernorm_launch(x2, r.n_max, L.norm3, b.t1, nullptr, 1.f, 1, st));
-    FA_RETURN_IF_ERR(gemm_rows(b.t1, D, r.n_max, L.q, GemmEpi().to(b.qd, D), r.mode, r.scratch, st));
-    FA_RETURN_IF_ERR(gemm_rows(r.memory, D, r.t_mem, L.kv, GemmEpi().to(b.kv, 2 * D), r.mode, r.scratch, st));
-    const int rows = r.heads * r.n_max;
+    // q / k in fp32 through the mode's GEMM; only utterance 0's rows are needed (seaco_paraformer/model.py:325: hotword_scores[0]),
+    // or with a probe list every utterance's rows over every memory
+    const int64_t mq = r.probe_rows ? Mq : r.n_max, mk = r.kv_index ? Mk : r.t_mem;
+    FA_RETURN_IF_ERR(layernorm_launch(x2, mq, L.norm3, b.t1, nullptr, 1.f, 1, st));
+    FA_RETURN_IF_ERR(gemm_rows(b.t1, D, mq, L.q, GemmEpi().to(b.qd, D), r.mode, r.scratch, st));
+    FA_RETURN_IF_ERR(gemm_rows(r.memory, D, mk, L.kv, GemmEpi().to(b.kv, 2 * D), r.mode, r.scratch, st));
+    const int rows = r.n_probe * r.heads * r.n_max;
     const size_t smem = attn_probs_smem(r.t_mem);              // <= kAttnProbsMaxSmem: checked by the entry point
     if (smem > 48 * 1024) FA_CUDA_OK(cudaFuncSetAttribute(attn_probs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attn_probs_kernel<<<(rows + 3) / 4, 128, smem, st>>>(b.qd, D, b.kv, 2 * D, r.heads, r.n_max, r.t_mem, r.mem_lens,
-                                                         attn_qscale(shape.head_dim), attn_probs);
+    attn_probs_kernel<<<(rows + 3) / 4, 128, smem, st>>>(b.qd, D, b.kv, 2 * D, r.heads, r.n_max, r.t_mem, r.mem_lens, r.probe_rows, r.kv_index,
+                                                         r.n_probe, attn_qscale(shape.head_dim), attn_probs);
     FA_CHECK_LAUNCH();
     return FA_OK;
   }
@@ -565,10 +586,17 @@ static int dec_finish(const DecRun& r, const FaDecoder* dec, float* y, float* hi
   return layernorm_launch(b.f, r.Mq(), dec->after_norm, hidden_out ? hidden_out : b.t1, nullptr, 1.f, 1, r.st);
 }
 
+// The contextual decoder's hotword memories: groups x nh_max rows of 512 (device); per utterance its key count and its memory (device;
+// index NULL: memory 0).  rows_h (host, grouped entry only): [lens | index] per utterance, copied into the workspace.
+struct HwMem {
+  const float* embed; const int32_t* lens; const int32_t* index; int groups, nh_max;
+  const int32_t* rows_h = nullptr;
+};
+
 static int decoder_forward_impl(const FaDecoder* dec, const float* enc, const int32_t* enc_lens, int32_t batch, int32_t t_max,
                                 const float* acoustic, int64_t ld_acoustic_rows, const int32_t* tok_lens, int32_t n_max,
                                 int32_t* argmax_ids, float* argmax_logp, float* logits, int32_t log_softmax, float* hidden_out,
-                                int32_t gemm_mode, void* workspace, size_t ws_bytes, fa_stream_t stream) {
+                                int32_t gemm_mode, void* workspace, size_t ws_bytes, fa_stream_t stream, const HwMem* grouped = nullptr) {
   if (!dec || !enc || !enc_lens || !acoustic || !tok_lens || !argmax_ids || !argmax_logp || batch <= 0 || t_max <= 0 ||
       n_max <= 0 || ld_acoustic_rows < n_max)
     return FA_ERR_ARG;
@@ -579,15 +607,19 @@ static int decoder_forward_impl(const FaDecoder* dec, const float* enc, const in
   const int V = dec->vocab;
   const bool tc = gemm_mode != FA_GEMM_F32_SIMT;
   const bool contextual = dec->has_bias != 0;
-  const int nh = dec->n_hotwords;
-  if (contextual && (!dec->hw_embed || !dec->hw_lens || nh <= 0 || dec->clas_scale != 1.0f)) return FA_ERR_UNSUPPORTED;
+  HwMem hw = grouped ? *grouped : HwMem{dec->hw_embed, dec->hw_lens, nullptr, 1, dec->n_hotwords};
+  if (contextual && (!hw.embed || (!grouped && !hw.lens) || hw.nh_max <= 0 || dec->clas_scale != 1.0f)) return FA_ERR_UNSUPPORTED;
   for (int l = 0; l < dec->n_layers; ++l) FA_RETURN_IF_ERR(dec_ffn_check(dec->layers[l], gemm_mode));   // nothing enqueued on a refusal
   if (contextual) FA_RETURN_IF_ERR(dec_ffn_check(dec->bias_last, gemm_mode));
   FA_RETURN_IF_ERR(dec_ffn_check(dec->last, gemm_mode));
   Arena a(workspace, ws_bytes);
   DecBuf b;
-  dec_carve(a, b, batch, t_max, n_max, V, gemm_mode, contextual ? nh : 0, false);
+  dec_carve(a, b, batch, t_max, n_max, V, gemm_mode, contextual ? hw.nh_max : 0, false, hw.groups, 0, grouped ? 2 * batch : 0);
   if (!a.ok()) return FA_ERR_WORKSPACE;
+  if (grouped) {
+    FA_CUDA_OK(cudaMemcpyAsync(b.ints, hw.rows_h, (size_t)2 * batch * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    hw.lens = b.ints; hw.index = b.ints + batch;
+  }
   const int npl = gemm_planes(gemm_mode);
   float* lg = logits ? logits : b.lg;
   if (tc) FA_RETURN_IF_ERR(split_rows_launch(enc, D, Mk, D, D, npl, b.mem_planes, st));   // memory is layer-invariant
@@ -609,12 +641,13 @@ static int decoder_forward_impl(const FaDecoder* dec, const float* enc, const in
     // bias decoder: cross attention of LN3(x_self_attn) over the hotword memory (identical for every utterance)
     FA_RETURN_IF_ERR(layernorm_launch(x_self, Mq, dec->bias_norm3, b.t1, nullptr, 1.f, 1, st));
     FA_RETURN_IF_ERR(gemm_rows(b.t1, D, Mq, dec->bias_q, GemmEpi().to(b.qd, D), gemm_mode, &b.scratch, st));
-    // the hotword k | v rows [nh, 1024] are the same for every utterance: one copy, attended with kv_shared (no per-utterance
-    // replication, so the hotword count is independent of t_max)
+    // the hotword k | v rows [groups, nh_max, 1024]: one copy per memory (no per-utterance replication, so the hotword count is
+    // independent of t_max), each utterance attending over its own; one memory is the kv_shared case
     float* kvh = b.kvh;
-    FA_RETURN_IF_ERR(gemm_rows(dec->hw_embed, D, nh, dec->bias_kv, GemmEpi().to(kvh, 2 * D), gemm_mode, &b.hw_scratch, st));
-    FA_RETURN_IF_ERR(attention_rows(b.qd, D, kvh, 2 * D, kvh + D, 2 * D, AttnShape{batch, dec->heads, 128, n_max, nh, 1}, dec->hw_lens,
-                                    AttnOut().to(b.ctx, D), gemm_mode, &b.hw_scratch, st));
+    FA_RETURN_IF_ERR(gemm_rows(hw.embed, D, (int64_t)hw.groups * hw.nh_max, dec->bias_kv, GemmEpi().to(kvh, 2 * D), gemm_mode, &b.hw_scratch, st));
+    AttnShape hs{batch, dec->heads, 128, n_max, hw.nh_max, 1};
+    hs.kv_batch = hw.groups; hs.kv_index = hw.index;
+    FA_RETURN_IF_ERR(attention_rows(b.qd, D, kvh, 2 * D, kvh + D, 2 * D, hs, hw.lens, AttnOut().to(b.ctx, D), gemm_mode, &b.hw_scratch, st));
     FA_RETURN_IF_ERR(gemm_rows(b.ctx, D, Mq, dec->bias_out, GemmEpi().to(b.cat + D, 2 * D), gemm_mode, &b.scratch, st));   // cat[:, 512:] = cx
     float* y2 = (x_self == b.ya) ? b.yb : b.ya;
     FA_RETURN_IF_ERR(gemm_rows(b.cat, 2 * D, Mq, dec->bias_output, GemmEpi().add(x_self, D).to(y2, D), gemm_mode, &b.scratch, st));
@@ -651,6 +684,42 @@ extern "C" int fa_paraformer_decoder_forward_hidden(const FaDecoder* dec, const 
                               logits, log_softmax, hidden, gemm_mode, workspace, ws_bytes, stream);
 }
 
+// rows_h [2 * batch] = [key count | memory] per utterance from lens_h [groups] and group_h [batch] (host), every group's length in
+// [1, nh_max] and every utterance's group in [0, groups); false: a refusal
+static bool hw_rows_host(const int32_t* lens_h, const int32_t* group_h, int32_t groups, int32_t nh_max, int32_t batch, std::vector<int32_t>& rows_h) {
+  if (!lens_h || !group_h || groups < 1 || nh_max < 1 || batch < 1) return false;
+  for (int32_t g = 0; g < groups; ++g)
+    if (lens_h[g] < 1 || lens_h[g] > nh_max) return false;
+  rows_h.resize((size_t)2 * batch);
+  for (int32_t b = 0; b < batch; ++b) {
+    if (group_h[b] < 0 || group_h[b] >= groups) return false;
+    rows_h[b] = lens_h[group_h[b]];
+    rows_h[batch + b] = group_h[b];
+  }
+  return true;
+}
+
+extern "C" size_t fa_paraformer_decoder_grouped_workspace_bytes(int32_t batch, int32_t t_max, int32_t n_max, int32_t vocab, int32_t gemm_mode,
+                                                                int32_t n_groups, int32_t nh_max) {
+  if (batch < 1 || n_groups < 1 || nh_max < 1) return 0;
+  Arena m = Arena::measuring();
+  DecBuf b;
+  dec_carve(m, b, batch, t_max, n_max, vocab, gemm_mode, nh_max, false, n_groups, 0, 2 * batch);
+  return m.bytes();
+}
+
+extern "C" int fa_paraformer_decoder_forward_grouped(const FaDecoder* dec, const float* enc, const int32_t* enc_lens, int32_t batch, int32_t t_max,
+                                                     const float* acoustic, int64_t ld_acoustic_rows, const int32_t* tok_lens, int32_t n_max,
+                                                     int32_t* argmax_ids, float* argmax_logp, float* logits, int32_t log_softmax, float* hidden,
+                                                     const float* hw_embed, const int32_t* hw_lens_h, const int32_t* row_group_h, int32_t n_groups,
+                                                     int32_t nh_max, int32_t gemm_mode, void* workspace, size_t ws_bytes, fa_stream_t stream) {
+  std::vector<int32_t> rows_h;
+  if (!dec || !dec->has_bias || !hw_embed || !hw_rows_host(hw_lens_h, row_group_h, n_groups, nh_max, batch, rows_h)) return FA_ERR_ARG;
+  HwMem hw{hw_embed, nullptr, nullptr, n_groups, nh_max, rows_h.data()};
+  return decoder_forward_impl(dec, enc, enc_lens, batch, t_max, acoustic, ld_acoustic_rows, tok_lens, n_max, argmax_ids, argmax_logp,
+                              logits, log_softmax, hidden, gemm_mode, workspace, ws_bytes, stream, &hw);
+}
+
 // A SAN-M decoder stack WITHOUT input / output layer over an arbitrary memory — the SeACo decoder of SeacoParaformer
 // (seaco_paraformer/model.py:100-110: ParaformerSANMDecoder(use_output_layer=False, wo_input_layer=True), FFN 1024, FSMN k = 21,
 // 6 attention layers) attending over the hotword embeddings.  mem_shared != 0: memory is [t_mem, 512], the same for every
@@ -665,12 +734,14 @@ extern "C" size_t fa_sanm_decoder_stack_workspace_bytes(int32_t batch, int32_t t
   return m.bytes();
 }
 
-extern "C" int fa_sanm_decoder_stack_forward(const FaDecoder* dec, const float* memory, const int32_t* mem_lens, int32_t mem_shared,
-                                             int32_t batch, int32_t t_mem, const float* x, int64_t ld_x_rows,
-                                             const int32_t* tok_lens, int32_t n_max, int32_t n_run, int32_t finish, float* hidden,
-                                             float* attn_probs, int32_t gemm_mode, void* workspace, size_t ws_bytes,
-                                             fa_stream_t stream) {
-  if (!dec || !memory || !mem_lens || !x || !tok_lens || batch <= 0 || t_mem <= 0 || n_max <= 0 || ld_x_rows < n_max || n_run < 0 ||
+// The grouped stack's memories: groups of t_mem rows; ints_h (host) = [key count | memory] per utterance, then the probed utterances,
+// copied into the workspace; or ints_d, the same already on the device (no copy)
+struct StackGroups { int groups, n_probe; const int32_t* ints_h; const int32_t* ints_d = nullptr; };
+
+static int stack_forward(const FaDecoder* dec, const float* memory, const int32_t* mem_lens, int32_t mem_shared, int32_t batch, int32_t t_mem,
+                         const float* x, int64_t ld_x_rows, const int32_t* tok_lens, int32_t n_max, int32_t n_run, int32_t finish, float* hidden,
+                         float* attn_probs, int32_t gemm_mode, void* workspace, size_t ws_bytes, fa_stream_t stream, const StackGroups* grouped) {
+  if (!dec || !memory || (!grouped && !mem_lens) || !x || !tok_lens || batch <= 0 || t_mem <= 0 || n_max <= 0 || ld_x_rows < n_max || n_run < 0 ||
       n_run > dec->n_layers || (!hidden && !attn_probs) || (attn_probs && n_run < 1))
     return FA_ERR_ARG;
   cudaStream_t st = (cudaStream_t)stream;
@@ -679,12 +750,22 @@ extern "C" int fa_sanm_decoder_stack_forward(const FaDecoder* dec, const float* 
   for (int l = 0; l < n_run; ++l) FA_RETURN_IF_ERR(dec_ffn_check(dec->layers[l], gemm_mode));   // nothing enqueued on a refusal
   if (!attn_probs && finish) FA_RETURN_IF_ERR(dec_ffn_check(dec->last, gemm_mode));
   if (attn_probs && attn_probs_smem(t_mem) > kAttnProbsMaxSmem) return FA_ERR_UNSUPPORTED;
+  const int n_ints = grouped ? 2 * batch + grouped->n_probe : 0;
   Arena a(workspace, ws_bytes);
   DecBuf b;
-  dec_carve(a, b, batch, t_mem, n_max, 0, gemm_mode, 0, true);
+  dec_carve(a, b, batch, t_mem, n_max, 0, gemm_mode, 0, true, 1, grouped ? grouped->groups : 0, n_ints);
   if (!a.ok()) return FA_ERR_WORKSPACE;
   const bool tc = gemm_mode != FA_GEMM_F32_SIMT;
   DecRun r{batch, n_max, t_mem, dec->heads, dec->fsmn_k, gemm_mode, mem_shared ? 1 : 0, memory, mem_lens, tok_lens, st, &b, &b.scratch};
+  if (grouped) {
+    const int32_t* ints = grouped->ints_d;
+    if (!ints) {
+      FA_CUDA_OK(cudaMemcpyAsync(b.ints, grouped->ints_h, (size_t)n_ints * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+      ints = b.ints;
+    }
+    r.mem_lens = ints; r.kv_index = ints + batch; r.mem_entries = grouped->groups;
+    r.probe_rows = ints + 2 * batch; r.n_probe = grouped->n_probe;
+  }
   if (tc) FA_RETURN_IF_ERR(split_rows_launch(memory, D, r.Mk(), D, D, gemm_planes(gemm_mode), b.mem_planes, st));
   FA_CUDA_OK(cudaMemcpy2DAsync(b.ya, (size_t)n_max * D * 4, x, (size_t)ld_x_rows * D * 4, (size_t)n_max * D * 4, batch,
                                cudaMemcpyDeviceToDevice, st));
@@ -700,6 +781,56 @@ extern "C" int fa_sanm_decoder_stack_forward(const FaDecoder* dec, const float* 
   FA_CUDA_OK(cudaMemcpyAsync(hidden, y, (size_t)r.Mq() * D * 4, cudaMemcpyDeviceToDevice, st));
   fa::count_launch();
   return FA_OK;
+}
+
+extern "C" int fa_sanm_decoder_stack_forward(const FaDecoder* dec, const float* memory, const int32_t* mem_lens, int32_t mem_shared,
+                                             int32_t batch, int32_t t_mem, const float* x, int64_t ld_x_rows,
+                                             const int32_t* tok_lens, int32_t n_max, int32_t n_run, int32_t finish, float* hidden,
+                                             float* attn_probs, int32_t gemm_mode, void* workspace, size_t ws_bytes,
+                                             fa_stream_t stream) {
+  return stack_forward(dec, memory, mem_lens, mem_shared, batch, t_mem, x, ld_x_rows, tok_lens, n_max, n_run, finish, hidden, attn_probs,
+                       gemm_mode, workspace, ws_bytes, stream, nullptr);
+}
+
+namespace fa {
+// fa_sanm_decoder_stack_forward_grouped without a probe, its per-utterance [key count | memory] already on the device (rows_d [2 * batch],
+// checked by the caller): a caller that uploads them with its memories saves a host-to-device copy between two stacks
+int sanm_stack_grouped_dev(const FaDecoder* dec, const float* memory, const int32_t* rows_d, int32_t n_groups, int32_t batch, int32_t t_mem,
+                           const float* x, int64_t ld_x_rows, const int32_t* tok_lens, int32_t n_max, int32_t n_run, float* hidden, int32_t gemm_mode,
+                           void* workspace, size_t ws_bytes, cudaStream_t st) {
+  if (!rows_d || n_groups < 1 || !hidden) return FA_ERR_ARG;
+  StackGroups g{n_groups, 0, nullptr};
+  g.ints_d = rows_d;
+  return stack_forward(dec, memory, nullptr, 0, batch, t_mem, x, ld_x_rows, tok_lens, n_max, n_run, 1, hidden, nullptr, gemm_mode, workspace,
+                       ws_bytes, (fa_stream_t)st, &g);
+}
+}  // namespace fa
+
+extern "C" size_t fa_sanm_decoder_stack_grouped_workspace_bytes(int32_t batch, int32_t n_groups, int32_t t_mem, int32_t n_max, int32_t n_probe,
+                                                                int32_t gemm_mode) {
+  if (batch < 1 || n_groups < 1 || t_mem < 1 || n_probe < 0) return 0;
+  Arena m = Arena::measuring();
+  DecBuf b;
+  dec_carve(m, b, batch, t_mem, n_max, 0, gemm_mode, 0, true, 1, n_groups, 2 * batch + n_probe);
+  return m.bytes();
+}
+
+extern "C" int fa_sanm_decoder_stack_forward_grouped(const FaDecoder* dec, const float* memory, const int32_t* mem_lens_h, const int32_t* row_group_h,
+                                                     int32_t n_groups, int32_t batch, int32_t t_mem, const float* x, int64_t ld_x_rows,
+                                                     const int32_t* tok_lens, int32_t n_max, int32_t n_run, int32_t finish, float* hidden,
+                                                     float* attn_probs, const int32_t* probe_rows_h, int32_t n_probe, int32_t gemm_mode,
+                                                     void* workspace, size_t ws_bytes, fa_stream_t stream) {
+  std::vector<int32_t> ints;
+  if (!hw_rows_host(mem_lens_h, row_group_h, n_groups, t_mem, batch, ints)) return FA_ERR_ARG;
+  if (attn_probs && (!probe_rows_h || n_probe < 1)) return FA_ERR_ARG;
+  if (!attn_probs) n_probe = 0;
+  for (int32_t p = 0; p < n_probe; ++p) {
+    if (probe_rows_h[p] < 0 || probe_rows_h[p] >= batch) return FA_ERR_ARG;
+    ints.push_back(probe_rows_h[p]);
+  }
+  const StackGroups g{n_groups, n_probe, ints.data()};
+  return stack_forward(dec, memory, nullptr, 0, batch, t_mem, x, ld_x_rows, tok_lens, n_max, n_run, finish, hidden, attn_probs, gemm_mode,
+                       workspace, ws_bytes, stream, &g);
 }
 
 // SeACo merge (seaco_paraformer/model.py:357-378 with seaco_weight = 1): per token row, if argmax(dha_pred) == NO_BIAS keep the

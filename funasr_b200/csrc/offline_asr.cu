@@ -15,6 +15,7 @@
 // Long audio (VAD segments decoded in packs) is offline_long.cu.  The tokenizer (ids -> text) stays with the caller, like every other
 // entry point of this ABI.
 #include "handle.h"
+#include "kernels.h"
 
 using namespace fa_handle;
 
@@ -81,7 +82,7 @@ bool build_paraformer(Model& m, Builder& b) {
   m.dec.fsmn_k = dk && dk->shape.size() == 3 ? (int)dk->shape[2] : m.kernel;
   dec_layer(m.dec.last, "decoder.decoders3.0", false);
   m.dec.after_norm = b.norm("decoder.after_norm"); m.dec.output = b.lin("decoder.output_layer");
-  m.dec.has_bias = 0;
+  m.dec.has_bias = m.contextual ? 1 : 0;                    // its hotword memories come with each pack (decode_batch)
   if (m.contextual) {
     dec_layer(m.dec.bias_last, "decoder.last_decoder", true);
     m.dec.bias_norm3 = b.norm("decoder.bias_decoder.norm3");
@@ -147,64 +148,169 @@ bool build_paraformer(Model& m, Builder& b) {
 }
 
 // SeACo's hotword biasing after the decoder (_seaco_decode_with_ASF, seaco_paraformer/model.py:271-382, as ParaformerEngine.seaco_decode
-// runs it): the host hotword rows hw_host [n_hw, 512] on the device; with more rows than nfilter, the attention-score filter on
-// utterance 0 (one host round trip: its probabilities out, fa_seaco_asf_select_host, the picked host rows back in); the SeACo decoder
-// over the acoustic embeddings and over the decoder's hidden states; hotword_output_layer's arg-max over their sum; the NO_BIAS merge
-// of the decoder's ids / best into *sids.  The workspace is sized for the stack and the arg-max.
-bool seaco_bias(Model& m, int B, int n_max, int n_cap, const float* hw_host, int n_hw, const float* acoustic, const float* hidden,
-                const int32_t* tok, const int32_t* ids, const float* best, int32_t** sids) {
+// runs it) for every reference pack of a GPU pack.  The reference gives each of its batches one hotword memory: the batch's rows, or
+// with more rows than nfilter the ones the attention-score filter (ASF) picks on the batch's utterance 0 over the batch's n_max query
+// rows.  SeacoPlan lays out the pack's memories from the host token counts; seaco_bias runs them.
+struct SeacoPlan {
+  std::vector<int> probe;                            // the reference packs the ASF runs on, and their n_max
+  std::vector<int32_t> probe_nmax;
+  std::vector<int> probe_set;                        // the distinct sets they filter, and per probe its index there
+  std::vector<int32_t> probe_group;
+  int probe_nmax_all = 0, probe_rows = 0;            // the probe's query rows and memory length
+  int groups = 0, rows_ub = 0;                       // the final memories and an upper bound of their length
+  bool any = false;                                  // some reference pack has hotword rows
+};
+
+SeacoPlan seaco_plan(const Model& m, const PackHotwords& hw, const std::vector<int32_t>& tok_h) {
+  SeacoPlan p;
+  std::vector<char> plain_used(hw.n.size(), 0);
+  for (const PackHotwords::Ref& r : hw.refs) {
+    if (r.set < 0) continue;
+    p.any = true;
+    int nmax = 0;
+    for (int i = r.first; i < r.first + r.count; ++i) nmax = std::max(nmax, tok_h[i]);
+    const int n = hw.n[r.set];
+    if (m.nfilter > 0 && m.nfilter < n && nmax > 0) {          // a batch without a token is never decoded (paraformer/model.py:615)
+      const int k = (int)(std::find(p.probe_set.begin(), p.probe_set.end(), r.set) - p.probe_set.begin());
+      if (k == (int)p.probe_set.size()) p.probe_set.push_back(r.set);
+      p.probe.push_back((int)(&r - hw.refs.data()));
+      p.probe_nmax.push_back(nmax);
+      p.probe_group.push_back(k);
+      p.probe_nmax_all = std::max(p.probe_nmax_all, nmax);
+      p.probe_rows = std::max(p.probe_rows, n);
+      ++p.groups;
+      p.rows_ub = std::max(p.rows_ub, m.nfilter + 1);          // fa_seaco_asf_select_host keeps nfilter rows and <s>
+    } else if (!plain_used[r.set]) {
+      plain_used[r.set] = 1;
+      ++p.groups;
+      p.rows_ub = std::max(p.rows_ub, n);
+    }
+  }
+  return p;
+}
+
+// The plan's memories over the GPU pack [B, n_max]: the ASF probes in one batched forward (the first row of each filtered reference pack,
+// gathered, each against its own set), one host round trip, each pack's [heads, n_max_ref, n] block cut out for fa_seaco_asf_select_host,
+// one upload of every memory; then the SeACo decoder over the acoustic embeddings and over the decoder's hidden states, each row against
+// its reference pack's memory; hotword_output_layer's arg-max over their sum; the NO_BIAS merge of the decoder's ids / best into *sids.
+// Rows of a reference pack without rows keep the decoder's ids (model.py:381-382).  The workspace is sized for every stage by the caller.
+bool seaco_bias(Model& m, const SeacoPlan& plan, const PackHotwords& hw, const std::vector<int32_t>& tok_h, int B, int n_max, int n_cap,
+                const float* acoustic, const float* hidden, const int32_t* tok, const int32_t* ids, const float* best, int32_t** sids) {
   cudaStream_t st = m.file.st;
   const int D = m.d_model, V = m.vocab, n_s = m.seaco_dec.n_layers, H = m.seaco_dec.heads;
   const int64_t rows = (int64_t)B * n_max;
-  const bool asf = m.nfilter > 0 && m.nfilter < n_hw;       // ASF (model.py:320-343): forward_asf6 on utterance 0
-  float *mem, *cif_att, *dec_att, *dha_best, *sbest, *probs = nullptr;
-  int32_t *dha_ids, *mem_lens;
+  const int R = (int)plan.probe.size(), Gp = (int)plan.probe_set.size(), NP = plan.probe_rows, QP = plan.probe_nmax_all;
+  const int G = plan.groups, NU = plan.rows_ub;
+  float *mem, *cif_att, *dec_att, *dha_best, *sbest, *probs = nullptr, *mem_p = nullptr, *hx = nullptr;
+  int32_t *dha_ids, *tok_p = nullptr, *rows_f;
   if (!carve(m.seaco_bias, "SeACo", [&](fa::Arena& a) {
-        mem = a.take<float>((size_t)n_hw * D);
+        mem = a.take<float>((size_t)G * NU * D);
         cif_att = a.take<float>((size_t)rows * D); dec_att = a.take<float>((size_t)rows * D);
         dha_ids = a.take<int32_t>(rows); dha_best = a.take<float>(rows);
         *sids = a.take<int32_t>(rows); sbest = a.take<float>(rows);
-        mem_lens = a.take<int32_t>(B);
-        if (asf) probs = a.take<float>((size_t)H * n_max * n_hw);
+        rows_f = a.take<int32_t>((size_t)2 * B);
+        if (R > 0) {
+          mem_p = a.take<float>((size_t)Gp * NP * D); hx = a.take<float>((size_t)R * n_max * D); tok_p = a.take<int32_t>(R);
+          probs = a.take<float>((size_t)R * H * QP * NP);
+        }
       }))
     return false;
-  cudaMemcpyAsync(mem, hw_host, (size_t)n_hw * D * 4, cudaMemcpyHostToDevice, st);
-  int n_sel = n_hw;
-  std::vector<float> picked_rows;
+  // each reference pack's memory: the picked rows of a filtered one, its set's rows (one copy per set) otherwise
+  std::vector<std::vector<float>> picked(hw.refs.size());
   int rc = FA_OK;
-  if (asf) {
-    const int32_t one = n_hw;
-    cudaMemcpyAsync(mem_lens, &one, 4, cudaMemcpyHostToDevice, st);
-    rc = fa_sanm_decoder_stack_forward(&m.seaco_dec, mem, mem_lens, 1, 1, n_hw, hidden, n_max, tok, n_max, 6, 0, nullptr, probs, m.mode,
-                                       m.ws.p, m.ws.cap, st);
+  std::vector<float> host_p;
+  std::vector<int32_t> lens_p(Gp), tok_ph(R), seq(R);
+  if (R > 0) {
+    host_p.assign((size_t)Gp * NP * D, 0.f);              // rows past a set's length are zeros: their projections are the bias
+    for (int g = 0; g < Gp; ++g) {
+      const int s = plan.probe_set[g];
+      lens_p[g] = hw.n[s];
+      std::copy(hw.rows[s], hw.rows[s] + (size_t)hw.n[s] * D, host_p.begin() + (size_t)g * NP * D);
+    }
+    for (int k = 0; k < R; ++k) {
+      const int first = hw.refs[plan.probe[k]].first;
+      tok_ph[k] = tok_h[first];
+      seq[k] = k;
+      cudaMemcpyAsync(hx + (size_t)k * n_max * D, hidden + (size_t)first * n_max * D, (size_t)n_max * D * 4, cudaMemcpyDeviceToDevice, st);
+    }
+    cudaMemcpyAsync(mem_p, host_p.data(), host_p.size() * 4, cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(tok_p, tok_ph.data(), (size_t)R * 4, cudaMemcpyHostToDevice, st);
+    rc = fa_sanm_decoder_stack_forward_grouped(&m.seaco_dec, mem_p, lens_p.data(), plan.probe_group.data(), Gp, R, NP, hx, n_max, tok_p, QP, 6, 0,
+                                               nullptr, probs, seq.data(), R, m.mode, m.ws.p, m.ws.cap, st);
     if (rc != FA_OK) { set_err(std::string("SeACo filter: ") + fa_status_string(rc)); return false; }
-    std::vector<float> probs_h((size_t)H * n_max * n_hw);
+    std::vector<float> probs_h((size_t)R * H * QP * NP);
     cudaMemcpyAsync(probs_h.data(), probs, probs_h.size() * 4, cudaMemcpyDeviceToHost, st);
     if (!sync_stream(st)) return false;
-    std::vector<int32_t> picked((size_t)n_hw);
-    n_sel = fa_seaco_asf_select_host(probs_h.data(), H, n_max, n_hw, m.nfilter, picked.data());
-    if (n_sel < 1) { set_err("fa_seaco_asf_select_host failed"); return false; }
-    picked_rows.resize((size_t)n_sel * D);
-    for (int j = 0; j < n_sel; ++j) std::copy(hw_host + (size_t)picked[j] * D, hw_host + (size_t)(picked[j] + 1) * D, picked_rows.begin() + (size_t)j * D);
-    cudaMemcpyAsync(mem, picked_rows.data(), picked_rows.size() * 4, cudaMemcpyHostToDevice, st);
+    for (int k = 0; k < R; ++k) {                          // the reference pack's own [heads, n_max_ref, n] block
+      const int s = plan.probe_set[plan.probe_group[k]], n = hw.n[s], q = plan.probe_nmax[k];
+      std::vector<float> blk((size_t)H * q * n);
+      for (int h = 0; h < H; ++h)
+        for (int i = 0; i < q; ++i)
+          std::copy_n(probs_h.begin() + (((size_t)k * H + h) * QP + i) * NP, n, blk.begin() + ((size_t)h * q + i) * n);
+      std::vector<int32_t> pick((size_t)n);
+      const int n_sel = fa_seaco_asf_select_host(blk.data(), H, q, n, m.nfilter, pick.data());
+      if (n_sel < 1) { set_err("fa_seaco_asf_select_host failed"); return false; }
+      std::vector<float>& out = picked[plan.probe[k]];
+      out.resize((size_t)n_sel * D);
+      for (int j = 0; j < n_sel; ++j) std::copy_n(hw.rows[s] + (size_t)pick[j] * D, D, out.begin() + (size_t)j * D);
+    }
   }
-  const std::vector<int32_t> lens_h(B, n_sel);
-  cudaMemcpyAsync(mem_lens, lens_h.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st);
-  rc = fa_sanm_decoder_stack_forward(&m.seaco_dec, mem, mem_lens, 1, B, n_sel, acoustic, n_cap, tok, n_max, n_s, 1, cif_att, nullptr, m.mode,
-                                     m.ws.p, m.ws.cap, st);
+  // the final memories, one upload; every row's memory (a row without rows reads memory 0 and keeps the decoder's ids)
+  std::vector<int32_t> lens_f, group_row(B, 0), set_group(hw.n.size(), -1);
+  int nf = 1;
+  for (size_t k = 0; k < hw.refs.size(); ++k) {
+    const PackHotwords::Ref& r = hw.refs[k];
+    if (r.set >= 0) nf = std::max(nf, picked[k].empty() ? hw.n[r.set] : (int)(picked[k].size() / D));
+  }
+  std::vector<float> host_f;
+  host_f.reserve((size_t)G * nf * D);
+  for (size_t k = 0; k < hw.refs.size(); ++k) {
+    const PackHotwords::Ref& r = hw.refs[k];
+    if (r.set < 0) continue;
+    int g = set_group[r.set];
+    if (!picked[k].empty() || g < 0) {
+      g = (int)lens_f.size();
+      const float* src = picked[k].empty() ? hw.rows[r.set] : picked[k].data();
+      const int n = picked[k].empty() ? hw.n[r.set] : (int)(picked[k].size() / D);
+      if (picked[k].empty()) set_group[r.set] = g;
+      lens_f.push_back(n);
+      host_f.insert(host_f.end(), src, src + (size_t)n * D);
+      host_f.resize((size_t)(g + 1) * nf * D, 0.f);
+    }
+    std::fill(group_row.begin() + r.first, group_row.begin() + r.first + r.count, g);
+  }
+  // every row's [key count | memory], uploaded beside the memories: the two stacks below then copy nothing between their launches
+  std::vector<int32_t> rows_h((size_t)2 * B);
+  for (int b = 0; b < B; ++b) { rows_h[b] = lens_f[group_row[b]]; rows_h[B + b] = group_row[b]; }
+  cudaMemcpyAsync(mem, host_f.data(), host_f.size() * 4, cudaMemcpyHostToDevice, st);
+  cudaMemcpyAsync(rows_f, rows_h.data(), rows_h.size() * 4, cudaMemcpyHostToDevice, st);
+  const int Gf = (int)lens_f.size();
+  rc = fa::sanm_stack_grouped_dev(&m.seaco_dec, mem, rows_f, Gf, B, nf, acoustic, n_cap, tok, n_max, n_s, cif_att, m.mode, m.ws.p, m.ws.cap, st);
   if (rc == FA_OK)
-    rc = fa_sanm_decoder_stack_forward(&m.seaco_dec, mem, mem_lens, 1, B, n_sel, hidden, n_max, tok, n_max, n_s, 1, dec_att, nullptr, m.mode,
-                                       m.ws.p, m.ws.cap, st);
+    rc = fa::sanm_stack_grouped_dev(&m.seaco_dec, mem, rows_f, Gf, B, nf, hidden, n_max, tok, n_max, n_s, dec_att, m.mode, m.ws.p, m.ws.cap, st);
   if (rc == FA_OK) rc = fa_linear_argmax(&m.hw_out, cif_att, dec_att, rows, dha_ids, dha_best, nullptr, m.mode, m.ws.p, m.ws.cap, st);
   if (rc == FA_OK) rc = fa_seaco_merge(ids, best, dha_ids, dha_best, rows, m.no_bias, *sids, sbest, nullptr, nullptr, nullptr, V, st);
   if (rc != FA_OK) { set_err(std::string("SeACo decoder: ") + fa_status_string(rc)); return false; }
-  return sync_stream(st);                                    // lens_h and picked_rows are host vectors of this frame
+  for (const PackHotwords::Ref& r : hw.refs)
+    if (r.set < 0)
+      cudaMemcpyAsync(*sids + (size_t)r.first * n_max, ids + (size_t)r.first * n_max, (size_t)r.count * n_max * 4, cudaMemcpyDeviceToDevice, st);
+  return sync_stream(st);                                    // the host vectors above are this frame's
+}
+
+// the workspace of seaco_bias's stages
+size_t seaco_ws_bytes(const Model& m, const SeacoPlan& p, int B, int n_max) {
+  const int R = (int)p.probe.size();
+  size_t ws = std::max(fa_sanm_decoder_stack_grouped_workspace_bytes(B, p.groups, p.rows_ub, n_max, 0, m.mode),
+                       fa_linear_argmax_workspace_bytes((int64_t)B * n_max, m.vocab, m.mode));
+  if (R > 0)
+    ws = std::max(ws, fa_sanm_decoder_stack_grouped_workspace_bytes(R, (int)p.probe_set.size(), p.probe_rows, p.probe_nmax_all, R, m.mode));
+  return ws;
 }
 
 // The recogniser over a padded batch already on the device: wav [B, stride] fp32, lens_h [B] samples (>= 400 each), ext_h [B] each
 // row's padded length in frames (decode_pack).  Everything after the pool gathered the pack's rows.
 std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const std::vector<int32_t>& ext_h,
-                                     const float* hw_embed, int32_t n_hotwords) {
+                                     const PackHotwords* hwp) {
   const int B = (int)lens_h.size(), D = m.d_model;
   cudaStream_t st = m.file.st;
   int t_max = 0;
@@ -250,43 +356,51 @@ std::unique_ptr<Result> decode_batch(Model& m, const float* wav, int64_t stride,
   for (int i = 0; i < B; ++i) n_max = r->token_num[i] > n_max ? r->token_num[i] : n_max;
   r->ids.resize(B);
   if (n_max < 1) return r;                                   // paraformer/model.py:615-616
-  const int nh = m.contextual ? n_hotwords : 0;
   // the timestamp head over the [B, 3T] upsampled frames shares the workspace with the decoder
   const int U = m.head.up_times, TU = T * U;
   const int64_t rows_up = (int64_t)B * TU;
-  const int n_sw = m.seaco && hw_embed ? n_hotwords : 0;     // SeACo hotword rows (none: the plain decoder distribution)
-  size_t ws_dec = fa_paraformer_decoder_workspace_bytes_hw(B, T, n_max, m.vocab, m.mode, nh);
+  // contextual: the pack's distinct hotword sets as memories [G, nh_max, 512], zero rows past a set's length (contextual_paraformer/
+  // model.py:350-372); every row's memory is its reference pack's
+  std::vector<float> hw_h;
+  std::vector<int32_t> hw_lens_h, hw_row_h(B, 0);
+  int nh_max = 0;
+  if (m.contextual && hwp) {
+    for (int32_t n : hwp->n) nh_max = std::max(nh_max, n);
+    hw_lens_h = hwp->n;
+    hw_h.assign(hwp->n.size() * (size_t)nh_max * D, 0.f);
+    for (size_t g = 0; g < hwp->n.size(); ++g) std::copy_n(hwp->rows[g], (size_t)hwp->n[g] * D, hw_h.begin() + g * nh_max * D);
+    for (const PackHotwords::Ref& r : hwp->refs) std::fill(hw_row_h.begin() + r.first, hw_row_h.begin() + r.first + r.count, r.set);
+  }
+  const int G = (int)hw_lens_h.size();
+  const SeacoPlan sp = m.seaco && hwp ? seaco_plan(m, *hwp, r->token_num) : SeacoPlan();
+  size_t ws_dec = G > 0 ? fa_paraformer_decoder_grouped_workspace_bytes(B, T, n_max, m.vocab, m.mode, G, nh_max)
+                        : fa_paraformer_decoder_workspace_bytes_hw(B, T, n_max, m.vocab, m.mode, 0);
   if (m.ts) ws_dec = std::max(ws_dec, fa_timestamp_head_ext_workspace_bytes(B, T, D, U, m.mode));
-  if (n_sw > 0)
-    ws_dec = std::max({ws_dec, fa_sanm_decoder_stack_workspace_bytes(B, n_sw, n_max, m.mode), fa_linear_argmax_workspace_bytes((int64_t)B * n_max, m.vocab, m.mode)});
-  int32_t *ids, *fids, *flens_out, *hw_lens = nullptr;
+  if (sp.any) ws_dec = std::max(ws_dec, seaco_ws_bytes(m, sp, B, n_max));
+  int32_t *ids, *fids, *flens_out;
   float *best, *us_alphas = nullptr, *us_peaks = nullptr, *hw = nullptr, *hidden = nullptr;
   if (!carve(m.decode, "decoder", [&](fa::Arena& a) {
         ids = a.take<int32_t>((size_t)B * n_max); best = a.take<float>((size_t)B * n_max); fids = a.take<int32_t>((size_t)B * n_max);
         flens_out = a.take<int32_t>(B);
         if (m.ts) { us_alphas = a.take<float>(rows_up); us_peaks = a.take<float>(rows_up); }
-        if (m.contextual) { hw = a.take<float>((size_t)nh * D); hw_lens = a.take<int32_t>(B); }
+        if (G > 0) hw = a.take<float>(hw_h.size());
         if (m.seaco) hidden = a.take<float>((size_t)B * n_max * D);
       }))
     return nullptr;
   if (!m.ws.reserve(ws_dec)) return fail("device allocation failed (decoder)");
-  if (m.contextual) {                                        // hotword memory [n_hw, 512] (contextual_paraformer/model.py:350-372) + per-utterance counts
-    std::vector<int32_t> hl(B, nh);
-    cudaMemcpyAsync(hw, hw_embed, (size_t)nh * D * 4, cudaMemcpyHostToDevice, st);
-    cudaMemcpyAsync(hw_lens, hl.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st);
-    cudaStreamSynchronize(st);                               // hl is a stack vector
-    m.dec.has_bias = 1; m.dec.n_hotwords = nh;
-    m.dec.hw_embed = hw; m.dec.hw_lens = hw_lens;
-  }
+  if (G > 0) cudaMemcpyAsync(hw, hw_h.data(), hw_h.size() * 4, cudaMemcpyHostToDevice, st);
   const int32_t* final_ids = ids;
   if (m.seaco) {                                             // return_hidden: the decoder_hidden the SeACo decoder attends from
     rc = fa_paraformer_decoder_forward_hidden(&m.dec, encb, flens, B, T, acoustic, n_cap, tok, n_max, ids, best, nullptr, 1, hidden, m.mode,
                                               m.ws.p, m.ws.cap, st);
-    if (rc == FA_OK && n_sw > 0) {
+    if (rc == FA_OK && sp.any) {
       int32_t* sids = nullptr;
-      if (!seaco_bias(m, B, n_max, n_cap, hw_embed, n_sw, acoustic, hidden, tok, ids, best, &sids)) return nullptr;
+      if (!seaco_bias(m, sp, *hwp, r->token_num, B, n_max, n_cap, acoustic, hidden, tok, ids, best, &sids)) return nullptr;
       final_ids = sids;
     }
+  } else if (G > 0) {
+    rc = fa_paraformer_decoder_forward_grouped(&m.dec, encb, flens, B, T, acoustic, n_cap, tok, n_max, ids, best, nullptr, 1, nullptr, hw,
+                                               hw_lens_h.data(), hw_row_h.data(), G, nh_max, m.mode, m.ws.p, m.ws.cap, st);
   } else {
     rc = fa_paraformer_decoder_forward(&m.dec, encb, flens, B, T, acoustic, n_cap, tok, n_max, ids, best, nullptr, 1, m.mode, m.ws.p, m.ws.cap, st);
   }
@@ -474,9 +588,9 @@ bool check_queries(const Model& m, const int32_t* lang, const int32_t* tn, int n
 }
 
 std::unique_ptr<Result> decode_pack(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const std::vector<int32_t>& ext_h,
-                                    const float* hw_embed, int32_t n_hotwords, const int32_t* lang, const int32_t* tn) {
+                                    const PackHotwords* hw, const int32_t* lang, const int32_t* tn) {
   // SenseVoice has no CIF predictor: its rows read nothing past their own length
-  return m.sv ? decode_sv(m, wav, stride, lens_h, lang, tn) : decode_batch(m, wav, stride, lens_h, ext_h, hw_embed, n_hotwords);
+  return m.sv ? decode_sv(m, wav, stride, lens_h, lang, tn) : decode_batch(m, wav, stride, lens_h, ext_h, hw);
 }
 
 }  // namespace fa_handle

@@ -13,6 +13,11 @@
 //   at most kPackSamples of padded audio, a larger reference pack alone), decodes each, and scatters the rows back.
 // Pack-level rules of the reference (a long-audio pack without a token empties its recording) apply per reference pack.  The leader
 // then marks the drained tickets done and wakes their threads; it leads again until its own ticket is done.  No thread is created.
+//
+// Hotword calls (contextual and SeACo Paraformer) pool like any other: the reference gives every utterance of a batch the same hotword
+// memory, and for SeACo with more rows than nfilter the attention-score filter of the batch's utterance 0, so the memory belongs to the
+// reference pack.  decode_pack takes each reference pack's rows and set; identical sets within a pass (the same count and the same
+// bytes: a server-wide list) are one set, projected once per GPU pack.
 #include "handle.h"
 #include <string.h>
 
@@ -24,6 +29,9 @@ namespace {
 const int64_t kVadGroupSamples = 3600LL * 16000;
 // padded 16 kHz samples of a GPU pack merged from several calls' reference packs: 300 s, the reference's default batch_size_s
 const int64_t kPackSamples = 300LL * 16000;
+// hotword memory rows of a GPU pack: (distinct sets + reference packs the SeACo filter runs on) x the longest set.  A reference pack
+// over it decodes alone; 4096 rows are 16 MB of bias k|v.
+const int64_t kPackHotwordRows = 4096;
 
 int64_t padded(int64_t n) { return (n + 3) / 4 * 4; }
 
@@ -40,7 +48,7 @@ int64_t ticket_samples(const Ticket& t) {
 }
 
 // The head of the queue and every later ticket that may share its packs, in arrival order, until an hour of padded audio.  Solo tickets
-// (hotword rows, diarization) run alone; long-audio tickets share a pass only with the same VAD handle and options.
+// (diarization) run alone; long-audio tickets share a pass only with the same VAD handle and options.
 std::vector<Ticket*> drain(Model& m) {
   std::vector<Ticket*> out{m.pool_q.front()};
   m.pool_q.pop_front();
@@ -67,6 +75,7 @@ struct RefPack {
   std::vector<int32_t> lens, lang, tn;               // 16 kHz samples, SenseVoice queries
   int ext = 0;                                       // LFR frames of its longest row
   int64_t lmax = 0;
+  int set = -1;                                      // its call's hotword set in the pass (-1: none)
   std::string bad;                                   // long audio: a segment under 400 samples, reported if the recording reaches it
   std::unique_ptr<Result> out;                       // its rows, scattered from the GPU pack
 };
@@ -82,7 +91,8 @@ struct LongRec {
 // a slice of one ticket's buffers: a whole utterance batch, or one long-audio recording
 struct Unit { Ticket* t; int first, count; };
 
-bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::vector<char>& failed, const std::vector<Ticket*>& pass) {
+bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::vector<char>& failed, const std::vector<Ticket*>& pass,
+                const PackHotwords& sets) {
   cudaStream_t st = m.file.st;
   // rows: long-audio recordings first (one batched VAD pass reads them as [nl, stride]), then the utterance batches
   std::vector<int> row(units.size());
@@ -120,6 +130,7 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
     const int ti = (int)(std::find(pass.begin(), pass.end(), &t) - pass.begin());
     if (!t.long_audio) {
       RefPack p{&t};
+      p.set = t.hw_set;
       for (int j = 0; j < t.batch; ++j) {
         p.starts.push_back((int64_t)(row[u] + j) * stride);
         p.lens.push_back((int32_t)t.n16[j]);
@@ -153,6 +164,7 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
       if (np < 0) { set_err("fa_pack_segments failed"); return false; }
       for (int64_t q = 0; q < np; ++q) {
         RefPack p{&t};
+        p.set = t.hw_set;
         for (int j = bounds[2 * q]; j < bounds[2 * q + 1]; ++j) {     // slice_padding_audio_samples (utils/vad_utils.py:44-51)
           const int s = lr.order[j];
           const int64_t b0 = (int64_t)segs[2 * s] * 16, b1 = std::min<int64_t>((int64_t)segs[2 * s + 1] * 16, n), len = b1 - b0;
@@ -176,29 +188,51 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
     }
     longs.push_back(std::move(lr));
   }
-  // GPU packs: reference packs by extent, merged while the padded audio fits kPackSamples; two packs of one call never share a GPU
-  // pack, so a lone caller decodes exactly its reference packs
+  // GPU packs: reference packs by extent, merged while the padded audio fits kPackSamples and the hotword memories kPackHotwordRows;
+  // two packs of one call never share a GPU pack, so a lone caller decodes exactly its reference packs
   std::vector<int> by_ext;
   for (size_t p = 0; p < packs.size(); ++p)
     if (packs[p].bad.empty()) by_ext.push_back((int)p);
   std::stable_sort(by_ext.begin(), by_ext.end(), [&](int a, int b) { return packs[a].ext < packs[b].ext; });
   std::vector<std::vector<int>> gpu;
-  int64_t g_rows = 0, g_lmax = 0;
+  int64_t g_rows = 0, g_lmax = 0, g_hw_max = 0, g_memories = 0;
+  std::vector<char> g_sets(sets.n.size(), 0);
   for (int p : by_ext) {
     const RefPack& rp = packs[p];
-    bool join = !gpu.empty() && (g_rows + (int64_t)rp.lens.size()) * padded(std::max(g_lmax, rp.lmax)) <= kPackSamples;
+    const int64_t n = rp.set >= 0 ? sets.n[rp.set] : 0;
+    const int64_t memories = g_memories + (rp.set >= 0 && !g_sets[rp.set]) + (m.seaco && m.nfilter > 0 && m.nfilter < n);
+    bool join = !gpu.empty() && (g_rows + (int64_t)rp.lens.size()) * padded(std::max(g_lmax, rp.lmax)) <= kPackSamples &&
+                memories * std::max(g_hw_max, n) <= kPackHotwordRows;
     for (size_t k = 0; join && k < (gpu.empty() ? 0 : gpu.back().size()); ++k) join = packs[gpu.back()[k]].t != rp.t;
-    if (!join) { gpu.emplace_back(); g_rows = 0; g_lmax = 0; }
+    if (!join) {
+      gpu.emplace_back(); g_rows = 0; g_lmax = 0; g_hw_max = 0; g_memories = 0;
+      std::fill(g_sets.begin(), g_sets.end(), 0);
+    }
     gpu.back().push_back(p);
     g_rows += (int64_t)rp.lens.size();
     g_lmax = std::max(g_lmax, rp.lmax);
+    g_hw_max = std::max(g_hw_max, n);
+    g_memories += (rp.set >= 0 && !g_sets[rp.set]) + (m.seaco && m.nfilter > 0 && m.nfilter < n);
+    if (rp.set >= 0) g_sets[rp.set] = 1;
   }
   for (const std::vector<int>& g : gpu) {
     std::vector<int64_t> starts;
     std::vector<int32_t> lens, ext, lang, tn;
     int64_t lmax = 0;
+    PackHotwords hw;                                         // the pack's sets, numbered in the pack
+    std::vector<int> local(sets.n.size(), -1);
     for (int p : g) {
       const RefPack& rp = packs[p];
+      int set = -1;
+      if (rp.set >= 0) {
+        if (local[rp.set] < 0) {
+          local[rp.set] = (int)hw.n.size();
+          hw.rows.push_back(sets.rows[rp.set]);
+          hw.n.push_back(sets.n[rp.set]);
+        }
+        set = local[rp.set];
+      }
+      hw.refs.push_back({(int)lens.size(), (int)rp.lens.size(), set});
       starts.insert(starts.end(), rp.starts.begin(), rp.starts.end());
       lens.insert(lens.end(), rp.lens.begin(), rp.lens.end());
       ext.insert(ext.end(), rp.lens.size(), rp.ext);
@@ -221,8 +255,7 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
         return false;
       if (!gather(recs, (int64_t)rows * stride, starts.data(), lens.data(), B, pstride, starts_d, lens_d, wav, st)) return false;
     }
-    const Ticket& t0 = *packs[g[0]].t;                       // hotword rows only reach a solo ticket's packs
-    std::unique_ptr<Result> r = decode_pack(m, wav, pstride, lens, ext, t0.hw_embed, t0.n_hotwords, lang.data(), tn.data());
+    std::unique_ptr<Result> r = decode_pack(m, wav, pstride, lens, ext, &hw, lang.data(), tn.data());
     if (!r) return false;
     ++m.pool_packs;
     int j = 0;
@@ -301,6 +334,19 @@ void run_pass(Model& m, const std::vector<Ticket*>& pass) {
   cudaSetDevice(m.file.device);
   m.pool_calls += (int64_t)pass.size();
   std::vector<char> failed(pass.size(), 0);
+  PackHotwords sets;                                         // the pass's distinct hotword sets: the same count and the same bytes
+  for (Ticket* t : pass) {
+    t->hw_set = -1;
+    if (!(m.contextual || m.seaco) || !t->hw_embed || t->n_hotwords < 1) continue;   // the other models ignore rows
+    const size_t bytes = (size_t)t->n_hotwords * 512 * sizeof(float);
+    for (size_t k = 0; k < sets.n.size() && t->hw_set < 0; ++k)
+      if (sets.n[k] == t->n_hotwords && (sets.rows[k] == t->hw_embed || memcmp(sets.rows[k], t->hw_embed, bytes) == 0)) t->hw_set = (int)k;
+    if (t->hw_set < 0) {
+      t->hw_set = (int)sets.n.size();
+      sets.rows.push_back(t->hw_embed);
+      sets.n.push_back(t->n_hotwords);
+    }
+  }
   const bool ok = no_throw(pass[0]->long_audio ? "fa_offline_infer_vad: " : "fa_offline_infer: ", [&] {
     std::vector<Unit> units;
     for (Ticket* t : pass) {
@@ -334,7 +380,7 @@ void run_pass(Model& m, const std::vector<Ticket*>& pass) {
         stride = w;
         rows += units[g1].count;
       }
-      if (!pool_group(m, std::vector<Unit>(units.begin() + g0, units.begin() + g1), stride, failed, pass)) return false;
+      if (!pool_group(m, std::vector<Unit>(units.begin() + g0, units.begin() + g1), stride, failed, pass, sets)) return false;
     }
     return true;
   });

@@ -521,7 +521,10 @@ const std::vector<std::vector<float>> CompileHotwordEmbedding(FUNASR_HANDLE hand
     for (size_t i = 0; i < lens.size(); ++i) out.emplace_back(rows.begin() + i * 512, rows.begin() + (i + 1) * 512);
     return out;
   }
-  if (!s || !fa_offline_is_contextual(s->h)) return out;
+  // a model without a hotword branch (Paraformer, BiCif): one zero row of encoder_size (paraformer.cpp:557-564), so a server that
+  // decodes only when the embedding is non-empty still decodes; infer_pcm passes no rows to such a model
+  if (s && !fa_offline_is_contextual(s->h)) return {std::vector<float>(512, 0.f)};
+  if (!s) return out;
   int64_t n_emb = 0, n_ih = 0, n_hh = 0, n_bi = 0, n_bh = 0;
   const float* emb = fa_offline_host_tensor(s->h, "bias_embed.weight", &n_emb);
   const float* w_ih = fa_offline_host_tensor(s->h, "bias_encoder.weight_ih_l0", &n_ih);

@@ -289,6 +289,17 @@ int fa_attention_tc_planes_ex(const void* q_planes, const void* k_planes, const 
 int fa_attention_f32_ex(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv,
                         const int32_t* key_lens, int32_t batch, int32_t heads, int32_t head_dim, int32_t tq, int32_t tk,
                         float* ctx, int64_t ld_ctx, int32_t kv_shared, fa_stream_t stream);
+/* Attention with a K / V entry per utterance: k / v hold kv_batch entries [kv_batch, tk, ld] and utterance b attends over entry
+ * kv_index_h[b] (host, each in [0, kv_batch), read before the call returns) with key_lens[b] (device) keys, through the same kernels as the calls above in any
+ * gemm_mode (fp32: the fp32 kernels' choice by head_dim; tensor cores: head_dim 128).  Every index 0 with one entry is kv_shared, index
+ * b with kv_batch = B the per-utterance case; a row gives exactly what the kv_shared call on its own entry gives, whatever the other
+ * entries hold (rows of an entry past its keys must be finite: the last 64-key chunk reads them and multiplies them by 0).  The
+ * workspace holds the index and, on the tensor cores, the operand planes; its query is exactly what the call carves.  Refusals
+ * (NULL arguments, an index outside [0, kv_batch)) come before any device work. */
+size_t fa_attention_grouped_workspace_bytes(int32_t batch, int32_t heads, int32_t tq, int32_t kv_batch, int32_t tk, int32_t gemm_mode);
+int fa_attention_grouped(const float* q, int64_t ldq, const float* k, int64_t ldk, const float* v, int64_t ldv, const int32_t* key_lens,
+                         const int32_t* kv_index_h, int32_t kv_batch, int32_t batch, int32_t heads, int32_t head_dim, int32_t tq, int32_t tk,
+                         float* ctx, int64_t ld_ctx, int32_t gemm_mode, void* workspace, size_t ws_bytes, fa_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Model-level entry points
@@ -415,6 +426,19 @@ int fa_paraformer_decoder_forward_hidden(const FaDecoder* dec, const float* enc,
                                          float* logits, int32_t log_softmax, float* hidden, int32_t gemm_mode,
                                          void* workspace, size_t ws_bytes, fa_stream_t stream);
 
+/* A contextual decoder (dec->has_bias) over G hotword memories instead of dec->hw_embed / hw_lens / n_hotwords: hw_embed [G, nh_max,
+ * 512] (device; rows past a memory's length must be finite, zeros are fine), hw_lens_h [G] (host, each in [1, nh_max]) and
+ * row_group_h [B] (host, each in [0, G)): utterance b's bias branch attends over memory row_group_h[b], exactly as
+ * fa_paraformer_decoder_forward(_hidden) gives it with that memory alone.  One bias k|v GEMM runs over all G * nh_max rows.  hidden
+ * may be NULL.  Refusals come before any device work; the workspace query is exactly what the call carves. */
+size_t fa_paraformer_decoder_grouped_workspace_bytes(int32_t batch, int32_t t_max, int32_t n_max, int32_t vocab, int32_t gemm_mode,
+                                                     int32_t n_groups, int32_t nh_max);
+int fa_paraformer_decoder_forward_grouped(const FaDecoder* dec, const float* enc, const int32_t* enc_lens, int32_t batch, int32_t t_max,
+                                          const float* acoustic, int64_t ld_acoustic_rows, const int32_t* tok_lens, int32_t n_max,
+                                          int32_t* argmax_ids, float* argmax_logp, float* logits, int32_t log_softmax, float* hidden,
+                                          const float* hw_embed, const int32_t* hw_lens_h, const int32_t* row_group_h, int32_t n_groups,
+                                          int32_t nh_max, int32_t gemm_mode, void* workspace, size_t ws_bytes, fa_stream_t stream);
+
 /* A SAN-M decoder stack WITHOUT input / output layer over an arbitrary memory: the SeACo decoder of SeacoParaformer
  * (seaco_paraformer/model.py:100-110: ParaformerSANMDecoder(use_output_layer=False, wo_input_layer=True), FFN 1024, FSMN k=21,
  * 6 attention layers) attending over the hotword embeddings.  Uses dec->layers / n_layers / heads / fsmn_k / last / after_norm.
@@ -431,6 +455,18 @@ int fa_sanm_decoder_stack_forward(const FaDecoder* dec, const float* memory, con
                                   int32_t batch, int32_t t_mem, const float* x, int64_t ld_x_rows, const int32_t* tok_lens,
                                   int32_t n_max, int32_t n_run, int32_t finish, float* hidden, float* attn_probs,
                                   int32_t gemm_mode, void* workspace, size_t ws_bytes, fa_stream_t stream);
+/* The same stack over G memories: memory [G, t_mem, 512] (device; rows past a memory's length must be finite), mem_lens_h [G] (host,
+ * each in [1, t_mem]) and row_group_h [B] (host, each in [0, G)): utterance b attends over memory row_group_h[b], exactly as the call
+ * above gives it with that memory shared.  attn_probs != 0 writes the matrices of the utterances probe_rows_h[0 .. n_probe) (host,
+ * each in [0, B)), each against its own memory: [n_probe, heads, n_max, t_mem], the keys past a memory's length 0.  Refusals come
+ * before any device work; the workspace query (n_probe 0 without attn_probs) is exactly what the call carves. */
+size_t fa_sanm_decoder_stack_grouped_workspace_bytes(int32_t batch, int32_t n_groups, int32_t t_mem, int32_t n_max, int32_t n_probe,
+                                                     int32_t gemm_mode);
+int fa_sanm_decoder_stack_forward_grouped(const FaDecoder* dec, const float* memory, const int32_t* mem_lens_h, const int32_t* row_group_h,
+                                          int32_t n_groups, int32_t batch, int32_t t_mem, const float* x, int64_t ld_x_rows,
+                                          const int32_t* tok_lens, int32_t n_max, int32_t n_run, int32_t finish, float* hidden,
+                                          float* attn_probs, const int32_t* probe_rows_h, int32_t n_probe, int32_t gemm_mode,
+                                          void* workspace, size_t ws_bytes, fa_stream_t stream);
 
 /* ids / best_logp [rows] = arg-max and its log-softmax value of (a (+ b)) W^T + bias — SeACo's hotword_output_layer over
  * cif_attended + dec_attended (seaco_paraformer/model.py:351-355); logp != NULL receives the full log-softmax rows [rows, out_f].
@@ -787,8 +823,12 @@ const char* fa_offline_last_error(void);
  * audio), decoding them together and waking their threads; the others wait.  The library creates no thread.  Each call still gets
  * exactly what it gets alone: every row carries the padded length of the batch the reference decodes it in (the call's whole batch;
  * a long recording's own packs), and the CIF predictor and timestamp head give it what that batch gives it
- * (fa_cif_predictor_forward_ext).  Calls with hotword rows and diarized calls (fa_offline_infer_vad_spk) pass through the same queue
- * but never share a pack with another call; long-audio calls share passes only with the same VAD handle and FaLongAudioOptions.
+ * (fa_cif_predictor_forward_ext).  Calls with hotword rows (contextual and SeACo models) share packs too: the reference gives every
+ * utterance of a batch that batch's hotword memory (for SeACo with more rows than nfilter, the rows the filter picks on the batch's
+ * utterance 0), so each reference pack keeps its own memory and each row attends over its own (fa_attention_grouped); identical rows
+ * (the same count and bytes) are one memory per pack, and a pack holds at most 4096 memory rows (memories x the longest).  Diarized
+ * calls (fa_offline_infer_vad_spk) pass through the same queue but never share a pack with another call; long-audio calls share
+ * passes only with the same VAD handle and FaLongAudioOptions.
  * A device failure during a pass fails every call of that pass with its message.  Other handles' calls hold the handle's lock
  * for their device work and run one after another.  A call that uses several handles (fa_offline_infer_vad*) locks them in the order
  * recogniser, VAD, speaker, so recognisers that share a VAD handle cannot deadlock.  fa_offline_last_error is per thread.  Uninit a

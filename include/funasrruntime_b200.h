@@ -4,7 +4,9 @@
  * header in place of the original for the offline ASR calls it makes.  One handle may be shared by any number of threads, as the
  * reference's servers share it among their decoder threads: FunOfflineInfer / FunOfflineInferBuffer, CompileHotwordEmbedding,
  * FsmnVad* and CTTransformer* are safe on shared handles (funasr_b200.h, "Threads"); FunOfflineInfer* calls from many threads on
- * one handle are decoded together in shared GPU packs, each giving what it gives alone.  thread_num and batch_size stay ignored:
+ * one handle are decoded together in shared GPU packs, with or without hotword rows, each giving what it gives alone.
+ * CompileHotwordEmbedding returns one zero row of 512 for a model without a hotword branch (Paraformer, BiCif), as the reference
+ * does, so a server that decodes only when the embedding is non-empty decodes; the row is not used.  thread_num and batch_size stay ignored:
  * segments are packed by "batch-size-s".
  * Differences, all at run time, none in the signatures:
  *   model_path["model-dir"] names a directory holding `model.fab2` (funasr_b200/pack.py, written from an unmodified model.pt +
