@@ -279,6 +279,11 @@ SIGNATURES = {
     "fa_spk_tridiagonalize_workspace_bytes": (_sz, [_i32]),
     "fa_spk_tridiagonalize": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
     "fa_spk_back_transform": (C.c_int, [_vp, _vp, _i32, _vp, _i32, _vp]),
+    "fa_spk_laplacian_batch_workspace_bytes": (_sz, [_vp, _i32, _i32]),
+    "fa_spk_laplacian_batch": (C.c_int, [_vp, _vp, _i32, _i32, C.c_double, _vp, _vp, _sz, _vp]),
+    "fa_spk_tridiagonalize_batch_workspace_bytes": (_sz, [_vp, _i32]),
+    "fa_spk_tridiagonalize_batch": (C.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "fa_spk_back_transform_batch": (C.c_int, [_vp, _vp, _vp, _vp, _i32, _vp, _vp]),
     "fa_sym_tridiag_smallest_host": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp]),
     "fa_spk_kmeans_host": (C.c_int, [_vp, _i64, _i32, _i32, C.c_uint64, _i32, _i32, _vp]),
     "fa_spk_merge_by_cos_host": (C.c_int, [_vp, _vp, _i64, _i32, C.c_double]),

@@ -295,9 +295,8 @@ struct Ticket {
   bool long_audio = false;                           // fa_offline_infer_vad*: VAD, then packs of each recording's segments
   Vad* vad = nullptr;
   FaLongAudioOptions opts{};
-  Spk* spk = nullptr;                                // diarized (solo)
+  Spk* spk = nullptr;                                // diarized: shares a pass only with the same speaker handle, or none
   int32_t preset_spk_num = 0;
-  bool solo() const { return spk != nullptr; }
   // written by the pass, read by the owner once done
   std::unique_ptr<Result> res;
   std::string err;
@@ -423,8 +422,19 @@ struct Spk {
   DevBuf spk_embed_rows, diarize, spk_cluster;
 };
 
-// LongAudioPipeline.generate's diarization of one device-resident recording rec [n] (segs: {start_ms, end_ms, n_tokens} triples)
-// -> spk [segments], on the speaker handle's stream; rec must be complete
-bool diarize(Spk& s, const float* rec, int64_t n, const std::vector<int32_t>& segs, int preset, std::vector<int32_t>& spk, const std::string& what);
+// One recording of the speaker stage: recs[off, off + n) of the stage's device buffer, its {start_ms, end_ms, n_tokens} segments and
+// its preset count (<= 0: none) -> one speaker per segment in *spk, or its own refusal in err (named by the prefix what)
+struct SpkJob {
+  int64_t off = 0, n = 0;
+  const std::vector<int32_t>* segs = nullptr;
+  int preset = 0;
+  std::string what;
+  std::vector<int32_t>* spk = nullptr;
+  std::string err;
+};
+// LongAudioPipeline.generate's diarization of many device-resident recordings at once (recs [n_recs], complete), on the speaker
+// handle's stream: every recording gets what it gets alone, and a refusal (a preset above the chunk count, 2048 or more chunks without
+// one) fails only its own job.  false: a device failure, with the message set.
+bool diarize(Spk& s, const float* recs, int64_t n_recs, std::vector<SpkJob>& jobs);
 
 }  // namespace fa_handle

@@ -1,6 +1,6 @@
 // Long audio through the handle API: the entries check their arguments and post the call to the recogniser's request pool
-// (offline_pool.cu), which runs the VAD, packs each recording's segments as the reference does and decodes them; fa_offline_infer_vad_spk
-// then diarizes every recording with the CAM++ handle (diarize).
+// (offline_pool.cu), which runs the VAD, packs each recording's segments as the reference does and decodes them; for fa_offline_infer_vad_spk
+// it then diarizes the recordings with the CAM++ handle, one speaker stage per group of the pass (diarize).
 #include "handle.h"
 
 using namespace fa_handle;

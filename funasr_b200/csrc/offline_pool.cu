@@ -18,6 +18,10 @@
 // memory, and for SeACo with more rows than nfilter the attention-score filter of the batch's utterance 0, so the memory belongs to the
 // reference pack.  decode_pack takes each reference pack's rows and set; identical sets within a pass (the same count and the same
 // bytes: a server-wide list) are one set, projected once per GPU pack.
+//
+// Diarized calls pool too: their reference packs merge like any other, and once a group's recordings are assembled one speaker stage
+// (diarize) embeds and clusters all of its diarized recordings together; each recording is still clustered on its own, as the
+// reference's ClusterBackend does, and a refusal of the stage fails only its own call.
 #include "handle.h"
 #include <string.h>
 
@@ -47,21 +51,23 @@ int64_t ticket_samples(const Ticket& t) {
   return s;
 }
 
-// The head of the queue and every later ticket that may share its packs, in arrival order, until an hour of padded audio.  Solo tickets
-// (diarization) run alone; long-audio tickets share a pass only with the same VAD handle and options.
+// The head of the queue and every later ticket that may share its packs, in arrival order, until an hour of padded audio.  Long-audio
+// tickets share a pass only with the same VAD handle and options, diarized tickets only with the same speaker handle (a pass takes at
+// most one speaker lock); the others stay queued for a later pass.
 std::vector<Ticket*> drain(Model& m) {
   std::vector<Ticket*> out{m.pool_q.front()};
   m.pool_q.pop_front();
-  if (out[0]->solo()) return out;
   const Ticket* key = out[0]->long_audio ? out[0] : nullptr;
+  Spk* spk = out[0]->spk;
   int64_t samples = ticket_samples(*out[0]);
   for (auto it = m.pool_q.begin(); it != m.pool_q.end();) {
     Ticket* c = *it;
-    if (c->solo() || (c->long_audio && key && (c->vad != key->vad || !same_opts(c->opts, key->opts)))) { ++it; continue; }
+    if ((c->long_audio && key && (c->vad != key->vad || !same_opts(c->opts, key->opts))) || (c->spk && spk && c->spk != spk)) { ++it; continue; }
     const int64_t s = ticket_samples(*c);
     if (samples + s > kVadGroupSamples) break;
     samples += s;
     if (c->long_audio && !key) key = c;
+    if (c->spk && !spk) spk = c->spk;
     out.push_back(c);
     it = m.pool_q.erase(it);
   }
@@ -278,17 +284,25 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
     t.res->token_num.swap(rp.out->token_num);
     if (m.ts) t.res->stamps.swap(rp.out->stamps);
   }
-  for (LongRec& lr : longs) {
+  // each recording's own failure, decided in recording order once the speaker stage has run: a short VAD segment where the reference
+  // reaches it, or a refusal of the speaker stage.  A ticket's later recordings in the group are not assembled after its first.
+  std::vector<std::string> rec_err(longs.size());
+  std::vector<int> job_of(longs.size(), -1);
+  std::vector<char> stopped(pass.size(), 0);
+  std::vector<SpkJob> jobs;
+  Spk* spk = nullptr;
+  for (size_t li = 0; li < longs.size(); ++li) {
+    LongRec& lr = longs[li];
     Ticket& t = *lr.t;
     const int ti = (int)(std::find(pass.begin(), pass.end(), &t) - pass.begin());
-    if (failed[ti]) continue;
+    if (failed[ti] || stopped[ti]) continue;
     const int64_t ns = (int64_t)lr.segs.size() / 2;
     std::vector<std::vector<int32_t>> seg_ids((size_t)ns), seg_stamps((size_t)ns);
     bool emptied = false;
     int beg = 0;
     for (int p : lr.packs) {                                 // the reference's pack loop: a bad segment fails the call where it is reached
       RefPack& rp = packs[p];
-      if (!rp.bad.empty()) { t.err = rp.bad; failed[ti] = 1; break; }
+      if (!rp.bad.empty()) { rec_err[li] = rp.bad; stopped[ti] = 1; break; }
       int tmax = 0;
       for (int32_t k : rp.out->token_num) tmax = std::max(tmax, k);
       // no token in the whole pack: the recording's result is empty (:990-999).  SenseVoiceSmall.inference returns a result for every
@@ -300,7 +314,7 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
       }
       beg += (int)rp.lens.size();
     }
-    if (failed[ti]) continue;
+    if (stopped[ti]) continue;
     std::vector<int32_t>&ids = t.res->ids[lr.i], &segs_out = t.res->segs[lr.i], &stamps = t.res->stamps[lr.i];
     for (int64_t s = 0; s < ns; ++s) {
       const int32_t k = emptied ? 0 : (int32_t)seg_ids[s].size();
@@ -310,11 +324,24 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
       for (int32_t v : seg_stamps[s]) stamps.push_back(v + lr.segs[2 * s]);      // absolute ms (auto_model.py:1008-1022)
     }
     t.res->token_num[lr.i] = (int32_t)ids.size();
-    // the recogniser's stream is idle here (its results are on the host); the speaker work runs on the speaker handle's stream
-    if (t.spk && !ids.empty() &&
-        !diarize(*t.spk, recs + (int64_t)lr.row * stride, t.n16[lr.i], segs_out, t.preset_spk_num, t.res->spk[lr.i],
-                 "recording " + std::to_string(lr.i) + ": "))
-      return false;
+    if (t.spk && !ids.empty()) {                             // diarize every recording that decoded a token
+      SpkJob jb;
+      jb.off = (int64_t)lr.row * stride; jb.n = t.n16[lr.i]; jb.segs = &segs_out; jb.preset = t.preset_spk_num;
+      jb.what = "recording " + std::to_string(lr.i) + ": "; jb.spk = &t.res->spk[lr.i];
+      job_of[li] = (int)jobs.size();
+      jobs.push_back(std::move(jb));
+      spk = t.spk;                                           // one speaker handle per pass (drain)
+    }
+  }
+  // one speaker stage over the group's diarized recordings.  The recogniser's stream is idle here (its results are on the host); the
+  // speaker work runs on the speaker handle's stream.
+  if (!jobs.empty() && !diarize(*spk, recs, (int64_t)rows * stride, jobs)) return false;
+  for (size_t li = 0; li < longs.size(); ++li) {
+    Ticket& t = *longs[li].t;
+    const int ti = (int)(std::find(pass.begin(), pass.end(), &t) - pass.begin());
+    if (failed[ti]) continue;
+    const std::string& e = !rec_err[li].empty() ? rec_err[li] : (job_of[li] >= 0 ? jobs[job_of[li]].err : rec_err[li]);
+    if (!e.empty()) { t.err = e; failed[ti] = 1; }
   }
   return true;
 }

@@ -1,6 +1,6 @@
 // Handle-style CAM++ speaker model: fa_spk_init (model file -> handle, the BatchNorms folded on the host), fa_spk_embed (host PCM ->
-// 192-dim embeddings), fa_spk_cluster (ClusterBackend over host embeddings), and diarize, which long audio (offline_long.cu) runs on a
-// recording already on the device.
+// 192-dim embeddings), fa_spk_cluster (ClusterBackend over host embeddings), and diarize, which the request pool (offline_pool.cu) runs
+// once over a group's diarized recordings already on the device.
 #include "handle.h"
 #include <math.h>
 
@@ -214,69 +214,137 @@ bool spk_embed_rows(Spk& s, const float* wav, int64_t stride, const int32_t* len
   return true;
 }
 
-// ClusterBackend over n embeddings emb_d [n, 192] on the device (emb_h: the same on the host) -> labels [n] (before correct_labels).
-// preset <= 0: no preset count.  Fewer than 20 -> one speaker; fewer than 2048 -> the spectral path (the Laplacian and its
-// tridiagonalisation on the device, the 16 smallest eigenvalues on the host, the eigengap count unless preset, k-means on the
-// back-transformed vectors); otherwise k-means on the normalised rows with a preset count; merge_by_cos when no count was preset.
-bool spk_cluster(Spk& s, const float* emb_d, int n, int preset, const float* emb_h, std::vector<int32_t>& labels, const std::string& what) {
-  labels.assign((size_t)n, 0);
-  if (n < 20) return true;
-  if (preset > n) { set_err(what + "preset_spk_num " + std::to_string(preset) + " exceeds the " + std::to_string(n) + " speaker chunks"); return false; }
-  std::vector<double> x;
-  int k = preset, dim = 0;
-  if (n < kSpectralMaxChunks) {
-    cudaStream_t st = s.file.st;
-    const size_t ws_bytes = std::max(fa_spk_laplacian_workspace_bytes(n, kSpkEmbDim), fa_spk_tridiagonalize_workspace_bytes(n));
-    const int m = std::max(std::min(kMaxSpks + 1, n), k);
-    double *lap, *d, *zd;
+// ClusterBackend's refusals for n chunks, in its order (empty: none): fewer than 20 chunks are one speaker whatever the preset; from 20
+// up a preset above the chunk count, and 2048 or more chunks without one (the reference's UMAP + HDBSCAN path), are refused
+std::string cluster_refusal(int n, int preset, const std::string& what) {
+  if (n < 20) return std::string();
+  if (preset > n) return what + "preset_spk_num " + std::to_string(preset) + " exceeds the " + std::to_string(n) + " speaker chunks";
+  if (n >= kSpectralMaxChunks && preset <= 0)
+    return what + std::to_string(n) + " speaker chunks without preset_spk_num: the reference clusters 2048 or more chunks with UMAP + "
+           "HDBSCAN, which this backend does not provide; pass preset_spk_num or diarize fewer than 2048 chunks";
+  return std::string();
+}
+
+// One embedding set of spk_cluster: n rows from row `first` of the embeddings, its preset count (<= 0: none) -> labels (before
+// correct_labels), or its own refusal in err
+struct ClusterSet {
+  int first = 0, n = 0, preset = 0;
+  std::string what;                                  // prefix of its messages
+  std::vector<int32_t> labels;
+  std::string err;
+};
+
+// ClusterBackend over every set of the embeddings emb_d [rows, 192] on the device (emb_h: the same on the host).  Fewer than 20 rows ->
+// one speaker; fewer than 2048 -> the spectral path, every such set together (one fa_spk_laplacian_batch and fa_spk_tridiagonalize_batch,
+// one copy of d / e to the host, the 16 smallest eigenvalues and the eigengap count unless preset per set on the host, one upload of
+// the eigenvectors, one fa_spk_back_transform_batch and one copy back), then k-means on the back-transformed vectors; otherwise k-means
+// on the normalised rows with a preset count; merge_by_cos when no count was preset.  false: a device failure.
+bool spk_cluster(Spk& s, const float* emb_d, const float* emb_h, std::vector<ClusterSet>& sets) {
+  cudaStream_t st = s.file.st;
+  std::vector<int> spectral;
+  for (size_t i = 0; i < sets.size(); ++i) {
+    ClusterSet& c = sets[i];
+    c.labels.assign((size_t)c.n, 0);
+    c.err = cluster_refusal(c.n, c.preset, c.what);
+    if (c.n >= 20 && c.err.empty() && c.n < kSpectralMaxChunks) spectral.push_back((int)i);
+  }
+  std::vector<std::vector<double>> x(sets.size());
+  std::vector<int> dims(sets.size(), 0), ks(sets.size(), 0);
+  if (!spectral.empty()) {
+    const int S = (int)spectral.size();
+    std::vector<int32_t> n((size_t)S), k((size_t)S);
+    std::vector<int64_t> vo((size_t)S + 1, 0), zo((size_t)S + 1, 0);
+    bool contiguous = true;
+    for (int i = 0; i < S; ++i) {
+      const ClusterSet& c = sets[spectral[i]];
+      n[i] = c.n;
+      k[i] = std::max(std::min(kMaxSpks + 1, c.n), c.preset);          // the vectors the set may ask for: max(m, preset)
+      vo[i + 1] = vo[i] + c.n;
+      zo[i + 1] = zo[i] + (int64_t)k[i] * c.n;
+      contiguous = contiguous && c.first == sets[spectral[0]].first + vo[i];
+    }
+    const int64_t rows = vo[S];
+    // Every set has at most 2047 rows, so sum n^2 <= 2047 sum n: a long-audio group (an hour of padded audio, under 4 800 chunks)
+    // needs at most 79 MB of Laplacians and no further split.
+    const size_t ws_bytes = std::max(fa_spk_laplacian_batch_workspace_bytes(n.data(), S, kSpkEmbDim), fa_spk_tridiagonalize_batch_workspace_bytes(n.data(), S));
+    int64_t squares = 0;
+    for (int32_t v : n) squares += (int64_t)v * v;
+    double *lap, *de, *tau, *zd;
+    float* packed = nullptr;
     void* ws;
     if (!carve(s.spk_cluster, "speaker clustering", [&](fa::Arena& a) {
-          lap = a.take<double>((size_t)n * n); d = a.take<double>((size_t)3 * n); zd = a.take<double>((size_t)m * n); ws = a.take<char>(ws_bytes);
+          lap = a.take<double>((size_t)squares); de = a.take<double>((size_t)2 * rows); tau = a.take<double>((size_t)rows);
+          zd = a.take<double>((size_t)zo[S]); ws = a.take<char>(ws_bytes);
+          if (!contiguous) packed = a.take<float>((size_t)rows * kSpkEmbDim);
         }))
       return false;
-    int rc = fa_spk_laplacian(emb_d, n, kSpkEmbDim, kSpkPval, lap, ws, ws_bytes, st);
-    if (rc == FA_OK) rc = fa_spk_tridiagonalize(lap, n, d, d + n, d + 2 * n, ws, ws_bytes, st);
-    if (rc != FA_OK) { set_err(what + "speaker clustering: " + fa_status_string(rc)); return false; }
-    std::vector<double> de((size_t)2 * n), w((size_t)m);
-    cudaMemcpyAsync(de.data(), d, (size_t)2 * n * 8, cudaMemcpyDeviceToHost, st);
-    if (!sync_stream(st)) return false;
-    if (k <= 0) {                                    // the largest gap among the 16 smallest eigenvalues (spec_embs)
-      fa_sym_tridiag_smallest_host(de.data(), de.data() + n, n, m, 0, w.data(), nullptr);
-      const int ne = std::min(kMaxSpks + 1, n);
-      double gmax = -INFINITY;
-      for (int i = 0; i + 1 < ne; ++i)
-        if (w[i + 1] - w[i] > gmax) { gmax = w[i + 1] - w[i]; k = i + 1; }
+    const float* emb = emb_d + (size_t)sets[spectral[0]].first * kSpkEmbDim;
+    if (!contiguous) {                               // the spectral sets' rows gathered in set order
+      for (int i = 0; i < S; ++i)
+        cudaMemcpyAsync(packed + vo[i] * kSpkEmbDim, emb_d + (size_t)sets[spectral[i]].first * kSpkEmbDim, (size_t)n[i] * kSpkEmbDim * 4,
+                        cudaMemcpyDeviceToDevice, st);
+      emb = packed;
     }
-    std::vector<double> z((size_t)k * n);
-    fa_sym_tridiag_smallest_host(de.data(), de.data() + n, n, std::max(m, k), k, w.data(), z.data());
-    cudaMemcpyAsync(zd, z.data(), z.size() * 8, cudaMemcpyHostToDevice, st);
-    rc = fa_spk_back_transform(lap, d + 2 * n, n, zd, k, st);
-    if (rc != FA_OK) { set_err(what + "speaker clustering: " + fa_status_string(rc)); return false; }
-    cudaMemcpyAsync(z.data(), zd, z.size() * 8, cudaMemcpyDeviceToHost, st);
+    int rc = fa_spk_laplacian_batch(emb, n.data(), S, kSpkEmbDim, kSpkPval, lap, ws, ws_bytes, st);
+    if (rc == FA_OK) rc = fa_spk_tridiagonalize_batch(lap, n.data(), S, de, de + rows, tau, ws, ws_bytes, st);
+    if (rc != FA_OK) { set_err(std::string("speaker clustering: ") + fa_status_string(rc)); return false; }
+    std::vector<double> de_h((size_t)2 * rows), z((size_t)zo[S]);
+    cudaMemcpyAsync(de_h.data(), de, de_h.size() * 8, cudaMemcpyDeviceToHost, st);
     if (!sync_stream(st)) return false;
-    x.resize((size_t)n * k);
-    for (int i = 0; i < n; ++i)
-      for (int j = 0; j < k; ++j) x[(size_t)i * k + j] = z[(size_t)j * n + i];
-    dim = k;
-  } else if (preset > 0) {                           // _normalize_rows in fp32
-    x.resize((size_t)n * kSpkEmbDim);
-    for (int i = 0; i < n; ++i) {
-      const float* r = emb_h + (size_t)i * kSpkEmbDim;
-      float ss = 0.f;
-      for (int c = 0; c < kSpkEmbDim; ++c) ss += r[c] * r[c];
-      float nrm = std::sqrt(ss);
-      if (nrm == 0.f) nrm = 1.f;
-      for (int c = 0; c < kSpkEmbDim; ++c) x[(size_t)i * kSpkEmbDim + c] = (double)(r[c] / nrm);
+    for (int i = 0; i < S; ++i) {
+      const ClusterSet& c = sets[spectral[i]];
+      const double *d = de_h.data() + vo[i], *e = de_h.data() + rows + vo[i];
+      const int m = std::max(std::min(kMaxSpks + 1, c.n), c.preset);
+      std::vector<double> w((size_t)m);
+      int kk = c.preset;
+      if (kk <= 0) {                                 // the largest gap among the 16 smallest eigenvalues (spec_embs)
+        fa_sym_tridiag_smallest_host(d, e, c.n, m, 0, w.data(), nullptr);
+        const int ne = std::min(kMaxSpks + 1, c.n);
+        double gmax = -INFINITY;
+        for (int j = 0; j + 1 < ne; ++j)
+          if (w[j + 1] - w[j] > gmax) { gmax = w[j + 1] - w[j]; kk = j + 1; }
+      }
+      k[i] = kk;
+      ks[spectral[i]] = kk;
+      fa_sym_tridiag_smallest_host(d, e, c.n, std::max(m, kk), kk, w.data(), z.data() + zo[i]);
     }
-    dim = kSpkEmbDim;
-  } else {
-    set_err(what + std::to_string(n) + " speaker chunks without preset_spk_num: the reference clusters 2048 or more chunks with UMAP + "
-            "HDBSCAN, which this backend does not provide; pass preset_spk_num or diarize fewer than 2048 chunks");
-    return false;
+    // the sets' vectors packed at their own k: z [sum k n]
+    std::vector<int64_t> zk((size_t)S + 1, 0);
+    for (int i = 0; i < S; ++i) zk[i + 1] = zk[i] + (int64_t)k[i] * n[i];
+    for (int i = 1; i < S; ++i) std::copy(z.begin() + zo[i], z.begin() + zo[i] + (int64_t)k[i] * n[i], z.begin() + zk[i]);
+    cudaMemcpyAsync(zd, z.data(), (size_t)zk[S] * 8, cudaMemcpyHostToDevice, st);
+    rc = fa_spk_back_transform_batch(lap, tau, n.data(), k.data(), S, zd, st);
+    if (rc != FA_OK) { set_err(std::string("speaker clustering: ") + fa_status_string(rc)); return false; }
+    cudaMemcpyAsync(z.data(), zd, (size_t)zk[S] * 8, cudaMemcpyDeviceToHost, st);
+    if (!sync_stream(st)) return false;
+    for (int i = 0; i < S; ++i) {
+      const int si = spectral[i], nn = n[i], kk = k[i];
+      const double* zi = z.data() + zk[i];
+      x[si].resize((size_t)nn * kk);
+      for (int r = 0; r < nn; ++r)
+        for (int j = 0; j < kk; ++j) x[si][(size_t)r * kk + j] = zi[(size_t)j * nn + r];
+      dims[si] = kk;
+    }
   }
-  if (fa_spk_kmeans_host(x.data(), n, dim, k, 0, 10, 300, labels.data()) != FA_OK) { set_err(what + "k-means failed"); return false; }
-  if (preset <= 0 && fa_spk_merge_by_cos_host(labels.data(), emb_h, n, kSpkEmbDim, kMergeThr) != FA_OK) {
-    set_err(what + "merge_by_cos failed"); return false;
+  for (size_t i = 0; i < sets.size(); ++i) {
+    ClusterSet& c = sets[i];
+    if (c.n < 20 || !c.err.empty()) continue;
+    const float* eh = emb_h + (size_t)c.first * kSpkEmbDim;
+    if (c.n >= kSpectralMaxChunks) {                 // _normalize_rows in fp32, with the preset count
+      x[i].resize((size_t)c.n * kSpkEmbDim);
+      for (int r = 0; r < c.n; ++r) {
+        const float* row = eh + (size_t)r * kSpkEmbDim;
+        float ss = 0.f;
+        for (int j = 0; j < kSpkEmbDim; ++j) ss += row[j] * row[j];
+        float nrm = std::sqrt(ss);
+        if (nrm == 0.f) nrm = 1.f;
+        for (int j = 0; j < kSpkEmbDim; ++j) x[i][(size_t)r * kSpkEmbDim + j] = (double)(row[j] / nrm);
+      }
+      dims[i] = kSpkEmbDim;
+      ks[i] = c.preset;
+    }
+    if (fa_spk_kmeans_host(x[i].data(), c.n, dims[i], ks[i], 0, 10, 300, c.labels.data()) != FA_OK) { c.err = c.what + "k-means failed"; continue; }
+    if (c.preset <= 0 && fa_spk_merge_by_cos_host(c.labels.data(), eh, c.n, kSpkEmbDim, kMergeThr) != FA_OK) c.err = c.what + "merge_by_cos failed";
   }
   return true;
 }
@@ -285,62 +353,100 @@ bool spk_cluster(Spk& s, const float* emb_d, int n, int preset, const float* emb
 
 namespace fa_handle {
 
-// sv_chunk windows over every VAD segment (vad_segment mode), gathered with zero tails and embedded in slices, clustered,
-// post-processed and distributed over the segments
-bool diarize(Spk& s, const float* rec, int64_t n, const std::vector<int32_t>& segs, int preset, std::vector<int32_t>& spk, const std::string& what) {
+// sv_chunk windows over every VAD segment of every job (vad_segment mode); each job's refusal decided from its chunk count before any
+// embedding; the chunks of the jobs that cluster gathered with zero tails and embedded together in slices, one copy of the embeddings
+// to the host; clustered together (spk_cluster); post-processed and distributed over each job's segments
+bool diarize(Spk& s, const float* recs, int64_t n_recs, std::vector<SpkJob>& jobs) {
   cudaStream_t st = s.file.st;
-  const int64_t ns = (int64_t)segs.size() / 3;
-  std::vector<int64_t> starts;
-  std::vector<double> times;
-  for (int64_t g = 0; g < ns; ++g) {                 // long_audio.speaker_chunks / diarization.chunk_bounds
-    const int64_t b0 = (int64_t)segs[3 * g] * 16, b1 = std::min<int64_t>((int64_t)segs[3 * g + 1] * 16, n), len = std::max<int64_t>(b1 - b0, 0);
-    int64_t last_ed = 0;
-    for (int64_t a = 0; a < len; a += kChunkShift) {
-      const int64_t ed = std::min<int64_t>(a + kChunkLen, len);
-      if (ed <= last_ed) break;
-      last_ed = ed;
-      const int64_t c0 = std::max<int64_t>(0, ed - kChunkLen);
-      starts.push_back(b0 + c0);
-      times.push_back((double)c0 / 16000 + (double)segs[3 * g] / 1000.0);
-      times.push_back((double)ed / 16000 + (double)segs[3 * g] / 1000.0);
-      starts.push_back(ed - c0);                     // interleaved: first sample, sample count
+  const int J = (int)jobs.size();
+  std::vector<std::vector<int64_t>> starts((size_t)J);             // per job, interleaved: first sample in recs, sample count
+  std::vector<std::vector<double>> times((size_t)J);
+  for (int q = 0; q < J; ++q) {
+    SpkJob& jb = jobs[q];
+    const std::vector<int32_t>& segs = *jb.segs;
+    const int64_t ns = (int64_t)segs.size() / 3;
+    for (int64_t g = 0; g < ns; ++g) {               // long_audio.speaker_chunks / diarization.chunk_bounds
+      const int64_t b0 = (int64_t)segs[3 * g] * 16, b1 = std::min<int64_t>((int64_t)segs[3 * g + 1] * 16, jb.n), len = std::max<int64_t>(b1 - b0, 0);
+      int64_t last_ed = 0;
+      for (int64_t a = 0; a < len; a += kChunkShift) {
+        const int64_t ed = std::min<int64_t>(a + kChunkLen, len);
+        if (ed <= last_ed) break;
+        last_ed = ed;
+        const int64_t c0 = std::max<int64_t>(0, ed - kChunkLen);
+        starts[q].push_back(jb.off + b0 + c0);
+        starts[q].push_back(ed - c0);
+        times[q].push_back((double)c0 / 16000 + (double)segs[3 * g] / 1000.0);
+        times[q].push_back((double)ed / 16000 + (double)segs[3 * g] / 1000.0);
+      }
     }
+    jb.spk->assign((size_t)ns, 0);
+    jb.err.clear();
   }
-  const int nc = (int)(starts.size() / 2);
-  spk.assign((size_t)ns, 0);
-  if (nc == 0) return true;
-  const int t_max = fbank_frames(kChunkLen);
-  const size_t per = fa_campplus_workspace_bytes(&s.model, 1, t_max, s.mode);
-  const int step = (int)std::max<size_t>(1, std::min<size_t>({(size_t)nc, kSpkWorkspaceCap / (per ? per : 1), (size_t)65535}));
-  float *emb, *wav;
-  int64_t* starts_d;
-  int32_t *lens_d, *full_d;
-  if (!carve(s.diarize, "speaker chunks", [&](fa::Arena& a) {
-        emb = a.take<float>((size_t)nc * kSpkEmbDim); wav = a.take<float>((size_t)step * kChunkLen);
-        starts_d = a.take<int64_t>(step); lens_d = a.take<int32_t>(step); full_d = a.take<int32_t>(step);
-      }))
-    return false;
-  const std::vector<int32_t> full((size_t)step, kChunkLen);    // every window counts as 1.5 s of samples, its zero tail included
-  cudaMemcpyAsync(full_d, full.data(), (size_t)step * 4, cudaMemcpyHostToDevice, st);
-  std::vector<int64_t> sb((size_t)step);
-  std::vector<int32_t> lb((size_t)step);
-  for (int c0 = 0; c0 < nc; c0 += step) {
-    const int nb = std::min(step, nc - c0);
-    if (!sync_stream(st)) return false;               // sb / lb are reused: the previous slice's copies are done
-    for (int r = 0; r < nb; ++r) { sb[r] = starts[2 * (c0 + r)]; lb[r] = (int32_t)starts[2 * (c0 + r) + 1]; }
-    if (!gather(rec, n, sb.data(), lb.data(), nb, kChunkLen, starts_d, lens_d, wav, st)) return false;
-    if (!spk_embed_rows(s, wav, kChunkLen, full_d, nb, t_max, emb + (size_t)c0 * kSpkEmbDim)) return false;
+  // the sets to cluster: every job of 20 chunks or more that is not refused, the spectral ones (fewer than 2048) first, so their rows
+  // are contiguous; fewer than 20 chunks are one speaker and need no embedding
+  std::vector<ClusterSet> sets;
+  std::vector<int> set_of((size_t)J, -1);
+  int rows = 0;
+  for (int pass = 0; pass < 2; ++pass)
+    for (int q = 0; q < J; ++q) {
+      const int nc = (int)(starts[q].size() / 2);
+      if (pass == 0) jobs[q].err = cluster_refusal(nc, jobs[q].preset, jobs[q].what);
+      if (nc < 20 || !jobs[q].err.empty() || (nc < kSpectralMaxChunks) != (pass == 0)) continue;
+      ClusterSet c;
+      c.first = rows; c.n = nc; c.preset = jobs[q].preset; c.what = jobs[q].what;
+      set_of[q] = (int)sets.size();
+      sets.push_back(std::move(c));
+      rows += nc;
+    }
+  if (rows > 0) {
+    std::vector<int64_t> win((size_t)2 * rows);      // the sets' windows in row order
+    for (int q = 0; q < J; ++q)
+      if (set_of[q] >= 0) std::copy(starts[q].begin(), starts[q].end(), win.begin() + 2 * (int64_t)sets[set_of[q]].first);
+    const int t_max = fbank_frames(kChunkLen);
+    const size_t per = fa_campplus_workspace_bytes(&s.model, 1, t_max, s.mode);
+    const int step = (int)std::max<size_t>(1, std::min<size_t>({(size_t)rows, kSpkWorkspaceCap / (per ? per : 1), (size_t)65535}));
+    float *emb, *wav;
+    int64_t* starts_d;
+    int32_t *lens_d, *full_d;
+    if (!carve(s.diarize, "speaker chunks", [&](fa::Arena& a) {
+          emb = a.take<float>((size_t)rows * kSpkEmbDim); wav = a.take<float>((size_t)step * kChunkLen);
+          starts_d = a.take<int64_t>(step); lens_d = a.take<int32_t>(step); full_d = a.take<int32_t>(step);
+        }))
+      return false;
+    const std::vector<int32_t> full((size_t)step, kChunkLen);  // every window counts as 1.5 s of samples, its zero tail included
+    cudaMemcpyAsync(full_d, full.data(), (size_t)step * 4, cudaMemcpyHostToDevice, st);
+    std::vector<int64_t> sb((size_t)step);
+    std::vector<int32_t> lb((size_t)step);
+    for (int c0 = 0; c0 < rows; c0 += step) {
+      const int nb = std::min(step, rows - c0);
+      if (!sync_stream(st)) return false;             // sb / lb are reused: the previous slice's copies are done
+      for (int r = 0; r < nb; ++r) { sb[r] = win[2 * (c0 + r)]; lb[r] = (int32_t)win[2 * (c0 + r) + 1]; }
+      if (!gather(recs, n_recs, sb.data(), lb.data(), nb, kChunkLen, starts_d, lens_d, wav, st)) return false;
+      if (!spk_embed_rows(s, wav, kChunkLen, full_d, nb, t_max, emb + (size_t)c0 * kSpkEmbDim)) return false;
+    }
+    std::vector<float> emb_h((size_t)rows * kSpkEmbDim);
+    cudaMemcpyAsync(emb_h.data(), emb, emb_h.size() * 4, cudaMemcpyDeviceToHost, st);
+    if (!sync_stream(st)) return false;
+    if (!spk_cluster(s, emb, emb_h.data(), sets)) return false;
   }
-  std::vector<float> emb_h((size_t)nc * kSpkEmbDim);
-  cudaMemcpyAsync(emb_h.data(), emb, emb_h.size() * 4, cudaMemcpyDeviceToHost, st);
-  if (!sync_stream(st)) return false;
-  std::vector<int32_t> labels;
-  if (!spk_cluster(s, emb, nc, preset, emb_h.data(), labels, what)) return false;
-  std::vector<double> turns((size_t)3 * nc);
-  const int64_t nt = fa_spk_postprocess_host(times.data(), labels.data(), nc, turns.data());
-  std::vector<int32_t> sent((size_t)2 * ns);
-  for (int64_t g = 0; g < ns; ++g) { sent[2 * g] = segs[3 * g]; sent[2 * g + 1] = segs[3 * g + 1]; }
-  if (nt < 0 || fa_spk_distribute_host(sent.data(), ns, turns.data(), nt, spk.data()) != FA_OK) { set_err(what + "speaker post-processing failed"); return false; }
+  for (int q = 0; q < J; ++q) {
+    SpkJob& jb = jobs[q];
+    const int nc = (int)(starts[q].size() / 2);
+    if (nc == 0 || !jb.err.empty()) continue;
+    std::vector<int32_t> labels((size_t)nc, 0);      // fewer than 20 chunks: one speaker
+    if (set_of[q] >= 0) {
+      ClusterSet& c = sets[set_of[q]];
+      if (!c.err.empty()) { jb.err = c.err; continue; }
+      labels.swap(c.labels);
+    }
+    const std::vector<int32_t>& segs = *jb.segs;
+    const int64_t ns = (int64_t)segs.size() / 3;
+    std::vector<double> turns((size_t)3 * nc);
+    const int64_t nt = fa_spk_postprocess_host(times[q].data(), labels.data(), nc, turns.data());
+    std::vector<int32_t> sent((size_t)2 * ns);
+    for (int64_t g = 0; g < ns; ++g) { sent[2 * g] = segs[3 * g]; sent[2 * g + 1] = segs[3 * g + 1]; }
+    if (nt < 0 || fa_spk_distribute_host(sent.data(), ns, turns.data(), nt, jb.spk->data()) != FA_OK) jb.err = jb.what + "speaker post-processing failed";
+  }
   return true;
 }
 
@@ -422,14 +528,18 @@ extern "C" int fa_spk_cluster(void* spk, const float* emb_host, int32_t n, int32
   }
   std::lock_guard<std::mutex> dev(s->mu);
   cudaSetDevice(s->file.device);
-  std::vector<int32_t> lab;
+  std::vector<ClusterSet> sets(1);
+  sets[0].n = n;
+  sets[0].preset = preset_spk_num;
   const bool ok = no_throw("fa_spk_cluster: ", [&] {
     float* emb;
     if (!carve(s->cluster_input, "speaker clustering", [&](fa::Arena& a) { emb = a.take<float>((size_t)n * kSpkEmbDim); })) return false;
     cudaMemcpyAsync(emb, emb_host, (size_t)n * kSpkEmbDim * 4, cudaMemcpyHostToDevice, s->file.st);
-    return spk_cluster(*s, emb, n, preset_spk_num, emb_host, lab, "");
+    if (!spk_cluster(*s, emb, emb_host, sets)) return false;
+    if (!sets[0].err.empty()) { set_err(sets[0].err); return false; }
+    return true;
   });
   if (!ok) return FA_ERR_CUDA;
-  std::copy(lab.begin(), lab.end(), labels);
+  std::copy(sets[0].labels.begin(), sets[0].labels.end(), labels);
   return FA_OK;
 }

@@ -7,15 +7,78 @@
 //                           column (reflector, symmetric mat-vec, rank-2 update); the reflectors stay in the matrix
 //   fa_spk_back_transform   Q z for the few tridiagonal eigenvectors the clustering uses
 //
+// Each has a _batch form over a ragged set of independent problems (a group's recordings), and the single entry is its one-set case.
+// The set is a grid dimension and a CTA past its set's extent returns at once, so the batch makes the launches of its largest set
+// (at most kSetsPerLaunch sets per launch) and every set does the same IEEE operations, in the same order, as it does alone.
+//
 // The small tridiagonal eigenproblem, the k-means and the post-processing run on the host (host_ops.cpp).  No launch waits on another
 // CTA: there is no cooperative launch and no grid-wide barrier, every dependency is a kernel boundary on the caller's stream.
 #include "common.cuh"
+#include <vector>
 
 namespace {
 
 constexpr int kMaxRows = 2047;          // the spectral path's largest input (ClusterBackend: fewer than 2048 chunks)
 constexpr int kSortKeys = 2048;
 constexpr int kMaxDim = 1024;
+constexpr int kSetsPerLaunch = 64;      // sets per launch of a batch: Sets<64> is a 2.5 KB kernel parameter, read in place (__grid_constant__)
+
+// Sets [first, first + count) of a batch, concatenated in set order: set s has n[s] rows, starts at row row[s] of the embeddings and
+// of d / e / tau / v / p, at entry mat[s] of the matrices, at partial part[s] of the symv partials and at entry z[s] of z
+template <int C>
+struct Sets {
+  int count;
+  int n[C];
+  int aux[C];                           // the Laplacian: the entries pruned per row; the back-transform: k
+  int64_t row[C], mat[C], part[C], z[C];
+  int max_n() const { int m = 0; for (int i = 0; i < count; ++i) m = n[i] > m ? n[i] : m; return m; }
+  int max_aux() const { int m = 0; for (int i = 0; i < count; ++i) m = aux[i] > m ? aux[i] : m; return m; }
+};
+
+// the batch's sets in launches of C, with their offsets (aux: NULL = 0; k: the back-transform's vectors per set)
+template <int C>
+std::vector<Sets<C>> make_sets(const int32_t* n, int32_t count, const int32_t* aux, const int32_t* k) {
+  std::vector<Sets<C>> out;
+  int64_t row = 0, mat = 0, part = 0, z = 0;
+  for (int i = 0; i < count; ++i) {
+    if (i % C == 0) out.push_back(Sets<C>{});
+    Sets<C>& s = out.back();
+    const int c = s.count++;
+    s.n[c] = n[i]; s.aux[c] = aux ? aux[i] : 0;
+    s.row[c] = row; s.mat[c] = mat; s.part[c] = part; s.z[c] = z;
+    row += n[i]; mat += (int64_t)n[i] * n[i]; part += (n[i] + 7) / 8; z += k ? (int64_t)k[i] * n[i] : 0;
+  }
+  return out;
+}
+
+// f(sets) -> status for each launch group of the batch, the first failure returned.  A one-set batch (the single entries) passes a
+// one-set parameter block, so its launches carry no larger parameters than the single entries always had.
+template <class F>
+int for_sets(const int32_t* n, int32_t count, const int32_t* aux, const int32_t* k, F f) {
+  if (count == 1) return f(make_sets<1>(n, count, aux, k)[0]);
+  for (const Sets<kSetsPerLaunch>& c : make_sets<kSetsPerLaunch>(n, count, aux, k)) {
+    const int rc = f(c);
+    if (rc != FA_OK) return rc;
+  }
+  return FA_OK;
+}
+
+// FA_OK, FA_ERR_ARG (NULL n, count < 1, an n[s] < 1) or FA_ERR_UNSUPPORTED (an n[s] > kMaxRows): the single entries' codes for n
+int check_sizes(const int32_t* n, int32_t count) {
+  if (!n || count < 1) return FA_ERR_ARG;
+  bool big = false;
+  for (int i = 0; i < count; ++i) {
+    if (n[i] < 1) return FA_ERR_ARG;
+    big = big || n[i] > kMaxRows;
+  }
+  return big ? FA_ERR_UNSUPPORTED : FA_OK;
+}
+
+int64_t sum_n(const int32_t* n, int32_t count, bool squares) {
+  int64_t t = 0;
+  for (int i = 0; i < count; ++i) t += squares ? (int64_t)n[i] * n[i] : n[i];
+  return t;
+}
 
 // ---- Laplacian
 
@@ -32,11 +95,16 @@ __global__ void __launch_bounds__(256) normalize_rows_kernel(const float* __rest
   for (int c = lane; c < dim; c += 32) xn[(int64_t)row * dim + c] = r[c] / nrm;
 }
 
-// s = xn xn^T in fp32: 64 x 64 output tiles, 4 x 4 per thread, 16-wide slices of the inner dimension
-__global__ void __launch_bounds__(256) cosine_kernel(const float* __restrict__ xn, int n, int dim, float* __restrict__ s) {
+// s = xn xn^T in fp32 per set (blockIdx.z): 64 x 64 output tiles, 4 x 4 per thread, 16-wide slices of the inner dimension
+template <class S>
+__global__ void __launch_bounds__(256) cosine_kernel(const float* __restrict__ xn, int dim, float* __restrict__ s, const __grid_constant__ S sets) {
   __shared__ float a[16][64 + 1], b[16][64 + 1];
+  const int n = sets.n[blockIdx.z];
   const int tx = threadIdx.x % 16, ty = threadIdx.x / 16;
   const int r0 = blockIdx.y * 64, c0 = blockIdx.x * 64;
+  if (r0 >= n || c0 >= n) return;
+  xn += sets.row[blockIdx.z] * dim;
+  s += sets.mat[blockIdx.z];
   float acc[4][4] = {};
   for (int k0 = 0; k0 < dim; k0 += 16) {
     for (int e = threadIdx.x; e < 16 * 64; e += 256) {
@@ -67,12 +135,16 @@ __device__ __forceinline__ uint32_t ordered_bits(float f) {     // ascending flo
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
-// p_pruning: the n_elems smallest entries of row blockIdx.x become 0, in place.  Keys (value, column) sorted ascending in shared
-// memory by a bitonic network, so equal values go in column order (numpy's argsort is unstable: the one place the two may differ).
-__global__ void __launch_bounds__(1024) prune_rows_kernel(float* __restrict__ s, int n, int n_elems) {
+// p_pruning: the n_elems smallest entries of row blockIdx.x of set blockIdx.y become 0, in place.  Keys (value, column) sorted ascending
+// in shared memory by a bitonic network, so equal values go in column order (numpy's argsort is unstable: the one place the two may
+// differ).
+template <class S>
+__global__ void __launch_bounds__(1024) prune_rows_kernel(float* __restrict__ s, const __grid_constant__ S sets) {
   __shared__ unsigned long long keys[kSortKeys];
   __shared__ unsigned char drop[kSortKeys];
-  float* row = s + (int64_t)blockIdx.x * n;
+  const int n = sets.n[blockIdx.y], n_elems = sets.aux[blockIdx.y];
+  if ((int)blockIdx.x >= n || n_elems <= 0) return;
+  float* row = s + sets.mat[blockIdx.y] + (int64_t)blockIdx.x * n;
   for (int c = threadIdx.x; c < kSortKeys; c += blockDim.x) {
     keys[c] = c < n ? ((unsigned long long)ordered_bits(row[c]) << 32) | (unsigned)c : ~0ull;
     drop[c] = 0;
@@ -105,10 +177,15 @@ __device__ __forceinline__ double block_sum(double v, double* red) {   // every 
   return t;
 }
 
-// m = 0.5 (p + p^T) (fp32) with a zero diagonal; lap row i = diag(sum_j |m_ij|) - m, float64.  One CTA per row.
-__global__ void __launch_bounds__(256) laplacian_kernel(const float* __restrict__ p, int n, double* __restrict__ lap) {
+// m = 0.5 (p + p^T) (fp32) with a zero diagonal; lap row i = diag(sum_j |m_ij|) - m, float64.  One CTA per row (blockIdx.x) of
+// each set (blockIdx.y).
+template <class S>
+__global__ void __launch_bounds__(256) laplacian_kernel(const float* __restrict__ p, double* __restrict__ lap, const __grid_constant__ S sets) {
   __shared__ double red[8];
-  const int i = blockIdx.x;
+  const int i = blockIdx.x, n = sets.n[blockIdx.y];
+  if (i >= n) return;
+  p += sets.mat[blockIdx.y];
+  lap += sets.mat[blockIdx.y];
   double deg = 0.0;
   for (int j = threadIdx.x; j < n; j += blockDim.x) {
     const float m = j == i ? 0.f : 0.5f * (p[(int64_t)i * n + j] + p[(int64_t)j * n + i]);
@@ -123,10 +200,16 @@ __global__ void __launch_bounds__(256) laplacian_kernel(const float* __restrict_
 
 // Column j: the reflector H = I - tau v v^T with H a[j+1:, j] = (beta, 0, ...).  Reads row j (the matrix is kept exactly symmetric);
 // writes d[j], e[j], tau[j], v (v[0] = 1) to vbuf, and keeps v[1:] in lap below the subdiagonal of column j and right of the
-// superdiagonal of row j (the back-transform reads the row).  j == n - 1 only writes d[n - 1].
-__global__ void __launch_bounds__(1024) reflector_kernel(double* __restrict__ lap, int n, int j, double* __restrict__ d, double* __restrict__ e,
-                                                         double* __restrict__ tau, double* __restrict__ vbuf) {
+// superdiagonal of row j (the back-transform reads the row).  j == n - 1 only writes d[n - 1]; a set with j >= n is done.  One CTA per
+// set (blockIdx.x).
+template <class S>
+__global__ void __launch_bounds__(1024) reflector_kernel(double* __restrict__ lap, int j, double* __restrict__ d, double* __restrict__ e,
+                                                         double* __restrict__ tau, double* __restrict__ vbuf, const __grid_constant__ S sets) {
   __shared__ double red[32];
+  const int n = sets.n[blockIdx.x];
+  if (j >= n) return;
+  const int64_t o = sets.row[blockIdx.x];
+  lap += sets.mat[blockIdx.x]; d += o; e += o; tau += o; vbuf += o;
   double* row = lap + (int64_t)j * n;
   const int m = n - j - 1;
   if (threadIdx.x == 0) d[j] = row[j];
@@ -153,12 +236,17 @@ __global__ void __launch_bounds__(1024) reflector_kernel(double* __restrict__ la
 }
 
 // p = tau A22 v over the trailing block A22 = lap[j+1:, j+1:], one warp per row; partial[blockIdx.x] = sum of p_t v_t over the block's
-// rows (fixed order, so the rank-2 update is deterministic)
-__global__ void __launch_bounds__(256) symv_kernel(const double* __restrict__ lap, int n, int j, const double* __restrict__ tau,
-                                                   const double* __restrict__ vbuf, double* __restrict__ p, double* __restrict__ partial) {
+// rows (fixed order, so the rank-2 update is deterministic).  Set blockIdx.y has (m + 7) / 8 blocks.
+template <class S>
+__global__ void __launch_bounds__(256) symv_kernel(const double* __restrict__ lap, int j, const double* __restrict__ tau,
+                                                   const double* __restrict__ vbuf, double* __restrict__ p, double* __restrict__ partial,
+                                                   const __grid_constant__ S sets) {
   __shared__ double v[kMaxRows];
   __shared__ double pv[8];
-  const int m = n - j - 1, off = j + 1;
+  const int n = sets.n[blockIdx.y], m = n - j - 1, off = j + 1;
+  if (m <= 0 || (int)blockIdx.x >= (m + 7) / 8) return;
+  const int64_t o = sets.row[blockIdx.y];
+  lap += sets.mat[blockIdx.y]; tau += o; vbuf += o; p += o; partial += sets.part[blockIdx.y];
   for (int t = threadIdx.x; t < m; t += blockDim.x) v[t] = vbuf[t];
   __syncthreads();
   const int w = threadIdx.x / 32, lane = threadIdx.x % 32, r = blockIdx.x * 8 + w;
@@ -183,12 +271,16 @@ __global__ void __launch_bounds__(256) symv_kernel(const double* __restrict__ la
 }
 
 // A22 -= v w^T + w v^T with w = p - (tau / 2)(p^T v) v.  Each entry's two products are rounded and added without contraction, so the
-// updated matrix stays exactly symmetric.  32 x 32 tiles, 4 rows per thread.
-__global__ void __launch_bounds__(256) rank2_kernel(double* __restrict__ lap, int n, int j, const double* __restrict__ tau,
+// updated matrix stays exactly symmetric.  32 x 32 tiles, 4 rows per thread; set blockIdx.z has (m + 31) / 32 tiles a side.
+template <class S>
+__global__ void __launch_bounds__(256) rank2_kernel(double* __restrict__ lap, int j, const double* __restrict__ tau,
                                                     const double* __restrict__ vbuf, const double* __restrict__ p,
-                                                    const double* __restrict__ partial, int n_partial) {
+                                                    const double* __restrict__ partial, const __grid_constant__ S sets) {
   __shared__ double c_sh;
-  const int m = n - j - 1, off = j + 1;
+  const int n = sets.n[blockIdx.z], m = n - j - 1, off = j + 1, n_partial = (m + 7) / 8;
+  if (m <= 0 || (int)blockIdx.x * 32 >= m || (int)blockIdx.y * 32 >= m) return;
+  const int64_t o = sets.row[blockIdx.z];
+  lap += sets.mat[blockIdx.z]; tau += o; vbuf += o; p += o; partial += sets.part[blockIdx.z];
   if (threadIdx.x == 0) {
     double pv = 0.0;
     for (int k = 0; k < n_partial; ++k) pv += partial[k];
@@ -208,12 +300,18 @@ __global__ void __launch_bounds__(256) rank2_kernel(double* __restrict__ lap, in
   }
 }
 
-// z (row blockIdx.x of z [k, n]) := H(0) H(1) ... H(n-2) z, applied last reflector first.  One CTA per vector, z in shared memory.
-__global__ void __launch_bounds__(512) back_transform_kernel(const double* __restrict__ lap, const double* __restrict__ tau, int n,
-                                                             double* __restrict__ z) {
+// z (row blockIdx.x of set blockIdx.y's z [k, n]) := H(0) H(1) ... H(n-2) z, applied last reflector first.  One CTA per (vector, set),
+// z in shared memory; n == 1 leaves z as it is.
+template <class S>
+__global__ void __launch_bounds__(512) back_transform_kernel(const double* __restrict__ lap, const double* __restrict__ tau, double* __restrict__ z,
+                                                             const __grid_constant__ S sets) {
   __shared__ double zs[kMaxRows];
   __shared__ double red[16];
-  double* zr = z + (int64_t)blockIdx.x * n;
+  const int n = sets.n[blockIdx.y];
+  if ((int)blockIdx.x >= sets.aux[blockIdx.y] || n == 1) return;
+  lap += sets.mat[blockIdx.y];
+  tau += sets.row[blockIdx.y];
+  double* zr = z + sets.z[blockIdx.y] + (int64_t)blockIdx.x * n;
   for (int t = threadIdx.x; t < n; t += blockDim.x) zs[t] = zr[t];
   __syncthreads();
   for (int j = n - 2; j >= 0; --j) {
@@ -230,11 +328,20 @@ __global__ void __launch_bounds__(512) back_transform_kernel(const double* __res
   for (int t = threadIdx.x; t < n; t += blockDim.x) zr[t] = zs[t];
 }
 
-// tridiagonalisation workspace: v [n], p [n], one partial per symv block
-fa::Arena tri_carve(fa::Arena a, int n, double** v, double** p, double** partial) {
-  *v = a.take<double>(n);
-  *p = a.take<double>(n);
-  *partial = a.take<double>((n + 7) / 8);
+// Laplacian workspace: the normalised rows [sum n, dim] and the similarities [sum n^2], fp32
+fa::Arena lap_carve(fa::Arena a, const int32_t* n, int32_t count, int dim, float** xn, float** s) {
+  *xn = a.take<float>((size_t)sum_n(n, count, false) * dim);
+  *s = a.take<float>((size_t)sum_n(n, count, true));
+  return a;
+}
+
+// tridiagonalisation workspace: v [sum n], p [sum n], one partial per symv block of each set
+fa::Arena tri_carve(fa::Arena a, const int32_t* n, int32_t count, double** v, double** p, double** partial) {
+  int64_t parts = 0;
+  for (int i = 0; i < count; ++i) parts += (n[i] + 7) / 8;
+  *v = a.take<double>((size_t)sum_n(n, count, false));
+  *p = a.take<double>((size_t)sum_n(n, count, false));
+  *partial = a.take<double>((size_t)parts);
   return a;
 }
 
@@ -242,71 +349,110 @@ fa::Arena tri_carve(fa::Arena a, int n, double** v, double** p, double** partial
 
 extern "C" double fa_spk_effective_pval(int32_t n, double pval) { return n * pval < 6 ? 6.0 / n : pval; }
 
-extern "C" size_t fa_spk_laplacian_workspace_bytes(int32_t n, int32_t dim) {
-  if (n < 1 || n > kMaxRows || dim < 1 || dim > kMaxDim) return 0;
-  fa::Arena a = fa::Arena::measuring();
-  a.take<float>((size_t)n * dim);
-  a.take<float>((size_t)n * n);
-  return a.bytes();
+extern "C" size_t fa_spk_laplacian_batch_workspace_bytes(const int32_t* n, int32_t count, int32_t dim) {
+  if (check_sizes(n, count) != FA_OK || dim < 1 || dim > kMaxDim) return 0;
+  float *xn, *s;
+  return lap_carve(fa::Arena::measuring(), n, count, dim, &xn, &s).bytes();
+}
+
+extern "C" size_t fa_spk_laplacian_workspace_bytes(int32_t n, int32_t dim) { return fa_spk_laplacian_batch_workspace_bytes(&n, 1, dim); }
+
+extern "C" int fa_spk_laplacian_batch(const float* emb, const int32_t* n, int32_t count, int32_t dim, double pval, double* lap, void* workspace,
+                                      size_t ws_bytes, fa_stream_t stream) {
+  const int sizes = check_sizes(n, count);
+  if (!emb || !lap || sizes == FA_ERR_ARG || dim < 1 || !(pval >= 0.0 && pval <= 1.0)) return FA_ERR_ARG;
+  if (sizes != FA_OK || dim > kMaxDim) return FA_ERR_UNSUPPORTED;
+  float *xn, *s;
+  const fa::Arena a = lap_carve(fa::Arena(workspace, ws_bytes), n, count, dim, &xn, &s);
+  if (!a.ok() || !xn || !s) return FA_ERR_WORKSPACE;
+  std::vector<int32_t> n_elems((size_t)count);
+  for (int i = 0; i < count; ++i) {
+    const double pv = fa_spk_effective_pval(n[i], pval);
+    n_elems[i] = (int)((1 - pv) * n[i]);                    // int((1 - pval) * n): float64, truncated
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t rows = sum_n(n, count, false);
+  normalize_rows_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(emb, (int)rows, dim, xn);
+  FA_CHECK_LAUNCH();
+  return for_sets(n, count, n_elems.data(), nullptr, [&](const auto& c) {
+    const int nmax = c.max_n(), tiles = (nmax + 63) / 64;
+    cosine_kernel<<<dim3(tiles, tiles, c.count), 256, 0, st>>>(xn, dim, s, c);
+    FA_CHECK_LAUNCH();
+    if (c.max_aux() > 0) {
+      prune_rows_kernel<<<dim3(nmax, c.count), 1024, 0, st>>>(s, c);
+      FA_CHECK_LAUNCH();
+    }
+    laplacian_kernel<<<dim3(nmax, c.count), 256, 0, st>>>(s, lap, c);
+    FA_CHECK_LAUNCH();
+    return FA_OK;
+  });
 }
 
 extern "C" int fa_spk_laplacian(const float* emb, int32_t n, int32_t dim, double pval, double* lap, void* workspace, size_t ws_bytes,
                                 fa_stream_t stream) {
-  if (!emb || !lap || n < 1 || dim < 1 || !(pval >= 0.0 && pval <= 1.0)) return FA_ERR_ARG;
-  if (n > kMaxRows || dim > kMaxDim) return FA_ERR_UNSUPPORTED;
-  fa::Arena a(workspace, ws_bytes);
-  float* xn = a.take<float>((size_t)n * dim);
-  float* s = a.take<float>((size_t)n * n);
-  if (!a.ok() || !xn || !s) return FA_ERR_WORKSPACE;
-  const double pv = fa_spk_effective_pval(n, pval);
-  const int n_elems = (int)((1 - pv) * n);                  // int((1 - pval) * n): float64, truncated
-  cudaStream_t st = (cudaStream_t)stream;
-  normalize_rows_kernel<<<(n + 7) / 8, 256, 0, st>>>(emb, n, dim, xn);
-  FA_CHECK_LAUNCH();
-  cosine_kernel<<<dim3((n + 63) / 64, (n + 63) / 64), 256, 0, st>>>(xn, n, dim, s);
-  FA_CHECK_LAUNCH();
-  if (n_elems > 0) {
-    prune_rows_kernel<<<n, 1024, 0, st>>>(s, n, n_elems);
-    FA_CHECK_LAUNCH();
-  }
-  laplacian_kernel<<<n, 256, 0, st>>>(s, n, lap);
-  FA_CHECK_LAUNCH();
-  return FA_OK;
+  return fa_spk_laplacian_batch(emb, &n, 1, dim, pval, lap, workspace, ws_bytes, stream);
 }
 
-extern "C" size_t fa_spk_tridiagonalize_workspace_bytes(int32_t n) {
-  if (n < 1 || n > kMaxRows) return 0;
+extern "C" size_t fa_spk_tridiagonalize_batch_workspace_bytes(const int32_t* n, int32_t count) {
+  if (check_sizes(n, count) != FA_OK) return 0;
   double *v, *p, *partial;
-  return tri_carve(fa::Arena::measuring(), n, &v, &p, &partial).bytes();
+  return tri_carve(fa::Arena::measuring(), n, count, &v, &p, &partial).bytes();
+}
+
+extern "C" size_t fa_spk_tridiagonalize_workspace_bytes(int32_t n) { return fa_spk_tridiagonalize_batch_workspace_bytes(&n, 1); }
+
+// Column j runs for every set with j < n in one launch each of the reflector, symv and rank-2 kernels: 3 (max n - 1) + 1 launches
+extern "C" int fa_spk_tridiagonalize_batch(double* lap, const int32_t* n, int32_t count, double* d, double* e, double* tau, void* workspace,
+                                           size_t ws_bytes, fa_stream_t stream) {
+  const int sizes = check_sizes(n, count);
+  if (!lap || !d || sizes == FA_ERR_ARG) return FA_ERR_ARG;
+  for (int i = 0; i < count; ++i)
+    if (n[i] > 1 && (!e || !tau)) return FA_ERR_ARG;
+  if (sizes != FA_OK) return FA_ERR_UNSUPPORTED;
+  double *v, *p, *partial;
+  const fa::Arena a = tri_carve(fa::Arena(workspace, ws_bytes), n, count, &v, &p, &partial);
+  if (!a.ok() || !v || !p || !partial) return FA_ERR_WORKSPACE;
+  cudaStream_t st = (cudaStream_t)stream;
+  return for_sets(n, count, nullptr, nullptr, [&](const auto& c) {
+    const int nmax = c.max_n();
+    for (int j = 0; j < nmax - 1; ++j) {
+      const int m = nmax - j - 1, blocks = (m + 7) / 8, tiles = (m + 31) / 32;
+      reflector_kernel<<<c.count, 1024, 0, st>>>(lap, j, d, e, tau, v, c);
+      FA_CHECK_LAUNCH();
+      symv_kernel<<<dim3(blocks, c.count), 256, 0, st>>>(lap, j, tau, v, p, partial, c);
+      FA_CHECK_LAUNCH();
+      rank2_kernel<<<dim3(tiles, tiles, c.count), 256, 0, st>>>(lap, j, tau, v, p, partial, c);
+      FA_CHECK_LAUNCH();
+    }
+    reflector_kernel<<<c.count, 1024, 0, st>>>(lap, nmax - 1, d, e, tau, v, c);
+    FA_CHECK_LAUNCH();
+    return FA_OK;
+  });
 }
 
 extern "C" int fa_spk_tridiagonalize(double* lap, int32_t n, double* d, double* e, double* tau, void* workspace, size_t ws_bytes,
                                      fa_stream_t stream) {
-  if (!lap || !d || n < 1 || (n > 1 && (!e || !tau))) return FA_ERR_ARG;
-  if (n > kMaxRows) return FA_ERR_UNSUPPORTED;
-  double *v, *p, *partial;
-  const fa::Arena a = tri_carve(fa::Arena(workspace, ws_bytes), n, &v, &p, &partial);
-  if (!a.ok() || !v || !p || !partial) return FA_ERR_WORKSPACE;
-  cudaStream_t st = (cudaStream_t)stream;
-  for (int j = 0; j < n - 1; ++j) {
-    const int m = n - j - 1, blocks = (m + 7) / 8, tiles = (m + 31) / 32;
-    reflector_kernel<<<1, 1024, 0, st>>>(lap, n, j, d, e, tau, v);
-    FA_CHECK_LAUNCH();
-    symv_kernel<<<blocks, 256, 0, st>>>(lap, n, j, tau, v, p, partial);
-    FA_CHECK_LAUNCH();
-    rank2_kernel<<<dim3(tiles, tiles), 256, 0, st>>>(lap, n, j, tau, v, p, partial, blocks);
-    FA_CHECK_LAUNCH();
+  return fa_spk_tridiagonalize_batch(lap, &n, 1, d, e, tau, workspace, ws_bytes, stream);
+}
+
+extern "C" int fa_spk_back_transform_batch(const double* lap, const double* tau, const int32_t* n, const int32_t* k, int32_t count, double* z,
+                                           fa_stream_t stream) {
+  const int sizes = check_sizes(n, count);
+  if (!lap || !z || !k || sizes == FA_ERR_ARG) return FA_ERR_ARG;
+  bool any = false;                                          // a set with n > 1: n == 1 leaves its z as it is
+  for (int i = 0; i < count; ++i) {
+    if (k[i] < 1 || k[i] > n[i] || (n[i] > 1 && !tau)) return FA_ERR_ARG;
+    any = any || n[i] > 1;
   }
-  reflector_kernel<<<1, 1024, 0, st>>>(lap, n, n - 1, d, e, tau, v);
-  FA_CHECK_LAUNCH();
-  return FA_OK;
+  if (sizes != FA_OK) return FA_ERR_UNSUPPORTED;
+  if (!any) return FA_OK;
+  return for_sets(n, count, k, k, [&](const auto& c) {
+    back_transform_kernel<<<dim3(c.max_aux(), c.count), 512, 0, (cudaStream_t)stream>>>(lap, tau, z, c);
+    FA_CHECK_LAUNCH();
+    return FA_OK;
+  });
 }
 
 extern "C" int fa_spk_back_transform(const double* lap, const double* tau, int32_t n, double* z, int32_t k, fa_stream_t stream) {
-  if (!lap || !z || n < 1 || k < 1 || k > n || (n > 1 && !tau)) return FA_ERR_ARG;
-  if (n > kMaxRows || k > 65535) return FA_ERR_UNSUPPORTED;
-  if (n == 1) return FA_OK;
-  back_transform_kernel<<<k, 512, 0, (cudaStream_t)stream>>>(lap, tau, n, z);
-  FA_CHECK_LAUNCH();
-  return FA_OK;
+  return fa_spk_back_transform_batch(lap, tau, &n, &k, 1, z, stream);
 }

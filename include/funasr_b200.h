@@ -827,8 +827,10 @@ const char* fa_offline_last_error(void);
  * utterance of a batch that batch's hotword memory (for SeACo with more rows than nfilter, the rows the filter picks on the batch's
  * utterance 0), so each reference pack keeps its own memory and each row attends over its own (fa_attention_grouped); identical rows
  * (the same count and bytes) are one memory per pack, and a pack holds at most 4096 memory rows (memories x the longest).  Diarized
- * calls (fa_offline_infer_vad_spk) pass through the same queue but never share a pack with another call; long-audio calls share
- * passes only with the same VAD handle and FaLongAudioOptions.
+ * calls (fa_offline_infer_vad_spk, fa_offline_infer_vad_audio with a speaker handle) share packs too, and each group of a pass runs
+ * one speaker stage over all of its diarized recordings (each still clustered on its own); a refusal of that stage fails only its own
+ * call.  Long-audio calls share passes only with the same VAD handle and FaLongAudioOptions, diarized calls only with the same
+ * speaker handle (preset_spk_num may differ).
  * A device failure during a pass fails every call of that pass with its message.  Other handles' calls hold the handle's lock
  * for their device work and run one after another.  A call that uses several handles (fa_offline_infer_vad*) locks them in the order
  * recogniser, VAD, speaker, so recognisers that share a VAD handle cannot deadlock.  fa_offline_last_error is per thread.  Uninit a
@@ -930,7 +932,11 @@ int fa_spk_cluster(void* spk, const float* emb_host, int32_t n, int32_t preset_s
  * recording that decoded at least one token, by LongAudioPipeline.generate's diarization in vad_segment mode: sv_chunk's 1.5 s windows
  * every 0.75 s over each VAD segment (the last pulled back), gathered from the device-resident recording with zero tails
  * (fa_gather_segments) and embedded in slices, clustered as fa_spk_cluster (preset_spk_num <= 0: none), post-processed (postprocess,
- * distribute_spk) -> one speaker per segment: fa_offline_result_spk.  spk must live on the recogniser's device.  NULL on error. */
+ * distribute_spk) -> one speaker per segment: fa_offline_result_spk.  The recordings of a pass's group are diarized together: their
+ * chunks embedded in shared slices with one host copy, the spectral recordings clustered through the _batch entries below, each with
+ * exactly its own result.  Refusals are decided from the chunk counts before any embedding, in ClusterBackend's order (fewer than 20
+ * chunks: one speaker; then preset_spk_num above the chunk count, or 2048 or more chunks without one), named "recording i: "; a call
+ * with several recordings fails with the first in recording order.  spk must live on the recogniser's device.  NULL on error. */
 void* fa_offline_infer_vad_spk(void* asr, void* vad, void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch,
                                int32_t pcm_format, const float* hw_embed, int32_t n_hotwords, const int32_t* language_ids,
                                const int32_t* textnorm_ids, const FaLongAudioOptions* opts, int32_t preset_spk_num);
@@ -998,6 +1004,24 @@ int fa_spk_tridiagonalize(double* lap, int32_t n, double* d, double* e, double* 
 /* z [k, n] (device, one tridiagonal eigenvector per row) := Q z with fa_spk_tridiagonalize's reflectors (lap, tau): the eigenvectors
  * of the Laplacian.  One CTA per vector. */
 int fa_spk_back_transform(const double* lap, const double* tau, int32_t n, double* z, int32_t k, fa_stream_t stream);
+/* The three above over a ragged batch of count independent problems of n[s] rows (host arrays; the entry derives the offsets):
+ * embeddings emb [sum n, dim], matrices lap [sum n^2], d / e / tau [sum n] each and z [sum k[s] n[s]] concatenated in set order (set
+ * s's e holds n[s] - 1 entries of its n[s]).  Each set gets exactly what the single entry gives it (its own effective pval and pruned
+ * entries; its own symv partials summed in the same order), and the single entries are the count = 1 case with the same workspace.
+ * One launch sequence serves up to 64 sets, a larger batch one sequence per 64: the Laplacian is one row normalisation over all rows
+ * and, per sequence, one cosine-tile, one pruning and one Laplacian launch; the tridiagonalisation runs column j of every set with
+ * j < n[s] - 1 in one launch each of its three kernels, 3 (max n - 1) + 1 launches; the back-transform is one CTA per (vector, set).
+ * Before any launch: a NULL array, count < 1, any n[s] < 1, k[s] < 1 or k[s] > n[s], dim < 1, a bad pval (FA_ERR_ARG), any
+ * n[s] > 2047 or dim > 1024 (FA_ERR_UNSUPPORTED), a short workspace (FA_ERR_WORKSPACE).  The workspace queries return 0 for those
+ * shapes. */
+size_t fa_spk_laplacian_batch_workspace_bytes(const int32_t* n, int32_t count, int32_t dim);
+int fa_spk_laplacian_batch(const float* emb, const int32_t* n, int32_t count, int32_t dim, double pval, double* lap, void* workspace,
+                           size_t ws_bytes, fa_stream_t stream);
+size_t fa_spk_tridiagonalize_batch_workspace_bytes(const int32_t* n, int32_t count);
+int fa_spk_tridiagonalize_batch(double* lap, const int32_t* n, int32_t count, double* d, double* e, double* tau, void* workspace,
+                                size_t ws_bytes, fa_stream_t stream);
+int fa_spk_back_transform_batch(const double* lap, const double* tau, const int32_t* n, const int32_t* k, int32_t count, double* z,
+                                fa_stream_t stream);
 /* Host only.  The m smallest eigenvalues w [m] of the symmetric tridiagonal (d [n], e [n - 1]) by bisection with Sturm counts, and the
  * eigenvectors of the first k (k <= m) as rows of z [k, n] by inverse iteration, Gram-Schmidt within clusters of close eigenvalues. */
 int fa_sym_tridiag_smallest_host(const double* d, const double* e, int32_t n, int32_t m, int32_t k, double* w, double* z);
