@@ -303,6 +303,8 @@ SIGNATURES = {
     "fa_punc_uninit": (None, [_vp]),
     "fa_punc_walk_host": (_vp, [C.POINTER(C.c_char_p), _i32, C.POINTER(C.c_char_p), _i32, C.POINTER(C.c_char_p), _i32, _i32, _i32, _i64,
                                 PUNC_SCORE_FN, _vp]),
+    "fa_punc_init_host": (_vp, [C.POINTER(C.c_char_p), _i32, C.POINTER(C.c_char_p), _i32, _i32, _i32, _i64, PUNC_SCORE_FN, _vp]),
+    "fa_punc_pool_stats": (C.c_int, [_vp, C.POINTER(_i64), C.POINTER(_i64)]),
 }
 
 

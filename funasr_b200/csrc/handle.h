@@ -8,7 +8,7 @@
 //   offline_spk.cu   CAM++ speaker embeddings, clustering, diarization: fa_spk_*
 //   offline_long.cu  long audio: fa_offline_infer_vad*, fa_offline_result_{segments,spk}
 //   offline_pool.cu  the recogniser's request pool: every decoding call's passes, GPU packs and scatter; fa_offline_pool_stats
-//   offline_punc.cu  CT-Transformer punctuation: fa_punc_*
+//   offline_punc.cu  CT-Transformer punctuation and its request pool (concurrent calls share lockstep steps): fa_punc_*
 //   offline_align.cu MonotonicAligner (fa-zh) forced alignment: fa_align_*
 #pragma once
 #include "common.cuh"
@@ -276,7 +276,8 @@ const T* result_row(const std::vector<std::vector<T>>* rows, int32_t index, int3
 // stream and buffers; argument checks run before it is taken.  A call that needs several handles takes their locks in one order,
 // recogniser -> VAD -> speaker (-> punctuation, aligner: never held with another), so two recognisers sharing a VAD cannot deadlock.
 // The recogniser's decoding calls do not take `mu` themselves: they post a Ticket to the handle's request pool (offline_pool.cu), and
-// the thread that leads the next pass decodes every queued compatible call in shared GPU packs.
+// the thread that leads the next pass decodes every queued compatible call in shared GPU packs.  Punctuation calls likewise post to
+// their handle's pool (offline_punc.cu), whose leader takes the punctuation lock for each lockstep step.
 struct Vad;
 struct Spk;
 struct Result;

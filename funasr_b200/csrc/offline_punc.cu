@@ -1,5 +1,15 @@
 // Handle-style CT-Transformer punctuation: fa_punc_init (model file -> handle), fa_punc_infer (many texts -> punctuated texts, every
 // text one window per lockstep step), fa_punc_walk_host (the same walk over any scorer).  The text walk is punc_text.cpp.
+//
+// Concurrent fa_punc_infer calls on one handle share steps.  A window's punctuation depends on that window only (punc_text.cpp), and
+// a step is one window per text, so the texts of many calls can advance in one lockstep walk, and a call can join it at any step
+// boundary.  A call checks its arguments and splits its texts into words on its own thread, then posts a ticket holding their walk
+// state.  The thread that finds no leader leads: under the device lock, each step admits the queued tickets in arrival order (while the
+// step's carve stays within kStepBytes; the first on an idle pool always), composes one padded step from every active text of every
+// admitted call, scores it, applies the results, and wakes the calls that ended.  It returns once its own call has ended, and a
+// waiter leads on.  The walk state lives in the tickets, not on a leader's stack.  A window over max_window fails only its own call,
+// before that step's scorer runs, with the message it gets alone; a scorer or device failure fails every call that had a window in
+// that step.  No thread is created.
 #include "handle.h"
 #include "punc_text.h"
 
@@ -9,6 +19,19 @@ namespace {
 
 // __punc_config__ of funasr_b200/pack.py:write_punc_model_file
 enum { kPuncLayers = 0, kPuncDModel, kPuncHeads, kPuncKernel, kPuncSentenceEnd, kPuncSplit, kPuncCfgLen };
+
+// a further call joins a step only while the step's device buffers (punc_step's carve) stay within this
+const size_t kStepBytes = size_t(1) << 30;
+
+// One fa_punc_infer call in the pool: its texts' walk state, stepped by whichever thread leads
+struct PuncTicket {
+  std::vector<fa_punc::Text> texts;
+  int64_t steps = 0;                                 // the steps it had a window in
+  // written by the leader, read by the owner once done
+  std::unique_ptr<fa_punc::Result> res;
+  std::string err;
+  bool done = false;
+};
 
 struct Punc {
   std::mutex mu;                                     // device lock
@@ -20,8 +43,19 @@ struct Punc {
   FaEncoder enc{};
   FaLinear out{};
   const float* embed = nullptr;
+  fa_punc_score_fn host_score = nullptr;             // fa_punc_init_host: steps call host_score(host_ctx, ...) in place of the network
+  void* host_ctx = nullptr;
   DevBuf punc_step;                                  // grown to the largest step's t_max
   std::vector<int32_t> host_io;                      // ids [batch, t_max] then lens [batch]: one host-to-device copy per step
+  // the pool: posted tickets in arrival order, admitted tickets with windows left (in admission order), whether a thread leads, the
+  // leader's step, counters since init
+  std::mutex pool_mu;
+  std::condition_variable pool_cv;
+  std::deque<PuncTicket*> queue;
+  std::vector<PuncTicket*> active;
+  bool busy = false;
+  fa_punc::Step step;
+  std::atomic<int64_t> pool_calls{0}, pool_steps{0};
 };
 
 // a newline-joined UTF-8 list stored as the bytes of an fp32 tensor
@@ -72,32 +106,205 @@ bool build_punc(Punc& p, Builder& b) {
   return b.ok;
 }
 
+// punc_step's device buffers for B windows of T words, taken from a
+struct StepBufs {
+  int32_t *ids_d, *pids;
+  float *x, *h, *best;
+  void* ws;
+  size_t ws_bytes;
+};
+void take_step(const Punc& p, fa::Arena& a, int32_t B, int32_t T, StepBufs& s) {
+  const int64_t M = (int64_t)B * T;
+  s.ws_bytes = std::max(fa_sanm_encoder_workspace_bytes(B, T, FA_GEMM_F32_SIMT), fa_linear_argmax_workspace_bytes(M, p.out.out_f, FA_GEMM_F32_SIMT));
+  s.ids_d = a.take<int32_t>(M + B); s.x = a.take<float>((size_t)M * p.d_in); s.h = a.take<float>((size_t)M * p.d_model);
+  s.pids = a.take<int32_t>(M); s.best = a.take<float>(M); s.ws = a.take<char>(s.ws_bytes);
+}
+
+// the bytes punc_step carves for B windows of T words (0 on a host handle)
+size_t step_bytes(const Punc& p, int64_t B, int64_t T) {
+  if (p.host_score) return 0;
+  if (B * T > INT32_MAX) return SIZE_MAX;
+  fa::Arena m = fa::Arena::measuring();
+  StepBufs s;
+  take_step(p, m, (int32_t)B, (int32_t)T, s);
+  return m.bytes();
+}
+
 // one lockstep step on the GPU: punc_forward (model.py:112-125) + arg-max over a padded batch of windows
 bool punc_step(Punc& p, const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, int32_t* punc_out, std::string& err) {
   cudaStream_t st = p.file.st;
   const int64_t M = (int64_t)B * T;
-  const int n_punc = p.out.out_f;
-  const size_t ws_bytes = std::max(fa_sanm_encoder_workspace_bytes(B, T, FA_GEMM_F32_SIMT), fa_linear_argmax_workspace_bytes(M, n_punc, FA_GEMM_F32_SIMT));
-  int32_t *ids_d, *pids;
-  float *x, *h, *best;
-  void* ws;
-  if (!carve(p.punc_step, "punctuation", [&](fa::Arena& a) {
-        ids_d = a.take<int32_t>(M + B); x = a.take<float>((size_t)M * p.d_in); h = a.take<float>((size_t)M * p.d_model);
-        pids = a.take<int32_t>(M); best = a.take<float>(M); ws = a.take<char>(ws_bytes);
-      })) {
+  StepBufs s;
+  if (!carve(p.punc_step, "punctuation", [&](fa::Arena& a) { take_step(p, a, B, T, s); })) {
     err = g_err;
     return false;
   }
   p.host_io.assign(ids, ids + M);
   p.host_io.insert(p.host_io.end(), lens, lens + B);
-  cudaMemcpyAsync(ids_d, p.host_io.data(), (size_t)(M + B) * 4, cudaMemcpyHostToDevice, st);
-  int rc = fa_embedding(ids_d, p.embed, p.d_in, p.n_embed, M, x, st);
-  if (rc == FA_OK) rc = fa_sanm_encoder_forward(&p.enc, x, ids_d + M, B, T, h, FA_GEMM_F32_SIMT, ws, ws_bytes, st);
-  if (rc == FA_OK) rc = fa_linear_argmax(&p.out, h, nullptr, M, pids, best, nullptr, FA_GEMM_F32_SIMT, ws, ws_bytes, st);
+  cudaMemcpyAsync(s.ids_d, p.host_io.data(), (size_t)(M + B) * 4, cudaMemcpyHostToDevice, st);
+  int rc = fa_embedding(s.ids_d, p.embed, p.d_in, p.n_embed, M, s.x, st);
+  if (rc == FA_OK) rc = fa_sanm_encoder_forward(&p.enc, s.x, s.ids_d + M, B, T, s.h, FA_GEMM_F32_SIMT, s.ws, s.ws_bytes, st);
+  if (rc == FA_OK) rc = fa_linear_argmax(&p.out, s.h, nullptr, M, s.pids, s.best, nullptr, FA_GEMM_F32_SIMT, s.ws, s.ws_bytes, st);
   if (rc != FA_OK) { err = std::string("punctuation forward: ") + fa_status_string(rc); return false; }
-  cudaMemcpyAsync(punc_out, pids, (size_t)M * 4, cudaMemcpyDeviceToHost, st);
+  cudaMemcpyAsync(punc_out, s.pids, (size_t)M * 4, cudaMemcpyDeviceToHost, st);
   if (!sync_stream(st)) { err = g_err; return false; }
   return true;
+}
+
+bool score_step(Punc& p, fa_punc::Step& s, std::string& err) {
+  if (!p.host_score) return punc_step(p, s.ids.data(), s.lens.data(), s.batch, s.t_max, s.pout.data(), err);
+  const int32_t rc = p.host_score(p.host_ctx, s.ids.data(), s.lens.data(), s.batch, s.t_max, s.pout.data());
+  if (rc != 0) err = "scorer failed (" + std::to_string(rc) + ")";
+  return rc == 0;
+}
+
+// t's result: every text's punctuated text and ids, and the steps it had a window in
+void finish(PuncTicket& t) {
+  t.res.reset(new fa_punc::Result());
+  const size_t n = t.texts.size();
+  t.res->text.resize(n);
+  t.res->ids.resize(n);
+  for (size_t i = 0; i < n; ++i) {
+    t.res->text[i].swap(t.texts[i].text);
+    t.res->ids[i].swap(t.texts[i].punc);
+  }
+  t.res->steps = t.steps;
+  t.texts.clear();
+}
+
+// Under pool_mu: queued tickets join the walk in arrival order while the next step's carve stays within kStepBytes; the first ticket
+// of an idle walk always joins, and a ticket that does not fit holds back those behind it
+void admit_queued(Punc& p) {
+  int64_t B = 0, T = 0;
+  auto extent = [&](const PuncTicket& t, int64_t& b, int64_t& tm) {
+    for (const fa_punc::Text& x : t.texts)
+      if (x.active()) { ++b; tm = std::max(tm, fa_punc::window_len(p.vocab, x)); }
+  };
+  for (const PuncTicket* t : p.active) extent(*t, B, T);
+  while (!p.queue.empty()) {
+    PuncTicket* t = p.queue.front();
+    int64_t b = B, tm = T;
+    extent(*t, b, tm);
+    if (!p.active.empty() && step_bytes(p, b, tm) > kStepBytes) break;
+    p.active.push_back(t);
+    p.queue.pop_front();
+    ++p.pool_calls;
+    B = b; T = tm;
+  }
+}
+
+// One step over every admitted call's active texts (the leader, outside pool_mu); the calls that ended leave p.active for `ended`,
+// with a result or a message
+void run_step(Punc& p, std::vector<PuncTicket*>& ended) {
+  std::vector<fa_punc::Text*> rows;
+  std::vector<PuncTicket*> owner;                    // per row
+  try {
+    for (PuncTicket* t : p.active) {                 // a window over max_window fails its call before the scorer runs, as alone
+      const size_t r0 = rows.size();
+      for (size_t i = 0; i < t->texts.size() && t->err.empty(); ++i) {
+        fa_punc::Text& x = t->texts[i];
+        if (!x.active()) continue;
+        if (!fa_punc::check_window(p.vocab, x, (int32_t)i, p.max_window, t->err)) break;
+        rows.push_back(&x);
+      }
+      if (!t->err.empty()) rows.resize(r0);
+      owner.resize(rows.size(), t);
+    }
+    if (!rows.empty()) {
+      fa_punc::compose(p.vocab, rows, p.step);
+      std::string err;
+      bool ok;
+      {
+        std::lock_guard<std::mutex> dev(p.mu);
+        ok = score_step(p, p.step, err);
+      }
+      if (ok) ++p.pool_steps;
+      for (size_t b = 0; b < rows.size(); ++b) {
+        PuncTicket* t = owner[b];
+        if (!ok) { t->err = err; continue; }       // a failed step fails every call that had a window in it
+        if (b == 0 || owner[b - 1] != t) ++t->steps;
+        if (t->err.empty()) fa_punc::apply(p.vocab, *rows[b], p.step, (int32_t)b, t->err);
+      }
+    }
+  } catch (const std::exception& e) {                // every admitted call ends with the message
+    for (PuncTicket* t : p.active)
+      if (t->err.empty()) t->err = std::string("fa_punc_infer: ") + e.what();
+  }
+  size_t keep = 0;
+  for (PuncTicket* t : p.active) {
+    bool left = false;
+    for (const fa_punc::Text& x : t->texts) left = left || x.active();
+    if (t->err.empty() && left) { p.active[keep++] = t; continue; }
+    if (t->err.empty()) finish(*t);
+    t->texts.clear();
+    ended.push_back(t);
+  }
+  p.active.resize(keep);
+}
+
+// t's call through the pool -> its result, or nullptr with its own message set as this thread's error
+void* pool_call(Punc& p, PuncTicket& t) {
+  // Whatever a step throws, leadership is given up and the waiters are woken, so one of them leads on; no exception crosses the C ABI.
+  struct Lead {
+    Punc& p;
+    std::unique_lock<std::mutex>& q;
+    ~Lead() {
+      if (!q.owns_lock()) q.lock();
+      p.busy = false;
+      p.pool_cv.notify_all();
+    }
+  };
+  std::string msg;
+  try {
+    std::unique_lock<std::mutex> q(p.pool_mu);
+    p.queue.push_back(&t);
+    while (!t.done) {
+      if (p.busy) {                                          // a leader is stepping: it admits this ticket at a step boundary
+        p.pool_cv.wait(q);
+        continue;
+      }
+      p.busy = true;
+      Lead lead{p, q};
+      if (!p.host_score) cudaSetDevice(p.file.device);
+      std::vector<PuncTicket*> ended;
+      while (!t.done) {
+        admit_queued(p);
+        q.unlock();
+        ended.clear();
+        run_step(p, ended);
+        q.lock();
+        for (PuncTicket* e : ended) e->done = true;
+        if (!ended.empty()) p.pool_cv.notify_all();
+      }
+    }
+  } catch (const std::exception& e) {
+    msg = std::string("fa_punc_infer: ") + e.what();
+    try {                                                   // never leave this ticket where a leader could still step it
+      std::unique_lock<std::mutex> q(p.pool_mu);
+      auto drop = [&](auto& c) {
+        auto it = std::find(c.begin(), c.end(), &t);
+        if (it == c.end()) return false;
+        c.erase(it);
+        return true;
+      };
+      if (!drop(p.queue)) p.pool_cv.wait(q, [&] { return t.done || (!p.busy && drop(p.active)); });
+    } catch (const std::exception&) {
+    }
+    t.res.reset();
+  }
+  if (!t.res) return fail(msg.empty() ? t.err : msg);
+  g_err.clear();
+  return t.res.release();
+}
+
+// fa_punc_init_host / fa_punc_walk_host: the caller's vocabulary, checked
+bool host_vocab(const char* const* tokens, int32_t n_tokens, const char* const* punc_list, int32_t n_punc, int32_t sentence_end_id,
+                int32_t split_size, fa_punc::Vocab& v) {
+  std::string err;
+  for (int32_t i = 0; i < n_tokens; ++i) if (!tokens[i]) { set_err("token " + std::to_string(i) + " is NULL"); return false; }
+  for (int32_t i = 0; i < n_punc; ++i) if (!punc_list[i]) { set_err("punctuation " + std::to_string(i) + " is NULL"); return false; }
+  std::vector<std::string> tok(tokens, tokens + n_tokens), pl(punc_list, punc_list + n_punc);
+  return v.init(tok, pl, sentence_end_id, split_size, err) || (set_err(err), false);
 }
 
 }  // namespace
@@ -115,16 +322,42 @@ extern "C" void* fa_punc_infer(void* punc, const char* const* texts, int32_t n) 
   if (!p || (!texts && n > 0) || n < 0) return fail("bad argument");
   for (int32_t i = 0; i < n; ++i)
     if (!texts[i]) return fail("text " + std::to_string(i) + " is NULL");
-  std::lock_guard<std::mutex> dev(p->mu);
-  cudaSetDevice(p->file.device);
-  std::unique_ptr<fa_punc::Result> r(new fa_punc::Result());
-  std::string err;
-  const fa_punc::Scorer score = [p](const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, int32_t* out, std::string& e) {
-    return punc_step(*p, ids, lens, B, T, out, e);
-  };
-  if (!no_throw("fa_punc_infer: ", [&] { return fa_punc::walk(p->vocab, texts, n, p->max_window, score, *r, err) || (set_err(err), false); }))
+  PuncTicket t;
+  bool any = false;
+  if (!no_throw("fa_punc_infer: ", [&] {
+        t.texts.reserve((size_t)n);
+        for (int32_t i = 0; i < n; ++i) {
+          t.texts.push_back(fa_punc::admit(p->vocab, texts[i]));
+          any = any || t.texts.back().active();
+        }
+        if (!any) finish(t);                                  // no window: "" and no ids, without the pool
+        return true;
+      }))
     return nullptr;
-  return r.release();
+  return any ? pool_call(*p, t) : t.res.release();
+}
+
+extern "C" void* fa_punc_init_host(const char* const* tokens, int32_t n_tokens, const char* const* punc_list, int32_t n_punc,
+                                   int32_t sentence_end_id, int32_t split_size, int64_t max_window, fa_punc_score_fn score_fn, void* ctx) {
+  g_err.clear();
+  if (!tokens || n_tokens < 1 || !punc_list || n_punc < 1 || !score_fn) return fail("bad argument");
+  std::unique_ptr<Punc> p;
+  const bool ok = no_throw("fa_punc_init_host: ", [&] {
+    p.reset(new Punc());
+    p->host_score = score_fn;
+    p->host_ctx = ctx;
+    p->max_window = max_window;
+    return host_vocab(tokens, n_tokens, punc_list, n_punc, sentence_end_id, split_size, p->vocab);
+  });
+  return ok ? p.release() : nullptr;
+}
+
+extern "C" int fa_punc_pool_stats(const void* punc, int64_t* calls, int64_t* steps) {
+  const Punc* p = static_cast<const Punc*>(punc);
+  if (!p || !calls || !steps) return FA_ERR_ARG;
+  *calls = p->pool_calls.load();
+  *steps = p->pool_steps.load();
+  return FA_OK;
 }
 
 extern "C" void* fa_punc_walk_host(const char* const* texts, int32_t n, const char* const* tokens, int32_t n_tokens, const char* const* punc_list,
@@ -135,18 +368,16 @@ extern "C" void* fa_punc_walk_host(const char* const* texts, int32_t n, const ch
   for (int32_t i = 0; i < n; ++i)
     if (!texts[i]) return fail("text " + std::to_string(i) + " is NULL");
   std::unique_ptr<fa_punc::Result> r(new fa_punc::Result());
-  std::string err;
   const bool ok = no_throw("fa_punc_walk_host: ", [&] {
-    for (int32_t i = 0; i < n_tokens; ++i) if (!tokens[i]) { err = "token " + std::to_string(i) + " is NULL"; set_err(err); return false; }
-    for (int32_t i = 0; i < n_punc; ++i) if (!punc_list[i]) { err = "punctuation " + std::to_string(i) + " is NULL"; set_err(err); return false; }
-    std::vector<std::string> tok(tokens, tokens + n_tokens), pl(punc_list, punc_list + n_punc);
     fa_punc::Vocab v;
+    std::string err;
     const fa_punc::Scorer score = [&](const int32_t* ids, const int32_t* lens, int32_t B, int32_t T, int32_t* out, std::string& e) {
       const int32_t rc = score_fn(ctx, ids, lens, B, T, out);
       if (rc != 0) e = "scorer failed (" + std::to_string(rc) + ")";
       return rc == 0;
     };
-    return (v.init(tok, pl, sentence_end_id, split_size, err) && fa_punc::walk(v, texts, n, max_window, score, *r, err)) || (set_err(err), false);
+    return host_vocab(tokens, n_tokens, punc_list, n_punc, sentence_end_id, split_size, v) &&
+           (fa_punc::walk(v, texts, n, max_window, score, *r, err) || (set_err(err), false));
   });
   return ok ? r.release() : nullptr;
 }

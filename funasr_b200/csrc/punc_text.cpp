@@ -40,16 +40,6 @@ std::string last_char(const std::string& s, size_t* at) {
   return s.substr(i);
 }
 
-struct Text {
-  std::vector<std::string> words;
-  std::vector<int32_t> ids;
-  int64_t n_windows = 0, next = 0;                 // split_to_mini_sentence's window count; the window the next step scores
-  std::vector<std::string> cache_words;            // the unfinished tail carried into the next window
-  std::vector<int32_t> cache_ids;
-  std::string text;
-  std::vector<int32_t> punc;
-};
-
 }  // namespace
 
 bool Vocab::init(const std::vector<std::string>& tokens, const std::vector<std::string>& punc_list, int32_t sentence_end, int32_t split,
@@ -89,115 +79,136 @@ std::vector<std::string> split_words(const std::string& s) {
   return words;
 }
 
-bool walk(const Vocab& v, const char* const* texts, int32_t n, int64_t max_window, const Scorer& score, Result& out, std::string& err) {
-  const int64_t split = v.split_size;
-  const std::vector<std::string>& pl = v.punc;
-  std::vector<Text> st((size_t)n);
-  for (int32_t t = 0; t < n; ++t) {
-    Text& x = st[t];
-    x.words = split_words(texts[t] ? texts[t] : "");
-    x.ids.reserve(x.words.size());
-    for (const std::string& w : x.words) {                  // tokens2ids: exact lookup, unknown -> <unk>
-      auto it = v.token_id.find(w);
-      x.ids.push_back(it != v.token_id.end() ? it->second : v.unk);
-    }
-    const int64_t nw = (int64_t)x.words.size();
-    x.n_windows = (nw + split - 1) / split;                // an empty or whitespace-only text: no window, "" and no ids
+Text admit(const Vocab& v, const char* text) {
+  Text x;
+  x.words = split_words(text ? text : "");
+  x.ids.reserve(x.words.size());
+  for (const std::string& w : x.words) {                    // tokens2ids: exact lookup, unknown -> <unk>
+    auto it = v.token_id.find(w);
+    x.ids.push_back(it != v.token_id.end() ? it->second : v.unk);
   }
-  auto is = [&](int32_t p, const char* s) { return pl[p] == s; };
-  std::vector<int32_t> active, ids, lens, pout;
+  const int64_t nw = (int64_t)x.words.size();
+  x.n_windows = (nw + v.split_size - 1) / v.split_size;    // an empty or whitespace-only text: no window, "" and no ids
+  return x;
+}
+
+int64_t window_len(const Vocab& v, const Text& x) {
+  return (int64_t)x.cache_ids.size() + std::min<int64_t>(v.split_size, (int64_t)x.words.size() - x.next * v.split_size);
+}
+
+bool check_window(const Vocab& v, const Text& x, int32_t index, int64_t max_window, std::string& err) {
+  const int64_t len = window_len(v, x);
+  if (max_window <= 0 || len <= max_window) return true;
+  err = "text " + std::to_string(index) + ": window " + std::to_string(x.next) + " holds " + std::to_string(len) +
+        " words (an unfinished sentence carried over), more than the attention kernel takes (" + std::to_string(max_window) + ")";
+  return false;
+}
+
+void compose(const Vocab& v, const std::vector<Text*>& rows, Step& s) {
+  const int64_t split = v.split_size;
+  int64_t t_max = 0;
+  for (const Text* x : rows) t_max = std::max(t_max, window_len(v, *x));
+  const int32_t B = (int32_t)rows.size();
+  s.batch = B;
+  s.t_max = (int32_t)t_max;
+  s.ids.assign((size_t)B * t_max, 0);
+  s.lens.assign((size_t)B, 0);
+  s.pout.assign((size_t)B * t_max, 0);
+  for (int32_t b = 0; b < B; ++b) {
+    const Text& x = *rows[b];
+    int32_t* row = s.ids.data() + (size_t)b * t_max;
+    std::copy(x.cache_ids.begin(), x.cache_ids.end(), row);
+    const int64_t w0 = x.next * split, w1 = std::min<int64_t>(w0 + split, (int64_t)x.ids.size());
+    std::copy(x.ids.begin() + w0, x.ids.begin() + w1, row + x.cache_ids.size());
+    s.lens[b] = (int32_t)(x.cache_ids.size() + (w1 - w0));
+  }
+}
+
+bool apply(const Vocab& v, Text& x, const Step& s, int32_t b, std::string& err) {
+  const std::vector<std::string>& pl = v.punc;
+  auto is = [&](int32_t p, const char* str) { return pl[p] == str; };
+  const int64_t split = v.split_size;
+  const int64_t L = s.lens[b], w0 = x.next * split, w1 = std::min<int64_t>(w0 + split, (int64_t)x.ids.size());
+  std::vector<int32_t> p(s.pout.begin() + (size_t)b * s.t_max, s.pout.begin() + (size_t)b * s.t_max + L);
+  for (int32_t q : p)
+    if (q < 0 || q >= (int32_t)pl.size()) { err = "scorer returned punctuation id " + std::to_string(q) + " outside the list"; return false; }
+  std::vector<std::string> ms(x.cache_words);
+  ms.insert(ms.end(), x.words.begin() + w0, x.words.begin() + w1);
+  std::vector<int32_t> mi(x.cache_ids);
+  mi.insert(mi.end(), x.ids.begin() + w0, x.ids.begin() + w1);
+  const bool last = x.next == x.n_windows - 1;
+  if (!last) {                                             // carry the unfinished tail over (model.py:350-374)
+    int64_t end = -1, comma = -1;
+    for (int64_t i = L - 2; i > 1; --i) {
+      if (is(p[i], "。") || is(p[i], "？")) { end = i; break; }
+      if (comma < 0 && is(p[i], "，")) comma = i;
+    }
+    if (end < 0 && L > 200 && comma >= 0) {               // cache_pop_trigger_limit: cut a long sentence at its last comma
+      end = comma;
+      p[end] = v.sentence_end_id;
+    }
+    x.cache_words.assign(ms.begin() + (end + 1), ms.end());
+    x.cache_ids.assign(mi.begin() + (end + 1), mi.end());
+    ms.resize((size_t)(end + 1));
+    p.resize((size_t)(end + 1));
+  } else {
+    x.cache_words.clear();
+    x.cache_ids.clear();
+  }
+  std::string piece;                                       // model.py:382-409
+  for (size_t i = 0; i < ms.size(); ++i) {
+    std::string& w = ms[i];
+    const bool lat = latin(w);
+    if ((i == 0 || is(p[i - 1], "。") || is(p[i - 1], "？")) && lat) {   // str.capitalize() of an ASCII word
+      w[0] = (char)toupper((unsigned char)w[0]);
+      for (size_t k = 1; k < w.size(); ++k) w[k] = (char)tolower((unsigned char)w[k]);
+    }
+    if (i == 0 && lat) w = " " + w;
+    if (i > 0 && lat && latin(ms[i - 1])) w = " " + w;
+    piece += w;
+    if (pl[p[i]] != "_") {
+      std::string r = pl[p[i]];
+      if (lat) r = r == "，" ? "," : r == "。" ? "." : r == "？" ? "?" : r;
+      piece += r;
+    }
+  }
+  x.text += piece;
+  if (last) {                                              // forced sentence end (model.py:413-449)
+    size_t at = 0;
+    const std::string c = last_char(x.text, &at);
+    bool force = true;
+    if (c == "，" || c == "、") x.text = x.text.substr(0, at) + "。";
+    else if (c == ",") x.text = x.text.substr(0, at) + ".";
+    else if (c != "。" && c != "？" && c.size() != 1) x.text += "。";
+    else if (c != "." && c != "?" && c.size() == 1) x.text += ".";
+    else force = false;
+    if (force && !p.empty()) p.back() = v.sentence_end_id;
+  }
+  x.punc.insert(x.punc.end(), p.begin(), p.end());
+  ++x.next;
+  return true;
+}
+
+bool walk(const Vocab& v, const char* const* texts, int32_t n, int64_t max_window, const Scorer& score, Result& out, std::string& err) {
+  std::vector<Text> st;
+  st.reserve((size_t)n);
+  for (int32_t t = 0; t < n; ++t) st.push_back(admit(v, texts[t]));
+  std::vector<Text*> rows;
+  Step s;
   out.steps = 0;
   for (;;) {
-    active.clear();
-    int64_t t_max = 0;
+    rows.clear();
     for (int32_t t = 0; t < n; ++t) {
-      Text& x = st[t];
-      if (x.next >= x.n_windows) continue;
-      const int64_t len = (int64_t)x.cache_ids.size() + std::min<int64_t>(split, (int64_t)x.words.size() - x.next * split);
-      if (max_window > 0 && len > max_window) {
-        err = "text " + std::to_string(t) + ": window " + std::to_string(x.next) + " holds " + std::to_string(len) +
-              " words (an unfinished sentence carried over), more than the attention kernel takes (" + std::to_string(max_window) + ")";
-        return false;
-      }
-      active.push_back(t);
-      t_max = std::max(t_max, len);
+      if (!st[t].active()) continue;
+      if (!check_window(v, st[t], t, max_window, err)) return false;
+      rows.push_back(&st[t]);
     }
-    if (active.empty()) break;
-    const int32_t B = (int32_t)active.size();
-    ids.assign((size_t)B * t_max, 0);
-    lens.assign((size_t)B, 0);
-    pout.assign((size_t)B * t_max, 0);
-    for (int32_t b = 0; b < B; ++b) {
-      const Text& x = st[active[b]];
-      int32_t* row = ids.data() + (size_t)b * t_max;
-      std::copy(x.cache_ids.begin(), x.cache_ids.end(), row);
-      const int64_t w0 = x.next * split, w1 = std::min<int64_t>(w0 + split, (int64_t)x.ids.size());
-      std::copy(x.ids.begin() + w0, x.ids.begin() + w1, row + x.cache_ids.size());
-      lens[b] = (int32_t)(x.cache_ids.size() + (w1 - w0));
-    }
-    if (!score(ids.data(), lens.data(), B, (int32_t)t_max, pout.data(), err)) return false;
+    if (rows.empty()) break;
+    compose(v, rows, s);
+    if (!score(s.ids.data(), s.lens.data(), s.batch, s.t_max, s.pout.data(), err)) return false;
     ++out.steps;
-    for (int32_t b = 0; b < B; ++b) {
-      Text& x = st[active[b]];
-      const int64_t L = lens[b], w0 = x.next * split, w1 = std::min<int64_t>(w0 + split, (int64_t)x.ids.size());
-      std::vector<int32_t> p(pout.begin() + (size_t)b * t_max, pout.begin() + (size_t)b * t_max + L);
-      for (int32_t q : p)
-        if (q < 0 || q >= (int32_t)pl.size()) { err = "scorer returned punctuation id " + std::to_string(q) + " outside the list"; return false; }
-      std::vector<std::string> ms(x.cache_words);
-      ms.insert(ms.end(), x.words.begin() + w0, x.words.begin() + w1);
-      std::vector<int32_t> mi(x.cache_ids);
-      mi.insert(mi.end(), x.ids.begin() + w0, x.ids.begin() + w1);
-      const bool last = x.next == x.n_windows - 1;
-      if (!last) {                                           // carry the unfinished tail over (model.py:350-374)
-        int64_t end = -1, comma = -1;
-        for (int64_t i = L - 2; i > 1; --i) {
-          if (is(p[i], "。") || is(p[i], "？")) { end = i; break; }
-          if (comma < 0 && is(p[i], "，")) comma = i;
-        }
-        if (end < 0 && L > 200 && comma >= 0) {             // cache_pop_trigger_limit: cut a long sentence at its last comma
-          end = comma;
-          p[end] = v.sentence_end_id;
-        }
-        x.cache_words.assign(ms.begin() + (end + 1), ms.end());
-        x.cache_ids.assign(mi.begin() + (end + 1), mi.end());
-        ms.resize((size_t)(end + 1));
-        p.resize((size_t)(end + 1));
-      } else {
-        x.cache_words.clear();
-        x.cache_ids.clear();
-      }
-      std::string piece;                                     // model.py:382-409
-      for (size_t i = 0; i < ms.size(); ++i) {
-        std::string& w = ms[i];
-        const bool lat = latin(w);
-        if ((i == 0 || is(p[i - 1], "。") || is(p[i - 1], "？")) && lat) {   // str.capitalize() of an ASCII word
-          w[0] = (char)toupper((unsigned char)w[0]);
-          for (size_t k = 1; k < w.size(); ++k) w[k] = (char)tolower((unsigned char)w[k]);
-        }
-        if (i == 0 && lat) w = " " + w;
-        if (i > 0 && lat && latin(ms[i - 1])) w = " " + w;
-        piece += w;
-        if (pl[p[i]] != "_") {
-          std::string r = pl[p[i]];
-          if (lat) r = r == "，" ? "," : r == "。" ? "." : r == "？" ? "?" : r;
-          piece += r;
-        }
-      }
-      x.text += piece;
-      if (last) {                                            // forced sentence end (model.py:413-449)
-        size_t at = 0;
-        const std::string c = last_char(x.text, &at);
-        bool force = true;
-        if (c == "，" || c == "、") x.text = x.text.substr(0, at) + "。";
-        else if (c == ",") x.text = x.text.substr(0, at) + ".";
-        else if (c != "。" && c != "？" && c.size() != 1) x.text += "。";
-        else if (c != "." && c != "?" && c.size() == 1) x.text += ".";
-        else force = false;
-        if (force && !p.empty()) p.back() = v.sentence_end_id;
-      }
-      x.punc.insert(x.punc.end(), p.begin(), p.end());
-      ++x.next;
-    }
+    for (int32_t b = 0; b < s.batch; ++b)
+      if (!apply(v, *rows[b], s, b, err)) return false;
   }
   out.text.resize((size_t)n);
   out.ids.resize((size_t)n);

@@ -135,6 +135,13 @@ class OfflinePunc:
         finally:
             self.lib.fa_punc_free_result(res)
 
+    def pool_stats(self):
+        """(calls, steps): the calls the handle's pool has admitted since init and the lockstep steps it ran them in; concurrent
+        `infer` calls from many threads share steps."""
+        c, s = C.c_int64(), C.c_int64()
+        _abi.check(self.lib.fa_punc_pool_stats(self.handle, C.byref(c), C.byref(s)), "fa_punc_pool_stats")
+        return c.value, s.value
+
     def close(self):
         if getattr(self, "handle", None):
             self.lib.fa_punc_uninit(self.handle)

@@ -831,10 +831,13 @@ const char* fa_offline_last_error(void);
  * one speaker stage over all of its diarized recordings (each still clustered on its own); a refusal of that stage fails only its own
  * call.  Long-audio calls share passes only with the same VAD handle and FaLongAudioOptions, diarized calls only with the same
  * speaker handle (preset_spk_num may differ).
- * A device failure during a pass fails every call of that pass with its message.  Other handles' calls hold the handle's lock
- * for their device work and run one after another.  A call that uses several handles (fa_offline_infer_vad*) locks them in the order
- * recogniser, VAD, speaker, so recognisers that share a VAD handle cannot deadlock.  fa_offline_last_error is per thread.  Uninit a
- * handle only after every call on it has returned. */
+ * A device failure during a pass fails every call of that pass with its message.  Punctuation calls (fa_punc_infer) on one handle
+ * share lockstep steps: the thread that finds no step running leads, each step admitting the queued calls in arrival order and scoring
+ * one window of every active text of every admitted call, and each text gets exactly what it gets alone (fa_punc_infer below).  The
+ * aligner's, the VAD-only (fa_vad_infer*) and the speaker-only (fa_spk_*) calls hold the handle's lock for their device work and run
+ * one after another.  A call that uses several handles (fa_offline_infer_vad*) locks them in the order recogniser, VAD, speaker, so
+ * recognisers that share a VAD handle cannot deadlock; the punctuation and aligner locks are never held with another.
+ * fa_offline_last_error is per thread.  Uninit a handle only after every call on it has returned. */
 /* Calls the recogniser handle's pool has decoded since init, and the GPU packs it decoded them in (packs < calls: calls were pooled).
  * 0, or FA_ERR_ARG for a NULL argument. */
 int fa_offline_pool_stats(const void* handle, int64_t* calls, int64_t* packs);
@@ -1047,16 +1050,24 @@ int fa_spk_distribute_host(const int32_t* sentences, int64_t ns, const double* t
  * alone.  An empty or whitespace-only text gives "" and no ids.  A window with more words than the fp32 attention kernel takes keys
  * (4 * t floats of shared memory within 160 KB, for heads narrower than 128) fails the call before that step's first launch, naming
  * the text: the carried tail grows without bound when the model predicts no comma and no sentence end.  NULL on error
- * (fa_offline_last_error()). */
+ * (fa_offline_last_error()).
+ * Concurrent calls on one handle pool: a call's texts join the lockstep walk of the calls already running at the next step boundary
+ * (in arrival order, while the step's device buffers stay within 1 GiB; a call alone always runs), and every step scores one window
+ * of every active text of every call as one batch.  A window's punctuation depends on that window only, so each call gets exactly
+ * what it gets alone: its texts, ids and steps.  An over-long window fails only its own call, with the message it gets alone; a
+ * failure of a step's forward fails every call that had a window in that step. */
 void* fa_punc_init(const char* model_file, int32_t device);
 void* fa_punc_infer(void* punc, const char* const* texts, int32_t n);
 /* text i (NUL-terminated UTF-8; NULL for an out-of-range index) / its n punctuation ids (NULL with 0 for an empty text) */
 const char* fa_punc_result_text(const void* result, int32_t index);
 const int32_t* fa_punc_result_ids(const void* result, int32_t index, int32_t* n);
-/* the lockstep steps the call ran (the longest text's window count) */
+/* the lockstep steps the call had a window in (its longest text's window count, pooled or alone) */
 int64_t fa_punc_result_steps(const void* result);
 void fa_punc_free_result(void* result);
 void fa_punc_uninit(void* punc);
+/* Calls the punctuation handle's pool has admitted since init, and the lockstep steps it ran them in (steps below the calls' own step
+ * counts summed: calls shared steps).  A call whose texts are all empty never enters the pool.  0, or FA_ERR_ARG for a NULL argument. */
+int fa_punc_pool_stats(const void* punc, int64_t* calls, int64_t* steps);
 /* Host only: the same walk with a caller's scorer in place of the network.  score_fn(ctx, ids [batch, t_max], lens [batch], batch,
  * t_max, punc_out [batch, t_max]) scores one lockstep step (row b valid for its first lens[b] entries, padding ids 0) and returns 0,
  * or nonzero to fail the call.  tokens [n_tokens] / punc_list [n_punc]: the vocabulary and the punctuation classes; split_size words per
@@ -1065,6 +1076,12 @@ void fa_punc_uninit(void* punc);
 typedef int32_t (*fa_punc_score_fn)(void* ctx, const int32_t* ids, const int32_t* lens, int32_t batch, int32_t t_max, int32_t* punc_out);
 void* fa_punc_walk_host(const char* const* texts, int32_t n, const char* const* tokens, int32_t n_tokens, const char* const* punc_list,
                         int32_t n_punc, int32_t sentence_end_id, int32_t split_size, int64_t max_window, fa_punc_score_fn score_fn, void* ctx);
+/* Host only: a punctuation handle whose steps call score_fn(ctx, ...) in place of the network, with the vocabulary, split_size and
+ * max_window of fa_punc_walk_host and its refusals.  fa_punc_infer, fa_punc_pool_stats and fa_punc_uninit take it, and concurrent
+ * calls pool exactly as on a fa_punc_init handle: a step's scorer call holds every admitted call's windows.  score_fn is called from
+ * whichever calling thread leads the step, one call at a time.  NULL on error (fa_offline_last_error()). */
+void* fa_punc_init_host(const char* const* tokens, int32_t n_tokens, const char* const* punc_list, int32_t n_punc, int32_t sentence_end_id,
+                        int32_t split_size, int64_t max_window, fa_punc_score_fn score_fn, void* ctx);
 
 #ifdef __cplusplus
 }

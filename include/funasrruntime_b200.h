@@ -4,7 +4,8 @@
  * header in place of the original for the offline ASR calls it makes.  One handle may be shared by any number of threads, as the
  * reference's servers share it among their decoder threads: FunOfflineInfer / FunOfflineInferBuffer, CompileHotwordEmbedding,
  * FsmnVad* and CTTransformer* are safe on shared handles (funasr_b200.h, "Threads"); FunOfflineInfer* calls from many threads on
- * one handle are decoded together in shared GPU packs, with or without hotword rows, each giving what it gives alone.
+ * one handle are decoded together in shared GPU packs, with or without hotword rows, each giving what it gives alone, and their
+ * punctuation ("punc-dir") and CTTransformerInfer calls on one handle share lockstep steps, each text punctuated as it is alone.
  * CompileHotwordEmbedding returns one zero row of 512 for a model without a hotword branch (Paraformer, BiCif), as the reference
  * does, so a server that decodes only when the embedding is non-empty decodes; the row is not used.  thread_num and batch_size stay ignored:
  * segments are packed by "batch-size-s".
