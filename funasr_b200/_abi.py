@@ -228,6 +228,8 @@ SIGNATURES = {
     "fa_campplus_features": (C.c_int, [_vp, _vp, _i32, _i64, _vp, _vp, _vp, _i32, _vp]),
     "fa_campplus_workspace_bytes": (_sz, [C.POINTER(FaCampplus), _i32, _i32, _i32]),
     "fa_campplus_forward": (C.c_int, [C.POINTER(FaCampplus), _vp, _i32, _i32, _vp, _i32, _vp, _sz, _vp]),
+    "fa_campplus_ext_workspace_bytes": (_sz, [C.POINTER(FaCampplus), _i32, _i32, _i32]),
+    "fa_campplus_forward_ext": (C.c_int, [C.POINTER(FaCampplus), _vp, _i32, _i32, _vp, _i32, _vp, _sz, _vp, _vp]),
     "fa_campplus_conv2d": (C.c_int, [C.POINTER(FaCamConv2d), _vp, _i32, _i32, _i32, _vp, _vp, _i32, _vp]),
     "fa_campplus_cam": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     "fa_campplus_stats_pool": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
@@ -270,6 +272,7 @@ SIGNATURES = {
     "fa_spk_uninit": (None, [_vp]),
     "fa_spk_embed": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp]),
     "fa_spk_cluster": (C.c_int, [_vp, _vp, _i32, _i32, _vp]),
+    "fa_spk_pool_stats": (C.c_int, [_vp, C.POINTER(_i64), C.POINTER(_i64)]),
     "fa_offline_infer_vad_spk": (_vp, [_vp, _vp, _vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp, _i32, _vp, _vp,
                                        C.POINTER(FaLongAudioOptions), _i32]),
     "fa_offline_result_spk": (C.POINTER(_i32), [_vp, _i32, C.POINTER(_i32)]),

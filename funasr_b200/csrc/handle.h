@@ -5,7 +5,7 @@
 //   handle_core.cu   file loader, Builder, plan_audio / upload (pcm16_to_f32_kernel, fa_ingest_pcm), fa_gather_segments
 //   offline_asr.cu   recogniser (Paraformer, contextual, BiCif, SeACo, SenseVoice): fa_offline_*
 //   offline_vad.cu   FSMN-VAD: fa_vad_*
-//   offline_spk.cu   CAM++ speaker embeddings, clustering, diarization: fa_spk_*
+//   offline_spk.cu   CAM++ speaker embeddings, clustering, diarization, and the speaker handle's request pool: fa_spk_*
 //   offline_long.cu  long audio: fa_offline_infer_vad*, fa_offline_result_{segments,spk}
 //   offline_pool.cu  the recogniser's request pool: every decoding call's passes, GPU packs and scatter; fa_offline_pool_stats
 //   offline_punc.cu  CT-Transformer punctuation and its request pool (concurrent calls share lockstep steps): fa_punc_*
@@ -253,9 +253,10 @@ bool plan_audio(const FaAudioFormat* fmt, ResampleCache& cache, Audio& a);
 const FaAudioFormat* pcm16k_format(int32_t pcm_format, FaAudioFormat& f);
 
 // B host recordings bufs[i] of n[i] frames in a's layout into 16 kHz rows of `stride` floats, *wav, carved from buf with the staged
-// bytes and the table: direct() as the 16 kHz entries always did, otherwise one fa_ingest_pcm launch
+// bytes and the table: direct() as the 16 kHz entries always did, otherwise one fa_ingest_pcm launch.  into: write the rows there
+// ([B, stride] on the device) instead, buf holding only the staged bytes and the table.
 bool upload(const void* const* bufs, const int64_t* n, int B, int64_t stride, const Audio& a, ResampleCache& cache, DevBuf& buf,
-            cudaStream_t st, float** wav);
+            cudaStream_t st, float** wav, float* into = nullptr);
 
 // rows segments of the device recording rec [n]: the host starts / lengths (samples) copied into starts_d / lens_d, then
 // fa_gather_segments into out [rows, stride] with zero tails.  The caller keeps the host arrays alive until the stream passes them.
@@ -277,9 +278,13 @@ const T* result_row(const std::vector<std::vector<T>>* rows, int32_t index, int3
 // recogniser -> VAD -> speaker (-> punctuation, aligner: never held with another), so two recognisers sharing a VAD cannot deadlock.
 // The recogniser's decoding calls do not take `mu` themselves: they post a Ticket to the handle's request pool (offline_pool.cu), and
 // the thread that leads the next pass decodes every queued compatible call in shared GPU packs.  Punctuation calls likewise post to
-// their handle's pool (offline_punc.cu), whose leader takes the punctuation lock for each lockstep step.
+// their handle's pool (offline_punc.cu), whose leader takes the punctuation lock for each lockstep step.  Speaker-only calls
+// (fa_spk_embed*, fa_spk_cluster) post to the speaker handle's pool (offline_spk.cu), whose leader takes only the speaker lock for its
+// pass; a recogniser's diarized pass takes that lock directly (diarize), after the recogniser and VAD locks, so the two interleave at
+// pass boundaries and cannot deadlock.
 struct Vad;
 struct Spk;
+struct SpkTicket;
 struct Result;
 
 // One call of fa_offline_infer* (an utterance batch) or fa_offline_infer_vad* (long audio), its arguments checked, waiting in the pool
@@ -419,8 +424,15 @@ struct Spk {
   std::vector<FaCamLayer> layers;
   ResampleCache resample;
   DevBuf upload;                                     // fa_spk_embed's batch
-  DevBuf embed, cluster_input;                       // fa_spk_embed's lengths and embeddings; fa_spk_cluster's embeddings
+  DevBuf embed, cluster_input;                       // a pass's lengths and embeddings; its clustering calls' embeddings
+  DevBuf pool_recs;                                  // one embedding pack's recordings when it holds several calls, one row each
   DevBuf spk_embed_rows, diarize, spk_cluster;
+  // the request pool: queued calls in arrival order, whether a leader is running a pass, counters since init
+  std::mutex pool_mu;
+  std::condition_variable pool_cv;
+  std::deque<SpkTicket*> pool_q;
+  bool pool_busy = false;
+  std::atomic<int64_t> pool_calls{0}, pool_passes{0};
 };
 
 // One recording of the speaker stage: recs[off, off + n) of the stage's device buffer, its {start_ms, end_ms, n_tokens} segments and

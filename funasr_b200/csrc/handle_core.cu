@@ -228,13 +228,13 @@ const FaAudioFormat* pcm16k_format(int32_t pcm_format, FaAudioFormat& f) {
 }
 
 bool upload(const void* const* bufs, const int64_t* n, int B, int64_t stride, const Audio& au, ResampleCache& cache, DevBuf& buf,
-            cudaStream_t st, float** wav) {
+            cudaStream_t st, float** wav, float* into) {
   const int64_t tot = (int64_t)B * stride;
   if (au.direct()) {
     const int32_t pcm_format = au.fmt.sample_format;
     int16_t* p16 = nullptr;
     if (!carve(buf, "waveforms", [&](fa::Arena& a) {
-          *wav = a.take<float>((size_t)(tot > 0 ? tot : 4));
+          *wav = into ? into : a.take<float>((size_t)(tot > 0 ? tot : 4));
           if (pcm_format == 1) p16 = a.take<int16_t>((size_t)tot);
         }))
       return false;
@@ -262,7 +262,7 @@ bool upload(const void* const* bufs, const int64_t* n, int B, int64_t stride, co
   float* w = nullptr;
   int32_t *first = nullptr, *n_taps = nullptr;
   if (!carve(buf, "waveforms", [&](fa::Arena& a) {
-        *wav = a.take<float>((size_t)(tot > 0 ? tot : 4));
+        *wav = into ? into : a.take<float>((size_t)(tot > 0 ? tot : 4));
         raw = a.take<unsigned char>((size_t)(bytes > 0 ? bytes : 16));
         rows_d = a.take<int64_t>((size_t)3 * B);
         if (au.tab) w = a.take<float>(au.tab->weights.size());

@@ -1,6 +1,11 @@
 // Handle-style CAM++ speaker model: fa_spk_init (model file -> handle, the BatchNorms folded on the host), fa_spk_embed (host PCM ->
-// 192-dim embeddings), fa_spk_cluster (ClusterBackend over host embeddings), and diarize, which the request pool (offline_pool.cu) runs
-// once over a group's diarized recordings already on the device.
+// 192-dim embeddings), fa_spk_cluster (ClusterBackend over host embeddings), and diarize, which the recogniser's request pool
+// (offline_pool.cu) runs once over a group's diarized recordings already on the device.
+//
+// Speaker-only calls share passes through the handle's own request pool: a call checks its arguments on its own thread and posts a
+// ticket; the thread that finds no pass running leads one over the queued calls (arrival order, up to an hour of padded audio and
+// kPoolClusterRows clustering rows) and wakes their threads.  Each call gets exactly what it gets alone: an embedding row carries its
+// call's padded length (fa_campplus_forward_ext), and each clustering call is one set of spk_cluster.
 #include "handle.h"
 #include <math.h>
 
@@ -19,6 +24,9 @@ const char* const kFcmBns[12] = {"bn1", "layer1.0.bn1", "layer1.0.bn2", "layer1.
 const int kFcmStride[12] = {1, 2, 1, 2, 1, 1, 2, 1, 2, 1, 1, 2};
 const int kSpkEmbDim = 192, kSpkMaxFrames = 18800, kChunkLen = 24000, kChunkShift = 12000;
 const size_t kSpkWorkspaceCap = (size_t)1 << 30;    // CampplusEngine.WORKSPACE_CAP: larger batches run in slices
+const int64_t kPoolSamples = 3600LL * 16000;        // padded 16 kHz samples of the embedding calls one pass takes (230 MB of fp32 rows)
+// clustering rows one pass takes: spectral sets are under 2048 rows each, so at most 2047 * 8192 doubles (134 MB) of Laplacians
+const int64_t kPoolClusterRows = 8192;
 const int kSpectralMaxChunks = 2048, kMaxSpks = 15;
 const double kSpkPval = 0.022, kMergeThr = 0.78;
 
@@ -191,13 +199,16 @@ bool build_spk(Spk& h, Builder& b) {
 int fbank_frames(int64_t n) { return n >= 400 ? (int)(1 + (n - 400) / 160) : 0; }
 
 // embeddings of a padded batch on the device (wav [B, stride], lens_d [B] on the device) -> emb [B, 192] on the device:
-// fa_campplus_features with t_max frames, then fa_campplus_forward in slices of CampplusEngine.embed_feats' workspace cap
-bool spk_embed_rows(Spk& s, const float* wav, int64_t stride, const int32_t* lens_d, int B, int t_max, float* emb) {
+// fa_campplus_features with t_max frames, then fa_campplus_forward in slices of CampplusEngine.embed_feats' workspace cap, or
+// fa_campplus_forward_ext with each row's padded length ext_h [B] (host, <= t_max)
+bool spk_embed_rows(Spk& s, const float* wav, int64_t stride, const int32_t* lens_d, int B, int t_max, float* emb,
+                    const int32_t* ext_h = nullptr) {
   cudaStream_t st = s.file.st;
   const size_t per = fa_campplus_workspace_bytes(&s.model, 1, t_max, s.mode);
   if (per == 0) { set_err("CAM++ takes 2 ... 18800 feature frames per input (got " + std::to_string(t_max) + ")"); return false; }
   const int step = (int)std::max<size_t>(1, std::min<size_t>((size_t)B, kSpkWorkspaceCap / per));
-  const size_t ws_bytes = fa_campplus_workspace_bytes(&s.model, step, t_max, s.mode);
+  const size_t ws_bytes = ext_h ? fa_campplus_ext_workspace_bytes(&s.model, step, t_max, s.mode)
+                                : fa_campplus_workspace_bytes(&s.model, step, t_max, s.mode);
   float* feats;
   int32_t* flens;
   void* ws;
@@ -208,7 +219,10 @@ bool spk_embed_rows(Spk& s, const float* wav, int64_t stride, const int32_t* len
   int rc = fa_campplus_features(wav, lens_d, B, stride, s.file.fbank_tables, feats, flens, t_max, st);
   for (int b0 = 0; b0 < B && rc == FA_OK; b0 += step) {
     const int nb = std::min(step, B - b0);
-    rc = fa_campplus_forward(&s.model, feats + (size_t)b0 * t_max * 80, nb, t_max, emb + (size_t)b0 * kSpkEmbDim, s.mode, ws, ws_bytes, st);
+    const float* f = feats + (size_t)b0 * t_max * 80;
+    float* e = emb + (size_t)b0 * kSpkEmbDim;
+    rc = ext_h ? fa_campplus_forward_ext(&s.model, f, nb, t_max, e, s.mode, ws, ws_bytes, st, ext_h + b0)
+               : fa_campplus_forward(&s.model, f, nb, t_max, e, s.mode, ws, ws_bytes, st);
   }
   if (rc != FA_OK) { set_err(std::string("CAM++: ") + fa_status_string(rc)); return false; }
   return true;
@@ -460,47 +474,243 @@ extern "C" void* fa_spk_init(const char* model_file, int32_t device, int32_t gem
 
 extern "C" void fa_spk_uninit(void* spk) { delete static_cast<Spk*>(spk); }
 
+namespace fa_handle {
+
+// One fa_spk_embed* or fa_spk_cluster call, its arguments checked, waiting in the speaker handle's pool
+struct SpkTicket {
+  bool cluster = false;
+  // fa_spk_embed*: batch rows of the caller's audio, their 16 kHz lengths, and the call's extent (fbank_frames of its longest row)
+  const void* const* bufs = nullptr;
+  const int64_t* n_samples = nullptr;
+  int batch = 0;
+  Audio au;
+  std::vector<int32_t> lens;
+  int t_max = 0;
+  int64_t stride = 0;                                // the call's padded row: its longest row rounded up to 4 samples
+  float* emb_host = nullptr;
+  // fa_spk_cluster: n host embeddings, the preset count (<= 0: none) -> labels
+  const float* emb_in = nullptr;
+  int n = 0, preset = 0;
+  int32_t* labels = nullptr;
+  // written by the pass, read by the owner once done
+  int rc = FA_ERR_CUDA;
+  std::string err;
+  bool done = false;
+};
+
+}  // namespace fa_handle
+
 namespace {
 
-// fa_spk_embed / fa_spk_embed_audio: every input checked at 16 kHz before any launch, then one padded 16 kHz batch
+int64_t ticket_samples(const SpkTicket& t) { return t.cluster ? 0 : (int64_t)t.batch * t.stride; }
+
+// The head of the queue and the calls behind it in arrival order, until an hour of padded audio or kPoolClusterRows clustering rows
+std::vector<SpkTicket*> drain(Spk& s) {
+  std::vector<SpkTicket*> out{s.pool_q.front()};
+  s.pool_q.pop_front();
+  int64_t samples = ticket_samples(*out[0]), rows = out[0]->cluster ? out[0]->n : 0;
+  while (!s.pool_q.empty()) {
+    SpkTicket* c = s.pool_q.front();
+    const int64_t sm = samples + ticket_samples(*c), r = rows + (c->cluster ? c->n : 0);
+    if (sm > kPoolSamples || r > kPoolClusterRows) break;
+    samples = sm;
+    rows = r;
+    out.push_back(c);
+    s.pool_q.pop_front();
+  }
+  return out;
+}
+
+// The embedding calls of a pass.  Calls in order of extent (arrival order within one), so each call's rows are contiguous; packs of
+// consecutive calls, a call of a larger extent joining while the pack stays within the workspace cap at that extent.  Per pack, in
+// turn: its calls uploaded in their own formats at the pack's row pitch, its longest row's (a pack of one call: that call's upload, as
+// before pooling; several: each written straight into the pack's buffer), so a pack holds its calls' own padded audio plus less than
+// one fbank frame per row, or, mixing extents, less than the workspace cap's share; fa_campplus_features at its extent and
+// fa_campplus_forward_ext with every row's own.  One copy of every embedding to the host.
+bool embed_pass(Spk& s, std::vector<SpkTicket*> ts) {
+  cudaStream_t st = s.file.st;
+  std::stable_sort(ts.begin(), ts.end(), [](const SpkTicket* a, const SpkTicket* b) { return a->t_max < b->t_max; });
+  const size_t nt = ts.size();
+  std::vector<int> first(nt + 1, 0);
+  for (size_t i = 0; i < nt; ++i) first[i + 1] = first[i] + ts[i]->batch;
+  const int R = first[nt];
+  std::vector<int32_t> lens((size_t)R), ext((size_t)R);
+  for (size_t i = 0; i < nt; ++i) {
+    std::copy(ts[i]->lens.begin(), ts[i]->lens.end(), lens.begin() + first[i]);
+    std::fill(ext.begin() + first[i], ext.begin() + first[i + 1], ts[i]->t_max);
+  }
+  int32_t* lens_d;
+  float* emb;
+  if (!carve(s.embed, "CAM++", [&](fa::Arena& a) { lens_d = a.take<int32_t>(R); emb = a.take<float>((size_t)R * kSpkEmbDim); })) return false;
+  cudaMemcpyAsync(lens_d, lens.data(), (size_t)R * 4, cudaMemcpyHostToDevice, st);
+  for (size_t i = 0; i < nt;) {
+    size_t j = i + 1;
+    int64_t rows = ts[i]->batch, stride = ts[i]->stride;
+    while (j < nt && (ts[j]->t_max == ts[j - 1]->t_max ||
+                      (size_t)(rows + ts[j]->batch) * fa_campplus_workspace_bytes(&s.model, 1, ts[j]->t_max, s.mode) <= kSpkWorkspaceCap)) {
+      stride = std::max(stride, ts[j]->stride);
+      rows += ts[j++]->batch;
+    }
+    float* recs = nullptr;
+    if (j > i + 1 && !carve(s.pool_recs, "recordings", [&](fa::Arena& a) { recs = a.take<float>((size_t)rows * stride); })) return false;
+    for (size_t k = i; k < j; ++k) {
+      const SpkTicket& t = *ts[k];
+      float* into = recs ? recs + (int64_t)(first[k] - first[i]) * stride : nullptr;
+      float* wav;
+      if (!upload(t.bufs, t.n_samples, t.batch, stride, t.au, s.resample, s.upload, st, &wav, into)) return false;
+      if (!recs) recs = wav;
+    }
+    // a pack of one extent (a lone call's) is fa_campplus_forward, bit for bit and with the kernels it always ran
+    const int r0 = first[i];
+    const bool one_extent = ts[i]->t_max == ts[j - 1]->t_max;
+    if (!spk_embed_rows(s, recs, stride, lens_d + r0, (int)rows, ts[j - 1]->t_max, emb + (size_t)r0 * kSpkEmbDim,
+                        one_extent ? nullptr : ext.data() + r0))
+      return false;
+    i = j;
+  }
+  std::vector<float> host(nt > 1 ? (size_t)R * kSpkEmbDim : 0);
+  float* dst = nt == 1 ? ts[0]->emb_host : host.data();
+  cudaMemcpyAsync(dst, emb, (size_t)R * kSpkEmbDim * 4, cudaMemcpyDeviceToHost, st);
+  if (!sync_stream(st)) return false;
+  for (size_t i = 0; i < nt; ++i) {
+    if (nt > 1) std::copy(host.begin() + (size_t)first[i] * kSpkEmbDim, host.begin() + (size_t)first[i + 1] * kSpkEmbDim, ts[i]->emb_host);
+    ts[i]->rc = FA_OK;
+  }
+  return true;
+}
+
+// The clustering calls of a pass: their embeddings in one buffer (a lone call's straight from its host array, as before pooling), one
+// spk_cluster over all their sets; a set's refusal fails only its own call, with the message it gets alone
+bool cluster_pass(Spk& s, const std::vector<SpkTicket*>& ts) {
+  std::vector<ClusterSet> sets(ts.size());
+  int64_t rows = 0;
+  for (size_t i = 0; i < ts.size(); ++i) {
+    sets[i].first = (int)rows;
+    sets[i].n = ts[i]->n;
+    sets[i].preset = ts[i]->preset;
+    rows += ts[i]->n;
+  }
+  std::vector<float> staged;
+  const float* emb_h = ts[0]->emb_in;
+  if (ts.size() > 1) {
+    staged.resize((size_t)rows * kSpkEmbDim);
+    for (size_t i = 0; i < ts.size(); ++i)
+      std::copy(ts[i]->emb_in, ts[i]->emb_in + (size_t)ts[i]->n * kSpkEmbDim, staged.begin() + (size_t)sets[i].first * kSpkEmbDim);
+    emb_h = staged.data();
+  }
+  float* emb;
+  if (!carve(s.cluster_input, "speaker clustering", [&](fa::Arena& a) { emb = a.take<float>((size_t)rows * kSpkEmbDim); })) return false;
+  cudaMemcpyAsync(emb, emb_h, (size_t)rows * kSpkEmbDim * 4, cudaMemcpyHostToDevice, s.file.st);
+  if (!spk_cluster(s, emb, emb_h, sets)) return false;
+  for (size_t i = 0; i < ts.size(); ++i) {
+    if (!sets[i].err.empty()) { ts[i]->err = sets[i].err; continue; }
+    std::copy(sets[i].labels.begin(), sets[i].labels.end(), ts[i]->labels);
+    ts[i]->rc = FA_OK;
+  }
+  return true;
+}
+
+// One pass under the speaker lock: the embedding calls, then the clustering calls.  A device failure fails every call of the pass.
+void run_pass(Spk& s, const std::vector<SpkTicket*>& pass) {
+  std::vector<SpkTicket*> emb, clu;
+  for (SpkTicket* t : pass) (t->cluster ? clu : emb).push_back(t);
+  {
+    std::lock_guard<std::mutex> dev(s.mu);
+    cudaSetDevice(s.file.device);
+    const bool ok = no_throw("fa_spk_embed: ", [&] { return emb.empty() || embed_pass(s, emb); }) &&
+                    no_throw("fa_spk_cluster: ", [&] { return clu.empty() || cluster_pass(s, clu); });
+    if (!ok)
+      for (SpkTicket* t : pass) { t->rc = FA_ERR_CUDA; t->err = g_err; }
+  }
+  ++s.pool_passes;
+  s.pool_calls += (int64_t)pass.size();
+}
+
+// t's call through the pool -> its status, with its own message set as this thread's error
+int pool_call(Spk& s, SpkTicket& t) {
+  // Whatever a pass throws, the tickets it drained end done (with a message when they have none), pool_busy is cleared and the
+  // waiters are woken, so the next caller can lead; no exception crosses the C ABI.
+  struct Lead {
+    Spk& s;
+    std::unique_lock<std::mutex>& q;
+    std::vector<SpkTicket*> pass;
+    ~Lead() {
+      if (!q.owns_lock()) q.lock();
+      for (SpkTicket* p : pass) {
+        if (p->rc != FA_OK && p->err.empty()) p->err = "fa_spk: the pass failed";
+        p->done = true;
+      }
+      s.pool_busy = false;
+      s.pool_cv.notify_all();
+    }
+  };
+  std::string msg;
+  try {
+    std::unique_lock<std::mutex> q(s.pool_mu);
+    s.pool_q.push_back(&t);
+    while (!t.done) {
+      if (s.pool_busy) {                                    // a leader is running a pass: it may drain this ticket
+        s.pool_cv.wait(q);
+        continue;
+      }
+      s.pool_busy = true;
+      Lead lead{s, q, {}};
+      lead.pass = drain(s);
+      q.unlock();
+      run_pass(s, lead.pass);
+    }
+  } catch (const std::exception& e) {
+    msg = std::string("fa_spk: ") + e.what();
+    try {                                                   // never leave this ticket where a leader could still write to it
+      std::unique_lock<std::mutex> q(s.pool_mu);
+      auto it = std::find(s.pool_q.begin(), s.pool_q.end(), &t);
+      if (it != s.pool_q.end()) s.pool_q.erase(it);
+      else s.pool_cv.wait(q, [&] { return t.done; });
+    } catch (const std::exception&) {
+    }
+    set_err(msg);
+    return FA_ERR_CUDA;
+  }
+  if (t.rc != FA_OK) { set_err(t.err); return t.rc; }
+  g_err.clear();
+  return FA_OK;
+}
+
+// fa_spk_embed / fa_spk_embed_audio: every input checked at 16 kHz on the calling thread, then the call's rows through the pool, padded
+// to its longest input
 int spk_embed(void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch, const FaAudioFormat* fmt, float* emb_host) {
   Spk* s = static_cast<Spk*>(spk);
   if (!s || !bufs || !n_samples || batch <= 0 || !emb_host) { set_err("fa_spk_embed: bad argument"); return FA_ERR_ARG; }
-  Audio au;
-  if (!plan_audio(fmt, s->resample, au)) return FA_ERR_ARG;
+  SpkTicket t;
+  if (!plan_audio(fmt, s->resample, t.au)) return FA_ERR_ARG;
   int64_t nmax = 0;
   int longest = 0;
-  std::vector<int32_t> lens_h(batch);
-  for (int32_t i = 0; i < batch; ++i) {              // every input checked before any launch
-    const int64_t n16 = n_samples[i] >= 0 && n_samples[i] <= 0x7fffffffLL ? au.len16(n_samples[i]) : n_samples[i];
-    if (!bufs[i] || n16 < 400 || n16 > 0x7fffffffLL) {
-      set_err("input " + std::to_string(i) + " has " + std::to_string(n16) + " samples" + au.at16k() + "; CAM++ needs at least 400 (one 25 ms frame)");
-      return FA_ERR_ARG;
+  const bool ok = no_throw("fa_spk_embed: ", [&] {
+    t.lens.resize(batch);
+    for (int32_t i = 0; i < batch; ++i) {            // every input checked before any launch
+      const int64_t n16 = n_samples[i] >= 0 && n_samples[i] <= 0x7fffffffLL ? t.au.len16(n_samples[i]) : n_samples[i];
+      if (!bufs[i] || n16 < 400 || n16 > 0x7fffffffLL) {
+        set_err("input " + std::to_string(i) + " has " + std::to_string(n16) + " samples" + t.au.at16k() + "; CAM++ needs at least 400 (one 25 ms frame)");
+        return false;
+      }
+      t.lens[i] = (int32_t)n16;
+      if (n16 > nmax) { nmax = n16; longest = i; }
     }
-    lens_h[i] = (int32_t)n16;
-    if (n16 > nmax) { nmax = n16; longest = i; }
-  }
-  const int t_max = fbank_frames(nmax);
-  if (t_max > kSpkMaxFrames) {
-    set_err("input " + std::to_string(longest) + " has " + std::to_string(t_max) + " feature frames; CAM++ takes at most " +
+    return true;
+  });
+  if (!ok) return FA_ERR_ARG;
+  t.t_max = fbank_frames(nmax);
+  if (t.t_max > kSpkMaxFrames) {
+    set_err("input " + std::to_string(longest) + " has " + std::to_string(t.t_max) + " feature frames; CAM++ takes at most " +
             std::to_string(kSpkMaxFrames) + " (MAX_FEAT_FRAMES)");
     return FA_ERR_UNSUPPORTED;
   }
-  std::lock_guard<std::mutex> dev(s->mu);
-  cudaSetDevice(s->file.device);
-  cudaStream_t st = s->file.st;
-  const int64_t stride = (nmax + 3) / 4 * 4;
-  const bool ok = no_throw("fa_spk_embed: ", [&] {
-    int32_t* lens;
-    float *emb, *wav;
-    if (!carve(s->embed, "CAM++", [&](fa::Arena& a) { lens = a.take<int32_t>(batch); emb = a.take<float>((size_t)batch * kSpkEmbDim); })) return false;
-    if (!upload(bufs, n_samples, batch, stride, au, s->resample, s->upload, st, &wav)) return false;
-    cudaMemcpyAsync(lens, lens_h.data(), (size_t)batch * 4, cudaMemcpyHostToDevice, st);
-    if (!spk_embed_rows(*s, wav, stride, lens, batch, t_max, emb)) return false;
-    cudaMemcpyAsync(emb_host, emb, (size_t)batch * kSpkEmbDim * 4, cudaMemcpyDeviceToHost, st);
-    return sync_stream(st);
-  });
-  return ok ? FA_OK : FA_ERR_CUDA;
+  t.bufs = bufs;
+  t.n_samples = n_samples;
+  t.batch = batch;
+  t.stride = (nmax + 3) / 4 * 4;
+  t.emb_host = emb_host;
+  return pool_call(*s, t);
 }
 
 }  // namespace
@@ -526,20 +736,19 @@ extern "C" int fa_spk_cluster(void* spk, const float* emb_host, int32_t n, int32
             "this backend does not provide; pass preset_spk_num or diarize fewer than 2048 chunks");
     return FA_ERR_UNSUPPORTED;
   }
-  std::lock_guard<std::mutex> dev(s->mu);
-  cudaSetDevice(s->file.device);
-  std::vector<ClusterSet> sets(1);
-  sets[0].n = n;
-  sets[0].preset = preset_spk_num;
-  const bool ok = no_throw("fa_spk_cluster: ", [&] {
-    float* emb;
-    if (!carve(s->cluster_input, "speaker clustering", [&](fa::Arena& a) { emb = a.take<float>((size_t)n * kSpkEmbDim); })) return false;
-    cudaMemcpyAsync(emb, emb_host, (size_t)n * kSpkEmbDim * 4, cudaMemcpyHostToDevice, s->file.st);
-    if (!spk_cluster(*s, emb, emb_host, sets)) return false;
-    if (!sets[0].err.empty()) { set_err(sets[0].err); return false; }
-    return true;
-  });
-  if (!ok) return FA_ERR_CUDA;
-  std::copy(sets[0].labels.begin(), sets[0].labels.end(), labels);
+  SpkTicket t;
+  t.cluster = true;
+  t.emb_in = emb_host;
+  t.n = n;
+  t.preset = preset_spk_num;
+  t.labels = labels;
+  return pool_call(*s, t);
+}
+
+extern "C" int fa_spk_pool_stats(const void* spk, int64_t* calls, int64_t* passes) {
+  const Spk* s = static_cast<const Spk*>(spk);
+  if (!s || !calls || !passes) return FA_ERR_ARG;
+  *calls = s->pool_calls.load();
+  *passes = s->pool_passes.load();
   return FA_OK;
 }

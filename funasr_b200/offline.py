@@ -227,6 +227,13 @@ class OfflineSpeaker:
             raise _abi.FunasrB200Error("fa_spk_embed failed: %s" % self.lib.fa_offline_last_error().decode())
         return out
 
+    def pool_stats(self):
+        """(calls, passes): the embedding and clustering calls the handle's pool has served since init and the passes it ran them in;
+        concurrent `embed` calls from many threads share passes."""
+        c, p = C.c_int64(), C.c_int64()
+        _abi.check(self.lib.fa_spk_pool_stats(self.handle, C.byref(c), C.byref(p)), "fa_spk_pool_stats")
+        return c.value, p.value
+
     def close(self):
         if getattr(self, "handle", None):
             self.lib.fa_spk_uninit(self.handle)

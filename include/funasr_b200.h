@@ -719,6 +719,14 @@ int fa_campplus_features(const float* wav, const int32_t* wav_lens, int32_t batc
 size_t fa_campplus_workspace_bytes(const FaCampplus* model, int32_t batch, int32_t t, int32_t gemm_mode);
 int fa_campplus_forward(const FaCampplus* model, const float* feats, int32_t batch, int32_t t, float* emb, int32_t gemm_mode,
                         void* workspace, size_t ws_bytes, fa_stream_t stream);
+/* fa_campplus_forward with a padded length per row: row b's embedding equals fa_campplus_forward on feats[b, :ext_h[b]] alone
+ * (a batch padded to ext_h[b] frames), bit for bit.  Frames at or past ext_h[b] are never read.  ext_h [B] is a HOST array,
+ * 2 <= ext_h[b] <= t (FA_ERR_ARG otherwise), t <= 18 800 (FA_ERR_UNSUPPORTED), both before anything is enqueued; it may be reused
+ * once the call returns.  ext_h[b] == t for every row is fa_campplus_forward bit for bit.  Workspace:
+ * fa_campplus_ext_workspace_bytes (0 where fa_campplus_workspace_bytes is 0, at least that much otherwise). */
+size_t fa_campplus_ext_workspace_bytes(const FaCampplus* model, int32_t batch, int32_t t, int32_t gemm_mode);
+int fa_campplus_forward_ext(const FaCampplus* model, const float* feats, int32_t batch, int32_t t, float* emb, int32_t gemm_mode,
+                            void* workspace, size_t ws_bytes, fa_stream_t stream, const int32_t* ext_h);
 /* Layer entry points of the forward (exposed for parity tests).  conv2d: x [B][f_in][t][c_in] channels last -> y [B][f_out][t][32],
  * y = act(conv(x) + b (+ res)), res in y's layout or NULL. */
 int fa_campplus_conv2d(const FaCamConv2d* conv, const float* x, int32_t batch, int32_t f_in, int32_t t, const float* res, float* y,
@@ -833,10 +841,14 @@ const char* fa_offline_last_error(void);
  * speaker handle (preset_spk_num may differ).
  * A device failure during a pass fails every call of that pass with its message.  Punctuation calls (fa_punc_infer) on one handle
  * share lockstep steps: the thread that finds no step running leads, each step admitting the queued calls in arrival order and scoring
- * one window of every active text of every admitted call, and each text gets exactly what it gets alone (fa_punc_infer below).  The
- * aligner's, the VAD-only (fa_vad_infer*) and the speaker-only (fa_spk_*) calls hold the handle's lock for their device work and run
- * one after another.  A call that uses several handles (fa_offline_infer_vad*) locks them in the order recogniser, VAD, speaker, so
- * recognisers that share a VAD handle cannot deadlock; the punctuation and aligner locks are never held with another.
+ * one window of every active text of every admitted call, and each text gets exactly what it gets alone (fa_punc_infer below).
+ * Speaker-only calls (fa_spk_embed*, fa_spk_cluster) on one handle share passes: the leader drains the queued calls in arrival order
+ * (up to an hour of padded audio and 8 192 clustering rows), embeds every row at its own call's padded length
+ * (fa_campplus_forward_ext) in packs sorted by that length, and clusters every clustering call's set in one batched spectral pass; each
+ * call gets exactly what it gets alone.  The aligner's and the VAD-only (fa_vad_infer*) calls hold the handle's lock for their device
+ * work and run one after another.  A call that uses several handles (fa_offline_infer_vad*) locks them in the order recogniser, VAD,
+ * speaker, so recognisers that share a VAD handle cannot deadlock; the speaker pool's leader holds only the speaker lock, and the
+ * punctuation and aligner locks are never held with another.
  * fa_offline_last_error is per thread.  Uninit a handle only after every call on it has returned. */
 /* Calls the recogniser handle's pool has decoded since init, and the GPU packs it decoded them in (packs < calls: calls were pooled).
  * 0, or FA_ERR_ARG for a NULL argument. */
@@ -919,18 +931,24 @@ int64_t fa_merge_vad(const int32_t* segments, int64_t n, int32_t max_length_ms, 
  * piece: a missing or misshapen tensor, another __spk_config__, a file that also carries another model kind's config.  The BatchNorms
  * are folded on the host in float64 exactly as CampplusEngine folds them, so embeddings are bit-identical to it in every gemm_mode.
  * fa_spk_embed: batch HOST recordings (pcm_format 0 = float32, 1 = s16le; 16 kHz; ragged) -> emb_host [batch, 192]: CAMPPlus.inference
- * (features zero-padded to the longest input, the padded frames taking part in every mean; fa_campplus_features, fa_campplus_forward in
- * slices of 1 GiB of workspace).  An input under 400 samples (FA_ERR_ARG) or with more than 18 800 feature frames (FA_ERR_UNSUPPORTED)
- * fails the call before any launch, naming the input.  FA_OK or a negative status (fa_offline_last_error()).
+ * (features zero-padded to the longest input, the padded frames taking part in every mean; fa_campplus_features, fa_campplus_forward
+ * in slices of 1 GiB of workspace, or fa_campplus_forward_ext at each call's padded length where pooled calls share a pack).  An input under 400 samples (FA_ERR_ARG) or with
+ * more than 18 800 feature frames (FA_ERR_UNSUPPORTED) fails the call on its own thread before it joins the pool, naming the input.
+ * Concurrent calls on one handle share passes (Threads above), and a lone call launches what one call launched before pooling.  FA_OK
+ * or a negative status (fa_offline_last_error()).
  * fa_spk_cluster: ClusterBackend()(emb_host [n, 192], oracle_num = preset_spk_num > 0 ? preset_spk_num : None) -> labels [n] (before
  * correct_labels): fewer than 20 rows one speaker; fewer than 2048 the spectral path (fa_spk_laplacian, fa_spk_tridiagonalize,
  * fa_sym_tridiag_smallest_host, fa_spk_back_transform, the eigengap count unless preset, k-means); 2048 or more k-means on the
- * normalised rows with a preset count, and without one FA_ERR_UNSUPPORTED (the reference's UMAP + HDBSCAN path is not provided);
- * merge_by_cos at 0.78 when no count is preset. */
+ * normalised rows with a preset count, and without one FA_ERR_UNSUPPORTED (the reference's UMAP + HDBSCAN path is not provided, refused
+ * on the calling thread); merge_by_cos at 0.78 when no count is preset.  Concurrent calls on one handle are clustered together (the
+ * _batch entries below), each set with exactly its own result; a refusal of one set (preset_spk_num above n) fails only its call. */
 void* fa_spk_init(const char* model_file, int32_t device, int32_t gemm_mode);
 void fa_spk_uninit(void* spk);
 int fa_spk_embed(void* spk, const void* const* bufs, const int64_t* n_samples, int32_t batch, int32_t pcm_format, float* emb_host);
 int fa_spk_cluster(void* spk, const float* emb_host, int32_t n, int32_t preset_spk_num, int32_t* labels);
+/* Calls the speaker handle's pool has served since init (fa_spk_embed*, fa_spk_cluster) and the passes it ran them in (passes < calls:
+ * calls were pooled).  0, or FA_ERR_ARG for a NULL argument. */
+int fa_spk_pool_stats(const void* spk, int64_t* calls, int64_t* passes);
 /* fa_offline_infer_vad (language_ids / textnorm_ids: fa_offline_infer_vad_sv's, NULL except on SenseVoice) followed, for every
  * recording that decoded at least one token, by LongAudioPipeline.generate's diarization in vad_segment mode: sv_chunk's 1.5 s windows
  * every 0.75 s over each VAD segment (the last pulled back), gathered from the device-resident recording with zero tails
