@@ -10,7 +10,7 @@ if [ "$(cat ../_build/flags 2>/dev/null)" != "$FLAGS" ]; then rm -f ../_build/*.
 objs=""
 pids=""
 for f in fbank layernorm gemm_f32 gemm_tc attention_tc attention_f32 fsmn cif decode_ops model handle_core offline_asr offline_vad offline_spk offline_long offline_pool offline_punc offline_align lstm hotword resample vad campplus spk_cluster; do
-  if [ ! -f ../_build/$f.o ] || [ $f.cu -nt ../_build/$f.o ] || [ common.cuh -nt ../_build/$f.o ] || [ kernels.h -nt ../_build/$f.o ] || [ handle.h -nt ../_build/$f.o ] || [ tc_common.cuh -nt ../_build/$f.o ] || [ ../../include/funasr_b200.h -nt ../_build/$f.o ] || [ punc_text.h -nt ../_build/$f.o ]; then
+  if [ ! -f ../_build/$f.o ] || [ $f.cu -nt ../_build/$f.o ] || [ common.cuh -nt ../_build/$f.o ] || [ kernels.h -nt ../_build/$f.o ] || [ handle.h -nt ../_build/$f.o ] || [ request_pool.h -nt ../_build/$f.o ] || [ tc_common.cuh -nt ../_build/$f.o ] || [ ../../include/funasr_b200.h -nt ../_build/$f.o ] || [ punc_text.h -nt ../_build/$f.o ]; then
     ( $NVCC $FLAGS -c $f.cu -o ../_build/$f.o 2> ../_build/$f.ptxas.log || { cat ../_build/$f.ptxas.log; rm -f ../_build/$f.o; exit 1; } ) &
     pids="$pids $!"
   fi

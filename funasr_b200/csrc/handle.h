@@ -12,10 +12,9 @@
 //   offline_align.cu MonotonicAligner (fa-zh) forced alignment: fa_align_*
 #pragma once
 #include "common.cuh"
+#include "request_pool.h"
 #include <algorithm>
 #include <atomic>
-#include <condition_variable>
-#include <deque>
 #include <exception>
 #include <map>
 #include <memory>
@@ -276,19 +275,20 @@ const T* result_row(const std::vector<std::vector<T>>* rows, int32_t index, int3
 // Any handle may be shared by many threads.  Each handle has a device lock (`mu`), held by a call for all of its work on the handle's
 // stream and buffers; argument checks run before it is taken.  A call that needs several handles takes their locks in one order,
 // recogniser -> VAD -> speaker (-> punctuation, aligner: never held with another), so two recognisers sharing a VAD cannot deadlock.
-// The recogniser's decoding calls do not take `mu` themselves: they post a Ticket to the handle's request pool (offline_pool.cu), and
-// the thread that leads the next pass decodes every queued compatible call in shared GPU packs.  Punctuation calls likewise post to
-// their handle's pool (offline_punc.cu), whose leader takes the punctuation lock for each lockstep step.  Speaker-only calls
-// (fa_spk_embed*, fa_spk_cluster) post to the speaker handle's pool (offline_spk.cu), whose leader takes only the speaker lock for its
-// pass; a recogniser's diarized pass takes that lock directly (diarize), after the recogniser and VAD locks, so the two interleave at
-// pass boundaries and cannot deadlock.
+// The recogniser's decoding calls, speaker-only calls (fa_spk_embed*, fa_spk_cluster) and punctuation calls do not take `mu`
+// themselves: they post a ticket to their handle's request pool (request_pool.h), whose leading thread runs rounds over every
+// caller's tickets, each round taking the device locks it needs.  A recogniser round is one pass that decodes the queued compatible
+// calls in shared GPU packs under the recogniser, VAD and speaker locks (offline_pool.cu); a speaker round is one pass under the
+// speaker lock alone (offline_spk.cu); a punctuation round is one lockstep step under the punctuation lock (offline_punc.cu).  A
+// recogniser's diarized pass takes the speaker lock directly (diarize), after the recogniser and VAD locks, so it and the speaker
+// pool's passes interleave at pass boundaries and cannot deadlock.
 struct Vad;
 struct Spk;
 struct SpkTicket;
 struct Result;
 
 // One call of fa_offline_infer* (an utterance batch) or fa_offline_infer_vad* (long audio), its arguments checked, waiting in the pool
-struct Ticket {
+struct Ticket : PoolTicket {
   const void* const* bufs = nullptr;
   const int64_t* n_samples = nullptr;                // the caller's frames
   int batch = 0;
@@ -303,10 +303,7 @@ struct Ticket {
   FaLongAudioOptions opts{};
   Spk* spk = nullptr;                                // diarized: shares a pass only with the same speaker handle, or none
   int32_t preset_spk_num = 0;
-  // written by the pass, read by the owner once done
-  std::unique_ptr<Result> res;
-  std::string err;
-  bool done = false;
+  std::unique_ptr<Result> res;                       // written by the pass, read by the owner once done
 };
 
 struct Model {
@@ -347,12 +344,8 @@ struct Model {
   DevBuf pool_recs;                                  // a pass's recordings and utterances, one row each (pool_group)
   DevBuf pack;                                       // pool_group: one GPU pack's gather offsets and padded rows
   DevBuf ws;                                         // the GEMM workspace every stage above uses in turn
-  // the request pool: queued tickets in arrival order, whether a leader is running a pass, counters since init
-  std::mutex pool_mu;
-  std::condition_variable pool_cv;
-  std::deque<Ticket*> pool_q;
-  bool pool_busy = false;
-  std::atomic<int64_t> pool_calls{0}, pool_packs{0};
+  RequestPool<Ticket> pool;                          // each round one pass (offline_pool.cu)
+  std::atomic<int64_t> pool_packs{0};                // GPU packs decoded since init
 };
 
 struct Result {
@@ -386,7 +379,7 @@ struct PackHotwords {
 // each reference pack's hotword biasing is the one the reference gives that batch.
 std::unique_ptr<Result> decode_pack(Model& m, const float* wav, int64_t stride, const std::vector<int32_t>& lens_h, const std::vector<int32_t>& ext_h,
                                     const PackHotwords* hw, const int32_t* lang, const int32_t* tn);
-// t's call through the recogniser's request pool: queued, decoded by whichever thread leads the pass that drains it -> its result, or
+// t's call through the recogniser's request pool: queued, decoded by whichever thread leads the pass that admits it -> its result, or
 // nullptr with its own message set as this thread's error
 void* pool_call(Model& m, Ticket& t);
 
@@ -427,12 +420,8 @@ struct Spk {
   DevBuf embed, cluster_input;                       // a pass's lengths and embeddings; its clustering calls' embeddings
   DevBuf pool_recs;                                  // one embedding pack's recordings when it holds several calls, one row each
   DevBuf spk_embed_rows, diarize, spk_cluster;
-  // the request pool: queued calls in arrival order, whether a leader is running a pass, counters since init
-  std::mutex pool_mu;
-  std::condition_variable pool_cv;
-  std::deque<SpkTicket*> pool_q;
-  bool pool_busy = false;
-  std::atomic<int64_t> pool_calls{0}, pool_passes{0};
+  RequestPool<SpkTicket> pool;                       // each round one pass of speaker-only calls (offline_spk.cu)
+  std::atomic<int64_t> pool_passes{0};               // passes run since init
 };
 
 // One recording of the speaker stage: recs[off, off + n) of the stage's device buffer, its {start_ms, end_ms, n_tokens} segments and

@@ -6,13 +6,14 @@
 // Rows of many calls can therefore share one pack: each row carries the extent of the batch the reference would decode it in, its
 // "reference pack".
 //
-// A call posts a Ticket and waits.  The thread that finds no pass running leads one: it drains the queued compatible tickets in arrival
-// order (up to an hour of padded audio), takes the device lock and, per group of rows:
+// A call posts a Ticket to the handle's request pool (request_pool.h).  Each round of the pool's leader is one pass: it admits the
+// head of the queue and the later compatible tickets in arrival order (up to an hour of padded audio), takes the device locks and,
+// per group of rows:
 //   uploads every recording and utterance batch into one buffer, runs one batched VAD pass over the long-audio recordings,
 //   forms each call's reference packs and their extents, merges reference packs of different calls into GPU packs (sorted by extent,
 //   at most kPackSamples of padded audio, a larger reference pack alone), decodes each, and scatters the rows back.
-// Pack-level rules of the reference (a long-audio pack without a token empties its recording) apply per reference pack.  The leader
-// then marks the drained tickets done and wakes their threads; it leads again until its own ticket is done.  No thread is created.
+// Pack-level rules of the reference (a long-audio pack without a token empties its recording) apply per reference pack.  Every ticket
+// of a pass ends with it.
 //
 // Hotword calls (contextual and SeACo Paraformer) pool like any other: the reference gives every utterance of a batch the same hotword
 // memory, and for SeACo with more rows than nfilter the attention-score filter of the batch's utterance 0, so the memory belongs to the
@@ -51,27 +52,24 @@ int64_t ticket_samples(const Ticket& t) {
   return s;
 }
 
-// The head of the queue and every later ticket that may share its packs, in arrival order, until an hour of padded audio.  Long-audio
-// tickets share a pass only with the same VAD handle and options, diarized tickets only with the same speaker handle (a pass takes at
-// most one speaker lock); the others stay queued for a later pass.
-std::vector<Ticket*> drain(Model& m) {
-  std::vector<Ticket*> out{m.pool_q.front()};
-  m.pool_q.pop_front();
-  const Ticket* key = out[0]->long_audio ? out[0] : nullptr;
-  Spk* spk = out[0]->spk;
-  int64_t samples = ticket_samples(*out[0]);
-  for (auto it = m.pool_q.begin(); it != m.pool_q.end();) {
+// A pass's admission: the head of the queue and every later ticket that may share its packs, in arrival order, until an hour of padded
+// audio.  Long-audio tickets share a pass only with the same VAD handle and options, diarized tickets only with the same speaker handle
+// (a pass takes at most one speaker lock); the others stay queued for a later pass.
+void admit(std::deque<Ticket*>& queue, std::vector<Ticket*>& pass) {
+  const Ticket* key = nullptr;
+  Spk* spk = nullptr;
+  int64_t samples = 0;
+  for (auto it = queue.begin(); it != queue.end();) {
     Ticket* c = *it;
     if ((c->long_audio && key && (c->vad != key->vad || !same_opts(c->opts, key->opts))) || (c->spk && spk && c->spk != spk)) { ++it; continue; }
     const int64_t s = ticket_samples(*c);
-    if (samples + s > kVadGroupSamples) break;
+    if (!pass.empty() && samples + s > kVadGroupSamples) break;
     samples += s;
     if (c->long_audio && !key) key = c;
     if (c->spk && !spk) spk = c->spk;
-    out.push_back(c);
-    it = m.pool_q.erase(it);
+    pass.push_back(c);
+    it = queue.erase(it);
   }
-  return out;
 }
 
 // rows the reference decodes together: a call's utterance batch, or one pack of one recording's VAD segments
@@ -97,8 +95,7 @@ struct LongRec {
 // a slice of one ticket's buffers: a whole utterance batch, or one long-audio recording
 struct Unit { Ticket* t; int first, count; };
 
-bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::vector<char>& failed, const std::vector<Ticket*>& pass,
-                const PackHotwords& sets) {
+bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, const PackHotwords& sets) {
   cudaStream_t st = m.file.st;
   // rows: long-audio recordings first (one batched VAD pass reads them as [nl, stride]), then the utterance batches
   std::vector<int> row(units.size());
@@ -106,7 +103,7 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
   for (int pass_long = 1; pass_long >= 0; --pass_long)
     for (size_t u = 0; u < units.size(); ++u)
       if (units[u].t->long_audio == (pass_long == 1)) { row[u] = rows; rows += units[u].count; nl += pass_long ? units[u].count : 0; }
-  // one unit (a lone caller): its upload is the group's buffer, as the take-turns path decoded from it; several: one copy each
+  // one unit (a lone caller): its upload is the group's buffer, as the take-turns path decoded from it; several: each written into it
   float* recs = nullptr;
   if (units.size() > 1 &&
       !carve(m.pool_recs, "recordings", [&](fa::Arena& a) { recs = a.take<float>((size_t)std::max<int64_t>((int64_t)rows * stride, 4)); }))
@@ -116,10 +113,10 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
   FaVadRunOptions vro{};
   for (size_t u = 0; u < units.size(); ++u) {
     const Unit& un = units[u];
-    float* wav = nullptr;
-    if (!upload(&un.t->bufs[un.first], &un.t->n_samples[un.first], un.count, stride, un.t->au, m.resample, m.upload, st, &wav)) return false;
-    if (units.size() == 1) recs = wav;
-    else if (stride > 0) cudaMemcpyAsync(recs + (int64_t)row[u] * stride, wav, (size_t)un.count * stride * 4, cudaMemcpyDeviceToDevice, st);
+    float* into = recs ? recs + (int64_t)row[u] * stride : nullptr;
+    float* wav;
+    if (!upload(&un.t->bufs[un.first], &un.t->n_samples[un.first], un.count, stride, un.t->au, m.resample, m.upload, st, &wav, into)) return false;
+    if (!recs) recs = wav;
     if (un.t->long_audio) { vad = un.t->vad; vro = un.t->opts.vad; }
   }
   for (size_t u = 0; u < units.size(); ++u)
@@ -133,7 +130,6 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
   int li = 0;
   for (size_t u = 0; u < units.size(); ++u) {
     Ticket& t = *units[u].t;
-    const int ti = (int)(std::find(pass.begin(), pass.end(), &t) - pass.begin());
     if (!t.long_audio) {
       RefPack p{&t};
       p.set = t.hw_set;
@@ -150,7 +146,7 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
       continue;
     }
     const VadResult& v = vr[li++];
-    if (failed[ti]) continue;
+    if (!t.err.empty()) continue;                            // failed in an earlier group
     const FaLongAudioOptions& o = t.opts;
     const int i = units[u].first;
     const int64_t n = t.n16[i];
@@ -285,24 +281,24 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
     if (m.ts) t.res->stamps.swap(rp.out->stamps);
   }
   // each recording's own failure, decided in recording order once the speaker stage has run: a short VAD segment where the reference
-  // reaches it, or a refusal of the speaker stage.  A ticket's later recordings in the group are not assembled after its first.
+  // reaches it, or a refusal of the speaker stage.  A ticket's later recordings in the group (consecutive in longs) are not assembled
+  // after its first.
   std::vector<std::string> rec_err(longs.size());
   std::vector<int> job_of(longs.size(), -1);
-  std::vector<char> stopped(pass.size(), 0);
+  const Ticket* stopped = nullptr;
   std::vector<SpkJob> jobs;
   Spk* spk = nullptr;
   for (size_t li = 0; li < longs.size(); ++li) {
     LongRec& lr = longs[li];
     Ticket& t = *lr.t;
-    const int ti = (int)(std::find(pass.begin(), pass.end(), &t) - pass.begin());
-    if (failed[ti] || stopped[ti]) continue;
+    if (!t.err.empty() || &t == stopped) continue;
     const int64_t ns = (int64_t)lr.segs.size() / 2;
     std::vector<std::vector<int32_t>> seg_ids((size_t)ns), seg_stamps((size_t)ns);
     bool emptied = false;
     int beg = 0;
     for (int p : lr.packs) {                                 // the reference's pack loop: a bad segment fails the call where it is reached
       RefPack& rp = packs[p];
-      if (!rp.bad.empty()) { rec_err[li] = rp.bad; stopped[ti] = 1; break; }
+      if (!rp.bad.empty()) { rec_err[li] = rp.bad; stopped = &t; break; }
       int tmax = 0;
       for (int32_t k : rp.out->token_num) tmax = std::max(tmax, k);
       // no token in the whole pack: the recording's result is empty (:990-999).  SenseVoiceSmall.inference returns a result for every
@@ -314,7 +310,7 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
       }
       beg += (int)rp.lens.size();
     }
-    if (stopped[ti]) continue;
+    if (stopped == &t) continue;
     std::vector<int32_t>&ids = t.res->ids[lr.i], &segs_out = t.res->segs[lr.i], &stamps = t.res->stamps[lr.i];
     for (int64_t s = 0; s < ns; ++s) {
       const int32_t k = emptied ? 0 : (int32_t)seg_ids[s].size();
@@ -330,7 +326,7 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
       jb.what = "recording " + std::to_string(lr.i) + ": "; jb.spk = &t.res->spk[lr.i];
       job_of[li] = (int)jobs.size();
       jobs.push_back(std::move(jb));
-      spk = t.spk;                                           // one speaker handle per pass (drain)
+      spk = t.spk;                                           // one speaker handle per pass (admit)
     }
   }
   // one speaker stage over the group's diarized recordings.  The recogniser's stream is idle here (its results are on the host); the
@@ -338,15 +334,13 @@ bool pool_group(Model& m, const std::vector<Unit>& units, int64_t stride, std::v
   if (!jobs.empty() && !diarize(*spk, recs, (int64_t)rows * stride, jobs)) return false;
   for (size_t li = 0; li < longs.size(); ++li) {
     Ticket& t = *longs[li].t;
-    const int ti = (int)(std::find(pass.begin(), pass.end(), &t) - pass.begin());
-    if (failed[ti]) continue;
-    const std::string& e = !rec_err[li].empty() ? rec_err[li] : (job_of[li] >= 0 ? jobs[job_of[li]].err : rec_err[li]);
-    if (!e.empty()) { t.err = e; failed[ti] = 1; }
+    if (!t.err.empty()) continue;
+    t.err = !rec_err[li].empty() ? rec_err[li] : (job_of[li] >= 0 ? jobs[job_of[li]].err : rec_err[li]);
   }
   return true;
 }
 
-// One pass over the drained tickets under the device locks (recogniser -> VAD -> speaker): every ticket ends with a result or a message
+// One pass over the admitted tickets under the device locks (recogniser -> VAD -> speaker): every ticket ends with a result or a message
 void run_pass(Model& m, const std::vector<Ticket*>& pass) {
   std::lock_guard<std::mutex> dev(m.mu);
   Vad* vad = nullptr;
@@ -359,8 +353,6 @@ void run_pass(Model& m, const std::vector<Ticket*>& pass) {
   if (vad) vad_lock = std::unique_lock<std::mutex>(vad->mu);
   if (spk) spk_lock = std::unique_lock<std::mutex>(spk->mu);
   cudaSetDevice(m.file.device);
-  m.pool_calls += (int64_t)pass.size();
-  std::vector<char> failed(pass.size(), 0);
   PackHotwords sets;                                         // the pass's distinct hotword sets: the same count and the same bytes
   for (Ticket* t : pass) {
     t->hw_set = -1;
@@ -407,16 +399,12 @@ void run_pass(Model& m, const std::vector<Ticket*>& pass) {
         stride = w;
         rows += units[g1].count;
       }
-      if (!pool_group(m, std::vector<Unit>(units.begin() + g0, units.begin() + g1), stride, failed, pass, sets)) return false;
+      if (!pool_group(m, std::vector<Unit>(units.begin() + g0, units.begin() + g1), stride, sets)) return false;
     }
     return true;
   });
-  const std::string msg = ok ? std::string() : g_err;       // a device failure: every ticket of the pass gets its message
-  for (size_t k = 0; k < pass.size(); ++k)
-    if (!ok || failed[k]) {
-      pass[k]->res.reset();
-      if (!ok) pass[k]->err = msg;
-    }
+  if (!ok)                                                   // a device failure: every ticket of the pass gets its message
+    for (Ticket* t : pass) t->err = g_err;
 }
 
 }  // namespace
@@ -424,49 +412,11 @@ void run_pass(Model& m, const std::vector<Ticket*>& pass) {
 namespace fa_handle {
 
 void* pool_call(Model& m, Ticket& t) {
-  // Whatever a pass throws, the tickets it drained end done (with a message when they have no result), pool_busy is cleared and the
-  // waiters are woken, so the next caller can lead; no exception crosses the C ABI.
-  struct Lead {
-    Model& m;
-    std::unique_lock<std::mutex>& q;
-    std::vector<Ticket*> pass;
-    ~Lead() {
-      if (!q.owns_lock()) q.lock();
-      for (Ticket* p : pass) {
-        if (!p->res && p->err.empty()) p->err = "fa_offline_infer: the pass failed";
-        p->done = true;
-      }
-      m.pool_busy = false;
-      m.pool_cv.notify_all();
-    }
-  };
-  std::string msg;
-  try {
-    std::unique_lock<std::mutex> q(m.pool_mu);
-    m.pool_q.push_back(&t);
-    while (!t.done) {
-      if (m.pool_busy) {                                    // a leader is running a pass: it may drain this ticket
-        m.pool_cv.wait(q);
-        continue;
-      }
-      m.pool_busy = true;
-      Lead lead{m, q, {}};
-      lead.pass = drain(m);
-      q.unlock();
-      run_pass(m, lead.pass);
-    }
-  } catch (const std::exception& e) {
-    msg = std::string("fa_offline_infer: ") + e.what();
-    try {                                                   // never leave this ticket where a leader could still write to it
-      std::unique_lock<std::mutex> q(m.pool_mu);
-      auto it = std::find(m.pool_q.begin(), m.pool_q.end(), &t);
-      if (it != m.pool_q.end()) m.pool_q.erase(it);
-      else m.pool_cv.wait(q, [&] { return t.done; });
-    } catch (const std::exception&) {
-    }
-    t.res.reset();
-  }
-  if (!t.res) return fail(msg.empty() ? t.err : msg);
+  m.pool.call(t, admit, [&](std::vector<Ticket*>& pass, std::vector<Ticket*>& ended) {
+    run_pass(m, pass);
+    ended.swap(pass);
+  }, "fa_offline_infer: ");
+  if (!t.err.empty()) return fail(t.err);
   g_err.clear();
   return t.res.release();
 }
@@ -476,7 +426,7 @@ void* pool_call(Model& m, Ticket& t) {
 extern "C" int fa_offline_pool_stats(const void* handle, int64_t* calls, int64_t* packs) {
   const Model* m = static_cast<const Model*>(handle);
   if (!m || !calls || !packs) return FA_ERR_ARG;
-  *calls = m->pool_calls.load();
+  *calls = m->pool.calls.load();
   *packs = m->pool_packs.load();
   return FA_OK;
 }

@@ -4,12 +4,12 @@
 // Concurrent fa_punc_infer calls on one handle share steps.  A window's punctuation depends on that window only (punc_text.cpp), and
 // a step is one window per text, so the texts of many calls can advance in one lockstep walk, and a call can join it at any step
 // boundary.  A call checks its arguments and splits its texts into words on its own thread, then posts a ticket holding their walk
-// state.  The thread that finds no leader leads: under the device lock, each step admits the queued tickets in arrival order (while the
-// step's carve stays within kStepBytes; the first on an idle pool always), composes one padded step from every active text of every
-// admitted call, scores it, applies the results, and wakes the calls that ended.  It returns once its own call has ended, and a
-// waiter leads on.  The walk state lives in the tickets, not on a leader's stack.  A window over max_window fails only its own call,
-// before that step's scorer runs, with the message it gets alone; a scorer or device failure fails every call that had a window in
-// that step.  No thread is created.
+// state to the handle's request pool (request_pool.h).  Each round of the pool's leader is one step: it admits the queued tickets in
+// arrival order (while the step's carve stays within kStepBytes; the first on an idle pool always), composes one padded step from
+// every active text of every admitted call, scores it under the device lock and applies the results; the calls that ended leave the
+// pool.  Admitted calls stay held across steps, so the walk state lives in the tickets, not on a leader's stack.  A window over
+// max_window fails only its own call, before that step's scorer runs, with the message it gets alone; a scorer or device failure fails
+// every call that had a window in that step.
 #include "handle.h"
 #include "punc_text.h"
 
@@ -24,13 +24,10 @@ enum { kPuncLayers = 0, kPuncDModel, kPuncHeads, kPuncKernel, kPuncSentenceEnd, 
 const size_t kStepBytes = size_t(1) << 30;
 
 // One fa_punc_infer call in the pool: its texts' walk state, stepped by whichever thread leads
-struct PuncTicket {
+struct PuncTicket : PoolTicket {
   std::vector<fa_punc::Text> texts;
   int64_t steps = 0;                                 // the steps it had a window in
-  // written by the leader, read by the owner once done
-  std::unique_ptr<fa_punc::Result> res;
-  std::string err;
-  bool done = false;
+  std::unique_ptr<fa_punc::Result> res;              // written by the leader, read by the owner once done
 };
 
 struct Punc {
@@ -47,15 +44,9 @@ struct Punc {
   void* host_ctx = nullptr;
   DevBuf punc_step;                                  // grown to the largest step's t_max
   std::vector<int32_t> host_io;                      // ids [batch, t_max] then lens [batch]: one host-to-device copy per step
-  // the pool: posted tickets in arrival order, admitted tickets with windows left (in admission order), whether a thread leads, the
-  // leader's step, counters since init
-  std::mutex pool_mu;
-  std::condition_variable pool_cv;
-  std::deque<PuncTicket*> queue;
-  std::vector<PuncTicket*> active;
-  bool busy = false;
-  fa_punc::Step step;
-  std::atomic<int64_t> pool_calls{0}, pool_steps{0};
+  RequestPool<PuncTicket> pool;                      // held: the admitted calls with windows left, in admission order
+  fa_punc::Step step;                                // the leader's step
+  std::atomic<int64_t> pool_steps{0};                // steps scored since init
 };
 
 // a newline-joined UTF-8 list stored as the bytes of an fp32 tensor
@@ -172,129 +163,69 @@ void finish(PuncTicket& t) {
   t.texts.clear();
 }
 
-// Under pool_mu: queued tickets join the walk in arrival order while the next step's carve stays within kStepBytes; the first ticket
-// of an idle walk always joins, and a ticket that does not fit holds back those behind it
-void admit_queued(Punc& p) {
+// A step's admission: queued tickets join the walk in arrival order while the next step's carve stays within kStepBytes; the first
+// ticket of an idle walk always joins, and a ticket that does not fit holds back those behind it
+void admit_queued(const Punc& p, std::deque<PuncTicket*>& queue, std::vector<PuncTicket*>& held) {
   int64_t B = 0, T = 0;
   auto extent = [&](const PuncTicket& t, int64_t& b, int64_t& tm) {
     for (const fa_punc::Text& x : t.texts)
       if (x.active()) { ++b; tm = std::max(tm, fa_punc::window_len(p.vocab, x)); }
   };
-  for (const PuncTicket* t : p.active) extent(*t, B, T);
-  while (!p.queue.empty()) {
-    PuncTicket* t = p.queue.front();
+  for (const PuncTicket* t : held) extent(*t, B, T);
+  while (!queue.empty()) {
+    PuncTicket* t = queue.front();
     int64_t b = B, tm = T;
     extent(*t, b, tm);
-    if (!p.active.empty() && step_bytes(p, b, tm) > kStepBytes) break;
-    p.active.push_back(t);
-    p.queue.pop_front();
-    ++p.pool_calls;
+    if (!held.empty() && step_bytes(p, b, tm) > kStepBytes) break;
+    held.push_back(t);
+    queue.pop_front();
     B = b; T = tm;
   }
 }
 
-// One step over every admitted call's active texts (the leader, outside pool_mu); the calls that ended leave p.active for `ended`,
-// with a result or a message
-void run_step(Punc& p, std::vector<PuncTicket*>& ended) {
-  std::vector<fa_punc::Text*> rows;
-  std::vector<PuncTicket*> owner;                    // per row
-  try {
-    for (PuncTicket* t : p.active) {                 // a window over max_window fails its call before the scorer runs, as alone
-      const size_t r0 = rows.size();
-      for (size_t i = 0; i < t->texts.size() && t->err.empty(); ++i) {
-        fa_punc::Text& x = t->texts[i];
-        if (!x.active()) continue;
-        if (!fa_punc::check_window(p.vocab, x, (int32_t)i, p.max_window, t->err)) break;
-        rows.push_back(&x);
-      }
-      if (!t->err.empty()) rows.resize(r0);
-      owner.resize(rows.size(), t);
-    }
-    if (!rows.empty()) {
-      fa_punc::compose(p.vocab, rows, p.step);
-      std::string err;
-      bool ok;
-      {
-        std::lock_guard<std::mutex> dev(p.mu);
-        ok = score_step(p, p.step, err);
-      }
-      if (ok) ++p.pool_steps;
-      for (size_t b = 0; b < rows.size(); ++b) {
-        PuncTicket* t = owner[b];
-        if (!ok) { t->err = err; continue; }       // a failed step fails every call that had a window in it
-        if (b == 0 || owner[b - 1] != t) ++t->steps;
-        if (t->err.empty()) fa_punc::apply(p.vocab, *rows[b], p.step, (int32_t)b, t->err);
-      }
-    }
-  } catch (const std::exception& e) {                // every admitted call ends with the message
-    for (PuncTicket* t : p.active)
-      if (t->err.empty()) t->err = std::string("fa_punc_infer: ") + e.what();
-  }
-  size_t keep = 0;
-  for (PuncTicket* t : p.active) {
-    bool left = false;
-    for (const fa_punc::Text& x : t->texts) left = left || x.active();
-    if (t->err.empty() && left) { p.active[keep++] = t; continue; }
-    if (t->err.empty()) finish(*t);
-    t->texts.clear();
-    ended.push_back(t);
-  }
-  p.active.resize(keep);
+bool has_ended(const PuncTicket& t) {
+  return !t.err.empty() || std::none_of(t.texts.begin(), t.texts.end(), [](const fa_punc::Text& x) { return x.active(); });
 }
 
-// t's call through the pool -> its result, or nullptr with its own message set as this thread's error
-void* pool_call(Punc& p, PuncTicket& t) {
-  // Whatever a step throws, leadership is given up and the waiters are woken, so one of them leads on; no exception crosses the C ABI.
-  struct Lead {
-    Punc& p;
-    std::unique_lock<std::mutex>& q;
-    ~Lead() {
-      if (!q.owns_lock()) q.lock();
-      p.busy = false;
-      p.pool_cv.notify_all();
+// One step over every held call's active texts; the calls that ended, with a result or a message, move from held to `ended`
+void run_step(Punc& p, std::vector<PuncTicket*>& held, std::vector<PuncTicket*>& ended) {
+  std::vector<fa_punc::Text*> rows;
+  std::vector<PuncTicket*> owner;                    // per row
+  for (PuncTicket* t : held) {                       // a window over max_window fails its call before the scorer runs, as alone
+    const size_t r0 = rows.size();
+    for (size_t i = 0; i < t->texts.size() && t->err.empty(); ++i) {
+      fa_punc::Text& x = t->texts[i];
+      if (!x.active()) continue;
+      if (!fa_punc::check_window(p.vocab, x, (int32_t)i, p.max_window, t->err)) break;
+      rows.push_back(&x);
     }
-  };
-  std::string msg;
-  try {
-    std::unique_lock<std::mutex> q(p.pool_mu);
-    p.queue.push_back(&t);
-    while (!t.done) {
-      if (p.busy) {                                          // a leader is stepping: it admits this ticket at a step boundary
-        p.pool_cv.wait(q);
-        continue;
-      }
-      p.busy = true;
-      Lead lead{p, q};
-      if (!p.host_score) cudaSetDevice(p.file.device);
-      std::vector<PuncTicket*> ended;
-      while (!t.done) {
-        admit_queued(p);
-        q.unlock();
-        ended.clear();
-        run_step(p, ended);
-        q.lock();
-        for (PuncTicket* e : ended) e->done = true;
-        if (!ended.empty()) p.pool_cv.notify_all();
-      }
-    }
-  } catch (const std::exception& e) {
-    msg = std::string("fa_punc_infer: ") + e.what();
-    try {                                                   // never leave this ticket where a leader could still step it
-      std::unique_lock<std::mutex> q(p.pool_mu);
-      auto drop = [&](auto& c) {
-        auto it = std::find(c.begin(), c.end(), &t);
-        if (it == c.end()) return false;
-        c.erase(it);
-        return true;
-      };
-      if (!drop(p.queue)) p.pool_cv.wait(q, [&] { return t.done || (!p.busy && drop(p.active)); });
-    } catch (const std::exception&) {
-    }
-    t.res.reset();
+    if (!t->err.empty()) rows.resize(r0);
+    owner.resize(rows.size(), t);
   }
-  if (!t.res) return fail(msg.empty() ? t.err : msg);
-  g_err.clear();
-  return t.res.release();
+  if (!rows.empty()) {
+    fa_punc::compose(p.vocab, rows, p.step);
+    std::string err;
+    bool ok;
+    if (!p.host_score) cudaSetDevice(p.file.device);
+    {
+      std::lock_guard<std::mutex> dev(p.mu);
+      ok = score_step(p, p.step, err);
+    }
+    if (ok) ++p.pool_steps;
+    for (size_t b = 0; b < rows.size(); ++b) {
+      PuncTicket* t = owner[b];
+      if (!ok) { t->err = err; continue; }         // a failed step fails every call that had a window in it
+      if (b == 0 || owner[b - 1] != t) ++t->steps;
+      if (t->err.empty()) fa_punc::apply(p.vocab, *rows[b], p.step, (int32_t)b, t->err);
+    }
+  }
+  for (PuncTicket* t : held) {
+    if (!has_ended(*t)) continue;
+    ended.push_back(t);
+    if (t->err.empty()) finish(*t);
+    t->texts.clear();
+  }
+  held.erase(std::remove_if(held.begin(), held.end(), [](const PuncTicket* t) { return has_ended(*t); }), held.end());
 }
 
 // fa_punc_init_host / fa_punc_walk_host: the caller's vocabulary, checked
@@ -334,7 +265,12 @@ extern "C" void* fa_punc_infer(void* punc, const char* const* texts, int32_t n) 
         return true;
       }))
     return nullptr;
-  return any ? pool_call(*p, t) : t.res.release();
+  if (!any) return t.res.release();
+  p->pool.call(t, [&](std::deque<PuncTicket*>& queue, std::vector<PuncTicket*>& held) { admit_queued(*p, queue, held); },
+               [&](std::vector<PuncTicket*>& held, std::vector<PuncTicket*>& ended) { run_step(*p, held, ended); }, "fa_punc_infer: ");
+  if (!t.err.empty()) return fail(t.err);
+  g_err.clear();
+  return t.res.release();
 }
 
 extern "C" void* fa_punc_init_host(const char* const* tokens, int32_t n_tokens, const char* const* punc_list, int32_t n_punc,
@@ -355,7 +291,7 @@ extern "C" void* fa_punc_init_host(const char* const* tokens, int32_t n_tokens, 
 extern "C" int fa_punc_pool_stats(const void* punc, int64_t* calls, int64_t* steps) {
   const Punc* p = static_cast<const Punc*>(punc);
   if (!p || !calls || !steps) return FA_ERR_ARG;
-  *calls = p->pool_calls.load();
+  *calls = p->pool.calls.load();
   *steps = p->pool_steps.load();
   return FA_OK;
 }

@@ -2,10 +2,10 @@
 // 192-dim embeddings), fa_spk_cluster (ClusterBackend over host embeddings), and diarize, which the recogniser's request pool
 // (offline_pool.cu) runs once over a group's diarized recordings already on the device.
 //
-// Speaker-only calls share passes through the handle's own request pool: a call checks its arguments on its own thread and posts a
-// ticket; the thread that finds no pass running leads one over the queued calls (arrival order, up to an hour of padded audio and
-// kPoolClusterRows clustering rows) and wakes their threads.  Each call gets exactly what it gets alone: an embedding row carries its
-// call's padded length (fa_campplus_forward_ext), and each clustering call is one set of spk_cluster.
+// Speaker-only calls share passes through the handle's own request pool (request_pool.h): a call checks its arguments on its own
+// thread and posts a ticket; each round of the pool's leader is one pass over the queued calls (arrival order, up to an hour of padded
+// audio and kPoolClusterRows clustering rows), and every call of a pass ends with it.  Each call gets exactly what it gets alone: an
+// embedding row carries its call's padded length (fa_campplus_forward_ext), and each clustering call is one set of spk_cluster.
 #include "handle.h"
 #include <math.h>
 
@@ -477,7 +477,7 @@ extern "C" void fa_spk_uninit(void* spk) { delete static_cast<Spk*>(spk); }
 namespace fa_handle {
 
 // One fa_spk_embed* or fa_spk_cluster call, its arguments checked, waiting in the speaker handle's pool
-struct SpkTicket {
+struct SpkTicket : PoolTicket {
   bool cluster = false;
   // fa_spk_embed*: batch rows of the caller's audio, their 16 kHz lengths, and the call's extent (fbank_frames of its longest row)
   const void* const* bufs = nullptr;
@@ -492,10 +492,6 @@ struct SpkTicket {
   const float* emb_in = nullptr;
   int n = 0, preset = 0;
   int32_t* labels = nullptr;
-  // written by the pass, read by the owner once done
-  int rc = FA_ERR_CUDA;
-  std::string err;
-  bool done = false;
 };
 
 }  // namespace fa_handle
@@ -504,21 +500,19 @@ namespace {
 
 int64_t ticket_samples(const SpkTicket& t) { return t.cluster ? 0 : (int64_t)t.batch * t.stride; }
 
-// The head of the queue and the calls behind it in arrival order, until an hour of padded audio or kPoolClusterRows clustering rows
-std::vector<SpkTicket*> drain(Spk& s) {
-  std::vector<SpkTicket*> out{s.pool_q.front()};
-  s.pool_q.pop_front();
-  int64_t samples = ticket_samples(*out[0]), rows = out[0]->cluster ? out[0]->n : 0;
-  while (!s.pool_q.empty()) {
-    SpkTicket* c = s.pool_q.front();
+// A pass's admission: the head of the queue and the calls behind it in arrival order, until an hour of padded audio or
+// kPoolClusterRows clustering rows
+void admit(std::deque<SpkTicket*>& queue, std::vector<SpkTicket*>& pass) {
+  int64_t samples = 0, rows = 0;
+  while (!queue.empty()) {
+    SpkTicket* c = queue.front();
     const int64_t sm = samples + ticket_samples(*c), r = rows + (c->cluster ? c->n : 0);
-    if (sm > kPoolSamples || r > kPoolClusterRows) break;
+    if (!pass.empty() && (sm > kPoolSamples || r > kPoolClusterRows)) break;
     samples = sm;
     rows = r;
-    out.push_back(c);
-    s.pool_q.pop_front();
+    pass.push_back(c);
+    queue.pop_front();
   }
-  return out;
 }
 
 // The embedding calls of a pass.  Calls in order of extent (arrival order within one), so each call's rows are contiguous; packs of
@@ -572,10 +566,9 @@ bool embed_pass(Spk& s, std::vector<SpkTicket*> ts) {
   float* dst = nt == 1 ? ts[0]->emb_host : host.data();
   cudaMemcpyAsync(dst, emb, (size_t)R * kSpkEmbDim * 4, cudaMemcpyDeviceToHost, st);
   if (!sync_stream(st)) return false;
-  for (size_t i = 0; i < nt; ++i) {
-    if (nt > 1) std::copy(host.begin() + (size_t)first[i] * kSpkEmbDim, host.begin() + (size_t)first[i + 1] * kSpkEmbDim, ts[i]->emb_host);
-    ts[i]->rc = FA_OK;
-  }
+  if (nt > 1)
+    for (size_t i = 0; i < nt; ++i)
+      std::copy(host.begin() + (size_t)first[i] * kSpkEmbDim, host.begin() + (size_t)first[i + 1] * kSpkEmbDim, ts[i]->emb_host);
   return true;
 }
 
@@ -603,9 +596,8 @@ bool cluster_pass(Spk& s, const std::vector<SpkTicket*>& ts) {
   cudaMemcpyAsync(emb, emb_h, (size_t)rows * kSpkEmbDim * 4, cudaMemcpyHostToDevice, s.file.st);
   if (!spk_cluster(s, emb, emb_h, sets)) return false;
   for (size_t i = 0; i < ts.size(); ++i) {
-    if (!sets[i].err.empty()) { ts[i]->err = sets[i].err; continue; }
-    std::copy(sets[i].labels.begin(), sets[i].labels.end(), ts[i]->labels);
-    ts[i]->rc = FA_OK;
+    if (!sets[i].err.empty()) ts[i]->err = sets[i].err;
+    else std::copy(sets[i].labels.begin(), sets[i].labels.end(), ts[i]->labels);
   }
   return true;
 }
@@ -620,58 +612,18 @@ void run_pass(Spk& s, const std::vector<SpkTicket*>& pass) {
     const bool ok = no_throw("fa_spk_embed: ", [&] { return emb.empty() || embed_pass(s, emb); }) &&
                     no_throw("fa_spk_cluster: ", [&] { return clu.empty() || cluster_pass(s, clu); });
     if (!ok)
-      for (SpkTicket* t : pass) { t->rc = FA_ERR_CUDA; t->err = g_err; }
+      for (SpkTicket* t : pass) t->err = g_err;
   }
   ++s.pool_passes;
-  s.pool_calls += (int64_t)pass.size();
 }
 
 // t's call through the pool -> its status, with its own message set as this thread's error
 int pool_call(Spk& s, SpkTicket& t) {
-  // Whatever a pass throws, the tickets it drained end done (with a message when they have none), pool_busy is cleared and the
-  // waiters are woken, so the next caller can lead; no exception crosses the C ABI.
-  struct Lead {
-    Spk& s;
-    std::unique_lock<std::mutex>& q;
-    std::vector<SpkTicket*> pass;
-    ~Lead() {
-      if (!q.owns_lock()) q.lock();
-      for (SpkTicket* p : pass) {
-        if (p->rc != FA_OK && p->err.empty()) p->err = "fa_spk: the pass failed";
-        p->done = true;
-      }
-      s.pool_busy = false;
-      s.pool_cv.notify_all();
-    }
-  };
-  std::string msg;
-  try {
-    std::unique_lock<std::mutex> q(s.pool_mu);
-    s.pool_q.push_back(&t);
-    while (!t.done) {
-      if (s.pool_busy) {                                    // a leader is running a pass: it may drain this ticket
-        s.pool_cv.wait(q);
-        continue;
-      }
-      s.pool_busy = true;
-      Lead lead{s, q, {}};
-      lead.pass = drain(s);
-      q.unlock();
-      run_pass(s, lead.pass);
-    }
-  } catch (const std::exception& e) {
-    msg = std::string("fa_spk: ") + e.what();
-    try {                                                   // never leave this ticket where a leader could still write to it
-      std::unique_lock<std::mutex> q(s.pool_mu);
-      auto it = std::find(s.pool_q.begin(), s.pool_q.end(), &t);
-      if (it != s.pool_q.end()) s.pool_q.erase(it);
-      else s.pool_cv.wait(q, [&] { return t.done; });
-    } catch (const std::exception&) {
-    }
-    set_err(msg);
-    return FA_ERR_CUDA;
-  }
-  if (t.rc != FA_OK) { set_err(t.err); return t.rc; }
+  s.pool.call(t, admit, [&](std::vector<SpkTicket*>& pass, std::vector<SpkTicket*>& ended) {
+    run_pass(s, pass);
+    ended.swap(pass);
+  }, "fa_spk: ");
+  if (!t.err.empty()) { set_err(t.err); return FA_ERR_CUDA; }
   g_err.clear();
   return FA_OK;
 }
@@ -748,7 +700,7 @@ extern "C" int fa_spk_cluster(void* spk, const float* emb_host, int32_t n, int32
 extern "C" int fa_spk_pool_stats(const void* spk, int64_t* calls, int64_t* passes) {
   const Spk* s = static_cast<const Spk*>(spk);
   if (!s || !calls || !passes) return FA_ERR_ARG;
-  *calls = s->pool_calls.load();
+  *calls = s->pool.calls.load();
   *passes = s->pool_passes.load();
   return FA_OK;
 }
